@@ -29,7 +29,6 @@ sys.path.insert(0, ROOT)
 
 HIDDEN = 128
 NUM_LAYERS = 8
-L2_BYTES = 126e6
 
 
 def measured_peaks():
@@ -38,44 +37,16 @@ def measured_peaks():
         with open(path) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback: H100 SXM data-sheet HBM3 bandwidth (not measured)"
 
 
 def measured_tensor_peak():
-    """(TFLOP/s, which).  The per-kernel numbers come from a timed region of ~0.1 s at full clocks (see `clocks` in the line), so the
-    BURST cuBLAS bf16 figure is the honest denominator here -- the sustained one was measured at a 1372 MHz power-capped median
-    (VERDICT r1: "burst is the right one here")."""
+    """(TFLOP/s, which): the dense bf16 tensor rate the per-kernel fractions are taken against."""
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         with open(path) as f:
             return float(json.load(f)["bf16_tflops"]), "MEASURED_PEAKS.json bf16_tflops (burst cuBLAS bf16; the timed region is ~0.1 s at full clocks)"
-    return 1590.0, "fallback 1.59 PFLOP/s burst (B200_PROFILING.md)"
-
-
-def tcgen05_peaks():
-    """This repo's own tensor-pipe ceiling: back-to-back tcgen05.mma issue rate (csrc/tc_peak.cu, tools/tc_peak.py; committed as
-    profiles/r02_tcgen05_peaks.json).  {"f16": TFLOP/s, "tf32": TFLOP/s} at N = 256 with the A operand in tensor memory, or {}."""
-    path = os.path.join(ROOT, "profiles", "r02_tcgen05_peaks.json")
-    try:
-        with open(path) as f:
-            res = json.load(f)["results"]
-        pick = lambda kind: max(r["tflops"] for r in res if r["kind"] == kind and r["N"] == 256)  # noqa: E731
-        return {"f16": pick("f16"), "tf32": pick("tf32"), "source": "profiles/r02_tcgen05_peaks.json (own tcgen05.mma issue-rate kernel, M=128 N=256)"}
-    except (OSError, ValueError, KeyError):
-        return {}
-
-
-def ncu_traffic(dtype: str):
-    """DRAM traffic per launch (dram__bytes_read.sum + dram__bytes_write.sum) of the CURRENT kernels, from the committed ncu
-    --set full capture: profiles/ncu_traffic.json, written by tools/ncu_summary.py --traffic from the .ncu-rep of the round.
-    Empty when no capture of this dtype's kernels is committed (traffic is then reported as null)."""
-    path = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    try:
-        with open(path) as f:
-            d = json.load(f)
-        return {k: float(v) for k, v in d.get(dtype, {}).get("kernels", {}).items()}, d.get(dtype, {}).get("source")
-    except (OSError, ValueError):
-        return {}, None
+    return 989.0, "fallback: H100 SXM data-sheet dense bf16 rate (not measured)"
 
 
 def usable_cores() -> int:
@@ -294,6 +265,22 @@ def cpu_reference_run(batch, gnn, agg: str, steps: int, warmup: int, budget_s: f
 
 
 # ------------------------------------------------------------------------------------------------------
+DUMP_ROWS = 65536
+
+
+def dump_outputs(out_dir: str, out: torch.Tensor) -> None:
+    """Writes the output node states of the timed path's last step: rows of a fixed seeded sample (the full [N, 128] fp32
+    array is 105 MB), float32, plus the sampled row indices (float64) -- 32.5 MB in all."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    n = out.shape[0]
+    rows = torch.randperm(n, generator=torch.Generator().manual_seed(1234))[:min(DUMP_ROWS, n)].sort().values
+    sample = out.detach()[rows.to(out.device)].float().cpu().numpy()
+    np.save(os.path.join(out_dir, "node_states_sample.npy"), sample)
+    np.save(os.path.join(out_dir, "node_states_sample_rows.npy"), rows.numpy().astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -311,7 +298,12 @@ def main():
     ap.add_argument("--no-train", action="store_true", help="skip the forward + backward extra measurement")
     ap.add_argument("--no-row-shard", action="store_true", help="skip the node-range-split (all-gather) extra measurement")
     ap.add_argument("--profile", action="store_true", help="only the HBM-resident loop (for runs under ncu); prints no bench line")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the output node states of the last timed step to DIR/*.npy (a fixed, seeded "
+                         "sample of %d rows, float32) so that two builds can be compared on identical inputs" % DUMP_ROWS)
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl == "reference" or args.profile):
+        ap.error("--dump-outputs writes the output of the timed GPU path: it cannot be combined with --impl reference or --profile")
     args.warmup = max(args.warmup, 3)
     if args.layers == "mlp":
         args.no_cpu_baseline = True      # the CPU-port leg is written for the headline (gated) stack
@@ -328,7 +320,7 @@ def main():
                     f"{NUM_LAYERS} {'Mlp' if args.layers == 'mlp' else 'Gated'}MessagePassingLayers ({args.agg}), {args.dtype}",
         "step": "edge-plan build + 8 layers on one minibatch",
         "parallelism": f"graph-sharded x{world} (no data-path collective)",
-        "l2": "per-layer working set (states in + packed copy + aggregate + states out: 0.42 GB fp32 / 0.16 GB bf16) > 126 MB L2 and "
+        "l2": "per-layer working set (states in + packed copy + aggregate + states out: 0.42 GB fp32 / 0.16 GB bf16) > 50 MB L2 and "
               "every layer reads what the previous one wrote; no explicit flush",
     }
 
@@ -382,10 +374,13 @@ def main():
     def expanded(adj):
         return list(adj) + [(t, s) for s, t in adj] + [(ident, ident)]
 
+    last = {}
+
     def step_resident():
         P.clear_plan_cache()  # every step is a new minibatch: the plan is rebuilt inside the timed region
         with torch.no_grad():
-            return gnn.gnn(h_dev, expanded(adj_dev), None, n2g, {}, {})
+            last["out"] = gnn.gnn(h_dev, expanded(adj_dev), None, n2g, {}, {})
+        return last["out"]
 
     def step_e2e():
         P.clear_plan_cache()
@@ -505,6 +500,8 @@ def main():
     with ClockSampler(local_rank) as clocks:
         ms_step, launches = timed(step_resident, args.steps, args.warmup)
     clock_summary = clocks.summary()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["out"])
     ms_e2e_serial, _ = timed(step_e2e, args.steps, args.warmup)
     pipe = PipelinedE2E()
     ms_e2e_eager, _ = timed(pipe.step, args.steps, args.warmup, finish=pipe.finish)
@@ -572,14 +569,13 @@ def main():
         "message": 2 * E * k_in * D,
         "gru": 2 * n_nodes * (3 * HIDDEN * D + 3 * HIDDEN * HIDDEN),
     }
-    # MMAs issued per reference product and their rate relative to the bf16 peak: fused fp32 = 3 kind::f16 products (3xFP16);
-    # unfused fp32 message / GRU = 3 kind::tf32 products at half the bf16 rate (3xTF32); bf16 = 1
+    # MMAs issued per reference product and their rate relative to the bf16 peak: fused fp32 = 3 f16 products (3xFP16);
+    # unfused fp32 message / GRU = 3 tf32 products at half the bf16 rate (3xTF32); bf16 = 1
     gru_ws = fused and os.environ.get("PTGNN_B200_GRU", "") != "tc"        # weights-stationary GRU kernel: 3xFP16 as well
     if args.dtype == "f32":
         exact_div = {"message": 3.0 if fused else 6.0, "gru": 3.0 if gru_ws else 6.0}
     else:
         exact_div = {"message": 1.0, "gru": 1.0}
-    own_peaks = tcgen05_peaks()
     kernel_names = {"message": "tc_pipeline_kernel<MsgPolicy> (edge messages)", "reduce": "segment_reduce_stream_kernel",
                     "gru": "tc_pipeline_kernel<GruPolicy> (GRUCell update)", "plan": "edge-plan kernels", "pack": "weight split/pack"}
     if args.dtype == "bf16":
@@ -589,7 +585,6 @@ def main():
         kernel_names.update(message="fused_aggregate_kernel (gather -> W_t -> segmented reduce, %s)" % ("3xFP16" if args.dtype == "f32" else "bf16"),
                             gru="gru_ws_kernel (weights-stationary GRUCell, %s)" % ("3xFP16" if args.dtype == "f32" else "bf16") if gru_ws else kernel_names["gru"],
                             pack="pack_states_kernel (fp32 -> fp16 hi|lo' rows) + weight packing", plan="edge-plan + block-plan kernels")
-    traffic, traffic_src = ncu_traffic(args.dtype)
     kernels = {}
     for name, (ms, cnt) in kt.items():
         if cnt:
@@ -600,7 +595,6 @@ def main():
                 entry["alg_bytes"] = alg_bytes[name]
                 entry["achieved_gbs"] = alg_bytes[name] / (avg_ms * 1e-3) / 1e9
                 entry["frac_hbm"] = entry["achieved_gbs"] / peak
-                entry["ncu_dram_bytes"] = traffic.get(name)
             if name in alg_flops:
                 entry["alg_tflops"] = alg_flops[name] / (avg_ms * 1e-3) / 1e12
                 entry["frac_tensor_bf16_peak"] = entry["alg_tflops"] / tensor_peak
@@ -618,8 +612,6 @@ def main():
         if name in alg_flops:
             entry["tensor_ceiling_tflops"] = ceiling
             entry["frac_tensor_exact_peak"] = entry["alg_tflops"] / ceiling
-            if own_peaks:      # the stricter denominator: this GPU's tcgen05 issue rate (kind::f16; kind::tf32 runs at half of it)
-                entry["frac_of_tcgen05_issue_rate"] = entry["alg_tflops"] / (own_peaks["f16"] / exact_div.get(name, 1.0))
     # the kernel with the largest share of the step
     dominant = max((k for k in kernels if "alg_bytes" in kernels[k] and k != "pack"),
                    key=lambda k: kernels[k]["avg_ms"] * kernels[k]["launches_per_step"])
@@ -627,18 +619,15 @@ def main():
     if dk["bound"] == "tensor":
         roofline = {
             "kernel": dk["kernel"], "bound": "tensor", "achieved": dk["alg_tflops"], "peak": dk["tensor_ceiling_tflops"], "unit": "TFLOP/s",
-            "frac": dk["frac_tensor_exact_peak"], "traffic": traffic.get(dominant), "traffic_source": traffic_src,
+            "frac": dk["frac_tensor_exact_peak"],
             "peak_source": tensor_src + " / %g (MMAs issued per fp32-exact product x rate ratio)" % exact_div.get(dominant, 1.0),
             "note": "dominant kernel by time. achieved = the reference's multiply-adds (x2) per launch / CUDA-event launch time; "
                     "kernels[*].floor_ms has both floors and kernels[*].frac_hbm the bandwidth view.",
         }
-        if own_peaks:
-            roofline["tcgen05_issue_rate"] = {"f16_tflops": own_peaks["f16"], "tf32_tflops": own_peaks["tf32"], "source": own_peaks["source"],
-                                              "frac": dk.get("frac_of_tcgen05_issue_rate")}
     else:
         roofline = {
             "kernel": dk["kernel"], "bound": "hbm", "achieved": dk["achieved_gbs"], "peak": peak, "unit": "GB/s",
-            "frac": dk["frac_hbm"], "traffic": traffic.get(dominant), "traffic_source": traffic_src, "peak_source": peak_src,
+            "frac": dk["frac_hbm"], "peak_source": peak_src,
             "note": "dominant kernel by time; algorithmic bytes per launch / CUDA-event launch time (kernels[*].floor_ms has both floors)",
         }
     b_min = 2 * n_nodes * HIDDEN * esz + 8 * E + (T * D * HIDDEN + 6 * HIDDEN * HIDDEN + 6 * HIDDEN) * esz

@@ -1,5 +1,5 @@
 /*
- * ptgnn_b200 -- C ABI of the B200-native message-passing hot path of microsoft/ptgnn.
+ * ptgnn_b200 -- C ABI of the H100-native message-passing hot path of microsoft/ptgnn.
  *
  * The reference is pure Python; the native boundary its hot path crosses is the third-party
  * torch_scatter operator (`torch_scatter.scatter`, called at
@@ -128,7 +128,7 @@ int ptgnn_b200_scatter_f32(const float *src, const int64_t *index, int64_t num_e
  * node-range shard (multi-GPU split of one connected graph) node_states holds the num_nodes OWNED rows (targets,
  * local ids) and gather_states the all-gathered [num_source_nodes, H] states (sources, global ids).
  * workspace >= ptgnn_b200_gated_workspace_bytes(...): message buffer [E, D] + aggregate [N, D] + packed / TF32-split
- * weights.  Dimensions that fit the tensor-core tiles (H % 32 == 0, D % 16 == 0) run on tcgen05 (3xTF32, fp32-exact);
+ * weights.  Dimensions that fit the tensor-core tiles (H % 32 == 0, D % 16 == 0) run on wgmma (3xTF32, fp32-exact);
  * other multiples of 4 run on the FFMA kernels.  PTGNN_B200_DISABLE_TC=1 forces the FFMA kernels.
  * ---------------------------------------------------------------------------------------------- */
 size_t ptgnn_b200_gated_workspace_bytes(int64_t num_nodes, int64_t num_edges, int32_t num_types, int32_t state_dim,
@@ -220,7 +220,7 @@ int ptgnn_b200_mlp_forward_bf16(const uint16_t *node_states, const uint16_t *gat
  * message tensor of gatedmessagepassing.py:64 / mlpmessagepassing.py:100-112 is never materialised.
  *
  * Block plan: the edges sorted, stably, by (target block, edge type, target), blocks of `block_targets`
- * (<= 240, multiple of 8; ptgnn_b200_block_plan_block_targets recommends one) consecutive target nodes:
+ * (<= 176, multiple of 8; ptgnn_b200_block_plan_block_targets recommends one) consecutive target nodes:
  *   group_off[ceil(N / B) * T + 1]  sorted-edge offsets of the (block, type) groups
  *   src_f[E]                        source node of the edge at sorted position j
  *   tl_f[E]                         target of that edge, relative to its block's first node

@@ -1,4 +1,4 @@
-"""ptgnn_b200 -- B200-native (sm_100a) implementation of microsoft/ptgnn's sparse message-passing hot path.
+"""ptgnn_b200 -- H100-native (sm_90a) implementation of microsoft/ptgnn's sparse message-passing hot path.
 
 Scope (BASELINE.json ``north_star``, SURVEY.md §8): ``GatedMessagePassingLayer`` / ``MlpMessagePassingLayer``,
 the ``GraphNeuralNetwork`` layer loop and the ``torch_scatter.scatter`` boundary below them, behind the reference's

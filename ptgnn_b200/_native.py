@@ -177,7 +177,7 @@ def current_stream(device: torch.device) -> int:
 def require_cuda(t: torch.Tensor, name: str, dtype: torch.dtype) -> torch.Tensor:
     if not t.is_cuda:
         raise NativeLibraryError(
-            f"{name} is on {t.device}; ptgnn_b200 only runs on CUDA (sm_100a) and has no CPU fallback"
+            f"{name} is on {t.device}; ptgnn_b200 only runs on CUDA (sm_90a) and has no CPU fallback"
         )
     if t.dtype != dtype:
         raise TypeError(f"{name} must be {dtype}, got {t.dtype}")

@@ -1,4 +1,4 @@
-"""In-tree build of libptgnn_b200.so (sm_100a only).  `python -m ptgnn_b200.build` or __graft_entry__.build()."""
+"""In-tree build of libptgnn_b200.so (sm_90a only: H100).  `python -m ptgnn_b200.build` or __graft_entry__.build()."""
 import os
 import subprocess
 import sys
@@ -6,10 +6,10 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libptgnn_b200.so")
-SOURCES = ["capi.cu", "plan.cu", "reduce.cu", "layers.cu", "layers_tc.cu", "layers_bf16.cu", "fused_mp.cu", "gru_ws.cu", "tc_peak.cu", "batching.cu", "gru_grad.cu"]
+SOURCES = ["capi.cu", "plan.cu", "reduce.cu", "layers.cu", "layers_tc.cu", "layers_bf16.cu", "fused_mp.cu", "gru_ws.cu", "batching.cu", "gru_grad.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "-Xptxas", "-v",
 ]
 

@@ -39,7 +39,7 @@ __global__ void __launch_bounds__(256) segment_map_kernel(const int32_t *__restr
 
 static unsigned grid_for(int64_t n) {
     const int64_t b = ceil_div(n, (int64_t)256);
-    return (unsigned)(b < 148 * 8 ? (b < 1 ? 1 : b) : 148 * 8);
+    return (unsigned)(b < 132 * 8 ? (b < 1 ? 1 : b) : 132 * 8);
 }
 
 }  // namespace ptgnn

@@ -1,4 +1,4 @@
-// Shared helpers for the ptgnn_b200 CUDA library (sm_100a only).
+// Shared helpers for the ptgnn_b200 CUDA library (sm_90a only: H100).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -90,8 +90,8 @@ template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
 
 // ---- L2 residency control ---------------------------------------------------------------------------------------
-// Optional (PTGNN_L2_HINTS=4): read the message rows in the reduce with an evict-first L2 policy.  Measured on B200:
-// no gain (and `cp.async ... L2::cache_hint` for the gathers faults), so the default is plain streaming loads.
+// Optional (PTGNN_L2_HINTS=4): read the message rows in the reduce with an evict-first L2 policy; the default is plain
+// streaming loads.
 __device__ __forceinline__ uint64_t l2_policy_evict_first() {
     uint64_t p;
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));

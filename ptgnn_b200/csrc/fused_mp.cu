@@ -1,4 +1,4 @@
-// Fused gather -> per-edge-type Linear -> segmented reduce on tcgen05 (see fused_mp.cuh for the design).
+// Fused gather -> per-edge-type Linear -> segmented reduce on wgmma (see fused_mp.cuh for the design).
 #include "fused_mp.cuh"
 
 #include <cuda_bf16.h>
@@ -18,22 +18,23 @@ using tc::mbar_init;
 using tc::mbar_wait;
 
 // ---- geometry ------------------------------------------------------------------------------------------------------
-constexpr int NUM_THREADS = 16 * 32;
-constexpr int MMA_WARP = 4;
-constexpr int GATHER_WARP0 = 5, GATHER_THREADS = 64;
-constexpr int SCHED_WARP = 7;
-constexpr int EPI_THREADS = 256;                       // two epilogue warpgroups (warps 0-3, 8-11): lower / upper half of a block's targets
-constexpr int NUM_CONSUMER_WARPS = 4 + 1 + 2 + 8;      // weight loaders, MMA, gatherers, epilogue (scheduler table readers)
+// Roles (12 warps): 0-3 and 4-7 CONSUMERS, two warpgroups | 8-9 ROW GATHERERS | 10 SCHEDULER | 11 idle.
+constexpr int NUM_THREADS = 12 * 32;
+constexpr int GATHER_WARP0 = 8, GATHER_THREADS = 64;
+constexpr int SCHED_WARP = 10;
+constexpr int NUM_CONSUMER_WARPS = 8 + 2;             // readers of the scheduler's table: consumers, gatherers
 constexpr int NUM_SLOTS = 3, LOOKAHEAD = 2;
 constexpr int SLOT_BYTES = 32768;
 constexpr int RING_BYTES = NUM_SLOTS * SLOT_BYTES;
 constexpr int META_RING = 8;
 constexpr int SCHED_RING = 4;
-// 512 threads launch with 128 registers each; warps 4-7 and the weight loaders give registers back, the two epilogue warpgroups take them:
-// (2 * 160 + 72 + 120) * 128 = 65536.  ptxas only extends a role's budget beyond the launch cap when that role is the LAST branch.
-constexpr int EPI_REGS = 160, W_REGS = 120, MID_REGS = 72;
-constexpr int ACC_TMEM_OFF = 256;                               // weight buffers below, accumulators above
-constexpr int EPI_BAR_ID = 2;
+// the producer warpgroup gives registers back, the two consumer warpgroups take them: (56 + 2 * 224) * 128 = 64512
+constexpr int CONSUMER_REGS = 224, PRODUCER_REGS = 56;
+static_assert(PRODUCER_REGS + 2 * CONSUMER_REGS <= 3 * 168, "register budgets exceed the launch allocation");
+constexpr int NMAX = 64;                                        // edges per MMA (accumulator columns)
+constexpr int ACC_PITCH = NMAX + 4;                             // accumulator tile: 128 features x NMAX columns, fp32
+constexpr int ACC_BYTES = kD * ACC_PITCH * 4;
+constexpr int MMA_BAR_ID = 1, EPI_BAR_ID = 2;
 
 struct Meta {                     // per sub-group: what the epilogue needs to know about the accumulator columns
     int32_t tloff[128];           // byte offset of the column's target row inside agg_s (0 for columns >= n)
@@ -45,10 +46,11 @@ struct Sched {                    // one target block: its id and the T+1 sorted
     int32_t blk, pad[3];
     int32_t off[PTGNN_MAX_EDGE_TYPES + 4];
 };
-constexpr int AGG_OFF = RING_BYTES;
+constexpr int ACC_OFF = RING_BYTES;
+constexpr int AGG_OFF = RING_BYTES + ACC_BYTES;
 __host__ __device__ constexpr int agg_bytes(int B) { return B * kD * 4; }
 constexpr int SMEM_TAIL = META_RING * (int)sizeof(Meta) + SCHED_RING * (int)sizeof(Sched) + 256 /*barriers*/;
-constexpr int smem_bytes(int B) { return 1024 + RING_BYTES + agg_bytes(B) + SMEM_TAIL; }
+constexpr int smem_bytes(int B) { return 1024 + RING_BYTES + ACC_BYTES + agg_bytes(B) + SMEM_TAIL; }
 static_assert(smem_bytes(kMaxBlockTargets) <= 232448, "shared memory budget");
 
 struct Params {
@@ -65,23 +67,6 @@ struct Params {
 };
 
 // ---- small PTX helpers ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void mma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tmem_st_32cols_u32(uint32_t taddr, const uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-          "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]),
-          "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]),
-          "r"(v[30]), "r"(v[31])
-        : "memory");
-}
 __device__ __forceinline__ uint4 ldg_nc_u4(const uint4 *p) {
     uint4 r;
     asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
@@ -89,25 +74,6 @@ __device__ __forceinline__ uint4 ldg_nc_u4(const uint4 *p) {
 }
 __device__ __forceinline__ void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 __device__ __forceinline__ uint32_t swz(int row, int q) { return (uint32_t)(row * 128 + ((q ^ (row & 7)) << 4)); }
-
-// Up to 32 mbarriers polled by ONE try_wait instruction per round: lane i checks (addr, parity) of its own barrier (inactive lanes
-// report done).  A phase check costs ~200 cycles even when the barrier is already complete (measured, tools/fused_trace.py), so
-// the MMA warp's three per-step waits (accumulator drained, rows landed, weights landed) are folded into one.
-__device__ __forceinline__ void mbar_wait_lanes(uint32_t addr, uint32_t parity, bool active) {
-    uint64_t t0 = 0;
-    for (uint32_t spin = 0;; ++spin) {
-        uint32_t done = 1;
-        if (active)
-            asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                         : "=r"(done) : "r"(addr), "r"(parity) : "memory");
-        if (__all_sync(0xffffffffu, done != 0)) return;
-        if ((spin & 0xFF) == 0xFF) {
-            const uint64_t now = tc::global_timer_ns();
-            if (t0 == 0) t0 = now;
-            else if (now - t0 > 2000000000ull) __trap();
-        }
-    }
-}
 
 // Debug timeline (PTGNN_FUSED_TRACE=1): CTA 0, one thread per role, records (clock64, step, tag) at the pipeline hand-offs into its
 // 2048-entry region of the trace buffer; read back with ptgnn_b200_debug_fused_trace (tools/fused_trace.py).
@@ -217,9 +183,8 @@ template <int RED> __device__ __forceinline__ float red_op(float a, float m) {
 // Write-out of a finished block: rows [row_lo, min(row_hi, rows of the block)) of agg_s, taken by the calling warp (ew of the four
 // of its group) 2 rows at a time; a row is reset to the identity as soon as it has been read.  The row loop is specialised at compile
 // time on the output format and on "plain sum" (no mean / max fix-up / activation / LayerNorm): the generic version executed ~180
-// instructions per row.  Register pressure matters here: the epilogue's column loop sits at the 128-register limit, and a 4-row
-// unroll (or a non-inlined call: ABI-constrained allocation) made ptxas spill around every LDTM of the column loop -- drain time
-// per sub-group went from 1,200 to 2,300 cycles (sessions r02g/r02h) -- so check `-Xptxas -v` for 0 spills after touching this.
+// instructions per row.  It runs in the consumer threads, which keep their weight fragments live across it: the fp32 instances
+// already spill a little (`-Xptxas -v`; DESIGN.md §9 item 2), so check that a change does not add to it.
 template <int RED>
 __device__ __forceinline__ void write_out_block(const Params *p, uint32_t agg_saddr, int row0, int row_lo, int row_hi, int ew, int lane) {
     const float IDENT = red_identity<RED>();
@@ -309,110 +274,40 @@ __device__ __forceinline__ void write_out_block(const Params *p, uint32_t agg_sa
 template <int NPROD, int K, int NSEG, int RED>
 __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const __grid_constant__ Params p) {
     constexpr int NPART = NPROD == 3 ? 2 : 1;                      // hi | lo' parts of a row / of the weights
-    constexpr int NMAX = NPROD == 3 ? 64 : (K <= 128 ? 128 : 64);  // edges per MMA (accumulator columns)
     constexpr int ROW_BYTES = K * 2 * NPART;                       // one packed state row
     constexpr int KCH = K / 64;                                    // 128-byte swizzled chunks per part
     constexpr int NT = NPART * KCH;                                // operand tiles per slot
     constexpr int TILE_BYTES = NMAX * 128;
     static_assert(NT * TILE_BYTES <= SLOT_BYTES, "slot size");
-    constexpr int WPART_COLS = K / 2;                              // TMEM columns of one weight part
-    constexpr int WBUF_COLS = NPART * WPART_COLS;
-    static_assert(2 * WBUF_COLS <= ACC_TMEM_OFF, "weight buffers");
-    constexpr int ACC_COLS = 128;                                  // per accumulator set: main [0, NMAX) | correction [64, 128)
-    static_assert(NPROD == 1 || NMAX == 64, "correction accumulator offset");
-    constexpr uint32_t FMT = NPROD == 3 ? 0u /*F16*/ : tc::FMT_BF16;
+    constexpr bool BF16 = NPROD == 1;
 
     extern __shared__ unsigned char smem_raw[];
     // 1024-byte aligned ring; the pad is added as an OFFSET so that the pointers keep the shared address space (an integer
     // round trip makes every access a generic LD/ST with 64-bit address arithmetic)
     unsigned char *ring = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    float *acc_s = reinterpret_cast<float *>(ring + ACC_OFF);
     float *agg_s = reinterpret_cast<float *>(ring + AGG_OFF);
     unsigned char *tail = ring + AGG_OFF + agg_bytes(p.B);
     Meta *meta_ring = reinterpret_cast<Meta *>(tail);
     Sched *sched = reinterpret_cast<Sched *>(tail + META_RING * sizeof(Meta));
     uint64_t *bars = reinterpret_cast<uint64_t *>(tail + META_RING * sizeof(Meta) + SCHED_RING * sizeof(Sched));
-    uint64_t *x_full = bars, *x_empty = bars + 3, *w_full = bars + 6, *w_empty = bars + 8, *acc_full = bars + 10,
-             *acc_empty = bars + 12, *sched_full = bars + 14, *sched_empty = bars + 18;
-    uint32_t *tmem_base_smem = reinterpret_cast<uint32_t *>(bars + 22);
+    uint64_t *x_full = bars, *x_empty = bars + 3, *sched_full = bars + 6, *sched_empty = bars + 10;
 
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
     const int lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
         // x_full: per gather thread one asynchronous arrival when its copies have landed (cp.async.mbarrier.arrive.noinc) and one
         // ordinary arrival that publishes the step's column metadata
-        for (int s = 0; s < NUM_SLOTS; ++s) { mbar_init(&x_full[s], 2 * GATHER_THREADS); mbar_init(&x_empty[s], 1); }
-        for (int b = 0; b < 2; ++b) {
-            mbar_init(&w_full[b], 128); mbar_init(&w_empty[b], 1);
-            mbar_init(&acc_full[b], 1); mbar_init(&acc_empty[b], 8);
-        }
+        for (int s = 0; s < NUM_SLOTS; ++s) { mbar_init(&x_full[s], 2 * GATHER_THREADS); mbar_init(&x_empty[s], 8); }
         for (int r = 0; r < SCHED_RING; ++r) { mbar_init(&sched_full[r], 1); mbar_init(&sched_empty[r], NUM_CONSUMER_WARPS); }
         tc::mbar_init_fence();
     }
-    if (warp == 0) tc::tmem_alloc<512>(tmem_base_smem);
-    tc::tc_fence_before_sync();
     __syncthreads();
-    tc::tc_fence_after_sync();
-    const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_base_smem, 0);
     const int T = p.T;
 
-    if (warp >= 4 && warp < 8) {
-        tc::reg_dealloc<MID_REGS>();
-        if (warp == MMA_WARP) {
-            // ============================================ MMA ISSUER ============================================
-            const bool leader = tc::elect_one();
-            StepGen<NSEG> gen{sched, sched_full, sched_empty, T, NMAX, lane};
-            uint32_t xs = 0, sg = 0, wl = 0, wl0 = 0;
-            Trace tr = make_trace(p.trace, 1, leader);
-            Step s;
-            for (;;) {
-                const int ev = gen.next(s);
-                if (ev == 2) break;
-                if (ev == 1) continue;
-                if (s.first_sub && s.seg == 0) { wl0 = wl; wl += NSEG; }
-                const uint32_t ab = sg & 1;
-                tr.mark(10, xs);
-                const uint32_t slot = xs % NUM_SLOTS;
-                const uint32_t wli = wl0 + s.seg, wb = wli & 1;
-                {   // lane 0: the epilogue has drained this accumulator set | lane 1: the rows have landed | lane 2: the weights have
-                    const uint32_t addr = lane == 0 ? smem_u32(&acc_empty[ab]) : (lane == 1 ? smem_u32(&x_full[slot]) : smem_u32(&w_full[wb]));
-                    const uint32_t parity = lane == 0 ? (((sg >> 1) & 1) ^ 1) : (lane == 1 ? ((xs / NUM_SLOTS) & 1) : ((wli >> 1) & 1));
-                    const bool active = lane == 0 ? s.seg == 0 : (lane == 1 ? true : (lane == 2 && s.first_sub));
-                    mbar_wait_lanes(addr, parity, active);
-                }
-                tc::fence_proxy_async_smem();          // rows written by cp.async (generic proxy) -> read by the MMA (async proxy)
-                tr.mark(13, xs);
-                tc::tc_fence_after_sync();
-                const uint32_t n16 = (uint32_t)(s.n + 15) & ~15u;
-                const uint32_t idesc = tc::make_instr_desc(FMT, 128, n16);
-                const uint32_t slot_addr = smem_u32(ring + slot * SLOT_BYTES);
-                const uint32_t d_main = tmem_base + ACC_TMEM_OFF + ab * ACC_COLS, d_corr = d_main + 64;
-                const uint32_t a_base = tmem_base + wb * WBUF_COLS;
-#pragma unroll
-                for (int ks = 0; ks < K / 16; ++ks) {
-                    const int kc = ks >> 2, kk = ks & 3;
-                    const uint32_t acc = (s.seg == 0 && ks == 0) ? 0u : 1u;
-                    const uint64_t x_hi = tc::make_smem_desc_sw128(slot_addr + kc * TILE_BYTES) + kk * 2;
-                    if (NPROD == 3) {
-                        const uint64_t x_lo = tc::make_smem_desc_sw128(slot_addr + (KCH + kc) * TILE_BYTES) + kk * 2;
-                        if (leader) {
-                            // x * w ~= hi*hi (main) + 2^-11 (hi*lo' + lo'*hi) (correction accumulator, scaled by 2^11)
-                            mma_f16_ts(d_main, a_base + ks * 8, x_hi, idesc, acc);
-                            mma_f16_ts(d_corr, a_base + ks * 8, x_lo, idesc, acc);
-                            mma_f16_ts(d_corr, a_base + WPART_COLS + ks * 8, x_hi, idesc, 1u);
-                        }
-                    } else {
-                        if (leader) mma_f16_ts(d_main, a_base + ks * 8, x_hi, idesc, acc);
-                    }
-                }
-                if (leader) tc::mma_commit(&x_empty[slot]);
-                if (leader && s.last_sub) tc::mma_commit(&w_empty[wb]);
-                if (leader && s.seg == NSEG - 1) tc::mma_commit(&acc_full[ab]);
-                __syncwarp();
-                tr.mark(14, xs);
-                ++xs;
-                if (s.seg == NSEG - 1) ++sg;
-            }
-        } else if (warp == SCHED_WARP) {
+    if (warp >= GATHER_WARP0) {
+        tc::reg_dealloc<PRODUCER_REGS>();
+        if (warp == SCHED_WARP) {
             // ============================================ SCHEDULER ============================================
             // Publishes, a few blocks ahead, the group-offset row of each target block this CTA owns (static round robin).
             for (uint32_t i = 0;; ++i) {
@@ -429,7 +324,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
                 if (lane == 0) mbar_arrive(&sched_full[r]);
                 if (!valid) break;
             }
-        } else {
+        } else if (warp < GATHER_WARP0 + GATHER_THREADS / 32) {
             // ============================================ ROW GATHERERS ============================================
             // 64 threads copy the packed state rows of every (sub-group, segment) into a ring slot with 16-byte cp.async:
             // thread g moves piece q = g & 7 of every 128-byte chunk of rows (g >> 3) + 8 i.  Tile (part, kc) of a slot holds
@@ -517,8 +412,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
             bool more = has_nxt;
             // Completion is signalled by the copies themselves (cp.async.mbarrier.arrive.noinc): the gatherers never wait for data, only
             // for a free slot, so a step's arrival is not held back by the issue of the next one (with cp.async.wait_group it was:
-            // measured 2800 cycles from slot grant to arrival, most of it the next step's slot wait).  The MMA warp makes the landed
-            // bytes visible to the tensor core's async proxy with fence.proxy.async after its wait.
+            // a step's arrival waited for the next step's slot).  The consumers make the landed bytes visible to the tensor core's async
+            // proxy with fence.proxy.async after their wait.
             while (more) {
                 const uint32_t slot = c_issue % NUM_SLOTS;
                 issue_next();
@@ -530,82 +425,32 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
             }
             cp_async_wait<0>();
         }
-    } else if (warp >= 12) {
-        // ============================================ WEIGHT LOADERS ============================================
-        // Thread d owns TMEM lane d = row d of W_t.  The packed weights are laid out so that a warp-wide 16-byte load is one
-        // contiguous 512-byte burst: wpack[(((t * NSEG + seg) * NPART + part) * (K / 8) + c4) * 128 + d] = columns 4 c4 .. 4 c4 + 3.
-        // All loads of a (type, segment) are in flight before the buffer's release is awaited.
-        tc::reg_dealloc<W_REGS>();
-        const int d = (warp & 3) * 32 + lane;
-        const uint32_t tmem_lane = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
-        StepGen<NSEG> gen{sched, sched_full, sched_empty, T, NMAX, lane};
-        uint32_t wl = 0;
-        Trace tr = make_trace(p.trace, 4, (warp & 3) == 0 && lane == 0);
-        Step s;
-        for (;;) {
-            const int ev = gen.next(s);
-            if (ev == 2) break;
-            if (ev == 1 || !s.first_sub) continue;
-            tr.mark(30, wl);
-            // 64 TMEM columns (16 16-byte loads, 64 registers) per round: 512 threads leave 128 registers per thread, so the 128
-            // columns of an fp32 (hi | lo') weight buffer go in two rounds; the first round's loads are issued before the
-            // buffer's release is awaited (the loaders run up to two groups ahead of the MMAs)
-            constexpr int ROUND = WBUF_COLS < 64 ? WBUF_COLS : 64, NROUNDS = WBUF_COLS / ROUND;
-            const uint4 *src = p.wpack + ((size_t)(s.t * NSEG + s.seg) * NPART * (K / 8)) * 128 + d;
-            uint32_t w[ROUND];
-            auto load_round = [&](int r) {
-#pragma unroll
-                for (int j = 0; j < ROUND / 4; ++j) {
-                    const uint4 v = ldg_nc_u4(src + (size_t)(r * (ROUND / 4) + j) * 128);
-                    w[4 * j] = v.x; w[4 * j + 1] = v.y; w[4 * j + 2] = v.z; w[4 * j + 3] = v.w;
-                }
-            };
-            load_round(0);
-            const uint32_t wb = wl & 1;
-            tr.mark(31, wl);
-            mbar_wait(&w_empty[wb], ((wl >> 1) & 1) ^ 1);        // the MMAs that read this buffer two loads ago are done
-            tr.mark(32, wl);
-            tc::tc_fence_after_sync();
-#pragma unroll
-            for (int r = 0; r < NROUNDS; ++r) {
-#pragma unroll
-                for (int j = 0; j < ROUND / 32; ++j) {
-                    uint32_t chunk[32];
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) chunk[i] = w[32 * j + i];
-                    tmem_st_32cols_u32(tmem_lane + wb * WBUF_COLS + r * ROUND + 32 * j, chunk);
-                }
-                if (r + 1 < NROUNDS) {
-                    tc::tmem_st_wait();                            // the stores have read their registers
-                    load_round(r + 1);
-                }
-            }
-            tc::tmem_st_wait();
-            tc::tc_fence_before_sync();
-            mbar_arrive(&w_full[wb]);
-            tr.mark(33, wl);
-            ++wl;
-        }
     } else {
-        // ============================================ EPILOGUE ============================================
-        // Thread d owns message feature d = TMEM lane d and column d of agg_s.  For every accumulator column (edge) in plan
-        // order: value = main (+ 2^-11 correction); at the first edge of a (target, type) segment the running value is
-        // (re)loaded from agg_s[target][d], at the last one it is stored back -- a target's messages are accumulated one by one
-        // in the reference's order, across types and sub-groups.
-        // TWO warpgroups (a single warp per scheduler is latency-bound: measured IPC 0.17): group 0 takes the columns whose
-        // target lies in the lower half of the block, group 1 the upper half.  Edges are sorted by target, so each group owns a
-        // contiguous column range of every sub-group (split = number of lower-half columns) and the two never touch the same
-        // agg_s row -- no synchronisation between them except at the block's write-out.
-        tc::reg_alloc<EPI_REGS>();                 // granted once warps 4-7 and 12-15 have released theirs
-        const int eg = warp >> 3, ew = warp & 3;             // warps 0-3: group 0, warps 8-11: group 1
+        // ============================================ CONSUMERS ============================================
+        // MMA: warpgroup eg computes message features [64 eg, 64 eg + 64) of every sub-group, A = W_t rows (register fragments,
+        // loaded from the packed weights when the (type, segment) changes), B = the gathered rows of the slot (N = 64 edges);
+        // the finished sub-group goes to acc_s[feature][edge] (main + 2^-11 correction).
+        // Epilogue: thread d of a warpgroup owns message feature d and column d of agg_s.  For every accumulator column (edge) in
+        // plan order: at the first edge of a (target, type) segment the running value is (re)loaded from agg_s[target][d], at the
+        // last one it is stored back -- a target's messages are accumulated one by one in the reference's order, across types
+        // and sub-groups.  Group 0 takes the columns whose target lies in the lower half of the block, group 1 the upper half.
+        // Edges are sorted by target, so each group owns a contiguous column range of every sub-group and the two never touch
+        // the same agg_s row -- no synchronisation between them except around acc_s and at the block's write-out.
+        tc::reg_alloc<CONSUMER_REGS>();
+        const int eg = warp >> 2, ew = warp & 3;
         const int d = ew * 32 + lane;
-        const uint32_t tmem_lane = tmem_base + ((uint32_t)(ew * 32) << 16) + ACC_TMEM_OFF;
+        const int gq = lane >> 2, tq = lane & 3;
+        const int f0 = 64 * eg + 16 * ew + gq;               // this thread's A / accumulator rows: features f0, f0 + 8
         const uint32_t aggcol_s = smem_u32(agg_s + d);      // shared-space address of agg_s[0][d]
+        const uint32_t accrow_s = smem_u32(acc_s + d * ACC_PITCH);
         const float IDENT = red_identity<RED>();
         StepGen<NSEG> gen{sched, sched_full, sched_empty, T, NMAX, lane};
         const int row_lo = eg == 0 ? 0 : (p.B >> 1), row_hi = eg == 0 ? (p.B >> 1) : p.B;     // rows this group initialises
         for (int r = row_lo; r < row_hi; ++r) agg_s[r * kD + d] = IDENT;
-        uint32_t sg = 0;
+        uint32_t sg = 0, xs = 0;
+        int w_t = -1, w_seg = -1;
+        uint32_t wf[NPART][K / 16][4];
+        float acc_m[32], acc_c[32];
         float acc = IDENT;
         Trace tr = make_trace(p.trace, 2 + eg, ew == 0 && lane == 0);
         Step s;
@@ -613,22 +458,76 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
             const int ev = gen.next(s);
             if (ev == 2) break;
             if (ev == 0) {
+                if (s.t != w_t || s.seg != w_seg) {
+                    // packed layout: wpack[(((t * NSEG + seg) * NPART + part) * (K / 8) + c4) * 128 + d] = columns 8 c4 .. + 7 of row d
+                    const uint32_t *wp = reinterpret_cast<const uint32_t *>(p.wpack + (size_t)(s.t * NSEG + s.seg) * NPART * (K / 8) * 128);
+#pragma unroll
+                    for (int part = 0; part < NPART; ++part)
+#pragma unroll
+                        for (int ks = 0; ks < K / 16; ++ks)
+#pragma unroll
+                            for (int i = 0; i < 4; ++i) {
+                                const int c4 = (part * (K / 8) + 2 * ks + (i >> 1)), f = f0 + 8 * (i & 1);
+                                wf[part][ks][i] = __ldg(wp + ((size_t)c4 * 128 + f) * 4 + tq);
+                            }
+                    w_t = s.t; w_seg = s.seg;
+                }
+                const uint32_t slot = xs % NUM_SLOTS;
+                tr.mark(13, xs);
+                mbar_wait(&x_full[slot], (xs / NUM_SLOTS) & 1);
+                tc::fence_proxy_async_smem();          // rows written by cp.async (generic proxy) -> read by the MMA (async proxy)
+                if (s.seg == 0) {
+#pragma unroll
+                    for (int i = 0; i < 32; ++i) { acc_m[i] = 0.0f; acc_c[i] = 0.0f; }
+                }
+                const uint32_t slot_addr = smem_u32(ring + slot * SLOT_BYTES);
+                tc::wgmma_fence();
+#pragma unroll
+                for (int ks = 0; ks < K / 16; ++ks) {
+                    const int kc = ks >> 2, kk = ks & 3;
+                    const uint64_t x_hi = tc::make_smem_desc_sw128(slot_addr + kc * TILE_BYTES) + kk * 2;
+                    tc::wgmma_16_rs_n64<BF16>(acc_m, wf[0][ks], x_hi);
+                    if (NPROD == 3) {
+                        // x * w ~= hi*hi (main) + 2^-11 (hi*lo' + lo'*hi) (correction accumulator, scaled by 2^11)
+                        const uint64_t x_lo = tc::make_smem_desc_sw128(slot_addr + (KCH + kc) * TILE_BYTES) + kk * 2;
+                        tc::wgmma_16_rs_n64<BF16>(acc_c, wf[0][ks], x_lo);
+                        tc::wgmma_16_rs_n64<BF16>(acc_c, wf[NPART - 1][ks], x_hi);
+                    }
+                }
+                tc::wgmma_commit();
+                tc::wgmma_wait<0>();
+                tc::fence_acc(acc_m);
+                tc::fence_acc(acc_c);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&x_empty[slot]);
+                tr.mark(14, xs);
+                ++xs;
                 if (s.seg != NSEG - 1) continue;
-                const uint32_t ab = sg & 1;
-                tr.mark(20, sg);
-                mbar_wait(&acc_full[ab], (sg >> 1) & 1);
+                // ---- the sub-group's messages -> acc_s (feature-major), then the reduction along the columns
+                named_bar_sync(MMA_BAR_ID, 256);        // both groups are done with the previous sub-group's acc_s
+#pragma unroll
+                for (int j = 0; j < 8; ++j)
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        float v0 = acc_m[4 * j + 2 * h], v1 = acc_m[4 * j + 2 * h + 1];
+                        if (NPROD == 3) { v0 = fmaf(acc_c[4 * j + 2 * h], 1.0f / 2048.0f, v0); v1 = fmaf(acc_c[4 * j + 2 * h + 1], 1.0f / 2048.0f, v1); }
+                        *reinterpret_cast<float2 *>(acc_s + (f0 + 8 * h) * ACC_PITCH + 8 * j + 2 * tq) = make_float2(v0, v1);
+                    }
+                named_bar_sync(MMA_BAR_ID, 256);
                 tr.mark(21, sg);
-                tc::tc_fence_after_sync();
                 const Meta *m = &meta_ring[sg % META_RING];
                 const int n = s.n;
                 int split = __popc(m->lowmask[0]) + __popc(m->lowmask[1]);
-                if (NMAX > 64) split += __popc(m->lowmask[2]) + __popc(m->lowmask[3]);
                 const int c_lo = eg == 0 ? 0 : split, c_hi = eg == 0 ? split : n;       // this group's columns
                 constexpr int W = 16;
                 for (int c0 = c_lo & ~15; c0 < c_hi; c0 += 16) {
-                    uint32_t vm[W], vc[W];
-                    tc::tmem_ld_16cols_async(tmem_lane + ab * ACC_COLS + c0, vm);
-                    if (NPROD == 3) tc::tmem_ld_16cols_async(tmem_lane + ab * ACC_COLS + 64 + c0, vc);
+                    uint32_t vm[W];
+#pragma unroll
+                    for (int j = 0; j < W / 4; ++j) {
+                        const float4 v4 = lds_f32x4(accrow_s + (uint32_t)(c0 + 4 * j) * 4u);
+                        vm[4 * j] = __float_as_uint(v4.x); vm[4 * j + 1] = __float_as_uint(v4.y);
+                        vm[4 * j + 2] = __float_as_uint(v4.z); vm[4 * j + 3] = __float_as_uint(v4.w);
+                    }
                     uint32_t addr[W];
 #pragma unroll
                     for (int j = 0; j < W / 4; ++j) {
@@ -646,7 +545,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
                     float pre[W];
 #pragma unroll
                     for (int c = 0; c < W; ++c) pre[c] = lds_f32(addr[c]);
-                    tc::tmem_ld_wait();
                     // t[c] = op(pre[c], v[c]) for every column (independent); a column that CONTINUES a segment (rare: most
                     // (target, type) segments hold one edge) then overwrites it with op(t[c-1], v[c]) -- a predicated op, in
                     // column order, so a target's messages are still combined one by one in plan order.  Columns of the other
@@ -654,21 +552,13 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
                     float t[W];
                     constexpr bool ADD = RED == PTGNN_REDUCE_SUM || RED == PTGNN_REDUCE_MEAN;
 #pragma unroll
-                    for (int c = 0; c < W; c += 2) {       // two columns per instruction: Blackwell's packed fp32 FMA / ADD (same rounding)
-                        float2 v = make_float2(__uint_as_float(vm[c]), __uint_as_float(vm[c + 1]));
-                        if (NPROD == 3) {
-                            v = __ffma2_rn(make_float2(__uint_as_float(vc[c]), __uint_as_float(vc[c + 1])), make_float2(1.0f / 2048.0f, 1.0f / 2048.0f), v);
-                        } else {                                   // the autocast Linear's bf16 output
-                            v.x = __bfloat162float(__float2bfloat16_rn(v.x));
-                            v.y = __bfloat162float(__float2bfloat16_rn(v.y));
+                    for (int c = 0; c < W; ++c) {
+                        float v = __uint_as_float(vm[c]);
+                        if (NPROD == 1) {                           // the autocast Linear's bf16 output
+                            v = __bfloat162float(__float2bfloat16_rn(v));
+                            vm[c] = __float_as_uint(v);
                         }
-                        vm[c] = __float_as_uint(v.x); vm[c + 1] = __float_as_uint(v.y);
-                        if (ADD) {
-                            const float2 s2 = __fadd2_rn(make_float2(pre[c], pre[c + 1]), v);
-                            t[c] = s2.x; t[c + 1] = s2.y;
-                        } else {
-                            t[c] = red_op<RED>(pre[c], v.x); t[c + 1] = red_op<RED>(pre[c + 1], v.y);
-                        }
+                        t[c] = ADD ? __fadd_rn(pre[c], v) : red_op<RED>(pre[c], v);
                     }
                     continue_segment<RED>(t[0], acc, __uint_as_float(vm[0]), startw & 1u);
 #pragma unroll
@@ -677,27 +567,19 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
 #pragma unroll
                     for (int c = 0; c < W; ++c) sts_f32_if(addr[c], t[c], storew & (1u << c));
                 }
-                tc::tc_fence_before_sync();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&acc_empty[ab]);
                 tr.mark(22, sg);
                 ++sg;
                 continue;
             }
             // ---- block finished.  Each group writes out ITS half of the rows as soon as its own four warps are done (no waiting for
-            // the other group).  The row loop is specialised at compile time on the output format and on "plain sum" (no mean /
-            // max fix-up / activation / LayerNorm): the generic version executed ~180 instructions per row, 13,600 cycles per block.
+            // the other group).
             tr.mark(23, sg);
-            if (eg == 0) named_bar_sync(EPI_BAR_ID, 128); else named_bar_sync(EPI_BAR_ID + 1, 128);
+            named_bar_sync(EPI_BAR_ID + eg, 128);
             write_out_block<RED>(&p, smem_u32(agg_s), s.blk * p.B, row_lo, row_hi, ew, lane);
-            if (eg == 0) named_bar_sync(EPI_BAR_ID, 128); else named_bar_sync(EPI_BAR_ID + 1, 128);
+            named_bar_sync(EPI_BAR_ID + eg, 128);
             tr.mark(24, sg);
         }
     }
-    tc::tc_fence_before_sync();
-    __syncthreads();
-    tc::tc_fence_after_sync();
-    if (warp == 0) tc::tmem_dealloc<512>(tmem_base);
 }
 
 // =====================================================================================================================
@@ -788,10 +670,10 @@ size_t packed_state_bytes(int nprod, int64_t rows, int K) {
     return nprod == 3 ? ws_slice((size_t)rows * K * 4 + 16, 1) : 0;
 }
 int recommended_block_targets(int64_t num_nodes) {
-    // the largest B <= kMaxBlockTargets (multiple of 8) for which the block count is a whole number of 148-CTA waves or less
+    // the largest B <= kMaxBlockTargets (multiple of 8) for which the block count is a whole number of waves of 132 CTAs (one per H100 SM) or less
     if (num_nodes <= 0) return kMaxBlockTargets;
-    const int64_t waves = ceil_div(num_nodes, (int64_t)kMaxBlockTargets * 148);
-    int64_t B = ceil_div(num_nodes, waves * 148);
+    const int64_t waves = ceil_div(num_nodes, (int64_t)kMaxBlockTargets * 132);
+    int64_t B = ceil_div(num_nodes, waves * 132);
     B = (B + 7) / 8 * 8;
     if (B < 8) B = 8;
     if (B > kMaxBlockTargets) B = kMaxBlockTargets;
@@ -805,8 +687,8 @@ int pack_weights(int nprod, int num_types, int K, int use_target, const float *c
     const int nseg = use_target ? 2 : 1;
     {
         TimedScope timed__(PTGNN_KERNEL_PACK, st);
-        if (nprod == 3) pack_weights_kernel<3><<<148, 256, 0, st>>>(src, num_types, K, nseg, static_cast<uint4 *>(packed), status);
-        else pack_weights_kernel<1><<<148, 256, 0, st>>>(src, num_types, K, nseg, static_cast<uint4 *>(packed), status);
+        if (nprod == 3) pack_weights_kernel<3><<<132, 256, 0, st>>>(src, num_types, K, nseg, static_cast<uint4 *>(packed), status);
+        else pack_weights_kernel<1><<<132, 256, 0, st>>>(src, num_types, K, nseg, static_cast<uint4 *>(packed), status);
     }
     PTGNN_LAUNCHED();
     return PTGNN_OK;
@@ -815,7 +697,7 @@ int pack_weights(int nprod, int num_types, int K, int use_target, const float *c
 int pack_states(const float *h, int64_t rows, int K, void *packed, int32_t *status, cudaStream_t st) {
     if (rows <= 0) return PTGNN_OK;
     const int64_t items = rows * (K / 8);
-    const unsigned grid = (unsigned)(ceil_div(items, 256) < 148 * 8 ? ceil_div(items, 256) : 148 * 8);
+    const unsigned grid = (unsigned)(ceil_div(items, 256) < 132 * 8 ? ceil_div(items, 256) : 132 * 8);
     {
         TimedScope timed__(PTGNN_KERNEL_PACK, st);
         pack_states_kernel<<<grid, 256, 0, st>>>(h, (long long)rows, K, static_cast<uint4 *>(packed), status);
@@ -830,9 +712,9 @@ static int launch_one(const Params &p, cudaStream_t st) {
     const int smem = smem_bytes(p.B);
     // per launch, not once per process: the attribute belongs to the current device's context
     PTGNN_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
-        sms = 148;
+        sms = 132;
     const int grid = p.num_blocks < sms ? p.num_blocks : sms;
     {
         TimedScope timed__(PTGNN_KERNEL_MESSAGE, st);

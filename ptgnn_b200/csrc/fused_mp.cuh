@@ -1,39 +1,36 @@
 // Fused gather -> per-edge-type Linear -> segmented reduce: the aggregation half of a message-passing layer in ONE
-// persistent tcgen05 kernel that never materialises the [E, D] message tensor.
+// persistent wgmma kernel that never materialises the [E, D] message tensor.
 //
 //   reference  ptgnn/neuralmodels/gnn/messagepassing/gatedmessagepassing.py:50-68   (F.embedding + Linear + cat + scatter)
 //              ptgnn/neuralmodels/gnn/messagepassing/mlpmessagepassing.py:82-112
 //              ptgnn/neuralmodels/gnn/messagepassing/abstractmessagepassing.py:38-50 (torch_scatter.scatter)
 //
-// Orientation.  The per-type weight W_t [D = 128, K] is the MMA's A operand (M = D) and lives in TENSOR MEMORY; the
-// gathered node-state rows are the B operand (N = edges of one (target block, edge type) group, any multiple of 16) in
-// shared memory; the accumulator is therefore msg^T: TMEM lane = message feature d, TMEM column = edge.  Two things
-// follow: (1) a group of n edges costs an N = ceil16(n) MMA, not a padded 128-row tile -- (block, type) groups hold a
-// few dozen edges; (2) the reduction over edges of the same target runs ALONG the columns of one lane, i.e. it is a
-// plain sequential loop in the epilogue thread that owns feature d: no shuffles, no atomics, accumulation in the
-// reference's edge order (per target: type-major, then list order), bit-reproducible.
+// Orientation.  The per-type weight W_t [D = 128, K] is the MMA's A operand (M = D, two warpgroups of 64 rows, held in
+// registers); the gathered node-state rows are the B operand (N = 64 edges of one (target block, edge type) sub-group) in
+// shared memory; the accumulator is therefore msg^T: row = message feature d, column = edge.  Two things follow: (1) a
+// group of n edges costs ceil(n / 64) N = 64 MMAs, not a padded 128-row tile -- (block, type) groups hold a few dozen
+// edges; (2) the reduction over edges of the same target runs ALONG the columns of one row: the accumulator goes through a
+// feature-major shared-memory tile and the thread that owns feature d runs a plain sequential loop over it: no shuffles,
+// no atomics, accumulation in the reference's edge order (per target: type-major, then list order), bit-reproducible.
 //
 // Work decomposition.  Targets are cut into blocks of B <= 256 consecutive nodes; the block plan (plan.cu) sorts the
 // edges by (block, type, target).  A CTA owns a block at a time and keeps its aggregate agg_s[B][D] fp32 in shared
 // memory across all edge types, then writes it once (optionally through mean / GELU / LayerNorm: the Mlp layer's
 // pre-dense epilogue).  HBM traffic per layer = gathered rows (L2-resident per graph) + agg once.
 //
-// Arithmetic.  NPROD = 1: bf16 states and weights, one kind::f16 MMA per K-step, fp32 accumulation (the reference under
+// Arithmetic.  NPROD = 1: bf16 states and weights, one bf16 MMA per K-step, fp32 accumulation (the reference under
 // torch.autocast(bfloat16); each message is rounded to bf16 before the fp32 reduction like the autocast Linear's
 // output).  NPROD = 3: fp32-exact "3xFP16": every fp32 value x is carried as two fp16 numbers, hi = rn(x) and
 // lo' = rn((x - hi) * 2^11) -- 22 significant bits, absolute error <= 2^-36 for tiny values -- and
-// x*w ~= hi*hi + 2^-11 (hi*lo' + lo'*hi): three kind::f16 MMAs per K-step (half the tensor time of 3xTF32), the two
+// x*w ~= hi*hi + 2^-11 (hi*lo' + lo'*hi): three f16 MMAs per K-step (half the tensor time of 3xTF32), the two
 // small products in a separate correction accumulator (tensor-core accumulation truncates).  |x| >= 65504 cannot be
 // represented: the packing kernels raise a status flag and the host raises (PTGNN_B200_FP32_MODE=tf32 selects the
 // unfused 3xTF32 kernels).
 //
-// Roles (16 warps):  0-3 and 8-11 EPILOGUE, two warpgroups: thread d <-> TMEM lane d; group 0 takes the columns whose target
-//   lies in the lower half of the block, group 1 the upper half (disjoint agg_s rows, no synchronisation between them) |
-//   4 MMA issuer | 5-6 ROW GATHERERS (16-byte cp.async into a 3-slot ring, SWIZZLE_128B K-major) |
-//   7 SCHEDULER (block -> group offsets table ring) |
-//   12-15 WEIGHT LOADERS (global -> registers -> tcgen05.st, TMEM A buffers, double buffered; setmaxnreg gives them the
-//   registers warps 4-7 release -- ptxas only extends a role's budget when that role is the LAST branch of the kernel).
-// TMEM (512 columns): [0,256) two weight buffers | [256,512) two accumulator sets (main | correction).
+// Roles (12 warps):  0-3 and 4-7 CONSUMERS, two warpgroups: MMAs for features [0,64) / [64,128), then the epilogue over all
+//   128 features -- group 0 takes the columns whose target lies in the lower half of the block, group 1 the upper half
+//   (disjoint agg_s rows) | 8-9 ROW GATHERERS (16-byte cp.async into a 3-slot ring, SWIZZLE_128B K-major) |
+//   10 SCHEDULER (block -> group offsets table ring).
 #pragma once
 #include "common.cuh"
 
@@ -41,7 +38,7 @@ namespace ptgnn {
 namespace fused {
 
 constexpr int kD = 128;                 // message dimension handled by this kernel (= MMA M)
-constexpr int kMaxBlockTargets = 240;   // agg_s = B * 512 bytes of shared memory
+constexpr int kMaxBlockTargets = 176;   // agg_s = B * 512 bytes of shared memory
 
 struct Epilogue {                       // applied to the aggregated row at write-out (Mlp layers), else act = NONE / ln = null
     int act;
@@ -50,7 +47,7 @@ struct Epilogue {                       // applied to the aggregated row at writ
 };
 
 bool supported(int nprod, int K, int D, int use_target);
-// bytes of the packed edge weights (TMEM-friendly layout), of one packed state row, and of the packed-state scratch
+// bytes of the packed edge weights (coalesced per-row layout), of one packed state row, and of the packed-state scratch
 size_t packed_weight_bytes(int nprod, int num_types, int K, int use_target);
 size_t packed_state_bytes(int nprod, int64_t rows, int K);
 int recommended_block_targets(int64_t num_nodes);

@@ -62,7 +62,7 @@ extern "C" int ptgnn_b200_gru_gate_grads_f32(const float *gi, const float *gh, c
     const long long blocks = (total + 255) / 256;
     {
         TimedScope timed__(PTGNN_KERNEL_GRU, st);
-        gru_gate_grads_kernel<<<(unsigned)(blocks < 148 * 16 ? blocks : 148 * 16), 256, 0, st>>>(gi, gh, h, grad_out, num_nodes, state_dim, d_gi, d_gh,
+        gru_gate_grads_kernel<<<(unsigned)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, st>>>(gi, gh, h, grad_out, num_nodes, state_dim, d_gi, d_gh,
                                                                                                  d_h_direct);
     }
     PTGNN_LAUNCHED();
@@ -114,7 +114,7 @@ extern "C" int ptgnn_b200_gather_split_f16(const float *x, const int32_t *index,
     const long long blocks = (total + 255) / 256;
     {
         TimedScope timed__(PTGNN_KERNEL_PACK, st);
-        gather_split_kernel<<<(unsigned)(blocks < 148 * 16 ? blocks : 148 * 16), 256, 0, st>>>(x, index, rows_out, cols, scale, static_cast<uint4 *>(hi),
+        gather_split_kernel<<<(unsigned)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, st>>>(x, index, rows_out, cols, scale, static_cast<uint4 *>(hi),
                                                                                                static_cast<uint4 *>(lo));
     }
     PTGNN_LAUNCHED();

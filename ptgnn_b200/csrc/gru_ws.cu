@@ -1,10 +1,9 @@
 // nn.GRUCell update, weights-stationary:  h' = GRUCell(agg, h)   (reference gatedmessagepassing.py:69)
 //
 // Why a second GRU kernel.  The round-1 pipeline (tc_pipeline.cuh, GruPolicy) walks (row tile, 32-hidden-unit block) tiles in
-// row-major order: every tile streams its gate-weight block again and every row tile is fetched once per block -- ~2.4 GB of
-// L2 -> SM traffic per launch at config 2, which is what bounds it (the L2 fabric delivers ~12 TB/s chip-wide), not the tensor
-// pipe.  Here a CTA keeps ONE hidden-unit block for its whole life: its gate weights are loaded into shared memory once and
-// stay (B operand of every MMA), and only the node rows stream through a TMA ring (A operand).  L2 traffic drops to the row
+// row-major order: every tile streams its gate-weight block again and every row tile is fetched once per block -- L2 -> SM
+// traffic, not the tensor pipe, is what bounds it.  Here a CTA keeps ONE hidden-unit block for its whole life: its gate
+// weights are loaded into shared memory once and stay (B operand of every MMA), and only the node rows stream through a TMA ring (A operand).  L2 traffic drops to the row
 // tiles alone.
 //
 // Arithmetic (same two modes as the fused aggregation kernel, fused_mp.cuh):
@@ -13,12 +12,12 @@
 //              hi*hi -> main accumulator, hi*lo' + lo'*hi -> correction accumulator (scaled by 2^11), fp32 h for the blend.
 //   NPROD = 1  bf16 operands (the reference under torch.autocast), fp32 accumulation and gate math.
 //
-// Accumulator columns of a tile (128 rows x 32 hidden units): [0,32) i_n | [32,64) r | [64,96) z | [96,128) h_n.
-//   state segment first: P2 = [0; W_hr; W_hz; W_hn] (128 rows) -- its first K-step runs N = 128 and overwrites all columns
-//   (the zero block initialises i_n), later K-steps N = 96 over rows 32..127; then the aggregate segment:
-//   P1 = [W_in; W_ir; W_iz] (96 rows) accumulates into columns 0..95.
-// Roles: warp 0 TMA producer | warp 1 MMA issuer | warps 4-11 epilogue, two sets of four on alternate tiles (TMEM: two
-// accumulator sets x (main 128 | correction 128) columns).
+// Accumulator blocks of a tile (128 rows x 32 hidden units, one 32-column wgmma block per gate): 0 i_n | 1 r | 2 z | 3 h_n,
+// zeroed at the start of the tile.  State segment: P2 = [0; W_hr; W_hz; W_hn] (128 rows), rows 32 j .. -> block j = 1..3;
+// aggregate segment: P1 = [W_in; W_ir; W_iz] (96 rows), rows 32 j .. -> block j = 0..2.
+// Roles: warp 0 TMA producer | warps 4-11 two consumer warpgroups (tile rows [0,64) / [64,128)): wgmma from the ring (A) and
+// the resident weights (B), then the gate math and the stores straight from the accumulator registers -- every gate block
+// has the same fragment layout, so a thread holds all four gates of each (row, hidden unit) it owns.
 #include "gru_ws.cuh"
 
 #include <cuda.h>
@@ -36,7 +35,8 @@ using tc::mbar_wait;
 
 constexpr int NUM_THREADS = 12 * 32;
 constexpr int TILE_M = 128;
-constexpr int IO_REGS = 64, EPI_REGS = 216;          // (64 + 216 + 216) * 128 = 63488
+constexpr int IO_REGS = 56, CONSUMER_REGS = 224;     // (56 + 2 * 224) * 128 = 64512 = 384 x 168, the launch allocation
+static_assert(IO_REGS + 2 * CONSUMER_REGS <= 3 * 168, "register budgets exceed the launch allocation");
 
 struct Params {
     CUtensorMap map_agg, map_h;          // A: [N, NPART * K] 16-bit, box {64, 128}
@@ -66,7 +66,7 @@ template <int NPROD>
 __global__ void __launch_bounds__(NUM_THREADS, 1) gru_ws_kernel(const __grid_constant__ Params p) {
     using G = Geometry<NPROD>;
     constexpr int NPART = G::NPART;
-    constexpr uint32_t FMT = NPROD == 3 ? 0u /*F16*/ : tc::FMT_BF16;
+    constexpr bool BF16 = NPROD == 1;
     extern __shared__ unsigned char smem_raw[];
     unsigned char *ring = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     unsigned char *bres = ring + G::RING_BYTES;                                   // resident weights: P2 tiles, then P1 tiles
@@ -74,24 +74,18 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gru_ws_kernel(const __grid_con
     unsigned char *p1res = bres + NPART * kch_h * G::P2_TILE;
     float4 *bias_s = reinterpret_cast<float4 *>(bres + G::b_bytes(p.H, p.D));
     uint64_t *bars = reinterpret_cast<uint64_t *>(reinterpret_cast<unsigned char *>(bias_s) + p.H * 16);
-    uint64_t *a_full = bars, *a_empty = bars + G::NUM_SLOTS, *acc_full = bars + 2 * G::NUM_SLOTS, *acc_empty = bars + 2 * G::NUM_SLOTS + 2;
-    uint64_t *b_full = bars + 2 * G::NUM_SLOTS + 4;
-    uint32_t *tmem_base_smem = reinterpret_cast<uint32_t *>(bars + 2 * G::NUM_SLOTS + 5);
+    uint64_t *a_full = bars, *a_empty = bars + G::NUM_SLOTS;
+    uint64_t *b_full = bars + 2 * G::NUM_SLOTS;
 
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
     const int lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
-        for (int s = 0; s < G::NUM_SLOTS; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(&acc_full[a], 1); mbar_init(&acc_empty[a], 4); }
+        for (int s = 0; s < G::NUM_SLOTS; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 8); }
         mbar_init(b_full, 1);
         tc::mbar_init_fence();
     }
-    if (warp == 2) tc::tmem_alloc<512>(tmem_base_smem);
     for (int j = threadIdx.x; j < p.H; j += NUM_THREADS) bias_s[j] = p.bias4[j];
-    tc::tc_fence_before_sync();
     __syncthreads();
-    tc::tc_fence_after_sync();
-    const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_base_smem, 0);
 
     // this CTA's hidden-unit block and its row tiles
     const int jb = blockIdx.x % p.n_jb;
@@ -130,200 +124,116 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gru_ws_kernel(const __grid_con
                     __syncwarp();
                 }
             }
-        } else if (warp == 1) {
-            // ============================================ MMA ISSUER ============================================
-            const bool leader = tc::elect_one();
-            mbar_wait(b_full, 0);
-            tc::tc_fence_after_sync();
-            const uint32_t idesc128 = tc::make_instr_desc(FMT, TILE_M, 128), idesc96 = tc::make_instr_desc(FMT, TILE_M, 96);
-            const uint32_t b2_addr = smem_u32(bres), b1_addr = smem_u32(p1res);
-            uint32_t c = 0, tcount = 0;
-            for (int rb = rb0; rb < p.n_rb; rb += rb_stride, ++tcount) {
-                const uint32_t set = tcount & 1;
-                mbar_wait(&acc_empty[set], ((tcount >> 1) & 1) ^ 1);
-                tc::tc_fence_after_sync();
-                const uint32_t d_main = tmem_base + set * 256, d_corr = d_main + 128;
-                for (int ch = 0; ch < chunks_per_tile; ++ch, ++c) {
-                    const uint32_t slot = c % G::NUM_SLOTS;
-                    mbar_wait(&a_full[slot], (c / G::NUM_SLOTS) & 1);
-                    tc::tc_fence_after_sync();
-                    const bool state_seg = ch < kch_h;
-                    const int kc = state_seg ? ch : ch - kch_h;
-                    const uint32_t a_addr = smem_u32(ring + slot * G::SLOT_BYTES);
-                    const uint64_t a_hi = tc::make_smem_desc_sw128(a_addr), a_lo = tc::make_smem_desc_sw128(a_addr + G::A_TILE);
-                    // B tile of this chunk: state segment = P2 (128 rows), aggregate segment = P1 (96 rows)
-                    const uint32_t b_hi_addr = state_seg ? b2_addr + kc * G::P2_TILE : b1_addr + kc * G::P1_TILE;
-                    const uint32_t b_lo_addr = state_seg ? b2_addr + (kch_h + kc) * G::P2_TILE : b1_addr + (kch_d + kc) * G::P1_TILE;
-#pragma unroll
-                    for (int ks = 0; ks < 4; ++ks) {
-                        const bool first = ch == 0 && ks == 0;            // overwrites every accumulator column (zero block -> i_n)
-                        const uint32_t row_off = (state_seg && !first) ? 32u * 128u : 0u;   // skip P2's zero block after the first step
-                        const uint32_t col_off = (state_seg && !first) ? 32u : 0u;
-                        const uint32_t idesc = first ? idesc128 : idesc96;
-                        const uint64_t b_hi = tc::make_smem_desc_sw128(b_hi_addr + row_off) + ks * 2;
-                        const uint32_t acc = first ? 0u : 1u;
-                        if (NPROD == 3) {
-                            const uint64_t b_lo = tc::make_smem_desc_sw128(b_lo_addr + row_off) + ks * 2;
-                            if (leader) {
-                                tc::mma_bf16_ss(d_main + col_off, a_hi + ks * 2, b_hi, idesc, acc);
-                                tc::mma_bf16_ss(d_corr + col_off, a_hi + ks * 2, b_lo, idesc, acc);
-                                tc::mma_bf16_ss(d_corr + col_off, a_lo + ks * 2, b_hi, idesc, 1u);
-                            }
-                        } else {
-                            if (leader) tc::mma_bf16_ss(d_main + col_off, a_hi + ks * 2, b_hi, idesc, acc);
-                        }
-                    }
-                    if (leader) tc::mma_commit(&a_empty[slot]);
-                    __syncwarp();
-                }
-                if (leader) tc::mma_commit(&acc_full[set]);
-                __syncwarp();
-            }
         }
     } else {
-        // ============================================ EPILOGUE ============================================
-        // Set s (four warps, one per TMEM lane quarter) takes tiles s, s + 2, ...: a lane owns one node row and, in two passes,
-        // 16 hidden units each: drain main (+ 2^-11 correction), gate math, blend with h, store 64 (32) contiguous bytes.
-        tc::reg_alloc<EPI_REGS>();
-        const int ew = warp - 4, quarter = warp & 3, set = ew >> 2;
-        const uint32_t tmem_lane = tmem_base + ((uint32_t)(quarter * 32) << 16) + set * 256;
-        const int rb_step = 2 * rb_stride;
-        struct Pre { long long off; float4 f[8]; };      // fp32: 2 passes x 16 floats; bf16: 2 passes x 32 bytes in f[0..3]
-        auto prefetch = [&](int rb, Pre &pre) {
-            const int row = rb * TILE_M + quarter * 32 + lane;
-            pre.off = row < p.num_nodes ? (long long)row * p.H + jb * 32 : -1;
+        // ============================================ CONSUMERS ============================================
+        tc::reg_alloc<CONSUMER_REGS>();
+        const int cw = warp - 4, wg = cw >> 2, wi = cw & 3;
+        const int gq = lane >> 2, tq = lane & 3;
+        mbar_wait(b_full, 0);
+        const uint32_t b2_addr = smem_u32(bres), b1_addr = smem_u32(p1res);
+        uint32_t c = 0;
+        for (int rb = rb0; rb < p.n_rb; rb += rb_stride) {
+            float acc_m[4][16], acc_c[4][16];
 #pragma unroll
-            for (int i = 0; i < 8; ++i) pre.f[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (pre.off >= 0) {
-                if (NPROD == 3) {
-                    const float4 *src = reinterpret_cast<const float4 *>(p.h32 + pre.off);
+            for (int b = 0; b < 4; ++b)
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) pre.f[i] = __ldg(src + i);
-                } else {
-                    const float4 *src = reinterpret_cast<const float4 *>(p.h16 + pre.off);
+                for (int i = 0; i < 16; ++i) { acc_m[b][i] = 0.0f; acc_c[b][i] = 0.0f; }
+            for (int ch = 0; ch < chunks_per_tile; ++ch, ++c) {
+                const uint32_t slot = c % G::NUM_SLOTS;
+                mbar_wait(&a_full[slot], (c / G::NUM_SLOTS) & 1);
+                const bool state_seg = ch < kch_h;
+                const int kc = state_seg ? ch : ch - kch_h;
+                const uint32_t a_addr = smem_u32(ring + slot * G::SLOT_BYTES) + wg * 64 * 128;
+                const uint64_t a_hi = tc::make_smem_desc_sw128(a_addr), a_lo = tc::make_smem_desc_sw128(a_addr + G::A_TILE);
+                // B tile of this chunk: state segment = P2 (blocks 1..3), aggregate segment = P1 (blocks 0..2)
+                const uint32_t b_hi_addr = state_seg ? b2_addr + kc * G::P2_TILE : b1_addr + kc * G::P1_TILE;
+                const uint32_t b_lo_addr = state_seg ? b2_addr + (kch_h + kc) * G::P2_TILE : b1_addr + (kch_d + kc) * G::P1_TILE;
+                const int jlo = state_seg ? 1 : 0;
+                tc::wgmma_fence();
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) pre.f[i] = __ldg(src + i);
-                }
-            }
-        };
-        Pre pre, pre_next;
-        int rb = rb0 + set * rb_stride;
-        if (rb < p.n_rb) prefetch(rb, pre);
-        for (uint32_t use = 0; rb < p.n_rb; rb += rb_step, ++use) {
-            const int nxt = rb + rb_step;
-            if (nxt < p.n_rb) prefetch(nxt, pre_next);
-            mbar_wait(&acc_full[set], use & 1);
-            tc::tc_fence_after_sync();
+                for (int j = 0; j < 4; ++j) {
+                    if (j >= jlo && j < jlo + 3) {
+                        const uint64_t b_hi = tc::make_smem_desc_sw128(b_hi_addr + 32 * j * 128);
+                        const uint64_t b_lo = tc::make_smem_desc_sw128(b_lo_addr + 32 * j * 128);
 #pragma unroll
-            for (int half = 0; half < 2; ++half) {
-                float acc[64];
-                {
-                    uint32_t m[4][16];
-#pragma unroll
-                    for (int g = 0; g < 4; ++g) tc::tmem_ld_16cols_async(tmem_lane + 32 * g + 16 * half, m[g]);
-                    if (NPROD == 3) {
-                        uint32_t cc[4][16];
-#pragma unroll
-                        for (int g = 0; g < 4; ++g) tc::tmem_ld_16cols_async(tmem_lane + 128 + 32 * g + 16 * half, cc[g]);
-                        tc::tmem_ld_wait();
-#pragma unroll
-                        for (int g = 0; g < 4; ++g)
-#pragma unroll
-                            for (int i = 0; i < 16; ++i)
-                                acc[16 * g + i] = fmaf(__uint_as_float(cc[g][i]), 1.0f / 2048.0f, __uint_as_float(m[g][i]));
-                    } else {
-                        tc::tmem_ld_wait();
-#pragma unroll
-                        for (int g = 0; g < 4; ++g)
-#pragma unroll
-                            for (int i = 0; i < 16; ++i) acc[16 * g + i] = __uint_as_float(m[g][i]);
-                    }
-                }
-                if (half == 1) {
-                    tc::tc_fence_before_sync();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&acc_empty[set]);      // the next tile's MMAs may overwrite this set
-                }
-                const int j0 = jb * 32 + 16 * half;
-                float hv[16];
-                if (NPROD == 3) {
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const float4 v = pre.f[4 * half + i];
-                        hv[4 * i] = v.x; hv[4 * i + 1] = v.y; hv[4 * i + 2] = v.z; hv[4 * i + 3] = v.w;
-                    }
-                } else {
-#pragma unroll
-                    for (int i = 0; i < 2; ++i) {
-                        const float4 v = pre.f[2 * half + i];
-                        const uint32_t w[4] = {__float_as_uint(v.x), __float_as_uint(v.y), __float_as_uint(v.z), __float_as_uint(v.w)};
-#pragma unroll
-                        for (int u = 0; u < 4; ++u) {
-                            const __nv_bfloat162 hp = *reinterpret_cast<const __nv_bfloat162 *>(&w[u]);
-                            hv[8 * i + 2 * u] = __low2float(hp); hv[8 * i + 2 * u + 1] = __high2float(hp);
-                        }
-                    }
-                }
-                float o[16];
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    const float4 b = bias_s[j0 + i];
-                    if (NPROD == 3) {
-                        const float rr = sigmoid_fast(acc[16 + i] + b.x);
-                        const float zz = sigmoid_fast(acc[32 + i] + b.y);
-                        const float nn = tanh_fast(acc[i] + b.z + rr * (acc[48 + i] + b.w));
-                        o[i] = (1.0f - zz) * nn + zz * hv[i];
-                    } else {
-                        const float rr = sigmoid_mufu(acc[16 + i] + b.x);
-                        const float zz = sigmoid_mufu(acc[32 + i] + b.y);
-                        const float nn = tanh_mufu(fmaf(rr, acc[48 + i] + b.w, acc[i] + b.z));
-                        o[i] = fmaf(zz, hv[i] - nn, nn);
-                    }
-                }
-                if (pre.off >= 0) {
-                    if (NPROD == 3) {
-                        float4 *dst = reinterpret_cast<float4 *>(static_cast<float *>(p.out) + pre.off + 16 * half);
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) dst[i] = make_float4(o[4 * i], o[4 * i + 1], o[4 * i + 2], o[4 * i + 3]);
-                        if (p.out_packed != nullptr) {      // same split as pack_states: hi = rn16(x), lo' = rn16((x - hi) * 2^11)
-                            uint32_t hw[8], lw[8];
-                            float big = 0.0f;
-#pragma unroll
-                            for (int i = 0; i < 8; ++i) {
-                                const __half2 h2 = __floats2half2_rn(o[2 * i], o[2 * i + 1]);
-                                const float2 f2 = __half22float2(h2);
-                                const __half2 l2 = __floats2half2_rn((o[2 * i] - f2.x) * 2048.0f, (o[2 * i + 1] - f2.y) * 2048.0f);
-                                hw[i] = *reinterpret_cast<const uint32_t *>(&h2);
-                                lw[i] = *reinterpret_cast<const uint32_t *>(&l2);
-                                big = fmaxf(big, fmaxf(fabsf(o[2 * i]), fabsf(o[2 * i + 1])));
+                        for (int ks = 0; ks < 4; ++ks) {
+                            tc::wgmma_16_ss_n32<BF16>(acc_m[j], a_hi + ks * 2, b_hi + ks * 2);
+                            if (NPROD == 3) {
+                                // x * w ~= hi*hi (main) + 2^-11 (hi*lo' + lo'*hi) (correction accumulator)
+                                tc::wgmma_16_ss_n32<BF16>(acc_c[j], a_hi + ks * 2, b_lo + ks * 2);
+                                tc::wgmma_16_ss_n32<BF16>(acc_c[j], a_lo + ks * 2, b_hi + ks * 2);
                             }
-                            // row r = (off - 32 jb) / H holds 2H halfs: hi at [0, H), lo' at [H, 2H)
-                            __half *rowp = p.out_packed + 2 * (pre.off - jb * 32) + jb * 32 + 16 * half;
-                            uint4 *dh = reinterpret_cast<uint4 *>(rowp), *dl = reinterpret_cast<uint4 *>(rowp + p.H);
-                            dh[0] = make_uint4(hw[0], hw[1], hw[2], hw[3]); dh[1] = make_uint4(hw[4], hw[5], hw[6], hw[7]);
-                            dl[0] = make_uint4(lw[0], lw[1], lw[2], lw[3]); dl[1] = make_uint4(lw[4], lw[5], lw[6], lw[7]);
-                            if (!(big < 65504.0f) && p.status != nullptr) *reinterpret_cast<volatile int32_t *>(p.status) = 1;
                         }
-                    } else {
-                        uint32_t w[8];
-#pragma unroll
-                        for (int i = 0; i < 8; ++i) {
-                            __nv_bfloat162 v = __floats2bfloat162_rn(o[2 * i], o[2 * i + 1]);
-                            w[i] = *reinterpret_cast<uint32_t *>(&v);
-                        }
-                        uint4 *dst = reinterpret_cast<uint4 *>(static_cast<__nv_bfloat16 *>(p.out) + pre.off + 16 * half);
-                        dst[0] = make_uint4(w[0], w[1], w[2], w[3]);
-                        dst[1] = make_uint4(w[4], w[5], w[6], w[7]);
                     }
                 }
+                tc::wgmma_commit();
+                tc::wgmma_wait<0>();
+#pragma unroll
+                for (int j = 0; j < 4; ++j) { tc::fence_acc(acc_m[j]); tc::fence_acc(acc_c[j]); }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&a_empty[slot]);
             }
-            pre = pre_next;
+            // ---- gate math straight from the fragments: register 4 i + 2 rh + e of every block = row (gq + 8 rh),
+            //      hidden unit 8 i + 2 tq + e of the block
+#pragma unroll
+            for (int rh = 0; rh < 2; ++rh) {
+                const int row = rb * TILE_M + 64 * wg + 16 * wi + gq + 8 * rh;
+                if (row >= p.num_nodes) continue;
+                const long long off = (long long)row * p.H + jb * 32;
+                float big = 0.0f;
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const int u = 8 * i + 2 * tq;
+                    float hv[2];
+                    if (NPROD == 3) {
+                        const float2 h2 = __ldg(reinterpret_cast<const float2 *>(p.h32 + off + u));
+                        hv[0] = h2.x; hv[1] = h2.y;
+                    } else {
+                        const __nv_bfloat162 h2 = *reinterpret_cast<const __nv_bfloat162 *>(p.h16 + off + u);
+                        hv[0] = __low2float(h2); hv[1] = __high2float(h2);
+                    }
+                    float o[2];
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int r = 4 * i + 2 * rh + e;
+                        float a[4];
+#pragma unroll
+                        for (int gt = 0; gt < 4; ++gt) a[gt] = NPROD == 3 ? fmaf(acc_c[gt][r], 1.0f / 2048.0f, acc_m[gt][r]) : acc_m[gt][r];
+                        const float4 b = bias_s[jb * 32 + u + e];
+                        if (NPROD == 3) {
+                            const float rr = sigmoid_fast(a[1] + b.x);
+                            const float zz = sigmoid_fast(a[2] + b.y);
+                            const float nn = tanh_fast(a[0] + b.z + rr * (a[3] + b.w));
+                            o[e] = (1.0f - zz) * nn + zz * hv[e];
+                        } else {
+                            const float rr = sigmoid_mufu(a[1] + b.x);
+                            const float zz = sigmoid_mufu(a[2] + b.y);
+                            const float nn = tanh_mufu(fmaf(rr, a[3] + b.w, a[0] + b.z));
+                            o[e] = fmaf(zz, hv[e] - nn, nn);
+                        }
+                    }
+                    if (NPROD == 3) {
+                        *reinterpret_cast<float2 *>(static_cast<float *>(p.out) + off + u) = make_float2(o[0], o[1]);
+                        if (p.out_packed != nullptr) {      // same split as pack_states: hi = rn16(x), lo' = rn16((x - hi) * 2^11)
+                            const __half2 h2 = __floats2half2_rn(o[0], o[1]);
+                            const float2 f2 = __half22float2(h2);
+                            const __half2 l2 = __floats2half2_rn((o[0] - f2.x) * 2048.0f, (o[1] - f2.y) * 2048.0f);
+                            // row r holds 2H halfs: hi at [0, H), lo' at [H, 2H)
+                            __half *rowp = p.out_packed + 2 * (long long)row * p.H + jb * 32 + u;
+                            *reinterpret_cast<__half2 *>(rowp) = h2;
+                            *reinterpret_cast<__half2 *>(rowp + p.H) = l2;
+                            big = fmaxf(big, fmaxf(fabsf(o[0]), fabsf(o[1])));
+                        }
+                    } else {
+                        *reinterpret_cast<__nv_bfloat162 *>(static_cast<__nv_bfloat16 *>(p.out) + off + u) = __floats2bfloat162_rn(o[0], o[1]);
+                    }
+                }
+                if (NPROD == 3 && p.out_packed != nullptr && !(big < 65504.0f) && p.status != nullptr)
+                    *reinterpret_cast<volatile int32_t *>(p.status) = 1;
+            }
         }
     }
-    tc::tc_fence_before_sync();
-    __syncthreads();
-    tc::tc_fence_after_sync();
-    if (warp == 2) tc::tmem_dealloc<512>(tmem_base);
 }
 
 // =====================================================================================================================
@@ -406,7 +316,7 @@ static int make_map16(CUtensorMap *map, const void *base, uint64_t rows, uint64_
 bool supported(int nprod, int H, int D) {
     if (H % 64 != 0 || D % 64 != 0 || H < 64 || D < 64) return false;
     const int smem = nprod == 3 ? Geometry<3>::smem_bytes(H, D) : Geometry<1>::smem_bytes(H, D);
-    return smem <= 232448 && 148 / (H / 32) >= 1;
+    return smem <= 232448 && 132 / (H / 32) >= 1;
 }
 size_t pack_bytes(int nprod, int H, int D) {
     const int npart = nprod == 3 ? 2 : 1;
@@ -426,8 +336,8 @@ int pack(int nprod, int H, int D, const float *w_ih, const float *w_hh, const fl
     pack_layout(nprod, H, D, static_cast<char *>(packed), p1, p2, bias4);
     {
         TimedScope timed__(PTGNN_KERNEL_PACK, st);
-        if (nprod == 3) pack_gru_ws_kernel<3><<<148, 256, 0, st>>>(w_ih, w_hh, b_ih, b_hh, H, D, p1, p2, bias4);
-        else pack_gru_ws_kernel<1><<<148, 256, 0, st>>>(w_ih, w_hh, b_ih, b_hh, H, D, p1, p2, bias4);
+        if (nprod == 3) pack_gru_ws_kernel<3><<<132, 256, 0, st>>>(w_ih, w_hh, b_ih, b_hh, H, D, p1, p2, bias4);
+        else pack_gru_ws_kernel<1><<<132, 256, 0, st>>>(w_ih, w_hh, b_ih, b_hh, H, D, p1, p2, bias4);
     }
     PTGNN_LAUNCHED();
     return PTGNN_OK;
@@ -453,8 +363,8 @@ int update(int nprod, const void *agg_rows, const void *h_rows, const void *h_pl
     p.h32 = static_cast<const float *>(h_plain); p.h16 = static_cast<const __nv_bfloat16 *>(h_plain);
     p.bias4 = bias4; p.out = out; p.out_packed = static_cast<__half *>(out_packed); p.status = status; p.num_nodes = (int)num_nodes; p.H = H; p.D = D; p.n_jb = (int)n_jb;
     p.n_rb = (int)ceil_div(num_nodes, TILE_M);
-    int dev = 0, sms = 148;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+    int dev = 0, sms = 132;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
     int groups = sms / (int)n_jb;                       // CTAs per hidden-unit block
     if (groups > p.n_rb) groups = p.n_rb;
     if (groups < 1) groups = 1;

@@ -1,4 +1,4 @@
-// GatedMessagePassingLayer / MlpMessagePassingLayer forward on B200 (fp32-exact path).
+// GatedMessagePassingLayer / MlpMessagePassingLayer forward on H100 (fp32-exact path).
 //
 //   reference ptgnn/neuralmodels/gnn/messagepassing/gatedmessagepassing.py:37-69
 //   reference ptgnn/neuralmodels/gnn/messagepassing/mlpmessagepassing.py:68-117  (+ ptgnn/neuralmodels/mlp.py:79-80)
@@ -282,7 +282,7 @@ static bool tc_enabled() {
 }
 
 // `fused` layouts (block plan given, dims supported): no [E, D] message buffer; instead the packed (hi | lo') fp16 copy
-// of the source states (Ns rows) and the TMEM-layout edge weights of the fused kernel.
+// of the source states (Ns rows) and the packed edge weights of the fused kernel.
 // out = act(y W^T + b): tensor cores (3xTF32) when the dims fit the tiles, FFMA tiles otherwise.  scratch >= tc::dense_split_bytes.
 static int dense_any(const float *y, int64_t rows, int D, const float *W, const float *bias, int out_dim, int act, float *out,
                      void *scratch, cudaStream_t st, bool pack = true) {
@@ -491,7 +491,7 @@ static int gated_forward_impl(const float *node_states, const float *gather_stat
     }
     {
         TimedScope timed__(PTGNN_KERNEL_PACK, st);
-        pack_gru_weights_kernel<<<148, 256, 0, st>>>(gru_w_ih, gru_w_hh, H, D, P1, P2);
+        pack_gru_weights_kernel<<<132, 256, 0, st>>>(gru_w_ih, gru_w_hh, H, D, P1, P2);
     }
     PTGNN_LAUNCHED();
     using Tile = GemmTile<6>;
@@ -866,7 +866,7 @@ extern "C" int ptgnn_b200_grucell_f32(const float *input, const float *hidden, i
     float *P1 = reinterpret_cast<float *>(ws), *P2 = reinterpret_cast<float *>(ws + o1);
     {
         TimedScope timed__(PTGNN_KERNEL_PACK, st);
-        pack_gru_weights_kernel<<<148, 256, 0, st>>>(w_ih, w_hh, H, D, P1, P2);
+        pack_gru_weights_kernel<<<132, 256, 0, st>>>(w_ih, w_hh, H, D, P1, P2);
     }
     PTGNN_LAUNCHED();
     using Tile = GemmTile<6>;

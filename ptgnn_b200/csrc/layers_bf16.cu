@@ -119,11 +119,11 @@ struct MsgPolicyB {
         return seg == 0 ? p.src32[e] : p.tgt32[e];
     }
     __device__ static int mma_groups(const Params &, const Tile &ti, int seg, MmaGroup (&g)[2]) {
-        g[0] = MmaGroup{ti.b_rows, 0, 0, seg == 0};
+        g[0] = MmaGroup{ti.b_rows, 0, 0};
         return 1;
     }
-    __device__ static void drain(const Params &, const Tile &ti, uint32_t tmem_lane, int half, float (&acc)[64]) {
-        drain_2x32(tmem_lane, 64 * half, ti.b_rows, acc);
+    __device__ static void drain(const Params &, const Tile &ti, const float *acc_row, int half, float (&acc)[64]) {
+        drain_2x32(acc_row, 64 * half, ti.b_rows, acc);
     }
     // only the raw load is issued a tile ahead: arithmetic on the loaded value would stall the in-order issue right there
     struct Pre { int32_t pos; };
@@ -176,11 +176,11 @@ struct GruPolicyB {
     }
     __device__ static int gather_row(const Params &, const Tile &, int, int) { return -1; }
     __device__ static int mma_groups(const Params &, const Tile &, int seg, MmaGroup (&g)[2]) {
-        g[0] = MmaGroup{128, 0, 0, seg == 0};
+        g[0] = MmaGroup{128, 0, 0};
         return 1;
     }
-    __device__ static void drain(const Params &, const Tile &, uint32_t tmem_lane, int half, float (&acc)[64]) {
-        drain_4x16(tmem_lane, 16 * half, acc);
+    __device__ static void drain(const Params &, const Tile &, const float *acc_row, int half, float (&acc)[64]) {
+        drain_4x16(acc_row, 16 * half, acc);
     }
     // a lane owns one node row and 16 hidden units of it: 32 bytes (one sector) of h in, 32 bytes of h' out
     struct Pre { long long off; uint4 h0, h1; };
@@ -256,11 +256,11 @@ struct DensePolicyB {
     }
     __device__ static int gather_row(const Params &, const Tile &, int, int) { return -1; }
     __device__ static int mma_groups(const Params &, const Tile &ti, int, MmaGroup (&g)[2]) {
-        g[0] = MmaGroup{ti.b_rows, 0, 0, true};
+        g[0] = MmaGroup{ti.b_rows, 0, 0};
         return 1;
     }
-    __device__ static void drain(const Params &, const Tile &ti, uint32_t tmem_lane, int half, float (&acc)[64]) {
-        drain_2x32(tmem_lane, 64 * half, ti.b_rows, acc);
+    __device__ static void drain(const Params &, const Tile &ti, const float *acc_row, int half, float (&acc)[64]) {
+        drain_2x32(acc_row, 64 * half, ti.b_rows, acc);
     }
     struct Pre { long long row_off; };     // 4-byte words of the bf16 output (no global load needed)
     __device__ static void prefetch(const Params &p, const Tile &ti, int quarter, int, int lane, Pre &pre) {
@@ -442,7 +442,7 @@ static int debug_bits() {
 }
 static int sm_count() {   // of the CURRENT device: a process may drive several GPUs (nothing cached across devices)
     int dev = 0, n = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     return n;
 }
 template <class Policy>
@@ -548,7 +548,7 @@ static int gated_forward_bf16_impl(const uint16_t *node_states, const uint16_t *
 
     // 0. weights -> bf16 (edge weights [T][D][H]; GRU gate blocks)
     if (pack) {
-        if (fused_path) {       // same bytes as the plain bf16 copy, in the fused kernel's TMEM-lane layout
+        if (fused_path) {       // same bytes as the plain bf16 copy, in the fused kernel's packed per-row layout
             const int prc = fused::pack_weights(1, num_types, H, 0, edge_weights, wb, bp->status, st);
             if (prc) return prc;
         } else {
@@ -557,13 +557,13 @@ static int gated_forward_bf16_impl(const uint16_t *node_states, const uint16_t *
             for (int t = 0; t < num_types; ++t) cs.w[t] = edge_weights[t];
             {
                 TimedScope timed__(PTGNN_KERNEL_PACK, st);
-                convert_weights_kernel<<<148, 256, 0, st>>>(cs, wb);
+                convert_weights_kernel<<<132, 256, 0, st>>>(cs, wb);
             }
             PTGNN_LAUNCHED();
         }
         {
             TimedScope timed__(PTGNN_KERNEL_PACK, st);
-            pack_gru_bf16_kernel<<<148, 256, 0, st>>>(gru_w_ih, gru_w_hh, H, D, p1, p2);
+            pack_gru_bf16_kernel<<<132, 256, 0, st>>>(gru_w_ih, gru_w_hh, H, D, p1, p2);
         }
         PTGNN_LAUNCHED();
         {
@@ -745,7 +745,7 @@ static int mlp_forward_bf16_impl(const uint16_t *node_states, const uint16_t *ga
         for (int t = 0; t < num_types; ++t) cs.w[t] = edge_weights[t];
         {
             TimedScope timed__(PTGNN_KERNEL_PACK, st);
-            convert_weights_kernel<<<148, 256, 0, st>>>(cs, wb);
+            convert_weights_kernel<<<132, 256, 0, st>>>(cs, wb);
         }
         PTGNN_LAUNCHED();
     }
@@ -754,7 +754,7 @@ static int mlp_forward_bf16_impl(const uint16_t *node_states, const uint16_t *ga
         cs.num = 1; cs.elems = out_dim * D; cs.w[0] = dense_weight;
         {
             TimedScope timed__(PTGNN_KERNEL_PACK, st);
-            convert_weights_kernel<<<148, 256, 0, st>>>(cs, wd);
+            convert_weights_kernel<<<132, 256, 0, st>>>(cs, wd);
         }
         PTGNN_LAUNCHED();
     }

@@ -1,4 +1,4 @@
-// Tensor-core (tcgen05, 3xTF32) versions of the three GEMM-bearing kernels of the hot path.  Same math and the same
+// Tensor-core (wgmma, 3xTF32) versions of the three GEMM-bearing kernels of the hot path.  Same math and the same
 // reference lines as layers.cu (gatedmessagepassing.py:54-60,69; mlpmessagepassing.py:88-98,116); the pipeline is in
 // tc_pipeline.cuh, the policies below only say where rows come from and what the epilogue does with the tile.
 #include "layers_tc.cuh"
@@ -143,12 +143,12 @@ struct MsgPolicy {
         return seg == 0 ? p.src32[e] : p.tgt32[e];
     }
     __device__ static int mma_groups(const Params &, const Tile &ti, int seg, MmaGroup (&g)[2]) {
-        g[0] = MmaGroup{ti.b_rows, 0, 0, seg == 0, 0};
+        g[0] = MmaGroup{ti.b_rows, 0, 0};
         return 1;
     }
     // warp `half` owns accumulator columns [64*half, 64*half + 64)
-    __device__ static void drain(const Params &, const Tile &ti, uint32_t tmem_lane, int half, float (&acc)[64]) {
-        tmem_drain_2x32(tmem_lane, 64 * half, ti.b_rows, acc);
+    __device__ static void drain(const Params &, const Tile &ti, const float *acc_row, int half, float (&acc)[64]) {
+        drain_2x32(acc_row, 64 * half, ti.b_rows, acc);
     }
     // only the raw load is issued a tile ahead: any arithmetic on the loaded value would stall the in-order issue right there
     struct Pre { int32_t pos; };
@@ -208,16 +208,15 @@ struct GruPolicy {
         return row < p.num_nodes ? row : -1;
     }
     __device__ static int mma_groups(const Params &, const Tile &, int seg, MmaGroup (&g)[2]) {
-        // seg 0: [i_n r z] += agg x [W_in W_ir W_iz]^T, N = 96; its very first K-step runs N = 128 over the zero block of
-        //        P1 so that it also clears the h_n columns.   seg 1: [r z h_n] += h x [W_hr W_hz W_hn]^T, N = 96.
-        if (seg == 0) g[0] = MmaGroup{96, 0, 0, true, 128};
-        else g[0] = MmaGroup{96, 32, 32, false, 0};
+        // seg 0: [i_n r z] += agg x [W_in W_ir W_iz]^T, N = 96.   seg 1: [r z h_n] += h x [W_hr W_hz W_hn]^T, N = 96.
+        if (seg == 0) g[0] = MmaGroup{96, 0, 0};
+        else g[0] = MmaGroup{96, 32, 32};
         return 1;
     }
     // accumulator columns: [0,32) i_n | [32,64) r | [64,96) z | [96,128) h_n (pre-activations without biases);
     // warp `half` owns hidden units j0 + 16*half .. +16 and therefore 16 columns of each gate group
-    __device__ static void drain(const Params &, const Tile &, uint32_t tmem_lane, int half, float (&acc)[64]) {
-        tmem_drain_4x16(tmem_lane, 16 * half, acc);
+    __device__ static void drain(const Params &, const Tile &, const float *acc_row, int half, float (&acc)[64]) {
+        drain_4x16(acc_row, 16 * half, acc);
     }
     // a lane owns one node row and 16 hidden units of it: 64 bytes of h, fetched one tile ahead
     struct Pre { long long row_off; float4 h[4]; };
@@ -282,11 +281,11 @@ struct DensePolicy {
         return row < p.num_nodes ? row : -1;
     }
     __device__ static int mma_groups(const Params &, const Tile &ti, int, MmaGroup (&g)[2]) {
-        g[0] = MmaGroup{ti.b_rows, 0, 0, true, 0};
+        g[0] = MmaGroup{ti.b_rows, 0, 0};
         return 1;
     }
-    __device__ static void drain(const Params &, const Tile &ti, uint32_t tmem_lane, int half, float (&acc)[64]) {
-        tmem_drain_2x32(tmem_lane, 64 * half, ti.b_rows, acc);
+    __device__ static void drain(const Params &, const Tile &ti, const float *acc_row, int half, float (&acc)[64]) {
+        drain_2x32(acc_row, 64 * half, ti.b_rows, acc);
     }
     struct Pre { long long row_off; };
     __device__ static void prefetch(const Params &p, const Tile &ti, int quarter, int, int lane, Pre &pre) {
@@ -315,7 +314,7 @@ struct DensePolicy {
 // =================================================================================================
 static int sm_count() {   // of the CURRENT device: a process may drive several GPUs (nothing cached across devices)
     int dev = 0, n = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     return n;
 }
 
@@ -380,7 +379,7 @@ int edge_messages(const float *h_src, const float *h_tgt, int H, int D, int use_
         for (int t = 0; t < num_types; ++t) ss.w[t] = weights[t];
         {
             TimedScope timed__(PTGNN_KERNEL_PACK, st);
-            split_weights_kernel<<<148, 256, 0, st>>>(ss, w_hi, w_lo);
+            split_weights_kernel<<<132, 256, 0, st>>>(ss, w_hi, w_lo);
         }
         PTGNN_LAUNCHED();
     }
@@ -412,7 +411,7 @@ int gru_update(const float *agg, const float *h, int64_t num_nodes, int H, int D
     if (pack) {
         {
             TimedScope timed__(PTGNN_KERNEL_PACK, st);
-            pack_split_gru_kernel<<<148, 256, 0, st>>>(w_ih, w_hh, H, D, p1_hi, p1_lo, p2_hi, p2_lo);
+            pack_split_gru_kernel<<<132, 256, 0, st>>>(w_ih, w_hh, H, D, p1_hi, p1_lo, p2_hi, p2_lo);
         }
         PTGNN_LAUNCHED();
         {
@@ -445,7 +444,7 @@ int dense_update(const float *y, int64_t num_nodes, int D, const float *W, const
         ss.num = 1; ss.elems = Hout * D; ss.w[0] = W;
         {
             TimedScope timed__(PTGNN_KERNEL_PACK, st);
-            split_weights_kernel<<<148, 256, 0, st>>>(ss, w_hi, w_lo);
+            split_weights_kernel<<<132, 256, 0, st>>>(ss, w_hi, w_lo);
         }
         PTGNN_LAUNCHED();
     }

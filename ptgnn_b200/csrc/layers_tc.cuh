@@ -1,4 +1,4 @@
-// Entry points of the tensor-core (tcgen05, 3xTF32) kernels; see layers_tc.cu.
+// Entry points of the tensor-core (wgmma, 3xTF32) kernels; see layers_tc.cu.
 #pragma once
 #include "common.cuh"
 

@@ -391,7 +391,7 @@ static int plan_build_phases(int phases, int64_t num_nodes, int64_t num_source_n
     char *ws = static_cast<char *>(workspace);
     int32_t *deg = reinterpret_cast<int32_t *>(ws + L.deg);
 
-    const unsigned grid = (unsigned)(ceil_div(E > 0 ? E : 1, 256) < 148 * 16 ? ceil_div(E > 0 ? E : 1, 256) : 148 * 16);
+    const unsigned grid = (unsigned)(ceil_div(E > 0 ? E : 1, 256) < 132 * 16 ? ceil_div(E > 0 ? E : 1, 256) : 132 * 16);
     int rc = PTGNN_OK;
     if (phases & 1) {
         PTGNN_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t), st));
@@ -481,7 +481,7 @@ extern "C" int ptgnn_b200_block_plan_build(int64_t num_nodes, int32_t num_types,
     TypeOffsets toff{};
     toff.num_types = T;
     for (int t = 0; t <= PTGNN_MAX_EDGE_TYPES; ++t) toff.off[t] = (int32_t)type_off[t < T ? t : T];
-    const unsigned grid = (unsigned)(ceil_div(E, 256) < 148 * 16 ? ceil_div(E, 256) : 148 * 16);
+    const unsigned grid = (unsigned)(ceil_div(E, 256) < 132 * 16 ? ceil_div(E, 256) : 132 * 16);
     {
         TimedScope timed__(PTGNN_KERNEL_PLAN, st);
         block_keys_kernel<<<grid, 256, 0, st>>>(toff, E, tgt32, B, keys, group_off);

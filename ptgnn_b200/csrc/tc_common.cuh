@@ -1,5 +1,5 @@
-// Blackwell (sm_100a) tensor-core plumbing for the fp32-exact GEMMs of the hot path: tcgen05.mma (kind::tf32, fp32
-// accumulate in TMEM), mbarrier pipelines, TMEM allocation and readback.  Hand-written inline PTX; no CUTLASS.
+// Hopper (sm_90a) tensor-core plumbing for the GEMMs of the hot path: wgmma (tf32 / f16 / bf16, fp32 accumulate in
+// registers), shared-memory matrix descriptors, mbarrier pipelines.  Hand-written inline PTX; no CUTLASS.
 //
 // fp32 accuracy on TF32 tensor cores ("3xTF32"): every fp32 operand x is split as x = hi + lo with
 // hi = x rounded to TF32 (low 13 mantissa bits zero) and lo = x - hi (exact in fp32, |lo| <= 2^-12 |x|).
@@ -7,10 +7,9 @@
 // parts (2^-23) are fp32-rounding level, which is what keeps the layer inside the north_star's 1e-5 tolerance (a single
 // TF32 product would be ~1e-3).
 //
-// Shared-memory operand layout (both A and B are K-major, rows of 32 fp32 = 128 bytes): the canonical
-// SWIZZLE_128B K-major layout -- 8-row groups of 1024 bytes, 16-byte chunk index XOR (row & 7).  One tcgen05.mma
-// consumes K = 8 fp32 (32 bytes) per instruction; advancing K inside the 128-byte row is a +32-byte bump of the
-// descriptor's start address.
+// Shared-memory operand layout (K-major, rows of 128 bytes): the canonical SWIZZLE_128B K-major layout -- 8-row groups
+// of 1024 bytes, 16-byte chunk index XOR (row & 7).  One wgmma consumes K = 8 fp32 or 16 16-bit values (32 bytes) per
+// instruction; advancing K inside the 128-byte row is a +32-byte bump of the descriptor's start address.
 #pragma once
 #include "common.cuh"
 
@@ -56,56 +55,77 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
 template <int REGS> __device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS)); }
 template <int REGS> __device__ __forceinline__ void reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS)); }
 
-// ---- proxy / tcgen05 fences ---------------------------------------------------------------------------
+// ---- proxy fence ----------------------------------------------------------------------------------------
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// ---- TMEM allocation (one full warp executes these) ---------------------------------------------------
-template <uint32_t COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t *smem_result) {
-    static_assert(COLS == 32 || COLS == 64 || COLS == 128 || COLS == 256 || COLS == 512, "TMEM columns: power of 2 >= 32");
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "n"(COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
 
 // ---- descriptors ----------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, K-major, SWIZZLE_128B: start address (>>4) bits [0,14), LBO bits [16,30) = 0
-// (single swizzle atom along K), SBO bits [32,46) = 1024 >> 4 (8-row group pitch), version bits [46,48) = 1 (sm_100),
-// layout type bits [61,64) = 2 (SWIZZLE_128B).  The tile base must be 1024-byte aligned (base_offset = 0).
+// Hopper wgmma shared-memory matrix descriptor, K-major, SWIZZLE_128B: start address (>>4) bits [0,14), leading byte offset
+// bits [16,30) (unused for a swizzled K-major operand whose K extent fits one 128-byte row; 1 by convention), stride byte
+// offset bits [32,46) = 1024 >> 4 (8-row group pitch), layout type bits [62,64) = 1 (SWIZZLE_128B).  The tile base must be
+// 1024-byte aligned; advancing K inside the 128-byte row is a +32-byte bump of the start address (+2 in the descriptor).
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr_bytes >> 4) & 0x3FFF);
+    d |= (uint64_t)1 << 16;
     d |= (uint64_t)(1024u >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-// Instruction descriptor (upper 32 bits of the idesc operand): D = F32 (bits [4,6) = 1), A/B format bits [7,10) /
-// [10,13) (0 = F16, 1 = BF16, 2 = TF32), both K-major (bits 15, 16 = 0), N >> 3 at bits [17,23), M >> 4 at bits [24,29).
-__host__ __device__ constexpr uint32_t make_instr_desc(uint32_t ab_format, uint32_t M, uint32_t N) {
-    return (1u << 4) | (ab_format << 7) | (ab_format << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-constexpr uint32_t FMT_BF16 = 1, FMT_TF32 = 2;
 
-// D[tmem] (+)= A[smem] * B[smem]^T ; one elected thread issues.
-__device__ __forceinline__ void mma_tf32_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
+// ---- wgmma (one warpgroup = 4 consecutive warps, all 128 threads execute every call) ----------------------------------
+// Accumulator fragment of an m64nN tile, per warp w of the warpgroup (rows 16 w ..), g = lane / 4, t = lane % 4:
+//   d[4 j + 0] = (row g, col 8 j + 2 t), d[4 j + 1] = (g, 8 j + 2 t + 1), d[4 j + 2] = (g + 8, 8 j + 2 t), d[4 j + 3] = (g + 8, 8 j + 2 t + 1).
+// Register A fragment (k8 tf32 / k16 16-bit): a[0] = (row g, k 2t.. or t), a[1] = (g + 8, same k), a[2] = (g, k + 8 / + 4),
+// a[3] = (g + 8, k + 8 / + 4) -- the mma.sync m16n8k16 / m16n8k8 A layout of the warp's 16 rows.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+template <int N> __device__ __forceinline__ void fence_acc(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void mma_bf16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+
+// D[64 x 32] += A[64 x 8] (tf32, registers) * B[32 x 8]^T (tf32, shared memory descriptor)
+__device__ __forceinline__ void wgmma_tf32_rs_n32(float (&d)[16], const uint32_t (&a)[4], uint64_t desc_b) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\twgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
 }
+// D[64 x 32] += A[64 x 16] * B[32 x 16]^T, both 16-bit operands from shared memory (K-major)
+template <bool BF16>
+__device__ __forceinline__ void wgmma_16_ss_n32(float (&d)[16], uint64_t desc_a, uint64_t desc_b) {
+    if (BF16)
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\twgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(desc_a), "l"(desc_b), "r"(1));
+    else
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\twgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(desc_a), "l"(desc_b), "r"(1));
+}
+// D[64 x 64] += A[64 x 16] (registers) * B[64 x 16]^T (shared memory, K-major)
+template <bool BF16>
+__device__ __forceinline__ void wgmma_16_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b) {
+    if (BF16)
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\twgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
+    else
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\twgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
+}
+
 // Tell the compiler a value is the same in every lane (broadcast from lane 0): it may then live in a uniform register.
 __device__ __forceinline__ uint32_t warp_uniform(uint32_t v) { return __shfl_sync(0xffffffffu, v, 0); }
 __device__ __forceinline__ int warp_uniform(int v) { return __shfl_sync(0xffffffffu, v, 0); }
@@ -114,106 +134,11 @@ template <class T> __device__ __forceinline__ const T *warp_uniform(const T *ptr
     const uint32_t lo = __shfl_sync(0xffffffffu, (uint32_t)v, 0), hi = __shfl_sync(0xffffffffu, (uint32_t)(v >> 32), 0);
     return reinterpret_cast<const T *>(((unsigned long long)hi << 32) | lo);
 }
-// One lane of a converged warp (the same one every time).  Issuing tcgen05.mma / commit under this predicate from a warp
-// that runs the whole loop converged lets the compiler keep descriptors in uniform registers; issuing them from an
-// `if (lane == 0)` region makes it wrap every MMA in an ELECT / R2UR.BROADCAST waterfall loop (~100 cycles per MMA).
+// One lane of a converged warp (the same one every time): TMA issue under this predicate keeps operands uniform.
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
     return pred != 0;
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void mma_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// ---- TMEM -> registers: warp w reads its 32-lane quarter (lanes 32*(w%4)..), 32 consecutive fp32 columns ------
-__device__ __forceinline__ void tmem_ld_32cols(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// Same loads WITHOUT the trailing wait: issue several, then tmem_ld_wait() once (the waits serialised ~200 ns each).
-__device__ __forceinline__ void tmem_ld_32cols_async(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_16cols_async(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_ld_16cols(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// ---- registers -> TMEM (A operand staging for TS-mode MMAs): this thread's lane, 32 consecutive columns -------
-__device__ __forceinline__ void tmem_st_32cols(uint32_t taddr, const float (&v)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-          "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-          "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-          "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15])),
-          "r"(__float_as_uint(v[16])), "r"(__float_as_uint(v[17])), "r"(__float_as_uint(v[18])), "r"(__float_as_uint(v[19])),
-          "r"(__float_as_uint(v[20])), "r"(__float_as_uint(v[21])), "r"(__float_as_uint(v[22])), "r"(__float_as_uint(v[23])),
-          "r"(__float_as_uint(v[24])), "r"(__float_as_uint(v[25])), "r"(__float_as_uint(v[26])), "r"(__float_as_uint(v[27])),
-          "r"(__float_as_uint(v[28])), "r"(__float_as_uint(v[29])), "r"(__float_as_uint(v[30])), "r"(__float_as_uint(v[31]))
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_16cols(uint32_t taddr, const float (&v)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-        ::"r"(taddr), "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-          "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-          "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-          "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15]))
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// D[tmem] (+)= A[tmem] * B[smem]^T  (A: lane = row, one fp32 column per k)
-__device__ __forceinline__ void mma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
 }
 
 // ---- 3xTF32 operand split -----------------------------------------------------------------------------------

@@ -1,30 +1,23 @@
-// Persistent, warp-specialised tcgen05 pipeline shared by the three GEMM-bearing kernels of the hot path
+// Persistent, warp-specialised Hopper (wgmma) pipeline shared by the three GEMM-bearing kernels of the round-1 path
 // (per-edge messages, GRUCell update, Mlp dense update).  fp32-exact via 3xTF32 (see tc_common.cuh).
 //
-//   warps 0-3  CONVERTERS each thread owns ONE row of every chunk: it reads its 32 raw fp32 from the slot, splits them into
-//                         TF32 hi/lo and writes both into TENSOR MEMORY (tcgen05.st), so the MMAs take A from TMEM ("TS"
-//                         form) and shared memory only feeds B.  The stores of chunk c stay in flight while the thread
-//                         waits for chunk c+1; then wait::st + arrive full[slot].
-//   warp  4    MMA        converged warp, one elected lane issues: wait full[slot]; per K=8 step hi*hi into the MAIN
-//                         accumulator and hi*lo + lo*hi into the CORRECTION accumulator (tensor-core accumulation
-//                         truncates, so the small terms must not perturb the main sum); tcgen05.commit -> empty[slot];
-//                         per tile commit -> tmem_full.
-//   warp  5    TMA        a ring ahead of the MMA warp: wait empty[slot]; bulk tensor copies of the pre-split weight tile
+//   warp  0    TMA        a ring ahead of the consumers: wait empty[slot]; bulk tensor copies of the pre-split weight tile
 //                         (hi, lo) and, for contiguous node rows, of the raw A tile -> landed[slot] (expect_tx).
-//   warps 6-7  GATHERERS  per-edge messages only: wait a_free[slot] (converters have read it); 16-byte cp.async (LDGSTS) of the gathered node-state
-//                         rows, completion signalled on landed[slot] by cp.async.mbarrier.arrive; row indices in shared
-//                         memory, fetched one (tile, segment) ahead.  ~53 GB/s per SM is the LDGSTS ceiling (probe in
-//                         tools/probes), 4x what TMA gather4 reaches -- and it needs its own warps to run at it.
-//   warps 8-15 EPILOGUE   wait tmem_full; drain main + correction into registers (row per thread, two warps per TMEM
-//                         lane quarter, half of the columns each); release the accumulators (tmem_empty) BEFORE the
-//                         policy's store phase (smem-transposed coalesced rows), so the next tile's MMAs overlap it.
-//
-// Why TS: an SS-mode tf32 MMA (128x128x8) reads 8 KB of operands from shared memory = the 64 cycles its math takes,
-// and the staging traffic then starves it (measured: tensor pipe 17 % active).  With A in TMEM an MMA reads 4 KB.
+//   warps 1-2  GATHERERS  per-edge messages only: wait a_free[slot] (consumers have read it); 16-byte cp.async (LDGSTS) of the
+//                         gathered node-state rows, completion signalled on landed[slot] by cp.async.mbarrier.arrive; row
+//                         indices in shared memory, fetched one (tile, segment) ahead.
+//   warps 4-11 CONSUMERS  two warpgroups, rows [0,64) and [64,128) of the 128-row tile.  Per chunk: wait landed[slot]; each
+//                         thread reads its A fragment (raw fp32) from the slot, splits it into TF32 hi / lo in registers and
+//                         arrives a_free; per K=8 step hi*hi into the MAIN accumulator and hi*lo + lo*hi into the CORRECTION
+//                         accumulator (tensor-core accumulation truncates, so the small terms must not perturb the main sum),
+//                         register-A wgmma against the B tiles of the slot; wait for the MMAs, arrive empty[slot].
+//                         Per tile: main + correction -> a shared-memory accumulator tile; then every consumer warp runs the
+//                         policy epilogue on one row per thread (quarter = 32 rows, half = 64 columns), the same code the
+//                         per-thread-row stores were written for.
 //
 // One CTA per SM (grid = #SMs), static round-robin over tiles.
-//   shared memory: 4 slots x 48 KB (raw A | B_hi | B_lo, 128-byte SWIZZLE_128B rows) + 1 KB row indices + 32 KB epilogue transpose
-//   tensor memory (512 columns): [0,128) main acc | [128,256) correction acc | [256,512) 4 x (A_hi 32 | A_lo 32)
+//   shared memory: 3 slots x 48 KB (raw A | B_hi | B_lo, 128-byte SWIZZLE_128B rows) + 1 KB row indices + the 128 x 132 fp32
+//   accumulator tile (whose rows also serve as the epilogue's transpose buffers once drained)
 // Every mbarrier wait is bounded (tc_common.cuh): a protocol bug traps instead of hanging the GPU.
 //
 // A Policy supplies:
@@ -35,8 +28,8 @@
 //   __device__ static Segment segment(const Params&, const Tile&, int seg);
 //   __device__ static int  gather_row(const Params&, const Tile&, int seg, int r);   only when GATHER (then a_map == nullptr)
 //   __device__ static int  mma_groups(const Params&, const Tile&, int seg, MmaGroup (&g)[2]);
-//   __device__ static void drain(const Params&, const Tile&, uint32_t tmem_lane, int half, float (&acc)[64]);
-//                          (read this warp's share of main + correction accumulators; tmem_ld_sum16/32 below)
+//   __device__ static void drain(const Params&, const Tile&, const float *acc_row, int half, float (&acc)[64]);
+//                          (read this thread's row of the accumulator tile; drain_2x32 / drain_4x16 below)
 //   __device__ static void tile_init(Tile&);   tiles are set up in increasing order per role: tile_setup may walk forward
 //   struct Pre;  __device__ static void prefetch(const Params&, const Tile&, int quarter, int half, int lane, Pre&);
 //                          (global-memory inputs of the store -- row offset (-1 = row not stored), GRU h -- one tile ahead)
@@ -51,33 +44,31 @@ namespace tc {
 
 constexpr int TILE_M = 128;
 constexpr int CHUNK_K = 32;                       // fp32 per k-chunk = one 128-byte swizzled row
-// Warp roles, in warpgroups of 4 so that setmaxnreg can move registers from the light roles to the epilogue:
-//   WG0 = warps 0-3 converters (112 regs) | WG1 = warp 4 MMA issuer, warp 5 TMA issuer, warps 6-7 row gatherers (48)
-//   WG2+WG3 = warps 8-15 epilogue (176)
-constexpr int NUM_PRODUCER_WARPS = 4;
-constexpr int PRODUCER_THREADS = NUM_PRODUCER_WARPS * 32;
-constexpr int MMA_WARP = 4;
-constexpr int TMA_WARP = 5;
-constexpr int FIRST_GATHER_WARP = 6;
+// Warp roles: WG0 = warp 0 TMA issuer, warps 1-2 row gatherers (warp 3 idle) | WG1 + WG2 = warps 4-11 consumers.
+// setmaxnreg moves registers from the producer warpgroup to the consumers: (56 + 2 * 224) * 128 = 64512 <= 65536.
+constexpr int TMA_WARP = 0;
+constexpr int FIRST_GATHER_WARP = 1;
 constexpr int GATHER_THREADS = 64;
-constexpr int FIRST_EPI_WARP = 8;
-constexpr int NUM_EPI_WARPS = 8;                  // two per TMEM lane quarter, each draining half of the columns
-constexpr int NUM_THREADS = 16 * 32;
-constexpr int PRODUCER_REGS = 112, MMA_REGS = 48, EPI_REGS = 176;   // (112 + 48 + 176 + 176) * 128 = 65536
+constexpr int FIRST_CONSUMER_WARP = 4;
+constexpr int NUM_CONSUMER_WARPS = 8;
+constexpr int NUM_THREADS = 12 * 32;
+constexpr int PRODUCER_REGS = 56, CONSUMER_REGS = 224;
+static_assert(PRODUCER_REGS + 2 * CONSUMER_REGS <= 3 * 168, "register budgets exceed the launch allocation");
 constexpr int OPERAND_BYTES = TILE_M * CHUNK_K * 4;   // 16 KB: one 128 x 32 fp32 operand tile
-constexpr int STAGE_BYTES_PER_WARP = 32 * 32 * 4;     // epilogue transpose buffer: 32 rows x 32 fp32
-constexpr int CORR_OFF = 128;                         // correction accumulator columns (relative to the main ones)
-constexpr int A_TMEM_OFF = 256;                       // TS: A operand ring, slot s at columns A_TMEM_OFF + 64 s (hi | lo)
+constexpr int STAGE_FLOATS_PER_WARP = 32 * 32;        // epilogue transpose buffer: 32 rows x 32 fp32
+constexpr int ACC_PITCH = 132;                        // accumulator tile row pitch (floats): conflict-free 16-byte row reads
 
-// Shared-memory ring: 4 slots x 48 KB (raw A | B_hi | B_lo).  Tensor memory (512 columns): [0,128) main accumulator |
-// [128,256) correction accumulator | [256,512) 4 x (A_hi 32 | A_lo 32) -- the A operand of every MMA comes from TMEM.
-constexpr int NUM_SLOTS = 4;
+// Shared-memory ring: 3 slots x 48 KB (raw A | B_hi | B_lo), then the accumulator tile.
+constexpr int NUM_SLOTS = 3;
 constexpr int SLOT_BYTES = 3 * OPERAND_BYTES;
 constexpr int B_HI_OFF = OPERAND_BYTES, B_LO_OFF = 2 * OPERAND_BYTES;
 constexpr int RING_BYTES = NUM_SLOTS * SLOT_BYTES;
 constexpr int INDEX_BYTES = 2 * TILE_M * 4;           // gather warps: row indices of the current / next (tile, segment)
 constexpr int BARRIER_BYTES = 256;
-constexpr int SMEM_BYTES = RING_BYTES + 1024 /*alignment slack*/ + BARRIER_BYTES + INDEX_BYTES + NUM_EPI_WARPS * STAGE_BYTES_PER_WARP;
+constexpr int ACC_BYTES = TILE_M * ACC_PITCH * 4;
+constexpr int SMEM_BYTES = RING_BYTES + 1024 /*alignment slack*/ + BARRIER_BYTES + INDEX_BYTES + ACC_BYTES;
+static_assert(SMEM_BYTES <= 232448, "shared memory budget");
+static_assert(4 * STAGE_FLOATS_PER_WARP <= 64 * ACC_PITCH, "a warpgroup's transpose buffers fit in its accumulator rows");
 
 struct Segment {        // one K-range of the tile's GEMM
     const float *a;     // gathered A rows (row pitch lda) -- used when a_map == nullptr
@@ -88,11 +79,8 @@ struct Segment {        // one K-range of the tile's GEMM
     int b_row0, b_col0, b_box_rows;
     int K;              // columns of this segment (multiple of 4)
 };
-struct MmaGroup {       // per K-step: B rows [row_off, row_off + n) -> accumulator columns [col_off, col_off + n)
-    int n, row_off, col_off;
-    bool fresh;         // true: the first K-step of this segment overwrites the accumulator columns
-    int n_first;        // width of that first (overwriting) K-step; > n lets it also clear columns that a later segment
-                        // accumulates into (the GRU's h_n block) -- 0 means n
+struct MmaGroup {       // per K-step: B rows [row_off, row_off + n) -> accumulator columns [col_off, col_off + n); col_off and
+    int n, row_off, col_off;   // row_off are multiples of 32 (the accumulators are zeroed at the start of every tile)
 };
 
 __device__ __forceinline__ uint32_t swz(int row, int q) { return (uint32_t)(row * 128 + ((q ^ (row & 7)) << 4)); }
@@ -114,7 +102,7 @@ __device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint64_t *bar) {
 __device__ __forceinline__ void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
 // ---- epilogue transposes through shared memory ---------------------------------------------------------------
-// The accumulator comes out of TMEM one ROW per thread; storing that directly makes every warp-wide store touch 32
+// The epilogue holds the accumulator one ROW per thread; storing that directly makes every warp-wide store touch 32
 // different 128-byte lines.  Staging 32 rows x NCOLS through a (chunk-XOR-swizzled) buffer lets each store
 // instruction write whole rows: 4 (NCOLS = 32) or 8 (NCOLS = 16) lines per instruction instead of 32.
 // `row_off` is this lane's destination element offset from `dst_base` (negative = row not stored).
@@ -143,37 +131,28 @@ __device__ __forceinline__ void warp_store_rows(float *stage, const float *v, fl
     }
     __syncwarp();
 }
-// accumulator value = main + correction; all TMEM loads of a drain are issued before ONE wait
-// drain 64 consecutive columns [c0, c0+64) (only the 32-column blocks below `ncols`); two loads in flight per wait
-__device__ __forceinline__ void tmem_drain_2x32(uint32_t taddr, int c0, int ncols, float (&acc)[64]) {
+// drain 64 consecutive columns [c0, c0+64) of this thread's accumulator row (only the 32-column blocks below `ncols`)
+__device__ __forceinline__ void drain_2x32(const float *row, int c0, int ncols, float (&acc)[64]) {
 #pragma unroll
     for (int b = 0; b < 2; ++b) {
         if (c0 + 32 * b < ncols) {   // warp-uniform
-            uint32_t m[32], c[32];
-            tmem_ld_32cols_async(taddr + c0 + 32 * b, m);
-            tmem_ld_32cols_async(taddr + c0 + 32 * b + CORR_OFF, c);
-            tmem_ld_wait();
 #pragma unroll
-            for (int i = 0; i < 32; ++i) acc[32 * b + i] = __uint_as_float(m[i]) + __uint_as_float(c[i]);
+            for (int i = 0; i < 8; ++i) {
+                const float4 v = *reinterpret_cast<const float4 *>(row + c0 + 32 * b + 4 * i);
+                acc[32 * b + 4 * i] = v.x; acc[32 * b + 4 * i + 1] = v.y; acc[32 * b + 4 * i + 2] = v.z; acc[32 * b + 4 * i + 3] = v.w;
+            }
         }
     }
 }
-// drain 4 groups of 16 columns at taddr + 32 g + off (GRU gate groups); four loads in flight per wait
-__device__ __forceinline__ void tmem_drain_4x16(uint32_t taddr, int off, float (&acc)[64]) {
+// drain 4 groups of 16 columns at 32 g + off (GRU gate groups)
+__device__ __forceinline__ void drain_4x16(const float *row, int off, float (&acc)[64]) {
 #pragma unroll
-    for (int gp = 0; gp < 2; ++gp) {
-        uint32_t m[2][16], c[2][16];
+    for (int g = 0; g < 4; ++g)
 #pragma unroll
-        for (int g = 0; g < 2; ++g) {
-            tmem_ld_16cols_async(taddr + 32 * (2 * gp + g) + off, m[g]);
-            tmem_ld_16cols_async(taddr + 32 * (2 * gp + g) + off + CORR_OFF, c[g]);
+        for (int i = 0; i < 4; ++i) {
+            const float4 v = *reinterpret_cast<const float4 *>(row + 32 * g + off + 4 * i);
+            acc[16 * g + 4 * i] = v.x; acc[16 * g + 4 * i + 1] = v.y; acc[16 * g + 4 * i + 2] = v.z; acc[16 * g + 4 * i + 3] = v.w;
         }
-        tmem_ld_wait();
-#pragma unroll
-        for (int g = 0; g < 2; ++g)
-#pragma unroll
-            for (int i = 0; i < 16; ++i) acc[16 * (2 * gp + g) + i] = __uint_as_float(m[g][i]) + __uint_as_float(c[g][i]);
-    }
 }
 
 // Optional timeline trace (PTGNN_TC_TRACE): CTA 0 records %globaltimer at pipeline hand-offs into 3 x 2048 slots.
@@ -191,173 +170,35 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
     // 1024-byte aligned ring (SWIZZLE_128B descriptors / TMA swizzle assume base_offset = 0)
     unsigned char *ring = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // offset form: keeps the shared address space
     uint64_t *bars = reinterpret_cast<uint64_t *>(ring + RING_BYTES);
-    uint64_t *full = bars, *empty = bars + NUM_SLOTS, *landed = bars + 2 * NUM_SLOTS;
-    uint64_t *a_free = bars + 3 * NUM_SLOTS;
-    uint64_t *tmem_full = bars + 4 * NUM_SLOTS, *tmem_empty = bars + 4 * NUM_SLOTS + 1;
-    uint32_t *tmem_base_smem = reinterpret_cast<uint32_t *>(bars + 4 * NUM_SLOTS + 2);
+    uint64_t *empty = bars, *landed = bars + NUM_SLOTS, *a_free = bars + 2 * NUM_SLOTS;
     int32_t *index_buf = reinterpret_cast<int32_t *>(ring + RING_BYTES + BARRIER_BYTES);
-    float *stage_base = reinterpret_cast<float *>(ring + RING_BYTES + BARRIER_BYTES + INDEX_BYTES);
+    float *acc_s = reinterpret_cast<float *>(ring + RING_BYTES + BARRIER_BYTES + INDEX_BYTES);
 
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // warp-uniform for the compiler
     const int lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
         for (int s = 0; s < NUM_SLOTS; ++s) {
-            mbar_init(&full[s], PRODUCER_THREADS);   // converters: A of this chunk is in TMEM (hi | lo)
-            mbar_init(&empty[s], 1);                 // MMA commit: smem slot + TMEM A buffer may be overwritten
+            mbar_init(&empty[s], NUM_CONSUMER_WARPS);    // consumers: the MMAs of this chunk are done, the slot may be refilled
             // operands of this chunk are in shared memory: the TMA warp's expect_tx arrival (+ its bytes) and, when A rows
             // are gathered, one cp.async-completion arrival per gather thread
             mbar_init(&landed[s], 1 + (Policy::GATHER ? GATHER_THREADS : 0));
-            // gathered rows only: the converters have read the slot's raw A tile -- the gatherers may refill it without
-            // waiting for the MMAs of the chunk (the MMAs read A from TMEM, only B from the slot)
-            mbar_init(&a_free[s], PRODUCER_THREADS);
+            // gathered rows only: the consumers have read the slot's raw A tile into registers -- the gatherers may refill it
+            // without waiting for the MMAs of the chunk (they read only B from the slot)
+            mbar_init(&a_free[s], NUM_CONSUMER_WARPS);
         }
-        mbar_init(tmem_full, 1);                     // MMA commit: accumulators of the tile are complete
-        mbar_init(tmem_empty, NUM_EPI_WARPS);        // epilogue: accumulators drained
         mbar_init_fence();
     }
-    if (warp == 0) tmem_alloc<512>(tmem_base_smem);
-    tc_fence_before_sync();
     __syncthreads();
-    tc_fence_after_sync();
-    const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_base_smem, 0);
     const int total_tiles = Policy::num_tiles(p);
-    // timing experiments only (PTGNN_TC_DEBUG; results are wrong when set): 1 = no MMAs, 2 = no loads, 4 = no stores,
-    // 8 = no A conversion
+    // timing experiments only (PTGNN_TC_DEBUG; results are wrong when set): 1 = no MMAs, 2 = no loads, 4 = no stores
     const int dbg = p.dbg;
     unsigned long long *trace_base = (p.trace != nullptr && blockIdx.x == 0) ? p.trace : nullptr;
 
-    if (warp < NUM_PRODUCER_WARPS) {
-        // =========================================== CONVERTERS ===========================================
-        // Thread r owns row r of every chunk: 32 raw fp32 from the slot -> TF32 hi / lo -> the slot's TMEM A buffer.  The
-        // tcgen05.st of chunk c is left in flight while the thread waits for chunk c+1 and reads its row; only then does it
-        // wait for the stores and hand chunk c to the MMA warp.
+    if (warp < FIRST_CONSUMER_WARP) {
         reg_dealloc<PRODUCER_REGS>();
-        const int my_row = warp * 32 + lane;
-        const uint32_t tmem_lane = tmem_base + ((uint32_t)(warp * 32) << 16);
-        Tracer tr{(trace_base && threadIdx.x == 0) ? trace_base : nullptr, 0, 1024};
-        uint32_t c = 0;
-        bool pending = false;
-        uint32_t pending_slot = 0;
-        typename Policy::Tile t;
-        Policy::tile_init(t);
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-            Policy::tile_setup(p, tile, t);
-            const int nseg = Policy::num_segments(p, t);
-            for (int seg = 0; seg < nseg; ++seg) {
-                const int nkc = (Policy::segment(p, t, seg).K + CHUNK_K - 1) / CHUNK_K;
-                for (int kc = 0; kc < nkc; ++kc, ++c) {
-                    const uint32_t slot = c % NUM_SLOTS, use = c / NUM_SLOTS;
-                    tr.mark(3);
-                    mbar_wait(&landed[slot], use & 1);
-                    tr.mark(5);
-                    const unsigned char *base = ring + slot * SLOT_BYTES;
-                    float4 raw[8];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) raw[j] = *reinterpret_cast<const float4 *>(base + swz(my_row, j));
-                    if (pending) {
-                        tmem_st_wait();
-                        tc_fence_before_sync();
-                        mbar_arrive(&full[pending_slot]);
-                        tr.mark(6);
-                    }
-                    float hi[32], lo[32];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        hi[4 * j] = tf32_hi(raw[j].x); hi[4 * j + 1] = tf32_hi(raw[j].y);
-                        hi[4 * j + 2] = tf32_hi(raw[j].z); hi[4 * j + 3] = tf32_hi(raw[j].w);
-                        lo[4 * j] = raw[j].x - hi[4 * j]; lo[4 * j + 1] = raw[j].y - hi[4 * j + 1];
-                        lo[4 * j + 2] = raw[j].z - hi[4 * j + 2]; lo[4 * j + 3] = raw[j].w - hi[4 * j + 3];
-                    }
-                    if (Policy::GATHER) {
-                        mbar_arrive(&a_free[slot]);                       // raw tile consumed (values are in registers)
-                        mbar_wait(&empty[slot], (use & 1) ^ 1);           // TMEM A buffer of the slot: MMAs of chunk c-4 done
-                        tc_fence_after_sync();
-                    }
-                    const uint32_t a_buf = tmem_lane + A_TMEM_OFF + slot * 64;
-                    if (!(dbg & 8)) {
-                        tmem_st_32cols(a_buf, hi);
-                        tmem_st_32cols(a_buf + 32, lo);
-                    }
-                    pending = true;
-                    pending_slot = slot;
-                }
-            }
-        }
-        if (pending) {
-            tmem_st_wait();
-            tc_fence_before_sync();
-            mbar_arrive(&full[pending_slot]);
-        }
-    } else if (warp < FIRST_EPI_WARP) {
-        reg_dealloc<MMA_REGS>();
-        if (warp == MMA_WARP) {
-            // =========================================== MMA ISSUER ===========================================
-            // The whole warp walks the loop converged (every lane polls the barriers) and one elected lane issues: the
-            // descriptors then live in uniform registers.  Issued from an `if (lane == 0)` region every tcgen05.mma was
-            // wrapped in an ELECT / R2UR.BROADCAST waterfall loop, ~100 cycles per instruction.
-            const bool leader = elect_one();
-            uint32_t c = 0, tcount = 0;
-            Tracer tr{(trace_base && leader) ? trace_base + 2048 : nullptr, 0, 2048};
-            typename Policy::Tile t;
-            Policy::tile_init(t);
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++tcount) {
-                tr.mark(10);
-                Policy::tile_setup(p, tile, t);
-                mbar_wait(tmem_empty, (tcount & 1) ^ 1);   // the epilogue has drained the accumulators
-                tr.mark(12);
-                tc_fence_after_sync();
-                const int nseg = Policy::num_segments(p, t);
-                for (int seg = 0; seg < nseg; ++seg) {
-                    const Segment sg = Policy::segment(p, t, seg);
-                    MmaGroup g[2];
-                    const int ng = Policy::mma_groups(p, t, seg, g);
-                    const int nkc = (sg.K + CHUNK_K - 1) / CHUNK_K;
-                    for (int kc = 0; kc < nkc; ++kc, ++c) {
-                        const uint32_t slot = c % NUM_SLOTS, use = c / NUM_SLOTS;
-                        tr.mark(13);
-                        mbar_wait(&full[slot], use & 1);
-                        tr.mark(14);
-                        tc_fence_after_sync();
-                        const uint32_t base = smem_u32(ring + slot * SLOT_BYTES);
-                        const uint32_t a_buf = tmem_base + A_TMEM_OFF + slot * 64;
-                        const int kvalid = min(CHUNK_K, sg.K - kc * CHUNK_K);
-                        const int ksteps = (dbg & 1) ? 0 : (kvalid + 7) / 8;
-                        // descriptors of K-step 0; later K-steps are +32 bytes (= +2 in the 16-byte address field) / +8 TMEM columns
-#pragma unroll
-                        for (int gi = 0; gi < 2; ++gi) {
-                            if (gi < ng) {
-                                const uint64_t b_hi0 = make_smem_desc_sw128(base + B_HI_OFF + g[gi].row_off * 128);
-                                const uint64_t b_lo0 = make_smem_desc_sw128(base + B_LO_OFF + g[gi].row_off * 128);
-                                const uint32_t idesc_n = make_instr_desc(FMT_TF32, TILE_M, (uint32_t)g[gi].n);
-                                const uint32_t d_main = tmem_base + g[gi].col_off, d_corr = d_main + CORR_OFF;
-                                const bool overwrite = g[gi].fresh && kc == 0;
-                                const uint32_t acc0 = overwrite ? 0u : 1u;
-                                const uint32_t idesc_first = (overwrite && g[gi].n_first > 0)
-                                                                 ? make_instr_desc(FMT_TF32, TILE_M, (uint32_t)g[gi].n_first) : idesc_n;
-#pragma unroll
-                                for (int ks = 0; ks < CHUNK_K / 8; ++ks) {
-                                    if (ks < ksteps && leader) {
-                                        const uint32_t first = ks == 0 ? acc0 : 1u;
-                                        const uint32_t idesc = ks == 0 ? idesc_first : idesc_n;
-                                        // x * w ~= hi*hi (main) + hi*lo + lo*hi (correction accumulator)
-                                        mma_tf32_ts(d_main, a_buf + ks * 8, b_hi0 + ks * 2, idesc, first);
-                                        mma_tf32_ts(d_corr, a_buf + ks * 8, b_lo0 + ks * 2, idesc, first);
-                                        mma_tf32_ts(d_corr, a_buf + 32 + ks * 8, b_hi0 + ks * 2, idesc, 1u);
-                                    }
-                                }
-                            }
-                        }
-                        if (leader) mma_commit(&empty[slot]);
-                        __syncwarp();
-                        tr.mark(15);
-                    }
-                }
-                if (leader) mma_commit(tmem_full);
-                __syncwarp();
-            }
-        } else if (warp == TMA_WARP) {
+        if (warp == TMA_WARP) {
             // =========================================== TMA WARP ===========================================
-            // Walks the same (tile, segment, k-chunk) sequence as the MMA warp, a whole ring ahead of it: waits for the
+            // Walks the same (tile, segment, k-chunk) sequence as the consumers, a whole ring ahead of them: waits for the
             // slot's release, then issues the bulk tensor copies of the chunk -- weights (hi, lo) and, for contiguous rows,
             // the raw A tile.  Converged warp + elected lane: all operands stay in uniform registers.
             const bool leader = elect_one();
@@ -386,8 +227,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
                     }
                 }
             }
-        } else if (Policy::GATHER) {
-            // =========================================== ROW GATHERERS (warps 6-7) ===========================================
+        } else if (Policy::GATHER && warp < FIRST_GATHER_WARP + GATHER_THREADS / 32) {
+            // =========================================== ROW GATHERERS (warps 1-2) ===========================================
             // 64 threads stage the gathered A rows of every chunk with 16-byte cp.async (LDGSTS, no registers): thread g
             // copies piece q = g & 7 of rows (g >> 3) + 8 i, i < 16.  Completion is signalled on landed[slot] by
             // cp.async.mbarrier.arrive, so nobody waits on cp.async groups.  The row indices of a (tile, segment) sit in
@@ -429,7 +270,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
                 const Segment sg = Policy::segment(p, t, seg);
                 const int nkc = (sg.K + CHUNK_K - 1) / CHUNK_K;
                 // this thread's 16 rows of the (tile, segment): indices -> registers once, so that the per-chunk loop is just
-                // address arithmetic + LDGSTS (64 threads must sustain the SM's ~53 GB/s LDGSTS rate)
+                // address arithmetic + LDGSTS
                 int rows[16];
 #pragma unroll
                 for (int i = 0; i < 16; ++i) rows[i] = rows_s[rsub + 8 * i];
@@ -459,18 +300,21 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
             cp_async_wait<0>();
         }
     } else {
-        // =========================================== EPILOGUE ===========================================
-        reg_alloc<EPI_REGS>();
-        const int ew = warp - FIRST_EPI_WARP;    // 0..7
-        const int quarter = warp & 3;            // TMEM lanes 32*quarter .. +31 are the ones this warp may read
-        const int half = ew >> 2;                // which half of the accumulator columns this warp drains
-        const uint32_t tmem_lane = tmem_base + ((uint32_t)(quarter * 32) << 16);
-        float *stage = stage_base + ew * (STAGE_BYTES_PER_WARP / 4);
-        uint32_t tcount = 0;
-        Tracer tr{(trace_base && ew == 0 && lane == 0) ? trace_base + 4096 : nullptr, 0, 2048};
+        // =========================================== CONSUMERS ===========================================
+        reg_alloc<CONSUMER_REGS>();
+        const int cw = warp - FIRST_CONSUMER_WARP;       // 0..7
+        const int wg = cw >> 2, wi = cw & 3;              // warpgroup: tile rows [64 wg, 64 wg + 64); warp: rows 16 wi ..
+        const int gq = lane >> 2, tq = lane & 3;
+        const int r0 = 64 * wg + 16 * wi + gq, r1 = r0 + 8;   // this thread's A / accumulator rows
+        // epilogue role of this warp: rows 32 quarter .. (inside the warpgroup's 64 rows), columns of `half`
+        const int quarter = 2 * wg + (wi & 1), half = wi >> 1;
+        const float *acc_row = acc_s + (quarter * 32 + lane) * ACC_PITCH;
+        float *stage = acc_s + wg * 64 * ACC_PITCH + wi * STAGE_FLOATS_PER_WARP;
+        const int bar_id = 2 + wg;                        // named barrier of this warpgroup's 128 threads
+        uint32_t c = 0;
+        Tracer tr{(trace_base && cw == 0 && lane == 0) ? trace_base + 2048 : nullptr, 0, 2048};
         typename Policy::Tile t, t_next;
-        // What the store needs from global memory (destination offsets, the GRU's h values) is fetched one tile ahead: the
-        // epilogue is a serial per-tile chain and a load issued at store time queues behind the gathers.
+        // What the store needs from global memory (destination offsets, the GRU's h values) is fetched one tile ahead.
         typename Policy::Pre pre, pre_next;
         int tile = blockIdx.x;
         Policy::tile_init(t);
@@ -478,22 +322,100 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
             Policy::tile_setup(p, tile, t);
             Policy::prefetch(p, t, quarter, half, lane, pre);
         }
-        for (; tile < total_tiles; tile += gridDim.x, ++tcount) {
+        for (; tile < total_tiles; tile += gridDim.x) {
             const int next = tile + gridDim.x;
             if (next < total_tiles) {
                 t_next = t;
                 Policy::tile_setup(p, next, t_next);
                 Policy::prefetch(p, t_next, quarter, half, lane, pre_next);
             }
-            tr.mark(20);
-            mbar_wait(tmem_full, tcount & 1);
-            tr.mark(21);
-            tc_fence_after_sync();
+            float acc_m[4][16], acc_c[4][16];
+#pragma unroll
+            for (int b = 0; b < 4; ++b)
+#pragma unroll
+                for (int i = 0; i < 16; ++i) { acc_m[b][i] = 0.0f; acc_c[b][i] = 0.0f; }
+            const int nseg = Policy::num_segments(p, t);
+            for (int seg = 0; seg < nseg; ++seg) {
+                const Segment sg = Policy::segment(p, t, seg);
+                MmaGroup g[2];
+                const int ng = Policy::mma_groups(p, t, seg, g);
+                const int nkc = (sg.K + CHUNK_K - 1) / CHUNK_K;
+                for (int kc = 0; kc < nkc; ++kc, ++c) {
+                    const uint32_t slot = c % NUM_SLOTS, use = c / NUM_SLOTS;
+                    tr.mark(13);
+                    mbar_wait(&landed[slot], use & 1);
+                    tr.mark(14);
+                    const unsigned char *base = ring + slot * SLOT_BYTES;
+                    // A fragment of K-step ks: rows r0 / r1, columns 8 ks + tq and 8 ks + tq + 4 -> TF32 hi / lo
+                    uint32_t a_hi[4][4], a_lo[4][4];
+#pragma unroll
+                    for (int ks = 0; ks < 4; ++ks) {
+                        const int rr[4] = {r0, r1, r0, r1};
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                            const int col = 8 * ks + tq + 4 * (i >> 1);
+                            const float x = *reinterpret_cast<const float *>(base + swz(rr[i], col >> 2) + (col & 3) * 4);
+                            const float h = tf32_hi(x);
+                            a_hi[ks][i] = __float_as_uint(h);
+                            a_lo[ks][i] = __float_as_uint(x - h);
+                        }
+                    }
+                    if (Policy::GATHER) {
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(&a_free[slot]);       // raw tile consumed (values are in registers)
+                    }
+                    const int kvalid = min(CHUNK_K, sg.K - kc * CHUNK_K);
+                    const int ksteps = (dbg & 1) ? 0 : (kvalid + 7) / 8;
+                    const uint32_t sbase = smem_u32(base);
+                    wgmma_fence();
+#pragma unroll
+                    for (int gi = 0; gi < 2; ++gi) {
+                        if (gi < ng) {
+                            const int jlo = g[gi].col_off >> 5, jhi = (g[gi].col_off + g[gi].n + 31) >> 5;
+#pragma unroll
+                            for (int j = 0; j < 4; ++j) {
+                                if (j >= jlo && j < jhi) {
+                                    const uint32_t brow = (uint32_t)(g[gi].row_off + 32 * j - g[gi].col_off);
+                                    const uint64_t b_hi0 = make_smem_desc_sw128(sbase + B_HI_OFF + brow * 128);
+                                    const uint64_t b_lo0 = make_smem_desc_sw128(sbase + B_LO_OFF + brow * 128);
+#pragma unroll
+                                    for (int ks = 0; ks < CHUNK_K / 8; ++ks) {
+                                        if (ks < ksteps) {
+                                            // x * w ~= hi*hi (main) + hi*lo + lo*hi (correction accumulator)
+                                            wgmma_tf32_rs_n32(acc_m[j], a_hi[ks], b_hi0 + ks * 2);
+                                            wgmma_tf32_rs_n32(acc_c[j], a_hi[ks], b_lo0 + ks * 2);
+                                            wgmma_tf32_rs_n32(acc_c[j], a_lo[ks], b_hi0 + ks * 2);
+                                        }
+                                    }
+                                }
+                            }
+                        }
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) { fence_acc(acc_m[j]); fence_acc(acc_c[j]); }
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&empty[slot]);            // B tiles of the slot consumed
+                    tr.mark(15);
+                }
+            }
+            // ---- accumulator tile -> shared memory (main + correction), then the policy epilogue, one row per thread
+            named_bar_sync(bar_id, 128);          // the warpgroup's previous epilogue no longer reads these rows
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const int col = 32 * j + 8 * i + 2 * tq;
+                    *reinterpret_cast<float2 *>(acc_s + r0 * ACC_PITCH + col) =
+                        make_float2(acc_m[j][4 * i] + acc_c[j][4 * i], acc_m[j][4 * i + 1] + acc_c[j][4 * i + 1]);
+                    *reinterpret_cast<float2 *>(acc_s + r1 * ACC_PITCH + col) =
+                        make_float2(acc_m[j][4 * i + 2] + acc_c[j][4 * i + 2], acc_m[j][4 * i + 3] + acc_c[j][4 * i + 3]);
+                }
+            named_bar_sync(bar_id, 128);
             float acc[64];
-            Policy::drain(p, t, tmem_lane, half, acc);
-            tc_fence_before_sync();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tmem_empty);   // the accumulators may be overwritten while we store
+            Policy::drain(p, t, acc_row, half, acc);
+            named_bar_sync(bar_id, 128);          // drained: the rows become the warps' transpose buffers
             tr.mark(22);
             if (!(dbg & 4)) Policy::store(p, t, acc, pre, half, lane, stage);
             tr.mark(23);
@@ -501,10 +423,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
             pre = pre_next;
         }
     }
-    tc_fence_before_sync();
-    __syncthreads();
-    tc_fence_after_sync();
-    if (warp == 0) tmem_dealloc<512>(tmem_base);
 }
 
 }  // namespace tc

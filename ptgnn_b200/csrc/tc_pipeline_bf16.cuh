@@ -1,16 +1,15 @@
-// bf16 variant of the persistent warp-specialised tcgen05 pipeline (see tc_pipeline.cuh for the fp32-exact one).
+// bf16 variant of the persistent warp-specialised wgmma pipeline (see tc_pipeline.cuh for the fp32-exact one).
 //
-// bf16 node states and weights, fp32 accumulation in TMEM -- the arithmetic of the reference's AMP path
+// bf16 node states and weights, fp32 accumulation in registers -- the arithmetic of the reference's AMP path
 // (torch.autocast: bf16 Linear / GRU GEMMs, fp32 scatter, abstractmessagepassing.py:43-50).  No operand splitting:
-// one tcgen05.mma.kind::f16 (K = 16) per K-step instead of three kind::tf32 (K = 8) ones, operands go from global
-// memory to the MMA without touching registers:
-//   warps 0-3  LOADERS   gathered bf16 rows via cp.async (LDGSTS, 16-byte pieces) or a TMA tile; weight tiles via TMA;
-//                        fence.proxy.async + arrive on full[slot] once this thread's pieces have landed
-//   warp  4    MMA       one thread: wait full[slot] + landed[slot]; K/16 MMAs (A, B from shared memory, SWIZZLE_128B
-//                        K-major descriptors); tcgen05.commit -> empty[slot]; per tile commit -> tmem_full[acc]
-//   warps 8-15 EPILOGUE  two sets of four warps on alternate tiles: drain the fp32 accumulator, release it, policy store
-//   shared memory: 6 slots x 32 KB (A 128 rows x 64 bf16 | B <= 128 rows x 64 bf16) + 32 KB transpose buffers
-//   tensor memory: 2 accumulator sets x 128 fp32 columns (MMAs of tile i+1 overlap the epilogue of tile i)
+// one bf16 wgmma (K = 16) per K-step, operands go from global memory to the MMA without touching registers:
+//   warps 0-3  LOADERS    gathered bf16 rows via cp.async (LDGSTS, 16-byte pieces) or a TMA tile; weight tiles via TMA;
+//                         fence.proxy.async + arrive on full[slot] once this thread's pieces have landed
+//   warps 4-11 CONSUMERS  two warpgroups (tile rows [0,64) / [64,128)): wait full[slot] + landed[slot]; K/16 wgmmas per
+//                         32-column block (A, B from shared memory, SWIZZLE_128B K-major descriptors); arrive empty[slot].
+//                         Per tile: accumulators -> a shared-memory tile, then the policy epilogue, one row per thread.
+//   shared memory: 3 slots x 32 KB (A 128 rows x 64 bf16 | B <= 128 rows x 64 bf16) + 32 KB transpose buffers +
+//                  the 128 x 132 fp32 accumulator tile
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -27,16 +26,21 @@ using tc::mbar_init;
 
 constexpr int TILE_M = 128;
 constexpr int CHUNK_K = 64;                        // bf16 per k-chunk = one 128-byte swizzled row
-constexpr int NUM_SLOTS = 6;
-constexpr int LOOKAHEAD = 4;
+constexpr int NUM_SLOTS = 3;
+constexpr int LOOKAHEAD = 2;
 constexpr int OPERAND_BYTES = TILE_M * 128;        // 16 KB
 constexpr int SLOT_BYTES = 2 * OPERAND_BYTES;      // A | B
 constexpr int RING_BYTES = NUM_SLOTS * SLOT_BYTES;
-constexpr int NUM_THREADS = 16 * 32;
-constexpr int NUM_EPI_WARPS = 8;
+constexpr int NUM_THREADS = 12 * 32;
+constexpr int NUM_CONSUMER_WARPS = 8;
 constexpr int STAGE_BYTES_PER_WARP = 32 * 32 * 4;
-constexpr int SMEM_BYTES = RING_BYTES + 1024 + 256 + NUM_EPI_WARPS * STAGE_BYTES_PER_WARP;
-constexpr int LOADER_REGS = 96, MMA_REGS = 40, EPI_REGS = 184;   // (96 + 40 + 184 + 184) * 128 = 64512
+constexpr int ACC_PITCH = tc::ACC_PITCH;
+constexpr int SMEM_BYTES = RING_BYTES + 1024 + 256 + NUM_CONSUMER_WARPS * STAGE_BYTES_PER_WARP + TILE_M * ACC_PITCH * 4;
+static_assert(SMEM_BYTES <= 232448, "shared memory budget");
+// setmaxnreg.inc only hands out registers other warpgroups of the CTA released: the three budgets must sum to 3 x 168, the
+// per-thread allocation of a 384-thread launch (__launch_bounds__(384, 1) caps the kernel at 168 registers).
+constexpr int LOADER_REGS = 104, CONSUMER_REGS = 200;
+static_assert(LOADER_REGS + 2 * CONSUMER_REGS <= 3 * 168, "register budgets exceed the launch allocation");
 
 struct Segment {        // one K-range of the tile's GEMM (all element counts in bf16)
     const __nv_bfloat16 *a;      // gathered A rows (row pitch lda) -- used when a_map == nullptr
@@ -54,23 +58,17 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_bf16_kernel(const 
     unsigned char *ring = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // offset form: keeps the shared address space
     uint64_t *bars = reinterpret_cast<uint64_t *>(ring + RING_BYTES);
     uint64_t *full = bars, *empty = bars + NUM_SLOTS, *landed = bars + 2 * NUM_SLOTS;
-    uint64_t *tmem_full = bars + 3 * NUM_SLOTS, *tmem_empty = bars + 3 * NUM_SLOTS + 2;
-    uint32_t *tmem_base_smem = reinterpret_cast<uint32_t *>(bars + 3 * NUM_SLOTS + 4);
     float *stage_base = reinterpret_cast<float *>(ring + RING_BYTES + 256);
+    float *acc_s = stage_base + NUM_CONSUMER_WARPS * STAGE_BYTES_PER_WARP / 4;
 
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // warp-uniform for the compiler
     const int lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
-        for (int s = 0; s < NUM_SLOTS; ++s) { mbar_init(&full[s], 128); mbar_init(&empty[s], 1); mbar_init(&landed[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(&tmem_full[a], 1); mbar_init(&tmem_empty[a], NUM_EPI_WARPS / 2); }
+        for (int s = 0; s < NUM_SLOTS; ++s) { mbar_init(&full[s], 128); mbar_init(&empty[s], NUM_CONSUMER_WARPS); mbar_init(&landed[s], 1); }
         tc::mbar_init_fence();
     }
-    if (warp == 0) tc::tmem_alloc<256>(tmem_base_smem);
     Policy::smem_init(p, stage_base);          // policy-owned tables in the staging area (e.g. the GRU biases)
-    tc::tc_fence_before_sync();
     __syncthreads();
-    tc::tc_fence_after_sync();
-    const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_base_smem, 0);
     const int total_tiles = Policy::num_tiles(p);
     unsigned long long *trace_base = (p.trace != nullptr && blockIdx.x == 0) ? p.trace : nullptr;
 
@@ -193,143 +191,105 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_bf16_kernel(const 
             }
         }
         cp_async_wait<0>();
-    } else if (warp < 8) {
-        // =========================================== MMA ISSUER ===========================================
-        tc::reg_dealloc<MMA_REGS>();
-        if (warp == 4) {
-            // the whole warp walks the loop converged (all lanes poll the barriers); one elected lane issues
-            const bool leader = tc::elect_one();
-            uint32_t c = 0, tcount = 0;
-            typename Policy::Tile t;
-            tc::Tracer tr{(trace_base && leader) ? trace_base + 2048 : nullptr, 0};
-            Policy::tile_init(t);
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++tcount) {
-                tr.mark(10);
-                Policy::tile_setup(p, tile, t);
-                const uint32_t acc = tcount & 1, acc_use = tcount >> 1;
-                mbar_wait(&tmem_empty[acc], (acc_use & 1) ^ 1);
-                tr.mark(12);
-                tc::tc_fence_after_sync();
-                const uint32_t tmem_acc = tmem_base + acc * 128;
-                const int nseg = Policy::num_segments(p, t);
-                for (int seg = 0; seg < nseg; ++seg) {
-                    const Segment sg = Policy::segment(p, t, seg);
-                    MmaGroup g[2];
-                    const int ng = Policy::mma_groups(p, t, seg, g);
-                    const int nkc = (sg.K + CHUNK_K - 1) / CHUNK_K;
-                    for (int kc = 0; kc < nkc; ++kc, ++c) {
-                        const uint32_t slot = c % NUM_SLOTS, use = c / NUM_SLOTS;
-                        tr.mark(13);
-                        mbar_wait(&full[slot], use & 1);
-                        tr.mark(14);
-                        if (!(p.dbg & 4)) mbar_wait(&landed[slot], use & 1);
-                        tr.mark(16);
-                        tc::tc_fence_after_sync();
-                        const uint32_t base = smem_u32(ring + slot * SLOT_BYTES);
-                        const int ksteps = (min(CHUNK_K, sg.K - kc * CHUNK_K) + 15) / 16;
-                        const uint64_t a0 = tc::make_smem_desc_sw128(base);
-#pragma unroll
-                        for (int gi = 0; gi < 2; ++gi) {
-                            if (gi < ng) {
-                                const uint64_t b0 = tc::make_smem_desc_sw128(base + OPERAND_BYTES + g[gi].row_off * 128);
-                                const uint32_t idesc = tc::make_instr_desc(tc::FMT_BF16, TILE_M, (uint32_t)g[gi].n);
-                                const uint32_t d = tmem_acc + g[gi].col_off;
-                                const uint32_t acc0 = (g[gi].fresh && kc == 0) ? 0u : 1u;
-#pragma unroll
-                                for (int ks = 0; ks < CHUNK_K / 16; ++ks)
-                                    if (ks < ksteps && !(p.dbg & 1) && leader) tc::mma_bf16_ss(d, a0 + ks * 2, b0 + ks * 2, idesc, ks == 0 ? acc0 : 1u);
-                            }
-                        }
-                        if (leader) tc::mma_commit(&empty[slot]);
-                        __syncwarp();
-                        tr.mark(15);
-                    }
-                }
-                if (leader) tc::mma_commit(&tmem_full[acc]);
-                __syncwarp();
-            }
-        }
     } else {
-        // =========================================== EPILOGUE ===========================================
-        // Two sets of four warps (one warp per TMEM lane quarter) take alternate tiles -- set s owns accumulator s.  The
-        // per-tile chain (wait, tcgen05.ld, transpose, stores queued behind the loaders' traffic) is latency-bound, so
-        // two tiles in flight per CTA double the epilogue rate; a warp covers its 32 rows in two 64-column passes.
-        tc::reg_alloc<EPI_REGS>();
-        const int ew = warp - 8, quarter = warp & 3, set = ew >> 2;
-        const uint32_t tmem_lane = tmem_base + ((uint32_t)(quarter * 32) << 16) + set * 128;
-        float *stage = stage_base + ew * (STAGE_BYTES_PER_WARP / 4);
+        // =========================================== CONSUMERS ===========================================
+        tc::reg_alloc<CONSUMER_REGS>();
+        const int cw = warp - 4;                          // 0..7
+        const int wg = cw >> 2, wi = cw & 3;              // warpgroup: tile rows [64 wg, 64 wg + 64)
+        const int gq = lane >> 2, tq = lane & 3;
+        const int r0 = 64 * wg + 16 * wi + gq, r1 = r0 + 8;
+        const int quarter = 2 * wg + (wi & 1), half = wi >> 1;   // epilogue: rows 32 quarter + lane, columns of `half`
+        const float *acc_row = acc_s + (quarter * 32 + lane) * ACC_PITCH;
+        float *stage = stage_base + cw * (STAGE_BYTES_PER_WARP / 4);
+        const int bar_id = 2 + wg;
+        uint32_t c = 0;
         typename Policy::Tile t, t_next;
-        // Everything the store needs from global memory (destination offsets, the GRU's h values) is fetched one tile
-        // ahead: a load issued when the accumulator is ready would queue behind the loaders' requests.
-        typename Policy::Pre pre[2], pre_next[2];
-        tc::Tracer tr{(trace_base && ew == 0 && lane == 0) ? trace_base + 4096 : nullptr, 0};
-        const int stride = 2 * gridDim.x;
-        int tile = blockIdx.x + set * gridDim.x;
+        // Everything the store needs from global memory (destination offsets, the GRU's h values) is fetched one tile ahead.
+        typename Policy::Pre pre, pre_next;
+        tc::Tracer tr{(trace_base && cw == 0 && lane == 0) ? trace_base + 2048 : nullptr, 0, 2048};
+        int tile = blockIdx.x;
         Policy::tile_init(t);
         if (tile < total_tiles) {
             Policy::tile_setup(p, tile, t);
-            Policy::prefetch(p, t, quarter, 0, lane, pre[0]);
-            Policy::prefetch(p, t, quarter, 1, lane, pre[1]);
+            Policy::prefetch(p, t, quarter, half, lane, pre);
         }
-        for (uint32_t use = 0; tile < total_tiles; tile += stride, ++use) {
-            const int next = tile + stride;
+        for (; tile < total_tiles; tile += gridDim.x) {
+            const int next = tile + gridDim.x;
             if (next < total_tiles) {
                 t_next = t;
                 Policy::tile_setup(p, next, t_next);
-                Policy::prefetch(p, t_next, quarter, 0, lane, pre_next[0]);
-                Policy::prefetch(p, t_next, quarter, 1, lane, pre_next[1]);
+                Policy::prefetch(p, t_next, quarter, half, lane, pre_next);
             }
-            tr.mark(20);
-            mbar_wait(&tmem_full[set], use & 1);
-            tr.mark(21);
-            tc::tc_fence_after_sync();
+            float acc[4][16];
 #pragma unroll
-            for (int pass = 0; pass < 2; ++pass) {
-                float v[64];
-                if (!(p.dbg & 8)) Policy::drain(p, t, tmem_lane, pass, v);
-                if (pass == 1) {
-                    tc::tc_fence_before_sync();
+            for (int b = 0; b < 4; ++b)
+#pragma unroll
+                for (int i = 0; i < 16; ++i) acc[b][i] = 0.0f;
+            const int nseg = Policy::num_segments(p, t);
+            for (int seg = 0; seg < nseg; ++seg) {
+                const Segment sg = Policy::segment(p, t, seg);
+                MmaGroup g[2];
+                const int ng = Policy::mma_groups(p, t, seg, g);
+                const int nkc = (sg.K + CHUNK_K - 1) / CHUNK_K;
+                for (int kc = 0; kc < nkc; ++kc, ++c) {
+                    const uint32_t slot = c % NUM_SLOTS, use = c / NUM_SLOTS;
+                    tr.mark(13);
+                    mbar_wait(&full[slot], use & 1);
+                    if (!(p.dbg & 4)) mbar_wait(&landed[slot], use & 1);
+                    tr.mark(14);
+                    const uint32_t base = smem_u32(ring + slot * SLOT_BYTES);
+                    const int ksteps = (p.dbg & 1) ? 0 : (min(CHUNK_K, sg.K - kc * CHUNK_K) + 15) / 16;
+                    const uint64_t a0 = tc::make_smem_desc_sw128(base + wg * 64 * 128);
+                    tc::wgmma_fence();
+#pragma unroll
+                    for (int gi = 0; gi < 2; ++gi) {
+                        if (gi < ng) {
+                            const int jlo = g[gi].col_off >> 5, jhi = (g[gi].col_off + g[gi].n + 31) >> 5;
+#pragma unroll
+                            for (int j = 0; j < 4; ++j) {
+                                if (j >= jlo && j < jhi) {
+                                    const uint32_t brow = (uint32_t)(g[gi].row_off + 32 * j - g[gi].col_off);
+                                    const uint64_t b0 = tc::make_smem_desc_sw128(base + OPERAND_BYTES + brow * 128);
+#pragma unroll
+                                    for (int ks = 0; ks < CHUNK_K / 16; ++ks)
+                                        if (ks < ksteps) tc::wgmma_16_ss_n32<true>(acc[j], a0 + ks * 2, b0 + ks * 2);
+                                }
+                            }
+                        }
+                    }
+                    tc::wgmma_commit();
+                    tc::wgmma_wait<0>();
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) tc::fence_acc(acc[j]);
                     __syncwarp();
-                    if (lane == 0) mbar_arrive(&tmem_empty[set]);
-                    tr.mark(22);
+                    if (lane == 0) mbar_arrive(&empty[slot]);
+                    tr.mark(15);
                 }
-                if (!(p.dbg & 2)) Policy::store(p, t, v, pre[pass], pass, lane, stage, stage_base);
             }
+            tc::named_bar_sync(bar_id, 128);      // the warpgroup's previous epilogue no longer reads these rows
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const int col = 32 * j + 8 * i + 2 * tq;
+                    *reinterpret_cast<float2 *>(acc_s + r0 * ACC_PITCH + col) = make_float2(acc[j][4 * i], acc[j][4 * i + 1]);
+                    *reinterpret_cast<float2 *>(acc_s + r1 * ACC_PITCH + col) = make_float2(acc[j][4 * i + 2], acc[j][4 * i + 3]);
+                }
+            tc::named_bar_sync(bar_id, 128);
+            float v[64];
+            if (!(p.dbg & 8)) Policy::drain(p, t, acc_row, half, v);
+            tr.mark(22);
+            if (!(p.dbg & 2)) Policy::store(p, t, v, pre, half, lane, stage, stage_base);
             tr.mark(23);
             t = t_next;
-            pre[0] = pre_next[0];
-            pre[1] = pre_next[1];
+            pre = pre_next;
         }
     }
-    tc::tc_fence_before_sync();
-    __syncthreads();
-    tc::tc_fence_after_sync();
-    if (warp == 0) tc::tmem_dealloc<256>(tmem_base);
 }
 
-// drain helpers (no correction accumulator in the bf16 path)
-__device__ __forceinline__ void drain_2x32(uint32_t taddr, int c0, int ncols, float (&acc)[64]) {
-    uint32_t m0[32], m1[32];
-    const bool b0 = c0 < ncols, b1 = c0 + 32 < ncols;
-    if (b0) tc::tmem_ld_32cols_async(taddr + c0, m0);
-    if (b1) tc::tmem_ld_32cols_async(taddr + c0 + 32, m1);
-    tc::tmem_ld_wait();
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-        if (b0) acc[i] = __uint_as_float(m0[i]);
-        if (b1) acc[32 + i] = __uint_as_float(m1[i]);
-    }
-}
-__device__ __forceinline__ void drain_4x16(uint32_t taddr, int off, float (&acc)[64]) {
-    uint32_t m[4][16];
-#pragma unroll
-    for (int g = 0; g < 4; ++g) tc::tmem_ld_16cols_async(taddr + 32 * g + off, m[g]);
-    tc::tmem_ld_wait();
-#pragma unroll
-    for (int g = 0; g < 4; ++g)
-#pragma unroll
-        for (int i = 0; i < 16; ++i) acc[16 * g + i] = __uint_as_float(m[g][i]);
-}
+// drain helpers: the accumulator tile layout is shared with the fp32 pipeline
+using tc::drain_2x32;
+using tc::drain_4x16;
 // two fp32 -> one packed bf16x2 word (round to nearest even)
 __device__ __forceinline__ float pack_bf16x2(float lo, float hi) {
     __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);

@@ -1,7 +1,7 @@
 """``GraphNeuralNetwork`` container with the reference's API, owning the layer loop.
 
 Counterpart of `/root/reference/ptgnn/neuralmodels/gnn/graphneuralnetwork.py:28-209` (class ``GraphNeuralNetwork``)
-and the carrier types of `/root/reference/ptgnn/neuralmodels/gnn/structs.py:52-76`.  Differences that matter on B200:
+and the carrier types of `ptgnn/neuralmodels/gnn/structs.py:52-76` of the reference.  Differences that matter on the GPU:
 the container builds the edge plan once per minibatch and shares it with all of its layers (the reference rebuilds the
 equivalent grouping inside every ``scatter`` call), and it never mutates the caller's ``adjacency_lists`` list in place.
 Metric bookkeeping (``num_graphs/num_nodes/num_edges``, post-expansion edge count) is bit-identical.

@@ -570,7 +570,7 @@ class MlpMessagePassingLayer(AbstractMessagePassingLayer):
             ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=h.device)
             out = torch.empty(num_nodes, out_dim, dtype=state_dtype, device=h.device)
             bp = plan.block_plan()
-            # derived copies of the edge weights (fp16 hi | lo' in the kernel's TMEM order) and of the dense weight (TF32 hi / lo): once
+            # derived copies of the edge weights (fp16 hi | lo' in the kernel's packed order) and of the dense weight (TF32 hi / lo): once
             # per parameter version, like the gated layer's (fp32 path; the bf16 path converts per call)
             cache_params = weights + ([d_w] if d_w is not None else [])
             cache, valid = self._weight_cache("mlp_f32_fused", 0 if bf16 else lib.ptgnn_b200_mlp_fused_weight_cache_bytes(

@@ -13,7 +13,7 @@ def pytest_configure(config):
         from ptgnn_b200 import _native
 
         _native.LIB_PATH = os.path.join(ROOT, os.environ["PTGNN_TOOLS_LIB"])
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100: `-m gpu`)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -1,5 +1,5 @@
 """The host-buffer C-ABI entry point (`ptgnn_b200_gated_gnn_forward_host_f32`) and the alternative operand-staging mode
-of the tcgen05 pipeline."""
+of the tensor-core pipeline."""
 import ctypes
 import os
 import subprocess

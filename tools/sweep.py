@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """BASELINE.json configs[4]: edges/s sweep over single random graphs (not block diagonal).
 
-    python tools/sweep.py [--out profiles/rNN_sweep.md] [--quick]
+    python tools/sweep.py [--out sweep.md] [--quick]
 
 One GatedMessagePassingLayer and one MlpMessagePassingLayer call per point (plan build excluded, it is once per
 minibatch): E in {1e4, 1e5, 1e6, 5e6}, N = E / 5, T in {1, 4, 16} (even split), H in {64, 128, 256}, sum and max.

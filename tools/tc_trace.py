@@ -1,4 +1,4 @@
-"""Debug: dump the CTA-0 timeline of one tcgen05 pipeline launch (PTGNN_TC_TRACE=<category>, 1 = message, 3 = gru)."""
+"""Debug: dump the CTA-0 timeline of one tensor-core pipeline launch (PTGNN_TC_TRACE=<category>, 1 = message, 3 = gru)."""
 import ctypes, os, sys
 sys.path.insert(0, os.getcwd())
 import numpy as np, torch
