@@ -34,12 +34,12 @@ static_assert(PRODUCER_REGS + 2 * CONSUMER_REGS <= 3 * 168, "register budgets ex
 constexpr int NMAX = 64;                                        // edges per MMA (accumulator columns)
 constexpr int ACC_PITCH = NMAX + 4;                             // accumulator tile: 128 features x NMAX columns, fp32
 constexpr int ACC_BYTES = kD * ACC_PITCH * 4;
-constexpr int MMA_BAR_ID = 1, EPI_BAR_ID = 2;
+constexpr int ALL_BAR_ID = 1, GRP_BAR_ID = 2;              // named barriers: both consumer warpgroups | warpgroup eg: 2 + eg
 
 struct Meta {                     // per sub-group: what the epilogue needs to know about the accumulator columns
     int32_t tloff[128];           // byte offset of the column's target row inside agg_s (0 for columns >= n)
     uint32_t endmask[4];          // bit c: column c is the last edge of its (target, type) segment
-    uint32_t lowmask[4];          // bit c: column c's target lies in the lower half of the block (epilogue warpgroup 0's columns)
+    uint32_t lowmask[4];          // bit c: column c's target lies in the lower half of the block (walked by the lower-half threads)
     int32_t n, pad[3];
 };
 struct Sched {                    // one target block: its id and the T+1 sorted-edge offsets of its (block, type) groups
@@ -76,16 +76,26 @@ __device__ __forceinline__ void named_bar_sync(int id, int threads) { asm volati
 __device__ __forceinline__ uint32_t swz(int row, int q) { return (uint32_t)(row * 128 + ((q ^ (row & 7)) << 4)); }
 
 // Debug timeline (PTGNN_FUSED_TRACE=1): CTA 0, one thread per role, records (clock64, step, tag) at the pipeline hand-offs into its
-// 2048-entry region of the trace buffer; read back with ptgnn_b200_debug_fused_trace (tools/fused_trace.py).
-struct Trace {
-    unsigned long long *buf;
-    int n;
-    __device__ __forceinline__ void mark(int tag, uint32_t step) {
-        if (buf != nullptr && n < 2048) buf[n++] = ((unsigned long long)clock64() << 24) | ((unsigned long long)(step & 0xFFFFu) << 8) | (unsigned)(tag & 0xFF);
-    }
-};
-__device__ __forceinline__ Trace make_trace(unsigned long long *base, int role, bool on) {
-    return Trace{(base != nullptr && blockIdx.x == 0 && on) ? base + role * 2048 : nullptr, 0};
+// TRACE_CAP-entry region of the trace buffer; read back with ptgnn_b200_debug_fused_trace (tools/fused_trace.py).
+// Roles: 0 = gatherer thread 0, 1 / 2 = lane 0 of warp 0 of consumer warpgroup 0 / 1.  Tags:
+//   gatherer  1 slot wait begins, 2 slot granted, 3 copies issued, 4 x_full arrival
+//   consumer 10 step begins, 11 the step's weight fragment loads issued (only when the (type, segment) changes; usually during
+//            the previous step or before a write-out, see the look-ahead below), 12 x_full acquired, 13 MMAs issued (the issue
+//            stalls until the fragments have arrived), 14 MMAs retired (step index); 20 staging begins, 21 staging done,
+//            22 column walk done (sub-group index); 23 / 24 write-out begins / ends
+// The write counters live in shared memory and the buffer pointer is read from the kernel parameters at every mark, so the
+// marks hold no registers across the code between them.
+constexpr int TRACE_ROLES = 3, TRACE_CAP = 8192;
+__shared__ uint32_t trace_n[TRACE_ROLES];
+__device__ __forceinline__ void trace_mark(const Params &p, int tag, uint32_t step) {
+    if (p.trace == nullptr || blockIdx.x != 0) return;
+    const int tid = (int)threadIdx.x;
+    const int role = tid == GATHER_WARP0 * 32 ? 0 : (tid == 0 ? 1 : (tid == 128 ? 2 : -1));
+    if (role < 0) return;
+    const uint32_t n = trace_n[role];
+    if (n >= TRACE_CAP) return;
+    p.trace[role * TRACE_CAP + n] = ((unsigned long long)clock64() << 24) | ((unsigned long long)(step & 0xFFFFu) << 8) | (unsigned)(tag & 0xFF);
+    trace_n[role] = n + 1;
 }
 
 // ---- the (block, group, sub-group, segment) walk every role performs in the same order -----------------------------------
@@ -180,13 +190,16 @@ template <int RED> __device__ __forceinline__ float red_op(float a, float m) {
 }
 
 // =====================================================================================================================
-// Write-out of a finished block: rows [row_lo, min(row_hi, rows of the block)) of agg_s, taken by the calling warp (ew of the four
-// of its group) 2 rows at a time; a row is reset to the identity as soon as it has been read.  The row loop is specialised at compile
-// time on the output format and on "plain sum" (no mean / max fix-up / activation / LayerNorm): the generic version executed ~180
-// instructions per row.  It runs in the consumer threads, which keep their weight fragments live across it: the fp32 instances
-// already spill a little (`-Xptxas -v`; DESIGN.md §9 item 2), so check that a change does not add to it.
-template <int RED>
-__device__ __forceinline__ void write_out_block(const Params *p, uint32_t agg_saddr, int row0, int row_lo, int row_hi, int ew, int lane) {
+// Write-out of a finished block: the calling thread takes float4 column q (features 4 q .. 4 q + 3) of rows row_lo + r_first,
+// + r_step, + 2 r_step, ... below min(row_hi, rows of the block), two rows per iteration; a value is reset to the identity as soon
+// as it has been read.  WHOLE_ROW: a warp owns whole rows (q = lane), which the LayerNorm epilogue needs for its row reductions;
+// otherwise a half-warp owns the 64 features of its warpgroup in a row.  The row loop is specialised at compile time on the output
+// format and on "plain sum" (no mean / max fix-up / activation / LayerNorm): the generic version executed ~180 instructions per
+// row.  It runs in the consumer threads, which keep their weight fragments live across it: the fp32 instances already spill a
+// little (`-Xptxas -v`), so check that a change does not add to it.
+template <int RED, bool WHOLE_ROW>
+__device__ __forceinline__ void write_out_block(const Params *p, uint32_t agg_saddr, int row0, int row_lo, int row_hi, int r_first,
+                                                int r_step, int q) {
     const float IDENT = red_identity<RED>();
     const int rows = min(p->B, p->num_nodes - row0);
     const int my_hi = min(row_hi, rows);
@@ -211,7 +224,7 @@ __device__ __forceinline__ void write_out_block(const Params *p, uint32_t agg_sa
                 a.x = apply_act(a.x, p->epi.act); a.y = apply_act(a.y, p->epi.act);
                 a.z = apply_act(a.z, p->epi.act); a.w = apply_act(a.w, p->epi.act);
             }
-            if (p->epi.ln_w != nullptr) {       // LayerNorm over the 128 features of the row (same order as reduce.cuh)
+            if (WHOLE_ROW && p->epi.ln_w != nullptr) {       // LayerNorm over the 128 features of the row (same order as reduce.cuh)
                 float sum = (a.x + a.y) + (a.z + a.w);
 #pragma unroll
                 for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
@@ -221,8 +234,8 @@ __device__ __forceinline__ void write_out_block(const Params *p, uint32_t agg_sa
 #pragma unroll
                 for (int o = 16; o > 0; o >>= 1) qq += __shfl_xor_sync(0xffffffffu, qq, o);
                 const float rstd = rsqrtf(qq / (float)kD + p->epi.ln_eps);
-                const float4 w = *reinterpret_cast<const float4 *>(p->epi.ln_w + lane * 4);
-                const float4 b = *reinterpret_cast<const float4 *>(p->epi.ln_b + lane * 4);
+                const float4 w = *reinterpret_cast<const float4 *>(p->epi.ln_w + q * 4);
+                const float4 b = *reinterpret_cast<const float4 *>(p->epi.ln_b + q * 4);
                 a.x = dx * rstd * w.x + b.x; a.y = dy * rstd * w.y + b.y;
                 a.z = dz * rstd * w.z + b.z; a.w = dw * rstd * w.w + b.w;
             }
@@ -231,37 +244,37 @@ __device__ __forceinline__ void write_out_block(const Params *p, uint32_t agg_sa
             __nv_bfloat162 lo = __floats2bfloat162_rn(a.x, a.y), hi = __floats2bfloat162_rn(a.z, a.w);
             uint2 pk;
             pk.x = *reinterpret_cast<uint32_t *>(&lo); pk.y = *reinterpret_cast<uint32_t *>(&hi);
-            reinterpret_cast<uint2 *>(p->out)[(size_t)v * (kD / 4) + lane] = pk;
+            reinterpret_cast<uint2 *>(p->out)[(size_t)v * (kD / 4) + q] = pk;
         } else if (MODE == 2) {      // fp16 (hi | lo') row: hi halfs at [0, 128), lo' halfs at [128, 256); packed conversions
             const __half2 h01 = __floats2half2_rn(a.x, a.y), h23 = __floats2half2_rn(a.z, a.w);
             const float2 f01 = __half22float2(h01), f23 = __half22float2(h23);
             const __half2 l01 = __floats2half2_rn((a.x - f01.x) * 2048.0f, (a.y - f01.y) * 2048.0f);
             const __half2 l23 = __floats2half2_rn((a.z - f23.x) * 2048.0f, (a.w - f23.y) * 2048.0f);
             uint2 *row = reinterpret_cast<uint2 *>(p->out) + (size_t)v * (2 * kD / 4);
-            row[lane] = make_uint2(*reinterpret_cast<const uint32_t *>(&h01), *reinterpret_cast<const uint32_t *>(&h23));
-            row[kD / 4 + lane] = make_uint2(*reinterpret_cast<const uint32_t *>(&l01), *reinterpret_cast<const uint32_t *>(&l23));
+            row[q] = make_uint2(*reinterpret_cast<const uint32_t *>(&h01), *reinterpret_cast<const uint32_t *>(&h23));
+            row[kD / 4 + q] = make_uint2(*reinterpret_cast<const uint32_t *>(&l01), *reinterpret_cast<const uint32_t *>(&l23));
             const float big = fmaxf(fmaxf(fabsf(a.x), fabsf(a.y)), fmaxf(fabsf(a.z), fabsf(a.w)));
             if (!(big < 65504.0f) && p->status != nullptr) *reinterpret_cast<volatile int32_t *>(p->status) = 1;
         } else {
-            reinterpret_cast<float4 *>(p->out)[(size_t)v * (kD / 4) + lane] = a;
+            reinterpret_cast<float4 *>(p->out)[(size_t)v * (kD / 4) + q] = a;
         }
     };
     // 2 rows per iteration (independent loads in flight); rows are reset as they are read: the next block needs no initialisation pass
     auto write_rows = [&](auto mode_tag, auto plain_tag) {
-        for (int r0 = row_lo + ew; r0 < my_hi; r0 += 4 * 2) {
+        for (int r0 = row_lo + r_first; r0 < my_hi; r0 += 2 * r_step) {
             float4 v4[2];
 #pragma unroll
             for (int u = 0; u < 2; ++u) {
-                const int r = r0 + 4 * u;
+                const int r = r0 + r_step * u;
                 if (r < my_hi) {
-                    const uint32_t rowa = agg_saddr + (uint32_t)(r * kD + lane * 4) * 4u;
+                    const uint32_t rowa = agg_saddr + (uint32_t)(r * kD + q * 4) * 4u;
                     v4[u] = lds_f32x4(rowa);
                     sts_f32x4(rowa, ident4);
                 }
             }
 #pragma unroll
             for (int u = 0; u < 2; ++u)
-                if (r0 + 4 * u < my_hi) finish_row(mode_tag, plain_tag, r0 + 4 * u, v4[u]);
+                if (r0 + r_step * u < my_hi) finish_row(mode_tag, plain_tag, r0 + r_step * u, v4[u]);
         }
     };
     const bool plain = RED == PTGNN_REDUCE_SUM && p->epi.act == PTGNN_ACT_NONE && p->epi.ln_w == nullptr;
@@ -300,6 +313,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
         // ordinary arrival that publishes the step's column metadata
         for (int s = 0; s < NUM_SLOTS; ++s) { mbar_init(&x_full[s], 2 * GATHER_THREADS); mbar_init(&x_empty[s], 8); }
         for (int r = 0; r < SCHED_RING; ++r) { mbar_init(&sched_full[r], 1); mbar_init(&sched_empty[r], NUM_CONSUMER_WARPS); }
+        for (int r = 0; r < TRACE_ROLES; ++r) trace_n[r] = 0;
         tc::mbar_init_fence();
     }
     __syncthreads();
@@ -334,7 +348,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
             const int q = g & 7, rsub = g >> 3;
             StepGen<NSEG> gen{sched, sched_full, sched_empty, T, NMAX, lane};
             uint32_t c_issue = 0, c_done = 0, sgc = 0;
-            Trace tr = make_trace(p.trace, 0, g == 0);
             // Everything a step needs from global memory (row indices, the targets of its columns) is loaded ONE STEP AHEAD:
             // `fetch` only issues the loads, the copies of the current step are issued while they are in flight, `finish_meta`
             // consumes them afterwards.
@@ -391,9 +404,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
                 finish_meta(cur);                      // consumes the loads of the PREVIOUS call
                 fetch();                               // loads for the following step: in flight during the copies below
                 const uint32_t slot = c_issue % NUM_SLOTS;
-                tr.mark(1, c_issue);
+                trace_mark(p, 1, c_issue);
                 mbar_wait(&x_empty[slot], ((c_issue / NUM_SLOTS) & 1) ^ 1);
-                tr.mark(2, c_issue);
+                trace_mark(p, 2, c_issue);
                 const unsigned char *rows = cur.seg == 0 ? p.src_rows : p.tgt_rows;
                 const uint32_t sbase = smem_u32(ring + slot * SLOT_BYTES) + swz(rsub, q);
 #pragma unroll
@@ -405,7 +418,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
                             cp_async16(sbase + ti * TILE_BYTES + i * 1024, src + (ti / KCH) * (K * 2) + (ti % KCH) * 128, 16);
                     }
                 }
-                tr.mark(3, c_issue);
+                trace_mark(p, 3, c_issue);
                 ++c_issue;
             };
             fetch();
@@ -419,7 +432,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
                 issue_next();
                 more = has_nxt;
                 asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(&x_full[slot])) : "memory");
-                tr.mark(4, c_done);
+                trace_mark(p, 4, c_done);
                 mbar_arrive(&x_full[slot]);            // release: this thread's metadata stores of the step
                 ++c_done;
             }
@@ -428,156 +441,220 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
     } else {
         // ============================================ CONSUMERS ============================================
         // MMA: warpgroup eg computes message features [64 eg, 64 eg + 64) of every sub-group, A = W_t rows (register fragments,
-        // loaded from the packed weights when the (type, segment) changes), B = the gathered rows of the slot (N = 64 edges);
-        // the finished sub-group goes to acc_s[feature][edge] (main + 2^-11 correction).
-        // Epilogue: thread d of a warpgroup owns message feature d and column d of agg_s.  For every accumulator column (edge) in
-        // plan order: at the first edge of a (target, type) segment the running value is (re)loaded from agg_s[target][d], at the
-        // last one it is stored back -- a target's messages are accumulated one by one in the reference's order, across types
-        // and sub-groups.  Group 0 takes the columns whose target lies in the lower half of the block, group 1 the upper half.
-        // Edges are sorted by target, so each group owns a contiguous column range of every sub-group and the two never touch
-        // the same agg_s row -- no synchronisation between them except around acc_s and at the block's write-out.
+        // loaded from the packed weights when the (type, segment) changes), B = the gathered rows of the slot, N = the
+        // sub-group's edge count rounded up to 16; the finished sub-group goes to rows [64 eg, 64 eg + 64) of
+        // acc_s[feature][edge] (main + 2^-11 correction).
+        // Reduction: thread d owns feature fw, i.e. column fw of agg_s, for the targets of one half of the block.  For every
+        // accumulator column (edge) of its half, in plan order: at the first edge of a (target, type) segment the running value is
+        // (re)loaded from agg_s[target][fw], at the last one it is stored back -- a target's messages are accumulated one by one in
+        // the reference's order, across types and sub-groups.  Edges are sorted by target, so each half owns a contiguous column
+        // range of every sub-group.  Two assignments:
+        //  * SPLIT (fp32, 3xFP16): warpgroup eg also reduces and writes out its own features, fw = 64 eg + (d & 63); warps 0-1 take
+        //    the lower half, warps 2-3 the upper half.  The warpgroups touch disjoint acc_s rows and disjoint agg_s columns, so they
+        //    never wait for each other (except around the LayerNorm write-out, which needs whole rows): one issues its three
+        //    products' MMAs while the other reduces.  How far they can drift apart is bounded by the x ring: a slot is refilled
+        //    only after all 8 consumer warps have released it.
+        //  * lock-step (bf16): fw = d, warpgroup eg takes half eg for all 128 features, so both meet around the staging.  A bf16
+        //    step's MMAs are too short to hide a column walk behind; split, the bf16 kernel was measured 6-12 % slower.
+        // Meta ring reuse: the gatherers write the metadata of step c before they wait for its slot, i.e. after every consumer
+        // warp has released step c - 1 - NUM_SLOTS; a warp that has released step k reads only metadata of sub-groups >= k's.  So
+        // the slowest reader is at most NUM_SLOTS + 1 = 4 sub-groups behind the writer, inside the META_RING = 8 entries.
+        // SPLIT: weight fragments are loaded one event ahead: right after a step's MMAs retire (or before a block's write-out)
+        // the walk is advanced to the next step, and if that step needs other weights their loads are issued then, so the L2
+        // round trip runs under the staging, the column walk and the write-out instead of in front of the next MMA.  Lock-step
+        // (bf16) loads them in line at the step (measured 1.5 % faster there).
         tc::reg_alloc<CONSUMER_REGS>();
+        constexpr bool SPLIT = NPROD == 3;
         const int eg = warp >> 2, ew = warp & 3;
         const int d = ew * 32 + lane;
         const int gq = lane >> 2, tq = lane & 3;
         const int f0 = 64 * eg + 16 * ew + gq;               // this thread's A / accumulator rows: features f0, f0 + 8
-        const uint32_t aggcol_s = smem_u32(agg_s + d);      // shared-space address of agg_s[0][d]
-        const uint32_t accrow_s = smem_u32(acc_s + d * ACC_PITCH);
+        // the feature this thread reduces, and which targets: 0 = the lower half of the block, 1 = the upper half
+        const int fw = SPLIT ? 64 * eg + (d & 63) : d, half = SPLIT ? d >> 6 : eg;
+        const uint32_t aggcol_s = smem_u32(agg_s + fw);     // shared-space address of agg_s[0][fw]
+        const uint32_t accrow_s = smem_u32(acc_s + fw * ACC_PITCH);
+        const int grp_bar = GRP_BAR_ID + eg;
+        const int stage_bar = SPLIT ? grp_bar : ALL_BAR_ID, stage_threads = SPLIT ? 128 : 256;   // around the staging
         const float IDENT = red_identity<RED>();
         StepGen<NSEG> gen{sched, sched_full, sched_empty, T, NMAX, lane};
-        const int row_lo = eg == 0 ? 0 : (p.B >> 1), row_hi = eg == 0 ? (p.B >> 1) : p.B;     // rows this group initialises
-        for (int r = row_lo; r < row_hi; ++r) agg_s[r * kD + d] = IDENT;
+        {
+            const int row_lo = half == 0 ? 0 : (p.B >> 1), row_hi = half == 0 ? (p.B >> 1) : p.B;     // the rows this thread walks
+            for (int r = row_lo; r < row_hi; ++r) agg_s[r * kD + fw] = IDENT;
+        }
         uint32_t sg = 0, xs = 0;
         int w_t = -1, w_seg = -1;
         uint32_t wf[NPART][K / 16][4];
         float acc_m[32], acc_c[32];
         float acc = IDENT;
-        Trace tr = make_trace(p.trace, 2 + eg, ew == 0 && lane == 0);
-        Step s;
-        for (;;) {
-            const int ev = gen.next(s);
-            if (ev == 2) break;
-            if (ev == 0) {
-                if (s.t != w_t || s.seg != w_seg) {
-                    // packed layout: wpack[(((t * NSEG + seg) * NPART + part) * (K / 8) + c4) * 128 + d] = columns 8 c4 .. + 7 of row d
-                    const uint32_t *wp = reinterpret_cast<const uint32_t *>(p.wpack + (size_t)(s.t * NSEG + s.seg) * NPART * (K / 8) * 128);
+        auto load_weights = [&](const Step &st) {
+            // packed layout: wpack[(((t * NSEG + seg) * NPART + part) * (K / 8) + c4) * 128 + d] = columns 8 c4 .. + 7 of row d
+            const uint32_t *wp = reinterpret_cast<const uint32_t *>(p.wpack + (size_t)(st.t * NSEG + st.seg) * NPART * (K / 8) * 128);
 #pragma unroll
-                    for (int part = 0; part < NPART; ++part)
+            for (int part = 0; part < NPART; ++part)
 #pragma unroll
-                        for (int ks = 0; ks < K / 16; ++ks)
+                for (int ks = 0; ks < K / 16; ++ks)
 #pragma unroll
-                            for (int i = 0; i < 4; ++i) {
-                                const int c4 = (part * (K / 8) + 2 * ks + (i >> 1)), f = f0 + 8 * (i & 1);
-                                wf[part][ks][i] = __ldg(wp + ((size_t)c4 * 128 + f) * 4 + tq);
-                            }
-                    w_t = s.t; w_seg = s.seg;
+                    for (int i = 0; i < 4; ++i) {
+                        const int c4 = (part * (K / 8) + 2 * ks + (i >> 1)), f = f0 + 8 * (i & 1);
+                        wf[part][ks][i] = __ldg(wp + ((size_t)c4 * 128 + f) * 4 + tq);
+                    }
+            w_t = st.t; w_seg = st.seg;
+            trace_mark(p, 11, xs);
+        };
+        // the MMAs of one step over the first 16 NB accumulator columns (NB = 1 .. 4)
+        auto mma = [&](auto nb_tag, uint32_t slot_addr) {
+            constexpr int NB = decltype(nb_tag)::value;
+#pragma unroll
+            for (int ks = 0; ks < K / 16; ++ks) {
+                const int kc = ks >> 2, kk = ks & 3;
+                const uint64_t x_hi = tc::make_smem_desc_sw128(slot_addr + kc * TILE_BYTES) + kk * 2;
+                const uint64_t x_lo = tc::make_smem_desc_sw128(slot_addr + (KCH + kc) * TILE_BYTES) + kk * 2;
+                auto one = [&](float (&dacc)[32], const uint32_t (&a)[4], uint64_t desc) {
+                    if (NB == 1) tc::wgmma_16_rs_n16<BF16>(dacc, a, desc);
+                    else if (NB == 2) tc::wgmma_16_rs_n32<BF16>(dacc, a, desc);
+                    else if (NB == 3) tc::wgmma_16_rs_n48<BF16>(dacc, a, desc);
+                    else tc::wgmma_16_rs_n64<BF16>(dacc, a, desc);
+                };
+                one(acc_m, wf[0][ks], x_hi);
+                if (NPROD == 3) {
+                    // x * w ~= hi*hi (main) + 2^-11 (hi*lo' + lo'*hi) (correction accumulator, scaled by 2^11)
+                    one(acc_c, wf[0][ks], x_lo);
+                    one(acc_c, wf[NPART - 1][ks], x_hi);
                 }
+            }
+        };
+        Step s, nx;
+        int ev = gen.next(s);
+        while (ev != 2) {
+            if (ev == 0) {
+                trace_mark(p, 10, xs);
+                if (s.t != w_t || s.seg != w_seg) load_weights(s);      // the first step, or the first after a block without steps
                 const uint32_t slot = xs % NUM_SLOTS;
-                tr.mark(13, xs);
                 mbar_wait(&x_full[slot], (xs / NUM_SLOTS) & 1);
                 tc::fence_proxy_async_smem();          // rows written by cp.async (generic proxy) -> read by the MMA (async proxy)
-                if (s.seg == 0) {
+                trace_mark(p, 12, xs);
+                // Branches around the MMAs and around writes to their registers test warp-uniform values (broadcast from lane 0):
+                // on a path ptxas cannot prove uniform it may serialise the wgmmas (C7520 in -Xptxas -v; none is reported now).
+                if (tc::warp_uniform(s.seg) == 0) {
 #pragma unroll
                     for (int i = 0; i < 32; ++i) { acc_m[i] = 0.0f; acc_c[i] = 0.0f; }
                 }
                 const uint32_t slot_addr = smem_u32(ring + slot * SLOT_BYTES);
+                const int nb = tc::warp_uniform((s.n + 15) >> 4);
                 tc::wgmma_fence();
-#pragma unroll
-                for (int ks = 0; ks < K / 16; ++ks) {
-                    const int kc = ks >> 2, kk = ks & 3;
-                    const uint64_t x_hi = tc::make_smem_desc_sw128(slot_addr + kc * TILE_BYTES) + kk * 2;
-                    tc::wgmma_16_rs_n64<BF16>(acc_m, wf[0][ks], x_hi);
-                    if (NPROD == 3) {
-                        // x * w ~= hi*hi (main) + 2^-11 (hi*lo' + lo'*hi) (correction accumulator, scaled by 2^11)
-                        const uint64_t x_lo = tc::make_smem_desc_sw128(slot_addr + (KCH + kc) * TILE_BYTES) + kk * 2;
-                        tc::wgmma_16_rs_n64<BF16>(acc_c, wf[0][ks], x_lo);
-                        tc::wgmma_16_rs_n64<BF16>(acc_c, wf[NPART - 1][ks], x_hi);
-                    }
-                }
+                using std::integral_constant;
+                if (nb == 1) mma(integral_constant<int, 1>{}, slot_addr);
+                else if (nb == 2) mma(integral_constant<int, 2>{}, slot_addr);
+                else if (nb == 3) mma(integral_constant<int, 3>{}, slot_addr);
+                else mma(integral_constant<int, 4>{}, slot_addr);
                 tc::wgmma_commit();
+                trace_mark(p, 13, xs);
                 tc::wgmma_wait<0>();
                 tc::fence_acc(acc_m);
                 tc::fence_acc(acc_c);
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&x_empty[slot]);
-                tr.mark(14, xs);
+                trace_mark(p, 14, xs);
                 ++xs;
-                if (s.seg != NSEG - 1) continue;
-                // ---- the sub-group's messages -> acc_s (feature-major), then the reduction along the columns
-                named_bar_sync(MMA_BAR_ID, 256);        // both groups are done with the previous sub-group's acc_s
+                const int evn = gen.next(nx);          // look ahead; the fragments are free until nx's MMAs
+                if (SPLIT && evn == 0 && (nx.t != w_t || nx.seg != w_seg)) load_weights(nx);
+                if (s.seg == NSEG - 1) {
+                    // ---- the sub-group's messages -> this group's rows of acc_s (feature-major), then the reduction along the columns
+                    trace_mark(p, 20, sg);
+                    named_bar_sync(stage_bar, stage_threads);    // the readers of these acc_s rows are done with the previous sub-group
 #pragma unroll
-                for (int j = 0; j < 8; ++j)
+                    for (int j = 0; j < 8; ++j) {
+                        if (8 * j < 16 * nb) {          // columns the MMA did not compute are never read
 #pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        float v0 = acc_m[4 * j + 2 * h], v1 = acc_m[4 * j + 2 * h + 1];
-                        if (NPROD == 3) { v0 = fmaf(acc_c[4 * j + 2 * h], 1.0f / 2048.0f, v0); v1 = fmaf(acc_c[4 * j + 2 * h + 1], 1.0f / 2048.0f, v1); }
-                        *reinterpret_cast<float2 *>(acc_s + (f0 + 8 * h) * ACC_PITCH + 8 * j + 2 * tq) = make_float2(v0, v1);
-                    }
-                named_bar_sync(MMA_BAR_ID, 256);
-                tr.mark(21, sg);
-                const Meta *m = &meta_ring[sg % META_RING];
-                const int n = s.n;
-                int split = __popc(m->lowmask[0]) + __popc(m->lowmask[1]);
-                const int c_lo = eg == 0 ? 0 : split, c_hi = eg == 0 ? split : n;       // this group's columns
-                constexpr int W = 16;
-                for (int c0 = c_lo & ~15; c0 < c_hi; c0 += 16) {
-                    uint32_t vm[W];
-#pragma unroll
-                    for (int j = 0; j < W / 4; ++j) {
-                        const float4 v4 = lds_f32x4(accrow_s + (uint32_t)(c0 + 4 * j) * 4u);
-                        vm[4 * j] = __float_as_uint(v4.x); vm[4 * j + 1] = __float_as_uint(v4.y);
-                        vm[4 * j + 2] = __float_as_uint(v4.z); vm[4 * j + 3] = __float_as_uint(v4.w);
-                    }
-                    uint32_t addr[W];
-#pragma unroll
-                    for (int j = 0; j < W / 4; ++j) {
-                        const int4 o = *reinterpret_cast<const int4 *>(&m->tloff[c0 + 4 * j]);
-                        addr[4 * j] = aggcol_s + o.x; addr[4 * j + 1] = aggcol_s + o.y;
-                        addr[4 * j + 2] = aggcol_s + o.z; addr[4 * j + 3] = aggcol_s + o.w;
-                    }
-                    const uint32_t endw = (m->endmask[c0 >> 5] >> (c0 & 31)) & 0xFFFFu;
-                    // the column before this batch ended a segment (or the batch opens the sub-group: always reload)
-                    const uint32_t prev_end = c0 == 0 ? 1u : (m->endmask[(c0 - 1) >> 5] >> ((c0 - 1) & 31)) & 1u;
-                    const uint32_t startw = (endw << 1) | prev_end;
-                    // columns of the batch that belong to this group: [max(c_lo, c0), min(c_hi, c0 + 16))
-                    const int first = c_lo > c0 ? c_lo - c0 : 0, last = c_hi - c0 < W ? c_hi - c0 : W;
-                    const uint32_t storew = endw & (0xFFFFu << first) & (0xFFFFu >> (W - last));
-                    float pre[W];
-#pragma unroll
-                    for (int c = 0; c < W; ++c) pre[c] = lds_f32(addr[c]);
-                    // t[c] = op(pre[c], v[c]) for every column (independent); a column that CONTINUES a segment (rare: most
-                    // (target, type) segments hold one edge) then overwrites it with op(t[c-1], v[c]) -- a predicated op, in
-                    // column order, so a target's messages are still combined one by one in plan order.  Columns of the other
-                    // group are computed but never stored; this group's first column always starts a segment.
-                    float t[W];
-                    constexpr bool ADD = RED == PTGNN_REDUCE_SUM || RED == PTGNN_REDUCE_MEAN;
-#pragma unroll
-                    for (int c = 0; c < W; ++c) {
-                        float v = __uint_as_float(vm[c]);
-                        if (NPROD == 1) {                           // the autocast Linear's bf16 output
-                            v = __bfloat162float(__float2bfloat16_rn(v));
-                            vm[c] = __float_as_uint(v);
+                        for (int h = 0; h < 2; ++h) {
+                            float v0 = acc_m[4 * j + 2 * h], v1 = acc_m[4 * j + 2 * h + 1];
+                            if (NPROD == 3) { v0 = fmaf(acc_c[4 * j + 2 * h], 1.0f / 2048.0f, v0); v1 = fmaf(acc_c[4 * j + 2 * h + 1], 1.0f / 2048.0f, v1); }
+                            *reinterpret_cast<float2 *>(acc_s + (f0 + 8 * h) * ACC_PITCH + 8 * j + 2 * tq) = make_float2(v0, v1);
                         }
-                        t[c] = ADD ? __fadd_rn(pre[c], v) : red_op<RED>(pre[c], v);
+                        }
                     }
-                    continue_segment<RED>(t[0], acc, __uint_as_float(vm[0]), startw & 1u);
+                    named_bar_sync(stage_bar, stage_threads);
+                    trace_mark(p, 21, sg);
+                    const Meta *m = &meta_ring[sg % META_RING];
+                    const int n = s.n;
+                    int split = __popc(m->lowmask[0]) + __popc(m->lowmask[1]);
+                    const int c_lo = half == 0 ? 0 : split, c_hi = half == 0 ? split : n;       // this thread's columns
+                    constexpr int W = 16;
+                    for (int c0 = c_lo & ~15; c0 < c_hi; c0 += 16) {
+                        uint32_t vm[W];
 #pragma unroll
-                    for (int c = 1; c < W; ++c) continue_segment<RED>(t[c], t[c - 1], __uint_as_float(vm[c]), startw & (1u << c));
-                    acc = t[W - 1];
+                        for (int j = 0; j < W / 4; ++j) {
+                            const float4 v4 = lds_f32x4(accrow_s + (uint32_t)(c0 + 4 * j) * 4u);
+                            vm[4 * j] = __float_as_uint(v4.x); vm[4 * j + 1] = __float_as_uint(v4.y);
+                            vm[4 * j + 2] = __float_as_uint(v4.z); vm[4 * j + 3] = __float_as_uint(v4.w);
+                        }
+                        uint32_t addr[W];
 #pragma unroll
-                    for (int c = 0; c < W; ++c) sts_f32_if(addr[c], t[c], storew & (1u << c));
+                        for (int j = 0; j < W / 4; ++j) {
+                            const int4 o = *reinterpret_cast<const int4 *>(&m->tloff[c0 + 4 * j]);
+                            addr[4 * j] = aggcol_s + o.x; addr[4 * j + 1] = aggcol_s + o.y;
+                            addr[4 * j + 2] = aggcol_s + o.z; addr[4 * j + 3] = aggcol_s + o.w;
+                        }
+                        const uint32_t endw = (m->endmask[c0 >> 5] >> (c0 & 31)) & 0xFFFFu;
+                        // the column before this batch ended a segment (or the batch opens the sub-group: always reload)
+                        const uint32_t prev_end = c0 == 0 ? 1u : (m->endmask[(c0 - 1) >> 5] >> ((c0 - 1) & 31)) & 1u;
+                        const uint32_t startw = (endw << 1) | prev_end;
+                        // columns of the batch that belong to this thread: [max(c_lo, c0), min(c_hi, c0 + 16))
+                        const int first = c_lo > c0 ? c_lo - c0 : 0, last = c_hi - c0 < W ? c_hi - c0 : W;
+                        const uint32_t storew = endw & (0xFFFFu << first) & (0xFFFFu >> (W - last));
+                        float pre[W];
+#pragma unroll
+                        for (int c = 0; c < W; ++c) pre[c] = lds_f32(addr[c]);
+                        // t[c] = op(pre[c], v[c]) for every column (independent); a column that CONTINUES a segment (rare: most
+                        // (target, type) segments hold one edge) then overwrites it with op(t[c-1], v[c]) -- a predicated op, in
+                        // column order, so a target's messages are still combined one by one in plan order.  Columns of the other
+                        // half are computed but never stored (those beyond the MMA's N hold stale values); this thread's first
+                        // column always starts a segment.
+                        float t[W];
+                        constexpr bool ADD = RED == PTGNN_REDUCE_SUM || RED == PTGNN_REDUCE_MEAN;
+#pragma unroll
+                        for (int c = 0; c < W; ++c) {
+                            float v = __uint_as_float(vm[c]);
+                            if (NPROD == 1) {                           // the autocast Linear's bf16 output
+                                v = __bfloat162float(__float2bfloat16_rn(v));
+                                vm[c] = __float_as_uint(v);
+                            }
+                            t[c] = ADD ? __fadd_rn(pre[c], v) : red_op<RED>(pre[c], v);
+                        }
+                        continue_segment<RED>(t[0], acc, __uint_as_float(vm[0]), startw & 1u);
+#pragma unroll
+                        for (int c = 1; c < W; ++c) continue_segment<RED>(t[c], t[c - 1], __uint_as_float(vm[c]), startw & (1u << c));
+                        acc = t[W - 1];
+#pragma unroll
+                        for (int c = 0; c < W; ++c) sts_f32_if(addr[c], t[c], storew & (1u << c));
+                    }
+                    trace_mark(p, 22, sg);
+                    ++sg;
                 }
-                tr.mark(22, sg);
-                ++sg;
+                s = nx; ev = evn;
                 continue;
             }
-            // ---- block finished.  Each group writes out ITS half of the rows as soon as its own four warps are done (no waiting for
-            // the other group).
-            tr.mark(23, sg);
-            named_bar_sync(EPI_BAR_ID + eg, 128);
-            write_out_block<RED>(&p, smem_u32(agg_s), s.blk * p.B, row_lo, row_hi, ew, lane);
-            named_bar_sync(EPI_BAR_ID + eg, 128);
-            tr.mark(24, sg);
+            // ---- block s.blk finished.  Each group writes out its 64 features of every row as soon as its own four warps are done
+            // (no waiting for the other group); the next sub-group's first staging barrier orders these reads and resets before
+            // that group's next column walk.  The LayerNorm epilogue needs whole rows: both groups meet, each writes out half of the
+            // rows, and they meet again before either walks the next block.
+            const int blk = s.blk;
+            const int evn = gen.next(nx);
+            if (SPLIT && evn == 0 && (nx.t != w_t || nx.seg != w_seg)) load_weights(nx);
+            trace_mark(p, 23, sg);
+            if (SPLIT && p.epi.ln_w == nullptr) {
+                named_bar_sync(grp_bar, 128);
+                write_out_block<RED, false>(&p, smem_u32(agg_s), blk * p.B, 0, p.B, 2 * ew + (lane >> 4), 8, 16 * eg + (lane & 15));
+            } else {
+                // whole rows, warpgroup eg the rows of half eg; in lock-step mode those are exactly the rows it walked
+                const int wbar = SPLIT ? ALL_BAR_ID : grp_bar, wthreads = SPLIT ? 256 : 128;
+                named_bar_sync(wbar, wthreads);
+                const int row_lo = eg == 0 ? 0 : (p.B >> 1), row_hi = eg == 0 ? (p.B >> 1) : p.B;
+                write_out_block<RED, true>(&p, smem_u32(agg_s), blk * p.B, row_lo, row_hi, ew, 4, lane);
+                named_bar_sync(wbar, wthreads);
+            }
+            trace_mark(p, 24, sg);
+            s = nx; ev = evn;
         }
     }
 }
@@ -742,8 +819,8 @@ static unsigned long long *trace_buffer() {
     static int want = -1;
     if (want < 0) { const char *e = getenv("PTGNN_FUSED_TRACE"); want = (e && e[0] == '1') ? 1 : 0; }
     if (!want) return nullptr;
-    if (!g_trace_dev && cudaMalloc(&g_trace_dev, 5 * 2048 * 8) != cudaSuccess) return nullptr;
-    cudaMemset(g_trace_dev, 0, 5 * 2048 * 8);
+    if (!g_trace_dev && cudaMalloc(&g_trace_dev, TRACE_ROLES * TRACE_CAP * 8) != cudaSuccess) return nullptr;
+    cudaMemset(g_trace_dev, 0, TRACE_ROLES * TRACE_CAP * 8);
     return g_trace_dev;
 }
 
@@ -782,10 +859,14 @@ int aggregate(const AggregateArgs &a, cudaStream_t st) {
 }  // namespace fused
 }  // namespace ptgnn
 
-// debug only (not part of the public header): copies the last fused-kernel timeline (5 roles x 2048 entries) to `out`; 0 if tracing is off
+// debug only (not part of the public header): copies the last fused-kernel timeline (TRACE_ROLES x TRACE_CAP entries) to `out`
+// when `out` is not null, and returns TRACE_CAP; 0 if tracing is off
 extern "C" int ptgnn_b200_debug_fused_trace(unsigned long long *out) {
-    if (!ptgnn::fused::g_trace_dev) return 0;
-    cudaDeviceSynchronize();
-    cudaMemcpy(out, ptgnn::fused::g_trace_dev, 5 * 2048 * 8, cudaMemcpyDeviceToHost);
-    return 1;
+    using namespace ptgnn::fused;
+    if (!g_trace_dev) return 0;
+    if (out != nullptr) {
+        cudaDeviceSynchronize();
+        cudaMemcpy(out, g_trace_dev, TRACE_ROLES * TRACE_CAP * 8, cudaMemcpyDeviceToHost);
+    }
+    return TRACE_CAP;
 }

@@ -8,8 +8,8 @@
 // Orientation.  The per-type weight W_t [D = 128, K] is the MMA's A operand (M = D, two warpgroups of 64 rows, held in
 // registers); the gathered node-state rows are the B operand (N = 64 edges of one (target block, edge type) sub-group) in
 // shared memory; the accumulator is therefore msg^T: row = message feature d, column = edge.  Two things follow: (1) a
-// group of n edges costs ceil(n / 64) N = 64 MMAs, not a padded 128-row tile -- (block, type) groups hold a few dozen
-// edges; (2) the reduction over edges of the same target runs ALONG the columns of one row: the accumulator goes through a
+// group of n edges costs ceil(n / 64) MMAs of at most N = 64 columns, each sized to its sub-group (N = 16 ceil(n' / 16)), not a
+// padded 128-row tile -- (block, type) groups hold a few dozen edges; (2) the reduction over edges of the same target runs ALONG the columns of one row: the accumulator goes through a
 // feature-major shared-memory tile and the thread that owns feature d runs a plain sequential loop over it: no shuffles,
 // no atomics, accumulation in the reference's edge order (per target: type-major, then list order), bit-reproducible.
 //
@@ -27,9 +27,11 @@
 // represented: the packing kernels raise a status flag and the host raises (PTGNN_B200_FP32_MODE=tf32 selects the
 // unfused 3xTF32 kernels).
 //
-// Roles (12 warps):  0-3 and 4-7 CONSUMERS, two warpgroups: MMAs for features [0,64) / [64,128), then the epilogue over all
-//   128 features -- group 0 takes the columns whose target lies in the lower half of the block, group 1 the upper half
-//   (disjoint agg_s rows) | 8-9 ROW GATHERERS (16-byte cp.async into a 3-slot ring, SWIZZLE_128B K-major) |
+// Roles (12 warps):  0-3 and 4-7 CONSUMERS, two warpgroups computing the MMAs for features [0,64) / [64,128).  fp32: each
+//   also reduces and writes out its own features (disjoint agg_s columns: the groups run independently, one's MMAs overlap the
+//   other's reduction); inside a group warps 0-1 reduce the columns whose target lies in the lower half of the block, warps
+//   2-3 the upper half.  bf16: lock-step, group 0 reduces all 128 features of the lower-half targets, group 1 the upper half |
+//   8-9 ROW GATHERERS (16-byte cp.async into a 3-slot ring, SWIZZLE_128B K-major) |
 //   10 SCHEDULER (block -> group offsets table ring).
 #pragma once
 #include "common.cuh"
