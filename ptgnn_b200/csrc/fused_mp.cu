@@ -349,8 +349,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
             StepGen<NSEG> gen{sched, sched_full, sched_empty, T, NMAX, lane};
             uint32_t c_issue = 0, c_done = 0, sgc = 0;
             // Everything a step needs from global memory (row indices, the targets of its columns) is loaded ONE STEP AHEAD:
-            // `fetch` only issues the loads, the copies of the current step are issued while they are in flight, `finish_meta`
-            // consumes them afterwards.
+            // `fetch` only issues the loads, right after the current step has been published; `finish_meta` and the copies of
+            // the next step consume them.  The look-up of the next step may wait for a scheduler entry (past blocks without
+            // edges), and the consumers release entries only when they have the current step: so it must come after the
+            // current step's x_full arrival (before it, a block with edges followed by three empty ones in this CTA's order
+            // deadlocked the kernel).
             Step cur, nxt;
             bool has_nxt = false;
             int idx_nxt[NMAX / 8];
@@ -396,13 +399,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
                 if (g == 0) m->n = st.n;
                 ++sgc;
             };
-            auto issue_next = [&]() {                  // issue the copies of `nxt`, prefetch the step after it
+            auto issue_next = [&]() {                  // issue the copies of `nxt`
                 cur = nxt;
                 int idx[NMAX / 8];
 #pragma unroll
                 for (int i = 0; i < NMAX / 8; ++i) idx[i] = idx_nxt[i];
-                finish_meta(cur);                      // consumes the loads of the PREVIOUS call
-                fetch();                               // loads for the following step: in flight during the copies below
+                finish_meta(cur);                      // consumes the loads of the last `fetch`
                 const uint32_t slot = c_issue % NUM_SLOTS;
                 trace_mark(p, 1, c_issue);
                 mbar_wait(&x_empty[slot], ((c_issue / NUM_SLOTS) & 1) ^ 1);
@@ -430,11 +432,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
             while (more) {
                 const uint32_t slot = c_issue % NUM_SLOTS;
                 issue_next();
-                more = has_nxt;
                 asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(&x_full[slot])) : "memory");
                 trace_mark(p, 4, c_done);
                 mbar_arrive(&x_full[slot]);            // release: this thread's metadata stores of the step
                 ++c_done;
+                fetch();                               // loads for the following step
+                more = has_nxt;
             }
             cp_async_wait<0>();
         }

@@ -24,6 +24,7 @@ class EdgePlan:
 
     __slots__ = (
         "num_nodes", "num_source_nodes", "num_edges", "num_types", "type_off", "type_off_c", "row_ptr", "src32", "tgt32", "status", "device", "_keepalive", "_validated", "_block", "_sorted", "_counts_c",
+        "_block_targets",
     )
 
     # status words (pinned host memory the kernels write directly, so the host can poll them without synchronising):
@@ -32,9 +33,18 @@ class EdgePlan:
     STATUS_WORDS = 4
 
     def __init__(self, adjacency_lists: Adjacency, num_nodes: int, validate: bool = False,
-                 num_source_nodes: Optional[int] = None):
+                 num_source_nodes: Optional[int] = None, block_targets: Optional[int] = None):
         """``num_nodes`` = number of TARGET rows (CSR rows).  ``num_source_nodes`` (default: the same) bounds the source
-        ids; it differs only for node-range shards, where targets are local rows and sources index the gathered states."""
+        ids; it differs only for node-range shards, where targets are local rows and sources index the gathered states.
+        ``block_targets`` fixes the fused kernel's target-block size B (a multiple of 8 in [8, 176]); None picks
+        ``recommended_block_targets(num_nodes)``.  Results do not depend on B; tests use it to reach block layouts (many
+        blocks per CTA, small or odd half-blocks) that the recommended size would not produce for their graph."""
+        if block_targets is not None:
+            bt = int(block_targets)
+            if bt != block_targets or bt % 8 != 0 or not 8 <= bt <= 176:     # 176 = fused_mp.cuh kMaxBlockTargets
+                raise ValueError(f"block_targets={block_targets!r} must be a multiple of 8 in [8, 176]")
+            block_targets = bt
+        self._block_targets = block_targets
         if len(adjacency_lists) > 128:
             raise NotImplementedError("more than 128 edge types")
         if len(adjacency_lists) == 0:
@@ -128,7 +138,9 @@ class EdgePlan:
     def block_plan(self) -> "N.BlockPlanStruct":
         if self._block is None:
             lib = N.lib()
-            B = int(lib.ptgnn_b200_block_plan_block_targets(self.num_nodes))
+            B = self._block_targets
+            if B is None:
+                B = int(lib.ptgnn_b200_block_plan_block_targets(self.num_nodes))
             nblk = (self.num_nodes + B - 1) // B
             dev = self.device
             group_off = torch.empty(nblk * self.num_types + 1, dtype=torch.int32, device=dev)

@@ -47,6 +47,26 @@ def test_block_plan_bit_exact(n, counts):
     assert int(P._native.lib().ptgnn_b200_block_plan_block_targets(10**8)) == 176   # large graphs get the largest block
 
 
+@pytest.mark.parametrize("block_targets", [8, 24, 88, 176])
+@pytest.mark.parametrize("n,counts", [(1000, [3000, 0, 1500, 700]), (5000, [20000, 1, 130]), (17, [5]), (240, [900, 900])])
+def test_block_plan_bit_exact_explicit_block_targets(n, counts, block_targets):
+    """EdgePlan(block_targets=B) builds its block plan at B (n = 1000, 5000, 17 are not multiples of any of these B; 240 is one
+    of 8 and 24 but not of 88 or 176)."""
+    import ptgnn_b200 as P
+
+    gen = torch.Generator().manual_seed(n)
+    adj = random_adjacency(gen, n, counts)
+    plan = P.EdgePlan(_dev(adj), n, block_targets=block_targets)
+    bp = plan.block_plan()
+    assert plan.block_targets == block_targets and bp.block_targets == block_targets
+    ref = O.block_plan(adj, n, block_targets)
+    _, group_off, src_f, tl_f, _ = plan._block
+    E = sum(counts)
+    assert np.array_equal(group_off.cpu().numpy(), ref["group_off"])
+    assert np.array_equal(src_f.cpu().numpy()[:E], ref["src_f"])
+    assert np.array_equal(tl_f.cpu().numpy()[:E], ref["tl_f"])
+
+
 @pytest.mark.parametrize("agg", ["sum", "mean", "max", "min"])
 @pytest.mark.parametrize("n,H,counts", [
     (3001, 128, [9000, 9000, 5000, 1, 130, 0, 2000]),
