@@ -100,6 +100,8 @@ __device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint64_t *bar) {
     asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+// Count towards named barrier `id` without waiting: the producer side of a barrier that other threads bar.sync on.
+__device__ __forceinline__ void named_bar_arrive(int id, int threads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
 // ---- epilogue transposes through shared memory ---------------------------------------------------------------
 // The epilogue holds the accumulator one ROW per thread; storing that directly makes every warp-wide store touch 32
