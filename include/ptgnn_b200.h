@@ -363,6 +363,40 @@ int ptgnn_b200_edge_messages_f32(const float *source_states, const float *target
                                  float *messages, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * GruGlobalStateUpdate (reference globalgraphexchange.py:13-72 with reduceops/varsizedsummary.py:26-81):
+ *   g[b] = readout_{n in graph b} x_n ;  h'_n = GRUCell(g[graph(n)], h_n)
+ *
+ * graph_readout: g [num_graphs, H] fp32 from the node states (fp32, or bf16 when bf16_states != 0; fp32 accumulation).
+ *   row_ptr [G+1] / perm [N] = the plan of the node -> graph map (ptgnn_b200_plan_build over the single edge list
+ *   (node_to_graph_idx, node_to_graph_idx) with G targets): the nodes grouped by graph, in node order inside each graph.
+ *   mode SUM / MEAN: s_n = 1 (mean divides by the graph's node count; a graph without nodes gives 0).
+ *   mode WEIGHTED_SUM: s_n = sigmoid(x_n . gate_weight), gate_weight [H] fp32 (WeightedSumVarSizedElementReduce);
+ *   s (optional, [N] fp32) receives s_n.  Deterministic: no float atomics (summation order: DESIGN.md §3.5).
+ *   H must be a multiple of 32 in [32, 256].
+ * global_gru_update: out = GRUCell(g[graph_of_node[n]], h_n) with g [num_graphs, summary_dim] fp32.  The input-side
+ *   pre-activations g W_ih^T + b_ih have num_graphs distinct rows: they are computed once as a table (ptgnn_b200_linear_f32),
+ *   then the weights-stationary GRU kernel runs over the node rows with state chunks only.  node_states / out_states: fp32
+ *   (3xFP16 products) or bf16 (bf16 products) [N, H]; packed_states_in / packed_states_out (optional, fp32 only): the packed
+ *   form of ptgnn_b200_gated_forward_fused_chained.  status (optional): status[0] = 1 if a state is outside the fp16 range.
+ *   H must be a multiple of 64 (ptgnn_b200_global_gru_supported), summary_dim a multiple of 4.  weight_cache: as for the
+ *   gated layer (the packed W_hh and biases; cache_valid = 0 re-derives them).
+ * ---------------------------------------------------------------------------------------------- */
+enum { PTGNN_READOUT_SUM = 0, PTGNN_READOUT_MEAN = 1, PTGNN_READOUT_WEIGHTED_SUM = 2 };
+size_t ptgnn_b200_graph_readout_workspace_bytes(int64_t num_nodes, int64_t num_graphs, int32_t state_dim);
+int ptgnn_b200_graph_readout(int32_t bf16_states, const void *node_states, int64_t num_nodes, int32_t state_dim, const int32_t *row_ptr,
+                             const int32_t *perm, int64_t num_graphs, const float *gate_weight /* NULL unless WEIGHTED_SUM */,
+                             int32_t mode, float *g, float *s /* optional */, void *workspace, size_t workspace_bytes, void *stream);
+int32_t ptgnn_b200_global_gru_supported(int32_t bf16_states, int32_t state_dim);
+size_t ptgnn_b200_global_gru_workspace_bytes(int32_t bf16_states, int64_t num_nodes, int64_t num_graphs, int32_t state_dim,
+                                             int32_t summary_dim);
+size_t ptgnn_b200_global_gru_weight_cache_bytes(int32_t bf16_states, int32_t state_dim);
+int ptgnn_b200_global_gru_update(int32_t bf16_states, const void *node_states, const void *packed_states_in, int64_t num_nodes,
+                                 int32_t state_dim, const int32_t *graph_of_node, int64_t num_graphs, const float *g, int32_t summary_dim,
+                                 const float *gru_w_ih, const float *gru_w_hh, const float *gru_b_ih, const float *gru_b_hh,
+                                 void *out_states, void *packed_states_out, int32_t *status, void *workspace, size_t workspace_bytes,
+                                 void *weight_cache, size_t weight_cache_bytes, int32_t cache_valid, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Host-buffer convenience entry point (used for the end-to-end measurement): all pointers are HOST
  * memory; copies inputs to the device, builds the plan, runs `num_layers` GatedMessagePassingLayers
  * (layer l uses weight set l; pass the same pointers to share weights), copies the final states back

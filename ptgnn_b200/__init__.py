@@ -9,6 +9,7 @@ from .aggregation import PnaMessageAggregation
 from .batching import MinibatchAssembler
 from .edgeplan import EdgePlan, clear_plan_cache, plan_for
 from .egc import EGCMessagePassingLayer
+from .globalexchange import AbstractGlobalGraphExchange, GruGlobalStateUpdate
 from .gnn import GnnOutput, GraphNeuralNetwork
 from .messagepassing import (
     MLP,
@@ -17,6 +18,12 @@ from .messagepassing import (
     GatedMessagePassingLayer,
     MlpMessagePassingLayer,
 )
+from .reduceops import (
+    AbstractVarSizedElementReduce,
+    ElementsToSummaryRepresentationInput,
+    SimpleVarSizedElementReduce,
+    WeightedSumVarSizedElementReduce,
+)
 from .residuallayers import ConcatResidualLayer, LinearResidualLayer, MeanResidualLayer
 from .scatter import scatter, scatter_add, scatter_max, scatter_mean, scatter_min, scatter_sum
 
@@ -24,5 +31,7 @@ __all__ = [
     "EdgePlan", "plan_for", "clear_plan_cache", "GnnOutput", "GraphNeuralNetwork", "MLP", "AbstractMessageAggregation",
     "PnaMessageAggregation", "AbstractMessagePassingLayer", "GatedMessagePassingLayer", "MlpMessagePassingLayer", "EGCMessagePassingLayer", "MeanResidualLayer",
     "ConcatResidualLayer", "LinearResidualLayer", "MinibatchAssembler", "scatter", "scatter_add",
+    "AbstractGlobalGraphExchange", "GruGlobalStateUpdate", "AbstractVarSizedElementReduce", "ElementsToSummaryRepresentationInput",
+    "SimpleVarSizedElementReduce", "WeightedSumVarSizedElementReduce",
     "scatter_sum", "scatter_mean", "scatter_max", "scatter_min",
 ]

@@ -13,6 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libptgnn_b200.so")
 
 REDUCE = {"sum": 0, "add": 0, "mean": 1, "max": 2, "min": 3}
+READOUT_SUM, READOUT_MEAN, READOUT_WEIGHTED_SUM = 0, 1, 2
 ACT_NONE, ACT_GELU, ACT_TANH, ACT_RELU = 0, 1, 2, 3
 
 c_i32, c_i64, c_f32, c_void_p, c_size_t = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_void_p, ctypes.c_size_t
@@ -85,6 +86,15 @@ SIGNATURES = {
     "ptgnn_b200_edge_messages_workspace_bytes": (c_size_t, [c_i32, c_i32, c_i32, c_i32]),
     "ptgnn_b200_edge_messages_f32": (ctypes.c_int, [c_void_p, c_void_p, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                                     c_i32, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "ptgnn_b200_graph_readout_workspace_bytes": (c_size_t, [c_i64, c_i64, c_i32]),
+    "ptgnn_b200_graph_readout": (ctypes.c_int, [c_i32, c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_i64, c_void_p, c_i32, c_void_p, c_void_p,
+                                                c_void_p, c_size_t, c_void_p]),
+    "ptgnn_b200_global_gru_supported": (c_i32, [c_i32, c_i32]),
+    "ptgnn_b200_global_gru_workspace_bytes": (c_size_t, [c_i32, c_i64, c_i64, c_i32, c_i32]),
+    "ptgnn_b200_global_gru_weight_cache_bytes": (c_size_t, [c_i32, c_i32]),
+    "ptgnn_b200_global_gru_update": (ctypes.c_int, [c_i32, c_void_p, c_void_p, c_i64, c_i32, c_void_p, c_i64, c_void_p, c_i32, c_void_p, c_void_p,
+                                                    c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_size_t,
+                                                    c_i32, c_void_p]),
     "ptgnn_b200_gated_gnn_forward_host_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_i32,
                                                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i32, c_void_p]),
 }

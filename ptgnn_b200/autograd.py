@@ -423,3 +423,88 @@ def gated_forward_composed(layer_weights, gru, node_states, adjacency_lists, edg
         msgs.append(_LinearFn.apply(x, w, None))
     agg = _SegmentReduceFn.apply(torch.cat(msgs, dim=0), plan, reduce_name)
     return _GRUCellFn.apply(agg, node_states, gru.weight_ih, gru.weight_hh, gru.bias_ih, gru.bias_hh)
+
+
+# =====================================================================================================================
+# GruGlobalStateUpdate (globalgraphexchange.py:13-72): readout g = reduce_{n in b} s_n x_n, dropout on g (a torch op between the two
+# Functions, so autograd keeps its mask), then h' = GRUCell(g[graph(n)], h_n).  fp32 states.
+# =====================================================================================================================
+class _GraphReadoutFn(torch.autograd.Function):
+    """g [G, H] on the native readout (weighted sum, sum, mean) or the segmented reduce with arg-max node ids (max, min)."""
+
+    @staticmethod
+    def forward(ctx, kind, plan, node_to_graph_idx, h, gate_weight):
+        from .reduceops import reduce_states
+
+        x = h.detach().contiguous()
+        ctx.kind, ctx.plan = kind, plan
+        if kind in ("max", "min"):
+            g, arg = C.segment_reduce(x, plan, N.REDUCE[kind], return_arg=True)
+            ctx.save_for_backward(arg)
+            return g
+        g, s = reduce_states(kind, None if gate_weight is None else gate_weight.detach(), x, node_to_graph_idx, plan, want_gates=True)
+        ctx.save_for_backward(x, s, gate_weight)
+        return g
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, d_g):
+        kind, plan = ctx.kind, ctx.plan
+        d_g = d_g.contiguous()
+        if kind in ("max", "min"):
+            (arg,) = ctx.saved_tensors
+            num_nodes = plan.num_edges
+            d_x = torch.zeros(num_nodes + 1, d_g.shape[1], dtype=d_g.dtype, device=d_g.device)   # row N takes the empty graphs' sentinel
+            d_x.scatter_(0, arg, d_g)                                                            # one graph per node: no collisions
+            return None, None, None, d_x[:num_nodes], None
+        x, s, w = ctx.saved_tensors
+        gid = plan.tgt32.long()
+        d_gn = d_g.index_select(0, gid)                                  # [N, H]: the gradient of each node's graph
+        if kind == "mean":
+            cnt = (plan.row_ptr[1:] - plan.row_ptr[:-1]).clamp(min=1).to(torch.float32)
+            return None, None, None, d_gn / cnt.index_select(0, gid)[:, None], None
+        if kind == "sum":
+            return None, None, None, d_gn, None
+        # weighted sum: d x_n = s_n d g_b + s_n (1 - s_n) (x_n . d g_b) w ;  d w = sum_n s_n (1 - s_n) (x_n . d g_b) x_n
+        q = s * (1.0 - s) * (x * d_gn).sum(dim=1)
+        d_x = s[:, None] * d_gn + q[:, None] * w.detach().reshape(1, -1)
+        return None, None, None, d_x, (q[None, :] @ x) if w.requires_grad else None
+
+
+def graph_readout_with_grad(kind, gate_weight, node_states, node_to_graph_idx, plan):
+    return _GraphReadoutFn.apply(kind, plan, node_to_graph_idx, node_states, gate_weight)
+
+
+class _GlobalGruFn(torch.autograd.Function):
+    """h' = GRUCell(g[graph(n)], h_n) on the table GRU kernel; backward: the GRUCell backward with the input side reduced per graph."""
+
+    @staticmethod
+    def forward(ctx, layer, plan, h, g, w_ih, w_hh, b_ih, b_hh):
+        with torch.no_grad():
+            out = layer.table_update(h.detach(), g.detach(), plan)
+        ctx.save_for_backward(h, g, w_ih, w_hh, b_ih, b_hh)
+        ctx.plan = plan
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        h, g, w_ih, w_hh, b_ih, b_hh = (t.detach().contiguous() for t in ctx.saved_tensors)
+        plan = ctx.plan
+        gi = C.linear(g, w_ih, b_ih).index_select(0, plan.tgt32.long())     # the [G, 3H] table, gathered per node
+        gh = C.linear(h, w_hh, b_hh)
+        d_gi, d_gh, d_h = torch.empty_like(gi), torch.empty_like(gh), torch.empty_like(h)
+        with torch.cuda.device(h.device):
+            rc = N.lib().ptgnn_b200_gru_gate_grads_f32(N.ptr(gi), N.ptr(gh), N.ptr(h), N.ptr(grad_out.contiguous()), h.shape[0], h.shape[1],
+                                                      N.ptr(d_gi), N.ptr(d_gh), N.ptr(d_h), N.current_stream(h.device))
+        N.check(rc, "ptgnn_b200_gru_gate_grads_f32")
+        d_h = d_h + C.linear(d_gh, w_hh.t().contiguous())
+        d_table = C.segment_reduce(d_gi, plan, N.REDUCE["sum"])             # [G, 3H]: per graph, in node order
+        d_g = C.linear(d_table, w_ih.t().contiguous())                      # [G, S]
+        with _exact_fp16_gemms():
+            d_w_hh = _mm_t_split(_split16(d_gh), _split16(h, False))
+        return None, None, d_h, d_g, d_table.t() @ g, d_w_hh, d_table.sum(dim=0), d_gh.sum(dim=0)
+
+
+def global_gru_with_grad(layer, node_states, summaries, plan, w_ih, w_hh, b_ih, b_hh):
+    return _GlobalGruFn.apply(layer, plan, node_states, summaries, w_ih, w_hh, b_ih, b_hh)

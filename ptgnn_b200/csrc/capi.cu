@@ -5,6 +5,8 @@
 #include <vector>
 
 #include "common.cuh"
+#include "fused_mp.cuh"
+#include "gru_ws.cuh"
 
 namespace ptgnn {
 
@@ -166,4 +168,87 @@ extern "C" int ptgnn_b200_gated_gnn_forward_host_f32(const float *node_states, i
         return PTGNN_E_INDEX;
     }
     return PTGNN_OK;
+}
+
+// ---- GruGlobalStateUpdate: input-side table + state-only weights-stationary GRU ---------------------------------------
+namespace {
+// workspace: gi table [G, 3H] fp32 | linear's workspace | packed states (fp32, when not handed in) | packed weights (no cache)
+struct GlobalGruWs { size_t gi, lin, xpack, wpack, total; };
+GlobalGruWs global_gru_layout(int bf16, int64_t N, int64_t G, int H, int S) {
+    GlobalGruWs w{};
+    const int nprod = bf16 ? 1 : 3;
+    w.gi = 0;
+    w.lin = ws_slice((size_t)G * 3 * H, 4);
+    w.xpack = w.lin + align_up(ptgnn_b200_linear_workspace_bytes(S, 3 * H), 256);
+    w.wpack = w.xpack + (bf16 ? 0 : align_up(fused::packed_state_bytes(3, N, H), 256));
+    w.total = w.wpack + align_up(gruws::pack_table_bytes(nprod, H), 256);
+    return w;
+}
+}  // namespace
+
+extern "C" int32_t ptgnn_b200_global_gru_supported(int32_t bf16_states, int32_t state_dim) {
+    return gruws::supported_table(bf16_states ? 1 : 3, state_dim) ? 1 : 0;
+}
+extern "C" size_t ptgnn_b200_global_gru_workspace_bytes(int32_t bf16_states, int64_t num_nodes, int64_t num_graphs, int32_t state_dim,
+                                                        int32_t summary_dim) {
+    if (num_nodes < 0 || num_graphs < 0 || summary_dim <= 0 || !ptgnn_b200_global_gru_supported(bf16_states, state_dim)) return 0;
+    return global_gru_layout(bf16_states, num_nodes, num_graphs, state_dim, summary_dim).total;
+}
+extern "C" size_t ptgnn_b200_global_gru_weight_cache_bytes(int32_t bf16_states, int32_t state_dim) {
+    if (!ptgnn_b200_global_gru_supported(bf16_states, state_dim)) return 0;
+    return gruws::pack_table_bytes(bf16_states ? 1 : 3, state_dim);
+}
+
+extern "C" int ptgnn_b200_global_gru_update(int32_t bf16_states, const void *node_states, const void *packed_states_in, int64_t num_nodes,
+                                            int32_t state_dim, const int32_t *graph_of_node, int64_t num_graphs, const float *g,
+                                            int32_t summary_dim, const float *gru_w_ih, const float *gru_w_hh, const float *gru_b_ih,
+                                            const float *gru_b_hh, void *out_states, void *packed_states_out, int32_t *status, void *workspace,
+                                            size_t workspace_bytes, void *weight_cache, size_t weight_cache_bytes, int32_t cache_valid,
+                                            void *stream) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int H = state_dim, S = summary_dim, nprod = bf16_states ? 1 : 3;
+    PTGNN_CHECK_ARG(num_nodes >= 0 && num_nodes < INT32_MAX && num_graphs >= 0 && num_graphs < INT32_MAX, "global_gru: sizes out of range");
+    if (!gruws::supported_table(nprod, H)) {
+        set_error("global_gru: state dim %d has no state-only GRU kernel (needs a multiple of 64)", H);
+        return PTGNN_E_UNSUPPORTED;
+    }
+    PTGNN_CHECK_ARG(S > 0 && S % 4 == 0 && S <= 4096, "global_gru: summary dim %d must be a multiple of 4 in [4, 4096]", S);
+    PTGNN_CHECK_ARG(!bf16_states || (packed_states_in == nullptr && packed_states_out == nullptr), "global_gru: packed states are fp32-only");
+    if (num_nodes == 0) return PTGNN_OK;
+    PTGNN_CHECK_ARG(num_graphs > 0, "global_gru: nodes without graphs");
+    PTGNN_CHECK_ARG(node_states && graph_of_node && g && gru_w_ih && gru_w_hh && gru_b_ih && gru_b_hh && out_states, "global_gru: null pointer");
+    const GlobalGruWs L = global_gru_layout(bf16_states, num_nodes, num_graphs, H, S);
+    if (workspace_bytes < L.total || !workspace) {
+        set_error("global_gru: workspace %zu < required %zu", workspace_bytes, L.total);
+        return PTGNN_E_WORKSPACE;
+    }
+    char *ws = static_cast<char *>(workspace);
+    char *wpack = ws + L.wpack;
+    bool pack = true;
+    if (weight_cache != nullptr) {
+        if (weight_cache_bytes < gruws::pack_table_bytes(nprod, H)) {
+            set_error("global_gru: weight cache %zu < required %zu", weight_cache_bytes, gruws::pack_table_bytes(nprod, H));
+            return PTGNN_E_WORKSPACE;
+        }
+        wpack = static_cast<char *>(weight_cache);
+        pack = !cache_valid;
+    }
+    if (pack) {
+        int rc = gruws::pack_table(nprod, H, gru_w_hh, gru_b_hh, wpack, st);
+        if (rc) return rc;
+    }
+    // the input side, once per graph: gi = g W_ih^T + b_ih  [G, 3H]
+    float *gi = reinterpret_cast<float *>(ws + L.gi);
+    int rc = ptgnn_b200_linear_f32(g, num_graphs, S, gru_w_ih, gru_b_ih, 3 * H, PTGNN_ACT_NONE, gi, ws + L.lin, L.xpack - L.lin, st);
+    if (rc) return rc;
+    const void *h_rows = node_states;
+    if (!bf16_states) {
+        h_rows = packed_states_in;
+        if (h_rows == nullptr) {
+            rc = fused::pack_states(static_cast<const float *>(node_states), num_nodes, H, ws + L.xpack, status, st);
+            if (rc) return rc;
+            h_rows = ws + L.xpack;
+        }
+    }
+    return gruws::update_table(nprod, h_rows, node_states, num_nodes, H, gi, graph_of_node, wpack, out_states, packed_states_out, status, st);
 }

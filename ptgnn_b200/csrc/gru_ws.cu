@@ -26,6 +26,12 @@
 // Within a tile, chunk c + 1's MMAs are issued before chunk c's slot is released (wgmma_wait<1>), and the blend's h loads are
 // issued before the last chunk's MMAs retire.  The gate math runs straight on the accumulator registers: every gate block
 // has the same fragment layout, so a thread holds all four gates of each (row, hidden unit) it owns.
+//
+// State-only instance (TABLE = true; GruGlobalStateUpdate, reference globalgraphexchange.py:47-64): the input of every row is
+// its graph's summary, so the input-side pre-activations gi = g W_ih^T + b_ih have only G distinct rows.  The caller computes
+// that [G, 3H] fp32 table once; the kernel keeps only P2 resident, streams only state chunks, and its epilogue takes i_r, i_z
+// and i_n from the table row of the row's graph:  r = sigma((h W_hr + b_hr) + gi_r), z likewise, n = tanh(gi_n + r (h W_hn + b_hn)).
+// The table loads are issued with the blend's h loads, before the last chunk's MMAs retire.
 #include "gru_ws.cuh"
 
 #include <cuda.h>
@@ -52,13 +58,15 @@ struct Params {
     CUtensorMap map_p1, map_p2;          // B: [n_jb * NPART * 96, D] and [n_jb * NPART * 96, H] 16-bit, box {64, NPART * 96}
     const float *h32;                    // NPROD 3: fp32 states for the blend
     const __nv_bfloat16 *h16;            // NPROD 1
-    const float4 *bias4;                 // (b_ir + b_hr, b_iz + b_hz, b_in, b_hn) per hidden unit
+    const float4 *bias4;                 // (b_ir + b_hr, b_iz + b_hz, b_in, b_hn) per hidden unit; TABLE: (b_hr, b_hz, 0, b_hn)
     void *out;                           // fp32 [N, H] (NPROD 3) or bf16 (NPROD 1)
     __half *out_packed;                  // optional (NPROD 3): the new states also as fp16 (hi | lo') rows of 2H halfs -- what the next
                                          // layer's fused aggregation and GRU take as MMA operands (saves its pack_states pass)
     int32_t *status;                     // optional: status[0] = 1 if a new state is outside the fp16 range (out_packed only)
     int num_nodes, H, D, n_jb, n_tiles;
     int num_slots;                       // ring depth: as many slots as the shared memory left by the weights holds (Geometry)
+    const float *gi;                     // TABLE: [G, 3H] fp32 input-side pre-activations (bias b_ih included), gates r, z, n
+    const int32_t *gid;                  // TABLE: [N] graph of every row
 };
 
 template <int NPROD> struct Geometry {
@@ -98,7 +106,7 @@ __device__ __forceinline__ void mma_chunk(float (&rz_m)[32], float (&x_m)[16], f
     }
 }
 
-template <int NPROD>
+template <int NPROD, bool TABLE>
 __global__ void __launch_bounds__(NUM_THREADS, 1) gru_ws_kernel(const __grid_constant__ Params p) {
     using G = Geometry<NPROD>;
     constexpr int NPART = G::NPART;
@@ -106,7 +114,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gru_ws_kernel(const __grid_con
     unsigned char *ring = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     const uint32_t num_slots = (uint32_t)p.num_slots;
     unsigned char *bres = ring + num_slots * G::SLOT_BYTES;                       // resident weights: state chunks, then aggregate chunks
-    const int kch_h = p.H / 64, kch_d = p.D / 64;
+    const int kch_h = p.H / 64, kch_d = TABLE ? 0 : p.D / 64;
     float4 *bias_s = reinterpret_cast<float4 *>(bres + G::b_bytes(p.H, p.D));
     uint64_t *bars = reinterpret_cast<uint64_t *>(reinterpret_cast<unsigned char *>(bias_s) + p.H * 16);
     uint64_t *a_full = bars, *a_empty = bars + G::MAX_SLOTS;
@@ -144,7 +152,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gru_ws_kernel(const __grid_con
             for (int t = t0; t < p.n_tiles; t += t_stride) {
                 for (int ch = 0; ch < chunks_per_tile; ++ch) {
                     mbar_wait(&a_empty[slot], phase ^ 1);
-                    const bool state_seg = ch < kch_h;
+                    const bool state_seg = TABLE || ch < kch_h;
                     const CUtensorMap *map = state_seg ? &p.map_h : &p.map_agg;
                     const int kc = state_seg ? ch : ch - kch_h, K = state_seg ? p.H : p.D;
                     unsigned char *dst = ring + slot * G::SLOT_BYTES;
@@ -188,7 +196,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gru_ws_kernel(const __grid_con
                 const uint64_t a_hi = tc::make_smem_desc_sw128(a_addr), a_lo = tc::make_smem_desc_sw128(a_addr + G::A_TILE);
                 const uint64_t b_hi = tc::make_smem_desc_sw128(b_addr + ch * G::B_TILE), b_lo = tc::make_smem_desc_sw128(b_addr + ch * G::B_TILE + 96 * 128);
                 tc::wgmma_fence();
-                if (ch < kch_h) mma_chunk<NPROD>(rz_m, hn_m, rz_c, hn_c, a_hi, a_lo, b_hi, b_lo);
+                if (TABLE || ch < kch_h) mma_chunk<NPROD>(rz_m, hn_m, rz_c, hn_c, a_hi, a_lo, b_hi, b_lo);
                 else mma_chunk<NPROD>(rz_m, in_m, rz_c, in_c, a_hi, a_lo, b_hi, b_lo);
                 tc::wgmma_commit();
                 if (ch > 0) {       // chunk ch - 1 has retired while chunk ch is queued behind it
@@ -204,13 +212,21 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gru_ws_kernel(const __grid_con
             // the blend's h, loaded while the last chunk's MMAs run.  Fragment register 4 i + 2 rh + e of every block = row
             // (gq + 8 rh), hidden unit 8 i + 2 tq + e of the block
             float hv[2][4][2];
+            float2 gv[TABLE ? 2 : 1][4][3];     // TABLE: (i_r, i_z, i_n) of hidden units u, u + 1 from the row's graph
 #pragma unroll
             for (int rh = 0; rh < 2; ++rh) {
                 const int row = t * TILE_M + 16 * wi + gq + 8 * rh;
                 const long long off = (long long)row * p.H + jb * 32;
+                const long long goff = TABLE && row < p.num_nodes ? (long long)__ldg(p.gid + row) * 3 * p.H + jb * 32 : 0;
 #pragma unroll
                 for (int q = 0; q < 4; ++q) {
                     const int u = 8 * q + 2 * tq;
+                    if (TABLE) {
+#pragma unroll
+                        for (int gt = 0; gt < 3; ++gt)
+                            gv[TABLE ? rh : 0][q][gt] = row < p.num_nodes ? __ldg(reinterpret_cast<const float2 *>(p.gi + goff + gt * p.H + u))
+                                                                          : make_float2(0.0f, 0.0f);
+                    }
                     if (row >= p.num_nodes) {
                         hv[rh][q][0] = hv[rh][q][1] = 0.0f;
                     } else if (NPROD == 3) {
@@ -223,7 +239,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gru_ws_kernel(const __grid_con
                 }
             }
             tc::wgmma_wait<0>();
-            tc::fence_acc(rz_m); tc::fence_acc(rz_c); tc::fence_acc(in_m); tc::fence_acc(in_c); tc::fence_acc(hn_m); tc::fence_acc(hn_c);
+            if (TABLE) {
+                tc::fence_acc(rz_m); tc::fence_acc(rz_c); tc::fence_acc(hn_m); tc::fence_acc(hn_c);
+            } else {
+                tc::fence_acc(rz_m); tc::fence_acc(rz_c); tc::fence_acc(in_m); tc::fence_acc(in_c); tc::fence_acc(hn_m); tc::fence_acc(hn_c);
+            }
             __syncwarp();
             if (lane == 0) mbar_arrive(&a_empty[prev_slot]);
             // ---- gate math straight from the fragments (z is columns 32.. of rz: its registers 16..)
@@ -245,7 +265,21 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gru_ws_kernel(const __grid_con
 #pragma unroll
                         for (int gt = 0; gt < 4; ++gt) a[gt] = NPROD == 3 ? fmaf(cg[gt], 1.0f / 2048.0f, mg[gt]) : mg[gt];
                         const float4 b = bias_s[jb * 32 + u + e];
-                        if (NPROD == 3) {
+                        if (TABLE) {
+                            const float2 *gp = gv[TABLE ? rh : 0][q];
+                            const float gr = e ? gp[0].y : gp[0].x, gz = e ? gp[1].y : gp[1].x, gn = e ? gp[2].y : gp[2].x;
+                            if (NPROD == 3) {
+                                const float rr = sigmoid_fast((a[1] + b.x) + gr);
+                                const float zz = sigmoid_fast((a[2] + b.y) + gz);
+                                const float nn = tanh_fast(gn + rr * (a[3] + b.w));
+                                o[e] = (1.0f - zz) * nn + zz * hv[rh][q][e];
+                            } else {
+                                const float rr = sigmoid_mufu((a[1] + b.x) + gr);
+                                const float zz = sigmoid_mufu((a[2] + b.y) + gz);
+                                const float nn = tanh_mufu(fmaf(rr, a[3] + b.w, gn));
+                                o[e] = fmaf(zz, hv[rh][q][e] - nn, nn);
+                            }
+                        } else if (NPROD == 3) {
                             const float rr = sigmoid_fast(a[1] + b.x);
                             const float zz = sigmoid_fast(a[2] + b.y);
                             const float nn = tanh_fast(a[0] + b.z + rr * (a[3] + b.w));
@@ -283,6 +317,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gru_ws_kernel(const __grid_con
 // =====================================================================================================================
 // gate-blocked weight packing:  P1[jb][part][96][D] = [W_ir; W_iz; W_in],  P2[jb][part][96][H] = [W_hr; W_hz; W_hn]
 // (weight_ih / weight_hh gate order is r, z, n);  NPROD 3: part 0 = fp16 hi, part 1 = fp16 lo';  NPROD 1: bf16.
+// State-only packing (D = 0, w_ih = b_ih = NULL): P2 and the biases of the hidden side only.
 // The parts of one jb are adjacent, so one TMA box of NPART * 96 rows is a chunk's whole B operand.
 // =====================================================================================================================
 __device__ __forceinline__ void split16(float x, uint16_t &hi, uint16_t &lo) {
@@ -300,7 +335,8 @@ __global__ void __launch_bounds__(256) pack_gru_ws_kernel(const float *__restric
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n1 + n2 + H; i += (long long)gridDim.x * blockDim.x) {
         if (i >= n1 + n2) {
             const int j = (int)(i - n1 - n2);
-            bias4[j] = make_float4(b_ih[j] + b_hh[j], b_ih[H + j] + b_hh[H + j], b_ih[2 * H + j], b_hh[2 * H + j]);
+            bias4[j] = b_ih != nullptr ? make_float4(b_ih[j] + b_hh[j], b_ih[H + j] + b_hh[H + j], b_ih[2 * H + j], b_hh[2 * H + j])
+                                       : make_float4(b_hh[j], b_hh[H + j], 0.0f, b_hh[2 * H + j]);   // state-only: b_ih is in the table
             continue;
         }
         float x;
@@ -416,17 +452,72 @@ int update(int nprod, const void *agg_rows, const void *h_rows, const void *h_pl
     const int grid = groups * (int)n_jb;
     if (nprod == 3) {
         const int smem = Geometry<3>::smem_bytes(H, D);
-        PTGNN_CUDA(cudaFuncSetAttribute(gru_ws_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        PTGNN_CUDA(cudaFuncSetAttribute(gru_ws_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         {
             TimedScope timed__(PTGNN_KERNEL_GRU, st);
-            gru_ws_kernel<3><<<grid, NUM_THREADS, smem, st>>>(p);
+            gru_ws_kernel<3, false><<<grid, NUM_THREADS, smem, st>>>(p);
         }
     } else {
         const int smem = Geometry<1>::smem_bytes(H, D);
-        PTGNN_CUDA(cudaFuncSetAttribute(gru_ws_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        PTGNN_CUDA(cudaFuncSetAttribute(gru_ws_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         {
             TimedScope timed__(PTGNN_KERNEL_GRU, st);
-            gru_ws_kernel<1><<<grid, NUM_THREADS, smem, st>>>(p);
+            gru_ws_kernel<1, false><<<grid, NUM_THREADS, smem, st>>>(p);
+        }
+    }
+    PTGNN_LAUNCHED();
+    return PTGNN_OK;
+}
+
+bool supported_table(int nprod, int H) {
+    if (H % 64 != 0 || H < 64) return false;
+    const int slots = nprod == 3 ? Geometry<3>::num_slots(H, 0) : Geometry<1>::num_slots(H, 0);
+    return slots >= 2 && 132 / (H / 32) >= 1;
+}
+size_t pack_table_bytes(int nprod, int H) { return pack_bytes(nprod, H, 0); }
+int pack_table(int nprod, int H, const float *w_hh, const float *b_hh, void *packed, cudaStream_t st) {
+    return pack(nprod, H, 0, nullptr, w_hh, nullptr, b_hh, packed, st);
+}
+
+int update_table(int nprod, const void *h_rows, const void *h_plain, int64_t num_nodes, int H, const float *gi, const int32_t *gid,
+                 const void *packed, void *out, void *out_packed, int32_t *status, cudaStream_t st) {
+    PTGNN_CHECK_ARG(supported_table(nprod, H), "gru_ws (state-only): unsupported H=%d", H);
+    PTGNN_CHECK_ARG(out_packed == nullptr || nprod == 3, "gru_ws: packed output is an fp32-path (3xFP16) feature");
+    if (num_nodes <= 0) return PTGNN_OK;
+    const int npart = nprod == 3 ? 2 : 1;
+    uint16_t *p1, *p2;
+    float4 *bias4;
+    pack_layout(nprod, H, 0, const_cast<char *>(static_cast<const char *>(packed)), p1, p2, bias4);
+    Params p{};
+    const uint64_t n_jb = H / 32;
+    const bool bf = nprod == 1;
+    int rc = make_map16(&p.map_h, h_rows, num_nodes, (uint64_t)npart * H, TILE_M, bf);
+    if (!rc) rc = make_map16(&p.map_p2, p2, n_jb * npart * 96, H, npart * 96, bf);
+    if (rc) return rc;
+    p.h32 = static_cast<const float *>(h_plain); p.h16 = static_cast<const __nv_bfloat16 *>(h_plain);
+    p.bias4 = bias4; p.gi = gi; p.gid = gid; p.out = out; p.out_packed = static_cast<__half *>(out_packed); p.status = status;
+    p.num_nodes = (int)num_nodes; p.H = H; p.D = 0; p.n_jb = (int)n_jb;
+    p.n_tiles = (int)ceil_div(num_nodes, TILE_M);
+    p.num_slots = nprod == 3 ? Geometry<3>::num_slots(H, 0) : Geometry<1>::num_slots(H, 0);
+    int dev = 0, sms = 132;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
+    int groups = sms / (int)n_jb;
+    if (groups > p.n_tiles) groups = p.n_tiles;
+    if (groups < 1) groups = 1;
+    const int grid = groups * (int)n_jb;
+    if (nprod == 3) {
+        const int smem = Geometry<3>::smem_bytes(H, 0);
+        PTGNN_CUDA(cudaFuncSetAttribute(gru_ws_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        {
+            TimedScope timed__(PTGNN_KERNEL_GRU, st);
+            gru_ws_kernel<3, true><<<grid, NUM_THREADS, smem, st>>>(p);
+        }
+    } else {
+        const int smem = Geometry<1>::smem_bytes(H, 0);
+        PTGNN_CUDA(cudaFuncSetAttribute(gru_ws_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        {
+            TimedScope timed__(PTGNN_KERNEL_GRU, st);
+            gru_ws_kernel<1, true><<<grid, NUM_THREADS, smem, st>>>(p);
         }
     }
     PTGNN_LAUNCHED();

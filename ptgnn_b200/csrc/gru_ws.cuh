@@ -17,5 +17,13 @@ int pack(int nprod, int H, int D, const float *w_ih, const float *w_hh, const fl
 int update(int nprod, const void *agg_rows, const void *h_rows, const void *h_plain, int64_t num_nodes, int H, int D, const void *packed,
            void *out, void *out_packed, int32_t *status, cudaStream_t st);
 
+// State-only instance: out = GRUCell(g[gid[n]], h_n) from the input-side table gi [G, 3H] fp32 (= g W_ih^T + b_ih, gates r, z, n).
+// `packed` holds the hidden side only (pack_table, >= pack_table_bytes); the other arguments are those of `update`.
+bool supported_table(int nprod, int H);
+size_t pack_table_bytes(int nprod, int H);
+int pack_table(int nprod, int H, const float *w_hh, const float *b_hh, void *packed, cudaStream_t st);
+int update_table(int nprod, const void *h_rows, const void *h_plain, int64_t num_nodes, int H, const float *gi, const int32_t *gid,
+                 const void *packed, void *out, void *out_packed, int32_t *status, cudaStream_t st);
+
 }  // namespace gruws
 }  // namespace ptgnn

@@ -207,6 +207,27 @@ class shared_plan:
         return False
 
 
+class shared_num_graphs:
+    """`with shared_num_graphs(G):` -- per-thread hand-off of the minibatch's graph count from a container to its global-exchange
+    layers (ptgnn_b200.globalexchange), which then never read it from the device.  None hands nothing over; nests."""
+
+    def __init__(self, num_graphs: Optional[int]):
+        self.num_graphs, self.previous = num_graphs, None
+
+    def __enter__(self):
+        self.previous = getattr(_TLS, "num_graphs", None)
+        _TLS.num_graphs = self.num_graphs
+        return self.num_graphs
+
+    def __exit__(self, *exc):
+        _TLS.num_graphs = self.previous
+        return False
+
+
+def current_num_graphs() -> Optional[int]:
+    return getattr(_TLS, "num_graphs", None)
+
+
 class state_chain:
     """`with state_chain() as chain:` -- per-thread hand-off of PACKED node states between consecutive layers of one layer loop.
     The fp32 fused path computes on fp16 (hi | lo') pairs; a GatedMessagePassingLayer called with `chain.want_output` set also

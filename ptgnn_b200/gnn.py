@@ -11,7 +11,7 @@ from typing import Any, Dict, List, NamedTuple, Optional, Tuple
 import torch
 from torch import nn
 
-from .edgeplan import EdgePlan, clear_plan_cache, plan_for, shared_plan, state_chain
+from .edgeplan import EdgePlan, clear_plan_cache, plan_for, shared_num_graphs, shared_plan, state_chain
 from .messagepassing import AbstractMessagePassingLayer
 
 
@@ -125,7 +125,10 @@ class GraphNeuralNetwork(nn.Module):
         reference_node_graph_idx: Dict[str, torch.Tensor],
         return_all_states: bool = False,
         plan: Optional[EdgePlan] = None,
+        num_graphs: Optional[int] = None,
     ) -> torch.Tensor:
+        """``num_graphs`` (optional): the number of graphs in the minibatch, handed to the global-exchange layers so that they do not
+        read ``node_to_graph_idx.max() + 1`` from the device."""
         if self.__edge_dropout_rate > 0 and self.training:
             # graphneuralnetwork.py:105-119: Bernoulli keep-mask per edge (device-side index bookkeeping; a new plan is built
             # for the surviving edges, so this also invalidates any plan handed in)
@@ -142,8 +145,9 @@ class GraphNeuralNetwork(nn.Module):
             plan = plan_for(adjacency_lists, node_representations.shape[0], plan)
         all_states = [node_representations]
         layers = list(self.__message_passing_layers)
-        # per-thread hand-offs: the layers of this call (and only they) reuse the plan, and pass their packed states on
-        with shared_plan(plan), state_chain() as chain:
+        # per-thread hand-offs: the layers of this call (and only they) reuse the plan and the graph count, and pass their packed
+        # states on
+        with shared_plan(plan), shared_num_graphs(num_graphs), state_chain() as chain:
             for i, layer in enumerate(layers):
                 chain.want_output = i + 1 < len(layers)
                 node_representations = layer(
@@ -160,13 +164,22 @@ class GraphNeuralNetwork(nn.Module):
         return node_representations
 
     def capture(self, node_states: torch.Tensor, adjacency_lists: List[Tuple[torch.Tensor, torch.Tensor]],
-                node_to_graph_idx: Optional[torch.Tensor] = None, return_all_states: bool = False) -> "GraphedLayerLoop":
+                node_to_graph_idx: Optional[torch.Tensor] = None, return_all_states: bool = False,
+                num_graphs: Optional[int] = None) -> "GraphedLayerLoop":
         """CUDA-graph the layer loop (edge plan + all layers) for FIXED shapes: the returned object replays it with one launch.
         ``node_states`` / ``adjacency_lists`` (already expanded, see ``expand_adjacency``) are the static input buffers -- refill
         them in place (e.g. with ``copy_`` from pinned host memory) and call ``replay()``.  The per-type edge COUNTS are frozen at
         capture; the edge contents, the node states and -- because the plan is rebuilt inside the graph -- the graph structure
-        are whatever the buffers hold at replay time.  Parameters must not change between capture and replay (eval mode)."""
-        return GraphedLayerLoop(self, node_states, adjacency_lists, node_to_graph_idx, return_all_states)
+        are whatever the buffers hold at replay time.  Parameters must not change between capture and replay (eval mode).
+        With global-exchange layers the number of graphs is frozen at capture too: ``num_graphs``, or -- when it is not given --
+        ``node_to_graph_idx.max() + 1``, read once before the warm-up; ``node_to_graph_idx`` is then a static input buffer as well."""
+        from .globalexchange import AbstractGlobalGraphExchange
+
+        if num_graphs is None and any(isinstance(layer, AbstractGlobalGraphExchange) for layer in self.__message_passing_layers):
+            if node_to_graph_idx is None:
+                raise ValueError("capture(): global-exchange layers need node_to_graph_idx")
+            num_graphs = int(node_to_graph_idx.max().item()) + 1 if node_to_graph_idx.numel() else 0
+        return GraphedLayerLoop(self, node_states, adjacency_lists, node_to_graph_idx, return_all_states, num_graphs)
 
     def expand_adjacency(self, adjacency_lists, num_nodes: int, device) -> List[Tuple[torch.Tensor, torch.Tensor]]:
         """Backward + self edge lists (graphneuralnetwork.py:172-186) as a NEW list."""
@@ -202,6 +215,8 @@ class GraphNeuralNetwork(nn.Module):
                 edge_features = edge_features + list(edge_features)
             if self.__add_self_edges:
                 edge_features.append(torch.zeros(num_nodes, edge_features[-1].shape[-1], device=device))
+        if "num_graphs" not in kwargs and isinstance(num_graphs, int):
+            kwargs["num_graphs"] = num_graphs
         output = self.gnn(initial, expanded, edge_features, node_to_graph_idx, reference_node_ids,
                           reference_node_graph_idx, **kwargs)
         self.__num_edges += sum(src.shape[0] for src, _ in expanded)
@@ -222,13 +237,15 @@ class GraphedLayerLoop:
     launches and ~10 ctypes calls per minibatch by one ``cudaGraphLaunch``: what the reference would get from
     ``torch.cuda.graphs`` around its own loop, here including the plan build."""
 
-    def __init__(self, gnn: GraphNeuralNetwork, node_states, adjacency_lists, node_to_graph_idx, return_all_states: bool):
+    def __init__(self, gnn: GraphNeuralNetwork, node_states, adjacency_lists, node_to_graph_idx, return_all_states: bool,
+                 num_graphs: Optional[int] = None):
         if gnn.training:
             raise RuntimeError("capture() needs eval mode (the derived-weight caches are only trusted there)")
         self.node_states, self.adjacency_lists = node_states, list(adjacency_lists)
         self._gnn = gnn
         dev = node_states.device
-        run = lambda: gnn.gnn(node_states, self.adjacency_lists, None, node_to_graph_idx, {}, {}, return_all_states=return_all_states)  # noqa: E731
+        run = lambda: gnn.gnn(node_states, self.adjacency_lists, None, node_to_graph_idx, {}, {}, return_all_states=return_all_states,  # noqa: E731
+                              num_graphs=num_graphs)
         side = torch.cuda.Stream(dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side), torch.no_grad():     # warm-up outside the graph: fills weight caches and allocator pools
@@ -242,9 +259,14 @@ class GraphedLayerLoop:
         with torch.no_grad(), torch.cuda.graph(self.graph):
             self.output = run()
         self._plan = plan_for(self.adjacency_lists, node_states.shape[0])    # built during capture; keeps its buffers and status words
+        self._graph_plan = None
+        if num_graphs is not None and node_to_graph_idx is not None:         # the global-exchange layers' node -> graph plan, likewise
+            self._graph_plan = plan_for([(node_to_graph_idx, node_to_graph_idx)], num_graphs)
         clear_plan_cache()
 
     def replay(self) -> torch.Tensor:
         self._plan.poll()          # errors the previous replay's kernels reported (bad indices, fp16-range overflow)
+        if self._graph_plan is not None:
+            self._graph_plan.poll()
         self.graph.replay()
         return self.output

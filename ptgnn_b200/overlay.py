@@ -5,8 +5,10 @@ factories import the layer classes by module path (`implementations/typilus/trai
 `varmisuse/train.py:17-25`) and its modules import ``torch_scatter`` by name (`abstractmessagepassing.py:4`).  ``install()``
 
 1. registers ``ptgnn_b200.torch_scatter_shim`` as ``torch_scatter`` (if the real wheel is absent, or ``force_torch_scatter``),
-2. pre-seeds ``sys.modules`` so that ``ptgnn.neuralmodels.gnn.messagepassing.{abstract,gated,mlp}messagepassing`` resolve to the
-   ptgnn_b200 classes (everything else -- residual layers, PNA, GraphNorm, embedders, trainers -- stays the reference's), and
+2. pre-seeds ``sys.modules`` so that ``ptgnn.neuralmodels.gnn.messagepassing.{abstract,gated,mlp}messagepassing`` and
+   ``...globalgraphexchange`` resolve to the ptgnn_b200 classes (everything else -- residual layers, PNA, GraphNorm, embedders,
+   trainers, and the reducers of ``reduceops.varsizedsummary``, whose attention variants must keep working -- stays the
+   reference's; the native ``GruGlobalStateUpdate`` reads the reference's WeightedSum and Simple reducers directly), and
    re-binds those names in reference modules that were imported earlier,
 3. replaces ``GraphNeuralNetwork`` inside the reference's ``graphneuralnetwork`` module (``GraphNeuralNetworkModel`` stays),
 4. registers the ptgnn_b200 container as a (virtual) ``ModuleWithMetrics`` so that a reference parent's ``report_metrics()`` /
@@ -21,6 +23,7 @@ import sys
 import types
 from typing import Dict
 
+from . import globalexchange as _gx
 from . import gnn as _gnn
 from . import messagepassing as _mp
 
@@ -28,6 +31,7 @@ _LAYER_MODULES = {
     "ptgnn.neuralmodels.gnn.messagepassing.abstractmessagepassing": ("AbstractMessagePassingLayer", "AbstractMessageAggregation"),
     "ptgnn.neuralmodels.gnn.messagepassing.gatedmessagepassing": ("GatedMessagePassingLayer",),
     "ptgnn.neuralmodels.gnn.messagepassing.mlpmessagepassing": ("MlpMessagePassingLayer",),
+    "ptgnn.neuralmodels.gnn.messagepassing.globalgraphexchange": ("AbstractGlobalGraphExchange", "GruGlobalStateUpdate"),
 }
 _saved: Dict[str, object] = {}
 
@@ -39,10 +43,14 @@ def _reference_importable() -> bool:
         return False
 
 
+def _native_class(name: str):
+    return getattr(_mp, name) if hasattr(_mp, name) else getattr(_gx, name)
+
+
 def _stub_module(name: str, names) -> types.ModuleType:
     m = types.ModuleType(name, f"ptgnn_b200 overlay of the reference module {name}")
     for n in names:
-        setattr(m, n, getattr(_mp, n))
+        setattr(m, n, _native_class(n))
     m.__ptgnn_b200_overlay__ = True
     return m
 
@@ -74,7 +82,7 @@ def install(force_torch_scatter: bool = False) -> Dict[str, object]:
             _saved[mod_name] = old
             for n in names:
                 if hasattr(old, n):
-                    replaced[getattr(old, n)] = getattr(_mp, n)
+                    replaced[getattr(old, n)] = _native_class(n)
         sys.modules[mod_name] = _stub_module(mod_name, names)
     for mod_name, mod in list(sys.modules.items()):      # `from ... import GatedMessagePassingLayer` bindings made earlier
         if mod is None or not mod_name.startswith("ptgnn.") or getattr(mod, "__ptgnn_b200_overlay__", False):
