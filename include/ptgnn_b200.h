@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define PTGNN_B200_ABI_VERSION 2
+#define PTGNN_B200_ABI_VERSION 3
 #define PTGNN_MAX_EDGE_TYPES 128 /* etype is stored as uint8 in the plan; 128 keeps launch params < 4 KB */
 
 enum {
@@ -133,23 +133,17 @@ int ptgnn_b200_scatter_f32(const float *src, const int64_t *index, int64_t num_e
  * ---------------------------------------------------------------------------------------------- */
 size_t ptgnn_b200_gated_workspace_bytes(int64_t num_nodes, int64_t num_edges, int32_t num_types, int32_t state_dim,
                                         int32_t message_dim);
-int ptgnn_b200_gated_forward_f32(const float *node_states, const float *gather_states /* NULL: node_states */,
-                                 int64_t num_nodes, int32_t state_dim, int32_t message_dim,
-                                 int32_t num_types, const int64_t *type_off /*[host]*/, const int32_t *row_ptr,
-                                 const int32_t *pos, const int32_t *src32,
-                                 const float *const *edge_weights /*[host] T device pointers*/, const float *gru_w_ih,
-                                 const float *gru_w_hh, const float *gru_b_ih, const float *gru_b_hh, int32_t reduce,
-                                 float *out_states, void *workspace, size_t workspace_bytes, void *stream);
 
 /* Weight cache (optional).  Every forward call first derives working copies of the parameters (TF32 hi/lo splits,
- * gate-blocked GRU packing; bf16 conversions in the bf16 variant).  A caller whose parameters do not change between calls
- * (inference, or between optimiser steps) can own that buffer: pass `weight_cache` (device memory of at least
- * `*_weight_cache_bytes`, 256-byte aligned) and `cache_valid` = 0 on the first call with a given set of parameter VALUES
- * (the copies are derived into the cache), 1 afterwards (they are reused; the parameter pointers are then not read by the
- * derivation).  `*_weight_cache_bytes` == 0 means these dimensions have nothing to cache: pass NULL.  Results are
- * bit-identical to the uncached entry points. */
+ * gate-blocked GRU packing; bf16 conversions in the bf16 variant).  weight_cache == NULL: they are derived into the workspace
+ * on every call.  A caller whose parameters do not change between calls (inference, or between optimiser steps) can own
+ * that buffer instead: pass `weight_cache` (device memory of at least `*_weight_cache_bytes`, 256-byte aligned) and
+ * `cache_valid` = 0 on the first call with a given set of parameter VALUES (the copies are derived into the cache), 1
+ * afterwards (they are reused; the parameter pointers are then not read by the derivation).  `*_weight_cache_bytes` == 0
+ * means these dimensions have nothing to cache: pass NULL.  Results are bit-identical with and without a cache. */
 size_t ptgnn_b200_gated_weight_cache_bytes(int32_t num_types, int32_t state_dim, int32_t message_dim);
-int ptgnn_b200_gated_forward_cached_f32(const float *node_states, const float *gather_states, int64_t num_nodes,
+int ptgnn_b200_gated_forward_cached_f32(const float *node_states, const float *gather_states /* NULL: node_states */,
+                                        int64_t num_nodes,
                                         int32_t state_dim, int32_t message_dim, int32_t num_types,
                                         const int64_t *type_off /*[host]*/, const int32_t *row_ptr, const int32_t *pos,
                                         const int32_t *src32, const float *const *edge_weights /*[host]*/,
@@ -157,28 +151,23 @@ int ptgnn_b200_gated_forward_cached_f32(const float *node_states, const float *g
                                         const float *gru_b_hh, int32_t reduce, float *out_states, void *workspace,
                                         size_t workspace_bytes, void *weight_cache, size_t weight_cache_bytes,
                                         int32_t cache_valid, void *stream);
+
+/* bf16 variant (BASELINE.json configs[3]): node_states / gather_states / out_states are bf16 [*, H] (raw uint16 bits),
+ * module parameters stay fp32 and are converted into the workspace or the weight cache; messages and aggregates are bf16 in
+ * HBM, every accumulation (tensor-core accumulators, segmented reduce, gate math) is fp32 -- the arithmetic of the reference
+ * under torch.autocast(bfloat16) (fp32 scatter: abstractmessagepassing.py:43-50).  Needs H % 32 == 0, D % 16 == 0,
+ * 64 <= D <= 256. */
+size_t ptgnn_b200_gated_workspace_bytes_bf16(int64_t num_nodes, int64_t num_edges, int32_t num_types, int32_t state_dim,
+                                             int32_t message_dim);
 size_t ptgnn_b200_gated_weight_cache_bytes_bf16(int32_t num_types, int32_t state_dim, int32_t message_dim);
-int ptgnn_b200_gated_forward_cached_bf16(const uint16_t *node_states, const uint16_t *gather_states, int64_t num_nodes,
-                                         int32_t state_dim, int32_t message_dim, int32_t num_types,
+int ptgnn_b200_gated_forward_cached_bf16(const uint16_t *node_states, const uint16_t *gather_states /* NULL: node_states */,
+                                         int64_t num_nodes, int32_t state_dim, int32_t message_dim, int32_t num_types,
                                          const int64_t *type_off /*[host]*/, const int32_t *row_ptr, const int32_t *pos,
-                                         const int32_t *src32, const float *const *edge_weights /*[host]*/,
+                                         const int32_t *src32, const float *const *edge_weights /*[host] T device pointers, fp32*/,
                                          const float *gru_w_ih, const float *gru_w_hh, const float *gru_b_ih,
                                          const float *gru_b_hh, int32_t reduce, uint16_t *out_states, void *workspace,
                                          size_t workspace_bytes, void *weight_cache, size_t weight_cache_bytes,
                                          int32_t cache_valid, void *stream);
-
-/* bf16 variant (BASELINE.json configs[3]): node_states / gather_states / out_states are bf16 [*, H] (raw uint16 bits),
- * module parameters stay fp32 and are converted per call; messages and aggregates are bf16 in HBM, every accumulation
- * (tensor-core accumulators, segmented reduce, gate math) is fp32 -- the arithmetic of the reference under
- * torch.autocast(bfloat16) (fp32 scatter: abstractmessagepassing.py:43-50).  Needs H % 32 == 0, D % 16 == 0, 64 <= D <= 256. */
-size_t ptgnn_b200_gated_workspace_bytes_bf16(int64_t num_nodes, int64_t num_edges, int32_t num_types, int32_t state_dim,
-                                             int32_t message_dim);
-int ptgnn_b200_gated_forward_bf16(const uint16_t *node_states, const uint16_t *gather_states /* NULL: node_states */,
-                                  int64_t num_nodes, int32_t state_dim, int32_t message_dim, int32_t num_types,
-                                  const int64_t *type_off /*[host]*/, const int32_t *row_ptr, const int32_t *pos,
-                                  const int32_t *src32, const float *const *edge_weights /*[host] T device pointers, fp32*/,
-                                  const float *gru_w_ih, const float *gru_w_hh, const float *gru_b_ih, const float *gru_b_hh,
-                                  int32_t reduce, uint16_t *out_states, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * MlpMessagePassingLayer.forward (mlpmessagepassing.py:68-117), eval mode, default message MLP
@@ -243,48 +232,46 @@ int ptgnn_b200_block_plan_build(int64_t num_nodes, int32_t num_types, const int6
                                 const int32_t *src32, const int32_t *tgt32, int32_t block_targets, int32_t *group_off,
                                 int32_t *src_f, uint8_t *tl_f, void *workspace, size_t workspace_bytes, void *stream);
 
-/* 1 if these dimensions run on the fused kernel (message_dim == 128; state_dim in {64, 128} for fp32 states,
- * {64, 128, 256} for bf16 states); otherwise use the unfused entry points above. */
+/* 1 if these dimensions run on the fused layer kernels (message_dim == 128; state_dim in {64, 128} for fp32 states,
+ * {64, 128, 256} for bf16 states; 0 for every shape under PTGNN_B200_DISABLE_TC=1); otherwise use the unfused entry points
+ * above. */
 int32_t ptgnn_b200_fused_supported(int32_t bf16_states, int32_t state_dim, int32_t message_dim);
 
-/* GatedMessagePassingLayer.forward through the fused kernel.  Same contract as ptgnn_b200_gated_forward_cached_{f32,bf16}
- * (node_states / gather_states / out_states are fp32 when bf16_states == 0, bf16 otherwise; `row_ptr` = CSR offsets of the
- * edge plan, used by reduce = mean); the edge arrays come from the block plan.  fp32 states are computed fp32-exactly with
- * three fp16 tensor-core products per term ("3xFP16", see csrc/fused_mp.cuh). */
-size_t ptgnn_b200_gated_fused_workspace_bytes(int32_t bf16_states, int64_t num_nodes, int64_t num_source_nodes,
-                                              int32_t num_types, int32_t state_dim, int32_t message_dim);
-size_t ptgnn_b200_gated_fused_weight_cache_bytes(int32_t bf16_states, int32_t num_types, int32_t state_dim, int32_t message_dim);
-int ptgnn_b200_gated_forward_fused(int32_t bf16_states, const void *node_states, const void *gather_states /* NULL: node_states */,
-                                   int64_t num_nodes, int64_t num_source_nodes, int32_t state_dim, int32_t message_dim,
-                                   int32_t num_types, const ptgnn_b200_block_plan *block_plan, const int32_t *row_ptr,
-                                   const float *const *edge_weights /*[host] T device pointers, fp32*/, const float *gru_w_ih,
-                                   const float *gru_w_hh, const float *gru_b_ih, const float *gru_b_hh, int32_t reduce,
-                                   void *out_states, void *workspace, size_t workspace_bytes, void *weight_cache,
-                                   size_t weight_cache_bytes, int32_t cache_valid, void *stream);
-
-/* The fp32 fused path computes on packed states: every fp32 state x as two fp16 numbers (hi | lo') in rows of 2 * state_dim
- * halfs (ptgnn_b200_packed_state_bytes per tensor).  In a stack of layers (GraphNeuralNetwork.gnn,
+/* GatedMessagePassingLayer.forward through the fused kernels: the fused aggregation, then the weights-stationary GRUCell.  Same
+ * contract as ptgnn_b200_gated_forward_cached_{f32,bf16} (node_states / gather_states / out_states are fp32 when
+ * bf16_states == 0, bf16 otherwise; weight_cache as described there, sized by ptgnn_b200_gated_fused_weight_cache_bytes;
+ * `row_ptr` = CSR offsets of the edge plan, used by reduce = mean); the edge arrays come from the block plan.  fp32 states are
+ * computed fp32-exactly with three fp16 tensor-core products per term ("3xFP16", see csrc/fused_mp.cuh).
+ *
+ * The fp32 path computes on packed states: every fp32 state x as two fp16 numbers (hi | lo') in rows of 2 * state_dim halfs
+ * (ptgnn_b200_packed_state_bytes per tensor).  In a stack of layers (GraphNeuralNetwork.gnn,
  * ptgnn/neuralmodels/gnn/graphneuralnetwork.py:121-131) the packing pass of layer i + 1 is redundant: the GRU kernel of layer i
- * can write its new states in both forms.  ptgnn_b200_gated_forward_fused_chained = ptgnn_b200_gated_forward_fused for fp32
- * states, plus
+ * can write its new states in both forms.  fp32 states only (both must be NULL for bf16 states):
  *   packed_states_in  (optional): the packed form of node_states, as written through packed_states_out by the previous layer;
  *   packed_states_out (optional): [num_nodes] packed rows, receives the packed form of out_states (bit-identical to what the
  *                                 next call would derive from out_states itself). */
+size_t ptgnn_b200_gated_fused_workspace_bytes(int32_t bf16_states, int64_t num_nodes, int64_t num_source_nodes,
+                                              int32_t num_types, int32_t state_dim, int32_t message_dim);
+size_t ptgnn_b200_gated_fused_weight_cache_bytes(int32_t bf16_states, int32_t num_types, int32_t state_dim, int32_t message_dim);
 size_t ptgnn_b200_packed_state_bytes(int64_t num_nodes, int32_t state_dim);
-int ptgnn_b200_gated_forward_fused_chained(const float *node_states, const float *gather_states /* NULL: node_states */,
-                                           const void *packed_states_in, int64_t num_nodes, int64_t num_source_nodes,
-                                           int32_t state_dim, int32_t message_dim, int32_t num_types,
-                                           const ptgnn_b200_block_plan *block_plan, const int32_t *row_ptr,
-                                           const float *const *edge_weights /*[host] T device pointers, fp32*/,
-                                           const float *gru_w_ih, const float *gru_w_hh, const float *gru_b_ih,
-                                           const float *gru_b_hh, int32_t reduce, float *out_states, void *packed_states_out,
-                                           void *workspace, size_t workspace_bytes, void *weight_cache, size_t weight_cache_bytes,
-                                           int32_t cache_valid, void *stream);
+int ptgnn_b200_gated_forward_fused(int32_t bf16_states, const void *node_states, const void *gather_states /* NULL: node_states */,
+                                   const void *packed_states_in /* NULL: packed here */, int64_t num_nodes,
+                                   int64_t num_source_nodes, int32_t state_dim, int32_t message_dim, int32_t num_types,
+                                   const ptgnn_b200_block_plan *block_plan, const int32_t *row_ptr,
+                                   const float *const *edge_weights /*[host] T device pointers, fp32*/, const float *gru_w_ih,
+                                   const float *gru_w_hh, const float *gru_b_ih, const float *gru_b_hh, int32_t reduce,
+                                   void *out_states, void *packed_states_out /* NULL: not written */, void *workspace,
+                                   size_t workspace_bytes, void *weight_cache, size_t weight_cache_bytes, int32_t cache_valid,
+                                   void *stream);
 
 /* MlpMessagePassingLayer.forward through the fused kernel (contract of ptgnn_b200_mlp_forward_{f32,bf16}); the message
- * activation and the LayerNorm run in the fused kernel's write-out. */
+ * activation and the LayerNorm run in the fused kernel's write-out.  weight_cache (optional, fp32 states; ignored for bf16
+ * states) [>= ptgnn_b200_mlp_fused_weight_cache_bytes] holds the packed edge weights and the split dense weight; pass
+ * cache_valid = 0 after the parameters changed (they are then re-derived into the cache), 1 to reuse them. */
 size_t ptgnn_b200_mlp_fused_workspace_bytes(int32_t bf16_states, int64_t num_nodes, int64_t num_source_nodes, int32_t num_types,
                                             int32_t in_dim, int32_t message_dim, int32_t out_dim, int32_t use_target_state);
+size_t ptgnn_b200_mlp_fused_weight_cache_bytes(int32_t bf16_states, int32_t num_types, int32_t in_dim, int32_t message_dim, int32_t out_dim,
+                                               int32_t use_target_state);
 int ptgnn_b200_mlp_forward_fused(int32_t bf16_states, const void *node_states, const void *gather_states /* NULL: node_states */,
                                  int64_t num_nodes, int64_t num_source_nodes, int32_t in_dim, int32_t message_dim,
                                  int32_t out_dim, int32_t num_types, const ptgnn_b200_block_plan *block_plan,
@@ -292,21 +279,7 @@ int ptgnn_b200_mlp_forward_fused(int32_t bf16_states, const void *node_states, c
                                  int32_t use_target_state, int32_t reduce, int32_t message_activation, const float *ln_weight,
                                  const float *ln_bias, float ln_eps, const float *dense_weight, const float *dense_bias,
                                  int32_t dense_activation, void *out_states, void *workspace, size_t workspace_bytes,
-                                 void *stream);
-
-/* ptgnn_b200_mlp_forward_fused with caller-owned derived weights (fp32 states): weight_cache [>= ptgnn_b200_mlp_fused_weight_cache_bytes]
- * holds the packed edge weights and the split dense weight; pass cache_valid = 0 after the parameters changed (they are then
- * re-derived into the cache), 1 to reuse them.  weight_cache == NULL or bf16 states: identical to ptgnn_b200_mlp_forward_fused. */
-size_t ptgnn_b200_mlp_fused_weight_cache_bytes(int32_t bf16_states, int32_t num_types, int32_t in_dim, int32_t message_dim, int32_t out_dim,
-                                               int32_t use_target_state);
-int ptgnn_b200_mlp_forward_fused_cached(int32_t bf16_states, const void *node_states, const void *gather_states /* NULL: node_states */,
-                                        int64_t num_nodes, int64_t num_source_nodes, int32_t in_dim, int32_t message_dim,
-                                        int32_t out_dim, int32_t num_types, const ptgnn_b200_block_plan *block_plan,
-                                        const int32_t *row_ptr, const float *const *edge_weights /*[host] T device pointers, fp32*/,
-                                        int32_t use_target_state, int32_t reduce, int32_t message_activation, const float *ln_weight,
-                                        const float *ln_bias, float ln_eps, const float *dense_weight, const float *dense_bias,
-                                        int32_t dense_activation, void *out_states, void *workspace, size_t workspace_bytes,
-                                        void *weight_cache, size_t weight_cache_bytes, int32_t cache_valid, void *stream);
+                                 void *weight_cache, size_t weight_cache_bytes, int32_t cache_valid, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Backward support (SURVEY.md section 8 row f-1; host side: ptgnn_b200/autograd.py).  The pointwise half of the GRUCell backward
@@ -377,7 +350,7 @@ int ptgnn_b200_edge_messages_f32(const float *source_states, const float *target
  *   pre-activations g W_ih^T + b_ih have num_graphs distinct rows: they are computed once as a table (ptgnn_b200_linear_f32),
  *   then the weights-stationary GRU kernel runs over the node rows with state chunks only.  node_states / out_states: fp32
  *   (3xFP16 products) or bf16 (bf16 products) [N, H]; packed_states_in / packed_states_out (optional, fp32 only): the packed
- *   form of ptgnn_b200_gated_forward_fused_chained.  status (optional): status[0] = 1 if a state is outside the fp16 range.
+ *   form of ptgnn_b200_gated_forward_fused.  status (optional): status[0] = 1 if a state is outside the fp16 range.
  *   H must be a multiple of 64 (ptgnn_b200_global_gru_supported), summary_dim a multiple of 4.  weight_cache: as for the
  *   gated layer (the packed W_hh and biases; cache_valid = 0 re-derives them).
  * ---------------------------------------------------------------------------------------------- */

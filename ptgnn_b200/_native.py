@@ -33,11 +33,7 @@ SIGNATURES = {
     "ptgnn_b200_scatter_workspace_bytes": (c_size_t, [c_i64, c_i64]),
     "ptgnn_b200_scatter_f32": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_i64, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "ptgnn_b200_gated_workspace_bytes": (c_size_t, [c_i64, c_i64, c_i32, c_i32, c_i32]),
-    "ptgnn_b200_gated_forward_f32": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                                    c_void_p, c_void_p, c_void_p, c_void_p, c_i32, c_void_p, c_void_p, c_size_t, c_void_p]),
     "ptgnn_b200_gated_workspace_bytes_bf16": (c_size_t, [c_i64, c_i64, c_i32, c_i32, c_i32]),
-    "ptgnn_b200_gated_forward_bf16": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p,
-                                                     c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i32, c_void_p, c_void_p, c_size_t, c_void_p]),
     "ptgnn_b200_gated_weight_cache_bytes": (c_size_t, [c_i32, c_i32, c_i32]),
     "ptgnn_b200_gated_forward_cached_f32": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p,
                                                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i32, c_void_p, c_void_p, c_size_t,
@@ -60,25 +56,19 @@ SIGNATURES = {
     "ptgnn_b200_fused_supported": (c_i32, [c_i32, c_i32, c_i32]),
     "ptgnn_b200_gated_fused_workspace_bytes": (c_size_t, [c_i32, c_i64, c_i64, c_i32, c_i32, c_i32]),
     "ptgnn_b200_gated_fused_weight_cache_bytes": (c_size_t, [c_i32, c_i32, c_i32, c_i32]),
-    "ptgnn_b200_gated_forward_fused": (ctypes.c_int, [c_i32, c_void_p, c_void_p, c_i64, c_i64, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p,
-                                                      c_void_p, c_void_p, c_void_p, c_void_p, c_i32, c_void_p, c_void_p, c_size_t, c_void_p,
-                                                      c_size_t, c_i32, c_void_p]),
     "ptgnn_b200_packed_state_bytes": (c_size_t, [c_i64, c_i32]),
-    "ptgnn_b200_gated_forward_fused_chained": (ctypes.c_int, [c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i32, c_i32, c_i32, c_void_p, c_void_p,
-                                                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i32, c_void_p, c_void_p,
-                                                              c_void_p, c_size_t, c_void_p, c_size_t, c_i32, c_void_p]),
+    "ptgnn_b200_gated_forward_fused": (ctypes.c_int, [c_i32, c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i32, c_i32, c_i32, c_void_p, c_void_p,
+                                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i32, c_void_p, c_void_p, c_void_p,
+                                                      c_size_t, c_void_p, c_size_t, c_i32, c_void_p]),
     "ptgnn_b200_mlp_fused_workspace_bytes": (c_size_t, [c_i32, c_i64, c_i64, c_i32, c_i32, c_i32, c_i32, c_i32]),
+    "ptgnn_b200_mlp_fused_weight_cache_bytes": (c_size_t, [c_i32, c_i32, c_i32, c_i32, c_i32, c_i32]),
     "ptgnn_b200_mlp_forward_fused": (ctypes.c_int, [c_i32, c_void_p, c_void_p, c_i64, c_i64, c_i32, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p,
                                                     c_i32, c_i32, c_i32, c_void_p, c_void_p, c_f32, c_void_p, c_void_p, c_i32, c_void_p, c_void_p,
-                                                    c_size_t, c_void_p]),
+                                                    c_size_t, c_void_p, c_size_t, c_i32, c_void_p]),
     "ptgnn_b200_gather_split_f16": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_void_p, c_void_p]),
     "ptgnn_b200_gru_gate_grads_f32": (ctypes.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_void_p, c_void_p]),
     "ptgnn_b200_offset_ids": (ctypes.c_int, [c_void_p, c_i64, c_void_p, c_void_p, c_i32, c_void_p, c_void_p]),
     "ptgnn_b200_segment_ids": (ctypes.c_int, [c_void_p, c_i32, c_i64, c_void_p, c_void_p]),
-    "ptgnn_b200_mlp_fused_weight_cache_bytes": (c_size_t, [c_i32, c_i32, c_i32, c_i32, c_i32, c_i32]),
-    "ptgnn_b200_mlp_forward_fused_cached": (ctypes.c_int, [c_i32, c_void_p, c_void_p, c_i64, c_i64, c_i32, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p,
-                                                           c_i32, c_i32, c_i32, c_void_p, c_void_p, c_f32, c_void_p, c_void_p, c_i32, c_void_p, c_void_p,
-                                                           c_size_t, c_void_p, c_size_t, c_i32, c_void_p]),
     "ptgnn_b200_linear_workspace_bytes": (c_size_t, [c_i32, c_i32]),
     "ptgnn_b200_linear_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_i32, c_i32, c_void_p, c_void_p, c_size_t, c_void_p]),
     "ptgnn_b200_grucell_workspace_bytes": (c_size_t, [c_i32, c_i32]),
@@ -106,7 +96,7 @@ class BlockPlanStruct(ctypes.Structure):
     _fields_ = [("block_targets", c_i32), ("group_off", c_void_p), ("src_f", c_void_p), ("tl_f", c_void_p), ("status", c_void_p)]
 
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 _lib: Optional[ctypes.CDLL] = None
 
 

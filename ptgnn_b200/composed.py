@@ -100,13 +100,12 @@ def aggregate(plan: EdgePlan, source_rows: torch.Tensor, weights: Sequence[torch
     where it takes the dimensions (D == 128, K in {64, 128}: no [E, D] message tensor), else ``edge_messages`` + ``segment_reduce``.
     Used by the backward passes (aggregate re-computation; d h_src on the transposed graph)."""
     import ctypes
-    import os
+
+    from .messagepassing import _use_fused
 
     D, K = weights[0].shape
     lib = N.lib()
-    fused_ok = (plan.num_edges > 0 and os.environ.get("PTGNN_B200_FUSED", "1") != "0" and os.environ.get("PTGNN_B200_FP32_MODE", "") != "tf32"
-                and bool(lib.ptgnn_b200_fused_supported(0, K, D)))
-    if not fused_ok:
+    if plan.num_edges == 0 or not _use_fused(lib, False, K, D):
         return segment_reduce(edge_messages(plan, source_rows, None, weights, False), plan, reduce_code)
     rows = N.require_cuda(source_rows, "source_rows", torch.float32)
     ws_list = [N.require_cuda(w, "edge weight", torch.float32) for w in weights]
@@ -118,7 +117,7 @@ def aggregate(plan: EdgePlan, source_rows: torch.Tensor, weights: Sequence[torch
     with torch.cuda.device(rows.device):       # the Mlp entry point without activation / LayerNorm / dense layer = the bare aggregation
         rc = lib.ptgnn_b200_mlp_forward_fused(0, N.ptr(rows), None, n, n, K, D, D, plan.num_types, ctypes.byref(bp), N.ptr(plan.row_ptr),
                                               N.ptr_table(ws_list), 0, reduce_code, N.ACT_NONE, None, None, 0.0, None, None, N.ACT_NONE,
-                                              N.ptr(out), N.ptr(ws), ws_bytes, N.current_stream(rows.device))
+                                              N.ptr(out), N.ptr(ws), ws_bytes, None, 0, 0, N.current_stream(rows.device))
     N.check(rc, "ptgnn_b200_mlp_forward_fused")
     return out
 

@@ -153,9 +153,9 @@ extern "C" int ptgnn_b200_gated_gnn_forward_host_f32(const float *node_states, i
         for (int t = 0; t < num_types; ++t) dev_w[t] = base + (size_t)t * H * H;
         float *wih = base + (size_t)num_types * H * H, *whh = wih + 3 * (size_t)H * H;
         float *bih = whh + 3 * (size_t)H * H, *bhh = bih + 3 * H;
-        rc = ptgnn_b200_gated_forward_f32(d_state[cur].as<float>(), nullptr, num_nodes, H, H, num_types, type_off.data(), row_ptr,
-                                          pos, src32, dev_w.data(), wih, whh, bih, bhh, reduce,
-                                          d_state[cur ^ 1].as<float>(), d_ws.p, ws_bytes, st);
+        rc = ptgnn_b200_gated_forward_cached_f32(d_state[cur].as<float>(), nullptr, num_nodes, H, H, num_types, type_off.data(),
+                                                 row_ptr, pos, src32, dev_w.data(), wih, whh, bih, bhh, reduce,
+                                                 d_state[cur ^ 1].as<float>(), d_ws.p, ws_bytes, nullptr, 0, 0, st);
         if (rc) return rc;
         cur ^= 1;
     }

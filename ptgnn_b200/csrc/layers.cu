@@ -12,9 +12,8 @@
 //      dense_update_kernel   Linear(+bias) + Tanh of the Mlp layer.
 #include <stdlib.h>
 
-#include "fused_mp.cuh"
-#include "gru_ws.cuh"
 #include "gemm_simt.cuh"
+#include "layers.cuh"
 #include "layers_tc.cuh"
 #include "reduce.cuh"
 
@@ -271,8 +270,7 @@ static int check_layer_dims(const char *who, int64_t N, int64_t E, int H, int D)
     return PTGNN_OK;
 }
 
-// Tensor cores are the default; PTGNN_B200_DISABLE_TC=1 forces the FFMA kernels (A/B measurements, debugging).
-static bool tc_enabled() {
+bool tc_enabled() {
     static int v = -1;
     if (v < 0) {
         const char *e = getenv("PTGNN_B200_DISABLE_TC");
@@ -281,11 +279,8 @@ static bool tc_enabled() {
     return v == 1;
 }
 
-// `fused` layouts (block plan given, dims supported): no [E, D] message buffer; instead the packed (hi | lo') fp16 copy
-// of the source states (Ns rows) and the packed edge weights of the fused kernel.
-// out = act(y W^T + b): tensor cores (3xTF32) when the dims fit the tiles, FFMA tiles otherwise.  scratch >= tc::dense_split_bytes.
-static int dense_any(const float *y, int64_t rows, int D, const float *W, const float *bias, int out_dim, int act, float *out,
-                     void *scratch, cudaStream_t st, bool pack = true) {
+int dense_any(const float *y, int64_t rows, int D, const float *W, const float *bias, int out_dim, int act, float *out,
+              void *scratch, cudaStream_t st, bool pack) {
     if (tc_enabled() && tc::supported_dense(D, out_dim)) return tc::dense_update(y, rows, D, W, bias, out_dim, act, out, scratch, st, pack);
     int rc;
     if (out_dim <= 64) {
@@ -311,35 +306,30 @@ static int dense_any(const float *y, int64_t rows, int D, const float *W, const 
     return PTGNN_OK;
 }
 
-struct GatedWs { size_t msg, agg, p1, p2, wsplit, grupack, xpack, xpack_own, total; };
-static GatedWs gated_ws_layout(int64_t N, int64_t Ns, int64_t E, int T, int H, int D, bool fused_path) {
+struct GatedWs { size_t msg, agg, p1, p2, wsplit, grupack, total; };
+static GatedWs gated_ws_layout(int64_t N, int64_t E, int T, int H, int D) {
     GatedWs w{};
     size_t o = 0;
     auto add = [&](size_t cnt) { size_t at = o; o += ws_slice(cnt, 4); return at; };
-    w.msg = add(fused_path ? 4 : (size_t)E * D + 4);
+    w.msg = add((size_t)E * D + 4);
     w.agg = add((size_t)N * D + 4);
     w.p1 = add((size_t)(H / 32 + 1) * 96 * D);
     w.p2 = add((size_t)(H / 32 + 1) * 96 * H);
-    w.wsplit = o; o += fused_path ? fused::packed_weight_bytes(3, T, H, 0) : tc::split_edge_weights_bytes(T, D, H);
-    w.grupack = o; o += tc::gru_pack_bytes(H + 32, D) + (fused_path && gruws::supported(3, H, D) ? gruws::pack_bytes(3, H, D) : 0);
-    w.xpack = o; o += fused_path ? fused::packed_state_bytes(3, Ns, H) : 0;
-    w.xpack_own = o; o += fused_path ? fused::packed_state_bytes(3, N, H) : 0;   // sharded run (gather_states given): this rank's rows for the GRU
+    w.wsplit = o; o += tc::split_edge_weights_bytes(T, D, H);
+    w.grupack = o; o += tc::gru_pack_bytes(H + 32, D);
     w.total = o;
     return w;
 }
 
-struct MlpWs { size_t msg, y, wsplit, dsplit, xpack, xpack_tgt, total; };
-static MlpWs mlp_ws_layout(int64_t N, int64_t Ns, int64_t E, int T, int H, int D, int Hout, int use_target, bool fused_path,
-                           bool separate_targets) {
+struct MlpWs { size_t msg, y, wsplit, dsplit, total; };
+static MlpWs mlp_ws_layout(int64_t N, int64_t E, int T, int H, int D, int Hout, int use_target) {
     MlpWs w{};
     size_t o = 0;
     auto add = [&](size_t cnt) { size_t at = o; o += ws_slice(cnt, 4); return at; };
-    w.msg = add(fused_path ? 4 : (size_t)E * D + 4);
+    w.msg = add((size_t)E * D + 4);
     w.y = add((size_t)N * D + 4);
-    w.wsplit = o; o += fused_path ? fused::packed_weight_bytes(3, T, H, use_target) : tc::split_edge_weights_bytes(T, D, use_target ? 2 * H : H);
+    w.wsplit = o; o += tc::split_edge_weights_bytes(T, D, use_target ? 2 * H : H);
     w.dsplit = o; o += tc::dense_split_bytes(Hout > 0 ? Hout : D, D);
-    w.xpack = o; o += fused_path ? fused::packed_state_bytes(3, Ns, H) : 0;
-    w.xpack_tgt = o; o += (fused_path && use_target && separate_targets) ? fused::packed_state_bytes(3, N, H) : 0;
     w.total = o;
     return w;
 }
@@ -351,7 +341,7 @@ using namespace ptgnn;
 extern "C" size_t ptgnn_b200_gated_workspace_bytes(int64_t num_nodes, int64_t num_edges, int32_t num_types,
                                                    int32_t state_dim, int32_t message_dim) {
     if (num_nodes < 0 || num_edges < 0 || num_types < 0 || state_dim <= 0 || message_dim <= 0) return 0;
-    return gated_ws_layout(num_nodes, num_nodes, num_edges, num_types, state_dim, message_dim, false).total;
+    return gated_ws_layout(num_nodes, num_edges, num_types, state_dim, message_dim).total;
 }
 
 // weight cache of the tensor-core path: [split edge weights | gate-blocked GRU weights + biases]; 0 when the dims run on
@@ -360,36 +350,17 @@ static size_t gated_cache_bytes(int T, int H, int D) {
     if (!tc_enabled() || !tc::supported_message(H, D) || !tc::supported_gru(H, D)) return 0;
     return tc::split_edge_weights_bytes(T, D, H) + tc::gru_pack_bytes(H, D);
 }
-static bool fused_f32_ok(int H, int D) { return tc_enabled() && fused::supported(3, H, D, 0) && tc::supported_gru(H, D); }
-// PTGNN_B200_GRU=tc selects the round-1 GRU pipeline (3xTF32, streams its weights per tile) behind the fused aggregation
-static bool gru_ws_enabled(int nprod, int H, int D) {
-    static int v = -1;
-    if (v < 0) { const char *e = getenv("PTGNN_B200_GRU"); v = (e && e[0] == 't') ? 0 : 1; }
-    return v == 1 && gruws::supported(nprod, H, D);
-}
-static size_t gated_fused_cache_bytes(int T, int H, int D) {
-    return fused::packed_weight_bytes(3, T, H, 0) + (gru_ws_enabled(3, H, D) ? gruws::pack_bytes(3, H, D) : tc::gru_pack_bytes(H, D));
-}
 
 static int gated_forward_impl(const float *node_states, const float *gather_states, int64_t num_nodes, int32_t state_dim,
                               int32_t message_dim, int32_t num_types, const int64_t *type_off, const int32_t *row_ptr,
                               const int32_t *pos, const int32_t *src32, const float *const *edge_weights,
                               const float *gru_w_ih, const float *gru_w_hh, const float *gru_b_ih, const float *gru_b_hh,
                               int32_t reduce, float *out_states, void *workspace, size_t workspace_bytes, void *weight_cache,
-                              size_t weight_cache_bytes, int32_t cache_valid, void *stream,
-                              const ptgnn_b200_block_plan *bp = nullptr, int64_t num_source_nodes = 0,
-                              const void *packed_in = nullptr, void *packed_out = nullptr) {
+                              size_t weight_cache_bytes, int32_t cache_valid, void *stream) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int H = state_dim, D = message_dim;
-    PTGNN_CHECK_ARG(num_types >= 0 && num_types <= PTGNN_MAX_EDGE_TYPES && (type_off || bp), "gated_forward: bad num_types=%d",
-                    num_types);
-    const bool fused_path = bp != nullptr;
-    if (fused_path && !fused_f32_ok(H, D)) {
-        set_error("gated_forward_fused: dims H=%d D=%d are not supported by the fused kernel", H, D);
-        return PTGNN_E_UNSUPPORTED;
-    }
-    const int64_t E = fused_path ? 0 : type_off[num_types];
-    if (num_source_nodes <= 0) num_source_nodes = num_nodes;
+    PTGNN_CHECK_ARG(num_types >= 0 && num_types <= PTGNN_MAX_EDGE_TYPES && type_off, "gated_forward: bad num_types=%d", num_types);
+    const int64_t E = type_off[num_types];
     int rc = check_layer_dims("gated_forward", num_nodes, E, H, D);
     if (rc) return rc;
     if (H % 32 != 0) {
@@ -401,8 +372,7 @@ static int gated_forward_impl(const float *node_states, const float *gather_stat
     PTGNN_CHECK_ARG(node_states && out_states && row_ptr && gru_w_ih && gru_w_hh && gru_b_ih && gru_b_hh,
                     "gated_forward: null pointer");
     PTGNN_CHECK_ARG(E == 0 || (pos && src32 && edge_weights), "gated_forward: null edge arrays");
-    PTGNN_CHECK_ARG(!fused_path || (bp->group_off && edge_weights && num_types > 0), "gated_forward_fused: null block plan arrays");
-    const GatedWs L = gated_ws_layout(num_nodes, num_source_nodes, E, num_types, H, D, fused_path);
+    const GatedWs L = gated_ws_layout(num_nodes, E, num_types, H, D);
     if (workspace_bytes < L.total || !workspace) {
         set_error("gated_forward: workspace %zu < required %zu", workspace_bytes, L.total);
         return PTGNN_E_WORKSPACE;
@@ -414,62 +384,15 @@ static int gated_forward_impl(const float *node_states, const float *gather_stat
     // derived weights: in the workspace (re-derived every call) or in the caller's cache (derived when !cache_valid)
     char *wsplit = ws + L.wsplit, *grupack = ws + L.grupack;
     bool pack = true;
-    const size_t need_cache = fused_path ? gated_fused_cache_bytes(num_types, H, D) : gated_cache_bytes(num_types, H, D);
+    const size_t need_cache = gated_cache_bytes(num_types, H, D);
     if (weight_cache != nullptr && need_cache > 0) {
         if (weight_cache_bytes < need_cache) {
             set_error("gated_forward: weight cache %zu < required %zu", weight_cache_bytes, need_cache);
             return PTGNN_E_WORKSPACE;
         }
         wsplit = static_cast<char *>(weight_cache);
-        grupack = wsplit + (fused_path ? fused::packed_weight_bytes(3, num_types, H, 0) : tc::split_edge_weights_bytes(num_types, D, H));
+        grupack = wsplit + tc::split_edge_weights_bytes(num_types, D, H);
         pack = !cache_valid;
-    }
-
-    if (fused_path) {
-        // 1+2. gather -> W_t -> segmented reduce in one kernel (no message buffer); fp32-exact via 3xFP16
-        if (pack) {
-            rc = fused::pack_weights(3, num_types, H, 0, edge_weights, wsplit, bp->status, st);
-            if (rc) return rc;
-        }
-        // packed_in (optional): node_states already as fp16 (hi | lo') rows -- the previous layer's GRU wrote them next to its
-        // fp32 output -- so the packing pass is skipped.  In a sharded run the gathered rows are a different tensor: they are
-        // packed here, and packed_in (this rank's rows) feeds the GRU.
-        const bool sharded = gather_states != nullptr && gather_states != node_states;
-        const void *src_rows = packed_in;
-        if (sharded || packed_in == nullptr) {
-            rc = fused::pack_states(gsrc, num_source_nodes, H, ws + L.xpack, bp->status, st);
-            if (rc) return rc;
-            src_rows = ws + L.xpack;
-        }
-        fused::AggregateArgs a{};
-        a.nprod = 3; a.src_rows = src_rows; a.tgt_rows = nullptr; a.num_nodes = num_nodes; a.K = H; a.num_types = num_types;
-        a.use_target = 0; a.reduce = reduce; a.block_targets = bp->block_targets; a.group_off = bp->group_off; a.src_f = bp->src_f;
-        a.tl_f = bp->tl_f; a.row_ptr = row_ptr; a.packed_weights = wsplit; a.epi = fused::Epilogue{PTGNN_ACT_NONE, nullptr, nullptr, 0.0f};
-        a.status = bp->status;
-        const bool ws_gru = gru_ws_enabled(3, H, D);
-        a.out = agg; a.out_mode = ws_gru ? 2 : 0;
-        rc = fused::aggregate(a, st);
-        if (rc) return rc;
-        if (!ws_gru) {
-            rc = tc::gru_update(agg, node_states, num_nodes, H, D, gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, out_states, grupack, pack, st);
-            if (rc || packed_out == nullptr) return rc;
-            return fused::pack_states(out_states, num_nodes, H, packed_out, bp->status, st);
-        }
-        // 3. GRUCell, weights-stationary, on the packed aggregate and the packed states (3xFP16)
-        if (pack) {
-            rc = gruws::pack(3, H, D, gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, grupack, st);
-            if (rc) return rc;
-        }
-        const void *h_rows = src_rows;
-        if (sharded) {      // the packed copy above holds the GATHERED rows; the GRU needs this rank's
-            h_rows = packed_in;
-            if (h_rows == nullptr) {
-                rc = fused::pack_states(node_states, num_nodes, H, ws + L.xpack_own, bp->status, st);
-                if (rc) return rc;
-                h_rows = ws + L.xpack_own;
-            }
-        }
-        return gruws::update(3, agg, h_rows, node_states, num_nodes, H, D, grupack, out_states, packed_out, bp->status, st);
     }
 
     // 1. per-edge messages, written at their target-sorted positions
@@ -507,18 +430,6 @@ static int gated_forward_impl(const float *node_states, const float *gather_stat
     return PTGNN_OK;
 }
 
-extern "C" int ptgnn_b200_gated_forward_f32(const float *node_states, const float *gather_states, int64_t num_nodes,
-                                            int32_t state_dim, int32_t message_dim, int32_t num_types,
-                                            const int64_t *type_off, const int32_t *row_ptr, const int32_t *pos,
-                                            const int32_t *src32, const float *const *edge_weights, const float *gru_w_ih,
-                                            const float *gru_w_hh, const float *gru_b_ih, const float *gru_b_hh,
-                                            int32_t reduce, float *out_states, void *workspace, size_t workspace_bytes,
-                                            void *stream) {
-    return gated_forward_impl(node_states, gather_states, num_nodes, state_dim, message_dim, num_types, type_off, row_ptr, pos,
-                              src32, edge_weights, gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, reduce, out_states, workspace,
-                              workspace_bytes, nullptr, 0, 0, stream);
-}
-
 extern "C" size_t ptgnn_b200_gated_weight_cache_bytes(int32_t num_types, int32_t state_dim, int32_t message_dim) {
     if (num_types < 0 || num_types > PTGNN_MAX_EDGE_TYPES || state_dim <= 0 || message_dim <= 0) return 0;
     return gated_cache_bytes(num_types, state_dim, message_dim);
@@ -540,35 +451,20 @@ extern "C" int ptgnn_b200_gated_forward_cached_f32(const float *node_states, con
 extern "C" size_t ptgnn_b200_mlp_workspace_bytes(int64_t num_nodes, int64_t num_edges, int32_t num_types, int32_t in_dim,
                                                  int32_t message_dim, int32_t out_dim, int32_t use_target_state) {
     if (num_nodes < 0 || num_edges < 0 || num_types < 0 || in_dim <= 0 || message_dim <= 0) return 0;
-    return mlp_ws_layout(num_nodes, num_nodes, num_edges, num_types, in_dim, message_dim, out_dim, use_target_state, false, false).total;
+    return mlp_ws_layout(num_nodes, num_edges, num_types, in_dim, message_dim, out_dim, use_target_state).total;
 }
 
-static size_t mlp_fused_cache_bytes(int T, int H, int D, int out_dim, int ut) {
-    return ws_slice(fused::packed_weight_bytes(3, T, H, ut), 1) + tc::dense_split_bytes(out_dim > 0 ? out_dim : D, D) + 256;
-}
-
-static int mlp_forward_impl(const float *node_states, const float *gather_states, int64_t num_nodes,
-                                          int32_t in_dim,
-                                          int32_t message_dim, int32_t out_dim, int32_t num_types,
-                                          const int64_t *type_off, const int32_t *row_ptr, const int32_t *pos,
-                                          const int32_t *src32, const int32_t *tgt32, const float *const *edge_weights,
-                                          int32_t use_target_state, int32_t reduce, int32_t message_activation,
-                                          const float *ln_weight, const float *ln_bias, float ln_eps,
-                                          const float *dense_weight, const float *dense_bias, int32_t dense_activation,
-                                          float *out_states, void *workspace, size_t workspace_bytes, void *stream,
-                                          const ptgnn_b200_block_plan *bp, int64_t num_source_nodes, void *weight_cache = nullptr,
-                                          size_t weight_cache_bytes = 0, int cache_valid = 0) {
+static int mlp_forward_impl(const float *node_states, const float *gather_states, int64_t num_nodes, int32_t in_dim,
+                            int32_t message_dim, int32_t out_dim, int32_t num_types, const int64_t *type_off,
+                            const int32_t *row_ptr, const int32_t *pos, const int32_t *src32, const int32_t *tgt32,
+                            const float *const *edge_weights, int32_t use_target_state, int32_t reduce,
+                            int32_t message_activation, const float *ln_weight, const float *ln_bias, float ln_eps,
+                            const float *dense_weight, const float *dense_bias, int32_t dense_activation, float *out_states,
+                            void *workspace, size_t workspace_bytes, void *stream) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int H = in_dim, D = message_dim;
-    PTGNN_CHECK_ARG(num_types >= 0 && num_types <= PTGNN_MAX_EDGE_TYPES && (type_off || bp), "mlp_forward: bad num_types=%d",
-                    num_types);
-    const bool fused_path = bp != nullptr;
-    if (fused_path && !(tc_enabled() && fused::supported(3, H, D, use_target_state))) {
-        set_error("mlp_forward_fused: dims H=%d D=%d are not supported by the fused kernel", H, D);
-        return PTGNN_E_UNSUPPORTED;
-    }
-    const int64_t E = fused_path ? 0 : type_off[num_types];
-    if (num_source_nodes <= 0) num_source_nodes = num_nodes;
+    PTGNN_CHECK_ARG(num_types >= 0 && num_types <= PTGNN_MAX_EDGE_TYPES && type_off, "mlp_forward: bad num_types=%d", num_types);
+    const int64_t E = type_off[num_types];
     int rc = check_layer_dims("mlp_forward", num_nodes, E, H, D);
     if (rc) return rc;
     PTGNN_CHECK_ARG(reduce >= PTGNN_REDUCE_SUM && reduce <= PTGNN_REDUCE_MIN, "mlp_forward: bad reduce %d", reduce);
@@ -581,9 +477,7 @@ static int mlp_forward_impl(const float *node_states, const float *gather_states
     PTGNN_CHECK_ARG(node_states && out_states && row_ptr, "mlp_forward: null pointer");
     PTGNN_CHECK_ARG(E == 0 || (pos && src32 && edge_weights && (!use_target_state || tgt32)),
                     "mlp_forward: null edge arrays");
-    PTGNN_CHECK_ARG(!fused_path || (bp->group_off && edge_weights && num_types > 0), "mlp_forward_fused: null block plan arrays");
-    const MlpWs L = mlp_ws_layout(num_nodes, num_source_nodes, E, num_types, H, D, out_dim, use_target_state, fused_path,
-                                  gather_states != nullptr);
+    const MlpWs L = mlp_ws_layout(num_nodes, E, num_types, H, D, out_dim, use_target_state);
     if (workspace_bytes < L.total || !workspace) {
         set_error("mlp_forward: workspace %zu < required %zu", workspace_bytes, L.total);
         return PTGNN_E_WORKSPACE;
@@ -594,55 +488,19 @@ static int mlp_forward_impl(const float *node_states, const float *gather_states
     const int ut = use_target_state ? 1 : 0;
     const float *gsrc = gather_states ? gather_states : node_states;   // rows that `src32` indexes (sharded runs)
 
-    // derived weights: in the workspace (re-derived every call) or in the caller's cache (derived when !cache_valid); fused path only
-    char *wsplit = ws + L.wsplit, *dsplit = ws + L.dsplit;
-    bool pack = true;
-    if (fused_path && weight_cache != nullptr) {
-        const size_t need = mlp_fused_cache_bytes(num_types, H, D, out_dim, ut);
-        if (weight_cache_bytes < need) {
-            set_error("mlp_forward_fused: weight cache %zu < required %zu", weight_cache_bytes, need);
-            return PTGNN_E_WORKSPACE;
-        }
-        wsplit = static_cast<char *>(weight_cache);
-        dsplit = wsplit + ws_slice(fused::packed_weight_bytes(3, num_types, H, ut), 1);
-        pack = !cache_valid;
-    }
-    if (fused_path) {
-        if (pack) {
-            rc = fused::pack_weights(3, num_types, H, ut, edge_weights, wsplit, bp->status, st);
-            if (rc) return rc;
-        }
-        rc = fused::pack_states(gsrc, num_source_nodes, H, ws + L.xpack, bp->status, st);
-        if (rc) return rc;
-        const void *tgt_rows = ws + L.xpack;
-        if (ut && gather_states != nullptr) {      // sharded run: targets are this rank's rows, not the gathered ones
-            rc = fused::pack_states(node_states, num_nodes, H, ws + L.xpack_tgt, bp->status, st);
-            if (rc) return rc;
-            tgt_rows = ws + L.xpack_tgt;
-        }
-        fused::AggregateArgs a{};
-        a.nprod = 3; a.src_rows = ws + L.xpack; a.tgt_rows = tgt_rows; a.num_nodes = num_nodes; a.K = H; a.num_types = num_types;
-        a.use_target = ut; a.reduce = reduce; a.block_targets = bp->block_targets; a.group_off = bp->group_off; a.src_f = bp->src_f;
-        a.tl_f = bp->tl_f; a.row_ptr = row_ptr; a.packed_weights = wsplit;
-        a.epi = fused::Epilogue{message_activation, ln_weight, ln_bias, ln_eps};
-        a.out = y; a.out_mode = 0; a.status = bp->status;
-        rc = fused::aggregate(a, st);
-        if (rc) return rc;
+    if (tc_enabled() && tc::supported_message(H, D)) {
+        rc = tc::edge_messages(gsrc, node_states, H, D, ut, num_types, type_off, edge_weights, src32, tgt32, pos, msg,
+                               ws + L.wsplit, true, st);
     } else {
-        if (tc_enabled() && tc::supported_message(H, D)) {
-            rc = tc::edge_messages(gsrc, node_states, H, D, ut, num_types, type_off, edge_weights, src32, tgt32, pos, msg,
-                                   ws + L.wsplit, true, st);
-        } else {
-            rc = launch_edge_messages(gsrc, node_states, H, D, ut, num_types, type_off, edge_weights, src32, tgt32, pos, msg,
-                                      st);
-        }
-        if (rc) return rc;
-        ReduceEpilogue epi{0, message_activation, ln_weight, ln_bias, ln_eps};
-        rc = launch_segment_reduce(msg, row_ptr, nullptr, num_nodes, E, D, reduce, y, nullptr, &epi, st);
-        if (rc) return rc;
+        rc = launch_edge_messages(gsrc, node_states, H, D, ut, num_types, type_off, edge_weights, src32, tgt32, pos, msg,
+                                  st);
     }
+    if (rc) return rc;
+    ReduceEpilogue epi{0, message_activation, ln_weight, ln_bias, ln_eps};
+    rc = launch_segment_reduce(msg, row_ptr, nullptr, num_nodes, E, D, reduce, y, nullptr, &epi, st);
+    if (rc) return rc;
     if (!dense_weight) return PTGNN_OK;
-    return dense_any(y, num_nodes, D, dense_weight, dense_bias, out_dim, dense_activation, out_states, dsplit, st, pack);
+    return dense_any(y, num_nodes, D, dense_weight, dense_bias, out_dim, dense_activation, out_states, ws + L.dsplit, st);
 }
 
 extern "C" int ptgnn_b200_mlp_forward_f32(const float *node_states, const float *gather_states, int64_t num_nodes,
@@ -655,143 +513,7 @@ extern "C" int ptgnn_b200_mlp_forward_f32(const float *node_states, const float 
                                           float *out_states, void *workspace, size_t workspace_bytes, void *stream) {
     return mlp_forward_impl(node_states, gather_states, num_nodes, in_dim, message_dim, out_dim, num_types, type_off, row_ptr, pos,
                             src32, tgt32, edge_weights, use_target_state, reduce, message_activation, ln_weight, ln_bias, ln_eps,
-                            dense_weight, dense_bias, dense_activation, out_states, workspace, workspace_bytes, stream, nullptr, 0);
-}
-
-// ---- fused entry points (fp32 states here, bf16 states in layers_bf16.cu) --------------------------------------------------
-namespace ptgnn {
-namespace tcb {
-size_t gated_fused_workspace_bytes_bf16(int64_t N, int T, int H, int D);
-size_t gated_fused_cache_bytes_bf16(int T, int H, int D);
-int gated_forward_fused_bf16(const uint16_t *node_states, const uint16_t *gather_states, int64_t num_nodes, int32_t state_dim,
-                             int32_t message_dim, int32_t num_types, const ptgnn_b200_block_plan *bp, const int32_t *row_ptr,
-                             const float *const *edge_weights, const float *gru_w_ih, const float *gru_w_hh, const float *gru_b_ih,
-                             const float *gru_b_hh, int32_t reduce, uint16_t *out_states, void *workspace, size_t workspace_bytes,
-                             void *weight_cache, size_t weight_cache_bytes, int32_t cache_valid, void *stream);
-size_t mlp_fused_workspace_bytes_bf16(int64_t N, int T, int H, int D, int Hout, int use_target);
-int mlp_forward_fused_bf16(const uint16_t *node_states, const uint16_t *gather_states, int64_t num_nodes, int32_t in_dim,
-                           int32_t message_dim, int32_t out_dim, int32_t num_types, const ptgnn_b200_block_plan *bp,
-                           const int32_t *row_ptr, const float *const *edge_weights, int32_t use_target_state, int32_t reduce,
-                           int32_t message_activation, const float *ln_weight, const float *ln_bias, float ln_eps,
-                           const float *dense_weight, const float *dense_bias, int32_t dense_activation, uint16_t *out_states,
-                           void *workspace, size_t workspace_bytes, void *stream);
-}  // namespace tcb
-}  // namespace ptgnn
-
-extern "C" int32_t ptgnn_b200_block_plan_block_targets(int64_t num_nodes) { return fused::recommended_block_targets(num_nodes); }
-
-extern "C" int32_t ptgnn_b200_fused_supported(int32_t bf16_states, int32_t state_dim, int32_t message_dim) {
-    if (!tc_enabled()) return 0;
-    if (bf16_states) return fused::supported(1, state_dim, message_dim, 0) && state_dim % 32 == 0 ? 1 : 0;
-    return fused_f32_ok(state_dim, message_dim) ? 1 : 0;
-}
-
-extern "C" size_t ptgnn_b200_gated_fused_workspace_bytes(int32_t bf16_states, int64_t num_nodes, int64_t num_source_nodes,
-                                                         int32_t num_types, int32_t state_dim, int32_t message_dim) {
-    if (num_nodes < 0 || num_types < 0 || state_dim <= 0 || message_dim <= 0) return 0;
-    if (num_source_nodes <= 0) num_source_nodes = num_nodes;
-    if (bf16_states) return tcb::gated_fused_workspace_bytes_bf16(num_nodes, num_types, state_dim, message_dim);
-    return gated_ws_layout(num_nodes, num_source_nodes, 0, num_types, state_dim, message_dim, true).total;
-}
-extern "C" size_t ptgnn_b200_gated_fused_weight_cache_bytes(int32_t bf16_states, int32_t num_types, int32_t state_dim,
-                                                            int32_t message_dim) {
-    if (num_types < 0 || num_types > PTGNN_MAX_EDGE_TYPES || state_dim <= 0 || message_dim <= 0) return 0;
-    if (bf16_states) return tcb::gated_fused_cache_bytes_bf16(num_types, state_dim, message_dim);
-    return gated_fused_cache_bytes(num_types, state_dim, message_dim);
-}
-extern "C" int ptgnn_b200_gated_forward_fused(int32_t bf16_states, const void *node_states, const void *gather_states,
-                                              int64_t num_nodes, int64_t num_source_nodes, int32_t state_dim, int32_t message_dim,
-                                              int32_t num_types, const ptgnn_b200_block_plan *block_plan, const int32_t *row_ptr,
-                                              const float *const *edge_weights, const float *gru_w_ih, const float *gru_w_hh,
-                                              const float *gru_b_ih, const float *gru_b_hh, int32_t reduce, void *out_states,
-                                              void *workspace, size_t workspace_bytes, void *weight_cache,
-                                              size_t weight_cache_bytes, int32_t cache_valid, void *stream) {
-    PTGNN_CHECK_ARG(block_plan != nullptr, "gated_forward_fused: null block plan");
-    if (bf16_states)
-        return tcb::gated_forward_fused_bf16(static_cast<const uint16_t *>(node_states), static_cast<const uint16_t *>(gather_states),
-                                             num_nodes, state_dim, message_dim, num_types, block_plan, row_ptr, edge_weights, gru_w_ih,
-                                             gru_w_hh, gru_b_ih, gru_b_hh, reduce, static_cast<uint16_t *>(out_states), workspace,
-                                             workspace_bytes, weight_cache, weight_cache_bytes, cache_valid, stream);
-    return gated_forward_impl(static_cast<const float *>(node_states), static_cast<const float *>(gather_states), num_nodes, state_dim,
-                              message_dim, num_types, nullptr, row_ptr, nullptr, nullptr, edge_weights, gru_w_ih, gru_w_hh, gru_b_ih,
-                              gru_b_hh, reduce, static_cast<float *>(out_states), workspace, workspace_bytes, weight_cache,
-                              weight_cache_bytes, cache_valid, stream, block_plan, num_source_nodes);
-}
-
-extern "C" size_t ptgnn_b200_packed_state_bytes(int64_t num_nodes, int32_t state_dim) {
-    if (num_nodes < 0 || state_dim <= 0) return 0;
-    return fused::packed_state_bytes(3, num_nodes, state_dim);
-}
-extern "C" int ptgnn_b200_gated_forward_fused_chained(const float *node_states, const float *gather_states, const void *packed_states_in,
-                                                      int64_t num_nodes, int64_t num_source_nodes, int32_t state_dim,
-                                                      int32_t message_dim, int32_t num_types, const ptgnn_b200_block_plan *block_plan,
-                                                      const int32_t *row_ptr, const float *const *edge_weights, const float *gru_w_ih,
-                                                      const float *gru_w_hh, const float *gru_b_ih, const float *gru_b_hh,
-                                                      int32_t reduce, float *out_states, void *packed_states_out, void *workspace,
-                                                      size_t workspace_bytes, void *weight_cache, size_t weight_cache_bytes,
-                                                      int32_t cache_valid, void *stream) {
-    PTGNN_CHECK_ARG(block_plan != nullptr, "gated_forward_fused_chained: null block plan");
-    return gated_forward_impl(node_states, gather_states, num_nodes, state_dim, message_dim, num_types, nullptr, row_ptr, nullptr, nullptr,
-                              edge_weights, gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, reduce, out_states, workspace, workspace_bytes,
-                              weight_cache, weight_cache_bytes, cache_valid, stream, block_plan, num_source_nodes, packed_states_in,
-                              packed_states_out);
-}
-
-extern "C" size_t ptgnn_b200_mlp_fused_workspace_bytes(int32_t bf16_states, int64_t num_nodes, int64_t num_source_nodes,
-                                                       int32_t num_types, int32_t in_dim, int32_t message_dim, int32_t out_dim,
-                                                       int32_t use_target_state) {
-    if (num_nodes < 0 || num_types < 0 || in_dim <= 0 || message_dim <= 0) return 0;
-    if (num_source_nodes <= 0) num_source_nodes = num_nodes;
-    if (bf16_states) return tcb::mlp_fused_workspace_bytes_bf16(num_nodes, num_types, in_dim, message_dim, out_dim, use_target_state);
-    return mlp_ws_layout(num_nodes, num_source_nodes, 0, num_types, in_dim, message_dim, out_dim, use_target_state, true, true).total;
-}
-extern "C" int ptgnn_b200_mlp_forward_fused(int32_t bf16_states, const void *node_states, const void *gather_states,
-                                            int64_t num_nodes, int64_t num_source_nodes, int32_t in_dim, int32_t message_dim,
-                                            int32_t out_dim, int32_t num_types, const ptgnn_b200_block_plan *block_plan,
-                                            const int32_t *row_ptr, const float *const *edge_weights, int32_t use_target_state,
-                                            int32_t reduce, int32_t message_activation, const float *ln_weight,
-                                            const float *ln_bias, float ln_eps, const float *dense_weight, const float *dense_bias,
-                                            int32_t dense_activation, void *out_states, void *workspace, size_t workspace_bytes,
-                                            void *stream) {
-    PTGNN_CHECK_ARG(block_plan != nullptr, "mlp_forward_fused: null block plan");
-    if (bf16_states)
-        return tcb::mlp_forward_fused_bf16(static_cast<const uint16_t *>(node_states), static_cast<const uint16_t *>(gather_states),
-                                           num_nodes, in_dim, message_dim, out_dim, num_types, block_plan, row_ptr, edge_weights,
-                                           use_target_state, reduce, message_activation, ln_weight, ln_bias, ln_eps, dense_weight,
-                                           dense_bias, dense_activation, static_cast<uint16_t *>(out_states), workspace,
-                                           workspace_bytes, stream);
-    return mlp_forward_impl(static_cast<const float *>(node_states), static_cast<const float *>(gather_states), num_nodes, in_dim,
-                            message_dim, out_dim, num_types, nullptr, row_ptr, nullptr, nullptr, nullptr, edge_weights,
-                            use_target_state, reduce, message_activation, ln_weight, ln_bias, ln_eps, dense_weight, dense_bias,
-                            dense_activation, static_cast<float *>(out_states), workspace, workspace_bytes, stream, block_plan,
-                            num_source_nodes);
-}
-
-extern "C" size_t ptgnn_b200_mlp_fused_weight_cache_bytes(int32_t bf16_states, int32_t num_types, int32_t in_dim, int32_t message_dim,
-                                                          int32_t out_dim, int32_t use_target_state) {
-    if (bf16_states || num_types <= 0 || in_dim <= 0 || message_dim <= 0) return 0;
-    if (!(tc_enabled() && fused::supported(3, in_dim, message_dim, use_target_state))) return 0;
-    return mlp_fused_cache_bytes(num_types, in_dim, message_dim, out_dim, use_target_state ? 1 : 0);
-}
-extern "C" int ptgnn_b200_mlp_forward_fused_cached(int32_t bf16_states, const void *node_states, const void *gather_states, int64_t num_nodes,
-                                                   int64_t num_source_nodes, int32_t in_dim, int32_t message_dim, int32_t out_dim,
-                                                   int32_t num_types, const ptgnn_b200_block_plan *block_plan, const int32_t *row_ptr,
-                                                   const float *const *edge_weights, int32_t use_target_state, int32_t reduce,
-                                                   int32_t message_activation, const float *ln_weight, const float *ln_bias, float ln_eps,
-                                                   const float *dense_weight, const float *dense_bias, int32_t dense_activation,
-                                                   void *out_states, void *workspace, size_t workspace_bytes, void *weight_cache,
-                                                   size_t weight_cache_bytes, int32_t cache_valid, void *stream) {
-    if (bf16_states || weight_cache == nullptr)
-        return ptgnn_b200_mlp_forward_fused(bf16_states, node_states, gather_states, num_nodes, num_source_nodes, in_dim, message_dim, out_dim,
-                                            num_types, block_plan, row_ptr, edge_weights, use_target_state, reduce, message_activation,
-                                            ln_weight, ln_bias, ln_eps, dense_weight, dense_bias, dense_activation, out_states, workspace,
-                                            workspace_bytes, stream);
-    PTGNN_CHECK_ARG(block_plan != nullptr, "mlp_forward_fused_cached: null block plan");
-    return mlp_forward_impl(static_cast<const float *>(node_states), static_cast<const float *>(gather_states), num_nodes, in_dim, message_dim,
-                            out_dim, num_types, nullptr, row_ptr, nullptr, nullptr, nullptr, edge_weights, use_target_state, reduce,
-                            message_activation, ln_weight, ln_bias, ln_eps, dense_weight, dense_bias, dense_activation,
-                            static_cast<float *>(out_states), workspace, workspace_bytes, stream, block_plan, num_source_nodes, weight_cache,
-                            weight_cache_bytes, cache_valid);
+                            dense_weight, dense_bias, dense_activation, out_states, workspace, workspace_bytes, stream);
 }
 
 /* ---- stand-alone pieces (MLP.forward, message MLPs with hidden layers, module aggregators) -------------------------------------- */

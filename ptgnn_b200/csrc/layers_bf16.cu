@@ -7,9 +7,8 @@
 #include <float.h>
 #include <stdlib.h>
 
+#include "layers.cuh"
 #include "layers_tc.cuh"
-#include "fused_mp.cuh"
-#include "gru_ws.cuh"
 #include "tc_pipeline_bf16.cuh"
 
 namespace ptgnn {
@@ -460,7 +459,7 @@ static int launch_pipeline(const typename Policy::Params &p, int total_tiles, in
     return PTGNN_OK;
 }
 
-struct WsB { size_t msg, agg, w, p1, p2, bias, gws, total; };
+struct WsB { size_t msg, agg, w, p1, p2, bias, total; };
 static WsB ws_layout(int64_t N, int64_t E, int T, int H, int D) {
     WsB w{};
     size_t o = 0;
@@ -471,9 +470,29 @@ static WsB ws_layout(int64_t N, int64_t E, int T, int H, int D) {
     w.p1 = add((size_t)(H / 32 + 1) * 128 * D);
     w.p2 = add((size_t)(H / 32 + 1) * 128 * H);
     w.bias = add((size_t)H * 8 + 8);
-    w.gws = add(gruws::supported(1, H, D) ? gruws::pack_bytes(1, H, D) / 2 + 8 : 8);   // weights-stationary GRU packing (fused path)
     w.total = o;
     return w;
+}
+
+size_t dense_weight_bytes(int Hout, int D) { return ws_slice((size_t)Hout * D + 8, 2); }
+
+int dense_update(const __nv_bfloat16 *y, int64_t rows, int D, const float *W, const float *bias, int Hout, int act,
+                 __nv_bfloat16 *out, void *scratch, cudaStream_t st) {
+    __nv_bfloat16 *wd = static_cast<__nv_bfloat16 *>(scratch);
+    ConvSrc cs{};
+    cs.num = 1; cs.elems = Hout * D; cs.w[0] = W;
+    {
+        TimedScope timed__(PTGNN_KERNEL_PACK, st);
+        convert_weights_kernel<<<132, 256, 0, st>>>(cs, wd);
+    }
+    PTGNN_LAUNCHED();
+    DensePolicyB::Params dp{};
+    int rc = make_map_bf16(&dp.map_y, y, rows, D, 128);
+    if (!rc) rc = make_map_bf16(&dp.map_w, wd, Hout, D, Hout < 128 ? Hout : 128);
+    if (rc) return rc;
+    dp.bias = bias; dp.out = out; dp.num_nodes = (int)rows; dp.D = D; dp.Hout = Hout; dp.act = act;
+    dp.n_blocks = (Hout + 127) / 128; dp.dbg = debug_bits(); dp.trace = tc::trace_buffer(PTGNN_KERNEL_DENSE + 10);
+    return launch_pipeline<DensePolicyB>(dp, (int)ceil_div(rows, TILE_M) * dp.n_blocks, PTGNN_KERNEL_DENSE, st);
 }
 
 }  // namespace tcb
@@ -500,16 +519,11 @@ static int gated_forward_bf16_impl(const uint16_t *node_states, const uint16_t *
                                    const float *const *edge_weights, const float *gru_w_ih, const float *gru_w_hh,
                                    const float *gru_b_ih, const float *gru_b_hh, int32_t reduce, uint16_t *out_states,
                                    void *workspace, size_t workspace_bytes, void *weight_cache, size_t weight_cache_bytes,
-                                   int32_t cache_valid, void *stream, const ptgnn_b200_block_plan *bp = nullptr) {
+                                   int32_t cache_valid, void *stream) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int H = state_dim, D = message_dim;
-    PTGNN_CHECK_ARG(num_types >= 0 && num_types <= PTGNN_MAX_EDGE_TYPES && (type_off || bp), "gated_forward_bf16: bad num_types=%d", num_types);
-    const bool fused_path = bp != nullptr;
-    if (fused_path && !fused::supported(1, H, D, 0)) {
-        set_error("gated_forward_fused (bf16): dims H=%d D=%d are not supported by the fused kernel", H, D);
-        return PTGNN_E_UNSUPPORTED;
-    }
-    const int64_t E = fused_path ? 0 : type_off[num_types];
+    PTGNN_CHECK_ARG(num_types >= 0 && num_types <= PTGNN_MAX_EDGE_TYPES && type_off, "gated_forward_bf16: bad num_types=%d", num_types);
+    const int64_t E = type_off[num_types];
     PTGNN_CHECK_ARG(num_nodes >= 0 && num_nodes < INT32_MAX && E >= 0 && E < INT32_MAX, "gated_forward_bf16: sizes out of range");
     if (H % 32 != 0 || D % 16 != 0 || H < 64 || D < 64 || D > 256 || H > 1024) {
         set_error("gated_forward_bf16: needs state dim %% 32 == 0 (>= 64) and message dim %% 16 == 0 in [64, 256]; got %d, %d", H, D);
@@ -519,7 +533,6 @@ static int gated_forward_bf16_impl(const uint16_t *node_states, const uint16_t *
     if (num_nodes == 0) return PTGNN_OK;
     PTGNN_CHECK_ARG(node_states && out_states && row_ptr && gru_w_ih && gru_w_hh && gru_b_ih && gru_b_hh, "gated_forward_bf16: null pointer");
     PTGNN_CHECK_ARG(E == 0 || (pos && src32 && edge_weights), "gated_forward_bf16: null edge arrays");
-    PTGNN_CHECK_ARG(!fused_path || (bp->group_off && edge_weights && num_types > 0), "gated_forward_fused (bf16): null block plan arrays");
     const WsB L = ws_layout(num_nodes, E, num_types, H, D);
     if (workspace_bytes < L.total || !workspace) {
         set_error("gated_forward_bf16: workspace %zu < required %zu", workspace_bytes, L.total);
@@ -548,19 +561,14 @@ static int gated_forward_bf16_impl(const uint16_t *node_states, const uint16_t *
 
     // 0. weights -> bf16 (edge weights [T][D][H]; GRU gate blocks)
     if (pack) {
-        if (fused_path) {       // same bytes as the plain bf16 copy, in the fused kernel's packed per-row layout
-            const int prc = fused::pack_weights(1, num_types, H, 0, edge_weights, wb, bp->status, st);
-            if (prc) return prc;
-        } else {
-            ConvSrc cs{};
-            cs.num = num_types; cs.elems = D * H;
-            for (int t = 0; t < num_types; ++t) cs.w[t] = edge_weights[t];
-            {
-                TimedScope timed__(PTGNN_KERNEL_PACK, st);
-                convert_weights_kernel<<<132, 256, 0, st>>>(cs, wb);
-            }
-            PTGNN_LAUNCHED();
+        ConvSrc cs{};
+        cs.num = num_types; cs.elems = D * H;
+        for (int t = 0; t < num_types; ++t) cs.w[t] = edge_weights[t];
+        {
+            TimedScope timed__(PTGNN_KERNEL_PACK, st);
+            convert_weights_kernel<<<132, 256, 0, st>>>(cs, wb);
         }
+        PTGNN_LAUNCHED();
         {
             TimedScope timed__(PTGNN_KERNEL_PACK, st);
             pack_gru_bf16_kernel<<<132, 256, 0, st>>>(gru_w_ih, gru_w_hh, H, D, p1, p2);
@@ -573,30 +581,9 @@ static int gated_forward_bf16_impl(const uint16_t *node_states, const uint16_t *
         PTGNN_LAUNCHED();
     }
 
-    int rc = PTGNN_OK;
-    if (fused_path) {
-        // 1+2. gather -> W_t -> segmented reduce in one kernel (no message buffer)
-        fused::AggregateArgs a{};
-        a.nprod = 1; a.src_rows = hsrc; a.tgt_rows = nullptr; a.num_nodes = num_nodes; a.K = H; a.num_types = num_types;
-        a.use_target = 0; a.reduce = reduce; a.block_targets = bp->block_targets; a.group_off = bp->group_off; a.src_f = bp->src_f;
-        a.tl_f = bp->tl_f; a.row_ptr = row_ptr; a.packed_weights = wb; a.epi = fused::Epilogue{PTGNN_ACT_NONE, nullptr, nullptr, 0.0f};
-        a.out = agg; a.out_mode = 1; a.status = bp->status;
-        rc = fused::aggregate(a, st);
-        if (rc) return rc;
-        static const bool ws_gru_on = [] { const char *e = getenv("PTGNN_B200_GRU"); return !(e && e[0] == 't'); }();
-        if (ws_gru_on && gruws::supported(1, H, D)) {
-            // 3. GRUCell, weights-stationary (the gate weights stay in shared memory, only node rows stream)
-            char *gws = wbase + (L.gws - L.w);
-            if (pack) {
-                rc = gruws::pack(1, H, D, gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, gws, st);
-                if (rc) return rc;
-            }
-            return gruws::update(1, agg, h, h, num_nodes, H, D, gws, out_states, nullptr, nullptr, st);
-        }
-    } else {
     // 1. messages
     MsgPolicyB::Params mp{};
-    rc = make_map_bf16(&mp.map_w, wb, (uint64_t)num_types * D, H, D < 128 ? D : 128);
+    int rc = make_map_bf16(&mp.map_w, wb, (uint64_t)num_types * D, H, D < 128 ? D : 128);
     if (rc) return rc;
     mp.h = hsrc; mp.h_tgt = h; mp.src32 = src32; mp.tgt32 = nullptr; mp.use_target = 0; mp.pos = pos; mp.msg = msg; mp.H = H; mp.D = D;
     mp.num_types = num_types;
@@ -615,7 +602,6 @@ static int gated_forward_bf16_impl(const uint16_t *node_states, const uint16_t *
     // 2. segmented reduce (fp32 accumulate, bf16 result)
     rc = reduce_bf16(reduce, msg, row_ptr, num_nodes, D, agg, nullptr, st);
     if (rc) return rc;
-    }
 
     // 3. GRUCell
     GruPolicyB::Params gp{};
@@ -628,18 +614,6 @@ static int gated_forward_bf16_impl(const uint16_t *node_states, const uint16_t *
     gp.h = h; gp.bias4 = bias4; gp.out = reinterpret_cast<__nv_bfloat16 *>(out_states);
     gp.num_nodes = (int)num_nodes; gp.H = H; gp.D = D; gp.n_jb = H / 32; gp.dbg = debug_bits(); gp.trace = tc::trace_buffer(PTGNN_KERNEL_GRU + 10);
     return launch_pipeline<GruPolicyB>(gp, (int)ceil_div(num_nodes, TILE_M) * gp.n_jb, PTGNN_KERNEL_GRU, st);
-}
-
-extern "C" int ptgnn_b200_gated_forward_bf16(const uint16_t *node_states, const uint16_t *gather_states, int64_t num_nodes,
-                                             int32_t state_dim, int32_t message_dim, int32_t num_types,
-                                             const int64_t *type_off, const int32_t *row_ptr, const int32_t *pos,
-                                             const int32_t *src32, const float *const *edge_weights, const float *gru_w_ih,
-                                             const float *gru_w_hh, const float *gru_b_ih, const float *gru_b_hh,
-                                             int32_t reduce, uint16_t *out_states, void *workspace, size_t workspace_bytes,
-                                             void *stream) {
-    return gated_forward_bf16_impl(node_states, gather_states, num_nodes, state_dim, message_dim, num_types, type_off, row_ptr,
-                                   pos, src32, edge_weights, gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, reduce, out_states,
-                                   workspace, workspace_bytes, nullptr, 0, 0, stream);
 }
 
 extern "C" size_t ptgnn_b200_gated_weight_cache_bytes_bf16(int32_t num_types, int32_t state_dim, int32_t message_dim) {
@@ -675,7 +649,7 @@ static MlpWsB mlp_ws_layout(int64_t N, int64_t E, int T, int H, int D, int Hout,
     w.msg = add((size_t)E * D + 8);
     w.y = add((size_t)N * D + 8);
     w.w = add((size_t)T * D * H * (use_target ? 2 : 1) + 8);
-    w.wd = add((size_t)Hout * D + 8);
+    w.wd = o; o += dense_weight_bytes(Hout, D);
     w.total = o;
     return w;
 }
@@ -689,23 +663,17 @@ extern "C" size_t ptgnn_b200_mlp_workspace_bytes_bf16(int64_t num_nodes, int64_t
 }
 
 static int mlp_forward_bf16_impl(const uint16_t *node_states, const uint16_t *gather_states, int64_t num_nodes,
-                                           int32_t in_dim, int32_t message_dim, int32_t out_dim, int32_t num_types,
-                                           const int64_t *type_off, const int32_t *row_ptr, const int32_t *pos,
-                                           const int32_t *src32, const int32_t *tgt32, const float *const *edge_weights,
-                                           int32_t use_target_state, int32_t reduce, int32_t message_activation,
-                                           const float *ln_weight, const float *ln_bias, float ln_eps,
-                                           const float *dense_weight, const float *dense_bias, int32_t dense_activation,
-                                           uint16_t *out_states, void *workspace, size_t workspace_bytes, void *stream,
-                                           const ptgnn_b200_block_plan *bp) {
+                                 int32_t in_dim, int32_t message_dim, int32_t out_dim, int32_t num_types,
+                                 const int64_t *type_off, const int32_t *row_ptr, const int32_t *pos,
+                                 const int32_t *src32, const int32_t *tgt32, const float *const *edge_weights,
+                                 int32_t use_target_state, int32_t reduce, int32_t message_activation,
+                                 const float *ln_weight, const float *ln_bias, float ln_eps,
+                                 const float *dense_weight, const float *dense_bias, int32_t dense_activation,
+                                 uint16_t *out_states, void *workspace, size_t workspace_bytes, void *stream) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int H = in_dim, D = message_dim, ut = use_target_state ? 1 : 0, Kw = H * (1 + ut);
-    PTGNN_CHECK_ARG(num_types >= 0 && num_types <= PTGNN_MAX_EDGE_TYPES && (type_off || bp), "mlp_forward_bf16: bad num_types=%d", num_types);
-    const bool fused_path = bp != nullptr;
-    if (fused_path && !fused::supported(1, H, D, ut)) {
-        set_error("mlp_forward_fused (bf16): dims H=%d D=%d are not supported by the fused kernel", H, D);
-        return PTGNN_E_UNSUPPORTED;
-    }
-    const int64_t E = fused_path ? 0 : type_off[num_types];
+    PTGNN_CHECK_ARG(num_types >= 0 && num_types <= PTGNN_MAX_EDGE_TYPES && type_off, "mlp_forward_bf16: bad num_types=%d", num_types);
+    const int64_t E = type_off[num_types];
     PTGNN_CHECK_ARG(num_nodes >= 0 && num_nodes < INT32_MAX && E >= 0 && E < INT32_MAX, "mlp_forward_bf16: sizes out of range");
     PTGNN_CHECK_ARG(dense_weight ? out_dim > 0 : out_dim == D, "mlp_forward_bf16: out_dim=%d inconsistent", out_dim);
     if (H % 32 != 0 || D % 16 != 0 || H < 64 || D < 64 || D > 256 || H > 1024 || (dense_weight && (out_dim % 16 != 0 || out_dim < 64))) {
@@ -730,16 +698,12 @@ static int mlp_forward_bf16_impl(const uint16_t *node_states, const uint16_t *ga
     const __nv_bfloat16 *h = reinterpret_cast<const __nv_bfloat16 *>(node_states);
     const __nv_bfloat16 *hsrc = gather_states ? reinterpret_cast<const __nv_bfloat16 *>(gather_states) : h;
     __nv_bfloat16 *out = reinterpret_cast<__nv_bfloat16 *>(out_states);
-    __nv_bfloat16 *msg = b16(L.msg), *wb = b16(L.w), *wd = b16(L.wd);
+    __nv_bfloat16 *msg = b16(L.msg), *wb = b16(L.w);
     __nv_bfloat16 *y = dense_weight ? b16(L.y) : out;
 
-    // 0. weights -> bf16
+    // 0. edge weights -> bf16
     int rc = PTGNN_OK;
-    if (fused_path) {
-        PTGNN_CHECK_ARG(bp->group_off && edge_weights && num_types > 0, "mlp_forward_fused (bf16): null block plan arrays");
-        rc = fused::pack_weights(1, num_types, H, ut, edge_weights, wb, bp->status, st);
-        if (rc) return rc;
-    } else if (num_types > 0) {
+    if (num_types > 0) {
         ConvSrc cs{};
         cs.num = num_types; cs.elems = D * Kw;
         for (int t = 0; t < num_types; ++t) cs.w[t] = edge_weights[t];
@@ -749,27 +713,7 @@ static int mlp_forward_bf16_impl(const uint16_t *node_states, const uint16_t *ga
         }
         PTGNN_LAUNCHED();
     }
-    if (dense_weight) {
-        ConvSrc cs{};
-        cs.num = 1; cs.elems = out_dim * D; cs.w[0] = dense_weight;
-        {
-            TimedScope timed__(PTGNN_KERNEL_PACK, st);
-            convert_weights_kernel<<<132, 256, 0, st>>>(cs, wd);
-        }
-        PTGNN_LAUNCHED();
-    }
 
-    if (fused_path) {
-        // 1+2. gather -> W_t -> segmented reduce (+ activation + LayerNorm at write-out) in one kernel
-        fused::AggregateArgs a{};
-        a.nprod = 1; a.src_rows = hsrc; a.tgt_rows = h; a.num_nodes = num_nodes; a.K = H; a.num_types = num_types;
-        a.use_target = ut; a.reduce = reduce; a.block_targets = bp->block_targets; a.group_off = bp->group_off; a.src_f = bp->src_f;
-        a.tl_f = bp->tl_f; a.row_ptr = row_ptr; a.packed_weights = wb;
-        a.epi = fused::Epilogue{message_activation, ln_weight, ln_bias, ln_eps};
-        a.out = y; a.out_mode = 1; a.status = bp->status;
-        rc = fused::aggregate(a, st);
-        if (rc || !dense_weight) return rc;
-    } else {
     // 1. messages  m_e = W_t [h_src ; h_tgt]
     if (E > 0) {
         MsgPolicyB::Params mp{};
@@ -794,16 +738,9 @@ static int mlp_forward_bf16_impl(const uint16_t *node_states, const uint16_t *ga
     const ReduceEpilogueB epi{message_activation, ln_weight, ln_bias, ln_eps};
     rc = reduce_bf16(reduce, msg, row_ptr, num_nodes, D, y, &epi, st);
     if (rc || !dense_weight) return rc;
-    }
 
     // 3. dense update
-    DensePolicyB::Params dp{};
-    rc = make_map_bf16(&dp.map_y, y, num_nodes, D, 128);
-    if (!rc) rc = make_map_bf16(&dp.map_w, wd, out_dim, D, out_dim < 128 ? out_dim : 128);
-    if (rc) return rc;
-    dp.bias = dense_bias; dp.out = out; dp.num_nodes = (int)num_nodes; dp.D = D; dp.Hout = out_dim; dp.act = dense_activation;
-    dp.n_blocks = (out_dim + 127) / 128; dp.dbg = debug_bits(); dp.trace = tc::trace_buffer(PTGNN_KERNEL_DENSE + 10);
-    return launch_pipeline<DensePolicyB>(dp, (int)ceil_div(num_nodes, TILE_M) * dp.n_blocks, PTGNN_KERNEL_DENSE, st);
+    return dense_update(y, num_nodes, D, dense_weight, dense_bias, out_dim, dense_activation, out, ws + L.wd, st);
 }
 
 extern "C" int ptgnn_b200_mlp_forward_bf16(const uint16_t *node_states, const uint16_t *gather_states, int64_t num_nodes,
@@ -816,37 +753,5 @@ extern "C" int ptgnn_b200_mlp_forward_bf16(const uint16_t *node_states, const ui
                                            uint16_t *out_states, void *workspace, size_t workspace_bytes, void *stream) {
     return mlp_forward_bf16_impl(node_states, gather_states, num_nodes, in_dim, message_dim, out_dim, num_types, type_off, row_ptr,
                                  pos, src32, tgt32, edge_weights, use_target_state, reduce, message_activation, ln_weight, ln_bias,
-                                 ln_eps, dense_weight, dense_bias, dense_activation, out_states, workspace, workspace_bytes, stream,
-                                 nullptr);
+                                 ln_eps, dense_weight, dense_bias, dense_activation, out_states, workspace, workspace_bytes, stream);
 }
-
-// ---- fused variants (called from the dtype-dispatching entry points in layers.cu) ---------------------------------------------
-namespace ptgnn {
-namespace tcb {
-size_t gated_fused_workspace_bytes_bf16(int64_t N, int T, int H, int D) { return ws_layout(N, 0, T, H, D).total; }
-size_t gated_fused_cache_bytes_bf16(int T, int H, int D) { return gated_cache_bytes_bf16(T, H, D); }
-int gated_forward_fused_bf16(const uint16_t *node_states, const uint16_t *gather_states, int64_t num_nodes, int32_t state_dim,
-                             int32_t message_dim, int32_t num_types, const ptgnn_b200_block_plan *bp, const int32_t *row_ptr,
-                             const float *const *edge_weights, const float *gru_w_ih, const float *gru_w_hh, const float *gru_b_ih,
-                             const float *gru_b_hh, int32_t reduce, uint16_t *out_states, void *workspace, size_t workspace_bytes,
-                             void *weight_cache, size_t weight_cache_bytes, int32_t cache_valid, void *stream) {
-    return gated_forward_bf16_impl(node_states, gather_states, num_nodes, state_dim, message_dim, num_types, nullptr, row_ptr,
-                                   nullptr, nullptr, edge_weights, gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, reduce, out_states,
-                                   workspace, workspace_bytes, weight_cache, weight_cache_bytes, cache_valid, stream, bp);
-}
-size_t mlp_fused_workspace_bytes_bf16(int64_t N, int T, int H, int D, int Hout, int use_target) {
-    return mlp_ws_layout(N, 0, T, H, D, Hout > 0 ? Hout : D, use_target).total;
-}
-int mlp_forward_fused_bf16(const uint16_t *node_states, const uint16_t *gather_states, int64_t num_nodes, int32_t in_dim,
-                           int32_t message_dim, int32_t out_dim, int32_t num_types, const ptgnn_b200_block_plan *bp,
-                           const int32_t *row_ptr, const float *const *edge_weights, int32_t use_target_state, int32_t reduce,
-                           int32_t message_activation, const float *ln_weight, const float *ln_bias, float ln_eps,
-                           const float *dense_weight, const float *dense_bias, int32_t dense_activation, uint16_t *out_states,
-                           void *workspace, size_t workspace_bytes, void *stream) {
-    return mlp_forward_bf16_impl(node_states, gather_states, num_nodes, in_dim, message_dim, out_dim, num_types, nullptr, row_ptr,
-                                 nullptr, nullptr, nullptr, edge_weights, use_target_state, reduce, message_activation, ln_weight,
-                                 ln_bias, ln_eps, dense_weight, dense_bias, dense_activation, out_states, workspace, workspace_bytes,
-                                 stream, bp);
-}
-}  // namespace tcb
-}  // namespace ptgnn

@@ -1,0 +1,294 @@
+// GatedMessagePassingLayer / MlpMessagePassingLayer forward through the fused aggregation (fused_mp.cuh): one host path per
+// layer class for both state dtypes.  nprod = 3: fp32 states, computed fp32-exactly as three fp16 products on packed
+// (hi | lo') rows; nprod = 1: bf16 states.
+//
+//   gated:  pack edge weights* -> pack states (fp32) -> fused aggregation -> pack GRU weights* -> weights-stationary GRU (gru_ws.cuh)
+//   Mlp:    pack edge weights* -> pack states (fp32) -> fused aggregation + activation / LayerNorm -> dense update
+//
+// * skipped when the caller's weight cache is valid.  The packing pass of the states is skipped when the caller hands in their
+// packed form (a stack of gated layers: the previous layer's GRU wrote it).
+#include "fused_mp.cuh"
+#include "gru_ws.cuh"
+#include "layers.cuh"
+#include "layers_tc.cuh"
+
+namespace ptgnn {
+namespace {
+
+// the dims the fused aggregation takes; PTGNN_B200_DISABLE_TC=1 keeps fp32 states on the FFMA kernels
+bool aggregate_ok(int nprod, int H, int D, int ut) { return (nprod == 1 || tc_enabled()) && fused::supported(nprod, H, D, ut); }
+// the gated layer also needs the weights-stationary GRU: no other GRU runs behind the fused aggregation
+bool gated_ok(int nprod, int H, int D) { return aggregate_ok(nprod, H, D, 0) && gruws::supported(nprod, H, D); }
+
+// [N, D] aggregate: packed fp16 pairs (the GRU's operand) or fp32 rows for fp32 states, bf16 rows for bf16 states
+size_t agg_bytes(int nprod, int64_t N, int D) { return ws_slice((size_t)N * D * (nprod == 3 ? 4 : 2) + 16, 1); }
+
+// derived weights (the caller's weight cache, or the workspace's tail without one): [packed edge weights | gru_ws packing]
+size_t gated_weight_bytes(int nprod, int T, int H, int D) {
+    return fused::packed_weight_bytes(nprod, T, H, 0) + gruws::pack_bytes(nprod, H, D);
+}
+// [packed edge weights | dense weight: TF32 hi / lo split (fp32) or bf16 copy]
+size_t mlp_weight_bytes(int nprod, int T, int H, int D, int Hout, int ut) {
+    const size_t dense = nprod == 3 ? tc::dense_split_bytes(Hout, D) : tcb::dense_weight_bytes(Hout, D);
+    return fused::packed_weight_bytes(nprod, T, H, ut) + dense + 256;
+}
+
+// workspace: agg | packed states (gathered rows) | packed own rows (sharded run: the GRU's h) | derived weights (no cache)
+struct GatedWs { size_t agg, xpack, xpack_own, weights, total; };
+GatedWs gated_layout(int nprod, int64_t N, int64_t Ns, int T, int H, int D) {
+    GatedWs w{};
+    w.xpack = agg_bytes(nprod, N, D);
+    w.xpack_own = w.xpack + fused::packed_state_bytes(nprod, Ns, H);
+    w.weights = w.xpack_own + fused::packed_state_bytes(nprod, N, H);
+    w.total = w.weights + gated_weight_bytes(nprod, T, H, D);
+    return w;
+}
+
+// workspace: y (pre-dense aggregate) | packed states (gathered rows) | packed target rows (sharded run) | derived weights
+struct MlpWs { size_t y, xpack, xpack_tgt, weights, total; };
+MlpWs mlp_layout(int nprod, int64_t N, int64_t Ns, int T, int H, int D, int Hout, int ut) {
+    MlpWs w{};
+    w.xpack = agg_bytes(nprod, N, D);
+    w.xpack_tgt = w.xpack + fused::packed_state_bytes(nprod, Ns, H);
+    w.weights = w.xpack_tgt + (ut ? fused::packed_state_bytes(nprod, N, H) : 0);
+    w.total = w.weights + mlp_weight_bytes(nprod, T, H, D, Hout, ut);
+    return w;
+}
+
+// the weight cache if one is given (derive into it unless cache_valid), else the workspace's area (derive every call)
+int weight_area(const char *who, char *ws_area, void *weight_cache, size_t weight_cache_bytes, size_t need, int cache_valid,
+                char *&area, bool &pack) {
+    area = ws_area;
+    pack = true;
+    if (weight_cache == nullptr) return PTGNN_OK;
+    if (weight_cache_bytes < need) {
+        set_error("%s: weight cache %zu < required %zu", who, weight_cache_bytes, need);
+        return PTGNN_E_WORKSPACE;
+    }
+    area = static_cast<char *>(weight_cache);
+    pack = !cache_valid;
+    return PTGNN_OK;
+}
+
+fused::AggregateArgs aggregate_args(int nprod, const ptgnn_b200_block_plan *bp, const int32_t *row_ptr, int64_t N, int H, int T, int reduce,
+                                    const void *packed_weights) {
+    fused::AggregateArgs a{};
+    a.nprod = nprod; a.num_nodes = N; a.K = H; a.num_types = T; a.reduce = reduce;
+    a.block_targets = bp->block_targets; a.group_off = bp->group_off; a.src_f = bp->src_f; a.tl_f = bp->tl_f; a.status = bp->status;
+    a.row_ptr = row_ptr; a.packed_weights = packed_weights;
+    a.epi = fused::Epilogue{PTGNN_ACT_NONE, nullptr, nullptr, 0.0f};
+    return a;
+}
+
+int gated_fused(int nprod, const void *node_states, const void *gather_states, const void *packed_in, int64_t N, int64_t Ns, int H,
+                int D, int T, const ptgnn_b200_block_plan *bp, const int32_t *row_ptr, const float *const *edge_weights,
+                const float *w_ih, const float *w_hh, const float *b_ih, const float *b_hh, int reduce, void *out_states,
+                void *packed_out, void *workspace, size_t workspace_bytes, void *weight_cache, size_t weight_cache_bytes,
+                int cache_valid, cudaStream_t st) {
+    PTGNN_CHECK_ARG(bp != nullptr, "gated_forward_fused: null block plan");
+    PTGNN_CHECK_ARG(T >= 0 && T <= PTGNN_MAX_EDGE_TYPES, "gated_forward_fused: bad num_types=%d", T);
+    if (!gated_ok(nprod, H, D)) {
+        set_error("gated_forward_fused: dims H=%d D=%d are not supported by the fused kernels (%s states)", H, D, nprod == 3 ? "fp32" : "bf16");
+        return PTGNN_E_UNSUPPORTED;
+    }
+    PTGNN_CHECK_ARG(nprod == 3 || (packed_in == nullptr && packed_out == nullptr), "gated_forward_fused: packed states are fp32-only");
+    PTGNN_CHECK_ARG(N >= 0 && N < INT32_MAX, "gated_forward_fused: sizes out of range");
+    PTGNN_CHECK_ARG(reduce >= PTGNN_REDUCE_SUM && reduce <= PTGNN_REDUCE_MIN, "gated_forward_fused: bad reduce %d", reduce);
+    if (N == 0) return PTGNN_OK;
+    PTGNN_CHECK_ARG(node_states && out_states && row_ptr && w_ih && w_hh && b_ih && b_hh, "gated_forward_fused: null pointer");
+    PTGNN_CHECK_ARG(bp->group_off && edge_weights && T > 0, "gated_forward_fused: null block plan arrays");
+    if (Ns <= 0) Ns = N;
+    const GatedWs L = gated_layout(nprod, N, Ns, T, H, D);
+    if (workspace_bytes < L.total || !workspace) {
+        set_error("gated_forward_fused: workspace %zu < required %zu", workspace_bytes, L.total);
+        return PTGNN_E_WORKSPACE;
+    }
+    char *ws = static_cast<char *>(workspace);
+    char *wpack;
+    bool pack;
+    int rc = weight_area("gated_forward_fused", ws + L.weights, weight_cache, weight_cache_bytes, gated_weight_bytes(nprod, T, H, D),
+                         cache_valid, wpack, pack);
+    if (rc) return rc;
+    char *grupack = wpack + fused::packed_weight_bytes(nprod, T, H, 0);
+    if (pack) {
+        rc = fused::pack_weights(nprod, T, H, 0, edge_weights, wpack, bp->status, st);
+        if (rc) return rc;
+    }
+
+    // the aggregation gathers src_rows (sources, global ids in a sharded run); the GRU reads h_rows (this rank's rows).  fp32:
+    // both as packed fp16 rows.  packed_in is node_states' packed form (written by the previous layer's GRU); in a sharded run the
+    // gathered rows are a different tensor and are packed here.
+    const void *gsrc = gather_states ? gather_states : node_states;
+    const void *src_rows = gsrc, *h_rows = node_states;
+    if (nprod == 3) {
+        const bool sharded = gather_states != nullptr && gather_states != node_states;
+        src_rows = h_rows = packed_in;
+        if (sharded || packed_in == nullptr) {
+            rc = fused::pack_states(static_cast<const float *>(gsrc), Ns, H, ws + L.xpack, bp->status, st);
+            if (rc) return rc;
+            src_rows = ws + L.xpack;
+            if (!sharded) h_rows = src_rows;
+        }
+        if (h_rows == nullptr) {
+            rc = fused::pack_states(static_cast<const float *>(node_states), N, H, ws + L.xpack_own, bp->status, st);
+            if (rc) return rc;
+            h_rows = ws + L.xpack_own;
+        }
+    }
+
+    // 1+2. gather -> W_t -> segmented reduce in one kernel (no message buffer)
+    fused::AggregateArgs a = aggregate_args(nprod, bp, row_ptr, N, H, T, reduce, wpack);
+    a.src_rows = src_rows; a.use_target = 0; a.tgt_rows = nullptr;
+    a.out = ws + L.agg; a.out_mode = nprod == 3 ? 2 : 1;
+    rc = fused::aggregate(a, st);
+    if (rc) return rc;
+    // 3. GRUCell, weights-stationary (the gate weights stay in shared memory, only node rows stream)
+    if (pack) {
+        rc = gruws::pack(nprod, H, D, w_ih, w_hh, b_ih, b_hh, grupack, st);
+        if (rc) return rc;
+    }
+    return gruws::update(nprod, ws + L.agg, h_rows, node_states, N, H, D, grupack, out_states, packed_out, bp->status, st);
+}
+
+int mlp_fused(int nprod, const void *node_states, const void *gather_states, int64_t N, int64_t Ns, int H, int D, int Hout, int T,
+              const ptgnn_b200_block_plan *bp, const int32_t *row_ptr, const float *const *edge_weights, int ut, int reduce,
+              int message_activation, const float *ln_weight, const float *ln_bias, float ln_eps, const float *dense_weight,
+              const float *dense_bias, int dense_activation, void *out_states, void *workspace, size_t workspace_bytes,
+              void *weight_cache, size_t weight_cache_bytes, int cache_valid, cudaStream_t st) {
+    PTGNN_CHECK_ARG(bp != nullptr, "mlp_forward_fused: null block plan");
+    PTGNN_CHECK_ARG(T >= 0 && T <= PTGNN_MAX_EDGE_TYPES, "mlp_forward_fused: bad num_types=%d", T);
+    if (!aggregate_ok(nprod, H, D, ut)) {
+        set_error("mlp_forward_fused: dims H=%d D=%d are not supported by the fused kernel (%s states)", H, D, nprod == 3 ? "fp32" : "bf16");
+        return PTGNN_E_UNSUPPORTED;
+    }
+    PTGNN_CHECK_ARG(N >= 0 && N < INT32_MAX, "mlp_forward_fused: sizes out of range");
+    PTGNN_CHECK_ARG(dense_weight ? Hout > 0 : Hout == D, "mlp_forward_fused: out_dim=%d inconsistent", Hout);
+    if (nprod == 1 && dense_weight && (Hout % 16 != 0 || Hout < 64)) {
+        set_error("mlp_forward_fused: bf16 states need output dim %% 16 == 0 (>= 64); got %d", Hout);
+        return PTGNN_E_UNSUPPORTED;
+    }
+    PTGNN_CHECK_ARG(reduce >= PTGNN_REDUCE_SUM && reduce <= PTGNN_REDUCE_MIN, "mlp_forward_fused: bad reduce %d", reduce);
+    PTGNN_CHECK_ARG(message_activation >= PTGNN_ACT_NONE && message_activation <= PTGNN_ACT_RELU &&
+                        dense_activation >= PTGNN_ACT_NONE && dense_activation <= PTGNN_ACT_RELU,
+                    "mlp_forward_fused: bad activation");
+    PTGNN_CHECK_ARG((ln_weight == nullptr) == (ln_bias == nullptr), "mlp_forward_fused: ln_weight/ln_bias must both be set");
+    if (N == 0) return PTGNN_OK;
+    PTGNN_CHECK_ARG(node_states && out_states && row_ptr, "mlp_forward_fused: null pointer");
+    PTGNN_CHECK_ARG(bp->group_off && edge_weights && T > 0, "mlp_forward_fused: null block plan arrays");
+    if (Ns <= 0) Ns = N;
+    const MlpWs L = mlp_layout(nprod, N, Ns, T, H, D, Hout, ut);
+    if (workspace_bytes < L.total || !workspace) {
+        set_error("mlp_forward_fused: workspace %zu < required %zu", workspace_bytes, L.total);
+        return PTGNN_E_WORKSPACE;
+    }
+    char *ws = static_cast<char *>(workspace);
+    char *wpack;
+    bool pack;
+    // bf16 states: the dense weight is converted every call, so there is nothing to cache
+    int rc = weight_area("mlp_forward_fused", ws + L.weights, nprod == 3 ? weight_cache : nullptr, weight_cache_bytes,
+                         mlp_weight_bytes(nprod, T, H, D, Hout, ut), cache_valid, wpack, pack);
+    if (rc) return rc;
+    char *dense_area = wpack + fused::packed_weight_bytes(nprod, T, H, ut);
+    if (pack) {
+        rc = fused::pack_weights(nprod, T, H, ut, edge_weights, wpack, bp->status, st);
+        if (rc) return rc;
+    }
+
+    const void *gsrc = gather_states ? gather_states : node_states;
+    const void *src_rows = gsrc, *tgt_rows = node_states;
+    if (nprod == 3) {
+        rc = fused::pack_states(static_cast<const float *>(gsrc), Ns, H, ws + L.xpack, bp->status, st);
+        if (rc) return rc;
+        src_rows = tgt_rows = ws + L.xpack;
+        if (ut && gather_states != nullptr) {      // sharded run: targets are this rank's rows, not the gathered ones
+            rc = fused::pack_states(static_cast<const float *>(node_states), N, H, ws + L.xpack_tgt, bp->status, st);
+            if (rc) return rc;
+            tgt_rows = ws + L.xpack_tgt;
+        }
+    }
+
+    // 1+2. gather -> W_t -> segmented reduce (+ activation + LayerNorm at write-out) in one kernel
+    void *y = dense_weight ? ws + L.y : out_states;
+    fused::AggregateArgs a = aggregate_args(nprod, bp, row_ptr, N, H, T, reduce, wpack);
+    a.src_rows = src_rows; a.use_target = ut; a.tgt_rows = tgt_rows;
+    a.epi = fused::Epilogue{message_activation, ln_weight, ln_bias, ln_eps};
+    a.out = y; a.out_mode = nprod == 3 ? 0 : 1;
+    rc = fused::aggregate(a, st);
+    if (rc || !dense_weight) return rc;
+    // 3. dense update
+    if (nprod == 3)
+        return dense_any(static_cast<const float *>(y), N, D, dense_weight, dense_bias, Hout, dense_activation,
+                         static_cast<float *>(out_states), dense_area, st, pack);
+    return tcb::dense_update(static_cast<const __nv_bfloat16 *>(y), N, D, dense_weight, dense_bias, Hout, dense_activation,
+                             static_cast<__nv_bfloat16 *>(out_states), dense_area, st);
+}
+
+}  // namespace
+}  // namespace ptgnn
+
+using namespace ptgnn;
+
+extern "C" int32_t ptgnn_b200_block_plan_block_targets(int64_t num_nodes) { return fused::recommended_block_targets(num_nodes); }
+
+extern "C" int32_t ptgnn_b200_fused_supported(int32_t bf16_states, int32_t state_dim, int32_t message_dim) {
+    return tc_enabled() && gated_ok(bf16_states ? 1 : 3, state_dim, message_dim) ? 1 : 0;
+}
+
+extern "C" size_t ptgnn_b200_packed_state_bytes(int64_t num_nodes, int32_t state_dim) {
+    if (num_nodes < 0 || state_dim <= 0) return 0;
+    return fused::packed_state_bytes(3, num_nodes, state_dim);
+}
+
+extern "C" size_t ptgnn_b200_gated_fused_workspace_bytes(int32_t bf16_states, int64_t num_nodes, int64_t num_source_nodes,
+                                                         int32_t num_types, int32_t state_dim, int32_t message_dim) {
+    if (num_nodes < 0 || num_types < 0 || state_dim <= 0 || message_dim <= 0) return 0;
+    if (num_source_nodes <= 0) num_source_nodes = num_nodes;
+    return gated_layout(bf16_states ? 1 : 3, num_nodes, num_source_nodes, num_types, state_dim, message_dim).total;
+}
+extern "C" size_t ptgnn_b200_gated_fused_weight_cache_bytes(int32_t bf16_states, int32_t num_types, int32_t state_dim,
+                                                            int32_t message_dim) {
+    if (num_types < 0 || num_types > PTGNN_MAX_EDGE_TYPES || state_dim <= 0 || message_dim <= 0) return 0;
+    return gated_weight_bytes(bf16_states ? 1 : 3, num_types, state_dim, message_dim);
+}
+extern "C" int ptgnn_b200_gated_forward_fused(int32_t bf16_states, const void *node_states, const void *gather_states,
+                                              const void *packed_states_in, int64_t num_nodes, int64_t num_source_nodes,
+                                              int32_t state_dim, int32_t message_dim, int32_t num_types,
+                                              const ptgnn_b200_block_plan *block_plan, const int32_t *row_ptr,
+                                              const float *const *edge_weights, const float *gru_w_ih, const float *gru_w_hh,
+                                              const float *gru_b_ih, const float *gru_b_hh, int32_t reduce, void *out_states,
+                                              void *packed_states_out, void *workspace, size_t workspace_bytes, void *weight_cache,
+                                              size_t weight_cache_bytes, int32_t cache_valid, void *stream) {
+    return gated_fused(bf16_states ? 1 : 3, node_states, gather_states, packed_states_in, num_nodes, num_source_nodes, state_dim,
+                       message_dim, num_types, block_plan, row_ptr, edge_weights, gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, reduce,
+                       out_states, packed_states_out, workspace, workspace_bytes, weight_cache, weight_cache_bytes, cache_valid,
+                       static_cast<cudaStream_t>(stream));
+}
+
+extern "C" size_t ptgnn_b200_mlp_fused_workspace_bytes(int32_t bf16_states, int64_t num_nodes, int64_t num_source_nodes,
+                                                       int32_t num_types, int32_t in_dim, int32_t message_dim, int32_t out_dim,
+                                                       int32_t use_target_state) {
+    if (num_nodes < 0 || num_types < 0 || in_dim <= 0 || message_dim <= 0) return 0;
+    if (num_source_nodes <= 0) num_source_nodes = num_nodes;
+    return mlp_layout(bf16_states ? 1 : 3, num_nodes, num_source_nodes, num_types, in_dim, message_dim, out_dim > 0 ? out_dim : message_dim,
+                      use_target_state ? 1 : 0).total;
+}
+extern "C" size_t ptgnn_b200_mlp_fused_weight_cache_bytes(int32_t bf16_states, int32_t num_types, int32_t in_dim, int32_t message_dim,
+                                                          int32_t out_dim, int32_t use_target_state) {
+    if (bf16_states || num_types <= 0 || in_dim <= 0 || message_dim <= 0) return 0;
+    const int ut = use_target_state ? 1 : 0;
+    if (!aggregate_ok(3, in_dim, message_dim, ut)) return 0;
+    return mlp_weight_bytes(3, num_types, in_dim, message_dim, out_dim > 0 ? out_dim : message_dim, ut);
+}
+extern "C" int ptgnn_b200_mlp_forward_fused(int32_t bf16_states, const void *node_states, const void *gather_states, int64_t num_nodes,
+                                            int64_t num_source_nodes, int32_t in_dim, int32_t message_dim, int32_t out_dim,
+                                            int32_t num_types, const ptgnn_b200_block_plan *block_plan, const int32_t *row_ptr,
+                                            const float *const *edge_weights, int32_t use_target_state, int32_t reduce,
+                                            int32_t message_activation, const float *ln_weight, const float *ln_bias, float ln_eps,
+                                            const float *dense_weight, const float *dense_bias, int32_t dense_activation,
+                                            void *out_states, void *workspace, size_t workspace_bytes, void *weight_cache,
+                                            size_t weight_cache_bytes, int32_t cache_valid, void *stream) {
+    return mlp_fused(bf16_states ? 1 : 3, node_states, gather_states, num_nodes, num_source_nodes, in_dim, message_dim, out_dim,
+                     num_types, block_plan, row_ptr, edge_weights, use_target_state ? 1 : 0, reduce, message_activation, ln_weight,
+                     ln_bias, ln_eps, dense_weight, dense_bias, dense_activation, out_states, workspace, workspace_bytes, weight_cache,
+                     weight_cache_bytes, cache_valid, static_cast<cudaStream_t>(stream));
+}

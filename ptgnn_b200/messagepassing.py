@@ -51,15 +51,11 @@ def _refuse_autograd(module: nn.Module, node_states: torch.Tensor) -> None:
         )
 
 
-def _fused_enabled() -> bool:
+def _use_fused(lib, bf16: bool, H: int, D: int) -> bool:
     """The fused gather -> Linear -> reduce kernel is the default wherever it supports the dimensions.  PTGNN_B200_FUSED=0
     selects the round-1 three-kernel path; PTGNN_B200_FP32_MODE=tf32 does so for fp32 states only (3xTF32 instead of 3xFP16:
     needed for states / weights beyond the fp16 range)."""
-    return os.environ.get("PTGNN_B200_FUSED", "1") != "0"
-
-
-def _use_fused(lib, bf16: bool, H: int, D: int) -> bool:
-    if not _fused_enabled() or (not bf16 and os.environ.get("PTGNN_B200_FP32_MODE", "") == "tf32"):
+    if os.environ.get("PTGNN_B200_FUSED", "1") == "0" or (not bf16 and os.environ.get("PTGNN_B200_FP32_MODE", "") == "tf32"):
         return False
     return bool(lib.ptgnn_b200_fused_supported(int(bf16), H, D))
 
@@ -300,51 +296,34 @@ class GatedMessagePassingLayer(AbstractMessagePassingLayer):
             if chain is not None and chain.want_output:
                 packed_out = torch.empty(max(lib.ptgnn_b200_packed_state_bytes(num_nodes, H), 1), dtype=torch.uint8, device=h.device)
             with torch.cuda.device(h.device):
-                if packed_in is not None or packed_out is not None:
-                    rc = lib.ptgnn_b200_gated_forward_fused_chained(
-                        N.ptr(h), N.ptr(gsrc), N.ptr(packed_in), num_nodes, ns, H, D, plan.num_types, ctypes.byref(bp), N.ptr(plan.row_ptr),
-                        N.ptr_table(weights), N.ptr(w_ih), N.ptr(w_hh), N.ptr(b_ih), N.ptr(b_hh), reduce, N.ptr(out), N.ptr(packed_out),
-                        N.ptr(ws), ws_bytes, N.ptr(cache), 0 if cache is None else cache.numel(), int(valid), N.current_stream(h.device),
-                    )
-                else:
-                    rc = lib.ptgnn_b200_gated_forward_fused(
-                        int(bf16), N.ptr(h), N.ptr(gsrc), num_nodes, ns, H, D, plan.num_types, ctypes.byref(bp), N.ptr(plan.row_ptr),
-                        N.ptr_table(weights), N.ptr(w_ih), N.ptr(w_hh), N.ptr(b_ih), N.ptr(b_hh), reduce, N.ptr(out), N.ptr(ws), ws_bytes,
-                        N.ptr(cache), 0 if cache is None else cache.numel(), int(valid), N.current_stream(h.device),
-                    )
+                rc = lib.ptgnn_b200_gated_forward_fused(
+                    int(bf16), N.ptr(h), N.ptr(gsrc), N.ptr(packed_in), num_nodes, ns, H, D, plan.num_types, ctypes.byref(bp),
+                    N.ptr(plan.row_ptr), N.ptr_table(weights), N.ptr(w_ih), N.ptr(w_hh), N.ptr(b_ih), N.ptr(b_hh), reduce, N.ptr(out),
+                    N.ptr(packed_out), N.ptr(ws), ws_bytes, N.ptr(cache), 0 if cache is None else cache.numel(), int(valid),
+                    N.current_stream(h.device),
+                )
             N.check(rc, "ptgnn_b200_gated_forward_fused")
             self._weight_cache_filled(kind, h.device)
             if chain is not None:
                 chain.store(out, packed_out)
             return out
-        if state_dtype == torch.bfloat16:   # bf16 states, fp32 parameters (converted inside the library), fp32 accumulation
-            cache, valid = self._weight_cache("bf16", lib.ptgnn_b200_gated_weight_cache_bytes_bf16(plan.num_types, H, D), params, h.device)
-            ws_bytes = lib.ptgnn_b200_gated_workspace_bytes_bf16(num_nodes, plan.num_edges, plan.num_types, H, D)
-            ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=h.device)
-            out = torch.empty_like(h)
-            with torch.cuda.device(h.device):
-                rc = lib.ptgnn_b200_gated_forward_cached_bf16(
-                    N.ptr(h), N.ptr(gsrc), num_nodes, H, D, plan.num_types, plan.type_off_c, N.ptr(plan.row_ptr), N.ptr(plan.pos),
-                    N.ptr(plan.src32), N.ptr_table(weights), N.ptr(w_ih), N.ptr(w_hh), N.ptr(b_ih), N.ptr(b_hh), reduce,
-                    N.ptr(out), N.ptr(ws), ws_bytes, N.ptr(cache), 0 if cache is None else cache.numel(), int(valid),
-                    N.current_stream(h.device),
-                )
-            N.check(rc, "ptgnn_b200_gated_forward_cached_bf16")
-            self._weight_cache_filled("bf16", h.device)
-            return out
-        cache, valid = self._weight_cache("f32", lib.ptgnn_b200_gated_weight_cache_bytes(plan.num_types, H, D), params, h.device)
-        ws_bytes = lib.ptgnn_b200_gated_workspace_bytes(num_nodes, plan.num_edges, plan.num_types, H, D)
+        # round-1 three-kernel path; bf16 states: fp32 parameters (converted inside the library), fp32 accumulation
+        kind, sfx = ("bf16", "_bf16") if bf16 else ("f32", "")
+        fwd = "ptgnn_b200_gated_forward_cached_" + kind
+        cache_bytes = getattr(lib, "ptgnn_b200_gated_weight_cache_bytes" + sfx)(plan.num_types, H, D)
+        cache, valid = self._weight_cache(kind, cache_bytes, params, h.device)
+        ws_bytes = getattr(lib, "ptgnn_b200_gated_workspace_bytes" + sfx)(num_nodes, plan.num_edges, plan.num_types, H, D)
         ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=h.device)
         out = torch.empty_like(h)
         with torch.cuda.device(h.device):
-            rc = lib.ptgnn_b200_gated_forward_cached_f32(
+            rc = getattr(lib, fwd)(
                 N.ptr(h), N.ptr(gsrc), num_nodes, H, D, plan.num_types, plan.type_off_c, N.ptr(plan.row_ptr), N.ptr(plan.pos),
                 N.ptr(plan.src32), N.ptr_table(weights), N.ptr(w_ih), N.ptr(w_hh), N.ptr(b_ih), N.ptr(b_hh), reduce,
                 N.ptr(out), N.ptr(ws), ws_bytes, N.ptr(cache), 0 if cache is None else cache.numel(), int(valid),
                 N.current_stream(h.device),
             )
-        N.check(rc, "ptgnn_b200_gated_forward_cached_f32")
-        self._weight_cache_filled("f32", h.device)
+        N.check(rc, fwd)
+        self._weight_cache_filled(kind, h.device)
         return out
 
     def _forward_with_edge_features(self, node_states, adjacency_lists, edge_features, gather_states, reduce: int) -> torch.Tensor:
@@ -576,41 +555,29 @@ class MlpMessagePassingLayer(AbstractMessagePassingLayer):
             cache, valid = self._weight_cache("mlp_f32_fused", 0 if bf16 else lib.ptgnn_b200_mlp_fused_weight_cache_bytes(
                 0, plan.num_types, H, D, out_dim, ut_i), cache_params, h.device)
             with torch.cuda.device(h.device):
-                rc = lib.ptgnn_b200_mlp_forward_fused_cached(
+                rc = lib.ptgnn_b200_mlp_forward_fused(
                     int(bf16), N.ptr(h), N.ptr(gsrc), num_nodes, ns, H, D, out_dim, plan.num_types, ctypes.byref(bp), N.ptr(plan.row_ptr),
                     N.ptr_table(weights), ut_i, reduce, msg_act, N.ptr(ln_w), N.ptr(ln_b), float(ln.eps) if ln is not None else 0.0,
                     N.ptr(d_w), N.ptr(d_b), dense_act, N.ptr(out), N.ptr(ws), ws_bytes, N.ptr(cache), 0 if cache is None else cache.numel(),
                     int(valid), N.current_stream(h.device),
                 )
-            N.check(rc, "ptgnn_b200_mlp_forward_fused_cached")
+            N.check(rc, "ptgnn_b200_mlp_forward_fused")
             self._weight_cache_filled("mlp_f32_fused", h.device)
             return apply_dropout(out)
-        if state_dtype == torch.bfloat16:   # bf16 states, fp32 parameters (converted inside the library), fp32 accumulation
-            ut = int(self.__use_target_state_as_message_input)
-            ws_bytes = lib.ptgnn_b200_mlp_workspace_bytes_bf16(num_nodes, plan.num_edges, plan.num_types, H, D, out_dim, ut)
-            ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=h.device)
-            out = torch.empty(num_nodes, out_dim, dtype=torch.bfloat16, device=h.device)
-            with torch.cuda.device(h.device):
-                rc = lib.ptgnn_b200_mlp_forward_bf16(
-                    N.ptr(h), N.ptr(gsrc), num_nodes, H, D, out_dim, plan.num_types, plan.type_off_c, N.ptr(plan.row_ptr), N.ptr(plan.pos),
-                    N.ptr(plan.src32), N.ptr(plan.tgt32), N.ptr_table(weights), ut, reduce, msg_act, N.ptr(ln_w), N.ptr(ln_b),
-                    float(ln.eps) if ln is not None else 0.0, N.ptr(d_w), N.ptr(d_b), dense_act, N.ptr(out), N.ptr(ws), ws_bytes,
-                    N.current_stream(h.device),
-                )
-            N.check(rc, "ptgnn_b200_mlp_forward_bf16")
-            return apply_dropout(out)
-        ws_bytes = lib.ptgnn_b200_mlp_workspace_bytes(
-            num_nodes, plan.num_edges, plan.num_types, H, D, out_dim, int(self.__use_target_state_as_message_input))
+        # round-1 three-kernel path; bf16 states: fp32 parameters (converted inside the library), fp32 accumulation
+        fwd = "ptgnn_b200_mlp_forward_" + ("bf16" if bf16 else "f32")
+        ws_bytes = getattr(lib, "ptgnn_b200_mlp_workspace_bytes" + ("_bf16" if bf16 else ""))(
+            num_nodes, plan.num_edges, plan.num_types, H, D, out_dim, ut_i)
         ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=h.device)
-        out = torch.empty(num_nodes, out_dim, dtype=torch.float32, device=h.device)
+        out = torch.empty(num_nodes, out_dim, dtype=state_dtype, device=h.device)
         with torch.cuda.device(h.device):
-            rc = lib.ptgnn_b200_mlp_forward_f32(
+            rc = getattr(lib, fwd)(
                 N.ptr(h), N.ptr(gsrc), num_nodes, H, D, out_dim, plan.num_types, plan.type_off_c, N.ptr(plan.row_ptr), N.ptr(plan.pos),
-                N.ptr(plan.src32), N.ptr(plan.tgt32), N.ptr_table(weights), int(self.__use_target_state_as_message_input),
-                reduce, msg_act, N.ptr(ln_w), N.ptr(ln_b), float(ln.eps) if ln is not None else 0.0, N.ptr(d_w), N.ptr(d_b),
-                dense_act, N.ptr(out), N.ptr(ws), ws_bytes, N.current_stream(h.device),
+                N.ptr(plan.src32), N.ptr(plan.tgt32), N.ptr_table(weights), ut_i, reduce, msg_act, N.ptr(ln_w), N.ptr(ln_b),
+                float(ln.eps) if ln is not None else 0.0, N.ptr(d_w), N.ptr(d_b), dense_act, N.ptr(out), N.ptr(ws), ws_bytes,
+                N.current_stream(h.device),
             )
-        N.check(rc, "ptgnn_b200_mlp_forward_f32")
+        N.check(rc, fwd)
         return apply_dropout(out)
 
     def _forward_composed(self, node_states, adjacency_lists, edge_features, gather_states) -> torch.Tensor:

@@ -27,7 +27,27 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(handle, name), f"{name} declared in include/ptgnn_b200.h but not exported"
     assert sorted(N.SIGNATURES) == declared, "ctypes SIGNATURES must cover exactly the header's entry points"
-    assert handle.ptgnn_b200_abi_version() == 2
+    assert handle.ptgnn_b200_abi_version() == 3
+
+
+def test_fused_supported_shapes():
+    """ptgnn_b200_fused_supported is 1 exactly on the shapes both fused layer kernels take (the fused aggregation and the
+    weights-stationary GRU): D = 128 with H in {64, 128} (fp32 states) / {64, 128, 256} (bf16 states); 0 for every shape under
+    PTGNN_B200_DISABLE_TC=1 (read once per process, hence the subprocess)."""
+    import subprocess
+    import sys
+
+    handle = N.lib()
+    dims = range(32, 513, 16)
+    expected = {0: {(64, 128), (128, 128)}, 1: {(64, 128), (128, 128), (256, 128)}}
+    for bf16, shapes in expected.items():
+        got = {(H, D) for H in dims for D in dims if handle.ptgnn_b200_fused_supported(bf16, H, D) == 1}
+        assert got == shapes, f"bf16_states={bf16}: {sorted(got)}"
+    script = ("from ptgnn_b200 import _native as N; h = N.lib(); r = range(32, 513, 16); "
+              "print(sum(h.ptgnn_b200_fused_supported(b, H, D) for b in (0, 1) for H in r for D in r))")
+    env = dict(os.environ, PTGNN_B200_DISABLE_TC="1")
+    out = subprocess.run([sys.executable, "-s", "-c", script], cwd=ROOT, env=env, capture_output=True, text=True, check=True)
+    assert out.stdout.strip() == "0"
 
 
 def test_workspace_size_queries_run_without_a_gpu():
