@@ -1,4 +1,5 @@
-// C-ABI glue: error string, launch counter, and the host-buffer entry point used for end-to-end measurement.
+// C-ABI glue: error string, launch counter, the host helpers every launcher shares (SM count, TMA maps), and the
+// host-buffer entry point used for end-to-end measurement.
 #include <stdarg.h>
 
 #include <mutex>
@@ -37,6 +38,45 @@ TimedScope::~TimedScope() {
         std::lock_guard<std::mutex> lk(g_timing_mu);
         g_timing_records.push_back({cat, a, b});
     }
+}
+
+int sm_count() {
+    int dev = 0, n = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
+    return n;
+}
+
+typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
+                                  const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+static EncodeTiledFn encode_tiled_fn() {
+    static EncodeTiledFn fn = nullptr;
+    if (!fn) {
+        void *ptr = nullptr;
+        cudaDriverEntryPointQueryResult qres;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
+            fn = reinterpret_cast<EncodeTiledFn>(ptr);
+    }
+    return fn;
+}
+
+int make_tensor_map_2d(CUtensorMap *map, CUtensorMapDataType dtype, const void *base, uint64_t rows, uint64_t cols,
+                       uint64_t pitch, uint32_t box_cols, uint32_t box_rows) {
+    EncodeTiledFn fn = encode_tiled_fn();
+    if (!fn) { set_error("cuTensorMapEncodeTiled entry point not available"); return PTGNN_E_CUDA; }
+    const uint64_t elem_bytes = dtype == CU_TENSOR_MAP_DATA_TYPE_FLOAT32 ? 4 : 2;
+    const cuuint64_t dims[2] = {cols, rows};
+    const cuuint64_t strides[1] = {pitch * elem_bytes};
+    const cuuint32_t box[2] = {box_cols, box_rows};
+    const cuuint32_t estr[2] = {1, 1};
+    const CUresult r = fn(map, dtype, 2, const_cast<void *>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        set_error("cuTensorMapEncodeTiled failed with CUresult %d (data type %d, [%llu, %llu] pitch %llu, box %u x %u)", (int)r, (int)dtype,
+                  (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)pitch, box_cols, box_rows);
+        return PTGNN_E_CUDA;
+    }
+    return PTGNN_OK;
 }
 
 namespace {

@@ -1,5 +1,6 @@
 // Shared helpers for the ptgnn_b200 CUDA library (sm_90a only: H100).
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -54,6 +55,28 @@ static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
 static inline size_t ws_slice(size_t count, size_t elt) { return align_up(count * elt, 256); }
 
+// SM count of the CURRENT device, queried per launch: a process may drive several GPUs (nothing cached across devices).
+int sm_count();
+
+// TMA map of a row-major 2-D array [rows, cols] of `dtype` (fp32, fp16 or bf16) with a row pitch of `pitch` elements:
+// box {box_cols, box_rows} (box_cols x element size = 128 bytes), SWIZZLE_128B, L2 128-byte promotion, out-of-bounds
+// elements read as zero.  The encoder comes from the driver through the runtime, so the library does not link libcuda.
+int make_tensor_map_2d(CUtensorMap *map, CUtensorMapDataType dtype, const void *base, uint64_t rows, uint64_t cols,
+                       uint64_t pitch, uint32_t box_cols, uint32_t box_rows);
+
+// Per-edge-type tile table of the message kernels: edge_off[t] is type t's first edge, tile_off[t] its first tile of
+// `tile_rows` edges; entries num_types .. PTGNN_MAX_EDGE_TYPES hold the totals.  Returns the number of tiles.
+static inline int build_type_tiles(const int64_t *type_off, int num_types, int tile_rows, int32_t *edge_off, int32_t *tile_off) {
+    int tiles = 0;
+    for (int t = 0; t < num_types; ++t) {
+        edge_off[t] = (int32_t)type_off[t];
+        tile_off[t] = tiles;
+        tiles += (int)ceil_div(type_off[t + 1] - type_off[t], tile_rows);
+    }
+    for (int t = num_types; t <= PTGNN_MAX_EDGE_TYPES; ++t) { edge_off[t] = (int32_t)type_off[num_types]; tile_off[t] = tiles; }
+    return tiles;
+}
+
 // ---- per-type edge tables passed by value as a kernel parameter (< 4 KB) -------------------------
 struct EdgeTables {
     const int64_t *src[PTGNN_MAX_EDGE_TYPES];
@@ -88,21 +111,6 @@ __device__ __forceinline__ void cp_async16(uint32_t dst_smem, const void *src, i
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
-
-// ---- L2 residency control ---------------------------------------------------------------------------------------
-// Optional (PTGNN_L2_HINTS=4): read the message rows in the reduce with an evict-first L2 policy; the default is plain
-// streaming loads.
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
-    uint64_t p;
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-    return p;
-}
-__device__ __forceinline__ float4 ld_stream_f4_hint(const float4 *p, uint64_t policy) {
-    float4 r;
-    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.f32 {%0,%1,%2,%3}, [%4], %5;"
-                 : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p), "l"(policy));
-    return r;
-}
 
 __device__ __forceinline__ float4 ld_stream_f4(const float4 *p) {  // read-once data: do not allocate in L1
     float4 r;

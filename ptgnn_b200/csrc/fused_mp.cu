@@ -792,9 +792,7 @@ static int launch_one(const Params &p, cudaStream_t st) {
     const int smem = smem_bytes(p.B);
     // per launch, not once per process: the attribute belongs to the current device's context
     PTGNN_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    int dev = 0, sms = 132;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
-        sms = 132;
+    const int sms = sm_count();
     const int grid = p.num_blocks < sms ? p.num_blocks : sms;
     {
         TimedScope timed__(PTGNN_KERNEL_MESSAGE, st);

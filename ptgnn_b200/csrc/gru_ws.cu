@@ -365,33 +365,8 @@ __global__ void __launch_bounds__(256) pack_gru_ws_kernel(const float *__restric
 }
 
 // =====================================================================================================================
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
-                                  const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn encode_tiled_fn() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void *ptr = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(ptr);
-    }
-    return fn;
-}
-// 16-bit row-major [rows, cols], box {64 columns = 128 bytes, box_rows}, SWIZZLE_128B, out-of-bounds -> 0
-static int make_map16(CUtensorMap *map, const void *base, uint64_t rows, uint64_t cols, uint32_t box_rows, bool bf16) {
-    EncodeTiledFn fn = encode_tiled_fn();
-    if (!fn) { set_error("cuTensorMapEncodeTiled entry point not available"); return PTGNN_E_CUDA; }
-    const cuuint64_t dims[2] = {cols, rows};
-    const cuuint64_t strides[1] = {cols * 2};
-    const cuuint32_t box[2] = {64, box_rows};
-    const cuuint32_t estr[2] = {1, 1};
-    const CUresult r = fn(map, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void *>(base), dims,
-                          strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled (gru_ws) failed with CUresult %d", (int)r); return PTGNN_E_CUDA; }
-    return PTGNN_OK;
-}
+// every operand is 16-bit (fp16 hi / lo parts, or bf16): TMA boxes are 64 columns = 128 bytes wide
+static CUtensorMapDataType map_type(int nprod) { return nprod == 1 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16; }
 
 bool supported(int nprod, int H, int D) {
     if (H % 64 != 0 || D % 64 != 0 || H < 64 || D < 64) return false;
@@ -434,19 +409,17 @@ int update(int nprod, const void *agg_rows, const void *h_rows, const void *h_pl
     pack_layout(nprod, H, D, const_cast<char *>(static_cast<const char *>(packed)), p1, p2, bias4);
     Params p{};
     const uint64_t n_jb = H / 32;
-    const bool bf = nprod == 1;
-    int rc = make_map16(&p.map_agg, agg_rows, num_nodes, (uint64_t)npart * D, TILE_M, bf);
-    if (!rc) rc = make_map16(&p.map_h, h_rows, num_nodes, (uint64_t)npart * H, TILE_M, bf);
-    if (!rc) rc = make_map16(&p.map_p1, p1, n_jb * npart * 96, D, npart * 96, bf);
-    if (!rc) rc = make_map16(&p.map_p2, p2, n_jb * npart * 96, H, npart * 96, bf);
+    const CUtensorMapDataType dt = map_type(nprod);
+    int rc = make_tensor_map_2d(&p.map_agg, dt, agg_rows, num_nodes, (uint64_t)npart * D, (uint64_t)npart * D, 64, TILE_M);
+    if (!rc) rc = make_tensor_map_2d(&p.map_h, dt, h_rows, num_nodes, (uint64_t)npart * H, (uint64_t)npart * H, 64, TILE_M);
+    if (!rc) rc = make_tensor_map_2d(&p.map_p1, dt, p1, n_jb * npart * 96, D, D, 64, npart * 96);
+    if (!rc) rc = make_tensor_map_2d(&p.map_p2, dt, p2, n_jb * npart * 96, H, H, 64, npart * 96);
     if (rc) return rc;
     p.h32 = static_cast<const float *>(h_plain); p.h16 = static_cast<const __nv_bfloat16 *>(h_plain);
     p.bias4 = bias4; p.out = out; p.out_packed = static_cast<__half *>(out_packed); p.status = status; p.num_nodes = (int)num_nodes; p.H = H; p.D = D; p.n_jb = (int)n_jb;
     p.n_tiles = (int)ceil_div(num_nodes, TILE_M);
     p.num_slots = nprod == 3 ? Geometry<3>::num_slots(H, D) : Geometry<1>::num_slots(H, D);
-    int dev = 0, sms = 132;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
-    int groups = sms / (int)n_jb;                       // CTAs per hidden-unit block
+    int groups = sm_count() / (int)n_jb;                // CTAs per hidden-unit block
     if (groups > p.n_tiles) groups = p.n_tiles;
     if (groups < 1) groups = 1;
     const int grid = groups * (int)n_jb;
@@ -490,18 +463,16 @@ int update_table(int nprod, const void *h_rows, const void *h_plain, int64_t num
     pack_layout(nprod, H, 0, const_cast<char *>(static_cast<const char *>(packed)), p1, p2, bias4);
     Params p{};
     const uint64_t n_jb = H / 32;
-    const bool bf = nprod == 1;
-    int rc = make_map16(&p.map_h, h_rows, num_nodes, (uint64_t)npart * H, TILE_M, bf);
-    if (!rc) rc = make_map16(&p.map_p2, p2, n_jb * npart * 96, H, npart * 96, bf);
+    const CUtensorMapDataType dt = map_type(nprod);
+    int rc = make_tensor_map_2d(&p.map_h, dt, h_rows, num_nodes, (uint64_t)npart * H, (uint64_t)npart * H, 64, TILE_M);
+    if (!rc) rc = make_tensor_map_2d(&p.map_p2, dt, p2, n_jb * npart * 96, H, H, 64, npart * 96);
     if (rc) return rc;
     p.h32 = static_cast<const float *>(h_plain); p.h16 = static_cast<const __nv_bfloat16 *>(h_plain);
     p.bias4 = bias4; p.gi = gi; p.gid = gid; p.out = out; p.out_packed = static_cast<__half *>(out_packed); p.status = status;
     p.num_nodes = (int)num_nodes; p.H = H; p.D = 0; p.n_jb = (int)n_jb;
     p.n_tiles = (int)ceil_div(num_nodes, TILE_M);
     p.num_slots = nprod == 3 ? Geometry<3>::num_slots(H, 0) : Geometry<1>::num_slots(H, 0);
-    int dev = 0, sms = 132;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
-    int groups = sms / (int)n_jb;
+    int groups = sm_count() / (int)n_jb;
     if (groups > p.n_tiles) groups = p.n_tiles;
     if (groups < 1) groups = 1;
     const int grid = groups * (int)n_jb;

@@ -223,41 +223,64 @@ static int set_smem(K kernel, int bytes) {
     return PTGNN_OK;
 }
 
+template <int TN>
+static int launch_edge_message_kernel(const MsgParams &p, int tiles, const float *h_src, const float *h_tgt, int H, int D,
+                                      int use_target, const int32_t *src32, const int32_t *tgt32, const int32_t *pos, float *msg,
+                                      cudaStream_t st) {
+    using Tile = GemmTile<TN>;
+    int rc = set_smem(edge_message_kernel<TN>, Tile::SMEM_BYTES);
+    if (rc) return rc;
+    dim3 grid(tiles, (unsigned)ceil_div(D, Tile::BN));
+    {
+        TimedScope timed__(PTGNN_KERNEL_MESSAGE, st);
+        edge_message_kernel<TN><<<grid, GEMM_THREADS, Tile::SMEM_BYTES, st>>>(p, h_src, h_tgt, H, use_target, D, src32, tgt32, pos, msg);
+    }
+    PTGNN_LAUNCHED();
+    return PTGNN_OK;
+}
+
 static int launch_edge_messages(const float *h_src, const float *h_tgt, int H, int D, int use_target, int num_types, const int64_t *type_off,
                                 const float *const *weights, const int32_t *src32, const int32_t *tgt32,
                                 const int32_t *pos, float *msg, cudaStream_t st) {
     MsgParams p{};
     p.num_types = num_types;
-    int tiles = 0;
-    for (int t = 0; t < num_types; ++t) {
-        p.weights[t] = weights[t];
-        p.edge_off[t] = (int32_t)type_off[t];
-        p.tile_off[t] = tiles;
-        tiles += (int)ceil_div(type_off[t + 1] - type_off[t], GEMM_BM);
-    }
-    for (int t = num_types; t <= PTGNN_MAX_EDGE_TYPES; ++t) {
-        p.edge_off[t] = (int32_t)type_off[num_types];
-        p.tile_off[t] = tiles;
-    }
+    for (int t = 0; t < num_types; ++t) p.weights[t] = weights[t];
+    const int tiles = build_type_tiles(type_off, num_types, GEMM_BM, p.edge_off, p.tile_off);
     if (tiles == 0) return PTGNN_OK;
-    if (D <= 64) {
-        using Tile = GemmTile<4>;
-        int rc = set_smem(edge_message_kernel<4>, Tile::SMEM_BYTES);
-        if (rc) return rc;
-        dim3 grid(tiles, (unsigned)ceil_div(D, Tile::BN));
-        {
-            TimedScope timed__(PTGNN_KERNEL_MESSAGE, st);
-            edge_message_kernel<4><<<grid, GEMM_THREADS, Tile::SMEM_BYTES, st>>>(p, h_src, h_tgt, H, use_target, D, src32, tgt32, pos, msg);
-        }
-    } else {
-        using Tile = GemmTile<8>;
-        int rc = set_smem(edge_message_kernel<8>, Tile::SMEM_BYTES);
-        if (rc) return rc;
-        dim3 grid(tiles, (unsigned)ceil_div(D, Tile::BN));
-        {
-            TimedScope timed__(PTGNN_KERNEL_MESSAGE, st);
-            edge_message_kernel<8><<<grid, GEMM_THREADS, Tile::SMEM_BYTES, st>>>(p, h_src, h_tgt, H, use_target, D, src32, tgt32, pos, msg);
-        }
+    if (D <= 64) return launch_edge_message_kernel<4>(p, tiles, h_src, h_tgt, H, D, use_target, src32, tgt32, pos, msg, st);
+    return launch_edge_message_kernel<8>(p, tiles, h_src, h_tgt, H, D, use_target, src32, tgt32, pos, msg, st);
+}
+
+template <int TN>
+static int launch_dense_kernel(const float *y, int64_t rows, int D, const float *W, const float *bias, int out_dim, int act, float *out,
+                               cudaStream_t st) {
+    using Tile = GemmTile<TN>;
+    int rc = set_smem(dense_update_kernel<TN>, Tile::SMEM_BYTES);
+    if (rc) return rc;
+    dim3 grid((unsigned)ceil_div(rows, GEMM_BM), (unsigned)ceil_div(out_dim, Tile::BN));
+    {
+        TimedScope timed__(PTGNN_KERNEL_DENSE, st);
+        dense_update_kernel<TN><<<grid, GEMM_THREADS, Tile::SMEM_BYTES, st>>>(y, (int)rows, D, W, bias, out_dim, act, out);
+    }
+    PTGNN_LAUNCHED();
+    return PTGNN_OK;
+}
+
+// FFMA GRUCell: packs the gate weights into P1 / P2 (workspace, re-derived every call), then one launch
+static int launch_gru_simt(const float *agg, const float *h, int64_t rows, int H, int D, const float *w_ih, const float *w_hh,
+                           const float *b_ih, const float *b_hh, float *out, float *P1, float *P2, cudaStream_t st) {
+    {
+        TimedScope timed__(PTGNN_KERNEL_PACK, st);
+        pack_gru_weights_kernel<<<132, 256, 0, st>>>(w_ih, w_hh, H, D, P1, P2);
+    }
+    PTGNN_LAUNCHED();
+    using Tile = GemmTile<6>;
+    int rc = set_smem(gru_update_kernel, Tile::SMEM_BYTES);
+    if (rc) return rc;
+    dim3 grid((unsigned)ceil_div(rows, GEMM_BM), H / 32);
+    {
+        TimedScope timed__(PTGNN_KERNEL_GRU, st);
+        gru_update_kernel<<<grid, GEMM_THREADS, Tile::SMEM_BYTES, st>>>(agg, h, (int)rows, H, D, P1, P2, b_ih, b_hh, out);
     }
     PTGNN_LAUNCHED();
     return PTGNN_OK;
@@ -282,28 +305,8 @@ bool tc_enabled() {
 int dense_any(const float *y, int64_t rows, int D, const float *W, const float *bias, int out_dim, int act, float *out,
               void *scratch, cudaStream_t st, bool pack) {
     if (tc_enabled() && tc::supported_dense(D, out_dim)) return tc::dense_update(y, rows, D, W, bias, out_dim, act, out, scratch, st, pack);
-    int rc;
-    if (out_dim <= 64) {
-        using Tile = GemmTile<4>;
-        rc = set_smem(dense_update_kernel<4>, Tile::SMEM_BYTES);
-        if (rc) return rc;
-        dim3 grid((unsigned)ceil_div(rows, GEMM_BM), (unsigned)ceil_div(out_dim, Tile::BN));
-        {
-            TimedScope timed__(PTGNN_KERNEL_DENSE, st);
-            dense_update_kernel<4><<<grid, GEMM_THREADS, Tile::SMEM_BYTES, st>>>(y, (int)rows, D, W, bias, out_dim, act, out);
-        }
-    } else {
-        using Tile = GemmTile<8>;
-        rc = set_smem(dense_update_kernel<8>, Tile::SMEM_BYTES);
-        if (rc) return rc;
-        dim3 grid((unsigned)ceil_div(rows, GEMM_BM), (unsigned)ceil_div(out_dim, Tile::BN));
-        {
-            TimedScope timed__(PTGNN_KERNEL_DENSE, st);
-            dense_update_kernel<8><<<grid, GEMM_THREADS, Tile::SMEM_BYTES, st>>>(y, (int)rows, D, W, bias, out_dim, act, out);
-        }
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    if (out_dim <= 64) return launch_dense_kernel<4>(y, rows, D, W, bias, out_dim, act, out, st);
+    return launch_dense_kernel<8>(y, rows, D, W, bias, out_dim, act, out, st);
 }
 
 struct GatedWs { size_t msg, agg, p1, p2, wsplit, grupack, total; };
@@ -412,22 +415,7 @@ static int gated_forward_impl(const float *node_states, const float *gather_stat
         return tc::gru_update(agg, node_states, num_nodes, H, D, gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, out_states,
                               grupack, pack, st);
     }
-    {
-        TimedScope timed__(PTGNN_KERNEL_PACK, st);
-        pack_gru_weights_kernel<<<132, 256, 0, st>>>(gru_w_ih, gru_w_hh, H, D, P1, P2);
-    }
-    PTGNN_LAUNCHED();
-    using Tile = GemmTile<6>;
-    rc = set_smem(gru_update_kernel, Tile::SMEM_BYTES);
-    if (rc) return rc;
-    dim3 grid((unsigned)ceil_div(num_nodes, GEMM_BM), H / 32);
-    {
-        TimedScope timed__(PTGNN_KERNEL_GRU, st);
-        gru_update_kernel<<<grid, GEMM_THREADS, Tile::SMEM_BYTES, st>>>(agg, node_states, (int)num_nodes, H, D, P1, P2,
-                                                                     gru_b_ih, gru_b_hh, out_states);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch_gru_simt(agg, node_states, num_nodes, H, D, gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, out_states, P1, P2, st);
 }
 
 extern "C" size_t ptgnn_b200_gated_weight_cache_bytes(int32_t num_types, int32_t state_dim, int32_t message_dim) {
@@ -496,7 +484,7 @@ static int mlp_forward_impl(const float *node_states, const float *gather_states
                                   st);
     }
     if (rc) return rc;
-    ReduceEpilogue epi{0, message_activation, ln_weight, ln_bias, ln_eps};
+    ReduceEpilogue epi{message_activation, ln_weight, ln_bias, ln_eps};
     rc = launch_segment_reduce(msg, row_ptr, nullptr, num_nodes, E, D, reduce, y, nullptr, &epi, st);
     if (rc) return rc;
     if (!dense_weight) return PTGNN_OK;
@@ -585,20 +573,6 @@ extern "C" int ptgnn_b200_grucell_f32(const float *input, const float *hidden, i
     const size_t o1 = ws_slice((size_t)(H / 32 + 1) * 96 * D, 4), o2 = ws_slice((size_t)(H / 32 + 1) * 96 * H, 4);
     if (tc_enabled() && tc::supported_gru(H, D))
         return tc::gru_update(input, hidden, rows, H, D, w_ih, w_hh, b_ih, b_hh, out, ws + o1 + o2, true, st);
-    float *P1 = reinterpret_cast<float *>(ws), *P2 = reinterpret_cast<float *>(ws + o1);
-    {
-        TimedScope timed__(PTGNN_KERNEL_PACK, st);
-        pack_gru_weights_kernel<<<132, 256, 0, st>>>(w_ih, w_hh, H, D, P1, P2);
-    }
-    PTGNN_LAUNCHED();
-    using Tile = GemmTile<6>;
-    rc = set_smem(gru_update_kernel, Tile::SMEM_BYTES);
-    if (rc) return rc;
-    dim3 grid((unsigned)ceil_div(rows, GEMM_BM), H / 32);
-    {
-        TimedScope timed__(PTGNN_KERNEL_GRU, st);
-        gru_update_kernel<<<grid, GEMM_THREADS, Tile::SMEM_BYTES, st>>>(input, hidden, (int)rows, H, D, P1, P2, b_ih, b_hh, out);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch_gru_simt(input, hidden, rows, H, D, w_ih, w_hh, b_ih, b_hh, out, reinterpret_cast<float *>(ws),
+                           reinterpret_cast<float *>(ws + o1), st);
 }

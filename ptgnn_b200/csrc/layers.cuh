@@ -15,9 +15,20 @@ int dense_any(const float *y, int64_t rows, int D, const float *W, const float *
               void *scratch, cudaStream_t st, bool pack = true);
 
 namespace tcb {
-// out = act(y W^T + b) with bf16 states: W (fp32 [Hout, D]) converted to bf16 into scratch (>= dense_weight_bytes), then bf16
-// products with fp32 accumulation.
+// The bf16 round-1 kernels (layers_bf16.cu): bf16 states, weights converted from fp32 into `scratch`, fp32 accumulation.
+// `pack` = false when `scratch` is a weight cache that already holds the converted weights.
+size_t edge_weight_bytes(int num_types, int D, int Kw);
+size_t gru_pack_bytes(int H, int D);
 size_t dense_weight_bytes(int Hout, int D);
+// messages[pos[e]] = W_t(e) [h_src[src(e)] ; h_tgt[tgt(e)]]   (scratch >= edge_weight_bytes, Kw = H or 2H with target states)
+int edge_messages(const __nv_bfloat16 *h_src, const __nv_bfloat16 *h_tgt, int H, int D, int use_target, int num_types,
+                  const int64_t *type_off, const float *const *weights, const int32_t *src32, const int32_t *tgt32,
+                  const int32_t *pos, __nv_bfloat16 *msg, void *scratch, bool pack, cudaStream_t st);
+// out = GRUCell(agg, h)                                       (scratch >= gru_pack_bytes)
+int gru_update(const __nv_bfloat16 *agg, const __nv_bfloat16 *h, int64_t num_nodes, int H, int D, const float *w_ih,
+               const float *w_hh, const float *b_ih, const float *b_hh, __nv_bfloat16 *out, void *scratch, bool pack,
+               cudaStream_t st);
+// out = act(y W^T + b); W (fp32 [Hout, D]) is converted on every call  (scratch >= dense_weight_bytes)
 int dense_update(const __nv_bfloat16 *y, int64_t rows, int D, const float *W, const float *bias, int Hout, int act,
                  __nv_bfloat16 *out, void *scratch, cudaStream_t st);
 }  // namespace tcb

@@ -5,7 +5,6 @@
 // Kernels: weight conversion/packing -> tc_pipeline_bf16_kernel<MsgPolicyB> -> segment_reduce_bf16_kernel ->
 // tc_pipeline_bf16_kernel<GruPolicyB>.
 #include <float.h>
-#include <stdlib.h>
 
 #include "layers.cuh"
 #include "layers_tc.cuh"
@@ -14,34 +13,7 @@
 namespace ptgnn {
 namespace tcb {
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn encode_tiled_fn() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void *ptr = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(ptr);
-    }
-    return fn;
-}
-// bf16 row-major [rows, cols], box = {64 columns (128 bytes), box_rows}, SWIZZLE_128B, OOB zero fill
-static int make_map_bf16(CUtensorMap *map, const __nv_bfloat16 *base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
-    EncodeTiledFn fn = encode_tiled_fn();
-    if (!fn) { set_error("cuTensorMapEncodeTiled entry point not available"); return PTGNN_E_CUDA; }
-    const cuuint64_t dims[2] = {cols, rows};
-    const cuuint64_t strides[1] = {cols * sizeof(__nv_bfloat16)};
-    const cuuint32_t box[2] = {(cuuint32_t)CHUNK_K, box_rows};
-    const cuuint32_t estr[2] = {1, 1};
-    const CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<__nv_bfloat16 *>(base), dims, strides, box,
-                          estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled (bf16) failed with CUresult %d", (int)r); return PTGNN_E_CUDA; }
-    return PTGNN_OK;
-}
+constexpr CUtensorMapDataType BF16 = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
 
 // ---- weights: fp32 module parameters -> bf16 working copies ---------------------------------------------------
 struct ConvSrc {
@@ -54,10 +26,6 @@ __global__ void convert_weights_kernel(const __grid_constant__ ConvSrc s, __nv_b
         out[i] = __float2bfloat16_rn(s.w[i / s.elems][i % s.elems]);
 }
 // same gate-blocked layout as the fp32 path: P1[jb] = [W_ir; W_iz; W_in; 0], P2[jb] = [W_hr; W_hz; 0; W_hn] (128 rows each)
-__global__ void pack_gru_bias_bf16_kernel(const float *__restrict__ b_ih, const float *__restrict__ b_hh, int H, float4 *__restrict__ bias4) {
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j < H) bias4[j] = make_float4(b_ih[j] + b_hh[j], b_ih[H + j] + b_hh[H + j], b_ih[2 * H + j], b_hh[2 * H + j]);
-}
 __global__ void pack_gru_bf16_kernel(const float *__restrict__ w_ih, const float *__restrict__ w_hh, int H, int D,
                                      __nv_bfloat16 *__restrict__ p1, __nv_bfloat16 *__restrict__ p2) {
     const int nblk = H / 32;
@@ -84,8 +52,7 @@ struct MsgPolicyB {
         const int32_t *src32, *tgt32, *pos;
         int use_target;
         __nv_bfloat16 *msg;                // [E, D] bf16 at target-sorted rows
-        unsigned long long *trace;
-        int H, D, num_types, n_blocks, dbg;   // dbg: PTGNN_TC_DEBUG ablation bits (1 no MMA, 2 no store, 4 no loads, 8 no drain)
+        int H, D, num_types, n_blocks;
         int32_t edge_off[PTGNN_MAX_EDGE_TYPES + 1];
         int32_t tile_off[PTGNN_MAX_EDGE_TYPES + 1];
     };
@@ -154,8 +121,7 @@ struct GruPolicyB {
         const __nv_bfloat16 *h;
         const float4 *bias4;   // (b_ir + b_hr, b_iz + b_hz, b_in, b_hn) per hidden unit
         __nv_bfloat16 *out;
-        unsigned long long *trace;
-        int num_nodes, H, D, n_jb, dbg;
+        int num_nodes, H, D, n_jb;
     };
     struct Tile { int row0, jb; };
     __device__ static int num_tiles(const Params &p) { return ((p.num_nodes + TILE_M - 1) / TILE_M) * p.n_jb; }
@@ -211,8 +177,7 @@ struct GruPolicyB {
 #pragma unroll
             for (int u = 0; u < 2; ++u) {
                 const int ii = 2 * i + u;
-                const float4 b = (p.dbg & 16) ? make_float4(0.1f, 0.2f, 0.3f, 0.4f) : bias_s[j0 + ii];
-                if (p.dbg & 32) { o[u] = acc[ii] + acc[16 + ii] + acc[32 + ii] + acc[48 + ii] + b.x + hv[u]; continue; }
+                const float4 b = bias_s[j0 + ii];
                 const float rr = sigmoid_mufu(acc[ii] + b.x);
                 const float zz = sigmoid_mufu(acc[16 + ii] + b.y);
                 const float nn = tanh_mufu(fmaf(rr, acc[48 + ii] + b.w, acc[32 + ii] + b.z));
@@ -220,7 +185,7 @@ struct GruPolicyB {
             }
             ow[i] = __float_as_uint(pack_bf16x2(o[0], o[1]));
         }
-        if (pre.off >= 0 && !(p.dbg & 64)) {
+        if (pre.off >= 0) {
             uint4 *dst = reinterpret_cast<uint4 *>(p.out + pre.off);
             dst[0] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
             dst[1] = make_uint4(ow[4], ow[5], ow[6], ow[7]);
@@ -234,8 +199,7 @@ struct DensePolicyB {
         CUtensorMap map_y, map_w;          // [N, D] box {64, 128}; [Hout, D] box {64, min(128, Hout)}
         const float *bias;                 // fp32 [Hout] or nullptr
         __nv_bfloat16 *out;                // [N, Hout]
-        unsigned long long *trace;
-        int num_nodes, D, Hout, act, n_blocks, dbg;
+        int num_nodes, D, Hout, act, n_blocks;
     };
     struct Tile { int row0, n0, b_rows; };
     __device__ static int num_tiles(const Params &p) { return ((p.num_nodes + TILE_M - 1) / TILE_M) * p.n_blocks; }
@@ -435,46 +399,63 @@ static int reduce_bf16(int reduce, const __nv_bfloat16 *msg, const int32_t *row_
     }
 }
 
-static int debug_bits() {
-    const char *e = getenv("PTGNN_TC_DEBUG");
-    return e ? atoi(e) : 0;
-}
-static int sm_count() {   // of the CURRENT device: a process may drive several GPUs (nothing cached across devices)
-    int dev = 0, n = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
-    return n;
-}
-template <class Policy>
-static int launch_pipeline(const typename Policy::Params &p, int total_tiles, int category, cudaStream_t st) {
-    if (total_tiles <= 0) return PTGNN_OK;
-    // per launch, not once per process: the attribute is per device (and per context)
-    PTGNN_CUDA(cudaFuncSetAttribute(tc_pipeline_bf16_kernel<Policy>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    const int sms = sm_count();
-    const int grid = total_tiles < sms ? total_tiles : sms;
-    {
-        TimedScope timed__(category, st);
-        tc_pipeline_bf16_kernel<Policy><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(p);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
-}
-
-struct WsB { size_t msg, agg, w, p1, p2, bias, total; };
-static WsB ws_layout(int64_t N, int64_t E, int T, int H, int D) {
-    WsB w{};
-    size_t o = 0;
-    auto add = [&](size_t cnt) { size_t at = o; o += ws_slice(cnt, 2); return at; };
-    w.msg = add((size_t)E * D + 8);
-    w.agg = add((size_t)N * D + 8);
-    w.w = add((size_t)T * D * H + 8);
-    w.p1 = add((size_t)(H / 32 + 1) * 128 * D);
-    w.p2 = add((size_t)(H / 32 + 1) * 128 * H);
-    w.bias = add((size_t)H * 8 + 8);
-    w.total = o;
-    return w;
-}
-
+size_t edge_weight_bytes(int num_types, int D, int Kw) { return ws_slice((size_t)num_types * D * Kw + 8, 2); }
+// GRU packing [P1 (K = D) | P2 (K = H) | bias4]: gate-blocked bf16 weights, 128 rows per block of 32 hidden units
+static size_t gru_part_bytes(int H, int K) { return ws_slice((size_t)(H / 32 + 1) * 128 * K, 2); }
+size_t gru_pack_bytes(int H, int D) { return gru_part_bytes(H, D) + gru_part_bytes(H, H) + ws_slice((size_t)H * 8 + 8, 2); }
 size_t dense_weight_bytes(int Hout, int D) { return ws_slice((size_t)Hout * D + 8, 2); }
+
+int edge_messages(const __nv_bfloat16 *h_src, const __nv_bfloat16 *h_tgt, int H, int D, int use_target, int num_types,
+                  const int64_t *type_off, const float *const *weights, const int32_t *src32, const int32_t *tgt32,
+                  const int32_t *pos, __nv_bfloat16 *msg, void *scratch, bool pack, cudaStream_t st) {
+    const int Kw = use_target ? 2 * H : H;
+    __nv_bfloat16 *wb = static_cast<__nv_bfloat16 *>(scratch);
+    if (pack) {   // false: `scratch` is a weight cache that already holds the bf16 copy of these weights
+        ConvSrc cs{};
+        cs.num = num_types; cs.elems = D * Kw;
+        for (int t = 0; t < num_types; ++t) cs.w[t] = weights[t];
+        {
+            TimedScope timed__(PTGNN_KERNEL_PACK, st);
+            convert_weights_kernel<<<132, 256, 0, st>>>(cs, wb);
+        }
+        PTGNN_LAUNCHED();
+    }
+    MsgPolicyB::Params p{};
+    const int rc = make_tensor_map_2d(&p.map_w, BF16, wb, (uint64_t)num_types * D, Kw, Kw, CHUNK_K, D < 128 ? D : 128);
+    if (rc) return rc;
+    p.h = h_src; p.h_tgt = h_tgt; p.src32 = src32; p.tgt32 = tgt32; p.use_target = use_target; p.pos = pos; p.msg = msg;
+    p.H = H; p.D = D; p.num_types = num_types; p.n_blocks = (D + 127) / 128;
+    const int tiles = build_type_tiles(type_off, num_types, TILE_M, p.edge_off, p.tile_off);
+    return tc::launch_pipeline(tc_pipeline_bf16_kernel<MsgPolicyB>, p, SMEM_BYTES, tiles * p.n_blocks, PTGNN_KERNEL_MESSAGE, st);
+}
+
+int gru_update(const __nv_bfloat16 *agg, const __nv_bfloat16 *h, int64_t num_nodes, int H, int D, const float *w_ih,
+               const float *w_hh, const float *b_ih, const float *b_hh, __nv_bfloat16 *out, void *scratch, bool pack,
+               cudaStream_t st) {
+    char *s = static_cast<char *>(scratch);
+    const size_t s1 = gru_part_bytes(H, D), s2 = gru_part_bytes(H, H);
+    __nv_bfloat16 *p1 = reinterpret_cast<__nv_bfloat16 *>(s), *p2 = reinterpret_cast<__nv_bfloat16 *>(s + s1);
+    float4 *bias4 = reinterpret_cast<float4 *>(s + s1 + s2);
+    if (pack) {
+        {
+            TimedScope timed__(PTGNN_KERNEL_PACK, st);
+            pack_gru_bf16_kernel<<<132, 256, 0, st>>>(w_ih, w_hh, H, D, p1, p2);
+        }
+        PTGNN_LAUNCHED();
+        const int rc = tc::pack_gru_bias(b_ih, b_hh, H, bias4, st);
+        if (rc) return rc;
+    }
+    GruPolicyB::Params p{};
+    const uint64_t prow = (uint64_t)(H / 32) * 128;
+    int rc = make_tensor_map_2d(&p.map_agg, BF16, agg, num_nodes, D, D, CHUNK_K, 128);
+    if (!rc) rc = make_tensor_map_2d(&p.map_h, BF16, h, num_nodes, H, H, CHUNK_K, 128);
+    if (!rc) rc = make_tensor_map_2d(&p.map_p1, BF16, p1, prow, D, D, CHUNK_K, 128);
+    if (!rc) rc = make_tensor_map_2d(&p.map_p2, BF16, p2, prow, H, H, CHUNK_K, 128);
+    if (rc) return rc;
+    p.h = h; p.bias4 = bias4; p.out = out; p.num_nodes = (int)num_nodes; p.H = H; p.D = D; p.n_jb = H / 32;
+    const int tiles = (int)ceil_div(num_nodes, TILE_M) * p.n_jb;
+    return tc::launch_pipeline(tc_pipeline_bf16_kernel<GruPolicyB>, p, SMEM_BYTES, tiles, PTGNN_KERNEL_GRU, st);
+}
 
 int dense_update(const __nv_bfloat16 *y, int64_t rows, int D, const float *W, const float *bias, int Hout, int act,
                  __nv_bfloat16 *out, void *scratch, cudaStream_t st) {
@@ -487,12 +468,26 @@ int dense_update(const __nv_bfloat16 *y, int64_t rows, int D, const float *W, co
     }
     PTGNN_LAUNCHED();
     DensePolicyB::Params dp{};
-    int rc = make_map_bf16(&dp.map_y, y, rows, D, 128);
-    if (!rc) rc = make_map_bf16(&dp.map_w, wd, Hout, D, Hout < 128 ? Hout : 128);
+    int rc = make_tensor_map_2d(&dp.map_y, BF16, y, rows, D, D, CHUNK_K, 128);
+    if (!rc) rc = make_tensor_map_2d(&dp.map_w, BF16, wd, Hout, D, D, CHUNK_K, Hout < 128 ? Hout : 128);
     if (rc) return rc;
     dp.bias = bias; dp.out = out; dp.num_nodes = (int)rows; dp.D = D; dp.Hout = Hout; dp.act = act;
-    dp.n_blocks = (Hout + 127) / 128; dp.dbg = debug_bits(); dp.trace = tc::trace_buffer(PTGNN_KERNEL_DENSE + 10);
-    return launch_pipeline<DensePolicyB>(dp, (int)ceil_div(rows, TILE_M) * dp.n_blocks, PTGNN_KERNEL_DENSE, st);
+    dp.n_blocks = (Hout + 127) / 128;
+    const int tiles = (int)ceil_div(rows, TILE_M) * dp.n_blocks;
+    return tc::launch_pipeline(tc_pipeline_bf16_kernel<DensePolicyB>, dp, SMEM_BYTES, tiles, PTGNN_KERNEL_DENSE, st);
+}
+
+// workspace of the gated layer: [msg | agg | bf16 edge weights | GRU packing (P1 | P2 | bias4)]
+struct WsB { size_t msg, agg, w, gru, total; };
+static WsB ws_layout(int64_t N, int64_t E, int T, int H, int D) {
+    WsB w{};
+    size_t o = 0;
+    w.msg = o; o += ws_slice((size_t)E * D + 8, 2);
+    w.agg = o; o += ws_slice((size_t)N * D + 8, 2);
+    w.w = o; o += edge_weight_bytes(T, D, H);
+    w.gru = o; o += gru_pack_bytes(H, D);
+    w.total = o;
+    return w;
 }
 
 }  // namespace tcb
@@ -539,10 +534,9 @@ static int gated_forward_bf16_impl(const uint16_t *node_states, const uint16_t *
         return PTGNN_E_WORKSPACE;
     }
     char *ws = static_cast<char *>(workspace);
-    auto b16 = [&](size_t off) { return reinterpret_cast<__nv_bfloat16 *>(ws + off); };
     const __nv_bfloat16 *h = reinterpret_cast<const __nv_bfloat16 *>(node_states);
     const __nv_bfloat16 *hsrc = gather_states ? reinterpret_cast<const __nv_bfloat16 *>(gather_states) : h;
-    __nv_bfloat16 *msg = b16(L.msg), *agg = b16(L.agg);
+    __nv_bfloat16 *msg = reinterpret_cast<__nv_bfloat16 *>(ws + L.msg), *agg = reinterpret_cast<__nv_bfloat16 *>(ws + L.agg);
     // derived weights live in the workspace (re-derived every call) or in the caller's cache (derived when !cache_valid)
     char *wbase = ws + L.w;
     bool pack = true;
@@ -555,65 +549,16 @@ static int gated_forward_bf16_impl(const uint16_t *node_states, const uint16_t *
         wbase = static_cast<char *>(weight_cache);
         pack = !cache_valid;
     }
-    __nv_bfloat16 *wb = reinterpret_cast<__nv_bfloat16 *>(wbase);
-    __nv_bfloat16 *p1 = reinterpret_cast<__nv_bfloat16 *>(wbase + (L.p1 - L.w)), *p2 = reinterpret_cast<__nv_bfloat16 *>(wbase + (L.p2 - L.w));
-    float4 *bias4 = reinterpret_cast<float4 *>(wbase + (L.bias - L.w));
 
-    // 0. weights -> bf16 (edge weights [T][D][H]; GRU gate blocks)
-    if (pack) {
-        ConvSrc cs{};
-        cs.num = num_types; cs.elems = D * H;
-        for (int t = 0; t < num_types; ++t) cs.w[t] = edge_weights[t];
-        {
-            TimedScope timed__(PTGNN_KERNEL_PACK, st);
-            convert_weights_kernel<<<132, 256, 0, st>>>(cs, wb);
-        }
-        PTGNN_LAUNCHED();
-        {
-            TimedScope timed__(PTGNN_KERNEL_PACK, st);
-            pack_gru_bf16_kernel<<<132, 256, 0, st>>>(gru_w_ih, gru_w_hh, H, D, p1, p2);
-        }
-        PTGNN_LAUNCHED();
-        {
-            TimedScope timed__(PTGNN_KERNEL_PACK, st);
-            pack_gru_bias_bf16_kernel<<<(H + 127) / 128, 128, 0, st>>>(gru_b_ih, gru_b_hh, H, bias4);
-        }
-        PTGNN_LAUNCHED();
-    }
-
-    // 1. messages
-    MsgPolicyB::Params mp{};
-    int rc = make_map_bf16(&mp.map_w, wb, (uint64_t)num_types * D, H, D < 128 ? D : 128);
+    // 1. messages (edge weights -> bf16 first when packing)
+    int rc = tcb::edge_messages(hsrc, h, H, D, 0, num_types, type_off, edge_weights, src32, nullptr, pos, msg, wbase, pack, st);
     if (rc) return rc;
-    mp.h = hsrc; mp.h_tgt = h; mp.src32 = src32; mp.tgt32 = nullptr; mp.use_target = 0; mp.pos = pos; mp.msg = msg; mp.H = H; mp.D = D;
-    mp.num_types = num_types;
-    mp.n_blocks = (D + 127) / 128;
-    mp.dbg = debug_bits(); mp.trace = tc::trace_buffer(PTGNN_KERNEL_MESSAGE + 10);
-    int tiles = 0;
-    for (int t = 0; t < num_types; ++t) {
-        mp.edge_off[t] = (int32_t)type_off[t];
-        mp.tile_off[t] = tiles;
-        tiles += (int)ceil_div(type_off[t + 1] - type_off[t], TILE_M);
-    }
-    for (int t = num_types; t <= PTGNN_MAX_EDGE_TYPES; ++t) { mp.edge_off[t] = (int32_t)type_off[num_types]; mp.tile_off[t] = tiles; }
-    rc = launch_pipeline<MsgPolicyB>(mp, tiles * mp.n_blocks, PTGNN_KERNEL_MESSAGE, st);
-    if (rc) return rc;
-
     // 2. segmented reduce (fp32 accumulate, bf16 result)
     rc = reduce_bf16(reduce, msg, row_ptr, num_nodes, D, agg, nullptr, st);
     if (rc) return rc;
-
-    // 3. GRUCell
-    GruPolicyB::Params gp{};
-    const uint64_t prow = (uint64_t)(H / 32) * 128;
-    rc = make_map_bf16(&gp.map_agg, agg, num_nodes, D, 128);
-    if (!rc) rc = make_map_bf16(&gp.map_h, h, num_nodes, H, 128);
-    if (!rc) rc = make_map_bf16(&gp.map_p1, p1, prow, D, 128);
-    if (!rc) rc = make_map_bf16(&gp.map_p2, p2, prow, H, 128);
-    if (rc) return rc;
-    gp.h = h; gp.bias4 = bias4; gp.out = reinterpret_cast<__nv_bfloat16 *>(out_states);
-    gp.num_nodes = (int)num_nodes; gp.H = H; gp.D = D; gp.n_jb = H / 32; gp.dbg = debug_bits(); gp.trace = tc::trace_buffer(PTGNN_KERNEL_GRU + 10);
-    return launch_pipeline<GruPolicyB>(gp, (int)ceil_div(num_nodes, TILE_M) * gp.n_jb, PTGNN_KERNEL_GRU, st);
+    // 3. GRUCell (gate-blocked weights and biases packed first when packing)
+    return tcb::gru_update(agg, h, num_nodes, H, D, gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, reinterpret_cast<__nv_bfloat16 *>(out_states),
+                           wbase + (L.gru - L.w), pack, st);
 }
 
 extern "C" size_t ptgnn_b200_gated_weight_cache_bytes_bf16(int32_t num_types, int32_t state_dim, int32_t message_dim) {
@@ -645,10 +590,9 @@ struct MlpWsB { size_t msg, y, w, wd, total; };
 static MlpWsB mlp_ws_layout(int64_t N, int64_t E, int T, int H, int D, int Hout, int use_target) {
     MlpWsB w{};
     size_t o = 0;
-    auto add = [&](size_t cnt) { size_t at = o; o += ws_slice(cnt, 2); return at; };
-    w.msg = add((size_t)E * D + 8);
-    w.y = add((size_t)N * D + 8);
-    w.w = add((size_t)T * D * H * (use_target ? 2 : 1) + 8);
+    w.msg = o; o += ws_slice((size_t)E * D + 8, 2);
+    w.y = o; o += ws_slice((size_t)N * D + 8, 2);
+    w.w = o; o += edge_weight_bytes(T, D, use_target ? 2 * H : H);
     w.wd = o; o += dense_weight_bytes(Hout, D);
     w.total = o;
     return w;
@@ -671,7 +615,7 @@ static int mlp_forward_bf16_impl(const uint16_t *node_states, const uint16_t *ga
                                  const float *dense_weight, const float *dense_bias, int32_t dense_activation,
                                  uint16_t *out_states, void *workspace, size_t workspace_bytes, void *stream) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int H = in_dim, D = message_dim, ut = use_target_state ? 1 : 0, Kw = H * (1 + ut);
+    const int H = in_dim, D = message_dim, ut = use_target_state ? 1 : 0;
     PTGNN_CHECK_ARG(num_types >= 0 && num_types <= PTGNN_MAX_EDGE_TYPES && type_off, "mlp_forward_bf16: bad num_types=%d", num_types);
     const int64_t E = type_off[num_types];
     PTGNN_CHECK_ARG(num_nodes >= 0 && num_nodes < INT32_MAX && E >= 0 && E < INT32_MAX, "mlp_forward_bf16: sizes out of range");
@@ -698,39 +642,13 @@ static int mlp_forward_bf16_impl(const uint16_t *node_states, const uint16_t *ga
     const __nv_bfloat16 *h = reinterpret_cast<const __nv_bfloat16 *>(node_states);
     const __nv_bfloat16 *hsrc = gather_states ? reinterpret_cast<const __nv_bfloat16 *>(gather_states) : h;
     __nv_bfloat16 *out = reinterpret_cast<__nv_bfloat16 *>(out_states);
-    __nv_bfloat16 *msg = b16(L.msg), *wb = b16(L.w);
+    __nv_bfloat16 *msg = b16(L.msg);
     __nv_bfloat16 *y = dense_weight ? b16(L.y) : out;
 
-    // 0. edge weights -> bf16
+    // 1. messages  m_e = W_t [h_src ; h_tgt]  (edge weights -> bf16 first)
     int rc = PTGNN_OK;
     if (num_types > 0) {
-        ConvSrc cs{};
-        cs.num = num_types; cs.elems = D * Kw;
-        for (int t = 0; t < num_types; ++t) cs.w[t] = edge_weights[t];
-        {
-            TimedScope timed__(PTGNN_KERNEL_PACK, st);
-            convert_weights_kernel<<<132, 256, 0, st>>>(cs, wb);
-        }
-        PTGNN_LAUNCHED();
-    }
-
-    // 1. messages  m_e = W_t [h_src ; h_tgt]
-    if (E > 0) {
-        MsgPolicyB::Params mp{};
-        rc = make_map_bf16(&mp.map_w, wb, (uint64_t)num_types * D, Kw, D < 128 ? D : 128);
-        if (rc) return rc;
-        mp.h = hsrc; mp.h_tgt = h; mp.src32 = src32; mp.tgt32 = tgt32; mp.use_target = ut; mp.pos = pos; mp.msg = msg; mp.H = H; mp.D = D;
-        mp.num_types = num_types;
-        mp.n_blocks = (D + 127) / 128;
-        mp.dbg = debug_bits(); mp.trace = tc::trace_buffer(PTGNN_KERNEL_MESSAGE + 10);
-        int tiles = 0;
-        for (int t = 0; t < num_types; ++t) {
-            mp.edge_off[t] = (int32_t)type_off[t];
-            mp.tile_off[t] = tiles;
-            tiles += (int)ceil_div(type_off[t + 1] - type_off[t], TILE_M);
-        }
-        for (int t = num_types; t <= PTGNN_MAX_EDGE_TYPES; ++t) { mp.edge_off[t] = (int32_t)type_off[num_types]; mp.tile_off[t] = tiles; }
-        rc = launch_pipeline<MsgPolicyB>(mp, tiles * mp.n_blocks, PTGNN_KERNEL_MESSAGE, st);
+        rc = tcb::edge_messages(hsrc, h, H, D, ut, num_types, type_off, edge_weights, src32, tgt32, pos, msg, ws + L.w, true, st);
         if (rc) return rc;
     }
 

@@ -3,46 +3,12 @@
 // tc_pipeline.cuh, the policies below only say where rows come from and what the epilogue does with the tile.
 #include "layers_tc.cuh"
 
-#include <stdlib.h>
-
 #include "tc_pipeline.cuh"
 
 namespace ptgnn {
 namespace tc {
 
-// =================================================================================================
-// TMA tensor maps (driver entry point fetched through the runtime: no libcuda link dependency)
-// =================================================================================================
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn encode_tiled_fn() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void *ptr = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(ptr);
-    }
-    return fn;
-}
-// fp32 row-major [rows, cols] (row pitch = pitch_elems), box = {32 columns (128 bytes), box_rows}, SWIZZLE_128B;
-// out-of-bounds elements are zero-filled.
-static int make_map_2d(CUtensorMap *map, const float *base, uint64_t rows, uint64_t cols, uint64_t pitch_elems,
-                       uint32_t box_rows) {
-    EncodeTiledFn fn = encode_tiled_fn();
-    if (!fn) { set_error("cuTensorMapEncodeTiled entry point not available"); return PTGNN_E_CUDA; }
-    const cuuint64_t dims[2] = {cols, rows};
-    const cuuint64_t strides[1] = {pitch_elems * sizeof(float)};
-    const cuuint32_t box[2] = {(cuuint32_t)CHUNK_K, box_rows};
-    const cuuint32_t estr[2] = {1, 1};
-    const CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(base), dims, strides, box, estr,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed with CUresult %d", (int)r); return PTGNN_E_CUDA; }
-    return PTGNN_OK;
-}
+constexpr CUtensorMapDataType F32 = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
 
 // =================================================================================================
 // weight preparation: fp32 -> (hi, lo) TF32 pairs, optionally re-packed for the GRU gate blocks
@@ -71,6 +37,14 @@ __global__ void split_weights_kernel(const __grid_constant__ SplitSrc s, float *
 __global__ void pack_gru_bias_kernel(const float *__restrict__ b_ih, const float *__restrict__ b_hh, int H, float4 *__restrict__ bias4) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j < H) bias4[j] = make_float4(b_ih[j] + b_hh[j], b_ih[H + j] + b_hh[H + j], b_ih[2 * H + j], b_hh[2 * H + j]);
+}
+int pack_gru_bias(const float *b_ih, const float *b_hh, int H, float4 *bias4, cudaStream_t st) {
+    {
+        TimedScope timed__(PTGNN_KERNEL_PACK, st);
+        pack_gru_bias_kernel<<<(H + 127) / 128, 128, 0, st>>>(b_ih, b_hh, H, bias4);
+    }
+    PTGNN_LAUNCHED();
+    return PTGNN_OK;
 }
 
 __global__ void pack_split_gru_kernel(const float *__restrict__ w_ih, const float *__restrict__ w_hh, int H, int D,
@@ -107,8 +81,7 @@ struct MsgPolicy {
         const float *h, *h_tgt;           // rows indexed by src32 / by tgt32
         const int32_t *src32, *tgt32, *pos;
         float *msg;
-        int H, D, Kw, use_target, num_types, n_blocks, dbg, store_hint;
-        unsigned long long *trace;
+        int H, D, Kw, use_target, num_types, n_blocks;
         int32_t edge_off[PTGNN_MAX_EDGE_TYPES + 1];
         int32_t tile_off[PTGNN_MAX_EDGE_TYPES + 1];
     };
@@ -159,12 +132,11 @@ struct MsgPolicy {
     }
     __device__ static void store(const Params &p, const Tile &ti, float (&acc)[64], const Pre &pre, int half, int lane, float *stage) {
         const long long row_off = pre.pos >= 0 ? (long long)pre.pos * p.D + ti.n0 : -1;
-        const uint64_t policy = p.store_hint ? l2_policy_evict_first() : 0;
 #pragma unroll
         for (int cb = 0; cb < 2; ++cb) {
             const int c0 = 64 * half + 32 * cb;
-            if (ti.b_rows - c0 >= 32) warp_store_rows<32>(stage, &acc[32 * cb], p.msg + c0, row_off, lane, policy);
-            else if (ti.b_rows - c0 >= 16) warp_store_rows<16>(stage, &acc[32 * cb], p.msg + c0, row_off, lane, policy);   // D % 32 == 16
+            if (ti.b_rows - c0 >= 32) warp_store_rows<32>(stage, &acc[32 * cb], p.msg + c0, row_off, lane);
+            else if (ti.b_rows - c0 >= 16) warp_store_rows<16>(stage, &acc[32 * cb], p.msg + c0, row_off, lane);   // D % 32 == 16
         }
     }
 };
@@ -180,8 +152,7 @@ struct GruPolicy {
         const float *h;
         const float4 *bias4;
         float *out;
-        int num_nodes, H, D, n_jb, dbg;
-        unsigned long long *trace;
+        int num_nodes, H, D, n_jb;
     };
     struct Tile { int row0, jb; };
 
@@ -257,8 +228,7 @@ struct DensePolicy {
         CUtensorMap map_y, map_w_hi, map_w_lo;   // [N, D] box {32,128}; [Hout, D] box {32, min(128, Hout)}
         const float *bias;
         float *out;
-        int num_nodes, D, Hout, act, n_blocks, dbg;
-        unsigned long long *trace;
+        int num_nodes, D, Hout, act, n_blocks;
     };
     struct Tile { int row0, n0, b_rows; };
 
@@ -312,53 +282,6 @@ struct DensePolicy {
 // =================================================================================================
 // launchers
 // =================================================================================================
-static int sm_count() {   // of the CURRENT device: a process may drive several GPUs (nothing cached across devices)
-    int dev = 0, n = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
-    return n;
-}
-
-int l2_hint_flags() {   // PTGNN_L2_HINTS bitmask (default 0): 1 = message stores, 4 = reduce loads with an L2 evict-first policy
-    static int v = -1;
-    if (v < 0) { const char *e = getenv("PTGNN_L2_HINTS"); v = e ? atoi(e) : 0; }
-    return v;
-}
-
-static int debug_flags() {
-    static int v = -1;
-    if (v < 0) { const char *e = getenv("PTGNN_TC_DEBUG"); v = e ? atoi(e) : 0; }
-    return v;
-}
-
-// PTGNN_TC_TRACE=<category>: timeline trace of CTA 0 for launches of that kernel category; read it back with
-// ptgnn_b200_debug_trace() (debug only, not part of the public header).
-static unsigned long long *g_trace_dev = nullptr;
-unsigned long long *trace_buffer(int category) {
-    static int want = -2;
-    if (want == -2) { const char *e = getenv("PTGNN_TC_TRACE"); want = e ? atoi(e) : -1; }
-    if (want != category) return nullptr;
-    if (!g_trace_dev) { if (cudaMalloc(&g_trace_dev, 3 * 2048 * 8) != cudaSuccess) return nullptr; }
-    cudaMemset(g_trace_dev, 0, 3 * 2048 * 8);
-    return g_trace_dev;
-}
-
-template <class Policy>
-static int launch_pipeline(typename Policy::Params &p, int total_tiles, int category, cudaStream_t st) {
-    if (total_tiles <= 0) return PTGNN_OK;
-    p.dbg = debug_flags();
-    p.trace = trace_buffer(category);
-    // per launch, not once per process: the attribute is per device (and per context)
-    PTGNN_CUDA(cudaFuncSetAttribute(tc_pipeline_kernel<Policy>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    const int sms = sm_count();
-    const int grid = total_tiles < sms ? total_tiles : sms;
-    {
-        TimedScope timed__(category, st);
-        tc_pipeline_kernel<Policy><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(p);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
-}
-
 size_t split_edge_weights_bytes(int num_types, int D, int Kw) { return 2 * ws_slice((size_t)num_types * D * Kw, 4); }
 size_t gru_pack_bytes(int H, int D) { return 2 * ws_slice((size_t)(H / 32) * 128 * D, 4) + 2 * ws_slice((size_t)(H / 32) * 128 * H, 4) + ws_slice((size_t)H * 4, 4); }
 size_t dense_split_bytes(int Hout, int D) { return 2 * ws_slice((size_t)Hout * D, 4); }
@@ -385,20 +308,13 @@ int edge_messages(const float *h_src, const float *h_tgt, int H, int D, int use_
     }
 
     MsgPolicy::Params p{};
-    int rc = make_map_2d(&p.map_w_hi, w_hi, (uint64_t)num_types * D, Kw, Kw, D < 128 ? D : 128);
-    if (!rc) rc = make_map_2d(&p.map_w_lo, w_lo, (uint64_t)num_types * D, Kw, Kw, D < 128 ? D : 128);
+    int rc = make_tensor_map_2d(&p.map_w_hi, F32, w_hi, (uint64_t)num_types * D, Kw, Kw, CHUNK_K, D < 128 ? D : 128);
+    if (!rc) rc = make_tensor_map_2d(&p.map_w_lo, F32, w_lo, (uint64_t)num_types * D, Kw, Kw, CHUNK_K, D < 128 ? D : 128);
     if (rc) return rc;
     p.h = h_src; p.h_tgt = h_tgt; p.src32 = src32; p.tgt32 = tgt32; p.pos = pos; p.msg = msg;
     p.H = H; p.D = D; p.Kw = Kw; p.use_target = use_target; p.num_types = num_types; p.n_blocks = (D + 127) / 128;
-    p.store_hint = (l2_hint_flags() & 1) ? 1 : 0;
-    int tiles = 0;
-    for (int t = 0; t < num_types; ++t) {
-        p.edge_off[t] = (int32_t)type_off[t];
-        p.tile_off[t] = tiles;
-        tiles += (int)ceil_div(type_off[t + 1] - type_off[t], TILE_M);
-    }
-    for (int t = num_types; t <= PTGNN_MAX_EDGE_TYPES; ++t) { p.edge_off[t] = (int32_t)type_off[num_types]; p.tile_off[t] = tiles; }
-    return launch_pipeline<MsgPolicy>(p, tiles * p.n_blocks, PTGNN_KERNEL_MESSAGE, st);
+    const int tiles = build_type_tiles(type_off, num_types, TILE_M, p.edge_off, p.tile_off);
+    return launch_pipeline(tc_pipeline_kernel<MsgPolicy>, p, SMEM_BYTES, tiles * p.n_blocks, PTGNN_KERNEL_MESSAGE, st);
 }
 
 int gru_update(const float *agg, const float *h, int64_t num_nodes, int H, int D, const float *w_ih, const float *w_hh,
@@ -414,25 +330,22 @@ int gru_update(const float *agg, const float *h, int64_t num_nodes, int H, int D
             pack_split_gru_kernel<<<132, 256, 0, st>>>(w_ih, w_hh, H, D, p1_hi, p1_lo, p2_hi, p2_lo);
         }
         PTGNN_LAUNCHED();
-        {
-            TimedScope timed__(PTGNN_KERNEL_PACK, st);
-            pack_gru_bias_kernel<<<(H + 127) / 128, 128, 0, st>>>(b_ih, b_hh, H, bias4);
-        }
-        PTGNN_LAUNCHED();
+        const int rc = pack_gru_bias(b_ih, b_hh, H, bias4, st);
+        if (rc) return rc;
     }
     GruPolicy::Params p{};
     const uint64_t prow = (uint64_t)(H / 32) * 128;
-    int rc = make_map_2d(&p.map_agg, agg, num_nodes, D, D, 128);
-    if (!rc) rc = make_map_2d(&p.map_h, h, num_nodes, H, H, 128);
-    if (!rc) rc = make_map_2d(&p.map_p1_hi, p1_hi, prow, D, D, 128);
-    if (!rc) rc = make_map_2d(&p.map_p1_lo, p1_lo, prow, D, D, 128);
-    if (!rc) rc = make_map_2d(&p.map_p2_hi, p2_hi, prow, H, H, 128);
-    if (!rc) rc = make_map_2d(&p.map_p2_lo, p2_lo, prow, H, H, 128);
+    int rc = make_tensor_map_2d(&p.map_agg, F32, agg, num_nodes, D, D, CHUNK_K, 128);
+    if (!rc) rc = make_tensor_map_2d(&p.map_h, F32, h, num_nodes, H, H, CHUNK_K, 128);
+    if (!rc) rc = make_tensor_map_2d(&p.map_p1_hi, F32, p1_hi, prow, D, D, CHUNK_K, 128);
+    if (!rc) rc = make_tensor_map_2d(&p.map_p1_lo, F32, p1_lo, prow, D, D, CHUNK_K, 128);
+    if (!rc) rc = make_tensor_map_2d(&p.map_p2_hi, F32, p2_hi, prow, H, H, CHUNK_K, 128);
+    if (!rc) rc = make_tensor_map_2d(&p.map_p2_lo, F32, p2_lo, prow, H, H, CHUNK_K, 128);
     if (rc) return rc;
     p.h = h; p.bias4 = bias4;
     p.out = out; p.num_nodes = (int)num_nodes; p.H = H; p.D = D; p.n_jb = H / 32;
     const int tiles = (int)ceil_div(num_nodes, TILE_M) * p.n_jb;
-    return launch_pipeline<GruPolicy>(p, tiles, PTGNN_KERNEL_GRU, st);
+    return launch_pipeline(tc_pipeline_kernel<GruPolicy>, p, SMEM_BYTES, tiles, PTGNN_KERNEL_GRU, st);
 }
 
 int dense_update(const float *y, int64_t num_nodes, int D, const float *W, const float *bias, int Hout, int act, float *out,
@@ -449,23 +362,15 @@ int dense_update(const float *y, int64_t num_nodes, int D, const float *W, const
         PTGNN_LAUNCHED();
     }
     DensePolicy::Params p{};
-    int rc = make_map_2d(&p.map_y, y, num_nodes, D, D, 128);
-    if (!rc) rc = make_map_2d(&p.map_w_hi, w_hi, Hout, D, D, Hout < 128 ? Hout : 128);
-    if (!rc) rc = make_map_2d(&p.map_w_lo, w_lo, Hout, D, D, Hout < 128 ? Hout : 128);
+    int rc = make_tensor_map_2d(&p.map_y, F32, y, num_nodes, D, D, CHUNK_K, 128);
+    if (!rc) rc = make_tensor_map_2d(&p.map_w_hi, F32, w_hi, Hout, D, D, CHUNK_K, Hout < 128 ? Hout : 128);
+    if (!rc) rc = make_tensor_map_2d(&p.map_w_lo, F32, w_lo, Hout, D, D, CHUNK_K, Hout < 128 ? Hout : 128);
     if (rc) return rc;
     p.bias = bias; p.out = out; p.num_nodes = (int)num_nodes; p.D = D; p.Hout = Hout;
     p.act = act; p.n_blocks = (Hout + 127) / 128;
     const int tiles = (int)ceil_div(num_nodes, TILE_M) * p.n_blocks;
-    return launch_pipeline<DensePolicy>(p, tiles, PTGNN_KERNEL_DENSE, st);
+    return launch_pipeline(tc_pipeline_kernel<DensePolicy>, p, SMEM_BYTES, tiles, PTGNN_KERNEL_DENSE, st);
 }
 
 }  // namespace tc
 }  // namespace ptgnn
-
-// debug only: copies the last timeline trace (3 x 2048 uint64) to `out`; returns 0 if tracing is off
-extern "C" int ptgnn_b200_debug_trace(unsigned long long *out) {
-    if (!ptgnn::tc::g_trace_dev) return 0;
-    cudaDeviceSynchronize();
-    cudaMemcpy(out, ptgnn::tc::g_trace_dev, 3 * 2048 * 8, cudaMemcpyDeviceToHost);
-    return 1;
-}

@@ -5,16 +5,16 @@
 namespace ptgnn {
 namespace tc {
 
-int l2_hint_flags();
 bool supported_message(int H, int D);
 bool supported_gru(int H, int D);
 bool supported_dense(int D, int Hout);
 
 size_t split_edge_weights_bytes(int num_types, int D, int Kw);
 size_t gru_pack_bytes(int H, int D);
-// debug: device buffer for a CTA-0 timeline when PTGNN_TC_TRACE == category (else nullptr); bf16 kernels use category + 10
-unsigned long long *trace_buffer(int category);
 size_t dense_split_bytes(int Hout, int D);
+
+// bias4[j] = (b_ir + b_hr, b_iz + b_hz, b_in, b_hn) for j < H: the GRU epilogues' biases (fp32 and bf16 pipelines)
+int pack_gru_bias(const float *b_ih, const float *b_hh, int H, float4 *bias4, cudaStream_t st);
 
 // `pack` = derive the TF32 (hi, lo) / gate-blocked copies of the weights into `scratch` first; false when `scratch` is a
 // caller-owned weight cache that already holds them (same weights as the call that filled it).

@@ -1,8 +1,6 @@
 // Dispatch + C ABI for the segmented reduce (see reduce.cuh) and the one-shot torch_scatter.scatter drop-in.
 #include "reduce.cuh"
 
-#include "layers_tc.cuh"
-
 namespace ptgnn {
 
 template <int RED, int LPR, int CHUNKS>
@@ -41,7 +39,6 @@ static int launch_stream(const float *msg, const int32_t *row_ptr, const int32_t
     const unsigned grid = (unsigned)ceil_div(N, 8 * 16);   // 8 warps x 16 rows per block
     ReduceEpilogue e{};
     if (epi) e = *epi;
-    e.hint = (tc::l2_hint_flags() & 4) ? 1 : 0;
     {
         TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
         if (epi) segment_reduce_stream_kernel<RED, CHUNKS, true><<<grid, 256, 0, st>>>(msg, row_ptr, perm, (int)N, D, out, e);

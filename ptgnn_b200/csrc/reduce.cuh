@@ -17,7 +17,6 @@
 namespace ptgnn {
 
 struct ReduceEpilogue {
-    int hint;            // != 0: read the message rows with an L2 evict-first policy (they are dead afterwards)
     int act;             // PTGNN_ACT_* applied to the aggregated row
     const float *ln_w;   // LayerNorm weight/bias (nullptr = no LayerNorm)
     const float *ln_b;
@@ -204,7 +203,6 @@ segment_reduce_stream_kernel(const float *__restrict__ msg, const int32_t *__res
     const size_t ld4 = (size_t)D / 4;
     const float4 *msg4 = reinterpret_cast<const float4 *>(msg);
     float4 *out4 = reinterpret_cast<float4 *>(out);
-    const uint64_t evict_first = l2_policy_evict_first();   // message rows are dead after this read
 
     int cur = 0;                                                    // row being accumulated (index inside the warp's block)
     int cur_end = __shfl_sync(0xffffffffu, bound, 1);
@@ -213,7 +211,8 @@ segment_reduce_stream_kernel(const float *__restrict__ msg, const int32_t *__res
         if (RED == PTGNN_REDUCE_MEAN) {
             const float cnt = (float)(count < 1 ? 1 : count);
 #pragma unroll
-            for (int c = 0; c < CHUNKS; ++c) { acc[c].x /= cnt; acc[c].y /= cnt; acc[c].z /= cnt; acc[c].w /= cnt; }
+            for (int c = 0; c < CHUNKS; ++c)   // own columns only: a division is a few dozen instructions and registers
+                if (col_ok[c]) { acc[c].x /= cnt; acc[c].y /= cnt; acc[c].z /= cnt; acc[c].w /= cnt; }
         }
         if (RED == PTGNN_REDUCE_MAX || RED == PTGNN_REDUCE_MIN) {   // never updated (values equal to the initial one never win) -> 0
             const float init = RED == PTGNN_REDUCE_MAX ? -FLT_MAX : FLT_MAX;
@@ -279,8 +278,7 @@ segment_reduce_stream_kernel(const float *__restrict__ msg, const int32_t *__res
                 const size_t row = perm != nullptr ? (size_t)__shfl_sync(0xffffffffu, my_row, u) : (size_t)(j + u);
 #pragma unroll
                 for (int c = 0; c < CHUNKS; ++c)
-                    if (col_ok[c]) m[u][c] = epi.hint ? ld_stream_f4_hint(msg4 + row * ld4 + c * 32 + lane, evict_first)
-                                                      : ld_stream_f4(msg4 + row * ld4 + c * 32 + lane);
+                    if (col_ok[c]) m[u][c] = ld_stream_f4(msg4 + row * ld4 + c * 32 + lane);
             }
         }
 #pragma unroll

@@ -108,16 +108,8 @@ __device__ __forceinline__ void named_bar_arrive(int id, int threads) { asm vola
 // different 128-byte lines.  Staging 32 rows x NCOLS through a (chunk-XOR-swizzled) buffer lets each store
 // instruction write whole rows: 4 (NCOLS = 32) or 8 (NCOLS = 16) lines per instruction instead of 32.
 // `row_off` is this lane's destination element offset from `dst_base` (negative = row not stored).
-__device__ __forceinline__ void st_global_f4(float *dst, const float4 &v, uint64_t policy) {
-    if (policy == 0) { *reinterpret_cast<float4 *>(dst) = v; return; }
-    asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(dst), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "l"(policy)
-                 : "memory");
-}
-// `policy` != 0: an L2 cache policy (createpolicy) for the stores, e.g. evict-first for the message rows -- they are
-// written once and read once by the reduce, and must not push the gathered node states out of L2.
 template <int NCOLS>
-__device__ __forceinline__ void warp_store_rows(float *stage, const float *v, float *dst_base, long long row_off, int lane,
-                                                uint64_t policy = 0) {
+__device__ __forceinline__ void warp_store_rows(float *stage, const float *v, float *dst_base, long long row_off, int lane) {
     constexpr int CPR = NCOLS / 4;   // 16-byte chunks per row
 #pragma unroll
     for (int j = 0; j < CPR; ++j)
@@ -129,7 +121,7 @@ __device__ __forceinline__ void warp_store_rows(float *stage, const float *v, fl
         const int idx = it * 32 + lane, row = idx / CPR, ch = idx % CPR;
         const float4 val = *reinterpret_cast<const float4 *>(stage + (row * CPR + (ch ^ (row & (CPR - 1)))) * 4);
         const long long off = __shfl_sync(0xffffffffu, row_off, row);
-        if (off >= 0) st_global_f4(dst_base + off + ch * 4, val, policy);
+        if (off >= 0) *reinterpret_cast<float4 *>(dst_base + off + ch * 4) = val;
     }
     __syncwarp();
 }
@@ -157,15 +149,6 @@ __device__ __forceinline__ void drain_4x16(const float *row, int off, float (&ac
         }
 }
 
-// Optional timeline trace (PTGNN_TC_TRACE): CTA 0 records %globaltimer at pipeline hand-offs into 3 x 2048 slots.
-struct Tracer {
-    unsigned long long *buf;
-    int n, cap;
-    __device__ __forceinline__ void mark(int tag) {
-        if (buf != nullptr && n < cap) { buf[n++] = (global_timer_ns() << 8) | (unsigned long long)(tag & 0xFF); }
-    }
-};
-
 template <class Policy>
 __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __grid_constant__ typename Policy::Params p) {
     extern __shared__ unsigned char smem_raw[];
@@ -192,9 +175,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
     }
     __syncthreads();
     const int total_tiles = Policy::num_tiles(p);
-    // timing experiments only (PTGNN_TC_DEBUG; results are wrong when set): 1 = no MMAs, 2 = no loads, 4 = no stores
-    const int dbg = p.dbg;
-    unsigned long long *trace_base = (p.trace != nullptr && blockIdx.x == 0) ? p.trace : nullptr;
 
     if (warp < FIRST_CONSUMER_WARP) {
         reg_dealloc<PRODUCER_REGS>();
@@ -219,12 +199,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
                         mbar_wait(&empty[slot], (use & 1) ^ 1);
                         unsigned char *base = ring + slot * SLOT_BYTES;
                         const int kchunk = kc * CHUNK_K;
-                        const bool go = !(dbg & 2);
-                        if (!go && leader) mbar_arrive(&landed[slot]);
-                        if (go && leader) mbar_expect_tx(&landed[slot], bytes);
-                        if (go && sg.a_map != nullptr && leader) tma_load_2d(base, sg.a_map, kchunk, sg.a_row0, &landed[slot]);
-                        if (go && leader) tma_load_2d(base + B_HI_OFF, sg.b_hi_map, sg.b_col0 + kchunk, sg.b_row0, &landed[slot]);
-                        if (go && leader) tma_load_2d(base + B_LO_OFF, sg.b_lo_map, sg.b_col0 + kchunk, sg.b_row0, &landed[slot]);
+                        if (leader) mbar_expect_tx(&landed[slot], bytes);
+                        if (sg.a_map != nullptr && leader) tma_load_2d(base, sg.a_map, kchunk, sg.a_row0, &landed[slot]);
+                        if (leader) tma_load_2d(base + B_HI_OFF, sg.b_hi_map, sg.b_col0 + kchunk, sg.b_row0, &landed[slot]);
+                        if (leader) tma_load_2d(base + B_LO_OFF, sg.b_lo_map, sg.b_col0 + kchunk, sg.b_row0, &landed[slot]);
                         __syncwarp();
                     }
                 }
@@ -237,7 +215,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
             // shared memory (two buffers); those of the next one are fetched from global memory one step ahead.
             const int g = (int)threadIdx.x - FIRST_GATHER_WARP * 32;
             const int q = g & 7, rsub = g >> 3;
-            Tracer tr{(trace_base && g == 0) ? trace_base + 1024 : nullptr, 0, 1024};
             uint32_t c = 0;
             int buf = 0;
             typename Policy::Tile t, t_next;
@@ -280,19 +257,15 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
                 const uint32_t soff = swz(rsub, q);     // rows rsub + 8 i share (row & 7): the swizzle term is per-thread constant
                 for (int kc = 0; kc < nkc; ++kc, ++c) {
                     const uint32_t slot = c % NUM_SLOTS, use = c / NUM_SLOTS;
-                    tr.mark(1);
                     mbar_wait(&a_free[slot], (use & 1) ^ 1);
-                    tr.mark(2);
                     const int kchunk = kc * CHUNK_K;
                     const bool k_ok = kchunk + q * 4 < sg.K;
                     const uint32_t sbase = smem_u32(ring + slot * SLOT_BYTES) + soff;
-                    if (!(dbg & 2)) {
 #pragma unroll
-                        for (int i = 0; i < 16; ++i) {
-                            const bool ok = k_ok && rows[i] >= 0;
-                            const float *src = ok ? a_q + (size_t)rows[i] * sg.lda + kchunk : sg.a;
-                            cp_async16(sbase + i * 1024, src, ok ? 16 : 0);
-                        }
+                    for (int i = 0; i < 16; ++i) {
+                        const bool ok = k_ok && rows[i] >= 0;
+                        const float *src = ok ? a_q + (size_t)rows[i] * sg.lda + kchunk : sg.a;
+                        cp_async16(sbase + i * 1024, src, ok ? 16 : 0);
                     }
                     cp_async_mbar_arrive_noinc(&landed[slot]);
                 }
@@ -311,10 +284,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
         // epilogue role of this warp: rows 32 quarter .. (inside the warpgroup's 64 rows), columns of `half`
         const int quarter = 2 * wg + (wi & 1), half = wi >> 1;
         const float *acc_row = acc_s + (quarter * 32 + lane) * ACC_PITCH;
-        float *stage = acc_s + wg * 64 * ACC_PITCH + wi * STAGE_FLOATS_PER_WARP;
         const int bar_id = 2 + wg;                        // named barrier of this warpgroup's 128 threads
         uint32_t c = 0;
-        Tracer tr{(trace_base && cw == 0 && lane == 0) ? trace_base + 2048 : nullptr, 0, 2048};
         typename Policy::Tile t, t_next;
         // What the store needs from global memory (destination offsets, the GRU's h values) is fetched one tile ahead.
         typename Policy::Pre pre, pre_next;
@@ -344,9 +315,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
                 const int nkc = (sg.K + CHUNK_K - 1) / CHUNK_K;
                 for (int kc = 0; kc < nkc; ++kc, ++c) {
                     const uint32_t slot = c % NUM_SLOTS, use = c / NUM_SLOTS;
-                    tr.mark(13);
                     mbar_wait(&landed[slot], use & 1);
-                    tr.mark(14);
                     const unsigned char *base = ring + slot * SLOT_BYTES;
                     // A fragment of K-step ks: rows r0 / r1, columns 8 ks + tq and 8 ks + tq + 4 -> TF32 hi / lo
                     uint32_t a_hi[4][4], a_lo[4][4];
@@ -367,7 +336,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
                         if (lane == 0) mbar_arrive(&a_free[slot]);       // raw tile consumed (values are in registers)
                     }
                     const int kvalid = min(CHUNK_K, sg.K - kc * CHUNK_K);
-                    const int ksteps = (dbg & 1) ? 0 : (kvalid + 7) / 8;
+                    const int ksteps = (kvalid + 7) / 8;
                     const uint32_t sbase = smem_u32(base);
                     wgmma_fence();
 #pragma unroll
@@ -399,7 +368,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
                     for (int j = 0; j < 4; ++j) { fence_acc(acc_m[j]); fence_acc(acc_c[j]); }
                     __syncwarp();
                     if (lane == 0) mbar_arrive(&empty[slot]);            // B tiles of the slot consumed
-                    tr.mark(15);
                 }
             }
             // ---- accumulator tile -> shared memory (main + correction), then the policy epilogue, one row per thread
@@ -418,13 +386,30 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
             float acc[64];
             Policy::drain(p, t, acc_row, half, acc);
             named_bar_sync(bar_id, 128);          // drained: the rows become the warps' transpose buffers
-            tr.mark(22);
-            if (!(dbg & 4)) Policy::store(p, t, acc, pre, half, lane, stage);
-            tr.mark(23);
+            // this warp's transpose buffer, addressed here rather than held across the tile loop: a pointer live through the
+            // MMAs made the GRU epilogue spill
+            Policy::store(p, t, acc, pre, half, lane, acc_s + wg * 64 * ACC_PITCH + wi * STAGE_FLOATS_PER_WARP);
             t = t_next;
             pre = pre_next;
         }
     }
+}
+
+// Host launch of either round-1 pipeline (tc_pipeline_kernel / tc_pipeline_bf16_kernel): one persistent CTA per SM, no more
+// CTAs than tiles.
+template <class Params>
+static int launch_pipeline(void (*kernel)(Params), const Params &p, int smem_bytes, int total_tiles, int category, cudaStream_t st) {
+    if (total_tiles <= 0) return PTGNN_OK;
+    // per launch, not once per process: the attribute is per device (and per context)
+    PTGNN_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+    const int sms = sm_count();
+    const int grid = total_tiles < sms ? total_tiles : sms;
+    {
+        TimedScope timed__(category, st);
+        kernel<<<grid, NUM_THREADS, smem_bytes, st>>>(p);
+    }
+    PTGNN_LAUNCHED();
+    return PTGNN_OK;
 }
 
 }  // namespace tc

@@ -31,7 +31,7 @@ constexpr int LOOKAHEAD = 2;
 constexpr int OPERAND_BYTES = TILE_M * 128;        // 16 KB
 constexpr int SLOT_BYTES = 2 * OPERAND_BYTES;      // A | B
 constexpr int RING_BYTES = NUM_SLOTS * SLOT_BYTES;
-constexpr int NUM_THREADS = 12 * 32;
+constexpr int NUM_THREADS = tc::NUM_THREADS;      // tc::launch_pipeline launches both pipelines with this block size
 constexpr int NUM_CONSUMER_WARPS = 8;
 constexpr int STAGE_BYTES_PER_WARP = 32 * 32 * 4;
 constexpr int ACC_PITCH = tc::ACC_PITCH;
@@ -70,14 +70,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_bf16_kernel(const 
     Policy::smem_init(p, stage_base);          // policy-owned tables in the staging area (e.g. the GRU biases)
     __syncthreads();
     const int total_tiles = Policy::num_tiles(p);
-    unsigned long long *trace_base = (p.trace != nullptr && blockIdx.x == 0) ? p.trace : nullptr;
 
     if (warp < 4) {
         // =========================================== LOADERS ===========================================
         tc::reg_dealloc<LOADER_REGS>();
         const int q = lane & 7, rsub = warp * 32 + (lane >> 3);
         const bool tma_leader = warp == 0 && tc::elect_one();   // issues the bulk tensor copies (uniform operands)
-        tc::Tracer tr{(trace_base && tma_leader) ? trace_base : nullptr, 0};
         constexpr int PPT = 8;
         struct Cursor { int tile, seg, kc; };
         typename Policy::Tile t_load, t_pref, t_proc;
@@ -129,23 +127,20 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_bf16_kernel(const 
 
         auto issue = [&]() {
             const uint32_t slot = c_load % NUM_SLOTS, use = c_load / NUM_SLOTS;
-            tr.mark(1);
             mbar_wait(&empty[slot], (use & 1) ^ 1);
-            tr.mark(2);
             unsigned char *base = ring + slot * SLOT_BYTES;
             const Segment &sg = sg_load;
             const int kchunk = cl.kc * CHUNK_K;
             if (warp == 0) {   // single predicated statements on warp-uniform operands: no R2UR waterfall around the TMA issue
-                const bool go = !(p.dbg & 4);
                 const CUtensorMap *am = tc::warp_uniform(sg.a_map), *bm = tc::warp_uniform(sg.b_map);
                 const int a_row0 = tc::warp_uniform(sg.a_row0), b_row0 = tc::warp_uniform(sg.b_row0);
                 const int b_col = tc::warp_uniform(sg.b_col0 + kchunk), a_col = tc::warp_uniform(kchunk);
                 const uint32_t bytes = tc::warp_uniform((uint32_t)sg.b_box_rows * 128u + (am != nullptr ? (uint32_t)OPERAND_BYTES : 0u));
-                if (go && tma_leader) tc::mbar_expect_tx(&landed[slot], bytes);
-                if (go && am != nullptr && tma_leader) tc::tma_load_2d(base, am, a_col, a_row0, &landed[slot]);
-                if (go && tma_leader) tc::tma_load_2d(base + OPERAND_BYTES, bm, b_col, b_row0, &landed[slot]);
+                if (tma_leader) tc::mbar_expect_tx(&landed[slot], bytes);
+                if (am != nullptr && tma_leader) tc::tma_load_2d(base, am, a_col, a_row0, &landed[slot]);
+                if (tma_leader) tc::tma_load_2d(base + OPERAND_BYTES, bm, b_col, b_row0, &landed[slot]);
             }
-            if (sg.a_map == nullptr && !(p.dbg & 4)) {
+            if (sg.a_map == nullptr) {
                 const bool k_ok = kchunk + q * 8 < sg.K;
                 const uint32_t sbase = smem_u32(base);
 #pragma unroll
@@ -175,12 +170,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_bf16_kernel(const 
             cp_async_commit();
         }
         while (proc_valid) {
-            tr.mark(3);
             cp_async_wait<LOOKAHEAD - 1>();           // this thread's gathered pieces of chunk c_proc have landed
             tc::fence_proxy_async_smem();             // ... and are visible to the tensor core (async proxy)
-            tr.mark(4);
             mbar_arrive(&full[c_proc % NUM_SLOTS]);
-            tr.mark(6);
             ++c_proc;
             if (load_valid) issue();
             cp_async_commit();
@@ -206,7 +198,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_bf16_kernel(const 
         typename Policy::Tile t, t_next;
         // Everything the store needs from global memory (destination offsets, the GRU's h values) is fetched one tile ahead.
         typename Policy::Pre pre, pre_next;
-        tc::Tracer tr{(trace_base && cw == 0 && lane == 0) ? trace_base + 2048 : nullptr, 0, 2048};
         int tile = blockIdx.x;
         Policy::tile_init(t);
         if (tile < total_tiles) {
@@ -233,12 +224,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_bf16_kernel(const 
                 const int nkc = (sg.K + CHUNK_K - 1) / CHUNK_K;
                 for (int kc = 0; kc < nkc; ++kc, ++c) {
                     const uint32_t slot = c % NUM_SLOTS, use = c / NUM_SLOTS;
-                    tr.mark(13);
                     mbar_wait(&full[slot], use & 1);
-                    if (!(p.dbg & 4)) mbar_wait(&landed[slot], use & 1);
-                    tr.mark(14);
+                    mbar_wait(&landed[slot], use & 1);
                     const uint32_t base = smem_u32(ring + slot * SLOT_BYTES);
-                    const int ksteps = (p.dbg & 1) ? 0 : (min(CHUNK_K, sg.K - kc * CHUNK_K) + 15) / 16;
+                    const int ksteps = (min(CHUNK_K, sg.K - kc * CHUNK_K) + 15) / 16;
                     const uint64_t a0 = tc::make_smem_desc_sw128(base + wg * 64 * 128);
                     tc::wgmma_fence();
 #pragma unroll
@@ -263,7 +252,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_bf16_kernel(const 
                     for (int j = 0; j < 4; ++j) tc::fence_acc(acc[j]);
                     __syncwarp();
                     if (lane == 0) mbar_arrive(&empty[slot]);
-                    tr.mark(15);
                 }
             }
             tc::named_bar_sync(bar_id, 128);      // the warpgroup's previous epilogue no longer reads these rows
@@ -277,10 +265,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_bf16_kernel(const 
                 }
             tc::named_bar_sync(bar_id, 128);
             float v[64];
-            if (!(p.dbg & 8)) Policy::drain(p, t, acc_row, half, v);
-            tr.mark(22);
-            if (!(p.dbg & 2)) Policy::store(p, t, v, pre, half, lane, stage, stage_base);
-            tr.mark(23);
+            Policy::drain(p, t, acc_row, half, v);
+            Policy::store(p, t, v, pre, half, lane, stage, stage_base);
             t = t_next;
             pre = pre_next;
         }

@@ -1,5 +1,5 @@
 """Kernel time of the fused aggregation / GRU kernels at config 2 (one Gated layer, library-side CUDA events):
-    PTGNN_FUSED_DBG=<bits> python tools/fused_time.py [f32|bf16] [label]"""
+    python tools/fused_time.py [f32|bf16] [label]"""
 import os
 import sys
 
@@ -36,4 +36,4 @@ with torch.no_grad():
     torch.cuda.synchronize()
     kt = N.read_kernel_timing()
     N.kernel_timing(False)
-print(f"{dtype} dbg={os.environ.get('PTGNN_FUSED_DBG', '0')} {label}: " + "  ".join(f"{k} {v[0] / max(v[1], 1):.4f} ms x{v[1]}" for k, v in kt.items() if v[1]))
+print(f"{dtype} {label}: " + "  ".join(f"{k} {v[0] / max(v[1], 1):.4f} ms x{v[1]}" for k, v in kt.items() if v[1]))
