@@ -370,6 +370,27 @@ int ptgnn_b200_global_gru_update(int32_t bf16_states, const void *node_states, c
                                  void *weight_cache, size_t weight_cache_bytes, int32_t cache_valid, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Attention readout (reference reduceops/varsizedsummary.py:84-178, SelfAttention / MultiheadSelfAttention reducers):
+ *   z_{n,h} = x_n . qt[b, h]  for the nodes n of graph b,
+ *   o[b, h] = sum_n softmax_n(z_{., h}) x_n  [G, heads, D] fp32,   lse[b, h] = log sum_n exp(z_{n,h})  [G, heads] fp32.
+ *   qt [G, heads, D] fp32 is the per-graph query folded through the key layer (W_{k,h}^T q_{b,h} / sqrt(d_h)).
+ *   x: fp32, or bf16 when bf16_states != 0 (fp32 arithmetic).  row_ptr / perm: the plan of the node -> graph map, as for
+ *   ptgnn_b200_graph_readout.  A graph without nodes gives o = 0 and lse = -inf.  Deterministic (DESIGN.md §3.7).
+ *   Supported: D in {32, 64, 128, 256}, heads in {1, 2, 4, 8} (ptgnn_b200_attention_readout_supported).
+ * attention_readout_backward_f32: from dO = dL/do [G, heads, D] and the forward's o and lse, writes d_x [N, D] (every node of
+ *   an in-range graph) and d_qt [G, heads, D].  fp32 states only.  The workspace size covers both calls.
+ * ---------------------------------------------------------------------------------------------- */
+int32_t ptgnn_b200_attention_readout_supported(int32_t bf16_states, int32_t state_dim, int32_t num_heads);
+size_t ptgnn_b200_attention_readout_workspace_bytes(int64_t num_nodes, int64_t num_graphs, int32_t state_dim, int32_t num_heads);
+int ptgnn_b200_attention_readout(int32_t bf16_states, const void *node_states, int64_t num_nodes, int32_t state_dim, int32_t num_heads,
+                                 const int32_t *row_ptr, const int32_t *perm, int64_t num_graphs, const float *qt, float *o, float *lse,
+                                 void *workspace, size_t workspace_bytes, void *stream);
+int ptgnn_b200_attention_readout_backward_f32(const float *node_states, int64_t num_nodes, int32_t state_dim, int32_t num_heads,
+                                              const int32_t *row_ptr, const int32_t *perm, int64_t num_graphs, const float *qt,
+                                              const float *o, const float *lse, const float *d_o, float *d_x, float *d_qt,
+                                              void *workspace, size_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Host-buffer convenience entry point (used for the end-to-end measurement): all pointers are HOST
  * memory; copies inputs to the device, builds the plan, runs `num_layers` GatedMessagePassingLayers
  * (layer l uses weight set l; pass the same pointers to share weights), copies the final states back

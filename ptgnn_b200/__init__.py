@@ -21,6 +21,8 @@ from .messagepassing import (
 from .reduceops import (
     AbstractVarSizedElementReduce,
     ElementsToSummaryRepresentationInput,
+    MultiheadSelfAttentionVarSizedElementReduce,
+    SelfAttentionVarSizedElementReduce,
     SimpleVarSizedElementReduce,
     WeightedSumVarSizedElementReduce,
 )
@@ -32,6 +34,7 @@ __all__ = [
     "PnaMessageAggregation", "AbstractMessagePassingLayer", "GatedMessagePassingLayer", "MlpMessagePassingLayer", "EGCMessagePassingLayer", "MeanResidualLayer",
     "ConcatResidualLayer", "LinearResidualLayer", "MinibatchAssembler", "scatter", "scatter_add",
     "AbstractGlobalGraphExchange", "GruGlobalStateUpdate", "AbstractVarSizedElementReduce", "ElementsToSummaryRepresentationInput",
-    "SimpleVarSizedElementReduce", "WeightedSumVarSizedElementReduce",
+    "SimpleVarSizedElementReduce", "WeightedSumVarSizedElementReduce", "SelfAttentionVarSizedElementReduce",
+    "MultiheadSelfAttentionVarSizedElementReduce",
     "scatter_sum", "scatter_mean", "scatter_max", "scatter_min",
 ]

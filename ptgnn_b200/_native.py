@@ -85,6 +85,12 @@ SIGNATURES = {
     "ptgnn_b200_global_gru_update": (ctypes.c_int, [c_i32, c_void_p, c_void_p, c_i64, c_i32, c_void_p, c_i64, c_void_p, c_i32, c_void_p, c_void_p,
                                                     c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_size_t,
                                                     c_i32, c_void_p]),
+    "ptgnn_b200_attention_readout_supported": (c_i32, [c_i32, c_i32, c_i32]),
+    "ptgnn_b200_attention_readout_workspace_bytes": (c_size_t, [c_i64, c_i64, c_i32, c_i32]),
+    "ptgnn_b200_attention_readout": (ctypes.c_int, [c_i32, c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_i64, c_void_p, c_void_p,
+                                                    c_void_p, c_void_p, c_size_t, c_void_p]),
+    "ptgnn_b200_attention_readout_backward_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_i64, c_void_p, c_void_p,
+                                                                 c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "ptgnn_b200_gated_gnn_forward_host_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_i32,
                                                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i32, c_void_p]),
 }

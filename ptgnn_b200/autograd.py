@@ -508,3 +508,35 @@ class _GlobalGruFn(torch.autograd.Function):
 
 def global_gru_with_grad(layer, node_states, summaries, plan, w_ih, w_hh, b_ih, b_hh):
     return _GlobalGruFn.apply(layer, plan, node_states, summaries, w_ih, w_hh, b_ih, b_hh)
+
+
+# =====================================================================================================================
+# Attention readout (varsizedsummary.py:84-178): o[b, h] = sum_n softmax_n(x_n . qt[b, h]) x_n on the native kernel; the G-row products
+# around it (qt from the queries and the key weight, value and output layers) are _LinearFn's.  fp32 states.
+# =====================================================================================================================
+class _AttentionReadoutFn(torch.autograd.Function):
+    """o [G, heads, D] from x [N, D] and qt [G, heads, D]; backward: d x and d qt on the native backward kernel (p re-computed from
+    the saved lse, no [N, heads] tensor kept)."""
+
+    @staticmethod
+    def forward(ctx, plan, heads, x, qt):
+        from .reduceops import native_attention_readout
+
+        xd, qd = x.detach().contiguous(), qt.detach().contiguous()
+        o, lse = native_attention_readout(xd, plan, qd, heads)
+        ctx.save_for_backward(xd, qd, o, lse)
+        ctx.plan = plan
+        return o
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, d_o):
+        from .reduceops import native_attention_readout_backward
+
+        x, qt, o, lse = ctx.saved_tensors
+        d_x, d_qt = native_attention_readout_backward(x, ctx.plan, qt, o, lse, d_o.contiguous().float())
+        return None, None, d_x, d_qt
+
+
+def attention_readout_with_grad(plan, heads, node_states, qt):
+    return _AttentionReadoutFn.apply(plan, heads, node_states, qt)

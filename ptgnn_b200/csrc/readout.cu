@@ -17,11 +17,11 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "readout.cuh"
 
 namespace ptgnn {
 namespace readout {
 
-constexpr int CHUNK = 32;           // rows per warp-chunk (DESIGN §3.5: the test bounds take gamma_{CHUNK + chunks} from it)
 constexpr int ROWS_AHEAD = 4;       // rows whose loads a warp issues before it consumes the first of them
 
 __global__ void __launch_bounds__(1024) readout_chunk_ptr_kernel(const int32_t *__restrict__ row_ptr, int G, int32_t *__restrict__ chunk_ptr) {
@@ -135,6 +135,14 @@ __global__ void __launch_bounds__(256) readout_finalize_kernel(const float *__re
     g[i] = acc;
 }
 
+void launch_chunk_ptr(const int32_t *row_ptr, int G, int32_t *chunk_ptr, cudaStream_t st) {
+    readout_chunk_ptr_kernel<<<1, 1024, 0, st>>>(row_ptr, G, chunk_ptr);
+}
+
+void launch_chunk_sum(const float *partial, const int32_t *row_ptr, const int32_t *chunk_ptr, int G, int width, float *out, cudaStream_t st) {
+    readout_finalize_kernel<<<(unsigned)ceil_div((int64_t)G * width, 256), 256, 0, st>>>(partial, row_ptr, chunk_ptr, G, width, 0, out);
+}
+
 bool supported(int H) { return H % 32 == 0 && H >= 32 && H <= 256; }
 
 // chunk_ptr [G + 1] | partial [N / CHUNK + G, H]  (the number of chunks is at most N / CHUNK + G)
@@ -191,7 +199,7 @@ extern "C" int ptgnn_b200_graph_readout(int32_t bf16_states, const void *node_st
     const float *w = mode == PTGNN_READOUT_WEIGHTED_SUM ? gate_weight : nullptr;
     {
         TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        readout::readout_chunk_ptr_kernel<<<1, 1024, 0, st>>>(row_ptr, G, chunk_ptr);
+        readout::launch_chunk_ptr(row_ptr, G, chunk_ptr, st);
     }
     PTGNN_LAUNCHED();
     if (num_nodes > 0) {

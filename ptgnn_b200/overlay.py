@@ -12,7 +12,11 @@ factories import the layer classes by module path (`implementations/typilus/trai
    re-binds those names in reference modules that were imported earlier,
 3. replaces ``GraphNeuralNetwork`` inside the reference's ``graphneuralnetwork`` module (``GraphNeuralNetworkModel`` stays),
 4. registers the ptgnn_b200 container as a (virtual) ``ModuleWithMetrics`` so that a reference parent's ``report_metrics()`` /
-   ``reset_metrics()`` see its ``num_graphs / num_nodes / num_edges`` (`baseneuralmodel/modulewithmetrics.py:44-57`).
+   ``reset_metrics()`` see its ``num_graphs / num_nodes / num_edges`` (`baseneuralmodel/modulewithmetrics.py:44-57`),
+5. with ``native_reducers=True`` only: re-binds ``SelfAttentionVarSizedElementReduce`` and
+   ``MultiheadSelfAttentionVarSizedElementReduce`` in ``ptgnn.neuralmodels.reduceops.varsizedsummary``, in ``ptgnn.neuralmodels.reduceops``
+   and in reference modules imported earlier, so that e.g. ``ptgnn.implementations.graph2seq`` builds its graph summary on the native
+   attention readout.  The default leaves every reducer the reference's.
 
 After ``install()``: ``import ptgnn.implementations.ppi.train`` etc. build ptgnn_b200 layers, unchanged.  ``uninstall()``
 restores the reference's classes.  The reference must be importable as ``ptgnn`` for steps 2-4 (it is not on the GPU test box;
@@ -33,6 +37,8 @@ _LAYER_MODULES = {
     "ptgnn.neuralmodels.gnn.messagepassing.mlpmessagepassing": ("MlpMessagePassingLayer",),
     "ptgnn.neuralmodels.gnn.messagepassing.globalgraphexchange": ("AbstractGlobalGraphExchange", "GruGlobalStateUpdate"),
 }
+_REDUCER_MODULES = ("ptgnn.neuralmodels.reduceops.varsizedsummary", "ptgnn.neuralmodels.reduceops")
+_NATIVE_REDUCERS = ("SelfAttentionVarSizedElementReduce", "MultiheadSelfAttentionVarSizedElementReduce")
 _saved: Dict[str, object] = {}
 
 
@@ -55,8 +61,37 @@ def _stub_module(name: str, names) -> types.ModuleType:
     return m
 
 
-def install(force_torch_scatter: bool = False) -> Dict[str, object]:
-    report: Dict[str, object] = {"torch_scatter": "real", "layers": False, "container": False, "metrics": False}
+def _rebind_everywhere(replaced: Dict[object, object]) -> None:
+    """Re-binds the values of ``replaced`` in every imported reference module (``from ... import X`` bindings made earlier)."""
+    for mod_name, mod in list(sys.modules.items()):
+        if mod is None or not mod_name.startswith("ptgnn.") or getattr(mod, "__ptgnn_b200_overlay__", False):
+            continue
+        for attr, val in list(vars(mod).items()):
+            try:
+                new = replaced.get(val)
+            except TypeError:        # unhashable module attribute
+                continue
+            if new is not None:
+                _saved.setdefault(f"{mod_name}:{attr}", val)
+                setattr(mod, attr, new)
+
+
+def _install_native_reducers() -> None:
+    from . import reduceops as _ro
+
+    importlib.import_module(_REDUCER_MODULES[0])
+    replaced = {}
+    for mod_name in _REDUCER_MODULES:
+        mod = sys.modules[mod_name]
+        for n in _NATIVE_REDUCERS:
+            old = getattr(mod, n, None)
+            if old is not None and old is not getattr(_ro, n):
+                replaced[old] = getattr(_ro, n)
+    _rebind_everywhere(replaced)       # the two reducer modules included
+
+
+def install(force_torch_scatter: bool = False, native_reducers: bool = False) -> Dict[str, object]:
+    report: Dict[str, object] = {"torch_scatter": "real", "layers": False, "container": False, "metrics": False, "reducers": False}
     # 1. torch_scatter
     have_real = False
     if not force_torch_scatter:
@@ -84,17 +119,7 @@ def install(force_torch_scatter: bool = False) -> Dict[str, object]:
                 if hasattr(old, n):
                     replaced[getattr(old, n)] = _native_class(n)
         sys.modules[mod_name] = _stub_module(mod_name, names)
-    for mod_name, mod in list(sys.modules.items()):      # `from ... import GatedMessagePassingLayer` bindings made earlier
-        if mod is None or not mod_name.startswith("ptgnn.") or getattr(mod, "__ptgnn_b200_overlay__", False):
-            continue
-        for attr, val in list(vars(mod).items()):
-            try:
-                new = replaced.get(val)
-            except TypeError:        # unhashable module attribute
-                continue
-            if new is not None:
-                _saved.setdefault(f"{mod_name}:{attr}", val)
-                setattr(mod, attr, new)
+    _rebind_everywhere(replaced)       # `from ... import GatedMessagePassingLayer` bindings made earlier
     report["layers"] = True
     # 3. the container class inside the reference's graphneuralnetwork module (GraphNeuralNetworkModel looks it up at call time)
     ref_gnn = importlib.import_module("ptgnn.neuralmodels.gnn.graphneuralnetwork")
@@ -107,6 +132,10 @@ def install(force_torch_scatter: bool = False) -> Dict[str, object]:
     report["container"] = True
     # 4. metrics protocol
     report["metrics"] = _gnn.register_with_reference_metrics()
+    # 5. the attention reducers (opt-in)
+    if native_reducers:
+        _install_native_reducers()
+        report["reducers"] = True
     return report
 
 
