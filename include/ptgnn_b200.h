@@ -14,8 +14,8 @@
  *
  * Index dtype: the reference delivers int64 index tensors (graphneuralnetwork.py:461-467); the edge
  * plan down-converts them once per minibatch to int32 (E, N < 2^31 is checked).
- * Floating-point dtype: fp32 state/weights (entry points suffixed _f32); bf16 state variants are
- * suffixed _bf16 (fp32 accumulation, like the reference's AMP path abstractmessagepassing.py:43-50).
+ * Floating-point dtype: fp32 weights; entry points suffixed _f32 take fp32 states, those with an `int32_t bf16_states`
+ * first argument take fp32 or bf16 states (fp32 accumulation, like the reference's AMP path abstractmessagepassing.py:43-50).
  */
 #ifndef PTGNN_B200_H_
 #define PTGNN_B200_H_
@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define PTGNN_B200_ABI_VERSION 3
+#define PTGNN_B200_ABI_VERSION 4
 #define PTGNN_MAX_EDGE_TYPES 128 /* etype is stored as uint8 in the plan; 128 keeps launch params < 4 KB */
 
 enum {
@@ -121,88 +121,62 @@ int ptgnn_b200_scatter_f32(const float *src, const int64_t *index, int64_t num_e
 /* ------------------------------------------------------------------------------------------------
  * GatedMessagePassingLayer.forward (gatedmessagepassing.py:37-69), eval mode, no edge features:
  *   m_e = W_{t(e)} h_{src(e)} ; a_v = reduce_{e: tgt(e)=v} m_e ; h'_v = GRUCell(a_v, h_v)
- * edge_weights: [host] array of T device pointers, each nn.Linear.weight [D, H] row-major.
- * gru_*: nn.GRUCell parameters weight_ih [3H, D], weight_hh [3H, H], bias_ih/bias_hh [3H] (gate order r,z,n).
+ * through the unfused kernels (messages -> segmented reduce -> GRUCell).
+ * bf16_states == 0: node_states / gather_states / out_states are fp32 [*, H].  Dimensions that fit the tensor-core tiles
+ * (H % 32 == 0, D % 16 == 0) run on wgmma (3xTF32, fp32-exact); other multiples of 4 run on the FFMA kernels.
+ * PTGNN_B200_DISABLE_TC=1 forces the FFMA kernels.
+ * bf16_states != 0 (BASELINE.json configs[3]): the states are bf16 (raw uint16 bits); module parameters stay fp32 and are
+ * converted into the workspace or the weight cache; messages and aggregates are bf16 in HBM, every accumulation (tensor-core
+ * accumulators, segmented reduce, gate math) is fp32 -- the arithmetic of the reference under torch.autocast(bfloat16) (fp32
+ * scatter: abstractmessagepassing.py:43-50).  Needs H % 32 == 0 (>= 64), D % 16 == 0, 64 <= D <= 256.
+ * edge_weights: [host] array of T device pointers, each nn.Linear.weight [D, H] row-major, fp32.
+ * gru_*: nn.GRUCell parameters weight_ih [3H, D], weight_hh [3H, H], bias_ih/bias_hh [3H] (gate order r,z,n), fp32.
  * type_off: [host] T+1 prefix offsets of the per-type edge counts (edge-id space).
  * gather_states: rows that the plan's source ids index.  NULL = node_states (the normal, single-GPU case).  For a
  * node-range shard (multi-GPU split of one connected graph) node_states holds the num_nodes OWNED rows (targets,
  * local ids) and gather_states the all-gathered [num_source_nodes, H] states (sources, global ids).
- * workspace >= ptgnn_b200_gated_workspace_bytes(...): message buffer [E, D] + aggregate [N, D] + packed / TF32-split
- * weights.  Dimensions that fit the tensor-core tiles (H % 32 == 0, D % 16 == 0) run on wgmma (3xTF32, fp32-exact);
- * other multiples of 4 run on the FFMA kernels.  PTGNN_B200_DISABLE_TC=1 forces the FFMA kernels.
+ * workspace >= ptgnn_b200_gated_workspace_bytes(...): message buffer [E, D] + aggregate [N, D] + derived weights.
+ *
+ * Weight cache (optional).  Every forward call first derives working copies of the parameters (TF32 hi/lo splits,
+ * gate-blocked GRU packing; bf16 conversions for bf16 states).  weight_cache == NULL: they are derived into the workspace on
+ * every call.  A caller whose parameters do not change between calls (inference, or between optimiser steps) can own that
+ * buffer instead: pass `weight_cache` (device memory of at least `*_weight_cache_bytes`, 256-byte aligned) and `cache_valid`
+ * = 0 on the first call with a given set of parameter VALUES (the copies are derived into the cache), 1 afterwards (they are
+ * reused; the parameter pointers are then not read by the derivation).  `*_weight_cache_bytes` == 0 means these dimensions
+ * have nothing to cache: pass NULL.  Results are bit-identical with and without a cache.
  * ---------------------------------------------------------------------------------------------- */
-size_t ptgnn_b200_gated_workspace_bytes(int64_t num_nodes, int64_t num_edges, int32_t num_types, int32_t state_dim,
-                                        int32_t message_dim);
-
-/* Weight cache (optional).  Every forward call first derives working copies of the parameters (TF32 hi/lo splits,
- * gate-blocked GRU packing; bf16 conversions in the bf16 variant).  weight_cache == NULL: they are derived into the workspace
- * on every call.  A caller whose parameters do not change between calls (inference, or between optimiser steps) can own
- * that buffer instead: pass `weight_cache` (device memory of at least `*_weight_cache_bytes`, 256-byte aligned) and
- * `cache_valid` = 0 on the first call with a given set of parameter VALUES (the copies are derived into the cache), 1
- * afterwards (they are reused; the parameter pointers are then not read by the derivation).  `*_weight_cache_bytes` == 0
- * means these dimensions have nothing to cache: pass NULL.  Results are bit-identical with and without a cache. */
-size_t ptgnn_b200_gated_weight_cache_bytes(int32_t num_types, int32_t state_dim, int32_t message_dim);
-int ptgnn_b200_gated_forward_cached_f32(const float *node_states, const float *gather_states /* NULL: node_states */,
-                                        int64_t num_nodes,
-                                        int32_t state_dim, int32_t message_dim, int32_t num_types,
-                                        const int64_t *type_off /*[host]*/, const int32_t *row_ptr, const int32_t *pos,
-                                        const int32_t *src32, const float *const *edge_weights /*[host]*/,
-                                        const float *gru_w_ih, const float *gru_w_hh, const float *gru_b_ih,
-                                        const float *gru_b_hh, int32_t reduce, float *out_states, void *workspace,
-                                        size_t workspace_bytes, void *weight_cache, size_t weight_cache_bytes,
-                                        int32_t cache_valid, void *stream);
-
-/* bf16 variant (BASELINE.json configs[3]): node_states / gather_states / out_states are bf16 [*, H] (raw uint16 bits),
- * module parameters stay fp32 and are converted into the workspace or the weight cache; messages and aggregates are bf16 in
- * HBM, every accumulation (tensor-core accumulators, segmented reduce, gate math) is fp32 -- the arithmetic of the reference
- * under torch.autocast(bfloat16) (fp32 scatter: abstractmessagepassing.py:43-50).  Needs H % 32 == 0, D % 16 == 0,
- * 64 <= D <= 256. */
-size_t ptgnn_b200_gated_workspace_bytes_bf16(int64_t num_nodes, int64_t num_edges, int32_t num_types, int32_t state_dim,
-                                             int32_t message_dim);
-size_t ptgnn_b200_gated_weight_cache_bytes_bf16(int32_t num_types, int32_t state_dim, int32_t message_dim);
-int ptgnn_b200_gated_forward_cached_bf16(const uint16_t *node_states, const uint16_t *gather_states /* NULL: node_states */,
-                                         int64_t num_nodes, int32_t state_dim, int32_t message_dim, int32_t num_types,
-                                         const int64_t *type_off /*[host]*/, const int32_t *row_ptr, const int32_t *pos,
-                                         const int32_t *src32, const float *const *edge_weights /*[host] T device pointers, fp32*/,
-                                         const float *gru_w_ih, const float *gru_w_hh, const float *gru_b_ih,
-                                         const float *gru_b_hh, int32_t reduce, uint16_t *out_states, void *workspace,
-                                         size_t workspace_bytes, void *weight_cache, size_t weight_cache_bytes,
-                                         int32_t cache_valid, void *stream);
+size_t ptgnn_b200_gated_workspace_bytes(int32_t bf16_states, int64_t num_nodes, int64_t num_edges, int32_t num_types,
+                                        int32_t state_dim, int32_t message_dim);
+size_t ptgnn_b200_gated_weight_cache_bytes(int32_t bf16_states, int32_t num_types, int32_t state_dim, int32_t message_dim);
+int ptgnn_b200_gated_forward(int32_t bf16_states, const void *node_states, const void *gather_states /* NULL: node_states */,
+                             int64_t num_nodes, int32_t state_dim, int32_t message_dim, int32_t num_types,
+                             const int64_t *type_off /*[host]*/, const int32_t *row_ptr, const int32_t *pos, const int32_t *src32,
+                             const float *const *edge_weights /*[host]*/, const float *gru_w_ih, const float *gru_w_hh,
+                             const float *gru_b_ih, const float *gru_b_hh, int32_t reduce, void *out_states, void *workspace,
+                             size_t workspace_bytes, void *weight_cache, size_t weight_cache_bytes, int32_t cache_valid,
+                             void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * MlpMessagePassingLayer.forward (mlpmessagepassing.py:68-117), eval mode, default message MLP
  * (mlp_hidden_layers = 0: one bias-free Linear, mlp.py:65-74), string aggregator, no edge features:
  *   m_e = W_{t(e)} [h_src ; h_tgt] ; a_v = reduce m_e ; h'_v = act2(W_d LN(act1(a_v)) + b_d)
- * edge_weights[t]: [D, 2H] (or [D, H] when use_target_state == 0).  ln_weight/ln_bias NULL => no LayerNorm;
- * dense_weight NULL => no dense layer (output dim = D).  dense_weight [Hout, D], dense_bias [Hout].
+ * through the unfused kernels.  edge_weights[t]: [D, 2H] (or [D, H] when use_target_state == 0).  ln_weight/ln_bias NULL =>
+ * no LayerNorm; dense_weight NULL => no dense layer (output dim = D).  dense_weight [Hout, D], dense_bias [Hout].  Every
+ * parameter is fp32 and is derived into the workspace per call (no weight cache).
+ * bf16_states == 0: fp32 states, dims multiples of 4.  bf16_states != 0: bf16 states (raw uint16 bits); messages bf16,
+ * aggregation + activation + LayerNorm in fp32, dense update bf16 with fp32 accumulation (the reference under
+ * torch.autocast(bfloat16)).  Needs in_dim % 32 == 0 (>= 64), message_dim % 16 == 0 in [64, 256], out_dim % 16 == 0 (>= 64)
+ * when a dense layer is present.
  * ---------------------------------------------------------------------------------------------- */
-size_t ptgnn_b200_mlp_workspace_bytes(int64_t num_nodes, int64_t num_edges, int32_t num_types, int32_t in_dim,
+size_t ptgnn_b200_mlp_workspace_bytes(int32_t bf16_states, int64_t num_nodes, int64_t num_edges, int32_t num_types, int32_t in_dim,
                                       int32_t message_dim, int32_t out_dim, int32_t use_target_state);
-int ptgnn_b200_mlp_forward_f32(const float *node_states, const float *gather_states /* NULL: node_states */,
-                               int64_t num_nodes, int32_t in_dim, int32_t message_dim,
-                               int32_t out_dim, int32_t num_types, const int64_t *type_off /*[host]*/,
-                               const int32_t *row_ptr, const int32_t *pos, const int32_t *src32, const int32_t *tgt32,
-                               const float *const *edge_weights /*[host] T device pointers*/,
-                               int32_t use_target_state, int32_t reduce, int32_t message_activation,
-                               const float *ln_weight, const float *ln_bias, float ln_eps, const float *dense_weight,
-                               const float *dense_bias, int32_t dense_activation, float *out_states, void *workspace,
-                               size_t workspace_bytes, void *stream);
-
-/* bf16 variant: node_states / gather_states / out_states are bf16 (raw uint16 bits), every parameter stays fp32 and is
- * converted per call; messages bf16, aggregation + activation + LayerNorm in fp32, dense update bf16 with fp32 accumulation
- * (the reference under torch.autocast(bfloat16)).  Needs in_dim % 32 == 0 (>= 64), message_dim % 16 == 0 in [64, 256],
- * out_dim % 16 == 0 (>= 64) when a dense layer is present. */
-size_t ptgnn_b200_mlp_workspace_bytes_bf16(int64_t num_nodes, int64_t num_edges, int32_t num_types, int32_t in_dim,
-                                           int32_t message_dim, int32_t out_dim, int32_t use_target_state);
-int ptgnn_b200_mlp_forward_bf16(const uint16_t *node_states, const uint16_t *gather_states /* NULL: node_states */,
-                                int64_t num_nodes, int32_t in_dim, int32_t message_dim, int32_t out_dim, int32_t num_types,
-                                const int64_t *type_off /*[host]*/, const int32_t *row_ptr, const int32_t *pos,
-                                const int32_t *src32, const int32_t *tgt32,
-                                const float *const *edge_weights /*[host] T device pointers, fp32*/,
-                                int32_t use_target_state, int32_t reduce, int32_t message_activation,
-                                const float *ln_weight, const float *ln_bias, float ln_eps, const float *dense_weight,
-                                const float *dense_bias, int32_t dense_activation, uint16_t *out_states, void *workspace,
-                                size_t workspace_bytes, void *stream);
+int ptgnn_b200_mlp_forward(int32_t bf16_states, const void *node_states, const void *gather_states /* NULL: node_states */,
+                           int64_t num_nodes, int32_t in_dim, int32_t message_dim, int32_t out_dim, int32_t num_types,
+                           const int64_t *type_off /*[host]*/, const int32_t *row_ptr, const int32_t *pos, const int32_t *src32,
+                           const int32_t *tgt32, const float *const *edge_weights /*[host] T device pointers*/,
+                           int32_t use_target_state, int32_t reduce, int32_t message_activation, const float *ln_weight,
+                           const float *ln_bias, float ln_eps, const float *dense_weight, const float *dense_bias,
+                           int32_t dense_activation, void *out_states, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused aggregation (round 2): gather -> per-type Linear -> segmented reduce in ONE kernel; the [E, D]
@@ -238,7 +212,7 @@ int ptgnn_b200_block_plan_build(int64_t num_nodes, int32_t num_types, const int6
 int32_t ptgnn_b200_fused_supported(int32_t bf16_states, int32_t state_dim, int32_t message_dim);
 
 /* GatedMessagePassingLayer.forward through the fused kernels: the fused aggregation, then the weights-stationary GRUCell.  Same
- * contract as ptgnn_b200_gated_forward_cached_{f32,bf16} (node_states / gather_states / out_states are fp32 when
+ * contract as ptgnn_b200_gated_forward (node_states / gather_states / out_states are fp32 when
  * bf16_states == 0, bf16 otherwise; weight_cache as described there, sized by ptgnn_b200_gated_fused_weight_cache_bytes;
  * `row_ptr` = CSR offsets of the edge plan, used by reduce = mean); the edge arrays come from the block plan.  fp32 states are
  * computed fp32-exactly with three fp16 tensor-core products per term ("3xFP16", see csrc/fused_mp.cuh).
@@ -264,7 +238,7 @@ int ptgnn_b200_gated_forward_fused(int32_t bf16_states, const void *node_states,
                                    size_t workspace_bytes, void *weight_cache, size_t weight_cache_bytes, int32_t cache_valid,
                                    void *stream);
 
-/* MlpMessagePassingLayer.forward through the fused kernel (contract of ptgnn_b200_mlp_forward_{f32,bf16}); the message
+/* MlpMessagePassingLayer.forward through the fused kernel (contract of ptgnn_b200_mlp_forward); the message
  * activation and the LayerNorm run in the fused kernel's write-out.  weight_cache (optional, fp32 states; ignored for bf16
  * states) [>= ptgnn_b200_mlp_fused_weight_cache_bytes] holds the packed edge weights and the split dense weight; pass
  * cache_valid = 0 after the parameters changed (they are then re-derived into the cache), 1 to reuse them. */

@@ -32,24 +32,15 @@ SIGNATURES = {
     "ptgnn_b200_segment_reduce_f32": (ctypes.c_int, [c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_void_p]),
     "ptgnn_b200_scatter_workspace_bytes": (c_size_t, [c_i64, c_i64]),
     "ptgnn_b200_scatter_f32": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_i64, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_gated_workspace_bytes": (c_size_t, [c_i64, c_i64, c_i32, c_i32, c_i32]),
-    "ptgnn_b200_gated_workspace_bytes_bf16": (c_size_t, [c_i64, c_i64, c_i32, c_i32, c_i32]),
-    "ptgnn_b200_gated_weight_cache_bytes": (c_size_t, [c_i32, c_i32, c_i32]),
-    "ptgnn_b200_gated_forward_cached_f32": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p,
-                                                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i32, c_void_p, c_void_p, c_size_t,
-                                                           c_void_p, c_size_t, c_i32, c_void_p]),
-    "ptgnn_b200_gated_weight_cache_bytes_bf16": (c_size_t, [c_i32, c_i32, c_i32]),
-    "ptgnn_b200_gated_forward_cached_bf16": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p,
-                                                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i32, c_void_p, c_void_p, c_size_t,
-                                                            c_void_p, c_size_t, c_i32, c_void_p]),
-    "ptgnn_b200_mlp_workspace_bytes": (c_size_t, [c_i64, c_i64, c_i32, c_i32, c_i32, c_i32, c_i32]),
-    "ptgnn_b200_mlp_forward_f32": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                                  c_void_p, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_f32, c_void_p, c_void_p, c_i32,
-                                                  c_void_p, c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_mlp_workspace_bytes_bf16": (c_size_t, [c_i64, c_i64, c_i32, c_i32, c_i32, c_i32, c_i32]),
-    "ptgnn_b200_mlp_forward_bf16": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                                   c_void_p, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_f32, c_void_p, c_void_p, c_i32,
-                                                   c_void_p, c_void_p, c_size_t, c_void_p]),
+    "ptgnn_b200_gated_workspace_bytes": (c_size_t, [c_i32, c_i64, c_i64, c_i32, c_i32, c_i32]),
+    "ptgnn_b200_gated_weight_cache_bytes": (c_size_t, [c_i32, c_i32, c_i32, c_i32]),
+    "ptgnn_b200_gated_forward": (ctypes.c_int, [c_i32, c_void_p, c_void_p, c_i64, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i32, c_void_p, c_void_p, c_size_t,
+                                                c_void_p, c_size_t, c_i32, c_void_p]),
+    "ptgnn_b200_mlp_workspace_bytes": (c_size_t, [c_i32, c_i64, c_i64, c_i32, c_i32, c_i32, c_i32, c_i32]),
+    "ptgnn_b200_mlp_forward": (ctypes.c_int, [c_i32, c_void_p, c_void_p, c_i64, c_i32, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                              c_void_p, c_void_p, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_f32, c_void_p, c_void_p, c_i32,
+                                              c_void_p, c_void_p, c_size_t, c_void_p]),
     "ptgnn_b200_block_plan_block_targets": (c_i32, [c_i64]),
     "ptgnn_b200_block_plan_workspace_bytes": (c_size_t, [c_i64, c_i64, c_i32, c_i32]),
     "ptgnn_b200_block_plan_build": (ctypes.c_int, [c_i64, c_i32, c_void_p, c_void_p, c_void_p, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
@@ -102,7 +93,7 @@ class BlockPlanStruct(ctypes.Structure):
     _fields_ = [("block_targets", c_i32), ("group_off", c_void_p), ("src_f", c_void_p), ("tl_f", c_void_p), ("status", c_void_p)]
 
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 _lib: Optional[ctypes.CDLL] = None
 
 

@@ -164,7 +164,7 @@ extern "C" int ptgnn_b200_gated_gnn_forward_host_f32(const float *node_states, i
     int32_t *src32 = reinterpret_cast<int32_t *>(pb + sN + 3 * sE), *tgt32 = reinterpret_cast<int32_t *>(pb + sN + 4 * sE);
 
     const size_t ws_plan = ptgnn_b200_plan_workspace_bytes(num_nodes, E);
-    const size_t ws_layer = ptgnn_b200_gated_workspace_bytes(num_nodes, E, num_types, H, H);
+    const size_t ws_layer = ptgnn_b200_gated_workspace_bytes(0, num_nodes, E, num_types, H, H);
     const size_t ws_bytes = ws_plan > ws_layer ? ws_plan : ws_layer;
     PTGNN_CUDA(d_ws.alloc(ws_bytes));
     int rc = ptgnn_b200_plan_build(num_nodes, num_nodes, num_types, dsrc.data(), dtgt.data(), counts, row_ptr, perm, pos, src_sorted,
@@ -193,9 +193,8 @@ extern "C" int ptgnn_b200_gated_gnn_forward_host_f32(const float *node_states, i
         for (int t = 0; t < num_types; ++t) dev_w[t] = base + (size_t)t * H * H;
         float *wih = base + (size_t)num_types * H * H, *whh = wih + 3 * (size_t)H * H;
         float *bih = whh + 3 * (size_t)H * H, *bhh = bih + 3 * H;
-        rc = ptgnn_b200_gated_forward_cached_f32(d_state[cur].as<float>(), nullptr, num_nodes, H, H, num_types, type_off.data(),
-                                                 row_ptr, pos, src32, dev_w.data(), wih, whh, bih, bhh, reduce,
-                                                 d_state[cur ^ 1].as<float>(), d_ws.p, ws_bytes, nullptr, 0, 0, st);
+        rc = ptgnn_b200_gated_forward(0, d_state[cur].p, nullptr, num_nodes, H, H, num_types, type_off.data(), row_ptr, pos, src32,
+                                      dev_w.data(), wih, whh, bih, bhh, reduce, d_state[cur ^ 1].p, d_ws.p, ws_bytes, nullptr, 0, 0, st);
         if (rc) return rc;
         cur ^= 1;
     }

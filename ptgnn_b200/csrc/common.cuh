@@ -1,6 +1,7 @@
 // Shared helpers for the ptgnn_b200 CUDA library (sm_90a only: H100).
 #pragma once
 #include <cuda.h>
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -117,6 +118,11 @@ __device__ __forceinline__ float4 ld_stream_f4(const float4 *p) {  // read-once 
     asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4];"
                  : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p));
     return r;
+}
+// two fp32 -> one packed bf16x2 word (round to nearest even)
+__device__ __forceinline__ float pack_bf16x2(float lo, float hi) {
+    __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
+    return __uint_as_float(*reinterpret_cast<uint32_t *>(&v));
 }
 
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }

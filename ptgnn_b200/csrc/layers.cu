@@ -1,4 +1,5 @@
-// GatedMessagePassingLayer / MlpMessagePassingLayer forward on H100 (fp32-exact path).
+// GatedMessagePassingLayer / MlpMessagePassingLayer forward on H100 through the unfused kernels: the FFMA kernels for fp32
+// states and the one host path per layer class for both state dtypes (the tensor-core kernels: layers_tc.cu, layers_bf16.cu).
 //
 //   reference ptgnn/neuralmodels/gnn/messagepassing/gatedmessagepassing.py:37-69
 //   reference ptgnn/neuralmodels/gnn/messagepassing/mlpmessagepassing.py:68-117  (+ ptgnn/neuralmodels/mlp.py:79-80)
@@ -11,6 +12,8 @@
 //   3. gru_update_kernel     nn.GRUCell: both GEMMs ([agg;h] x packed gate weights) + gate math in one pass, or
 //      dense_update_kernel   Linear(+bias) + Tanh of the Mlp layer.
 #include <stdlib.h>
+
+#include <type_traits>
 
 #include "gemm_simt.cuh"
 #include "layers.cuh"
@@ -266,9 +269,12 @@ static int launch_dense_kernel(const float *y, int64_t rows, int D, const float 
     return PTGNN_OK;
 }
 
-// FFMA GRUCell: packs the gate weights into P1 / P2 (workspace, re-derived every call), then one launch
+// FFMA GRUCell: packs the gate weights into `scratch` (P1 | P2, gru_simt_bytes; re-derived every call), then one launch
+static size_t gru_simt_part(int H, int K) { return ws_slice((size_t)(H / 32 + 1) * 96 * K, 4); }
+static size_t gru_simt_bytes(int H, int D) { return gru_simt_part(H, D) + gru_simt_part(H, H); }
 static int launch_gru_simt(const float *agg, const float *h, int64_t rows, int H, int D, const float *w_ih, const float *w_hh,
-                           const float *b_ih, const float *b_hh, float *out, float *P1, float *P2, cudaStream_t st) {
+                           const float *b_ih, const float *b_hh, float *out, char *scratch, cudaStream_t st) {
+    float *P1 = reinterpret_cast<float *>(scratch), *P2 = reinterpret_cast<float *>(scratch + gru_simt_part(H, D));
     {
         TimedScope timed__(PTGNN_KERNEL_PACK, st);
         pack_gru_weights_kernel<<<132, 256, 0, st>>>(w_ih, w_hh, H, D, P1, P2);
@@ -309,199 +315,229 @@ int dense_any(const float *y, int64_t rows, int D, const float *W, const float *
     return launch_dense_kernel<8>(y, rows, D, W, bias, out_dim, act, out, st);
 }
 
-struct GatedWs { size_t msg, agg, p1, p2, wsplit, grupack, total; };
-static GatedWs gated_ws_layout(int64_t N, int64_t E, int T, int H, int D) {
+// =================================================================================================
+// The unfused layers: messages -> segmented reduce -> GRUCell / dense update, one host path per layer class for both state
+// dtypes (`T` = float or __nv_bfloat16).  Each step has one overload per dtype: fp32 states run on the tensor cores (3xTF32)
+// where the dims fit the tiles and on the FFMA kernels otherwise or under PTGNN_B200_DISABLE_TC=1; bf16 states run on the
+// tensor cores (layers_bf16.cu).  `scratch` receives the derived weights first unless `pack` is false (a weight cache holds them).
+// =================================================================================================
+static int edge_messages(const float *h_src, const float *h_tgt, int H, int D, int use_target, int num_types, const int64_t *type_off,
+                         const float *const *weights, const int32_t *src32, const int32_t *tgt32, const int32_t *pos, float *msg,
+                         void *scratch, bool pack, cudaStream_t st) {
+    if (tc_enabled() && tc::supported_message(H, D))
+        return tc::edge_messages(h_src, h_tgt, H, D, use_target, num_types, type_off, weights, src32, tgt32, pos, msg, scratch, pack, st);
+    return launch_edge_messages(h_src, h_tgt, H, D, use_target, num_types, type_off, weights, src32, tgt32, pos, msg, st);
+}
+using tcb::edge_messages;
+
+// ffma_scratch (fp32 states): >= gru_simt_bytes, for the FFMA kernel's packing
+static int gru_update(const float *agg, const float *h, int64_t rows, int H, int D, const float *w_ih, const float *w_hh,
+                      const float *b_ih, const float *b_hh, float *out, void *scratch, char *ffma_scratch, bool pack, cudaStream_t st) {
+    if (tc_enabled() && tc::supported_gru(H, D)) return tc::gru_update(agg, h, rows, H, D, w_ih, w_hh, b_ih, b_hh, out, scratch, pack, st);
+    return launch_gru_simt(agg, h, rows, H, D, w_ih, w_hh, b_ih, b_hh, out, ffma_scratch, st);
+}
+static int gru_update(const __nv_bfloat16 *agg, const __nv_bfloat16 *h, int64_t rows, int H, int D, const float *w_ih,
+                      const float *w_hh, const float *b_ih, const float *b_hh, __nv_bfloat16 *out, void *scratch, char *, bool pack,
+                      cudaStream_t st) {
+    return tcb::gru_update(agg, h, rows, H, D, w_ih, w_hh, b_ih, b_hh, out, scratch, pack, st);
+}
+
+static int dense_update(const float *y, int64_t rows, int D, const float *W, const float *bias, int Hout, int act, float *out,
+                        void *scratch, cudaStream_t st) {
+    return dense_any(y, rows, D, W, bias, Hout, act, out, scratch, st);
+}
+using tcb::dense_update;
+
+// The shapes each state dtype takes.  fp32: multiples of 4 (PTGNN_E_INVALID otherwise) and, for the GRU, H % 32 == 0
+// (PTGNN_E_UNSUPPORTED otherwise).  bf16, the tensor-core tiles (PTGNN_E_UNSUPPORTED otherwise): H % 32 == 0 (>= 64),
+// D % 16 == 0 in [64, 256], and Hout % 16 == 0 (>= 64) with a dense layer (Hout = 0: none).
+static int check_unfused_dims(const char *who, bool bf16, int64_t N, int64_t E, int H, int D, int Hout, bool gru) {
+    if (!bf16) {
+        const int rc = check_layer_dims(who, N, E, H, D);
+        if (rc || !gru || H % 32 == 0) return rc;
+        set_error("%s: state dim %d must be a multiple of 32 for the GRU kernel", who, H);
+        return PTGNN_E_UNSUPPORTED;
+    }
+    PTGNN_CHECK_ARG(N >= 0 && N < INT32_MAX && E >= 0 && E < INT32_MAX, "%s: sizes out of range", who);
+    if (H % 32 != 0 || D % 16 != 0 || H < 64 || D < 64 || D > 256 || H > 1024 || (Hout != 0 && (Hout % 16 != 0 || Hout < 64))) {
+        set_error("%s: bf16 states need state dim %% 32 == 0 (>= 64), message dim %% 16 == 0 in [64, 256], output dim %% 16 == 0 "
+                  "(>= 64); got %d, %d, %d", who, H, D, Hout);
+        return PTGNN_E_UNSUPPORTED;
+    }
+    return PTGNN_OK;
+}
+
+// [rows, D] messages or aggregates in the state dtype
+static size_t rows_bytes(bool bf16, int64_t rows, int D) { return ws_slice((size_t)rows * D * (bf16 ? 2 : 4) + 16, 1); }
+// the edge weights in the message kernels' format: TF32 (hi, lo) split (fp32 states) or bf16 copy
+static size_t msg_weight_bytes(bool bf16, int T, int D, int Kw) {
+    return bf16 ? tcb::edge_weight_bytes(T, D, Kw) : tc::split_edge_weights_bytes(T, D, Kw);
+}
+
+// gated workspace: msg | agg | FFMA GRU packing (fp32) | derived weights = [edge weights | GRU packing] (without a weight cache)
+struct GatedWs { size_t msg, agg, simt, weights, total; };
+static GatedWs gated_layout(bool bf16, int64_t N, int64_t E, int T, int H, int D) {
     GatedWs w{};
-    size_t o = 0;
-    auto add = [&](size_t cnt) { size_t at = o; o += ws_slice(cnt, 4); return at; };
-    w.msg = add((size_t)E * D + 4);
-    w.agg = add((size_t)N * D + 4);
-    w.p1 = add((size_t)(H / 32 + 1) * 96 * D);
-    w.p2 = add((size_t)(H / 32 + 1) * 96 * H);
-    w.wsplit = o; o += tc::split_edge_weights_bytes(T, D, H);
-    w.grupack = o; o += tc::gru_pack_bytes(H + 32, D);
-    w.total = o;
+    w.agg = rows_bytes(bf16, E, D);
+    w.simt = w.agg + rows_bytes(bf16, N, D);
+    w.weights = w.simt + (bf16 ? 0 : gru_simt_bytes(H, D));
+    w.total = w.weights + msg_weight_bytes(bf16, T, D, H) + (bf16 ? tcb::gru_pack_bytes(H, D) : tc::gru_pack_bytes(H + 32, D));
     return w;
 }
 
-struct MlpWs { size_t msg, y, wsplit, dsplit, total; };
-static MlpWs mlp_ws_layout(int64_t N, int64_t E, int T, int H, int D, int Hout, int use_target) {
-    MlpWs w{};
-    size_t o = 0;
-    auto add = [&](size_t cnt) { size_t at = o; o += ws_slice(cnt, 4); return at; };
-    w.msg = add((size_t)E * D + 4);
-    w.y = add((size_t)N * D + 4);
-    w.wsplit = o; o += tc::split_edge_weights_bytes(T, D, use_target ? 2 * H : H);
-    w.dsplit = o; o += tc::dense_split_bytes(Hout > 0 ? Hout : D, D);
-    w.total = o;
-    return w;
-}
-
-}  // namespace ptgnn
-
-using namespace ptgnn;
-
-extern "C" size_t ptgnn_b200_gated_workspace_bytes(int64_t num_nodes, int64_t num_edges, int32_t num_types,
-                                                   int32_t state_dim, int32_t message_dim) {
-    if (num_nodes < 0 || num_edges < 0 || num_types < 0 || state_dim <= 0 || message_dim <= 0) return 0;
-    return gated_ws_layout(num_nodes, num_edges, num_types, state_dim, message_dim).total;
-}
-
-// weight cache of the tensor-core path: [split edge weights | gate-blocked GRU weights + biases]; 0 when the dims run on
-// the FFMA kernels (nothing worth caching there)
-static size_t gated_cache_bytes(int T, int H, int D) {
+// gated weight cache: [edge weights | GRU packing]; 0 when fp32 states run a step on the FFMA kernels (nothing worth caching)
+static size_t gated_cache_bytes(bool bf16, int T, int H, int D) {
+    if (bf16) return tcb::edge_weight_bytes(T, D, H) + tcb::gru_pack_bytes(H, D);
     if (!tc_enabled() || !tc::supported_message(H, D) || !tc::supported_gru(H, D)) return 0;
     return tc::split_edge_weights_bytes(T, D, H) + tc::gru_pack_bytes(H, D);
 }
 
-static int gated_forward_impl(const float *node_states, const float *gather_states, int64_t num_nodes, int32_t state_dim,
-                              int32_t message_dim, int32_t num_types, const int64_t *type_off, const int32_t *row_ptr,
-                              const int32_t *pos, const int32_t *src32, const float *const *edge_weights,
-                              const float *gru_w_ih, const float *gru_w_hh, const float *gru_b_ih, const float *gru_b_hh,
-                              int32_t reduce, float *out_states, void *workspace, size_t workspace_bytes, void *weight_cache,
-                              size_t weight_cache_bytes, int32_t cache_valid, void *stream) {
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int H = state_dim, D = message_dim;
+// Mlp workspace: msg | y (the aggregate before the dense layer) | edge weights | dense weight (derived every call, no cache)
+struct MlpWs { size_t msg, y, weights, dense, total; };
+static MlpWs mlp_layout(bool bf16, int64_t N, int64_t E, int T, int H, int D, int Hout, int ut) {
+    MlpWs w{};
+    w.y = rows_bytes(bf16, E, D);
+    w.weights = w.y + rows_bytes(bf16, N, D);
+    w.dense = w.weights + msg_weight_bytes(bf16, T, D, ut ? 2 * H : H);
+    w.total = w.dense + (bf16 ? tcb::dense_weight_bytes(Hout, D) : tc::dense_split_bytes(Hout, D));
+    return w;
+}
+
+template <typename T>
+static int gated_unfused(const void *node_states, const void *gather_states, int64_t N, int H, int D, int num_types,
+                         const int64_t *type_off, const int32_t *row_ptr, const int32_t *pos, const int32_t *src32,
+                         const float *const *edge_weights, const float *w_ih, const float *w_hh, const float *b_ih,
+                         const float *b_hh, int reduce, void *out_states, void *workspace, size_t workspace_bytes,
+                         void *weight_cache, size_t weight_cache_bytes, int cache_valid, cudaStream_t st) {
+    constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
     PTGNN_CHECK_ARG(num_types >= 0 && num_types <= PTGNN_MAX_EDGE_TYPES && type_off, "gated_forward: bad num_types=%d", num_types);
     const int64_t E = type_off[num_types];
-    int rc = check_layer_dims("gated_forward", num_nodes, E, H, D);
+    int rc = check_unfused_dims("gated_forward", BF16, N, E, H, D, 0, true);
     if (rc) return rc;
-    if (H % 32 != 0) {
-        set_error("gated_forward: state dim %d must be a multiple of 32 for the GRU kernel", H);
-        return PTGNN_E_UNSUPPORTED;
-    }
     PTGNN_CHECK_ARG(reduce >= PTGNN_REDUCE_SUM && reduce <= PTGNN_REDUCE_MIN, "gated_forward: bad reduce %d", reduce);
-    if (num_nodes == 0) return PTGNN_OK;
-    PTGNN_CHECK_ARG(node_states && out_states && row_ptr && gru_w_ih && gru_w_hh && gru_b_ih && gru_b_hh,
-                    "gated_forward: null pointer");
+    if (N == 0) return PTGNN_OK;
+    PTGNN_CHECK_ARG(node_states && out_states && row_ptr && w_ih && w_hh && b_ih && b_hh, "gated_forward: null pointer");
     PTGNN_CHECK_ARG(E == 0 || (pos && src32 && edge_weights), "gated_forward: null edge arrays");
-    const GatedWs L = gated_ws_layout(num_nodes, E, num_types, H, D);
+    const GatedWs L = gated_layout(BF16, N, E, num_types, H, D);
     if (workspace_bytes < L.total || !workspace) {
         set_error("gated_forward: workspace %zu < required %zu", workspace_bytes, L.total);
         return PTGNN_E_WORKSPACE;
     }
     char *ws = static_cast<char *>(workspace);
-    float *msg = reinterpret_cast<float *>(ws + L.msg), *agg = reinterpret_cast<float *>(ws + L.agg);
-    float *P1 = reinterpret_cast<float *>(ws + L.p1), *P2 = reinterpret_cast<float *>(ws + L.p2);
-    const float *gsrc = gather_states ? gather_states : node_states;   // rows that `src32` indexes (sharded runs)
-    // derived weights: in the workspace (re-derived every call) or in the caller's cache (derived when !cache_valid)
-    char *wsplit = ws + L.wsplit, *grupack = ws + L.grupack;
-    bool pack = true;
-    const size_t need_cache = gated_cache_bytes(num_types, H, D);
-    if (weight_cache != nullptr && need_cache > 0) {
-        if (weight_cache_bytes < need_cache) {
-            set_error("gated_forward: weight cache %zu < required %zu", weight_cache_bytes, need_cache);
-            return PTGNN_E_WORKSPACE;
-        }
-        wsplit = static_cast<char *>(weight_cache);
-        grupack = wsplit + tc::split_edge_weights_bytes(num_types, D, H);
-        pack = !cache_valid;
-    }
+    // a weight cache is not used for dims that have nothing to cache
+    const size_t need = gated_cache_bytes(BF16, num_types, H, D);
+    char *area;
+    bool pack;
+    rc = weight_area("gated_forward", ws + L.weights, need > 0 ? weight_cache : nullptr, weight_cache_bytes, need, cache_valid,
+                     area, pack);
+    if (rc) return rc;
+    char *grupack = area + msg_weight_bytes(BF16, num_types, D, H);
+    const T *h = static_cast<const T *>(node_states);
+    const T *hsrc = gather_states ? static_cast<const T *>(gather_states) : h;   // rows that `src32` indexes (sharded runs)
+    T *msg = reinterpret_cast<T *>(ws + L.msg), *agg = reinterpret_cast<T *>(ws + L.agg);
 
     // 1. per-edge messages, written at their target-sorted positions
-    if (tc_enabled() && tc::supported_message(H, D)) {
-        rc = tc::edge_messages(gsrc, node_states, H, D, 0, num_types, type_off, edge_weights, src32, nullptr, pos, msg,
-                               wsplit, pack, st);
-    } else {
-        rc = launch_edge_messages(gsrc, node_states, H, D, 0, num_types, type_off, edge_weights, src32, nullptr, pos, msg,
-                                  st);
-    }
+    rc = edge_messages(hsrc, h, H, D, 0, num_types, type_off, edge_weights, src32, nullptr, pos, msg, area, pack, st);
     if (rc) return rc;
-    // 2. streaming segmented reduce
-    rc = launch_segment_reduce(msg, row_ptr, nullptr, num_nodes, E, D, reduce, agg, nullptr, nullptr, st);
+    // 2. streaming segmented reduce (fp32 accumulation)
+    rc = launch_segment_reduce(msg, row_ptr, nullptr, N, E, D, reduce, agg, nullptr, nullptr, st);
     if (rc) return rc;
     // 3. GRUCell
-    if (tc_enabled() && tc::supported_gru(H, D)) {
-        return tc::gru_update(agg, node_states, num_nodes, H, D, gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, out_states,
-                              grupack, pack, st);
-    }
-    return launch_gru_simt(agg, node_states, num_nodes, H, D, gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, out_states, P1, P2, st);
+    return gru_update(agg, h, N, H, D, w_ih, w_hh, b_ih, b_hh, static_cast<T *>(out_states), grupack, ws + L.simt, pack, st);
 }
 
-extern "C" size_t ptgnn_b200_gated_weight_cache_bytes(int32_t num_types, int32_t state_dim, int32_t message_dim) {
-    if (num_types < 0 || num_types > PTGNN_MAX_EDGE_TYPES || state_dim <= 0 || message_dim <= 0) return 0;
-    return gated_cache_bytes(num_types, state_dim, message_dim);
-}
-
-extern "C" int ptgnn_b200_gated_forward_cached_f32(const float *node_states, const float *gather_states, int64_t num_nodes,
-                                                   int32_t state_dim, int32_t message_dim, int32_t num_types,
-                                                   const int64_t *type_off, const int32_t *row_ptr, const int32_t *pos,
-                                                   const int32_t *src32, const float *const *edge_weights,
-                                                   const float *gru_w_ih, const float *gru_w_hh, const float *gru_b_ih,
-                                                   const float *gru_b_hh, int32_t reduce, float *out_states, void *workspace,
-                                                   size_t workspace_bytes, void *weight_cache, size_t weight_cache_bytes,
-                                                   int32_t cache_valid, void *stream) {
-    return gated_forward_impl(node_states, gather_states, num_nodes, state_dim, message_dim, num_types, type_off, row_ptr, pos,
-                              src32, edge_weights, gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, reduce, out_states, workspace,
-                              workspace_bytes, weight_cache, weight_cache_bytes, cache_valid, stream);
-}
-
-extern "C" size_t ptgnn_b200_mlp_workspace_bytes(int64_t num_nodes, int64_t num_edges, int32_t num_types, int32_t in_dim,
-                                                 int32_t message_dim, int32_t out_dim, int32_t use_target_state) {
-    if (num_nodes < 0 || num_edges < 0 || num_types < 0 || in_dim <= 0 || message_dim <= 0) return 0;
-    return mlp_ws_layout(num_nodes, num_edges, num_types, in_dim, message_dim, out_dim, use_target_state).total;
-}
-
-static int mlp_forward_impl(const float *node_states, const float *gather_states, int64_t num_nodes, int32_t in_dim,
-                            int32_t message_dim, int32_t out_dim, int32_t num_types, const int64_t *type_off,
-                            const int32_t *row_ptr, const int32_t *pos, const int32_t *src32, const int32_t *tgt32,
-                            const float *const *edge_weights, int32_t use_target_state, int32_t reduce,
-                            int32_t message_activation, const float *ln_weight, const float *ln_bias, float ln_eps,
-                            const float *dense_weight, const float *dense_bias, int32_t dense_activation, float *out_states,
-                            void *workspace, size_t workspace_bytes, void *stream) {
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int H = in_dim, D = message_dim;
+template <typename T>
+static int mlp_unfused(const void *node_states, const void *gather_states, int64_t N, int H, int D, int Hout, int num_types,
+                       const int64_t *type_off, const int32_t *row_ptr, const int32_t *pos, const int32_t *src32, const int32_t *tgt32,
+                       const float *const *edge_weights, int ut, int reduce, int message_activation, const float *ln_weight,
+                       const float *ln_bias, float ln_eps, const float *dense_weight, const float *dense_bias, int dense_activation,
+                       void *out_states, void *workspace, size_t workspace_bytes, cudaStream_t st) {
+    constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
     PTGNN_CHECK_ARG(num_types >= 0 && num_types <= PTGNN_MAX_EDGE_TYPES && type_off, "mlp_forward: bad num_types=%d", num_types);
     const int64_t E = type_off[num_types];
-    int rc = check_layer_dims("mlp_forward", num_nodes, E, H, D);
+    PTGNN_CHECK_ARG(dense_weight ? Hout > 0 : Hout == D, "mlp_forward: out_dim=%d inconsistent", Hout);
+    int rc = check_unfused_dims("mlp_forward", BF16, N, E, H, D, dense_weight ? Hout : 0, false);
     if (rc) return rc;
     PTGNN_CHECK_ARG(reduce >= PTGNN_REDUCE_SUM && reduce <= PTGNN_REDUCE_MIN, "mlp_forward: bad reduce %d", reduce);
     PTGNN_CHECK_ARG(message_activation >= PTGNN_ACT_NONE && message_activation <= PTGNN_ACT_RELU &&
                         dense_activation >= PTGNN_ACT_NONE && dense_activation <= PTGNN_ACT_RELU,
                     "mlp_forward: bad activation");
     PTGNN_CHECK_ARG((ln_weight == nullptr) == (ln_bias == nullptr), "mlp_forward: ln_weight/ln_bias must both be set");
-    PTGNN_CHECK_ARG(dense_weight ? out_dim > 0 : out_dim == D, "mlp_forward: out_dim=%d inconsistent", out_dim);
-    if (num_nodes == 0) return PTGNN_OK;
+    if (N == 0) return PTGNN_OK;
     PTGNN_CHECK_ARG(node_states && out_states && row_ptr, "mlp_forward: null pointer");
-    PTGNN_CHECK_ARG(E == 0 || (pos && src32 && edge_weights && (!use_target_state || tgt32)),
-                    "mlp_forward: null edge arrays");
-    const MlpWs L = mlp_ws_layout(num_nodes, E, num_types, H, D, out_dim, use_target_state);
+    PTGNN_CHECK_ARG(E == 0 || (pos && src32 && edge_weights && (!ut || tgt32)), "mlp_forward: null edge arrays");
+    const MlpWs L = mlp_layout(BF16, N, E, num_types, H, D, Hout, ut);
     if (workspace_bytes < L.total || !workspace) {
         set_error("mlp_forward: workspace %zu < required %zu", workspace_bytes, L.total);
         return PTGNN_E_WORKSPACE;
     }
     char *ws = static_cast<char *>(workspace);
-    float *msg = reinterpret_cast<float *>(ws + L.msg);
-    float *y = dense_weight ? reinterpret_cast<float *>(ws + L.y) : out_states;
-    const int ut = use_target_state ? 1 : 0;
-    const float *gsrc = gather_states ? gather_states : node_states;   // rows that `src32` indexes (sharded runs)
+    const T *h = static_cast<const T *>(node_states);
+    const T *hsrc = gather_states ? static_cast<const T *>(gather_states) : h;   // rows that `src32` indexes (sharded runs)
+    T *out = static_cast<T *>(out_states);
+    T *msg = reinterpret_cast<T *>(ws + L.msg);
+    T *y = dense_weight ? reinterpret_cast<T *>(ws + L.y) : out;
 
-    if (tc_enabled() && tc::supported_message(H, D)) {
-        rc = tc::edge_messages(gsrc, node_states, H, D, ut, num_types, type_off, edge_weights, src32, tgt32, pos, msg,
-                               ws + L.wsplit, true, st);
-    } else {
-        rc = launch_edge_messages(gsrc, node_states, H, D, ut, num_types, type_off, edge_weights, src32, tgt32, pos, msg,
-                                  st);
+    // 1. messages  m_e = W_t [h_src ; h_tgt]
+    if (num_types > 0) {
+        rc = edge_messages(hsrc, h, H, D, ut, num_types, type_off, edge_weights, src32, tgt32, pos, msg, ws + L.weights, true, st);
+        if (rc) return rc;
     }
-    if (rc) return rc;
-    ReduceEpilogue epi{message_activation, ln_weight, ln_bias, ln_eps};
-    rc = launch_segment_reduce(msg, row_ptr, nullptr, num_nodes, E, D, reduce, y, nullptr, &epi, st);
-    if (rc) return rc;
-    if (!dense_weight) return PTGNN_OK;
-    return dense_any(y, num_nodes, D, dense_weight, dense_bias, out_dim, dense_activation, out_states, ws + L.dsplit, st);
+    // 2. segmented reduce + activation + LayerNorm (fp32), one rounding to the state dtype
+    const ReduceEpilogue epi{message_activation, ln_weight, ln_bias, ln_eps};
+    rc = launch_segment_reduce(msg, row_ptr, nullptr, N, E, D, reduce, y, nullptr, &epi, st);
+    if (rc || !dense_weight) return rc;
+    // 3. dense update
+    return dense_update(y, N, D, dense_weight, dense_bias, Hout, dense_activation, out, ws + L.dense, st);
 }
 
-extern "C" int ptgnn_b200_mlp_forward_f32(const float *node_states, const float *gather_states, int64_t num_nodes,
-                                          int32_t in_dim, int32_t message_dim, int32_t out_dim, int32_t num_types,
-                                          const int64_t *type_off, const int32_t *row_ptr, const int32_t *pos,
-                                          const int32_t *src32, const int32_t *tgt32, const float *const *edge_weights,
-                                          int32_t use_target_state, int32_t reduce, int32_t message_activation,
-                                          const float *ln_weight, const float *ln_bias, float ln_eps,
-                                          const float *dense_weight, const float *dense_bias, int32_t dense_activation,
-                                          float *out_states, void *workspace, size_t workspace_bytes, void *stream) {
-    return mlp_forward_impl(node_states, gather_states, num_nodes, in_dim, message_dim, out_dim, num_types, type_off, row_ptr, pos,
-                            src32, tgt32, edge_weights, use_target_state, reduce, message_activation, ln_weight, ln_bias, ln_eps,
-                            dense_weight, dense_bias, dense_activation, out_states, workspace, workspace_bytes, stream);
+}  // namespace ptgnn
+
+using namespace ptgnn;
+
+extern "C" size_t ptgnn_b200_gated_workspace_bytes(int32_t bf16_states, int64_t num_nodes, int64_t num_edges, int32_t num_types,
+                                                   int32_t state_dim, int32_t message_dim) {
+    if (num_nodes < 0 || num_edges < 0 || num_types < 0 || state_dim <= 0 || message_dim <= 0) return 0;
+    return gated_layout(bf16_states != 0, num_nodes, num_edges, num_types, state_dim, message_dim).total;
+}
+
+extern "C" size_t ptgnn_b200_gated_weight_cache_bytes(int32_t bf16_states, int32_t num_types, int32_t state_dim, int32_t message_dim) {
+    if (num_types < 0 || num_types > PTGNN_MAX_EDGE_TYPES || state_dim <= 0 || message_dim <= 0) return 0;
+    return gated_cache_bytes(bf16_states != 0, num_types, state_dim, message_dim);
+}
+
+extern "C" int ptgnn_b200_gated_forward(int32_t bf16_states, const void *node_states, const void *gather_states, int64_t num_nodes,
+                                        int32_t state_dim, int32_t message_dim, int32_t num_types, const int64_t *type_off,
+                                        const int32_t *row_ptr, const int32_t *pos, const int32_t *src32,
+                                        const float *const *edge_weights, const float *gru_w_ih, const float *gru_w_hh,
+                                        const float *gru_b_ih, const float *gru_b_hh, int32_t reduce, void *out_states,
+                                        void *workspace, size_t workspace_bytes, void *weight_cache, size_t weight_cache_bytes,
+                                        int32_t cache_valid, void *stream) {
+    return (bf16_states ? gated_unfused<__nv_bfloat16> : gated_unfused<float>)(
+        node_states, gather_states, num_nodes, state_dim, message_dim, num_types, type_off, row_ptr, pos, src32, edge_weights,
+        gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, reduce, out_states, workspace, workspace_bytes, weight_cache, weight_cache_bytes,
+        cache_valid, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" size_t ptgnn_b200_mlp_workspace_bytes(int32_t bf16_states, int64_t num_nodes, int64_t num_edges, int32_t num_types,
+                                                 int32_t in_dim, int32_t message_dim, int32_t out_dim, int32_t use_target_state) {
+    if (num_nodes < 0 || num_edges < 0 || num_types < 0 || in_dim <= 0 || message_dim <= 0) return 0;
+    if (bf16_states && out_dim <= 0) return 0;
+    return mlp_layout(bf16_states != 0, num_nodes, num_edges, num_types, in_dim, message_dim, out_dim > 0 ? out_dim : message_dim,
+                      use_target_state ? 1 : 0).total;
+}
+
+extern "C" int ptgnn_b200_mlp_forward(int32_t bf16_states, const void *node_states, const void *gather_states, int64_t num_nodes,
+                                      int32_t in_dim, int32_t message_dim, int32_t out_dim, int32_t num_types, const int64_t *type_off,
+                                      const int32_t *row_ptr, const int32_t *pos, const int32_t *src32, const int32_t *tgt32,
+                                      const float *const *edge_weights, int32_t use_target_state, int32_t reduce,
+                                      int32_t message_activation, const float *ln_weight, const float *ln_bias, float ln_eps,
+                                      const float *dense_weight, const float *dense_bias, int32_t dense_activation, void *out_states,
+                                      void *workspace, size_t workspace_bytes, void *stream) {
+    return (bf16_states ? mlp_unfused<__nv_bfloat16> : mlp_unfused<float>)(
+        node_states, gather_states, num_nodes, in_dim, message_dim, out_dim, num_types, type_off, row_ptr, pos, src32, tgt32,
+        edge_weights, use_target_state ? 1 : 0, reduce, message_activation, ln_weight, ln_bias, ln_eps, dense_weight, dense_bias,
+        dense_activation, out_states, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
 /* ---- stand-alone pieces (MLP.forward, message MLPs with hidden layers, module aggregators) -------------------------------------- */
@@ -545,18 +581,13 @@ extern "C" int ptgnn_b200_edge_messages_f32(const float *source_states, const fl
         set_error("edge_messages: workspace too small");
         return PTGNN_E_WORKSPACE;
     }
-    const int ut = use_target_state ? 1 : 0;
-    if (tc_enabled() && tc::supported_message(in_dim, message_dim))
-        return tc::edge_messages(source_states, target_states, in_dim, message_dim, ut, num_types, type_off, edge_weights, src32, tgt32,
-                                 out_row, messages, workspace, true, st);
-    return launch_edge_messages(source_states, target_states, in_dim, message_dim, ut, num_types, type_off, edge_weights, src32, tgt32,
-                                out_row, messages, st);
+    return edge_messages(source_states, target_states, in_dim, message_dim, use_target_state ? 1 : 0, num_types, type_off, edge_weights,
+                         src32, tgt32, out_row, messages, workspace, true, st);
 }
 
 extern "C" size_t ptgnn_b200_grucell_workspace_bytes(int32_t state_dim, int32_t input_dim) {
     if (state_dim <= 0 || input_dim <= 0) return 0;
-    return ws_slice((size_t)(state_dim / 32 + 1) * 96 * input_dim, 4) + ws_slice((size_t)(state_dim / 32 + 1) * 96 * state_dim, 4) +
-           tc::gru_pack_bytes(state_dim + 32, input_dim) + 256;
+    return gru_simt_bytes(state_dim, input_dim) + tc::gru_pack_bytes(state_dim + 32, input_dim) + 256;
 }
 extern "C" int ptgnn_b200_grucell_f32(const float *input, const float *hidden, int64_t rows, int32_t state_dim, int32_t input_dim,
                                       const float *w_ih, const float *w_hh, const float *b_ih, const float *b_hh, float *out,
@@ -569,10 +600,6 @@ extern "C" int ptgnn_b200_grucell_f32(const float *input, const float *hidden, i
     if (rows == 0) return PTGNN_OK;
     PTGNN_CHECK_ARG(input && hidden && w_ih && w_hh && b_ih && b_hh && out, "grucell: null pointer");
     if (workspace_bytes < ptgnn_b200_grucell_workspace_bytes(H, D) || !workspace) { set_error("grucell: workspace too small"); return PTGNN_E_WORKSPACE; }
-    char *ws = static_cast<char *>(workspace);
-    const size_t o1 = ws_slice((size_t)(H / 32 + 1) * 96 * D, 4), o2 = ws_slice((size_t)(H / 32 + 1) * 96 * H, 4);
-    if (tc_enabled() && tc::supported_gru(H, D))
-        return tc::gru_update(input, hidden, rows, H, D, w_ih, w_hh, b_ih, b_hh, out, ws + o1 + o2, true, st);
-    return launch_gru_simt(input, hidden, rows, H, D, w_ih, w_hh, b_ih, b_hh, out, reinterpret_cast<float *>(ws),
-                           reinterpret_cast<float *>(ws + o1), st);
+    char *ws = static_cast<char *>(workspace);   // [FFMA packing | tensor-core packing]
+    return gru_update(input, hidden, rows, H, D, w_ih, w_hh, b_ih, b_hh, out, ws + gru_simt_bytes(H, D), ws, true, st);
 }

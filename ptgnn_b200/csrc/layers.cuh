@@ -14,6 +14,22 @@ bool tc_enabled();
 int dense_any(const float *y, int64_t rows, int D, const float *W, const float *bias, int out_dim, int act, float *out,
               void *scratch, cudaStream_t st, bool pack = true);
 
+// Where a layer call's derived weights live: the weight cache if one is given (derived into it unless cache_valid), else the
+// workspace's area (derived every call).
+inline int weight_area(const char *who, char *ws_area, void *weight_cache, size_t weight_cache_bytes, size_t need, int cache_valid,
+                       char *&area, bool &pack) {
+    area = ws_area;
+    pack = true;
+    if (weight_cache == nullptr) return PTGNN_OK;
+    if (weight_cache_bytes < need) {
+        set_error("%s: weight cache %zu < required %zu", who, weight_cache_bytes, need);
+        return PTGNN_E_WORKSPACE;
+    }
+    area = static_cast<char *>(weight_cache);
+    pack = !cache_valid;
+    return PTGNN_OK;
+}
+
 namespace tcb {
 // The bf16 round-1 kernels (layers_bf16.cu): bf16 states, weights converted from fp32 into `scratch`, fp32 accumulation.
 // `pack` = false when `scratch` is a weight cache that already holds the converted weights.

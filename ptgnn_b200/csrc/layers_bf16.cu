@@ -1,11 +1,9 @@
-// bf16 GatedMessagePassingLayer forward (BASELINE.json configs[3]: bf16 states): bf16 node states / messages / weights,
+// The bf16 steps of the unfused layers (BASELINE.json configs[3]: bf16 states): bf16 node states / messages / weights,
 // fp32 accumulation everywhere (tensor-core accumulators, segmented reduce, gate math) -- the arithmetic of the
 // reference under torch.autocast(bfloat16), whose scatter is always fp32 (abstractmessagepassing.py:43-50).
-//   reference ptgnn/neuralmodels/gnn/messagepassing/gatedmessagepassing.py:37-69
-// Kernels: weight conversion/packing -> tc_pipeline_bf16_kernel<MsgPolicyB> -> segment_reduce_bf16_kernel ->
-// tc_pipeline_bf16_kernel<GruPolicyB>.
-#include <float.h>
-
+//   reference ptgnn/neuralmodels/gnn/messagepassing/gatedmessagepassing.py:37-69, mlpmessagepassing.py:68-117
+// Kernels: weight conversion/packing -> tc_pipeline_bf16_kernel<MsgPolicyB> -> segment_reduce_stream_kernel (reduce.cuh) ->
+// tc_pipeline_bf16_kernel<GruPolicyB> or <DensePolicyB>.  The host path that runs them: layers.cu.
 #include "layers.cuh"
 #include "layers_tc.cuh"
 #include "tc_pipeline_bf16.cuh"
@@ -251,154 +249,6 @@ struct DensePolicyB {
     }
 };
 
-// ---- segmented reduce over bf16 message rows (fp32 accumulation, bf16 result) ------------------------------------
-// Same flat streaming walk as segment_reduce_stream_kernel (reduce.cuh); a lane owns 4 consecutive bf16 columns
-// (8-byte loads), CHUNKS x 128 columns per row.
-// WITH_EPI (Mlp layers): activation + LayerNorm of the aggregated row in fp32 before the single rounding to bf16
-// (mlpmessagepassing.py:114-116; the same epilogue as segment_reduce_stream_kernel).
-struct ReduceEpilogueB { int act; const float *ln_w, *ln_b; float ln_eps; };
-template <int RED, int CHUNKS, bool WITH_EPI>
-__global__ void __launch_bounds__(256)
-segment_reduce_bf16_kernel(const __nv_bfloat16 *__restrict__ msg, const int32_t *__restrict__ row_ptr, int num_nodes, int D,
-                           __nv_bfloat16 *__restrict__ out, const ReduceEpilogueB epi) {
-    constexpr int ROWS_PER_WARP = 16;
-    constexpr int UNROLL = CHUNKS == 1 ? 8 : 4;
-    const int lane = threadIdx.x & 31;
-    const int r0 = (blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * ROWS_PER_WARP;
-    if (r0 >= num_nodes) return;
-    const int nrows = min(ROWS_PER_WARP, num_nodes - r0);
-    const int bound = row_ptr[r0 + min(lane, nrows)];
-    const int j_begin = __shfl_sync(0xffffffffu, bound, 0), j_end = __shfl_sync(0xffffffffu, bound, nrows);
-    bool col_ok[CHUNKS];
-    float4 acc[CHUNKS];
-    const float init = RED == PTGNN_REDUCE_MAX ? -FLT_MAX : (RED == PTGNN_REDUCE_MIN ? FLT_MAX : 0.0f);
-#pragma unroll
-    for (int c = 0; c < CHUNKS; ++c) { col_ok[c] = (c * 32 + lane) * 4 < D; acc[c] = make_float4(init, init, init, init); }
-    const size_t ld2 = (size_t)D / 4;   // row pitch in uint2 (4 bf16)
-    const uint2 *msg2 = reinterpret_cast<const uint2 *>(msg);
-    uint2 *out2 = reinterpret_cast<uint2 *>(out);
-    int cur = 0, cur_end = __shfl_sync(0xffffffffu, bound, 1);
-
-    auto flush = [&](int row, int count) {
-#pragma unroll
-        for (int c = 0; c < CHUNKS; ++c) {
-            float4 a = acc[c];
-            if (RED == PTGNN_REDUCE_MEAN) { const float n = (float)(count < 1 ? 1 : count); a.x /= n; a.y /= n; a.z /= n; a.w /= n; }
-            if (RED == PTGNN_REDUCE_MAX || RED == PTGNN_REDUCE_MIN) {
-                if (a.x == init) a.x = 0.f; if (a.y == init) a.y = 0.f; if (a.z == init) a.z = 0.f; if (a.w == init) a.w = 0.f;
-            }
-            if (WITH_EPI) { a.x = apply_act(a.x, epi.act); a.y = apply_act(a.y, epi.act); a.z = apply_act(a.z, epi.act); a.w = apply_act(a.w, epi.act); }
-            acc[c] = a;
-        }
-        if (WITH_EPI && epi.ln_w != nullptr) {
-            float s = 0.0f;
-#pragma unroll
-            for (int c = 0; c < CHUNKS; ++c)
-                if (col_ok[c]) s += (acc[c].x + acc[c].y) + (acc[c].z + acc[c].w);
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-            const float mean = s / (float)D;
-            float q = 0.0f;
-#pragma unroll
-            for (int c = 0; c < CHUNKS; ++c)
-                if (col_ok[c]) {
-                    const float dx = acc[c].x - mean, dy = acc[c].y - mean, dz = acc[c].z - mean, dw = acc[c].w - mean;
-                    q += (dx * dx + dy * dy) + (dz * dz + dw * dw);
-                }
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
-            const float rstd = rsqrtf(q / (float)D + epi.ln_eps);
-#pragma unroll
-            for (int c = 0; c < CHUNKS; ++c)
-                if (col_ok[c]) {
-                    const int col = (c * 32 + lane) * 4;
-                    const float4 w = *reinterpret_cast<const float4 *>(epi.ln_w + col);
-                    const float4 b = *reinterpret_cast<const float4 *>(epi.ln_b + col);
-                    acc[c].x = (acc[c].x - mean) * rstd * w.x + b.x; acc[c].y = (acc[c].y - mean) * rstd * w.y + b.y;
-                    acc[c].z = (acc[c].z - mean) * rstd * w.z + b.z; acc[c].w = (acc[c].w - mean) * rstd * w.w + b.w;
-                }
-        }
-#pragma unroll
-        for (int c = 0; c < CHUNKS; ++c) {
-            const float4 a = acc[c];
-            if (col_ok[c]) {
-                uint2 o;
-                o.x = __float_as_uint(pack_bf16x2(a.x, a.y));
-                o.y = __float_as_uint(pack_bf16x2(a.z, a.w));
-                out2[(size_t)(r0 + row) * ld2 + c * 32 + lane] = o;
-            }
-            acc[c] = make_float4(init, init, init, init);
-        }
-    };
-    auto comb = [&](float &a, float m) {
-        if (RED == PTGNN_REDUCE_MAX) { if (m > a) a = m; }
-        else if (RED == PTGNN_REDUCE_MIN) { if (m < a) a = m; }
-        else a += m;
-    };
-    for (int j = j_begin; j < j_end; j += UNROLL) {
-        uint2 m[UNROLL][CHUNKS];
-#pragma unroll
-        for (int u = 0; u < UNROLL; ++u)
-            if (j + u < j_end) {
-#pragma unroll
-                for (int c = 0; c < CHUNKS; ++c)
-                    if (col_ok[c]) m[u][c] = __ldg(msg2 + (size_t)(j + u) * ld2 + c * 32 + lane);
-            }
-#pragma unroll
-        for (int u = 0; u < UNROLL; ++u) {
-            const int jj = j + u;
-            if (jj < j_end) {
-                while (jj >= cur_end) {
-                    const int beg = __shfl_sync(0xffffffffu, bound, cur);
-                    flush(cur, cur_end - beg);
-                    ++cur;
-                    cur_end = __shfl_sync(0xffffffffu, bound, cur + 1);
-                }
-#pragma unroll
-                for (int c = 0; c < CHUNKS; ++c)
-                    if (col_ok[c]) {
-                        const __nv_bfloat162 lo = *reinterpret_cast<const __nv_bfloat162 *>(&m[u][c].x);
-                        const __nv_bfloat162 hi = *reinterpret_cast<const __nv_bfloat162 *>(&m[u][c].y);
-                        comb(acc[c].x, __low2float(lo)); comb(acc[c].y, __high2float(lo));
-                        comb(acc[c].z, __low2float(hi)); comb(acc[c].w, __high2float(hi));
-                    }
-            }
-        }
-    }
-    for (; cur < nrows; ++cur) {
-        const int beg = __shfl_sync(0xffffffffu, bound, cur), end = __shfl_sync(0xffffffffu, bound, cur + 1);
-        flush(cur, end - beg);
-    }
-}
-
-template <int RED>
-static int launch_reduce_bf16(const __nv_bfloat16 *msg, const int32_t *row_ptr, int64_t N, int D, __nv_bfloat16 *out,
-                              const ReduceEpilogueB *epi, cudaStream_t st) {
-    const unsigned grid = (unsigned)ceil_div(N, 8 * 16);
-    const ReduceEpilogueB e = epi ? *epi : ReduceEpilogueB{PTGNN_ACT_NONE, nullptr, nullptr, 0.0f};
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        if (epi) {
-            if (D <= 128) segment_reduce_bf16_kernel<RED, 1, true><<<grid, 256, 0, st>>>(msg, row_ptr, (int)N, D, out, e);
-            else segment_reduce_bf16_kernel<RED, 2, true><<<grid, 256, 0, st>>>(msg, row_ptr, (int)N, D, out, e);
-        } else {
-            if (D <= 128) segment_reduce_bf16_kernel<RED, 1, false><<<grid, 256, 0, st>>>(msg, row_ptr, (int)N, D, out, e);
-            else segment_reduce_bf16_kernel<RED, 2, false><<<grid, 256, 0, st>>>(msg, row_ptr, (int)N, D, out, e);
-        }
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
-}
-static int reduce_bf16(int reduce, const __nv_bfloat16 *msg, const int32_t *row_ptr, int64_t N, int D, __nv_bfloat16 *out,
-                       const ReduceEpilogueB *epi, cudaStream_t st) {
-    switch (reduce) {
-        case PTGNN_REDUCE_SUM: return launch_reduce_bf16<PTGNN_REDUCE_SUM>(msg, row_ptr, N, D, out, epi, st);
-        case PTGNN_REDUCE_MEAN: return launch_reduce_bf16<PTGNN_REDUCE_MEAN>(msg, row_ptr, N, D, out, epi, st);
-        case PTGNN_REDUCE_MAX: return launch_reduce_bf16<PTGNN_REDUCE_MAX>(msg, row_ptr, N, D, out, epi, st);
-        default: return launch_reduce_bf16<PTGNN_REDUCE_MIN>(msg, row_ptr, N, D, out, epi, st);
-    }
-}
-
 size_t edge_weight_bytes(int num_types, int D, int Kw) { return ws_slice((size_t)num_types * D * Kw + 8, 2); }
 // GRU packing [P1 (K = D) | P2 (K = H) | bias4]: gate-blocked bf16 weights, 128 rows per block of 32 hidden units
 static size_t gru_part_bytes(int H, int K) { return ws_slice((size_t)(H / 32 + 1) * 128 * K, 2); }
@@ -477,199 +327,5 @@ int dense_update(const __nv_bfloat16 *y, int64_t rows, int D, const float *W, co
     return tc::launch_pipeline(tc_pipeline_bf16_kernel<DensePolicyB>, dp, SMEM_BYTES, tiles, PTGNN_KERNEL_DENSE, st);
 }
 
-// workspace of the gated layer: [msg | agg | bf16 edge weights | GRU packing (P1 | P2 | bias4)]
-struct WsB { size_t msg, agg, w, gru, total; };
-static WsB ws_layout(int64_t N, int64_t E, int T, int H, int D) {
-    WsB w{};
-    size_t o = 0;
-    w.msg = o; o += ws_slice((size_t)E * D + 8, 2);
-    w.agg = o; o += ws_slice((size_t)N * D + 8, 2);
-    w.w = o; o += edge_weight_bytes(T, D, H);
-    w.gru = o; o += gru_pack_bytes(H, D);
-    w.total = o;
-    return w;
-}
-
 }  // namespace tcb
 }  // namespace ptgnn
-
-using namespace ptgnn;
-using namespace ptgnn::tcb;
-
-extern "C" size_t ptgnn_b200_gated_workspace_bytes_bf16(int64_t num_nodes, int64_t num_edges, int32_t num_types,
-                                                        int32_t state_dim, int32_t message_dim) {
-    if (num_nodes < 0 || num_edges < 0 || num_types < 0 || state_dim <= 0 || message_dim <= 0) return 0;
-    return ws_layout(num_nodes, num_edges, num_types, state_dim, message_dim).total;
-}
-
-// weight cache of the bf16 path: the tail of the workspace layout [bf16 edge weights | P1 | P2 | bias4]
-static size_t gated_cache_bytes_bf16(int T, int H, int D) {
-    const WsB L = ws_layout(0, 0, T, H, D);
-    return L.total - L.w;
-}
-
-static int gated_forward_bf16_impl(const uint16_t *node_states, const uint16_t *gather_states, int64_t num_nodes,
-                                   int32_t state_dim, int32_t message_dim, int32_t num_types, const int64_t *type_off,
-                                   const int32_t *row_ptr, const int32_t *pos, const int32_t *src32,
-                                   const float *const *edge_weights, const float *gru_w_ih, const float *gru_w_hh,
-                                   const float *gru_b_ih, const float *gru_b_hh, int32_t reduce, uint16_t *out_states,
-                                   void *workspace, size_t workspace_bytes, void *weight_cache, size_t weight_cache_bytes,
-                                   int32_t cache_valid, void *stream) {
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int H = state_dim, D = message_dim;
-    PTGNN_CHECK_ARG(num_types >= 0 && num_types <= PTGNN_MAX_EDGE_TYPES && type_off, "gated_forward_bf16: bad num_types=%d", num_types);
-    const int64_t E = type_off[num_types];
-    PTGNN_CHECK_ARG(num_nodes >= 0 && num_nodes < INT32_MAX && E >= 0 && E < INT32_MAX, "gated_forward_bf16: sizes out of range");
-    if (H % 32 != 0 || D % 16 != 0 || H < 64 || D < 64 || D > 256 || H > 1024) {
-        set_error("gated_forward_bf16: needs state dim %% 32 == 0 (>= 64) and message dim %% 16 == 0 in [64, 256]; got %d, %d", H, D);
-        return PTGNN_E_UNSUPPORTED;
-    }
-    PTGNN_CHECK_ARG(reduce >= PTGNN_REDUCE_SUM && reduce <= PTGNN_REDUCE_MIN, "gated_forward_bf16: bad reduce %d", reduce);
-    if (num_nodes == 0) return PTGNN_OK;
-    PTGNN_CHECK_ARG(node_states && out_states && row_ptr && gru_w_ih && gru_w_hh && gru_b_ih && gru_b_hh, "gated_forward_bf16: null pointer");
-    PTGNN_CHECK_ARG(E == 0 || (pos && src32 && edge_weights), "gated_forward_bf16: null edge arrays");
-    const WsB L = ws_layout(num_nodes, E, num_types, H, D);
-    if (workspace_bytes < L.total || !workspace) {
-        set_error("gated_forward_bf16: workspace %zu < required %zu", workspace_bytes, L.total);
-        return PTGNN_E_WORKSPACE;
-    }
-    char *ws = static_cast<char *>(workspace);
-    const __nv_bfloat16 *h = reinterpret_cast<const __nv_bfloat16 *>(node_states);
-    const __nv_bfloat16 *hsrc = gather_states ? reinterpret_cast<const __nv_bfloat16 *>(gather_states) : h;
-    __nv_bfloat16 *msg = reinterpret_cast<__nv_bfloat16 *>(ws + L.msg), *agg = reinterpret_cast<__nv_bfloat16 *>(ws + L.agg);
-    // derived weights live in the workspace (re-derived every call) or in the caller's cache (derived when !cache_valid)
-    char *wbase = ws + L.w;
-    bool pack = true;
-    if (weight_cache != nullptr) {
-        const size_t need = gated_cache_bytes_bf16(num_types, H, D);
-        if (weight_cache_bytes < need) {
-            set_error("gated_forward_bf16: weight cache %zu < required %zu", weight_cache_bytes, need);
-            return PTGNN_E_WORKSPACE;
-        }
-        wbase = static_cast<char *>(weight_cache);
-        pack = !cache_valid;
-    }
-
-    // 1. messages (edge weights -> bf16 first when packing)
-    int rc = tcb::edge_messages(hsrc, h, H, D, 0, num_types, type_off, edge_weights, src32, nullptr, pos, msg, wbase, pack, st);
-    if (rc) return rc;
-    // 2. segmented reduce (fp32 accumulate, bf16 result)
-    rc = reduce_bf16(reduce, msg, row_ptr, num_nodes, D, agg, nullptr, st);
-    if (rc) return rc;
-    // 3. GRUCell (gate-blocked weights and biases packed first when packing)
-    return tcb::gru_update(agg, h, num_nodes, H, D, gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, reinterpret_cast<__nv_bfloat16 *>(out_states),
-                           wbase + (L.gru - L.w), pack, st);
-}
-
-extern "C" size_t ptgnn_b200_gated_weight_cache_bytes_bf16(int32_t num_types, int32_t state_dim, int32_t message_dim) {
-    if (num_types < 0 || num_types > PTGNN_MAX_EDGE_TYPES || state_dim <= 0 || message_dim <= 0) return 0;
-    return gated_cache_bytes_bf16(num_types, state_dim, message_dim);
-}
-
-extern "C" int ptgnn_b200_gated_forward_cached_bf16(const uint16_t *node_states, const uint16_t *gather_states,
-                                                    int64_t num_nodes, int32_t state_dim, int32_t message_dim,
-                                                    int32_t num_types, const int64_t *type_off, const int32_t *row_ptr,
-                                                    const int32_t *pos, const int32_t *src32,
-                                                    const float *const *edge_weights, const float *gru_w_ih,
-                                                    const float *gru_w_hh, const float *gru_b_ih, const float *gru_b_hh,
-                                                    int32_t reduce, uint16_t *out_states, void *workspace,
-                                                    size_t workspace_bytes, void *weight_cache, size_t weight_cache_bytes,
-                                                    int32_t cache_valid, void *stream) {
-    return gated_forward_bf16_impl(node_states, gather_states, num_nodes, state_dim, message_dim, num_types, type_off, row_ptr,
-                                   pos, src32, edge_weights, gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, reduce, out_states,
-                                   workspace, workspace_bytes, weight_cache, weight_cache_bytes, cache_valid, stream);
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// MlpMessagePassingLayer with bf16 states (mlpmessagepassing.py:68-117 under torch.autocast(bfloat16)): bf16 messages,
-// fp32 aggregation + GELU + LayerNorm, bf16 dense update with fp32 accumulation.  Parameters arrive in fp32.
-// ---------------------------------------------------------------------------------------------------------------
-namespace ptgnn {
-namespace tcb {
-struct MlpWsB { size_t msg, y, w, wd, total; };
-static MlpWsB mlp_ws_layout(int64_t N, int64_t E, int T, int H, int D, int Hout, int use_target) {
-    MlpWsB w{};
-    size_t o = 0;
-    w.msg = o; o += ws_slice((size_t)E * D + 8, 2);
-    w.y = o; o += ws_slice((size_t)N * D + 8, 2);
-    w.w = o; o += edge_weight_bytes(T, D, use_target ? 2 * H : H);
-    w.wd = o; o += dense_weight_bytes(Hout, D);
-    w.total = o;
-    return w;
-}
-}  // namespace tcb
-}  // namespace ptgnn
-
-extern "C" size_t ptgnn_b200_mlp_workspace_bytes_bf16(int64_t num_nodes, int64_t num_edges, int32_t num_types, int32_t in_dim,
-                                                      int32_t message_dim, int32_t out_dim, int32_t use_target_state) {
-    if (num_nodes < 0 || num_edges < 0 || num_types < 0 || in_dim <= 0 || message_dim <= 0 || out_dim <= 0) return 0;
-    return mlp_ws_layout(num_nodes, num_edges, num_types, in_dim, message_dim, out_dim, use_target_state).total;
-}
-
-static int mlp_forward_bf16_impl(const uint16_t *node_states, const uint16_t *gather_states, int64_t num_nodes,
-                                 int32_t in_dim, int32_t message_dim, int32_t out_dim, int32_t num_types,
-                                 const int64_t *type_off, const int32_t *row_ptr, const int32_t *pos,
-                                 const int32_t *src32, const int32_t *tgt32, const float *const *edge_weights,
-                                 int32_t use_target_state, int32_t reduce, int32_t message_activation,
-                                 const float *ln_weight, const float *ln_bias, float ln_eps,
-                                 const float *dense_weight, const float *dense_bias, int32_t dense_activation,
-                                 uint16_t *out_states, void *workspace, size_t workspace_bytes, void *stream) {
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int H = in_dim, D = message_dim, ut = use_target_state ? 1 : 0;
-    PTGNN_CHECK_ARG(num_types >= 0 && num_types <= PTGNN_MAX_EDGE_TYPES && type_off, "mlp_forward_bf16: bad num_types=%d", num_types);
-    const int64_t E = type_off[num_types];
-    PTGNN_CHECK_ARG(num_nodes >= 0 && num_nodes < INT32_MAX && E >= 0 && E < INT32_MAX, "mlp_forward_bf16: sizes out of range");
-    PTGNN_CHECK_ARG(dense_weight ? out_dim > 0 : out_dim == D, "mlp_forward_bf16: out_dim=%d inconsistent", out_dim);
-    if (H % 32 != 0 || D % 16 != 0 || H < 64 || D < 64 || D > 256 || H > 1024 || (dense_weight && (out_dim % 16 != 0 || out_dim < 64))) {
-        set_error("mlp_forward_bf16: needs state dim %% 32 == 0 (>= 64), message dim %% 16 == 0 in [64, 256], output dim %% 16 == 0 (>= 64); "
-                  "got %d, %d, %d", H, D, out_dim);
-        return PTGNN_E_UNSUPPORTED;
-    }
-    PTGNN_CHECK_ARG(reduce >= PTGNN_REDUCE_SUM && reduce <= PTGNN_REDUCE_MIN, "mlp_forward_bf16: bad reduce %d", reduce);
-    PTGNN_CHECK_ARG(message_activation >= PTGNN_ACT_NONE && message_activation <= PTGNN_ACT_RELU &&
-                        dense_activation >= PTGNN_ACT_NONE && dense_activation <= PTGNN_ACT_RELU, "mlp_forward_bf16: bad activation");
-    PTGNN_CHECK_ARG((ln_weight == nullptr) == (ln_bias == nullptr), "mlp_forward_bf16: ln_weight/ln_bias must both be set");
-    if (num_nodes == 0) return PTGNN_OK;
-    PTGNN_CHECK_ARG(node_states && out_states && row_ptr, "mlp_forward_bf16: null pointer");
-    PTGNN_CHECK_ARG(E == 0 || (pos && src32 && edge_weights && (!ut || tgt32)), "mlp_forward_bf16: null edge arrays");
-    const MlpWsB L = mlp_ws_layout(num_nodes, E, num_types, H, D, out_dim, ut);
-    if (workspace_bytes < L.total || !workspace) {
-        set_error("mlp_forward_bf16: workspace %zu < required %zu", workspace_bytes, L.total);
-        return PTGNN_E_WORKSPACE;
-    }
-    char *ws = static_cast<char *>(workspace);
-    auto b16 = [&](size_t off) { return reinterpret_cast<__nv_bfloat16 *>(ws + off); };
-    const __nv_bfloat16 *h = reinterpret_cast<const __nv_bfloat16 *>(node_states);
-    const __nv_bfloat16 *hsrc = gather_states ? reinterpret_cast<const __nv_bfloat16 *>(gather_states) : h;
-    __nv_bfloat16 *out = reinterpret_cast<__nv_bfloat16 *>(out_states);
-    __nv_bfloat16 *msg = b16(L.msg);
-    __nv_bfloat16 *y = dense_weight ? b16(L.y) : out;
-
-    // 1. messages  m_e = W_t [h_src ; h_tgt]  (edge weights -> bf16 first)
-    int rc = PTGNN_OK;
-    if (num_types > 0) {
-        rc = tcb::edge_messages(hsrc, h, H, D, ut, num_types, type_off, edge_weights, src32, tgt32, pos, msg, ws + L.w, true, st);
-        if (rc) return rc;
-    }
-
-    // 2. aggregate + activation + LayerNorm (fp32) -> y (bf16)
-    const ReduceEpilogueB epi{message_activation, ln_weight, ln_bias, ln_eps};
-    rc = reduce_bf16(reduce, msg, row_ptr, num_nodes, D, y, &epi, st);
-    if (rc || !dense_weight) return rc;
-
-    // 3. dense update
-    return dense_update(y, num_nodes, D, dense_weight, dense_bias, out_dim, dense_activation, out, ws + L.wd, st);
-}
-
-extern "C" int ptgnn_b200_mlp_forward_bf16(const uint16_t *node_states, const uint16_t *gather_states, int64_t num_nodes,
-                                           int32_t in_dim, int32_t message_dim, int32_t out_dim, int32_t num_types,
-                                           const int64_t *type_off, const int32_t *row_ptr, const int32_t *pos,
-                                           const int32_t *src32, const int32_t *tgt32, const float *const *edge_weights,
-                                           int32_t use_target_state, int32_t reduce, int32_t message_activation,
-                                           const float *ln_weight, const float *ln_bias, float ln_eps,
-                                           const float *dense_weight, const float *dense_bias, int32_t dense_activation,
-                                           uint16_t *out_states, void *workspace, size_t workspace_bytes, void *stream) {
-    return mlp_forward_bf16_impl(node_states, gather_states, num_nodes, in_dim, message_dim, out_dim, num_types, type_off, row_ptr,
-                                 pos, src32, tgt32, edge_weights, use_target_state, reduce, message_activation, ln_weight, ln_bias,
-                                 ln_eps, dense_weight, dense_bias, dense_activation, out_states, workspace, workspace_bytes, stream);
-}

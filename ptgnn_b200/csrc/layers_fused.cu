@@ -55,21 +55,6 @@ MlpWs mlp_layout(int nprod, int64_t N, int64_t Ns, int T, int H, int D, int Hout
     return w;
 }
 
-// the weight cache if one is given (derive into it unless cache_valid), else the workspace's area (derive every call)
-int weight_area(const char *who, char *ws_area, void *weight_cache, size_t weight_cache_bytes, size_t need, int cache_valid,
-                char *&area, bool &pack) {
-    area = ws_area;
-    pack = true;
-    if (weight_cache == nullptr) return PTGNN_OK;
-    if (weight_cache_bytes < need) {
-        set_error("%s: weight cache %zu < required %zu", who, weight_cache_bytes, need);
-        return PTGNN_E_WORKSPACE;
-    }
-    area = static_cast<char *>(weight_cache);
-    pack = !cache_valid;
-    return PTGNN_OK;
-}
-
 fused::AggregateArgs aggregate_args(int nprod, const ptgnn_b200_block_plan *bp, const int32_t *row_ptr, int64_t N, int H, int T, int reduce,
                                     const void *packed_weights) {
     fused::AggregateArgs a{};

@@ -1,4 +1,6 @@
 // Dispatch + C ABI for the segmented reduce (see reduce.cuh) and the one-shot torch_scatter.scatter drop-in.
+#include <type_traits>
+
 #include "reduce.cuh"
 
 namespace ptgnn {
@@ -33,16 +35,16 @@ static int launch_shape(const float *msg, const int32_t *row_ptr, const int32_t 
     return PTGNN_OK;
 }
 
-template <int RED, int CHUNKS>
-static int launch_stream(const float *msg, const int32_t *row_ptr, const int32_t *perm, int64_t N, int D, float *out,
+template <typename T, int RED, int CHUNKS>
+static int launch_stream(const T *msg, const int32_t *row_ptr, const int32_t *perm, int64_t N, int D, T *out,
                          const ReduceEpilogue *epi, cudaStream_t st) {
     const unsigned grid = (unsigned)ceil_div(N, 8 * 16);   // 8 warps x 16 rows per block
     ReduceEpilogue e{};
     if (epi) e = *epi;
     {
         TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        if (epi) segment_reduce_stream_kernel<RED, CHUNKS, true><<<grid, 256, 0, st>>>(msg, row_ptr, perm, (int)N, D, out, e);
-        else segment_reduce_stream_kernel<RED, CHUNKS, false><<<grid, 256, 0, st>>>(msg, row_ptr, perm, (int)N, D, out, e);
+        if (epi) segment_reduce_stream_kernel<T, RED, CHUNKS, true><<<grid, 256, 0, st>>>(msg, row_ptr, perm, (int)N, D, out, e);
+        else segment_reduce_stream_kernel<T, RED, CHUNKS, false><<<grid, 256, 0, st>>>(msg, row_ptr, perm, (int)N, D, out, e);
     }
     PTGNN_LAUNCHED();
     return PTGNN_OK;
@@ -55,18 +57,30 @@ static int launch_red(const float *msg, const int32_t *row_ptr, const int32_t *p
     if (D <= 64) return launch_shape<RED, 16, 1>(msg, row_ptr, perm, N, E, D, out, arg_out, epi, st);
     const bool want_arg = arg_out && (RED == PTGNN_REDUCE_MAX || RED == PTGNN_REDUCE_MIN);
     if (!want_arg) {   // wide rows without arg: streaming kernel
-        if (D <= 128) return launch_stream<RED, 1>(msg, row_ptr, perm, N, D, out, epi, st);
-        if (D <= 256) return launch_stream<RED, 2>(msg, row_ptr, perm, N, D, out, epi, st);
-        return launch_stream<RED, 4>(msg, row_ptr, perm, N, D, out, epi, st);
+        if (D <= 128) return launch_stream<float, RED, 1>(msg, row_ptr, perm, N, D, out, epi, st);
+        if (D <= 256) return launch_stream<float, RED, 2>(msg, row_ptr, perm, N, D, out, epi, st);
+        return launch_stream<float, RED, 4>(msg, row_ptr, perm, N, D, out, epi, st);
     }
     if (D <= 128) return launch_shape<RED, 32, 1>(msg, row_ptr, perm, N, E, D, out, arg_out, epi, st);
     if (D <= 256) return launch_shape<RED, 32, 2>(msg, row_ptr, perm, N, E, D, out, arg_out, epi, st);
     return launch_shape<RED, 32, 4>(msg, row_ptr, perm, N, E, D, out, arg_out, epi, st);
 }
 
-int launch_segment_reduce(const float *msg, const int32_t *row_ptr, const int32_t *perm, int64_t N, int64_t E, int D,
-                          int reduce, float *out, int64_t *arg_out, const ReduceEpilogue *epi, cudaStream_t st) {
-    PTGNN_CHECK_ARG(D > 0 && D % 4 == 0 && D <= 512, "segment_reduce: dim=%d must be a multiple of 4 and <= 512", D);
+// bf16 rows: always the streaming kernel (also at D <= 64)
+template <int RED>
+static int launch_red(const __nv_bfloat16 *msg, const int32_t *row_ptr, const int32_t *, int64_t N, int64_t, int D,
+                      __nv_bfloat16 *out, int64_t *, const ReduceEpilogue *epi, cudaStream_t st) {
+    if (D <= 128) return launch_stream<__nv_bfloat16, RED, 1>(msg, row_ptr, nullptr, N, D, out, epi, st);
+    return launch_stream<__nv_bfloat16, RED, 2>(msg, row_ptr, nullptr, N, D, out, epi, st);
+}
+
+template <typename T>
+int launch_segment_reduce(const T *msg, const int32_t *row_ptr, const int32_t *perm, int64_t N, int64_t E, int D,
+                          int reduce, T *out, int64_t *arg_out, const ReduceEpilogue *epi, cudaStream_t st) {
+    constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
+    PTGNN_CHECK_ARG(D > 0 && D % 4 == 0 && D <= (BF16 ? 256 : 512), "segment_reduce: dim=%d must be a multiple of 4 and <= %d", D,
+                    BF16 ? 256 : 512);
+    PTGNN_CHECK_ARG(!BF16 || (perm == nullptr && arg_out == nullptr), "segment_reduce: bf16 rows take no perm and no arg output");
     PTGNN_CHECK_ARG(N >= 0 && N < INT32_MAX && E >= 0 && E < INT32_MAX, "segment_reduce: sizes out of range");
     if (N == 0) return PTGNN_OK;
     PTGNN_CHECK_ARG(row_ptr && out && (msg || E == 0), "segment_reduce: null pointer");
@@ -78,6 +92,10 @@ int launch_segment_reduce(const float *msg, const int32_t *row_ptr, const int32_
         default: set_error("segment_reduce: unknown reduce %d", reduce); return PTGNN_E_INVALID;
     }
 }
+template int launch_segment_reduce<float>(const float *, const int32_t *, const int32_t *, int64_t, int64_t, int, int, float *,
+                                          int64_t *, const ReduceEpilogue *, cudaStream_t);
+template int launch_segment_reduce<__nv_bfloat16>(const __nv_bfloat16 *, const int32_t *, const int32_t *, int64_t, int64_t, int, int,
+                                                  __nv_bfloat16 *, int64_t *, const ReduceEpilogue *, cudaStream_t);
 
 }  // namespace ptgnn
 

@@ -12,6 +12,8 @@
 #pragma once
 #include <float.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace ptgnn {
@@ -38,6 +40,48 @@ __device__ __forceinline__ void red_combine(float &a, int &arg, float m, int e) 
     } else {
         a += m;
     }
+}
+
+// The Mlp layer's epilogue on one aggregated row held by LPR lanes (lane `sl` holds columns (c * LPR + sl) * 4 .. + 3 of
+// chunk c): the message activation, then LayerNorm over the row's D columns.  Every lane of the warp must call it (the
+// LayerNorm sums are full-warp shuffles).
+template <int LPR, int CHUNKS>
+__device__ __forceinline__ void row_epilogue(float4 (&acc)[CHUNKS], const bool (&col_ok)[CHUNKS], int sl, int D,
+                                             const ReduceEpilogue &epi) {
+#pragma unroll
+    for (int c = 0; c < CHUNKS; ++c) {
+        acc[c].x = apply_act(acc[c].x, epi.act); acc[c].y = apply_act(acc[c].y, epi.act);
+        acc[c].z = apply_act(acc[c].z, epi.act); acc[c].w = apply_act(acc[c].w, epi.act);
+    }
+    if (epi.ln_w == nullptr) return;
+    float s = 0.0f;
+#pragma unroll
+    for (int c = 0; c < CHUNKS; ++c)
+        if (col_ok[c]) s += (acc[c].x + acc[c].y) + (acc[c].z + acc[c].w);
+#pragma unroll
+    for (int o = LPR / 2; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    const float mean = s / (float)D;
+    float q = 0.0f;
+#pragma unroll
+    for (int c = 0; c < CHUNKS; ++c)
+        if (col_ok[c]) {
+            const float dx = acc[c].x - mean, dy = acc[c].y - mean, dz = acc[c].z - mean, dw = acc[c].w - mean;
+            q += (dx * dx + dy * dy) + (dz * dz + dw * dw);
+        }
+#pragma unroll
+    for (int o = LPR / 2; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
+    const float rstd = rsqrtf(q / (float)D + epi.ln_eps);
+#pragma unroll
+    for (int c = 0; c < CHUNKS; ++c)
+        if (col_ok[c]) {
+            const int col = (c * LPR + sl) * 4;
+            const float4 w = *reinterpret_cast<const float4 *>(epi.ln_w + col);
+            const float4 b = *reinterpret_cast<const float4 *>(epi.ln_b + col);
+            acc[c].x = (acc[c].x - mean) * rstd * w.x + b.x;
+            acc[c].y = (acc[c].y - mean) * rstd * w.y + b.y;
+            acc[c].z = (acc[c].z - mean) * rstd * w.z + b.z;
+            acc[c].w = (acc[c].w - mean) * rstd * w.w + b.w;
+        }
 }
 
 // LPR = lanes per row (8/16/32), CHUNKS = float4 per lane (row width D <= LPR*4*CHUNKS).
@@ -121,43 +165,7 @@ segment_reduce_kernel(const float *__restrict__ msg, const int32_t *__restrict__
     }
 
     // ---- optional fused epilogue: activation + LayerNorm over the row ------------------------------
-    if (WITH_EPI) {
-#pragma unroll
-        for (int c = 0; c < CHUNKS; ++c) {
-            acc[c].x = apply_act(acc[c].x, epi.act); acc[c].y = apply_act(acc[c].y, epi.act);
-            acc[c].z = apply_act(acc[c].z, epi.act); acc[c].w = apply_act(acc[c].w, epi.act);
-        }
-        if (epi.ln_w != nullptr) {
-            float s = 0.0f;
-#pragma unroll
-            for (int c = 0; c < CHUNKS; ++c)
-                if (col_ok[c]) s += (acc[c].x + acc[c].y) + (acc[c].z + acc[c].w);
-#pragma unroll
-            for (int o = LPR / 2; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-            const float mean = s / (float)D;
-            float q = 0.0f;
-#pragma unroll
-            for (int c = 0; c < CHUNKS; ++c)
-                if (col_ok[c]) {
-                    const float dx = acc[c].x - mean, dy = acc[c].y - mean, dz = acc[c].z - mean, dw = acc[c].w - mean;
-                    q += (dx * dx + dy * dy) + (dz * dz + dw * dw);
-                }
-#pragma unroll
-            for (int o = LPR / 2; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
-            const float rstd = rsqrtf(q / (float)D + epi.ln_eps);
-#pragma unroll
-            for (int c = 0; c < CHUNKS; ++c)
-                if (col_ok[c]) {
-                    const int col = (c * LPR + sl) * 4;
-                    const float4 w = *reinterpret_cast<const float4 *>(epi.ln_w + col);
-                    const float4 b = *reinterpret_cast<const float4 *>(epi.ln_b + col);
-                    acc[c].x = (acc[c].x - mean) * rstd * w.x + b.x;
-                    acc[c].y = (acc[c].y - mean) * rstd * w.y + b.y;
-                    acc[c].z = (acc[c].z - mean) * rstd * w.z + b.z;
-                    acc[c].w = (acc[c].w - mean) * rstd * w.w + b.w;
-                }
-        }
-    }
+    if constexpr (WITH_EPI) row_epilogue<LPR, CHUNKS>(acc, col_ok, sl, D, epi);
 
     if (!row_ok) return;
     float4 *out4 = reinterpret_cast<float4 *>(out);
@@ -172,19 +180,47 @@ segment_reduce_kernel(const float *__restrict__ msg, const int32_t *__restrict__
     }
 }
 
+// Row access of the streaming reduce, per element type: a lane moves 4 consecutive columns of a row at a time.  fp32 rows:
+// 16-byte loads that bypass L1 (read-once data).  bf16 rows: 8-byte loads, widened to fp32 when accumulated, one rounding to
+// bf16 at the store.
+template <typename T> struct Row4;
+template <> struct Row4<float> {
+    using Raw = float4;
+    static __device__ __forceinline__ Raw load(const float *rows, size_t i) { return ld_stream_f4(reinterpret_cast<const float4 *>(rows) + i); }
+    static __device__ __forceinline__ float4 widen(Raw r) { return r; }
+    static __device__ __forceinline__ void store(float *rows, size_t i, float4 a) { reinterpret_cast<float4 *>(rows)[i] = a; }
+};
+template <> struct Row4<__nv_bfloat16> {
+    using Raw = uint2;
+    static __device__ __forceinline__ Raw load(const __nv_bfloat16 *rows, size_t i) { return __ldg(reinterpret_cast<const uint2 *>(rows) + i); }
+    static __device__ __forceinline__ float4 widen(Raw r) {
+        const __nv_bfloat162 lo = *reinterpret_cast<const __nv_bfloat162 *>(&r.x);
+        const __nv_bfloat162 hi = *reinterpret_cast<const __nv_bfloat162 *>(&r.y);
+        return make_float4(__low2float(lo), __high2float(lo), __low2float(hi), __high2float(hi));
+    }
+    static __device__ __forceinline__ void store(__nv_bfloat16 *rows, size_t i, float4 a) {
+        uint2 o;
+        o.x = __float_as_uint(pack_bf16x2(a.x, a.y));
+        o.y = __float_as_uint(pack_bf16x2(a.z, a.w));
+        reinterpret_cast<uint2 *>(rows)[i] = o;
+    }
+};
+
 // ---------------------------------------------------------------------------------------------------------------
-// Streaming variant for row widths > 64 floats (one warp-wide float4 load = CHUNKS x 512 bytes of one message row).
-// A warp owns ROWS_PER_WARP consecutive target rows and walks the FLAT range of their messages, always keeping
-// UNROLL row loads in flight regardless of where the row boundaries fall (the per-row kernel above drains its
+// Streaming variant for wide rows (one warp-wide load = CHUNKS x 128 columns of one message row), fp32 or bf16 rows with
+// fp32 accumulation.  A warp owns ROWS_PER_WARP consecutive target rows and walks the FLAT range of their messages, always
+// keeping UNROLL row loads in flight regardless of where the row boundaries fall (the per-row kernel above drains its
 // pipeline at every row end -- at an average in-degree of 5.4 that left HBM ~45 % idle).  Row boundaries come from
 // the CSR offsets held one per lane and are applied warp-uniformly, so the accumulation order inside a row is still
 // the plan (= reference edge) order and empty rows fall out of the same loop.
 // ---------------------------------------------------------------------------------------------------------------
-template <int RED, int CHUNKS, bool WITH_EPI>
+template <typename T, int RED, int CHUNKS, bool WITH_EPI>
 __global__ void __launch_bounds__(256)
-segment_reduce_stream_kernel(const float *__restrict__ msg, const int32_t *__restrict__ row_ptr,
-                             const int32_t *__restrict__ perm, int num_nodes, int D, float *__restrict__ out,
+segment_reduce_stream_kernel(const T *__restrict__ msg, const int32_t *__restrict__ row_ptr,
+                             const int32_t *__restrict__ perm, int num_nodes, int D, T *__restrict__ out,
                              ReduceEpilogue epi) {
+    using IO = Row4<T>;
+    constexpr bool PERM = std::is_same<T, float>::value;    // bf16 rows are the layers' messages, already in plan order
     constexpr int ROWS_PER_WARP = 16;
     constexpr int UNROLL = CHUNKS == 1 ? 8 : (CHUNKS == 2 ? 4 : 2);
     const int lane = threadIdx.x & 31;
@@ -200,9 +236,7 @@ segment_reduce_stream_kernel(const float *__restrict__ msg, const int32_t *__res
     float4 acc[CHUNKS];
 #pragma unroll
     for (int c = 0; c < CHUNKS; ++c) { col_ok[c] = (c * 32 + lane) * 4 < D; red_init<RED>(acc[c]); }
-    const size_t ld4 = (size_t)D / 4;
-    const float4 *msg4 = reinterpret_cast<const float4 *>(msg);
-    float4 *out4 = reinterpret_cast<float4 *>(out);
+    const size_t ld4 = (size_t)D / 4;                               // row pitch in groups of 4 columns
 
     int cur = 0;                                                    // row being accumulated (index inside the warp's block)
     int cur_end = __shfl_sync(0xffffffffu, bound, 1);
@@ -224,61 +258,25 @@ segment_reduce_stream_kernel(const float *__restrict__ msg, const int32_t *__res
                 if (acc[c].w == init) acc[c].w = 0.0f;
             }
         }
-        if (WITH_EPI) {
-#pragma unroll
-            for (int c = 0; c < CHUNKS; ++c) {
-                acc[c].x = apply_act(acc[c].x, epi.act); acc[c].y = apply_act(acc[c].y, epi.act);
-                acc[c].z = apply_act(acc[c].z, epi.act); acc[c].w = apply_act(acc[c].w, epi.act);
-            }
-            if (epi.ln_w != nullptr) {
-                float s = 0.0f;
-#pragma unroll
-                for (int c = 0; c < CHUNKS; ++c)
-                    if (col_ok[c]) s += (acc[c].x + acc[c].y) + (acc[c].z + acc[c].w);
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-                const float mean = s / (float)D;
-                float q = 0.0f;
-#pragma unroll
-                for (int c = 0; c < CHUNKS; ++c)
-                    if (col_ok[c]) {
-                        const float dx = acc[c].x - mean, dy = acc[c].y - mean, dz = acc[c].z - mean, dw = acc[c].w - mean;
-                        q += (dx * dx + dy * dy) + (dz * dz + dw * dw);
-                    }
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
-                const float rstd = rsqrtf(q / (float)D + epi.ln_eps);
-#pragma unroll
-                for (int c = 0; c < CHUNKS; ++c)
-                    if (col_ok[c]) {
-                        const int col = (c * 32 + lane) * 4;
-                        const float4 w = *reinterpret_cast<const float4 *>(epi.ln_w + col);
-                        const float4 b = *reinterpret_cast<const float4 *>(epi.ln_b + col);
-                        acc[c].x = (acc[c].x - mean) * rstd * w.x + b.x;
-                        acc[c].y = (acc[c].y - mean) * rstd * w.y + b.y;
-                        acc[c].z = (acc[c].z - mean) * rstd * w.z + b.z;
-                        acc[c].w = (acc[c].w - mean) * rstd * w.w + b.w;
-                    }
-            }
-        }
+        if constexpr (WITH_EPI) row_epilogue<32, CHUNKS>(acc, col_ok, lane, D, epi);
 #pragma unroll
         for (int c = 0; c < CHUNKS; ++c) {
-            if (col_ok[c]) out4[(size_t)(r0 + row) * ld4 + c * 32 + lane] = acc[c];
+            if (col_ok[c]) IO::store(out, (size_t)(r0 + row) * ld4 + c * 32 + lane, acc[c]);
             red_init<RED>(acc[c]);
         }
     };
 
     for (int j = j_begin; j < j_end; j += UNROLL) {
-        float4 m[UNROLL][CHUNKS];
+        typename IO::Raw m[UNROLL][CHUNKS];
         int my_row = 0;
-        if (perm != nullptr && lane < UNROLL && j + lane < j_end) my_row = perm[j + lane];
+        if (PERM && perm != nullptr && lane < UNROLL && j + lane < j_end) my_row = perm[j + lane];
 #pragma unroll
         for (int u = 0; u < UNROLL; ++u) {
             if (j + u < j_end) {
-                const size_t row = perm != nullptr ? (size_t)__shfl_sync(0xffffffffu, my_row, u) : (size_t)(j + u);
+                const size_t row = PERM && perm != nullptr ? (size_t)__shfl_sync(0xffffffffu, my_row, u) : (size_t)(j + u);
 #pragma unroll
                 for (int c = 0; c < CHUNKS; ++c)
-                    if (col_ok[c]) m[u][c] = ld_stream_f4(msg4 + row * ld4 + c * 32 + lane);
+                    if (col_ok[c]) m[u][c] = IO::load(msg, row * ld4 + c * 32 + lane);
             }
         }
 #pragma unroll
@@ -294,11 +292,12 @@ segment_reduce_stream_kernel(const float *__restrict__ msg, const int32_t *__res
 #pragma unroll
                 for (int c = 0; c < CHUNKS; ++c) {
                     if (col_ok[c]) {
+                        const float4 v = IO::widen(m[u][c]);
                         int dummy = 0;
-                        red_combine<RED>(acc[c].x, dummy, m[u][c].x, 0);
-                        red_combine<RED>(acc[c].y, dummy, m[u][c].y, 0);
-                        red_combine<RED>(acc[c].z, dummy, m[u][c].z, 0);
-                        red_combine<RED>(acc[c].w, dummy, m[u][c].w, 0);
+                        red_combine<RED>(acc[c].x, dummy, v.x, 0);
+                        red_combine<RED>(acc[c].y, dummy, v.y, 0);
+                        red_combine<RED>(acc[c].z, dummy, v.z, 0);
+                        red_combine<RED>(acc[c].w, dummy, v.w, 0);
                     }
                 }
             }
@@ -311,8 +310,10 @@ segment_reduce_stream_kernel(const float *__restrict__ msg, const int32_t *__res
     }
 }
 
-// Host-side dispatch.  D must be a multiple of 4 and <= 512.
-int launch_segment_reduce(const float *msg, const int32_t *row_ptr, const int32_t *perm, int64_t N, int64_t E, int D,
-                          int reduce, float *out, int64_t *arg_out, const ReduceEpilogue *epi, cudaStream_t st);
+// Host-side dispatch (reduce.cu), for fp32 and bf16 rows.  fp32: D a multiple of 4 and <= 512.  bf16 (the unfused layers'
+// messages): D a multiple of 4 and <= 256, always on the streaming kernel, no perm, no arg_out.
+template <typename T>
+int launch_segment_reduce(const T *msg, const int32_t *row_ptr, const int32_t *perm, int64_t N, int64_t E, int D,
+                          int reduce, T *out, int64_t *arg_out, const ReduceEpilogue *epi, cudaStream_t st);
 
 }  // namespace ptgnn

@@ -276,11 +276,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_bf16_kernel(const 
 // drain helpers: the accumulator tile layout is shared with the fp32 pipeline
 using tc::drain_2x32;
 using tc::drain_4x16;
-// two fp32 -> one packed bf16x2 word (round to nearest even)
-__device__ __forceinline__ float pack_bf16x2(float lo, float hi) {
-    __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-    return __uint_as_float(*reinterpret_cast<uint32_t *>(&v));
-}
 
 }  // namespace tcb
 }  // namespace ptgnn

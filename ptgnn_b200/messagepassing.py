@@ -263,9 +263,7 @@ class GatedMessagePassingLayer(AbstractMessagePassingLayer):
         h = N.require_cuda(node_states, "node_states", state_dtype)
         num_nodes, H = h.shape
         D = self.__message_dimension
-        gsrc = None if gather_states is None else N.require_cuda(gather_states, "gather_states", state_dtype)
-        if gsrc is not None and (gsrc.dim() != 2 or gsrc.shape[1] != H):
-            raise ValueError("gather_states must be [num_source_nodes, H]")
+        gsrc = self._gather_source(gather_states, h)
         plan = self._plan(adjacency_lists, num_nodes, None if gsrc is None else gsrc.shape[0])
         gru = self.__state_update
         weights = [N.require_cuda(lin.weight, "edge weight", torch.float32) for lin in linears]
@@ -308,21 +306,19 @@ class GatedMessagePassingLayer(AbstractMessagePassingLayer):
                 chain.store(out, packed_out)
             return out
         # round-1 three-kernel path; bf16 states: fp32 parameters (converted inside the library), fp32 accumulation
-        kind, sfx = ("bf16", "_bf16") if bf16 else ("f32", "")
-        fwd = "ptgnn_b200_gated_forward_cached_" + kind
-        cache_bytes = getattr(lib, "ptgnn_b200_gated_weight_cache_bytes" + sfx)(plan.num_types, H, D)
-        cache, valid = self._weight_cache(kind, cache_bytes, params, h.device)
-        ws_bytes = getattr(lib, "ptgnn_b200_gated_workspace_bytes" + sfx)(num_nodes, plan.num_edges, plan.num_types, H, D)
+        kind = "bf16" if bf16 else "f32"
+        cache, valid = self._weight_cache(kind, lib.ptgnn_b200_gated_weight_cache_bytes(int(bf16), plan.num_types, H, D), params, h.device)
+        ws_bytes = lib.ptgnn_b200_gated_workspace_bytes(int(bf16), num_nodes, plan.num_edges, plan.num_types, H, D)
         ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=h.device)
         out = torch.empty_like(h)
         with torch.cuda.device(h.device):
-            rc = getattr(lib, fwd)(
-                N.ptr(h), N.ptr(gsrc), num_nodes, H, D, plan.num_types, plan.type_off_c, N.ptr(plan.row_ptr), N.ptr(plan.pos),
+            rc = lib.ptgnn_b200_gated_forward(
+                int(bf16), N.ptr(h), N.ptr(gsrc), num_nodes, H, D, plan.num_types, plan.type_off_c, N.ptr(plan.row_ptr), N.ptr(plan.pos),
                 N.ptr(plan.src32), N.ptr_table(weights), N.ptr(w_ih), N.ptr(w_hh), N.ptr(b_ih), N.ptr(b_hh), reduce,
                 N.ptr(out), N.ptr(ws), ws_bytes, N.ptr(cache), 0 if cache is None else cache.numel(), int(valid),
                 N.current_stream(h.device),
             )
-        N.check(rc, fwd)
+        N.check(rc, "ptgnn_b200_gated_forward")
         self._weight_cache_filled(kind, h.device)
         return out
 
@@ -565,19 +561,17 @@ class MlpMessagePassingLayer(AbstractMessagePassingLayer):
             self._weight_cache_filled("mlp_f32_fused", h.device)
             return apply_dropout(out)
         # round-1 three-kernel path; bf16 states: fp32 parameters (converted inside the library), fp32 accumulation
-        fwd = "ptgnn_b200_mlp_forward_" + ("bf16" if bf16 else "f32")
-        ws_bytes = getattr(lib, "ptgnn_b200_mlp_workspace_bytes" + ("_bf16" if bf16 else ""))(
-            num_nodes, plan.num_edges, plan.num_types, H, D, out_dim, ut_i)
+        ws_bytes = lib.ptgnn_b200_mlp_workspace_bytes(int(bf16), num_nodes, plan.num_edges, plan.num_types, H, D, out_dim, ut_i)
         ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=h.device)
         out = torch.empty(num_nodes, out_dim, dtype=state_dtype, device=h.device)
         with torch.cuda.device(h.device):
-            rc = getattr(lib, fwd)(
-                N.ptr(h), N.ptr(gsrc), num_nodes, H, D, out_dim, plan.num_types, plan.type_off_c, N.ptr(plan.row_ptr), N.ptr(plan.pos),
+            rc = lib.ptgnn_b200_mlp_forward(
+                int(bf16), N.ptr(h), N.ptr(gsrc), num_nodes, H, D, out_dim, plan.num_types, plan.type_off_c, N.ptr(plan.row_ptr), N.ptr(plan.pos),
                 N.ptr(plan.src32), N.ptr(plan.tgt32), N.ptr_table(weights), ut_i, reduce, msg_act, N.ptr(ln_w), N.ptr(ln_b),
                 float(ln.eps) if ln is not None else 0.0, N.ptr(d_w), N.ptr(d_b), dense_act, N.ptr(out), N.ptr(ws), ws_bytes,
                 N.current_stream(h.device),
             )
-        N.check(rc, fwd)
+        N.check(rc, "ptgnn_b200_mlp_forward")
         return apply_dropout(out)
 
     def _forward_composed(self, node_states, adjacency_lists, edge_features, gather_states) -> torch.Tensor:

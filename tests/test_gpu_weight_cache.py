@@ -1,4 +1,4 @@
-"""Derived-weight cache of GatedMessagePassingLayer (ptgnn_b200_gated_forward_cached_*): results must be bit-identical
+"""Derived-weight cache of GatedMessagePassingLayer (ptgnn_b200_gated_forward, ptgnn_b200_gated_forward_fused): results must be bit-identical
 to the fill path, and any in-place parameter update must invalidate it."""
 import copy
 

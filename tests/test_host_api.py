@@ -27,7 +27,7 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(handle, name), f"{name} declared in include/ptgnn_b200.h but not exported"
     assert sorted(N.SIGNATURES) == declared, "ctypes SIGNATURES must cover exactly the header's entry points"
-    assert handle.ptgnn_b200_abi_version() == 3
+    assert handle.ptgnn_b200_abi_version() == 4
 
 
 def test_fused_supported_shapes():
@@ -53,9 +53,56 @@ def test_fused_supported_shapes():
 def test_workspace_size_queries_run_without_a_gpu():
     handle = N.lib()
     assert handle.ptgnn_b200_plan_workspace_bytes(1000, 5000) > 4 * 5000 * 4
-    assert handle.ptgnn_b200_gated_workspace_bytes(1000, 5000, 17, 128, 128) >= 5000 * 128 * 4 + 1000 * 128 * 4
-    assert handle.ptgnn_b200_mlp_workspace_bytes(1000, 5000, 17, 128, 128, 128, 1) >= 5000 * 128 * 4
+    assert handle.ptgnn_b200_gated_workspace_bytes(0, 1000, 5000, 17, 128, 128) >= 5000 * 128 * 4 + 1000 * 128 * 4
+    assert handle.ptgnn_b200_mlp_workspace_bytes(0, 1000, 5000, 17, 128, 128, 128, 1) >= 5000 * 128 * 4
     assert handle.ptgnn_b200_scatter_workspace_bytes(1000, 5000) > handle.ptgnn_b200_plan_workspace_bytes(1000, 5000)
+
+
+# (N, E, T, H, D) -> workspace bytes of the unfused gated layer, fp32 / bf16 states
+_GATED_WS = {
+    (1000, 5000, 17, 128, 128): (7269376, 2423808),
+    (777, 4321, 3, 64, 64): (2044416, 777216),
+    (500, 3001, 5, 256, 256): (12994560, 3632640),
+    (1000, 5000, 4, 96, 36): (1851392, 597248),      # fp32 states: FFMA dims
+    (123, 0, 2, 64, 128): (1105408, 213760),
+}
+# (T, H, D) -> weight-cache bytes of the unfused gated layer, fp32 / bf16 states (fp32: 0 unless every step runs on tensor cores)
+_GATED_CACHE = {(17, 128, 128): (3278848, 887296), (3, 64, 64): (361472, 124416), (5, 256, 256): (6819840, 1839616),
+                (4, 96, 36): (0, 164864), (2, 32, 16): (0, 27648), (2, 64, 128): (525312, 181760)}
+# (N, E, T, H, D, out_dim, use_target_state) -> workspace bytes of the unfused Mlp layer, fp32 / bf16 states
+_MLP_WS = {
+    (1000, 5000, 17, 128, 128, 128, 0): (5431808, 2126848),
+    (1000, 5000, 17, 128, 128, 192, 1): (7725568, 2700288),
+    (777, 4321, 3, 64, 64, 64, 1): (1534976, 710656),
+    (500, 3001, 5, 256, 256, 192, 0): (6600192, 2547200),
+    (1000, 5000, 4, 96, 36, 36, 0): (985600, 463104),
+    (1000, 5000, 4, 96, 36, 192, 1): (1140736, 502016),
+    (1000, 5000, 4, 96, 36, 0, 1): (1096192, 0),     # out_dim <= 0: the message dim for fp32 states, no size for bf16
+    (123, 0, 2, 64, 128, 128, 1): (456704, 130816),
+}
+
+
+def test_unfused_layer_buffer_sizes_are_pinned():
+    """The unfused layers' workspace and weight-cache layouts, per state dtype: exact byte counts (a layout change is an ABI
+    change for callers that keep buffers across calls)."""
+    import subprocess
+    import sys
+
+    handle = N.lib()
+    for bf16 in (0, 1):
+        for args, want in _GATED_WS.items():
+            assert handle.ptgnn_b200_gated_workspace_bytes(bf16, *args) == want[bf16], (bf16, args)
+        for args, want in _GATED_CACHE.items():
+            assert handle.ptgnn_b200_gated_weight_cache_bytes(bf16, *args) == want[bf16], (bf16, args)
+        for args, want in _MLP_WS.items():
+            assert handle.ptgnn_b200_mlp_workspace_bytes(bf16, *args) == want[bf16], (bf16, args)
+    # PTGNN_B200_DISABLE_TC=1 (read once per process): fp32 states run on the FFMA kernels and cache nothing; bf16 unchanged
+    script = ("from ptgnn_b200 import _native as N; h = N.lib(); "
+              "print(h.ptgnn_b200_gated_weight_cache_bytes(0, 17, 128, 128), h.ptgnn_b200_gated_weight_cache_bytes(1, 17, 128, 128), "
+              "h.ptgnn_b200_gated_workspace_bytes(0, 1000, 5000, 17, 128, 128))")
+    env = dict(os.environ, PTGNN_B200_DISABLE_TC="1")
+    out = subprocess.run([sys.executable, "-s", "-c", script], cwd=ROOT, env=env, capture_output=True, text=True, check=True)
+    assert out.stdout.split() == ["0", "887296", "7269376"]
 
 
 def test_no_cpu_fallback():
