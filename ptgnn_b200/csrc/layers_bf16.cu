@@ -42,6 +42,19 @@ __global__ void pack_gru_bf16_kernel(const float *__restrict__ w_ih, const float
     }
 }
 
+// Stores the first `cols` (a multiple of 16) of a warp's 64 bf16 columns, packed two per word in `w`.  warp_store_rows
+// counts 4-byte words in powers of two, so 48 columns go out as 32 + 16.
+__device__ __forceinline__ void store_cols(int cols, float *stage, const float (&w)[32], float *dst, long long row_off, int lane) {
+    if (cols >= 64) {
+        tc::warp_store_rows<32>(stage, w, dst, row_off, lane);
+    } else if (cols >= 32) {
+        tc::warp_store_rows<16>(stage, w, dst, row_off, lane);
+        if (cols >= 48) tc::warp_store_rows<8>(stage, w + 16, dst + 16, row_off, lane);
+    } else {
+        tc::warp_store_rows<8>(stage, w, dst, row_off, lane);
+    }
+}
+
 // ---- policy: per-edge messages -------------------------------------------------------------------------------
 struct MsgPolicyB {
     struct Params {
@@ -106,9 +119,7 @@ struct MsgPolicyB {
 #pragma unroll
         for (int i = 0; i < 32; ++i) w[i] = pack_bf16x2(acc[2 * i], acc[2 * i + 1]);
         float *dst = reinterpret_cast<float *>(p.msg) + c0 / 2;
-        if (ti.b_rows - c0 >= 64) tc::warp_store_rows<32>(stage, w, dst, row_off, lane);
-        else if (ti.b_rows - c0 >= 32) tc::warp_store_rows<16>(stage, w, dst, row_off, lane);
-        else tc::warp_store_rows<8>(stage, w, dst, row_off, lane);   // 16 columns
+        store_cols(ti.b_rows - c0, stage, w, dst, row_off, lane);
     }
 };
 
@@ -243,9 +254,7 @@ struct DensePolicyB {
             w[i] = pack_bf16x2(v0, v1);
         }
         float *dst = reinterpret_cast<float *>(p.out) + c0 / 2;
-        if (ti.b_rows - c0 >= 64) tc::warp_store_rows<32>(stage, w, dst, pre.row_off, lane);
-        else if (ti.b_rows - c0 >= 32) tc::warp_store_rows<16>(stage, w, dst, pre.row_off, lane);
-        else tc::warp_store_rows<8>(stage, w, dst, pre.row_off, lane);   // 16 columns
+        store_cols(ti.b_rows - c0, stage, w, dst, pre.row_off, lane);
     }
 };
 

@@ -28,8 +28,8 @@ Where [m - e, m + e] contains no bf16 rounding midpoint that is exactly bf16(m);
 message that cancels to far below its mass (|m| < e) may be several of its own ulps off.  Such messages widen the bound of
 their aggregate by that distance (plus the fp32 re-rounding of a sum that saw them).  The output may differ by 1 bf16 ulp.
 
-An activation after the aggregate propagates the bound through its Lipschitz constant (GELU 1.13, Tanh 1, ReLU 1) and adds
-its own fp32 evaluation error, 8u (|x| + |act(x)|).
+An activation after the aggregate propagates the bound through its Lipschitz constant (GELU 1.13, ReLU 1; tanh: its largest
+slope within the bound) and adds its own fp32 evaluation error, 8u (|x| + |act(x)|).
 """
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -124,9 +124,21 @@ def _bf16_ulp(x: torch.Tensor) -> torch.Tensor:
     return torch.exp2(torch.floor(torch.log2(a)) - 7)
 
 
-def aggregate(tgt, m, err, num_nodes: int, reduce: str, bf16: bool, act: Optional[str] = None):
+def activation_bound(pre: torch.Tensor, bnd: torch.Tensor, act: Optional[str]):
+    """-> (act(pre), bound): ``bnd`` through the activation's slope plus its fp32 evaluation error.  The slope is the
+    Lipschitz constant, except for tanh: its largest slope on [pre - bnd, pre + bnd], 1 - tanh^2(max(|pre| - bnd, 0)) (a
+    saturated tanh must not pass a bf16 ulp of its input on unchanged)."""
+    ref = _act64(pre, act)
+    if act is None:
+        return ref, bnd
+    slope = 1 - torch.tanh((pre.abs() - bnd).clamp(min=0)) ** 2 if act == "tanh" else LIPSCHITZ[act]
+    return ref, slope * bnd + 8 * U * (pre.abs() + ref.abs())
+
+
+def aggregate(tgt, m, err, num_nodes: int, reduce: str, bf16: bool, act: Optional[str] = None, round_bf16: bool = True):
     """-> (ref [N, D] float64, bound [N, D] float64, pre [N, D] float64): the expected output, the allowed |got - ref| per
-    element, and the aggregate before the activation (for epilogues checked elsewhere, e.g. LayerNorm)."""
+    element, and the aggregate before the activation (for epilogues checked elsewhere, e.g. LayerNorm).  bf16 with
+    round_bf16=False: the fp32 value before the output's rounding to bf16 (for an epilogue that rounds later)."""
     N, D = num_nodes, m.shape[1]
     cnt = torch.zeros(N, dtype=torch.float64).index_add_(0, tgt, torch.ones(tgt.shape[0], dtype=torch.float64))
     empty = (cnt == 0)[:, None].expand(N, D)
@@ -154,10 +166,8 @@ def aggregate(tgt, m, err, num_nodes: int, reduce: str, bf16: bool, act: Optiona
             if reduce == "mean":
                 pre = pre / c
                 bnd = bnd / c + U * (pre.abs() + bnd / c)
-    ref = _act64(pre, act)
-    if act is not None:
-        bnd = LIPSCHITZ[act] * bnd + 8 * U * (pre.abs() + ref.abs())
-    if bf16:
+    ref, bnd = activation_bound(pre, bnd, act)
+    if bf16 and round_bf16:
         ref_b = ref.to(torch.float32).to(torch.bfloat16).double()
         bnd = bnd + _bf16_ulp(ref_b.abs() + bnd)
         ref = ref_b
