@@ -1,6 +1,6 @@
 // nn.GRUCell update, weights-stationary:  h' = GRUCell(agg, h)   (reference gatedmessagepassing.py:69)
 //
-// Why a second GRU kernel.  The round-1 pipeline (tc_pipeline.cuh, GruPolicy) walks (row tile, 32-hidden-unit block) tiles in
+// Why a second GRU kernel.  The round-1 pipeline (tc_pipeline.cuh, GruPolicy in layers_tc.cu) walks (row tile, 32-hidden-unit block) tiles in
 // row-major order: every tile streams its gate-weight block again and every row tile is fetched once per block -- L2 -> SM
 // traffic, not the tensor pipe, is what bounds it.  Here a CTA keeps ONE hidden-unit block for its whole life: its gate
 // weights are loaded into shared memory once and stay (B operand of every MMA), and only the node rows stream through a TMA ring (A operand).  L2 traffic drops to the row

@@ -1,5 +1,5 @@
 // GatedMessagePassingLayer / MlpMessagePassingLayer forward on H100 through the unfused kernels: the FFMA kernels for fp32
-// states and the one host path per layer class for both state dtypes (the tensor-core kernels: layers_tc.cu, layers_bf16.cu).
+// states and the one host path per layer class for both state dtypes (the tensor-core kernels: layers_tc.cu).
 //
 //   reference ptgnn/neuralmodels/gnn/messagepassing/gatedmessagepassing.py:37-69
 //   reference ptgnn/neuralmodels/gnn/messagepassing/mlpmessagepassing.py:68-117  (+ ptgnn/neuralmodels/mlp.py:79-80)
@@ -317,36 +317,31 @@ int dense_any(const float *y, int64_t rows, int D, const float *W, const float *
 
 // =================================================================================================
 // The unfused layers: messages -> segmented reduce -> GRUCell / dense update, one host path per layer class for both state
-// dtypes (`T` = float or __nv_bfloat16).  Each step has one overload per dtype: fp32 states run on the tensor cores (3xTF32)
-// where the dims fit the tiles and on the FFMA kernels otherwise or under PTGNN_B200_DISABLE_TC=1; bf16 states run on the
-// tensor cores (layers_bf16.cu).  `scratch` receives the derived weights first unless `pack` is false (a weight cache holds them).
+// dtypes (`T` = float or __nv_bfloat16).  fp32 states run on the tensor cores (3xTF32) where the dims fit the tiles and on
+// the FFMA kernels otherwise or under PTGNN_B200_DISABLE_TC=1; bf16 states always run on the tensor cores (layers_tc.cu).
+// `scratch` receives the derived weights first unless `pack` is false (a weight cache holds them).
 // =================================================================================================
-static int edge_messages(const float *h_src, const float *h_tgt, int H, int D, int use_target, int num_types, const int64_t *type_off,
-                         const float *const *weights, const int32_t *src32, const int32_t *tgt32, const int32_t *pos, float *msg,
+template <typename T>
+static int edge_messages(const T *h_src, const T *h_tgt, int H, int D, int use_target, int num_types, const int64_t *type_off,
+                         const float *const *weights, const int32_t *src32, const int32_t *tgt32, const int32_t *pos, T *msg,
                          void *scratch, bool pack, cudaStream_t st) {
-    if (tc_enabled() && tc::supported_message(H, D))
-        return tc::edge_messages(h_src, h_tgt, H, D, use_target, num_types, type_off, weights, src32, tgt32, pos, msg, scratch, pack, st);
-    return launch_edge_messages(h_src, h_tgt, H, D, use_target, num_types, type_off, weights, src32, tgt32, pos, msg, st);
+    if constexpr (std::is_same<T, float>::value) {
+        if (!tc_enabled() || !tc::supported_message(H, D))
+            return launch_edge_messages(h_src, h_tgt, H, D, use_target, num_types, type_off, weights, src32, tgt32, pos, msg, st);
+    }
+    return tc::edge_messages(h_src, h_tgt, H, D, use_target, num_types, type_off, weights, src32, tgt32, pos, msg, scratch, pack, st);
 }
-using tcb::edge_messages;
 
 // ffma_scratch (fp32 states): >= gru_simt_bytes, for the FFMA kernel's packing
-static int gru_update(const float *agg, const float *h, int64_t rows, int H, int D, const float *w_ih, const float *w_hh,
-                      const float *b_ih, const float *b_hh, float *out, void *scratch, char *ffma_scratch, bool pack, cudaStream_t st) {
-    if (tc_enabled() && tc::supported_gru(H, D)) return tc::gru_update(agg, h, rows, H, D, w_ih, w_hh, b_ih, b_hh, out, scratch, pack, st);
-    return launch_gru_simt(agg, h, rows, H, D, w_ih, w_hh, b_ih, b_hh, out, ffma_scratch, st);
+template <typename T>
+static int gru_update(const T *agg, const T *h, int64_t rows, int H, int D, const float *w_ih, const float *w_hh, const float *b_ih,
+                      const float *b_hh, T *out, void *scratch, char *ffma_scratch, bool pack, cudaStream_t st) {
+    if constexpr (std::is_same<T, float>::value) {
+        if (!tc_enabled() || !tc::supported_gru(H, D))
+            return launch_gru_simt(agg, h, rows, H, D, w_ih, w_hh, b_ih, b_hh, out, ffma_scratch, st);
+    }
+    return tc::gru_update(agg, h, rows, H, D, w_ih, w_hh, b_ih, b_hh, out, scratch, pack, st);
 }
-static int gru_update(const __nv_bfloat16 *agg, const __nv_bfloat16 *h, int64_t rows, int H, int D, const float *w_ih,
-                      const float *w_hh, const float *b_ih, const float *b_hh, __nv_bfloat16 *out, void *scratch, char *, bool pack,
-                      cudaStream_t st) {
-    return tcb::gru_update(agg, h, rows, H, D, w_ih, w_hh, b_ih, b_hh, out, scratch, pack, st);
-}
-
-static int dense_update(const float *y, int64_t rows, int D, const float *W, const float *bias, int Hout, int act, float *out,
-                        void *scratch, cudaStream_t st) {
-    return dense_any(y, rows, D, W, bias, Hout, act, out, scratch, st);
-}
-using tcb::dense_update;
 
 // The shapes each state dtype takes.  fp32: multiples of 4 (PTGNN_E_INVALID otherwise) and, for the GRU, H % 32 == 0
 // (PTGNN_E_UNSUPPORTED otherwise).  bf16, the tensor-core tiles (PTGNN_E_UNSUPPORTED otherwise): H % 32 == 0 (>= 64),
@@ -369,10 +364,6 @@ static int check_unfused_dims(const char *who, bool bf16, int64_t N, int64_t E, 
 
 // [rows, D] messages or aggregates in the state dtype
 static size_t rows_bytes(bool bf16, int64_t rows, int D) { return ws_slice((size_t)rows * D * (bf16 ? 2 : 4) + 16, 1); }
-// the edge weights in the message kernels' format: TF32 (hi, lo) split (fp32 states) or bf16 copy
-static size_t msg_weight_bytes(bool bf16, int T, int D, int Kw) {
-    return bf16 ? tcb::edge_weight_bytes(T, D, Kw) : tc::split_edge_weights_bytes(T, D, Kw);
-}
 
 // gated workspace: msg | agg | FFMA GRU packing (fp32) | derived weights = [edge weights | GRU packing] (without a weight cache)
 struct GatedWs { size_t msg, agg, simt, weights, total; };
@@ -381,15 +372,15 @@ static GatedWs gated_layout(bool bf16, int64_t N, int64_t E, int T, int H, int D
     w.agg = rows_bytes(bf16, E, D);
     w.simt = w.agg + rows_bytes(bf16, N, D);
     w.weights = w.simt + (bf16 ? 0 : gru_simt_bytes(H, D));
-    w.total = w.weights + msg_weight_bytes(bf16, T, D, H) + (bf16 ? tcb::gru_pack_bytes(H, D) : tc::gru_pack_bytes(H + 32, D));
+    // fp32 states size the GRU packing for one gate block more than they use
+    w.total = w.weights + tc::edge_weight_bytes(bf16, T, D, H) + tc::gru_pack_bytes(bf16, bf16 ? H : H + 32, D);
     return w;
 }
 
 // gated weight cache: [edge weights | GRU packing]; 0 when fp32 states run a step on the FFMA kernels (nothing worth caching)
 static size_t gated_cache_bytes(bool bf16, int T, int H, int D) {
-    if (bf16) return tcb::edge_weight_bytes(T, D, H) + tcb::gru_pack_bytes(H, D);
-    if (!tc_enabled() || !tc::supported_message(H, D) || !tc::supported_gru(H, D)) return 0;
-    return tc::split_edge_weights_bytes(T, D, H) + tc::gru_pack_bytes(H, D);
+    if (!bf16 && (!tc_enabled() || !tc::supported_message(H, D) || !tc::supported_gru(H, D))) return 0;
+    return tc::edge_weight_bytes(bf16, T, D, H) + tc::gru_pack_bytes(bf16, H, D);
 }
 
 // Mlp workspace: msg | y (the aggregate before the dense layer) | edge weights | dense weight (derived every call, no cache)
@@ -398,8 +389,8 @@ static MlpWs mlp_layout(bool bf16, int64_t N, int64_t E, int T, int H, int D, in
     MlpWs w{};
     w.y = rows_bytes(bf16, E, D);
     w.weights = w.y + rows_bytes(bf16, N, D);
-    w.dense = w.weights + msg_weight_bytes(bf16, T, D, ut ? 2 * H : H);
-    w.total = w.dense + (bf16 ? tcb::dense_weight_bytes(Hout, D) : tc::dense_split_bytes(Hout, D));
+    w.dense = w.weights + tc::edge_weight_bytes(bf16, T, D, ut ? 2 * H : H);
+    w.total = w.dense + tc::dense_weight_bytes(bf16, Hout, D);
     return w;
 }
 
@@ -431,7 +422,7 @@ static int gated_unfused(const void *node_states, const void *gather_states, int
     rc = weight_area("gated_forward", ws + L.weights, need > 0 ? weight_cache : nullptr, weight_cache_bytes, need, cache_valid,
                      area, pack);
     if (rc) return rc;
-    char *grupack = area + msg_weight_bytes(BF16, num_types, D, H);
+    char *grupack = area + tc::edge_weight_bytes(BF16, num_types, D, H);
     const T *h = static_cast<const T *>(node_states);
     const T *hsrc = gather_states ? static_cast<const T *>(gather_states) : h;   // rows that `src32` indexes (sharded runs)
     T *msg = reinterpret_cast<T *>(ws + L.msg), *agg = reinterpret_cast<T *>(ws + L.agg);
@@ -488,7 +479,8 @@ static int mlp_unfused(const void *node_states, const void *gather_states, int64
     rc = launch_segment_reduce(msg, row_ptr, nullptr, N, E, D, reduce, y, nullptr, &epi, st);
     if (rc || !dense_weight) return rc;
     // 3. dense update
-    return dense_update(y, N, D, dense_weight, dense_bias, Hout, dense_activation, out, ws + L.dense, st);
+    if constexpr (BF16) return tc::dense_update(y, N, D, dense_weight, dense_bias, Hout, dense_activation, out, ws + L.dense, st, true);
+    else return dense_any(y, N, D, dense_weight, dense_bias, Hout, dense_activation, out, ws + L.dense, st);
 }
 
 }  // namespace ptgnn
@@ -543,7 +535,7 @@ extern "C" int ptgnn_b200_mlp_forward(int32_t bf16_states, const void *node_stat
 /* ---- stand-alone pieces (MLP.forward, message MLPs with hidden layers, module aggregators) -------------------------------------- */
 extern "C" size_t ptgnn_b200_linear_workspace_bytes(int32_t in_dim, int32_t out_dim) {
     if (in_dim <= 0 || out_dim <= 0) return 0;
-    return tc::dense_split_bytes(out_dim, in_dim) + 256;
+    return tc::dense_weight_bytes(false, out_dim, in_dim) + 256;
 }
 extern "C" int ptgnn_b200_linear_f32(const float *x, int64_t rows, int32_t in_dim, const float *weight, const float *bias,
                                      int32_t out_dim, int32_t activation, float *out, void *workspace, size_t workspace_bytes,
@@ -563,7 +555,7 @@ extern "C" int ptgnn_b200_linear_f32(const float *x, int64_t rows, int32_t in_di
 
 extern "C" size_t ptgnn_b200_edge_messages_workspace_bytes(int32_t num_types, int32_t in_dim, int32_t message_dim, int32_t use_target_state) {
     if (num_types < 0 || in_dim <= 0 || message_dim <= 0) return 0;
-    return tc::split_edge_weights_bytes(num_types, message_dim, use_target_state ? 2 * in_dim : in_dim) + 256;
+    return tc::edge_weight_bytes(false, num_types, message_dim, use_target_state ? 2 * in_dim : in_dim) + 256;
 }
 extern "C" int ptgnn_b200_edge_messages_f32(const float *source_states, const float *target_states, int32_t in_dim, int32_t message_dim,
                                             int32_t num_types, const int64_t *type_off, const int32_t *src32, const int32_t *tgt32,
@@ -587,7 +579,7 @@ extern "C" int ptgnn_b200_edge_messages_f32(const float *source_states, const fl
 
 extern "C" size_t ptgnn_b200_grucell_workspace_bytes(int32_t state_dim, int32_t input_dim) {
     if (state_dim <= 0 || input_dim <= 0) return 0;
-    return gru_simt_bytes(state_dim, input_dim) + tc::gru_pack_bytes(state_dim + 32, input_dim) + 256;
+    return gru_simt_bytes(state_dim, input_dim) + tc::gru_pack_bytes(false, state_dim + 32, input_dim) + 256;
 }
 extern "C" int ptgnn_b200_grucell_f32(const float *input, const float *hidden, int64_t rows, int32_t state_dim, int32_t input_dim,
                                       const float *w_ih, const float *w_hh, const float *b_ih, const float *b_hh, float *out,

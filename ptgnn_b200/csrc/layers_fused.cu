@@ -29,8 +29,7 @@ size_t gated_weight_bytes(int nprod, int T, int H, int D) {
 }
 // [packed edge weights | dense weight: TF32 hi / lo split (fp32) or bf16 copy]
 size_t mlp_weight_bytes(int nprod, int T, int H, int D, int Hout, int ut) {
-    const size_t dense = nprod == 3 ? tc::dense_split_bytes(Hout, D) : tcb::dense_weight_bytes(Hout, D);
-    return fused::packed_weight_bytes(nprod, T, H, ut) + dense + 256;
+    return fused::packed_weight_bytes(nprod, T, H, ut) + tc::dense_weight_bytes(nprod == 1, Hout, D) + 256;
 }
 
 // workspace: agg | packed states (gathered rows) | packed own rows (sharded run: the GRU's h) | derived weights (no cache)
@@ -204,8 +203,8 @@ int mlp_fused(int nprod, const void *node_states, const void *gather_states, int
     if (nprod == 3)
         return dense_any(static_cast<const float *>(y), N, D, dense_weight, dense_bias, Hout, dense_activation,
                          static_cast<float *>(out_states), dense_area, st, pack);
-    return tcb::dense_update(static_cast<const __nv_bfloat16 *>(y), N, D, dense_weight, dense_bias, Hout, dense_activation,
-                             static_cast<__nv_bfloat16 *>(out_states), dense_area, st);
+    return tc::dense_update(static_cast<const __nv_bfloat16 *>(y), N, D, dense_weight, dense_bias, Hout, dense_activation,
+                            static_cast<__nv_bfloat16 *>(out_states), dense_area, st, true);
 }
 
 }  // namespace

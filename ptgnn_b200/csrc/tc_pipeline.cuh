@@ -25,7 +25,7 @@
 //   __device__ static int  num_tiles(const Params&);
 //   __device__ static void tile_setup(const Params&, int tile, Tile&);
 //   __device__ static int  num_segments(const Params&, const Tile&);
-//   __device__ static Segment segment(const Params&, const Tile&, int seg);
+//   __device__ static Segment<float> segment(const Params&, const Tile&, int seg);
 //   __device__ static int  gather_row(const Params&, const Tile&, int seg, int r);   only when GATHER (then a_map == nullptr)
 //   __device__ static int  mma_groups(const Params&, const Tile&, int seg, MmaGroup (&g)[2]);
 //   __device__ static void drain(const Params&, const Tile&, const float *acc_row, int half, float (&acc)[64]);
@@ -33,7 +33,10 @@
 //   __device__ static void tile_init(Tile&);   tiles are set up in increasing order per role: tile_setup may walk forward
 //   struct Pre;  __device__ static void prefetch(const Params&, const Tile&, int quarter, int half, int lane, Pre&);
 //                          (global-memory inputs of the store -- row offset (-1 = row not stored), GRU h -- one tile ahead)
-//   __device__ static void store(const Params&, const Tile&, float (&acc)[64], const Pre&, int half, int lane, float* stage);
+//   __device__ static void smem_init(const Params&, float *tables);   bf16 pipeline only: fills its policy tables
+//   __device__ static void store(const Params&, const Tile&, float (&acc)[64], const Pre&, int half, int lane, float* stage,
+//                                float* tables);   (tables: nullptr here, the smem_init area in the bf16 pipeline)
+// The policies (layers_tc.cu) serve both pipelines; the bf16 one (tc_pipeline_bf16.cuh) takes Segment<__nv_bfloat16>.
 #pragma once
 #include <cuda.h>
 
@@ -70,14 +73,17 @@ constexpr int SMEM_BYTES = RING_BYTES + 1024 /*alignment slack*/ + BARRIER_BYTES
 static_assert(SMEM_BYTES <= 232448, "shared memory budget");
 static_assert(4 * STAGE_FLOATS_PER_WARP <= 64 * ACC_PITCH, "a warpgroup's transpose buffers fit in its accumulator rows");
 
+template <class T>       // T = float (this pipeline) or __nv_bfloat16 (tc_pipeline_bf16.cuh); element counts are in T
 struct Segment {        // one K-range of the tile's GEMM
-    const float *a;     // gathered A rows (row pitch lda) -- used when a_map == nullptr
+    const T *a;         // gathered A rows (row pitch lda) -- used when a_map == nullptr
     int lda;
-    const CUtensorMap *a_map;    // contiguous A rows: TMA box {32 cols, 128 rows} at (k, a_row0)
+    const CUtensorMap *a_map;    // contiguous A rows: TMA box {CHUNK_K cols, 128 rows} at (k, a_row0)
     int a_row0;
-    const CUtensorMap *b_hi_map, *b_lo_map;   // TMA box {32 cols, b_box_rows} at (b_col0 + k, b_row0)
+    // TMA box {CHUNK_K cols, b_box_rows} at (b_col0 + k, b_row0): B (fp32: its TF32 hi half) and the TF32 lo half of B (the
+    // bf16 pipeline ignores b_lo_map)
+    const CUtensorMap *b_map, *b_lo_map;
     int b_row0, b_col0, b_box_rows;
-    int K;              // columns of this segment (multiple of 4)
+    int K;              // columns of this segment (multiple of 4 fp32 / 8 bf16)
 };
 struct MmaGroup {       // per K-step: B rows [row_off, row_off + n) -> accumulator columns [col_off, col_off + n); col_off and
     int n, row_off, col_off;   // row_off are multiples of 32 (the accumulators are zeroed at the start of every tile)
@@ -191,7 +197,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
                 Policy::tile_setup(p, tile, t);
                 const int nseg = Policy::num_segments(p, t);
                 for (int seg = 0; seg < nseg; ++seg) {
-                    const Segment sg = Policy::segment(p, t, seg);
+                    const Segment<float> sg = Policy::segment(p, t, seg);
                     const int nkc = (sg.K + CHUNK_K - 1) / CHUNK_K;
                     const uint32_t bytes = 2u * (uint32_t)sg.b_box_rows * 128u + (sg.a_map != nullptr ? (uint32_t)OPERAND_BYTES : 0u);
                     for (int kc = 0; kc < nkc; ++kc, ++c) {
@@ -201,7 +207,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
                         const int kchunk = kc * CHUNK_K;
                         if (leader) mbar_expect_tx(&landed[slot], bytes);
                         if (sg.a_map != nullptr && leader) tma_load_2d(base, sg.a_map, kchunk, sg.a_row0, &landed[slot]);
-                        if (leader) tma_load_2d(base + B_HI_OFF, sg.b_hi_map, sg.b_col0 + kchunk, sg.b_row0, &landed[slot]);
+                        if (leader) tma_load_2d(base + B_HI_OFF, sg.b_map, sg.b_col0 + kchunk, sg.b_row0, &landed[slot]);
                         if (leader) tma_load_2d(base + B_LO_OFF, sg.b_lo_map, sg.b_col0 + kchunk, sg.b_row0, &landed[slot]);
                         __syncwarp();
                     }
@@ -246,7 +252,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
                     v0 = Policy::gather_row(p, t_next, seg_n, g);
                     v1 = Policy::gather_row(p, t_next, seg_n, g + 64);
                 }
-                const Segment sg = Policy::segment(p, t, seg);
+                const Segment<float> sg = Policy::segment(p, t, seg);
                 const int nkc = (sg.K + CHUNK_K - 1) / CHUNK_K;
                 // this thread's 16 rows of the (tile, segment): indices -> registers once, so that the per-chunk loop is just
                 // address arithmetic + LDGSTS
@@ -309,7 +315,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
                 for (int i = 0; i < 16; ++i) { acc_m[b][i] = 0.0f; acc_c[b][i] = 0.0f; }
             const int nseg = Policy::num_segments(p, t);
             for (int seg = 0; seg < nseg; ++seg) {
-                const Segment sg = Policy::segment(p, t, seg);
+                const Segment<float> sg = Policy::segment(p, t, seg);
                 MmaGroup g[2];
                 const int ng = Policy::mma_groups(p, t, seg, g);
                 const int nkc = (sg.K + CHUNK_K - 1) / CHUNK_K;
@@ -388,7 +394,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
             named_bar_sync(bar_id, 128);          // drained: the rows become the warps' transpose buffers
             // this warp's transpose buffer, addressed here rather than held across the tile loop: a pointer live through the
             // MMAs made the GRU epilogue spill
-            Policy::store(p, t, acc, pre, half, lane, acc_s + wg * 64 * ACC_PITCH + wi * STAGE_FLOATS_PER_WARP);
+            Policy::store(p, t, acc, pre, half, lane, acc_s + wg * 64 * ACC_PITCH + wi * STAGE_FLOATS_PER_WARP, nullptr);
             t = t_next;
             pre = pre_next;
         }

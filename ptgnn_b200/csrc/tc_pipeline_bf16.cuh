@@ -42,16 +42,6 @@ static_assert(SMEM_BYTES <= 232448, "shared memory budget");
 constexpr int LOADER_REGS = 104, CONSUMER_REGS = 200;
 static_assert(LOADER_REGS + 2 * CONSUMER_REGS <= 3 * 168, "register budgets exceed the launch allocation");
 
-struct Segment {        // one K-range of the tile's GEMM (all element counts in bf16)
-    const __nv_bfloat16 *a;      // gathered A rows (row pitch lda) -- used when a_map == nullptr
-    int lda;
-    const CUtensorMap *a_map;    // contiguous A rows: TMA box {64 cols, 128 rows} at (k, a_row0)
-    int a_row0;
-    const CUtensorMap *b_map;    // TMA box {64 cols, b_box_rows} at (b_col0 + k, b_row0)
-    int b_row0, b_col0, b_box_rows;
-    int K;                       // multiple of 8
-};
-
 template <class Policy>
 __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_bf16_kernel(const __grid_constant__ typename Policy::Params p) {
     extern __shared__ unsigned char smem_raw[];
@@ -79,7 +69,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_bf16_kernel(const 
         constexpr int PPT = 8;
         struct Cursor { int tile, seg, kc; };
         typename Policy::Tile t_load, t_pref, t_proc;
-        Segment sg_load, sg_proc;
+        tc::Segment<__nv_bfloat16> sg_load, sg_proc;
         int rows_load[PPT], rows_pref[PPT];
         const unsigned char *rowp[PPT];
         uint32_t soff[PPT];
@@ -129,7 +119,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_bf16_kernel(const 
             const uint32_t slot = c_load % NUM_SLOTS, use = c_load / NUM_SLOTS;
             mbar_wait(&empty[slot], (use & 1) ^ 1);
             unsigned char *base = ring + slot * SLOT_BYTES;
-            const Segment &sg = sg_load;
+            const tc::Segment<__nv_bfloat16> &sg = sg_load;
             const int kchunk = cl.kc * CHUNK_K;
             if (warp == 0) {   // single predicated statements on warp-uniform operands: no R2UR waterfall around the TMA issue
                 const CUtensorMap *am = tc::warp_uniform(sg.a_map), *bm = tc::warp_uniform(sg.b_map);
@@ -218,7 +208,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_bf16_kernel(const 
                 for (int i = 0; i < 16; ++i) acc[b][i] = 0.0f;
             const int nseg = Policy::num_segments(p, t);
             for (int seg = 0; seg < nseg; ++seg) {
-                const Segment sg = Policy::segment(p, t, seg);
+                const tc::Segment<__nv_bfloat16> sg = Policy::segment(p, t, seg);
                 MmaGroup g[2];
                 const int ng = Policy::mma_groups(p, t, seg, g);
                 const int nkc = (sg.K + CHUNK_K - 1) / CHUNK_K;
@@ -272,10 +262,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_bf16_kernel(const 
         }
     }
 }
-
-// drain helpers: the accumulator tile layout is shared with the fp32 pipeline
-using tc::drain_2x32;
-using tc::drain_4x16;
 
 }  // namespace tcb
 }  // namespace ptgnn

@@ -80,11 +80,26 @@ _MLP_WS = {
     (1000, 5000, 4, 96, 36, 0, 1): (1096192, 0),     # out_dim <= 0: the message dim for fp32 states, no size for bf16
     (123, 0, 2, 64, 128, 128, 1): (456704, 130816),
 }
+# (N, N_src (0: N), T, H, D, out_dim (0: no dense layer), use_target_state) -> workspace bytes of the fused Mlp layer, fp32 / bf16
+_MLP_FUSED_WS = {
+    (1000, 0, 17, 128, 128, 128, 0): (2269952, 846592),
+    (1000, 0, 17, 64, 128, 192, 1): (2335744, 862976),
+    (777, 500, 3, 128, 128, 0, 1): (1576960, 429056),
+    (500, 0, 5, 256, 128, 0, 0): (1555200, 489216),
+    (123, 0, 2, 64, 128, 112, 0): (275456, 93696),
+}
+# (T, H, D, out_dim, use_target_state) -> weight-cache bytes of the fused Mlp layer, fp32 / bf16 (fp32: 0 off the fused dims)
+_MLP_FUSED_CACHE = {(17, 128, 128, 128, 0): (1245440, 0), (17, 64, 128, 192, 1): (1310976, 0), (3, 128, 128, 0, 1): (524544, 0),
+                    (5, 256, 128, 0, 0): (0, 0), (2, 64, 128, 112, 0): (180480, 0)}
+# the stand-alone fp32 pieces: (in_dim, out_dim), (T, in_dim, message_dim, use_target_state), (state_dim, input_dim)
+_LINEAR_WS = {(128, 128): 131328, (36, 200): 58112, (256, 64): 131328, (32, 16): 4352, (4, 4): 768}
+_EDGE_MESSAGES_WS = {(17, 128, 128, 0): 2228480, (3, 64, 192, 1): 590080, (1, 36, 16, 0): 4864, (5, 256, 112, 1): 2294016}
+_GRUCELL_WS = {(128, 128): 1968896, (64, 36): 522496, (256, 256): 6787840, (96, 32): 854272}
 
 
 def test_unfused_layer_buffer_sizes_are_pinned():
-    """The unfused layers' workspace and weight-cache layouts, per state dtype: exact byte counts (a layout change is an ABI
-    change for callers that keep buffers across calls)."""
+    """The layers' and stand-alone pieces' workspace and weight-cache layouts, per state dtype: exact byte counts (a layout
+    change is an ABI change for callers that keep buffers across calls)."""
     import subprocess
     import sys
 
@@ -96,6 +111,16 @@ def test_unfused_layer_buffer_sizes_are_pinned():
             assert handle.ptgnn_b200_gated_weight_cache_bytes(bf16, *args) == want[bf16], (bf16, args)
         for args, want in _MLP_WS.items():
             assert handle.ptgnn_b200_mlp_workspace_bytes(bf16, *args) == want[bf16], (bf16, args)
+        for args, want in _MLP_FUSED_WS.items():
+            assert handle.ptgnn_b200_mlp_fused_workspace_bytes(bf16, *args) == want[bf16], (bf16, args)
+        for args, want in _MLP_FUSED_CACHE.items():
+            assert handle.ptgnn_b200_mlp_fused_weight_cache_bytes(bf16, *args) == want[bf16], (bf16, args)
+    for args, want in _LINEAR_WS.items():
+        assert handle.ptgnn_b200_linear_workspace_bytes(*args) == want, args
+    for args, want in _EDGE_MESSAGES_WS.items():
+        assert handle.ptgnn_b200_edge_messages_workspace_bytes(*args) == want, args
+    for args, want in _GRUCELL_WS.items():
+        assert handle.ptgnn_b200_grucell_workspace_bytes(*args) == want, args
     # PTGNN_B200_DISABLE_TC=1 (read once per process): fp32 states run on the FFMA kernels and cache nothing; bf16 unchanged
     script = ("from ptgnn_b200 import _native as N; h = N.lib(); "
               "print(h.ptgnn_b200_gated_weight_cache_bytes(0, 17, 128, 128), h.ptgnn_b200_gated_weight_cache_bytes(1, 17, 128, 128), "

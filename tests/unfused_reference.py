@@ -2,7 +2,7 @@
 them through their tile edges.
 
 The kernels: the 3xTF32 tensor-core pipeline (csrc/tc_pipeline.cuh with the message, GRU and dense policies of
-csrc/layers_tc.cu), its bf16 version (csrc/tc_pipeline_bf16.cuh, csrc/layers_bf16.cu), the FFMA kernels (csrc/layers.cu,
+csrc/layers_tc.cu), its bf16 version (csrc/tc_pipeline_bf16.cuh, same policies), the FFMA kernels (csrc/layers.cu,
 csrc/gemm_simt.cuh) and the two segmented reduces (csrc/reduce.cuh).  u = 2^-24 throughout; the sequential fp32 sum, the
 bf16 message model and the bf16 rounding window come from ``fused_reference``.  The float64 products run on whatever device
 the inputs are on (a float64 GEMM errs by ~2^-50 of the mass, far below every bound here).
