@@ -365,6 +365,27 @@ int ptgnn_b200_attention_readout_backward_f32(const float *node_states, int64_t 
                                               void *workspace, size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Chunked per-graph self-attention (reference gnn/messagepassing/selfattmessagepassing.py:59-117, MultiHeadSelfAttentionMessagePassing):
+ *   qkv [rows, heads, 2 dk + dv] (head block [a | b | v]); graph g owns rows [row_ptr[g], row_ptr[g + 1]), cut into chunks of
+ *   max_chunk consecutive rows (the last one partial); for rows i, j of the same chunk
+ *   o[i, h] = sum_j softmax_j(a_{i,h} . b_{j,h} / sqrt(dk)) v_{j,h}  [rows, heads, dv],   lse[i, h] = log sum_j exp(...)  [rows, heads] fp32.
+ *   qkv and o: fp32 (3xFP16 tensor-core products; status[0] = 1 if |qkv| >= 65504), or bf16 when bf16_states != 0 (one bf16 product,
+ *   fp32 softmax).  row_ptr: the plan of the node -> graph map (ptgnn_b200_graph_readout); its last entry must be rows.  The chunk
+ *   table is built on the device: no host synchronisation.  Deterministic (DESIGN.md §3.8).
+ *   Supported: dk, dv in {16, 32, 64, 128}, any head count, any max_chunk >= 1 (ptgnn_b200_selfatt_supported).
+ * selfatt_backward_f32: from dO = dL/do [rows, heads, dv] and the forward's o and lse, writes d_qkv [rows, heads, 2 dk + dv]
+ *   (every row, once; no atomics).  fp32 only.  The workspace size covers both calls.
+ * ---------------------------------------------------------------------------------------------- */
+int32_t ptgnn_b200_selfatt_supported(int32_t bf16_states, int32_t key_query_dim, int32_t value_dim);
+size_t ptgnn_b200_selfatt_workspace_bytes(int64_t rows, int64_t num_graphs, int32_t num_heads);
+int ptgnn_b200_selfatt_forward(int32_t bf16_states, const void *qkv, int64_t rows, int32_t num_heads, int32_t key_query_dim,
+                               int32_t value_dim, const int32_t *row_ptr, int64_t num_graphs, int64_t max_chunk, void *o, float *lse,
+                               int32_t *status, void *workspace, size_t workspace_bytes, void *stream);
+int ptgnn_b200_selfatt_backward_f32(const float *qkv, int64_t rows, int32_t num_heads, int32_t key_query_dim, int32_t value_dim,
+                                    const int32_t *row_ptr, int64_t num_graphs, int64_t max_chunk, const float *o, const float *lse,
+                                    const float *d_o, float *d_qkv, void *workspace, size_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Host-buffer convenience entry point (used for the end-to-end measurement): all pointers are HOST
  * memory; copies inputs to the device, builds the plan, runs `num_layers` GatedMessagePassingLayers
  * (layer l uses weight set l; pass the same pointers to share weights), copies the final states back

@@ -26,6 +26,7 @@ from .reduceops import (
     SimpleVarSizedElementReduce,
     WeightedSumVarSizedElementReduce,
 )
+from .selfattention import MultiHeadSelfAttentionMessagePassing
 from .residuallayers import ConcatResidualLayer, LinearResidualLayer, MeanResidualLayer
 from .scatter import scatter, scatter_add, scatter_max, scatter_mean, scatter_min, scatter_sum
 
@@ -35,6 +36,6 @@ __all__ = [
     "ConcatResidualLayer", "LinearResidualLayer", "MinibatchAssembler", "scatter", "scatter_add",
     "AbstractGlobalGraphExchange", "GruGlobalStateUpdate", "AbstractVarSizedElementReduce", "ElementsToSummaryRepresentationInput",
     "SimpleVarSizedElementReduce", "WeightedSumVarSizedElementReduce", "SelfAttentionVarSizedElementReduce",
-    "MultiheadSelfAttentionVarSizedElementReduce",
+    "MultiheadSelfAttentionVarSizedElementReduce", "MultiHeadSelfAttentionMessagePassing",
     "scatter_sum", "scatter_mean", "scatter_max", "scatter_min",
 ]

@@ -82,6 +82,12 @@ SIGNATURES = {
                                                     c_void_p, c_void_p, c_size_t, c_void_p]),
     "ptgnn_b200_attention_readout_backward_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_i64, c_void_p, c_void_p,
                                                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "ptgnn_b200_selfatt_supported": (c_i32, [c_i32, c_i32, c_i32]),
+    "ptgnn_b200_selfatt_workspace_bytes": (c_size_t, [c_i64, c_i64, c_i32]),
+    "ptgnn_b200_selfatt_forward": (ctypes.c_int, [c_i32, c_void_p, c_i64, c_i32, c_i32, c_i32, c_void_p, c_i64, c_i64, c_void_p, c_void_p,
+                                                  c_void_p, c_void_p, c_size_t, c_void_p]),
+    "ptgnn_b200_selfatt_backward_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_i32, c_void_p, c_i64, c_i64, c_void_p, c_void_p,
+                                                       c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "ptgnn_b200_gated_gnn_forward_host_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_i32,
                                                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i32, c_void_p]),
 }

@@ -540,3 +540,35 @@ class _AttentionReadoutFn(torch.autograd.Function):
 
 def attention_readout_with_grad(plan, heads, node_states, qt):
     return _AttentionReadoutFn.apply(plan, heads, node_states, qt)
+
+
+# =====================================================================================================================
+# MultiHeadSelfAttentionMessagePassing (selfattmessagepassing.py:92-117): o_i = sum_j softmax_j(a_i . b_j / sqrt(dk)) v_j within the
+# chunks of each graph, on the native kernel; the node-sized products around it are _LinearFn's.  fp32 states.
+# =====================================================================================================================
+class _SelfAttentionFn(torch.autograd.Function):
+    """o [R, heads * dv] from t [R, heads * (2 dk + dv)]; backward: d t on the native backward kernels (p re-computed from the saved
+    lse: no [L, L] tensor is kept)."""
+
+    @staticmethod
+    def forward(ctx, plan, heads, dk, dv, max_chunk, t):
+        from .selfattention import native_selfatt
+
+        td = t.detach().contiguous()
+        o, lse = native_selfatt(td, plan, heads, dk, dv, max_chunk)
+        ctx.save_for_backward(td, o, lse)
+        ctx.plan, ctx.dims = plan, (heads, dk, dv, max_chunk)
+        return o
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, d_o):
+        from .selfattention import native_selfatt_backward
+
+        t, o, lse = ctx.saved_tensors
+        d_t = native_selfatt_backward(t, ctx.plan, *ctx.dims, o, lse, d_o.contiguous().float())
+        return None, None, None, None, None, d_t
+
+
+def selfatt_with_grad(plan, heads, dk, dv, max_chunk, t):
+    return _SelfAttentionFn.apply(plan, heads, dk, dv, max_chunk, t)

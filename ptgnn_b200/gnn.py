@@ -171,13 +171,15 @@ class GraphNeuralNetwork(nn.Module):
         them in place (e.g. with ``copy_`` from pinned host memory) and call ``replay()``.  The per-type edge COUNTS are frozen at
         capture; the edge contents, the node states and -- because the plan is rebuilt inside the graph -- the graph structure
         are whatever the buffers hold at replay time.  Parameters must not change between capture and replay (eval mode).
-        With global-exchange layers the number of graphs is frozen at capture too: ``num_graphs``, or -- when it is not given --
+        With global-exchange or self-attention layers the number of graphs is frozen at capture too: ``num_graphs``, or -- when it is not given --
         ``node_to_graph_idx.max() + 1``, read once before the warm-up; ``node_to_graph_idx`` is then a static input buffer as well."""
         from .globalexchange import AbstractGlobalGraphExchange
+        from .selfattention import MultiHeadSelfAttentionMessagePassing
 
-        if num_graphs is None and any(isinstance(layer, AbstractGlobalGraphExchange) for layer in self.__message_passing_layers):
+        per_graph = (AbstractGlobalGraphExchange, MultiHeadSelfAttentionMessagePassing)
+        if num_graphs is None and any(isinstance(layer, per_graph) for layer in self.__message_passing_layers):
             if node_to_graph_idx is None:
-                raise ValueError("capture(): global-exchange layers need node_to_graph_idx")
+                raise ValueError("capture(): global-exchange and self-attention layers need node_to_graph_idx")
             num_graphs = int(node_to_graph_idx.max().item()) + 1 if node_to_graph_idx.numel() else 0
         return GraphedLayerLoop(self, node_states, adjacency_lists, node_to_graph_idx, return_all_states, num_graphs)
 

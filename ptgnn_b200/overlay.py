@@ -16,7 +16,10 @@ factories import the layer classes by module path (`implementations/typilus/trai
 5. with ``native_reducers=True`` only: re-binds ``SelfAttentionVarSizedElementReduce`` and
    ``MultiheadSelfAttentionVarSizedElementReduce`` in ``ptgnn.neuralmodels.reduceops.varsizedsummary``, in ``ptgnn.neuralmodels.reduceops``
    and in reference modules imported earlier, so that e.g. ``ptgnn.implementations.graph2seq`` builds its graph summary on the native
-   attention readout.  The default leaves every reducer the reference's.
+   attention readout.  The default leaves every reducer the reference's,
+6. with ``native_selfattention=True`` only: pre-seeds / re-binds ``MultiHeadSelfAttentionMessagePassing`` at
+   ``ptgnn.neuralmodels.gnn.messagepassing.selfattmessagepassing`` (the native chunked attention kernel, DESIGN.md §3.8) like the
+   layers of step 2.  The default leaves the reference's class in place.
 
 After ``install()``: ``import ptgnn.implementations.ppi.train`` etc. build ptgnn_b200 layers, unchanged.  ``uninstall()``
 restores the reference's classes.  The reference must be importable as ``ptgnn`` for steps 2-4 (it is not on the GPU test box;
@@ -39,6 +42,8 @@ _LAYER_MODULES = {
 }
 _REDUCER_MODULES = ("ptgnn.neuralmodels.reduceops.varsizedsummary", "ptgnn.neuralmodels.reduceops")
 _NATIVE_REDUCERS = ("SelfAttentionVarSizedElementReduce", "MultiheadSelfAttentionVarSizedElementReduce")
+_SELFATT_MODULE = "ptgnn.neuralmodels.gnn.messagepassing.selfattmessagepassing"
+_SELFATT_CLASS = "MultiHeadSelfAttentionMessagePassing"
 _saved: Dict[str, object] = {}
 
 
@@ -90,8 +95,26 @@ def _install_native_reducers() -> None:
     _rebind_everywhere(replaced)       # the two reducer modules included
 
 
-def install(force_torch_scatter: bool = False, native_reducers: bool = False) -> Dict[str, object]:
-    report: Dict[str, object] = {"torch_scatter": "real", "layers": False, "container": False, "metrics": False, "reducers": False}
+def _install_native_selfattention() -> None:
+    from . import selfattention as _sa
+
+    native = getattr(_sa, _SELFATT_CLASS)
+    replaced = {}
+    old = sys.modules.get(_SELFATT_MODULE)
+    if old is not None and not getattr(old, "__ptgnn_b200_overlay__", False):
+        _saved[_SELFATT_MODULE] = old
+        if hasattr(old, _SELFATT_CLASS):
+            replaced[getattr(old, _SELFATT_CLASS)] = native
+    m = types.ModuleType(_SELFATT_MODULE, f"ptgnn_b200 overlay of the reference module {_SELFATT_MODULE}")
+    setattr(m, _SELFATT_CLASS, native)
+    m.__ptgnn_b200_overlay__ = True
+    sys.modules[_SELFATT_MODULE] = m
+    _rebind_everywhere(replaced)
+
+
+def install(force_torch_scatter: bool = False, native_reducers: bool = False, native_selfattention: bool = False) -> Dict[str, object]:
+    report: Dict[str, object] = {"torch_scatter": "real", "layers": False, "container": False, "metrics": False, "reducers": False,
+                                 "selfattention": False}
     # 1. torch_scatter
     have_real = False
     if not force_torch_scatter:
@@ -136,6 +159,10 @@ def install(force_torch_scatter: bool = False, native_reducers: bool = False) ->
     if native_reducers:
         _install_native_reducers()
         report["reducers"] = True
+    # 6. the self-attention layer (opt-in)
+    if native_selfattention:
+        _install_native_selfattention()
+        report["selfattention"] = True
     return report
 
 
@@ -154,7 +181,7 @@ def uninstall() -> None:
                 setattr(sys.modules[mod_name], attr, val)
         else:
             sys.modules[key] = val
-    for mod_name in _LAYER_MODULES:
+    for mod_name in (*_LAYER_MODULES, _SELFATT_MODULE):
         if getattr(sys.modules.get(mod_name), "__ptgnn_b200_overlay__", False):
             del sys.modules[mod_name]
     for name in ("torch_scatter", "torch_scatter.composite"):
