@@ -386,6 +386,29 @@ int ptgnn_b200_selfatt_backward_f32(const float *qkv, int64_t rows, int32_t num_
                                     const float *d_o, float *d_qkv, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * GraphNorm (reference gnn/messagepassing/graphnorm.py:9-54), per graph g and column d:
+ *   mu = mean_{i in g} x_i,  s_i = x_i - alpha mu,  sigma^2 = mean_{i in g} s_i^2 + eps,  y_i = gamma s_i / sqrt(sigma^2) + bias
+ *   x and y [N, D]: fp32, or bf16 when bf16_states != 0 (fp32 statistics); gamma, alpha, bias [D] fp32.  row_ptr / perm: the plan
+ *   of the node -> graph map, as for ptgnn_b200_graph_readout; graph_of_node [N]: its int32 graph id per node (the plan's target
+ *   list).  mean and rstd = 1 / sqrt(sigma^2) [G, D] fp32 are written for the backward (a graph without nodes: 0 and 1 / sqrt(eps)).
+ *   No host synchronisation, no float atomics: deterministic (summation order: DESIGN.md §3.9).
+ *   Supported: D a multiple of 32 in [32, 256] (ptgnn_b200_graph_norm_supported).  gamma, alpha, bias, mean, rstd and fp32 states
+ *   16-byte aligned, bf16 states 8-byte aligned.
+ * graph_norm_backward_f32: from d_out = dL/dy [N, D] and the forward's mean and rstd (and its eps), writes d_x [N, D] and d_gamma,
+ *   d_alpha, d_bias [D] (summed over the graphs in graph order).  fp32 states only.  The workspace size covers both calls.
+ * ---------------------------------------------------------------------------------------------- */
+int32_t ptgnn_b200_graph_norm_supported(int32_t state_dim);
+size_t ptgnn_b200_graph_norm_workspace_bytes(int64_t num_nodes, int64_t num_graphs, int32_t state_dim);
+int ptgnn_b200_graph_norm_forward(int32_t bf16_states, const void *node_states, int64_t num_nodes, int32_t state_dim, const int32_t *row_ptr,
+                                  const int32_t *perm, const int32_t *graph_of_node, int64_t num_graphs, const float *gamma,
+                                  const float *alpha, const float *bias, float eps, void *out, float *mean, float *rstd, void *workspace,
+                                  size_t workspace_bytes, void *stream);
+int ptgnn_b200_graph_norm_backward_f32(const float *node_states, const float *d_out, int64_t num_nodes, int32_t state_dim,
+                                       const int32_t *row_ptr, const int32_t *perm, const int32_t *graph_of_node, int64_t num_graphs,
+                                       const float *gamma, const float *alpha, float eps, const float *mean, const float *rstd, float *d_x,
+                                       float *d_gamma, float *d_alpha, float *d_bias, void *workspace, size_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Host-buffer convenience entry point (used for the end-to-end measurement): all pointers are HOST
  * memory; copies inputs to the device, builds the plan, runs `num_layers` GatedMessagePassingLayers
  * (layer l uses weight set l; pass the same pointers to share weights), copies the final states back

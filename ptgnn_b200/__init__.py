@@ -27,6 +27,7 @@ from .reduceops import (
     WeightedSumVarSizedElementReduce,
 )
 from .selfattention import MultiHeadSelfAttentionMessagePassing
+from .graphnorm import GraphNorm
 from .residuallayers import ConcatResidualLayer, LinearResidualLayer, MeanResidualLayer
 from .scatter import scatter, scatter_add, scatter_max, scatter_mean, scatter_min, scatter_sum
 
@@ -36,6 +37,6 @@ __all__ = [
     "ConcatResidualLayer", "LinearResidualLayer", "MinibatchAssembler", "scatter", "scatter_add",
     "AbstractGlobalGraphExchange", "GruGlobalStateUpdate", "AbstractVarSizedElementReduce", "ElementsToSummaryRepresentationInput",
     "SimpleVarSizedElementReduce", "WeightedSumVarSizedElementReduce", "SelfAttentionVarSizedElementReduce",
-    "MultiheadSelfAttentionVarSizedElementReduce", "MultiHeadSelfAttentionMessagePassing",
+    "MultiheadSelfAttentionVarSizedElementReduce", "MultiHeadSelfAttentionMessagePassing", "GraphNorm",
     "scatter_sum", "scatter_mean", "scatter_max", "scatter_min",
 ]

@@ -572,3 +572,34 @@ class _SelfAttentionFn(torch.autograd.Function):
 
 def selfatt_with_grad(plan, heads, dk, dv, max_chunk, t):
     return _SelfAttentionFn.apply(plan, heads, dk, dv, max_chunk, t)
+
+
+# =====================================================================================================================
+# GraphNorm (graphnorm.py:36-46): y = gamma (x - alpha mu_g) / sqrt(sigma_g^2) + bias per graph, on the native kernels.  fp32 states.
+# =====================================================================================================================
+class _GraphNormFn(torch.autograd.Function):
+    """y [N, D] from x [N, D] and the [1, D] parameters; backward: d x and the parameter gradients on the native backward kernels
+    (the normalised states are recomputed from the saved [G, D] mean and rstd: no [N, D] tensor is kept besides x)."""
+
+    @staticmethod
+    def forward(ctx, plan, eps, x, gamma, alpha, bias):
+        from .graphnorm import native_graph_norm
+
+        xd = x.detach().contiguous()
+        y, mean, rstd = native_graph_norm(xd, plan, gamma, alpha, bias, eps)
+        ctx.save_for_backward(xd, gamma, alpha, mean, rstd)
+        ctx.plan, ctx.eps = plan, eps
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, d_y):
+        from .graphnorm import native_graph_norm_backward
+
+        x, gamma, alpha, mean, rstd = ctx.saved_tensors
+        d_x, d_gamma, d_alpha, d_bias = native_graph_norm_backward(x, ctx.plan, gamma, alpha, ctx.eps, mean, rstd, d_y.contiguous().float())
+        return None, None, d_x, d_gamma.reshape(gamma.shape), d_alpha.reshape(alpha.shape), d_bias.reshape(gamma.shape)
+
+
+def graph_norm_with_grad(plan, eps, node_states, gamma, alpha, bias):
+    return _GraphNormFn.apply(plan, eps, node_states, gamma, alpha, bias)

@@ -6,8 +6,8 @@ factories import the layer classes by module path (`implementations/typilus/trai
 
 1. registers ``ptgnn_b200.torch_scatter_shim`` as ``torch_scatter`` (if the real wheel is absent, or ``force_torch_scatter``),
 2. pre-seeds ``sys.modules`` so that ``ptgnn.neuralmodels.gnn.messagepassing.{abstract,gated,mlp}messagepassing`` and
-   ``...globalgraphexchange`` resolve to the ptgnn_b200 classes (everything else -- residual layers, PNA, GraphNorm, embedders,
-   trainers, and the reducers of ``reduceops.varsizedsummary``, whose attention variants must keep working -- stays the
+   ``...globalgraphexchange`` resolve to the ptgnn_b200 classes (everything else -- residual layers, PNA, GraphNorm (unless
+   step 7), embedders, trainers, and the reducers of ``reduceops.varsizedsummary``, whose attention variants must keep working -- stays the
    reference's; the native ``GruGlobalStateUpdate`` reads the reference's WeightedSum and Simple reducers directly), and
    re-binds those names in reference modules that were imported earlier,
 3. replaces ``GraphNeuralNetwork`` inside the reference's ``graphneuralnetwork`` module (``GraphNeuralNetworkModel`` stays),
@@ -19,7 +19,9 @@ factories import the layer classes by module path (`implementations/typilus/trai
    attention readout.  The default leaves every reducer the reference's,
 6. with ``native_selfattention=True`` only: pre-seeds / re-binds ``MultiHeadSelfAttentionMessagePassing`` at
    ``ptgnn.neuralmodels.gnn.messagepassing.selfattmessagepassing`` (the native chunked attention kernel, DESIGN.md §3.8) like the
-   layers of step 2.  The default leaves the reference's class in place.
+   layers of step 2.  The default leaves the reference's class in place,
+7. with ``native_graphnorm=True`` only: pre-seeds / re-binds ``GraphNorm`` at ``ptgnn.neuralmodels.gnn.messagepassing.graphnorm``
+   (the native per-graph normalisation kernels, DESIGN.md §3.9) in the same way.  The default leaves the reference's class in place.
 
 After ``install()``: ``import ptgnn.implementations.ppi.train`` etc. build ptgnn_b200 layers, unchanged.  ``uninstall()``
 restores the reference's classes.  The reference must be importable as ``ptgnn`` for steps 2-4 (it is not on the GPU test box;
@@ -44,6 +46,8 @@ _REDUCER_MODULES = ("ptgnn.neuralmodels.reduceops.varsizedsummary", "ptgnn.neura
 _NATIVE_REDUCERS = ("SelfAttentionVarSizedElementReduce", "MultiheadSelfAttentionVarSizedElementReduce")
 _SELFATT_MODULE = "ptgnn.neuralmodels.gnn.messagepassing.selfattmessagepassing"
 _SELFATT_CLASS = "MultiHeadSelfAttentionMessagePassing"
+_GRAPHNORM_MODULE = "ptgnn.neuralmodels.gnn.messagepassing.graphnorm"
+_GRAPHNORM_CLASS = "GraphNorm"
 _saved: Dict[str, object] = {}
 
 
@@ -95,26 +99,38 @@ def _install_native_reducers() -> None:
     _rebind_everywhere(replaced)       # the two reducer modules included
 
 
-def _install_native_selfattention() -> None:
-    from . import selfattention as _sa
-
-    native = getattr(_sa, _SELFATT_CLASS)
+def _install_native_class(mod_name: str, class_name: str, native) -> None:
+    """Pre-seeds ``mod_name`` with a module holding only ``native`` as ``class_name`` and re-binds the reference's class wherever an
+    earlier import bound it; ``uninstall()`` restores the reference's module."""
     replaced = {}
-    old = sys.modules.get(_SELFATT_MODULE)
+    old = sys.modules.get(mod_name)
     if old is not None and not getattr(old, "__ptgnn_b200_overlay__", False):
-        _saved[_SELFATT_MODULE] = old
-        if hasattr(old, _SELFATT_CLASS):
-            replaced[getattr(old, _SELFATT_CLASS)] = native
-    m = types.ModuleType(_SELFATT_MODULE, f"ptgnn_b200 overlay of the reference module {_SELFATT_MODULE}")
-    setattr(m, _SELFATT_CLASS, native)
+        _saved[mod_name] = old
+        if hasattr(old, class_name):
+            replaced[getattr(old, class_name)] = native
+    m = types.ModuleType(mod_name, f"ptgnn_b200 overlay of the reference module {mod_name}")
+    setattr(m, class_name, native)
     m.__ptgnn_b200_overlay__ = True
-    sys.modules[_SELFATT_MODULE] = m
+    sys.modules[mod_name] = m
     _rebind_everywhere(replaced)
 
 
-def install(force_torch_scatter: bool = False, native_reducers: bool = False, native_selfattention: bool = False) -> Dict[str, object]:
+def _install_native_selfattention() -> None:
+    from . import selfattention as _sa
+
+    _install_native_class(_SELFATT_MODULE, _SELFATT_CLASS, getattr(_sa, _SELFATT_CLASS))
+
+
+def _install_native_graphnorm() -> None:
+    from . import graphnorm as _gn
+
+    _install_native_class(_GRAPHNORM_MODULE, _GRAPHNORM_CLASS, getattr(_gn, _GRAPHNORM_CLASS))
+
+
+def install(force_torch_scatter: bool = False, native_reducers: bool = False, native_selfattention: bool = False,
+            native_graphnorm: bool = False) -> Dict[str, object]:
     report: Dict[str, object] = {"torch_scatter": "real", "layers": False, "container": False, "metrics": False, "reducers": False,
-                                 "selfattention": False}
+                                 "selfattention": False, "graphnorm": False}
     # 1. torch_scatter
     have_real = False
     if not force_torch_scatter:
@@ -163,6 +179,10 @@ def install(force_torch_scatter: bool = False, native_reducers: bool = False, na
     if native_selfattention:
         _install_native_selfattention()
         report["selfattention"] = True
+    # 7. GraphNorm (opt-in)
+    if native_graphnorm:
+        _install_native_graphnorm()
+        report["graphnorm"] = True
     return report
 
 
@@ -181,7 +201,7 @@ def uninstall() -> None:
                 setattr(sys.modules[mod_name], attr, val)
         else:
             sys.modules[key] = val
-    for mod_name in (*_LAYER_MODULES, _SELFATT_MODULE):
+    for mod_name in (*_LAYER_MODULES, _SELFATT_MODULE, _GRAPHNORM_MODULE):
         if getattr(sys.modules.get(mod_name), "__ptgnn_b200_overlay__", False):
             del sys.modules[mod_name]
     for name in ("torch_scatter", "torch_scatter.composite"):
