@@ -1,9 +1,9 @@
 // Per-graph attention readout (the reference's SelfAttention / MultiheadSelfAttention reducers, reduceops/varsizedsummary.py:84-178):
 //   z_{n,h} = x_n . qt[b, h]  (qt = W_{k,h}^T q_{b,h} / sqrt(d_h): a [G, heads, D] table, computed by the host on G rows)
 //   o[b, h] = sum_{n in graph b} softmax_n(z_{., h}) x_n,   lse[b, h] = log sum_{n in graph b} exp(z_{n,h})
-// so keys, values and the [N, heads, D] products never exist: the states are read once.  The chunking is readout.cu's: every graph
-// is cut into chunks of CHUNK consecutive positions of the plan's stable node order, one warp per chunk:
-//   1. readout::launch_chunk_ptr        chunk_ptr[b] = sum_{b' < b} ceil(count_b' / CHUNK)
+// so keys, values and the [N, heads, D] products never exist: the states are read once.  Every graph is cut into warp chunks of the
+// plan's node order (pergraph.cuh), one warp per chunk:
+//   1. pergraph::launch_chunk_ptr       chunk_ptr[b] = sum_{b' < b} ceil(count_b' / CHUNK)
 //   2. attn_readout_chunk_kernel        one warp per chunk, lane l holds features l, l + 32, ...: per row in node order and per head, z
 //                                       as a per-lane fmaf chain then a xor-butterfly (every lane holds the same z), and an online
 //                                       softmax (running max m, sum l, acc[D]; a new maximum rescales l and acc by expf(m_old - z))
@@ -13,42 +13,17 @@
 //                                       nodes gives o = 0 and lse = -inf.
 // Backward (fp32 states), with delta[b, h] = o . dO (computed by the warp when its chunk's graph changes):
 //   p = expf(z - lse), dp = x . dO[b, h], ds = p (dp - delta);  dx_n = sum_h p dO[b, h] + ds qt[b, h], written once per row;
-//   dqt[b, h] = sum_n ds x_n: per-chunk partials in node order, added in chunk order (readout::launch_chunk_sum).
+//   dqt[b, h] = sum_n ds x_n: per-chunk partials in node order, added in chunk order (pergraph::launch_chunk_sum).
 // No float atomics anywhere: results are bit-identical from run to run.  Summation order and error bound: DESIGN.md §3.7.
-#include <cuda_bf16.h>
 #include <math.h>
 
-#include <algorithm>
-
 #include "common.cuh"
-#include "readout.cuh"
+#include "pergraph.cuh"
 
 namespace ptgnn {
 namespace attn_readout {
 
-using readout::CHUNK;
-
-template <bool BF16>
-__device__ __forceinline__ float load_state(const void *x, long long i) {
-    if (BF16) return __bfloat162float(static_cast<const __nv_bfloat16 *>(x)[i]);
-    return __ldg(static_cast<const float *>(x) + i);
-}
-
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o >= 1; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
-// the graph of chunk c: the largest b with chunk_ptr[b] <= c (graphs without nodes have no chunk)
-__device__ __forceinline__ int graph_of_chunk(const int32_t *__restrict__ chunk_ptr, int G, int c) {
-    int lo = 0, hi = G - 1;
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (chunk_ptr[mid] <= c) lo = mid; else hi = mid - 1;
-    }
-    return lo;
-}
+using namespace pergraph;
 
 template <int VPL, int HEADS, bool BF16>
 __global__ void __launch_bounds__(256, 1) attn_readout_chunk_kernel(const void *__restrict__ x, const int32_t *__restrict__ row_ptr,
@@ -63,7 +38,7 @@ __global__ void __launch_bounds__(256, 1) attn_readout_chunk_kernel(const void *
     float q[HEADS][VPL];
     int q_graph = -1;
     for (int c = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5); c < num_chunks; c += warps) {
-        const int b = graph_of_chunk(chunk_ptr, G, c);
+        const int b = graph_of(chunk_ptr, G, c);
         if (b != q_graph) {                 // consecutive chunks of a warp mostly share their graph
 #pragma unroll
             for (int h = 0; h < HEADS; ++h)
@@ -71,8 +46,7 @@ __global__ void __launch_bounds__(256, 1) attn_readout_chunk_kernel(const void *
                 for (int k = 0; k < VPL; ++k) q[h][k] = __ldg(qt + ((long long)b * HEADS + h) * D + 32 * k + lane);
             q_graph = b;
         }
-        const int start = row_ptr[b] + (c - chunk_ptr[b]) * CHUNK;
-        const int end = min(start + CHUNK, row_ptr[b + 1]);
+        const Rows r = chunk_rows(row_ptr, chunk_ptr, b, c);
         float m[HEADS], l[HEADS], acc[HEADS][VPL];
 #pragma unroll
         for (int h = 0; h < HEADS; ++h) {
@@ -81,15 +55,10 @@ __global__ void __launch_bounds__(256, 1) attn_readout_chunk_kernel(const void *
 #pragma unroll
             for (int k = 0; k < VPL; ++k) acc[h][k] = 0.0f;
         }
-        for (int p = start; p < end; p += ROWS_AHEAD) {
-            float xv[ROWS_AHEAD][VPL];
+        for (int p = r.start; p < r.end; p += ROWS_AHEAD) {
             int node[ROWS_AHEAD];
-#pragma unroll
-            for (int u = 0; u < ROWS_AHEAD; ++u) {
-                node[u] = p + u < end ? perm[p + u] : -1;
-#pragma unroll
-                for (int k = 0; k < VPL; ++k) xv[u][k] = node[u] >= 0 ? load_state<BF16>(x, (long long)node[u] * D + 32 * k + lane) : 0.0f;
-            }
+            float xv[ROWS_AHEAD][VPL];
+            load_rows<ROWS_AHEAD, VPL, BF16>(x, perm, p, r.end, lane, node, xv);
 #pragma unroll
             for (int u = 0; u < ROWS_AHEAD; ++u) {
                 if (node[u] < 0) break;
@@ -168,7 +137,7 @@ __global__ void __launch_bounds__(32 * Bwd<VPL, HEADS>::WARPS, 1) attn_readout_b
     float lse_b[HEADS], delta[HEADS];
     int graph = -1;
     for (int c = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5); c < num_chunks; c += warps) {
-        const int b = graph_of_chunk(chunk_ptr, G, c);
+        const int b = graph_of(chunk_ptr, G, c);
         if (b != graph) {
             __syncwarp();
 #pragma unroll
@@ -188,14 +157,13 @@ __global__ void __launch_bounds__(32 * Bwd<VPL, HEADS>::WARPS, 1) attn_readout_b
             __syncwarp();
             graph = b;
         }
-        const int start = row_ptr[b] + (c - chunk_ptr[b]) * CHUNK;
-        const int end = min(start + CHUNK, row_ptr[b + 1]);
+        const Rows r = chunk_rows(row_ptr, chunk_ptr, b, c);
         float dq[HEADS][VPL];
 #pragma unroll
         for (int h = 0; h < HEADS; ++h)
 #pragma unroll
             for (int k = 0; k < VPL; ++k) dq[h][k] = 0.0f;
-        for (int p = start; p < end; ++p) {
+        for (int p = r.start; p < r.end; ++p) {
             // keeps the shared-memory rows from being hoisted out of the row loop into registers (HEADS * VPL * 2 of them)
             asm volatile("" ::: "memory");
             const long long node = perm[p];
@@ -238,14 +206,11 @@ bool supported(int D, int heads) {
     return (D == 32 || D == 64 || D == 128 || D == 256) && (heads == 1 || heads == 2 || heads == 4 || heads == 8);
 }
 
-static size_t max_chunks(int64_t N, int64_t G) { return (size_t)N / CHUNK + (size_t)G + 1; }
-
-// chunk_ptr [G + 1] | m [chunks, heads] | l [chunks, heads] | acc [chunks, heads, D]   (forward)
+// chunk_ptr [G + 1] | m [chunks, heads] | l [chunks, heads] | acc [chunks, heads, D]   (forward, chunks = N / CHUNK + G + 1)
 // chunk_ptr [G + 1] | dqt partials [chunks, heads, D]                                (backward: fits in the forward's layout)
-static size_t ws_chunk_ptr(int64_t G) { return ws_slice((size_t)G + 1, 4); }
-static size_t ws_ml(int64_t N, int64_t G, int heads) { return ws_slice(max_chunks(N, G) * heads, 4); }
+static size_t ws_ml(int64_t N, int64_t G, int heads) { return ws_slice(partial_rows(N, G) * heads, 4); }
 size_t workspace_bytes(int64_t N, int64_t G, int D, int heads) {
-    return ws_chunk_ptr(G) + 2 * ws_ml(N, G, heads) + ws_slice(max_chunks(N, G) * heads * D, 4);
+    return ws_chunk_ptr(G) + 2 * ws_ml(N, G, heads) + ws_slice(partial_rows(N, G) * heads * D, 4);
 }
 
 #define PTGNN_ATTN_HEADS(VPL, HEADS_CASE)                                                                                              \
@@ -271,15 +236,14 @@ static void launch_forward(int D, int heads, int grid, cudaStream_t st, const vo
 #undef PTGNN_FWD
 }
 
-static void launch_backward(int D, int heads, int64_t chunks, cudaStream_t st, const float *x, const int32_t *row_ptr, const int32_t *perm,
-                            const int32_t *chunk_ptr, int G, const float *qt, const float *o, const float *lse, const float *d_o,
-                            float *d_x, float *part_dq) {
-    const int64_t max_warps = (int64_t)sm_count() * 64;
+static void launch_backward(int D, int heads, int64_t N, int64_t num_graphs, cudaStream_t st, const float *x, const int32_t *row_ptr,
+                            const int32_t *perm, const int32_t *chunk_ptr, int G, const float *qt, const float *o, const float *lse,
+                            const float *d_o, float *d_x, float *part_dq) {
 #define PTGNN_BWD(V, H)                                                                                                                \
     do {                                                                                                                               \
         constexpr int W = Bwd<V, H>::WARPS;                                                                                            \
-        const int grid = (int)std::min<int64_t>(ceil_div(chunks, W), max_warps / W);                                                  \
-        attn_readout_backward_chunk_kernel<V, H><<<grid, 32 * W, 0, st>>>(x, row_ptr, perm, chunk_ptr, G, qt, o, lse, d_o, d_x, part_dq); \
+        attn_readout_backward_chunk_kernel<V, H><<<chunk_grid(N, num_graphs, W), 32 * W, 0, st>>>(x, row_ptr, perm, chunk_ptr, G, qt, o,  \
+                                                                                                  lse, d_o, d_x, part_dq);             \
     } while (0)
     PTGNN_ATTN_DISPATCH(PTGNN_BWD)
 #undef PTGNN_BWD
@@ -303,18 +267,14 @@ extern "C" size_t ptgnn_b200_attention_readout_workspace_bytes(int64_t num_nodes
 // shared argument checks of the two entry points; returns PTGNN_OK or an error code (set_error done)
 static int attn_check(const char *what, const void *x, int64_t num_nodes, int32_t D, int32_t heads, const int32_t *row_ptr, const int32_t *perm,
                       int64_t num_graphs, const float *qt, const float *o, const float *lse, void *workspace, size_t workspace_bytes) {
-    PTGNN_CHECK_ARG(num_nodes >= 0 && num_nodes < INT32_MAX && num_graphs >= 0 && num_graphs < INT32_MAX, "%s: sizes out of range", what);
+    PTGNN_CHECK_GRAPH_SIZES(what, num_nodes, num_graphs);
     if (!attn_readout::supported(D, heads)) {
         set_error("%s: state dim %d / heads %d not supported (D in {32, 64, 128, 256}, heads in {1, 2, 4, 8})", what, D, heads);
         return PTGNN_E_UNSUPPORTED;
     }
     if (num_graphs == 0) return PTGNN_OK;
     PTGNN_CHECK_ARG(row_ptr && qt && o && lse && (num_nodes == 0 || (x && perm)), "%s: null pointer", what);
-    const size_t need = attn_readout::workspace_bytes(num_nodes, num_graphs, D, heads);
-    if (workspace_bytes < need || !workspace) {
-        set_error("%s: workspace %zu < required %zu", what, workspace_bytes, need);
-        return PTGNN_E_WORKSPACE;
-    }
+    PTGNN_CHECK_WORKSPACE(what, workspace, workspace_bytes, attn_readout::workspace_bytes(num_nodes, num_graphs, D, heads));
     return PTGNN_OK;
 }
 
@@ -329,17 +289,14 @@ extern "C" int ptgnn_b200_attention_readout(int32_t bf16_states, const void *nod
     const int G = (int)num_graphs;
     char *ws = static_cast<char *>(workspace);
     int32_t *chunk_ptr = reinterpret_cast<int32_t *>(ws);
-    float *part_m = reinterpret_cast<float *>(ws + attn_readout::ws_chunk_ptr(num_graphs));
-    float *part_l = reinterpret_cast<float *>(ws + attn_readout::ws_chunk_ptr(num_graphs) + attn_readout::ws_ml(num_nodes, num_graphs, heads));
-    float *part_acc = reinterpret_cast<float *>(ws + attn_readout::ws_chunk_ptr(num_graphs) + 2 * attn_readout::ws_ml(num_nodes, num_graphs, heads));
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        readout::launch_chunk_ptr(row_ptr, G, chunk_ptr, st);
-    }
+    const size_t ml = attn_readout::ws_ml(num_nodes, num_graphs, heads);
+    float *part_m = reinterpret_cast<float *>(ws + pergraph::ws_chunk_ptr(num_graphs));
+    float *part_l = reinterpret_cast<float *>(ws + pergraph::ws_chunk_ptr(num_graphs) + ml);
+    float *part_acc = reinterpret_cast<float *>(ws + pergraph::ws_chunk_ptr(num_graphs) + 2 * ml);
+    pergraph::launch_chunk_ptr(row_ptr, G, chunk_ptr, st);
     PTGNN_LAUNCHED();
     if (num_nodes > 0) {
-        const int64_t max_chunks = num_nodes / readout::CHUNK + num_graphs;
-        const int grid = (int)std::min<int64_t>(ceil_div(max_chunks, 8), (int64_t)sm_count() * 8);
+        const int grid = pergraph::chunk_grid(num_nodes, num_graphs);
         {
             TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
             if (bf16_states) attn_readout::launch_forward<true>(D, heads, grid, st, node_states, row_ptr, perm, chunk_ptr, G, qt, part_m, part_l, part_acc);
@@ -369,24 +326,18 @@ extern "C" int ptgnn_b200_attention_readout_backward_f32(const float *node_state
     const int G = (int)num_graphs;
     char *ws = static_cast<char *>(workspace);
     int32_t *chunk_ptr = reinterpret_cast<int32_t *>(ws);
-    float *part_dq = reinterpret_cast<float *>(ws + attn_readout::ws_chunk_ptr(num_graphs));
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        readout::launch_chunk_ptr(row_ptr, G, chunk_ptr, st);
-    }
+    float *part_dq = reinterpret_cast<float *>(ws + pergraph::ws_chunk_ptr(num_graphs));
+    pergraph::launch_chunk_ptr(row_ptr, G, chunk_ptr, st);
     PTGNN_LAUNCHED();
     if (num_nodes > 0) {
         {
             TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-            attn_readout::launch_backward(D, heads, num_nodes / readout::CHUNK + num_graphs, st, node_states, row_ptr, perm, chunk_ptr, G, qt, o,
-                                          lse, d_o, d_x, part_dq);
+            attn_readout::launch_backward(D, heads, num_nodes, num_graphs, st, node_states, row_ptr, perm, chunk_ptr, G, qt, o, lse, d_o, d_x,
+                                          part_dq);
         }
         PTGNN_LAUNCHED();
     }
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        readout::launch_chunk_sum(part_dq, row_ptr, chunk_ptr, G, heads * D, d_qt, st);
-    }
+    pergraph::launch_chunk_sum(part_dq, row_ptr, chunk_ptr, G, heads * D, d_qt, st);
     PTGNN_LAUNCHED();
     return PTGNN_OK;
 }

@@ -257,10 +257,7 @@ extern "C" int ptgnn_b200_global_gru_update(int32_t bf16_states, const void *nod
     PTGNN_CHECK_ARG(num_graphs > 0, "global_gru: nodes without graphs");
     PTGNN_CHECK_ARG(node_states && graph_of_node && g && gru_w_ih && gru_w_hh && gru_b_ih && gru_b_hh && out_states, "global_gru: null pointer");
     const GlobalGruWs L = global_gru_layout(bf16_states, num_nodes, num_graphs, H, S);
-    if (workspace_bytes < L.total || !workspace) {
-        set_error("global_gru: workspace %zu < required %zu", workspace_bytes, L.total);
-        return PTGNN_E_WORKSPACE;
-    }
+    PTGNN_CHECK_WORKSPACE("global_gru", workspace, workspace_bytes, L.total);
     char *ws = static_cast<char *>(workspace);
     char *wpack = ws + L.wpack;
     bool pack = true;

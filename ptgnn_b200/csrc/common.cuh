@@ -24,6 +24,16 @@ extern std::atomic<int64_t> g_launch_count;
         }                               \
     } while (0)
 
+// Returns PTGNN_E_WORKSPACE unless `workspace` is non-null and holds at least `need` bytes.
+#define PTGNN_CHECK_WORKSPACE(what, workspace, workspace_bytes, need)                                              \
+    do {                                                                                                          \
+        const size_t need__ = (need);                                                                             \
+        if ((workspace_bytes) < need__ || !(workspace)) {                                                         \
+            ::ptgnn::set_error("%s: workspace %zu < required %zu", what, (size_t)(workspace_bytes), need__);      \
+            return PTGNN_E_WORKSPACE;                                                                             \
+        }                                                                                                         \
+    } while (0)
+
 #define PTGNN_CUDA(call)                                                                          \
     do {                                                                                          \
         cudaError_t err__ = (call);                                                               \

@@ -1,10 +1,9 @@
 // Per-graph normalisation (GraphNorm, reference gnn/messagepassing/graphnorm.py:9-54, arXiv:2009.03294), per graph g and column d:
 //   mu = mean_{i in g} x_i,   s_i = x_i - alpha mu,   sigma^2 = mean_{i in g} s_i^2 + eps,   y_i = gamma s_i / sqrt(sigma^2) + beta
 //
-// The graphs are those of the plan of (n2g, n2g) (readout.cu): row_ptr groups the nodes by graph, perm lists each graph's nodes in
-// node order, and every graph is cut into chunks of readout::CHUNK consecutive positions of that order, one warp per chunk.
+// Every graph is cut into warp chunks of the plan's node order (pergraph.cuh), one warp per chunk.
 // Forward (x read twice; no float atomics):
-//   1. readout::launch_chunk_ptr      chunk_ptr[b] = sum_{b' < b} ceil(count_b' / CHUNK)
+//   1. pergraph::launch_chunk_ptr     chunk_ptr[b] = sum_{b' < b} ceil(count_b' / CHUNK)
 //   2. graphnorm_stats_kernel         one warp per chunk: the chunk's sum over its rows in node order, its mean m_c = sum / n_c and
 //                                     M2_c = sum (x - m_c)^2 over the rows again (the second read of the chunk hits L1 / L2)
 //   3. graphnorm_combine_kernel       one thread per (graph, column): the chunks combined in chunk order by Chan's rule,
@@ -15,7 +14,7 @@
 //                                     dtype
 // Backward (fp32), from x, dy and the saved mu and rstd (x^ = s rstd is recomputed, nothing [N, D] is saved):
 //   5. graphnorm_bwd_chunk_kernel     one warp per chunk: A_c = sum dy, B_c = sum dy x^ over its rows in node order
-//   6. readout::launch_chunk_sum      A_g, B_g: the graph's partials added in chunk order
+//   6. pergraph::launch_chunk_sum     A_g, B_g: the graph's partials added in chunk order
 //   7. graphnorm_bwd_graph_kernel     k = gamma rstd, S_g = k (A - (1 - alpha) mu rstd B) (= sum_i dL/ds_i), c1 = B / n, c2 = alpha S / n;
 //                                     a one-node graph takes 1 - x^2 = eps rstd^2 instead of cancelling it: k = gamma rstd eps rstd^2 (1 - alpha),
 //                                     c1 = c2 = 0, S = gamma rstd eps rstd^2 A
@@ -28,36 +27,21 @@
 #include <algorithm>
 
 #include "common.cuh"
-#include "readout.cuh"
+#include "pergraph.cuh"
 
 namespace ptgnn {
 namespace graphnorm {
 
-using readout::CHUNK;
+using namespace pergraph;
 constexpr int ROWS_AHEAD = 4;       // rows whose loads a warp issues before it consumes the first of them
-
-template <bool BF16>
-__device__ __forceinline__ float load_x(const void *x, long long i) {
-    if (BF16) return __bfloat162float(static_cast<const __nv_bfloat16 *>(x)[i]);
-    return __ldg(static_cast<const float *>(x) + i);
-}
-
-// the graph of chunk c: the largest b with chunk_ptr[b] <= c (graphs without nodes own no chunk)
-__device__ __forceinline__ int graph_of_chunk(const int32_t *__restrict__ chunk_ptr, int G, int c) {
-    int lo = 0, hi = G - 1;
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (chunk_ptr[mid] <= c) lo = mid; else hi = mid - 1;
-    }
-    return lo;
-}
 
 // t = (1 - alpha) mu and s = (x - mu) + t: the forward's and the backward's shifted value, with the t of sigma^2 (so that a graph whose
 // rows all equal mu gets s = t exactly, consistent with its sigma^2 = t^2 + eps, and s = 0 when alpha = 1)
 __device__ __forceinline__ float shift_of(float a, float mu) { return __fmul_rn(__fsub_rn(1.0f, a), mu); }
 __device__ __forceinline__ float shifted(float x, float a, float mu) { return __fadd_rn(__fsub_rn(x, mu), shift_of(a, mu)); }
 
-// lane l holds columns l, l + 32, ..., l + 32 (VPL - 1): every warp-wide load is one coalesced row segment.
+// lane l holds columns l, l + 32, ..., l + 32 (VPL - 1), as in pergraph::load_rows.  The row loops below keep a scalar node per row
+// instead of calling load_rows: nvcc compiles these two kernels to longer code from the shared form.
 // partial[c] = [mean_c (D) | M2_c (D)]
 template <int VPL, bool BF16>
 __global__ void __launch_bounds__(256) graphnorm_stats_kernel(const void *__restrict__ x, const int32_t *__restrict__ row_ptr,
@@ -68,44 +52,42 @@ __global__ void __launch_bounds__(256) graphnorm_stats_kernel(const void *__rest
     const int warps = (int)(gridDim.x * blockDim.x) >> 5;
     const int num_chunks = chunk_ptr[G];
     for (int c = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5); c < num_chunks; c += warps) {
-        const int b = graph_of_chunk(chunk_ptr, G, c);
-        const int start = row_ptr[b] + (c - chunk_ptr[b]) * CHUNK;
-        const int end = min(start + CHUNK, row_ptr[b + 1]);
+        const Rows r = chunk_rows(row_ptr, chunk_ptr, graph_of(chunk_ptr, G, c), c);
         float acc[VPL];
 #pragma unroll
         for (int k = 0; k < VPL; ++k) acc[k] = 0.0f;
-        for (int p = start; p < end; p += ROWS_AHEAD) {
+        for (int p = r.start; p < r.end; p += ROWS_AHEAD) {
             float xv[ROWS_AHEAD][VPL];
 #pragma unroll
             for (int u = 0; u < ROWS_AHEAD; ++u) {
-                const int node = p + u < end ? perm[p + u] : -1;
+                const int node = p + u < r.end ? perm[p + u] : -1;
 #pragma unroll
-                for (int k = 0; k < VPL; ++k) xv[u][k] = node >= 0 ? load_x<BF16>(x, (long long)node * D + 32 * k + lane) : 0.0f;
+                for (int k = 0; k < VPL; ++k) xv[u][k] = node >= 0 ? load_state<BF16>(x, (long long)node * D + 32 * k + lane) : 0.0f;
             }
 #pragma unroll
             for (int u = 0; u < ROWS_AHEAD; ++u)
-                if (p + u < end)
+                if (p + u < r.end)
 #pragma unroll
                     for (int k = 0; k < VPL; ++k) acc[k] = __fadd_rn(acc[k], xv[u][k]);
         }
-        const float n = (float)(end - start);
+        const float n = (float)(r.end - r.start);
         float mean[VPL], m2[VPL];
 #pragma unroll
         for (int k = 0; k < VPL; ++k) {
             mean[k] = __fdiv_rn(acc[k], n);
             m2[k] = 0.0f;
         }
-        for (int p = start; p < end; p += ROWS_AHEAD) {
+        for (int p = r.start; p < r.end; p += ROWS_AHEAD) {
             float xv[ROWS_AHEAD][VPL];
 #pragma unroll
             for (int u = 0; u < ROWS_AHEAD; ++u) {
-                const int node = p + u < end ? perm[p + u] : -1;
+                const int node = p + u < r.end ? perm[p + u] : -1;
 #pragma unroll
-                for (int k = 0; k < VPL; ++k) xv[u][k] = node >= 0 ? load_x<BF16>(x, (long long)node * D + 32 * k + lane) : 0.0f;
+                for (int k = 0; k < VPL; ++k) xv[u][k] = node >= 0 ? load_state<BF16>(x, (long long)node * D + 32 * k + lane) : 0.0f;
             }
 #pragma unroll
             for (int u = 0; u < ROWS_AHEAD; ++u)
-                if (p + u < end)
+                if (p + u < r.end)
 #pragma unroll
                     for (int k = 0; k < VPL; ++k) {
                         const float d = __fsub_rn(xv[u][k], mean[k]);
@@ -213,9 +195,8 @@ __global__ void __launch_bounds__(256) graphnorm_bwd_chunk_kernel(const float *_
 #pragma unroll
     for (int k = 0; k < VPL; ++k) av[k] = alpha[32 * k + lane];
     for (int c = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5); c < num_chunks; c += warps) {
-        const int b = graph_of_chunk(chunk_ptr, G, c);
-        const int start = row_ptr[b] + (c - chunk_ptr[b]) * CHUNK;
-        const int end = min(start + CHUNK, row_ptr[b + 1]);
+        const int b = graph_of(chunk_ptr, G, c);
+        const Rows rows = chunk_rows(row_ptr, chunk_ptr, b, c);
         float mu[VPL], r[VPL], A[VPL], B[VPL];
 #pragma unroll
         for (int k = 0; k < VPL; ++k) {
@@ -224,11 +205,11 @@ __global__ void __launch_bounds__(256) graphnorm_bwd_chunk_kernel(const float *_
             A[k] = 0.0f;
             B[k] = 0.0f;
         }
-        for (int p = start; p < end; p += ROWS_AHEAD) {
+        for (int p = rows.start; p < rows.end; p += ROWS_AHEAD) {
             float xv[ROWS_AHEAD][VPL], gv[ROWS_AHEAD][VPL];
 #pragma unroll
             for (int u = 0; u < ROWS_AHEAD; ++u) {
-                const int node = p + u < end ? perm[p + u] : -1;
+                const int node = p + u < rows.end ? perm[p + u] : -1;
 #pragma unroll
                 for (int k = 0; k < VPL; ++k) {
                     const long long o = (long long)node * D + 32 * k + lane;
@@ -238,7 +219,7 @@ __global__ void __launch_bounds__(256) graphnorm_bwd_chunk_kernel(const float *_
             }
 #pragma unroll
             for (int u = 0; u < ROWS_AHEAD; ++u)
-                if (p + u < end)
+                if (p + u < rows.end)
 #pragma unroll
                     for (int k = 0; k < VPL; ++k) {
                         const float xhat = __fmul_rn(shifted(xv[u][k], av[k], mu[k]), r[k]);
@@ -330,42 +311,27 @@ __global__ void __launch_bounds__(256) graphnorm_param_grad_kernel(const float *
 
 bool supported(int D) { return D % 32 == 0 && D >= 32 && D <= 256; }
 
-// chunk_ptr [G + 1] | partial [N / CHUNK + G, 2 D] | AB [G, 2 D] | coef [4, G, D]  (the forward uses the first two)
-static size_t ws_chunk_ptr(int64_t G) { return ws_slice((size_t)G + 1, 4); }
-static size_t ws_partial(int64_t N, int64_t G, int D) { return ws_slice(((size_t)N / CHUNK + (size_t)G + 1) * 2 * D, 4); }
+// chunk_ptr [G + 1] | partial [N / CHUNK + G + 1, 2 D] | AB [G, 2 D] | coef [4, G, D]  (the forward uses the first two)
+static size_t ws_partial(int64_t N, int64_t G, int D) { return ws_slice(partial_rows(N, G) * 2 * D, 4); }
 static size_t ws_ab(int64_t G, int D) { return ws_slice((size_t)G * 2 * D, 4); }
 size_t workspace_bytes(int64_t N, int64_t G, int D) { return ws_chunk_ptr(G) + ws_partial(N, G, D) + ws_ab(G, D) + ws_slice((size_t)G * 4 * D, 4); }
 
-static int chunk_grid(int64_t N, int64_t G) { return (int)std::min<int64_t>(ceil_div(N / CHUNK + G, 8), 132 * 8); }
 static int flat_grid(long long groups) { return (int)std::min<long long>(ceil_div(groups, 256), (long long)sm_count() * 16); }
-
-#define PTGNN_GN_VPL(LAUNCH) \
-    switch (D / 32) {        \
-        case 1: LAUNCH(1); break; \
-        case 2: LAUNCH(2); break; \
-        case 3: LAUNCH(3); break; \
-        case 4: LAUNCH(4); break; \
-        case 5: LAUNCH(5); break; \
-        case 6: LAUNCH(6); break; \
-        case 7: LAUNCH(7); break; \
-        default: LAUNCH(8); break; \
-    }
 
 template <bool BF16>
 static void launch_stats(int D, int grid, cudaStream_t st, const void *x, const int32_t *row_ptr, const int32_t *perm, const int32_t *chunk_ptr,
                          int G, float *partial) {
 #define PTGNN_GN_STATS(V) graphnorm_stats_kernel<V, BF16><<<grid, 256, 0, st>>>(x, row_ptr, perm, chunk_ptr, G, partial)
-    PTGNN_GN_VPL(PTGNN_GN_STATS)
+    PTGNN_VPL_DISPATCH(D, PTGNN_GN_STATS)
 #undef PTGNN_GN_STATS
 }
 
 static void launch_bwd_chunks(int D, int grid, cudaStream_t st, const float *x, const float *dy, const int32_t *row_ptr, const int32_t *perm,
                               const int32_t *chunk_ptr, int G, const float *mean, const float *rstd, const float *alpha, float *partial) {
 #define PTGNN_GN_BWD(V) graphnorm_bwd_chunk_kernel<V><<<grid, 256, 0, st>>>(x, dy, row_ptr, perm, chunk_ptr, G, mean, rstd, alpha, partial)
-    PTGNN_GN_VPL(PTGNN_GN_BWD)
+    PTGNN_VPL_DISPATCH(D, PTGNN_GN_BWD)
 #undef PTGNN_GN_BWD
 }
-#undef PTGNN_GN_VPL
 
 }  // namespace graphnorm
 }  // namespace ptgnn
@@ -385,7 +351,7 @@ static bool aligned16(const void *p) { return ((uintptr_t)p & 15) == 0; }
 static int graph_norm_check(const char *what, const void *x, int64_t num_nodes, int32_t D, const int32_t *row_ptr, const int32_t *perm,
                             const int32_t *graph_of_node, int64_t num_graphs, const float *gamma, const float *alpha, const float *mean,
                             const float *rstd, void *workspace, size_t workspace_bytes) {
-    PTGNN_CHECK_ARG(num_nodes >= 0 && num_nodes < INT32_MAX && num_graphs >= 0 && num_graphs < INT32_MAX, "%s: sizes out of range", what);
+    PTGNN_CHECK_GRAPH_SIZES(what, num_nodes, num_graphs);
     if (!graphnorm::supported(D)) {
         set_error("%s: state dim %d must be a multiple of 32 in [32, 256]", what, D);
         return PTGNN_E_UNSUPPORTED;
@@ -395,11 +361,7 @@ static int graph_norm_check(const char *what, const void *x, int64_t num_nodes, 
     PTGNN_CHECK_ARG(row_ptr && gamma && alpha && mean && rstd && (num_nodes == 0 || (x && perm && graph_of_node)), "%s: null pointer", what);
     PTGNN_CHECK_ARG(aligned16(gamma) && aligned16(alpha) && aligned16(mean) && aligned16(rstd) && ((uintptr_t)x & 7) == 0,
                     "%s: gamma, alpha, mean and rstd must be 16-byte aligned, the states 8-byte aligned", what);
-    const size_t need = graphnorm::workspace_bytes(num_nodes, num_graphs, D);
-    if (workspace_bytes < need || !workspace) {
-        set_error("%s: workspace %zu < required %zu", what, workspace_bytes, need);
-        return PTGNN_E_WORKSPACE;
-    }
+    PTGNN_CHECK_WORKSPACE(what, workspace, workspace_bytes, graphnorm::workspace_bytes(num_nodes, num_graphs, D));
     return PTGNN_OK;
 }
 
@@ -415,13 +377,10 @@ extern "C" int ptgnn_b200_graph_norm_forward(int32_t bf16_states, const void *no
     const int G = (int)num_graphs, D = state_dim;
     char *ws = static_cast<char *>(workspace);
     int32_t *chunk_ptr = reinterpret_cast<int32_t *>(ws);
-    float *partial = reinterpret_cast<float *>(ws + graphnorm::ws_chunk_ptr(num_graphs));
+    float *partial = reinterpret_cast<float *>(ws + pergraph::ws_chunk_ptr(num_graphs));
     const long long groups = num_nodes * D / 4;
-    const int grid_c = graphnorm::chunk_grid(num_nodes, num_graphs), grid_f = graphnorm::flat_grid(groups);
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        readout::launch_chunk_ptr(row_ptr, G, chunk_ptr, st);
-    }
+    const int grid_c = pergraph::chunk_grid(num_nodes, num_graphs), grid_f = graphnorm::flat_grid(groups);
+    pergraph::launch_chunk_ptr(row_ptr, G, chunk_ptr, st);
     PTGNN_LAUNCHED();
     if (num_nodes > 0) {
         {
@@ -471,17 +430,14 @@ extern "C" int ptgnn_b200_graph_norm_backward_f32(const float *node_states, cons
     }
     char *ws = static_cast<char *>(workspace);
     int32_t *chunk_ptr = reinterpret_cast<int32_t *>(ws);
-    ws += graphnorm::ws_chunk_ptr(num_graphs);
+    ws += pergraph::ws_chunk_ptr(num_graphs);
     float *partial = reinterpret_cast<float *>(ws);
     ws += graphnorm::ws_partial(num_nodes, num_graphs, D);
     float *AB = reinterpret_cast<float *>(ws);
     float *coef = reinterpret_cast<float *>(ws + graphnorm::ws_ab(num_graphs, D));
     const long long groups = num_nodes * D / 4;
-    const int grid_c = graphnorm::chunk_grid(num_nodes, num_graphs), grid_f = graphnorm::flat_grid(groups);
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        readout::launch_chunk_ptr(row_ptr, G, chunk_ptr, st);
-    }
+    const int grid_c = pergraph::chunk_grid(num_nodes, num_graphs), grid_f = graphnorm::flat_grid(groups);
+    pergraph::launch_chunk_ptr(row_ptr, G, chunk_ptr, st);
     PTGNN_LAUNCHED();
     if (num_nodes > 0) {
         {
@@ -490,10 +446,7 @@ extern "C" int ptgnn_b200_graph_norm_backward_f32(const float *node_states, cons
         }
         PTGNN_LAUNCHED();
     }
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        readout::launch_chunk_sum(partial, row_ptr, chunk_ptr, G, 2 * D, AB, st);
-    }
+    pergraph::launch_chunk_sum(partial, row_ptr, chunk_ptr, G, 2 * D, AB, st);
     PTGNN_LAUNCHED();
     {
         TimedScope timed__(PTGNN_KERNEL_REDUCE, st);

@@ -410,10 +410,7 @@ static int gated_unfused(const void *node_states, const void *gather_states, int
     PTGNN_CHECK_ARG(node_states && out_states && row_ptr && w_ih && w_hh && b_ih && b_hh, "gated_forward: null pointer");
     PTGNN_CHECK_ARG(E == 0 || (pos && src32 && edge_weights), "gated_forward: null edge arrays");
     const GatedWs L = gated_layout(BF16, N, E, num_types, H, D);
-    if (workspace_bytes < L.total || !workspace) {
-        set_error("gated_forward: workspace %zu < required %zu", workspace_bytes, L.total);
-        return PTGNN_E_WORKSPACE;
-    }
+    PTGNN_CHECK_WORKSPACE("gated_forward", workspace, workspace_bytes, L.total);
     char *ws = static_cast<char *>(workspace);
     // a weight cache is not used for dims that have nothing to cache
     const size_t need = gated_cache_bytes(BF16, num_types, H, D);
@@ -458,10 +455,7 @@ static int mlp_unfused(const void *node_states, const void *gather_states, int64
     PTGNN_CHECK_ARG(node_states && out_states && row_ptr, "mlp_forward: null pointer");
     PTGNN_CHECK_ARG(E == 0 || (pos && src32 && edge_weights && (!ut || tgt32)), "mlp_forward: null edge arrays");
     const MlpWs L = mlp_layout(BF16, N, E, num_types, H, D, Hout, ut);
-    if (workspace_bytes < L.total || !workspace) {
-        set_error("mlp_forward: workspace %zu < required %zu", workspace_bytes, L.total);
-        return PTGNN_E_WORKSPACE;
-    }
+    PTGNN_CHECK_WORKSPACE("mlp_forward", workspace, workspace_bytes, L.total);
     char *ws = static_cast<char *>(workspace);
     const T *h = static_cast<const T *>(node_states);
     const T *hsrc = gather_states ? static_cast<const T *>(gather_states) : h;   // rows that `src32` indexes (sharded runs)

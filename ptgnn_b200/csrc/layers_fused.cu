@@ -83,10 +83,7 @@ int gated_fused(int nprod, const void *node_states, const void *gather_states, c
     PTGNN_CHECK_ARG(bp->group_off && edge_weights && T > 0, "gated_forward_fused: null block plan arrays");
     if (Ns <= 0) Ns = N;
     const GatedWs L = gated_layout(nprod, N, Ns, T, H, D);
-    if (workspace_bytes < L.total || !workspace) {
-        set_error("gated_forward_fused: workspace %zu < required %zu", workspace_bytes, L.total);
-        return PTGNN_E_WORKSPACE;
-    }
+    PTGNN_CHECK_WORKSPACE("gated_forward_fused", workspace, workspace_bytes, L.total);
     char *ws = static_cast<char *>(workspace);
     char *wpack;
     bool pack;
@@ -161,10 +158,7 @@ int mlp_fused(int nprod, const void *node_states, const void *gather_states, int
     PTGNN_CHECK_ARG(bp->group_off && edge_weights && T > 0, "mlp_forward_fused: null block plan arrays");
     if (Ns <= 0) Ns = N;
     const MlpWs L = mlp_layout(nprod, N, Ns, T, H, D, Hout, ut);
-    if (workspace_bytes < L.total || !workspace) {
-        set_error("mlp_forward_fused: workspace %zu < required %zu", workspace_bytes, L.total);
-        return PTGNN_E_WORKSPACE;
-    }
+    PTGNN_CHECK_WORKSPACE("mlp_forward_fused", workspace, workspace_bytes, L.total);
     char *ws = static_cast<char *>(workspace);
     char *wpack;
     bool pack;

@@ -384,10 +384,7 @@ static int plan_build_phases(int phases, int64_t num_nodes, int64_t num_source_n
     for (int t = num_types + 1; t <= PTGNN_MAX_EDGE_TYPES; ++t) { tabs.off[t] = E; toff.off[t] = (int32_t)E; }
 
     const PlanWs L = plan_ws_layout(num_nodes, E);
-    if (workspace_bytes < L.total || (L.total && !workspace)) {
-        set_error("plan_build: workspace %zu < required %zu", workspace_bytes, L.total);
-        return PTGNN_E_WORKSPACE;
-    }
+    PTGNN_CHECK_WORKSPACE("plan_build", workspace, workspace_bytes, L.total);
     char *ws = static_cast<char *>(workspace);
     int32_t *deg = reinterpret_cast<int32_t *>(ws + L.deg);
 
@@ -469,10 +466,7 @@ extern "C" int ptgnn_b200_block_plan_build(int64_t num_nodes, int32_t num_types,
                     (long long)nblk, T, B);
     PTGNN_CHECK_ARG(group_off, "block_plan_build: null group_off");
     const BlockPlanWs L = block_plan_ws_layout(num_nodes, E, T, B);
-    if (workspace_bytes < L.total || !workspace) {
-        set_error("block_plan_build: workspace %zu < required %zu", workspace_bytes, L.total);
-        return PTGNN_E_WORKSPACE;
-    }
+    PTGNN_CHECK_WORKSPACE("block_plan_build", workspace, workspace_bytes, L.total);
     PTGNN_CUDA(cudaMemsetAsync(group_off, 0, sizeof(int32_t) * (size_t)(groups + 1), st));
     if (E == 0 || num_nodes == 0) return PTGNN_OK;
     PTGNN_CHECK_ARG(src32 && tgt32 && src_f && tl_f, "block_plan_build: null edge array");

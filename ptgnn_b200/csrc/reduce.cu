@@ -141,10 +141,7 @@ extern "C" int ptgnn_b200_scatter_f32(const float *src, const int64_t *index, in
                                       int64_t num_nodes, int32_t reduce, float *out, int64_t *arg_out, int32_t *status,
                                       void *workspace, size_t workspace_bytes, void *stream) {
     const ScatterWs L = scatter_ws_layout(num_nodes, num_edges);
-    if (workspace_bytes < L.total || !workspace) {
-        set_error("scatter: workspace %zu < required %zu", workspace_bytes, L.total);
-        return PTGNN_E_WORKSPACE;
-    }
+    PTGNN_CHECK_WORKSPACE("scatter", workspace, workspace_bytes, L.total);
     char *ws = static_cast<char *>(workspace);
     auto p32 = [&](size_t off) { return reinterpret_cast<int32_t *>(ws + off); };
     // torch_scatter treats `index` as both the (unused) source and the target list: a 1-type edge set.

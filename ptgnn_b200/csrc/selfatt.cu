@@ -3,7 +3,7 @@
 //   s_ij = a_i . b_j / sqrt(dk),  p_ij = softmax_j(s_ij),  o_i = sum_j p_ij v_j   for i, j in the same chunk,
 // where graph g owns the row range [off_g, off_g + c_g) (off = the plan's row_ptr of (n2g, n2g)) and that range is cut into chunks
 // of L = max_num_nodes consecutive rows, the last one partial.  Every chunk is cut into tiles of 64 rows; the tile table
-// (selfatt_tile_ptr_kernel, one CTA, exclusive scan: tile_ptr[g] = sum_{g' < g} tiles(c_g')) is built on the device, so no count
+// (pergraph::item_ptr_kernel, one CTA, exclusive scan: tile_ptr[g] = sum_{g' < g} tiles(c_g')) is built on the device, so no count
 // is read by the host.  The launch bound ceil(R / 64) + ceil(R / L) + G covers every tile; CTAs past tile_ptr[G] exit.
 //
 // Forward (one warpgroup per (tile of query rows i, head)): the query tile's a rows sit in shared memory (SWIZZLE_128B K-major,
@@ -30,53 +30,13 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "pergraph.cuh"
 #include "tc_common.cuh"
 
 namespace ptgnn {
 namespace selfatt {
 
 constexpr int TILE = 64;    // rows of a query tile, and of the backward's key tiles
-
-__device__ __forceinline__ int graph_tiles(int count, int L) {
-    const int tpc = (L + TILE - 1) / TILE;
-    return (count / L) * tpc + (count % L + TILE - 1) / TILE;
-}
-
-__global__ void __launch_bounds__(1024) selfatt_tile_ptr_kernel(const int32_t *__restrict__ row_ptr, int G, int L, int32_t *__restrict__ tile_ptr) {
-    __shared__ int32_t warp_sums[32];
-    __shared__ int32_t carry;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    for (int base = 0; base < G; base += 1024) {
-        const int b = base + (int)threadIdx.x;
-        const int c = b < G ? graph_tiles(row_ptr[b + 1] - row_ptr[b], L) : 0;
-        int v = c;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int t = __shfl_up_sync(0xffffffffu, v, o);
-            if (lane >= o) v += t;
-        }
-        if (lane == 31) warp_sums[warp] = v;
-        __syncthreads();
-        if (warp == 0) {
-            int w = warp_sums[lane];
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const int t = __shfl_up_sync(0xffffffffu, w, o);
-                if (lane >= o) w += t;
-            }
-            warp_sums[lane] = w;
-        }
-        __syncthreads();
-        const int excl = carry + (warp ? warp_sums[warp - 1] : 0) + v - c;
-        if (b < G) tile_ptr[b] = excl;
-        __syncthreads();
-        if (threadIdx.x == 1023) carry = excl + c;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) tile_ptr[G] = carry;
-}
 
 struct Tile {
     int start, end;     // the chunk: rows [start, end)
@@ -86,11 +46,7 @@ struct Tile {
 // tile t -> its graph (the largest g with tile_ptr[g] <= t: graphs without nodes have no tile), chunk and rows
 __device__ __forceinline__ bool tile_of(const int32_t *__restrict__ row_ptr, const int32_t *__restrict__ tile_ptr, int G, int L, int t, Tile &tl) {
     if (t >= tile_ptr[G]) return false;
-    int lo = 0, hi = G - 1;
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (tile_ptr[mid] <= t) lo = mid; else hi = mid - 1;
-    }
+    const int lo = pergraph::graph_of(tile_ptr, G, t);
     const int lt = t - tile_ptr[lo], tpc = (L + TILE - 1) / TILE;
     tl.start = row_ptr[lo] + (lt / tpc) * L;
     tl.end = row_ptr[lo + 1] - tl.start > L ? tl.start + L : row_ptr[lo + 1];
@@ -545,12 +501,17 @@ bool supported(int dk, int dv) {
     return ok(dk) && ok(dv);
 }
 
+// tile_ptr[g] = sum_{g' < g} tiles(c_g'), tile_ptr[G] = the number of tiles
+static void launch_tile_ptr(const int32_t *row_ptr, int G, int L, int32_t *tile_ptr, cudaStream_t st) {
+    TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
+    pergraph::item_ptr_kernel<<<1, 1024, 0, st>>>(row_ptr, G, pergraph::ChunkTiles<TILE>{L}, tile_ptr);
+}
+
 // tile bound: sum_g tiles(c_g) <= sum_g (c_g / 64 + c_g / L + 1) <= ceil(R / 64) + ceil(R / L) + G
 static int64_t max_tiles(int64_t rows, int64_t G, int64_t L) { return ceil_div(rows, TILE) + ceil_div(rows, L) + G; }
 
 // tile_ptr [G + 1] | delta [rows, heads] (backward)
-static size_t ws_tile_ptr(int64_t G) { return ws_slice((size_t)G + 1, 4); }
-size_t workspace_bytes(int64_t rows, int64_t G, int heads) { return ws_tile_ptr(G) + ws_slice((size_t)rows * heads, 4); }
+size_t workspace_bytes(int64_t rows, int64_t G, int heads) { return pergraph::ws_chunk_ptr(G) + ws_slice((size_t)rows * heads, 4); }
 
 #define PTGNN_SELFATT_DV(DK, CASE)                                                                                                     \
     switch (dv) {                                                                                                                      \
@@ -631,11 +592,7 @@ static int selfatt_check(const char *what, const void *qkv, int64_t rows, int32_
     }
     if (num_graphs == 0 || rows == 0) return PTGNN_OK;
     PTGNN_CHECK_ARG(qkv && row_ptr && o && lse, "%s: null pointer", what);
-    const size_t need = selfatt::workspace_bytes(rows, num_graphs, heads);
-    if (workspace_bytes < need || !workspace) {
-        set_error("%s: workspace %zu < required %zu", what, workspace_bytes, need);
-        return PTGNN_E_WORKSPACE;
-    }
+    PTGNN_CHECK_WORKSPACE(what, workspace, workspace_bytes, selfatt::workspace_bytes(rows, num_graphs, heads));
     return PTGNN_OK;
 }
 
@@ -648,10 +605,7 @@ extern "C" int ptgnn_b200_selfatt_forward(int32_t bf16_states, const void *qkv, 
     if (rc != PTGNN_OK || num_graphs == 0 || rows == 0) return rc;
     const int G = (int)num_graphs, L = (int)std::min<int64_t>(max_chunk, rows);   // a chunk never holds more than `rows` rows
     int32_t *tile_ptr = static_cast<int32_t *>(workspace);
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        selfatt::selfatt_tile_ptr_kernel<<<1, 1024, 0, st>>>(row_ptr, G, L, tile_ptr);
-    }
+    selfatt::launch_tile_ptr(row_ptr, G, L, tile_ptr, st);
     PTGNN_LAUNCHED();
     const dim3 grid((unsigned)selfatt::max_tiles(rows, num_graphs, L), (unsigned)num_heads);
     const float sqrt_dk = sqrtf((float)key_query_dim);
@@ -677,11 +631,8 @@ extern "C" int ptgnn_b200_selfatt_backward_f32(const float *qkv, int64_t rows, i
     const int G = (int)num_graphs, L = (int)std::min<int64_t>(max_chunk, rows);
     char *ws = static_cast<char *>(workspace);
     int32_t *tile_ptr = reinterpret_cast<int32_t *>(ws);
-    float *delta = reinterpret_cast<float *>(ws + selfatt::ws_tile_ptr(num_graphs));
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        selfatt::selfatt_tile_ptr_kernel<<<1, 1024, 0, st>>>(row_ptr, G, L, tile_ptr);
-    }
+    float *delta = reinterpret_cast<float *>(ws + pergraph::ws_chunk_ptr(num_graphs));
+    selfatt::launch_tile_ptr(row_ptr, G, L, tile_ptr, st);
     PTGNN_LAUNCHED();
     const long long rh = (long long)rows * num_heads;
     {

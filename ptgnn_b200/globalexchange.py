@@ -52,6 +52,25 @@ def num_graphs_of(node_to_graph_idx: torch.Tensor) -> int:
     return count
 
 
+def per_graph_layer_plan(layer: nn.Module, node_states: torch.Tensor, node_to_graph_idx: torch.Tensor, gather_states: Optional[torch.Tensor],
+                         state_dim: int, grad_fp32_only: bool = False) -> Tuple[EdgePlan, bool, bool]:
+    """The opening of a per-graph layer's forward: (the graph plan, whether gradients are needed, whether the states are bf16).
+    Refuses node-range shards (a graph can straddle ranks) and gradients with bf16 states, or with any states but fp32 when
+    ``grad_fp32_only`` (a layer whose backward kernels read the states as they are, not an fp32 copy).  The plan is built last, so a
+    refused call does no device work."""
+    from . import autograd as _ag
+
+    name = type(layer).__name__
+    if gather_states is not None:
+        raise NotImplementedError(f"{name} on node-range shards: a graph can straddle ranks (shard by graph instead)")
+    _check_states(node_states, state_dim, name)
+    grad = _ag.needs_grad(layer, node_states)
+    bf16 = node_states.dtype == torch.bfloat16
+    if grad and (bf16 or (grad_fp32_only and node_states.dtype != torch.float32)):
+        raise NotImplementedError(f"{name} with gradients: fp32 states only, got {node_states.dtype} (call it under torch.no_grad())")
+    return graph_plan(node_to_graph_idx, num_graphs_of(node_to_graph_idx)), grad, bf16
+
+
 class AbstractGlobalGraphExchange(AbstractMessagePassingLayer):
     def __init__(self, global_graph_representation_module: AbstractVarSizedElementReduce, dropout_rate: float = 0.0):
         super().__init__()
@@ -77,15 +96,10 @@ class AbstractGlobalGraphExchange(AbstractMessagePassingLayer):
         edge_features: List[torch.Tensor] = None,
         gather_states: Optional[torch.Tensor] = None,
     ) -> torch.Tensor:
-        if gather_states is not None:
-            raise NotImplementedError("global graph exchange on node-range shards: a graph can straddle ranks (shard by graph instead)")
         from . import autograd as _ag
 
-        _check_states(node_states, self.input_state_dimension, type(self).__name__)
-        grad = _ag.needs_grad(self, node_states)
-        if grad and node_states.dtype != torch.float32:
-            raise NotImplementedError("global graph exchange with gradients: fp32 states only")
-        plan = graph_plan(node_to_graph_idx, num_graphs_of(node_to_graph_idx))
+        plan, grad, _ = per_graph_layer_plan(self, node_states, node_to_graph_idx, gather_states, self.input_state_dimension,
+                                             grad_fp32_only=True)
         reducer = self.__global_graph_representation_module
         native = readout_of(reducer)
         if native is None:

@@ -21,7 +21,8 @@ from torch import nn
 
 from . import _native as N
 from .edgeplan import EdgePlan
-from .messagepassing import AbstractMessagePassingLayer, _check_states
+from .messagepassing import AbstractMessagePassingLayer, _check_shape
+from .reduceops import graph_states
 
 _DIMS = "a state dimension that is a multiple of 32 in [32, 256]"
 
@@ -41,24 +42,18 @@ def _params(gamma: torch.Tensor, alpha: torch.Tensor, bias: torch.Tensor, D: int
     return out
 
 
-def _check(x: torch.Tensor, plan: EdgePlan) -> Tuple[int, int]:
-    if x.dim() != 2:
-        raise ValueError(f"node_states must be [num_nodes, D], got {tuple(x.shape)}")
-    num_nodes, D = x.shape
-    if plan.num_edges != num_nodes:
-        raise ValueError("node_to_graph_idx and node_states disagree on the number of nodes")
+def _states(x: torch.Tensor, plan: EdgePlan) -> Tuple[torch.Tensor, bool, int, int]:
+    x, bf16, num_nodes, D = graph_states(x, plan)
     if not N.lib().ptgnn_b200_graph_norm_supported(D):
         raise NotImplementedError(f"the GraphNorm kernels take {_DIMS}, got D={D}")
-    return num_nodes, D
+    return _aligned(x, "node_states", x.dtype), bf16, num_nodes, D
 
 
 def native_graph_norm(x: torch.Tensor, plan: EdgePlan, gamma: torch.Tensor, alpha: torch.Tensor, bias: torch.Tensor, eps: float,
                       out: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
     """``ptgnn_b200_graph_norm_forward``: (y [N, D] in x's dtype, mean [G, D] fp32, rstd [G, D] fp32) for x [N, D] fp32 or bf16 and the
     plan of the node -> graph map (``reduceops.graph_plan``).  ``out``: an aligned contiguous [N, D] tensor of x's dtype for y."""
-    dtype = torch.bfloat16 if x.dtype == torch.bfloat16 else torch.float32
-    x = _aligned(x, "node_states", dtype)
-    num_nodes, D = _check(x, plan)
+    x, bf16, num_nodes, D = _states(x, plan)
     g, a, b = _params(gamma, alpha, bias, D, x.device)
     G = plan.num_nodes
     lib = N.lib()
@@ -70,7 +65,7 @@ def native_graph_norm(x: torch.Tensor, plan: EdgePlan, gamma: torch.Tensor, alph
     rstd = torch.empty(G, D, dtype=torch.float32, device=x.device)
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=x.device)
     with torch.cuda.device(x.device):
-        rc = lib.ptgnn_b200_graph_norm_forward(int(dtype == torch.bfloat16), N.ptr(x), num_nodes, D, N.ptr(plan.row_ptr), N.ptr(plan.perm),
+        rc = lib.ptgnn_b200_graph_norm_forward(int(bf16), N.ptr(x), num_nodes, D, N.ptr(plan.row_ptr), N.ptr(plan.perm),
                                                N.ptr(plan.tgt32), G, N.ptr(g), N.ptr(a), N.ptr(b), float(eps), N.ptr(y), N.ptr(mean),
                                                N.ptr(rstd), N.ptr(ws), ws_bytes, N.current_stream(x.device))
     N.check(rc, "ptgnn_b200_graph_norm_forward")
@@ -80,14 +75,12 @@ def native_graph_norm(x: torch.Tensor, plan: EdgePlan, gamma: torch.Tensor, alph
 def native_graph_norm_backward(x: torch.Tensor, plan: EdgePlan, gamma: torch.Tensor, alpha: torch.Tensor, eps: float, mean: torch.Tensor,
                                rstd: torch.Tensor, d_y: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
     """``ptgnn_b200_graph_norm_backward_f32``: (d x [N, D], d gamma [D], d alpha [D], d bias [D]) from d y [N, D].  fp32."""
-    x = _aligned(x, "node_states", torch.float32)
-    num_nodes, D = _check(x, plan)
+    x, _, num_nodes, D = _states(N.require_cuda(x, "node_states", torch.float32), plan)
     d_y = _aligned(d_y, "d_out", torch.float32)
     G = plan.num_nodes
     mean, rstd = _aligned(mean, "mean", torch.float32), _aligned(rstd, "rstd", torch.float32)
     for t, n, shape in ((d_y, "d_out", (num_nodes, D)), (mean, "mean", (G, D)), (rstd, "rstd", (G, D))):
-        if tuple(t.shape) != shape:
-            raise ValueError(f"{n} must have shape {shape}, got {tuple(t.shape)}")
+        _check_shape(t, shape, n)
     g, a, _ = _params(gamma, alpha, alpha, D, x.device)
     lib = N.lib()
     ws_bytes = lib.ptgnn_b200_graph_norm_workspace_bytes(num_nodes, G, D)
@@ -131,20 +124,11 @@ class GraphNorm(AbstractMessagePassingLayer):
         gather_states: Optional[torch.Tensor] = None,
     ) -> torch.Tensor:
         from . import autograd as _ag
-        from .globalexchange import num_graphs_of
-        from .reduceops import graph_plan
+        from .globalexchange import per_graph_layer_plan
 
-        name = type(self).__name__
-        if gather_states is not None:
-            raise NotImplementedError(f"{name} on node-range shards: a graph can straddle ranks (shard by graph instead)")
-        _check_states(node_states, self.__input_state_dim, name)
         if not N.lib().ptgnn_b200_graph_norm_supported(self.__input_state_dim):
-            raise NotImplementedError(f"{name}: the GraphNorm kernels take {_DIMS}, got D={self.__input_state_dim}")
-        bf16 = node_states.dtype == torch.bfloat16
-        grad = _ag.needs_grad(self, node_states)
-        if grad and bf16:
-            raise NotImplementedError(f"{name} with gradients: fp32 states only (call it under torch.no_grad() for bf16)")
-        plan = graph_plan(node_to_graph_idx, num_graphs_of(node_to_graph_idx))
+            raise NotImplementedError(f"{type(self).__name__}: the GraphNorm kernels take {_DIMS}, got D={self.__input_state_dim}")
+        plan, grad, bf16 = per_graph_layer_plan(self, node_states, node_to_graph_idx, gather_states, self.__input_state_dim)
         if grad:
             out = _ag.graph_norm_with_grad(plan, self.__eps, node_states.to(torch.float32), self.gamma, self.alpha, self.bias)
         else:

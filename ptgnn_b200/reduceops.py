@@ -14,13 +14,14 @@ and the reference's own instances of the same two classes directly (``readout_of
 """
 import math
 from abc import abstractmethod
-from typing import NamedTuple, Optional, Union
+from typing import NamedTuple, Optional, Tuple, Union
 
 import torch
 from torch import nn
 
 from . import _native as N
 from .edgeplan import EdgePlan, plan_for
+from .messagepassing import _check_shape
 
 
 class ElementsToSummaryRepresentationInput(NamedTuple):
@@ -49,16 +50,23 @@ def graph_plan(node_to_graph_idx: torch.Tensor, num_graphs: int) -> EdgePlan:
     return plan_for([(n2g, n2g)], int(num_graphs))
 
 
+def graph_states(node_states: torch.Tensor, plan: EdgePlan, name: str = "node_states") -> Tuple[torch.Tensor, bool, int, int]:
+    """The rows of a per-graph kernel's input, one per node of ``plan`` (``graph_plan``): (the contiguous CUDA tensor, bf16, N, D).
+    bf16 stays bf16, anything else must be fp32."""
+    bf16 = node_states.dtype == torch.bfloat16
+    x = N.require_cuda(node_states, name, torch.bfloat16 if bf16 else torch.float32)
+    if x.dim() != 2:
+        raise ValueError(f"{name} must be [num_nodes, D], got {tuple(x.shape)}")
+    num_nodes, D = x.shape
+    if plan.num_edges != num_nodes:
+        raise ValueError(f"node_to_graph_idx and {name} disagree on the number of nodes")
+    return x, bf16, num_nodes, D
+
+
 def native_readout(node_states: torch.Tensor, plan: EdgePlan, mode: int, gate_weight: Optional[torch.Tensor] = None,
                    want_gates: bool = False):
     """``ptgnn_b200_graph_readout``: (g [G, H] fp32, s [N] fp32 or None).  fp32 or bf16 states; H a multiple of 32 in [32, 256]."""
-    dtype = torch.bfloat16 if node_states.dtype == torch.bfloat16 else torch.float32
-    x = N.require_cuda(node_states, "node_states", dtype)
-    if x.dim() != 2:
-        raise ValueError(f"node_states must be [num_nodes, H], got {tuple(x.shape)}")
-    num_nodes, H = x.shape
-    if plan.num_edges != num_nodes:
-        raise ValueError("node_to_graph_idx and node_states disagree on the number of nodes")
+    x, bf16, num_nodes, H = graph_states(node_states, plan)
     G = plan.num_nodes
     lib = N.lib()
     ws_bytes = lib.ptgnn_b200_graph_readout_workspace_bytes(num_nodes, G, H)
@@ -67,13 +75,12 @@ def native_readout(node_states: torch.Tensor, plan: EdgePlan, mode: int, gate_we
     w = None
     if mode == N.READOUT_WEIGHTED_SUM:
         w = N.require_cuda(gate_weight, "weights_layer.weight", torch.float32)
-        if tuple(w.shape) != (1, H):        # raw pointers cross the C ABI next
-            raise ValueError(f"weights_layer.weight must have shape (1, {H}), got {tuple(w.shape)}")
+        _check_shape(w, (1, H), "weights_layer.weight")      # raw pointers cross the C ABI next
     g = torch.empty(G, H, dtype=torch.float32, device=x.device)
     s = torch.empty(num_nodes, dtype=torch.float32, device=x.device) if want_gates and w is not None else None
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=x.device)
     with torch.cuda.device(x.device):
-        rc = lib.ptgnn_b200_graph_readout(int(dtype == torch.bfloat16), N.ptr(x), num_nodes, H, N.ptr(plan.row_ptr),
+        rc = lib.ptgnn_b200_graph_readout(int(bf16), N.ptr(x), num_nodes, H, N.ptr(plan.row_ptr),
                                           N.ptr(plan.perm) if num_nodes else None, G, N.ptr(w), mode, N.ptr(g), N.ptr(s), N.ptr(ws),
                                           ws_bytes, N.current_stream(x.device))
     N.check(rc, "ptgnn_b200_graph_readout")
@@ -146,26 +153,19 @@ class WeightedSumVarSizedElementReduce(AbstractVarSizedElementReduce):
 def native_attention_readout(node_states: torch.Tensor, plan: EdgePlan, qt: torch.Tensor, heads: int):
     """``ptgnn_b200_attention_readout``: (o [G, heads, D] fp32, lse [G, heads] fp32) with o[b, h] = sum_n softmax_n(x_n . qt[b, h]) x_n
     over the nodes of graph b.  fp32 or bf16 states; D in {32, 64, 128, 256}, heads in {1, 2, 4, 8}."""
-    dtype = torch.bfloat16 if node_states.dtype == torch.bfloat16 else torch.float32
-    x = N.require_cuda(node_states, "node_states", dtype)
-    if x.dim() != 2:
-        raise ValueError(f"node_states must be [num_nodes, D], got {tuple(x.shape)}")
-    num_nodes, D = x.shape
-    if plan.num_edges != num_nodes:
-        raise ValueError("node_to_graph_idx and node_states disagree on the number of nodes")
+    x, bf16, num_nodes, D = graph_states(node_states, plan)
     G = plan.num_nodes
     lib = N.lib()
-    if not lib.ptgnn_b200_attention_readout_supported(int(dtype == torch.bfloat16), D, heads):
+    if not lib.ptgnn_b200_attention_readout_supported(int(bf16), D, heads):
         raise NotImplementedError(f"the attention readout kernel takes D in {{32, 64, 128, 256}} and heads in {{1, 2, 4, 8}}, got D={D}, heads={heads}")
     q = N.require_cuda(qt, "qt", torch.float32)
-    if tuple(q.shape) != (G, heads, D):        # raw pointers cross the C ABI next
-        raise ValueError(f"qt must have shape ({G}, {heads}, {D}), got {tuple(q.shape)}")
+    _check_shape(q, (G, heads, D), "qt")        # raw pointers cross the C ABI next
     ws_bytes = lib.ptgnn_b200_attention_readout_workspace_bytes(num_nodes, G, D, heads)
     o = torch.empty(G, heads, D, dtype=torch.float32, device=x.device)
     lse = torch.empty(G, heads, dtype=torch.float32, device=x.device)
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=x.device)
     with torch.cuda.device(x.device):
-        rc = lib.ptgnn_b200_attention_readout(int(dtype == torch.bfloat16), N.ptr(x), num_nodes, D, heads, N.ptr(plan.row_ptr),
+        rc = lib.ptgnn_b200_attention_readout(int(bf16), N.ptr(x), num_nodes, D, heads, N.ptr(plan.row_ptr),
                                               N.ptr(plan.perm) if num_nodes else None, G, N.ptr(q), N.ptr(o), N.ptr(lse), N.ptr(ws), ws_bytes,
                                               N.current_stream(x.device))
     N.check(rc, "ptgnn_b200_attention_readout")
@@ -175,16 +175,13 @@ def native_attention_readout(node_states: torch.Tensor, plan: EdgePlan, qt: torc
 def native_attention_readout_backward(node_states: torch.Tensor, plan: EdgePlan, qt: torch.Tensor, o: torch.Tensor, lse: torch.Tensor,
                                       d_o: torch.Tensor):
     """``ptgnn_b200_attention_readout_backward_f32``: (d_x [N, D], d_qt [G, heads, D]) from d_o [G, heads, D].  fp32 states."""
-    x = N.require_cuda(node_states, "node_states", torch.float32)
-    num_nodes, D = x.shape
+    x, _, num_nodes, D = graph_states(N.require_cuda(node_states, "node_states", torch.float32), plan)
     G, heads = plan.num_nodes, qt.shape[1]
     tabs = [N.require_cuda(t, n, torch.float32) for t, n in ((qt, "qt"), (o, "o"), (d_o, "d_o"))]
     for t, n in zip(tabs, ("qt", "o", "d_o")):
-        if tuple(t.shape) != (G, heads, D):
-            raise ValueError(f"{n} must have shape ({G}, {heads}, {D}), got {tuple(t.shape)}")
+        _check_shape(t, (G, heads, D), n)
     lse = N.require_cuda(lse, "lse", torch.float32)
-    if tuple(lse.shape) != (G, heads):
-        raise ValueError(f"lse must have shape ({G}, {heads}), got {tuple(lse.shape)}")
+    _check_shape(lse, (G, heads), "lse")
     lib = N.lib()
     ws_bytes = lib.ptgnn_b200_attention_readout_workspace_bytes(num_nodes, G, D, heads)
     if ws_bytes == 0:

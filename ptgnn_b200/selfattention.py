@@ -26,37 +26,33 @@ from torch import nn
 
 from . import _native as N
 from .edgeplan import EdgePlan
-from .messagepassing import AbstractMessagePassingLayer, _check_states
+from .messagepassing import AbstractMessagePassingLayer, _check_shape
+from .reduceops import graph_states
 
 _RELU = nn.ReLU()
 _DIMS = "dk and dv in {16, 32, 64, 128}"
 
 
-def _check_qkv(t: torch.Tensor, plan: EdgePlan, heads: int, dk: int, dv: int) -> int:
-    rows = t.shape[0]
-    if t.dim() != 2 or t.shape[1] != heads * (2 * dk + dv):
-        raise ValueError(f"qkv must be [rows, {heads * (2 * dk + dv)}], got {tuple(t.shape)}")
-    if plan.num_edges != rows:
-        raise ValueError("node_to_graph_idx and node_states disagree on the number of nodes")
-    return rows
+def _qkv(t: torch.Tensor, plan: EdgePlan, heads: int, dk: int, dv: int) -> Tuple[torch.Tensor, bool, int]:
+    t, bf16, rows, _ = graph_states(t, plan, "qkv")
+    _check_shape(t, (rows, heads * (2 * dk + dv)), "qkv")
+    return t, bf16, rows
 
 
 def native_selfatt(t: torch.Tensor, plan: EdgePlan, heads: int, dk: int, dv: int, max_chunk: int) -> Tuple[torch.Tensor, torch.Tensor]:
     """``ptgnn_b200_selfatt_forward``: (o [R, heads * dv] in t's dtype, lse [R, heads] fp32) for t [R, heads * (2 dk + dv)] fp32 or bf16
     and the plan of the node -> graph map."""
-    dtype = torch.bfloat16 if t.dtype == torch.bfloat16 else torch.float32
-    t = N.require_cuda(t, "qkv", dtype)
-    rows = _check_qkv(t, plan, heads, dk, dv)
+    t, bf16, rows = _qkv(t, plan, heads, dk, dv)
     lib = N.lib()
-    if not lib.ptgnn_b200_selfatt_supported(int(dtype == torch.bfloat16), dk, dv):
+    if not lib.ptgnn_b200_selfatt_supported(int(bf16), dk, dv):
         raise NotImplementedError(f"the self-attention kernel takes {_DIMS}, got dk={dk}, dv={dv}")
     G = plan.num_nodes
     ws_bytes = lib.ptgnn_b200_selfatt_workspace_bytes(rows, G, heads)
-    o = torch.empty(rows, heads * dv, dtype=dtype, device=t.device)
+    o = torch.empty(rows, heads * dv, dtype=t.dtype, device=t.device)
     lse = torch.empty(rows, heads, dtype=torch.float32, device=t.device)
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=t.device)
     with torch.cuda.device(t.device):
-        rc = lib.ptgnn_b200_selfatt_forward(int(dtype == torch.bfloat16), N.ptr(t), rows, heads, dk, dv, N.ptr(plan.row_ptr), G, int(max_chunk),
+        rc = lib.ptgnn_b200_selfatt_forward(int(bf16), N.ptr(t), rows, heads, dk, dv, N.ptr(plan.row_ptr), G, int(max_chunk),
                                             N.ptr(o), N.ptr(lse), plan.status.data_ptr() + 4, N.ptr(ws), ws_bytes, N.current_stream(t.device))
     N.check(rc, "ptgnn_b200_selfatt_forward")
     return o, lse
@@ -65,13 +61,11 @@ def native_selfatt(t: torch.Tensor, plan: EdgePlan, heads: int, dk: int, dv: int
 def native_selfatt_backward(t: torch.Tensor, plan: EdgePlan, heads: int, dk: int, dv: int, max_chunk: int, o: torch.Tensor,
                             lse: torch.Tensor, d_o: torch.Tensor) -> torch.Tensor:
     """``ptgnn_b200_selfatt_backward_f32``: d t [R, heads * (2 dk + dv)] from d o [R, heads * dv].  fp32."""
-    t = N.require_cuda(t, "qkv", torch.float32)
-    rows = _check_qkv(t, plan, heads, dk, dv)
+    t, _, rows = _qkv(N.require_cuda(t, "qkv", torch.float32), plan, heads, dk, dv)
     o, d_o = N.require_cuda(o, "o", torch.float32), N.require_cuda(d_o, "d_o", torch.float32)
     lse = N.require_cuda(lse, "lse", torch.float32)
     for x, n, shape in ((o, "o", (rows, heads * dv)), (d_o, "d_o", (rows, heads * dv)), (lse, "lse", (rows, heads))):
-        if tuple(x.shape) != shape:
-            raise ValueError(f"{n} must have shape {shape}, got {tuple(x.shape)}")
+        _check_shape(x, shape, n)
     lib = N.lib()
     if not lib.ptgnn_b200_selfatt_supported(0, dk, dv):
         raise NotImplementedError(f"the self-attention kernel takes {_DIMS}, got dk={dk}, dv={dv}")
@@ -131,28 +125,20 @@ class MultiHeadSelfAttentionMessagePassing(AbstractMessagePassingLayer):
     ) -> torch.Tensor:
         from . import autograd as _ag
         from . import composed as C
-        from .globalexchange import num_graphs_of
-        from .reduceops import graph_plan
+        from .globalexchange import per_graph_layer_plan
 
         name = type(self).__name__
-        if gather_states is not None:
-            raise NotImplementedError(f"{name} on node-range shards: a graph can straddle ranks (shard by graph instead)")
         if self.__target_reference != "all":
             raise NotImplementedError(f"{name}: target_reference other than 'all' (the reference's branch adds all node states to the "
                                       "referenced rows and only works when every node is referenced)")
-        _check_states(node_states, self.input_state_dimension, name)
         if self.training and self.__dropout_layer.p > 0:
             raise NotImplementedError(f"{name}: training-mode dropout with p > 0 (the mask on the attention probabilities)")
         heads, dk, dv = self.__num_heads, self.__key_query_dim, self.__value_dim
-        bf16 = node_states.dtype == torch.bfloat16
-        grad = _ag.needs_grad(self, node_states)
-        if grad and bf16:
-            raise NotImplementedError(f"{name} with gradients: fp32 states only (call it under torch.no_grad() for bf16)")
-        if not N.lib().ptgnn_b200_selfatt_supported(int(bf16), dk, dv):
+        if not N.lib().ptgnn_b200_selfatt_supported(int(node_states.dtype == torch.bfloat16), dk, dv):
             raise NotImplementedError(f"{name}: the self-attention kernel takes {_DIMS}, got dk={dk}, dv={dv}")
         if self.__max_num_nodes < 1:
             raise ValueError(f"{name}: max_num_nodes must be >= 1, got {self.__max_num_nodes}")
-        plan = graph_plan(node_to_graph_idx, num_graphs_of(node_to_graph_idx))
+        plan, grad, bf16 = per_graph_layer_plan(self, node_states, node_to_graph_idx, gather_states, self.input_state_dimension)
         x = node_states.to(torch.float32)
         linear = _ag._LinearFn.apply if grad else C.linear
         t = linear(x, self.__selfatt_head_transforms.weight, None)

@@ -8,7 +8,7 @@ round-to-nearest intrinsic, and torch's float32 CPU ops round the same way), so 
 """
 import torch
 
-CHUNK = 32              # readout::CHUNK: rows per warp-chunk
+CHUNK = 32              # pergraph::CHUNK: rows per warp-chunk
 U = 2.0 ** -24          # unit roundoff of fp32
 
 

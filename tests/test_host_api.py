@@ -192,6 +192,24 @@ def test_unsupported_configurations_fail_loudly():
             P.MlpMessagePassingLayer(32, 32, 32, 1, "sum").eval()(torch.zeros(4, 32, 1), adj)
 
 
+def test_per_graph_layers_refuse_before_building_the_plan():
+    # On CPU tensors a call that gets as far as the graph plan raises NativeLibraryError; a refused call raises before it.
+    n2g = torch.zeros(4, dtype=torch.int64)
+    exchange = P.GruGlobalStateUpdate(P.SimpleVarSizedElementReduce("max"), 32, 32)      # GRUCell parameters: gradients are on
+    for dtype in (torch.float16, torch.float64, torch.bfloat16):          # its readout and GRU kernels read fp32 states as they are
+        with pytest.raises(NotImplementedError):
+            exchange(torch.zeros(4, 32, dtype=dtype), [], n2g)
+    with pytest.raises(N.NativeLibraryError):
+        exchange(torch.zeros(4, 32), [], n2g)
+    norm = P.GraphNorm(32)
+    with pytest.raises(NotImplementedError):
+        norm(torch.zeros(4, 32, dtype=torch.bfloat16), [], n2g)
+    with pytest.raises(N.NativeLibraryError):                             # GraphNorm trains on an fp32 copy of fp64 states
+        norm(torch.zeros(4, 32, dtype=torch.float64), [], n2g)
+    with pytest.raises(NotImplementedError):                              # the layer's own checks come before the shape check
+        P.MultiHeadSelfAttentionMessagePassing(32, 16, 16, 32, 64, 2, target_reference="tok")(torch.zeros(4, 48), [], n2g)
+
+
 def test_container_metrics_protocol():
     layer = P.GatedMessagePassingLayer(32, 32, 3, "sum")
     gnn = P.GraphNeuralNetwork([layer, layer], torch.nn.Identity(), True, True)
