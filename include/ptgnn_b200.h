@@ -409,6 +409,29 @@ int ptgnn_b200_graph_norm_backward_f32(const float *node_states, const float *d_
                                        float *d_gamma, float *d_alpha, float *d_bias, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * PnaMessageAggregation (reference gnn/messagepassing/pna_aggregation.py:27-56), per target v with in-degree k and
+ * den = k + 1e-5 (fp32):
+ *   S = [sum | mean = sum / den | max | min | std = sqrt(sum_e (relu(m_e^2 - mean^2) + 1e-10))],   out [N, 15 D] fp32 =
+ *   [S | S p1 | S m1] with p1 = log(k + 1) / delta, m1 = 1 / (p1 + 1e-3).  max / min: strict compare (first occurrence wins ties,
+ *   NaN never wins), 0 for an empty target.
+ *   messages [E, D] in edge order: fp32, or bf16 when bf16_messages != 0 (fp32 arithmetic; S rounded to bf16 before the scalers,
+ *   the output stays fp32).  row_ptr / perm: the plan of the message targets (edges summed in plan order = edge order).
+ *   arg_max, arg_min [N, D] int32 (optional, both or neither): the winning edge ids, E for an empty target; the backward needs them.
+ *   No workspace, no host synchronisation, no float atomics: deterministic (DESIGN.md §3.10).
+ *   Supported: D a multiple of 4 in [4, 512] (ptgnn_b200_pna_supported).  out and the arg ids 16-byte aligned, fp32 messages
+ *   16-byte aligned, bf16 messages 8-byte aligned.
+ * pna_backward_f32: from the forward's fp32 messages, out and arg ids and d_out = dL/dout [N, 15 D], writes every row of
+ *   d_messages [E, D] once (16-byte aligned).  fp32 messages only.
+ * ---------------------------------------------------------------------------------------------- */
+int32_t ptgnn_b200_pna_supported(int32_t message_dim);
+int ptgnn_b200_pna_forward(int32_t bf16_messages, const void *messages, int64_t num_edges, int32_t message_dim, const int32_t *row_ptr,
+                           const int32_t *perm, int64_t num_targets, float delta, float *out, int32_t *arg_max, int32_t *arg_min,
+                           void *stream);
+int ptgnn_b200_pna_backward_f32(const float *messages, int64_t num_edges, int32_t message_dim, const int32_t *row_ptr, const int32_t *perm,
+                                int64_t num_targets, float delta, const float *out, const int32_t *arg_max, const int32_t *arg_min,
+                                const float *d_out, float *d_messages, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Host-buffer convenience entry point (used for the end-to-end measurement): all pointers are HOST
  * memory; copies inputs to the device, builds the plan, runs `num_layers` GatedMessagePassingLayers
  * (layer l uses weight set l; pass the same pointers to share weights), copies the final states back

@@ -95,6 +95,11 @@ SIGNATURES = {
     "ptgnn_b200_graph_norm_backward_f32": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_void_p, c_i64, c_void_p,
                                                           c_void_p, c_f32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                                           c_void_p, c_size_t, c_void_p]),
+    "ptgnn_b200_pna_supported": (c_i32, [c_i32]),
+    "ptgnn_b200_pna_forward": (ctypes.c_int, [c_i32, c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_i64, c_f32, c_void_p, c_void_p, c_void_p,
+                                              c_void_p]),
+    "ptgnn_b200_pna_backward_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_i64, c_f32, c_void_p, c_void_p, c_void_p,
+                                                   c_void_p, c_void_p, c_void_p]),
     "ptgnn_b200_gated_gnn_forward_host_f32":(ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_i32,
                                                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i32, c_void_p]),
 }

@@ -248,7 +248,7 @@ class _MlpLayerFunction(torch.autograd.Function):
         adj: List[Tuple[torch.Tensor, torch.Tensor]] = ctx.adjacency_lists
         reduce_name, use_target = ctx.reduce_name, ctx.use_target
         message_activation, ln, dense, dense_activation = ctx.modules
-        reduce = N.REDUCE[reduce_name]
+        pna = None if isinstance(reduce_name, str) else reduce_name          # the native PnaMessageAggregation module
         g = grad_out.contiguous().float()
         h = h.detach().contiguous()
         num_nodes, H = h.shape
@@ -256,14 +256,19 @@ class _MlpLayerFunction(torch.autograd.Function):
         plan = plan_for(adj, num_nodes)
         E = plan.num_edges
 
-        # ---- 1. re-compute the aggregate on the native kernels
+        # ---- 1. re-compute the aggregate on the native kernels (PNA: with its arg ids; the messages are kept for its backward)
         msg = C.edge_messages(plan, h, h if use_target else None, W, use_target)
         arg = None
-        if reduce_name in ("max", "min"):
-            agg, arg = C.segment_reduce(msg, plan, reduce, return_arg=True)
+        if pna is not None:
+            from .aggregation import native_pna
+
+            agg, arg_max, arg_min = native_pna(msg, plan, pna.delta, want_arg=True)
+        elif reduce_name in ("max", "min"):
+            agg, arg = C.segment_reduce(msg, plan, N.REDUCE[reduce_name], return_arg=True)
         else:
-            agg = C.segment_reduce(msg, plan, reduce)
-        del msg
+            agg = C.segment_reduce(msg, plan, N.REDUCE[reduce_name])
+        if pna is None:
+            del msg
 
         # ---- 2. node-sized tail (activation, LayerNorm, dense): local autograd over library ops
         agg_leaf = agg.detach().requires_grad_(True)
@@ -280,7 +285,7 @@ class _MlpLayerFunction(torch.autograd.Function):
         d_W = []
         Ws = [w[:, :H].contiguous() for w in W]                              # columns multiplying h_src
         Wg = [w[:, H:].contiguous() for w in W] if use_target else None      # columns multiplying h_tgt
-        if reduce_name in ("sum", "mean"):
+        if pna is None and reduce_name in ("sum", "mean"):
             if reduce_name == "mean":
                 cnt = (plan.row_ptr[1:] - plan.row_ptr[:-1]).clamp(min=1).to(torch.float32)
                 d_agg = (d_agg / cnt[:, None]).contiguous()
@@ -302,11 +307,17 @@ class _MlpLayerFunction(torch.autograd.Function):
                     tplan = plan_for([(tgt, tgt) for _src, tgt in adj], num_nodes)
                     d_h = d_h + C.aggregate(tplan, d_agg, [w.t().contiguous() for w in Wg], N.REDUCE["sum"])
         else:
-            D = d_agg.shape[1]
-            d_msg = torch.zeros(E + 1, D, dtype=torch.float32, device=h.device)
-            d_msg.scatter_(0, arg, d_agg)
+            # per-edge message gradients: routed to the winning edges (max / min), or the PNA backward
+            if pna is not None:
+                from .aggregation import native_pna_backward
+
+                d_msg = native_pna_backward(msg, plan, pna.delta, agg, arg_max, arg_min, d_agg)
+                del msg
+            else:
+                d_msg = torch.zeros(E + 1, d_agg.shape[1], dtype=torch.float32, device=h.device)
+                d_msg = d_msg.scatter_(0, arg, d_agg)[:E]
             with _exact_fp16_gemms():
-                a_all, b_all = _split16(d_msg[:E]), _split16(h, False, plan.src32)
+                a_all, b_all = _split16(d_msg), _split16(h, False, plan.src32)
                 g_all = _split16(h, False, plan.tgt32) if use_target else None
             lo = 0
             for t, ((src, tgt), w) in enumerate(zip(adj, W)):
@@ -328,6 +339,7 @@ class _MlpLayerFunction(torch.autograd.Function):
 
 def mlp_forward_with_grad(layer, node_states, adjacency_lists, reduce_name, use_target, message_activation, ln, dense, dense_activation,
                           weights):
+    """``reduce_name``: "sum", "mean", "max", "min", or the layer's native ``PnaMessageAggregation`` module."""
     tail_params: List[Optional[torch.Tensor]] = []
     if ln is not None:
         tail_params += [ln.weight, ln.bias]
@@ -603,3 +615,33 @@ class _GraphNormFn(torch.autograd.Function):
 
 def graph_norm_with_grad(plan, eps, node_states, gamma, alpha, bias):
     return _GraphNormFn.apply(plan, eps, node_states, gamma, alpha, bias)
+
+
+# =====================================================================================================================
+# PnaMessageAggregation (pna_aggregation.py:27-56): [S | S p1 | S m1] per target on the native kernel.  fp32 messages.
+# =====================================================================================================================
+class _PnaFn(torch.autograd.Function):
+    """out [N, 15 D] from messages [E, D]; backward: d messages on the native backward kernel, which reads the mean and std back from
+    the saved output and the max / min winners from the saved [N, D] arg ids (no [E, D] tensor is kept besides the messages)."""
+
+    @staticmethod
+    def forward(ctx, plan, delta, messages):
+        from .aggregation import native_pna
+
+        m = messages.detach()
+        out, arg_max, arg_min = native_pna(m, plan, delta, want_arg=True)
+        ctx.save_for_backward(m, out, arg_max, arg_min)
+        ctx.plan, ctx.delta = plan, delta
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, d_out):
+        from .aggregation import native_pna_backward
+
+        m, out, arg_max, arg_min = ctx.saved_tensors
+        return None, None, native_pna_backward(m, ctx.plan, ctx.delta, out, arg_max, arg_min, d_out.contiguous().float())
+
+
+def pna_with_grad(plan, delta, messages):
+    return _PnaFn.apply(plan, delta, messages)

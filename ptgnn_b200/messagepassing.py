@@ -479,15 +479,19 @@ class MlpMessagePassingLayer(AbstractMessagePassingLayer):
         mlps = self.__edge_message_transformation_layers
         assert len(adjacency_lists) == len(mlps), "The number of adjacency lists must be equal to the number of edge types."
         from . import autograd as _ag
-        default_config = (isinstance(self.__aggregation_fn, str) and self.__features_dim == 0
-                          and not any(m.num_hidden_layers != 0 or m.uses_biases for m in mlps))
+        from .aggregation import PnaMessageAggregation
+
+        plain_mlp = self.__features_dim == 0 and not any(m.num_hidden_layers != 0 or m.uses_biases for m in mlps)
+        default_config = plain_mlp and isinstance(self.__aggregation_fn, str)
+        # the native PNA aggregator after a default message MLP: messages from the native message kernel, then the PNA kernel
+        # (composed path without gradients, _MlpLayerFunction's PNA mode with them)
+        pna_config = plain_mlp and isinstance(self.__aggregation_fn, PnaMessageAggregation)
         grad = _ag.needs_grad(self, node_states)
-        if grad and (not default_config or gather_states is not None or node_states.dtype != torch.float32):
+        if grad and (not (default_config or pna_config) or gather_states is not None or node_states.dtype != torch.float32):
             _refuse_autograd(self, node_states)
-        if not default_config:
+        if not (default_config or pna_config):
             return self._forward_composed(node_states, adjacency_lists, edge_features, gather_states)
         _check_no_edge_features(edge_features)
-        reduce = _reduce_code(self.__aggregation_fn)
 
         ln: Optional[nn.LayerNorm] = None
         dense: Optional[nn.Linear] = None
@@ -513,6 +517,9 @@ class MlpMessagePassingLayer(AbstractMessagePassingLayer):
             return apply_dropout(_ag.mlp_forward_with_grad(
                 self, node_states, adjacency_lists, self.__aggregation_fn, self.__use_target_state_as_message_input,
                 self.__message_activation, ln, dense, dense_act_module, [m.single_linear.weight for m in mlps]))
+        if pna_config:
+            return apply_dropout(self._forward_composed(node_states, adjacency_lists, edge_features, gather_states, dropout_by_caller=True))
+        reduce = _reduce_code(self.__aggregation_fn)
         msg_act = _activation_code(self.__message_activation, "message_activation")
         dense_act = N.ACT_NONE if dense_act_module is None else _activation_code(dense_act_module, "dense_activation")
 
@@ -574,16 +581,21 @@ class MlpMessagePassingLayer(AbstractMessagePassingLayer):
         N.check(rc, "ptgnn_b200_mlp_forward")
         return apply_dropout(out)
 
-    def _forward_composed(self, node_states, adjacency_lists, edge_features, gather_states) -> torch.Tensor:
+    def _forward_composed(self, node_states, adjacency_lists, edge_features, gather_states, dropout_by_caller: bool = False) -> torch.Tensor:
         """Module aggregators (PNA ...), message MLPs with hidden layers / biases, edge features (mlpmessagepassing.py:82-117 in
-        full generality): stand-alone native pieces + the module's own tail -- see ptgnn_b200/composed.py.  fp32 states only."""
+        full generality): stand-alone native pieces + the module's own tail -- see ptgnn_b200/composed.py.  fp32 states only.
+        The native PnaMessageAggregation runs on the layer's own plan.  ``dropout_by_caller``: the caller applies the tail's output
+        Dropout to the result (a torch op, as in the default configuration), so it is left out here; otherwise training-mode dropout
+        with p > 0 is refused."""
         from . import composed as C
+        from .aggregation import PnaMessageAggregation, pna
 
+        native_pna = isinstance(self.__aggregation_fn, PnaMessageAggregation)
         if node_states.dtype != torch.float32:
             raise NotImplementedError("this MlpMessagePassingLayer configuration has no bf16 kernel")
         _check_states(node_states, self.__input_state_dim, "MlpMessagePassingLayer")
         for m in self.__state_update:
-            if isinstance(m, nn.Dropout) and self.training and m.p > 0:
+            if isinstance(m, nn.Dropout) and self.training and m.p > 0 and not dropout_by_caller:
                 raise NotImplementedError("training-mode dropout has no native kernel (forward-only)")
         h = N.require_cuda(node_states, "node_states", torch.float32)
         gsrc = h if gather_states is None else N.require_cuda(gather_states, "gather_states", torch.float32)
@@ -608,11 +620,13 @@ class MlpMessagePassingLayer(AbstractMessagePassingLayer):
             msg = nxt
         if isinstance(self.__aggregation_fn, str):
             agg = C.segment_reduce(msg, plan, _reduce_code(self.__aggregation_fn))
+        elif native_pna:    # the messages are in edge order: the layer's plan groups them by target
+            agg = pna(msg, plan, self.__aggregation_fn.delta)
         else:   # e.g. the reference's PnaMessageAggregation: messages + concatenated targets, as mlpmessagepassing.py:100-112 passes them
             agg = self.__aggregation_fn(msg, plan.tgt32.to(torch.int64), h.shape[0])
         if self.__message_activation is not None:
             agg = self.__message_activation(agg)
-        return self.__state_update(agg)
+        return self.__state_update[:-1](agg) if dropout_by_caller else self.__state_update(agg)
 
     @property
     def input_state_dimension(self) -> int:

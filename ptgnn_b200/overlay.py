@@ -6,7 +6,7 @@ factories import the layer classes by module path (`implementations/typilus/trai
 
 1. registers ``ptgnn_b200.torch_scatter_shim`` as ``torch_scatter`` (if the real wheel is absent, or ``force_torch_scatter``),
 2. pre-seeds ``sys.modules`` so that ``ptgnn.neuralmodels.gnn.messagepassing.{abstract,gated,mlp}messagepassing`` and
-   ``...globalgraphexchange`` resolve to the ptgnn_b200 classes (everything else -- residual layers, PNA, GraphNorm (unless
+   ``...globalgraphexchange`` resolve to the ptgnn_b200 classes (everything else -- residual layers, PNA (unless step 8), GraphNorm (unless
    step 7), embedders, trainers, and the reducers of ``reduceops.varsizedsummary``, whose attention variants must keep working -- stays the
    reference's; the native ``GruGlobalStateUpdate`` reads the reference's WeightedSum and Simple reducers directly), and
    re-binds those names in reference modules that were imported earlier,
@@ -21,7 +21,10 @@ factories import the layer classes by module path (`implementations/typilus/trai
    ``ptgnn.neuralmodels.gnn.messagepassing.selfattmessagepassing`` (the native chunked attention kernel, DESIGN.md §3.8) like the
    layers of step 2.  The default leaves the reference's class in place,
 7. with ``native_graphnorm=True`` only: pre-seeds / re-binds ``GraphNorm`` at ``ptgnn.neuralmodels.gnn.messagepassing.graphnorm``
-   (the native per-graph normalisation kernels, DESIGN.md §3.9) in the same way.  The default leaves the reference's class in place.
+   (the native per-graph normalisation kernels, DESIGN.md §3.9) in the same way.  The default leaves the reference's class in place,
+8. with ``native_pna=True`` only: pre-seeds / re-binds ``PnaMessageAggregation`` at
+   ``ptgnn.neuralmodels.gnn.messagepassing.pna_aggregation`` (the native PNA kernel, DESIGN.md §3.10) in the same way, so that an
+   ``MlpMessagePassingLayer`` built with it runs PNA on the kernel and trains.  The default leaves the reference's class in place.
 
 After ``install()``: ``import ptgnn.implementations.ppi.train`` etc. build ptgnn_b200 layers, unchanged.  ``uninstall()``
 restores the reference's classes.  The reference must be importable as ``ptgnn`` for steps 2-4 (it is not on the GPU test box;
@@ -48,6 +51,8 @@ _SELFATT_MODULE = "ptgnn.neuralmodels.gnn.messagepassing.selfattmessagepassing"
 _SELFATT_CLASS = "MultiHeadSelfAttentionMessagePassing"
 _GRAPHNORM_MODULE = "ptgnn.neuralmodels.gnn.messagepassing.graphnorm"
 _GRAPHNORM_CLASS = "GraphNorm"
+_PNA_MODULE = "ptgnn.neuralmodels.gnn.messagepassing.pna_aggregation"
+_PNA_CLASS = "PnaMessageAggregation"
 _saved: Dict[str, object] = {}
 
 
@@ -127,10 +132,16 @@ def _install_native_graphnorm() -> None:
     _install_native_class(_GRAPHNORM_MODULE, _GRAPHNORM_CLASS, getattr(_gn, _GRAPHNORM_CLASS))
 
 
+def _install_native_pna() -> None:
+    from . import aggregation as _agg
+
+    _install_native_class(_PNA_MODULE, _PNA_CLASS, getattr(_agg, _PNA_CLASS))
+
+
 def install(force_torch_scatter: bool = False, native_reducers: bool = False, native_selfattention: bool = False,
-            native_graphnorm: bool = False) -> Dict[str, object]:
+            native_graphnorm: bool = False, native_pna: bool = False) -> Dict[str, object]:
     report: Dict[str, object] = {"torch_scatter": "real", "layers": False, "container": False, "metrics": False, "reducers": False,
-                                 "selfattention": False, "graphnorm": False}
+                                 "selfattention": False, "graphnorm": False, "pna": False}
     # 1. torch_scatter
     have_real = False
     if not force_torch_scatter:
@@ -183,6 +194,10 @@ def install(force_torch_scatter: bool = False, native_reducers: bool = False, na
     if native_graphnorm:
         _install_native_graphnorm()
         report["graphnorm"] = True
+    # 8. PnaMessageAggregation (opt-in)
+    if native_pna:
+        _install_native_pna()
+        report["pna"] = True
     return report
 
 
@@ -201,7 +216,7 @@ def uninstall() -> None:
                 setattr(sys.modules[mod_name], attr, val)
         else:
             sys.modules[key] = val
-    for mod_name in (*_LAYER_MODULES, _SELFATT_MODULE, _GRAPHNORM_MODULE):
+    for mod_name in (*_LAYER_MODULES, _SELFATT_MODULE, _GRAPHNORM_MODULE, _PNA_MODULE):
         if getattr(sys.modules.get(mod_name), "__ptgnn_b200_overlay__", False):
             del sys.modules[mod_name]
     for name in ("torch_scatter", "torch_scatter.composite"):

@@ -11,11 +11,13 @@ fallback); fp32 arithmetic (other floating dtypes are computed in fp32 and cast 
 Shapes the kernels do not take directly -- reduction along a dimension other than 0, 1-D inputs, row widths that are not a
 multiple of 4 -- are brought to ``[E, D]`` form by a transpose / zero-padding around the same kernels.
 """
+import importlib
 from typing import Optional, Tuple
 
 import torch
 
-from .. import scatter as _native
+# the submodule itself: the package attribute `ptgnn_b200.scatter` is re-bound to the function of that name by ptgnn_b200/__init__
+_native = importlib.import_module("..scatter", __package__)
 
 __version__ = "2.0.9+ptgnn_b200"
 
