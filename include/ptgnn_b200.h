@@ -432,6 +432,28 @@ int ptgnn_b200_pna_backward_f32(const float *messages, int64_t num_edges, int32_
                                 const float *d_out, float *d_messages, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Copy attention of the graph2seq decoder (reference neuralmodels/sequence/grucopydecoder.py:95-97, 122-124), for the memory rows i
+ * of graph g and the decoder steps l:
+ *   s[i, l] = c_i . o[g, l]  [rows, steps] fp32, in the caller's row order,   lse[g, l] = log sum_i exp(s[i, l])  [G, steps] fp32.
+ *   copy_reps c [rows, hidden]: fp32, or bf16 when bf16_copy != 0 (fp32 arithmetic); o [G, steps, hidden] fp32: the decoder's GRU
+ *   outputs.  row_ptr / perm: the plan of the row -> graph map, as for ptgnn_b200_graph_readout.  A graph without rows gives
+ *   lse = -inf.  No host synchronisation, no float atomics: deterministic (DESIGN.md §3.11).
+ *   Supported: hidden in {32, 64, 128, 256}, steps in [1, 8] (ptgnn_b200_copy_attention_supported).
+ * copy_attention_backward_f32: from d_s = dL/ds [rows, steps], d_lse = dL/dlse [G, steps] and the forward's lse, writes
+ *   d_copy_reps [rows, hidden] (every row of an in-range graph, once) and d_o [G, steps, hidden] (0 for a graph without rows).
+ *   fp32 only.  The workspace size covers both calls.
+ * ---------------------------------------------------------------------------------------------- */
+int32_t ptgnn_b200_copy_attention_supported(int32_t bf16_copy, int32_t hidden_dim, int32_t steps);
+size_t ptgnn_b200_copy_attention_workspace_bytes(int64_t num_rows, int64_t num_graphs, int32_t hidden_dim, int32_t steps);
+int ptgnn_b200_copy_attention(int32_t bf16_copy, const void *copy_reps, int64_t num_rows, int32_t hidden_dim, int32_t steps,
+                              const int32_t *row_ptr, const int32_t *perm, int64_t num_graphs, const float *o, float *s, float *lse,
+                              void *workspace, size_t workspace_bytes, void *stream);
+int ptgnn_b200_copy_attention_backward_f32(const float *copy_reps, int64_t num_rows, int32_t hidden_dim, int32_t steps,
+                                           const int32_t *row_ptr, const int32_t *perm, int64_t num_graphs, const float *o,
+                                           const float *lse, const float *d_s, const float *d_lse, float *d_copy_reps, float *d_o,
+                                           void *workspace, size_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Host-buffer convenience entry point (used for the end-to-end measurement): all pointers are HOST
  * memory; copies inputs to the device, builds the plan, runs `num_layers` GatedMessagePassingLayers
  * (layer l uses weight set l; pass the same pointers to share weights), copies the final states back

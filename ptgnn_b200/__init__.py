@@ -7,6 +7,7 @@ is the host-side mirror of the reference interface.  There is no CPU / PyTorch f
 """
 from .aggregation import PnaMessageAggregation
 from .batching import MinibatchAssembler
+from .decoder import GruCopyingDecoder
 from .edgeplan import EdgePlan, clear_plan_cache, plan_for
 from .egc import EGCMessagePassingLayer
 from .globalexchange import AbstractGlobalGraphExchange, GruGlobalStateUpdate
@@ -37,6 +38,6 @@ __all__ = [
     "ConcatResidualLayer", "LinearResidualLayer", "MinibatchAssembler", "scatter", "scatter_add",
     "AbstractGlobalGraphExchange", "GruGlobalStateUpdate", "AbstractVarSizedElementReduce", "ElementsToSummaryRepresentationInput",
     "SimpleVarSizedElementReduce", "WeightedSumVarSizedElementReduce", "SelfAttentionVarSizedElementReduce",
-    "MultiheadSelfAttentionVarSizedElementReduce", "MultiHeadSelfAttentionMessagePassing", "GraphNorm",
+    "MultiheadSelfAttentionVarSizedElementReduce", "MultiHeadSelfAttentionMessagePassing", "GraphNorm", "GruCopyingDecoder",
     "scatter_sum", "scatter_mean", "scatter_max", "scatter_min",
 ]

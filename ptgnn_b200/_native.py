@@ -100,6 +100,12 @@ SIGNATURES = {
                                               c_void_p]),
     "ptgnn_b200_pna_backward_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_i64, c_f32, c_void_p, c_void_p, c_void_p,
                                                    c_void_p, c_void_p, c_void_p]),
+    "ptgnn_b200_copy_attention_supported": (c_i32, [c_i32, c_i32, c_i32]),
+    "ptgnn_b200_copy_attention_workspace_bytes": (c_size_t, [c_i64, c_i64, c_i32, c_i32]),
+    "ptgnn_b200_copy_attention": (ctypes.c_int, [c_i32, c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_i64, c_void_p, c_void_p, c_void_p,
+                                                 c_void_p, c_size_t, c_void_p]),
+    "ptgnn_b200_copy_attention_backward_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_i64, c_void_p, c_void_p,
+                                                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "ptgnn_b200_gated_gnn_forward_host_f32":(ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_i32,
                                                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i32, c_void_p]),
 }

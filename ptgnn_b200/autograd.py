@@ -645,3 +645,57 @@ class _PnaFn(torch.autograd.Function):
 
 def pna_with_grad(plan, delta, messages):
     return _PnaFn.apply(plan, delta, messages)
+
+
+# =====================================================================================================================
+# GruCopyingDecoder (grucopydecoder.py:95-97, 122-124): the copy scores s[i, l] = c_i . o[graph(i), l] and their per-sample logsumexp
+# on the native kernel.  fp32 copy representations.
+# =====================================================================================================================
+class _CopyAttentionFn(torch.autograd.Function):
+    """(s [M, L], lse [G, L]) from c [M, H] and o [G, L, H]; backward: d c and d o on the native backward kernel (s and p re-computed
+    from c, o and the saved lse: no [M, L] tensor is kept)."""
+
+    @staticmethod
+    def forward(ctx, plan, c, o):
+        from .decoder import native_copy_attention
+
+        cd, od = c.detach().contiguous(), o.detach().contiguous()
+        s, lse = native_copy_attention(cd, plan, od)
+        ctx.save_for_backward(cd, od, lse)
+        ctx.plan = plan
+        return s, lse
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, d_s, d_lse):
+        from .decoder import native_copy_attention_backward
+
+        c, o, lse = ctx.saved_tensors
+        d_c, d_o = native_copy_attention_backward(c, ctx.plan, o, lse, d_s.contiguous().float(), d_lse.contiguous().float())
+        return None, d_c, d_o
+
+
+def copy_attention_with_grad(plan, copy_reps, o):
+    return _CopyAttentionFn.apply(plan, copy_reps, o)
+
+
+class _GatherByGraphFn(torch.autograd.Function):
+    """x[graph(row)] [M, L] for x [G, L] and the rows of a graph plan; backward: the rows of each graph summed in row order on the native
+    segmented reduce (columns padded to a multiple of 4).  The library's backward of an index gather adds with float atomics, so its
+    result changes from run to run."""
+
+    @staticmethod
+    def forward(ctx, plan, index, x):
+        ctx.plan = plan
+        return x.index_select(0, index)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        L = g.shape[1]
+        g = F_.pad(g.contiguous().float(), (0, (-L) % 4))
+        return None, None, C.segment_reduce(g, ctx.plan, N.REDUCE["sum"])[:, :L]
+
+
+def gather_by_graph(plan, index, x):
+    return _GatherByGraphFn.apply(plan, index, x)

@@ -24,7 +24,12 @@ factories import the layer classes by module path (`implementations/typilus/trai
    (the native per-graph normalisation kernels, DESIGN.md §3.9) in the same way.  The default leaves the reference's class in place,
 8. with ``native_pna=True`` only: pre-seeds / re-binds ``PnaMessageAggregation`` at
    ``ptgnn.neuralmodels.gnn.messagepassing.pna_aggregation`` (the native PNA kernel, DESIGN.md §3.10) in the same way, so that an
-   ``MlpMessagePassingLayer`` built with it runs PNA on the kernel and trains.  The default leaves the reference's class in place.
+   ``MlpMessagePassingLayer`` built with it runs PNA on the kernel and trains.  The default leaves the reference's class in place,
+9. with ``native_decoder=True`` only: re-binds ``GruCopyingDecoder`` inside ``ptgnn.neuralmodels.sequence.grucopydecoder`` and in
+   reference modules imported earlier (the native copy and memory attention kernels, DESIGN.md §3.11), so that
+   ``GruCopyingDecoderModel.build_neural_module`` builds the native class.  The module itself stays the reference's: it also holds
+   ``DecoderData``, ``TokenizedOutput`` and ``GruCopyingDecoderModel``, which graph2seq imports.  The default leaves the reference's
+   class in place.
 
 After ``install()``: ``import ptgnn.implementations.ppi.train`` etc. build ptgnn_b200 layers, unchanged.  ``uninstall()``
 restores the reference's classes.  The reference must be importable as ``ptgnn`` for steps 2-4 (it is not on the GPU test box;
@@ -53,6 +58,7 @@ _GRAPHNORM_MODULE = "ptgnn.neuralmodels.gnn.messagepassing.graphnorm"
 _GRAPHNORM_CLASS = "GraphNorm"
 _PNA_MODULE = "ptgnn.neuralmodels.gnn.messagepassing.pna_aggregation"
 _PNA_CLASS = "PnaMessageAggregation"
+_DECODER_MODULE = "ptgnn.neuralmodels.sequence.grucopydecoder"
 _saved: Dict[str, object] = {}
 
 
@@ -138,10 +144,18 @@ def _install_native_pna() -> None:
     _install_native_class(_PNA_MODULE, _PNA_CLASS, getattr(_agg, _PNA_CLASS))
 
 
+def _install_native_decoder() -> None:
+    from . import decoder as _dec
+
+    old = importlib.import_module(_DECODER_MODULE).GruCopyingDecoder
+    if old is not _dec.GruCopyingDecoder:
+        _rebind_everywhere({old: _dec.GruCopyingDecoder})      # the decoder module included
+
+
 def install(force_torch_scatter: bool = False, native_reducers: bool = False, native_selfattention: bool = False,
-            native_graphnorm: bool = False, native_pna: bool = False) -> Dict[str, object]:
+            native_graphnorm: bool = False, native_pna: bool = False, native_decoder: bool = False) -> Dict[str, object]:
     report: Dict[str, object] = {"torch_scatter": "real", "layers": False, "container": False, "metrics": False, "reducers": False,
-                                 "selfattention": False, "graphnorm": False, "pna": False}
+                                 "selfattention": False, "graphnorm": False, "pna": False, "decoder": False}
     # 1. torch_scatter
     have_real = False
     if not force_torch_scatter:
@@ -198,6 +212,10 @@ def install(force_torch_scatter: bool = False, native_reducers: bool = False, na
     if native_pna:
         _install_native_pna()
         report["pna"] = True
+    # 9. GruCopyingDecoder (opt-in)
+    if native_decoder:
+        _install_native_decoder()
+        report["decoder"] = True
     return report
 
 
