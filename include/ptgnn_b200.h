@@ -27,6 +27,8 @@
 extern "C" {
 #endif
 
+/* Moves only when an existing entry point changes its signature or meaning; added entry points leave it alone (a library built
+ * before they existed is reported by name when it is loaded). */
 #define PTGNN_B200_ABI_VERSION 4
 #define PTGNN_MAX_EDGE_TYPES 128 /* etype is stored as uint8 in the plan; 128 keeps launch params < 4 KB */
 
@@ -452,6 +454,37 @@ int ptgnn_b200_copy_attention_backward_f32(const float *copy_reps, int64_t num_r
                                            const int32_t *row_ptr, const int32_t *perm, int64_t num_graphs, const float *o,
                                            const float *lse, const float *d_s, const float *d_lse, float *d_copy_reps, float *d_o,
                                            void *workspace, size_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Embedding bag of the node embedders (reference neuralmodels/embeddings/strelementrepresentationmodel.py:16-89, TokenUnitEmbedder and
+ * SubtokenUnitEmbedder):
+ *   out[i, :] = pool_{s < len_i} table[ids[i, s], :]   [rows, dim], fp32 or bf16 when bf16_out != 0 (fp32 accumulation, rounded once)
+ *   table [vocab, dim] fp32; ids [rows, slots] int64 as the reference delivers them; lengths [rows] int64 (clamped to [0, slots]) or
+ *   NULL = every slot valid (token mode: slots = 1).  The valid slots are added in slot order.  pool MEAN divides by
+ *   fl(len) + 1e-10 (strelementrepresentationmodel.py:76); len = 0 gives 0 for SUM / MEAN and -inf for MAX.  MAX: the lowest slot wins
+ *   a tie; arg_out (optional) [rows, dim] uint8 receives the winning slot, which the backward needs.
+ *   status (optional): a device-accessible int32 (the plan's convention above); an id outside [0, vocab) is read as row 0 and
+ *   counted there.  Padding slots are never dereferenced.  No host synchronisation, deterministic (DESIGN.md §3.12).
+ *   Supported: dim in [1, 512] (16-byte loads when dim % 4 == 0: table and fp32 out then 16-byte, bf16 out 8-byte, arg_out 4-byte
+ *   aligned), slots in [1, 64] (ptgnn_b200_embedding_bag_supported).
+ * embedding_bag_pairs: the (row, token id) pair of every slot e = i slots + s, as the int64 edge lists of ptgnn_b200_plan_build with
+ *   num_nodes = vocab + 1 and num_source_nodes = rows: padding slots target the sink row `vocab`, out-of-range ids row 0.
+ * embedding_bag_backward_f32: d_table[v, :] = sum over the valid (i, s) with ids[i, s] = v of c_i d_out[i, :] (c = 1, 1 / (fl(len) +
+ *   1e-10), or [arg[i, :] == s] for MAX) from the row_ptr / perm of that plan: every row of d_table [vocab, dim] is written once
+ *   (zeros for a token that does not occur).  Occurrences are added in plan order in warp chunks, chunks in chunk order; no float
+ *   atomics.  fp32 only.
+ * ---------------------------------------------------------------------------------------------- */
+enum { PTGNN_POOL_SUM = 0, PTGNN_POOL_MEAN = 1, PTGNN_POOL_MAX = 2 };
+int32_t ptgnn_b200_embedding_bag_supported(int32_t dim, int32_t slots);
+int ptgnn_b200_embedding_bag(int32_t bf16_out, const float *table, int64_t vocab, int32_t dim, const int64_t *ids,
+                             const int64_t *lengths /* NULL: all slots */, int64_t rows, int32_t slots, int32_t pool, void *out,
+                             uint8_t *arg_out /* optional, MAX */, int32_t *status /* optional */, void *stream);
+int ptgnn_b200_embedding_bag_pairs(const int64_t *ids, const int64_t *lengths, int64_t rows, int32_t slots, int64_t vocab, int64_t *src,
+                                   int64_t *tgt, void *stream);
+size_t ptgnn_b200_embedding_bag_backward_workspace_bytes(int64_t rows, int32_t slots, int64_t vocab, int32_t dim);
+int ptgnn_b200_embedding_bag_backward_f32(const float *d_out, int64_t rows, int32_t slots, int32_t dim, const int64_t *lengths,
+                                          const uint8_t *arg /* MAX only */, int32_t pool, const int32_t *row_ptr, const int32_t *perm,
+                                          int64_t vocab, float *d_table, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Host-buffer convenience entry point (used for the end-to-end measurement): all pointers are HOST

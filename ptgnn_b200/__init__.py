@@ -8,6 +8,7 @@ is the host-side mirror of the reference interface.  There is no CPU / PyTorch f
 from .aggregation import PnaMessageAggregation
 from .batching import MinibatchAssembler
 from .decoder import GruCopyingDecoder
+from .embeddings import SubtokenUnitEmbedder, TokenUnitEmbedder
 from .edgeplan import EdgePlan, clear_plan_cache, plan_for
 from .egc import EGCMessagePassingLayer
 from .globalexchange import AbstractGlobalGraphExchange, GruGlobalStateUpdate
@@ -39,5 +40,6 @@ __all__ = [
     "AbstractGlobalGraphExchange", "GruGlobalStateUpdate", "AbstractVarSizedElementReduce", "ElementsToSummaryRepresentationInput",
     "SimpleVarSizedElementReduce", "WeightedSumVarSizedElementReduce", "SelfAttentionVarSizedElementReduce",
     "MultiheadSelfAttentionVarSizedElementReduce", "MultiHeadSelfAttentionMessagePassing", "GraphNorm", "GruCopyingDecoder",
+    "TokenUnitEmbedder", "SubtokenUnitEmbedder",
     "scatter_sum", "scatter_mean", "scatter_max", "scatter_min",
 ]

@@ -14,6 +14,7 @@ LIB_PATH = os.path.join(_HERE, "libptgnn_b200.so")
 
 REDUCE = {"sum": 0, "add": 0, "mean": 1, "max": 2, "min": 3}
 READOUT_SUM, READOUT_MEAN, READOUT_WEIGHTED_SUM = 0, 1, 2
+POOL = {"sum": 0, "mean": 1, "max": 2}
 ACT_NONE, ACT_GELU, ACT_TANH, ACT_RELU = 0, 1, 2, 3
 
 c_i32, c_i64, c_f32, c_void_p, c_size_t = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_void_p, ctypes.c_size_t
@@ -106,6 +107,13 @@ SIGNATURES = {
                                                  c_void_p, c_size_t, c_void_p]),
     "ptgnn_b200_copy_attention_backward_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_i64, c_void_p, c_void_p,
                                                               c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "ptgnn_b200_embedding_bag_supported": (c_i32, [c_i32, c_i32]),
+    "ptgnn_b200_embedding_bag": (ctypes.c_int, [c_i32, c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p,
+                                                c_void_p, c_void_p]),
+    "ptgnn_b200_embedding_bag_pairs": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_i64, c_void_p, c_void_p, c_void_p]),
+    "ptgnn_b200_embedding_bag_backward_workspace_bytes": (c_size_t, [c_i64, c_i32, c_i64, c_i32]),
+    "ptgnn_b200_embedding_bag_backward_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_i32, c_void_p, c_void_p,
+                                                             c_i64, c_void_p, c_void_p, c_size_t, c_void_p]),
     "ptgnn_b200_gated_gnn_forward_host_f32":(ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_i32,
                                                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i32, c_void_p]),
 }
@@ -117,7 +125,7 @@ class BlockPlanStruct(ctypes.Structure):
     _fields_ = [("block_targets", c_i32), ("group_off", c_void_p), ("src_f", c_void_p), ("tl_f", c_void_p), ("status", c_void_p)]
 
 
-ABI_VERSION = 4
+ABI_VERSION = 4        # moves only on incompatible changes of an existing entry point (include/ptgnn_b200.h)
 _lib: Optional[ctypes.CDLL] = None
 
 
@@ -136,7 +144,11 @@ def lib() -> ctypes.CDLL:
             )
         handle = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
-            fn = getattr(handle, name)  # AttributeError if the symbol is not exported
+            try:
+                fn = getattr(handle, name)
+            except AttributeError:      # a library built before this entry point was added (the ABI version only moves on incompatible changes)
+                raise NativeLibraryError(f"{LIB_PATH} does not export {name}: it is older than this package; rebuild it with "
+                                         "`python -m ptgnn_b200.build`") from None
             fn.restype = res
             fn.argtypes = args
         if handle.ptgnn_b200_abi_version() != ABI_VERSION:

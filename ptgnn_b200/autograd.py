@@ -648,6 +648,37 @@ def pna_with_grad(plan, delta, messages):
 
 
 # =====================================================================================================================
+# TokenUnitEmbedder / SubtokenUnitEmbedder (strelementrepresentationmodel.py:16-89): the pooled table rows on the native embedding-bag
+# kernel.  fp32 output.
+# =====================================================================================================================
+class _EmbeddingBagFn(torch.autograd.Function):
+    """out [B, D] from table [V, D] and ids [B, S]; backward: d table on the native sorted, atomic-free kernel.  Saves the ids, the
+    lengths and (max) the [B, D] uint8 winning slots: no [B, S, D] tensor exists in either direction."""
+
+    @staticmethod
+    def forward(ctx, table, ids, lengths, mode, status):
+        from .embeddings import native_embedding_bag
+
+        out, arg = native_embedding_bag(table.detach(), ids, lengths, mode, want_arg=True, status=status)
+        ctx.save_for_backward(ids, lengths, arg)     # an in-place change of the ids before the backward is then an error, not a wrong gradient
+        ctx.mode, ctx.vocab = mode, table.shape[0]
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, d_out):
+        from .embeddings import native_embedding_bag_backward
+
+        ids, lengths, arg = ctx.saved_tensors
+        d_table = native_embedding_bag_backward(d_out.contiguous().float(), ids, lengths, ctx.mode, ctx.vocab, arg)
+        return d_table, None, None, None, None
+
+
+def embedding_bag_with_grad(table, ids, lengths, mode, status=None):
+    return _EmbeddingBagFn.apply(table, ids, lengths, mode, status)
+
+
+# =====================================================================================================================
 # GruCopyingDecoder (grucopydecoder.py:95-97, 122-124): the copy scores s[i, l] = c_i . o[graph(i), l] and their per-sample logsumexp
 # on the native kernel.  fp32 copy representations.
 # =====================================================================================================================

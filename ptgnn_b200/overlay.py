@@ -29,7 +29,12 @@ factories import the layer classes by module path (`implementations/typilus/trai
    reference modules imported earlier (the native copy and memory attention kernels, DESIGN.md §3.11), so that
    ``GruCopyingDecoderModel.build_neural_module`` builds the native class.  The module itself stays the reference's: it also holds
    ``DecoderData``, ``TokenizedOutput`` and ``GruCopyingDecoderModel``, which graph2seq imports.  The default leaves the reference's
-   class in place.
+   class in place,
+10. with ``native_embedders=True`` only: re-binds ``TokenUnitEmbedder`` and ``SubtokenUnitEmbedder`` inside
+   ``ptgnn.neuralmodels.embeddings.strelementrepresentationmodel`` and in reference modules imported earlier (the native
+   embedding-bag kernels, DESIGN.md §3.12), so that ``StrElementRepresentationModel.build_neural_module`` builds the native classes for
+   ``"token"``, ``"subtoken"`` and ``"bpe"``.  The module stays the reference's: it also holds ``StrElementRepresentationModel``,
+   ``CnnConfig`` and ``CharUnitEmbedder``, which ``"char"`` still builds.  The default leaves the reference's classes in place.
 
 After ``install()``: ``import ptgnn.implementations.ppi.train`` etc. build ptgnn_b200 layers, unchanged.  ``uninstall()``
 restores the reference's classes.  The reference must be importable as ``ptgnn`` for steps 2-4 (it is not on the GPU test box;
@@ -59,6 +64,8 @@ _GRAPHNORM_CLASS = "GraphNorm"
 _PNA_MODULE = "ptgnn.neuralmodels.gnn.messagepassing.pna_aggregation"
 _PNA_CLASS = "PnaMessageAggregation"
 _DECODER_MODULE = "ptgnn.neuralmodels.sequence.grucopydecoder"
+_EMBEDDER_MODULE = "ptgnn.neuralmodels.embeddings.strelementrepresentationmodel"
+_NATIVE_EMBEDDERS = ("TokenUnitEmbedder", "SubtokenUnitEmbedder")
 _saved: Dict[str, object] = {}
 
 
@@ -152,10 +159,19 @@ def _install_native_decoder() -> None:
         _rebind_everywhere({old: _dec.GruCopyingDecoder})      # the decoder module included
 
 
+def _install_native_embedders() -> None:
+    from . import embeddings as _emb
+
+    mod = importlib.import_module(_EMBEDDER_MODULE)
+    replaced = {getattr(mod, n): getattr(_emb, n) for n in _NATIVE_EMBEDDERS if getattr(mod, n) is not getattr(_emb, n)}
+    _rebind_everywhere(replaced)       # the embedder module included
+
+
 def install(force_torch_scatter: bool = False, native_reducers: bool = False, native_selfattention: bool = False,
-            native_graphnorm: bool = False, native_pna: bool = False, native_decoder: bool = False) -> Dict[str, object]:
+            native_graphnorm: bool = False, native_pna: bool = False, native_decoder: bool = False,
+            native_embedders: bool = False) -> Dict[str, object]:
     report: Dict[str, object] = {"torch_scatter": "real", "layers": False, "container": False, "metrics": False, "reducers": False,
-                                 "selfattention": False, "graphnorm": False, "pna": False, "decoder": False}
+                                 "selfattention": False, "graphnorm": False, "pna": False, "decoder": False, "embedders": False}
     # 1. torch_scatter
     have_real = False
     if not force_torch_scatter:
@@ -216,6 +232,10 @@ def install(force_torch_scatter: bool = False, native_reducers: bool = False, na
     if native_decoder:
         _install_native_decoder()
         report["decoder"] = True
+    # 10. TokenUnitEmbedder / SubtokenUnitEmbedder (opt-in)
+    if native_embedders:
+        _install_native_embedders()
+        report["embedders"] = True
     return report
 
 
