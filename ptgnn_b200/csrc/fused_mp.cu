@@ -18,28 +18,30 @@ using tc::mbar_init;
 using tc::mbar_wait;
 
 // ---- geometry ------------------------------------------------------------------------------------------------------
-// Roles (12 warps): 0-3 and 4-7 CONSUMERS, two warpgroups | 8-9 ROW GATHERERS | 10 SCHEDULER | 11 idle.
-constexpr int NUM_THREADS = 12 * 32;
+// Roles (16 warps): 0-3 and 4-7 CONSUMERS, two warpgroups | 8-9 ROW GATHERERS | 10 SCHEDULER | 11 idle | 12-15 REDUCER.
+constexpr int NUM_THREADS = 16 * 32;
 constexpr int GATHER_WARP0 = 8, GATHER_THREADS = 64;
 constexpr int SCHED_WARP = 10;
-constexpr int NUM_CONSUMER_WARPS = 8 + 2;             // readers of the scheduler's table: consumers, gatherers
+constexpr int REDUCER_WARP0 = 12;
+constexpr int SCHED_READER_WARPS = 8 + 2 + 4;          // readers of the scheduler's table: consumers, gatherers, reducer
 constexpr int NUM_SLOTS = 3, LOOKAHEAD = 2;
 constexpr int SLOT_BYTES = 32768;
 constexpr int RING_BYTES = NUM_SLOTS * SLOT_BYTES;
 constexpr int META_RING = 8;
 constexpr int SCHED_RING = 4;
-// the producer warpgroup gives registers back, the two consumer warpgroups take them: (56 + 2 * 224) * 128 = 64512
-constexpr int CONSUMER_REGS = 224, PRODUCER_REGS = 56;
-static_assert(PRODUCER_REGS + 2 * CONSUMER_REGS <= 3 * 168, "register budgets exceed the launch allocation");
+// The launch gives every thread 128 registers; the producer and reducer warpgroups give some back and the two consumer
+// warpgroups take them (setmaxnreg, multiples of 8): (56 + 2 * 184 + 88) * 128 = 65536.  A consumer holds its weight fragments
+// (64 registers) and the main + correction accumulators (64); the reducer its 16-column walk batch.
+constexpr int PRODUCER_REGS = 56, CONSUMER_REGS = 184, REDUCER_REGS = 88;
+static_assert(PRODUCER_REGS + 2 * CONSUMER_REGS + REDUCER_REGS <= 4 * 128, "register budgets exceed the launch allocation");
 constexpr int NMAX = 64;                                        // edges per MMA (accumulator columns)
 constexpr int ACC_PITCH = NMAX + 4;                             // accumulator tile: 128 features x NMAX columns, fp32
 constexpr int ACC_BYTES = kD * ACC_PITCH * 4;
-constexpr int ALL_BAR_ID = 1, GRP_BAR_ID = 2;              // named barriers: both consumer warpgroups | warpgroup eg: 2 + eg
+constexpr int RED_BAR_ID = 1;                                   // named barrier of the reducer's four warps
 
 struct Meta {                     // per sub-group: what the epilogue needs to know about the accumulator columns
     int32_t tloff[128];           // byte offset of the column's target row inside agg_s (0 for columns >= n)
     uint32_t endmask[4];          // bit c: column c is the last edge of its (target, type) segment
-    uint32_t lowmask[4];          // bit c: column c's target lies in the lower half of the block (walked by the lower-half threads)
     int32_t n, pad[3];
 };
 struct Sched {                    // one target block: its id and the T+1 sorted-edge offsets of its (block, type) groups
@@ -77,20 +79,22 @@ __device__ __forceinline__ uint32_t swz(int row, int q) { return (uint32_t)(row 
 
 // Debug timeline (PTGNN_FUSED_TRACE=1): CTA 0, one thread per role, records (clock64, step, tag) at the pipeline hand-offs into its
 // TRACE_CAP-entry region of the trace buffer; read back with ptgnn_b200_debug_fused_trace (tools/fused_trace.py).
-// Roles: 0 = gatherer thread 0, 1 / 2 = lane 0 of warp 0 of consumer warpgroup 0 / 1.  Tags:
+// Roles: 0 = gatherer thread 0, 1 / 2 = lane 0 of warp 0 of consumer warpgroup 0 / 1, 3 = lane 0 of reducer warp 0.  Tags:
 //   gatherer  1 slot wait begins, 2 slot granted, 3 copies issued, 4 x_full arrival
 //   consumer 10 step begins, 11 the step's weight fragment loads issued (only when the (type, segment) changes; usually during
-//            the previous step or before a write-out, see the look-ahead below), 12 x_full acquired, 13 MMAs issued (the issue
-//            stalls until the fragments have arrived), 14 MMAs retired (step index); 20 staging begins, 21 staging done,
-//            22 column walk done (sub-group index); 23 / 24 write-out begins / ends
+//            the previous step, see the look-ahead below), 12 x_full acquired, 13 MMAs issued (the issue stalls until the
+//            fragments have arrived), 14 MMAs retired (step index); 20 acc_empty wait begins, 21 acc_s free (staging begins),
+//            22 staging done, acc_full arrival (sub-group index)
+//   reducer  30 acc_full wait begins, 31 acc_full acquired (column walk begins), 32 column walk done, acc_empty arrival
+//            (sub-group index); 33 / 34 write-out begins / ends (sub-group count)
 // The write counters live in shared memory and the buffer pointer is read from the kernel parameters at every mark, so the
 // marks hold no registers across the code between them.
-constexpr int TRACE_ROLES = 3, TRACE_CAP = 8192;
+constexpr int TRACE_ROLES = 4, TRACE_CAP = 8192;
 __shared__ uint32_t trace_n[TRACE_ROLES];
 __device__ __forceinline__ void trace_mark(const Params &p, int tag, uint32_t step) {
     if (p.trace == nullptr || blockIdx.x != 0) return;
     const int tid = (int)threadIdx.x;
-    const int role = tid == GATHER_WARP0 * 32 ? 0 : (tid == 0 ? 1 : (tid == 128 ? 2 : -1));
+    const int role = tid == GATHER_WARP0 * 32 ? 0 : (tid == 0 ? 1 : (tid == 128 ? 2 : (tid == REDUCER_WARP0 * 32 ? 3 : -1)));
     if (role < 0) return;
     const uint32_t n = trace_n[role];
     if (n >= TRACE_CAP) return;
@@ -99,45 +103,42 @@ __device__ __forceinline__ void trace_mark(const Params &p, int tag, uint32_t st
 }
 
 // ---- the (block, group, sub-group, segment) walk every role performs in the same order -----------------------------------
-struct Step { int blk, t, e, n, seg; bool first_sub, last_sub; };
+struct Step { int blk, t, e, n, seg; };
 template <int NSEG>
 struct StepGen {
     const Sched *sched;
     uint64_t *sfull, *sempty;
     int T, nmax, lane;
     uint32_t it = 0;
-    const Sched *tab = nullptr;
-    int blk = -1, t = 0, e0 = 0, e = 0, e1 = 0, seg = 0;
-    bool in_block = false;
+    const Sched *tab = nullptr;        // the current block's table entry, nullptr between blocks
+    int blk = -1, t = 0, e = 0, e1 = 0, seg = 0;
     // 0: `s` is the next step | 1: the block s.blk has no more steps | 2: no more blocks
     __device__ __forceinline__ int next(Step &s) {
         for (;;) {
-            if (!in_block) {
+            if (tab == nullptr) {
                 const uint32_t r = it % SCHED_RING;
                 mbar_wait(&sfull[r], (it / SCHED_RING) & 1);
-                tab = &sched[r];
-                blk = tab->blk;
+                blk = sched[r].blk;
                 if (blk < 0) return 2;
-                in_block = true;
+                tab = &sched[r];
                 t = -1; e = e1 = 0; seg = 0;
             }
             if (e < e1) {
                 s.blk = blk; s.t = t; s.e = e; s.n = min(nmax, e1 - e); s.seg = seg;
-                s.first_sub = e == e0; s.last_sub = e + nmax >= e1;
                 if (++seg == NSEG) { seg = 0; e += nmax; }
                 return 0;
             }
             ++t;
             while (t < T && tab->off[t + 1] == tab->off[t]) ++t;
             if (t >= T) {
-                in_block = false;
+                tab = nullptr;
                 s.blk = blk;
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&sempty[it % SCHED_RING]);     // this warp no longer reads the table
                 ++it;
                 return 1;
             }
-            e0 = e = tab->off[t]; e1 = tab->off[t + 1]; seg = 0;
+            e = tab->off[t]; e1 = tab->off[t + 1]; seg = 0;
         }
     }
 };
@@ -190,19 +191,15 @@ template <int RED> __device__ __forceinline__ float red_op(float a, float m) {
 }
 
 // =====================================================================================================================
-// Write-out of a finished block: the calling thread takes float4 column q (features 4 q .. 4 q + 3) of rows row_lo + r_first,
-// + r_step, + 2 r_step, ... below min(row_hi, rows of the block), two rows per iteration; a value is reset to the identity as soon
-// as it has been read.  WHOLE_ROW: a warp owns whole rows (q = lane), which the LayerNorm epilogue needs for its row reductions;
-// otherwise a half-warp owns the 64 features of its warpgroup in a row.  The row loop is specialised at compile time on the output
-// format and on "plain sum" (no mean / max fix-up / activation / LayerNorm): the generic version executed ~180 instructions per
-// row.  It runs in the consumer threads, which keep their weight fragments live across it: the fp32 instances already spill a
-// little (`-Xptxas -v`), so check that a change does not add to it.
-template <int RED, bool WHOLE_ROW>
-__device__ __forceinline__ void write_out_block(const Params *p, uint32_t agg_saddr, int row0, int row_lo, int row_hi, int r_first,
-                                                int r_step, int q) {
+// Write-out of a finished block by the reducer: warp r_first of the reducer takes whole rows r_first, + r_step, + 2 r_step, ...
+// of the block, lane q its float4 column q (features 4 q .. 4 q + 3), two rows per iteration; a value is reset to the identity as
+// soon as it has been read.  Whole rows are what the LayerNorm epilogue needs for its row reductions, and each row goes out as
+// one contiguous warp-wide store.  The row loop is specialised at compile time on the output format and on "plain sum" (no mean
+// / max fix-up / activation / LayerNorm): the generic version executed ~180 instructions per row.
+template <int RED>
+__device__ __forceinline__ void write_out_block(const Params *p, uint32_t agg_saddr, int row0, int r_first, int r_step, int q) {
     const float IDENT = red_identity<RED>();
-    const int rows = min(p->B, p->num_nodes - row0);
-    const int my_hi = min(row_hi, rows);
+    const int my_hi = min(p->B, p->num_nodes - row0);
     const float4 ident4 = make_float4(IDENT, IDENT, IDENT, IDENT);
     auto finish_row = [&](auto mode_tag, auto plain_tag, int r, float4 a) {
         constexpr int MODE = decltype(mode_tag)::value;
@@ -224,7 +221,7 @@ __device__ __forceinline__ void write_out_block(const Params *p, uint32_t agg_sa
                 a.x = apply_act(a.x, p->epi.act); a.y = apply_act(a.y, p->epi.act);
                 a.z = apply_act(a.z, p->epi.act); a.w = apply_act(a.w, p->epi.act);
             }
-            if (WHOLE_ROW && p->epi.ln_w != nullptr) {       // LayerNorm over the 128 features of the row (same order as reduce.cuh)
+            if (p->epi.ln_w != nullptr) {       // LayerNorm over the 128 features of the row (same order as reduce.cuh)
                 float sum = (a.x + a.y) + (a.z + a.w);
 #pragma unroll
                 for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
@@ -261,7 +258,7 @@ __device__ __forceinline__ void write_out_block(const Params *p, uint32_t agg_sa
     };
     // 2 rows per iteration (independent loads in flight); rows are reset as they are read: the next block needs no initialisation pass
     auto write_rows = [&](auto mode_tag, auto plain_tag) {
-        for (int r0 = row_lo + r_first; r0 < my_hi; r0 += 2 * r_step) {
+        for (int r0 = r_first; r0 < my_hi; r0 += 2 * r_step) {
             float4 v4[2];
 #pragma unroll
             for (int u = 0; u < 2; ++u) {
@@ -305,6 +302,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
     Sched *sched = reinterpret_cast<Sched *>(tail + META_RING * sizeof(Meta));
     uint64_t *bars = reinterpret_cast<uint64_t *>(tail + META_RING * sizeof(Meta) + SCHED_RING * sizeof(Sched));
     uint64_t *x_full = bars, *x_empty = bars + 3, *sched_full = bars + 6, *sched_empty = bars + 10;
+    uint64_t *acc_full = bars + 14, *acc_empty = bars + 15;
 
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
     const int lane = threadIdx.x & 31;
@@ -312,14 +310,102 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
         // x_full: per gather thread one asynchronous arrival when its copies have landed (cp.async.mbarrier.arrive.noinc) and one
         // ordinary arrival that publishes the step's column metadata
         for (int s = 0; s < NUM_SLOTS; ++s) { mbar_init(&x_full[s], 2 * GATHER_THREADS); mbar_init(&x_empty[s], 8); }
-        for (int r = 0; r < SCHED_RING; ++r) { mbar_init(&sched_full[r], 1); mbar_init(&sched_empty[r], NUM_CONSUMER_WARPS); }
+        for (int r = 0; r < SCHED_RING; ++r) { mbar_init(&sched_full[r], 1); mbar_init(&sched_empty[r], SCHED_READER_WARPS); }
+        mbar_init(acc_full, 8);                // the consumer warps, after staging a sub-group
+        mbar_init(acc_empty, 4);               // the reducer warps, after their column walk has read it
         for (int r = 0; r < TRACE_ROLES; ++r) trace_n[r] = 0;
         tc::mbar_init_fence();
     }
     __syncthreads();
     const int T = p.T;
 
-    if (warp >= GATHER_WARP0) {
+    if (warp >= REDUCER_WARP0) {
+        // ============================================ REDUCER ============================================
+        // Owns agg_s.  Thread d owns feature d, i.e. column d of agg_s, for every target of the block.  For every accumulator
+        // column (edge) of a staged sub-group, in plan order: at the first edge of a (target, type) segment the running value is
+        // (re)loaded from agg_s[target][d], at the last one it is stored back -- a target's messages are accumulated one by one
+        // in the reference's order, across types and sub-groups.  Then it writes out and resets every finished block, with the
+        // mean / activation / LayerNorm epilogue; its warps own whole rows there.
+        // The walk reads the sub-group's column metadata from the Meta ring.  The gatherers write the metadata of sub-group c
+        // before they wait for its slot, i.e. after the consumers have released sub-group c - 1 - NUM_SLOTS; a consumer releases
+        // a sub-group only after it has staged the one before, which waits until the reducer is done with the one before that.
+        // So the reducer reads metadata at most NUM_SLOTS + 2 = 5 sub-groups behind the writer, inside the META_RING = 8 entries.
+        tc::reg_dealloc<REDUCER_REGS>();
+        const int d = (int)threadIdx.x - REDUCER_WARP0 * 32, rw = warp - REDUCER_WARP0;
+        const uint32_t aggcol_s = smem_u32(agg_s + d);      // shared-space address of agg_s[0][d]
+        const uint32_t accrow_s = smem_u32(acc_s + d * ACC_PITCH);
+        const float IDENT = red_identity<RED>();
+        for (int r = 0; r < p.B; ++r) agg_s[r * kD + d] = IDENT;
+        StepGen<NSEG> gen{sched, sched_full, sched_empty, T, NMAX, lane};
+        uint32_t sg = 0;
+        float acc = IDENT;
+        Step s;
+        for (int ev; (ev = gen.next(s)) != 2;) {
+            if (ev == 1) {
+                // ---- block s.blk finished: every thread's last stores precede the write-out's reads of whole rows, and the
+                // write-out's resets precede the next block's walk
+                trace_mark(p, 33, sg);
+                named_bar_sync(RED_BAR_ID, 128);
+                write_out_block<RED>(&p, smem_u32(agg_s), s.blk * p.B, rw, 4, lane);
+                named_bar_sync(RED_BAR_ID, 128);
+                trace_mark(p, 34, sg);
+                continue;
+            }
+            if (s.seg != NSEG - 1) continue;
+            trace_mark(p, 30, sg);
+            mbar_wait(acc_full, sg & 1);
+            trace_mark(p, 31, sg);
+            const Meta *m = &meta_ring[sg % META_RING];
+            const int n = s.n;
+            constexpr int W = 16;
+            for (int c0 = 0; c0 < n; c0 += W) {
+                uint32_t vm[W];
+#pragma unroll
+                for (int j = 0; j < W / 4; ++j) {
+                    const float4 v4 = lds_f32x4(accrow_s + (uint32_t)(c0 + 4 * j) * 4u);
+                    vm[4 * j] = __float_as_uint(v4.x); vm[4 * j + 1] = __float_as_uint(v4.y);
+                    vm[4 * j + 2] = __float_as_uint(v4.z); vm[4 * j + 3] = __float_as_uint(v4.w);
+                }
+                uint32_t addr[W];
+#pragma unroll
+                for (int j = 0; j < W / 4; ++j) {
+                    const int4 o = *reinterpret_cast<const int4 *>(&m->tloff[c0 + 4 * j]);
+                    addr[4 * j] = aggcol_s + o.x; addr[4 * j + 1] = aggcol_s + o.y;
+                    addr[4 * j + 2] = aggcol_s + o.z; addr[4 * j + 3] = aggcol_s + o.w;
+                }
+                // bit c: column c0 + c ends a segment (never set for columns >= n, so those are never stored)
+                const uint32_t endw = (m->endmask[c0 >> 5] >> (c0 & 31)) & 0xFFFFu;
+                // the column before this batch ended a segment (or the batch opens the sub-group: always reload)
+                const uint32_t prev_end = c0 == 0 ? 1u : (m->endmask[(c0 - 1) >> 5] >> ((c0 - 1) & 31)) & 1u;
+                const uint32_t startw = (endw << 1) | prev_end;
+                float pre[W];
+#pragma unroll
+                for (int c = 0; c < W; ++c) pre[c] = lds_f32(addr[c]);
+                // t[c] = op(pre[c], v[c]) for every column (independent); a column that CONTINUES a segment (rare: most
+                // (target, type) segments hold one edge) then overwrites it with op(t[c-1], v[c]) -- a predicated op, in column
+                // order, so a target's messages are still combined one by one in plan order.  Columns beyond n (up to the MMA's
+                // N) are computed but never stored.
+                float t[W];
+                constexpr bool ADD = RED == PTGNN_REDUCE_SUM || RED == PTGNN_REDUCE_MEAN;
+#pragma unroll
+                for (int c = 0; c < W; ++c) {
+                    const float v = __uint_as_float(vm[c]);
+                    t[c] = ADD ? __fadd_rn(pre[c], v) : red_op<RED>(pre[c], v);
+                }
+                continue_segment<RED>(t[0], acc, __uint_as_float(vm[0]), startw & 1u);
+#pragma unroll
+                for (int c = 1; c < W; ++c) continue_segment<RED>(t[c], t[c - 1], __uint_as_float(vm[c]), startw & (1u << c));
+                acc = t[W - 1];
+#pragma unroll
+                for (int c = 0; c < W; ++c) sts_f32_if(addr[c], t[c], endw & (1u << c));
+            }
+            // every column of acc_s has been read: the consumers may stage the next sub-group
+            __syncwarp();
+            if (lane == 0) mbar_arrive(acc_empty);
+            trace_mark(p, 32, sg);
+            ++sg;
+        }
+    } else if (warp >= GATHER_WARP0) {
         tc::reg_dealloc<PRODUCER_REGS>();
         if (warp == SCHED_WARP) {
             // ============================================ SCHEDULER ============================================
@@ -393,8 +479,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
                     const bool end = valid && tl_b[half] != tl_a[half];      // last column (tl_b = -2) or the target changes
                     m->tloff[c] = valid ? tl_a[half] * (kD * 4) : 0;
                     const uint32_t word = __ballot_sync(0xffffffffu, end);
-                    const uint32_t low = __ballot_sync(0xffffffffu, valid && tl_a[half] < (p.B >> 1));
-                    if (lane == 0) { m->endmask[c >> 5] = word; m->lowmask[c >> 5] = low; }
+                    if (lane == 0) m->endmask[c >> 5] = word;
                 }
                 if (g == 0) m->n = st.n;
                 ++sgc;
@@ -447,48 +532,24 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
         // loaded from the packed weights when the (type, segment) changes), B = the gathered rows of the slot, N = the
         // sub-group's edge count rounded up to 16; the finished sub-group goes to rows [64 eg, 64 eg + 64) of
         // acc_s[feature][edge] (main + 2^-11 correction).
-        // Reduction: thread d owns feature fw, i.e. column fw of agg_s, for the targets of one half of the block.  For every
-        // accumulator column (edge) of its half, in plan order: at the first edge of a (target, type) segment the running value is
-        // (re)loaded from agg_s[target][fw], at the last one it is stored back -- a target's messages are accumulated one by one in
-        // the reference's order, across types and sub-groups.  Edges are sorted by target, so each half owns a contiguous column
-        // range of every sub-group.  Two assignments:
-        //  * SPLIT (fp32, 3xFP16): warpgroup eg also reduces and writes out its own features, fw = 64 eg + (d & 63); warps 0-1 take
-        //    the lower half, warps 2-3 the upper half.  The warpgroups touch disjoint acc_s rows and disjoint agg_s columns, so they
-        //    never wait for each other (except around the LayerNorm write-out, which needs whole rows): one issues its three
-        //    products' MMAs while the other reduces.  How far they can drift apart is bounded by the x ring: a slot is refilled
-        //    only after all 8 consumer warps have released it.
-        //  * lock-step (bf16): fw = d, warpgroup eg takes half eg for all 128 features, so both meet around the staging.  A bf16
-        //    step's MMAs are too short to hide a column walk behind; split, the bf16 kernel was measured 6-12 % slower.
-        // Meta ring reuse: the gatherers write the metadata of step c before they wait for its slot, i.e. after every consumer
-        // warp has released step c - 1 - NUM_SLOTS; a warp that has released step k reads only metadata of sub-groups >= k's.  So
-        // the slowest reader is at most NUM_SLOTS + 1 = 4 sub-groups behind the writer, inside the META_RING = 8 entries.
-        // SPLIT: weight fragments are loaded one event ahead: right after a step's MMAs retire (or before a block's write-out)
-        // the walk is advanced to the next step, and if that step needs other weights their loads are issued then, so the L2
-        // round trip runs under the staging, the column walk and the write-out instead of in front of the next MMA.  Lock-step
-        // (bf16) loads them in line at the step (measured 1.5 % faster there).
+        // The consumers only fetch, multiply and stage; the reducer owns the reduction and the write-out.  The two warpgroups
+        // meet only through acc_s: a warpgroup waits on acc_empty (the reducer has walked the previous sub-group) before it
+        // stages, and its warps arrive on acc_full when they have.  One acc_s buffer is enough: while the reducer walks
+        // sub-group k the consumers already run the MMAs of k + 1 in registers.  How far the warpgroups drift apart is bounded
+        // by the x ring (a slot is refilled only after all 8 consumer warps have released it) and by acc_empty.
+        // Weight fragments are loaded one step ahead: right after a step's MMAs retire the walk is advanced to the next step,
+        // and if that step needs other weights their loads are issued then, so the L2 round trip runs under the acc_empty wait
+        // and the staging instead of in front of the next MMA.  That look-ahead never waits for the scheduler (it stops at the
+        // end of the block); the look-up of the next block comes after the block's last sub-group has been staged.
         tc::reg_alloc<CONSUMER_REGS>();
-        constexpr bool SPLIT = NPROD == 3;
         const int eg = warp >> 2, ew = warp & 3;
-        const int d = ew * 32 + lane;
         const int gq = lane >> 2, tq = lane & 3;
         const int f0 = 64 * eg + 16 * ew + gq;               // this thread's A / accumulator rows: features f0, f0 + 8
-        // the feature this thread reduces, and which targets: 0 = the lower half of the block, 1 = the upper half
-        const int fw = SPLIT ? 64 * eg + (d & 63) : d, half = SPLIT ? d >> 6 : eg;
-        const uint32_t aggcol_s = smem_u32(agg_s + fw);     // shared-space address of agg_s[0][fw]
-        const uint32_t accrow_s = smem_u32(acc_s + fw * ACC_PITCH);
-        const int grp_bar = GRP_BAR_ID + eg;
-        const int stage_bar = SPLIT ? grp_bar : ALL_BAR_ID, stage_threads = SPLIT ? 128 : 256;   // around the staging
-        const float IDENT = red_identity<RED>();
         StepGen<NSEG> gen{sched, sched_full, sched_empty, T, NMAX, lane};
-        {
-            const int row_lo = half == 0 ? 0 : (p.B >> 1), row_hi = half == 0 ? (p.B >> 1) : p.B;     // the rows this thread walks
-            for (int r = row_lo; r < row_hi; ++r) agg_s[r * kD + fw] = IDENT;
-        }
         uint32_t sg = 0, xs = 0;
         int w_t = -1, w_seg = -1;
         uint32_t wf[NPART][K / 16][4];
         float acc_m[32], acc_c[32];
-        float acc = IDENT;
         auto load_weights = [&](const Step &st) {
             // packed layout: wpack[(((t * NSEG + seg) * NPART + part) * (K / 8) + c4) * 128 + d] = columns 8 c4 .. + 7 of row d
             const uint32_t *wp = reinterpret_cast<const uint32_t *>(p.wpack + (size_t)(st.t * NSEG + st.seg) * NPART * (K / 8) * 128);
@@ -531,7 +592,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
         while (ev != 2) {
             if (ev == 0) {
                 trace_mark(p, 10, xs);
-                if (s.t != w_t || s.seg != w_seg) load_weights(s);      // the first step, or the first after a block without steps
+                if (s.t != w_t || s.seg != w_seg) load_weights(s);      // a block's first step: the look-ahead stops at block ends
                 const uint32_t slot = xs % NUM_SLOTS;
                 mbar_wait(&x_full[slot], (xs / NUM_SLOTS) & 1);
                 tc::fence_proxy_async_smem();          // rows written by cp.async (generic proxy) -> read by the MMA (async proxy)
@@ -554,110 +615,43 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
                 trace_mark(p, 13, xs);
                 tc::wgmma_wait<0>();
                 tc::fence_acc(acc_m);
-                tc::fence_acc(acc_c);
+                if (NPROD == 3) tc::fence_acc(acc_c);
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&x_empty[slot]);
                 trace_mark(p, 14, xs);
                 ++xs;
                 const int evn = gen.next(nx);          // look ahead; the fragments are free until nx's MMAs
-                if (SPLIT && evn == 0 && (nx.t != w_t || nx.seg != w_seg)) load_weights(nx);
+                if (evn == 0 && (nx.t != w_t || nx.seg != w_seg)) load_weights(nx);
                 if (s.seg == NSEG - 1) {
-                    // ---- the sub-group's messages -> this group's rows of acc_s (feature-major), then the reduction along the columns
+                    // ---- the sub-group's messages -> this group's rows of acc_s (feature-major), for the reducer's column walk
                     trace_mark(p, 20, sg);
-                    named_bar_sync(stage_bar, stage_threads);    // the readers of these acc_s rows are done with the previous sub-group
+                    mbar_wait(acc_empty, (sg & 1) ^ 1);    // the reducer has walked the previous sub-group
+                    trace_mark(p, 21, sg);
 #pragma unroll
                     for (int j = 0; j < 8; ++j) {
                         if (8 * j < 16 * nb) {          // columns the MMA did not compute are never read
 #pragma unroll
                         for (int h = 0; h < 2; ++h) {
                             float v0 = acc_m[4 * j + 2 * h], v1 = acc_m[4 * j + 2 * h + 1];
-                            if (NPROD == 3) { v0 = fmaf(acc_c[4 * j + 2 * h], 1.0f / 2048.0f, v0); v1 = fmaf(acc_c[4 * j + 2 * h + 1], 1.0f / 2048.0f, v1); }
+                            if (NPROD == 3) {
+                                v0 = fmaf(acc_c[4 * j + 2 * h], 1.0f / 2048.0f, v0); v1 = fmaf(acc_c[4 * j + 2 * h + 1], 1.0f / 2048.0f, v1);
+                            } else {                    // the autocast Linear's bf16 output
+                                v0 = __bfloat162float(__float2bfloat16_rn(v0)); v1 = __bfloat162float(__float2bfloat16_rn(v1));
+                            }
                             *reinterpret_cast<float2 *>(acc_s + (f0 + 8 * h) * ACC_PITCH + 8 * j + 2 * tq) = make_float2(v0, v1);
                         }
                         }
                     }
-                    named_bar_sync(stage_bar, stage_threads);
-                    trace_mark(p, 21, sg);
-                    const Meta *m = &meta_ring[sg % META_RING];
-                    const int n = s.n;
-                    int split = __popc(m->lowmask[0]) + __popc(m->lowmask[1]);
-                    const int c_lo = half == 0 ? 0 : split, c_hi = half == 0 ? split : n;       // this thread's columns
-                    constexpr int W = 16;
-                    for (int c0 = c_lo & ~15; c0 < c_hi; c0 += 16) {
-                        uint32_t vm[W];
-#pragma unroll
-                        for (int j = 0; j < W / 4; ++j) {
-                            const float4 v4 = lds_f32x4(accrow_s + (uint32_t)(c0 + 4 * j) * 4u);
-                            vm[4 * j] = __float_as_uint(v4.x); vm[4 * j + 1] = __float_as_uint(v4.y);
-                            vm[4 * j + 2] = __float_as_uint(v4.z); vm[4 * j + 3] = __float_as_uint(v4.w);
-                        }
-                        uint32_t addr[W];
-#pragma unroll
-                        for (int j = 0; j < W / 4; ++j) {
-                            const int4 o = *reinterpret_cast<const int4 *>(&m->tloff[c0 + 4 * j]);
-                            addr[4 * j] = aggcol_s + o.x; addr[4 * j + 1] = aggcol_s + o.y;
-                            addr[4 * j + 2] = aggcol_s + o.z; addr[4 * j + 3] = aggcol_s + o.w;
-                        }
-                        const uint32_t endw = (m->endmask[c0 >> 5] >> (c0 & 31)) & 0xFFFFu;
-                        // the column before this batch ended a segment (or the batch opens the sub-group: always reload)
-                        const uint32_t prev_end = c0 == 0 ? 1u : (m->endmask[(c0 - 1) >> 5] >> ((c0 - 1) & 31)) & 1u;
-                        const uint32_t startw = (endw << 1) | prev_end;
-                        // columns of the batch that belong to this thread: [max(c_lo, c0), min(c_hi, c0 + 16))
-                        const int first = c_lo > c0 ? c_lo - c0 : 0, last = c_hi - c0 < W ? c_hi - c0 : W;
-                        const uint32_t storew = endw & (0xFFFFu << first) & (0xFFFFu >> (W - last));
-                        float pre[W];
-#pragma unroll
-                        for (int c = 0; c < W; ++c) pre[c] = lds_f32(addr[c]);
-                        // t[c] = op(pre[c], v[c]) for every column (independent); a column that CONTINUES a segment (rare: most
-                        // (target, type) segments hold one edge) then overwrites it with op(t[c-1], v[c]) -- a predicated op, in
-                        // column order, so a target's messages are still combined one by one in plan order.  Columns of the other
-                        // half are computed but never stored (those beyond the MMA's N hold stale values); this thread's first
-                        // column always starts a segment.
-                        float t[W];
-                        constexpr bool ADD = RED == PTGNN_REDUCE_SUM || RED == PTGNN_REDUCE_MEAN;
-#pragma unroll
-                        for (int c = 0; c < W; ++c) {
-                            float v = __uint_as_float(vm[c]);
-                            if (NPROD == 1) {                           // the autocast Linear's bf16 output
-                                v = __bfloat162float(__float2bfloat16_rn(v));
-                                vm[c] = __float_as_uint(v);
-                            }
-                            t[c] = ADD ? __fadd_rn(pre[c], v) : red_op<RED>(pre[c], v);
-                        }
-                        continue_segment<RED>(t[0], acc, __uint_as_float(vm[0]), startw & 1u);
-#pragma unroll
-                        for (int c = 1; c < W; ++c) continue_segment<RED>(t[c], t[c - 1], __uint_as_float(vm[c]), startw & (1u << c));
-                        acc = t[W - 1];
-#pragma unroll
-                        for (int c = 0; c < W; ++c) sts_f32_if(addr[c], t[c], storew & (1u << c));
-                    }
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(acc_full);  // release: the warp's acc_s stores
                     trace_mark(p, 22, sg);
                     ++sg;
                 }
                 s = nx; ev = evn;
                 continue;
             }
-            // ---- block s.blk finished.  Each group writes out its 64 features of every row as soon as its own four warps are done
-            // (no waiting for the other group); the next sub-group's first staging barrier orders these reads and resets before
-            // that group's next column walk.  The LayerNorm epilogue needs whole rows: both groups meet, each writes out half of the
-            // rows, and they meet again before either walks the next block.
-            const int blk = s.blk;
-            const int evn = gen.next(nx);
-            if (SPLIT && evn == 0 && (nx.t != w_t || nx.seg != w_seg)) load_weights(nx);
-            trace_mark(p, 23, sg);
-            if (SPLIT && p.epi.ln_w == nullptr) {
-                named_bar_sync(grp_bar, 128);
-                write_out_block<RED, false>(&p, smem_u32(agg_s), blk * p.B, 0, p.B, 2 * ew + (lane >> 4), 8, 16 * eg + (lane & 15));
-            } else {
-                // whole rows, warpgroup eg the rows of half eg; in lock-step mode those are exactly the rows it walked
-                const int wbar = SPLIT ? ALL_BAR_ID : grp_bar, wthreads = SPLIT ? 256 : 128;
-                named_bar_sync(wbar, wthreads);
-                const int row_lo = eg == 0 ? 0 : (p.B >> 1), row_hi = eg == 0 ? (p.B >> 1) : p.B;
-                write_out_block<RED, true>(&p, smem_u32(agg_s), blk * p.B, row_lo, row_hi, ew, 4, lane);
-                named_bar_sync(wbar, wthreads);
-            }
-            trace_mark(p, 24, sg);
-            s = nx; ev = evn;
+            // ---- block s.blk finished (the reducer writes it out): look up the next block's first step
+            ev = gen.next(s);
         }
     }
 }

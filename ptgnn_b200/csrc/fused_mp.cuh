@@ -27,12 +27,13 @@
 // represented: the packing kernels raise a status flag and the host raises (PTGNN_B200_FP32_MODE=tf32 selects the
 // unfused 3xTF32 kernels).
 //
-// Roles (12 warps):  0-3 and 4-7 CONSUMERS, two warpgroups computing the MMAs for features [0,64) / [64,128).  fp32: each
-//   also reduces and writes out its own features (disjoint agg_s columns: the groups run independently, one's MMAs overlap the
-//   other's reduction); inside a group warps 0-1 reduce the columns whose target lies in the lower half of the block, warps
-//   2-3 the upper half.  bf16: lock-step, group 0 reduces all 128 features of the lower-half targets, group 1 the upper half |
+// Roles (16 warps):  0-3 and 4-7 CONSUMERS, two warpgroups computing the MMAs for features [0,64) / [64,128) and staging
+//   them into the feature-major tile acc_s; they never touch agg_s |
 //   8-9 ROW GATHERERS (16-byte cp.async into a 3-slot ring, SWIZZLE_128B K-major) |
-//   10 SCHEDULER (block -> group offsets table ring).
+//   10 SCHEDULER (block -> group offsets table ring) |
+//   12-15 REDUCER: owns agg_s; thread d walks feature d of every staged sub-group, then writes out and resets every finished
+//   block (mean / activation / LayerNorm epilogue).  Consumers and reducer hand acc_s over with two mbarriers (acc_full,
+//   acc_empty), so the walk and the write-out run while the consumers already multiply the next sub-group.
 #pragma once
 #include "common.cuh"
 

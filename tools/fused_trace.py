@@ -36,7 +36,7 @@ lib = N.lib()
 lib.ptgnn_b200_debug_fused_trace.argtypes = [ctypes.c_void_p]
 cap = lib.ptgnn_b200_debug_fused_trace(None)
 assert cap > 0, "tracing is off"
-roles = ["gather", "wg0", "wg1"]
+roles = ["gather", "wg0", "wg1", "reducer"]
 buf = (ctypes.c_ulonglong * (len(roles) * cap))()
 lib.ptgnn_b200_debug_fused_trace(buf)
 ev = {}
@@ -82,20 +82,27 @@ for name in ("wg0", "wg1"):
     span = max(c for c, _, _ in evs) - min(c for c, _, _ in evs)
     st = by_step(name, (10, 11, 12, 13, 14))
     sub = by_step(name, (20, 21, 22))
-    wo = [(c, t) for c, _, t in evs if t in (23, 24)]
     print(f"{name}: span {span} cycles, {len(st)} steps, {len(sub)} sub-groups, "
-          f"{sum(1 for _, t in wo if t == 23)} write-outs, weights reloaded on {sum(1 for v in st.values() if 11 in v)} steps")
+          f"weights reloaded on {sum(1 for v in st.values() if 11 in v)} steps")
     order = sorted(evs)
-    # fragment loads are issued in line (after the step's 10) or, with a look-ahead, after the previous step's 14 / before a write-out
+    # fragment loads are issued in line (after the step's 10) or, with a look-ahead, after the previous step's 14
     line("weight fetch issue (prev event -> 11)", [c - order[i - 1][0] for i, (c, _, t) in enumerate(order) if t == 11 and i > 0], span)
     line("x_full wait (10 or 11 -> 12)", [v[12] - max(v[10], v.get(11, 0)) for v in st.values() if 10 in v and 12 in v], span)
     line("MMA issue, new weights (12->13)", [v[13] - v[12] for v in st.values() if 11 in v and 12 in v and 13 in v], span)
     line("MMA issue, same weights (12->13)", [v[13] - v[12] for v in st.values() if 11 not in v and 12 in v and 13 in v], span)
     line("MMA retire (13->14)", [v[14] - v[13] for v in st.values() if 13 in v and 14 in v], span)
-    line("staging incl. barriers (20->21)", [v[21] - v[20] for v in sub.values() if 20 in v and 21 in v], span)
-    line("column walk (21->22)", [v[22] - v[21] for v in sub.values() if 21 in v and 22 in v], span)
-    ends = [c for c, t in wo if t == 23]
-    outs = [c for c, t in wo if t == 24]
-    line("write-out incl. barriers (23->24)", [b_ - a for a, b_ in zip(ends, outs)], span)
+    line("acc_empty wait (20->21)", [v[21] - v[20] for v in sub.values() if 20 in v and 21 in v], span)
+    line("staging (21->22)", [v[22] - v[21] for v in sub.values() if 21 in v and 22 in v], span)
     # from the previous event to a step's begin (10): loop overhead, block-table waits
     line("before step begin (prev event -> 10)", [c - order[i - 1][0] for i, (c, _, t) in enumerate(order) if t == 10 and i > 0], span)
+evs = ev["reducer"]
+if evs:
+    span = max(c for c, _, _ in evs) - min(c for c, _, _ in evs)
+    sub = by_step("reducer", (30, 31, 32))
+    wo = [(c, t) for c, _, t in evs if t in (33, 34)]
+    print(f"reducer: span {span} cycles, {len(sub)} sub-groups, {sum(1 for _, t in wo if t == 33)} write-outs")
+    line("acc_full wait (30->31)", [v[31] - v[30] for v in sub.values() if 30 in v and 31 in v], span)
+    line("column walk (31->32)", [v[32] - v[31] for v in sub.values() if 31 in v and 32 in v], span)
+    begins = [c for c, t in wo if t == 33]
+    ends = [c for c, t in wo if t == 34]
+    line("write-out incl. barriers (33->34)", [b_ - a for a, b_ in zip(begins, ends)], span)
