@@ -487,6 +487,39 @@ int ptgnn_b200_embedding_bag_backward_f32(const float *d_out, int64_t rows, int3
                                           int64_t vocab, float *d_table, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Character CNN of the char node embedder (reference neuralmodels/embeddings/strelementrepresentationmodel.py:100-142,
+ * CharUnitEmbedder), for each token t of chars [rows, max_chars] int64 (ids in [0, chars)):
+ *   a1[t, r] = relu(b1 + sum_{tap < l1_window} W1[:, chars[t, r + tap], tap]),  a2 = relu(conv(a1, W2) + b2),
+ *   out[t, d] = max over positions p of conv(a2, W3)[t, d, p]   [rows, dim], fp32, or bf16 when bf16_out != 0
+ * with W1 [l1_filters, chars, l1_window], b1 [l1_filters], W2 [l2_filters, l1_filters, l2_window], b2 [l2_filters],
+ * W3 [dim, l2_filters, out_window] (nn.Conv1d layouts, fp32).  One kernel; only the ids and out touch global memory per token.
+ * fp32: 3xFP16 tensor-core products; bf16: one bf16 product, a1, a2 and the conv output rounded to bf16 as autocast's conv1d does.
+ * The lowest position wins a tie of the max, NaN propagates; arg_out (optional) [rows, dim] uint8 receives the winning position.
+ * status (optional): two device-accessible int32 words: [0] counts ids outside [0, chars) (read as 0), [1] is set to 1 when an
+ * fp32 operand is outside the fp16 range (|x| >= 65504).  No host synchronisation, no float atomics (DESIGN.md §3.13).
+ *   Supported (ptgnn_b200_char_cnn_supported): chars >= 1, l1_filters, l2_filters in {64, 128, 256}, windows in [1, 5],
+ *   dim in [1, 256], max_chars in [l1_window + l2_window + out_window - 2, 32], rows * max_chars < 2^31.
+ * char_cnn_workspace_bytes / char_cnn_prepare: the derived weights (W1 as a [chars * l1_window, l1_filters] gather table, the biases,
+ *   W2 and W3 split and pre-swizzled into tensor-core stages) in a 1024-byte aligned buffer; prepare once per parameter version,
+ *   pass the same buffer and bf16 flag to the forward.  prepare sets status[1] for an fp32 weight outside the fp16 range.
+ * char_cnn_materialise_f32 (training backward): the same kernel, fp32, writes the post-ReLU activations a1 [rows * (max_chars -
+ *   l1_window + 1), l1_filters] and a2 [rows * (max_chars - l1_window - l2_window + 2), l2_filters] (token-major) instead of out.
+ * ---------------------------------------------------------------------------------------------- */
+int32_t ptgnn_b200_char_cnn_supported(int32_t chars, int32_t l1_filters, int32_t l1_window, int32_t l2_filters, int32_t l2_window,
+                                      int32_t dim, int32_t out_window, int32_t max_chars);
+size_t ptgnn_b200_char_cnn_workspace_bytes(int32_t bf16, int32_t chars, int32_t l1_filters, int32_t l1_window, int32_t l2_filters,
+                                           int32_t l2_window, int32_t dim, int32_t out_window);
+int ptgnn_b200_char_cnn_prepare(int32_t bf16, const float *w1, const float *b1, const float *w2, const float *b2, const float *w3,
+                                int32_t chars, int32_t l1_filters, int32_t l1_window, int32_t l2_filters, int32_t l2_window, int32_t dim,
+                                int32_t out_window, void *prepared, size_t prepared_bytes, int32_t *status, void *stream);
+int ptgnn_b200_char_cnn_forward(int32_t bf16_out, const int64_t *chars_ids, int64_t rows, int32_t max_chars, int32_t chars,
+                                int32_t l1_filters, int32_t l1_window, int32_t l2_filters, int32_t l2_window, int32_t dim, int32_t out_window,
+                                const void *prepared, size_t prepared_bytes, void *out, uint8_t *arg_out, int32_t *status, void *stream);
+int ptgnn_b200_char_cnn_materialise_f32(const int64_t *chars_ids, int64_t rows, int32_t max_chars, int32_t chars, int32_t l1_filters,
+                                        int32_t l1_window, int32_t l2_filters, int32_t l2_window, int32_t dim, int32_t out_window,
+                                        const void *prepared, size_t prepared_bytes, float *a1, float *a2, int32_t *status, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Host-buffer convenience entry point (used for the end-to-end measurement): all pointers are HOST
  * memory; copies inputs to the device, builds the plan, runs `num_layers` GatedMessagePassingLayers
  * (layer l uses weight set l; pass the same pointers to share weights), copies the final states back

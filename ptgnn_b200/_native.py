@@ -114,6 +114,13 @@ SIGNATURES = {
     "ptgnn_b200_embedding_bag_backward_workspace_bytes": (c_size_t, [c_i64, c_i32, c_i64, c_i32]),
     "ptgnn_b200_embedding_bag_backward_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_i32, c_void_p, c_void_p,
                                                              c_i64, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "ptgnn_b200_char_cnn_supported": (c_i32, [c_i32] * 8),
+    "ptgnn_b200_char_cnn_workspace_bytes": (c_size_t, [c_i32] * 8),
+    "ptgnn_b200_char_cnn_prepare": (ctypes.c_int, [c_i32] + [c_void_p] * 5 + [c_i32] * 7 + [c_void_p, c_size_t, c_void_p, c_void_p]),
+    "ptgnn_b200_char_cnn_forward": (ctypes.c_int, [c_i32, c_void_p, c_i64, c_i32] + [c_i32] * 7 + [c_void_p, c_size_t, c_void_p, c_void_p,
+                                                                                               c_void_p, c_void_p]),
+    "ptgnn_b200_char_cnn_materialise_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32] + [c_i32] * 7 + [c_void_p, c_size_t, c_void_p, c_void_p,
+                                                                                                 c_void_p, c_void_p]),
     "ptgnn_b200_gated_gnn_forward_host_f32":(ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_i32,
                                                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i32, c_void_p]),
 }

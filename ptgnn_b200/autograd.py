@@ -679,6 +679,87 @@ def embedding_bag_with_grad(table, ids, lengths, mode, status=None):
 
 
 # =====================================================================================================================
+# CharUnitEmbedder (strelementrepresentationmodel.py:100-142): the character CNN on the native kernel.  fp32.
+# =====================================================================================================================
+CHAR_BACKWARD_CHUNK = 4096      # tokens per backward chunk: the backward's workspace is bounded by this, not by B
+
+
+def _col2im(y: torch.Tensor, Bc: int, L_out: int, w: int, F: int, L_in: int) -> torch.Tensor:
+    """d input [Bc, L_in, F] of a convolution from y [Bc L_out, w F] = d out W_tap for every tap: the taps added in tap order."""
+    yv = y.view(Bc, L_out, w, F)
+    d = torch.zeros(Bc, L_in, F, dtype=torch.float32, device=y.device)
+    for tap in range(w):
+        d[:, tap:tap + L_out] += yv[:, :, tap]
+    return d
+
+
+def _char_cnn_backward(d_out, chars, arg, prepared, shape, w2, w3):
+    """Gradients of (W1, b1, W2, b2, W3) from d_out [B, D] fp32, in chunks of CHAR_BACKWARD_CHUNK tokens whose results are added in
+    chunk order.  Per chunk: the kernel's materialise mode gives a1 and a2; d_out goes to its winning positions; dW3 and dW2 are split
+    fp16 library GEMMs over the im2col of a2 and a1; d a2 and d a1 are native ``linear`` products followed by a col2im that adds the taps
+    in a fixed order; dW1 is the table gradient of an embedding bag over the (token, position) rows.  No float atomics."""
+    from .embeddings import native_char_cnn_materialise, native_embedding_bag_backward
+
+    V, F1, k1, F2, k2, D, k3 = shape
+    B, L = chars.shape
+    L1, L2 = L - k1 + 1, L - k1 - k2 + 2
+    L3 = L2 - k3 + 1
+    dev = d_out.device
+    f32 = dict(dtype=torch.float32, device=dev)
+    d_t1, d_b1 = torch.zeros(V * k1, F1, **f32), torch.zeros(F1, **f32)
+    d_w2, d_b2, d_w3 = torch.zeros(F2, F1 * k2, **f32), torch.zeros(F2, **f32), torch.zeros(D, F2 * k3, **f32)
+    w3cat = w3.detach().permute(2, 1, 0).reshape(k3 * F2, D).contiguous()      # [tap F2 + k, d] = W3[d, k, tap]
+    w2cat = w2.detach().permute(2, 1, 0).reshape(k2 * F1, F2).contiguous()
+    taps = torch.arange(k1, device=dev)
+    for c0 in range(0, B, CHAR_BACKWARD_CHUNK):
+        ch = chars[c0:c0 + CHAR_BACKWARD_CHUNK]
+        Bc = ch.shape[0]
+        a1, a2 = native_char_cnn_materialise(ch, shape, prepared)
+        dl3 = torch.zeros(Bc, L3, D, **f32)
+        dl3.scatter_(1, arg[c0:c0 + Bc].long().unsqueeze(1), d_out[c0:c0 + Bc].unsqueeze(1))
+        dl3 = dl3.view(Bc * L3, D)
+        x3 = a2.view(Bc, L2, F2).unfold(1, k3, 1).reshape(Bc * L3, F2 * k3)
+        with _exact_fp16_gemms():
+            d_w3 += _mm_t_split(_split16(dl3), _split16(x3))
+        dl2 = _col2im(C.linear(dl3, w3cat), Bc, L3, k3, F2, L2).mul_(a2.view(Bc, L2, F2) > 0).view(Bc * L2, F2)
+        d_b2 += dl2.sum(dim=0)
+        x2 = a1.view(Bc, L1, F1).unfold(1, k2, 1).reshape(Bc * L2, F1 * k2)
+        with _exact_fp16_gemms():
+            d_w2 += _mm_t_split(_split16(dl2), _split16(x2))
+        dl1 = _col2im(C.linear(dl2, w2cat), Bc, L2, k2, F1, L1).mul_(a1.view(Bc, L1, F1) > 0).view(Bc * L1, F1)
+        d_b1 += dl1.sum(dim=0)
+        valid = (ch >= 0) & (ch < V)        # the kernel read an out-of-range id as character 0: so does its gradient
+        ids = (torch.where(valid, ch, torch.zeros_like(ch)).unfold(1, k1, 1) * k1 + taps).reshape(Bc * L1, k1)
+        d_t1 += native_embedding_bag_backward(dl1, ids, None, "sum", V * k1)
+    d_w1 = d_t1.view(V, k1, F1).permute(2, 0, 1).contiguous()
+    return d_w1, d_b1, d_w2.view(F2, F1, k2), d_b2, d_w3.view(D, F2, k3)
+
+
+class _CharCnnFn(torch.autograd.Function):
+    """out [B, D] fp32 from chars [B, L] and the five parameters; saves the ids and the [B, D] uint8 winning positions only."""
+
+    @staticmethod
+    def forward(ctx, chars, shape, prepared, status, w1, b1, w2, b2, w3):
+        from .embeddings import native_char_cnn
+
+        out, arg = native_char_cnn(chars, shape, prepared, want_arg=True, status=status)
+        ctx.save_for_backward(chars, arg, w2, w3)
+        ctx.shape, ctx.prepared = shape, prepared
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, d_out):
+        chars, arg, w2, w3 = ctx.saved_tensors
+        grads = _char_cnn_backward(d_out.contiguous().float(), chars, arg, ctx.prepared, ctx.shape, w2, w3)
+        return (None, None, None, None) + grads
+
+
+def char_cnn_with_grad(chars, shape, prepared, status, w1, b1, w2, b2, w3):
+    return _CharCnnFn.apply(N.require_cuda(chars, "chars", torch.int64), shape, prepared, status, w1, b1, w2, b2, w3)
+
+
+# =====================================================================================================================
 # GruCopyingDecoder (grucopydecoder.py:95-97, 122-124): the copy scores s[i, l] = c_i . o[graph(i), l] and their per-sample logsumexp
 # on the native kernel.  fp32 copy representations.
 # =====================================================================================================================

@@ -18,11 +18,16 @@ valid slots of a row in slot order in registers and writes the ``[B, D]`` result
 * An id outside ``[0, V)`` is read as row 0 and counted in a pinned status word that every call polls without synchronising: the
   ``IndexError`` is raised by the first call after the kernel ran.  Nothing in the forward synchronises, so it can be captured.
 
-Not supported (``NotImplementedError``): D > 512, more than 64 slots, gradients with a bf16 output, a dense output with D not a
-multiple of 4 (the native ``linear`` operator), and ``CharUnitEmbedder`` (stays the reference's).
+Not supported (``NotImplementedError``): D > 512, more than 64 slots, gradients with a bf16 output, and a dense output with D not a
+multiple of 4 (the native ``linear`` operator).
+
+``CharUnitEmbedder`` (strelementrepresentationmodel.py:100-142) runs its three convolutions and the max over positions as one native
+kernel, ``ptgnn_b200_char_cnn_forward`` (DESIGN.md §3.13): the one-hot input and the [B, F, L] conv outputs never exist.  Its derived
+weights (W1 as a gather table, W2 / W3 split and pre-swizzled) are kept per parameter version in eval mode, like the transformed table
+above.  Gradients (fp32) are ``autograd._CharCnnFn``: token chunks, each re-running the kernel in its "materialise" mode.
 """
 import math
-from typing import Optional, Tuple
+from typing import NamedTuple, Optional, Tuple
 
 import torch
 from torch import nn
@@ -57,9 +62,10 @@ def _bag_args(ids: torch.Tensor, lengths: Optional[torch.Tensor], D: int, mode: 
     return ids, lengths, B, S
 
 
-def new_status() -> torch.Tensor:
-    """A pinned int32 word for the kernels' count of out-of-range ids (polled by the host without synchronising)."""
-    return torch.zeros(1, dtype=torch.int32).pin_memory()
+def new_status(words: int = 1) -> torch.Tensor:
+    """A pinned int32 word for the kernels' count of out-of-range ids (polled by the host without synchronising); the char CNN uses a
+    second word for its fp16-range flag."""
+    return torch.zeros(words, dtype=torch.int32).pin_memory()
 
 
 def poll_status(status: torch.Tensor, vocab: int) -> None:
@@ -175,10 +181,12 @@ class _NativeEmbedder(nn.Module):
     deep-copied (the reference saves a model by pickling the whole module, abstractneuralmodel.py:155-163, and a restored tensor
     attribute would be pageable or device memory, not the pinned word the kernel and the synchronisation-free poll need)."""
 
+    _STATUS_WORDS = 1
+
     def __init__(self):
         super().__init__()
         self._status: Optional[torch.Tensor] = None
-        self._transformed = None        # eval mode: (key, table W^T)
+        self._transformed = None        # eval mode: (key, table W^T) or the char CNN's (key, prepared weights)
 
     def __getstate__(self):
         state = self.__dict__.copy()
@@ -191,12 +199,12 @@ class _NativeEmbedder(nn.Module):
         # the word is pinned when the module reaches the GPU, so that a first forward inside a CUDA-graph capture allocates nothing
         # on the host
         if self._status is None and any(p.is_cuda for p in self.parameters()):
-            self._status = new_status()
+            self._status = new_status(self._STATUS_WORDS)
         return out
 
     def _status_word(self) -> torch.Tensor:
         if self._status is None:        # built on the GPU directly, or restored from a pickle
-            self._status = new_status()
+            self._status = new_status(self._STATUS_WORDS)
         return self._status
 
 
@@ -284,3 +292,145 @@ class SubtokenUnitEmbedder(_NativeEmbedder):
             out = _linear(_bag(table, token_idxs, lengths, kind, torch.float32, status), weight).to(out_dtype)
         poll_status(status, V)
         return self.__dropout_layer(out)
+
+
+# ---------------------------------------------------------------------------------------------------------------------------------
+# CharUnitEmbedder
+# ---------------------------------------------------------------------------------------------------------------------------------
+class CnnConfig(NamedTuple):
+    """The reference's ``CnnConfig`` (strelementrepresentationmodel.py:92-97); any object with these five fields is accepted."""
+    l1_filters: int
+    l1_window_size: int
+    l2_filters: int
+    l2_window_size: int
+    lout_window_size: int
+
+
+def char_cnn_shape(conv1: nn.Conv1d, conv2: nn.Conv1d, conv3: nn.Conv1d) -> Tuple[int, int, int, int, int, int, int]:
+    """(C, F1, w1, F2, w2, D, w3) of the three convolutions."""
+    return (conv1.in_channels, conv1.out_channels, conv1.kernel_size[0], conv2.out_channels, conv2.kernel_size[0], conv3.out_channels,
+            conv3.kernel_size[0])
+
+
+def char_cnn_check(shape, L: int) -> None:
+    C, F1, w1, F2, w2, D, w3 = shape
+    if L < w1 + w2 + w3 - 2:
+        raise RuntimeError(f"CharUnitEmbedder: {L} characters per token are fewer than the {w1 + w2 + w3 - 2} the three windows need")
+    if not N.lib().ptgnn_b200_char_cnn_supported(C, F1, w1, F2, w2, D, w3, L):
+        raise NotImplementedError(f"the char CNN kernel takes l1 / l2 filters in {{64, 128, 256}}, windows in [1, 5], an embedding size in "
+                                  f"[1, 256] and up to 32 characters per token; got C={C}, F1={F1}, w1={w1}, F2={F2}, w2={w2}, D={D}, "
+                                  f"w3={w3}, L={L}")
+
+
+def char_cnn_prepare(shape, w1, b1, w2, b2, w3, bf16: bool, status: Optional[torch.Tensor]) -> torch.Tensor:
+    """``ptgnn_b200_char_cnn_prepare``: the derived weights (gather table, biases, split and pre-swizzled W2 / W3) as a uint8 tensor."""
+    lib = N.lib()
+    nbytes = lib.ptgnn_b200_char_cnn_workspace_bytes(int(bf16), *shape)
+    dev = w1.device
+    buf = torch.empty(nbytes + 1024, dtype=torch.uint8, device=dev)
+    off = (-buf.data_ptr()) % 1024
+    prepared = buf[off:off + nbytes]
+    ws = [N.require_cuda(t.detach(), name, torch.float32) for t, name in ((w1, "W1"), (b1, "b1"), (w2, "W2"), (b2, "b2"), (w3, "W3"))]
+    with torch.cuda.device(dev):
+        rc = lib.ptgnn_b200_char_cnn_prepare(int(bf16), *[N.ptr(t) for t in ws], *shape, N.ptr(prepared), nbytes, N.ptr(status),
+                                             N.current_stream(dev))
+    N.check(rc, "ptgnn_b200_char_cnn_prepare")
+    return prepared
+
+
+def native_char_cnn(chars: torch.Tensor, shape, prepared: torch.Tensor, bf16: bool = False, want_arg: bool = False,
+                    status: Optional[torch.Tensor] = None):
+    """``ptgnn_b200_char_cnn_forward``: out [B, D] (fp32, or bf16 with ``bf16``) from chars [B, L] int64 and ``char_cnn_prepare``d
+    weights of the same ``bf16`` flag.  ``want_arg``: also the [B, D] uint8 winning positions."""
+    chars = N.require_cuda(chars, "chars", torch.int64)
+    if chars.dim() != 2:
+        raise ValueError(f"chars must be [B, max_num_chars], got {tuple(chars.shape)}")
+    B, L = chars.shape
+    char_cnn_check(shape, L)
+    D = shape[5]
+    out = torch.empty(B, D, dtype=torch.bfloat16 if bf16 else torch.float32, device=chars.device)
+    arg = torch.empty(B, D, dtype=torch.uint8, device=chars.device) if want_arg else None
+    if B:
+        with torch.cuda.device(chars.device):
+            rc = N.lib().ptgnn_b200_char_cnn_forward(int(bf16), N.ptr(chars), B, L, *shape, N.ptr(prepared), prepared.numel(), N.ptr(out),
+                                                     N.ptr(arg), N.ptr(status), N.current_stream(chars.device))
+        N.check(rc, "ptgnn_b200_char_cnn_forward")
+    return (out, arg) if want_arg else out
+
+
+def native_char_cnn_materialise(chars: torch.Tensor, shape, prepared: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """``ptgnn_b200_char_cnn_materialise_f32``: the post-ReLU a1 [B (L - w1 + 1), F1] and a2 [B (L - w1 - w2 + 2), F2] of fp32
+    ``prepared`` weights."""
+    B, L = chars.shape
+    C, F1, w1, F2, w2, D, w3 = shape
+    L1, L2 = L - w1 + 1, L - w1 - w2 + 2
+    a1 = torch.empty(B * L1, F1, dtype=torch.float32, device=chars.device)
+    a2 = torch.empty(B * L2, F2, dtype=torch.float32, device=chars.device)
+    if B:
+        with torch.cuda.device(chars.device):
+            rc = N.lib().ptgnn_b200_char_cnn_materialise_f32(N.ptr(chars), B, L, *shape, N.ptr(prepared), prepared.numel(), N.ptr(a1), N.ptr(a2),
+                                                             None, N.current_stream(chars.device))
+        N.check(rc, "ptgnn_b200_char_cnn_materialise_f32")
+    return a1, a2
+
+
+def poll_char_status(status: torch.Tensor, vocab: int) -> None:
+    poll_status(status, vocab)
+    if int(status[1]):
+        status[1] = 0
+        raise FloatingPointError("CharUnitEmbedder: an fp32 weight or activation is outside the fp16 range (|x| >= 65504) of the "
+                                 "kernel's split products; results are not valid")
+
+
+class CharUnitEmbedder(_NativeEmbedder):
+    _STATUS_WORDS = 2
+
+    def __init__(self, num_chars: int, embedding_size: int, config: CnnConfig, dropout_rate: float = 0.0):
+        super().__init__()
+        self.__num_chars_in_vocabulary = num_chars
+        self.__conv_l1 = nn.Conv1d(in_channels=num_chars, out_channels=config.l1_filters, kernel_size=config.l1_window_size)
+        self.__conv_l2 = nn.Conv1d(in_channels=config.l1_filters, out_channels=config.l2_filters, kernel_size=config.l2_window_size)
+        self.__conv_l3 = nn.Conv1d(in_channels=config.l2_filters, out_channels=embedding_size, kernel_size=config.lout_window_size,
+                                   bias=False)
+        self.__dropout = nn.Dropout(p=dropout_rate)
+
+    def _params(self):
+        return (self.__conv_l1.weight, self.__conv_l1.bias, self.__conv_l2.weight, self.__conv_l2.bias, self.__conv_l3.weight)
+
+    def _prepared(self, shape, bf16: bool, status: torch.Tensor) -> torch.Tensor:
+        """The derived weights.  Kept in eval mode while no parameter was modified in place, re-assigned or moved; derived on every
+        call in training mode (edits through ``.data`` do not move the version counter)."""
+        params = self._params()
+        if self.training:
+            return char_cnn_prepare(shape, *params, bf16, status)
+        key = (bf16,) + tuple((p.data_ptr(), p._version, p.device, p.dtype) for p in params)
+        if self._transformed is None or self._transformed[0] != key:
+            self._transformed = (key, char_cnn_prepare(shape, *params, bf16, status))
+        return self._transformed[1]
+
+    def forward(self, chars: torch.Tensor) -> torch.Tensor:
+        """
+        :param chars: [B, max_num_chars] int64
+        :return: [B, D] (fp32; bf16 under ``torch.autocast("cuda", bfloat16)``)
+        """
+        params = self._params()
+        N.require_cuda(params[0], "conv_l1 weight", torch.float32)
+        if chars.dim() != 2:
+            raise ValueError(f"chars must be [B, max_num_chars], got {tuple(chars.shape)}")
+        shape = char_cnn_shape(self.__conv_l1, self.__conv_l2, self.__conv_l3)
+        char_cnn_check(shape, chars.shape[1])
+        bf16 = _bf16_autocast(params[0].device)
+        grad = _wants_grad(*params)
+        if bf16 and grad:
+            raise NotImplementedError("CharUnitEmbedder: gradients with a bf16 output have no native kernel; train in fp32")
+        status = self._status_word()
+        poll_char_status(status, self.__num_chars_in_vocabulary)
+        prepared = self._prepared(shape, bf16, status)
+        if grad:
+            from . import autograd as _ag
+
+            out = _ag.char_cnn_with_grad(chars, shape, prepared, status, *params)
+        else:
+            out = native_char_cnn(chars, shape, prepared, bf16, status=status)
+        poll_char_status(status, self.__num_chars_in_vocabulary)
+        return self.__dropout(out)

@@ -34,7 +34,10 @@ factories import the layer classes by module path (`implementations/typilus/trai
    ``ptgnn.neuralmodels.embeddings.strelementrepresentationmodel`` and in reference modules imported earlier (the native
    embedding-bag kernels, DESIGN.md §3.12), so that ``StrElementRepresentationModel.build_neural_module`` builds the native classes for
    ``"token"``, ``"subtoken"`` and ``"bpe"``.  The module stays the reference's: it also holds ``StrElementRepresentationModel``,
-   ``CnnConfig`` and ``CharUnitEmbedder``, which ``"char"`` still builds.  The default leaves the reference's classes in place.
+   ``CnnConfig`` and ``CharUnitEmbedder``, which ``"char"`` still builds.  The default leaves the reference's classes in place,
+11. with ``native_char_embedder=True`` only: re-binds ``CharUnitEmbedder`` inside the same module and in reference modules imported
+   earlier (the native character-CNN kernel, DESIGN.md §3.13), so that ``"char"`` (VarMisuse's ``CandidateNodeAnnotationModel``) builds
+   the native class.  ``native_embedders=True`` alone leaves the reference's ``CharUnitEmbedder`` in place.
 
 After ``install()``: ``import ptgnn.implementations.ppi.train`` etc. build ptgnn_b200 layers, unchanged.  ``uninstall()``
 restores the reference's classes.  The reference must be importable as ``ptgnn`` for steps 2-4 (it is not on the GPU test box;
@@ -66,6 +69,7 @@ _PNA_CLASS = "PnaMessageAggregation"
 _DECODER_MODULE = "ptgnn.neuralmodels.sequence.grucopydecoder"
 _EMBEDDER_MODULE = "ptgnn.neuralmodels.embeddings.strelementrepresentationmodel"
 _NATIVE_EMBEDDERS = ("TokenUnitEmbedder", "SubtokenUnitEmbedder")
+_NATIVE_CHAR_EMBEDDER = "CharUnitEmbedder"
 _saved: Dict[str, object] = {}
 
 
@@ -159,19 +163,20 @@ def _install_native_decoder() -> None:
         _rebind_everywhere({old: _dec.GruCopyingDecoder})      # the decoder module included
 
 
-def _install_native_embedders() -> None:
+def _install_native_embedders(names=_NATIVE_EMBEDDERS) -> None:
     from . import embeddings as _emb
 
     mod = importlib.import_module(_EMBEDDER_MODULE)
-    replaced = {getattr(mod, n): getattr(_emb, n) for n in _NATIVE_EMBEDDERS if getattr(mod, n) is not getattr(_emb, n)}
+    replaced = {getattr(mod, n): getattr(_emb, n) for n in names if getattr(mod, n) is not getattr(_emb, n)}
     _rebind_everywhere(replaced)       # the embedder module included
 
 
 def install(force_torch_scatter: bool = False, native_reducers: bool = False, native_selfattention: bool = False,
             native_graphnorm: bool = False, native_pna: bool = False, native_decoder: bool = False,
-            native_embedders: bool = False) -> Dict[str, object]:
+            native_embedders: bool = False, native_char_embedder: bool = False) -> Dict[str, object]:
     report: Dict[str, object] = {"torch_scatter": "real", "layers": False, "container": False, "metrics": False, "reducers": False,
-                                 "selfattention": False, "graphnorm": False, "pna": False, "decoder": False, "embedders": False}
+                                 "selfattention": False, "graphnorm": False, "pna": False, "decoder": False, "embedders": False,
+                                 "char_embedder": False}
     # 1. torch_scatter
     have_real = False
     if not force_torch_scatter:
@@ -236,6 +241,10 @@ def install(force_torch_scatter: bool = False, native_reducers: bool = False, na
     if native_embedders:
         _install_native_embedders()
         report["embedders"] = True
+    # 11. CharUnitEmbedder (opt-in)
+    if native_char_embedder:
+        _install_native_embedders((_NATIVE_CHAR_EMBEDDER,))
+        report["char_embedder"] = True
     return report
 
 
