@@ -257,6 +257,26 @@ int ptgnn_b200_mlp_forward_fused(int32_t bf16_states, const void *node_states, c
                                  int32_t dense_activation, void *out_states, void *workspace, size_t workspace_bytes,
                                  void *weight_cache, size_t weight_cache_bytes, int32_t cache_valid, void *stream);
 
+/* EGCMessagePassingLayer.forward (egcmessagepassing.py:54-91, eval mode) through the fused kernel:
+ *   out[n, o] = sum_b w[n, hd * bases + b] * reduce_{e -> n} (bases_t(e) h_src(e))[(hd * bases + b) * dh + c],  o = hd * dh + c,
+ *   w = h weight_coeffs^T + bias,  dh = out_dim / num_heads.
+ * bases_weights: [host] T device pointers to the reference's bases[t].weight [num_bases * out_dim, in_dim] fp32, in its row order;
+ * coeff_weight [num_heads * num_bases, in_dim] and coeff_bias fp32.  The message features are cut into num_bases * out_dim / 128 slabs
+ * of 128, each one fused-aggregation launch whose write-out sums the bases of its output columns: no [E, num_bases * out_dim] message
+ * tensor.  bf16 states give bf16 output, rounded where autocast rounds.  Supported (ptgnn_b200_egc_supported): the fused kernel's
+ * in_dim, num_bases in {1, 2, 4, 8}, out_dim a multiple of num_heads and of 128 / num_bases.  weight_cache (optional)
+ * [>= ptgnn_b200_egc_fused_weight_cache_bytes] holds the packed slabs; cache_valid = 1 reuses them.  Never synchronises. */
+int32_t ptgnn_b200_egc_supported(int32_t bf16_states, int32_t in_dim, int32_t out_dim, int32_t num_heads, int32_t num_bases);
+size_t ptgnn_b200_egc_fused_workspace_bytes(int32_t bf16_states, int64_t num_nodes, int32_t num_types, int32_t in_dim, int32_t out_dim,
+                                            int32_t num_heads, int32_t num_bases);
+size_t ptgnn_b200_egc_fused_weight_cache_bytes(int32_t bf16_states, int32_t num_types, int32_t in_dim, int32_t out_dim, int32_t num_heads,
+                                               int32_t num_bases);
+int ptgnn_b200_egc_forward_fused(int32_t bf16_states, const void *node_states, int64_t num_nodes, int32_t in_dim, int32_t out_dim,
+                                 int32_t num_heads, int32_t num_bases, int32_t num_types, const ptgnn_b200_block_plan *block_plan,
+                                 const int32_t *row_ptr, const float *const *bases_weights, const float *coeff_weight,
+                                 const float *coeff_bias, int32_t reduce, void *out_states, void *workspace, size_t workspace_bytes,
+                                 void *weight_cache, size_t weight_cache_bytes, int32_t cache_valid, void *stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Backward support (SURVEY.md section 8 row f-1; host side: ptgnn_b200/autograd.py).  The pointwise half of the GRUCell backward
  * (torch.nn.GRUCell, gatedmessagepassing.py:69): gi / gh [N, 3H] = gate pre-activations (order r, z, n), h [N, H] the previous

@@ -57,6 +57,12 @@ SIGNATURES = {
     "ptgnn_b200_mlp_forward_fused": (ctypes.c_int, [c_i32, c_void_p, c_void_p, c_i64, c_i64, c_i32, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p,
                                                     c_i32, c_i32, c_i32, c_void_p, c_void_p, c_f32, c_void_p, c_void_p, c_i32, c_void_p, c_void_p,
                                                     c_size_t, c_void_p, c_size_t, c_i32, c_void_p]),
+    "ptgnn_b200_egc_supported": (c_i32, [c_i32] * 5),
+    "ptgnn_b200_egc_fused_workspace_bytes": (c_size_t, [c_i32, c_i64] + [c_i32] * 5),
+    "ptgnn_b200_egc_fused_weight_cache_bytes": (c_size_t, [c_i32] * 6),
+    "ptgnn_b200_egc_forward_fused": (ctypes.c_int, [c_i32, c_void_p, c_i64] + [c_i32] * 5 + [c_void_p] * 5 + [c_i32, c_void_p, c_void_p,
+                                                                                                            c_size_t, c_void_p, c_size_t,
+                                                                                                            c_i32, c_void_p]),
     "ptgnn_b200_gather_split_f16": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_void_p, c_void_p]),
     "ptgnn_b200_gru_gate_grads_f32": (ctypes.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_void_p, c_void_p]),
     "ptgnn_b200_offset_ids": (ctypes.c_int, [c_void_p, c_i64, c_void_p, c_void_p, c_i32, c_void_p, c_void_p]),

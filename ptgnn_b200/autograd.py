@@ -173,45 +173,137 @@ class _GatedLayerFunction(torch.autograd.Function):
         d_agg, d_h, d_w_ih, d_w_hh, d_b_ih, d_b_hh = _gru_backward(g, agg, h, w_ih, w_hh, b_ih.detach(), b_hh.detach())
 
         # ---- 3. aggregation + per-type Linear backward
-        d_W = []
-        if reduce_name in ("sum", "mean"):
-            if reduce_name == "mean":
-                cnt = (plan.row_ptr[1:] - plan.row_ptr[:-1]).clamp(min=1).to(torch.float32)
-                d_agg = d_agg / cnt[:, None]
-            with _exact_fp16_gemms():
-                a_all = _split16(d_agg, True, plan.tgt32)                    # [E, D] rows of d_agg, cat(types) order
-                b_all = _split16(h, False, plan.src32)                       # [E, H] source states
-                for t, w in enumerate(W):
-                    lo_, hi_ = plan.type_off[t], plan.type_off[t + 1]
-                    d_W.append(_mm_t_split(_slice(a_all, lo_, hi_), _slice(b_all, lo_, hi_)) if hi_ > lo_ else torch.zeros_like(w))
-            if E > 0:
-                # d h_src[u] = sum over edges (u -> v, type t) of W_t^T d_agg[v]: the forward's aggregation on the transposed graph
-                rev = [(tgt, src) for src, tgt in adj]
-                rplan = plan_for(rev, num_nodes)
-                d_h = d_h + C.aggregate(rplan, d_agg.contiguous(), [w.t().contiguous() for w in W], N.REDUCE["sum"])
-        else:
-            D = d_agg.shape[1]
-            d_msg = torch.zeros(E + 1, D, dtype=torch.float32, device=h.device)      # row E takes the empty targets' sentinel
-            d_msg.scatter_(0, arg, d_agg)                                            # each (edge, feature) has one target: no collisions
-            with _exact_fp16_gemms():
-                a_all = _split16(d_msg[:E])
-                b_all = _split16(h, False, plan.src32)
-            lo = 0
-            for (src, tgt), w in zip(adj, W):
-                e_t = src.numel()
-                part = d_msg[lo:lo + e_t]
-                lo += e_t
-                if e_t == 0:
-                    d_W.append(torch.zeros_like(w))
-                    continue
-                with _exact_fp16_gemms():
-                    d_W.append(_mm_t_split(_slice(a_all, lo - e_t, lo), _slice(b_all, lo - e_t, lo)))
-                d_h = d_h + scatter_sum(C.linear(part.contiguous(), w.t().contiguous()), src, dim=0, dim_size=num_nodes)
+        d_W, d_h = _aggregation_backward(plan, adj, h, W, d_agg, reduce_name, arg, d_h)
         return (None, None, None, d_h, d_w_ih, d_w_hh, d_b_ih, d_b_hh, *d_W)
+
+
+def _aggregation_backward(plan, adj, h, W, d_agg, reduce_name, arg, d_h, b_all=None):
+    """Backward of agg = reduce_{e -> v} W_t(e) h[src(e)] (bias-free per-type Linear, then sum / mean / max / min) from d_agg [N, D]:
+    returns (d_W per type, d_h + the h part).  arg: the winning edge ids of max / min ([N, D], E for empty targets).  b_all: the
+    3xFP16 split of the gathered source states, ``_split16(h, False, plan.src32)``, when the caller reuses it across calls.
+    sum / mean: split fp16 GEMMs over edges, and the forward's aggregation on the transposed graph with W_t^T; max / min: the message
+    gradients routed to the winning edges, the split GEMMs, and the native scatter-add by source."""
+    num_nodes = h.shape[0]
+    E = plan.num_edges
+    d_W = []
+    if reduce_name in ("sum", "mean"):
+        if reduce_name == "mean":
+            cnt = (plan.row_ptr[1:] - plan.row_ptr[:-1]).clamp(min=1).to(torch.float32)
+            d_agg = d_agg / cnt[:, None]
+        with _exact_fp16_gemms():
+            a_all = _split16(d_agg, True, plan.tgt32)                    # [E, D] rows of d_agg, cat(types) order
+            if b_all is None:
+                b_all = _split16(h, False, plan.src32)                   # [E, H] source states
+            for t, w in enumerate(W):
+                lo_, hi_ = plan.type_off[t], plan.type_off[t + 1]
+                d_W.append(_mm_t_split(_slice(a_all, lo_, hi_), _slice(b_all, lo_, hi_)) if hi_ > lo_ else torch.zeros_like(w))
+        if E > 0:
+            # d h_src[u] = sum over edges (u -> v, type t) of W_t^T d_agg[v]: the forward's aggregation on the transposed graph
+            rev = [(tgt, src) for src, tgt in adj]
+            rplan = plan_for(rev, num_nodes)
+            d_h = d_h + C.aggregate(rplan, d_agg.contiguous(), [w.t().contiguous() for w in W], N.REDUCE["sum"])
+    else:
+        D = d_agg.shape[1]
+        d_msg = torch.zeros(E + 1, D, dtype=torch.float32, device=h.device)      # row E takes the empty targets' sentinel
+        d_msg.scatter_(0, arg, d_agg)                                            # each (edge, feature) has one target: no collisions
+        with _exact_fp16_gemms():
+            a_all = _split16(d_msg[:E])
+            if b_all is None:
+                b_all = _split16(h, False, plan.src32)
+        lo = 0
+        for (src, tgt), w in zip(adj, W):
+            e_t = src.numel()
+            part = d_msg[lo:lo + e_t]
+            lo += e_t
+            if e_t == 0:
+                d_W.append(torch.zeros_like(w))
+                continue
+            with _exact_fp16_gemms():
+                d_W.append(_mm_t_split(_slice(a_all, lo - e_t, lo), _slice(b_all, lo - e_t, lo)))
+            d_h = d_h + scatter_sum(C.linear(part.contiguous(), w.t().contiguous()), src, dim=0, dim_size=num_nodes)
+    return d_W, d_h
 
 
 def gated_forward_with_grad(layer, node_states, adjacency_lists, reduce_name, w_ih, w_hh, b_ih, b_hh, weights):
     return _GatedLayerFunction.apply(layer, adjacency_lists, reduce_name, node_states, w_ih, w_hh, b_ih, b_hh, *weights)
+
+
+# =====================================================================================================================
+# EGCMessagePassingLayer (egcmessagepassing.py:54-91) on its fused slabs (DESIGN.md §3.14):
+#   out[n, o] = sum_b w[n, hd bases + b] A[n, r(o, b)],  w = h Wc^T + bc,  A = reduce_{e -> n} W_t(e) h[src(e)],  r(o, b) = (hd bases + b) dh + c
+# =====================================================================================================================
+def egc_slab_rows(s: int, out: int, heads: int, bases: int, device) -> torch.Tensor:
+    """Reference rows of bases[t].weight in slab s: position p = j bases + b <- row r(o, b), o = s 128 / bases + j."""
+    p = torch.arange(128, device=device)
+    o = s * (128 // bases) + p // bases
+    dh = out // heads
+    return ((o // dh) * bases + p % bases) * dh + o % dh
+
+
+class _EgcLayerFunction(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, layer, adjacency_lists, reduce_name, dims, h, coeff_weight, coeff_bias, *weights):
+        with torch.no_grad():
+            out = layer(h.detach(), adjacency_lists)
+        ctx.save_for_backward(h, coeff_weight, coeff_bias, *weights)
+        ctx.adjacency_lists, ctx.reduce_name, ctx.dims = adjacency_lists, reduce_name, dims
+        return out
+
+    @staticmethod
+    @once_differentiable          # the backward runs native kernels: no double backward
+    def backward(ctx, grad_out):
+        h, cw, cb, *weights = (t.detach() for t in ctx.saved_tensors)
+        adj = ctx.adjacency_lists
+        reduce_name = ctx.reduce_name
+        _in_dim, out, heads, bases = ctx.dims
+        g = grad_out.contiguous().float()
+        h, cw = h.contiguous(), cw.contiguous()
+        W = [w.contiguous() for w in weights]
+        num_nodes = h.shape[0]
+        plan = plan_for(adj, num_nodes)
+        per, dh = 128 // bases, out // heads
+
+        # 1. the coefficients, on the native dense kernel as in the forward
+        w = C.linear(h, cw, cb).view(num_nodes, heads, bases)
+        prod = torch.empty(num_nodes, out, bases, dtype=torch.float32, device=h.device)       # G[n, o] A[n, r(o, b)], node-sized
+        d_h = torch.zeros_like(h)
+        d_slabs = [[] for _ in W]
+        with _exact_fp16_gemms():
+            b_all = _split16(h, False, plan.src32)                       # the gathered source states, once for every slab
+        for s in range(bases * out // 128):
+            rows = egc_slab_rows(s, out, heads, bases, h.device)
+            Ws = [wt.index_select(0, rows) for wt in W]                 # [128, H]: the slab's rows, in slab order
+            # 2. the slab's aggregate A_s [N, 128] (and, for max / min, which edge won each (target, feature))
+            arg = None
+            if reduce_name in ("max", "min"):
+                msg = C.edge_messages(plan, h, None, Ws, False)
+                agg, arg = C.segment_reduce(msg, plan, N.REDUCE[reduce_name], return_arg=True)
+                del msg
+            else:
+                agg = C.aggregate(plan, h, Ws, N.REDUCE[reduce_name])
+            # 3. node-side terms: the slab's columns o = s per + j, their heads and coefficient rows
+            cols = slice(s * per, (s + 1) * per)
+            hd = torch.arange(s * per, (s + 1) * per, device=h.device) // dh
+            g_s = g[:, cols].unsqueeze(-1)                                       # [N, per, 1]
+            prod[:, cols] = g_s * agg.view(num_nodes, per, bases)
+            d_agg = (w.index_select(1, hd) * g_s).reshape(num_nodes, 128)        # dA_s[n, j bases + b] = w[n, hd(j), b] G[n, o]
+            # 4. the slab's weight gradients and its part of d h
+            d_Ws, d_h = _aggregation_backward(plan, adj, h, Ws, d_agg, reduce_name, arg, d_h, b_all)
+            for t, d in enumerate(d_Ws):
+                d_slabs[t].append(d)
+        # 5. slab order -> the reference's row order
+        inv = torch.argsort(torch.cat([egc_slab_rows(s, out, heads, bases, h.device) for s in range(bases * out // 128)]))
+        d_W = [torch.cat(ds, dim=0).index_select(0, inv) for ds in d_slabs]
+        # 6. the coefficient Linear
+        d_w = prod.view(num_nodes, heads, dh, bases).sum(dim=2).reshape(num_nodes, heads * bases)
+        with _exact_fp16_gemms():
+            d_cw = _mm_t_split(_split16(d_w), _split16(h, False))
+        d_h = d_h + C.linear(d_w.contiguous(), cw.t().contiguous())
+        return (None, None, None, None, d_h, d_cw, d_w.sum(dim=0), *d_W)
+
+
+def egc_forward_with_grad(layer, node_states, adjacency_lists, reduce_name, coeff_weight, coeff_bias, weights):
+    return _EgcLayerFunction.apply(layer, adjacency_lists, reduce_name, layer._dims, node_states, coeff_weight, coeff_bias, *weights)
 
 
 # =====================================================================================================================

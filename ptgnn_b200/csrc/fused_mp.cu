@@ -66,7 +66,11 @@ struct Params {
     int32_t *status;
     unsigned long long *trace;     // debug (PTGNN_FUSED_TRACE=1): per-role event timeline of CTA 0, else nullptr
     Epilogue epi;
+    EgcEpilogue egc;               // read by the EPI_EGC instances only
 };
+// the write-out, fixed at compile time so that each instance carries only its own: the aggregate (+ mean / activation / LayerNorm)
+// or the EGC combination of the bases
+constexpr int EPI_AGG = 0, EPI_EGC = 1;
 
 // ---- small PTX helpers ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint4 ldg_nc_u4(const uint4 *p) {
@@ -281,7 +285,84 @@ __device__ __forceinline__ void write_out_block(const Params *p, uint32_t agg_sa
     else { if (plain) write_rows(integral_constant<int, 0>{}, integral_constant<bool, true>{}); else write_rows(integral_constant<int, 0>{}, integral_constant<bool, false>{}); }
 }
 
-template <int NPROD, int K, int NSEG, int RED>
+__device__ __forceinline__ float bf16r(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
+
+// EGC write-out of a finished block (EgcEpilogue): the same row walk as write_out_block.  Lane q's float4 holds slab features 4 q ..
+// 4 q + 3, i.e. bases (4 q) % bases .. of output column(s) col0 + 4 q / bases: bases = 4 -> one column per lane, 8 -> a lane pair
+// (the even lane's partial sum goes to the odd lane with one shuffle, which adds its own four products to it: base order), 2 -> two
+// columns, 1 -> four.  After the mean division / empty-target fix, each column is sum_b w_b A_b: fp32 states -- products rounded to
+// fp32 and added in base order; bf16 states (out_mode 1) -- A rounded to bf16 (the reference's aggregate is cast back to the message
+// dtype), each product rounded to bf16, the sum in fp32 rounded once (autocast's elementwise product and fp32-accumulated sum).
+// Explicit _rn operations: no multiply-add contraction.
+template <int RED>
+__device__ __forceinline__ void write_out_block_egc(const Params *p, uint32_t agg_saddr, int row0, int r_first, int r_step, int q) {
+    const float IDENT = red_identity<RED>();
+    const int my_hi = min(p->B, p->num_nodes - row0);
+    const float4 ident4 = make_float4(IDENT, IDENT, IDENT, IDENT);
+    const EgcEpilogue &e = p->egc;
+    const bool bf = p->out_mode == 1;
+    for (int r = r_first; r < my_hi; r += r_step) {
+        const uint32_t rowa = agg_saddr + (uint32_t)(r * kD + q * 4) * 4u;
+        const float4 a4 = lds_f32x4(rowa);
+        sts_f32x4(rowa, ident4);
+        const int v = row0 + r;
+        float x[4] = {a4.x, a4.y, a4.z, a4.w};
+        float cdiv = 1.0f;
+        if (RED == PTGNN_REDUCE_MEAN) {
+            const int cnt = __ldg(p->row_ptr + v + 1) - __ldg(p->row_ptr + v);
+            cdiv = (float)(cnt < 1 ? 1 : cnt);
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            if (RED == PTGNN_REDUCE_MEAN) x[i] /= cdiv;
+            if ((RED == PTGNN_REDUCE_MAX || RED == PTGNN_REDUCE_MIN) && x[i] == IDENT) x[i] = 0.0f;
+            if (bf) x[i] = bf16r(x[i]);
+        }
+        const float *crow = e.coef + (size_t)v * e.coef_stride;
+        auto prod = [&](float A, float w) { const float t = __fmul_rn(A, w); return bf ? bf16r(t) : t; };
+        const size_t orow = (size_t)v * e.out_stride;
+        auto store1 = [&](int o, float s) {
+            if (bf) reinterpret_cast<__nv_bfloat16 *>(p->out)[orow + o] = __float2bfloat16_rn(s);
+            else reinterpret_cast<float *>(p->out)[orow + o] = s;
+        };
+        if (e.bases == 4 || e.bases == 8) {
+            const int o = e.col0 + (e.bases == 4 ? q : q >> 1);
+            const int b0 = e.bases == 4 ? 0 : 4 * (q & 1);
+            const float4 w = *reinterpret_cast<const float4 *>(crow + (o / e.dh) * e.bases + b0);
+            const float p0 = prod(x[0], w.x), p1 = prod(x[1], w.y), p2 = prod(x[2], w.z), p3 = prod(x[3], w.w);
+            float s = __fadd_rn(__fadd_rn(__fadd_rn(p0, p1), p2), p3);
+            if (e.bases == 8) {
+                const float lower = __shfl_xor_sync(0xffffffffu, s, 1);        // the even lane's bases 0 .. 3
+                s = __fadd_rn(__fadd_rn(__fadd_rn(__fadd_rn(lower, p0), p1), p2), p3);
+                if ((q & 1) == 0) continue;
+            }
+            store1(o, s);
+        } else if (e.bases == 2) {
+            const int o = e.col0 + 2 * q;
+            const float2 w0 = *reinterpret_cast<const float2 *>(crow + (o / e.dh) * 2);
+            const float2 w1 = *reinterpret_cast<const float2 *>(crow + ((o + 1) / e.dh) * 2);
+            const float s0 = __fadd_rn(prod(x[0], w0.x), prod(x[1], w0.y));
+            const float s1 = __fadd_rn(prod(x[2], w1.x), prod(x[3], w1.y));
+            if (bf) *reinterpret_cast<__nv_bfloat162 *>(reinterpret_cast<__nv_bfloat16 *>(p->out) + orow + o) = __floats2bfloat162_rn(s0, s1);
+            else *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p->out) + orow + o) = make_float2(s0, s1);
+        } else {
+            const int o = e.col0 + 4 * q;
+            float s[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) s[i] = prod(x[i], __ldg(crow + (o + i) / e.dh));
+            if (bf) {
+                __nv_bfloat162 lo = __floats2bfloat162_rn(s[0], s[1]), hi = __floats2bfloat162_rn(s[2], s[3]);
+                uint2 pk;
+                pk.x = *reinterpret_cast<uint32_t *>(&lo); pk.y = *reinterpret_cast<uint32_t *>(&hi);
+                *reinterpret_cast<uint2 *>(reinterpret_cast<__nv_bfloat16 *>(p->out) + orow + o) = pk;
+            } else {
+                *reinterpret_cast<float4 *>(reinterpret_cast<float *>(p->out) + orow + o) = make_float4(s[0], s[1], s[2], s[3]);
+            }
+        }
+    }
+}
+
+template <int NPROD, int K, int NSEG, int RED, int EPI>
 __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const __grid_constant__ Params p) {
     constexpr int NPART = NPROD == 3 ? 2 : 1;                      // hi | lo' parts of a row / of the weights
     constexpr int ROW_BYTES = K * 2 * NPART;                       // one packed state row
@@ -346,7 +427,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
                 // write-out's resets precede the next block's walk
                 trace_mark(p, 33, sg);
                 named_bar_sync(RED_BAR_ID, 128);
-                write_out_block<RED>(&p, smem_u32(agg_s), s.blk * p.B, rw, 4, lane);
+                if constexpr (EPI == EPI_EGC) write_out_block_egc<RED>(&p, smem_u32(agg_s), s.blk * p.B, rw, 4, lane);
+                else write_out_block<RED>(&p, smem_u32(agg_s), s.blk * p.B, rw, 4, lane);
                 named_bar_sync(RED_BAR_ID, 128);
                 trace_mark(p, 34, sg);
                 continue;
@@ -689,7 +771,7 @@ struct WeightSrc {
 // out[(((t * nseg + seg) * npart + part) * (K / 8) + c4) * 128 + d] = 8 elements k = seg K + 8 c4 .. + 7 of row d
 template <int NPROD>
 __global__ void __launch_bounds__(256) pack_weights_kernel(const __grid_constant__ WeightSrc src, int num_types, int K, int nseg,
-                                                           uint4 *__restrict__ out, int32_t *__restrict__ status) {
+                                                           RowMap rows, uint4 *__restrict__ out, int32_t *__restrict__ status) {
     constexpr int NPART = NPROD == 3 ? 2 : 1;
     const int per_mat = nseg * (K / 8) * 128;             // (seg, c4, d) triples per type
     const long long total = (long long)num_types * per_mat;
@@ -700,7 +782,12 @@ __global__ void __launch_bounds__(256) pack_weights_kernel(const __grid_constant
         const int seg = r / ((K / 8) * 128);
         r -= seg * (K / 8) * 128;
         const int c4 = r / 128, d = r % 128;
-        const float *row = src.w[t] + (size_t)d * (nseg * K) + seg * K + c4 * 8;
+        int srow = d;
+        if (rows.bases > 0) {
+            const int o = rows.col0 + d / rows.bases, b = d % rows.bases;
+            srow = ((o / rows.dh) * rows.bases + b) * rows.dh + o % rows.dh;
+        }
+        const float *row = src.w[t] + (size_t)srow * (nseg * K) + seg * K + c4 * 8;
         float x[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) x[j] = row[j];
@@ -755,14 +842,14 @@ int recommended_block_targets(int64_t num_nodes) {
 }
 
 int pack_weights(int nprod, int num_types, int K, int use_target, const float *const *weights, void *packed, int32_t *status,
-                 cudaStream_t st) {
+                 cudaStream_t st, RowMap rows) {
     WeightSrc src{};
     for (int t = 0; t < num_types; ++t) src.w[t] = weights[t];
     const int nseg = use_target ? 2 : 1;
     {
         TimedScope timed__(PTGNN_KERNEL_PACK, st);
-        if (nprod == 3) pack_weights_kernel<3><<<132, 256, 0, st>>>(src, num_types, K, nseg, static_cast<uint4 *>(packed), status);
-        else pack_weights_kernel<1><<<132, 256, 0, st>>>(src, num_types, K, nseg, static_cast<uint4 *>(packed), status);
+        if (nprod == 3) pack_weights_kernel<3><<<132, 256, 0, st>>>(src, num_types, K, nseg, rows, static_cast<uint4 *>(packed), status);
+        else pack_weights_kernel<1><<<132, 256, 0, st>>>(src, num_types, K, nseg, rows, static_cast<uint4 *>(packed), status);
     }
     PTGNN_LAUNCHED();
     return PTGNN_OK;
@@ -780,9 +867,9 @@ int pack_states(const float *h, int64_t rows, int K, void *packed, int32_t *stat
     return PTGNN_OK;
 }
 
-template <int NPROD, int K, int NSEG, int RED>
+template <int NPROD, int K, int NSEG, int RED, int EPI = EPI_AGG>
 static int launch_one(const Params &p, cudaStream_t st) {
-    auto kernel = fused_aggregate_kernel<NPROD, K, NSEG, RED>;
+    auto kernel = fused_aggregate_kernel<NPROD, K, NSEG, RED, EPI>;
     const int smem = smem_bytes(p.B);
     // per launch, not once per process: the attribute belongs to the current device's context
     PTGNN_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
@@ -795,17 +882,18 @@ static int launch_one(const Params &p, cudaStream_t st) {
     PTGNN_LAUNCHED();
     return PTGNN_OK;
 }
-template <int NPROD, int K, int NSEG>
+template <int NPROD, int K, int NSEG, int EPI = EPI_AGG>
 static int launch_red(const Params &p, cudaStream_t st) {
     switch (p.reduce) {
-        case PTGNN_REDUCE_SUM: return launch_one<NPROD, K, NSEG, PTGNN_REDUCE_SUM>(p, st);
-        case PTGNN_REDUCE_MEAN: return launch_one<NPROD, K, NSEG, PTGNN_REDUCE_MEAN>(p, st);
-        case PTGNN_REDUCE_MAX: return launch_one<NPROD, K, NSEG, PTGNN_REDUCE_MAX>(p, st);
-        default: return launch_one<NPROD, K, NSEG, PTGNN_REDUCE_MIN>(p, st);
+        case PTGNN_REDUCE_SUM: return launch_one<NPROD, K, NSEG, PTGNN_REDUCE_SUM, EPI>(p, st);
+        case PTGNN_REDUCE_MEAN: return launch_one<NPROD, K, NSEG, PTGNN_REDUCE_MEAN, EPI>(p, st);
+        case PTGNN_REDUCE_MAX: return launch_one<NPROD, K, NSEG, PTGNN_REDUCE_MAX, EPI>(p, st);
+        default: return launch_one<NPROD, K, NSEG, PTGNN_REDUCE_MIN, EPI>(p, st);
     }
 }
 template <int NPROD, int K>
-static int launch_seg(const Params &p, int use_target, cudaStream_t st) {
+static int launch_seg(const Params &p, int use_target, bool egc, cudaStream_t st) {
+    if (egc) return launch_red<NPROD, K, 1, EPI_EGC>(p, st);
     return use_target ? launch_red<NPROD, K, 2>(p, st) : launch_red<NPROD, K, 1>(p, st);
 }
 
@@ -838,16 +926,25 @@ int aggregate(const AggregateArgs &a, cudaStream_t st) {
     p.num_blocks = (int)ceil_div(a.num_nodes, a.block_targets);
     p.T = a.num_types; p.reduce = a.reduce; p.out_mode = a.out_mode; p.status = a.status; p.epi = a.epi;
     p.trace = trace_buffer();
+    const bool egc = a.egc != nullptr;
+    if (egc) {
+        const EgcEpilogue &e = *a.egc;
+        PTGNN_CHECK_ARG(!a.use_target && (a.out_mode == 0 || a.out_mode == 1), "fused aggregate: the EGC write-out takes one segment, fp32 / bf16 output");
+        PTGNN_CHECK_ARG((e.bases == 1 || e.bases == 2 || e.bases == 4 || e.bases == 8) && e.dh > 0 && e.coef && e.col0 >= 0 &&
+                            e.col0 + kD / e.bases <= e.out_stride && e.coef_stride % 4 == 0,
+                        "fused aggregate: bad EGC write-out (bases %d, dh %d, col0 %d, stride %d)", e.bases, e.dh, e.col0, e.out_stride);
+        p.egc = e;
+    }
 #ifdef PTGNN_FUSED_QUICK   // compile-time experiments (ptxas -v / SASS of the benchmarked instances only); never defined in the build
     return a.nprod == 3 ? launch_one<3, 128, 1, PTGNN_REDUCE_SUM>(p, st) : launch_one<1, 128, 1, PTGNN_REDUCE_SUM>(p, st);
 #else
     if (a.nprod == 3) {
-        if (a.K == 64) return launch_seg<3, 64>(p, a.use_target, st);
-        return launch_seg<3, 128>(p, a.use_target, st);
+        if (a.K == 64) return launch_seg<3, 64>(p, a.use_target, egc, st);
+        return launch_seg<3, 128>(p, a.use_target, egc, st);
     }
-    if (a.K == 64) return launch_seg<1, 64>(p, a.use_target, st);
-    if (a.K == 128) return launch_seg<1, 128>(p, a.use_target, st);
-    return launch_seg<1, 256>(p, a.use_target, st);
+    if (a.K == 64) return launch_seg<1, 64>(p, a.use_target, egc, st);
+    if (a.K == 128) return launch_seg<1, 128>(p, a.use_target, egc, st);
+    return launch_seg<1, 256>(p, a.use_target, egc, st);
 #endif
 }
 

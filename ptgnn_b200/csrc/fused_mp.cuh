@@ -49,15 +49,29 @@ struct Epilogue {                       // applied to the aggregated row at writ
     float ln_eps;
 };
 
+// EGC write-out (EGCMessagePassingLayer, one launch per slab of 128 message features).  Slab position p = j * bases + b holds base b
+// of output column o = col0 + j; the block row of node n is written as 128 / bases columns out[n, col0 + j] =
+// sum_b coef[n, (o / dh) * bases + b] * agg[n, p], row stride out_stride.  coef: fp32 [N, coef_stride] (bf16-rounded values for bf16 states).
+struct EgcEpilogue {
+    const float *coef;
+    int coef_stride, bases, dh, col0, out_stride;
+};
+
 bool supported(int nprod, int K, int D, int use_target);
 // bytes of the packed edge weights (coalesced per-row layout), of one packed state row, and of the packed-state scratch
 size_t packed_weight_bytes(int nprod, int num_types, int K, int use_target);
 size_t packed_state_bytes(int nprod, int64_t rows, int K);
 int recommended_block_targets(int64_t num_nodes);
 
-// weights[t]: fp32 [128, nseg*K] row-major (nn.Linear.weight) -> packed
+// Row map of an EGC slab: packed row p = j * bases + b <- row ((o / dh) * bases + b) * dh + o % dh of the reference's
+// bases[t].weight [bases * out, K], o = col0 + j.  bases = 0: the identity (packed row p <- row p).
+struct RowMap {
+    int bases, dh, col0;
+};
+
+// weights[t]: fp32 [128, nseg*K] row-major (nn.Linear.weight; with a row map: the rows it selects) -> packed
 int pack_weights(int nprod, int num_types, int K, int use_target, const float *const *weights, void *packed, int32_t *status,
-                 cudaStream_t st);
+                 cudaStream_t st, RowMap rows = RowMap{0, 0, 0});
 // fp32 states [rows, K] -> fp16 (hi | lo') rows of 4K bytes   (NPROD = 3 only; bf16 states are gathered as they are)
 int pack_states(const float *h, int64_t rows, int K, void *packed, int32_t *status, cudaStream_t st);
 
@@ -75,6 +89,7 @@ struct AggregateArgs {
     void *out;                      // [num_nodes, 128]: out_mode 0 = fp32, 1 = bf16, 2 = packed fp16 (hi | lo') rows of 256 halfs
     int out_mode;                   //   (2 = what the weights-stationary GRU kernel takes as its A operand)
     int32_t *status;                // optional: status[0] = 1 if an aggregate is outside the fp16 range (out_mode 2)
+    const EgcEpilogue *egc;         // non-null: the EGC write-out (out_mode 0 or 1, one segment) instead of `epi`
 };
 int aggregate(const AggregateArgs &a, cudaStream_t st);
 

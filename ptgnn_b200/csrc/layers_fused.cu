@@ -201,10 +201,153 @@ int mlp_fused(int nprod, const void *node_states, const void *gather_states, int
                             static_cast<__nv_bfloat16 *>(out_states), dense_area, st, true);
 }
 
+// ---- EGCMessagePassingLayer: S = bases * out / 128 slabs of the fused aggregation, each with the EGC write-out ----------------------
+bool egc_ok(int nprod, int H, int out, int heads, int bases) {
+    return aggregate_ok(nprod, H, fused::kD, 0) && (bases == 1 || bases == 2 || bases == 4 || bases == 8) && heads > 0 && out > 0 &&
+           out % heads == 0 && out % (fused::kD / bases) == 0 && heads * bases <= 4096;
+}
+int egc_slabs(int out, int bases) { return bases * out / fused::kD; }
+int egc_coef_cols(int heads, int bases) { return (heads * bases + 3) / 4 * 4; }     // the dense kernel's multiple of 4
+size_t egc_weight_bytes(int nprod, int T, int H, int out, int bases) {
+    return (size_t)egc_slabs(out, bases) * fused::packed_weight_bytes(nprod, T, H, 0);
+}
+
+// workspace: coefficients [N, hbp] fp32 | the coefficient Linear's weight [hbp, H] and bias [hbp] (zero-padded; bf16-rounded for
+// bf16 states) | the dense kernel's workspace | packed states (fp32) or the states as fp32 (bf16) | packed slabs (no cache)
+struct EgcWs { size_t coef, cw, cb, lin, x, weights, total; };
+EgcWs egc_layout(int nprod, int64_t N, int T, int H, int out, int heads, int bases) {
+    const int hbp = egc_coef_cols(heads, bases);
+    EgcWs w{};
+    w.cw = ws_slice((size_t)N * hbp, 4);
+    w.cb = w.cw + ws_slice((size_t)hbp * H, 4);
+    w.lin = w.cb + ws_slice((size_t)hbp, 4);
+    w.x = w.lin + align_up(ptgnn_b200_linear_workspace_bytes(H, hbp), 256);
+    w.weights = w.x + (nprod == 3 ? fused::packed_state_bytes(3, N, H) : ws_slice((size_t)N * H, 4));
+    w.total = w.weights + egc_weight_bytes(nprod, T, H, out, bases);
+    return w;
+}
+
+// dst[r, c] (row stride dst_stride) = src[r, c] (fp32 or bf16, rows of `cols`), rounded to bf16 if round_bf16.  In place is fine.
+__global__ void __launch_bounds__(256) egc_copy_kernel(const void *src, int src_bf16, long long rows, int cols, int dst_stride, float *dst,
+                                                       int round_bf16) {
+    const long long total = rows * cols;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const long long r = i / cols;
+        const int c = (int)(i - r * cols);
+        float x = src_bf16 ? __bfloat162float(static_cast<const __nv_bfloat16 *>(src)[i]) : static_cast<const float *>(src)[i];
+        if (round_bf16) x = __bfloat162float(__float2bfloat16_rn(x));
+        dst[r * dst_stride + c] = x;
+    }
+}
+int egc_copy(const void *src, int src_bf16, int64_t rows, int cols, int dst_stride, float *dst, int round_bf16, cudaStream_t st) {
+    if (rows <= 0 || cols <= 0) return PTGNN_OK;
+    const int64_t blocks = ceil_div(rows * cols, (int64_t)256);
+    egc_copy_kernel<<<(unsigned)(blocks < 132 * 8 ? blocks : 132 * 8), 256, 0, st>>>(src, src_bf16, (long long)rows, cols, dst_stride, dst,
+                                                                                      round_bf16);
+    PTGNN_LAUNCHED();
+    return PTGNN_OK;
+}
+
+int egc_fused(int nprod, const void *node_states, int64_t N, int H, int out, int heads, int bases, int T, const ptgnn_b200_block_plan *bp,
+              const int32_t *row_ptr, const float *const *bases_weights, const float *coeff_weight, const float *coeff_bias, int reduce,
+              void *out_states, void *workspace, size_t workspace_bytes, void *weight_cache, size_t weight_cache_bytes, int cache_valid,
+              cudaStream_t st) {
+    PTGNN_CHECK_ARG(bp != nullptr, "egc_forward_fused: null block plan");
+    PTGNN_CHECK_ARG(T >= 0 && T <= PTGNN_MAX_EDGE_TYPES, "egc_forward_fused: bad num_types=%d", T);
+    if (!egc_ok(nprod, H, out, heads, bases)) {
+        set_error("egc_forward_fused: H=%d out=%d heads=%d bases=%d are not supported by the fused kernel (%s states)", H, out, heads, bases,
+                  nprod == 3 ? "fp32" : "bf16");
+        return PTGNN_E_UNSUPPORTED;
+    }
+    PTGNN_CHECK_ARG(N >= 0 && N < INT32_MAX, "egc_forward_fused: sizes out of range");
+    PTGNN_CHECK_ARG(reduce >= PTGNN_REDUCE_SUM && reduce <= PTGNN_REDUCE_MIN, "egc_forward_fused: bad reduce %d", reduce);
+    if (N == 0) return PTGNN_OK;
+    PTGNN_CHECK_ARG(node_states && out_states && row_ptr && coeff_weight && coeff_bias, "egc_forward_fused: null pointer");
+    PTGNN_CHECK_ARG(bp->group_off && bases_weights && T > 0, "egc_forward_fused: null block plan arrays");
+    const EgcWs L = egc_layout(nprod, N, T, H, out, heads, bases);
+    PTGNN_CHECK_WORKSPACE("egc_forward_fused", workspace, workspace_bytes, L.total);
+    char *ws = static_cast<char *>(workspace);
+    char *wpack;
+    bool pack;
+    int rc = weight_area("egc_forward_fused", ws + L.weights, weight_cache, weight_cache_bytes, egc_weight_bytes(nprod, T, H, out, bases),
+                         cache_valid, wpack, pack);
+    if (rc) return rc;
+    const int S = egc_slabs(out, bases), per_slab = fused::kD / bases;
+    const size_t slab_bytes = fused::packed_weight_bytes(nprod, T, H, 0);
+    if (pack) {
+        for (int s = 0; s < S; ++s) {
+            rc = fused::pack_weights(nprod, T, H, 0, bases_weights, wpack + s * slab_bytes, bp->status, st,
+                                     fused::RowMap{bases, out / heads, s * per_slab});
+            if (rc) return rc;
+        }
+    }
+
+    // coefficients w = weight_coeffs(h) [N, heads * bases] on the dense kernel (rows padded to a multiple of 4 with zeros).  bf16
+    // states: as autocast's Linear -- states, weight and bias rounded to bf16, fp32 accumulation (bf16 x bf16 products are exact in
+    // the dense kernel's split), the output rounded to bf16
+    const int hb = heads * bases, hbp = egc_coef_cols(heads, bases);
+    const bool bf = nprod == 1;
+    float *coef = reinterpret_cast<float *>(ws + L.coef), *cw = reinterpret_cast<float *>(ws + L.cw), *cb = reinterpret_cast<float *>(ws + L.cb);
+    PTGNN_CUDA(cudaMemsetAsync(cw, 0, L.lin - L.cw, st));           // weight and bias, padding rows included
+    if ((rc = egc_copy(coeff_weight, 0, hb, H, H, cw, bf, st))) return rc;
+    if ((rc = egc_copy(coeff_bias, 0, 1, hb, hb, cb, bf, st))) return rc;
+    const float *x = static_cast<const float *>(node_states);
+    if (bf) {
+        if ((rc = egc_copy(node_states, 1, N, H, H, reinterpret_cast<float *>(ws + L.x), 0, st))) return rc;
+        x = reinterpret_cast<const float *>(ws + L.x);
+    }
+    rc = ptgnn_b200_linear_f32(x, N, H, cw, cb, hbp, PTGNN_ACT_NONE, coef, ws + L.lin, L.x - L.lin, st);
+    if (rc) return rc;
+    if (bf && (rc = egc_copy(coef, 0, N, hbp, hbp, coef, 1, st))) return rc;
+
+    const void *src_rows = node_states;
+    if (!bf) {
+        rc = fused::pack_states(static_cast<const float *>(node_states), N, H, ws + L.x, bp->status, st);
+        if (rc) return rc;
+        src_rows = ws + L.x;
+    }
+    // one launch per slab: gather -> the slab's rows of W_t -> segmented reduce -> sum over the bases into its output columns
+    for (int s = 0; s < S; ++s) {
+        const fused::EgcEpilogue e{coef, hbp, bases, out / heads, s * per_slab, out};
+        fused::AggregateArgs a = aggregate_args(nprod, bp, row_ptr, N, H, T, reduce, wpack + s * slab_bytes);
+        a.src_rows = src_rows; a.use_target = 0; a.tgt_rows = nullptr;
+        a.out = out_states; a.out_mode = bf ? 1 : 0;
+        a.egc = &e;
+        rc = fused::aggregate(a, st);
+        if (rc) return rc;
+    }
+    return PTGNN_OK;
+}
+
 }  // namespace
 }  // namespace ptgnn
 
 using namespace ptgnn;
+
+extern "C" int32_t ptgnn_b200_egc_supported(int32_t bf16_states, int32_t in_dim, int32_t out_dim, int32_t num_heads, int32_t num_bases) {
+    return egc_ok(bf16_states ? 1 : 3, in_dim, out_dim, num_heads, num_bases) ? 1 : 0;
+}
+extern "C" size_t ptgnn_b200_egc_fused_workspace_bytes(int32_t bf16_states, int64_t num_nodes, int32_t num_types, int32_t in_dim,
+                                                       int32_t out_dim, int32_t num_heads, int32_t num_bases) {
+    const int nprod = bf16_states ? 1 : 3;
+    if (num_nodes < 0 || num_types < 0 || num_types > PTGNN_MAX_EDGE_TYPES || !egc_ok(nprod, in_dim, out_dim, num_heads, num_bases)) return 0;
+    return egc_layout(nprod, num_nodes, num_types, in_dim, out_dim, num_heads, num_bases).total;
+}
+extern "C" size_t ptgnn_b200_egc_fused_weight_cache_bytes(int32_t bf16_states, int32_t num_types, int32_t in_dim, int32_t out_dim,
+                                                          int32_t num_heads, int32_t num_bases) {
+    const int nprod = bf16_states ? 1 : 3;
+    if (num_types <= 0 || num_types > PTGNN_MAX_EDGE_TYPES || !egc_ok(nprod, in_dim, out_dim, num_heads, num_bases)) return 0;
+    return egc_weight_bytes(nprod, num_types, in_dim, out_dim, num_bases);
+}
+extern "C" int ptgnn_b200_egc_forward_fused(int32_t bf16_states, const void *node_states, int64_t num_nodes, int32_t in_dim, int32_t out_dim,
+                                            int32_t num_heads, int32_t num_bases, int32_t num_types, const ptgnn_b200_block_plan *block_plan,
+                                            const int32_t *row_ptr, const float *const *bases_weights, const float *coeff_weight,
+                                            const float *coeff_bias, int32_t reduce, void *out_states, void *workspace, size_t workspace_bytes,
+                                            void *weight_cache, size_t weight_cache_bytes, int32_t cache_valid, void *stream) {
+    return egc_fused(bf16_states ? 1 : 3, node_states, num_nodes, in_dim, out_dim, num_heads, num_bases, num_types, block_plan, row_ptr,
+                     bases_weights, coeff_weight, coeff_bias, reduce, out_states, workspace, workspace_bytes, weight_cache, weight_cache_bytes,
+                     cache_valid, static_cast<cudaStream_t>(stream));
+}
 
 extern "C" int32_t ptgnn_b200_block_plan_block_targets(int64_t num_nodes) { return fused::recommended_block_targets(num_nodes); }
 

@@ -37,7 +37,11 @@ factories import the layer classes by module path (`implementations/typilus/trai
    ``CnnConfig`` and ``CharUnitEmbedder``, which ``"char"`` still builds.  The default leaves the reference's classes in place,
 11. with ``native_char_embedder=True`` only: re-binds ``CharUnitEmbedder`` inside the same module and in reference modules imported
    earlier (the native character-CNN kernel, DESIGN.md §3.13), so that ``"char"`` (VarMisuse's ``CandidateNodeAnnotationModel``) builds
-   the native class.  ``native_embedders=True`` alone leaves the reference's ``CharUnitEmbedder`` in place.
+   the native class.  ``native_embedders=True`` alone leaves the reference's ``CharUnitEmbedder`` in place,
+12. with ``native_egc=True`` only: pre-seeds / re-binds ``EGCMessagePassingLayer`` at
+   ``ptgnn.neuralmodels.gnn.messagepassing.egcmessagepassing`` (the fused aggregation kernel with the EGC write-out, DESIGN.md §3.14) in
+   the same way as step 8, so that a GNN built with EGC layers runs them natively and trains.  The default leaves the reference's class
+   in place.
 
 After ``install()``: ``import ptgnn.implementations.ppi.train`` etc. build ptgnn_b200 layers, unchanged.  ``uninstall()``
 restores the reference's classes.  The reference must be importable as ``ptgnn`` for steps 2-4 (it is not on the GPU test box;
@@ -70,6 +74,8 @@ _DECODER_MODULE = "ptgnn.neuralmodels.sequence.grucopydecoder"
 _EMBEDDER_MODULE = "ptgnn.neuralmodels.embeddings.strelementrepresentationmodel"
 _NATIVE_EMBEDDERS = ("TokenUnitEmbedder", "SubtokenUnitEmbedder")
 _NATIVE_CHAR_EMBEDDER = "CharUnitEmbedder"
+_EGC_MODULE = "ptgnn.neuralmodels.gnn.messagepassing.egcmessagepassing"
+_EGC_CLASS = "EGCMessagePassingLayer"
 _saved: Dict[str, object] = {}
 
 
@@ -155,6 +161,12 @@ def _install_native_pna() -> None:
     _install_native_class(_PNA_MODULE, _PNA_CLASS, getattr(_agg, _PNA_CLASS))
 
 
+def _install_native_egc() -> None:
+    from . import egc as _egc
+
+    _install_native_class(_EGC_MODULE, _EGC_CLASS, getattr(_egc, _EGC_CLASS))
+
+
 def _install_native_decoder() -> None:
     from . import decoder as _dec
 
@@ -173,10 +185,10 @@ def _install_native_embedders(names=_NATIVE_EMBEDDERS) -> None:
 
 def install(force_torch_scatter: bool = False, native_reducers: bool = False, native_selfattention: bool = False,
             native_graphnorm: bool = False, native_pna: bool = False, native_decoder: bool = False,
-            native_embedders: bool = False, native_char_embedder: bool = False) -> Dict[str, object]:
+            native_embedders: bool = False, native_char_embedder: bool = False, native_egc: bool = False) -> Dict[str, object]:
     report: Dict[str, object] = {"torch_scatter": "real", "layers": False, "container": False, "metrics": False, "reducers": False,
                                  "selfattention": False, "graphnorm": False, "pna": False, "decoder": False, "embedders": False,
-                                 "char_embedder": False}
+                                 "char_embedder": False, "egc": False}
     # 1. torch_scatter
     have_real = False
     if not force_torch_scatter:
@@ -245,6 +257,10 @@ def install(force_torch_scatter: bool = False, native_reducers: bool = False, na
     if native_char_embedder:
         _install_native_embedders((_NATIVE_CHAR_EMBEDDER,))
         report["char_embedder"] = True
+    # 12. EGCMessagePassingLayer (opt-in)
+    if native_egc:
+        _install_native_egc()
+        report["egc"] = True
     return report
 
 
@@ -263,7 +279,7 @@ def uninstall() -> None:
                 setattr(sys.modules[mod_name], attr, val)
         else:
             sys.modules[key] = val
-    for mod_name in (*_LAYER_MODULES, _SELFATT_MODULE, _GRAPHNORM_MODULE, _PNA_MODULE):
+    for mod_name in (*_LAYER_MODULES, _SELFATT_MODULE, _GRAPHNORM_MODULE, _PNA_MODULE, _EGC_MODULE):
         if getattr(sys.modules.get(mod_name), "__ptgnn_b200_overlay__", False):
             del sys.modules[mod_name]
     for name in ("torch_scatter", "torch_scatter.composite"):
