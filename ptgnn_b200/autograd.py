@@ -71,32 +71,44 @@ class _exact_fp16_gemms:
         return False
 
 
-def _split16(x: torch.Tensor, scaled: bool = True, index: Optional[torch.Tensor] = None):
+def _pow2_scale(x: torch.Tensor):
+    """(scale, inv_scale) as fp32 device scalars: the power of two that brings the largest |element| of x to [512, 1024).  Multiplying
+    by it is exact in fp32's normal range, and nothing synchronises."""
+    amax = torch.linalg.vector_norm(x, ord=float("inf")).clamp(min=1e-30)
+    scale = torch.exp2(torch.floor(torch.log2(1024.0 / amax))).to(torch.float32)
+    return scale, 1.0 / scale
+
+
+def _split16(x: torch.Tensor, index: Optional[torch.Tensor] = None, scale=None):
     """fp32 [rows, cols] -> (hi, lo, inv_scale) with (hi + lo / 2048) * inv_scale ~= x[index] (index: int32 row ids, None = all rows in
-    order); hi, lo fp16: the 3xFP16 split of the forward kernels (22 significant bits).  scaled: first multiply by the power of two
-    that brings the largest element to ~2^10 -- gradients are routinely below fp16's normal range (states and aggregates are not: the
-    forward already requires them to fit).  Gather, scaling and split are one native pass; nothing synchronises."""
+    order); hi, lo fp16: the 3xFP16 split of the forward kernels (22 significant bits) of x times ``_pow2_scale(x)``.  The scaling keeps
+    gradients (routinely below fp16's normal range) and states beyond fp16's range (PTGNN_B200_FP32_MODE=tf32) at full precision.
+    scale: that pair when the caller already has it.  Gather, scaling and split are one native pass; nothing synchronises."""
     rows = x.shape[0] if index is None else int(index.shape[0])
     cols = x.shape[1]
     hi = torch.empty(rows, cols, dtype=torch.float16, device=x.device)
     lo = torch.empty(rows, cols, dtype=torch.float16, device=x.device)
     if rows == 0 or x.numel() == 0:
         return hi, lo, 1.0
-    scale, inv = None, 1.0
-    if scaled:
-        amax = torch.linalg.vector_norm(x, ord=float("inf")).clamp(min=1e-30)
-        scale = torch.exp2(torch.floor(torch.log2(1024.0 / amax))).to(torch.float32)
-        inv = 1.0 / scale
+    scale, inv = _pow2_scale(x) if scale is None else scale
     x = x.contiguous()
     if cols % 8 != 0:      # rare shapes: torch ops
         v = x if index is None else x.index_select(0, index.long())
-        v = v * scale if scale is not None else v
+        v = v * scale
         hi = v.half()
         return hi, torch.sub(v, hi).mul_(2048.0).half(), inv
     with torch.cuda.device(x.device):
         rc = N.lib().ptgnn_b200_gather_split_f16(N.ptr(x), N.ptr(index), rows, cols, N.ptr(scale), N.ptr(hi), N.ptr(lo), N.current_stream(x.device))
     N.check(rc, "ptgnn_b200_gather_split_f16")
     return hi, lo, inv
+
+
+def _add_aggregate(d_h: torch.Tensor, plan, x: torch.Tensor, weights, scale) -> torch.Tensor:
+    """d_h + sum_{e -> v} W_t(e) x[src(e)] for a gradient x: ``C.aggregate`` on x times its ``_pow2_scale`` pair ``scale``, scaled back in
+    the add.  The fused kernel splits its operand into fp16 pairs without scaling, which represents x only to 2^-36 absolute (no
+    precision left for a gradient of 1e-8) and overflows at 65504; the power of two makes both exact in fp32's normal range."""
+    s, inv = scale
+    return torch.addcmul(d_h, C.aggregate(plan, x * s, weights, N.REDUCE["sum"]), inv)
 
 
 def _mm_t_split(a, b):
@@ -131,7 +143,7 @@ def _gru_backward(g, agg, h, w_ih, w_hh, b_ih, b_hh):
     d_agg = C.linear(d_gi, w_ih.t().contiguous())                        # [N, D]
     with _exact_fp16_gemms():
         s_gi, s_gh = _split16(d_gi), _split16(d_gh)
-        d_w_ih, d_w_hh = _mm_t_split(s_gi, _split16(agg, False)), _mm_t_split(s_gh, _split16(h, False))
+        d_w_ih, d_w_hh = _mm_t_split(s_gi, _split16(agg)), _mm_t_split(s_gh, _split16(h))
     return d_agg, d_h, d_w_ih, d_w_hh, d_gi.sum(dim=0), d_gh.sum(dim=0)
 
 
@@ -180,7 +192,7 @@ class _GatedLayerFunction(torch.autograd.Function):
 def _aggregation_backward(plan, adj, h, W, d_agg, reduce_name, arg, d_h, b_all=None):
     """Backward of agg = reduce_{e -> v} W_t(e) h[src(e)] (bias-free per-type Linear, then sum / mean / max / min) from d_agg [N, D]:
     returns (d_W per type, d_h + the h part).  arg: the winning edge ids of max / min ([N, D], E for empty targets).  b_all: the
-    3xFP16 split of the gathered source states, ``_split16(h, False, plan.src32)``, when the caller reuses it across calls.
+    3xFP16 split of the gathered source states, ``_split16(h, plan.src32)``, when the caller reuses it across calls.
     sum / mean: split fp16 GEMMs over edges, and the forward's aggregation on the transposed graph with W_t^T; max / min: the message
     gradients routed to the winning edges, the split GEMMs, and the native scatter-add by source."""
     num_nodes = h.shape[0]
@@ -190,10 +202,11 @@ def _aggregation_backward(plan, adj, h, W, d_agg, reduce_name, arg, d_h, b_all=N
         if reduce_name == "mean":
             cnt = (plan.row_ptr[1:] - plan.row_ptr[:-1]).clamp(min=1).to(torch.float32)
             d_agg = d_agg / cnt[:, None]
+        scale = _pow2_scale(d_agg)
         with _exact_fp16_gemms():
-            a_all = _split16(d_agg, True, plan.tgt32)                    # [E, D] rows of d_agg, cat(types) order
+            a_all = _split16(d_agg, plan.tgt32, scale)                   # [E, D] rows of d_agg, cat(types) order
             if b_all is None:
-                b_all = _split16(h, False, plan.src32)                   # [E, H] source states
+                b_all = _split16(h, plan.src32)                          # [E, H] source states
             for t, w in enumerate(W):
                 lo_, hi_ = plan.type_off[t], plan.type_off[t + 1]
                 d_W.append(_mm_t_split(_slice(a_all, lo_, hi_), _slice(b_all, lo_, hi_)) if hi_ > lo_ else torch.zeros_like(w))
@@ -201,7 +214,7 @@ def _aggregation_backward(plan, adj, h, W, d_agg, reduce_name, arg, d_h, b_all=N
             # d h_src[u] = sum over edges (u -> v, type t) of W_t^T d_agg[v]: the forward's aggregation on the transposed graph
             rev = [(tgt, src) for src, tgt in adj]
             rplan = plan_for(rev, num_nodes)
-            d_h = d_h + C.aggregate(rplan, d_agg.contiguous(), [w.t().contiguous() for w in W], N.REDUCE["sum"])
+            d_h = _add_aggregate(d_h, rplan, d_agg.contiguous(), [w.t().contiguous() for w in W], scale)
     else:
         D = d_agg.shape[1]
         d_msg = torch.zeros(E + 1, D, dtype=torch.float32, device=h.device)      # row E takes the empty targets' sentinel
@@ -209,7 +222,7 @@ def _aggregation_backward(plan, adj, h, W, d_agg, reduce_name, arg, d_h, b_all=N
         with _exact_fp16_gemms():
             a_all = _split16(d_msg[:E])
             if b_all is None:
-                b_all = _split16(h, False, plan.src32)
+                b_all = _split16(h, plan.src32)
         lo = 0
         for (src, tgt), w in zip(adj, W):
             e_t = src.numel()
@@ -269,7 +282,7 @@ class _EgcLayerFunction(torch.autograd.Function):
         d_h = torch.zeros_like(h)
         d_slabs = [[] for _ in W]
         with _exact_fp16_gemms():
-            b_all = _split16(h, False, plan.src32)                       # the gathered source states, once for every slab
+            b_all = _split16(h, plan.src32)                              # the gathered source states, once for every slab
         for s in range(bases * out // 128):
             rows = egc_slab_rows(s, out, heads, bases, h.device)
             Ws = [wt.index_select(0, rows) for wt in W]                 # [128, H]: the slab's rows, in slab order
@@ -297,7 +310,7 @@ class _EgcLayerFunction(torch.autograd.Function):
         # 6. the coefficient Linear
         d_w = prod.view(num_nodes, heads, dh, bases).sum(dim=2).reshape(num_nodes, heads * bases)
         with _exact_fp16_gemms():
-            d_cw = _mm_t_split(_split16(d_w), _split16(h, False))
+            d_cw = _mm_t_split(_split16(d_w), _split16(h))
         d_h = d_h + C.linear(d_w.contiguous(), cw.t().contiguous())
         return (None, None, None, None, d_h, d_cw, d_w.sum(dim=0), *d_W)
 
@@ -381,9 +394,10 @@ class _MlpLayerFunction(torch.autograd.Function):
             if reduce_name == "mean":
                 cnt = (plan.row_ptr[1:] - plan.row_ptr[:-1]).clamp(min=1).to(torch.float32)
                 d_agg = (d_agg / cnt[:, None]).contiguous()
+            scale = _pow2_scale(d_agg)
             with _exact_fp16_gemms():
-                a_all, b_all = _split16(d_agg, True, plan.tgt32), _split16(h, False, plan.src32)
-                g_all = _split16(h, False, plan.tgt32) if use_target else None
+                a_all, b_all = _split16(d_agg, plan.tgt32, scale), _split16(h, plan.src32)
+                g_all = _split16(h, plan.tgt32) if use_target else None
                 for t, w in enumerate(W):
                     lo_, hi_ = plan.type_off[t], plan.type_off[t + 1]
                     if hi_ == lo_:
@@ -394,10 +408,10 @@ class _MlpLayerFunction(torch.autograd.Function):
                     d_W.append(torch.cat([d_w, _mm_t_split(a, _slice(g_all, lo_, hi_))], dim=1) if use_target else d_w)
             if E > 0:
                 rplan = plan_for([(tgt, src) for src, tgt in adj], num_nodes)                     # transposed graph: d h_src
-                d_h = d_h + C.aggregate(rplan, d_agg, [w.t().contiguous() for w in Ws], N.REDUCE["sum"])
+                d_h = _add_aggregate(d_h, rplan, d_agg, [w.t().contiguous() for w in Ws], scale)
                 if use_target:                                                                     # d h_tgt: every edge sends W_g^T d_agg[v] to its own target v
                     tplan = plan_for([(tgt, tgt) for _src, tgt in adj], num_nodes)
-                    d_h = d_h + C.aggregate(tplan, d_agg, [w.t().contiguous() for w in Wg], N.REDUCE["sum"])
+                    d_h = _add_aggregate(d_h, tplan, d_agg, [w.t().contiguous() for w in Wg], scale)
         else:
             # per-edge message gradients: routed to the winning edges (max / min), or the PNA backward
             if pna is not None:
@@ -409,8 +423,8 @@ class _MlpLayerFunction(torch.autograd.Function):
                 d_msg = torch.zeros(E + 1, d_agg.shape[1], dtype=torch.float32, device=h.device)
                 d_msg = d_msg.scatter_(0, arg, d_agg)[:E]
             with _exact_fp16_gemms():
-                a_all, b_all = _split16(d_msg), _split16(h, False, plan.src32)
-                g_all = _split16(h, False, plan.tgt32) if use_target else None
+                a_all, b_all = _split16(d_msg), _split16(h, plan.src32)
+                g_all = _split16(h, plan.tgt32) if use_target else None
             lo = 0
             for t, ((src, tgt), w) in enumerate(zip(adj, W)):
                 e_t = src.numel()
@@ -606,7 +620,7 @@ class _GlobalGruFn(torch.autograd.Function):
         d_table = C.segment_reduce(d_gi, plan, N.REDUCE["sum"])             # [G, 3H]: per graph, in node order
         d_g = C.linear(d_table, w_ih.t().contiguous())                      # [G, S]
         with _exact_fp16_gemms():
-            d_w_hh = _mm_t_split(_split16(d_gh), _split16(h, False))
+            d_w_hh = _mm_t_split(_split16(d_gh), _split16(h))
         return None, None, d_h, d_g, d_table.t() @ g, d_w_hh, d_table.sum(dim=0), d_gh.sum(dim=0)
 
 
