@@ -1,22 +1,21 @@
-"""Backward of ``GatedMessagePassingLayer`` (SURVEY.md §8 row f-1, first cut): makes the layer usable under ``torch.autograd``
-(`/root/reference/ptgnn/baseneuralmodel/trainer.py:221-236` calls ``loss.backward()`` through the layers).
+"""Backward passes of the native layers and operators, so that they train under ``torch.autograd`` (the reference's trainer calls
+``loss.backward()`` through the layers: ptgnn/baseneuralmodel/trainer.py:221-236).
 
-The forward is the unchanged native forward (fused aggregation + GRU kernels).  The backward re-computes what it needs and keeps the
-edge-sized work on the native kernels:
+Each Function's forward is the unchanged native forward.  Its backward re-computes what it needs and keeps the edge-sized work on the
+native kernels.  The three trainable message-passing layers (gated, Mlp with the default message MLP, EGC) share one backward for
+their aggregation agg = reduce_{e -> v} W_t(e) [h_src(e) ; h_tgt(e)], ``_aggregation_backward``:
 
-* aggregate re-computation: ``edge_messages`` + ``segment_reduce`` kernels (with the arg-max edge ids for max / min);
-* GRU: gate pre-activations and the two input-gradient products on the native dense kernel (``composed.linear``), the gate
-  derivatives as pointwise torch ops;
-* ``d h_src``: sum / mean -- the SAME gather -> Linear -> segmented-reduce kernels run on the transposed graph (edges reversed,
-  weights ``W_t^T``, states = ``d agg``); max / min -- the routed message gradients times ``W_t`` on the dense kernel, then the
-  native scatter-add by source;
-* parameter gradients (``dW_t``, ``dW_ih``, ``dW_hh``): plain ``[out, rows] x [rows, in]`` GEMMs with a huge K (rows = edges or
-  nodes) -- library GEMMs on the tensor cores in the forward's 3xFP16 split (three cuBLAS fp16 GEMMs with fp32 accumulation per
-  product, operands scaled by a power of two first); bias gradients are column sums.
+* ``d h``: sum / mean -- the forward's aggregation kernels on the transposed graph (edges reversed, or from each target to itself
+  for the ``h_tgt`` columns; weights ``W_t^T``; states ``d agg`` scaled by a power of two); max / min and PNA -- the per-edge message
+  gradients times ``W_t`` on the dense kernel, then the native scatter-add by source (and by target for the ``h_tgt`` columns);
+* parameter gradients (``dW_t``, and the GRU's ``dW_ih``, ``dW_hh``): plain ``[out, rows] x [rows, in]`` GEMMs with a huge K (rows =
+  edges or nodes) -- library GEMMs on the tensor cores in the forward's 3xFP16 split (``_mm_t_split``: three cuBLAS fp16 GEMMs with
+  fp32 accumulation per product, operands scaled by a power of two first); bias gradients are column sums.
 
-``MlpMessagePassingLayer`` (default message MLP) follows the same scheme; its node-sized tail (activation, LayerNorm, dense layer:
-mlpmessagepassing.py:114-117) is differentiated by a local ``torch.autograd.grad`` over library ops, and its output Dropout is a torch
-op applied outside the Function.
+The GRUs (gated layer, GruGlobalStateUpdate) take their gate pre-activations and input-gradient products on the native dense kernel
+(``composed.linear``) and the gate derivatives from one native pointwise kernel (``_gru_gate_grads``).  The Mlp layer's node-sized
+tail (activation, LayerNorm, dense layer: mlpmessagepassing.py:114-117) is differentiated by a local ``torch.autograd.grad`` over
+library ops, and its output Dropout is a torch op applied outside the Function.
 
 The gated layer's training-mode dropout (a per-edge mask on the gathered rows, gatedmessagepassing.py:59) and edge features under
 autograd need the gathered ``[E_t, H]`` rows to exist: they run as the reference writes the layer, with the Linear / scatter / GRUCell
@@ -57,18 +56,6 @@ def output_dropout_suppressed() -> bool:
 
 def needs_grad(module: torch.nn.Module, node_states: torch.Tensor) -> bool:
     return torch.is_grad_enabled() and (node_states.requires_grad or any(p.requires_grad for p in module.parameters()))
-
-
-class _exact_fp16_gemms:
-    """cuBLAS fp16 GEMMs with fp32 accumulation all the way (no reduced-precision split-K reductions) while the split products run."""
-
-    def __enter__(self):
-        self.previous = torch.backends.cuda.matmul.allow_fp16_reduced_precision_reduction
-        torch.backends.cuda.matmul.allow_fp16_reduced_precision_reduction = False
-
-    def __exit__(self, *exc):
-        torch.backends.cuda.matmul.allow_fp16_reduced_precision_reduction = self.previous
-        return False
 
 
 def _pow2_scale(x: torch.Tensor):
@@ -114,12 +101,18 @@ def _add_aggregate(d_h: torch.Tensor, plan, x: torch.Tensor, weights, scale) -> 
 def _mm_t_split(a, b):
     """A^T B in fp32 accuracy on the tensor cores for A = (hi, lo, inv) [K, M], B = (hi, lo, inv) [K, N]: three library fp16 GEMMs with
     fp32 accumulation (hi*hi + 2^-11 (hi*lo + lo*hi)) -- the K = edges / nodes parameter-gradient products were 39 % of a training
-    step as fp32 SIMT GEMMs."""
+    step as fp32 SIMT GEMMs.  The GEMMs accumulate in fp32 all the way: reduced-precision split-K reductions are off while they run."""
     a_hi, a_lo, a_inv = a
     b_hi, b_lo, b_inv = b
-    main = torch.mm(a_hi.t(), b_hi, out_dtype=torch.float32)
-    corr = torch.mm(a_hi.t(), b_lo, out_dtype=torch.float32)
-    corr.add_(torch.mm(a_lo.t(), b_hi, out_dtype=torch.float32))
+    matmul = torch.backends.cuda.matmul
+    previous = matmul.allow_fp16_reduced_precision_reduction
+    matmul.allow_fp16_reduced_precision_reduction = False
+    try:
+        main = torch.mm(a_hi.t(), b_hi, out_dtype=torch.float32)
+        corr = torch.mm(a_hi.t(), b_lo, out_dtype=torch.float32)
+        corr.add_(torch.mm(a_lo.t(), b_hi, out_dtype=torch.float32))
+    finally:
+        matmul.allow_fp16_reduced_precision_reduction = previous
     return main.add_(corr, alpha=1.0 / 2048.0).mul_(a_inv * b_inv)
 
 
@@ -128,22 +121,35 @@ def _slice(split, lo_, hi_):
     return hi[lo_:hi_], lo[lo_:hi_], inv
 
 
-def _gru_backward(g, agg, h, w_ih, w_hh, b_ih, b_hh):
-    """Gradients of torch.nn.GRUCell (gate order r, z, n) w.r.t. (input, hidden, weight_ih, weight_hh, bias_ih, bias_hh): gate
-    pre-activations and the two input-gradient products on the native dense kernel, the gate derivatives in one native pointwise
-    kernel, the parameter gradients ([3H, N] x [N, .], K = num_nodes) as split fp16 library GEMMs."""
-    gi = C.linear(agg, w_ih, b_ih)
-    gh = C.linear(h, w_hh, b_hh)
+def _mean_divisor(plan) -> torch.Tensor:
+    """[segments] fp32: each segment's length (a target's in-degree, a graph's node count), at least 1 -- what mean divides by."""
+    return (plan.row_ptr[1:] - plan.row_ptr[:-1]).clamp(min=1).to(torch.float32)
+
+
+def _route_to_arg(g: torch.Tensor, arg: torch.Tensor, rows: int) -> torch.Tensor:
+    """Backward of a max / min reduction over ``rows`` input rows: [rows, C] zeros with each element g[v, c] at row arg[v, c].  Empty
+    segments point at the sentinel row ``rows``, which is dropped; every (row, column) belongs to one segment, so nothing collides."""
+    return torch.zeros(rows + 1, g.shape[1], dtype=g.dtype, device=g.device).scatter_(0, arg, g)[:rows]
+
+
+def _gru_gate_grads(g, gi, gh, h, w_hh):
+    """(d gi, d gh, d h) of torch.nn.GRUCell (gate order r, z, n) from its gate pre-activations gi, gh: the gate derivatives in one native
+    pointwise kernel; d h is the direct path plus the product through W_hh on the native dense kernel."""
     d_gi, d_gh, d_h = torch.empty_like(gi), torch.empty_like(gh), torch.empty_like(h)
     with torch.cuda.device(h.device):
         rc = N.lib().ptgnn_b200_gru_gate_grads_f32(N.ptr(gi), N.ptr(gh), N.ptr(h), N.ptr(g), h.shape[0], h.shape[1], N.ptr(d_gi), N.ptr(d_gh),
                                                   N.ptr(d_h), N.current_stream(h.device))
     N.check(rc, "ptgnn_b200_gru_gate_grads_f32")
-    d_h = d_h + C.linear(d_gh, w_hh.t().contiguous())                    # direct path + through W_hh
+    return d_gi, d_gh, d_h + C.linear(d_gh, w_hh.t().contiguous())
+
+
+def _gru_backward(g, agg, h, w_ih, w_hh, b_ih, b_hh):
+    """Gradients of torch.nn.GRUCell w.r.t. (input, hidden, weight_ih, weight_hh, bias_ih, bias_hh): gate pre-activations and the two
+    input-gradient products on the native dense kernel, the parameter gradients ([3H, N] x [N, .], K = num_nodes) as split fp16
+    library GEMMs."""
+    d_gi, d_gh, d_h = _gru_gate_grads(g, C.linear(agg, w_ih, b_ih), C.linear(h, w_hh, b_hh), h, w_hh)
     d_agg = C.linear(d_gi, w_ih.t().contiguous())                        # [N, D]
-    with _exact_fp16_gemms():
-        s_gi, s_gh = _split16(d_gi), _split16(d_gh)
-        d_w_ih, d_w_hh = _mm_t_split(s_gi, _split16(agg)), _mm_t_split(s_gh, _split16(h))
+    d_w_ih, d_w_hh = _mm_t_split(_split16(d_gi), _split16(agg)), _mm_t_split(_split16(d_gh), _split16(h))
     return d_agg, d_h, d_w_ih, d_w_hh, d_gi.sum(dim=0), d_gh.sum(dim=0)
 
 
@@ -162,78 +168,73 @@ class _GatedLayerFunction(torch.autograd.Function):
     def backward(ctx, grad_out):
         h, w_ih, w_hh, b_ih, b_hh, *weights = ctx.saved_tensors
         adj: List[Tuple[torch.Tensor, torch.Tensor]] = ctx.adjacency_lists
-        reduce_name = ctx.reduce_name
-        reduce = N.REDUCE[reduce_name]
         g = grad_out.contiguous().float()
         h = h.detach().contiguous()
-        num_nodes, H = h.shape
         W = [w.detach().contiguous() for w in weights]
         w_ih, w_hh = w_ih.detach().contiguous(), w_hh.detach().contiguous()
-        plan = plan_for(adj, num_nodes)
-        E = plan.num_edges
-
-        # ---- 1. re-compute the aggregate (and, for max / min, which edge won each (target, feature))
-        arg = None
-        if reduce_name in ("max", "min"):
-            msg = C.edge_messages(plan, h, None, W, False)                   # [E, D], cat(types) order
-            agg, arg = C.segment_reduce(msg, plan, reduce, return_arg=True)
-            del msg
-        else:
-            agg = C.aggregate(plan, h, W, reduce)                            # the fused kernel where it takes the dimensions
-
-        # ---- 2. GRUCell backward
+        plan = plan_for(adj, h.shape[0])
+        agg, arg = _recompute_aggregate(plan, h, W, ctx.reduce_name)
         d_agg, d_h, d_w_ih, d_w_hh, d_b_ih, d_b_hh = _gru_backward(g, agg, h, w_ih, w_hh, b_ih.detach(), b_hh.detach())
-
-        # ---- 3. aggregation + per-type Linear backward
-        d_W, d_h = _aggregation_backward(plan, adj, h, W, d_agg, reduce_name, arg, d_h)
+        d_W, d_h = _aggregation_backward(plan, adj, h, W, d_agg, ctx.reduce_name, arg, d_h)
         return (None, None, None, d_h, d_w_ih, d_w_hh, d_b_ih, d_b_hh, *d_W)
 
 
-def _aggregation_backward(plan, adj, h, W, d_agg, reduce_name, arg, d_h, b_all=None):
-    """Backward of agg = reduce_{e -> v} W_t(e) h[src(e)] (bias-free per-type Linear, then sum / mean / max / min) from d_agg [N, D]:
-    returns (d_W per type, d_h + the h part).  arg: the winning edge ids of max / min ([N, D], E for empty targets).  b_all: the
-    3xFP16 split of the gathered source states, ``_split16(h, plan.src32)``, when the caller reuses it across calls.
-    sum / mean: split fp16 GEMMs over edges, and the forward's aggregation on the transposed graph with W_t^T; max / min: the message
-    gradients routed to the winning edges, the split GEMMs, and the native scatter-add by source."""
+def _recompute_aggregate(plan, h, W, reduce_name):
+    """(agg, arg) of agg = reduce_{e -> v} W_t(e) h[src(e)]: arg, for max / min, is which edge won each (target, feature), from the
+    messages and the segmented reduce; sum / mean run the fused kernel where it takes the dimensions, and arg is None."""
+    if reduce_name in ("max", "min"):
+        msg = C.edge_messages(plan, h, None, W, False)                       # [E, D], cat(types) order
+        return C.segment_reduce(msg, plan, N.REDUCE[reduce_name], return_arg=True)
+    return C.aggregate(plan, h, W, N.REDUCE[reduce_name]), None
+
+
+def _aggregation_backward(plan, adj, h, W, d_agg, reduce_name, arg, d_h, b_all=None, *, W_tgt=None, d_msg=None):
+    """Backward of agg = reduce_{e -> v} W_t(e) [h[src(e)] ; h[tgt(e)]] (bias-free per-type Linear, then sum / mean / max / min) from
+    d_agg [N, D]: returns (d_W per type, d_h + the h part).  W: the columns of W_t that multiply h_src; W_tgt: those that multiply h_tgt
+    (None: the messages read h_src only), and d_W[t] is then [d W_src ; d W_tgt] along dim 1.  arg: the winning edge ids of max / min
+    ([N, D], E for empty targets).  d_msg: the per-edge message gradients [E, D] when the caller has them (PNA's backward); they replace
+    the routing of d_agg through arg.  b_all: the 3xFP16 split of the gathered source states, ``_split16(h, plan.src32)``, when the
+    caller reuses it across calls.
+    sum / mean: split fp16 GEMMs over edges, and the forward's aggregation with W_t^T on the transposed graph (and, for h_tgt, on the
+    graph of each edge's target to itself); otherwise: split fp16 GEMMs over the message gradients, and per type the native linear
+    with W_t^T and scatter-add by source (and by target)."""
     num_nodes = h.shape[0]
     E = plan.num_edges
-    d_W = []
-    if reduce_name in ("sum", "mean"):
+    dense = d_msg is None and reduce_name in ("sum", "mean")
+    if dense:
         if reduce_name == "mean":
-            cnt = (plan.row_ptr[1:] - plan.row_ptr[:-1]).clamp(min=1).to(torch.float32)
-            d_agg = d_agg / cnt[:, None]
-        scale = _pow2_scale(d_agg)
-        with _exact_fp16_gemms():
-            a_all = _split16(d_agg, plan.tgt32, scale)                   # [E, D] rows of d_agg, cat(types) order
-            if b_all is None:
-                b_all = _split16(h, plan.src32)                          # [E, H] source states
-            for t, w in enumerate(W):
-                lo_, hi_ = plan.type_off[t], plan.type_off[t + 1]
-                d_W.append(_mm_t_split(_slice(a_all, lo_, hi_), _slice(b_all, lo_, hi_)) if hi_ > lo_ else torch.zeros_like(w))
-        if E > 0:
-            # d h_src[u] = sum over edges (u -> v, type t) of W_t^T d_agg[v]: the forward's aggregation on the transposed graph
-            rev = [(tgt, src) for src, tgt in adj]
-            rplan = plan_for(rev, num_nodes)
-            d_h = _add_aggregate(d_h, rplan, d_agg.contiguous(), [w.t().contiguous() for w in W], scale)
+            d_agg = d_agg / _mean_divisor(plan)[:, None]
+        d_agg = d_agg.contiguous()
+        scale = _pow2_scale(d_agg)                                       # one scale for a_all and the transposed aggregations
+        a_all = _split16(d_agg, plan.tgt32, scale)                       # [E, D] rows of d_agg, cat(types) order
     else:
-        D = d_agg.shape[1]
-        d_msg = torch.zeros(E + 1, D, dtype=torch.float32, device=h.device)      # row E takes the empty targets' sentinel
-        d_msg.scatter_(0, arg, d_agg)                                            # each (edge, feature) has one target: no collisions
-        with _exact_fp16_gemms():
-            a_all = _split16(d_msg[:E])
-            if b_all is None:
-                b_all = _split16(h, plan.src32)
-        lo = 0
-        for (src, tgt), w in zip(adj, W):
-            e_t = src.numel()
-            part = d_msg[lo:lo + e_t]
-            lo += e_t
-            if e_t == 0:
-                d_W.append(torch.zeros_like(w))
-                continue
-            with _exact_fp16_gemms():
-                d_W.append(_mm_t_split(_slice(a_all, lo - e_t, lo), _slice(b_all, lo - e_t, lo)))
-            d_h = d_h + scatter_sum(C.linear(part.contiguous(), w.t().contiguous()), src, dim=0, dim_size=num_nodes)
+        if d_msg is None:
+            d_msg = _route_to_arg(d_agg, arg, E)
+        a_all = _split16(d_msg)
+    if b_all is None:
+        b_all = _split16(h, plan.src32)                                  # [E, H] source states
+    g_all = None if W_tgt is None else _split16(h, plan.tgt32)           # [E, H] target states
+    d_W = []
+    for t, ((src, tgt), w) in enumerate(zip(adj, W)):
+        lo, hi = plan.type_off[t], plan.type_off[t + 1]
+        if hi == lo:
+            d_W.append(w.new_zeros(w.shape[0], w.shape[1] + (0 if W_tgt is None else W_tgt[t].shape[1])))
+            continue
+        a = _slice(a_all, lo, hi)
+        d_w = _mm_t_split(a, _slice(b_all, lo, hi))
+        d_W.append(d_w if W_tgt is None else torch.cat([d_w, _mm_t_split(a, _slice(g_all, lo, hi))], dim=1))
+        if not dense:
+            part = d_msg[lo:hi].contiguous()
+            d_h = d_h + scatter_sum(C.linear(part, w.t().contiguous()), src, dim=0, dim_size=num_nodes)
+            if W_tgt is not None:
+                d_h = d_h + scatter_sum(C.linear(part, W_tgt[t].t().contiguous()), tgt, dim=0, dim_size=num_nodes)
+    if dense and E > 0:
+        # d h_src[u] = sum over edges (u -> v, type t) of W_t^T d_agg[v]: the forward's aggregation on the transposed graph
+        rplan = plan_for([(tgt, src) for src, tgt in adj], num_nodes)
+        d_h = _add_aggregate(d_h, rplan, d_agg, [w.t().contiguous() for w in W], scale)
+        if W_tgt is not None:      # d h_tgt: every edge sends W_tgt^T d_agg[v] to its own target v
+            tplan = plan_for([(tgt, tgt) for _src, tgt in adj], num_nodes)
+            d_h = _add_aggregate(d_h, tplan, d_agg, [w.t().contiguous() for w in W_tgt], scale)
     return d_W, d_h
 
 
@@ -281,19 +282,12 @@ class _EgcLayerFunction(torch.autograd.Function):
         prod = torch.empty(num_nodes, out, bases, dtype=torch.float32, device=h.device)       # G[n, o] A[n, r(o, b)], node-sized
         d_h = torch.zeros_like(h)
         d_slabs = [[] for _ in W]
-        with _exact_fp16_gemms():
-            b_all = _split16(h, plan.src32)                              # the gathered source states, once for every slab
+        b_all = _split16(h, plan.src32)                                  # the gathered source states, once for every slab
         for s in range(bases * out // 128):
             rows = egc_slab_rows(s, out, heads, bases, h.device)
             Ws = [wt.index_select(0, rows) for wt in W]                 # [128, H]: the slab's rows, in slab order
             # 2. the slab's aggregate A_s [N, 128] (and, for max / min, which edge won each (target, feature))
-            arg = None
-            if reduce_name in ("max", "min"):
-                msg = C.edge_messages(plan, h, None, Ws, False)
-                agg, arg = C.segment_reduce(msg, plan, N.REDUCE[reduce_name], return_arg=True)
-                del msg
-            else:
-                agg = C.aggregate(plan, h, Ws, N.REDUCE[reduce_name])
+            agg, arg = _recompute_aggregate(plan, h, Ws, reduce_name)
             # 3. node-side terms: the slab's columns o = s per + j, their heads and coefficient rows
             cols = slice(s * per, (s + 1) * per)
             hd = torch.arange(s * per, (s + 1) * per, device=h.device) // dh
@@ -309,8 +303,7 @@ class _EgcLayerFunction(torch.autograd.Function):
         d_W = [torch.cat(ds, dim=0).index_select(0, inv) for ds in d_slabs]
         # 6. the coefficient Linear
         d_w = prod.view(num_nodes, heads, dh, bases).sum(dim=2).reshape(num_nodes, heads * bases)
-        with _exact_fp16_gemms():
-            d_cw = _mm_t_split(_split16(d_w), _split16(h))
+        d_cw = _mm_t_split(_split16(d_w), _split16(h))
         d_h = d_h + C.linear(d_w.contiguous(), cw.t().contiguous())
         return (None, None, None, None, d_h, d_cw, d_w.sum(dim=0), *d_W)
 
@@ -359,7 +352,6 @@ class _MlpLayerFunction(torch.autograd.Function):
         num_nodes, H = h.shape
         W = [w.detach().contiguous() for w in weights]
         plan = plan_for(adj, num_nodes)
-        E = plan.num_edges
 
         # ---- 1. re-compute the aggregate on the native kernels (PNA: with its arg ids; the messages are kept for its backward)
         msg = C.edge_messages(plan, h, h if use_target else None, W, use_target)
@@ -385,61 +377,16 @@ class _MlpLayerFunction(torch.autograd.Function):
         it = iter(grads[1:])
         d_tail = [next(it) if p.requires_grad else None for p in tail_params]
 
-        # ---- 3. aggregation + per-type Linear backward
-        d_h = torch.zeros_like(h)
-        d_W = []
+        # ---- 3. aggregation + per-type Linear backward (PNA: from the per-edge message gradients of its own backward)
+        d_msg = None
+        if pna is not None:
+            from .aggregation import native_pna_backward
+
+            d_msg = native_pna_backward(msg, plan, pna.delta, agg, arg_max, arg_min, d_agg)
+            del msg
         Ws = [w[:, :H].contiguous() for w in W]                              # columns multiplying h_src
         Wg = [w[:, H:].contiguous() for w in W] if use_target else None      # columns multiplying h_tgt
-        if pna is None and reduce_name in ("sum", "mean"):
-            if reduce_name == "mean":
-                cnt = (plan.row_ptr[1:] - plan.row_ptr[:-1]).clamp(min=1).to(torch.float32)
-                d_agg = (d_agg / cnt[:, None]).contiguous()
-            scale = _pow2_scale(d_agg)
-            with _exact_fp16_gemms():
-                a_all, b_all = _split16(d_agg, plan.tgt32, scale), _split16(h, plan.src32)
-                g_all = _split16(h, plan.tgt32) if use_target else None
-                for t, w in enumerate(W):
-                    lo_, hi_ = plan.type_off[t], plan.type_off[t + 1]
-                    if hi_ == lo_:
-                        d_W.append(torch.zeros_like(w))
-                        continue
-                    a = _slice(a_all, lo_, hi_)
-                    d_w = _mm_t_split(a, _slice(b_all, lo_, hi_))                                  # [D, H]: columns multiplying h_src
-                    d_W.append(torch.cat([d_w, _mm_t_split(a, _slice(g_all, lo_, hi_))], dim=1) if use_target else d_w)
-            if E > 0:
-                rplan = plan_for([(tgt, src) for src, tgt in adj], num_nodes)                     # transposed graph: d h_src
-                d_h = _add_aggregate(d_h, rplan, d_agg, [w.t().contiguous() for w in Ws], scale)
-                if use_target:                                                                     # d h_tgt: every edge sends W_g^T d_agg[v] to its own target v
-                    tplan = plan_for([(tgt, tgt) for _src, tgt in adj], num_nodes)
-                    d_h = _add_aggregate(d_h, tplan, d_agg, [w.t().contiguous() for w in Wg], scale)
-        else:
-            # per-edge message gradients: routed to the winning edges (max / min), or the PNA backward
-            if pna is not None:
-                from .aggregation import native_pna_backward
-
-                d_msg = native_pna_backward(msg, plan, pna.delta, agg, arg_max, arg_min, d_agg)
-                del msg
-            else:
-                d_msg = torch.zeros(E + 1, d_agg.shape[1], dtype=torch.float32, device=h.device)
-                d_msg = d_msg.scatter_(0, arg, d_agg)[:E]
-            with _exact_fp16_gemms():
-                a_all, b_all = _split16(d_msg), _split16(h, plan.src32)
-                g_all = _split16(h, plan.tgt32) if use_target else None
-            lo = 0
-            for t, ((src, tgt), w) in enumerate(zip(adj, W)):
-                e_t = src.numel()
-                part = d_msg[lo:lo + e_t].contiguous()
-                lo += e_t
-                if e_t == 0:
-                    d_W.append(torch.zeros_like(w))
-                    continue
-                with _exact_fp16_gemms():
-                    a = _slice(a_all, lo - e_t, lo)
-                    d_w = _mm_t_split(a, _slice(b_all, lo - e_t, lo))
-                    d_W.append(torch.cat([d_w, _mm_t_split(a, _slice(g_all, lo - e_t, lo))], dim=1) if use_target else d_w)
-                d_h = d_h + scatter_sum(C.linear(part, Ws[t].t().contiguous()), src, dim=0, dim_size=num_nodes)
-                if use_target:
-                    d_h = d_h + scatter_sum(C.linear(part, Wg[t].t().contiguous()), tgt, dim=0, dim_size=num_nodes)
+        d_W, d_h = _aggregation_backward(plan, adj, h, Ws, d_agg, reduce_name, arg, torch.zeros_like(h), W_tgt=Wg, d_msg=d_msg)
         return (None, None, None, None, None, None, d_h, *d_tail, *d_W)
 
 
@@ -472,8 +419,7 @@ class _LinearFn(torch.autograd.Function):
     def backward(ctx, g):
         x, weight = ctx.saved_tensors
         g = g.contiguous()
-        with _exact_fp16_gemms():
-            d_w = _mm_t_split(_split16(g), _split16(x.detach()))
+        d_w = _mm_t_split(_split16(g), _split16(x.detach()))
         return C.linear(g, weight.detach().t().contiguous()), d_w, (g.sum(dim=0) if ctx.has_bias else None)
 
 
@@ -496,15 +442,11 @@ class _SegmentReduceFn(torch.autograd.Function):
     def backward(ctx, g):
         plan, reduce_name = ctx.plan, ctx.reduce_name
         g = g.contiguous()
-        E = plan.num_edges
         if reduce_name in ("max", "min"):
             (arg,) = ctx.saved_tensors
-            d_msg = torch.zeros(E + 1, g.shape[1], dtype=g.dtype, device=g.device)
-            d_msg.scatter_(0, arg, g)
-            return d_msg[:E], None, None
+            return _route_to_arg(g, arg, plan.num_edges), None, None
         if reduce_name == "mean":
-            cnt = (plan.row_ptr[1:] - plan.row_ptr[:-1]).clamp(min=1).to(g.dtype)
-            g = g / cnt[:, None]
+            g = g / _mean_divisor(plan)[:, None]
         return g.index_select(0, plan.tgt32.long()), None, None
 
 
@@ -571,16 +513,12 @@ class _GraphReadoutFn(torch.autograd.Function):
         d_g = d_g.contiguous()
         if kind in ("max", "min"):
             (arg,) = ctx.saved_tensors
-            num_nodes = plan.num_edges
-            d_x = torch.zeros(num_nodes + 1, d_g.shape[1], dtype=d_g.dtype, device=d_g.device)   # row N takes the empty graphs' sentinel
-            d_x.scatter_(0, arg, d_g)                                                            # one graph per node: no collisions
-            return None, None, None, d_x[:num_nodes], None
+            return None, None, None, _route_to_arg(d_g, arg, plan.num_edges), None      # the plan's edges are the nodes
         x, s, w = ctx.saved_tensors
         gid = plan.tgt32.long()
         d_gn = d_g.index_select(0, gid)                                  # [N, H]: the gradient of each node's graph
         if kind == "mean":
-            cnt = (plan.row_ptr[1:] - plan.row_ptr[:-1]).clamp(min=1).to(torch.float32)
-            return None, None, None, d_gn / cnt.index_select(0, gid)[:, None], None
+            return None, None, None, d_gn / _mean_divisor(plan).index_select(0, gid)[:, None], None
         if kind == "sum":
             return None, None, None, d_gn, None
         # weighted sum: d x_n = s_n d g_b + s_n (1 - s_n) (x_n . d g_b) w ;  d w = sum_n s_n (1 - s_n) (x_n . d g_b) x_n
@@ -610,17 +548,10 @@ class _GlobalGruFn(torch.autograd.Function):
         h, g, w_ih, w_hh, b_ih, b_hh = (t.detach().contiguous() for t in ctx.saved_tensors)
         plan = ctx.plan
         gi = C.linear(g, w_ih, b_ih).index_select(0, plan.tgt32.long())     # the [G, 3H] table, gathered per node
-        gh = C.linear(h, w_hh, b_hh)
-        d_gi, d_gh, d_h = torch.empty_like(gi), torch.empty_like(gh), torch.empty_like(h)
-        with torch.cuda.device(h.device):
-            rc = N.lib().ptgnn_b200_gru_gate_grads_f32(N.ptr(gi), N.ptr(gh), N.ptr(h), N.ptr(grad_out.contiguous()), h.shape[0], h.shape[1],
-                                                      N.ptr(d_gi), N.ptr(d_gh), N.ptr(d_h), N.current_stream(h.device))
-        N.check(rc, "ptgnn_b200_gru_gate_grads_f32")
-        d_h = d_h + C.linear(d_gh, w_hh.t().contiguous())
+        d_gi, d_gh, d_h = _gru_gate_grads(grad_out.contiguous(), gi, C.linear(h, w_hh, b_hh), h, w_hh)
         d_table = C.segment_reduce(d_gi, plan, N.REDUCE["sum"])             # [G, 3H]: per graph, in node order
         d_g = C.linear(d_table, w_ih.t().contiguous())                      # [G, S]
-        with _exact_fp16_gemms():
-            d_w_hh = _mm_t_split(_split16(d_gh), _split16(h))
+        d_w_hh = _mm_t_split(_split16(d_gh), _split16(h))
         return None, None, d_h, d_g, d_table.t() @ g, d_w_hh, d_table.sum(dim=0), d_gh.sum(dim=0)
 
 
@@ -825,13 +756,11 @@ def _char_cnn_backward(d_out, chars, arg, prepared, shape, w2, w3):
         dl3.scatter_(1, arg[c0:c0 + Bc].long().unsqueeze(1), d_out[c0:c0 + Bc].unsqueeze(1))
         dl3 = dl3.view(Bc * L3, D)
         x3 = a2.view(Bc, L2, F2).unfold(1, k3, 1).reshape(Bc * L3, F2 * k3)
-        with _exact_fp16_gemms():
-            d_w3 += _mm_t_split(_split16(dl3), _split16(x3))
+        d_w3 += _mm_t_split(_split16(dl3), _split16(x3))
         dl2 = _col2im(C.linear(dl3, w3cat), Bc, L3, k3, F2, L2).mul_(a2.view(Bc, L2, F2) > 0).view(Bc * L2, F2)
         d_b2 += dl2.sum(dim=0)
         x2 = a1.view(Bc, L1, F1).unfold(1, k2, 1).reshape(Bc * L2, F1 * k2)
-        with _exact_fp16_gemms():
-            d_w2 += _mm_t_split(_split16(dl2), _split16(x2))
+        d_w2 += _mm_t_split(_split16(dl2), _split16(x2))
         dl1 = _col2im(C.linear(dl2, w2cat), Bc, L2, k2, F1, L1).mul_(a1.view(Bc, L1, F1) > 0).view(Bc * L1, F1)
         d_b1 += dl1.sum(dim=0)
         valid = (ch >= 0) & (ch < V)        # the kernel read an out-of-range id as character 0: so does its gradient
