@@ -119,3 +119,141 @@ def bound(x, n2g, gamma, alpha, bias, eps=1e-10, G=None):
     g_r = gamma.abs() * r[n2g]
     out = g_r * (alpha.abs() * E[n2g] + U * ((x - mu[n2g]).abs() + s.abs() + 2 * t[n2g].abs()) + s.abs() * er[n2g]) + 2 * U * (g_r * s).abs() + U * y.abs()
     return out * 1.01 + 1e-30
+
+
+def gamma_n(n):
+    """gamma_n = n u / (1 - n u): the relative error bound of n roundings (tensor or number)."""
+    return n * U / (1 - n * U)
+
+
+def _bwd_inputs(x, dy, n2g, mean, rstd, gamma, alpha, eps, G):
+    G = int(n2g.max()) + 1 if G is None else G
+    x, dy = x.double(), dy.double()
+    D = x.shape[1]
+    gamma, alpha = (p.double().reshape(1, D) for p in (gamma, alpha))
+    counts = torch.bincount(n2g, minlength=G)
+    return x, dy, mean.double(), rstd.double(), gamma, alpha, float(torch.tensor(eps, dtype=torch.float32)), counts, G, D
+
+
+def backward_formula(x, dy, n2g, mean, rstd, gamma, alpha, eps=1e-10, G=None):
+    """(dx [N, D], d gamma [D], d alpha [D], d beta [D]) in float64 from exactly the kernels' inputs: x, dy, the forward's mean and
+    rstd [G, D], gamma, alpha and eps as float32 (the kernel receives eps as a float).  Per graph and column, with x^ = s rstd,
+    s = (x - mu) + (1 - alpha) mu, k = gamma rstd, A = sum dy, B = sum dy x^ and n rows:
+        dL/ds_i = k (dy_i - x^_i B / n),   S = sum_i dL/ds_i = k (A - (1 - alpha) mu rstd B),   dx_i = dL/ds_i - alpha S / n
+    and for a one-node graph, where 1 - x^2 = eps rstd^2 exactly: dL/ds = k eps rstd^2 dy, S = k eps rstd^2 A, dx = (1 - alpha) dL/ds.
+    d gamma = sum_g B, d beta = sum_g A, d alpha = -sum_g mu S.  With the exact float64 mean and rstd this is the gradient."""
+    x, dy, mu, r, gamma, alpha, eps, counts, G, D = _bwd_inputs(x, dy, n2g, mean, rstd, gamma, alpha, eps, G)
+    s = (x - mu[n2g]) + (1.0 - alpha) * mu[n2g]
+    xh = s * r[n2g]
+    A = torch.zeros(G, D, dtype=torch.float64).index_add(0, n2g, dy)
+    B = torch.zeros(G, D, dtype=torch.float64).index_add(0, n2g, dy * xh)
+    n = counts.double().clamp(min=1)[:, None]
+    k = gamma * r
+    one = (counts == 1)[:, None]
+    ke = k * eps * r * r
+    S = torch.where(one, ke * A, k * (A - (1.0 - alpha) * mu * r * B))
+    dls = torch.where(one[n2g], ke[n2g] * dy, k[n2g] * (dy - xh * (B / n)[n2g]))
+    dx = dls - (alpha * S / n)[n2g]
+    return dx, B.sum(0), -(mu * S).sum(0), A.sum(0)
+
+
+def backward_bound(x, dy, n2g, mean, rstd, gamma, alpha, eps=1e-10, G=None):
+    """Per-element bounds (dx [N, D], d gamma, d alpha, d beta [D]) on |kernel - backward_formula| for the fp32 backward (DESIGN.md
+    §4), in float64, from the §3.9 order.  Every term is a sum of absolute values, so cancellation in dy - x^ c1, in A - P B or in
+    1 - x^2 is covered.  With u = 2^-24, gamma_n = n u / (1 - n u), k chunks in the graph and t = (1 - alpha) mu, P = t rstd:
+        x^     e_x = rstd (u |x - mu| + u |s| + 3u |t|) + u |x^|           (x - mu, t's two roundings, + t, * rstd)
+        A      e_A = gamma_{32+k} sum |dy|                                 (the chunk's chain of <= 32 rows, then k chunk additions)
+        B      e_B = sum |dy| e_x + gamma_{33+k} sum |dy x^|               (the product, then the same chains)
+        S      e_S = |k| (e_A + |P| e_B + 4u |P B| + u (|A| + |P B|)) + 2u |k (A - P B)|   (P: 3 roundings, P B and the difference
+                                                                                  one each; k = gamma rstd and k (A - P B) one each)
+        c1     e_1 = (e_B + u |B|) / n,   c2  e_2 = (|alpha| e_S + 2u |alpha S|) / n
+        dx     |d| <= |k| (|x^| e_1 + |c1| e_x + u |x^ c1| + u (|dy| + |x^ c1|)) + u |k| |dy - x^ c1| + u |k (dy - x^ c1)| + e_2
+                      + u (|k (dy - x^ c1)| + |c2|)
+    A one-node graph (1 - x^2 = eps rstd^2, no c1 or c2): k' = k eps rstd^2 (1 - alpha) carries 6 roundings, so
+        dx  |d| <= 7u |k' dy|,   S  e_S = |k eps rstd^2| (e_A + 5u |A|)
+    The parameter sums over G graphs in order: d beta  sum_g e_A + gamma_G sum_g |A|,  d gamma  sum_g e_B + gamma_G sum_g |B|,
+    d alpha  sum_g (|mu| e_S + u |mu S|) + gamma_G sum_g |mu S|.  Second-order terms: 1 % slack, plus 1e-37 absolute."""
+    x, dy, mu, r, gamma, alpha, eps, counts, G, D = _bwd_inputs(x, dy, n2g, mean, rstd, gamma, alpha, eps, G)
+    mun, rn = mu[n2g], r[n2g]
+    t = (1.0 - alpha) * mu
+    s = (x - mun) + t[n2g]
+    xh = s * rn
+    e_x = rn * (U * (x - mun).abs() + U * s.abs() + 3 * U * t[n2g].abs()) + U * xh.abs()
+    chunks = ((counts + CHUNK - 1) // CHUNK).double()[:, None]
+    gsum = lambda v: torch.zeros(G, D, dtype=torch.float64).index_add(0, n2g, v)  # noqa: E731
+    A, B = gsum(dy), gsum(dy * xh)
+    e_A = gamma_n(32 + chunks) * gsum(dy.abs())
+    e_B = gsum(dy.abs() * e_x) + gamma_n(33 + chunks) * gsum((dy * xh).abs())
+    k = gamma * r
+    P = t * r
+    W = A - P * B
+    e_S = k.abs() * (e_A + P.abs() * e_B + 4 * U * (P * B).abs() + U * (A.abs() + (P * B).abs())) + 2 * U * (k * W).abs()
+    S = k * W
+    n = counts.double().clamp(min=1)[:, None]
+    c1 = B / n
+    e_1 = (e_B + U * B.abs()) / n
+    e_2 = (alpha.abs() * e_S + 2 * U * (alpha * S).abs()) / n
+    kn, c1n = k[n2g], c1[n2g]
+    d1 = dy - xh * c1n
+    b_dx = (kn.abs() * (xh.abs() * e_1[n2g] + c1n.abs() * e_x + U * (xh * c1n).abs() + U * (dy.abs() + (xh * c1n).abs()))
+            + 2 * U * (kn * d1).abs() + e_2[n2g] + U * ((kn * d1).abs() + (alpha * S / n)[n2g].abs()))
+    one = (counts == 1)[:, None]
+    ke = k * eps * r * r
+    b_dx = torch.where(one[n2g], 7 * U * ((ke * (1.0 - alpha))[n2g] * dy).abs(), b_dx)
+    e_S = torch.where(one, ke.abs() * (e_A + 5 * U * A.abs()), e_S)
+    S = torch.where(one, ke * A, S)
+    gG = gamma_n(G)
+    b_gamma = e_B.sum(0) + gG * B.abs().sum(0)
+    b_beta = e_A.sum(0) + gG * A.abs().sum(0)
+    b_alpha = (mu.abs() * e_S + U * (mu * S).abs()).sum(0) + gG * (mu * S).abs().sum(0)
+    return tuple(b * 1.01 + 1e-37 for b in (b_dx, b_gamma, b_alpha, b_beta))
+
+
+def emulate_backward(x, dy, n2g, mean, rstd, gamma, alpha, eps=1e-10, G=None, mutant=None):
+    """(dx [N, D], d gamma [D], d alpha [D], d beta [D]) by the backward kernels' float32 operations in their order (DESIGN.md §3.9),
+    bit for bit: A_c, B_c over each chunk's rows in node order, the chunk sums in chunk order from 0, k, c1, c2 and S per graph (the
+    one-node branch included), dx, and the parameter sums over the graphs in order from 0.  ``mutant`` (the bound must reject each):
+    "no_one_node_branch" runs the general formula on one-node graphs, "c2_without_alpha" drops alpha from c2."""
+    G = int(n2g.max()) + 1 if G is None else G
+    x32, dy32 = x.float(), dy.float()
+    D = x32.shape[1]
+    gamma, alpha = (p.float().reshape(1, D) for p in (gamma, alpha))
+    mu, r = mean.float(), rstd.float()
+    eps32 = torch.tensor(eps, dtype=torch.float32)
+    order, counts, cs, cl, cg, cj = chunks(n2g, G)
+    t = (1.0 - alpha) * mu
+    xh = ((x32 - mu[n2g]) + t[n2g]) * r[n2g]
+    xs, gs, hs = x32[order], dy32[order], xh[order]
+    C = cs.numel()
+    Ac, Bc = torch.zeros(C, D), torch.zeros(C, D)
+    for i in range(CHUNK):
+        m = cl > i
+        Ac[m] = Ac[m] + gs[cs[m] + i]
+        Bc[m] = Bc[m] + gs[cs[m] + i] * hs[cs[m] + i]
+    A, B = torch.zeros(G, D), torch.zeros(G, D)
+    for j in range(int(cj.max()) + 1 if C else 0):
+        sel = cj == j
+        A[cg[sel]] = A[cg[sel]] + Ac[sel]
+        B[cg[sel]] = B[cg[sel]] + Bc[sel]
+    k = gamma * r
+    S = k * (A - (t * r) * B)
+    n = counts.float()[:, None]
+    has = counts[:, None] > 0
+    c1 = torch.where(has, B / n.clamp(min=1), torch.zeros(()))
+    aS = S if mutant == "c2_without_alpha" else alpha * S
+    c2 = torch.where(has, aS / n.clamp(min=1), torch.zeros(()))
+    coef_k = k
+    if mutant != "no_one_node_branch":
+        one = (counts == 1)[:, None]
+        ke = k * (eps32 * (r * r))
+        coef_k = torch.where(one, ke * (1.0 - alpha), k)
+        c1 = torch.where(one, torch.zeros(()), c1)
+        c2 = torch.where(one, torch.zeros(()), c2)
+        S = torch.where(one, ke * A, S)
+    dx = coef_k[n2g] * (dy32 - xh * c1[n2g]) - c2[n2g]
+    sg, sb, sa = torch.zeros(D), torch.zeros(D), torch.zeros(D)
+    for b in range(G):
+        sb = sb + A[b]
+        sg = sg + B[b]
+        sa = sa + mu[b] * S[b]
+    return dx, sg, -sa, sb

@@ -1,7 +1,8 @@
 """Attention reducers on the GPU: the attention readout kernel against float64 with per-element bounds, the reducer modules against
 the float64 restatement and the reference's fixtures, bf16 against the reference's autocast fixture, no host synchronisation, peak
-memory at graph2seq's shape, and training against torch.autograd through the float64 restatement.  Every case runs twice and must
-be bit-identical.
+memory at graph2seq's shape, and training against torch.autograd through the float64 restatement.  The kernel's backward
+(native_attention_readout_backward) against float64 under attention_readout_reference.kernel_backward_bound, with
+backward(2^k dO) = 2^k backward(dO).  Every case runs twice and must be bit-identical.
 
 Kernel bound (DESIGN.md §3.7 gives the order).  With u = 2^-24 and gamma_k = k u / (1 - k u):
 * a logit z is a per-lane fmaf chain over D / 32 features and a five-level butterfly: |dz| <= eps = gamma_{D/32+5} sum_f |x_f qt_f|.
@@ -461,3 +462,91 @@ def test_global_gru_update_with_native_multihead_reducer_trains():
     _grads_close(hd.grad, h64.grad, "d h")
     for name, param in layer.named_parameters():
         _grads_close(param.grad, sd[name].grad, f"d {name}")
+
+
+# ---- the kernel's backward, element by element ---------------------------------------------------------------------------------
+SCALES = (-37, -27, -17, 17)        # the gradient magnitudes of test_gpu_backward_edges.py: backward(2^k dO) = 2^k backward(dO)
+BWD_PAIRS = [(D, heads) for D in (32, 64, 128, 256) for heads in (1, 2, 4, 8)]
+
+
+def _check_backward(x, n2g, G, qt, heads, what, scales=SCALES):
+    """native_attention_readout_backward twice (bit-identical) on the forward kernel's o and lse, against kernel_backward_formula
+    under kernel_backward_bound (float64 on the GPU), and backward(2^k dO) = 2^k backward(dO) bit for bit for k in ``scales``."""
+    from ptgnn_b200.reduceops import graph_plan, native_attention_readout, native_attention_readout_backward
+
+    x, n2g, qt = x.cuda(), n2g.cuda(), qt.cuda()
+    plan = graph_plan(n2g, G)
+    o, lse = native_attention_readout(x, plan, qt, heads)
+    d_o = torch.randn(G, heads, x.shape[1], generator=torch.Generator(device="cuda").manual_seed(G + heads), device="cuda")
+    runs = [native_attention_readout_backward(x, plan, qt, o, lse, d_o) for _ in range(2)]
+    plan.validate()
+    assert all(torch.equal(a, b) for a, b in zip(*runs)), f"{what}: two backward runs differ"
+    ref = AR.kernel_backward_formula(x, qt, o, lse, d_o, n2g, G)
+    bnd = AR.kernel_backward_bound(x, qt, o, lse, d_o, n2g, G)
+    for name, g, r, b in zip(("dx", "d qt"), runs[0], ref, bnd):
+        err = (g.double() - r).abs()
+        bad = int((err > b).sum())
+        assert bad == 0, f"{what} {name}: {bad} elements over the bound (worst ratio {float((err / b).max()):.2f})"
+    for k in scales:
+        scaled = native_attention_readout_backward(x, plan, qt, o, lse, d_o * 2.0 ** k)
+        assert all(torch.equal(s, g * 2.0 ** k) for s, g in zip(scaled, runs[0])), f"{what}: backward(2^{k} dO) != 2^{k} backward(dO)"
+    return runs[0]
+
+
+@pytest.mark.parametrize("D,heads", BWD_PAIRS)
+@pytest.mark.parametrize("layout", ["sizes", "one_big", "config2", "unsorted_gaps"])
+def test_kernel_backward_against_float64(layout, D, heads):
+    gen = torch.Generator().manual_seed(len(layout) * 1000 + D + heads + 1)
+    n2g, G = _n2g_layout(layout, gen)
+    x = torch.randn(n2g.shape[0], D, generator=gen) * 0.5
+    qt = torch.randn(G, heads, D, generator=gen) * (4.0 / D ** 0.5)
+    _check_backward(x, n2g, G, qt, heads, f"{layout} D={D} heads={heads}")
+
+
+@pytest.mark.parametrize("D,heads", [(32, 2), (256, 8)])
+@pytest.mark.parametrize("layout", ["one_graph_300k", "12000x30"])
+def test_kernel_backward_more_chunks_than_resident_warps(layout, D, heads):
+    """More chunks than the 64 warps per SM the backward's grid holds, so warps walk several chunks: of one graph (the cached qt, dO
+    and delta reused) or of consecutive graphs (reloaded when the graph changes)."""
+    gen = torch.Generator().manual_seed(D + heads)
+    if layout == "one_graph_300k":
+        n2g, G = torch.zeros(300_000, dtype=torch.int64), 1
+    else:
+        n2g, G = torch.randperm(12_000 * 30, generator=gen) % 12_000, 12_000
+    chunks = int(torch.ceil(torch.bincount(n2g, minlength=G) / CHUNK).sum())
+    resident = 64 * torch.cuda.get_device_properties(0).multi_processor_count
+    assert chunks > resident, f"{layout}: {chunks} chunks do not exceed {resident} resident warps"
+    x = torch.randn(n2g.shape[0], D, generator=gen) * 0.5
+    qt = torch.randn(G, heads, D, generator=gen) * (4.0 / D ** 0.5)
+    _check_backward(x, n2g, G, qt, heads, f"{layout} D={D} heads={heads}")
+
+
+@pytest.mark.parametrize("heads", [1, 4, 8])
+def test_kernel_backward_logit_extremes(heads):
+    """The forward test's logits in [-100, 100] with every graph's maximum in its last row: p down to e^-200 (the bound alone, scaled
+    products can be subnormal)."""
+    D = 64
+    gen = torch.Generator().manual_seed(heads)
+    n2g, G = _n2g_layout("sizes", gen)
+    x = torch.randn(n2g.shape[0], D, generator=gen) * 0.5
+    qt = torch.zeros(G, heads, D)
+    for h in range(heads):
+        qt[:, h, h] = 1.0
+    x[:, :heads] = torch.rand(n2g.shape[0], heads, generator=gen) * 200 - 100
+    x[torch.cumsum(torch.bincount(n2g, minlength=G), 0) - 1, :heads] = 100.0
+    _check_backward(x, n2g, G, qt, heads, f"extreme heads={heads}", scales=())
+
+
+def test_kernel_backward_without_nodes_gives_zero():
+    from ptgnn_b200.reduceops import graph_plan, native_attention_readout_backward
+
+    G, heads, D = 3, 2, 64
+    plan = graph_plan(torch.zeros(0, dtype=torch.int64, device="cuda"), G)
+    x = torch.zeros(0, D, device="cuda")
+    qt, o, d_o = (torch.randn(G, heads, D, device="cuda") for _ in range(3))
+    d_x, d_qt = native_attention_readout_backward(x, plan, qt, o, torch.full((G, heads), -math.inf, device="cuda"), d_o)
+    assert d_x.shape == (0, D) and torch.equal(d_qt, torch.zeros_like(d_qt)), "no node: d qt must be exactly 0"
+
+
+def test_kernel_backward_parametrisation_reaches_every_instance():
+    assert len(set(BWD_PAIRS)) == 16, "attn_readout_backward_chunk_kernel<VPL, HEADS>: 16 instances"

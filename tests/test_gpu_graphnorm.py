@@ -1,7 +1,8 @@
 """GraphNorm on the GPU: the kernels against the float32 emulation of their order bit for bit and against float64 element by element
 under the bound of DESIGN.md §4 (graphnorm_reference.bound), the layer against the reference's fixtures, bf16 under the bf16 rule,
 gradients against torch.autograd through the float64 restatement, run-to-run identity, no host synchronisation with the graph count
-handed in, CUDA-graph capture inside a container, and the unsupported cases."""
+handed in, CUDA-graph capture inside a container, the unsupported cases, and the backward kernels (native_graph_norm_backward) against
+emulate_backward bit for bit and against float64 under graphnorm_reference.backward_bound, with backward(2^k dy) = 2^k backward(dy)."""
 import os
 
 import numpy as np
@@ -243,3 +244,62 @@ def test_unsupported_cases_raise():
                 P.GraphNorm(D).cuda()(torch.randn(10, D, device="cuda"), [], n2g, {}, {}, [])
     with torch.no_grad():       # bf16 without gradients runs
         assert P.GraphNorm(32).cuda()(x.bfloat16(), [], n2g, {}, {}, []).dtype == torch.bfloat16
+
+
+# ---- backward kernels, element by element ------------------------------------------------------------------------------------
+SCALES = (-37, -27, -17, 17)        # the gradient magnitudes of test_gpu_backward_edges.py: backward(2^k dy) = 2^k backward(dy)
+EDGE_COUNTS = [1, 31, 32, 33, 0, 64, 65, 1000, 1]      # the forward's edge sizes; graphs 2 and 6 get all-equal rows
+BWD_SHAPES = {f"edges_d{D}_a{a}": (EDGE_COUNTS, D, True, a) for D in range(32, 257, 32) for a in (0.0, 0.5, 1.0, 1.7)}
+BWD_SHAPES.update({name: (counts, D, shuffle, None) for name, (counts, D, shuffle) in SHAPES.items()})
+
+
+def backward_kernel(x, dy, n2g, G, gamma, alpha, mean, rstd):
+    """Two runs of native_graph_norm_backward, which must agree bit for bit: (dx, d gamma, d alpha, d beta) on the CPU."""
+    from ptgnn_b200.graphnorm import native_graph_norm_backward
+    from ptgnn_b200.reduceops import graph_plan
+
+    plan = graph_plan(n2g, G)
+    runs = [native_graph_norm_backward(x, plan, gamma.cuda(), alpha.cuda(), 1e-10, mean, rstd, dy) for _ in range(2)]
+    plan.validate()
+    assert all(torch.equal(a, b) for a, b in zip(*runs)), "two backward runs differ"
+    return [t.cpu() for t in runs[0]]
+
+
+@pytest.mark.parametrize("shape", list(BWD_SHAPES))
+def test_backward_kernels_against_emulation_and_float64(shape):
+    """The backward kernels equal emulate_backward bit for bit and backward_formula within backward_bound, on the forward kernels'
+    mean and rstd; backward(2^k dy) = 2^k backward(dy) bit for bit."""
+    counts, D, shuffle, a = BWD_SHAPES[shape]
+    n2g = graph_map(counts, shuffle, D + len(counts) + 1)
+    G = len(counts)
+    gen = torch.Generator().manual_seed(len(counts) * 11 + D)
+    x = torch.randn(n2g.numel(), D, generator=gen) * 2.0 + torch.randn(G, D, generator=gen)[n2g] * 3.0
+    if counts is EDGE_COUNTS:
+        for g in (2, 6):
+            x[n2g == g] = torch.randn(D, generator=gen) * 3.0
+    dy = torch.randn(n2g.numel(), D, generator=gen)
+    gamma, alpha, bias = params(D, D + 1)
+    if a is not None:
+        alpha = torch.full((1, D), a)
+    xd, dyd, n2gd = x.cuda(), dy.cuda(), n2g.cuda()
+    _, mean, rstd = GR.emulate_forward(x, n2g, gamma, alpha, bias, G=G)
+    _, kmean, krstd = kernel(xd, n2gd, G, gamma, alpha, bias)
+    assert torch.equal(kmean, mean) and torch.equal(krstd, rstd)
+    got = backward_kernel(xd, dyd, n2gd, G, gamma, alpha, kmean.cuda(), krstd.cuda())
+    emu = GR.emulate_backward(x, dy, n2g, mean, rstd, gamma, alpha, G=G)
+    names = ("dx", "d gamma", "d alpha", "d beta")
+    for name, g, e in zip(names, got, emu):
+        assert torch.equal(g, e), f"{shape} {name}: differs from the emulated kernel order ({int((g != e).sum())} elements)"
+    ref = GR.backward_formula(x, dy, n2g, mean, rstd, gamma, alpha, G=G)
+    bnd = GR.backward_bound(x, dy, n2g, mean, rstd, gamma, alpha, G=G)
+    for name, g, r, b in zip(names, got, ref, bnd):
+        bad = int(((g.double() - r).abs() > b).sum())
+        assert bad == 0, f"{shape} {name}: {bad} elements over the bound (worst ratio {float(((g.double() - r).abs() / b).max()):.2f})"
+    for k in SCALES:
+        scaled = backward_kernel(xd, dyd * 2.0 ** k, n2gd, G, gamma, alpha, kmean.cuda(), krstd.cuda())
+        for name, g, s in zip(names, got, scaled):
+            assert torch.equal(s, g * 2.0 ** k), f"{shape} {name}: backward(2^{k} dy) != 2^{k} backward(dy)"
+
+
+def test_backward_shapes_reach_every_vpl_instance():
+    assert sorted({D // 32 for _, D, _, _ in BWD_SHAPES.values()}) == list(range(1, 9)), "graphnorm_bwd_chunk_kernel<VPL>: 8 instances"

@@ -1,7 +1,9 @@
 """MultiHeadSelfAttentionMessagePassing on the GPU: the chunked attention kernel against float64 element by element under the bound of
-DESIGN.md §4 (selfattention_reference.bound), the layer against the float64 restatement and the reference's fixtures, bf16 against
-the reference's autocast fixture, gradients against torch.autograd through the float64 restatement, run-to-run identity, no host
-synchronisation with the graph count handed in, CUDA-graph capture inside a container, and the unsupported cases."""
+DESIGN.md §4 (selfattention_reference.bound), the layer against the float64 restatement and the reference's fixtures, bf16 against the
+reference's autocast fixture, gradients against torch.autograd through the float64 restatement, run-to-run identity, no host
+synchronisation with the graph count handed in, CUDA-graph capture inside a container, the unsupported cases, and the backward kernels
+(native_selfatt_backward) against float64 element by element under selfattention_reference.backward_bound, with backward(2^k dO) = 2^k
+backward(dO)."""
 import os
 
 import numpy as np
@@ -240,3 +242,100 @@ def test_unsupported_cases_raise():
         P.MultiHeadSelfAttentionMessagePassing(32, 16, 16, 32, 64, 2).cuda().eval()(x, [], n2g, {}, {}, [], gather_states=x)
     with torch.no_grad():       # eval mode with p > 0 is the identity and runs
         P.MultiHeadSelfAttentionMessagePassing(32, 16, 16, 32, 64, 2, dropout_rate=0.1).cuda().eval()(x, [], n2g, {}, {}, [])
+
+
+# ---- backward kernels, element by element ------------------------------------------------------------------------------------
+SCALES = (-37, -27, -17, 17)        # the gradient magnitudes of test_gpu_backward_edges.py: backward(2^k dO) = 2^k backward(dO)
+PAIRS = [(dk, dv) for dk in (16, 32, 64, 128) for dv in (16, 32, 64, 128)]
+SIZES = [0, 1, 63, 64, 65, 250, 251, 1000]
+
+
+def bwd_map(kind, seed):
+    """(n2g, G): the sizes in graph order, or shuffled with an empty graph in between and two trailing empty graphs."""
+    if kind == "sorted":
+        return torch.repeat_interleave(torch.arange(len(SIZES)), torch.tensor(SIZES)), len(SIZES)
+    counts = SIZES[1:4] + [0] + SIZES[4:] + [0, 0]
+    n2g = torch.repeat_interleave(torch.arange(len(counts)), torch.tensor(counts))
+    return n2g[torch.randperm(n2g.numel(), generator=torch.Generator().manual_seed(seed))], len(counts)
+
+
+def check_backward(t, n2g, G, heads, dk, dv, L, what, scales=SCALES):
+    """native_selfatt_backward twice (bit-identical) on the forward kernel's o and lse, against backward_formula under backward_bound
+    (float64 on the GPU), and backward(2^k dO) = 2^k backward(dO) bit for bit for k in ``scales``.  Returns the worst err / bound."""
+    from ptgnn_b200.reduceops import graph_plan
+    from ptgnn_b200.selfattention import native_selfatt, native_selfatt_backward
+
+    t, n2g = t.cuda(), n2g.cuda()
+    plan = graph_plan(n2g, G)
+    o, lse = native_selfatt(t, plan, heads, dk, dv, L)
+    gen = torch.Generator(device="cuda").manual_seed(t.shape[0] + dk + dv + L)
+    d_o = torch.randn(t.shape[0], heads * dv, generator=gen, device="cuda")
+    runs = [native_selfatt_backward(t, plan, heads, dk, dv, L, o, lse, d_o) for _ in range(2)]
+    plan.validate()
+    assert torch.equal(runs[0], runs[1]), f"{what}: two backward runs differ"
+    got = runs[0]
+    ref = SR.backward_formula(t, o, lse, d_o, n2g.cpu(), heads, dk, L)
+    bnd = SR.backward_bound(t, o, lse, d_o, n2g.cpu(), heads, dk, L)
+    err = (got.double() - ref).abs()
+    bad = int((err > bnd).sum())
+    ratio = float((err / bnd).max())
+    assert bad == 0, f"{what}: {bad} elements over the bound (worst ratio {ratio:.2f})"
+    for k in scales:
+        assert torch.equal(native_selfatt_backward(t, plan, heads, dk, dv, L, o, lse, d_o * 2.0 ** k), got * 2.0 ** k), \
+            f"{what}: backward(2^{k} dO) != 2^{k} backward(dO)"
+    return ratio
+
+
+@pytest.mark.parametrize("kind", ["sorted", "unsorted"])
+@pytest.mark.parametrize("dk,dv", PAIRS)
+def test_backward_kernels_every_instance(dk, dv, kind):
+    n2g, G = bwd_map(kind, dk + dv)
+    t = torch.randn(n2g.numel(), 3 * (2 * dk + dv), generator=torch.Generator().manual_seed(dk * 7 + dv))
+    check_backward(t, n2g, G, 3, dk, dv, 250, f"dk={dk} dv={dv} {kind}")
+
+
+@pytest.mark.parametrize("kind", ["sorted", "unsorted"])
+@pytest.mark.parametrize("L", [1, 16, 63, 64, 65, 1000])
+def test_backward_kernels_chunk_lengths(L, kind):
+    """L = 1000 holds the largest graph in one chunk; 250 runs in test_backward_kernels_every_instance."""
+    n2g, G = bwd_map(kind, L)
+    t = torch.randn(n2g.numel(), 3 * (2 * 64 + 32), generator=torch.Generator().manual_seed(L))
+    check_backward(t, n2g, G, 3, 64, 32, L, f"L={L} {kind}")
+
+
+@pytest.mark.parametrize("L", [2, 250])
+def test_backward_kernels_more_graphs_than_one_scan_block(L):
+    """3,000 graphs of 0 to 5 rows: the tile scan (pergraph::item_ptr_kernel) carries its sum over three blocks of 1,024 graphs."""
+    gen = torch.Generator().manual_seed(L)
+    counts = torch.randint(0, 6, (3000,), generator=gen)
+    n2g = torch.repeat_interleave(torch.arange(3000), counts)
+    t = torch.randn(n2g.numel(), 3 * (2 * 16 + 16), generator=gen)
+    check_backward(t, n2g, 3000, 3, 16, 16, L, f"3,000 graphs L={L}")
+
+
+def test_backward_kernels_graph2seq_shape():
+    n2g = torch.repeat_interleave(torch.arange(80), 2560)        # 204,800 rows, 880 chunks of at most 250 rows, 8 heads
+    t = torch.randn(n2g.numel(), 8 * (2 * 16 + 16), generator=torch.Generator().manual_seed(80))
+    check_backward(t, n2g, 80, 8, 16, 16, 250, "80 x 2,560")
+
+
+@pytest.mark.parametrize("case", ["max_in_last_block", "all_equal"])
+def test_backward_kernels_logit_extremes(case):
+    """The forward test's logits: +-80 with the maximum in the chunk's last key block (p down to e^-160, below float32's range, so the
+    bound alone: scaled products can be subnormal), and all-equal logits."""
+    heads, dk, dv, L = 2, 16, 16, 250
+    n = 250 + 130
+    gen = torch.Generator().manual_seed(8)
+    t = torch.zeros(n, heads, 2 * dk + dv)
+    t[:, :, 2 * dk:] = torch.randn(n, heads, dv, generator=gen)
+    if case == "max_in_last_block":
+        t[:, :, 0] = 4.0
+        t[:, :, dk] = -80.0
+        t[249, :, dk] = 80.0
+        t[n - 1, :, dk] = 80.0
+    check_backward(t.reshape(n, -1), torch.zeros(n, dtype=torch.int64), 1, heads, dk, dv, L, case,
+                   scales=() if case == "max_in_last_block" else SCALES)
+
+
+def test_backward_parametrisation_reaches_every_instance():
+    assert len(set(PAIRS)) == 16, "selfatt_bwd_kv_kernel / selfatt_bwd_q_kernel<DK, DV>: 16 instances each"

@@ -142,3 +142,57 @@ print("ok")
 """
     r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300, cwd="/tmp")
     assert r.returncode == 0 and "ok" in r.stdout, r.stdout + r.stderr
+
+
+# ---- the attention readout kernel's backward ----------------------------------------------------------------------------------
+def _kernel_forward64(x, qt, n2g, G):
+    """float64 (o [G, heads, D], lse [G, heads]) of the kernel's operation: o[b, h] = sum_n softmax_n(x_n . qt[b, h]) x_n."""
+    heads = qt.shape[1]
+    z = (x[:, None, :] * qt[n2g]).sum(-1)                            # [N, heads]
+    p = torch.exp(AR.segment_log_softmax(z, n2g))
+    o = torch.zeros(G, heads, x.shape[1], dtype=x.dtype).index_add(0, n2g, p[:, :, None] * x[:, None, :])
+    lse = torch.stack([torch.logsumexp(z[n2g == b], 0) if bool((n2g == b).any()) else torch.full((heads,), -float("inf"), dtype=x.dtype)
+                       for b in range(G)])
+    return o, lse
+
+
+def _readout_case(D, heads, seed):
+    """A shuffled map with graphs of 1, 31, 32, 33 and 101 rows, an empty graph between them and a trailing one."""
+    gen = torch.Generator().manual_seed(seed)
+    counts = [1, 31, 0, 32, 33, 101, 0]
+    n2g = torch.repeat_interleave(torch.arange(len(counts)), torch.tensor(counts))
+    n2g = n2g[torch.randperm(n2g.numel(), generator=gen)]
+    G = len(counts)
+    x = torch.randn(n2g.numel(), D, generator=gen) * 0.5
+    qt = torch.randn(G, heads, D, generator=gen) * (4.0 / D ** 0.5)
+    return n2g, G, x, qt, torch.randn(G, heads, D, generator=gen)
+
+
+@pytest.mark.parametrize("D,heads", [(32, 1), (64, 2), (128, 4)])
+def test_kernel_backward_formula_equals_autograd_through_the_float64_forward(D, heads):
+    n2g, G, x, qt, d_o = _readout_case(D, heads, D + heads)
+    x64, q64 = x.double().requires_grad_(True), qt.double().requires_grad_(True)
+    o, lse = _kernel_forward64(x64, q64, n2g, G)
+    (o * d_o.double()).sum().backward()
+    dx, dq = AR.kernel_backward_formula(x64.detach(), q64.detach(), o.detach(), lse.detach(), d_o, n2g, G)
+    for name, got, ref in (("dx", dx, x64.grad), ("d qt", dq, q64.grad)):
+        err = float((got - ref).abs().max() / ref.abs().max())
+        assert err <= 1e-12, f"D={D} heads={heads} {name}: {err:.2e}"
+
+
+@pytest.mark.parametrize("D,heads", [(32, 2), (64, 1)])
+def test_kernel_backward_emulation_is_inside_the_bound_and_the_mutants_are_not(D, heads):
+    """The float32 emulation of the backward kernel's order (3 warps over 9 chunks: warps cross graphs), on the float32-rounded exact
+    o and lse, against kernel_backward_formula under kernel_backward_bound; each named mutant falls outside it."""
+    n2g, G, x, qt, d_o = _readout_case(D, heads, 7 * D + heads)
+    o, lse = (t.float() for t in _kernel_forward64(x.double(), qt.double(), n2g, G))
+    ref = AR.kernel_backward_formula(x, qt, o, lse, d_o, n2g, G)
+    bnd = AR.kernel_backward_bound(x, qt, o, lse, d_o, n2g, G)
+
+    def ratios(got):
+        return [float(((g.double() - r).abs() / b).max()) for g, r, b in zip(got, ref, bnd)]
+
+    worst = ratios(AR.emulate_kernel_backward(x, qt, o, lse, d_o, n2g, G))
+    assert max(worst) <= 1.0, f"emulated kernel order exceeds the bound (dx, d qt: {worst})"
+    for m in ("no_ds_qt", "stale_delta", "stale_qt", "drop_last_dq"):
+        assert max(ratios(AR.emulate_kernel_backward(x, qt, o, lse, d_o, n2g, G, mutant=m))) > 1.0, f"the bound does not reject {m}"

@@ -135,3 +135,82 @@ def test_overlay_pre_seeds_the_native_graphnorm_before_the_reference_module_is_i
         "assert M is P.GraphNorm\nprint('GRAPHNORM-PRESEED-OK')\n" % ROOT)
     r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300, cwd="/tmp")
     assert r.returncode == 0 and "GRAPHNORM-PRESEED-OK" in r.stdout, r.stdout + r.stderr[-3000:]
+
+
+# ---- backward ---------------------------------------------------------------------------------------------------------------
+EPS32 = float(torch.tensor(1e-10, dtype=torch.float32))     # the eps the kernels receive (a float)
+
+
+def _bwd_case(counts, D, alpha_value, seed, equal_rows=()):
+    """(x, dy, n2g, G, gamma, alpha) on a shuffled map with the given graph sizes; the graphs in ``equal_rows`` have all rows equal."""
+    gen = torch.Generator().manual_seed(seed)
+    n2g = torch.repeat_interleave(torch.arange(len(counts)), torch.tensor(counts))
+    n2g = n2g[torch.randperm(n2g.numel(), generator=gen)]
+    G = len(counts)
+    x = torch.randn(n2g.numel(), D, generator=gen) * 2.0 + torch.randn(G, D, generator=gen)[n2g] * 3.0
+    for g in equal_rows:
+        x[n2g == g] = torch.randn(D, generator=gen) * 3.0
+    dy = torch.randn(n2g.numel(), D, generator=gen)
+    gamma = 1.0 + 0.5 * torch.randn(1, D, generator=gen)
+    alpha = torch.full((1, D), alpha_value) if alpha_value is not None else torch.rand(1, D, generator=gen) * 1.5
+    return x, dy, n2g, G, gamma, alpha
+
+
+def _exact_stats(x64, n2g, alpha64, eps, G):
+    mean = GR.scatter_mean(x64, n2g, G)
+    sigma2 = GR.scatter_mean((x64 - alpha64 * mean[n2g]) ** 2, n2g, G) + eps
+    return mean, 1.0 / torch.sqrt(sigma2)
+
+
+BWD_CASES = {"sizes_alpha_rand": ([1, 31, 32, 33, 0, 1, 64, 65, 200], None, ()), "alpha0": ([1, 5, 33, 0, 70], 0.0, ()),
+             "alpha_half": ([1, 5, 33, 0, 70], 0.5, (1,)), "alpha1": ([1, 5, 33, 0, 70], 1.0, (2,)),
+             "alpha1.7": ([1, 5, 33, 0, 70], 1.7, (1, 4))}
+
+
+@pytest.mark.parametrize("eps", [EPS32, 0.25])
+@pytest.mark.parametrize("case", list(BWD_CASES))
+def test_backward_formula_equals_autograd_through_the_float64_forward(case, eps):
+    """With the exact float64 mean and rstd, backward_formula is the gradient of layer_forward (one-node graphs and graphs of equal
+    rows included).  Relative to each gradient's largest element: autograd itself cancels in 1 - x^2 on a one-node graph, where the
+    formula does not.  eps = 0.25 makes the one-node gradient large enough to be pinned too."""
+    counts, a, equal = BWD_CASES[case]
+    x, dy, n2g, G, gamma, alpha = _bwd_case(counts, 64, a, len(counts) + int(10 * (a or 0)), equal)
+    x64, g64, a64, b64 = (t.double().requires_grad_(True) for t in (x, gamma, alpha, torch.zeros(1, 64)))
+    GR.layer_forward(x64, n2g, g64, a64, b64, eps=eps, G=G).backward(dy.double())
+    mean, rstd = _exact_stats(x64.detach(), n2g, alpha.double(), eps, G)
+    got = GR.backward_formula(x, dy, n2g, mean, rstd, gamma, alpha, eps=eps, G=G)
+    for name, g, ref in zip(("dx", "d gamma", "d alpha", "d beta"), got, (x64.grad, g64.grad[0], a64.grad[0], b64.grad[0])):
+        err = float((g - ref).abs().max() / ref.abs().max())
+        assert err <= 1e-12, f"{case} eps={eps} {name}: {err:.2e}"
+    one = torch.bincount(n2g, minlength=G) == 1
+    rows = one[n2g]
+    if eps == 0.25 and a != 1.0:
+        rel = ((got[0][rows] - x64.grad[rows]).abs() / x64.grad[rows].abs()).max()
+        assert float(rel) <= 1e-12, f"{case}: one-node rows {float(rel):.2e}"
+
+
+def _emulated_pair(counts, D, a, seed, equal=()):
+    x, dy, n2g, G, gamma, alpha = _bwd_case(counts, D, a, seed, equal)
+    _, mean, rstd = GR.emulate_forward(x, n2g, gamma, alpha, torch.zeros(1, D), G=G)
+    return x, dy, n2g, G, gamma, alpha, mean, rstd
+
+
+@pytest.mark.parametrize("case", list(BWD_CASES))
+def test_backward_emulation_is_inside_the_bound_and_the_mutants_are_not(case):
+    """The float32 emulation of the backward kernels' order against backward_formula on the forward's float32 statistics, under
+    backward_bound; the one-node branch removed (the general formula on count 1) and c2 without alpha fall outside it."""
+    counts, a, equal = BWD_CASES[case]
+    args = _emulated_pair(counts, 64, a, 3 * len(counts), equal)
+    x, dy, n2g, G, gamma, alpha, mean, rstd = args
+    ref = GR.backward_formula(*args[:2], n2g, mean, rstd, gamma, alpha, eps=1e-10, G=G)
+    bnd = GR.backward_bound(*args[:2], n2g, mean, rstd, gamma, alpha, eps=1e-10, G=G)
+
+    def over(got):
+        return [float(((g.double() - r).abs() / b).max()) for g, r, b in zip(got, ref, bnd)]
+
+    worst = over(GR.emulate_backward(x, dy, n2g, mean, rstd, gamma, alpha, G=G))
+    assert max(worst) <= 1.0, f"{case}: emulated kernel order exceeds the bound (dx, dgamma, dalpha, dbeta ratios {worst})"
+    if a != 1.0:            # alpha = 1: s = 0 on a one-node graph, where both branches give exactly 0
+        assert over(GR.emulate_backward(x, dy, n2g, mean, rstd, gamma, alpha, G=G, mutant="no_one_node_branch"))[0] > 1.0, case
+    if a not in (0.0, 1.0):  # alpha S = S at alpha = 1, and c2 = 0 at alpha = 0
+        assert max(over(GR.emulate_backward(x, dy, n2g, mean, rstd, gamma, alpha, G=G, mutant="c2_without_alpha"))) > 1.0, case

@@ -124,3 +124,53 @@ def test_overlay_pre_seeds_the_native_layer_before_the_reference_module_is_impor
         "assert M is P.MultiHeadSelfAttentionMessagePassing\nprint('SELFATT-PRESEED-OK')\n" % ROOT)
     r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300, cwd="/tmp")
     assert r.returncode == 0 and "SELFATT-PRESEED-OK" in r.stdout, r.stdout + r.stderr[-3000:]
+
+
+# ---- backward ---------------------------------------------------------------------------------------------------------------
+def _exact_forward(t64, n2g, heads, dk, L):
+    """float64 (o, lse) of the attention."""
+    a, b, _ = SR.split_heads(t64, heads, dk)
+    lse = torch.cat([torch.logsumexp(torch.einsum("khd,vhd->khv", a[s:e], b[s:e]) / dk ** 0.5, dim=-1) for s, e in SR.chunks(n2g, L)])
+    return SR.attention(t64, n2g, heads, dk, L), lse
+
+
+def _bwd_inputs(counts, heads, dk, dv, seed):
+    gen = torch.Generator().manual_seed(seed)
+    n2g = torch.repeat_interleave(torch.arange(len(counts)), torch.tensor(counts))
+    n2g = n2g[torch.randperm(n2g.numel(), generator=gen)]
+    t = torch.randn(n2g.numel(), heads * (2 * dk + dv), generator=gen)
+    return n2g, t, torch.randn(n2g.numel(), heads * dv, generator=gen)
+
+
+BWD_COUNTS = [1, 16, 17, 0, 64, 65, 130]
+
+
+@pytest.mark.parametrize("dk,dv,L", [(16, 32, 70), (32, 16, 1000), (64, 64, 1)])
+def test_backward_formula_equals_autograd_through_the_float64_forward(dk, dv, L):
+    heads = 2
+    n2g, t, d_o = _bwd_inputs(BWD_COUNTS, heads, dk, dv, dk + dv + L)
+    t64 = t.double().requires_grad_(True)
+    SR.attention(t64, n2g, heads, dk, L).backward(d_o.double())
+    o, lse = _exact_forward(t64.detach(), n2g, heads, dk, L)
+    got = SR.backward_formula(t64.detach(), o, lse, d_o, n2g, heads, dk, L)
+    err = float((got - t64.grad).abs().max() / t64.grad.abs().max())
+    assert err <= 1e-12, f"dk={dk} dv={dv} L={L}: {err:.2e}"
+
+
+MUTANTS = ["no_delta", "db_unscaled", "kv_own_tile", "q_short"]
+
+
+@pytest.mark.parametrize("dk,dv", [(16, 16), (32, 64)])
+def test_backward_emulation_is_inside_the_bound_and_the_mutants_are_not(dk, dv):
+    """The float32 emulation of the backward kernels' order, on the float32-rounded exact o and lse, against backward_formula under
+    backward_bound; each named mutant falls outside it (L = 100: chunks of 1 to 100 rows, two of them longer than a 64-row tile)."""
+    heads, L = 2, 100
+    n2g, t, d_o = _bwd_inputs(BWD_COUNTS, heads, dk, dv, 5 + dk)
+    o, lse = (z.float() for z in _exact_forward(t.double(), n2g, heads, dk, L))
+    ref = SR.backward_formula(t, o, lse, d_o, n2g, heads, dk, L)
+    bnd = SR.backward_bound(t, o, lse, d_o, n2g, heads, dk, L)
+    ratio = float(((SR.emulate_backward(t, o, lse, d_o, n2g, heads, dk, L).double() - ref).abs() / bnd).max())
+    assert ratio <= 1.0, f"emulated kernel order exceeds the bound ({ratio:.2f})"
+    for m in MUTANTS:
+        mut = SR.emulate_backward(t, o, lse, d_o, n2g, heads, dk, L, mutant=m).double()
+        assert bool(((mut - ref).abs() > bnd).any()), f"the bound does not reject {m}"
