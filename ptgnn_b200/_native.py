@@ -5,12 +5,14 @@ PyTorch is used only for device memory (``Tensor.data_ptr()``), streams and ``to
 """
 import ctypes
 import os
+import re
 from typing import Optional, Sequence
 
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libptgnn_b200.so")
+HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "ptgnn_b200.h")
 
 REDUCE = {"sum": 0, "add": 0, "mean": 1, "max": 2, "min": 3}
 READOUT_SUM, READOUT_MEAN, READOUT_WEIGHTED_SUM = 0, 1, 2
@@ -19,118 +21,46 @@ ACT_NONE, ACT_GELU, ACT_TANH, ACT_RELU = 0, 1, 2, 3
 
 c_i32, c_i64, c_f32, c_void_p, c_size_t = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_void_p, ctypes.c_size_t
 
-# symbol -> (restype, argtypes); must list every function include/ptgnn_b200.h declares (tests check this).
-SIGNATURES = {
-    "ptgnn_b200_abi_version": (ctypes.c_int, []),
-    "ptgnn_b200_last_error": (ctypes.c_char_p, []),
-    "ptgnn_b200_launch_count": (c_i64, []),
-    "ptgnn_b200_kernel_timing_enable": (ctypes.c_int, [c_i32]),
-    "ptgnn_b200_kernel_timing_read": (ctypes.c_int, [c_void_p, c_void_p, c_i32]),
-    "ptgnn_b200_plan_workspace_bytes": (c_size_t, [c_i64, c_i64]),
-    "ptgnn_b200_plan_build": (ctypes.c_int, [c_i64, c_i64, c_i32, c_void_p, c_void_p, c_void_p] + [c_void_p] * 8 + [c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_plan_convert": (ctypes.c_int, [c_i64, c_i64, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_plan_sort": (ctypes.c_int, [c_i64, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_segment_reduce_f32": (ctypes.c_int, [c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_void_p]),
-    "ptgnn_b200_scatter_workspace_bytes": (c_size_t, [c_i64, c_i64]),
-    "ptgnn_b200_scatter_f32": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_i64, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_gated_workspace_bytes": (c_size_t, [c_i32, c_i64, c_i64, c_i32, c_i32, c_i32]),
-    "ptgnn_b200_gated_weight_cache_bytes": (c_size_t, [c_i32, c_i32, c_i32, c_i32]),
-    "ptgnn_b200_gated_forward": (ctypes.c_int, [c_i32, c_void_p, c_void_p, c_i64, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p,
-                                                c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i32, c_void_p, c_void_p, c_size_t,
-                                                c_void_p, c_size_t, c_i32, c_void_p]),
-    "ptgnn_b200_mlp_workspace_bytes": (c_size_t, [c_i32, c_i64, c_i64, c_i32, c_i32, c_i32, c_i32, c_i32]),
-    "ptgnn_b200_mlp_forward": (ctypes.c_int, [c_i32, c_void_p, c_void_p, c_i64, c_i32, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p,
-                                              c_void_p, c_void_p, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_f32, c_void_p, c_void_p, c_i32,
-                                              c_void_p, c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_block_plan_block_targets": (c_i32, [c_i64]),
-    "ptgnn_b200_block_plan_workspace_bytes": (c_size_t, [c_i64, c_i64, c_i32, c_i32]),
-    "ptgnn_b200_block_plan_build": (ctypes.c_int, [c_i64, c_i32, c_void_p, c_void_p, c_void_p, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_fused_supported": (c_i32, [c_i32, c_i32, c_i32]),
-    "ptgnn_b200_gated_fused_workspace_bytes": (c_size_t, [c_i32, c_i64, c_i64, c_i32, c_i32, c_i32]),
-    "ptgnn_b200_gated_fused_weight_cache_bytes": (c_size_t, [c_i32, c_i32, c_i32, c_i32]),
-    "ptgnn_b200_packed_state_bytes": (c_size_t, [c_i64, c_i32]),
-    "ptgnn_b200_gated_forward_fused": (ctypes.c_int, [c_i32, c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i32, c_i32, c_i32, c_void_p, c_void_p,
-                                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i32, c_void_p, c_void_p, c_void_p,
-                                                      c_size_t, c_void_p, c_size_t, c_i32, c_void_p]),
-    "ptgnn_b200_mlp_fused_workspace_bytes": (c_size_t, [c_i32, c_i64, c_i64, c_i32, c_i32, c_i32, c_i32, c_i32]),
-    "ptgnn_b200_mlp_fused_weight_cache_bytes": (c_size_t, [c_i32, c_i32, c_i32, c_i32, c_i32, c_i32]),
-    "ptgnn_b200_mlp_forward_fused": (ctypes.c_int, [c_i32, c_void_p, c_void_p, c_i64, c_i64, c_i32, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p,
-                                                    c_i32, c_i32, c_i32, c_void_p, c_void_p, c_f32, c_void_p, c_void_p, c_i32, c_void_p, c_void_p,
-                                                    c_size_t, c_void_p, c_size_t, c_i32, c_void_p]),
-    "ptgnn_b200_egc_supported": (c_i32, [c_i32] * 5),
-    "ptgnn_b200_egc_fused_workspace_bytes": (c_size_t, [c_i32, c_i64] + [c_i32] * 5),
-    "ptgnn_b200_egc_fused_weight_cache_bytes": (c_size_t, [c_i32] * 6),
-    "ptgnn_b200_egc_forward_fused": (ctypes.c_int, [c_i32, c_void_p, c_i64] + [c_i32] * 5 + [c_void_p] * 5 + [c_i32, c_void_p, c_void_p,
-                                                                                                            c_size_t, c_void_p, c_size_t,
-                                                                                                            c_i32, c_void_p]),
-    "ptgnn_b200_gather_split_f16": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "ptgnn_b200_gru_gate_grads_f32": (ctypes.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "ptgnn_b200_offset_ids": (ctypes.c_int, [c_void_p, c_i64, c_void_p, c_void_p, c_i32, c_void_p, c_void_p]),
-    "ptgnn_b200_segment_ids": (ctypes.c_int, [c_void_p, c_i32, c_i64, c_void_p, c_void_p]),
-    "ptgnn_b200_linear_workspace_bytes": (c_size_t, [c_i32, c_i32]),
-    "ptgnn_b200_linear_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_i32, c_i32, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_grucell_workspace_bytes": (c_size_t, [c_i32, c_i32]),
-    "ptgnn_b200_grucell_f32": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_edge_messages_workspace_bytes": (c_size_t, [c_i32, c_i32, c_i32, c_i32]),
-    "ptgnn_b200_edge_messages_f32": (ctypes.c_int, [c_void_p, c_void_p, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                                    c_i32, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_graph_readout_workspace_bytes": (c_size_t, [c_i64, c_i64, c_i32]),
-    "ptgnn_b200_graph_readout": (ctypes.c_int, [c_i32, c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_i64, c_void_p, c_i32, c_void_p, c_void_p,
-                                                c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_global_gru_supported": (c_i32, [c_i32, c_i32]),
-    "ptgnn_b200_global_gru_workspace_bytes": (c_size_t, [c_i32, c_i64, c_i64, c_i32, c_i32]),
-    "ptgnn_b200_global_gru_weight_cache_bytes": (c_size_t, [c_i32, c_i32]),
-    "ptgnn_b200_global_gru_update": (ctypes.c_int, [c_i32, c_void_p, c_void_p, c_i64, c_i32, c_void_p, c_i64, c_void_p, c_i32, c_void_p, c_void_p,
-                                                    c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_size_t,
-                                                    c_i32, c_void_p]),
-    "ptgnn_b200_attention_readout_supported": (c_i32, [c_i32, c_i32, c_i32]),
-    "ptgnn_b200_attention_readout_workspace_bytes": (c_size_t, [c_i64, c_i64, c_i32, c_i32]),
-    "ptgnn_b200_attention_readout": (ctypes.c_int, [c_i32, c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_i64, c_void_p, c_void_p,
-                                                    c_void_p, c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_attention_readout_backward_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_i64, c_void_p, c_void_p,
-                                                                 c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_selfatt_supported": (c_i32, [c_i32, c_i32, c_i32]),
-    "ptgnn_b200_selfatt_workspace_bytes": (c_size_t, [c_i64, c_i64, c_i32]),
-    "ptgnn_b200_selfatt_forward": (ctypes.c_int, [c_i32, c_void_p, c_i64, c_i32, c_i32, c_i32, c_void_p, c_i64, c_i64, c_void_p, c_void_p,
-                                                  c_void_p, c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_selfatt_backward_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_i32, c_void_p, c_i64, c_i64, c_void_p, c_void_p,
-                                                       c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_graph_norm_supported": (c_i32, [c_i32]),
-    "ptgnn_b200_graph_norm_workspace_bytes": (c_size_t, [c_i64, c_i64, c_i32]),
-    "ptgnn_b200_graph_norm_forward": (ctypes.c_int, [c_i32, c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_void_p,
-                                                     c_void_p, c_f32, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_graph_norm_backward_f32": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_void_p, c_i64, c_void_p,
-                                                          c_void_p, c_f32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                                          c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_pna_supported": (c_i32, [c_i32]),
-    "ptgnn_b200_pna_forward": (ctypes.c_int, [c_i32, c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_i64, c_f32, c_void_p, c_void_p, c_void_p,
-                                              c_void_p]),
-    "ptgnn_b200_pna_backward_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_i64, c_f32, c_void_p, c_void_p, c_void_p,
-                                                   c_void_p, c_void_p, c_void_p]),
-    "ptgnn_b200_copy_attention_supported": (c_i32, [c_i32, c_i32, c_i32]),
-    "ptgnn_b200_copy_attention_workspace_bytes": (c_size_t, [c_i64, c_i64, c_i32, c_i32]),
-    "ptgnn_b200_copy_attention": (ctypes.c_int, [c_i32, c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_i64, c_void_p, c_void_p, c_void_p,
-                                                 c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_copy_attention_backward_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_i64, c_void_p, c_void_p,
-                                                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_embedding_bag_supported": (c_i32, [c_i32, c_i32]),
-    "ptgnn_b200_embedding_bag": (ctypes.c_int, [c_i32, c_void_p, c_i64, c_i32, c_void_p, c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p,
-                                                c_void_p, c_void_p]),
-    "ptgnn_b200_embedding_bag_pairs": (ctypes.c_int, [c_void_p, c_void_p, c_i64, c_i32, c_i64, c_void_p, c_void_p, c_void_p]),
-    "ptgnn_b200_embedding_bag_backward_workspace_bytes": (c_size_t, [c_i64, c_i32, c_i64, c_i32]),
-    "ptgnn_b200_embedding_bag_backward_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_i32, c_void_p, c_void_p,
-                                                             c_i64, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "ptgnn_b200_char_cnn_supported": (c_i32, [c_i32] * 8),
-    "ptgnn_b200_char_cnn_workspace_bytes": (c_size_t, [c_i32] * 8),
-    "ptgnn_b200_char_cnn_prepare": (ctypes.c_int, [c_i32] + [c_void_p] * 5 + [c_i32] * 7 + [c_void_p, c_size_t, c_void_p, c_void_p]),
-    "ptgnn_b200_char_cnn_forward": (ctypes.c_int, [c_i32, c_void_p, c_i64, c_i32] + [c_i32] * 7 + [c_void_p, c_size_t, c_void_p, c_void_p,
-                                                                                               c_void_p, c_void_p]),
-    "ptgnn_b200_char_cnn_materialise_f32": (ctypes.c_int, [c_void_p, c_i64, c_i32] + [c_i32] * 7 + [c_void_p, c_size_t, c_void_p, c_void_p,
-                                                                                                 c_void_p, c_void_p]),
-    "ptgnn_b200_gated_gnn_forward_host_f32":(ctypes.c_int, [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_i32,
-                                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i32, c_void_p]),
-}
 
+class NativeLibraryError(RuntimeError):
+    pass
+
+
+_SCALAR_TYPES = {"int": c_i32, "int32_t": c_i32, "int64_t": c_i64, "size_t": c_size_t, "float": c_f32}
+
+
+def _ctype(decl: str, proto: str, result: bool = False):
+    words = re.sub(r"\bconst\b", " ", decl).replace("*", " * ").split()
+    if "*" in words:
+        if not result:
+            return c_void_p          # callers pass Tensor.data_ptr(), None, host arrays or ctypes.byref(...)
+        if words == ["char", "*"]:
+            return ctypes.c_char_p
+    else:
+        base = " ".join(words if result or len(words) == 1 else words[:-1])      # a parameter drops its name
+        if base in _SCALAR_TYPES:
+            return _SCALAR_TYPES[base]
+    raise NativeLibraryError(f"no ctypes type for `{decl.strip()}` in the C ABI prototype `{proto}`")
+
+
+def parse_signatures(header: str) -> dict:
+    """{name: (restype, argtypes)} of every ``ptgnn_b200_*`` prototype in the C header text ``header``.  A type without a
+    mapping raises NativeLibraryError: a wrong guess would pass every call through ctypes and corrupt it."""
+    text = re.sub(r"/\*.*?\*/|//[^\n]*|^[ \t]*#[^\n]*", " ", header, flags=re.S | re.M)
+    signatures = {}
+    for statement in text.split(";"):
+        m = re.search(r"([\w\s*]*?)\b(ptgnn_b200_\w+)\s*\(([^()]*)\)\s*$", statement)
+        if m is not None:
+            result, name, params = m.group(1), m.group(2), m.group(3).strip()
+            proto = " ".join(m.group(0).split())
+            signatures[name] = (_ctype(result, proto, result=True),
+                                [] if params == "void" else [_ctype(p, proto) for p in params.split(",")])
+    return signatures
+
+
+# symbol -> (restype, argtypes) of every function include/ptgnn_b200.h declares: the header is the only place they are written
+with open(HEADER_PATH, encoding="utf-8") as _f:
+    SIGNATURES = parse_signatures(_f.read())
 
 
 class BlockPlanStruct(ctypes.Structure):
@@ -140,10 +70,6 @@ class BlockPlanStruct(ctypes.Structure):
 
 ABI_VERSION = 4        # moves only on incompatible changes of an existing entry point (include/ptgnn_b200.h)
 _lib: Optional[ctypes.CDLL] = None
-
-
-class NativeLibraryError(RuntimeError):
-    pass
 
 
 def lib() -> ctypes.CDLL:
@@ -175,6 +101,17 @@ def check(rc: int, what: str) -> None:
         msg = lib().ptgnn_b200_last_error().decode("utf-8", "replace")
         codes = {-1: ValueError, -2: NotImplementedError, -3: RuntimeError, -4: RuntimeError, -5: IndexError}
         raise codes.get(rc, RuntimeError)(f"{what} failed (code {rc}): {msg}")
+
+
+def call(name: str, device, *args) -> None:
+    """Enqueues the entry point ``name`` on ``device``'s current stream: ``args`` are its parameters except the trailing ``stream``.
+    The argument count is checked first (ctypes rejects too few arguments but passes surplus ones through); a nonzero return code
+    raises as in ``check``."""
+    if len(args) + 1 != len(SIGNATURES[name][1]):
+        raise TypeError(f"{name} takes {len(SIGNATURES[name][1]) - 1} arguments before its stream, got {len(args)}")
+    with torch.cuda.device(device):
+        rc = getattr(lib(), name)(*args, current_stream(device))
+    check(rc, name)
 
 
 def launch_count() -> int:

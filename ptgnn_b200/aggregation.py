@@ -43,12 +43,9 @@ def native_pna(messages: torch.Tensor, plan: EdgePlan, delta: float, want_arg: b
     n, D = plan.num_nodes, m.shape[1]
     out = torch.empty(n, 15 * D, dtype=torch.float32, device=m.device)
     args = torch.empty(2, n, D, dtype=torch.int32, device=m.device) if want_arg else None
-    with torch.cuda.device(m.device):
-        rc = N.lib().ptgnn_b200_pna_forward(int(bf16), N.ptr(m), plan.num_edges, D, N.ptr(plan.row_ptr),
-                                            N.ptr(plan.perm) if plan.num_edges else None, n, float(delta), N.ptr(out),
-                                            N.ptr(args[0]) if want_arg else None, N.ptr(args[1]) if want_arg else None,
-                                            N.current_stream(m.device))
-    N.check(rc, "ptgnn_b200_pna_forward")
+    N.call("ptgnn_b200_pna_forward", m.device, int(bf16), N.ptr(m), plan.num_edges, D, N.ptr(plan.row_ptr),
+           N.ptr(plan.perm) if plan.num_edges else None, n, float(delta), N.ptr(out), N.ptr(args[0]) if want_arg else None,
+           N.ptr(args[1]) if want_arg else None)
     return (out, args[0], args[1]) if want_arg else (out, None, None)
 
 
@@ -68,11 +65,9 @@ def native_pna_backward(messages: torch.Tensor, plan: EdgePlan, delta: float, ou
         tensors.append(t if t.data_ptr() % 16 == 0 else t.clone())
     out, d_out, arg_max, arg_min = tensors
     d_m = torch.empty_like(m)
-    with torch.cuda.device(m.device):
-        rc = N.lib().ptgnn_b200_pna_backward_f32(N.ptr(m), plan.num_edges, D, N.ptr(plan.row_ptr), N.ptr(plan.perm) if plan.num_edges else None,
-                                                 n, float(delta), N.ptr(out), N.ptr(arg_max), N.ptr(arg_min), N.ptr(d_out), N.ptr(d_m),
-                                                 N.current_stream(m.device))
-    N.check(rc, "ptgnn_b200_pna_backward_f32")
+    N.call("ptgnn_b200_pna_backward_f32", m.device, N.ptr(m), plan.num_edges, D, N.ptr(plan.row_ptr),
+           N.ptr(plan.perm) if plan.num_edges else None, n, float(delta), N.ptr(out), N.ptr(arg_max), N.ptr(arg_min), N.ptr(d_out),
+           N.ptr(d_m))
     return d_m
 
 

@@ -84,9 +84,7 @@ def _split16(x: torch.Tensor, index: Optional[torch.Tensor] = None, scale=None):
         v = v * scale
         hi = v.half()
         return hi, torch.sub(v, hi).mul_(2048.0).half(), inv
-    with torch.cuda.device(x.device):
-        rc = N.lib().ptgnn_b200_gather_split_f16(N.ptr(x), N.ptr(index), rows, cols, N.ptr(scale), N.ptr(hi), N.ptr(lo), N.current_stream(x.device))
-    N.check(rc, "ptgnn_b200_gather_split_f16")
+    N.call("ptgnn_b200_gather_split_f16", x.device, N.ptr(x), N.ptr(index), rows, cols, N.ptr(scale), N.ptr(hi), N.ptr(lo))
     return hi, lo, inv
 
 
@@ -136,10 +134,8 @@ def _gru_gate_grads(g, gi, gh, h, w_hh):
     """(d gi, d gh, d h) of torch.nn.GRUCell (gate order r, z, n) from its gate pre-activations gi, gh: the gate derivatives in one native
     pointwise kernel; d h is the direct path plus the product through W_hh on the native dense kernel."""
     d_gi, d_gh, d_h = torch.empty_like(gi), torch.empty_like(gh), torch.empty_like(h)
-    with torch.cuda.device(h.device):
-        rc = N.lib().ptgnn_b200_gru_gate_grads_f32(N.ptr(gi), N.ptr(gh), N.ptr(h), N.ptr(g), h.shape[0], h.shape[1], N.ptr(d_gi), N.ptr(d_gh),
-                                                  N.ptr(d_h), N.current_stream(h.device))
-    N.check(rc, "ptgnn_b200_gru_gate_grads_f32")
+    N.call("ptgnn_b200_gru_gate_grads_f32", h.device, N.ptr(gi), N.ptr(gh), N.ptr(h), N.ptr(g), h.shape[0], h.shape[1], N.ptr(d_gi),
+           N.ptr(d_gh), N.ptr(d_h))
     return d_gi, d_gh, d_h + C.linear(d_gh, w_hh.t().contiguous())
 
 

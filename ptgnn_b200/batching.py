@@ -113,35 +113,29 @@ class MinibatchAssembler:
         ptr_dev = dev[: ptr_words * 8].view(torch.int64)
         id_dev = dev[ptr_words * 8:].view(torch.int32)
 
-        lib = N.lib()
-        stream = N.current_stream(device)
-
         def offset(id_slot: int, ptr_slot: int, total: int) -> torch.Tensor:
             out = torch.empty(total, dtype=torch.int64, device=device)
             if total:
-                rc = lib.ptgnn_b200_offset_ids(id_dev[id_off[id_slot]:].data_ptr(), total, ptr_dev[ptr_off[ptr_slot]:].data_ptr(),
-                                               ptr_dev.data_ptr(), G, out.data_ptr(), stream)
-                N.check(rc, "ptgnn_b200_offset_ids")
+                N.call("ptgnn_b200_offset_ids", device, id_dev[id_off[id_slot]:].data_ptr(), total, ptr_dev[ptr_off[ptr_slot]:].data_ptr(),
+                       ptr_dev.data_ptr(), G, out.data_ptr())
             return out
 
         def segments(ptr_slot: int, total: int) -> torch.Tensor:
             out = torch.empty(total, dtype=torch.int64, device=device)
             if total:
-                rc = lib.ptgnn_b200_segment_ids(ptr_dev[ptr_off[ptr_slot]:].data_ptr(), G, total, out.data_ptr(), stream)
-                N.check(rc, "ptgnn_b200_segment_ids")
+                N.call("ptgnn_b200_segment_ids", device, ptr_dev[ptr_off[ptr_slot]:].data_ptr(), G, total, out.data_ptr())
             return out
 
-        with torch.cuda.device(device):
-            adjacency_lists: List[Optional[Tuple[torch.Tensor, torch.Tensor]]] = [None] * self.num_edge_types
-            reference_node_ids: Dict[str, torch.Tensor] = {}
-            reference_node_graph_idx: Dict[str, torch.Tensor] = {}
-            for kind, key, ptr_slot, id_slot, total in jobs:
-                if kind == "adj":
-                    adjacency_lists[key] = (offset(id_slot, ptr_slot, total), offset(id_slot + 1, ptr_slot, total))
-                else:
-                    reference_node_ids[key] = offset(id_slot, ptr_slot, total)
-                    reference_node_graph_idx[key] = segments(ptr_slot, total)
-            node_to_graph_idx = segments(0, num_nodes)
+        adjacency_lists: List[Optional[Tuple[torch.Tensor, torch.Tensor]]] = [None] * self.num_edge_types
+        reference_node_ids: Dict[str, torch.Tensor] = {}
+        reference_node_graph_idx: Dict[str, torch.Tensor] = {}
+        for kind, key, ptr_slot, id_slot, total in jobs:
+            if kind == "adj":
+                adjacency_lists[key] = (offset(id_slot, ptr_slot, total), offset(id_slot + 1, ptr_slot, total))
+            else:
+                reference_node_ids[key] = offset(id_slot, ptr_slot, total)
+                reference_node_graph_idx[key] = segments(ptr_slot, total)
+        node_to_graph_idx = segments(0, num_nodes)
         return {
             "adjacency_lists": adjacency_lists,
             "node_to_graph_idx": node_to_graph_idx,

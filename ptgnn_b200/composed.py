@@ -51,10 +51,8 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] =
     lib = N.lib()
     ws_bytes = lib.ptgnn_b200_linear_workspace_bytes(xw.shape[1], n_out + n_pad)
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=x.device)
-    with torch.cuda.device(x.device):
-        rc = lib.ptgnn_b200_linear_f32(N.ptr(xw), rows, xw.shape[1], N.ptr(ww), N.ptr(b), n_out + n_pad, act_code or N.ACT_NONE, N.ptr(out),
-                                       N.ptr(ws), ws_bytes, N.current_stream(x.device))
-    N.check(rc, "ptgnn_b200_linear_f32")
+    N.call("ptgnn_b200_linear_f32", x.device, N.ptr(xw), rows, xw.shape[1], N.ptr(ww), N.ptr(b), n_out + n_pad, act_code or N.ACT_NONE,
+           N.ptr(out), N.ptr(ws), ws_bytes)
     out = out[:, :n_out] if n_pad else out
     return post(out) if post is not None else out
 
@@ -73,11 +71,8 @@ def edge_messages(plan: EdgePlan, source_rows: torch.Tensor, target_rows: Option
     H = source_rows.shape[1]
     ws_bytes = lib.ptgnn_b200_edge_messages_workspace_bytes(plan.num_types, H, D, int(use_target))
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=source_rows.device)
-    with torch.cuda.device(source_rows.device):
-        rc = lib.ptgnn_b200_edge_messages_f32(N.ptr(source_rows), N.ptr(target_rows), H, D, plan.num_types, plan.type_off_c, N.ptr(plan.src32),
-                                              N.ptr(plan.tgt32), N.ptr(ident), N.ptr_table(ws_list), int(use_target), N.ptr(out), N.ptr(ws),
-                                              ws_bytes, N.current_stream(source_rows.device))
-    N.check(rc, "ptgnn_b200_edge_messages_f32")
+    N.call("ptgnn_b200_edge_messages_f32", source_rows.device, N.ptr(source_rows), N.ptr(target_rows), H, D, plan.num_types, plan.type_off_c,
+           N.ptr(plan.src32), N.ptr(plan.tgt32), N.ptr(ident), N.ptr_table(ws_list), int(use_target), N.ptr(out), N.ptr(ws), ws_bytes)
     return out
 
 
@@ -87,11 +82,8 @@ def segment_reduce(messages: torch.Tensor, plan: EdgePlan, reduce_code: int, ret
     E, D = messages.shape
     out = torch.empty(plan.num_nodes, D, dtype=torch.float32, device=messages.device)
     arg = torch.empty(plan.num_nodes, D, dtype=torch.int64, device=messages.device) if return_arg else None
-    lib = N.lib()
-    with torch.cuda.device(messages.device):
-        rc = lib.ptgnn_b200_segment_reduce_f32(N.ptr(messages), N.ptr(plan.row_ptr), N.ptr(plan.perm) if E else None, plan.num_nodes, E, D,
-                                               reduce_code, N.ptr(out), N.ptr(arg), N.current_stream(messages.device))
-    N.check(rc, "ptgnn_b200_segment_reduce_f32")
+    N.call("ptgnn_b200_segment_reduce_f32", messages.device, N.ptr(messages), N.ptr(plan.row_ptr), N.ptr(plan.perm) if E else None,
+           plan.num_nodes, E, D, reduce_code, N.ptr(out), N.ptr(arg))
     return (out, arg) if return_arg else out
 
 
@@ -114,11 +106,10 @@ def aggregate(plan: EdgePlan, source_rows: torch.Tensor, weights: Sequence[torch
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=rows.device)
     out = torch.empty(n, D, dtype=torch.float32, device=rows.device)
     bp = plan.block_plan()
-    with torch.cuda.device(rows.device):       # the Mlp entry point without activation / LayerNorm / dense layer = the bare aggregation
-        rc = lib.ptgnn_b200_mlp_forward_fused(0, N.ptr(rows), None, n, n, K, D, D, plan.num_types, ctypes.byref(bp), N.ptr(plan.row_ptr),
-                                              N.ptr_table(ws_list), 0, reduce_code, N.ACT_NONE, None, None, 0.0, None, None, N.ACT_NONE,
-                                              N.ptr(out), N.ptr(ws), ws_bytes, None, 0, 0, N.current_stream(rows.device))
-    N.check(rc, "ptgnn_b200_mlp_forward_fused")
+    # the Mlp entry point without activation / LayerNorm / dense layer = the bare aggregation
+    N.call("ptgnn_b200_mlp_forward_fused", rows.device, 0, N.ptr(rows), None, n, n, K, D, D, plan.num_types, ctypes.byref(bp),
+           N.ptr(plan.row_ptr), N.ptr_table(ws_list), 0, reduce_code, N.ACT_NONE, None, None, 0.0, None, None, N.ACT_NONE, N.ptr(out),
+           N.ptr(ws), ws_bytes, None, 0, 0)
     return out
 
 
@@ -130,10 +121,8 @@ def grucell(inp: torch.Tensor, hidden: torch.Tensor, gru: nn.GRUCell) -> torch.T
     ws_bytes = lib.ptgnn_b200_grucell_workspace_bytes(H, D)
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=hidden.device)
     p = [N.require_cuda(t, "gru parameter", torch.float32) for t in (gru.weight_ih, gru.weight_hh, gru.bias_ih, gru.bias_hh)]
-    with torch.cuda.device(hidden.device):
-        rc = lib.ptgnn_b200_grucell_f32(N.ptr(inp.contiguous()), N.ptr(hidden), rows, H, D, N.ptr(p[0]), N.ptr(p[1]), N.ptr(p[2]), N.ptr(p[3]),
-                                        N.ptr(out), N.ptr(ws), ws_bytes, N.current_stream(hidden.device))
-    N.check(rc, "ptgnn_b200_grucell_f32")
+    N.call("ptgnn_b200_grucell_f32", hidden.device, N.ptr(inp.contiguous()), N.ptr(hidden), rows, H, D, N.ptr(p[0]), N.ptr(p[1]), N.ptr(p[2]),
+           N.ptr(p[3]), N.ptr(out), N.ptr(ws), ws_bytes)
     return out
 
 

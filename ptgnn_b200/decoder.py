@@ -55,10 +55,8 @@ def native_copy_attention(copy_reps: torch.Tensor, plan: EdgePlan, o: torch.Tens
     s = torch.empty(num_rows, L, dtype=torch.float32, device=c.device)
     lse = torch.empty(G, L, dtype=torch.float32, device=c.device)
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=c.device)
-    with torch.cuda.device(c.device):
-        rc = lib.ptgnn_b200_copy_attention(int(bf16), N.ptr(c), num_rows, H, L, N.ptr(plan.row_ptr), N.ptr(plan.perm) if num_rows else None,
-                                           G, N.ptr(q), N.ptr(s), N.ptr(lse), N.ptr(ws), ws_bytes, N.current_stream(c.device))
-    N.check(rc, "ptgnn_b200_copy_attention")
+    N.call("ptgnn_b200_copy_attention", c.device, int(bf16), N.ptr(c), num_rows, H, L, N.ptr(plan.row_ptr),
+           N.ptr(plan.perm) if num_rows else None, G, N.ptr(q), N.ptr(s), N.ptr(lse), N.ptr(ws), ws_bytes)
     return s, lse
 
 
@@ -80,11 +78,9 @@ def native_copy_attention_backward(copy_reps: torch.Tensor, plan: EdgePlan, o: t
     d_c = torch.empty_like(c)
     d_o = torch.empty(G, L, H, dtype=torch.float32, device=c.device)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=c.device)
-    with torch.cuda.device(c.device):
-        rc = lib.ptgnn_b200_copy_attention_backward_f32(N.ptr(c), num_rows, H, L, N.ptr(plan.row_ptr), N.ptr(plan.perm) if num_rows else None,
-                                                        G, N.ptr(q), N.ptr(tabs[0]), N.ptr(tabs[1]), N.ptr(tabs[2]), N.ptr(d_c), N.ptr(d_o),
-                                                        N.ptr(ws), ws_bytes, N.current_stream(c.device))
-    N.check(rc, "ptgnn_b200_copy_attention_backward_f32")
+    N.call("ptgnn_b200_copy_attention_backward_f32", c.device, N.ptr(c), num_rows, H, L, N.ptr(plan.row_ptr),
+           N.ptr(plan.perm) if num_rows else None, G, N.ptr(q), N.ptr(tabs[0]), N.ptr(tabs[1]), N.ptr(tabs[2]), N.ptr(d_c), N.ptr(d_o),
+           N.ptr(ws), ws_bytes)
     return d_c, d_o
 
 

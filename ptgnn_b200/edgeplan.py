@@ -78,13 +78,8 @@ class EdgePlan:
         lib = N.lib()
         ws_bytes = lib.ptgnn_b200_plan_workspace_bytes(num_nodes, E)
         ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=device)
-        with torch.cuda.device(device):
-            rc = lib.ptgnn_b200_plan_convert(
-                num_nodes, self.num_source_nodes, len(counts), N.ptr_table(srcs), N.ptr_table(tgts), self._counts_c,
-                N.ptr(self.row_ptr), N.ptr(self.src32), N.ptr(self.tgt32), N.ptr(self.status), N.ptr(ws), ws_bytes,
-                N.current_stream(device),
-            )
-        N.check(rc, "ptgnn_b200_plan_convert")
+        N.call("ptgnn_b200_plan_convert", device, num_nodes, self.num_source_nodes, len(counts), N.ptr_table(srcs), N.ptr_table(tgts),
+               self._counts_c, N.ptr(self.row_ptr), N.ptr(self.src32), N.ptr(self.tgt32), N.ptr(self.status), N.ptr(ws), ws_bytes)
         self._keepalive = (srcs, tgts)
         self._validated = False
         if validate:
@@ -100,11 +95,8 @@ class EdgePlan:
                 lib = N.lib()
                 ws_bytes = lib.ptgnn_b200_plan_workspace_bytes(self.num_nodes, E)
                 ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
-                with torch.cuda.device(dev):
-                    rc = lib.ptgnn_b200_plan_sort(self.num_nodes, self.num_types, self._counts_c, N.ptr(perm), N.ptr(pos), N.ptr(src_sorted),
-                                                  N.ptr(etype_sorted), N.ptr(self.src32), N.ptr(self.tgt32), N.ptr(ws), ws_bytes,
-                                                  N.current_stream(dev))
-                N.check(rc, "ptgnn_b200_plan_sort")
+                N.call("ptgnn_b200_plan_sort", dev, self.num_nodes, self.num_types, self._counts_c, N.ptr(perm), N.ptr(pos), N.ptr(src_sorted),
+                       N.ptr(etype_sorted), N.ptr(self.src32), N.ptr(self.tgt32), N.ptr(ws), ws_bytes)
             self._sorted = (perm, pos, src_sorted, etype_sorted)
         return self._sorted
 
@@ -148,11 +140,8 @@ class EdgePlan:
             tl_f = torch.empty(max(self.num_edges, 1), dtype=torch.uint8, device=dev)
             ws_bytes = lib.ptgnn_b200_block_plan_workspace_bytes(self.num_nodes, self.num_edges, self.num_types, B)
             ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
-            with torch.cuda.device(dev):
-                rc = lib.ptgnn_b200_block_plan_build(self.num_nodes, self.num_types, self.type_off_c, N.ptr(self.src32), N.ptr(self.tgt32),
-                                                     B, N.ptr(group_off), N.ptr(src_f), N.ptr(tl_f), N.ptr(ws), ws_bytes,
-                                                     N.current_stream(dev))
-            N.check(rc, "ptgnn_b200_block_plan_build")
+            N.call("ptgnn_b200_block_plan_build", dev, self.num_nodes, self.num_types, self.type_off_c, N.ptr(self.src32), N.ptr(self.tgt32),
+                   B, N.ptr(group_off), N.ptr(src_f), N.ptr(tl_f), N.ptr(ws), ws_bytes)
             struct = N.BlockPlanStruct(B, N.ptr(group_off), N.ptr(src_f), N.ptr(tl_f), self.status.data_ptr() + 4)
             self._block = (struct, group_off, src_f, tl_f, B)
         return self._block[0]

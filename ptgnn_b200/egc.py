@@ -94,13 +94,9 @@ class EGCMessagePassingLayer(AbstractMessagePassingLayer):
         ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=h.device)
         result = torch.empty(n, out, dtype=h.dtype, device=h.device)
         bp = plan.block_plan()
-        with torch.cuda.device(h.device):
-            rc = lib.ptgnn_b200_egc_forward_fused(
-                int(bf16), N.ptr(h), n, in_dim, out, heads, bases, T, ctypes.byref(bp), N.ptr(plan.row_ptr), N.ptr_table(weights), N.ptr(cw),
-                N.ptr(cb), reduce, N.ptr(result), N.ptr(ws), ws_bytes, N.ptr(cache), 0 if cache is None else cache.numel(), int(valid),
-                N.current_stream(h.device),
-            )
-        N.check(rc, "ptgnn_b200_egc_forward_fused")
+        N.call("ptgnn_b200_egc_forward_fused", h.device, int(bf16), N.ptr(h), n, in_dim, out, heads, bases, T, ctypes.byref(bp),
+               N.ptr(plan.row_ptr), N.ptr_table(weights), N.ptr(cw), N.ptr(cb), reduce, N.ptr(result), N.ptr(ws), ws_bytes, N.ptr(cache),
+               0 if cache is None else cache.numel(), int(valid))
         self._weight_cache_filled(kind, h.device)
         return result
 

@@ -94,10 +94,8 @@ def native_embedding_bag(table: torch.Tensor, ids: torch.Tensor, lengths: Option
         raise ValueError(f"out must be an aligned contiguous {(B, D)} {out_dtype} tensor")
     arg = torch.empty(B, D, dtype=torch.uint8, device=table.device) if want_arg and mode == "max" else None
     if B and S:
-        with torch.cuda.device(table.device):
-            rc = N.lib().ptgnn_b200_embedding_bag(int(out_dtype == torch.bfloat16), N.ptr(table), V, D, N.ptr(ids), N.ptr(lengths), B, S,
-                                                  N.POOL[mode], N.ptr(out), N.ptr(arg), N.ptr(status), N.current_stream(table.device))
-        N.check(rc, "ptgnn_b200_embedding_bag")
+        N.call("ptgnn_b200_embedding_bag", table.device, int(out_dtype == torch.bfloat16), N.ptr(table), V, D, N.ptr(ids), N.ptr(lengths), B,
+               S, N.POOL[mode], N.ptr(out), N.ptr(arg), N.ptr(status))
     elif B:
         out.fill_(-math.inf if mode == "max" else 0.0)
     return (out, arg) if want_arg else out
@@ -109,9 +107,7 @@ def occurrence_plan(ids: torch.Tensor, lengths: Optional[torch.Tensor], vocab: i
     B, S = ids.shape
     dev = ids.device
     src, tgt = torch.empty(B * S, dtype=torch.int64, device=dev), torch.empty(B * S, dtype=torch.int64, device=dev)
-    with torch.cuda.device(dev):
-        rc = N.lib().ptgnn_b200_embedding_bag_pairs(N.ptr(ids), N.ptr(lengths), B, S, vocab, N.ptr(src), N.ptr(tgt), N.current_stream(dev))
-    N.check(rc, "ptgnn_b200_embedding_bag_pairs")
+    N.call("ptgnn_b200_embedding_bag_pairs", dev, N.ptr(ids), N.ptr(lengths), B, S, vocab, N.ptr(src), N.ptr(tgt))
     plan = EdgePlan([(src, tgt)], vocab + 1, num_source_nodes=B)
     plan.perm                           # the sorted arrays are built on first access
     return plan
@@ -142,10 +138,8 @@ def native_embedding_bag_backward(d_out: torch.Tensor, ids: torch.Tensor, length
         raise ValueError("plan does not belong to these ids")
     ws_bytes = lib.ptgnn_b200_embedding_bag_backward_workspace_bytes(B, S, vocab, D)
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        rc = lib.ptgnn_b200_embedding_bag_backward_f32(N.ptr(d_out), B, S, D, N.ptr(lengths), N.ptr(arg), N.POOL[mode], N.ptr(plan.row_ptr),
-                                                       N.ptr(plan.perm), vocab, N.ptr(d_table), N.ptr(ws), ws_bytes, N.current_stream(dev))
-    N.check(rc, "ptgnn_b200_embedding_bag_backward_f32")
+    N.call("ptgnn_b200_embedding_bag_backward_f32", dev, N.ptr(d_out), B, S, D, N.ptr(lengths), N.ptr(arg), N.POOL[mode], N.ptr(plan.row_ptr),
+           N.ptr(plan.perm), vocab, N.ptr(d_table), N.ptr(ws), ws_bytes)
     return d_table
 
 
@@ -331,10 +325,7 @@ def char_cnn_prepare(shape, w1, b1, w2, b2, w3, bf16: bool, status: Optional[tor
     off = (-buf.data_ptr()) % 1024
     prepared = buf[off:off + nbytes]
     ws = [N.require_cuda(t.detach(), name, torch.float32) for t, name in ((w1, "W1"), (b1, "b1"), (w2, "W2"), (b2, "b2"), (w3, "W3"))]
-    with torch.cuda.device(dev):
-        rc = lib.ptgnn_b200_char_cnn_prepare(int(bf16), *[N.ptr(t) for t in ws], *shape, N.ptr(prepared), nbytes, N.ptr(status),
-                                             N.current_stream(dev))
-    N.check(rc, "ptgnn_b200_char_cnn_prepare")
+    N.call("ptgnn_b200_char_cnn_prepare", dev, int(bf16), *[N.ptr(t) for t in ws], *shape, N.ptr(prepared), nbytes, N.ptr(status))
     return prepared
 
 
@@ -351,10 +342,8 @@ def native_char_cnn(chars: torch.Tensor, shape, prepared: torch.Tensor, bf16: bo
     out = torch.empty(B, D, dtype=torch.bfloat16 if bf16 else torch.float32, device=chars.device)
     arg = torch.empty(B, D, dtype=torch.uint8, device=chars.device) if want_arg else None
     if B:
-        with torch.cuda.device(chars.device):
-            rc = N.lib().ptgnn_b200_char_cnn_forward(int(bf16), N.ptr(chars), B, L, *shape, N.ptr(prepared), prepared.numel(), N.ptr(out),
-                                                     N.ptr(arg), N.ptr(status), N.current_stream(chars.device))
-        N.check(rc, "ptgnn_b200_char_cnn_forward")
+        N.call("ptgnn_b200_char_cnn_forward", chars.device, int(bf16), N.ptr(chars), B, L, *shape, N.ptr(prepared), prepared.numel(),
+               N.ptr(out), N.ptr(arg), N.ptr(status))
     return (out, arg) if want_arg else out
 
 
@@ -367,10 +356,8 @@ def native_char_cnn_materialise(chars: torch.Tensor, shape, prepared: torch.Tens
     a1 = torch.empty(B * L1, F1, dtype=torch.float32, device=chars.device)
     a2 = torch.empty(B * L2, F2, dtype=torch.float32, device=chars.device)
     if B:
-        with torch.cuda.device(chars.device):
-            rc = N.lib().ptgnn_b200_char_cnn_materialise_f32(N.ptr(chars), B, L, *shape, N.ptr(prepared), prepared.numel(), N.ptr(a1), N.ptr(a2),
-                                                             None, N.current_stream(chars.device))
-        N.check(rc, "ptgnn_b200_char_cnn_materialise_f32")
+        N.call("ptgnn_b200_char_cnn_materialise_f32", chars.device, N.ptr(chars), B, L, *shape, N.ptr(prepared), prepared.numel(), N.ptr(a1),
+               N.ptr(a2), None)
     return a1, a2
 
 

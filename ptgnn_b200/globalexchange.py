@@ -174,13 +174,9 @@ class GruGlobalStateUpdate(AbstractGlobalGraphExchange):
         packed_out = None
         if chain is not None and chain.want_output:
             packed_out = torch.empty(max(lib.ptgnn_b200_packed_state_bytes(num_nodes, H), 1), dtype=torch.uint8, device=h.device)
-        with torch.cuda.device(h.device):
-            rc = lib.ptgnn_b200_global_gru_update(
-                int(bf16), N.ptr(h), N.ptr(packed_in), num_nodes, H, N.ptr(plan.tgt32), plan.num_nodes, N.ptr(g), S, N.ptr(p[0]),
-                N.ptr(p[1]), N.ptr(p[2]), N.ptr(p[3]), N.ptr(out), N.ptr(packed_out), plan.status.data_ptr() + 4, N.ptr(ws), ws_bytes,
-                N.ptr(cache), 0 if cache is None else cache.numel(), int(valid), N.current_stream(h.device),
-            )
-        N.check(rc, "ptgnn_b200_global_gru_update")
+        N.call("ptgnn_b200_global_gru_update", h.device, int(bf16), N.ptr(h), N.ptr(packed_in), num_nodes, H, N.ptr(plan.tgt32), plan.num_nodes,
+               N.ptr(g), S, N.ptr(p[0]), N.ptr(p[1]), N.ptr(p[2]), N.ptr(p[3]), N.ptr(out), N.ptr(packed_out), plan.status.data_ptr() + 4,
+               N.ptr(ws), ws_bytes, N.ptr(cache), 0 if cache is None else cache.numel(), int(valid))
         self._weight_cache_filled(kind, h.device)
         if chain is not None:
             chain.store(out, packed_out)

@@ -64,11 +64,8 @@ def native_graph_norm(x: torch.Tensor, plan: EdgePlan, gamma: torch.Tensor, alph
     mean = torch.empty(G, D, dtype=torch.float32, device=x.device)
     rstd = torch.empty(G, D, dtype=torch.float32, device=x.device)
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=x.device)
-    with torch.cuda.device(x.device):
-        rc = lib.ptgnn_b200_graph_norm_forward(int(bf16), N.ptr(x), num_nodes, D, N.ptr(plan.row_ptr), N.ptr(plan.perm),
-                                               N.ptr(plan.tgt32), G, N.ptr(g), N.ptr(a), N.ptr(b), float(eps), N.ptr(y), N.ptr(mean),
-                                               N.ptr(rstd), N.ptr(ws), ws_bytes, N.current_stream(x.device))
-    N.check(rc, "ptgnn_b200_graph_norm_forward")
+    N.call("ptgnn_b200_graph_norm_forward", x.device, int(bf16), N.ptr(x), num_nodes, D, N.ptr(plan.row_ptr), N.ptr(plan.perm),
+           N.ptr(plan.tgt32), G, N.ptr(g), N.ptr(a), N.ptr(b), float(eps), N.ptr(y), N.ptr(mean), N.ptr(rstd), N.ptr(ws), ws_bytes)
     return y, mean, rstd
 
 
@@ -87,11 +84,9 @@ def native_graph_norm_backward(x: torch.Tensor, plan: EdgePlan, gamma: torch.Ten
     d_x = torch.empty_like(x)
     d_params = torch.empty(3, D, dtype=torch.float32, device=x.device)
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=x.device)
-    with torch.cuda.device(x.device):
-        rc = lib.ptgnn_b200_graph_norm_backward_f32(N.ptr(x), N.ptr(d_y), num_nodes, D, N.ptr(plan.row_ptr), N.ptr(plan.perm), N.ptr(plan.tgt32),
-                                                    G, N.ptr(g), N.ptr(a), float(eps), N.ptr(mean), N.ptr(rstd), N.ptr(d_x), N.ptr(d_params[0]),
-                                                    N.ptr(d_params[1]), N.ptr(d_params[2]), N.ptr(ws), ws_bytes, N.current_stream(x.device))
-    N.check(rc, "ptgnn_b200_graph_norm_backward_f32")
+    N.call("ptgnn_b200_graph_norm_backward_f32", x.device, N.ptr(x), N.ptr(d_y), num_nodes, D, N.ptr(plan.row_ptr), N.ptr(plan.perm),
+           N.ptr(plan.tgt32), G, N.ptr(g), N.ptr(a), float(eps), N.ptr(mean), N.ptr(rstd), N.ptr(d_x), N.ptr(d_params[0]),
+           N.ptr(d_params[1]), N.ptr(d_params[2]), N.ptr(ws), ws_bytes)
     return d_x, d_params[0], d_params[1], d_params[2]
 
 

@@ -295,14 +295,10 @@ class GatedMessagePassingLayer(AbstractMessagePassingLayer):
             packed_out = None
             if chain is not None and chain.want_output:
                 packed_out = torch.empty(max(lib.ptgnn_b200_packed_state_bytes(num_nodes, H), 1), dtype=torch.uint8, device=h.device)
-            with torch.cuda.device(h.device):
-                rc = lib.ptgnn_b200_gated_forward_fused(
-                    int(bf16), N.ptr(h), N.ptr(gsrc), N.ptr(packed_in), num_nodes, ns, H, D, plan.num_types, ctypes.byref(bp),
-                    N.ptr(plan.row_ptr), N.ptr_table(weights), N.ptr(w_ih), N.ptr(w_hh), N.ptr(b_ih), N.ptr(b_hh), reduce, N.ptr(out),
-                    N.ptr(packed_out), N.ptr(ws), ws_bytes, N.ptr(cache), 0 if cache is None else cache.numel(), int(valid),
-                    N.current_stream(h.device),
-                )
-            N.check(rc, "ptgnn_b200_gated_forward_fused")
+            N.call("ptgnn_b200_gated_forward_fused", h.device, int(bf16), N.ptr(h), N.ptr(gsrc), N.ptr(packed_in), num_nodes, ns, H, D,
+                   plan.num_types, ctypes.byref(bp), N.ptr(plan.row_ptr), N.ptr_table(weights), N.ptr(w_ih), N.ptr(w_hh), N.ptr(b_ih),
+                   N.ptr(b_hh), reduce, N.ptr(out), N.ptr(packed_out), N.ptr(ws), ws_bytes, N.ptr(cache),
+                   0 if cache is None else cache.numel(), int(valid))
             self._weight_cache_filled(kind, h.device)
             if chain is not None:
                 chain.store(out, packed_out)
@@ -313,14 +309,9 @@ class GatedMessagePassingLayer(AbstractMessagePassingLayer):
         ws_bytes = lib.ptgnn_b200_gated_workspace_bytes(int(bf16), num_nodes, plan.num_edges, plan.num_types, H, D)
         ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=h.device)
         out = torch.empty_like(h)
-        with torch.cuda.device(h.device):
-            rc = lib.ptgnn_b200_gated_forward(
-                int(bf16), N.ptr(h), N.ptr(gsrc), num_nodes, H, D, plan.num_types, plan.type_off_c, N.ptr(plan.row_ptr), N.ptr(plan.pos),
-                N.ptr(plan.src32), N.ptr_table(weights), N.ptr(w_ih), N.ptr(w_hh), N.ptr(b_ih), N.ptr(b_hh), reduce,
-                N.ptr(out), N.ptr(ws), ws_bytes, N.ptr(cache), 0 if cache is None else cache.numel(), int(valid),
-                N.current_stream(h.device),
-            )
-        N.check(rc, "ptgnn_b200_gated_forward")
+        N.call("ptgnn_b200_gated_forward", h.device, int(bf16), N.ptr(h), N.ptr(gsrc), num_nodes, H, D, plan.num_types, plan.type_off_c,
+               N.ptr(plan.row_ptr), N.ptr(plan.pos), N.ptr(plan.src32), N.ptr_table(weights), N.ptr(w_ih), N.ptr(w_hh), N.ptr(b_ih),
+               N.ptr(b_hh), reduce, N.ptr(out), N.ptr(ws), ws_bytes, N.ptr(cache), 0 if cache is None else cache.numel(), int(valid))
         self._weight_cache_filled(kind, h.device)
         return out
 
@@ -559,28 +550,20 @@ class MlpMessagePassingLayer(AbstractMessagePassingLayer):
             cache_params = weights + ([d_w] if d_w is not None else [])
             cache, valid = self._weight_cache("mlp_f32_fused", 0 if bf16 else lib.ptgnn_b200_mlp_fused_weight_cache_bytes(
                 0, plan.num_types, H, D, out_dim, ut_i), cache_params, h.device)
-            with torch.cuda.device(h.device):
-                rc = lib.ptgnn_b200_mlp_forward_fused(
-                    int(bf16), N.ptr(h), N.ptr(gsrc), num_nodes, ns, H, D, out_dim, plan.num_types, ctypes.byref(bp), N.ptr(plan.row_ptr),
-                    N.ptr_table(weights), ut_i, reduce, msg_act, N.ptr(ln_w), N.ptr(ln_b), float(ln.eps) if ln is not None else 0.0,
-                    N.ptr(d_w), N.ptr(d_b), dense_act, N.ptr(out), N.ptr(ws), ws_bytes, N.ptr(cache), 0 if cache is None else cache.numel(),
-                    int(valid), N.current_stream(h.device),
-                )
-            N.check(rc, "ptgnn_b200_mlp_forward_fused")
+            N.call("ptgnn_b200_mlp_forward_fused", h.device, int(bf16), N.ptr(h), N.ptr(gsrc), num_nodes, ns, H, D, out_dim, plan.num_types,
+                   ctypes.byref(bp), N.ptr(plan.row_ptr), N.ptr_table(weights), ut_i, reduce, msg_act, N.ptr(ln_w), N.ptr(ln_b),
+                   float(ln.eps) if ln is not None else 0.0, N.ptr(d_w), N.ptr(d_b), dense_act, N.ptr(out), N.ptr(ws), ws_bytes,
+                   N.ptr(cache), 0 if cache is None else cache.numel(), int(valid))
             self._weight_cache_filled("mlp_f32_fused", h.device)
             return apply_dropout(out)
         # round-1 three-kernel path; bf16 states: fp32 parameters (converted inside the library), fp32 accumulation
         ws_bytes = lib.ptgnn_b200_mlp_workspace_bytes(int(bf16), num_nodes, plan.num_edges, plan.num_types, H, D, out_dim, ut_i)
         ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=h.device)
         out = torch.empty(num_nodes, out_dim, dtype=state_dtype, device=h.device)
-        with torch.cuda.device(h.device):
-            rc = lib.ptgnn_b200_mlp_forward(
-                int(bf16), N.ptr(h), N.ptr(gsrc), num_nodes, H, D, out_dim, plan.num_types, plan.type_off_c, N.ptr(plan.row_ptr), N.ptr(plan.pos),
-                N.ptr(plan.src32), N.ptr(plan.tgt32), N.ptr_table(weights), ut_i, reduce, msg_act, N.ptr(ln_w), N.ptr(ln_b),
-                float(ln.eps) if ln is not None else 0.0, N.ptr(d_w), N.ptr(d_b), dense_act, N.ptr(out), N.ptr(ws), ws_bytes,
-                N.current_stream(h.device),
-            )
-        N.check(rc, "ptgnn_b200_mlp_forward")
+        N.call("ptgnn_b200_mlp_forward", h.device, int(bf16), N.ptr(h), N.ptr(gsrc), num_nodes, H, D, out_dim, plan.num_types, plan.type_off_c,
+               N.ptr(plan.row_ptr), N.ptr(plan.pos), N.ptr(plan.src32), N.ptr(plan.tgt32), N.ptr_table(weights), ut_i, reduce, msg_act,
+               N.ptr(ln_w), N.ptr(ln_b), float(ln.eps) if ln is not None else 0.0, N.ptr(d_w), N.ptr(d_b), dense_act, N.ptr(out), N.ptr(ws),
+               ws_bytes)
         return apply_dropout(out)
 
     def _forward_composed(self, node_states, adjacency_lists, edge_features, gather_states, dropout_by_caller: bool = False) -> torch.Tensor:

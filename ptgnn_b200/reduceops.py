@@ -79,11 +79,8 @@ def native_readout(node_states: torch.Tensor, plan: EdgePlan, mode: int, gate_we
     g = torch.empty(G, H, dtype=torch.float32, device=x.device)
     s = torch.empty(num_nodes, dtype=torch.float32, device=x.device) if want_gates and w is not None else None
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=x.device)
-    with torch.cuda.device(x.device):
-        rc = lib.ptgnn_b200_graph_readout(int(bf16), N.ptr(x), num_nodes, H, N.ptr(plan.row_ptr),
-                                          N.ptr(plan.perm) if num_nodes else None, G, N.ptr(w), mode, N.ptr(g), N.ptr(s), N.ptr(ws),
-                                          ws_bytes, N.current_stream(x.device))
-    N.check(rc, "ptgnn_b200_graph_readout")
+    N.call("ptgnn_b200_graph_readout", x.device, int(bf16), N.ptr(x), num_nodes, H, N.ptr(plan.row_ptr), N.ptr(plan.perm) if num_nodes else None,
+           G, N.ptr(w), mode, N.ptr(g), N.ptr(s), N.ptr(ws), ws_bytes)
     return g, s
 
 
@@ -164,11 +161,8 @@ def native_attention_readout(node_states: torch.Tensor, plan: EdgePlan, qt: torc
     o = torch.empty(G, heads, D, dtype=torch.float32, device=x.device)
     lse = torch.empty(G, heads, dtype=torch.float32, device=x.device)
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=x.device)
-    with torch.cuda.device(x.device):
-        rc = lib.ptgnn_b200_attention_readout(int(bf16), N.ptr(x), num_nodes, D, heads, N.ptr(plan.row_ptr),
-                                              N.ptr(plan.perm) if num_nodes else None, G, N.ptr(q), N.ptr(o), N.ptr(lse), N.ptr(ws), ws_bytes,
-                                              N.current_stream(x.device))
-    N.check(rc, "ptgnn_b200_attention_readout")
+    N.call("ptgnn_b200_attention_readout", x.device, int(bf16), N.ptr(x), num_nodes, D, heads, N.ptr(plan.row_ptr),
+           N.ptr(plan.perm) if num_nodes else None, G, N.ptr(q), N.ptr(o), N.ptr(lse), N.ptr(ws), ws_bytes)
     return o, lse
 
 
@@ -189,12 +183,9 @@ def native_attention_readout_backward(node_states: torch.Tensor, plan: EdgePlan,
     d_x = torch.empty_like(x)
     d_qt = torch.empty(G, heads, D, dtype=torch.float32, device=x.device)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
-    with torch.cuda.device(x.device):
-        rc = lib.ptgnn_b200_attention_readout_backward_f32(N.ptr(x), num_nodes, D, heads, N.ptr(plan.row_ptr),
-                                                           N.ptr(plan.perm) if num_nodes else None, G, N.ptr(tabs[0]), N.ptr(tabs[1]),
-                                                           N.ptr(lse), N.ptr(tabs[2]), N.ptr(d_x), N.ptr(d_qt), N.ptr(ws), ws_bytes,
-                                                           N.current_stream(x.device))
-    N.check(rc, "ptgnn_b200_attention_readout_backward_f32")
+    N.call("ptgnn_b200_attention_readout_backward_f32", x.device, N.ptr(x), num_nodes, D, heads, N.ptr(plan.row_ptr),
+           N.ptr(plan.perm) if num_nodes else None, G, N.ptr(tabs[0]), N.ptr(tabs[1]), N.ptr(lse), N.ptr(tabs[2]), N.ptr(d_x), N.ptr(d_qt),
+           N.ptr(ws), ws_bytes)
     return d_x, d_qt
 
 

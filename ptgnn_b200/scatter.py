@@ -71,10 +71,8 @@ def _run(src: torch.Tensor, index: torch.Tensor, dim: int, dim_size: Optional[in
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=src.device)
     _poll_status()
     status = torch.zeros(1, dtype=torch.int32).pin_memory()     # written by the kernels, polled without synchronising
-    with torch.cuda.device(src.device):
-        rc = lib.ptgnn_b200_scatter_f32(N.ptr(src), N.ptr(index), E, D, dim_size, N.REDUCE[reduce], N.ptr(out), N.ptr(arg),
-                                        status.data_ptr(), N.ptr(ws), ws_bytes, N.current_stream(src.device))
-    N.check(rc, "ptgnn_b200_scatter_f32")
+    N.call("ptgnn_b200_scatter_f32", src.device, N.ptr(src), N.ptr(index), E, D, dim_size, N.REDUCE[reduce], N.ptr(out), N.ptr(arg),
+           status.data_ptr(), N.ptr(ws), ws_bytes)
     _PENDING.append((status, dim_size))
     return out, arg
 

@@ -51,10 +51,8 @@ def native_selfatt(t: torch.Tensor, plan: EdgePlan, heads: int, dk: int, dv: int
     o = torch.empty(rows, heads * dv, dtype=t.dtype, device=t.device)
     lse = torch.empty(rows, heads, dtype=torch.float32, device=t.device)
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=t.device)
-    with torch.cuda.device(t.device):
-        rc = lib.ptgnn_b200_selfatt_forward(int(bf16), N.ptr(t), rows, heads, dk, dv, N.ptr(plan.row_ptr), G, int(max_chunk),
-                                            N.ptr(o), N.ptr(lse), plan.status.data_ptr() + 4, N.ptr(ws), ws_bytes, N.current_stream(t.device))
-    N.check(rc, "ptgnn_b200_selfatt_forward")
+    N.call("ptgnn_b200_selfatt_forward", t.device, int(bf16), N.ptr(t), rows, heads, dk, dv, N.ptr(plan.row_ptr), G, int(max_chunk), N.ptr(o),
+           N.ptr(lse), plan.status.data_ptr() + 4, N.ptr(ws), ws_bytes)
     return o, lse
 
 
@@ -73,10 +71,8 @@ def native_selfatt_backward(t: torch.Tensor, plan: EdgePlan, heads: int, dk: int
     ws_bytes = lib.ptgnn_b200_selfatt_workspace_bytes(rows, G, heads)
     d_t = torch.empty_like(t)
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=t.device)
-    with torch.cuda.device(t.device):
-        rc = lib.ptgnn_b200_selfatt_backward_f32(N.ptr(t), rows, heads, dk, dv, N.ptr(plan.row_ptr), G, int(max_chunk), N.ptr(o), N.ptr(lse),
-                                                 N.ptr(d_o), N.ptr(d_t), N.ptr(ws), ws_bytes, N.current_stream(t.device))
-    N.check(rc, "ptgnn_b200_selfatt_backward_f32")
+    N.call("ptgnn_b200_selfatt_backward_f32", t.device, N.ptr(t), rows, heads, dk, dv, N.ptr(plan.row_ptr), G, int(max_chunk), N.ptr(o),
+           N.ptr(lse), N.ptr(d_o), N.ptr(d_t), N.ptr(ws), ws_bytes)
     return d_t
 
 

@@ -1,5 +1,6 @@
 """CPU-side checks of the drop-in boundary: the C-ABI library loads and exports every symbol the header declares, the
 module API mirrors the reference's, and the product refuses to run without CUDA (no CPU fallback)."""
+import ctypes
 import inspect
 import os
 import re
@@ -28,6 +29,36 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(handle, name), f"{name} declared in include/ptgnn_b200.h but not exported"
     assert sorted(N.SIGNATURES) == declared, "ctypes SIGNATURES must cover exactly the header's entry points"
     assert handle.ptgnn_b200_abi_version() == 4
+
+
+def test_signatures_are_parsed_from_the_header():
+    i32, i64, f32, size, P = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_size_t, ctypes.c_void_p
+    sig = N.SIGNATURES
+    assert sig["ptgnn_b200_last_error"] == (ctypes.c_char_p, [])
+    assert sig["ptgnn_b200_plan_workspace_bytes"] == (size, [i64, i64])
+    assert sig["ptgnn_b200_graph_norm_forward"] == (i32, [i32, P, i64, i32, P, P, P, i64, P, P, P, f32, P, P, P, P, size, P])
+    assert sig["ptgnn_b200_gated_forward_fused"] == (i32, [i32, P, P, P, i64, i64, i32, i32, i32, P, P, P, P, P, P, P, i32, P, P, P, size, P,
+                                                           size, i32, P])
+    assert N.parse_signatures("/* ptgnn_b200_x(double); */\n#define A 1\nint32_t ptgnn_b200_x(const float *const *w, float eps, // e\n"
+                              "  size_t n);\nint ptgnn_b200_y(void);") == {"ptgnn_b200_x": (i32, [P, f32, size]), "ptgnn_b200_y": (i32, [])}
+    for proto in ("int ptgnn_b200_x(double eps);", "int ptgnn_b200_x(unsigned n);", "void ptgnn_b200_x(int32_t n);",
+                  "float *ptgnn_b200_x(int32_t n);", "int ptgnn_b200_x();"):
+        with pytest.raises(N.NativeLibraryError, match="ptgnn_b200_x"):
+            N.parse_signatures(proto)
+
+
+def test_call_checks_the_argument_count_before_touching_cuda(monkeypatch):
+    def no_cuda(*args, **kwargs):
+        raise AssertionError("reached CUDA")
+
+    monkeypatch.setattr(torch.cuda, "device", no_cuda)
+    monkeypatch.setattr(N, "current_stream", no_cuda)
+    n = len(N.SIGNATURES["ptgnn_b200_segment_ids"][1]) - 1        # every parameter but the stream
+    for count in (n - 1, n + 1):
+        with pytest.raises(TypeError, match="ptgnn_b200_segment_ids"):
+            N.call("ptgnn_b200_segment_ids", "cuda", *[0] * count)
+    with pytest.raises(AssertionError, match="reached CUDA"):
+        N.call("ptgnn_b200_segment_ids", "cuda", *[0] * n)
 
 
 def test_fused_supported_shapes():
