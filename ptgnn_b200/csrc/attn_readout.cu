@@ -208,9 +208,17 @@ bool supported(int D, int heads) {
 
 // chunk_ptr [G + 1] | m [chunks, heads] | l [chunks, heads] | acc [chunks, heads, D]   (forward, chunks = N / CHUNK + G + 1)
 // chunk_ptr [G + 1] | dqt partials [chunks, heads, D]                                (backward: fits in the forward's layout)
-static size_t ws_ml(int64_t N, int64_t G, int heads) { return ws_slice(partial_rows(N, G) * heads, 4); }
-size_t workspace_bytes(int64_t N, int64_t G, int D, int heads) {
-    return ws_chunk_ptr(G) + 2 * ws_ml(N, G, heads) + ws_slice(partial_rows(N, G) * heads * D, 4);
+struct Ws { size_t chunk_ptr, m, l, acc, dq, total; };
+static Ws layout(int64_t N, int64_t G, int D, int heads) {
+    Layout l;
+    Ws w;
+    w.chunk_ptr = l.add((size_t)G + 1, 4);
+    w.m = l.add(partial_rows(N, G) * heads, 4);
+    w.l = l.add(partial_rows(N, G) * heads, 4);
+    w.acc = l.add(partial_rows(N, G) * heads * D, 4);
+    w.dq = w.m;
+    w.total = l.total;
+    return w;
 }
 
 #define PTGNN_ATTN_HEADS(VPL, HEADS_CASE)                                                                                              \
@@ -229,22 +237,22 @@ size_t workspace_bytes(int64_t N, int64_t G, int D, int heads) {
     }
 
 template <bool BF16>
-static void launch_forward(int D, int heads, int grid, cudaStream_t st, const void *x, const int32_t *row_ptr, const int32_t *perm,
-                           const int32_t *chunk_ptr, int G, const float *qt, float *m, float *l, float *acc) {
-#define PTGNN_FWD(V, H) attn_readout_chunk_kernel<V, H, BF16><<<grid, 256, 0, st>>>(x, row_ptr, perm, chunk_ptr, G, qt, m, l, acc)
+static int launch_forward(int D, int heads, int grid, cudaStream_t st, const void *x, const int32_t *row_ptr, const int32_t *perm,
+                          const int32_t *chunk_ptr, int G, const float *qt, float *m, float *l, float *acc) {
+#define PTGNN_FWD(V, H) return launch(PTGNN_KERNEL_REDUCE, st, attn_readout_chunk_kernel<V, H, BF16>, grid, 256, 0, x, row_ptr, perm, chunk_ptr, G, qt, m, l, acc)
     PTGNN_ATTN_DISPATCH(PTGNN_FWD)
 #undef PTGNN_FWD
 }
 
-static void launch_backward(int D, int heads, int64_t N, int64_t num_graphs, cudaStream_t st, const float *x, const int32_t *row_ptr,
-                            const int32_t *perm, const int32_t *chunk_ptr, int G, const float *qt, const float *o, const float *lse,
-                            const float *d_o, float *d_x, float *part_dq) {
+static int launch_backward(int D, int heads, int64_t N, int64_t num_graphs, cudaStream_t st, const float *x, const int32_t *row_ptr,
+                           const int32_t *perm, const int32_t *chunk_ptr, int G, const float *qt, const float *o, const float *lse,
+                           const float *d_o, float *d_x, float *part_dq) {
 #define PTGNN_BWD(V, H)                                                                                                                \
-    do {                                                                                                                               \
+    {                                                                                                                                  \
         constexpr int W = Bwd<V, H>::WARPS;                                                                                            \
-        attn_readout_backward_chunk_kernel<V, H><<<chunk_grid(N, num_graphs, W), 32 * W, 0, st>>>(x, row_ptr, perm, chunk_ptr, G, qt, o,  \
-                                                                                                  lse, d_o, d_x, part_dq);             \
-    } while (0)
+        return launch(PTGNN_KERNEL_REDUCE, st, attn_readout_backward_chunk_kernel<V, H>, chunk_grid(N, num_graphs, W), 32 * W, 0, x, row_ptr, \
+                      perm, chunk_ptr, G, qt, o, lse, d_o, d_x, part_dq);                                                              \
+    }
     PTGNN_ATTN_DISPATCH(PTGNN_BWD)
 #undef PTGNN_BWD
 }
@@ -261,7 +269,7 @@ extern "C" int32_t ptgnn_b200_attention_readout_supported(int32_t bf16_states, i
 
 extern "C" size_t ptgnn_b200_attention_readout_workspace_bytes(int64_t num_nodes, int64_t num_graphs, int32_t state_dim, int32_t num_heads) {
     if (num_nodes < 0 || num_graphs < 0 || !attn_readout::supported(state_dim, num_heads)) return 0;
-    return attn_readout::workspace_bytes(num_nodes, num_graphs, state_dim, num_heads);
+    return attn_readout::layout(num_nodes, num_graphs, state_dim, num_heads).total;
 }
 
 // shared argument checks of the two entry points; returns PTGNN_OK or an error code (set_error done)
@@ -274,7 +282,7 @@ static int attn_check(const char *what, const void *x, int64_t num_nodes, int32_
     }
     if (num_graphs == 0) return PTGNN_OK;
     PTGNN_CHECK_ARG(row_ptr && qt && o && lse && (num_nodes == 0 || (x && perm)), "%s: null pointer", what);
-    PTGNN_CHECK_WORKSPACE(what, workspace, workspace_bytes, attn_readout::workspace_bytes(num_nodes, num_graphs, D, heads));
+    PTGNN_CHECK_WORKSPACE(what, workspace, workspace_bytes, attn_readout::layout(num_nodes, num_graphs, D, heads).total);
     return PTGNN_OK;
 }
 
@@ -287,30 +295,20 @@ extern "C" int ptgnn_b200_attention_readout(int32_t bf16_states, const void *nod
                               workspace_bytes);
     if (rc != PTGNN_OK || num_graphs == 0) return rc;
     const int G = (int)num_graphs;
+    const attn_readout::Ws L = attn_readout::layout(num_nodes, num_graphs, D, heads);
     char *ws = static_cast<char *>(workspace);
-    int32_t *chunk_ptr = reinterpret_cast<int32_t *>(ws);
-    const size_t ml = attn_readout::ws_ml(num_nodes, num_graphs, heads);
-    float *part_m = reinterpret_cast<float *>(ws + pergraph::ws_chunk_ptr(num_graphs));
-    float *part_l = reinterpret_cast<float *>(ws + pergraph::ws_chunk_ptr(num_graphs) + ml);
-    float *part_acc = reinterpret_cast<float *>(ws + pergraph::ws_chunk_ptr(num_graphs) + 2 * ml);
-    pergraph::launch_chunk_ptr(row_ptr, G, chunk_ptr, st);
-    PTGNN_LAUNCHED();
+    int32_t *chunk_ptr = reinterpret_cast<int32_t *>(ws + L.chunk_ptr);
+    float *part_m = reinterpret_cast<float *>(ws + L.m);
+    float *part_l = reinterpret_cast<float *>(ws + L.l);
+    float *part_acc = reinterpret_cast<float *>(ws + L.acc);
+    PTGNN_TRY(pergraph::launch_chunk_ptr(row_ptr, G, chunk_ptr, st));
     if (num_nodes > 0) {
         const int grid = pergraph::chunk_grid(num_nodes, num_graphs);
-        {
-            TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-            if (bf16_states) attn_readout::launch_forward<true>(D, heads, grid, st, node_states, row_ptr, perm, chunk_ptr, G, qt, part_m, part_l, part_acc);
-            else attn_readout::launch_forward<false>(D, heads, grid, st, node_states, row_ptr, perm, chunk_ptr, G, qt, part_m, part_l, part_acc);
-        }
-        PTGNN_LAUNCHED();
+        if (bf16_states) PTGNN_TRY(attn_readout::launch_forward<true>(D, heads, grid, st, node_states, row_ptr, perm, chunk_ptr, G, qt, part_m, part_l, part_acc));
+        else PTGNN_TRY(attn_readout::launch_forward<false>(D, heads, grid, st, node_states, row_ptr, perm, chunk_ptr, G, qt, part_m, part_l, part_acc));
     }
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        attn_readout::attn_readout_finalize_kernel<<<(unsigned)ceil_div((int64_t)G * heads * D, 256), 256, 0, st>>>(part_m, part_l, part_acc,
-                                                                                                                     chunk_ptr, G, heads, D, o, lse);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch(PTGNN_KERNEL_REDUCE, st, attn_readout::attn_readout_finalize_kernel, (unsigned)ceil_div((int64_t)G * heads * D, 256), 256, 0,
+                  part_m, part_l, part_acc, chunk_ptr, G, heads, D, o, lse);
 }
 
 extern "C" int ptgnn_b200_attention_readout_backward_f32(const float *node_states, int64_t num_nodes, int32_t state_dim, int32_t num_heads,
@@ -324,20 +322,13 @@ extern "C" int ptgnn_b200_attention_readout_backward_f32(const float *node_state
     if (rc != PTGNN_OK || num_graphs == 0) return rc;
     PTGNN_CHECK_ARG(d_o && d_qt && (num_nodes == 0 || d_x), "attention_readout_backward: null pointer");
     const int G = (int)num_graphs;
+    const attn_readout::Ws L = attn_readout::layout(num_nodes, num_graphs, D, heads);
     char *ws = static_cast<char *>(workspace);
-    int32_t *chunk_ptr = reinterpret_cast<int32_t *>(ws);
-    float *part_dq = reinterpret_cast<float *>(ws + pergraph::ws_chunk_ptr(num_graphs));
-    pergraph::launch_chunk_ptr(row_ptr, G, chunk_ptr, st);
-    PTGNN_LAUNCHED();
-    if (num_nodes > 0) {
-        {
-            TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-            attn_readout::launch_backward(D, heads, num_nodes, num_graphs, st, node_states, row_ptr, perm, chunk_ptr, G, qt, o, lse, d_o, d_x,
-                                          part_dq);
-        }
-        PTGNN_LAUNCHED();
-    }
-    pergraph::launch_chunk_sum(part_dq, row_ptr, chunk_ptr, G, heads * D, d_qt, st);
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    int32_t *chunk_ptr = reinterpret_cast<int32_t *>(ws + L.chunk_ptr);
+    float *part_dq = reinterpret_cast<float *>(ws + L.dq);
+    PTGNN_TRY(pergraph::launch_chunk_ptr(row_ptr, G, chunk_ptr, st));
+    if (num_nodes > 0)
+        PTGNN_TRY(attn_readout::launch_backward(D, heads, num_nodes, num_graphs, st, node_states, row_ptr, perm, chunk_ptr, G, qt, o, lse, d_o,
+                                                d_x, part_dq));
+    return pergraph::launch_chunk_sum(part_dq, row_ptr, chunk_ptr, G, heads * D, d_qt, st);
 }

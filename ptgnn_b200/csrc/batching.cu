@@ -51,12 +51,8 @@ extern "C" int ptgnn_b200_offset_ids(const int32_t *local_ids, int64_t num_items
     if (num_items == 0) return PTGNN_OK;
     PTGNN_CHECK_ARG(num_graphs > 0 && local_ids && item_ptr && node_ptr && out, "offset_ids: null pointer / no graphs");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    {
-        TimedScope timed__(PTGNN_KERNEL_PLAN, st);
-        segment_map_kernel<true><<<grid_for(num_items), 256, 0, st>>>(local_ids, num_items, item_ptr, node_ptr, num_graphs, out);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch(PTGNN_KERNEL_PLAN, st, segment_map_kernel<true>, grid_for(num_items), 256, 0, local_ids, num_items, item_ptr, node_ptr, num_graphs,
+                  out);
 }
 
 extern "C" int ptgnn_b200_segment_ids(const int64_t *item_ptr, int32_t num_segments, int64_t num_items, int64_t *out, void *stream) {
@@ -65,10 +61,6 @@ extern "C" int ptgnn_b200_segment_ids(const int64_t *item_ptr, int32_t num_segme
     if (num_items == 0) return PTGNN_OK;
     PTGNN_CHECK_ARG(num_segments > 0 && item_ptr && out, "segment_ids: null pointer / no segments");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    {
-        TimedScope timed__(PTGNN_KERNEL_PLAN, st);
-        segment_map_kernel<false><<<grid_for(num_items), 256, 0, st>>>(nullptr, num_items, item_ptr, nullptr, num_segments, out);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch(PTGNN_KERNEL_PLAN, st, segment_map_kernel<false>, grid_for(num_items), 256, 0, nullptr, num_items, item_ptr, nullptr, num_segments,
+                  out);
 }

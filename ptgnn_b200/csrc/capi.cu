@@ -2,17 +2,19 @@
 // host-buffer entry point used for end-to-end measurement.
 #include <stdarg.h>
 
+#include <atomic>
 #include <mutex>
 #include <vector>
 
 #include "common.cuh"
 #include "fused_mp.cuh"
 #include "gru_ws.cuh"
+#include "layers.cuh"
 
 namespace ptgnn {
 
 static thread_local char g_error[512] = "";
-std::atomic<int64_t> g_launch_count{0};
+static std::atomic<int64_t> g_launch_count{0};
 
 void set_error(const char *fmt, ...) {
     va_list ap;
@@ -38,6 +40,12 @@ TimedScope::~TimedScope() {
         std::lock_guard<std::mutex> lk(g_timing_mu);
         g_timing_records.push_back({cat, a, b});
     }
+}
+
+int launched() {
+    g_launch_count.fetch_add(1);
+    PTGNN_CUDA(cudaGetLastError());
+    return PTGNN_OK;
 }
 
 int sm_count() {
@@ -212,15 +220,16 @@ extern "C" int ptgnn_b200_gated_gnn_forward_host_f32(const float *node_states, i
 // ---- GruGlobalStateUpdate: input-side table + state-only weights-stationary GRU ---------------------------------------
 namespace {
 // workspace: gi table [G, 3H] fp32 | linear's workspace | packed states (fp32, when not handed in) | packed weights (no cache)
-struct GlobalGruWs { size_t gi, lin, xpack, wpack, total; };
+struct GlobalGruWs { size_t gi, lin, xpack, wpack, total, lin_bytes; };
 GlobalGruWs global_gru_layout(int bf16, int64_t N, int64_t G, int H, int S) {
-    GlobalGruWs w{};
-    const int nprod = bf16 ? 1 : 3;
-    w.gi = 0;
-    w.lin = ws_slice((size_t)G * 3 * H, 4);
-    w.xpack = w.lin + align_up(ptgnn_b200_linear_workspace_bytes(S, 3 * H), 256);
-    w.wpack = w.xpack + (bf16 ? 0 : align_up(fused::packed_state_bytes(3, N, H), 256));
-    w.total = w.wpack + align_up(gruws::pack_table_bytes(nprod, H), 256);
+    Layout l;
+    GlobalGruWs w;
+    w.gi = l.add((size_t)G * 3 * H, 4);
+    w.lin_bytes = ws_slice(ptgnn_b200_linear_workspace_bytes(S, 3 * H), 1);
+    w.lin = l.add_bytes(w.lin_bytes);
+    w.xpack = l.add(bf16 ? 0 : fused::packed_state_bytes(3, N, H), 1);
+    w.wpack = l.add(gruws::pack_table_bytes(bf16 ? 1 : 3, H), 1);
+    w.total = l.total;
     return w;
 }
 }  // namespace
@@ -259,23 +268,13 @@ extern "C" int ptgnn_b200_global_gru_update(int32_t bf16_states, const void *nod
     const GlobalGruWs L = global_gru_layout(bf16_states, num_nodes, num_graphs, H, S);
     PTGNN_CHECK_WORKSPACE("global_gru", workspace, workspace_bytes, L.total);
     char *ws = static_cast<char *>(workspace);
-    char *wpack = ws + L.wpack;
-    bool pack = true;
-    if (weight_cache != nullptr) {
-        if (weight_cache_bytes < gruws::pack_table_bytes(nprod, H)) {
-            set_error("global_gru: weight cache %zu < required %zu", weight_cache_bytes, gruws::pack_table_bytes(nprod, H));
-            return PTGNN_E_WORKSPACE;
-        }
-        wpack = static_cast<char *>(weight_cache);
-        pack = !cache_valid;
-    }
-    if (pack) {
-        int rc = gruws::pack_table(nprod, H, gru_w_hh, gru_b_hh, wpack, st);
-        if (rc) return rc;
-    }
+    char *wpack;
+    bool pack;
+    PTGNN_TRY(weight_area("global_gru", ws + L.wpack, weight_cache, weight_cache_bytes, gruws::pack_table_bytes(nprod, H), cache_valid, wpack, pack));
+    if (pack) PTGNN_TRY(gruws::pack_table(nprod, H, gru_w_hh, gru_b_hh, wpack, st));
     // the input side, once per graph: gi = g W_ih^T + b_ih  [G, 3H]
     float *gi = reinterpret_cast<float *>(ws + L.gi);
-    int rc = ptgnn_b200_linear_f32(g, num_graphs, S, gru_w_ih, gru_b_ih, 3 * H, PTGNN_ACT_NONE, gi, ws + L.lin, L.xpack - L.lin, st);
+    int rc = ptgnn_b200_linear_f32(g, num_graphs, S, gru_w_ih, gru_b_ih, 3 * H, PTGNN_ACT_NONE, gi, ws + L.lin, L.lin_bytes, st);
     if (rc) return rc;
     const void *h_rows = node_states;
     if (!bf16_states) {

@@ -399,26 +399,18 @@ __global__ void __launch_bounds__(128 * NWG, 1) char_cnn_kernel(const Args a) {
 }
 
 template <bool BF16, int NWG>
-static int launch(const Args &a, cudaStream_t st) {
+static int launch_cnn(const Args &a, cudaStream_t st) {
     using K = Cfg<BF16, NWG>;
-    const size_t smem = K::smem(a.s.F1, a.s.F2);
-    auto kern = char_cnn_kernel<BF16, NWG>;
-    PTGNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int T = min(K::M / a.s.L1(), K::TMAX);
     const long long tiles = (a.B + T - 1) / T;
     const int grid = (int)(tiles < sm_count() ? tiles : sm_count());
-    {
-        TimedScope timed__(PTGNN_KERNEL_DENSE, st);
-        kern<<<grid, K::THREADS, smem, st>>>(a);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch(PTGNN_KERNEL_DENSE, st, char_cnn_kernel<BF16, NWG>, grid, K::THREADS, K::smem(a.s.F1, a.s.F2), a);
 }
 
 template <bool BF16>
 static int run(const Args &a, cudaStream_t st) {
     // two warpgroups (128 rows) when a2 can overwrite a1 (F2 <= 128), else one (64 rows) so that both regions fit
-    return Cfg<BF16, 2>::alias(a.s.F2) ? launch<BF16, 2>(a, st) : launch<BF16, 1>(a, st);
+    return Cfg<BF16, 2>::alias(a.s.F2) ? launch_cnn<BF16, 2>(a, st) : launch_cnn<BF16, 1>(a, st);
 }
 
 }  // namespace charcnn
@@ -460,20 +452,11 @@ extern "C" int ptgnn_b200_char_cnn_prepare(int32_t bf16, const float *w1, const 
     uint8_t *base = static_cast<uint8_t *>(prepared);
     float *t1 = reinterpret_cast<float *>(base + p.t1), *b1o = reinterpret_cast<float *>(base + p.b1), *b2o = reinterpret_cast<float *>(base + p.b2);
     const int grid = 4 * sm_count();
-    {
-        TimedScope timed__(PTGNN_KERNEL_PACK, st);
-        if (bf16) {
-            charcnn::prepare_t1_kernel<true><<<grid, 256, 0, st>>>(w1, b1, b2, chars, l1_filters, l1_window, l2_filters, t1, b1o, b2o);
-            charcnn::prepare_stage_kernel<true><<<grid, 256, 0, st>>>(w2, l2_filters, l1_filters, l2_window, base + p.w2, status);
-            charcnn::prepare_stage_kernel<true><<<grid, 256, 0, st>>>(w3, dim, l2_filters, out_window, base + p.w3, status);
-        } else {
-            charcnn::prepare_t1_kernel<false><<<grid, 256, 0, st>>>(w1, b1, b2, chars, l1_filters, l1_window, l2_filters, t1, b1o, b2o);
-            charcnn::prepare_stage_kernel<false><<<grid, 256, 0, st>>>(w2, l2_filters, l1_filters, l2_window, base + p.w2, status);
-            charcnn::prepare_stage_kernel<false><<<grid, 256, 0, st>>>(w3, dim, l2_filters, out_window, base + p.w3, status);
-        }
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    auto t1_kernel = bf16 ? charcnn::prepare_t1_kernel<true> : charcnn::prepare_t1_kernel<false>;
+    auto stage_kernel = bf16 ? charcnn::prepare_stage_kernel<true> : charcnn::prepare_stage_kernel<false>;
+    PTGNN_TRY(launch(PTGNN_KERNEL_PACK, st, t1_kernel, grid, 256, 0, w1, b1, b2, chars, l1_filters, l1_window, l2_filters, t1, b1o, b2o));
+    PTGNN_TRY(launch(PTGNN_KERNEL_PACK, st, stage_kernel, grid, 256, 0, w2, l2_filters, l1_filters, l2_window, base + p.w2, status));
+    return launch(PTGNN_KERNEL_PACK, st, stage_kernel, grid, 256, 0, w3, dim, l2_filters, out_window, base + p.w3, status);
 }
 
 static int char_cnn_common(int32_t bf16, const int64_t *ids, int64_t rows, int32_t max_chars, int32_t chars, int32_t l1_filters,

@@ -6,15 +6,12 @@
 #include <stdint.h>
 #include <stdio.h>
 
-#include <atomic>
-
 #include "../../include/ptgnn_b200.h"
 
 namespace ptgnn {
 
 // ---- error reporting ---------------------------------------------------------------------------
 void set_error(const char *fmt, ...);
-extern std::atomic<int64_t> g_launch_count;
 
 #define PTGNN_CHECK_ARG(cond, ...)      \
     do {                                \
@@ -44,6 +41,13 @@ extern std::atomic<int64_t> g_launch_count;
         }                                                                                         \
     } while (0)
 
+// Returns the status of `call` (a PTGNN_* code) unless it is PTGNN_OK.
+#define PTGNN_TRY(call)                        \
+    do {                                       \
+        const int rc__ = (call);               \
+        if (rc__ != PTGNN_OK) return rc__;     \
+    } while (0)
+
 // RAII bracket around one kernel launch: when per-kernel timing is enabled (bench.py's roofline leg) it records a
 // CUDA event on the launch stream before and after; otherwise it costs one relaxed atomic load.
 struct TimedScope {
@@ -54,17 +58,40 @@ struct TimedScope {
     ~TimedScope();
 };
 
-// Call right after a kernel launch: counts it and surfaces launch-configuration errors.
-#define PTGNN_LAUNCHED()                                   \
-    do {                                                   \
-        ::ptgnn::g_launch_count.fetch_add(1);              \
-        PTGNN_CUDA(cudaGetLastError());                    \
-    } while (0)
+// Counts one launch and turns a launch-configuration error into PTGNN_E_CUDA.
+int launched();
+
+// The only way the library launches a kernel: raises the kernel's dynamic shared-memory limit when `smem` is above the
+// 48 KB default (a per-device attribute, so set on every such launch), brackets the launch with a timing record of
+// `category` (PTGNN_KERNEL_*), and counts it, so ptgnn_b200_launch_count and the timing records see every launch once.
+template <class... P, class... A>
+int launch(int category, cudaStream_t st, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, A &&...args) {
+    if (smem > 48 * 1024) PTGNN_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    {
+        TimedScope timed(category, st);
+        kernel<<<grid, block, smem, st>>>(static_cast<A &&>(args)...);
+    }
+    return launched();
+}
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
 static inline size_t ws_slice(size_t count, size_t elt) { return align_up(count * elt, 256); }
+
+// A workspace layout written once: slices are added in order, each at the running offset, and the running offset is the
+// total the size query reports and the entry point checks.
+struct Layout {
+    size_t total = 0;
+    // a slice of `count` elements of `elt` bytes, rounded up to 256 bytes
+    size_t add(size_t count, size_t elt) { return add_bytes(ws_slice(count, elt)); }
+    // a slice of exactly `bytes` bytes (for sizes that are already aligned or pad on their own)
+    size_t add_bytes(size_t bytes) {
+        const size_t at = total;
+        total += bytes;
+        return at;
+    }
+};
 
 // SM count of the CURRENT device, queried per launch: a process may drive several GPUs (nothing cached across devices).
 int sm_count();

@@ -167,10 +167,17 @@ __global__ void __launch_bounds__(256, 1) copy_attn_backward_chunk_kernel(
 bool supported(int D, int steps) { return (D == 32 || D == 64 || D == 128 || D == 256) && steps >= 1 && steps <= 8; }
 
 // chunk_ptr [G + 1] | m [chunks, steps] | l [chunks, steps]        (forward, chunks = M / CHUNK + G + 1)
-// chunk_ptr [G + 1] | dO partials [chunks, steps, D]                 (backward)
-static size_t ws_ml(int64_t N, int64_t G, int steps) { return ws_slice(partial_rows(N, G) * steps, 4); }
-size_t workspace_bytes(int64_t N, int64_t G, int D, int steps) {
-    return ws_chunk_ptr(G) + std::max(2 * ws_ml(N, G, steps), ws_slice(partial_rows(N, G) * steps * D, 4));
+// chunk_ptr [G + 1] | dO partials [chunks, steps, D]                 (backward, over the forward's m and l)
+struct Ws { size_t chunk_ptr, m, l, d_o, total; };
+static Ws layout(int64_t N, int64_t G, int D, int steps) {
+    Layout l;
+    Ws w;
+    w.chunk_ptr = l.add((size_t)G + 1, 4);
+    const size_t ml = ws_slice(partial_rows(N, G) * steps, 4);
+    w.m = w.d_o = l.add_bytes(std::max(2 * ml, ws_slice(partial_rows(N, G) * steps * D, 4)));
+    w.l = w.m + ml;
+    w.total = l.total;
+    return w;
 }
 
 #define PTGNN_COPY_STEPS(VPL, STEPS_CASE)                                                                                              \
@@ -189,18 +196,19 @@ size_t workspace_bytes(int64_t N, int64_t G, int D, int steps) {
     }
 
 template <bool BF16>
-static void launch_forward(int D, int steps, int grid, cudaStream_t st, const void *c, const int32_t *row_ptr, const int32_t *perm,
-                           const int32_t *chunk_ptr, int G, const float *o, float *s, float *m, float *l) {
-#define PTGNN_FWD(V, S) copy_attn_chunk_kernel<V, S, BF16><<<grid, 256, 0, st>>>(c, row_ptr, perm, chunk_ptr, G, steps, o, s, m, l)
+static int launch_forward(int D, int steps, int grid, cudaStream_t st, const void *c, const int32_t *row_ptr, const int32_t *perm,
+                          const int32_t *chunk_ptr, int G, const float *o, float *s, float *m, float *l) {
+#define PTGNN_FWD(V, S) return launch(PTGNN_KERNEL_REDUCE, st, copy_attn_chunk_kernel<V, S, BF16>, grid, 256, 0, c, row_ptr, perm, chunk_ptr, G, steps, o, s, m, l)
     PTGNN_COPY_DISPATCH(PTGNN_FWD)
 #undef PTGNN_FWD
 }
 
-static void launch_backward(int D, int steps, int grid, cudaStream_t st, const float *c, const int32_t *row_ptr, const int32_t *perm,
-                            const int32_t *chunk_ptr, int G, const float *o, const float *lse, const float *d_s, const float *d_lse,
-                            float *d_c, float *part_do) {
+static int launch_backward(int D, int steps, int grid, cudaStream_t st, const float *c, const int32_t *row_ptr, const int32_t *perm,
+                           const int32_t *chunk_ptr, int G, const float *o, const float *lse, const float *d_s, const float *d_lse,
+                           float *d_c, float *part_do) {
 #define PTGNN_BWD(V, S)                                                                                                                \
-    copy_attn_backward_chunk_kernel<V, S><<<grid, 256, 0, st>>>(c, row_ptr, perm, chunk_ptr, G, steps, o, lse, d_s, d_lse, d_c, part_do)
+    return launch(PTGNN_KERNEL_REDUCE, st, copy_attn_backward_chunk_kernel<V, S>, grid, 256, 0, c, row_ptr, perm, chunk_ptr, G, steps, o, lse, d_s, \
+                  d_lse, d_c, part_do)
     PTGNN_COPY_DISPATCH(PTGNN_BWD)
 #undef PTGNN_BWD
 }
@@ -217,7 +225,7 @@ extern "C" int32_t ptgnn_b200_copy_attention_supported(int32_t bf16_copy, int32_
 
 extern "C" size_t ptgnn_b200_copy_attention_workspace_bytes(int64_t num_rows, int64_t num_graphs, int32_t hidden_dim, int32_t steps) {
     if (num_rows < 0 || num_graphs < 0 || !copy_attn::supported(hidden_dim, steps)) return 0;
-    return copy_attn::workspace_bytes(num_rows, num_graphs, hidden_dim, steps);
+    return copy_attn::layout(num_rows, num_graphs, hidden_dim, steps).total;
 }
 
 // shared argument checks of the two entry points; returns PTGNN_OK or an error code (set_error done)
@@ -230,7 +238,7 @@ static int copy_check(const char *what, const void *c, int64_t num_rows, int32_t
     }
     if (num_graphs == 0) return PTGNN_OK;
     PTGNN_CHECK_ARG(row_ptr && o && lse && (num_rows == 0 || (c && perm)), "%s: null pointer", what);
-    PTGNN_CHECK_WORKSPACE(what, workspace, workspace_bytes, copy_attn::workspace_bytes(num_rows, num_graphs, D, steps));
+    PTGNN_CHECK_WORKSPACE(what, workspace, workspace_bytes, copy_attn::layout(num_rows, num_graphs, D, steps).total);
     return PTGNN_OK;
 }
 
@@ -243,27 +251,19 @@ extern "C" int ptgnn_b200_copy_attention(int32_t bf16_copy, const void *copy_rep
     if (rc != PTGNN_OK || num_graphs == 0) return rc;
     PTGNN_CHECK_ARG(num_rows == 0 || s, "copy_attention: null pointer");
     const int G = (int)num_graphs;
+    const copy_attn::Ws L = copy_attn::layout(num_rows, num_graphs, D, steps);
     char *ws = static_cast<char *>(workspace);
-    int32_t *chunk_ptr = reinterpret_cast<int32_t *>(ws);
-    float *part_m = reinterpret_cast<float *>(ws + pergraph::ws_chunk_ptr(num_graphs));
-    float *part_l = reinterpret_cast<float *>(ws + pergraph::ws_chunk_ptr(num_graphs) + copy_attn::ws_ml(num_rows, num_graphs, steps));
-    pergraph::launch_chunk_ptr(row_ptr, G, chunk_ptr, st);
-    PTGNN_LAUNCHED();
+    int32_t *chunk_ptr = reinterpret_cast<int32_t *>(ws + L.chunk_ptr);
+    float *part_m = reinterpret_cast<float *>(ws + L.m);
+    float *part_l = reinterpret_cast<float *>(ws + L.l);
+    PTGNN_TRY(pergraph::launch_chunk_ptr(row_ptr, G, chunk_ptr, st));
     if (num_rows > 0) {
         const int grid = pergraph::chunk_grid(num_rows, num_graphs);
-        {
-            TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-            if (bf16_copy) copy_attn::launch_forward<true>(D, steps, grid, st, copy_reps, row_ptr, perm, chunk_ptr, G, o, s, part_m, part_l);
-            else copy_attn::launch_forward<false>(D, steps, grid, st, copy_reps, row_ptr, perm, chunk_ptr, G, o, s, part_m, part_l);
-        }
-        PTGNN_LAUNCHED();
+        if (bf16_copy) PTGNN_TRY(copy_attn::launch_forward<true>(D, steps, grid, st, copy_reps, row_ptr, perm, chunk_ptr, G, o, s, part_m, part_l));
+        else PTGNN_TRY(copy_attn::launch_forward<false>(D, steps, grid, st, copy_reps, row_ptr, perm, chunk_ptr, G, o, s, part_m, part_l));
     }
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        copy_attn::copy_attn_finalize_kernel<<<(unsigned)ceil_div((int64_t)G * steps, 256), 256, 0, st>>>(part_m, part_l, chunk_ptr, G, steps, lse);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch(PTGNN_KERNEL_REDUCE, st, copy_attn::copy_attn_finalize_kernel, (unsigned)ceil_div((int64_t)G * steps, 256), 256, 0, part_m, part_l,
+                  chunk_ptr, G, steps, lse);
 }
 
 extern "C" int ptgnn_b200_copy_attention_backward_f32(const float *copy_reps, int64_t num_rows, int32_t hidden_dim, int32_t steps,
@@ -277,20 +277,13 @@ extern "C" int ptgnn_b200_copy_attention_backward_f32(const float *copy_reps, in
     if (rc != PTGNN_OK || num_graphs == 0) return rc;
     PTGNN_CHECK_ARG(d_lse && d_o && (num_rows == 0 || (d_s && d_copy_reps)), "copy_attention_backward: null pointer");
     const int G = (int)num_graphs;
+    const copy_attn::Ws L = copy_attn::layout(num_rows, num_graphs, D, steps);
     char *ws = static_cast<char *>(workspace);
-    int32_t *chunk_ptr = reinterpret_cast<int32_t *>(ws);
-    float *part_do = reinterpret_cast<float *>(ws + pergraph::ws_chunk_ptr(num_graphs));
-    pergraph::launch_chunk_ptr(row_ptr, G, chunk_ptr, st);
-    PTGNN_LAUNCHED();
-    if (num_rows > 0) {
-        {
-            TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-            copy_attn::launch_backward(D, steps, pergraph::chunk_grid(num_rows, num_graphs), st, copy_reps, row_ptr, perm, chunk_ptr, G, o, lse,
-                                       d_s, d_lse, d_copy_reps, part_do);
-        }
-        PTGNN_LAUNCHED();
-    }
-    pergraph::launch_chunk_sum(part_do, row_ptr, chunk_ptr, G, steps * D, d_o, st);
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    int32_t *chunk_ptr = reinterpret_cast<int32_t *>(ws + L.chunk_ptr);
+    float *part_do = reinterpret_cast<float *>(ws + L.d_o);
+    PTGNN_TRY(pergraph::launch_chunk_ptr(row_ptr, G, chunk_ptr, st));
+    if (num_rows > 0)
+        PTGNN_TRY(copy_attn::launch_backward(D, steps, pergraph::chunk_grid(num_rows, num_graphs), st, copy_reps, row_ptr, perm, chunk_ptr, G, o,
+                                             lse, d_s, d_lse, d_copy_reps, part_do));
+    return pergraph::launch_chunk_sum(part_do, row_ptr, chunk_ptr, G, steps * D, d_o, st);
 }

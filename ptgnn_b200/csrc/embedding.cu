@@ -187,12 +187,20 @@ __global__ void __launch_bounds__(256) embedding_bag_backward_kernel(const float
 bool supported(int D, int S) { return D >= 1 && D <= MAX_D && S >= 1 && S <= MAX_S; }
 
 // chunk_ptr [V + 1] | partial [B S / CHUNK + V + 1, D]
-size_t backward_workspace_bytes(int64_t B, int S, int64_t V, int D) { return ws_chunk_ptr(V) + ws_slice(partial_rows(B * S, V) * D, 4); }
+struct BackwardWs { size_t chunk_ptr, partial, total; };
+static BackwardWs backward_layout(int64_t B, int S, int64_t V, int D) {
+    Layout l;
+    BackwardWs w;
+    w.chunk_ptr = l.add((size_t)V + 1, 4);
+    w.partial = l.add(partial_rows(B * S, V) * D, 4);
+    w.total = l.total;
+    return w;
+}
 
 template <int VEC, typename OUT>
-static void launch_forward(int pool, unsigned grid, cudaStream_t st, const float *table, const int64_t *ids, const int64_t *lengths, long long B,
-                           int S, int D, long long V, OUT *out, uint8_t *arg, int32_t *status) {
-#define PTGNN_EMBAG(P) embedding_bag_kernel<VEC, OUT, P><<<grid, 256, 0, st>>>(table, ids, lengths, B, S, D, V, out, arg, status)
+static int launch_forward(int pool, unsigned grid, cudaStream_t st, const float *table, const int64_t *ids, const int64_t *lengths, long long B,
+                          int S, int D, long long V, OUT *out, uint8_t *arg, int32_t *status) {
+#define PTGNN_EMBAG(P) return launch(PTGNN_KERNEL_REDUCE, st, embedding_bag_kernel<VEC, OUT, P>, grid, 256, 0, table, ids, lengths, B, S, D, V, out, arg, status)
     switch (pool) {
         case PTGNN_POOL_SUM: PTGNN_EMBAG(PTGNN_POOL_SUM); break;
         case PTGNN_POOL_MEAN: PTGNN_EMBAG(PTGNN_POOL_MEAN); break;
@@ -202,9 +210,11 @@ static void launch_forward(int pool, unsigned grid, cudaStream_t st, const float
 }
 
 template <int VEC>
-static void launch_backward(int pool, int grid, cudaStream_t st, const float *d_out, const int64_t *lengths, const uint8_t *arg,
-                            const int32_t *row_ptr, const int32_t *perm, const int32_t *chunk_ptr, int V, int S, int D, float *partial) {
-#define PTGNN_EMBAG(P) embedding_bag_backward_kernel<VEC, P><<<grid, 256, 0, st>>>(d_out, lengths, arg, row_ptr, perm, chunk_ptr, V, S, D, partial)
+static int launch_backward(int pool, int grid, cudaStream_t st, const float *d_out, const int64_t *lengths, const uint8_t *arg,
+                           const int32_t *row_ptr, const int32_t *perm, const int32_t *chunk_ptr, int V, int S, int D, float *partial) {
+#define PTGNN_EMBAG(P)                                                                                                                  \
+    return launch(PTGNN_KERNEL_REDUCE, st, embedding_bag_backward_kernel<VEC, P>, grid, 256, 0, d_out, lengths, arg, row_ptr, perm, chunk_ptr, V, \
+                  S, D, partial)
     switch (pool) {
         case PTGNN_POOL_SUM: PTGNN_EMBAG(PTGNN_POOL_SUM); break;
         case PTGNN_POOL_MEAN: PTGNN_EMBAG(PTGNN_POOL_MEAN); break;
@@ -245,20 +255,14 @@ extern "C" int ptgnn_b200_embedding_bag(int32_t bf16_out, const float *table, in
     PTGNN_CHECK_ARG(!vec || (aligned(table, 16) && aligned(out, bf16_out ? 8 : 16) && aligned(arg_out, 4)),
                     "embedding_bag: the table and fp32 rows must be 16-byte, bf16 rows 8-byte, arg_out 4-byte aligned");
     const unsigned grid = (unsigned)ceil_div(rows * (vec ? dim / 4 : dim), 256);
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        if (bf16_out) {
-            __nv_bfloat16 *o = static_cast<__nv_bfloat16 *>(out);
-            if (vec) embag::launch_forward<4>(pool, grid, st, table, ids, lengths, rows, slots, dim, vocab, o, arg_out, status);
-            else embag::launch_forward<1>(pool, grid, st, table, ids, lengths, rows, slots, dim, vocab, o, arg_out, status);
-        } else {
-            float *o = static_cast<float *>(out);
-            if (vec) embag::launch_forward<4>(pool, grid, st, table, ids, lengths, rows, slots, dim, vocab, o, arg_out, status);
-            else embag::launch_forward<1>(pool, grid, st, table, ids, lengths, rows, slots, dim, vocab, o, arg_out, status);
-        }
+    if (bf16_out) {
+        __nv_bfloat16 *o = static_cast<__nv_bfloat16 *>(out);
+        if (vec) return embag::launch_forward<4>(pool, grid, st, table, ids, lengths, rows, slots, dim, vocab, o, arg_out, status);
+        return embag::launch_forward<1>(pool, grid, st, table, ids, lengths, rows, slots, dim, vocab, o, arg_out, status);
     }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    float *o = static_cast<float *>(out);
+    if (vec) return embag::launch_forward<4>(pool, grid, st, table, ids, lengths, rows, slots, dim, vocab, o, arg_out, status);
+    return embag::launch_forward<1>(pool, grid, st, table, ids, lengths, rows, slots, dim, vocab, o, arg_out, status);
 }
 
 extern "C" int ptgnn_b200_embedding_bag_pairs(const int64_t *ids, const int64_t *lengths, int64_t rows, int32_t slots, int64_t vocab,
@@ -267,17 +271,13 @@ extern "C" int ptgnn_b200_embedding_bag_pairs(const int64_t *ids, const int64_t 
     const int rc = embag_check("embedding_bag_pairs", rows, slots, vocab, 4, PTGNN_POOL_SUM);
     if (rc != PTGNN_OK || rows == 0) return rc;
     PTGNN_CHECK_ARG(ids && src && tgt, "embedding_bag_pairs: null pointer");
-    {
-        TimedScope timed__(PTGNN_KERNEL_PLAN, st);
-        embag::embedding_bag_pairs_kernel<<<(unsigned)ceil_div(rows * slots, 256), 256, 0, st>>>(ids, lengths, rows, slots, vocab, src, tgt);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch(PTGNN_KERNEL_PLAN, st, embag::embedding_bag_pairs_kernel, (unsigned)ceil_div(rows * slots, 256), 256, 0, ids, lengths, rows, slots,
+                  vocab, src, tgt);
 }
 
 extern "C" size_t ptgnn_b200_embedding_bag_backward_workspace_bytes(int64_t rows, int32_t slots, int64_t vocab, int32_t dim) {
     if (rows < 0 || vocab < 0 || !embag::supported(dim, slots)) return 0;
-    return embag::backward_workspace_bytes(rows, slots, vocab, dim);
+    return embag::backward_layout(rows, slots, vocab, dim).total;
 }
 
 extern "C" int ptgnn_b200_embedding_bag_backward_f32(const float *d_out, int64_t rows, int32_t slots, int32_t dim, const int64_t *lengths,
@@ -290,22 +290,17 @@ extern "C" int ptgnn_b200_embedding_bag_backward_f32(const float *d_out, int64_t
     PTGNN_CHECK_ARG(pool != PTGNN_POOL_MAX || rows == 0 || arg, "embedding_bag_backward: max needs the forward's arg slots");
     const bool vec = dim % 4 == 0;
     PTGNN_CHECK_ARG(!vec || (aligned(d_out, 16) && aligned(d_table, 16)), "embedding_bag_backward: d_out and d_table must be 16-byte aligned");
-    PTGNN_CHECK_WORKSPACE("embedding_bag_backward", workspace, workspace_bytes, embag::backward_workspace_bytes(rows, slots, vocab, dim));
+    const embag::BackwardWs L = embag::backward_layout(rows, slots, vocab, dim);
+    PTGNN_CHECK_WORKSPACE("embedding_bag_backward", workspace, workspace_bytes, L.total);
     const int V = (int)vocab;
-    int32_t *chunk_ptr = static_cast<int32_t *>(workspace);
-    float *partial = reinterpret_cast<float *>(static_cast<char *>(workspace) + pergraph::ws_chunk_ptr(vocab));
-    pergraph::launch_chunk_ptr(row_ptr, V, chunk_ptr, st);      // the sink row V of the plan is left out of the walk
-    PTGNN_LAUNCHED();
+    char *ws = static_cast<char *>(workspace);
+    int32_t *chunk_ptr = reinterpret_cast<int32_t *>(ws + L.chunk_ptr);
+    float *partial = reinterpret_cast<float *>(ws + L.partial);
+    PTGNN_TRY(pergraph::launch_chunk_ptr(row_ptr, V, chunk_ptr, st));      // the sink row V of the plan is left out of the walk
     if (rows > 0) {
         const int grid = pergraph::chunk_grid(rows * slots, vocab);
-        {
-            TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-            if (vec) embag::launch_backward<4>(pool, grid, st, d_out, lengths, arg, row_ptr, perm, chunk_ptr, V, slots, dim, partial);
-            else embag::launch_backward<1>(pool, grid, st, d_out, lengths, arg, row_ptr, perm, chunk_ptr, V, slots, dim, partial);
-        }
-        PTGNN_LAUNCHED();
+        if (vec) PTGNN_TRY(embag::launch_backward<4>(pool, grid, st, d_out, lengths, arg, row_ptr, perm, chunk_ptr, V, slots, dim, partial));
+        else PTGNN_TRY(embag::launch_backward<1>(pool, grid, st, d_out, lengths, arg, row_ptr, perm, chunk_ptr, V, slots, dim, partial));
     }
-    pergraph::launch_chunk_sum(partial, row_ptr, chunk_ptr, V, dim, d_table, st);
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return pergraph::launch_chunk_sum(partial, row_ptr, chunk_ptr, V, dim, d_table, st);
 }

@@ -846,41 +846,22 @@ int pack_weights(int nprod, int num_types, int K, int use_target, const float *c
     WeightSrc src{};
     for (int t = 0; t < num_types; ++t) src.w[t] = weights[t];
     const int nseg = use_target ? 2 : 1;
-    {
-        TimedScope timed__(PTGNN_KERNEL_PACK, st);
-        if (nprod == 3) pack_weights_kernel<3><<<132, 256, 0, st>>>(src, num_types, K, nseg, rows, static_cast<uint4 *>(packed), status);
-        else pack_weights_kernel<1><<<132, 256, 0, st>>>(src, num_types, K, nseg, rows, static_cast<uint4 *>(packed), status);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch(PTGNN_KERNEL_PACK, st, nprod == 3 ? pack_weights_kernel<3> : pack_weights_kernel<1>, 132, 256, 0, src, num_types, K, nseg, rows,
+                  static_cast<uint4 *>(packed), status);
 }
 
 int pack_states(const float *h, int64_t rows, int K, void *packed, int32_t *status, cudaStream_t st) {
     if (rows <= 0) return PTGNN_OK;
     const int64_t items = rows * (K / 8);
     const unsigned grid = (unsigned)(ceil_div(items, 256) < 132 * 8 ? ceil_div(items, 256) : 132 * 8);
-    {
-        TimedScope timed__(PTGNN_KERNEL_PACK, st);
-        pack_states_kernel<<<grid, 256, 0, st>>>(h, (long long)rows, K, static_cast<uint4 *>(packed), status);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch(PTGNN_KERNEL_PACK, st, pack_states_kernel, grid, 256, 0, h, (long long)rows, K, static_cast<uint4 *>(packed), status);
 }
 
 template <int NPROD, int K, int NSEG, int RED, int EPI = EPI_AGG>
 static int launch_one(const Params &p, cudaStream_t st) {
-    auto kernel = fused_aggregate_kernel<NPROD, K, NSEG, RED, EPI>;
-    const int smem = smem_bytes(p.B);
-    // per launch, not once per process: the attribute belongs to the current device's context
-    PTGNN_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     const int sms = sm_count();
     const int grid = p.num_blocks < sms ? p.num_blocks : sms;
-    {
-        TimedScope timed__(PTGNN_KERNEL_MESSAGE, st);
-        kernel<<<grid, NUM_THREADS, smem, st>>>(p);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch(PTGNN_KERNEL_MESSAGE, st, fused_aggregate_kernel<NPROD, K, NSEG, RED, EPI>, grid, NUM_THREADS, smem_bytes(p.B), p);
 }
 template <int NPROD, int K, int NSEG, int EPI = EPI_AGG>
 static int launch_red(const Params &p, cudaStream_t st) {

@@ -312,23 +312,32 @@ __global__ void __launch_bounds__(256) graphnorm_param_grad_kernel(const float *
 bool supported(int D) { return D % 32 == 0 && D >= 32 && D <= 256; }
 
 // chunk_ptr [G + 1] | partial [N / CHUNK + G + 1, 2 D] | AB [G, 2 D] | coef [4, G, D]  (the forward uses the first two)
-static size_t ws_partial(int64_t N, int64_t G, int D) { return ws_slice(partial_rows(N, G) * 2 * D, 4); }
-static size_t ws_ab(int64_t G, int D) { return ws_slice((size_t)G * 2 * D, 4); }
-size_t workspace_bytes(int64_t N, int64_t G, int D) { return ws_chunk_ptr(G) + ws_partial(N, G, D) + ws_ab(G, D) + ws_slice((size_t)G * 4 * D, 4); }
+struct Ws { size_t chunk_ptr, partial, ab, coef, total; };
+static Ws layout(int64_t N, int64_t G, int D) {
+    Layout l;
+    Ws w;
+    w.chunk_ptr = l.add((size_t)G + 1, 4);
+    w.partial = l.add(partial_rows(N, G) * 2 * D, 4);
+    w.ab = l.add((size_t)G * 2 * D, 4);
+    w.coef = l.add((size_t)G * 4 * D, 4);
+    w.total = l.total;
+    return w;
+}
 
 static int flat_grid(long long groups) { return (int)std::min<long long>(ceil_div(groups, 256), (long long)sm_count() * 16); }
 
 template <bool BF16>
-static void launch_stats(int D, int grid, cudaStream_t st, const void *x, const int32_t *row_ptr, const int32_t *perm, const int32_t *chunk_ptr,
-                         int G, float *partial) {
-#define PTGNN_GN_STATS(V) graphnorm_stats_kernel<V, BF16><<<grid, 256, 0, st>>>(x, row_ptr, perm, chunk_ptr, G, partial)
+static int launch_stats(int D, int grid, cudaStream_t st, const void *x, const int32_t *row_ptr, const int32_t *perm, const int32_t *chunk_ptr,
+                        int G, float *partial) {
+#define PTGNN_GN_STATS(V) return launch(PTGNN_KERNEL_REDUCE, st, graphnorm_stats_kernel<V, BF16>, grid, 256, 0, x, row_ptr, perm, chunk_ptr, G, partial)
     PTGNN_VPL_DISPATCH(D, PTGNN_GN_STATS)
 #undef PTGNN_GN_STATS
 }
 
-static void launch_bwd_chunks(int D, int grid, cudaStream_t st, const float *x, const float *dy, const int32_t *row_ptr, const int32_t *perm,
-                              const int32_t *chunk_ptr, int G, const float *mean, const float *rstd, const float *alpha, float *partial) {
-#define PTGNN_GN_BWD(V) graphnorm_bwd_chunk_kernel<V><<<grid, 256, 0, st>>>(x, dy, row_ptr, perm, chunk_ptr, G, mean, rstd, alpha, partial)
+static int launch_bwd_chunks(int D, int grid, cudaStream_t st, const float *x, const float *dy, const int32_t *row_ptr, const int32_t *perm,
+                             const int32_t *chunk_ptr, int G, const float *mean, const float *rstd, const float *alpha, float *partial) {
+#define PTGNN_GN_BWD(V)                                                                                                                 \
+    return launch(PTGNN_KERNEL_REDUCE, st, graphnorm_bwd_chunk_kernel<V>, grid, 256, 0, x, dy, row_ptr, perm, chunk_ptr, G, mean, rstd, alpha, partial)
     PTGNN_VPL_DISPATCH(D, PTGNN_GN_BWD)
 #undef PTGNN_GN_BWD
 }
@@ -342,7 +351,7 @@ extern "C" int32_t ptgnn_b200_graph_norm_supported(int32_t state_dim) { return g
 
 extern "C" size_t ptgnn_b200_graph_norm_workspace_bytes(int64_t num_nodes, int64_t num_graphs, int32_t state_dim) {
     if (num_nodes < 0 || num_graphs < 0 || !graphnorm::supported(state_dim)) return 0;
-    return graphnorm::workspace_bytes(num_nodes, num_graphs, state_dim);
+    return graphnorm::layout(num_nodes, num_graphs, state_dim).total;
 }
 
 static bool aligned16(const void *p) { return ((uintptr_t)p & 15) == 0; }
@@ -361,7 +370,7 @@ static int graph_norm_check(const char *what, const void *x, int64_t num_nodes, 
     PTGNN_CHECK_ARG(row_ptr && gamma && alpha && mean && rstd && (num_nodes == 0 || (x && perm && graph_of_node)), "%s: null pointer", what);
     PTGNN_CHECK_ARG(aligned16(gamma) && aligned16(alpha) && aligned16(mean) && aligned16(rstd) && ((uintptr_t)x & 7) == 0,
                     "%s: gamma, alpha, mean and rstd must be 16-byte aligned, the states 8-byte aligned", what);
-    PTGNN_CHECK_WORKSPACE(what, workspace, workspace_bytes, graphnorm::workspace_bytes(num_nodes, num_graphs, D));
+    PTGNN_CHECK_WORKSPACE(what, workspace, workspace_bytes, graphnorm::layout(num_nodes, num_graphs, D).total);
     return PTGNN_OK;
 }
 
@@ -375,40 +384,22 @@ extern "C" int ptgnn_b200_graph_norm_forward(int32_t bf16_states, const void *no
     if (rc != PTGNN_OK || num_graphs == 0) return rc;
     PTGNN_CHECK_ARG(bias && (num_nodes == 0 || out), "graph_norm_forward: null pointer");
     const int G = (int)num_graphs, D = state_dim;
+    const graphnorm::Ws L = graphnorm::layout(num_nodes, num_graphs, D);
     char *ws = static_cast<char *>(workspace);
-    int32_t *chunk_ptr = reinterpret_cast<int32_t *>(ws);
-    float *partial = reinterpret_cast<float *>(ws + pergraph::ws_chunk_ptr(num_graphs));
+    int32_t *chunk_ptr = reinterpret_cast<int32_t *>(ws + L.chunk_ptr);
+    float *partial = reinterpret_cast<float *>(ws + L.partial);
     const long long groups = num_nodes * D / 4;
     const int grid_c = pergraph::chunk_grid(num_nodes, num_graphs), grid_f = graphnorm::flat_grid(groups);
-    pergraph::launch_chunk_ptr(row_ptr, G, chunk_ptr, st);
-    PTGNN_LAUNCHED();
+    PTGNN_TRY(pergraph::launch_chunk_ptr(row_ptr, G, chunk_ptr, st));
     if (num_nodes > 0) {
-        {
-            TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-            if (bf16_states) graphnorm::launch_stats<true>(D, grid_c, st, node_states, row_ptr, perm, chunk_ptr, G, partial);
-            else graphnorm::launch_stats<false>(D, grid_c, st, node_states, row_ptr, perm, chunk_ptr, G, partial);
-        }
-        PTGNN_LAUNCHED();
+        if (bf16_states) PTGNN_TRY(graphnorm::launch_stats<true>(D, grid_c, st, node_states, row_ptr, perm, chunk_ptr, G, partial));
+        else PTGNN_TRY(graphnorm::launch_stats<false>(D, grid_c, st, node_states, row_ptr, perm, chunk_ptr, G, partial));
     }
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        graphnorm::graphnorm_combine_kernel<<<(unsigned)ceil_div((int64_t)G * D, 256), 256, 0, st>>>(partial, row_ptr, chunk_ptr, G, D, alpha,
-                                                                                                      eps, mean, rstd);
-    }
-    PTGNN_LAUNCHED();
-    if (num_nodes > 0) {
-        {
-            TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-            if (bf16_states)
-                graphnorm::graphnorm_apply_kernel<true><<<grid_f, 256, 0, st>>>(node_states, graph_of_node, groups, D, mean, rstd, gamma, alpha,
-                                                                                 bias, out);
-            else
-                graphnorm::graphnorm_apply_kernel<false><<<grid_f, 256, 0, st>>>(node_states, graph_of_node, groups, D, mean, rstd, gamma, alpha,
-                                                                                  bias, out);
-        }
-        PTGNN_LAUNCHED();
-    }
-    return PTGNN_OK;
+    PTGNN_TRY(launch(PTGNN_KERNEL_REDUCE, st, graphnorm::graphnorm_combine_kernel, (unsigned)ceil_div((int64_t)G * D, 256), 256, 0, partial, row_ptr,
+                     chunk_ptr, G, D, alpha, eps, mean, rstd));
+    if (num_nodes == 0) return PTGNN_OK;
+    return launch(PTGNN_KERNEL_REDUCE, st, bf16_states ? graphnorm::graphnorm_apply_kernel<true> : graphnorm::graphnorm_apply_kernel<false>, grid_f,
+                  256, 0, node_states, graph_of_node, groups, D, mean, rstd, gamma, alpha, bias, out);
 }
 
 extern "C" int ptgnn_b200_graph_norm_backward_f32(const float *node_states, const float *d_out, int64_t num_nodes, int32_t state_dim,
@@ -428,44 +419,23 @@ extern "C" int ptgnn_b200_graph_norm_backward_f32(const float *node_states, cons
         PTGNN_CUDA(cudaMemsetAsync(d_bias, 0, sizeof(float) * D, st));
         return PTGNN_OK;
     }
+    const graphnorm::Ws L = graphnorm::layout(num_nodes, num_graphs, D);
     char *ws = static_cast<char *>(workspace);
-    int32_t *chunk_ptr = reinterpret_cast<int32_t *>(ws);
-    ws += pergraph::ws_chunk_ptr(num_graphs);
-    float *partial = reinterpret_cast<float *>(ws);
-    ws += graphnorm::ws_partial(num_nodes, num_graphs, D);
-    float *AB = reinterpret_cast<float *>(ws);
-    float *coef = reinterpret_cast<float *>(ws + graphnorm::ws_ab(num_graphs, D));
+    int32_t *chunk_ptr = reinterpret_cast<int32_t *>(ws + L.chunk_ptr);
+    float *partial = reinterpret_cast<float *>(ws + L.partial);
+    float *AB = reinterpret_cast<float *>(ws + L.ab);
+    float *coef = reinterpret_cast<float *>(ws + L.coef);
     const long long groups = num_nodes * D / 4;
     const int grid_c = pergraph::chunk_grid(num_nodes, num_graphs), grid_f = graphnorm::flat_grid(groups);
-    pergraph::launch_chunk_ptr(row_ptr, G, chunk_ptr, st);
-    PTGNN_LAUNCHED();
-    if (num_nodes > 0) {
-        {
-            TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-            graphnorm::launch_bwd_chunks(D, grid_c, st, node_states, d_out, row_ptr, perm, chunk_ptr, G, mean, rstd, alpha, partial);
-        }
-        PTGNN_LAUNCHED();
-    }
-    pergraph::launch_chunk_sum(partial, row_ptr, chunk_ptr, G, 2 * D, AB, st);
-    PTGNN_LAUNCHED();
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        graphnorm::graphnorm_bwd_graph_kernel<<<(unsigned)ceil_div((int64_t)G * D, 256), 256, 0, st>>>(AB, row_ptr, G, D, mean, rstd, gamma,
-                                                                                                        alpha, eps, coef);
-    }
-    PTGNN_LAUNCHED();
-    if (num_nodes > 0) {
-        {
-            TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-            graphnorm::graphnorm_bwd_apply_kernel<<<grid_f, 256, 0, st>>>(node_states, d_out, graph_of_node, groups, G, D, mean, rstd, alpha, coef,
-                                                                          d_x);
-        }
-        PTGNN_LAUNCHED();
-    }
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        graphnorm::graphnorm_param_grad_kernel<<<(unsigned)ceil_div(D, 256), 256, 0, st>>>(AB, mean, coef, G, D, d_gamma, d_alpha, d_bias);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    PTGNN_TRY(pergraph::launch_chunk_ptr(row_ptr, G, chunk_ptr, st));
+    if (num_nodes > 0)
+        PTGNN_TRY(graphnorm::launch_bwd_chunks(D, grid_c, st, node_states, d_out, row_ptr, perm, chunk_ptr, G, mean, rstd, alpha, partial));
+    PTGNN_TRY(pergraph::launch_chunk_sum(partial, row_ptr, chunk_ptr, G, 2 * D, AB, st));
+    PTGNN_TRY(launch(PTGNN_KERNEL_REDUCE, st, graphnorm::graphnorm_bwd_graph_kernel, (unsigned)ceil_div((int64_t)G * D, 256), 256, 0, AB, row_ptr, G,
+                     D, mean, rstd, gamma, alpha, eps, coef));
+    if (num_nodes > 0)
+        PTGNN_TRY(launch(PTGNN_KERNEL_REDUCE, st, graphnorm::graphnorm_bwd_apply_kernel, grid_f, 256, 0, node_states, d_out, graph_of_node, groups, G,
+                         D, mean, rstd, alpha, coef, d_x));
+    return launch(PTGNN_KERNEL_REDUCE, st, graphnorm::graphnorm_param_grad_kernel, (unsigned)ceil_div(D, 256), 256, 0, AB, mean, coef, G, D, d_gamma,
+                  d_alpha, d_bias);
 }

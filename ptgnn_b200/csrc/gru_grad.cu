@@ -60,13 +60,8 @@ extern "C" int ptgnn_b200_gru_gate_grads_f32(const float *gi, const float *gh, c
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const long long total = (long long)num_nodes * (state_dim / 4);
     const long long blocks = (total + 255) / 256;
-    {
-        TimedScope timed__(PTGNN_KERNEL_GRU, st);
-        gru_gate_grads_kernel<<<(unsigned)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, st>>>(gi, gh, h, grad_out, num_nodes, state_dim, d_gi, d_gh,
-                                                                                                 d_h_direct);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch(PTGNN_KERNEL_GRU, st, gru_gate_grads_kernel, (unsigned)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, gi, gh, h, grad_out,
+                  num_nodes, state_dim, d_gi, d_gh, d_h_direct);
 }
 
 // Operand preparation for the parameter-gradient GEMMs (dW = A^T B with K = edges or nodes, run as three fp16 tensor-core GEMMs):
@@ -112,11 +107,6 @@ extern "C" int ptgnn_b200_gather_split_f16(const float *x, const int32_t *index,
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const long long total = (long long)rows_out * (cols / 8);
     const long long blocks = (total + 255) / 256;
-    {
-        TimedScope timed__(PTGNN_KERNEL_PACK, st);
-        gather_split_kernel<<<(unsigned)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, st>>>(x, index, rows_out, cols, scale, static_cast<uint4 *>(hi),
-                                                                                               static_cast<uint4 *>(lo));
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch(PTGNN_KERNEL_PACK, st, gather_split_kernel, (unsigned)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, x, index, rows_out, cols,
+                  scale, static_cast<uint4 *>(hi), static_cast<uint4 *>(lo));
 }

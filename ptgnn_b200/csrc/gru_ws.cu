@@ -389,13 +389,8 @@ int pack(int nprod, int H, int D, const float *w_ih, const float *w_hh, const fl
     uint16_t *p1, *p2;
     float4 *bias4;
     pack_layout(nprod, H, D, static_cast<char *>(packed), p1, p2, bias4);
-    {
-        TimedScope timed__(PTGNN_KERNEL_PACK, st);
-        if (nprod == 3) pack_gru_ws_kernel<3><<<132, 256, 0, st>>>(w_ih, w_hh, b_ih, b_hh, H, D, p1, p2, bias4);
-        else pack_gru_ws_kernel<1><<<132, 256, 0, st>>>(w_ih, w_hh, b_ih, b_hh, H, D, p1, p2, bias4);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch(PTGNN_KERNEL_PACK, st, nprod == 3 ? pack_gru_ws_kernel<3> : pack_gru_ws_kernel<1>, 132, 256, 0, w_ih, w_hh, b_ih, b_hh, H, D, p1,
+                  p2, bias4);
 }
 
 int update(int nprod, const void *agg_rows, const void *h_rows, const void *h_plain, int64_t num_nodes, int H, int D, const void *packed,
@@ -423,23 +418,8 @@ int update(int nprod, const void *agg_rows, const void *h_rows, const void *h_pl
     if (groups > p.n_tiles) groups = p.n_tiles;
     if (groups < 1) groups = 1;
     const int grid = groups * (int)n_jb;
-    if (nprod == 3) {
-        const int smem = Geometry<3>::smem_bytes(H, D);
-        PTGNN_CUDA(cudaFuncSetAttribute(gru_ws_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        {
-            TimedScope timed__(PTGNN_KERNEL_GRU, st);
-            gru_ws_kernel<3, false><<<grid, NUM_THREADS, smem, st>>>(p);
-        }
-    } else {
-        const int smem = Geometry<1>::smem_bytes(H, D);
-        PTGNN_CUDA(cudaFuncSetAttribute(gru_ws_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        {
-            TimedScope timed__(PTGNN_KERNEL_GRU, st);
-            gru_ws_kernel<1, false><<<grid, NUM_THREADS, smem, st>>>(p);
-        }
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    if (nprod == 3) return launch(PTGNN_KERNEL_GRU, st, gru_ws_kernel<3, false>, grid, NUM_THREADS, Geometry<3>::smem_bytes(H, D), p);
+    return launch(PTGNN_KERNEL_GRU, st, gru_ws_kernel<1, false>, grid, NUM_THREADS, Geometry<1>::smem_bytes(H, D), p);
 }
 
 bool supported_table(int nprod, int H) {
@@ -476,23 +456,8 @@ int update_table(int nprod, const void *h_rows, const void *h_plain, int64_t num
     if (groups > p.n_tiles) groups = p.n_tiles;
     if (groups < 1) groups = 1;
     const int grid = groups * (int)n_jb;
-    if (nprod == 3) {
-        const int smem = Geometry<3>::smem_bytes(H, 0);
-        PTGNN_CUDA(cudaFuncSetAttribute(gru_ws_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        {
-            TimedScope timed__(PTGNN_KERNEL_GRU, st);
-            gru_ws_kernel<3, true><<<grid, NUM_THREADS, smem, st>>>(p);
-        }
-    } else {
-        const int smem = Geometry<1>::smem_bytes(H, 0);
-        PTGNN_CUDA(cudaFuncSetAttribute(gru_ws_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        {
-            TimedScope timed__(PTGNN_KERNEL_GRU, st);
-            gru_ws_kernel<1, true><<<grid, NUM_THREADS, smem, st>>>(p);
-        }
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    if (nprod == 3) return launch(PTGNN_KERNEL_GRU, st, gru_ws_kernel<3, true>, grid, NUM_THREADS, Geometry<3>::smem_bytes(H, 0), p);
+    return launch(PTGNN_KERNEL_GRU, st, gru_ws_kernel<1, true>, grid, NUM_THREADS, Geometry<1>::smem_bytes(H, 0), p);
 }
 
 }  // namespace gruws

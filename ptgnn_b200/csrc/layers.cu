@@ -220,26 +220,14 @@ dense_update_kernel(const float *__restrict__ y, int num_nodes, int D, const flo
 // =================================================================================================
 // host-side launchers
 // =================================================================================================
-template <typename K>
-static int set_smem(K kernel, int bytes) {
-    PTGNN_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-    return PTGNN_OK;
-}
-
 template <int TN>
 static int launch_edge_message_kernel(const MsgParams &p, int tiles, const float *h_src, const float *h_tgt, int H, int D,
                                       int use_target, const int32_t *src32, const int32_t *tgt32, const int32_t *pos, float *msg,
                                       cudaStream_t st) {
     using Tile = GemmTile<TN>;
-    int rc = set_smem(edge_message_kernel<TN>, Tile::SMEM_BYTES);
-    if (rc) return rc;
-    dim3 grid(tiles, (unsigned)ceil_div(D, Tile::BN));
-    {
-        TimedScope timed__(PTGNN_KERNEL_MESSAGE, st);
-        edge_message_kernel<TN><<<grid, GEMM_THREADS, Tile::SMEM_BYTES, st>>>(p, h_src, h_tgt, H, use_target, D, src32, tgt32, pos, msg);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    const dim3 grid(tiles, (unsigned)ceil_div(D, Tile::BN));
+    return launch(PTGNN_KERNEL_MESSAGE, st, edge_message_kernel<TN>, grid, GEMM_THREADS, Tile::SMEM_BYTES, p, h_src, h_tgt, H, use_target, D, src32,
+                  tgt32, pos, msg);
 }
 
 static int launch_edge_messages(const float *h_src, const float *h_tgt, int H, int D, int use_target, int num_types, const int64_t *type_off,
@@ -258,15 +246,8 @@ template <int TN>
 static int launch_dense_kernel(const float *y, int64_t rows, int D, const float *W, const float *bias, int out_dim, int act, float *out,
                                cudaStream_t st) {
     using Tile = GemmTile<TN>;
-    int rc = set_smem(dense_update_kernel<TN>, Tile::SMEM_BYTES);
-    if (rc) return rc;
-    dim3 grid((unsigned)ceil_div(rows, GEMM_BM), (unsigned)ceil_div(out_dim, Tile::BN));
-    {
-        TimedScope timed__(PTGNN_KERNEL_DENSE, st);
-        dense_update_kernel<TN><<<grid, GEMM_THREADS, Tile::SMEM_BYTES, st>>>(y, (int)rows, D, W, bias, out_dim, act, out);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    const dim3 grid((unsigned)ceil_div(rows, GEMM_BM), (unsigned)ceil_div(out_dim, Tile::BN));
+    return launch(PTGNN_KERNEL_DENSE, st, dense_update_kernel<TN>, grid, GEMM_THREADS, Tile::SMEM_BYTES, y, (int)rows, D, W, bias, out_dim, act, out);
 }
 
 // FFMA GRUCell: packs the gate weights into `scratch` (P1 | P2, gru_simt_bytes; re-derived every call), then one launch
@@ -275,21 +256,9 @@ static size_t gru_simt_bytes(int H, int D) { return gru_simt_part(H, D) + gru_si
 static int launch_gru_simt(const float *agg, const float *h, int64_t rows, int H, int D, const float *w_ih, const float *w_hh,
                            const float *b_ih, const float *b_hh, float *out, char *scratch, cudaStream_t st) {
     float *P1 = reinterpret_cast<float *>(scratch), *P2 = reinterpret_cast<float *>(scratch + gru_simt_part(H, D));
-    {
-        TimedScope timed__(PTGNN_KERNEL_PACK, st);
-        pack_gru_weights_kernel<<<132, 256, 0, st>>>(w_ih, w_hh, H, D, P1, P2);
-    }
-    PTGNN_LAUNCHED();
-    using Tile = GemmTile<6>;
-    int rc = set_smem(gru_update_kernel, Tile::SMEM_BYTES);
-    if (rc) return rc;
-    dim3 grid((unsigned)ceil_div(rows, GEMM_BM), H / 32);
-    {
-        TimedScope timed__(PTGNN_KERNEL_GRU, st);
-        gru_update_kernel<<<grid, GEMM_THREADS, Tile::SMEM_BYTES, st>>>(agg, h, (int)rows, H, D, P1, P2, b_ih, b_hh, out);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    PTGNN_TRY(launch(PTGNN_KERNEL_PACK, st, pack_gru_weights_kernel, 132, 256, 0, w_ih, w_hh, H, D, P1, P2));
+    const dim3 grid((unsigned)ceil_div(rows, GEMM_BM), H / 32);
+    return launch(PTGNN_KERNEL_GRU, st, gru_update_kernel, grid, GEMM_THREADS, GemmTile<6>::SMEM_BYTES, agg, h, (int)rows, H, D, P1, P2, b_ih, b_hh, out);
 }
 
 static int check_layer_dims(const char *who, int64_t N, int64_t E, int H, int D) {
@@ -368,12 +337,14 @@ static size_t rows_bytes(bool bf16, int64_t rows, int D) { return ws_slice((size
 // gated workspace: msg | agg | FFMA GRU packing (fp32) | derived weights = [edge weights | GRU packing] (without a weight cache)
 struct GatedWs { size_t msg, agg, simt, weights, total; };
 static GatedWs gated_layout(bool bf16, int64_t N, int64_t E, int T, int H, int D) {
-    GatedWs w{};
-    w.agg = rows_bytes(bf16, E, D);
-    w.simt = w.agg + rows_bytes(bf16, N, D);
-    w.weights = w.simt + (bf16 ? 0 : gru_simt_bytes(H, D));
+    Layout l;
+    GatedWs w;
+    w.msg = l.add_bytes(rows_bytes(bf16, E, D));
+    w.agg = l.add_bytes(rows_bytes(bf16, N, D));
+    w.simt = l.add_bytes(bf16 ? 0 : gru_simt_bytes(H, D));
     // fp32 states size the GRU packing for one gate block more than they use
-    w.total = w.weights + tc::edge_weight_bytes(bf16, T, D, H) + tc::gru_pack_bytes(bf16, bf16 ? H : H + 32, D);
+    w.weights = l.add_bytes(tc::edge_weight_bytes(bf16, T, D, H) + tc::gru_pack_bytes(bf16, bf16 ? H : H + 32, D));
+    w.total = l.total;
     return w;
 }
 
@@ -386,11 +357,13 @@ static size_t gated_cache_bytes(bool bf16, int T, int H, int D) {
 // Mlp workspace: msg | y (the aggregate before the dense layer) | edge weights | dense weight (derived every call, no cache)
 struct MlpWs { size_t msg, y, weights, dense, total; };
 static MlpWs mlp_layout(bool bf16, int64_t N, int64_t E, int T, int H, int D, int Hout, int ut) {
-    MlpWs w{};
-    w.y = rows_bytes(bf16, E, D);
-    w.weights = w.y + rows_bytes(bf16, N, D);
-    w.dense = w.weights + tc::edge_weight_bytes(bf16, T, D, ut ? 2 * H : H);
-    w.total = w.dense + tc::dense_weight_bytes(bf16, Hout, D);
+    Layout l;
+    MlpWs w;
+    w.msg = l.add_bytes(rows_bytes(bf16, E, D));
+    w.y = l.add_bytes(rows_bytes(bf16, N, D));
+    w.weights = l.add_bytes(tc::edge_weight_bytes(bf16, T, D, ut ? 2 * H : H));
+    w.dense = l.add_bytes(tc::dense_weight_bytes(bf16, Hout, D));
+    w.total = l.total;
     return w;
 }
 

@@ -35,22 +35,26 @@ size_t mlp_weight_bytes(int nprod, int T, int H, int D, int Hout, int ut) {
 // workspace: agg | packed states (gathered rows) | packed own rows (sharded run: the GRU's h) | derived weights (no cache)
 struct GatedWs { size_t agg, xpack, xpack_own, weights, total; };
 GatedWs gated_layout(int nprod, int64_t N, int64_t Ns, int T, int H, int D) {
-    GatedWs w{};
-    w.xpack = agg_bytes(nprod, N, D);
-    w.xpack_own = w.xpack + fused::packed_state_bytes(nprod, Ns, H);
-    w.weights = w.xpack_own + fused::packed_state_bytes(nprod, N, H);
-    w.total = w.weights + gated_weight_bytes(nprod, T, H, D);
+    Layout l;
+    GatedWs w;
+    w.agg = l.add_bytes(agg_bytes(nprod, N, D));
+    w.xpack = l.add_bytes(fused::packed_state_bytes(nprod, Ns, H));
+    w.xpack_own = l.add_bytes(fused::packed_state_bytes(nprod, N, H));
+    w.weights = l.add_bytes(gated_weight_bytes(nprod, T, H, D));
+    w.total = l.total;
     return w;
 }
 
 // workspace: y (pre-dense aggregate) | packed states (gathered rows) | packed target rows (sharded run) | derived weights
 struct MlpWs { size_t y, xpack, xpack_tgt, weights, total; };
 MlpWs mlp_layout(int nprod, int64_t N, int64_t Ns, int T, int H, int D, int Hout, int ut) {
-    MlpWs w{};
-    w.xpack = agg_bytes(nprod, N, D);
-    w.xpack_tgt = w.xpack + fused::packed_state_bytes(nprod, Ns, H);
-    w.weights = w.xpack_tgt + (ut ? fused::packed_state_bytes(nprod, N, H) : 0);
-    w.total = w.weights + mlp_weight_bytes(nprod, T, H, D, Hout, ut);
+    Layout l;
+    MlpWs w;
+    w.y = l.add_bytes(agg_bytes(nprod, N, D));
+    w.xpack = l.add_bytes(fused::packed_state_bytes(nprod, Ns, H));
+    w.xpack_tgt = l.add_bytes(ut ? fused::packed_state_bytes(nprod, N, H) : 0);
+    w.weights = l.add_bytes(mlp_weight_bytes(nprod, T, H, D, Hout, ut));
+    w.total = l.total;
     return w;
 }
 
@@ -214,16 +218,20 @@ size_t egc_weight_bytes(int nprod, int T, int H, int out, int bases) {
 
 // workspace: coefficients [N, hbp] fp32 | the coefficient Linear's weight [hbp, H] and bias [hbp] (zero-padded; bf16-rounded for
 // bf16 states) | the dense kernel's workspace | packed states (fp32) or the states as fp32 (bf16) | packed slabs (no cache)
-struct EgcWs { size_t coef, cw, cb, lin, x, weights, total; };
+struct EgcWs { size_t coef, cw, cb, lin, x, weights, total, params_bytes, lin_bytes; };
 EgcWs egc_layout(int nprod, int64_t N, int T, int H, int out, int heads, int bases) {
     const int hbp = egc_coef_cols(heads, bases);
-    EgcWs w{};
-    w.cw = ws_slice((size_t)N * hbp, 4);
-    w.cb = w.cw + ws_slice((size_t)hbp * H, 4);
-    w.lin = w.cb + ws_slice((size_t)hbp, 4);
-    w.x = w.lin + align_up(ptgnn_b200_linear_workspace_bytes(H, hbp), 256);
-    w.weights = w.x + (nprod == 3 ? fused::packed_state_bytes(3, N, H) : ws_slice((size_t)N * H, 4));
-    w.total = w.weights + egc_weight_bytes(nprod, T, H, out, bases);
+    Layout l;
+    EgcWs w;
+    w.coef = l.add((size_t)N * hbp, 4);
+    w.cw = l.add((size_t)hbp * H, 4);
+    w.cb = l.add((size_t)hbp, 4);
+    w.params_bytes = l.total - w.cw;
+    w.lin_bytes = ws_slice(ptgnn_b200_linear_workspace_bytes(H, hbp), 1);
+    w.lin = l.add_bytes(w.lin_bytes);
+    w.x = nprod == 3 ? l.add_bytes(fused::packed_state_bytes(3, N, H)) : l.add((size_t)N * H, 4);
+    w.weights = l.add_bytes(egc_weight_bytes(nprod, T, H, out, bases));
+    w.total = l.total;
     return w;
 }
 
@@ -242,10 +250,8 @@ __global__ void __launch_bounds__(256) egc_copy_kernel(const void *src, int src_
 int egc_copy(const void *src, int src_bf16, int64_t rows, int cols, int dst_stride, float *dst, int round_bf16, cudaStream_t st) {
     if (rows <= 0 || cols <= 0) return PTGNN_OK;
     const int64_t blocks = ceil_div(rows * cols, (int64_t)256);
-    egc_copy_kernel<<<(unsigned)(blocks < 132 * 8 ? blocks : 132 * 8), 256, 0, st>>>(src, src_bf16, (long long)rows, cols, dst_stride, dst,
-                                                                                      round_bf16);
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch(PTGNN_KERNEL_PACK, st, egc_copy_kernel, (unsigned)(blocks < 132 * 8 ? blocks : 132 * 8), 256, 0, src, src_bf16, (long long)rows,
+                  cols, dst_stride, dst, round_bf16);
 }
 
 int egc_fused(int nprod, const void *node_states, int64_t N, int H, int out, int heads, int bases, int T, const ptgnn_b200_block_plan *bp,
@@ -288,7 +294,7 @@ int egc_fused(int nprod, const void *node_states, int64_t N, int H, int out, int
     const int hb = heads * bases, hbp = egc_coef_cols(heads, bases);
     const bool bf = nprod == 1;
     float *coef = reinterpret_cast<float *>(ws + L.coef), *cw = reinterpret_cast<float *>(ws + L.cw), *cb = reinterpret_cast<float *>(ws + L.cb);
-    PTGNN_CUDA(cudaMemsetAsync(cw, 0, L.lin - L.cw, st));           // weight and bias, padding rows included
+    PTGNN_CUDA(cudaMemsetAsync(cw, 0, L.params_bytes, st));           // weight and bias, padding rows included
     if ((rc = egc_copy(coeff_weight, 0, hb, H, H, cw, bf, st))) return rc;
     if ((rc = egc_copy(coeff_bias, 0, 1, hb, hb, cb, bf, st))) return rc;
     const float *x = static_cast<const float *>(node_states);
@@ -296,7 +302,7 @@ int egc_fused(int nprod, const void *node_states, int64_t N, int H, int out, int
         if ((rc = egc_copy(node_states, 1, N, H, H, reinterpret_cast<float *>(ws + L.x), 0, st))) return rc;
         x = reinterpret_cast<const float *>(ws + L.x);
     }
-    rc = ptgnn_b200_linear_f32(x, N, H, cw, cb, hbp, PTGNN_ACT_NONE, coef, ws + L.lin, L.x - L.lin, st);
+    rc = ptgnn_b200_linear_f32(x, N, H, cw, cb, hbp, PTGNN_ACT_NONE, coef, ws + L.lin, L.lin_bytes, st);
     if (rc) return rc;
     if (bf && (rc = egc_copy(coef, 0, N, hbp, hbp, coef, 1, st))) return rc;
 

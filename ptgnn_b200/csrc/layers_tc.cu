@@ -66,12 +66,7 @@ static int derive_weights(const float *const *w, int num, int elems, T *out, T *
     WeightSrc s{};
     s.num = num; s.elems = elems;
     for (int t = 0; t < num; ++t) s.w[t] = w[t];
-    {
-        TimedScope timed__(PTGNN_KERNEL_PACK, st);
-        derive_weights_kernel<T><<<132, 256, 0, st>>>(s, out, lo);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch(PTGNN_KERNEL_PACK, st, derive_weights_kernel<T>, 132, 256, 0, s, out, lo);
 }
 
 // bias4[j] = (b_ir + b_hr, b_iz + b_hz, b_in, b_hn): one 16-byte load per hidden unit in the GRU epilogues
@@ -80,12 +75,7 @@ __global__ void pack_gru_bias_kernel(const float *__restrict__ b_ih, const float
     if (j < H) bias4[j] = make_float4(b_ih[j] + b_hh[j], b_ih[H + j] + b_hh[H + j], b_ih[2 * H + j], b_hh[2 * H + j]);
 }
 static int pack_gru_bias(const float *b_ih, const float *b_hh, int H, float4 *bias4, cudaStream_t st) {
-    {
-        TimedScope timed__(PTGNN_KERNEL_PACK, st);
-        pack_gru_bias_kernel<<<(H + 127) / 128, 128, 0, st>>>(b_ih, b_hh, H, bias4);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch(PTGNN_KERNEL_PACK, st, pack_gru_bias_kernel, (H + 127) / 128, 128, 0, b_ih, b_hh, H, bias4);
 }
 
 // Gate-blocked GRU weights, 32 hidden units per block jb, 128 rows per block.  The two dtypes order the gate blocks
@@ -500,14 +490,9 @@ int gru_update(const T *agg, const T *h, int64_t num_nodes, int H, int D, const 
     T *p1_lo = reinterpret_cast<T *>(s + s1), *p2_lo = reinterpret_cast<T *>(s + 2 * s1 + s2);   // fp32 only
     float4 *bias4 = reinterpret_cast<float4 *>(s + B_MAPS<T> * (s1 + s2));
     if (pack) {
-        {
-            TimedScope timed__(PTGNN_KERNEL_PACK, st);
-            if constexpr (IS_F32<T>) pack_split_gru_kernel<<<132, 256, 0, st>>>(w_ih, w_hh, H, D, p1, p1_lo, p2, p2_lo);
-            else pack_gru_bf16_kernel<<<132, 256, 0, st>>>(w_ih, w_hh, H, D, p1, p2);
-        }
-        PTGNN_LAUNCHED();
-        const int rc = pack_gru_bias(b_ih, b_hh, H, bias4, st);
-        if (rc) return rc;
+        if constexpr (IS_F32<T>) PTGNN_TRY(launch(PTGNN_KERNEL_PACK, st, pack_split_gru_kernel, 132, 256, 0, w_ih, w_hh, H, D, p1, p1_lo, p2, p2_lo));
+        else PTGNN_TRY(launch(PTGNN_KERNEL_PACK, st, pack_gru_bf16_kernel, 132, 256, 0, w_ih, w_hh, H, D, p1, p2));
+        PTGNN_TRY(pack_gru_bias(b_ih, b_hh, H, bias4, st));
     }
     typename GruPolicy<T>::Params p{};
     const uint64_t prow = (uint64_t)(H / 32) * 128;

@@ -114,7 +114,7 @@ __device__ __forceinline__ float warp_sum(float v) {
     return v;
 }
 
-// LAUNCH(VPL) for a row width D = 32 VPL in [32, 256] (checked by the caller)
+// LAUNCH(VPL) (a `return launch(...)`) for a row width D = 32 VPL in [32, 256] (checked by the caller)
 #define PTGNN_VPL_DISPATCH(D, LAUNCH) \
     switch ((D) / 32) {               \
         case 1: LAUNCH(1); break;     \
@@ -131,8 +131,6 @@ __device__ __forceinline__ float warp_sum(float v) {
 static inline int64_t max_chunks(int64_t N, int64_t G) { return N / CHUNK + G; }
 // rows of a per-chunk partial table
 static inline size_t partial_rows(int64_t N, int64_t G) { return (size_t)max_chunks(N, G) + 1; }
-// chunk_ptr [G + 1]: the head of every per-graph workspace
-static inline size_t ws_chunk_ptr(int64_t G) { return ws_slice((size_t)G + 1, 4); }
 // CTAs of a chunk kernel with `warps` warps per CTA: one warp per chunk, at most 64 warps per SM (the warps loop over the chunks)
 static inline int chunk_grid(int64_t N, int64_t G, int warps = 8) {
     return (int)std::min<int64_t>(ceil_div(max_chunks(N, G), warps), (int64_t)sm_count() * 64 / warps);
@@ -144,9 +142,9 @@ static inline int chunk_grid(int64_t N, int64_t G, int warps = 8) {
                     what)
 
 // chunk_ptr[b] = sum_{b' < b} ceil(count_b' / CHUNK), chunk_ptr[G] = the number of chunks
-void launch_chunk_ptr(const int32_t *row_ptr, int G, int32_t *chunk_ptr, cudaStream_t st);
+int launch_chunk_ptr(const int32_t *row_ptr, int G, int32_t *chunk_ptr, cudaStream_t st);
 // out[b][f] = sum over graph b's chunks c, in chunk order from 0, of partial[c][f] (f < width); a graph without nodes gives 0
-void launch_chunk_sum(const float *partial, const int32_t *row_ptr, const int32_t *chunk_ptr, int G, int width, float *out, cudaStream_t st);
+int launch_chunk_sum(const float *partial, const int32_t *row_ptr, const int32_t *chunk_ptr, int G, int width, float *out, cudaStream_t st);
 
 }  // namespace pergraph
 }  // namespace ptgnn

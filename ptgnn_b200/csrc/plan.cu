@@ -103,22 +103,9 @@ static int exclusive_scan_i32(const int32_t *in, int32_t *out, int64_t n, int32_
                               cudaStream_t st) {
     if (n <= 0) return PTGNN_OK;
     const int64_t nb = ceil_div(n, SCAN_CHUNK);
-    {
-        TimedScope timed__(PTGNN_KERNEL_PLAN, st);
-        scan_block_sums_kernel<<<(unsigned)nb, SCAN_THREADS, 0, st>>>(in, n, sums);
-    }
-    PTGNN_LAUNCHED();
-    {
-        TimedScope timed__(PTGNN_KERNEL_PLAN, st);
-        scan_sums_kernel<<<1, 1024, 0, st>>>(sums, nb);
-    }
-    PTGNN_LAUNCHED();
-    {
-        TimedScope timed__(PTGNN_KERNEL_PLAN, st);
-        scan_apply_kernel<<<(unsigned)nb, SCAN_THREADS, 0, st>>>(in, n, sums, out, out_total);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    PTGNN_TRY(launch(PTGNN_KERNEL_PLAN, st, scan_block_sums_kernel, (unsigned)nb, SCAN_THREADS, 0, in, n, sums));
+    PTGNN_TRY(launch(PTGNN_KERNEL_PLAN, st, scan_sums_kernel, 1, 1024, 0, sums, nb));
+    return launch(PTGNN_KERNEL_PLAN, st, scan_apply_kernel, (unsigned)nb, SCAN_THREADS, 0, in, n, sums, out, out_total);
 }
 
 // =================================================================================================
@@ -244,19 +231,18 @@ struct PlanWs {
     size_t deg, scan_sums, keys_a, keys_b, vals_a, vals_b, hist, hist_sums, total;
 };
 static PlanWs plan_ws_layout(int64_t N, int64_t E) {
-    PlanWs w{};
     const int64_t nblk = ceil_div(E > 0 ? E : 1, SORT_CHUNK);
-    size_t o = 0;
-    auto add = [&](size_t cnt) { size_t at = o; o += ws_slice(cnt, 4); return at; };
-    w.deg = add((size_t)N + 1);
-    w.scan_sums = add(scan_workspace_elems(N + 1));
-    w.keys_a = add((size_t)E + 1);
-    w.keys_b = add((size_t)E + 1);
-    w.vals_a = add((size_t)E + 1);
-    w.vals_b = add((size_t)E + 1);
-    w.hist = add((size_t)RADIX * nblk);
-    w.hist_sums = add(scan_workspace_elems((int64_t)RADIX * nblk));
-    w.total = o;
+    Layout l;
+    PlanWs w;
+    w.deg = l.add((size_t)N + 1, 4);
+    w.scan_sums = l.add(scan_workspace_elems(N + 1), 4);
+    w.keys_a = l.add((size_t)E + 1, 4);
+    w.keys_b = l.add((size_t)E + 1, 4);
+    w.vals_a = l.add((size_t)E + 1, 4);
+    w.vals_b = l.add((size_t)E + 1, 4);
+    w.hist = l.add((size_t)RADIX * nblk, 4);
+    w.hist_sums = l.add(scan_workspace_elems((int64_t)RADIX * nblk), 4);
+    w.total = l.total;
     return w;
 }
 
@@ -275,19 +261,10 @@ static int sort_edges_by_key(const int32_t *keys_in, int key_bits, int64_t E, in
     for (int p = 0; p < passes; ++p) {
         int32_t *kout = keys[p & 1];
         int32_t *vout = (p == passes - 1) ? perm : vals[p & 1];
-        {
-            TimedScope timed__(PTGNN_KERNEL_PLAN, st);
-            radix_hist_kernel<<<(unsigned)nblk, SORT_THREADS, 0, st>>>(kin, E, p * RADIX_BITS, hist);
-        }
-        PTGNN_LAUNCHED();
-        int rc = exclusive_scan_i32(hist, hist, (int64_t)RADIX * nblk, hist_sums, nullptr, st);
-        if (rc) return rc;
-        {
-            TimedScope timed__(PTGNN_KERNEL_PLAN, st);
-            radix_scatter_kernel<<<(unsigned)nblk, SORT_THREADS, 0, st>>>(kin, vin, E, p * RADIX_BITS, p == 0, hist, kout,
-                                                                      vout);
-        }
-        PTGNN_LAUNCHED();
+        PTGNN_TRY(launch(PTGNN_KERNEL_PLAN, st, radix_hist_kernel, (unsigned)nblk, SORT_THREADS, 0, kin, E, p * RADIX_BITS, hist));
+        PTGNN_TRY(exclusive_scan_i32(hist, hist, (int64_t)RADIX * nblk, hist_sums, nullptr, st));
+        PTGNN_TRY(launch(PTGNN_KERNEL_PLAN, st, radix_scatter_kernel, (unsigned)nblk, SORT_THREADS, 0, kin, vin, E, p * RADIX_BITS, p == 0, hist, kout,
+                         vout));
         kin = kout;
         vin = vout;
     }
@@ -332,15 +309,14 @@ __global__ void __launch_bounds__(256) block_finalize_kernel(int64_t num_edges, 
 }
 struct BlockPlanWs { size_t keys, perm, scan_sums, plan, total; };
 static BlockPlanWs block_plan_ws_layout(int64_t N, int64_t E, int T, int B) {
-    BlockPlanWs w{};
     const int64_t nblk = ceil_div(N > 0 ? N : 1, B), groups = nblk * (T > 0 ? T : 1) + 1;
-    size_t o = 0;
-    auto add = [&](size_t cnt) { size_t at = o; o += ws_slice(cnt, 4); return at; };
-    w.keys = add((size_t)E + 1);
-    w.perm = add((size_t)E + 1);
-    w.scan_sums = add(scan_workspace_elems(groups));
-    w.plan = o; o += plan_ws_layout(N, E).total;
-    w.total = o;
+    Layout l;
+    BlockPlanWs w;
+    w.keys = l.add((size_t)E + 1, 4);
+    w.perm = l.add((size_t)E + 1, 4);
+    w.scan_sums = l.add(scan_workspace_elems(groups), 4);
+    w.plan = l.add_bytes(plan_ws_layout(N, E).total);
+    w.total = l.total;
     return w;
 }
 
@@ -399,11 +375,7 @@ static int plan_build_phases(int phases, int64_t num_nodes, int64_t num_source_n
         }
         PTGNN_CHECK_ARG(src32 && tgt32, "plan_build: null output array");
         PTGNN_CHECK_ARG(num_nodes > 0, "plan_build: edges given but num_nodes == 0");
-        {
-            TimedScope timed__(PTGNN_KERNEL_PLAN, st);
-            convert_count_kernel<<<grid, 256, 0, st>>>(tabs, num_nodes, num_source_nodes, E, src32, tgt32, deg, status);
-        }
-        PTGNN_LAUNCHED();
+        PTGNN_TRY(launch(PTGNN_KERNEL_PLAN, st, convert_count_kernel, grid, 256, 0, tabs, num_nodes, num_source_nodes, E, src32, tgt32, deg, status));
         // row_ptr[0..N] = exclusive scan of deg[0..N] (deg[N] == 0, so row_ptr[N] == E)
         rc = exclusive_scan_i32(deg, row_ptr, num_nodes + 1, reinterpret_cast<int32_t *>(ws + L.scan_sums), nullptr, st);
         if (rc) return rc;
@@ -412,12 +384,7 @@ static int plan_build_phases(int phases, int64_t num_nodes, int64_t num_source_n
     PTGNN_CHECK_ARG(perm && pos && src_sorted && etype_sorted && src32 && tgt32, "plan_build: null output array");
     rc = sort_edges_by_target(tgt32, num_nodes, E, perm, ws, L, st);
     if (rc) return rc;
-    {
-        TimedScope timed__(PTGNN_KERNEL_PLAN, st);
-        finalize_plan_kernel<<<grid, 256, 0, st>>>(toff, E, perm, src32, pos, src_sorted, etype_sorted);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch(PTGNN_KERNEL_PLAN, st, finalize_plan_kernel, grid, 256, 0, toff, E, perm, src32, pos, src_sorted, etype_sorted);
 }
 
 extern "C" int ptgnn_b200_plan_build(int64_t num_nodes, int64_t num_source_nodes, int32_t num_types,
@@ -476,20 +443,11 @@ extern "C" int ptgnn_b200_block_plan_build(int64_t num_nodes, int32_t num_types,
     toff.num_types = T;
     for (int t = 0; t <= PTGNN_MAX_EDGE_TYPES; ++t) toff.off[t] = (int32_t)type_off[t < T ? t : T];
     const unsigned grid = (unsigned)(ceil_div(E, 256) < 132 * 16 ? ceil_div(E, 256) : 132 * 16);
-    {
-        TimedScope timed__(PTGNN_KERNEL_PLAN, st);
-        block_keys_kernel<<<grid, 256, 0, st>>>(toff, E, tgt32, B, keys, group_off);
-    }
-    PTGNN_LAUNCHED();
+    PTGNN_TRY(launch(PTGNN_KERNEL_PLAN, st, block_keys_kernel, grid, 256, 0, toff, E, tgt32, B, keys, group_off));
     int rc = exclusive_scan_i32(group_off, group_off, groups + 1, reinterpret_cast<int32_t *>(ws + L.scan_sums), nullptr, st);
     if (rc) return rc;
     const int32_t *sorted_keys = nullptr;
     rc = sort_edges_by_key(keys, bits_for(nblk * T * B), E, perm, ws + L.plan, plan_ws_layout(num_nodes, E), st, &sorted_keys);
     if (rc) return rc;
-    {
-        TimedScope timed__(PTGNN_KERNEL_PLAN, st);
-        block_finalize_kernel<<<grid, 256, 0, st>>>(E, B, perm, sorted_keys, src32, src_f, tl_f);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch(PTGNN_KERNEL_PLAN, st, block_finalize_kernel, grid, 256, 0, E, B, perm, sorted_keys, src32, src_f, tl_f);
 }

@@ -298,28 +298,19 @@ bool supported(int D) { return D % 4 == 0 && D >= 4 && D <= MAX_D; }
 static unsigned grid_of(int64_t N) { return (unsigned)ceil_div(N, (int64_t)ROWS_PER_WARP * WARPS); }
 
 template <typename T, bool ARG>
-static void launch_forward(const T *msg, const int32_t *row_ptr, const int32_t *perm, int N, int E, int D, float delta, float *out,
-                           int32_t *arg_max, int32_t *arg_min, cudaStream_t st) {
-    const unsigned grid = grid_of(N);
-    switch ((D + 127) / 128) {
-        case 1: pna_forward_kernel<T, 1, ARG><<<grid, WARPS * 32, 0, st>>>(msg, row_ptr, perm, N, E, D, delta, out, arg_max, arg_min); break;
-        case 2: pna_forward_kernel<T, 2, ARG><<<grid, WARPS * 32, 0, st>>>(msg, row_ptr, perm, N, E, D, delta, out, arg_max, arg_min); break;
-        case 3: pna_forward_kernel<T, 3, ARG><<<grid, WARPS * 32, 0, st>>>(msg, row_ptr, perm, N, E, D, delta, out, arg_max, arg_min); break;
-        default: pna_forward_kernel<T, 4, ARG><<<grid, WARPS * 32, 0, st>>>(msg, row_ptr, perm, N, E, D, delta, out, arg_max, arg_min); break;
-    }
+static int launch_forward(const T *msg, const int32_t *row_ptr, const int32_t *perm, int N, int E, int D, float delta, float *out,
+                          int32_t *arg_max, int32_t *arg_min, cudaStream_t st) {
+    const int c = (D + 127) / 128;
+    auto kernel = c == 1 ? pna_forward_kernel<T, 1, ARG> : c == 2 ? pna_forward_kernel<T, 2, ARG> : c == 3 ? pna_forward_kernel<T, 3, ARG>
+                                                                                                         : pna_forward_kernel<T, 4, ARG>;
+    return launch(PTGNN_KERNEL_REDUCE, st, kernel, grid_of(N), WARPS * 32, 0, msg, row_ptr, perm, N, E, D, delta, out, arg_max, arg_min);
 }
 
-static void launch_backward(const float *msg, const int32_t *row_ptr, const int32_t *perm, int N, int D, float delta, const float *out,
-                            const int32_t *arg_max, const int32_t *arg_min, const float *d_out, float *d_msg, cudaStream_t st) {
-    const unsigned grid = grid_of(N);
-    switch ((D + 127) / 128) {
-#define PTGNN_PNA_BWD(C) pna_backward_kernel<C><<<grid, WARPS * 32, 0, st>>>(msg, row_ptr, perm, N, D, delta, out, arg_max, arg_min, d_out, d_msg)
-        case 1: PTGNN_PNA_BWD(1); break;
-        case 2: PTGNN_PNA_BWD(2); break;
-        case 3: PTGNN_PNA_BWD(3); break;
-        default: PTGNN_PNA_BWD(4); break;
-#undef PTGNN_PNA_BWD
-    }
+static int launch_backward(const float *msg, const int32_t *row_ptr, const int32_t *perm, int N, int D, float delta, const float *out,
+                           const int32_t *arg_max, const int32_t *arg_min, const float *d_out, float *d_msg, cudaStream_t st) {
+    const int c = (D + 127) / 128;
+    auto kernel = c == 1 ? pna_backward_kernel<1> : c == 2 ? pna_backward_kernel<2> : c == 3 ? pna_backward_kernel<3> : pna_backward_kernel<4>;
+    return launch(PTGNN_KERNEL_REDUCE, st, kernel, grid_of(N), WARPS * 32, 0, msg, row_ptr, perm, N, D, delta, out, arg_max, arg_min, d_out, d_msg);
 }
 
 }  // namespace pna
@@ -355,20 +346,14 @@ extern "C" int ptgnn_b200_pna_forward(int32_t bf16_messages, const void *message
                              bf16_messages ? 8 : 16);
     if (rc != PTGNN_OK || num_targets == 0) return rc;
     const int N = (int)num_targets, E = (int)num_edges, D = message_dim;
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        if (bf16_messages) {
-            const __nv_bfloat16 *m = static_cast<const __nv_bfloat16 *>(messages);
-            if (arg_max) pna::launch_forward<__nv_bfloat16, true>(m, row_ptr, perm, N, E, D, delta, out, arg_max, arg_min, st);
-            else pna::launch_forward<__nv_bfloat16, false>(m, row_ptr, perm, N, E, D, delta, out, nullptr, nullptr, st);
-        } else {
-            const float *m = static_cast<const float *>(messages);
-            if (arg_max) pna::launch_forward<float, true>(m, row_ptr, perm, N, E, D, delta, out, arg_max, arg_min, st);
-            else pna::launch_forward<float, false>(m, row_ptr, perm, N, E, D, delta, out, nullptr, nullptr, st);
-        }
+    if (bf16_messages) {
+        const __nv_bfloat16 *m = static_cast<const __nv_bfloat16 *>(messages);
+        if (arg_max) return pna::launch_forward<__nv_bfloat16, true>(m, row_ptr, perm, N, E, D, delta, out, arg_max, arg_min, st);
+        return pna::launch_forward<__nv_bfloat16, false>(m, row_ptr, perm, N, E, D, delta, out, nullptr, nullptr, st);
     }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    const float *m = static_cast<const float *>(messages);
+    if (arg_max) return pna::launch_forward<float, true>(m, row_ptr, perm, N, E, D, delta, out, arg_max, arg_min, st);
+    return pna::launch_forward<float, false>(m, row_ptr, perm, N, E, D, delta, out, nullptr, nullptr, st);
 }
 
 extern "C" int ptgnn_b200_pna_backward_f32(const float *messages, int64_t num_edges, int32_t message_dim, const int32_t *row_ptr,
@@ -381,10 +366,5 @@ extern "C" int ptgnn_b200_pna_backward_f32(const float *messages, int64_t num_ed
     PTGNN_CHECK_ARG(num_edges == 0 || d_messages, "pna_backward: null pointer");
     PTGNN_CHECK_ARG(aligned(d_out, 16) && aligned(d_messages, 16), "pna_backward: d_out and d_messages must be 16-byte aligned");
     if (num_targets == 0 || num_edges == 0) return PTGNN_OK;
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        pna::launch_backward(messages, row_ptr, perm, (int)num_targets, message_dim, delta, out, arg_max, arg_min, d_out, d_messages, st);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return pna::launch_backward(messages, row_ptr, perm, (int)num_targets, message_dim, delta, out, arg_max, arg_min, d_out, d_messages, st);
 }

@@ -80,12 +80,20 @@ __global__ void __launch_bounds__(256) readout_finalize_kernel(const float *__re
 bool supported(int H) { return H % 32 == 0 && H >= 32 && H <= 256; }
 
 // chunk_ptr [G + 1] | partial [N / CHUNK + G + 1, H]
-size_t workspace_bytes(int64_t N, int64_t G, int H) { return ws_chunk_ptr(G) + ws_slice(partial_rows(N, G) * H, 4); }
+struct Ws { size_t chunk_ptr, partial, total; };
+static Ws layout(int64_t N, int64_t G, int H) {
+    Layout l;
+    Ws w;
+    w.chunk_ptr = l.add((size_t)G + 1, 4);
+    w.partial = l.add(partial_rows(N, G) * H, 4);
+    w.total = l.total;
+    return w;
+}
 
 template <bool BF16>
-static void launch_chunks(int H, int grid, cudaStream_t st, const void *x, const int32_t *row_ptr, const int32_t *perm, const int32_t *chunk_ptr,
-                          int G, const float *w, float *partial, float *s_out) {
-#define PTGNN_READOUT(V) readout_chunk_kernel<V, BF16><<<grid, 256, 0, st>>>(x, row_ptr, perm, chunk_ptr, G, w, partial, s_out)
+static int launch_chunks(int H, int grid, cudaStream_t st, const void *x, const int32_t *row_ptr, const int32_t *perm, const int32_t *chunk_ptr,
+                         int G, const float *w, float *partial, float *s_out) {
+#define PTGNN_READOUT(V) return launch(PTGNN_KERNEL_REDUCE, st, readout_chunk_kernel<V, BF16>, grid, 256, 0, x, row_ptr, perm, chunk_ptr, G, w, partial, s_out)
     PTGNN_VPL_DISPATCH(H, PTGNN_READOUT)
 #undef PTGNN_READOUT
 }
@@ -94,14 +102,13 @@ static void launch_chunks(int H, int grid, cudaStream_t st, const void *x, const
 
 namespace pergraph {
 
-void launch_chunk_ptr(const int32_t *row_ptr, int G, int32_t *chunk_ptr, cudaStream_t st) {
-    TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-    item_ptr_kernel<<<1, 1024, 0, st>>>(row_ptr, G, WarpChunks{}, chunk_ptr);
+int launch_chunk_ptr(const int32_t *row_ptr, int G, int32_t *chunk_ptr, cudaStream_t st) {
+    return launch(PTGNN_KERNEL_REDUCE, st, item_ptr_kernel<WarpChunks>, 1, 1024, 0, row_ptr, G, WarpChunks{}, chunk_ptr);
 }
 
-void launch_chunk_sum(const float *partial, const int32_t *row_ptr, const int32_t *chunk_ptr, int G, int width, float *out, cudaStream_t st) {
-    TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-    readout::readout_finalize_kernel<<<(unsigned)ceil_div((int64_t)G * width, 256), 256, 0, st>>>(partial, row_ptr, chunk_ptr, G, width, 0, out);
+int launch_chunk_sum(const float *partial, const int32_t *row_ptr, const int32_t *chunk_ptr, int G, int width, float *out, cudaStream_t st) {
+    return launch(PTGNN_KERNEL_REDUCE, st, readout::readout_finalize_kernel, (unsigned)ceil_div((int64_t)G * width, 256), 256, 0, partial, row_ptr,
+                  chunk_ptr, G, width, 0, out);
 }
 
 }  // namespace pergraph
@@ -111,7 +118,7 @@ using namespace ptgnn;
 
 extern "C" size_t ptgnn_b200_graph_readout_workspace_bytes(int64_t num_nodes, int64_t num_graphs, int32_t state_dim) {
     if (num_nodes < 0 || num_graphs < 0 || !readout::supported(state_dim)) return 0;
-    return readout::workspace_bytes(num_nodes, num_graphs, state_dim);
+    return readout::layout(num_nodes, num_graphs, state_dim).total;
 }
 
 extern "C" int ptgnn_b200_graph_readout(int32_t bf16_states, const void *node_states, int64_t num_nodes, int32_t state_dim,
@@ -128,27 +135,19 @@ extern "C" int ptgnn_b200_graph_readout(int32_t bf16_states, const void *node_st
     PTGNN_CHECK_ARG(mode != PTGNN_READOUT_WEIGHTED_SUM || gate_weight != nullptr, "graph_readout: the weighted sum needs gate_weight");
     if (num_graphs == 0) return PTGNN_OK;
     PTGNN_CHECK_ARG(row_ptr && g && (num_nodes == 0 || (node_states && perm)), "graph_readout: null pointer");
-    PTGNN_CHECK_WORKSPACE("graph_readout", workspace, workspace_bytes, readout::workspace_bytes(num_nodes, num_graphs, H));
+    const readout::Ws L = readout::layout(num_nodes, num_graphs, H);
+    PTGNN_CHECK_WORKSPACE("graph_readout", workspace, workspace_bytes, L.total);
     const int G = (int)num_graphs;
-    int32_t *chunk_ptr = static_cast<int32_t *>(workspace);
-    float *partial = reinterpret_cast<float *>(static_cast<char *>(workspace) + pergraph::ws_chunk_ptr(num_graphs));
+    char *ws = static_cast<char *>(workspace);
+    int32_t *chunk_ptr = reinterpret_cast<int32_t *>(ws + L.chunk_ptr);
+    float *partial = reinterpret_cast<float *>(ws + L.partial);
     const float *w = mode == PTGNN_READOUT_WEIGHTED_SUM ? gate_weight : nullptr;
-    pergraph::launch_chunk_ptr(row_ptr, G, chunk_ptr, st);
-    PTGNN_LAUNCHED();
+    PTGNN_TRY(pergraph::launch_chunk_ptr(row_ptr, G, chunk_ptr, st));
     if (num_nodes > 0) {
         const int grid = pergraph::chunk_grid(num_nodes, num_graphs);
-        {
-            TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-            if (bf16_states) readout::launch_chunks<true>(H, grid, st, node_states, row_ptr, perm, chunk_ptr, G, w, partial, w ? s : nullptr);
-            else readout::launch_chunks<false>(H, grid, st, node_states, row_ptr, perm, chunk_ptr, G, w, partial, w ? s : nullptr);
-        }
-        PTGNN_LAUNCHED();
+        if (bf16_states) PTGNN_TRY(readout::launch_chunks<true>(H, grid, st, node_states, row_ptr, perm, chunk_ptr, G, w, partial, w ? s : nullptr));
+        else PTGNN_TRY(readout::launch_chunks<false>(H, grid, st, node_states, row_ptr, perm, chunk_ptr, G, w, partial, w ? s : nullptr));
     }
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        readout::readout_finalize_kernel<<<(unsigned)ceil_div((int64_t)G * H, 256), 256, 0, st>>>(partial, row_ptr, chunk_ptr, G, H,
-                                                                                                 mode == PTGNN_READOUT_MEAN, g);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch(PTGNN_KERNEL_REDUCE, st, readout::readout_finalize_kernel, (unsigned)ceil_div((int64_t)G * H, 256), 256, 0, partial, row_ptr,
+                  chunk_ptr, G, H, mode == PTGNN_READOUT_MEAN ? 1 : 0, g);
 }

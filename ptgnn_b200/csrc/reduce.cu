@@ -12,27 +12,14 @@ static int launch_shape(const float *msg, const int32_t *row_ptr, const int32_t 
     const unsigned grid = (unsigned)ceil_div(N, ROWS_PER_BLOCK);
     ReduceEpilogue e{};
     if (epi) e = *epi;
-    if (epi) {
-        {
-            TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-            segment_reduce_kernel<RED, LPR, CHUNKS, false, true>
-            <<<grid, 256, 0, st>>>(msg, row_ptr, perm, (int)N, (int)E, D, out, nullptr, e);
-        }
-    } else if (arg_out && (RED == PTGNN_REDUCE_MAX || RED == PTGNN_REDUCE_MIN)) {
-        {
-            TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-            segment_reduce_kernel<RED, LPR, CHUNKS, true, false>
-            <<<grid, 256, 0, st>>>(msg, row_ptr, perm, (int)N, (int)E, D, out, arg_out, e);
-        }
-    } else {
-        {
-            TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-            segment_reduce_kernel<RED, LPR, CHUNKS, false, false>
-            <<<grid, 256, 0, st>>>(msg, row_ptr, perm, (int)N, (int)E, D, out, nullptr, e);
-        }
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    if (epi)
+        return launch(PTGNN_KERNEL_REDUCE, st, segment_reduce_kernel<RED, LPR, CHUNKS, false, true>, grid, 256, 0, msg, row_ptr, perm, (int)N, (int)E,
+                      D, out, nullptr, e);
+    if (arg_out && (RED == PTGNN_REDUCE_MAX || RED == PTGNN_REDUCE_MIN))
+        return launch(PTGNN_KERNEL_REDUCE, st, segment_reduce_kernel<RED, LPR, CHUNKS, true, false>, grid, 256, 0, msg, row_ptr, perm, (int)N, (int)E,
+                      D, out, arg_out, e);
+    return launch(PTGNN_KERNEL_REDUCE, st, segment_reduce_kernel<RED, LPR, CHUNKS, false, false>, grid, 256, 0, msg, row_ptr, perm, (int)N, (int)E, D,
+                  out, nullptr, e);
 }
 
 template <typename T, int RED, int CHUNKS>
@@ -41,13 +28,8 @@ static int launch_stream(const T *msg, const int32_t *row_ptr, const int32_t *pe
     const unsigned grid = (unsigned)ceil_div(N, 8 * 16);   // 8 warps x 16 rows per block
     ReduceEpilogue e{};
     if (epi) e = *epi;
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        if (epi) segment_reduce_stream_kernel<T, RED, CHUNKS, true><<<grid, 256, 0, st>>>(msg, row_ptr, perm, (int)N, D, out, e);
-        else segment_reduce_stream_kernel<T, RED, CHUNKS, false><<<grid, 256, 0, st>>>(msg, row_ptr, perm, (int)N, D, out, e);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch(PTGNN_KERNEL_REDUCE, st, epi ? segment_reduce_stream_kernel<T, RED, CHUNKS, true> : segment_reduce_stream_kernel<T, RED, CHUNKS, false>,
+                  grid, 256, 0, msg, row_ptr, perm, (int)N, D, out, e);
 }
 
 template <int RED>
@@ -114,20 +96,18 @@ struct ScatterWs {
     size_t row_ptr, perm, pos, src_sorted, etype_sorted, src32, tgt32, status, plan, total;
 };
 ScatterWs scatter_ws_layout(int64_t N, int64_t E) {
-    ScatterWs w{};
-    size_t o = 0;
-    auto add = [&](size_t cnt, size_t elt) { size_t at = o; o += ws_slice(cnt, elt); return at; };
-    w.row_ptr = add((size_t)N + 1, 4);
-    w.perm = add((size_t)E + 1, 4);
-    w.pos = add((size_t)E + 1, 4);
-    w.src_sorted = add((size_t)E + 1, 4);
-    w.etype_sorted = add((size_t)E + 1, 1);
-    w.src32 = add((size_t)E + 1, 4);
-    w.tgt32 = add((size_t)E + 1, 4);
-    w.status = add(1, 4);
-    w.plan = o;
-    o += ptgnn_b200_plan_workspace_bytes(N, E);
-    w.total = o;
+    Layout l;
+    ScatterWs w;
+    w.row_ptr = l.add((size_t)N + 1, 4);
+    w.perm = l.add((size_t)E + 1, 4);
+    w.pos = l.add((size_t)E + 1, 4);
+    w.src_sorted = l.add((size_t)E + 1, 4);
+    w.etype_sorted = l.add((size_t)E + 1, 1);
+    w.src32 = l.add((size_t)E + 1, 4);
+    w.tgt32 = l.add((size_t)E + 1, 4);
+    w.status = l.add(1, 4);
+    w.plan = l.add_bytes(ptgnn_b200_plan_workspace_bytes(N, E));
+    w.total = l.total;
     return w;
 }
 }  // namespace

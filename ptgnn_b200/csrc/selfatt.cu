@@ -502,16 +502,24 @@ bool supported(int dk, int dv) {
 }
 
 // tile_ptr[g] = sum_{g' < g} tiles(c_g'), tile_ptr[G] = the number of tiles
-static void launch_tile_ptr(const int32_t *row_ptr, int G, int L, int32_t *tile_ptr, cudaStream_t st) {
-    TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-    pergraph::item_ptr_kernel<<<1, 1024, 0, st>>>(row_ptr, G, pergraph::ChunkTiles<TILE>{L}, tile_ptr);
+static int launch_tile_ptr(const int32_t *row_ptr, int G, int L, int32_t *tile_ptr, cudaStream_t st) {
+    return launch(PTGNN_KERNEL_REDUCE, st, pergraph::item_ptr_kernel<pergraph::ChunkTiles<TILE>>, 1, 1024, 0, row_ptr, G,
+                  pergraph::ChunkTiles<TILE>{L}, tile_ptr);
 }
 
 // tile bound: sum_g tiles(c_g) <= sum_g (c_g / 64 + c_g / L + 1) <= ceil(R / 64) + ceil(R / L) + G
 static int64_t max_tiles(int64_t rows, int64_t G, int64_t L) { return ceil_div(rows, TILE) + ceil_div(rows, L) + G; }
 
 // tile_ptr [G + 1] | delta [rows, heads] (backward)
-size_t workspace_bytes(int64_t rows, int64_t G, int heads) { return pergraph::ws_chunk_ptr(G) + ws_slice((size_t)rows * heads, 4); }
+struct Ws { size_t tile_ptr, delta, total; };
+static Ws layout(int64_t rows, int64_t G, int heads) {
+    Layout l;
+    Ws w;
+    w.tile_ptr = l.add((size_t)G + 1, 4);
+    w.delta = l.add((size_t)rows * heads, 4);
+    w.total = l.total;
+    return w;
+}
 
 #define PTGNN_SELFATT_DV(DK, CASE)                                                                                                     \
     switch (dv) {                                                                                                                      \
@@ -529,40 +537,26 @@ size_t workspace_bytes(int64_t rows, int64_t G, int heads) { return pergraph::ws
     }
 
 template <bool BF16>
-static cudaError_t launch_forward(int dk, int dv, dim3 grid, cudaStream_t st, const void *t, int heads, const int32_t *row_ptr,
-                                  const int32_t *tile_ptr, int G, int L, float sqrt_dk, void *o, float *lse, int32_t *status) {
-    cudaError_t err = cudaSuccess;
+static int launch_forward(int dk, int dv, dim3 grid, cudaStream_t st, const void *t, int heads, const int32_t *row_ptr, const int32_t *tile_ptr,
+                          int G, int L, float sqrt_dk, void *o, float *lse, int32_t *status) {
 #define PTGNN_FWD(DK, DV)                                                                                                              \
-    do {                                                                                                                               \
-        constexpr int smem = Fwd<DK, DV, BF16>::SMEM;                                                                                  \
-        err = cudaFuncSetAttribute(selfatt_fwd_kernel<DK, DV, BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);               \
-        if (err == cudaSuccess)                                                                                                        \
-            selfatt_fwd_kernel<DK, DV, BF16><<<grid, 128, smem, st>>>(t, heads, row_ptr, tile_ptr, G, L, sqrt_dk, o, lse, status);     \
-    } while (0)
+    return launch(PTGNN_KERNEL_REDUCE, st, selfatt_fwd_kernel<DK, DV, BF16>, grid, 128, Fwd<DK, DV, BF16>::SMEM, t, heads, row_ptr, tile_ptr, G, L, \
+                  sqrt_dk, o, lse, status)
     PTGNN_SELFATT_DISPATCH(PTGNN_FWD)
 #undef PTGNN_FWD
-    return err;
 }
 
-static cudaError_t launch_backward(int dk, int dv, dim3 grid, cudaStream_t st, const float *t, int heads, const int32_t *row_ptr,
-                                   const int32_t *tile_ptr, int G, int L, float sqrt_dk, const float *lse, const float *delta,
-                                   const float *d_o, float *d_t) {
-    cudaError_t err = cudaSuccess;
+static int launch_backward(int dk, int dv, dim3 grid, cudaStream_t st, const float *t, int heads, const int32_t *row_ptr, const int32_t *tile_ptr,
+                           int G, int L, float sqrt_dk, const float *lse, const float *delta, const float *d_o, float *d_t) {
 #define PTGNN_BWD(DK, DV)                                                                                                              \
-    do {                                                                                                                               \
-        constexpr int kv = Bwd<DK, DV>::KV_FLOATS * 4, q = Bwd<DK, DV>::Q_FLOATS * 4;                                                 \
-        err = cudaFuncSetAttribute(selfatt_bwd_kv_kernel<DK, DV>, cudaFuncAttributeMaxDynamicSharedMemorySize, kv);                    \
-        if (err == cudaSuccess) err = cudaFuncSetAttribute(selfatt_bwd_q_kernel<DK, DV>, cudaFuncAttributeMaxDynamicSharedMemorySize, q); \
-        if (err == cudaSuccess) {                                                                                                      \
-            selfatt_bwd_kv_kernel<DK, DV><<<grid, 256, kv, st>>>(t, heads, row_ptr, tile_ptr, G, L, sqrt_dk, lse, delta, d_o, d_t);    \
-            err = cudaGetLastError();                                                                                                  \
-        }                                                                                                                              \
-        if (err == cudaSuccess)                                                                                                        \
-            selfatt_bwd_q_kernel<DK, DV><<<grid, 256, q, st>>>(t, heads, row_ptr, tile_ptr, G, L, sqrt_dk, lse, delta, d_o, d_t);      \
-    } while (0)
+    {                                                                                                                                  \
+        PTGNN_TRY(launch(PTGNN_KERNEL_REDUCE, st, selfatt_bwd_kv_kernel<DK, DV>, grid, 256, Bwd<DK, DV>::KV_FLOATS * 4, t, heads, row_ptr,   \
+                         tile_ptr, G, L, sqrt_dk, lse, delta, d_o, d_t));                                                              \
+        return launch(PTGNN_KERNEL_REDUCE, st, selfatt_bwd_q_kernel<DK, DV>, grid, 256, Bwd<DK, DV>::Q_FLOATS * 4, t, heads, row_ptr, tile_ptr, \
+                      G, L, sqrt_dk, lse, delta, d_o, d_t);                                                                            \
+    }
     PTGNN_SELFATT_DISPATCH(PTGNN_BWD)
 #undef PTGNN_BWD
-    return err;
 }
 
 }  // namespace selfatt
@@ -577,7 +571,7 @@ extern "C" int32_t ptgnn_b200_selfatt_supported(int32_t bf16_states, int32_t key
 
 extern "C" size_t ptgnn_b200_selfatt_workspace_bytes(int64_t rows, int64_t num_graphs, int32_t num_heads) {
     if (rows < 0 || num_graphs < 0 || num_heads <= 0) return 0;
-    return selfatt::workspace_bytes(rows, num_graphs, num_heads);
+    return selfatt::layout(rows, num_graphs, num_heads).total;
 }
 
 // shared argument checks; returns PTGNN_OK or an error code (set_error done)
@@ -592,7 +586,7 @@ static int selfatt_check(const char *what, const void *qkv, int64_t rows, int32_
     }
     if (num_graphs == 0 || rows == 0) return PTGNN_OK;
     PTGNN_CHECK_ARG(qkv && row_ptr && o && lse, "%s: null pointer", what);
-    PTGNN_CHECK_WORKSPACE(what, workspace, workspace_bytes, selfatt::workspace_bytes(rows, num_graphs, heads));
+    PTGNN_CHECK_WORKSPACE(what, workspace, workspace_bytes, selfatt::layout(rows, num_graphs, heads).total);
     return PTGNN_OK;
 }
 
@@ -604,20 +598,13 @@ extern "C" int ptgnn_b200_selfatt_forward(int32_t bf16_states, const void *qkv, 
                                  workspace, workspace_bytes);
     if (rc != PTGNN_OK || num_graphs == 0 || rows == 0) return rc;
     const int G = (int)num_graphs, L = (int)std::min<int64_t>(max_chunk, rows);   // a chunk never holds more than `rows` rows
-    int32_t *tile_ptr = static_cast<int32_t *>(workspace);
-    selfatt::launch_tile_ptr(row_ptr, G, L, tile_ptr, st);
-    PTGNN_LAUNCHED();
+    int32_t *tile_ptr = reinterpret_cast<int32_t *>(static_cast<char *>(workspace) + selfatt::layout(rows, num_graphs, num_heads).tile_ptr);
+    PTGNN_TRY(selfatt::launch_tile_ptr(row_ptr, G, L, tile_ptr, st));
     const dim3 grid((unsigned)selfatt::max_tiles(rows, num_graphs, L), (unsigned)num_heads);
     const float sqrt_dk = sqrtf((float)key_query_dim);
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        const cudaError_t err = bf16_states
-            ? selfatt::launch_forward<true>(key_query_dim, value_dim, grid, st, qkv, num_heads, row_ptr, tile_ptr, G, L, sqrt_dk, o, lse, status)
-            : selfatt::launch_forward<false>(key_query_dim, value_dim, grid, st, qkv, num_heads, row_ptr, tile_ptr, G, L, sqrt_dk, o, lse, status);
-        PTGNN_CUDA(err);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    if (bf16_states)
+        return selfatt::launch_forward<true>(key_query_dim, value_dim, grid, st, qkv, num_heads, row_ptr, tile_ptr, G, L, sqrt_dk, o, lse, status);
+    return selfatt::launch_forward<false>(key_query_dim, value_dim, grid, st, qkv, num_heads, row_ptr, tile_ptr, G, L, sqrt_dk, o, lse, status);
 }
 
 extern "C" int ptgnn_b200_selfatt_backward_f32(const float *qkv, int64_t rows, int32_t num_heads, int32_t key_query_dim, int32_t value_dim,
@@ -629,23 +616,15 @@ extern "C" int ptgnn_b200_selfatt_backward_f32(const float *qkv, int64_t rows, i
     if (rc != PTGNN_OK || num_graphs == 0 || rows == 0) return rc;
     PTGNN_CHECK_ARG(d_o && d_qkv, "selfatt_backward: null pointer");
     const int G = (int)num_graphs, L = (int)std::min<int64_t>(max_chunk, rows);
+    const selfatt::Ws W = selfatt::layout(rows, num_graphs, num_heads);
     char *ws = static_cast<char *>(workspace);
-    int32_t *tile_ptr = reinterpret_cast<int32_t *>(ws);
-    float *delta = reinterpret_cast<float *>(ws + pergraph::ws_chunk_ptr(num_graphs));
-    selfatt::launch_tile_ptr(row_ptr, G, L, tile_ptr, st);
-    PTGNN_LAUNCHED();
+    int32_t *tile_ptr = reinterpret_cast<int32_t *>(ws + W.tile_ptr);
+    float *delta = reinterpret_cast<float *>(ws + W.delta);
+    PTGNN_TRY(selfatt::launch_tile_ptr(row_ptr, G, L, tile_ptr, st));
     const long long rh = (long long)rows * num_heads;
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        selfatt::selfatt_delta_kernel<<<(unsigned)ceil_div(rh, 256), 256, 0, st>>>(d_o, static_cast<const float *>(o), rh, value_dim, delta);
-    }
-    PTGNN_LAUNCHED();
+    PTGNN_TRY(launch(PTGNN_KERNEL_REDUCE, st, selfatt::selfatt_delta_kernel, (unsigned)ceil_div(rh, 256), 256, 0, d_o, static_cast<const float *>(o),
+                     rh, value_dim, delta));
     const dim3 grid((unsigned)selfatt::max_tiles(rows, num_graphs, L), (unsigned)num_heads);
-    {
-        TimedScope timed__(PTGNN_KERNEL_REDUCE, st);
-        PTGNN_CUDA(selfatt::launch_backward(key_query_dim, value_dim, grid, st, qkv, num_heads, row_ptr, tile_ptr, G, L,
-                                            sqrtf((float)key_query_dim), lse, delta, d_o, d_qkv));
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return selfatt::launch_backward(key_query_dim, value_dim, grid, st, qkv, num_heads, row_ptr, tile_ptr, G, L, sqrtf((float)key_query_dim), lse,
+                                    delta, d_o, d_qkv);
 }

@@ -406,16 +406,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
 template <class Params>
 static int launch_pipeline(void (*kernel)(Params), const Params &p, int smem_bytes, int total_tiles, int category, cudaStream_t st) {
     if (total_tiles <= 0) return PTGNN_OK;
-    // per launch, not once per process: the attribute is per device (and per context)
-    PTGNN_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
     const int sms = sm_count();
     const int grid = total_tiles < sms ? total_tiles : sms;
-    {
-        TimedScope timed__(category, st);
-        kernel<<<grid, NUM_THREADS, smem_bytes, st>>>(p);
-    }
-    PTGNN_LAUNCHED();
-    return PTGNN_OK;
+    return launch(category, st, kernel, grid, NUM_THREADS, smem_bytes, p);
 }
 
 }  // namespace tc

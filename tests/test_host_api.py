@@ -127,6 +127,48 @@ _LINEAR_WS = {(128, 128): 131328, (36, 200): 58112, (256, 64): 131328, (32, 16):
 _EDGE_MESSAGES_WS = {(17, 128, 128, 0): 2228480, (3, 64, 192, 1): 590080, (1, 36, 16, 0): 4864, (5, 256, 112, 1): 2294016}
 _GRUCELL_WS = {(128, 128): 1968896, (64, 36): 522496, (256, 256): 6787840, (96, 32): 854272}
 
+# every other size query of the header: name -> {arguments (bf16_states first where the query takes it): bytes}; 0 marks an
+# unsupported shape
+_OTHER_SIZES = {
+    "plan_workspace_bytes": {(1000, 5000): 88576, (777, 4321): 76544, (0, 0): 2816, (5, 0): 2816, (100000, 1): 402688},
+    "scatter_workspace_bytes": {(1000, 5000): 199168, (777, 4321): 171520, (0, 0): 4864, (5, 0): 4864, (100000, 1): 804608},
+    "block_plan_workspace_bytes": {(1000, 5000, 17, 64): 129280, (777, 4321, 3, 64): 111616, (0, 0, 1, 64): 3584, (5, 0, 2, 64): 3584,
+        (4096, 70000, 33, 64): 1733632},
+    "gated_fused_workspace_bytes": {(0, 1000, 0, 17, 128, 128): 3046144, (0, 777, 500, 3, 64, 128): 972288,
+        (0, 0, 0, 2, 128, 128): 527104, (0, 500, 0, 5, 256, 128): 3119872, (0, 1000, 0, 4, 96, 36): 1262848,
+        (1, 1000, 0, 17, 128, 128): 1011968, (1, 777, 500, 3, 64, 128): 323072, (1, 0, 0, 2, 128, 128): 264448,
+        (1, 500, 0, 5, 256, 128): 1049856, (1, 1000, 0, 4, 96, 36): 248064},
+    "gated_fused_weight_cache_bytes": {(0, 17, 128, 128): 1509376, (0, 3, 64, 128): 246784, (0, 5, 256, 128): 1839104,
+        (0, 1, 128, 128): 460800, (0, 4, 96, 36): 350208, (1, 17, 128, 128): 755712, (1, 3, 64, 128): 123904, (1, 5, 256, 128): 921600,
+        (1, 1, 128, 128): 231424, (1, 4, 96, 36): 175872},
+    "packed_state_bytes": {(1000, 128): 512256, (777, 64): 199168, (0, 128): 256, (1, 256): 1280, (5000, 96): 1920256},
+    "egc_fused_workspace_bytes": {(0, 1000, 17, 128, 128, 8, 4): 5146368, (0, 777, 3, 64, 128, 4, 2): 427520,
+        (0, 0, 2, 128, 128, 8, 4): 574208, (0, 500, 5, 256, 128, 8, 8): 0, (0, 1000, 4, 96, 36, 2, 2): 0,
+        (1, 1000, 17, 128, 128, 8, 4): 2917888, (1, 777, 3, 64, 128, 4, 2): 328960, (1, 0, 2, 128, 128, 8, 4): 311808,
+        (1, 500, 5, 256, 128, 8, 8): 3458560, (1, 1000, 4, 96, 36, 2, 2): 0},
+    "egc_fused_weight_cache_bytes": {(0, 17, 128, 128, 8, 4): 4456448, (0, 3, 64, 128, 4, 2): 196608, (0, 5, 256, 128, 8, 8): 0,
+        (0, 1, 128, 128, 1, 1): 65536, (0, 4, 96, 36, 2, 2): 0, (1, 17, 128, 128, 8, 4): 2228224, (1, 3, 64, 128, 4, 2): 98304,
+        (1, 5, 256, 128, 8, 8): 2621440, (1, 1, 128, 128, 1, 1): 32768, (1, 4, 96, 36, 2, 2): 0},
+    "global_gru_workspace_bytes": {(0, 1000, 10, 128, 128): 1119744, (0, 777, 3, 64, 36): 307200, (0, 0, 0, 128, 64): 395776,
+        (0, 5, 1, 256, 256): 2372096, (0, 1000, 10, 96, 128): 0, (1, 1000, 10, 128, 128): 509184, (1, 777, 3, 64, 36): 83456,
+        (1, 0, 0, 128, 64): 297216, (1, 5, 1, 256, 256): 1973504, (1, 1000, 10, 96, 128): 0},
+    "global_gru_weight_cache_bytes": {(0, 64): 50176, (0, 128): 198656, (0, 192): 445440, (0, 256): 790528, (0, 96): 0, (1, 64): 25600,
+        (1, 128): 100352, (1, 192): 224256, (1, 256): 397312, (1, 96): 0},
+    "graph_readout_workspace_bytes": {(1000, 10, 128): 21760, (777, 3, 64): 7424, (0, 0, 32): 512, (0, 5, 256): 6400, (33, 1, 96): 1536,
+        (10, 2, 36): 0},
+    "attention_readout_workspace_bytes": {(1000, 10, 128, 8): 175360, (777, 3, 64, 1): 7936, (0, 0, 32, 4): 1280, (0, 5, 256, 2): 13056,
+        (33, 1, 96, 3): 0},
+    "selfatt_workspace_bytes": {(1000, 10, 8): 32256, (777, 3, 1): 3584, (0, 0, 4): 256, (0, 5, 2): 256, (4096, 1, 3): 49408},
+    "graph_norm_workspace_bytes": {(1000, 10, 128): 73984, (777, 3, 64): 19200, (0, 0, 32): 512, (0, 5, 256): 43264, (33, 1, 96): 4864},
+    "copy_attention_workspace_bytes": {(1000, 10, 128, 4): 86272, (777, 3, 64, 1): 7424, (0, 0, 32, 7): 1280, (0, 5, 256, 2): 12544,
+        (33, 1, 96, 3): 0},
+    "embedding_bag_backward_workspace_bytes": {(1000, 8, 5000, 128): 2708736, (777, 1, 100, 63): 32256, (0, 4, 10, 64): 3072,
+        (5, 0, 10, 64): 0, (33, 3, 0, 32): 768},
+    "char_cnn_workspace_bytes": {(0, 98, 64, 3, 128, 5, 128, 2): 372736, (0, 256, 256, 5, 64, 3, 64, 4): 1574912,
+        (0, 0, 64, 3, 64, 3, 64, 2): 0, (0, 98, 128, 1, 256, 1, 200, 1): 445440, (0, 98, 64, 3, 64, 3, 300, 2): 0,
+        (1, 98, 64, 3, 128, 5, 128, 2): 225280, (1, 256, 256, 5, 64, 3, 64, 4): 1443840, (1, 0, 64, 3, 64, 3, 64, 2): 0,
+        (1, 98, 128, 1, 256, 1, 200, 1): 248832, (1, 98, 64, 3, 64, 3, 300, 2): 0},
+}
 
 def test_unfused_layer_buffer_sizes_are_pinned():
     """The layers' and stand-alone pieces' workspace and weight-cache layouts, per state dtype: exact byte counts (a layout
@@ -159,6 +201,16 @@ def test_unfused_layer_buffer_sizes_are_pinned():
     env = dict(os.environ, PTGNN_B200_DISABLE_TC="1")
     out = subprocess.run([sys.executable, "-s", "-c", script], cwd=ROOT, env=env, capture_output=True, text=True, check=True)
     assert out.stdout.split() == ["0", "887296", "7269376"]
+
+
+def test_every_other_buffer_size_is_pinned():
+    """The plan, per-graph, fused-layer, embedding and char-CNN workspace and weight-cache layouts: exact byte counts, including
+    zero nodes and zero graphs."""
+    handle = N.lib()
+    for name, cases in _OTHER_SIZES.items():
+        query = getattr(handle, "ptgnn_b200_" + name)
+        for args, want in cases.items():
+            assert query(*args) == want, (name, args)
 
 
 def test_no_cpu_fallback():
