@@ -540,6 +540,35 @@ int ptgnn_b200_char_cnn_materialise_f32(const int64_t *chars_ids, int64_t rows, 
                                         const void *prepared, size_t prepared_bytes, float *a1, float *a2, int32_t *status, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Linear feature embedder (reference neuralmodels/embeddings/linearmapembedding.py:13-29, LinearFeatureEmbedder):
+ *   out[n, d] = act(sum_{f < in_dim} x[n, f] W[d, f])   x [rows, in_dim] fp32 row-major, W [out_dim, in_dim] fp32 (nn.Linear.weight),
+ *   act = PTGNN_ACT_*; out [rows, out_dim] fp32, or bf16 when bf16_out != 0 (bf16 operands, one product; the pre-activation and the
+ *   result rounded to bf16, as autocast's Linear and the activation of its bf16 output round them).  fp32: 3xFP16 tensor-core products.
+ *   One persistent kernel: each CTA keeps its column slice of the prepared W in shared memory and streams 128-row tiles of x.
+ *   packed_out (optional, fp32 only): ptgnn_b200_packed_state_bytes(rows, out_dim) bytes, receives the packed form of out -- what
+ *   the fused layers take as packed_states_in (bit-identical to packing out).  pre_out (optional, fp32) [rows, out_dim]: the value
+ *   before the activation (the GELU backward reads it).
+ *   status (optional): a device-accessible int32 set to 1 when an fp32 operand of x or W, or a packed output value, is outside the
+ *   fp16 range (|x| >= 65504).  No host synchronisation, deterministic (DESIGN.md §3.15).
+ *   Supported (ptgnn_b200_feature_embed_supported): in_dim in [1, 512], out_dim a multiple of 8 in [8, 256]; otherwise
+ *   PTGNN_E_UNSUPPORTED.  out, packed_out and pre_out 16-byte aligned, x 4-byte aligned.
+ * feature_embed_workspace_bytes / feature_embed_prepare: W split (fp32) or rounded (bf16), zero-padded and pre-swizzled per column
+ *   block into a 16-byte aligned buffer; prepare once per parameter version and pass the same buffer and bf16 flag to the forward.
+ *   prepare sets status for a weight outside the fp16 range.
+ * activation_grad_f32: grad_pre = grad_out * act'(pre), elementwise over count values; `saved` is the output for RELU and TANH and
+ *   the pre-activation for GELU (NONE copies grad_out).
+ * ---------------------------------------------------------------------------------------------- */
+int32_t ptgnn_b200_feature_embed_supported(int32_t in_dim, int32_t out_dim);
+size_t ptgnn_b200_feature_embed_workspace_bytes(int32_t bf16, int32_t in_dim, int32_t out_dim);
+int ptgnn_b200_feature_embed_prepare(int32_t bf16, const float *weight, int32_t in_dim, int32_t out_dim, void *prepared,
+                                     size_t prepared_bytes, int32_t *status, void *stream);
+int ptgnn_b200_feature_embed_forward(int32_t bf16_out, const float *x, int64_t rows, int32_t in_dim, int32_t out_dim, int32_t activation,
+                                     const void *prepared, size_t prepared_bytes, void *out, void *packed_out /* optional */,
+                                     float *pre_out /* optional */, int32_t *status, void *stream);
+int ptgnn_b200_activation_grad_f32(int32_t activation, const float *grad_out, const float *saved, int64_t count, float *grad_pre,
+                                   void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Host-buffer convenience entry point (used for the end-to-end measurement): all pointers are HOST
  * memory; copies inputs to the device, builds the plan, runs `num_layers` GatedMessagePassingLayers
  * (layer l uses weight set l; pass the same pointers to share weights), copies the final states back

@@ -791,6 +791,41 @@ def char_cnn_with_grad(chars, shape, prepared, status, w1, b1, w2, b2, w3):
 
 
 # =====================================================================================================================
+# LinearFeatureEmbedder (linearmapembedding.py:13-29): act(x W^T) on the native feature-embedding kernel.  fp32.
+# =====================================================================================================================
+class _FeatureEmbedFn(torch.autograd.Function):
+    """out [N, D] from x [N, F] and W [D, F].  act' is read from what torch's own backward reads, so nothing is recomputed: the output
+    for ReLU and Tanh (already kept as the result), the pre-activation for GELU (one more [N, D] fp32 write in the same launch, cheaper
+    than re-running the GEMM, which reads x again); None needs neither.  Backward: d pre on one native pointwise pass, dW = d pre^T x as
+    split fp16 library GEMMs (K = N), dx on the native dense kernel only when x requires a gradient."""
+
+    @staticmethod
+    def forward(ctx, x, weight, prepared, act, status):
+        from .embeddings import native_feature_embed
+
+        out, _, pre = native_feature_embed(x.detach(), prepared, weight.shape[0], act, want_pre=act == N.ACT_GELU, status=status)
+        ctx.act = act
+        ctx.save_for_backward(x, weight, pre if act == N.ACT_GELU else (None if act == N.ACT_NONE else out))
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        from .embeddings import native_activation_grad
+
+        x, weight, saved = ctx.saved_tensors
+        g = g.contiguous().float()
+        d_pre = g if ctx.act == N.ACT_NONE else native_activation_grad(ctx.act, g, saved)
+        d_w = _mm_t_split(_split16(d_pre), _split16(x.detach())) if ctx.needs_input_grad[1] else None
+        d_x = C.linear(d_pre, weight.detach().t().contiguous()) if ctx.needs_input_grad[0] else None
+        return d_x, d_w, None, None, None
+
+
+def feature_embed_with_grad(x, weight, prepared, act, status=None):
+    return _FeatureEmbedFn.apply(x, weight, prepared, act, status)
+
+
+# =====================================================================================================================
 # GruCopyingDecoder (grucopydecoder.py:95-97, 122-124): the copy scores s[i, l] = c_i . o[graph(i), l] and their per-sample logsumexp
 # on the native kernel.  fp32 copy representations.
 # =====================================================================================================================

@@ -25,6 +25,13 @@ multiple of 4 (the native ``linear`` operator).
 kernel, ``ptgnn_b200_char_cnn_forward`` (DESIGN.md §3.13): the one-hot input and the [B, F, L] conv outputs never exist.  Its derived
 weights (W1 as a gather table, W2 / W3 split and pre-swizzled) are kept per parameter version in eval mode, like the transformed table
 above.  Gradients (fp32) are ``autograd._CharCnnFn``: token chunks, each re-running the kernel in its "materialise" mode.
+
+``LinearFeatureEmbedder`` (linearmapembedding.py:13-29, the node embedder of the PPI model) is ``act(features W^T)`` on one persistent
+kernel, ``ptgnn_b200_feature_embed_forward`` (DESIGN.md §3.15): the activation is applied in its epilogue, and inside a container's layer
+loop it also writes the packed (hi | lo') rows of its fp32 output for the first fused layer.  Its prepared weights are kept per parameter
+version in eval mode.  Gradients (fp32) are ``autograd._FeatureEmbedFn``.  Not supported (``NotImplementedError``): an embedding size
+that is not a multiple of 8 in [8, 256], an input size outside [1, 512], activations other than None, ReLU, Tanh and GELU(erf), and
+gradients with a bf16 output.
 """
 import math
 from typing import NamedTuple, Optional, Tuple
@@ -421,3 +428,120 @@ class CharUnitEmbedder(_NativeEmbedder):
             out = native_char_cnn(chars, shape, prepared, bf16, status=status)
         poll_char_status(status, self.__num_chars_in_vocabulary)
         return self.__dropout(out)
+
+
+# ---------------------------------------------------------------------------------------------------------------------------------
+# LinearFeatureEmbedder
+# ---------------------------------------------------------------------------------------------------------------------------------
+def feature_embed_check(F: int, D: int) -> None:
+    if not N.lib().ptgnn_b200_feature_embed_supported(F, D):
+        raise NotImplementedError(f"the feature-embedding kernel takes an input size in [1, 512] and an embedding size that is a multiple "
+                                  f"of 8 in [8, 256]; got input_element_size={F}, output_embedding_size={D}")
+
+
+def feature_embed_prepare(weight: torch.Tensor, bf16: bool, status: Optional[torch.Tensor]) -> torch.Tensor:
+    """``ptgnn_b200_feature_embed_prepare``: W [D, F] split (fp32) or rounded (bf16), padded and pre-swizzled, as a uint8 tensor."""
+    D, F = weight.shape
+    w = N.require_cuda(weight.detach(), "weight", torch.float32)
+    nbytes = N.lib().ptgnn_b200_feature_embed_workspace_bytes(int(bf16), F, D)
+    prepared = torch.empty(nbytes, dtype=torch.uint8, device=w.device)
+    N.call("ptgnn_b200_feature_embed_prepare", w.device, int(bf16), N.ptr(w), F, D, N.ptr(prepared), nbytes, N.ptr(status))
+    return prepared
+
+
+def native_feature_embed(x: torch.Tensor, prepared: torch.Tensor, D: int, activation: int, bf16: bool = False, want_packed: bool = False,
+                         want_pre: bool = False, status: Optional[torch.Tensor] = None):
+    """``ptgnn_b200_feature_embed_forward``: (out [N, D], packed or None, pre or None) from x [N, F] fp32 and ``feature_embed_prepare``d
+    weights of the same ``bf16`` flag.  out is fp32, or bf16 with ``bf16``.  ``want_packed`` (fp32): also the packed (hi | lo') rows the
+    fused layers take as their packed input; ``want_pre`` (fp32): also the pre-activation [N, D]."""
+    x = N.require_cuda(x, "features", torch.float32)
+    if x.dim() != 2:
+        raise ValueError(f"features must be [N, F], got {tuple(x.shape)}")
+    rows, F = x.shape
+    feature_embed_check(F, D)
+    dev = x.device
+    out = torch.empty(rows, D, dtype=torch.bfloat16 if bf16 else torch.float32, device=dev)
+    packed = pre = None
+    if want_packed and not bf16:
+        packed = torch.empty(max(N.lib().ptgnn_b200_packed_state_bytes(rows, D), 1), dtype=torch.uint8, device=dev)
+    if want_pre and not bf16:
+        pre = torch.empty(rows, D, dtype=torch.float32, device=dev)
+    if rows:
+        N.call("ptgnn_b200_feature_embed_forward", dev, int(bf16), N.ptr(x), rows, F, D, activation, N.ptr(prepared), prepared.numel(),
+               N.ptr(out), N.ptr(packed), N.ptr(pre), N.ptr(status))
+    return out, packed, pre
+
+
+def native_activation_grad(activation: int, grad_out: torch.Tensor, saved: torch.Tensor) -> torch.Tensor:
+    """``ptgnn_b200_activation_grad_f32``: grad_out act'(pre), with ``saved`` the output (ReLU, Tanh) or the pre-activation (GELU)."""
+    grad_out = N.require_cuda(grad_out, "grad_out", torch.float32)
+    saved = N.require_cuda(saved, "saved", torch.float32)
+    d_pre = torch.empty_like(grad_out)
+    N.call("ptgnn_b200_activation_grad_f32", grad_out.device, activation, N.ptr(grad_out), N.ptr(saved), grad_out.numel(), N.ptr(d_pre))
+    return d_pre
+
+
+def poll_feature_status(status: torch.Tensor) -> None:
+    if int(status[0]):
+        status[0] = 0
+        raise FloatingPointError("LinearFeatureEmbedder: an fp32 feature, weight or output is outside the fp16 range (|x| >= 65504) of "
+                                 "the kernel's split products; results are not valid")
+
+
+class LinearFeatureEmbedder(_NativeEmbedder):
+    """``activation(features W^T)`` on one native kernel (DESIGN.md §3.15).  Inside a container's layer loop (``edgeplan.state_chain``)
+    the fp32 forward also writes the packed form of its output, so that a first fused layer skips its packing pass."""
+
+    def __init__(self, input_element_size: int, output_embedding_size: int, activation: Optional[nn.Module] = None):
+        super().__init__()
+        self.__linear_map = nn.Linear(input_element_size, output_embedding_size, bias=False)
+        nn.init.xavier_uniform_(self.__linear_map.weight)
+        self.__activation = activation
+
+    def _prepared(self, weight: torch.Tensor, bf16: bool, status: torch.Tensor) -> torch.Tensor:
+        """The prepared weights.  Kept in eval mode while the weight was not modified in place, re-assigned or moved; derived on every
+        call in training mode (edits through ``.data`` do not move the version counter)."""
+        if self.training:
+            return feature_embed_prepare(weight, bf16, status)
+        key = (bf16, weight.data_ptr(), weight._version, weight.device, weight.dtype)
+        if self._transformed is None or self._transformed[0] != key:
+            self._transformed = (key, feature_embed_prepare(weight, bf16, status))
+        return self._transformed[1]
+
+    def forward(self, features: torch.Tensor) -> torch.Tensor:
+        """
+        :param features: [N, input_element_size] fp32
+        :return: [N, output_embedding_size] (fp32; bf16 under ``torch.autocast("cuda", bfloat16)``)
+        """
+        from .edgeplan import current_state_chain
+        from .messagepassing import _activation_code
+
+        weight = self.__linear_map.weight
+        D, F = weight.shape
+        feature_embed_check(F, D)
+        act = _activation_code(self.__activation, "LinearFeatureEmbedder activation")
+        if features.dim() != 2 or features.shape[1] != F:
+            raise ValueError(f"features must be [N, {F}], got {tuple(features.shape)}")
+        bf16 = _bf16_autocast(weight.device)
+        grad = _wants_grad(weight, features)
+        if bf16 and grad:
+            raise NotImplementedError("LinearFeatureEmbedder: gradients with a bf16 output have no native kernel; train in fp32")
+        N.require_cuda(weight, "weight", torch.float32)
+        if bf16 and features.dtype in (torch.bfloat16, torch.float16):
+            features = features.float()          # exact; the kernel rounds to bf16 as autocast's Linear would
+        x = N.require_cuda(features, "features", torch.float32)
+        status = self._status_word()
+        poll_feature_status(status)
+        prepared = self._prepared(weight, bf16, status)
+        if grad:
+            from . import autograd as _ag
+
+            out = _ag.feature_embed_with_grad(x, weight, prepared, act, status)
+        else:
+            chain = None if bf16 else current_state_chain()
+            out, packed, _ = native_feature_embed(x, prepared, D, act, bf16, want_packed=chain is not None and chain.want_output,
+                                                  status=status)
+            if chain is not None:
+                chain.store(out, packed)
+        poll_feature_status(status)
+        return out

@@ -11,7 +11,7 @@ from typing import Any, Dict, List, NamedTuple, Optional, Tuple
 import torch
 from torch import nn
 
-from .edgeplan import EdgePlan, clear_plan_cache, plan_for, shared_num_graphs, shared_plan, state_chain
+from .edgeplan import EdgePlan, clear_plan_cache, current_state_chain, plan_for, shared_num_graphs, shared_plan, state_chain
 from .messagepassing import AbstractMessagePassingLayer
 
 
@@ -145,9 +145,12 @@ class GraphNeuralNetwork(nn.Module):
             plan = plan_for(adjacency_lists, node_representations.shape[0], plan)
         all_states = [node_representations]
         layers = list(self.__message_passing_layers)
+        outer = current_state_chain()      # forward(): the node embedder may have left the packed form of node_representations there
         # per-thread hand-offs: the layers of this call (and only they) reuse the plan and the graph count, and pass their packed
         # states on
         with shared_plan(plan), shared_num_graphs(num_graphs), state_chain() as chain:
+            if outer is not None:
+                chain.store(node_representations, outer.lookup(node_representations))
             for i, layer in enumerate(layers):
                 chain.want_output = i + 1 < len(layers)
                 node_representations = layer(
@@ -206,6 +209,22 @@ class GraphNeuralNetwork(nn.Module):
         num_graphs,
         **kwargs,
     ) -> GnnOutput:
+        # the node embedder runs in a hand-off of its own: a native LinearFeatureEmbedder also writes the packed form of its fp32 output
+        # there when the first layer takes packed states, and gnn() passes it on to that layer, which then skips its packing pass
+        with state_chain() as chain:
+            chain.want_output = self._first_layer_takes_packed_states()
+            return self._forward(node_data, adjacency_lists, edge_feature_data, node_to_graph_idx, reference_node_ids,
+                                 reference_node_graph_idx, num_graphs, **kwargs)
+
+    def _first_layer_takes_packed_states(self) -> bool:
+        from .globalexchange import GruGlobalStateUpdate
+        from .messagepassing import GatedMessagePassingLayer
+
+        layers = self.__message_passing_layers
+        return len(layers) > 0 and isinstance(layers[0], (GatedMessagePassingLayer, GruGlobalStateUpdate))
+
+    def _forward(self, node_data, adjacency_lists, edge_feature_data, node_to_graph_idx, reference_node_ids, reference_node_graph_idx,
+                 num_graphs, **kwargs) -> GnnOutput:
         initial = self.__node_embedder(**node_data)
         device = node_to_graph_idx.device
         num_nodes = node_to_graph_idx.shape[0]

@@ -41,7 +41,11 @@ factories import the layer classes by module path (`implementations/typilus/trai
 12. with ``native_egc=True`` only: pre-seeds / re-binds ``EGCMessagePassingLayer`` at
    ``ptgnn.neuralmodels.gnn.messagepassing.egcmessagepassing`` (the fused aggregation kernel with the EGC write-out, DESIGN.md §3.14) in
    the same way as step 8, so that a GNN built with EGC layers runs them natively and trains.  The default leaves the reference's class
-   in place.
+   in place,
+13. with ``native_feature_embedder=True`` only: re-binds ``LinearFeatureEmbedder`` inside
+   ``ptgnn.neuralmodels.embeddings.linearmapembedding`` and in reference modules imported earlier (the native feature-embedding kernel,
+   DESIGN.md §3.15), so that ``FeatureRepresentationModel.build_neural_module`` (the PPI model's node embedder) builds the native class.
+   The module stays the reference's: it also holds ``FeatureRepresentationModel``.  The default leaves the reference's class in place.
 
 After ``install()``: ``import ptgnn.implementations.ppi.train`` etc. build ptgnn_b200 layers, unchanged.  ``uninstall()``
 restores the reference's classes.  The reference must be importable as ``ptgnn`` for steps 2-4 (it is not on the GPU test box;
@@ -76,6 +80,8 @@ _NATIVE_EMBEDDERS = ("TokenUnitEmbedder", "SubtokenUnitEmbedder")
 _NATIVE_CHAR_EMBEDDER = "CharUnitEmbedder"
 _EGC_MODULE = "ptgnn.neuralmodels.gnn.messagepassing.egcmessagepassing"
 _EGC_CLASS = "EGCMessagePassingLayer"
+_FEATURE_EMBEDDER_MODULE = "ptgnn.neuralmodels.embeddings.linearmapembedding"
+_FEATURE_EMBEDDER_CLASS = "LinearFeatureEmbedder"
 _saved: Dict[str, object] = {}
 
 
@@ -183,12 +189,21 @@ def _install_native_embedders(names=_NATIVE_EMBEDDERS) -> None:
     _rebind_everywhere(replaced)       # the embedder module included
 
 
+def _install_native_feature_embedder() -> None:
+    from . import embeddings as _emb
+
+    old = getattr(importlib.import_module(_FEATURE_EMBEDDER_MODULE), _FEATURE_EMBEDDER_CLASS)
+    if old is not _emb.LinearFeatureEmbedder:
+        _rebind_everywhere({old: _emb.LinearFeatureEmbedder})      # the embedder module included
+
+
 def install(force_torch_scatter: bool = False, native_reducers: bool = False, native_selfattention: bool = False,
             native_graphnorm: bool = False, native_pna: bool = False, native_decoder: bool = False,
-            native_embedders: bool = False, native_char_embedder: bool = False, native_egc: bool = False) -> Dict[str, object]:
+            native_embedders: bool = False, native_char_embedder: bool = False, native_egc: bool = False,
+            native_feature_embedder: bool = False) -> Dict[str, object]:
     report: Dict[str, object] = {"torch_scatter": "real", "layers": False, "container": False, "metrics": False, "reducers": False,
                                  "selfattention": False, "graphnorm": False, "pna": False, "decoder": False, "embedders": False,
-                                 "char_embedder": False, "egc": False}
+                                 "char_embedder": False, "egc": False, "feature_embedder": False}
     # 1. torch_scatter
     have_real = False
     if not force_torch_scatter:
@@ -261,6 +276,10 @@ def install(force_torch_scatter: bool = False, native_reducers: bool = False, na
     if native_egc:
         _install_native_egc()
         report["egc"] = True
+    # 13. LinearFeatureEmbedder (opt-in)
+    if native_feature_embedder:
+        _install_native_feature_embedder()
+        report["feature_embedder"] = True
     return report
 
 
