@@ -569,6 +569,37 @@ int ptgnn_b200_activation_grad_f32(int32_t activation, const float *grad_out, co
                                    void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * VarMisuse candidate selection (reference implementations/varmisuse/varmisuse.py:58-91, VarMisuseGraphModel.forward):
+ *   score[k] = w[:H] . h[candidate_nodes[k]] + w[H:] . h[slot_nodes[candidate_slot[k]]]      k < num_candidates (K)
+ *   lse[j]   = log sum_{k : candidate_slot[k] = j} exp(score[k])   (-inf for a slot without candidates)   j < num_slots (J)
+ *   argmax[j] = the first such k with the largest score (K for a slot without candidates)
+ *   loss[0]  = -(1/S) sum_{s < S} (score[correct[s]] - lse[candidate_slot[correct[s]]])   S = num_correct (NaN for S = 0)
+ *   h [num_nodes, state_dim] fp32, or bf16 when bf16_states != 0 (w is then rounded to bf16; products accumulate in fp32); w [2 state_dim]
+ *   fp32 (the Linear(2H -> 1).weight).  row_ptr [J + 1] / perm [K]: the plan of (candidate_slot, candidate_slot) with J targets, which
+ *   groups the candidates by slot in their original order.  hits (optional, device int64): when S == J, the number of slots s with
+ *   argmax[s] == correct[s] is ADDED to it (the accuracy metric).  status (device-accessible int32): incremented for every candidate or
+ *   slot node id outside [0, num_nodes) (its row reads as zeros) and every correct id outside [0, K) (its term is skipped).  No workspace.
+ * varmisuse_backward_f32: d_states [num_nodes, state_dim] (every row written) and d_weight [2 state_dim] for d loss = grad_loss[0] (a device
+ *   scalar), from the forward's score and lse.  node_row_ptr [num_nodes + 1] / node_perm [K + J]: the plan of the ids
+ *   cat(candidate_nodes, slot_nodes) with num_nodes targets.  Workspace: ptgnn_b200_varmisuse_workspace_bytes(K, J, state_dim).
+ *   Supported (ptgnn_b200_varmisuse_supported): state_dim a multiple of 4 in [4, 1024]; otherwise PTGNN_E_UNSUPPORTED.  h, w and d_states
+ *   16-byte aligned.  No float atomics, no host synchronisation: results are bit-identical from run to run (DESIGN.md §3.16).
+ * ---------------------------------------------------------------------------------------------- */
+int32_t ptgnn_b200_varmisuse_supported(int32_t state_dim);
+size_t ptgnn_b200_varmisuse_workspace_bytes(int64_t num_candidates, int64_t num_slots, int32_t state_dim);
+int ptgnn_b200_varmisuse_forward(int32_t bf16_states, const void *node_states, int64_t num_nodes, int32_t state_dim,
+                                 const int64_t *candidate_nodes, const int64_t *candidate_slot, const int32_t *row_ptr, const int32_t *perm,
+                                 int64_t num_candidates, const int64_t *slot_nodes, int64_t num_slots, const int64_t *correct,
+                                 int64_t num_correct, const float *weight, float *score, float *lse, int64_t *argmax, float *loss,
+                                 int64_t *hits /* optional */, int32_t *status, void *stream);
+int ptgnn_b200_varmisuse_backward_f32(const float *node_states, int64_t num_nodes, int32_t state_dim, const int64_t *candidate_nodes,
+                                      const int64_t *candidate_slot, const int32_t *row_ptr, const int32_t *perm, int64_t num_candidates,
+                                      const int64_t *slot_nodes, int64_t num_slots, const int64_t *correct, int64_t num_correct,
+                                      const float *weight, const float *score, const float *lse, const float *grad_loss,
+                                      const int32_t *node_row_ptr, const int32_t *node_perm, float *d_states, float *d_weight,
+                                      void *workspace, size_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Host-buffer convenience entry point (used for the end-to-end measurement): all pointers are HOST
  * memory; copies inputs to the device, builds the plan, runs `num_layers` GatedMessagePassingLayers
  * (layer l uses weight set l; pass the same pointers to share weights), copies the final states back

@@ -13,6 +13,7 @@ from .edgeplan import EdgePlan, clear_plan_cache, plan_for
 from .egc import EGCMessagePassingLayer
 from .globalexchange import AbstractGlobalGraphExchange, GruGlobalStateUpdate
 from .gnn import GnnOutput, GraphNeuralNetwork
+from .heads import VarMisuseGraphModel
 from .messagepassing import (
     MLP,
     AbstractMessageAggregation,
@@ -41,5 +42,6 @@ __all__ = [
     "SimpleVarSizedElementReduce", "WeightedSumVarSizedElementReduce", "SelfAttentionVarSizedElementReduce",
     "MultiheadSelfAttentionVarSizedElementReduce", "MultiHeadSelfAttentionMessagePassing", "GraphNorm", "GruCopyingDecoder",
     "TokenUnitEmbedder", "SubtokenUnitEmbedder", "CharUnitEmbedder", "LinearFeatureEmbedder",
+    "VarMisuseGraphModel",
     "scatter_sum", "scatter_mean", "scatter_max", "scatter_min",
 ]

@@ -877,3 +877,34 @@ class _GatherByGraphFn(torch.autograd.Function):
 
 def gather_by_graph(plan, index, x):
     return _GatherByGraphFn.apply(plan, index, x)
+
+
+# =====================================================================================================================
+# VarMisuse candidate selection (varmisuse.py:76-91): the per-slot log-softmax of the candidate scores and the mean NLL of the correct
+# candidates, on the native kernels.  fp32 states.
+# =====================================================================================================================
+class _VarMisuseFn(torch.autograd.Function):
+    """loss [] from h [N, H] and the score weight [1, 2H]; backward: d h and d w on the native backward kernels (the softmax re-computed
+    from the saved [K] scores and [J] logsumexps).  ``ops``: ``heads.varmisuse_inputs``."""
+
+    @staticmethod
+    def forward(ctx, ops, hits, h, weight):
+        from .heads import native_varmisuse
+
+        loss, score, lse, _ = native_varmisuse(*ops, hits=hits)
+        ctx.ops = ops
+        ctx.save_for_backward(score, lse)
+        return loss
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        from .heads import native_varmisuse_backward
+
+        score, lse = ctx.saved_tensors
+        d_h, d_w = native_varmisuse_backward(*ctx.ops, score, lse, g.contiguous().float())
+        return None, None, d_h, d_w.view(1, -1)
+
+
+def varmisuse_with_grad(ops, hits, node_states, weight):
+    return _VarMisuseFn.apply(ops, hits, node_states, weight)

@@ -29,7 +29,7 @@ class EdgePlan:
 
     # status words (pinned host memory the kernels write directly, so the host can poll them without synchronising):
     # [0] number of out-of-range edge indices, [1] a node state / [2] an edge weight outside the fp16 range of the fp32-exact
-    # fused path (csrc/fused_mp.cuh)
+    # fused path (csrc/fused_mp.cuh), [3] number of out-of-range indices a task head met (heads.py: candidate, slot node or correct ids)
     STATUS_WORDS = 4
 
     def __init__(self, adjacency_lists: Adjacency, num_nodes: int, validate: bool = False,
@@ -125,6 +125,11 @@ class EdgePlan:
             raise FloatingPointError(
                 f"{what} outside the fp16 range (|x| >= 65504, inf or NaN) reached the fp32-exact fused kernel (3xFP16 split); "
                 "set PTGNN_B200_FP32_MODE=tf32 to use the unfused 3xTF32 kernels for such inputs")
+        bad = int(st[3])
+        if bad:
+            st[3] = 0          # the head's other inputs change from call to call, while this plan may be reused
+            raise ValueError(f"{bad} task-head indices out of range (a candidate or slot node id outside [0, N), or a correct candidate "
+                             "outside [0, K)); the kernels skipped them, results are not valid")
 
     # ---- block plan of the fused kernel (built on first use, shared by all layers of the minibatch) ---------------------
     def block_plan(self) -> "N.BlockPlanStruct":

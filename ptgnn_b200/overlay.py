@@ -45,7 +45,13 @@ factories import the layer classes by module path (`implementations/typilus/trai
 13. with ``native_feature_embedder=True`` only: re-binds ``LinearFeatureEmbedder`` inside
    ``ptgnn.neuralmodels.embeddings.linearmapembedding`` and in reference modules imported earlier (the native feature-embedding kernel,
    DESIGN.md §3.15), so that ``FeatureRepresentationModel.build_neural_module`` (the PPI model's node embedder) builds the native class.
-   The module stays the reference's: it also holds ``FeatureRepresentationModel``.  The default leaves the reference's class in place.
+   The module stays the reference's: it also holds ``FeatureRepresentationModel``.  The default leaves the reference's class in place,
+14. with ``native_heads=True`` only: re-binds ``VarMisuseGraphModel`` inside ``ptgnn.implementations.varmisuse.varmisuse`` and in reference
+   modules imported earlier (the native candidate-selection kernels, DESIGN.md §3.16), so that ``VarMisuseModel.build_neural_module``
+   builds the native class, and registers it with the reference's ``ModuleWithMetrics``.  The module stays the reference's: it also holds
+   ``VarMisuseModel``.  That module is imported first, before any other step: if it cannot be imported (on Python 3.12 its annotation
+   ``GraphData[Tuple[str, bool]]`` raises ``TypeError``), ``install()`` raises ``ImportError`` and changes nothing.  The default leaves
+   the reference's class in place; on the torch_scatter shim that class gets no gradient through its log-softmax normaliser (DESIGN.md §6).
 
 After ``install()``: ``import ptgnn.implementations.ppi.train`` etc. build ptgnn_b200 layers, unchanged.  ``uninstall()``
 restores the reference's classes.  The reference must be importable as ``ptgnn`` for steps 2-4 (it is not on the GPU test box;
@@ -82,6 +88,8 @@ _EGC_MODULE = "ptgnn.neuralmodels.gnn.messagepassing.egcmessagepassing"
 _EGC_CLASS = "EGCMessagePassingLayer"
 _FEATURE_EMBEDDER_MODULE = "ptgnn.neuralmodels.embeddings.linearmapembedding"
 _FEATURE_EMBEDDER_CLASS = "LinearFeatureEmbedder"
+_HEAD_MODULE = "ptgnn.implementations.varmisuse.varmisuse"
+_HEAD_CLASS = "VarMisuseGraphModel"
 _saved: Dict[str, object] = {}
 
 
@@ -197,13 +205,24 @@ def _install_native_feature_embedder() -> None:
         _rebind_everywhere({old: _emb.LinearFeatureEmbedder})      # the embedder module included
 
 
+def _install_native_heads() -> None:
+    from . import heads as _heads
+
+    old = getattr(importlib.import_module(_HEAD_MODULE), _HEAD_CLASS)
+    if old is not _heads.VarMisuseGraphModel:
+        _rebind_everywhere({old: _heads.VarMisuseGraphModel})      # the head module included
+    _heads.register_with_reference_metrics()
+
+
 def install(force_torch_scatter: bool = False, native_reducers: bool = False, native_selfattention: bool = False,
             native_graphnorm: bool = False, native_pna: bool = False, native_decoder: bool = False,
             native_embedders: bool = False, native_char_embedder: bool = False, native_egc: bool = False,
-            native_feature_embedder: bool = False) -> Dict[str, object]:
+            native_feature_embedder: bool = False, native_heads: bool = False) -> Dict[str, object]:
     report: Dict[str, object] = {"torch_scatter": "real", "layers": False, "container": False, "metrics": False, "reducers": False,
                                  "selfattention": False, "graphnorm": False, "pna": False, "decoder": False, "embedders": False,
-                                 "char_embedder": False, "egc": False, "feature_embedder": False}
+                                 "char_embedder": False, "egc": False, "feature_embedder": False,
+                                 "heads": False}
+    previous_scatter = {name: sys.modules.get(name) for name in ("torch_scatter", "torch_scatter.composite")}
     # 1. torch_scatter
     have_real = False
     if not force_torch_scatter:
@@ -221,6 +240,22 @@ def install(force_torch_scatter: bool = False, native_reducers: bool = False, na
     if not _reference_importable():
         report["note"] = "reference package `ptgnn` not importable: only the torch_scatter shim was installed"
         return report
+    if native_heads:
+        # the head module is imported (it needs the torch_scatter of step 1) before anything else changes: if it cannot be imported,
+        # install() undoes step 1, forgets the reference modules the attempt imported, and raises, leaving no step half-applied
+        loaded = set(sys.modules)
+        try:
+            importlib.import_module(_HEAD_MODULE)
+        except Exception as e:
+            for name in set(sys.modules) - loaded:
+                del sys.modules[name]
+            for name, mod in previous_scatter.items():
+                if mod is None:
+                    sys.modules.pop(name, None)
+                else:
+                    sys.modules[name] = mod
+            raise ImportError(f"native_heads=True: the reference module {_HEAD_MODULE} cannot be imported ({type(e).__name__}: {e}); "
+                              "nothing was installed") from e
     # 2. layer modules: replace already-imported reference classes, pre-seed the ones not imported yet
     replaced = {}
     for mod_name, names in _LAYER_MODULES.items():
@@ -280,6 +315,10 @@ def install(force_torch_scatter: bool = False, native_reducers: bool = False, na
     if native_feature_embedder:
         _install_native_feature_embedder()
         report["feature_embedder"] = True
+    # 14. VarMisuseGraphModel (opt-in)
+    if native_heads:
+        _install_native_heads()
+        report["heads"] = True
     return report
 
 
