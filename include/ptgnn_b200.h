@@ -600,6 +600,54 @@ int ptgnn_b200_varmisuse_backward_f32(const float *node_states, int64_t num_node
                                       void *workspace, size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Classification heads (reference implementations/typilus/graph2class.py:63-102, Graph2ClassModule; implementations/ppi/ppi.py:13-62,
+ * PPIClassification):
+ *   logits[r, c] = x[row(r)] . W[c] + bias[c]      r < rows, c < num_classes (C); row(r) = row_idx[r], or r when row_idx is null
+ * classify_prepare: W [C, state_dim] into the feature embedder's prepared format (ptgnn_b200_feature_embed_prepare's kernel; C padded
+ * to 16), a 16-byte aligned buffer of ptgnn_b200_classify_prepared_bytes(bf16, state_dim, C) bytes; status[1] is set for a weight outside
+ * the fp16 range.  bf16: one bf16 product of bf16-rounded operands, the logits and the
+ * bias rounded to bf16 as autocast's Linear (bf16_states: node_states are bf16, else fp32); otherwise the 3xFP16 split (DESIGN.md §3.1).
+ * classify_forward, by mode:
+ *   PTGNN_CLASSIFY_LOGITS  lse [rows], argmax [rows] (the first largest logit), max_prob [rows] (the softmax's largest probability) and
+ *                          logits [rows, C], each optional.  No loss.
+ *   PTGNN_CLASSIFY_CE      targets: int64 [rows] class ids, -100 ignored.  loss[0] = mean over the other rows of lse - logit[target]
+ *                          (NaN without one), lse and argmax as above, valid_count[0] = the rows counted (for the backward); hits
+ *                          (optional, device int64): the number of rows with argmax == target is ADDED to it.
+ *   PTGNN_CLASSIFY_BCE     targets: bool (one byte) [rows, C].  loss[0] = (1 / rows) sum of the stable BCE-with-logits terms; metrics
+ *                          (optional, device fp64 [3]): fscore, precision and recall of the predictions sigmoid(logit) >= 0.5 (computed
+ *                          as torch does, rounded to bf16 with bf16) from the integer TP, FP, FN, with ppi.py:50-52's fp32 formulas,
+ *                          each times rows, ADDED to metrics[0..2].
+ *   safe_idx (optional, int32 [rows], with row_idx): row_idx[r] where it lies in [0, num_nodes), else 0 -- the ids a backward gathers and
+ *   scatters through without a bounds check.  num_nodes must then be at most INT32_MAX.
+ *   status (device-accessible int32 [2]): [0] is incremented for every row_idx outside [0, num_nodes) (the row reads as zeros) and every CE
+ *   target outside [0, C) other than -100 (its term is skipped); [1] is set when an fp32 value is outside the fp16 range.
+ *   Workspace: ptgnn_b200_classify_workspace_bytes(bf16, rows, state_dim, C).
+ * classify_backward_f32: d_logits [rows, C] for d loss = grad_loss[0] (a device scalar): (g / valid_count) (softmax - onehot(target)) on
+ *   counted rows and 0 elsewhere (CE, from the forward's lse and valid_count), (g / rows) (sigmoid - target) (BCE); 0 on every row
+ *   whose row_idx lies outside [0, num_nodes).  The logits are
+ *   recomputed from the fp32 prepared weights; d W, d bias and d states are products of d_logits the caller forms.
+ * Supported (ptgnn_b200_classify_supported): state_dim a multiple of 8 in [8, 256], C in [1, 256]; otherwise PTGNN_E_UNSUPPORTED.
+ * rows at most INT32_MAX; node_states and prepared 16-byte aligned.  No float atomics, no host synchronisation: results are bit-identical from run to run
+ * (DESIGN.md §3.17).
+ * ---------------------------------------------------------------------------------------------- */
+enum { PTGNN_CLASSIFY_LOGITS = 0, PTGNN_CLASSIFY_CE = 1, PTGNN_CLASSIFY_BCE = 2 };
+int32_t ptgnn_b200_classify_supported(int32_t state_dim, int32_t num_classes);
+size_t ptgnn_b200_classify_prepared_bytes(int32_t bf16, int32_t state_dim, int32_t num_classes);
+int ptgnn_b200_classify_prepare(int32_t bf16, const float *weight, int32_t state_dim, int32_t num_classes, void *prepared,
+                                size_t prepared_bytes, int32_t *status, void *stream);
+size_t ptgnn_b200_classify_workspace_bytes(int32_t bf16, int64_t rows, int32_t state_dim, int32_t num_classes);
+int ptgnn_b200_classify_forward(int32_t mode, int32_t bf16, int32_t bf16_states, const void *node_states, int64_t num_nodes,
+                                int32_t state_dim, const int64_t *row_idx /* optional */, int64_t rows, int32_t num_classes,
+                                const void *prepared, size_t prepared_bytes, const float *bias, const void *targets, float *logits,
+                                float *loss, float *lse, int64_t *argmax, float *max_prob, int32_t *valid_count, int64_t *hits,
+                                double *metrics, int32_t *safe_idx, void *workspace, size_t workspace_bytes, int32_t *status,
+                                void *stream);
+int ptgnn_b200_classify_backward_f32(int32_t mode, const float *node_states, int64_t num_nodes, int32_t state_dim,
+                                     const int64_t *row_idx /* optional */, int64_t rows, int32_t num_classes, const void *prepared,
+                                     size_t prepared_bytes, const float *bias, const void *targets, const float *lse,
+                                     const int32_t *valid_count, const float *grad_loss, float *d_logits, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Host-buffer convenience entry point (used for the end-to-end measurement): all pointers are HOST
  * memory; copies inputs to the device, builds the plan, runs `num_layers` GatedMessagePassingLayers
  * (layer l uses weight set l; pass the same pointers to share weights), copies the final states back

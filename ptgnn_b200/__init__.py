@@ -13,7 +13,7 @@ from .edgeplan import EdgePlan, clear_plan_cache, plan_for
 from .egc import EGCMessagePassingLayer
 from .globalexchange import AbstractGlobalGraphExchange, GruGlobalStateUpdate
 from .gnn import GnnOutput, GraphNeuralNetwork
-from .heads import VarMisuseGraphModel
+from .heads import Graph2ClassModule, PPIClassification, VarMisuseGraphModel
 from .messagepassing import (
     MLP,
     AbstractMessageAggregation,
@@ -42,6 +42,6 @@ __all__ = [
     "SimpleVarSizedElementReduce", "WeightedSumVarSizedElementReduce", "SelfAttentionVarSizedElementReduce",
     "MultiheadSelfAttentionVarSizedElementReduce", "MultiHeadSelfAttentionMessagePassing", "GraphNorm", "GruCopyingDecoder",
     "TokenUnitEmbedder", "SubtokenUnitEmbedder", "CharUnitEmbedder", "LinearFeatureEmbedder",
-    "VarMisuseGraphModel",
+    "VarMisuseGraphModel", "Graph2ClassModule", "PPIClassification",
     "scatter_sum", "scatter_mean", "scatter_max", "scatter_min",
 ]

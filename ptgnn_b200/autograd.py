@@ -908,3 +908,60 @@ class _VarMisuseFn(torch.autograd.Function):
 
 def varmisuse_with_grad(ops, hits, node_states, weight):
     return _VarMisuseFn.apply(ops, hits, node_states, weight)
+
+
+# =====================================================================================================================
+# Classification heads (graph2class.py:63-102, ppi.py:13-62): the Linear and its cross-entropy or BCE loss on the native kernel.  fp32.
+# =====================================================================================================================
+class _ClassifyFn(torch.autograd.Function):
+    """loss [] from h [N, H], W [C, H] and b [C]; backward: d logits from one launch that recomputes the logits (from the saved [R] lse
+    and valid-row count for CE), then ``heads.classify_input_grads``.  ``ops``: ``heads.ClassifyOps``."""
+
+    @staticmethod
+    def forward(ctx, ops, hits, metrics, h, weight, bias):
+        from .heads import native_classify
+
+        loss, lse, _, valid, _, _, safe_idx = native_classify(ops, weight.shape[0], hits=hits, metrics=metrics)
+        ctx.ops, ctx.safe_idx = ops, safe_idx
+        ctx.save_for_backward(weight, lse, valid)
+        return loss
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        from .heads import classify_input_grads, native_classify_backward
+
+        weight, lse, valid = ctx.saved_tensors
+        d_logits = native_classify_backward(ctx.ops, weight.shape[0], lse, valid, g.contiguous().float())
+        d_h, d_w, d_b = classify_input_grads(ctx.ops, ctx.safe_idx, weight, d_logits, *ctx.needs_input_grad[3:6])
+        return None, None, None, d_h, d_w, d_b
+
+
+def classify_with_grad(ops, hits, metrics, node_states, weight, bias):
+    return _ClassifyFn.apply(ops, hits, metrics, node_states, weight, bias)
+
+
+class _ClassifyLogitsFn(torch.autograd.Function):
+    """logits [R, C] (Graph2ClassModule._logits) with the head's backward for an upstream d logits."""
+
+    @staticmethod
+    def forward(ctx, ops, h, weight, bias):
+        from .heads import native_classify
+
+        _, _, _, _, _, logits, safe_idx = native_classify(ops, weight.shape[0], want_logits=True)
+        ctx.ops, ctx.safe_idx = ops, safe_idx
+        ctx.save_for_backward(weight)
+        return logits
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        from .heads import classify_input_grads
+
+        (weight,) = ctx.saved_tensors
+        d_h, d_w, d_b = classify_input_grads(ctx.ops, ctx.safe_idx, weight, g.contiguous().float(), *ctx.needs_input_grad[1:4])
+        return None, d_h, d_w, d_b
+
+
+def classify_logits_with_grad(ops, node_states, weight, bias):
+    return _ClassifyLogitsFn.apply(ops, node_states, weight, bias)

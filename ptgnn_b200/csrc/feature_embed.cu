@@ -18,50 +18,10 @@
 #include <cuda_fp16.h>
 #include <math.h>
 
-#include "common.cuh"
-#include "tc_common.cuh"
+#include "feature_embed.cuh"
 
 namespace ptgnn {
 namespace featemb {
-
-constexpr int BM = 128;                 // rows per tile (two warpgroups)
-constexpr int THREADS = 256;
-constexpr int KC = 64;                  // X columns per ring stage (one 128-byte swizzled K block of W)
-constexpr int PITCH = KC + 8;           // floats per staged row: rows 32 bytes apart in bank space, the fragment loads are conflict-free
-constexpr int STAGE = BM * PITCH * 4;   // bytes per ring stage
-constexpr int MAX_F = 512;
-constexpr int MAX_D = 256;
-constexpr int MAX_DC = 128;             // columns per CTA: two m64n64 accumulator halves
-constexpr size_t W_BUDGET = 128 * 1024;
-constexpr size_t SMEM_MAX = 227 * 1024;
-
-static bool supported(int F, int D) { return F >= 1 && F <= MAX_F && D >= 8 && D <= MAX_D && D % 8 == 0; }
-
-// Column blocking and prepared-weight sizes of one (F, D, dtype)
-struct Geometry {
-    int KP, KB, DP, Dc, nblk, copies;
-    size_t block_bytes;                  // one column block's prepared weights = its shared-memory copy
-};
-static Geometry geometry(int F, int D, bool bf16) {
-    Geometry g;
-    g.KP = (F + 15) / 16 * 16;
-    g.KB = (g.KP + KC - 1) / KC;
-    g.DP = (D + 15) / 16 * 16;
-    g.copies = bf16 ? 1 : 2;
-    g.Dc = g.DP < MAX_DC ? g.DP : MAX_DC;
-    while ((size_t)g.copies * g.KB * g.Dc * 128 > W_BUDGET) g.Dc -= 16;   // F = 512 fp32: 64 columns per CTA
-    g.nblk = (g.DP + g.Dc - 1) / g.Dc;
-    g.block_bytes = (size_t)g.copies * g.KB * g.Dc * 128;
-    return g;
-}
-static int stages(const Geometry &g) {
-    const size_t s = (SMEM_MAX - 1024 - g.block_bytes) / STAGE;
-    return s >= 4 ? 4 : (int)s;          // >= 2: the weight slice is at most W_BUDGET
-}
-
-__device__ __forceinline__ uint32_t sw128(int row, int k) {
-    return (uint32_t)(row * 128 + ((((k >> 3) ^ (row & 7)) << 4) | ((k & 7) << 1)));
-}
 
 // ---- preparation: W [D, F] -> per column block, per copy, per 64-wide K block: Dc rows x 128 bytes, SWIZZLE_128B K-major ----------
 template <bool BF16>
@@ -101,38 +61,6 @@ struct Args {
     float *pre;                          // optional: [N, D] fp32 pre-activation
     int32_t *status;
 };
-
-__device__ __forceinline__ void cp_async_ca(uint32_t dst, const void *src, int bytes, int src_bytes) {
-    if (bytes == 16) asm volatile("cp.async.ca.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst), "l"(src), "r"(src_bytes));
-    else if (bytes == 8) asm volatile("cp.async.ca.shared.global [%0], [%1], 8, %2;\n" ::"r"(dst), "l"(src), "r"(src_bytes));
-    else asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;\n" ::"r"(dst), "l"(src), "r"(src_bytes));
-}
-
-template <bool BF16>
-__device__ __forceinline__ void mma_cols(float (&d)[32], const uint32_t (&a)[4], uint64_t desc, int width) {
-    switch (width) {
-        case 64: tc::wgmma_16_rs_n64<BF16>(d, a, desc); break;
-        case 48: tc::wgmma_16_rs_n48<BF16>(d, a, desc); break;
-        case 32: tc::wgmma_16_rs_n32<BF16>(d, a, desc); break;
-        default: tc::wgmma_16_rs_n16<BF16>(d, a, desc); break;
-    }
-}
-
-// two fp32 -> the 16-bit operand pair(s) of one A register: hi (fp16 or bf16) and, fp32, lo' = rn16((x - hi) 2^11)
-template <bool BF16>
-__device__ __forceinline__ void split2(float2 v, uint32_t &hi, uint32_t &lo, bool &bad) {
-    if (BF16) {
-        __nv_bfloat162 b = __floats2bfloat162_rn(v.x, v.y);
-        hi = *reinterpret_cast<uint32_t *>(&b);
-    } else {
-        const __half h0 = __float2half_rn(v.x), h1 = __float2half_rn(v.y);
-        const __half l0 = __float2half_rn((v.x - __half2float(h0)) * 2048.0f), l1 = __float2half_rn((v.y - __half2float(h1)) * 2048.0f);
-        __half2 hh = __halves2half2(h0, h1), ll = __halves2half2(l0, l1);
-        hi = *reinterpret_cast<uint32_t *>(&hh);
-        lo = *reinterpret_cast<uint32_t *>(&ll);
-        bad |= !(fabsf(v.x) < 65504.0f) | !(fabsf(v.y) < 65504.0f);
-    }
-}
 
 template <bool BF16, int S>
 __global__ void __launch_bounds__(THREADS, 1) feature_embed_kernel(const Args a) {
@@ -337,6 +265,15 @@ static int feature_embed_check(const char *what, int32_t in_dim, int32_t out_dim
     return PTGNN_OK;
 }
 
+// the one preparation of W [D, F] for the feature embedder and the classification heads (classify.cu: W [C, H], any C in [1, MAX_D])
+int featemb::launch_prepare(bool bf16, const float *weight, int F, int D, const Geometry &g, uint8_t *prepared, int32_t *status,
+                            cudaStream_t st) {
+    const long long n = (long long)g.nblk * g.KB * g.Dc * 64;
+    const int grid = (int)(ceil_div(n, 256) < 4 * sm_count() ? ceil_div(n, 256) : 4 * sm_count());
+    return launch(PTGNN_KERNEL_PACK, st, bf16 ? featemb::prepare_kernel<true> : featemb::prepare_kernel<false>, grid, 256, 0, weight, F, D,
+                  g.Dc, g.KB, g.nblk, prepared, status);
+}
+
 extern "C" int ptgnn_b200_feature_embed_prepare(int32_t bf16, const float *weight, int32_t in_dim, int32_t out_dim, void *prepared,
                                                 size_t prepared_bytes, int32_t *status, void *stream) {
     PTGNN_TRY(feature_embed_check("feature_embed_prepare", in_dim, out_dim));
@@ -344,11 +281,8 @@ extern "C" int ptgnn_b200_feature_embed_prepare(int32_t bf16, const float *weigh
     const featemb::Geometry g = featemb::geometry(in_dim, out_dim, bf16 != 0);
     PTGNN_CHECK_WORKSPACE("feature_embed_prepare", prepared, prepared_bytes, (size_t)g.nblk * g.block_bytes);
     PTGNN_CHECK_ARG(reinterpret_cast<uintptr_t>(prepared) % 16 == 0, "feature_embed_prepare: the prepared buffer must be 16-byte aligned");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const long long n = (long long)g.nblk * g.KB * g.Dc * 64;
-    const int grid = (int)(ceil_div(n, 256) < 4 * sm_count() ? ceil_div(n, 256) : 4 * sm_count());
-    return launch(PTGNN_KERNEL_PACK, st, bf16 ? featemb::prepare_kernel<true> : featemb::prepare_kernel<false>, grid, 256, 0, weight, in_dim,
-                  out_dim, g.Dc, g.KB, g.nblk, static_cast<uint8_t *>(prepared), status);
+    return featemb::launch_prepare(bf16 != 0, weight, in_dim, out_dim, g, static_cast<uint8_t *>(prepared), status,
+                                   static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int ptgnn_b200_feature_embed_forward(int32_t bf16_out, const float *x, int64_t rows, int32_t in_dim, int32_t out_dim,

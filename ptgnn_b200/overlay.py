@@ -51,7 +51,13 @@ factories import the layer classes by module path (`implementations/typilus/trai
    builds the native class, and registers it with the reference's ``ModuleWithMetrics``.  The module stays the reference's: it also holds
    ``VarMisuseModel``.  That module is imported first, before any other step: if it cannot be imported (on Python 3.12 its annotation
    ``GraphData[Tuple[str, bool]]`` raises ``TypeError``), ``install()`` raises ``ImportError`` and changes nothing.  The default leaves
-   the reference's class in place; on the torch_scatter shim that class gets no gradient through its log-softmax normaliser (DESIGN.md §6).
+   the reference's class in place; on the torch_scatter shim that class gets no gradient through its log-softmax normaliser (DESIGN.md §6),
+15. with ``native_graph2class_head=True`` only: re-binds ``Graph2ClassModule`` inside ``ptgnn.implementations.typilus.graph2class`` and
+   in reference modules imported earlier (the native classification kernel, DESIGN.md §3.17), so that ``Graph2Class.build_neural_module``
+   builds the native class.  The module is imported first, with the same refusal as step 14,
+16. with ``native_ppi_head=True`` only: the same for ``PPIClassification`` inside ``ptgnn.implementations.ppi.ppi``.  On Python 3.12 that
+   module cannot be imported (``TensorizedGraphData[np.ndarray]`` raises ``TypeError`` at class creation): ``install()`` raises
+   ``ImportError`` and changes nothing.
 
 After ``install()``: ``import ptgnn.implementations.ppi.train`` etc. build ptgnn_b200 layers, unchanged.  ``uninstall()``
 restores the reference's classes.  The reference must be importable as ``ptgnn`` for steps 2-4 (it is not on the GPU test box;
@@ -90,6 +96,10 @@ _FEATURE_EMBEDDER_MODULE = "ptgnn.neuralmodels.embeddings.linearmapembedding"
 _FEATURE_EMBEDDER_CLASS = "LinearFeatureEmbedder"
 _HEAD_MODULE = "ptgnn.implementations.varmisuse.varmisuse"
 _HEAD_CLASS = "VarMisuseGraphModel"
+_GRAPH2CLASS_MODULE = "ptgnn.implementations.typilus.graph2class"
+_GRAPH2CLASS_CLASS = "Graph2ClassModule"
+_PPI_MODULE = "ptgnn.implementations.ppi.ppi"
+_PPI_CLASS = "PPIClassification"
 _saved: Dict[str, object] = {}
 
 
@@ -205,23 +215,43 @@ def _install_native_feature_embedder() -> None:
         _rebind_everywhere({old: _emb.LinearFeatureEmbedder})      # the embedder module included
 
 
-def _install_native_heads() -> None:
+def _install_native_head(module: str, name: str) -> None:
     from . import heads as _heads
 
-    old = getattr(importlib.import_module(_HEAD_MODULE), _HEAD_CLASS)
-    if old is not _heads.VarMisuseGraphModel:
-        _rebind_everywhere({old: _heads.VarMisuseGraphModel})      # the head module included
+    old, new = getattr(importlib.import_module(module), name), getattr(_heads, name)
+    if old is not new:
+        _rebind_everywhere({old: new})      # the head module included
     _heads.register_with_reference_metrics()
+
+
+def _import_head_modules(wanted: Dict[str, str], previous_scatter: Dict[str, object]) -> None:
+    """Imports the reference module of every head flag in ``wanted`` ({flag: module}) before anything else changes.  If one cannot be
+    imported, undoes step 1, forgets the reference modules the attempt imported, and raises ImportError, leaving no step half-applied."""
+    loaded = set(sys.modules)
+    for flag, module in wanted.items():
+        try:
+            importlib.import_module(module)
+        except Exception as e:
+            for name in set(sys.modules) - loaded:
+                del sys.modules[name]
+            for name, mod in previous_scatter.items():
+                if mod is None:
+                    sys.modules.pop(name, None)
+                else:
+                    sys.modules[name] = mod
+            raise ImportError(f"{flag}=True: the reference module {module} cannot be imported ({type(e).__name__}: {e}); "
+                              "nothing was installed") from e
 
 
 def install(force_torch_scatter: bool = False, native_reducers: bool = False, native_selfattention: bool = False,
             native_graphnorm: bool = False, native_pna: bool = False, native_decoder: bool = False,
             native_embedders: bool = False, native_char_embedder: bool = False, native_egc: bool = False,
-            native_feature_embedder: bool = False, native_heads: bool = False) -> Dict[str, object]:
+            native_feature_embedder: bool = False, native_heads: bool = False, native_graph2class_head: bool = False,
+            native_ppi_head: bool = False) -> Dict[str, object]:
     report: Dict[str, object] = {"torch_scatter": "real", "layers": False, "container": False, "metrics": False, "reducers": False,
                                  "selfattention": False, "graphnorm": False, "pna": False, "decoder": False, "embedders": False,
                                  "char_embedder": False, "egc": False, "feature_embedder": False,
-                                 "heads": False}
+                                 "heads": False, "graph2class_head": False, "ppi_head": False}
     previous_scatter = {name: sys.modules.get(name) for name in ("torch_scatter", "torch_scatter.composite")}
     # 1. torch_scatter
     have_real = False
@@ -240,22 +270,10 @@ def install(force_torch_scatter: bool = False, native_reducers: bool = False, na
     if not _reference_importable():
         report["note"] = "reference package `ptgnn` not importable: only the torch_scatter shim was installed"
         return report
-    if native_heads:
-        # the head module is imported (it needs the torch_scatter of step 1) before anything else changes: if it cannot be imported,
-        # install() undoes step 1, forgets the reference modules the attempt imported, and raises, leaving no step half-applied
-        loaded = set(sys.modules)
-        try:
-            importlib.import_module(_HEAD_MODULE)
-        except Exception as e:
-            for name in set(sys.modules) - loaded:
-                del sys.modules[name]
-            for name, mod in previous_scatter.items():
-                if mod is None:
-                    sys.modules.pop(name, None)
-                else:
-                    sys.modules[name] = mod
-            raise ImportError(f"native_heads=True: the reference module {_HEAD_MODULE} cannot be imported ({type(e).__name__}: {e}); "
-                              "nothing was installed") from e
+    # the head modules are imported (they need the torch_scatter of step 1) before anything else changes
+    heads = {"native_heads": _HEAD_MODULE, "native_graph2class_head": _GRAPH2CLASS_MODULE, "native_ppi_head": _PPI_MODULE}
+    flags = {"native_heads": native_heads, "native_graph2class_head": native_graph2class_head, "native_ppi_head": native_ppi_head}
+    _import_head_modules({flag: module for flag, module in heads.items() if flags[flag]}, previous_scatter)
     # 2. layer modules: replace already-imported reference classes, pre-seed the ones not imported yet
     replaced = {}
     for mod_name, names in _LAYER_MODULES.items():
@@ -317,8 +335,15 @@ def install(force_torch_scatter: bool = False, native_reducers: bool = False, na
         report["feature_embedder"] = True
     # 14. VarMisuseGraphModel (opt-in)
     if native_heads:
-        _install_native_heads()
+        _install_native_head(_HEAD_MODULE, _HEAD_CLASS)
         report["heads"] = True
+    # 15, 16. Graph2ClassModule, PPIClassification (opt-in)
+    if native_graph2class_head:
+        _install_native_head(_GRAPH2CLASS_MODULE, _GRAPH2CLASS_CLASS)
+        report["graph2class_head"] = True
+    if native_ppi_head:
+        _install_native_head(_PPI_MODULE, _PPI_CLASS)
+        report["ppi_head"] = True
     return report
 
 
