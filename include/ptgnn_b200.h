@@ -648,6 +648,32 @@ int ptgnn_b200_classify_backward_f32(int32_t mode, const float *node_states, int
                                      const int32_t *valid_count, const float *grad_loss, float *d_logits, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Token selection of graph2seq's greedy decoding (reference neuralmodels/sequence/grucopydecoder.py:406-455), one decoder step, one
+ * CTA per graph g:
+ *   Z = logsumexp(logits[g, :V] ∪ {lse_copy[g]}),  lp_v = logits[g, v] - Z,  c_i = copy_scores[i] - Z   (fp32)
+ *   T = the K = min(100, V) largest lp, the lower id first among equal values.
+ *   Groups: the copy rows of g sharing a key (a vocabulary id < V, or V + j for the minibatch's j-th out-of-vocabulary string), in
+ *   first-occurrence order: group_ptr [G + 1] indexes group_key / member_ptr [groups (+ 1)]; member_rows [M] are the rows of each
+ *   group in row order.  A group scores lp_key ⊕ c_i1 ⊕ ... when its key is in T, else c_i1 ⊕ ... (⊕: numpy's float32 logaddexp, in
+ *   row order); a member of T without a group scores lp.  The winner is the highest score, a tie going to T (larger lp, then lower id)
+ *   before the groups outside T (first occurrence first).
+ *   State [G] (in/out): done int32, length int32, logprob fp32, tokens [G, max_len] int32 keys, next_ids int64.  A done graph feeds
+ *   end_id and is otherwise unchanged; else logprob += the winner's score, end_id marks it done, any other key is appended to tokens,
+ *   and next_ids = the key when it is below V, else unk_id.  At step 0 done, length and logprob are read as 0 (no initialisation
+ *   needed).  step must lie in [0, max_len).
+ *   Workspace: ptgnn_b200_decode_select_workspace_bytes(G, V) bytes; after the call it holds (Z, winning score) fp32 per graph
+ *   ([G][2]; NaN for a graph that was already done).  No host synchronisation, no float atomics: deterministic (DESIGN.md §3.18).
+ *   Supported (ptgnn_b200_decode_select_supported): V in [1, 65536]; otherwise PTGNN_E_UNSUPPORTED.
+ * ---------------------------------------------------------------------------------------------- */
+int32_t ptgnn_b200_decode_select_supported(int32_t vocab);
+size_t ptgnn_b200_decode_select_workspace_bytes(int64_t num_graphs, int32_t vocab);
+int ptgnn_b200_decode_select(const float *logits, int64_t num_graphs, int32_t vocab, const float *copy_scores, int64_t num_rows,
+                             const float *lse_copy, const int32_t *group_ptr, const int32_t *group_key, const int32_t *member_ptr,
+                             const int32_t *member_rows, int32_t end_id, int32_t unk_id, int32_t step, int32_t max_len, int32_t *done,
+                             int32_t *length, float *logprob, int32_t *tokens, int64_t *next_ids, void *workspace, size_t workspace_bytes,
+                             void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Host-buffer convenience entry point (used for the end-to-end measurement): all pointers are HOST
  * memory; copies inputs to the device, builds the plan, runs `num_layers` GatedMessagePassingLayers
  * (layer l uses weight set l; pass the same pointers to share weights), copies the final states back

@@ -57,7 +57,11 @@ factories import the layer classes by module path (`implementations/typilus/trai
    builds the native class.  The module is imported first, with the same refusal as step 14,
 16. with ``native_ppi_head=True`` only: the same for ``PPIClassification`` inside ``ptgnn.implementations.ppi.ppi``.  On Python 3.12 that
    module cannot be imported (``TensorizedGraphData[np.ndarray]`` raises ``TypeError`` at class creation): ``install()`` raises
-   ``ImportError`` and changes nothing.
+   ``ImportError`` and changes nothing,
+17. with ``native_greedy_decode=True`` only: replaces the method ``greedy_decode`` of the reference's ``GruCopyingDecoderModel`` with
+   ``ptgnn_b200.decoding.greedy_decode`` (the decode loop on the device, DESIGN.md §3.18), which takes the same arguments and returns
+   the same result.  It works with the reference's decoder module and with the native one, so it does not need ``native_decoder``.  The
+   default leaves the reference's method in place.
 
 After ``install()``: ``import ptgnn.implementations.ppi.train`` etc. build ptgnn_b200 layers, unchanged.  ``uninstall()``
 restores the reference's classes.  The reference must be importable as ``ptgnn`` for steps 2-4 (it is not on the GPU test box;
@@ -100,6 +104,7 @@ _GRAPH2CLASS_MODULE = "ptgnn.implementations.typilus.graph2class"
 _GRAPH2CLASS_CLASS = "Graph2ClassModule"
 _PPI_MODULE = "ptgnn.implementations.ppi.ppi"
 _PPI_CLASS = "PPIClassification"
+_GREEDY_DECODE = "GruCopyingDecoderModel.greedy_decode"
 _saved: Dict[str, object] = {}
 
 
@@ -199,6 +204,21 @@ def _install_native_decoder() -> None:
         _rebind_everywhere({old: _dec.GruCopyingDecoder})      # the decoder module included
 
 
+def _native_greedy_decode(self, *, input_concrete_values, input_memories, input_memories_origin_idx, initial_states, neural_model):
+    from . import decoding as _decoding
+
+    return _decoding.greedy_decode(self, input_concrete_values=input_concrete_values, input_memories=input_memories,
+                                   input_memories_origin_idx=input_memories_origin_idx, initial_states=initial_states,
+                                   neural_model=neural_model)
+
+
+def _install_native_greedy_decode() -> None:
+    model = importlib.import_module(_DECODER_MODULE).GruCopyingDecoderModel
+    if model.__dict__.get("greedy_decode") is not _native_greedy_decode:
+        _saved[_GREEDY_DECODE] = (model, model.__dict__["greedy_decode"])
+        model.greedy_decode = _native_greedy_decode
+
+
 def _install_native_embedders(names=_NATIVE_EMBEDDERS) -> None:
     from . import embeddings as _emb
 
@@ -247,11 +267,11 @@ def install(force_torch_scatter: bool = False, native_reducers: bool = False, na
             native_graphnorm: bool = False, native_pna: bool = False, native_decoder: bool = False,
             native_embedders: bool = False, native_char_embedder: bool = False, native_egc: bool = False,
             native_feature_embedder: bool = False, native_heads: bool = False, native_graph2class_head: bool = False,
-            native_ppi_head: bool = False) -> Dict[str, object]:
+            native_ppi_head: bool = False, native_greedy_decode: bool = False) -> Dict[str, object]:
     report: Dict[str, object] = {"torch_scatter": "real", "layers": False, "container": False, "metrics": False, "reducers": False,
                                  "selfattention": False, "graphnorm": False, "pna": False, "decoder": False, "embedders": False,
                                  "char_embedder": False, "egc": False, "feature_embedder": False,
-                                 "heads": False, "graph2class_head": False, "ppi_head": False}
+                                 "heads": False, "graph2class_head": False, "ppi_head": False, "greedy_decode": False}
     previous_scatter = {name: sys.modules.get(name) for name in ("torch_scatter", "torch_scatter.composite")}
     # 1. torch_scatter
     have_real = False
@@ -344,6 +364,10 @@ def install(force_torch_scatter: bool = False, native_reducers: bool = False, na
     if native_ppi_head:
         _install_native_head(_PPI_MODULE, _PPI_CLASS)
         report["ppi_head"] = True
+    # 17. GruCopyingDecoderModel.greedy_decode (opt-in)
+    if native_greedy_decode:
+        _install_native_greedy_decode()
+        report["greedy_decode"] = True
     return report
 
 
@@ -356,6 +380,9 @@ def uninstall() -> None:
             pkg = sys.modules.get("ptgnn.neuralmodels.gnn")
             if pkg is not None and getattr(pkg, "GraphNeuralNetwork", None) is _gnn.GraphNeuralNetwork:
                 pkg.GraphNeuralNetwork = val
+        elif key == _GREEDY_DECODE:
+            model, method = val
+            model.greedy_decode = method
         elif ":" in key:
             mod_name, attr = key.split(":", 1)
             if mod_name in sys.modules:
