@@ -108,6 +108,71 @@ static int exclusive_scan_i32(const int32_t *in, int32_t *out, int64_t n, int32_
     return launch(PTGNN_KERNEL_PLAN, st, scan_apply_kernel, (unsigned)nb, SCAN_THREADS, 0, in, n, sums, out, out_total);
 }
 
+// Single-pass exclusive scan with decoupled look-back: one launch.  `state` holds scan_workspace_elems(n) zeroed words: [0] is a
+// ticket that hands out tiles in launch order (so every tile's predecessors are running or done), [1 + i] tile i's published sum.
+// A published word is kind << 31 | (sum + 1): 0 = nothing yet, kind 0 = the tile's own sum, kind 1 = the inclusive prefix through
+// the tile.  Sums stay below 2^31 - 1 (every scanned array totals at most E < INT32_MAX), so value and kind fit one word.
+constexpr uint32_t TILE_INCLUSIVE = 1u << 31;
+
+__device__ __forceinline__ uint32_t load_tile_word(const uint32_t *p) {
+    uint32_t v;
+    asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p));
+    return v;
+}
+
+__global__ void __launch_bounds__(SCAN_THREADS) scan_lookback_kernel(const int32_t *in /*may alias out*/, int64_t n, int32_t *out,
+                                                                     uint32_t *__restrict__ state) {
+    __shared__ int s_tile, s_prefix;
+    if (threadIdx.x == 0) s_tile = (int)atomicAdd(state, 1u);
+    __syncthreads();
+    const int tile = s_tile;
+    const int64_t base = (int64_t)tile * SCAN_CHUNK + (int64_t)threadIdx.x * SCAN_ITEMS;
+    int v[SCAN_ITEMS];
+    int s = 0;
+#pragma unroll
+    for (int i = 0; i < SCAN_ITEMS; ++i) {
+        v[i] = base + i < n ? in[base + i] : 0;
+        s += v[i];
+    }
+    int total;
+    int ex = block_exclusive_scan<SCAN_THREADS>(s, &total);
+    uint32_t *words = state + 1;
+    if (threadIdx.x == 0) atomicExch(&words[tile], (tile == 0 ? TILE_INCLUSIVE : 0u) | (uint32_t)(total + 1));
+    if (threadIdx.x < 32) {  // warp 0 walks back over the predecessors, 32 tiles per step, nearest in lane 0
+        const int lane = threadIdx.x;
+        int prefix = 0;
+        for (int p = tile - 1 - lane; tile > 0; p -= 32) {
+            uint32_t w;
+            do {
+                w = p >= 0 ? load_tile_word(&words[p]) : (TILE_INCLUSIVE | 1u);
+            } while (__any_sync(0xffffffffu, w == 0));
+            const unsigned inclusive = __ballot_sync(0xffffffffu, w & TILE_INCLUSIVE);
+            const int upto = inclusive ? __ffs(inclusive) - 1 : 31;
+            int part = lane <= upto ? (int)(w & ~TILE_INCLUSIVE) - 1 : 0;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+            prefix += part;
+            if (inclusive) break;
+        }
+        if (lane == 0) {
+            if (tile > 0) atomicExch(&words[tile], TILE_INCLUSIVE | (uint32_t)(prefix + total + 1));
+            s_prefix = prefix;
+        }
+    }
+    __syncthreads();
+    ex += s_prefix;
+#pragma unroll
+    for (int i = 0; i < SCAN_ITEMS; ++i) {
+        if (base + i < n) out[base + i] = ex;
+        ex += v[i];
+    }
+}
+
+static int single_pass_scan_i32(const int32_t *in, int32_t *out, int64_t n, uint32_t *state, cudaStream_t st) {
+    if (n <= 0) return PTGNN_OK;
+    return launch(PTGNN_KERNEL_PLAN, st, scan_lookback_kernel, (unsigned)ceil_div(n, SCAN_CHUNK), SCAN_THREADS, 0, in, n, out, state);
+}
+
 // =================================================================================================
 // pass 0: int64 -> int32 down-conversion, range check, in-degree histogram
 // =================================================================================================
@@ -116,16 +181,23 @@ __global__ void __launch_bounds__(256) convert_count_kernel(const __grid_constan
                                                             int32_t *__restrict__ tgt32, int32_t *__restrict__ deg,
                                                             int32_t *__restrict__ status) {
     int bad = 0;
-    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < num_edges;
-         e += (int64_t)gridDim.x * blockDim.x) {
-        const int t = type_of_edge(tabs.off, tabs.num_types, e);
-        const int64_t i = e - tabs.off[t];
-        int64_t s = tabs.src[t][i], v = tabs.tgt[t][i];
-        if (s < 0 || s >= num_source_nodes) { s = 0; ++bad; }
-        if (v < 0 || v >= num_nodes) { v = 0; ++bad; }
-        src32[e] = (int32_t)s;
-        tgt32[e] = (int32_t)v;
-        atomicAdd(&deg[v], 1);
+    const int lane = threadIdx.x & 31;
+    // the whole warp walks the loop together, so edges of one warp into the same target (a hub) add to its degree once
+    for (int64_t base = (int64_t)blockIdx.x * blockDim.x; base < num_edges; base += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t e = base + threadIdx.x;
+        int64_t v = -1;
+        if (e < num_edges) {
+            const int t = type_of_edge(tabs.off, tabs.num_types, e);
+            const int64_t i = e - tabs.off[t];
+            int64_t s = tabs.src[t][i];
+            v = tabs.tgt[t][i];
+            if (s < 0 || s >= num_source_nodes) { s = 0; ++bad; }
+            if (v < 0 || v >= num_nodes) { v = 0; ++bad; }
+            src32[e] = (int32_t)s;
+            tgt32[e] = (int32_t)v;
+        }
+        const unsigned peers = __match_any_sync(0xffffffffu, (int)v);
+        if (v >= 0 && lane == __ffs(peers) - 1) atomicAdd(&deg[v], __popc(peers));
     }
     if (bad) atomicAdd(status, bad);
 }
@@ -246,10 +318,9 @@ static PlanWs plan_ws_layout(int64_t N, int64_t E) {
     return w;
 }
 
-// Stable LSD radix sort of (keys, edge id) over the low `key_bits` bits into `perm`; `keys` is not modified.  If
-// `sorted_keys` != nullptr it receives a pointer to the sorted key array (one of the workspace buffers).
+// Stable LSD radix sort of (keys, edge id) over the low `key_bits` bits into `perm`; `keys` is not modified.
 static int sort_edges_by_key(const int32_t *keys_in, int key_bits, int64_t E, int32_t *perm, char *ws, const PlanWs &L,
-                             cudaStream_t st, const int32_t **sorted_keys = nullptr) {
+                             cudaStream_t st) {
     const int64_t nblk = ceil_div(E, SORT_CHUNK);
     int32_t *keys[2] = {reinterpret_cast<int32_t *>(ws + L.keys_a), reinterpret_cast<int32_t *>(ws + L.keys_b)};
     int32_t *vals[2] = {reinterpret_cast<int32_t *>(ws + L.vals_a), reinterpret_cast<int32_t *>(ws + L.vals_b)};
@@ -268,7 +339,6 @@ static int sort_edges_by_key(const int32_t *keys_in, int key_bits, int64_t E, in
         kin = kout;
         vin = vout;
     }
-    if (sorted_keys) *sorted_keys = kin;
     return PTGNN_OK;
 }
 static int bits_for(int64_t n) {
@@ -283,40 +353,241 @@ static int sort_edges_by_target(const int32_t *tgt32, int64_t N, int64_t E, int3
 }
 
 // =================================================================================================
-// block plan for the fused gather -> Linear -> reduce kernel (fused_mp.cu): edges sorted, stably, by
-// (target block, edge type, target).  key = (block * T + type) * B + (target - block * B) < ceil(N / B) * T * B: for config 2
-// that is 22 bits = three 8-bit radix passes.  B <= 256, types <= 128.
+// block plan for the fused gather -> Linear -> reduce kernel (fused_mp.cu): edges ordered by (target block, edge type,
+// target - block start, edge id).  B <= 256, types <= 128.  Four launches:
+//   count    each edge takes a slot in its (block, type) group from an atomic counter in group_off
+//   scan     group_off = exclusive scan of the counts (single pass)
+//   scatter  edge e writes the word (tl << 32 | e) to group_off[g] + slot: groups are in place, their insides in atomic order
+//   order    each group sorts its words, which are distinct, and writes src_f / tl_f: the result is the same whatever order
+//            the atomics handed out.  Groups of up to kWarpGroup edges are sorted by one warp in shared memory; larger ones
+//            (a hub target, or many edges of one type into one block) by the whole CTA, with stable 8-bit radix passes
+//            through the workspace.
 // =================================================================================================
-__global__ void __launch_bounds__(256) block_keys_kernel(const __grid_constant__ TypeOffsets toff, int64_t num_edges,
-                                                         const int32_t *__restrict__ tgt32, int B, int32_t *__restrict__ keys,
-                                                         int32_t *__restrict__ group_count) {
+__device__ __forceinline__ void group_of_edge(const TypeOffsets &toff, const int32_t *tgt32, int B, int64_t e, int &g, int &tl) {
+    const int t = type_of_edge(toff.off, toff.num_types, e);
+    const int v = tgt32[e];
+    const int blk = v / B;
+    tl = v - blk * B;
+    g = blk * toff.num_types + t;
+}
+
+// Also clears the tile words of the scan that follows.
+__global__ void __launch_bounds__(256) block_count_kernel(const __grid_constant__ TypeOffsets toff, int64_t num_edges,
+                                                          const int32_t *__restrict__ tgt32, int B, int32_t *__restrict__ group_count,
+                                                          int32_t *__restrict__ slot, uint32_t *__restrict__ scan_state,
+                                                          int64_t scan_state_words) {
+    if (blockIdx.x == 0)
+        for (int64_t i = threadIdx.x; i < scan_state_words; i += blockDim.x) scan_state[i] = 0;
+    const int lane = threadIdx.x & 31;
+    // the whole warp walks the loop together, so edges of one group that share a warp take their slots with one atomic
+    for (int64_t base = (int64_t)blockIdx.x * blockDim.x; base < num_edges; base += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t e = base + threadIdx.x;
+        int g = -1, tl;
+        if (e < num_edges) group_of_edge(toff, tgt32, B, e, g, tl);
+        const unsigned peers = __match_any_sync(0xffffffffu, g);
+        const int leader = __ffs(peers) - 1;
+        int first = 0;
+        if (g >= 0 && lane == leader) first = atomicAdd(&group_count[g], __popc(peers));
+        first = __shfl_sync(0xffffffffu, first, leader);
+        if (g >= 0) slot[e] = first + __popc(peers & ((1u << lane) - 1u));
+    }
+}
+
+__global__ void __launch_bounds__(256) block_scatter_kernel(const __grid_constant__ TypeOffsets toff, int64_t num_edges,
+                                                            const int32_t *__restrict__ tgt32, int B, const int32_t *__restrict__ group_off,
+                                                            const int32_t *__restrict__ slot, uint64_t *__restrict__ words) {
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < num_edges; e += (int64_t)gridDim.x * blockDim.x) {
-        const int t = type_of_edge(toff.off, toff.num_types, e);
-        const int v = tgt32[e];
-        const int blk = v / B, tl = v - blk * B;
-        keys[e] = (blk * toff.num_types + t) * B + tl;
-        atomicAdd(&group_count[(int64_t)blk * toff.num_types + t], 1);
+        int g, tl;
+        group_of_edge(toff, tgt32, B, e, g, tl);
+        words[group_off[g] + slot[e]] = (uint64_t)tl << 32 | (uint32_t)e;
     }
 }
-__global__ void __launch_bounds__(256) block_finalize_kernel(int64_t num_edges, int B, const int32_t *__restrict__ perm,
-                                                             const int32_t *__restrict__ sorted_keys,
-                                                             const int32_t *__restrict__ src32, int32_t *__restrict__ src_f,
-                                                             uint8_t *__restrict__ tl_f) {
-    for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < num_edges; j += (int64_t)gridDim.x * blockDim.x) {
-        src_f[j] = src32[perm[j]];
-        tl_f[j] = (uint8_t)(sorted_keys[j] % B);
+
+constexpr int ORDER_THREADS = 512;
+constexpr int ORDER_WARPS = ORDER_THREADS / 32;   // one group per warp: a CTA takes ORDER_WARPS consecutive groups
+constexpr int kWarpGroup = 256;                   // largest group a warp sorts in shared memory (a whole block of self edges at B = 256)
+constexpr int ORDER_ROUNDS = 8;                   // 32-word rounds per warp and chunk in the CTA path
+constexpr int ORDER_CHUNK = ORDER_THREADS * ORDER_ROUNDS;
+constexpr int ORDER_DIGITS = 5;                   // 8-bit digits of the word: four of e, then tl
+
+union OrderSmem {
+    uint64_t words[ORDER_WARPS][kWarpGroup];
+    struct {
+        int hist[ORDER_DIGITS][RADIX];
+        int warp_hist[ORDER_WARPS][RADIX];
+        int base[RADIX];
+        unsigned uniform;
+    } cta;
+};
+
+__device__ __forceinline__ int word_digit(uint64_t w, int d) { return (int)(w >> (d < 4 ? 8 * d : 32)) & (RADIX - 1); }
+__device__ __forceinline__ void write_edge(uint64_t w, int64_t j, const int32_t *src32, int32_t *src_f, uint8_t *tl_f) {
+    src_f[j] = src32[(uint32_t)w];
+    tl_f[j] = (uint8_t)(w >> 32);
+}
+
+// One group of n <= 32 * R words in shared memory, sorted by one warp: the rank of a word is how many words of the group are
+// smaller.  Lane l holds words l, l + 32, ...; each shared word is read once (a broadcast) and compared with all of them.
+template <int R>
+__device__ __forceinline__ void order_small_group(const uint64_t *s, int n, int64_t j0, const int32_t *src32, int32_t *src_f,
+                                                  uint8_t *tl_f) {
+    const int lane = threadIdx.x & 31;
+    uint64_t w[R];
+    int rank[R];
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+        w[r] = r * 32 + lane < n ? s[r * 32 + lane] : ~0ull;
+        rank[r] = 0;
+    }
+#pragma unroll 4
+    for (int k = 0; k < n; ++k) {
+        const uint64_t x = s[k];
+#pragma unroll
+        for (int r = 0; r < R; ++r) rank[r] += x < w[r];
+    }
+#pragma unroll
+    for (int r = 0; r < R; ++r)
+        if (r * 32 + lane < n) write_edge(w[r], j0 + rank[r], src32, src_f, tl_f);
+}
+
+// One group of n > kWarpGroup words at a[0..n), sorted by the whole CTA: the digit histograms come from one read (they do not
+// depend on the order), digits every word shares are skipped, and each remaining digit is one stable pass, chunk by chunk
+// in input order (within a chunk ranks go by (warp, round, lane), i.e. input position).  Passes alternate between a and b;
+// the last one writes src_f / tl_f at j0 + rank.
+__device__ void order_large_group(uint64_t *a, uint64_t *b, int n, int64_t j0, const int32_t *src32, int32_t *src_f, uint8_t *tl_f,
+                                  OrderSmem &sm) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int i = threadIdx.x; i < ORDER_DIGITS * RADIX; i += ORDER_THREADS) (&sm.cta.hist[0][0])[i] = 0;
+    if (threadIdx.x == 0) sm.cta.uniform = 0;
+    __syncthreads();
+    for (int64_t c0 = 0; c0 < n; c0 += ORDER_CHUNK) {
+        uint64_t w[ORDER_ROUNDS];
+#pragma unroll
+        for (int r = 0; r < ORDER_ROUNDS; ++r) {
+            const int64_t i = c0 + r * ORDER_THREADS + threadIdx.x;
+            w[r] = i < n ? a[i] : 0;
+        }
+#pragma unroll
+        for (int r = 0; r < ORDER_ROUNDS; ++r)
+            if (c0 + r * ORDER_THREADS + threadIdx.x < n)
+#pragma unroll
+                for (int d = 0; d < ORDER_DIGITS; ++d) atomicAdd(&sm.cta.hist[d][word_digit(w[r], d)], 1);
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < ORDER_DIGITS * RADIX; i += ORDER_THREADS)
+        if ((&sm.cta.hist[0][0])[i] == n) atomicOr(&sm.cta.uniform, 1u << (i / RADIX));
+    __syncthreads();
+    const unsigned passes = ~sm.cta.uniform & ((1u << ORDER_DIGITS) - 1);   // n > 1 distinct words: never empty
+    const int last = 31 - __clz(passes);
+    uint64_t *in = a, *out = b;
+    for (int d = 0; d <= last; ++d) {
+        if (!(passes >> d & 1)) continue;
+        if (threadIdx.x < 32) {   // base = exclusive scan of this digit's histogram
+            int c[RADIX / 32], s = 0;
+#pragma unroll
+            for (int k = 0; k < RADIX / 32; ++k) { c[k] = sm.cta.hist[d][lane * (RADIX / 32) + k]; s += c[k]; }
+            int run = warp_inclusive_scan(s) - s;
+#pragma unroll
+            for (int k = 0; k < RADIX / 32; ++k) { sm.cta.base[lane * (RADIX / 32) + k] = run; run += c[k]; }
+        }
+        for (int64_t c0 = 0; c0 < n; c0 += ORDER_CHUNK) {
+            for (int i = threadIdx.x; i < ORDER_WARPS * RADIX; i += ORDER_THREADS) (&sm.cta.warp_hist[0][0])[i] = 0;
+            __syncthreads();
+            uint64_t w[ORDER_ROUNDS];
+            int digit[ORDER_ROUNDS];
+#pragma unroll
+            for (int r = 0; r < ORDER_ROUNDS; ++r) {   // all loads in flight before the warp-synchronous part
+                const int64_t i = c0 + (warp * ORDER_ROUNDS + r) * 32 + lane;
+                w[r] = i < n ? in[i] : 0;
+                digit[r] = i < n ? -1 : RADIX;             // RADIX = no word
+            }
+#pragma unroll
+            for (int r = 0; r < ORDER_ROUNDS; ++r) {
+                if (digit[r] < 0) digit[r] = word_digit(w[r], d);
+                const unsigned peers = __match_any_sync(0xffffffffu, digit[r]);
+                if (digit[r] < RADIX && lane == __ffs(peers) - 1) sm.cta.warp_hist[warp][digit[r]] += __popc(peers);
+                __syncwarp();
+            }
+            __syncthreads();
+            for (int k = threadIdx.x; k < RADIX; k += ORDER_THREADS) {   // per digit: exclusive prefix over warps, carried across chunks
+                int run = sm.cta.base[k];
+                for (int v = 0; v < ORDER_WARPS; ++v) {
+                    const int c = sm.cta.warp_hist[v][k];
+                    sm.cta.warp_hist[v][k] = run;
+                    run += c;
+                }
+                sm.cta.base[k] = run;
+            }
+            __syncthreads();
+#pragma unroll
+            for (int r = 0; r < ORDER_ROUNDS; ++r) {
+                const bool valid = digit[r] < RADIX;
+                const unsigned peers = __match_any_sync(0xffffffffu, digit[r]);
+                int dst = 0;
+                if (valid) dst = sm.cta.warp_hist[warp][digit[r]] + __popc(peers & ((1u << lane) - 1u));
+                __syncwarp();
+                if (valid && lane == __ffs(peers) - 1) sm.cta.warp_hist[warp][digit[r]] += __popc(peers);
+                __syncwarp();
+                if (valid) {
+                    if (d == last) write_edge(w[r], j0 + dst, src32, src_f, tl_f);
+                    else out[dst] = w[r];
+                }
+            }
+            __syncthreads();
+        }
+        uint64_t *t = in; in = out; out = t;
     }
 }
-struct BlockPlanWs { size_t keys, perm, scan_sums, plan, total; };
+
+__global__ void __launch_bounds__(ORDER_THREADS, 2) block_order_kernel(int64_t num_groups, const int32_t *__restrict__ group_off,
+                                                                    uint64_t *__restrict__ words, uint64_t *__restrict__ tmp,
+                                                                    const int32_t *__restrict__ src32, int32_t *__restrict__ src_f,
+                                                                    uint8_t *__restrict__ tl_f) {
+    __shared__ OrderSmem sm;
+    __shared__ int off[ORDER_WARPS + 1];
+    const int64_t g0 = (int64_t)blockIdx.x * ORDER_WARPS;
+    const int ng = (int)(num_groups - g0 < ORDER_WARPS ? num_groups - g0 : ORDER_WARPS);
+    if (threadIdx.x <= ng) off[threadIdx.x] = group_off[g0 + threadIdx.x];
+    __syncthreads();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (warp < ng) {
+        const int j0 = off[warp], n = off[warp + 1] - j0;
+        if (n <= kWarpGroup) {
+            uint64_t *s = sm.words[warp];
+            for (int i = lane; i < n; i += 32) s[i] = words[j0 + i];
+            __syncwarp();
+            switch ((n + 31) / 32) {
+                case 1: order_small_group<1>(s, n, j0, src32, src_f, tl_f); break;
+                case 2: order_small_group<2>(s, n, j0, src32, src_f, tl_f); break;
+                case 3: order_small_group<3>(s, n, j0, src32, src_f, tl_f); break;
+                case 4: order_small_group<4>(s, n, j0, src32, src_f, tl_f); break;
+                case 5: order_small_group<5>(s, n, j0, src32, src_f, tl_f); break;
+                case 6: order_small_group<6>(s, n, j0, src32, src_f, tl_f); break;
+                case 7: order_small_group<7>(s, n, j0, src32, src_f, tl_f); break;
+                case 8: order_small_group<8>(s, n, j0, src32, src_f, tl_f); break;
+                default: break;   // n == 0
+            }
+        }
+    }
+    __syncthreads();
+    for (int k = 0; k < ng; ++k) {
+        const int j0 = off[k], n = off[k + 1] - j0;
+        if (n > kWarpGroup) order_large_group(words + j0, tmp + j0, n, j0, src32, src_f, tl_f, sm);
+    }
+}
+
+struct BlockPlanWs { size_t slot, words, tmp, scan_state, total; };
 static BlockPlanWs block_plan_ws_layout(int64_t N, int64_t E, int T, int B) {
     const int64_t nblk = ceil_div(N > 0 ? N : 1, B), groups = nblk * (T > 0 ? T : 1) + 1;
     Layout l;
     BlockPlanWs w;
-    w.keys = l.add((size_t)E + 1, 4);
-    w.perm = l.add((size_t)E + 1, 4);
-    w.scan_sums = l.add(scan_workspace_elems(groups), 4);
-    w.plan = l.add_bytes(plan_ws_layout(N, E).total);
-    w.total = l.total;
+    w.slot = l.add((size_t)E + 1, 4);
+    w.words = l.add((size_t)E + 1, 8);
+    w.tmp = l.add((size_t)E + 1, 8);
+    w.scan_state = l.add(scan_workspace_elems(groups), 4);
+    // The size query is part of the ABI (callers keep buffers across calls): it stays at what the radix-sorted block plan
+    // reserved, keys + perm + group scan + a whole edge plan, which holds the slices above for every N, E, T and B.
+    w.total = 2 * ws_slice((size_t)E + 1, 4) + ws_slice(scan_workspace_elems(groups), 4) + plan_ws_layout(N, E).total;
     return w;
 }
 
@@ -365,10 +636,10 @@ static int plan_build_phases(int phases, int64_t num_nodes, int64_t num_source_n
     int32_t *deg = reinterpret_cast<int32_t *>(ws + L.deg);
 
     const unsigned grid = (unsigned)(ceil_div(E > 0 ? E : 1, 256) < 132 * 16 ? ceil_div(E > 0 ? E : 1, 256) : 132 * 16);
-    int rc = PTGNN_OK;
     if (phases & 1) {
         PTGNN_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t), st));
-        PTGNN_CUDA(cudaMemsetAsync(deg, 0, sizeof(int32_t) * (size_t)(num_nodes + 1), st));
+        // deg and the row_ptr scan's tile words are adjacent slices: one memset clears both
+        PTGNN_CUDA(cudaMemsetAsync(deg, 0, L.keys_a - L.deg, st));
         if (E == 0) {
             PTGNN_CUDA(cudaMemsetAsync(row_ptr, 0, sizeof(int32_t) * (size_t)(num_nodes + 1), st));
             return PTGNN_OK;
@@ -377,13 +648,11 @@ static int plan_build_phases(int phases, int64_t num_nodes, int64_t num_source_n
         PTGNN_CHECK_ARG(num_nodes > 0, "plan_build: edges given but num_nodes == 0");
         PTGNN_TRY(launch(PTGNN_KERNEL_PLAN, st, convert_count_kernel, grid, 256, 0, tabs, num_nodes, num_source_nodes, E, src32, tgt32, deg, status));
         // row_ptr[0..N] = exclusive scan of deg[0..N] (deg[N] == 0, so row_ptr[N] == E)
-        rc = exclusive_scan_i32(deg, row_ptr, num_nodes + 1, reinterpret_cast<int32_t *>(ws + L.scan_sums), nullptr, st);
-        if (rc) return rc;
+        PTGNN_TRY(single_pass_scan_i32(deg, row_ptr, num_nodes + 1, reinterpret_cast<uint32_t *>(ws + L.scan_sums), st));
     }
     if (!(phases & 2) || E == 0) return PTGNN_OK;
     PTGNN_CHECK_ARG(perm && pos && src_sorted && etype_sorted && src32 && tgt32, "plan_build: null output array");
-    rc = sort_edges_by_target(tgt32, num_nodes, E, perm, ws, L, st);
-    if (rc) return rc;
+    PTGNN_TRY(sort_edges_by_target(tgt32, num_nodes, E, perm, ws, L, st));
     return launch(PTGNN_KERNEL_PLAN, st, finalize_plan_kernel, grid, 256, 0, toff, E, perm, src32, pos, src_sorted, etype_sorted);
 }
 
@@ -429,8 +698,7 @@ extern "C" int ptgnn_b200_block_plan_build(int64_t num_nodes, int32_t num_types,
     const int64_t E = type_off[T];
     PTGNN_CHECK_ARG(E >= 0 && E < INT32_MAX, "block_plan_build: edge count out of range");
     const int64_t nblk = ceil_div(num_nodes, B), groups = nblk * T;
-    PTGNN_CHECK_ARG(nblk * T * B < ((int64_t)1 << 31), "block_plan_build: %lld blocks x %d types x %d targets overflow the 31-bit sort key",
-                    (long long)nblk, T, B);
+    PTGNN_CHECK_ARG(groups < INT32_MAX, "block_plan_build: %lld blocks x %d types overflow the 31-bit group index", (long long)nblk, T);
     PTGNN_CHECK_ARG(group_off, "block_plan_build: null group_off");
     const BlockPlanWs L = block_plan_ws_layout(num_nodes, E, T, B);
     PTGNN_CHECK_WORKSPACE("block_plan_build", workspace, workspace_bytes, L.total);
@@ -438,16 +706,17 @@ extern "C" int ptgnn_b200_block_plan_build(int64_t num_nodes, int32_t num_types,
     if (E == 0 || num_nodes == 0) return PTGNN_OK;
     PTGNN_CHECK_ARG(src32 && tgt32 && src_f && tl_f, "block_plan_build: null edge array");
     char *ws = static_cast<char *>(workspace);
-    int32_t *keys = reinterpret_cast<int32_t *>(ws + L.keys), *perm = reinterpret_cast<int32_t *>(ws + L.perm);
+    int32_t *slot = reinterpret_cast<int32_t *>(ws + L.slot);
+    uint64_t *words = reinterpret_cast<uint64_t *>(ws + L.words), *tmp = reinterpret_cast<uint64_t *>(ws + L.tmp);
+    uint32_t *scan_state = reinterpret_cast<uint32_t *>(ws + L.scan_state);
     TypeOffsets toff{};
     toff.num_types = T;
     for (int t = 0; t <= PTGNN_MAX_EDGE_TYPES; ++t) toff.off[t] = (int32_t)type_off[t < T ? t : T];
     const unsigned grid = (unsigned)(ceil_div(E, 256) < 132 * 16 ? ceil_div(E, 256) : 132 * 16);
-    PTGNN_TRY(launch(PTGNN_KERNEL_PLAN, st, block_keys_kernel, grid, 256, 0, toff, E, tgt32, B, keys, group_off));
-    int rc = exclusive_scan_i32(group_off, group_off, groups + 1, reinterpret_cast<int32_t *>(ws + L.scan_sums), nullptr, st);
-    if (rc) return rc;
-    const int32_t *sorted_keys = nullptr;
-    rc = sort_edges_by_key(keys, bits_for(nblk * T * B), E, perm, ws + L.plan, plan_ws_layout(num_nodes, E), st, &sorted_keys);
-    if (rc) return rc;
-    return launch(PTGNN_KERNEL_PLAN, st, block_finalize_kernel, grid, 256, 0, E, B, perm, sorted_keys, src32, src_f, tl_f);
+    PTGNN_TRY(launch(PTGNN_KERNEL_PLAN, st, block_count_kernel, grid, 256, 0, toff, E, tgt32, B, group_off, slot, scan_state,
+                     (int64_t)scan_workspace_elems(groups + 1)));
+    PTGNN_TRY(single_pass_scan_i32(group_off, group_off, groups + 1, scan_state, st));
+    PTGNN_TRY(launch(PTGNN_KERNEL_PLAN, st, block_scatter_kernel, grid, 256, 0, toff, E, tgt32, B, group_off, slot, words));
+    return launch(PTGNN_KERNEL_PLAN, st, block_order_kernel, (unsigned)ceil_div(groups, ORDER_WARPS), ORDER_THREADS, 0, groups, group_off,
+                  words, tmp, src32, src_f, tl_f);
 }
