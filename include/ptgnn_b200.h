@@ -185,7 +185,7 @@ int ptgnn_b200_mlp_forward(int32_t bf16_states, const void *node_states, const v
  * message tensor of gatedmessagepassing.py:64 / mlpmessagepassing.py:100-112 is never materialised.
  *
  * Block plan: the edges sorted, stably, by (target block, edge type, target), blocks of `block_targets`
- * (<= 176, multiple of 8; ptgnn_b200_block_plan_block_targets recommends one) consecutive target nodes:
+ * (<= 240, multiple of 8) consecutive target nodes:
  *   group_off[ceil(N / B) * T + 1]  sorted-edge offsets of the (block, type) groups
  *   src_f[E]                        source node of the edge at sorted position j
  *   tl_f[E]                         target of that edge, relative to its block's first node
@@ -202,7 +202,11 @@ typedef struct {
     int32_t *status;
 } ptgnn_b200_block_plan;
 
+/* Recommended block sizes: whole waves of one CTA per SM, then the largest multiple of 8 up to the cap.
+ * _block_targets caps B at 176, the limit of earlier releases, and keeps recommending what it always did;
+ * _large_block_targets caps it at 240, the fused kernel's limit (fewer blocks: each per-type weight load serves more edges). */
 int32_t ptgnn_b200_block_plan_block_targets(int64_t num_nodes);
+int32_t ptgnn_b200_block_plan_large_block_targets(int64_t num_nodes);
 size_t ptgnn_b200_block_plan_workspace_bytes(int64_t num_nodes, int64_t num_edges, int32_t num_types, int32_t block_targets);
 int ptgnn_b200_block_plan_build(int64_t num_nodes, int32_t num_types, const int64_t *type_off /*[host]*/,
                                 const int32_t *src32, const int32_t *tgt32, int32_t block_targets, int32_t *group_off,

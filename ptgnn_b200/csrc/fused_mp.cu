@@ -24,9 +24,6 @@ constexpr int GATHER_WARP0 = 8, GATHER_THREADS = 64;
 constexpr int SCHED_WARP = 10;
 constexpr int REDUCER_WARP0 = 12;
 constexpr int SCHED_READER_WARPS = 8 + 2 + 4;          // readers of the scheduler's table: consumers, gatherers, reducer
-constexpr int NUM_SLOTS = 3, LOOKAHEAD = 2;
-constexpr int SLOT_BYTES = 32768;
-constexpr int RING_BYTES = NUM_SLOTS * SLOT_BYTES;
 constexpr int META_RING = 8;
 constexpr int SCHED_RING = 4;
 // The launch gives every thread 128 registers; the producer and reducer warpgroups give some back and the two consumer
@@ -48,12 +45,29 @@ struct Sched {                    // one target block: its id and the T+1 sorted
     int32_t blk, pad[3];
     int32_t off[PTGNN_MAX_EDGE_TYPES + 4];
 };
-constexpr int ACC_OFF = RING_BYTES;
-constexpr int AGG_OFF = RING_BYTES + ACC_BYTES;
 __host__ __device__ constexpr int agg_bytes(int B) { return B * kD * 4; }
 constexpr int SMEM_TAIL = META_RING * (int)sizeof(Meta) + SCHED_RING * (int)sizeof(Sched) + 256 /*barriers*/;
-constexpr int smem_bytes(int B) { return 1024 + RING_BYTES + ACC_BYTES + agg_bytes(B) + SMEM_TAIL; }
-static_assert(smem_bytes(kMaxBlockTargets) <= 232448, "shared memory budget");
+
+// Shared memory of an instance: [ring of NUM_SLOTS slots][acc_s][agg_s: B rows][Meta ring][Sched ring][barriers], behind up to
+// 1 KB of alignment pad.  A slot holds the gathered rows of one (sub-group, segment): NT = parts x K / 64 operand tiles of
+// NMAX rows x 128 bytes.  Two-tile instances (bf16 K <= 128, fp32 K = 64) keep three 16 KB slots.  Four-tile instances (fp32
+// K = 128, bf16 K = 256) keep two 32 KB slots: three would not leave room for agg_s at B = 240.  (Three slots of 48-column
+// sub-groups with a 48-column accumulator tile fit as well; at config 2 the fp32 kernel took 0.459 ms per launch that way
+// against 0.440 ms with two 64-column slots, H100 80GB HBM3 at 700 W.)
+template <int NPROD, int K>
+struct Geom {
+    static constexpr int NT = (NPROD == 3 ? 2 : 1) * (K / 64);  // operand tiles per slot
+    static constexpr int NUM_SLOTS = NT <= 2 ? 3 : 2;
+    static constexpr int SLOT_BYTES = NT * NMAX * 128;
+    static constexpr int RING_BYTES = NUM_SLOTS * SLOT_BYTES;
+    static constexpr int ACC_OFF = RING_BYTES;
+    static constexpr int AGG_OFF = RING_BYTES + ACC_BYTES;
+    static constexpr int smem_bytes(int B) { return 1024 + RING_BYTES + ACC_BYTES + agg_bytes(B) + SMEM_TAIL; }
+    static_assert(smem_bytes(kMaxBlockTargets) <= 232448, "shared memory budget");
+    static_assert(2 * NUM_SLOTS + 2 * SCHED_RING + 2 <= 256 / 8, "barrier area");
+    // the reducer reads a sub-group's Meta at most NUM_SLOTS + 2 sub-groups behind its writer (see the reducer)
+    static_assert(NUM_SLOTS + 2 < META_RING, "Meta ring too short for the slot count");
+};
 
 struct Params {
     const unsigned char *src_rows, *tgt_rows;
@@ -369,21 +383,23 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
     constexpr int KCH = K / 64;                                    // 128-byte swizzled chunks per part
     constexpr int NT = NPART * KCH;                                // operand tiles per slot
     constexpr int TILE_BYTES = NMAX * 128;
-    static_assert(NT * TILE_BYTES <= SLOT_BYTES, "slot size");
+    using G = Geom<NPROD, K>;
+    constexpr int NUM_SLOTS = G::NUM_SLOTS, SLOT_BYTES = G::SLOT_BYTES;
+    static_assert(NT == G::NT, "slot size");
     constexpr bool BF16 = NPROD == 1;
 
     extern __shared__ unsigned char smem_raw[];
     // 1024-byte aligned ring; the pad is added as an OFFSET so that the pointers keep the shared address space (an integer
     // round trip makes every access a generic LD/ST with 64-bit address arithmetic)
     unsigned char *ring = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    float *acc_s = reinterpret_cast<float *>(ring + ACC_OFF);
-    float *agg_s = reinterpret_cast<float *>(ring + AGG_OFF);
-    unsigned char *tail = ring + AGG_OFF + agg_bytes(p.B);
+    float *acc_s = reinterpret_cast<float *>(ring + G::ACC_OFF);
+    float *agg_s = reinterpret_cast<float *>(ring + G::AGG_OFF);
+    unsigned char *tail = ring + G::AGG_OFF + agg_bytes(p.B);
     Meta *meta_ring = reinterpret_cast<Meta *>(tail);
     Sched *sched = reinterpret_cast<Sched *>(tail + META_RING * sizeof(Meta));
     uint64_t *bars = reinterpret_cast<uint64_t *>(tail + META_RING * sizeof(Meta) + SCHED_RING * sizeof(Sched));
-    uint64_t *x_full = bars, *x_empty = bars + 3, *sched_full = bars + 6, *sched_empty = bars + 10;
-    uint64_t *acc_full = bars + 14, *acc_empty = bars + 15;
+    uint64_t *x_full = bars, *x_empty = bars + NUM_SLOTS, *sched_full = bars + 2 * NUM_SLOTS, *sched_empty = sched_full + SCHED_RING;
+    uint64_t *acc_full = sched_empty + SCHED_RING, *acc_empty = acc_full + 1;
 
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
     const int lane = threadIdx.x & 31;
@@ -410,7 +426,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
         // The walk reads the sub-group's column metadata from the Meta ring.  The gatherers write the metadata of sub-group c
         // before they wait for its slot, i.e. after the consumers have released sub-group c - 1 - NUM_SLOTS; a consumer releases
         // a sub-group only after it has staged the one before, which waits until the reducer is done with the one before that.
-        // So the reducer reads metadata at most NUM_SLOTS + 2 = 5 sub-groups behind the writer, inside the META_RING = 8 entries.
+        // So the reducer reads metadata at most NUM_SLOTS + 2 sub-groups behind the writer (5 with three slots, 4 with two), inside
+        // the META_RING = 8 entries (Geom asserts NUM_SLOTS + 2 < META_RING).
         tc::reg_dealloc<REDUCER_REGS>();
         const int d = (int)threadIdx.x - REDUCER_WARP0 * 32, rw = warp - REDUCER_WARP0;
         const uint32_t aggcol_s = smem_u32(agg_s + d);      // shared-space address of agg_s[0][d]
@@ -830,14 +847,14 @@ size_t packed_weight_bytes(int nprod, int num_types, int K, int use_target) {
 size_t packed_state_bytes(int nprod, int64_t rows, int K) {
     return nprod == 3 ? ws_slice((size_t)rows * K * 4 + 16, 1) : 0;
 }
-int recommended_block_targets(int64_t num_nodes) {
-    // the largest B <= kMaxBlockTargets (multiple of 8) for which the block count is a whole number of waves of 132 CTAs (one per H100 SM) or less
-    if (num_nodes <= 0) return kMaxBlockTargets;
-    const int64_t waves = ceil_div(num_nodes, (int64_t)kMaxBlockTargets * 132);
+int recommended_block_targets(int64_t num_nodes, int max_block_targets) {
+    // the largest B <= max_block_targets (multiple of 8) for which the block count is a whole number of waves of 132 CTAs (one per H100 SM) or less
+    if (num_nodes <= 0) return max_block_targets;
+    const int64_t waves = ceil_div(num_nodes, (int64_t)max_block_targets * 132);
     int64_t B = ceil_div(num_nodes, waves * 132);
     B = (B + 7) / 8 * 8;
     if (B < 8) B = 8;
-    if (B > kMaxBlockTargets) B = kMaxBlockTargets;
+    if (B > max_block_targets) B = max_block_targets;
     return (int)B;
 }
 
@@ -861,7 +878,8 @@ template <int NPROD, int K, int NSEG, int RED, int EPI = EPI_AGG>
 static int launch_one(const Params &p, cudaStream_t st) {
     const int sms = sm_count();
     const int grid = p.num_blocks < sms ? p.num_blocks : sms;
-    return launch(PTGNN_KERNEL_MESSAGE, st, fused_aggregate_kernel<NPROD, K, NSEG, RED, EPI>, grid, NUM_THREADS, smem_bytes(p.B), p);
+    return launch(PTGNN_KERNEL_MESSAGE, st, fused_aggregate_kernel<NPROD, K, NSEG, RED, EPI>, grid, NUM_THREADS,
+                  Geom<NPROD, K>::smem_bytes(p.B), p);
 }
 template <int NPROD, int K, int NSEG, int EPI = EPI_AGG>
 static int launch_red(const Params &p, cudaStream_t st) {

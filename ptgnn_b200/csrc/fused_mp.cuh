@@ -13,7 +13,7 @@
 // feature-major shared-memory tile and the thread that owns feature d runs a plain sequential loop over it: no shuffles,
 // no atomics, accumulation in the reference's edge order (per target: type-major, then list order), bit-reproducible.
 //
-// Work decomposition.  Targets are cut into blocks of B <= 256 consecutive nodes; the block plan (plan.cu) sorts the
+// Work decomposition.  Targets are cut into blocks of B <= 240 consecutive nodes; the block plan (plan.cu) sorts the
 // edges by (block, type, target).  A CTA owns a block at a time and keeps its aggregate agg_s[B][D] fp32 in shared
 // memory across all edge types, then writes it once (optionally through mean / GELU / LayerNorm: the Mlp layer's
 // pre-dense epilogue).  HBM traffic per layer = gathered rows (L2-resident per graph) + agg once.
@@ -29,7 +29,7 @@
 //
 // Roles (16 warps):  0-3 and 4-7 CONSUMERS, two warpgroups computing the MMAs for features [0,64) / [64,128) and staging
 //   them into the feature-major tile acc_s; they never touch agg_s |
-//   8-9 ROW GATHERERS (16-byte cp.async into a 3-slot ring, SWIZZLE_128B K-major) |
+//   8-9 ROW GATHERERS (16-byte cp.async into a 2- or 3-slot ring, SWIZZLE_128B K-major; Geom in fused_mp.cu) |
 //   10 SCHEDULER (block -> group offsets table ring) |
 //   12-15 REDUCER: owns agg_s; thread d walks feature d of every staged sub-group, then writes out and resets every finished
 //   block (mean / activation / LayerNorm epilogue).  Consumers and reducer hand acc_s over with two mbarriers (acc_full,
@@ -41,7 +41,8 @@ namespace ptgnn {
 namespace fused {
 
 constexpr int kD = 128;                 // message dimension handled by this kernel (= MMA M)
-constexpr int kMaxBlockTargets = 176;   // agg_s = B * 512 bytes of shared memory
+constexpr int kMaxBlockTargets = 240;   // agg_s = B * 512 bytes of shared memory (Geom in fused_mp.cu sizes the rest)
+constexpr int kMaxDefaultBlockTargets = 176;   // cap of ptgnn_b200_block_plan_block_targets and of EdgePlan's default
 
 struct Epilogue {                       // applied to the aggregated row at write-out (Mlp layers), else act = NONE / ln = null
     int act;
@@ -61,7 +62,8 @@ bool supported(int nprod, int K, int D, int use_target);
 // bytes of the packed edge weights (coalesced per-row layout), of one packed state row, and of the packed-state scratch
 size_t packed_weight_bytes(int nprod, int num_types, int K, int use_target);
 size_t packed_state_bytes(int nprod, int64_t rows, int K);
-int recommended_block_targets(int64_t num_nodes);
+// the largest B <= max_block_targets (a multiple of 8) that covers the nodes in whole waves of one CTA per SM
+int recommended_block_targets(int64_t num_nodes, int max_block_targets);
 
 // Row map of an EGC slab: packed row p = j * bases + b <- row ((o / dh) * bases + b) * dh + o % dh of the reference's
 // bases[t].weight [bases * out, K], o = col0 + j.  bases = 0: the identity (packed row p <- row p).

@@ -355,7 +355,12 @@ extern "C" int ptgnn_b200_egc_forward_fused(int32_t bf16_states, const void *nod
                      cache_valid, static_cast<cudaStream_t>(stream));
 }
 
-extern "C" int32_t ptgnn_b200_block_plan_block_targets(int64_t num_nodes) { return fused::recommended_block_targets(num_nodes); }
+extern "C" int32_t ptgnn_b200_block_plan_block_targets(int64_t num_nodes) {
+    return fused::recommended_block_targets(num_nodes, fused::kMaxDefaultBlockTargets);
+}
+extern "C" int32_t ptgnn_b200_block_plan_large_block_targets(int64_t num_nodes) {
+    return fused::recommended_block_targets(num_nodes, fused::kMaxBlockTargets);
+}
 
 extern "C" int32_t ptgnn_b200_fused_supported(int32_t bf16_states, int32_t state_dim, int32_t message_dim) {
     return tc_enabled() && gated_ok(bf16_states ? 1 : 3, state_dim, message_dim) ? 1 : 0;

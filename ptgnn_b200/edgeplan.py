@@ -24,7 +24,7 @@ class EdgePlan:
 
     __slots__ = (
         "num_nodes", "num_source_nodes", "num_edges", "num_types", "type_off", "type_off_c", "row_ptr", "src32", "tgt32", "status", "device", "_keepalive", "_validated", "_block", "_sorted", "_counts_c",
-        "_block_targets",
+        "_block_targets", "_large_blocks",
     )
 
     # status words (pinned host memory the kernels write directly, so the host can poll them without synchronising):
@@ -33,18 +33,22 @@ class EdgePlan:
     STATUS_WORDS = 4
 
     def __init__(self, adjacency_lists: Adjacency, num_nodes: int, validate: bool = False,
-                 num_source_nodes: Optional[int] = None, block_targets: Optional[int] = None):
+                 num_source_nodes: Optional[int] = None, block_targets: Optional[int] = None, large_blocks: bool = False):
         """``num_nodes`` = number of TARGET rows (CSR rows).  ``num_source_nodes`` (default: the same) bounds the source
         ids; it differs only for node-range shards, where targets are local rows and sources index the gathered states.
-        ``block_targets`` fixes the fused kernel's target-block size B (a multiple of 8 in [8, 176]); None picks
-        ``recommended_block_targets(num_nodes)``.  Results do not depend on B; tests use it to reach block layouts (many
-        blocks per CTA, small or odd half-blocks) that the recommended size would not produce for their graph."""
+        ``block_targets`` fixes the fused kernel's target-block size B (a multiple of 8 in [8, 176], or in [8, 240] with
+        ``large_blocks``); None picks ``ptgnn_b200_block_plan_block_targets(num_nodes)``, or with ``large_blocks``
+        ``ptgnn_b200_block_plan_large_block_targets(num_nodes)``.  ``plan_for`` (the layers' plan) sets ``large_blocks``: fewer,
+        larger blocks make each per-type weight load of the fused kernel serve more edges.  Results do not depend on B; tests
+        use it to reach block layouts (many blocks per CTA, small or odd half-blocks) that the recommended size would not
+        produce for their graph."""
         if block_targets is not None:
-            bt = int(block_targets)
-            if bt != block_targets or bt % 8 != 0 or not 8 <= bt <= 176:     # 176 = fused_mp.cuh kMaxBlockTargets
-                raise ValueError(f"block_targets={block_targets!r} must be a multiple of 8 in [8, 176]")
+            bt, top = int(block_targets), 240 if large_blocks else 176     # fused_mp.cuh kMaxBlockTargets / kMaxDefaultBlockTargets
+            if bt != block_targets or bt % 8 != 0 or not 8 <= bt <= top:
+                raise ValueError(f"block_targets={block_targets!r} must be a multiple of 8 in [8, {top}]")
             block_targets = bt
         self._block_targets = block_targets
+        self._large_blocks = bool(large_blocks)
         if len(adjacency_lists) > 128:
             raise NotImplementedError("more than 128 edge types")
         if len(adjacency_lists) == 0:
@@ -137,7 +141,8 @@ class EdgePlan:
             lib = N.lib()
             B = self._block_targets
             if B is None:
-                B = int(lib.ptgnn_b200_block_plan_block_targets(self.num_nodes))
+                recommend = lib.ptgnn_b200_block_plan_large_block_targets if self._large_blocks else lib.ptgnn_b200_block_plan_block_targets
+                B = int(recommend(self.num_nodes))
             nblk = (self.num_nodes + B - 1) // B
             dev = self.device
             group_off = torch.empty(nblk * self.num_types + 1, dtype=torch.int32, device=dev)
@@ -274,7 +279,7 @@ def plan_for(adjacency_lists: Adjacency, num_nodes: int, plan: Optional[EdgePlan
         _CACHE.move_to_end(key)
         hit.poll()
         return hit
-    built = EdgePlan(adjacency_lists, num_nodes, num_source_nodes=num_source_nodes)
+    built = EdgePlan(adjacency_lists, num_nodes, num_source_nodes=num_source_nodes, large_blocks=True)
     _CACHE[key] = built
     while len(_CACHE) > _CACHE_SIZE:
         _CACHE.popitem(last=False)
