@@ -126,7 +126,6 @@ int ptgnn_b200_scatter_f32(const float *src, const int64_t *index, int64_t num_e
  * through the unfused kernels (messages -> segmented reduce -> GRUCell).
  * bf16_states == 0: node_states / gather_states / out_states are fp32 [*, H].  Dimensions that fit the tensor-core tiles
  * (H % 32 == 0, D % 16 == 0) run on wgmma (3xTF32, fp32-exact); other multiples of 4 run on the FFMA kernels.
- * PTGNN_B200_DISABLE_TC=1 forces the FFMA kernels.
  * bf16_states != 0 (BASELINE.json configs[3]): the states are bf16 (raw uint16 bits); module parameters stay fp32 and are
  * converted into the workspace or the weight cache; messages and aggregates are bf16 in HBM, every accumulation (tensor-core
  * accumulators, segmented reduce, gate math) is fp32 -- the arithmetic of the reference under torch.autocast(bfloat16) (fp32
@@ -213,8 +212,7 @@ int ptgnn_b200_block_plan_build(int64_t num_nodes, int32_t num_types, const int6
                                 int32_t *src_f, uint8_t *tl_f, void *workspace, size_t workspace_bytes, void *stream);
 
 /* 1 if these dimensions run on the fused layer kernels (message_dim == 128; state_dim in {64, 128} for fp32 states,
- * {64, 128, 256} for bf16 states; 0 for every shape under PTGNN_B200_DISABLE_TC=1); otherwise use the unfused entry points
- * above. */
+ * {64, 128, 256} for bf16 states); otherwise use the unfused entry points above. */
 int32_t ptgnn_b200_fused_supported(int32_t bf16_states, int32_t state_dim, int32_t message_dim);
 
 /* GatedMessagePassingLayer.forward through the fused kernels: the fused aggregation, then the weights-stationary GRUCell.  Same

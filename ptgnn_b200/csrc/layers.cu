@@ -11,8 +11,6 @@
 //   2. segment_reduce_kernel (reduce.cuh) streaming CSR reduce = torch_scatter.scatter (+ GELU/LayerNorm for Mlp).
 //   3. gru_update_kernel     nn.GRUCell: both GEMMs ([agg;h] x packed gate weights) + gate math in one pass, or
 //      dense_update_kernel   Linear(+bias) + Tanh of the Mlp layer.
-#include <stdlib.h>
-
 #include <type_traits>
 
 #include "gemm_simt.cuh"
@@ -268,18 +266,9 @@ static int check_layer_dims(const char *who, int64_t N, int64_t E, int H, int D)
     return PTGNN_OK;
 }
 
-bool tc_enabled() {
-    static int v = -1;
-    if (v < 0) {
-        const char *e = getenv("PTGNN_B200_DISABLE_TC");
-        v = (e && e[0] == '1') ? 0 : 1;
-    }
-    return v == 1;
-}
-
 int dense_any(const float *y, int64_t rows, int D, const float *W, const float *bias, int out_dim, int act, float *out,
               void *scratch, cudaStream_t st, bool pack) {
-    if (tc_enabled() && tc::supported_dense(D, out_dim)) return tc::dense_update(y, rows, D, W, bias, out_dim, act, out, scratch, st, pack);
+    if (tc::supported_dense(D, out_dim)) return tc::dense_update(y, rows, D, W, bias, out_dim, act, out, scratch, st, pack);
     if (out_dim <= 64) return launch_dense_kernel<4>(y, rows, D, W, bias, out_dim, act, out, st);
     return launch_dense_kernel<8>(y, rows, D, W, bias, out_dim, act, out, st);
 }
@@ -287,7 +276,7 @@ int dense_any(const float *y, int64_t rows, int D, const float *W, const float *
 // =================================================================================================
 // The unfused layers: messages -> segmented reduce -> GRUCell / dense update, one host path per layer class for both state
 // dtypes (`T` = float or __nv_bfloat16).  fp32 states run on the tensor cores (3xTF32) where the dims fit the tiles and on
-// the FFMA kernels otherwise or under PTGNN_B200_DISABLE_TC=1; bf16 states always run on the tensor cores (layers_tc.cu).
+// the FFMA kernels otherwise; bf16 states always run on the tensor cores (layers_tc.cu).
 // `scratch` receives the derived weights first unless `pack` is false (a weight cache holds them).
 // =================================================================================================
 template <typename T>
@@ -295,7 +284,7 @@ static int edge_messages(const T *h_src, const T *h_tgt, int H, int D, int use_t
                          const float *const *weights, const int32_t *src32, const int32_t *tgt32, const int32_t *pos, T *msg,
                          void *scratch, bool pack, cudaStream_t st) {
     if constexpr (std::is_same<T, float>::value) {
-        if (!tc_enabled() || !tc::supported_message(H, D))
+        if (!tc::supported_message(H, D))
             return launch_edge_messages(h_src, h_tgt, H, D, use_target, num_types, type_off, weights, src32, tgt32, pos, msg, st);
     }
     return tc::edge_messages(h_src, h_tgt, H, D, use_target, num_types, type_off, weights, src32, tgt32, pos, msg, scratch, pack, st);
@@ -306,7 +295,7 @@ template <typename T>
 static int gru_update(const T *agg, const T *h, int64_t rows, int H, int D, const float *w_ih, const float *w_hh, const float *b_ih,
                       const float *b_hh, T *out, void *scratch, char *ffma_scratch, bool pack, cudaStream_t st) {
     if constexpr (std::is_same<T, float>::value) {
-        if (!tc_enabled() || !tc::supported_gru(H, D))
+        if (!tc::supported_gru(H, D))
             return launch_gru_simt(agg, h, rows, H, D, w_ih, w_hh, b_ih, b_hh, out, ffma_scratch, st);
     }
     return tc::gru_update(agg, h, rows, H, D, w_ih, w_hh, b_ih, b_hh, out, scratch, pack, st);
@@ -350,7 +339,7 @@ static GatedWs gated_layout(bool bf16, int64_t N, int64_t E, int T, int H, int D
 
 // gated weight cache: [edge weights | GRU packing]; 0 when fp32 states run a step on the FFMA kernels (nothing worth caching)
 static size_t gated_cache_bytes(bool bf16, int T, int H, int D) {
-    if (!bf16 && (!tc_enabled() || !tc::supported_message(H, D) || !tc::supported_gru(H, D))) return 0;
+    if (!bf16 && (!tc::supported_message(H, D) || !tc::supported_gru(H, D))) return 0;
     return tc::edge_weight_bytes(bf16, T, D, H) + tc::gru_pack_bytes(bf16, H, D);
 }
 

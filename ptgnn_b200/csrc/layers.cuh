@@ -4,9 +4,6 @@
 
 namespace ptgnn {
 
-// Tensor cores are the default; PTGNN_B200_DISABLE_TC=1 forces the FFMA kernels (A/B measurements, debugging).
-bool tc_enabled();
-
 // out = act(y W^T + b) with fp32 states: tensor cores (3xTF32) when the dims fit the tiles, FFMA tiles otherwise.
 // scratch >= tc::dense_weight_bytes(false, ..); pack = false when scratch is a weight cache that already holds the split of W.
 int dense_any(const float *y, int64_t rows, int D, const float *W, const float *bias, int out_dim, int act, float *out,

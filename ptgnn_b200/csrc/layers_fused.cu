@@ -15,10 +15,8 @@
 namespace ptgnn {
 namespace {
 
-// the dims the fused aggregation takes; PTGNN_B200_DISABLE_TC=1 keeps fp32 states on the FFMA kernels
-bool aggregate_ok(int nprod, int H, int D, int ut) { return (nprod == 1 || tc_enabled()) && fused::supported(nprod, H, D, ut); }
-// the gated layer also needs the weights-stationary GRU: no other GRU runs behind the fused aggregation
-bool gated_ok(int nprod, int H, int D) { return aggregate_ok(nprod, H, D, 0) && gruws::supported(nprod, H, D); }
+// the dims the fused aggregation takes that the weights-stationary GRU takes too: no other GRU runs behind the fused aggregation
+bool gated_ok(int nprod, int H, int D) { return fused::supported(nprod, H, D, 0) && gruws::supported(nprod, H, D); }
 
 // [N, D] aggregate: packed fp16 pairs (the GRU's operand) or fp32 rows for fp32 states, bf16 rows for bf16 states
 size_t agg_bytes(int nprod, int64_t N, int D) { return ws_slice((size_t)N * D * (nprod == 3 ? 4 : 2) + 16, 1); }
@@ -142,7 +140,7 @@ int mlp_fused(int nprod, const void *node_states, const void *gather_states, int
               void *weight_cache, size_t weight_cache_bytes, int cache_valid, cudaStream_t st) {
     PTGNN_CHECK_ARG(bp != nullptr, "mlp_forward_fused: null block plan");
     PTGNN_CHECK_ARG(T >= 0 && T <= PTGNN_MAX_EDGE_TYPES, "mlp_forward_fused: bad num_types=%d", T);
-    if (!aggregate_ok(nprod, H, D, ut)) {
+    if (!fused::supported(nprod, H, D, ut)) {
         set_error("mlp_forward_fused: dims H=%d D=%d are not supported by the fused kernel (%s states)", H, D, nprod == 3 ? "fp32" : "bf16");
         return PTGNN_E_UNSUPPORTED;
     }
@@ -207,7 +205,7 @@ int mlp_fused(int nprod, const void *node_states, const void *gather_states, int
 
 // ---- EGCMessagePassingLayer: S = bases * out / 128 slabs of the fused aggregation, each with the EGC write-out ----------------------
 bool egc_ok(int nprod, int H, int out, int heads, int bases) {
-    return aggregate_ok(nprod, H, fused::kD, 0) && (bases == 1 || bases == 2 || bases == 4 || bases == 8) && heads > 0 && out > 0 &&
+    return fused::supported(nprod, H, fused::kD, 0) && (bases == 1 || bases == 2 || bases == 4 || bases == 8) && heads > 0 && out > 0 &&
            out % heads == 0 && out % (fused::kD / bases) == 0 && heads * bases <= 4096;
 }
 int egc_slabs(int out, int bases) { return bases * out / fused::kD; }
@@ -363,7 +361,7 @@ extern "C" int32_t ptgnn_b200_block_plan_large_block_targets(int64_t num_nodes) 
 }
 
 extern "C" int32_t ptgnn_b200_fused_supported(int32_t bf16_states, int32_t state_dim, int32_t message_dim) {
-    return tc_enabled() && gated_ok(bf16_states ? 1 : 3, state_dim, message_dim) ? 1 : 0;
+    return gated_ok(bf16_states ? 1 : 3, state_dim, message_dim) ? 1 : 0;
 }
 
 extern "C" size_t ptgnn_b200_packed_state_bytes(int64_t num_nodes, int32_t state_dim) {
@@ -408,7 +406,7 @@ extern "C" size_t ptgnn_b200_mlp_fused_weight_cache_bytes(int32_t bf16_states, i
                                                           int32_t out_dim, int32_t use_target_state) {
     if (bf16_states || num_types <= 0 || in_dim <= 0 || message_dim <= 0) return 0;
     const int ut = use_target_state ? 1 : 0;
-    if (!aggregate_ok(3, in_dim, message_dim, ut)) return 0;
+    if (!fused::supported(3, in_dim, message_dim, ut)) return 0;
     return mlp_weight_bytes(3, num_types, in_dim, message_dim, out_dim > 0 ? out_dim : message_dim, ut);
 }
 extern "C" int ptgnn_b200_mlp_forward_fused(int32_t bf16_states, const void *node_states, const void *gather_states, int64_t num_nodes,

@@ -7,7 +7,6 @@ The reference re-derives the same information inside every layer call: it concat
 (``ptgnn_b200_plan_build``: int64->int32, degree histogram, scan, stable radix sort by target) and reused by all
 L layers (the reference's weight-shared stacks call the same layer 7-8 times on the same adjacency).
 """
-import os
 import threading
 from collections import OrderedDict
 from typing import List, Optional, Sequence, Tuple
@@ -261,8 +260,6 @@ class state_chain:
 
 
 def current_state_chain() -> Optional[state_chain]:
-    if os.environ.get("PTGNN_B200_CHAIN", "1") == "0":
-        return None
     return getattr(_TLS, "chain", None)
 
 

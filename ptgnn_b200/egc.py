@@ -9,7 +9,7 @@ per-node combination of the aggregated bases with weights from one more Linear (
   of 128, each one launch of the fused aggregation kernel whose write-out sums the bases of its output columns -- no
   ``[E, bases * out]`` message tensor.  fp32 states (3xFP16, fp32-exact) and bf16 states (bf16 output, rounded where autocast
   rounds); fp32 states train through ``autograd._EgcLayerFunction``.
-* Composed path, every other shape, and ``PTGNN_B200_FUSED=0`` / ``PTGNN_B200_FP32_MODE=tf32``: the stand-alone native kernels
+* Composed path, every other shape, and fp32 states under ``PTGNN_B200_FP32_MODE=tf32``: the stand-alone native kernels
   (``edge_messages``, ``segment_reduce``, ``linear``) and a node-sized pointwise combination.  Forward only; fp32 states.
 
 Training-mode dropout with ``p > 0`` (a mask on the gathered ``[E_t, H]`` rows, :76) has no native path and raises.
@@ -26,7 +26,8 @@ from .messagepassing import AbstractMessagePassingLayer, _check_shape, _check_st
 
 
 def use_fused(lib, bf16: bool, in_dim: int, out: int, heads: int, bases: int) -> bool:
-    """The fused slabs wherever the library takes the dimensions; the same switches as the other layers select the composed path."""
+    """The fused slabs wherever the library takes the dimensions; PTGNN_B200_FP32_MODE=tf32 selects the composed path for fp32
+    states, as it selects the round-1 path for the other layers."""
     return fused_allowed(bf16) and bool(lib.ptgnn_b200_egc_supported(int(bf16), in_dim, out, heads, bases))
 
 

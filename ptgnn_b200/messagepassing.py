@@ -52,10 +52,10 @@ def _refuse_autograd(module: nn.Module, node_states: torch.Tensor) -> None:
 
 
 def fused_allowed(bf16: bool) -> bool:
-    """The fused gather -> Linear -> reduce kernel is the default wherever it supports the dimensions.  PTGNN_B200_FUSED=0
-    selects the round-1 three-kernel path; PTGNN_B200_FP32_MODE=tf32 does so for fp32 states only (3xTF32 instead of 3xFP16:
-    needed for states / weights beyond the fp16 range)."""
-    return not (os.environ.get("PTGNN_B200_FUSED", "1") == "0" or (not bf16 and os.environ.get("PTGNN_B200_FP32_MODE", "") == "tf32"))
+    """The fused gather -> Linear -> reduce kernel runs wherever it supports the dimensions, except for fp32 states under
+    PTGNN_B200_FP32_MODE=tf32, which selects the round-1 three-kernel path (3xTF32 instead of 3xFP16: needed for states /
+    weights beyond the fp16 range)."""
+    return bf16 or os.environ.get("PTGNN_B200_FP32_MODE", "") != "tf32"
 
 
 def _use_fused(lib, bf16: bool, H: int, D: int) -> bool:

@@ -1,9 +1,11 @@
 """Shared test helpers: golden-fixture loading and conversion between the reference ``state_dict`` layout, the
 oracle's functional arguments and ptgnn_b200 modules."""
+import contextlib
 import os
 from typing import Dict, List, Tuple
 
 import numpy as np
+import pytest
 import torch
 
 GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -56,6 +58,18 @@ def assert_close(actual: torch.Tensor, expected: torch.Tensor, tol: float = TOL,
     err = (actual - expected).abs() / expected.abs().clamp(min=1.0)
     worst = float(err.max()) if err.numel() else 0.0
     assert worst <= tol, f"{what}: max scaled error {worst:.3e} > {tol:.1e}"
+
+
+@contextlib.contextmanager
+def unchained():
+    """Inside the block no layer sees a state chain (edgeplan.state_chain): every layer packs its own states.  The reference run
+    for the packed-state hand-off between layers, which must be bit-identical to it."""
+    from ptgnn_b200 import edgeplan, globalexchange, gnn, messagepassing
+
+    with pytest.MonkeyPatch.context() as mp:
+        for module in (edgeplan, messagepassing, globalexchange, gnn):   # embeddings looks it up in edgeplan at call time
+            mp.setattr(module, "current_state_chain", lambda: None)
+        yield
 
 
 def random_adjacency(gen: torch.Generator, num_nodes: int, counts, low: int = 0):

@@ -119,7 +119,7 @@ def test_no_edge_sized_message_tensor(monkeypatch):
     msg_bytes = E_ * 512 * 4
 
     def peak(fused: bool):
-        monkeypatch.setenv("PTGNN_B200_FUSED", "1" if fused else "0")
+        monkeypatch.setenv("PTGNN_B200_FP32_MODE", "" if fused else "tf32")
         plan = P.EdgePlan(adj, n)
         with torch.no_grad(), P.edgeplan.shared_plan(plan):
             layer(h, adj)                       # warm: the weight cache and the plan's arrays
@@ -150,11 +150,11 @@ def test_paths(monkeypatch):
     with pytest.raises(NotImplementedError):
         with torch.no_grad():
             layer(h.cuda().to(torch.bfloat16), adj_d)
-    # PTGNN_B200_FUSED=0 on a supported shape: the composed path, within 2e-5 of the fused result
+    # PTGNN_B200_FP32_MODE=tf32 on a supported shape: the composed path, within 2e-5 of the fused result
     layer, *_ = _layer(128, 128, 8, 4, "mean")
     h = torch.randn(n, 128, generator=torch.Generator().manual_seed(8))
     fused = _run(layer, h, adj_d, n)
-    monkeypatch.setenv("PTGNN_B200_FUSED", "0")
+    monkeypatch.setenv("PTGNN_B200_FP32_MODE", "tf32")
     assert not _uses_fused(128, 128, 8, 4)
     composed = _run(layer, h, adj_d, n)
     scale = composed.abs().max()

@@ -132,10 +132,10 @@ def test_packed_output_is_the_split_of_the_fp32_output(act):
         assert torch.equal(rows[:, 64:].view(torch.int16), lo.view(torch.int16))
 
 
-def test_first_fused_layer_takes_the_packed_output_bit_identically(monkeypatch):
+def test_first_fused_layer_takes_the_packed_output_bit_identically():
     """Embedder, then a fused gated layer in a container: the same output with and without the hand-off, one launch (the packing
     pass) fewer with it."""
-    from helpers import random_adjacency
+    from helpers import random_adjacency, unchained
 
     n, F, H = 6000, 50, 64
     gen = torch.Generator().manual_seed(9)
@@ -152,10 +152,9 @@ def test_first_fused_layer_takes_the_packed_output_bit_identically(monkeypatch):
         l0 = N.launch_count()
         chained = gnn(**kw).output_node_representations
         l1 = N.launch_count()
-        monkeypatch.setenv("PTGNN_B200_CHAIN", "0")
-        plain = gnn(**kw).output_node_representations
+        with unchained():
+            plain = gnn(**kw).output_node_representations
         l2 = N.launch_count()
-        monkeypatch.delenv("PTGNN_B200_CHAIN")
     assert torch.equal(chained, plain)
     assert (l2 - l1) - (l1 - l0) == 1, f"chained {l1 - l0} launches, unchained {l2 - l1}"
 

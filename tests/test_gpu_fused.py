@@ -147,9 +147,9 @@ def test_fused_equals_unfused_and_is_deterministic(monkeypatch):
         with torch.no_grad():
             a = layer(h, _dev(adj))
             b = layer(h, _dev(adj))
-            monkeypatch.setenv("PTGNN_B200_FUSED", "0")
+            monkeypatch.setenv("PTGNN_B200_FP32_MODE", "tf32")
             c = layer(h, _dev(adj))
-            monkeypatch.delenv("PTGNN_B200_FUSED")
+            monkeypatch.delenv("PTGNN_B200_FP32_MODE")
         assert torch.equal(a, b)
         assert_close(a, c, what=f"fused vs unfused {agg}")
 

@@ -13,7 +13,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import assert_close, gated_oracle_args
+from helpers import assert_close, gated_oracle_args, unchained
 import global_exchange_reference as GX
 from oracle import ptgnn_oracle as O
 
@@ -282,7 +282,7 @@ def _stack_inputs(N, H, T, seed):
     return h, adj, n2g
 
 
-def test_varmisuse_stack_chain_capture_and_sync_free(monkeypatch):
+def test_varmisuse_stack_chain_capture_and_sync_free():
     N, H, T = 8000, 64, 3
     h, adj, n2g = _stack_inputs(N, H, T, 5)
     gnn, layers = _varmisuse_stack(H, T, 6)
@@ -292,9 +292,8 @@ def test_varmisuse_stack_chain_capture_and_sync_free(monkeypatch):
     with torch.no_grad():
         chained = gnn.gnn(hd, adj_d, None, n2g_d, {}, {}, num_graphs=G)
         again = gnn.gnn(hd, adj_d, None, n2g_d, {}, {})                 # count read from the device instead
-        monkeypatch.setenv("PTGNN_B200_CHAIN", "0")
-        plain = gnn.gnn(hd, adj_d, None, n2g_d, {}, {}, num_graphs=G)
-        monkeypatch.delenv("PTGNN_B200_CHAIN")
+        with unchained():
+            plain = gnn.gnn(hd, adj_d, None, n2g_d, {}, {}, num_graphs=G)
     assert torch.equal(chained, again) and torch.equal(chained, plain), "chained / unchained / handed-over count runs differ"
     ref = _stack_oracle(layers, h, adj, n2g)
     err = ((chained.cpu().double() - ref).abs() / ref.abs().clamp(min=1)).max().item()

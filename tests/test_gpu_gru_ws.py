@@ -11,7 +11,7 @@ import pytest
 import torch
 
 import fused_reference as R
-from helpers import assert_close, gated_oracle_args, random_adjacency
+from helpers import assert_close, gated_oracle_args, random_adjacency, unchained
 from oracle import ptgnn_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -72,7 +72,7 @@ def test_gru_ws_bf16(N, H):
 
 @pytest.mark.parametrize("H", [64, 128])
 @pytest.mark.parametrize("N", [63, 65, 129, 64 * (33 * 3 + 5) + 17])
-def test_gru_ws_packed_output_chains_bit_identical(N, H, monkeypatch):
+def test_gru_ws_packed_output_chains_bit_identical(N, H):
     """In a container, each layer's GRU also writes its output as the packed fp16 (hi | lo') rows the next layer takes.  The
     chained run must equal the run that packs every layer's input itself, which holds only if the packed output equals
     pack_states(out) bit for bit, the rows of the partial last tile included."""
@@ -88,7 +88,6 @@ def test_gru_ws_packed_output_chains_bit_identical(N, H, monkeypatch):
     gnn = P.GraphNeuralNetwork([P.GatedMessagePassingLayer(H, D, T, "sum") for _ in range(3)], _Embed(), False, False).cuda().eval()
     with torch.no_grad():
         chained = gnn.gnn(h, adj_d, None, None, {}, {}, return_all_states=True)
-        monkeypatch.setenv("PTGNN_B200_CHAIN", "0")
-        plain = gnn.gnn(h, adj_d, None, None, {}, {}, return_all_states=True)
-        monkeypatch.delenv("PTGNN_B200_CHAIN")
+        with unchained():
+            plain = gnn.gnn(h, adj_d, None, None, {}, {}, return_all_states=True)
     assert torch.equal(chained, plain), "chained layer outputs differ from the unchained ones"

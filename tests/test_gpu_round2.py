@@ -4,7 +4,7 @@ stack with a residual layer between gated layers, inference_mode, two devices in
 import pytest
 import torch
 
-from helpers import GOLDEN_DIR, assert_close, gated_oracle_args, golden_adjacency, golden_state_dict, load_golden  # noqa: F401
+from helpers import GOLDEN_DIR, assert_close, gated_oracle_args, golden_adjacency, golden_state_dict, load_golden, unchained  # noqa: F401
 from oracle import ptgnn_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -213,7 +213,7 @@ def test_inference_mode_layer_and_container():
 
 # ---- 7. two devices in ONE process (ADVICE r1: per-device kernel attributes) ------------------------------------------------------
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two visible GPUs")
-def test_two_devices_in_one_process():
+def test_two_devices_in_one_process(monkeypatch):
     import ptgnn_b200 as P
 
     gen = torch.Generator().manual_seed(8)
@@ -223,14 +223,12 @@ def test_two_devices_in_one_process():
     h = torch.randn(n, H, generator=gen)
     outs = []
     for dev in ("cuda:0", "cuda:1"):
-        for fused in ("1", "0"):
-            import os
-            os.environ["PTGNN_B200_FUSED"] = fused
+        for mode in ("", "tf32"):                                 # the fused path, then the round-1 path
+            monkeypatch.setenv("PTGNN_B200_FP32_MODE", mode)
             torch.manual_seed(8)
             layer = P.GatedMessagePassingLayer(H, H, 1, "sum").to(dev).eval()
             with torch.no_grad():
                 outs.append(layer(h.to(dev), [(s.to(dev), t.to(dev)) for s, t in adj]).cpu())
-            os.environ.pop("PTGNN_B200_FUSED")
     assert torch.equal(outs[0], outs[2]) and torch.equal(outs[1], outs[3])
 
 
@@ -267,7 +265,7 @@ def test_captured_layer_loop_matches_eager_and_follows_its_buffers(dtype):
 
 
 # ---- 9. packed states handed from layer to layer (edgeplan.state_chain) ------------------------------------------------------------
-def test_state_chain_is_bit_identical_and_skips_the_packing_passes(monkeypatch):
+def test_state_chain_is_bit_identical_and_skips_the_packing_passes():
     """Inside a container's layer loop the GRU kernel of layer i also writes the fp16 (hi | lo') form of its output and layer i + 1
     skips its packing pass: results bit-identical to the unchained run, L - 1 fewer launches; a tensor that is not the previous
     layer's output (here: a residual sum) falls back to packing; a stand-alone layer call never chains."""
@@ -287,17 +285,15 @@ def test_state_chain_is_bit_identical_and_skips_the_packing_passes(monkeypatch):
         l0 = N.launch_count()
         chained = gnn.gnn(h, adj, None, None, {}, {})
         l1 = N.launch_count()
-        monkeypatch.setenv("PTGNN_B200_CHAIN", "0")
-        plain = gnn.gnn(h, adj, None, None, {}, {})
+        with unchained():
+            plain = gnn.gnn(h, adj, None, None, {}, {})
         l2 = N.launch_count()
-        monkeypatch.delenv("PTGNN_B200_CHAIN")
         assert torch.equal(chained, plain)
         assert (l2 - l1) - (l1 - l0) == L - 1, f"chained {l1 - l0} launches, unchained {l2 - l1}"
         # every layer's own output is the same with and without the hand-off (all states)
         a = gnn.gnn(h, adj, None, None, {}, {}, return_all_states=True)
-        monkeypatch.setenv("PTGNN_B200_CHAIN", "0")
-        b = gnn.gnn(h, adj, None, None, {}, {}, return_all_states=True)
-        monkeypatch.delenv("PTGNN_B200_CHAIN")
+        with unchained():
+            b = gnn.gnn(h, adj, None, None, {}, {}, return_all_states=True)
         assert torch.equal(a, b)
         # a layer that gets a different tensor than the previous layer's output must not use the stale packed copy
         join = P.MeanResidualLayer(128)

@@ -3,18 +3,15 @@ per element (tests/unfused_reference.py): the 3xTF32 message, GRU and dense pipe
 kernels and both segmented reduces.
 
 Operators run through their stand-alone entry points (``composed.edge_messages / segment_reduce / grucell / linear``,
-``scatter``) so that any (H, D, N) can be reached; the bf16 kernels and the reduce epilogue through layers with
-PTGNN_B200_FUSED=0 (or the fused path where it takes the shape).  Graphs come from ``unfused_reference.structured_graph``:
-per-type edge counts at the 128-edge tile boundary between large types, >= 3 waves of tiles, a hub, runs of empty rows
-placed against the streaming reduce's 16-row warp blocks, N = 0 / +-1 (mod 16) and (mod 128).  Before each call a block of
+``scatter``) so that any (H, D, N) can be reached; the bf16 kernels and the reduce epilogue through layers at shapes the
+fused kernel does not take (or the fused path where it does), fp32 layers at H = D = 128 with PTGNN_B200_FP32_MODE=tf32.  The
+shape alone picks the tensor-core or the FFMA kernels (``unfused_reference.fp32_*_mode``); the FFMA cases use shapes that fit
+no tensor-core tile.  Graphs come from ``unfused_reference.structured_graph``: per-type edge counts at the 128-edge tile
+boundary between large types, >= 3 waves of tiles, a hub, runs of empty rows placed against the streaming reduce's 16-row warp blocks, N = 0 / +-1 (mod 16) and (mod 128).  Before each call a block of
 memory is filled with NaN and freed, so that the caching allocator hands NaN back and an element no kernel wrote shows.
-Every case runs twice and must be bit-identical (no float atomics on these paths).  The FFMA kernels run again in a
-subprocess with PTGNN_B200_DISABLE_TC=1 (read once per process)."""
+Every case runs twice and must be bit-identical (no float atomics on these paths)."""
 import functools
 import math
-import os
-import subprocess
-import sys
 
 import pytest
 import torch
@@ -24,7 +21,6 @@ import unfused_reference as R
 from helpers import gated_oracle_args
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 NODES = (12800, 12801, 12799, 12816)
 ACTS = {None: None, "gelu": torch.nn.GELU, "tanh": torch.nn.Tanh, "relu": torch.nn.ReLU}
 AGGS = ("sum", "mean", "max", "min")
@@ -38,9 +34,6 @@ def _with_nodes(cases):
     out = [tuple(c) + (NODES[i % len(NODES)],) for i, c in enumerate(cases)]
     assert {n % 128 for *_, n in out} >= ({0, 1, 127} if len(out) >= 4 else {0, 1})
     return out
-
-
-ffma_only = pytest.mark.skipif(R.tc_enabled(), reason="FFMA shapes: run by test_ffma_kernels_in_subprocess")
 
 
 @functools.lru_cache(maxsize=4)
@@ -91,10 +84,6 @@ def _states(N, H, seed, scale=1.0):
     return torch.randn(N, H, generator=torch.Generator().manual_seed(seed)) * scale
 
 
-def _mode_tag():
-    return "tc" if R.tc_enabled() else "ffma"
-
-
 # ---- fp32 messages ---------------------------------------------------------------------------------------------------
 MSG = _with_nodes([(32, 16, False), (36, 48, True), (44, 112, True), (100, 144, True), (128, 240, False), (132, 272, True),
                    (256, 512, False), (36, 512, False)])
@@ -123,7 +112,6 @@ def test_fp32_messages(H, D, ut, N):
 FFMA_MSG = _with_nodes([(36, 20, True), (44, 36, False), (100, 68, True), (4, 100, False), (132, 260, False)])
 
 
-@ffma_only
 @pytest.mark.parametrize("H,D,ut,N", FFMA_MSG)
 def test_ffma_messages(H, D, ut, N):
     _fp32_messages_case(H, D, ut, N, H + D)
@@ -216,8 +204,7 @@ EPI = _with_nodes([(16, None, "sum"), (32, "gelu", "mean"), (48, "tanh", "max"),
 
 
 @pytest.mark.parametrize("D,act,agg,N", EPI, ids=[f"D{d}-{a}-{g}-N{n}" for d, a, g, n in EPI])
-def test_fp32_reduce_epilogue_layer_norm(monkeypatch, D, act, agg, N):
-    monkeypatch.setenv("PTGNN_B200_FUSED", "0")
+def test_fp32_reduce_epilogue_layer_norm(D, act, agg, N):
     adj, adj_d = _graph(N)
     H, ut = 64, D % 32 == 0
     layer, w, extra = _mlp(H, D, D, len(adj), agg, ut, act=act, ln=True, seed=D)
@@ -227,17 +214,16 @@ def test_fp32_reduce_epilogue_layer_norm(monkeypatch, D, act, agg, N):
     _, bnd, pre = FR.aggregate(tgt, m, err, N, agg, False)
     x, bx = FR.activation_bound(pre, bnd, act)
     y, by = R.layer_norm(x, bx, *extra["ln"], 1e-5)
-    _check(got, y, by, f"fp32 reduce+LayerNorm ({_mode_tag()})", f"LayerNorm D={D} act={act} {agg}")
+    _check(got, y, by, f"fp32 reduce+LayerNorm ({R.fp32_message_mode(H, D)})", f"LayerNorm D={D} act={act} {agg}")
 
 
 # ---- bf16 messages + bf16 streaming reduce ---------------------------------------------------------------------------
-BF16_MSG = _with_nodes([(64, 64, "sum"), (64, 80, "mean"), (128, 112, "sum"), (64, 128, "max"), (128, 144, "min"),
+BF16_MSG = _with_nodes([(64, 64, "sum"), (64, 80, "mean"), (128, 112, "sum"), (96, 128, "max"), (128, 144, "min"),
                         (64, 176, "sum"), (128, 240, "mean"), (64, 256, "max")])
 
 
 @pytest.mark.parametrize("H,D,agg,N", BF16_MSG, ids=[f"H{h}-D{d}-{a}-N{n}" for h, d, a, n in BF16_MSG])
-def test_bf16_messages_and_reduce(monkeypatch, H, D, agg, N):
-    monkeypatch.setenv("PTGNN_B200_FUSED", "0")
+def test_bf16_messages_and_reduce(H, D, agg, N):
     adj, adj_d = _graph(N)
     ut = D % 32 == 16
     layer, w, _ = _mlp(H, D, D, len(adj), agg, ut, seed=D + 1)
@@ -252,8 +238,7 @@ BF16_EPI = _with_nodes([(64, 112, "gelu", "sum"), (128, 176, "tanh", "max"), (64
 
 
 @pytest.mark.parametrize("H,D,act,agg,N", BF16_EPI, ids=[f"H{h}-D{d}-{a}-{g}-N{n}" for h, d, a, g, n in BF16_EPI])
-def test_bf16_reduce_epilogue_layer_norm(monkeypatch, H, D, act, agg, N):
-    monkeypatch.setenv("PTGNN_B200_FUSED", "0")
+def test_bf16_reduce_epilogue_layer_norm(H, D, act, agg, N):
     adj, adj_d = _graph(N)
     ut = D % 32 == 0
     layer, w, extra = _mlp(H, D, D, len(adj), agg, ut, act=act, ln=True, seed=D + 3)
@@ -294,8 +279,7 @@ def test_fp32_gru(H, D, N):
     _fp32_gru_case(H, D, N, H + D + N)
 
 
-@ffma_only
-@pytest.mark.parametrize("H,D,N", [(32, 20, 129), (64, 100, 127), (96, 36, 12800)])
+@pytest.mark.parametrize("H,D,N", [(32, 20, 129), (64, 28, 127), (96, 12, 12800)])   # D < 32: the FFMA GRU
 def test_ffma_gru(H, D, N):
     _fp32_gru_case(H, D, N, H + D)
 
@@ -305,10 +289,9 @@ BF16_GRU = _with_nodes([(64, 112, "sum"), (96, 176, "max"), (160, 240, "mean"), 
 
 
 @pytest.mark.parametrize("H,D,agg,N", BF16_GRU, ids=[f"H{h}-D{d}-{a}-N{n}" for h, d, a, n in BF16_GRU])
-def test_bf16_gated_layer(monkeypatch, H, D, agg, N):
+def test_bf16_gated_layer(H, D, agg, N):
     import ptgnn_b200 as P
 
-    monkeypatch.setenv("PTGNN_B200_FUSED", "0")
     adj, adj_d = _graph(N)
     torch.manual_seed(H)
     layer = P.GatedMessagePassingLayer(H, D, len(adj), agg).cuda().eval()
@@ -349,24 +332,21 @@ def test_fp32_dense(D, Hout, bias, act, N):
     _fp32_dense_case(D, Hout, bias, act, N, D + Hout)
 
 
-@ffma_only
 @pytest.mark.parametrize("D,Hout,N", _with_nodes([(20, 68), (36, 100), (4, 36), (100, 4)]))
 def test_ffma_dense(D, Hout, N):
     _fp32_dense_case(D, Hout, True, "gelu", N, D + Hout + 1)
 
 
-# ---- bf16 dense (Mlp layer with a dense layer; fused aggregation at D = 128, and unfused) --------------------------------
+# ---- bf16 dense (Mlp layer with a dense layer at D = 128: fused aggregation at H = 64, unfused at H = 96) -------------------
 BF16_DENSE = _with_nodes([(64, True, "sum"), (112, True, "max"), (112, False, "sum"), (176, False, "max"), (240, True, "max"),
                           (240, False, "sum"), (304, True, "sum"), (304, False, "max")])
 
 
 @pytest.mark.parametrize("Hout,fused,agg,N", BF16_DENSE,
                          ids=[f"Hout{h}-{'fused' if f else 'unfused'}-{a}-N{n}" for h, f, a, n in BF16_DENSE])
-def test_bf16_dense(monkeypatch, Hout, fused, agg, N):
-    if not fused:
-        monkeypatch.setenv("PTGNN_B200_FUSED", "0")
+def test_bf16_dense(Hout, fused, agg, N):
     adj, adj_d = _graph(N)
-    H, D = 64, 128
+    H, D = 64 if fused else 96, 128
     layer, w, extra = _mlp(H, D, Hout, len(adj), agg, True, dense=True, dense_act="tanh", seed=Hout)
     h = _states(N, H, Hout).to(torch.bfloat16)
     got = _layer_run(layer, h, adj_d, _msg_bytes(N, 60_000, max(D, Hout), True))
@@ -376,16 +356,17 @@ def test_bf16_dense(monkeypatch, Hout, fused, agg, N):
 
 
 # ---- fp32 layers on the structured graph: bounds composed from the operator bounds --------------------------------------
-GATED = _with_nodes([(env, agg) for env in (("PTGNN_B200_FUSED", "0"), ("PTGNN_B200_FP32_MODE", "tf32")) for agg in ("sum", "max")])
+# H = D = 128 (the fused kernel's shape) on the 3xTF32 kernels under PTGNN_B200_FP32_MODE=tf32; D = 20: FFMA messages and GRU
+GATED = _with_nodes([(128, 128, True, agg) for agg in AGGS] + [(64, 20, False, "sum")])
 
 
-@pytest.mark.parametrize("env,agg,N", GATED, ids=[f"{e[0]}={e[1]}-{a}-N{n}" for e, a, n in GATED])
-def test_fp32_layers_gated(monkeypatch, env, agg, N):
+@pytest.mark.parametrize("H,D,tf32,agg,N", GATED, ids=[f"H{h}-D{d}{'-tf32' if t else ''}-{a}-N{n}" for h, d, t, a, n in GATED])
+def test_fp32_layers_gated(monkeypatch, H, D, tf32, agg, N):
     import ptgnn_b200 as P
 
-    monkeypatch.setenv(*env)
+    if tf32:
+        monkeypatch.setenv("PTGNN_B200_FP32_MODE", "tf32")
     adj, adj_d = _graph(N)
-    H, D = 128, 128
     torch.manual_seed(7)
     layer = P.GatedMessagePassingLayer(H, D, len(adj), agg).cuda().eval()
     args = gated_oracle_args({k: v.detach().cpu() for k, v in layer.state_dict().items()})
@@ -395,12 +376,13 @@ def test_fp32_layers_gated(monkeypatch, env, agg, N):
     _, bnd, pre = FR.aggregate(tgt, m, err, N, agg, False)
     ref, bound = R.gru(pre.cuda(), bnd.cuda(), h.cuda(), args["gru_w_ih"], args["gru_w_hh"], args["gru_b_ih"], args["gru_b_hh"],
                        mode=R.fp32_gru_mode(H, D))
-    _check(got, ref, bound, f"fp32 gated layer ({_mode_tag()})", f"gated {env[0]}={env[1]} {agg}")
+    _check(got, ref, bound, f"fp32 gated layer ({R.fp32_message_mode(H, D)})", f"gated H={H} D={D} tf32={tf32} {agg}")
 
 
-@pytest.mark.parametrize("H,D,Hout,agg,N", _with_nodes([(64, 112, 144, "mean"), (36, 128, 48, "min"), (64, 64, 112, "max")]))
-def test_fp32_layers_mlp(monkeypatch, H, D, Hout, agg, N):
-    monkeypatch.setenv("PTGNN_B200_FUSED", "0")
+# the last case: FFMA messages (D % 16 != 0) and FFMA dense (Hout % 16 != 0)
+@pytest.mark.parametrize("H,D,Hout,agg,N", _with_nodes([(64, 112, 144, "mean"), (36, 128, 48, "min"), (64, 64, 112, "max"),
+                                                        (36, 36, 100, "sum")]))
+def test_fp32_layers_mlp(H, D, Hout, agg, N):
     adj, adj_d = _graph(N)
     layer, w, extra = _mlp(H, D, Hout, len(adj), agg, True, act="gelu", ln=True, dense=True, dense_act="tanh", seed=H + D)
     h = _states(N, H, H + D)
@@ -410,18 +392,7 @@ def test_fp32_layers_mlp(monkeypatch, H, D, Hout, agg, N):
     x, bx = FR.activation_bound(pre, bnd, "gelu")
     y, by = R.layer_norm(x, bx, *extra["ln"], 1e-5)
     ref, bound = R.dense(y.cuda(), by.cuda(), *extra["dense"], "tanh", R.fp32_dense_mode(D, Hout))
-    _check(got, ref, bound, f"fp32 Mlp layer ({_mode_tag()})", f"Mlp H={H} D={D} Hout={Hout} {agg}")
-
-
-# ---- the FFMA kernels ----------------------------------------------------------------------------------------------------
-@pytest.mark.skipif(not R.tc_enabled(), reason="already running on the FFMA kernels")
-def test_ffma_kernels_in_subprocess():
-    env = dict(os.environ, PTGNN_B200_DISABLE_TC="1")
-    r = subprocess.run([sys.executable, "-m", "pytest", os.path.relpath(__file__, ROOT), "-q", "-s", "-m", "gpu", "-p", "no:cacheprovider",
-                        "-k", "ffma or fp32_messages or fp32_gru or fp32_dense or fp32_layers or fp32_reduce_epilogue or zz_report"],
-                       cwd=ROOT, env=env, capture_output=True, text=True, timeout=1200)
-    print("\n".join(line for line in r.stdout.splitlines() if line.startswith("worst")))
-    assert r.returncode == 0, r.stdout[-4000:] + r.stderr[-2000:]
+    _check(got, ref, bound, f"fp32 Mlp layer ({R.fp32_message_mode(H, D)})", f"Mlp H={H} D={D} Hout={Hout} {agg}")
 
 
 def test_zz_report_worst_ratios():

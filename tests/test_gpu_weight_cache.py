@@ -29,12 +29,9 @@ def test_weight_cache_reuse_and_invalidation(dtype):
         out_hit = layer(h, adj)             # reuses them
         l2 = N.launch_count()
     assert torch.equal(out_fill, out_hit)
-    # fused path: edge-weight packing + GRU gate-block packing, exactly (2 launches); round-1 path (PTGNN_B200_FUSED=0): 3 launches
-    import os
-    if os.environ.get("PTGNN_B200_FUSED", "1") == "0":
-        assert (l2 - l1) == (l1 - l0) - 3, "the cached call must skip exactly the three weight-derivation launches"
-    else:   # fused path: a cached call launches only the compute kernels -- (state packing,) fused aggregation, GRU
-        assert (l2 - l1) == (3 if dtype == torch.float32 else 2) and (l1 - l0) == (l2 - l1) + 2
+    # a cached call launches only the compute kernels -- (state packing,) fused aggregation, GRU -- and skips exactly the two
+    # weight-derivation launches: edge-weight packing and GRU gate-block packing
+    assert (l2 - l1) == (3 if dtype == torch.float32 else 2) and (l1 - l0) == (l2 - l1) + 2
 
     # in-place update (what load_state_dict / an optimiser step does): the cache must not be used
     with torch.no_grad():

@@ -51,7 +51,6 @@ Then h' = (1 - z) n + z h moves by |1 - z| dn + dz (|n - h| + dn) plus 3u (|(1 -
 Every GRU and LayerNorm bound is widened by 2 % for the second-order terms dropped above.
 """
 import math
-import os
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -64,10 +63,6 @@ ABS_TF32 = 2.0 ** -100
 SM_COUNT = 132                      # H100 SXM: the persistent pipelines launch one CTA per SM
 TILE_M = 128                        # edges / rows per tile of the tensor-core pipelines
 WARP_ROWS = 16                      # target rows per warp of the streaming reduce
-
-
-def tc_enabled() -> bool:
-    return os.environ.get("PTGNN_B200_DISABLE_TC", "") != "1"
 
 
 def gamma(n) -> float:
@@ -93,15 +88,15 @@ def gemm_constant(mode: str, *Ks: int) -> float:
 
 def fp32_message_mode(H: int, D: int) -> str:
     """Which kernel computes fp32 messages (layers.cu edge_messages; tc::supported_message)."""
-    return "tc" if tc_enabled() and H % 4 == 0 and D % 16 == 0 and H >= 32 and D >= 16 else "ffma"
+    return "tc" if H % 4 == 0 and D % 16 == 0 and H >= 32 and D >= 16 else "ffma"
 
 
 def fp32_gru_mode(H: int, D: int) -> str:
-    return "tc" if tc_enabled() and H % 32 == 0 and D % 4 == 0 and D >= 32 else "ffma"
+    return "tc" if H % 32 == 0 and D % 4 == 0 and D >= 32 else "ffma"
 
 
 def fp32_dense_mode(D: int, Hout: int) -> str:
-    return "tc" if tc_enabled() and D % 4 == 0 and Hout % 16 == 0 and D >= 32 else "ffma"
+    return "tc" if D % 4 == 0 and Hout % 16 == 0 and D >= 32 else "ffma"
 
 
 _bf16 = FR._bf16

@@ -76,17 +76,18 @@ def kernel_time(fn, calls=10):
     return {k: {"ms_per_call": v[0] / calls, "launches_per_call": v[1] / calls} for k, v in kt.items() if v[1]}
 
 
-def with_env(value, fn):
+def with_fp32_mode(value, fn):
+    """fn under PTGNN_B200_FP32_MODE=value: "tf32" selects the composed path for fp32 states, "" the fused slabs."""
     def run():
-        old = os.environ.get("PTGNN_B200_FUSED")
-        os.environ["PTGNN_B200_FUSED"] = value
+        old = os.environ.get("PTGNN_B200_FP32_MODE")
+        os.environ["PTGNN_B200_FP32_MODE"] = value
         try:
             return fn()
         finally:
             if old is None:
-                del os.environ["PTGNN_B200_FUSED"]
+                del os.environ["PTGNN_B200_FP32_MODE"]
             else:
-                os.environ["PTGNN_B200_FUSED"] = old
+                os.environ["PTGNN_B200_FP32_MODE"] = old
     return run
 
 
@@ -103,10 +104,10 @@ def case(name, batch, agg, calls):
     with torch.no_grad(), P.edgeplan.shared_plan(plan):
         for dtype in ("fp32", "bf16"):
             h = h32 if dtype == "fp32" else h32.to(torch.bfloat16)
-            fused = with_env("1", lambda: layer(h, adj))
+            fused = with_fp32_mode("", lambda: layer(h, adj))
             r = {}
             if dtype == "fp32":
-                composed = with_env("0", lambda: layer(h, adj))
+                composed = with_fp32_mode("tf32", lambda: layer(h, adj))
                 tf, tc = time_alternating([fused, composed], calls)
                 r["fused_forward"], r["composed_forward"] = tf, tc
                 a, b = fused(), composed()

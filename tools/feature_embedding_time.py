@@ -8,12 +8,13 @@ and bf16 (autocast).  Per shape and dtype:
 * the module's eval forward and the library's F.linear + ReLU (TF32 off for fp32: true fp32; bf16 under autocast), CUDA events around
   each call, calls alternating between the variants;
 * fp32: a container of the embedder and one fused gated layer (message dimension 128, 3 edge types, 4 N edges each), with and without the packed hand-off
-  (PTGNN_B200_CHAIN=0), alternating: the difference is what the first layer saves by skipping its packing pass.
+  (``current_state_chain`` replaced by ``lambda: None``), alternating: the difference is what the first layer saves by skipping its packing pass.
 Times are the median and the 10th / 90th percentile.  The card's name, power limit and max SM clock are read in the same run.
 
     python tools/feature_embedding_time.py [--calls 50] [--out /tmp/feature_embedding_time.json]
 """
 import argparse
+import contextlib
 import json
 import os
 import statistics
@@ -26,6 +27,7 @@ import torch.nn.functional as F_
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import ptgnn_b200 as P  # noqa: E402
 from ptgnn_b200 import _native as N  # noqa: E402
+from ptgnn_b200 import edgeplan, globalexchange, gnn as gnn_module, messagepassing  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12
 SHAPES = {"ppi": (44_906, 50, 64), "large": (200_000, 128, 128)}
@@ -72,6 +74,20 @@ def kernel_ms(f, calls):
         per_call.append(ms)
     N.kernel_timing(False)
     return stats(per_call)
+
+
+@contextlib.contextmanager
+def no_state_chain():
+    """Inside the block no layer sees a state chain: every layer packs its own input states."""
+    modules = (edgeplan, messagepassing, globalexchange, gnn_module)
+    current = edgeplan.current_state_chain
+    for module in modules:
+        module.current_state_chain = lambda: None
+    try:
+        yield
+    finally:
+        for module in modules:
+            module.current_state_chain = current
 
 
 def fmt(t):
@@ -128,18 +144,13 @@ def main():
                 gnn(**kw)
 
         def unchained():
-            os.environ["PTGNN_B200_CHAIN"] = "0"
-            try:
-                with torch.no_grad():
-                    gnn(**kw)
-            finally:
-                del os.environ["PTGNN_B200_CHAIN"]
+            with torch.no_grad(), no_state_chain():
+                gnn(**kw)
 
         with torch.no_grad():
             with_handoff = gnn(**kw).output_node_representations
-            os.environ["PTGNN_B200_CHAIN"] = "0"
-            without = gnn(**kw).output_node_representations
-            del os.environ["PTGNN_B200_CHAIN"]
+            with no_state_chain():
+                without = gnn(**kw).output_node_representations
             same = torch.equal(with_handoff, without)
         c = time_alternating([chained, unchained], args.calls)
         row["container_fp32"] = {"chained_ms": c[0], "unchained_ms": c[1], "saved_ms": c[1][0] - c[0][0], "bit_identical": same}

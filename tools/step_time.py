@@ -1,5 +1,5 @@
 """Whole-step time of the config-2 layer loop (8 GatedMessagePassingLayers, plan build included, states resident), CUDA events:
-    [PTGNN_TOOLS_LIB=tools/_variants/lib....so] [PTGNN_B200_CHAIN=0] python tools/step_time.py [f32|bf16] [label]
+    [PTGNN_TOOLS_LIB=tools/_variants/lib....so] python tools/step_time.py [f32|bf16] [label]
 A/B tool: variants of the library are timed on the SAME box in one session (box-to-box spread is several percent)."""
 import os
 import sys
@@ -12,16 +12,21 @@ import torch  # noqa: E402
 
 from ptgnn_b200 import _native as N  # noqa: E402
 
+chain = True
 if os.environ.get("PTGNN_TOOLS_LIB"):
     N.LIB_PATH = os.path.join(ROOT, os.environ["PTGNN_TOOLS_LIB"])
     probe = ctypes.CDLL(N.LIB_PATH)
     for name in list(N.SIGNATURES):          # older builds lack the newest entry points
         if not hasattr(probe, name):
             del N.SIGNATURES[name]
-            os.environ["PTGNN_B200_CHAIN"] = "0"
+            chain = False
 import ptgnn_b200 as P  # noqa: E402
+from ptgnn_b200 import edgeplan, globalexchange, gnn as gnn_module, messagepassing  # noqa: E402
 from ptgnn_b200.synthetic import graph2class_batch  # noqa: E402
 
+if not chain:                                   # older builds: no packed-state hand-off between layers
+    for module in (edgeplan, messagepassing, globalexchange, gnn_module):
+        module.current_state_chain = lambda: None
 dtype = sys.argv[1] if len(sys.argv) > 1 else "f32"
 label = sys.argv[2] if len(sys.argv) > 2 else ""
 b = graph2class_batch()
@@ -68,4 +73,4 @@ with torch.no_grad():
 kt = N.read_kernel_timing()
 N.kernel_timing(False)
 print("   kernels: " + "  ".join(f"{k} {v[0] / max(v[1], 1):.4f} ms x{v[1] // 5}" for k, v in kt.items() if v[1]))
-print(f"{dtype} chain={os.environ.get('PTGNN_B200_CHAIN', '1')} {label}: step median {times[len(times) // 2]:.3f} ms  min {times[0]:.3f}  p90 {times[17]:.3f}")
+print(f"{dtype} chain={int(chain)} {label}: step median {times[len(times) // 2]:.3f} ms  min {times[0]:.3f}  p90 {times[17]:.3f}")
