@@ -676,6 +676,31 @@ int ptgnn_b200_decode_select(const float *logits, int64_t num_graphs, int32_t vo
                              void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Beam search of graph2seq's decoder, one decoder step (DESIGN.md §3.19).  Each graph g has K = beam_width slots; a slot is live, done
+ * or empty.  Row g·K + k of logits [G·K, V], column k of copy_scores [M, K] and lse_copy [G, K] belong to slot k of graph g.  Group
+ * tables as for ptgnn_b200_decode_select.
+ *   Candidates: a live slot's dictionary is greedy decoding's (decode_select) for its row; an entry's total is fl(total + score) in
+ *   fp32, and its K best entries in greedy's order are kept.  A done slot has one candidate, itself, total unchanged.  An empty slot has
+ *   none.  Per graph the K best candidates by (total descending, slot ascending, the order within the slot) become the new slots in
+ *   that order; a selected END (or a done slot) makes the new slot done; if fewer than K exist, the rest are empty.
+ *   state (int32, in/out, G·K·(2·max_len + 4) words): backpointers [max_len][G][K] (the parent slot; -1 for an empty slot), keys
+ *   [max_len][G][K] (the selected key; -1 for a done slot passing through or an empty slot), totals [G][K] fp32, lengths [G][K], done
+ *   flags [G][K], empty flags [G][K].  At step 0 the state is read as: slot 0 live with total 0 and length 0, the others empty.
+ *   next_ids [G·K] int64 (out): the key when below V, unk_id for a copy outside the vocabulary, end_id for a done or empty slot.
+ *   gather_idx [G·K] int64 (out): g·K + parent slot (an empty slot: itself), the row each slot's hidden state comes from.
+ *   Workspace: ptgnn_b200_beam_select_workspace_bytes(G, V, K) bytes; after the call it starts with Z [G][K] fp32 (NaN for a slot that
+ *   was not live).  Two launches; no host synchronisation, no float atomics: deterministic.
+ *   Supported (ptgnn_b200_beam_select_supported): V in [1, 65536], K in [1, 8]; otherwise PTGNN_E_UNSUPPORTED.
+ * ---------------------------------------------------------------------------------------------- */
+int32_t ptgnn_b200_beam_select_supported(int32_t vocab, int32_t beam_width);
+size_t ptgnn_b200_beam_select_workspace_bytes(int64_t num_graphs, int32_t vocab, int32_t beam_width);
+int ptgnn_b200_beam_select(const float *logits, int64_t num_graphs, int32_t vocab, int32_t beam_width, const float *copy_scores,
+                           int64_t num_rows, const float *lse_copy, const int32_t *group_ptr, const int32_t *group_key,
+                           const int32_t *member_ptr, const int32_t *member_rows, int32_t end_id, int32_t unk_id, int32_t step,
+                           int32_t max_len, int32_t *state, int64_t *next_ids, int64_t *gather_idx, void *workspace,
+                           size_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Host-buffer convenience entry point (used for the end-to-end measurement): all pointers are HOST
  * memory; copies inputs to the device, builds the plan, runs `num_layers` GatedMessagePassingLayers
  * (layer l uses weight set l; pass the same pointers to share weights), copies the final states back

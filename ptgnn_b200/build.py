@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libptgnn_b200.so")
-SOURCES = ["capi.cu", "plan.cu", "reduce.cu", "layers.cu", "layers_tc.cu", "layers_fused.cu", "fused_mp.cu", "gru_ws.cu", "batching.cu", "gru_grad.cu", "readout.cu", "attn_readout.cu", "selfatt.cu", "graphnorm.cu", "pna.cu", "copy_attn.cu", "embedding.cu", "char_cnn.cu", "feature_embed.cu", "heads.cu", "classify.cu", "decode_select.cu"]
+SOURCES = ["capi.cu", "plan.cu", "reduce.cu", "layers.cu", "layers_tc.cu", "layers_fused.cu", "fused_mp.cu", "gru_ws.cu", "batching.cu", "gru_grad.cu", "readout.cu", "attn_readout.cu", "selfatt.cu", "graphnorm.cu", "pna.cu", "copy_attn.cu", "embedding.cu", "char_cnn.cu", "feature_embed.cu", "heads.cu", "classify.cu", "decode_select.cu", "beam_select.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",

@@ -61,7 +61,12 @@ factories import the layer classes by module path (`implementations/typilus/trai
 17. with ``native_greedy_decode=True`` only: replaces the method ``greedy_decode`` of the reference's ``GruCopyingDecoderModel`` with
    ``ptgnn_b200.decoding.greedy_decode`` (the decode loop on the device, DESIGN.md §3.18), which takes the same arguments and returns
    the same result.  It works with the reference's decoder module and with the native one, so it does not need ``native_decoder``.  The
-   default leaves the reference's method in place.
+   default leaves the reference's method in place,
+18. with ``native_beam_decode=True`` only: adds a method ``beam_decode`` to the reference's ``GruCopyingDecoderModel`` (the arguments of
+   ``greedy_decode`` plus ``beam_width``; ``ptgnn_b200.decoding.beam_decode``, beam search on the device, DESIGN.md §3.19) and a method
+   ``beam_decode(data, trained_network, device, beam_width)`` to the reference's ``Graph2Seq`` (``ptgnn.implementations.graph2seq
+   .graph2seq``), which walks the data in minibatches of 50 as its ``greedy_decode`` does and returns, per datapoint, the hypotheses
+   best first.  The reference has no beam search, so the default adds nothing and ``uninstall()`` removes both methods.
 
 After ``install()``: ``import ptgnn.implementations.ppi.train`` etc. build ptgnn_b200 layers, unchanged.  ``uninstall()``
 restores the reference's classes.  The reference must be importable as ``ptgnn`` for steps 2-4 (it is not on the GPU test box;
@@ -71,6 +76,8 @@ import importlib
 import sys
 import types
 from typing import Dict
+
+import torch
 
 from . import globalexchange as _gx
 from . import gnn as _gnn
@@ -105,6 +112,8 @@ _GRAPH2CLASS_CLASS = "Graph2ClassModule"
 _PPI_MODULE = "ptgnn.implementations.ppi.ppi"
 _PPI_CLASS = "PPIClassification"
 _GREEDY_DECODE = "GruCopyingDecoderModel.greedy_decode"
+_GRAPH2SEQ_MODULE = "ptgnn.implementations.graph2seq.graph2seq"
+_BEAM_DECODE = "beam_decode"         # _saved[_BEAM_DECODE]: the classes the method was added to
 _saved: Dict[str, object] = {}
 
 
@@ -219,6 +228,47 @@ def _install_native_greedy_decode() -> None:
         model.greedy_decode = _native_greedy_decode
 
 
+def _native_beam_decode(self, *, input_concrete_values, input_memories, input_memories_origin_idx, initial_states, neural_model,
+                        beam_width):
+    from . import decoding as _decoding
+
+    return _decoding.beam_decode(self, input_concrete_values=input_concrete_values, input_memories=input_memories,
+                                 input_memories_origin_idx=input_memories_origin_idx, initial_states=initial_states,
+                                 neural_model=neural_model, beam_width=beam_width)
+
+
+def _graph2seq_beam_decode(self, data, trained_network, device, beam_width):
+    """Beam search over ``data`` (CodeGraph2Seq datapoints): per minibatch of up to 50, the GNN, the initial decoder states and the
+    backbone memories of ``trained_network``, then the decoder model's ``beam_decode``.  Returns one list of (tokens, fp32 total) per
+    datapoint, best first."""
+    decoder_model = self._Graph2Seq__decoder_model
+    results = []
+    batches = self.minibatch_iterator(self.tensorize_dataset(iter(data), return_input_data=True), device, max_minibatch_size=50)
+    for mb_data, samples in batches:
+        values = [s["node_labels"][i].lower() for s in samples for i in s["backbone_sequence"]]
+        with torch.no_grad():
+            out = trained_network._gnn(**mb_data["encoder_mb_data"])
+            backbone = out.node_idx_references["backbone_nodes"]
+            results.extend(decoder_model.beam_decode(
+                input_concrete_values=values, input_memories=out.output_node_representations[backbone],
+                input_memories_origin_idx=out.node_graph_idx_reference["backbone_nodes"],
+                initial_states=trained_network._get_initial_decoder_states(out), neural_model=trained_network._decoder,
+                beam_width=beam_width))
+    if len(results) != len(data):
+        raise ValueError(f"beam_decode: {len(data)} datapoints but {len(results)} were decoded (some could not be tensorized)")
+    return results
+
+
+def _install_native_beam_decode() -> None:
+    targets = ((importlib.import_module(_DECODER_MODULE).GruCopyingDecoderModel, _native_beam_decode),
+               (importlib.import_module(_GRAPH2SEQ_MODULE).Graph2Seq, _graph2seq_beam_decode))
+    added = _saved.setdefault(_BEAM_DECODE, [])
+    for cls, method in targets:
+        if _BEAM_DECODE not in cls.__dict__:
+            cls.beam_decode = method
+            added.append(cls)
+
+
 def _install_native_embedders(names=_NATIVE_EMBEDDERS) -> None:
     from . import embeddings as _emb
 
@@ -267,11 +317,12 @@ def install(force_torch_scatter: bool = False, native_reducers: bool = False, na
             native_graphnorm: bool = False, native_pna: bool = False, native_decoder: bool = False,
             native_embedders: bool = False, native_char_embedder: bool = False, native_egc: bool = False,
             native_feature_embedder: bool = False, native_heads: bool = False, native_graph2class_head: bool = False,
-            native_ppi_head: bool = False, native_greedy_decode: bool = False) -> Dict[str, object]:
+            native_ppi_head: bool = False, native_greedy_decode: bool = False, native_beam_decode: bool = False) -> Dict[str, object]:
     report: Dict[str, object] = {"torch_scatter": "real", "layers": False, "container": False, "metrics": False, "reducers": False,
                                  "selfattention": False, "graphnorm": False, "pna": False, "decoder": False, "embedders": False,
                                  "char_embedder": False, "egc": False, "feature_embedder": False,
-                                 "heads": False, "graph2class_head": False, "ppi_head": False, "greedy_decode": False}
+                                 "heads": False, "graph2class_head": False, "ppi_head": False, "greedy_decode": False,
+                                 "beam_decode": False}
     previous_scatter = {name: sys.modules.get(name) for name in ("torch_scatter", "torch_scatter.composite")}
     # 1. torch_scatter
     have_real = False
@@ -368,6 +419,10 @@ def install(force_torch_scatter: bool = False, native_reducers: bool = False, na
     if native_greedy_decode:
         _install_native_greedy_decode()
         report["greedy_decode"] = True
+    # 18. GruCopyingDecoderModel.beam_decode and Graph2Seq.beam_decode (opt-in)
+    if native_beam_decode:
+        _install_native_beam_decode()
+        report["beam_decode"] = True
     return report
 
 
@@ -383,6 +438,10 @@ def uninstall() -> None:
         elif key == _GREEDY_DECODE:
             model, method = val
             model.greedy_decode = method
+        elif key == _BEAM_DECODE:
+            for cls in val:
+                if _BEAM_DECODE in cls.__dict__:
+                    delattr(cls, _BEAM_DECODE)
         elif ":" in key:
             mod_name, attr = key.split(":", 1)
             if mod_name in sys.modules:
