@@ -13,8 +13,8 @@ import pytest
 import torch
 
 import fused_reference as R
-from helpers import assert_close, gated_oracle_args
-from oracle import ptgnn_oracle as O
+import unfused_reference as UR
+from helpers import gated_oracle_args
 
 pytestmark = pytest.mark.gpu
 
@@ -178,8 +178,8 @@ LN = [(bf16, act, agg) for bf16 in (False, True) for act, agg in ((None, "sum"),
 
 @pytest.mark.parametrize("bf16,act,agg", LN, ids=[f"{'bf16' if b else 'fp32'}-{a}-{g}" for b, a, g in LN])
 def test_fused_layernorm_epilogue(bf16, act, agg):
-    """LayerNorm (whole-row write-out) with and without an activation, and after a mean: fp32 within 1e-5 of the float64
-    reference (scaled by max(1, |ref|)); bf16 on the bars of test_gpu_fused.py::test_fused_gated_bf16."""
+    """LayerNorm (whole-row write-out) with and without an activation, and after a mean: the aggregate's bound carried through the
+    activation and LayerNorm (unfused_reference.layer_norm), then the bf16 rounding."""
     adj, adj_d, N = _graph(24)
     h = _states(N, 128, bf16, 1.0, 51)
     layer, w = _mlp(128, T_DEFAULT, agg, True, act=act, ln=True, seed=51)
@@ -190,17 +190,14 @@ def test_fused_layernorm_epilogue(bf16, act, agg):
     sd = {k: v.double().cpu() for k, v in layer.state_dict().items()}
     ln_w, ln_b = sd["_MlpMessagePassingLayer__state_update.0.weight"], sd["_MlpMessagePassingLayer__state_update.0.bias"]
     got = _run(layer, h, adj_d, N, 24)
-    _, _, pre = R.aggregate(*R.messages(h, adj, w, True, bf16), N, agg, bf16)
-    ref = torch.nn.functional.layer_norm(R._act64(pre, act), (128,), ln_w, ln_b, 1e-5)
+    y, by, _ = R.aggregate(*R.messages(h, adj, w, True, bf16), N, agg, bf16, act=act, round_bf16=False)
+    ref, bound = UR.layer_norm(y, by, ln_w, ln_b, 1e-5)
     if bf16:
-        rel = ((got - ref).norm() / ref.norm()).item()
-        frac = ((got - ref).abs() <= 1e-2 * ref.abs().clamp(min=1)).double().mean().item()
-        assert rel <= 1e-2 and frac >= 0.999, f"bf16 LayerNorm act={act} {agg}: rel L2 {rel:.2e}, within 1e-2: {frac:.4f}"
-    else:
-        assert_close(got, ref, what=f"fp32 LayerNorm act={act} {agg}")
+        ref, bound = UR.round_bf16(ref, bound)
+    _check(got, ref, bound, f"{'bf16' if bf16 else 'fp32'} LayerNorm", f"LayerNorm act={act} {agg}")
 
 
-# ---- the gated layer on the same graphs: fp32 aggregate in out_mode 2 -> weights-stationary GRU; bf16 lock-step -------------
+# ---- the gated layer on the same graphs: aggregate (fp32: out_mode 2) -> weights-stationary GRU, bound through the GRU --------
 @pytest.mark.parametrize("bf16", [False, True])
 @pytest.mark.parametrize("agg", AGGS)
 def test_fused_gated_structured(agg, bf16):
@@ -210,20 +207,14 @@ def test_fused_gated_structured(agg, bf16):
     h = _states(N, 128, bf16, 0.5, 61)
     torch.manual_seed(61)
     layer = P.GatedMessagePassingLayer(128, 128, T_DEFAULT, agg).cuda().eval()
-    sd = {k: v.clone().cpu() for k, v in layer.state_dict().items()}
-    args = gated_oracle_args(sd)
+    args = gated_oracle_args({k: v.clone().cpu() for k, v in layer.state_dict().items()})
     got = _run(layer, h, adj_d, N, 8)
-    if bf16:      # the bars of test_gpu_fused.py::test_fused_gated_bf16
-        ref = O.gated_layer_forward(h.float(), adj, [torch.empty(a[0].shape[0], 0) for a in adj], aggregation_fn=agg, **args)
-        rel = ((got - ref).norm() / ref.norm()).item()
-        frac = ((got - ref).abs() <= 1e-2 * ref.abs().clamp(min=1)).float().mean().item()
-        assert rel <= 1e-2 and frac >= 0.999, f"bf16 gated {agg}: rel L2 {rel:.2e}, within 1e-2: {frac:.4f}"
-        return
-    tgt, m, err = R.messages(h, adj, args["edge_weights"], False, False)
-    _, _, agg64 = R.aggregate(tgt, m, err, N, agg, False)
-    assert float(agg64.abs().max()) < 65504           # the fp16 (hi | lo') aggregate holds it: no status flag (checked in _run)
-    ref = O.gru_cell(agg64, h.double(), *(args[k].double() for k in ("gru_w_ih", "gru_w_hh", "gru_b_ih", "gru_b_hh")))
-    assert_close(got, ref, what=f"fp32 gated {agg}")
+    x, ex, _ = R.aggregate(*R.messages(h, adj, args["edge_weights"], False, bf16), N, agg, bf16)
+    if not bf16:
+        assert float(x.abs().max()) < 65504           # the fp16 (hi | lo') aggregate holds it: no status flag (checked in _run)
+    ref, bound = UR.gru(x.cuda(), ex.cuda(), h.cuda(), *(args[k] for k in ("gru_w_ih", "gru_w_hh", "gru_b_ih", "gru_b_hh")),
+                        mode="bf16" if bf16 else "3xfp16")
+    _check(got, ref.cpu(), bound.cpu(), f"{'bf16' if bf16 else 'fp32'} gated", f"gated {agg}")
 
 
 # ---- regression: a block with edges followed by three blocks without edges in one CTA's round-robin order ----------------------

@@ -24,7 +24,17 @@ gates.  A kernel that runs hi*hi alone errs by ~2^-11 / sqrt(K) of the mass and 
 FFMA kernels: a plain fp32 fma chain over K terms and the bias: gamma_{K+1} (mass + |b|), gamma_n = n u / (1 - n u).
 
 bf16 tensor cores: bf16 operands, exact products, fp32 accumulation per 16-wide k-step: (4 S + 4) u of the mass with
-S = sum ceil(K / 16) (``fused_reference.bf16_window_constant``).  Messages follow ``fused_reference.messages``; every
+S = sum ceil(K / 16) (``fused_reference.bf16_window_constant``).
+
+3xFP16 (mode '3xfp16': the weights-stationary GRU, csrc/gru_ws.cu, on fp32 states).  The aggregate arrives as the fused
+write-out's fp16 (hi | lo') split, the states as ``pack_states`` rows and the weights as ``pack_gru_ws_kernel`` packs them, all
+with the same split: hi = fl16(x), lo' = fl16(2^11 (x - hi)).  The kernel adds hi*hi into the main accumulator and hi*lo' then
+lo'*hi into the correction accumulator, 16-wide k-steps each, and combines them as fmaf(corr, 2^-11, main).  That is the
+arithmetic of ``fused_reference``'s messages, so per gate group the constant is the same, (14 + 2 S) u of the mass, plus
+2^-36 (sum_k |x_k| + sum_k |w_k|) for operands whose lo' is an fp16 subnormal; here S = (H + D) / 16 for r and z (state and
+aggregate chunks share their accumulator), D / 16 for i_n and H / 16 for h_n.  S reaches 28 at H = 448 in the state-only
+instance, past the 2^-18 that ``fused_reference.fp32_message_constant`` asserts for messages, so this constant has its own
+function (``f16x3_constant``).  Messages follow ``fused_reference.messages``; every
 other bf16 output (aggregate, LayerNorm output, dense output, GRU output) is the bf16 rounding of an fp32 value within its
 fp32 bound e of the reference, so it lies within e + 1 bf16 ulp of the rounded reference.
 
@@ -47,8 +57,16 @@ tanh' <= 1 carry them through the gates; then each approximate function adds its
   * tanh_fast(x) = 1 - 2 rcp.approx(__expf(2x) + 1): the same with s = sigma(-2x) and 2x, doubled, plus 4u (|t| + 1) for
     the final subtraction.  This also covers the FFMA kernel's expf / tanhf (within 2 ulp).
   * tanh.approx.f32 (bf16 GRU, and sigmoid as 0.5 tanh(x / 2) + 0.5): relative error <= 2^-10.98; we use 2^-10.9 |t| + 2^-20.
-Then h' = (1 - z) n + z h moves by |1 - z| dn + dz (|n - h| + dn) plus 3u (|(1 - z) n| + |z h|) + u |h'|.
+Then h' = (1 - z) n + z h moves by |1 - z| dn + dz (|n - h| + dn) plus 3u (|(1 - z) n| + |z h|) + u |h'|.  The bf16 kernels
+blend as fmaf(z, h - n, n) instead: the rounding of h - n, scaled by z, adds u z |h - n|, which the terms above do not hold when
+z -> 1 and |n| >> |h| (then |(1 - z) n| and |z h| are both small while |z (h - n)| is about |n|).
 Every GRU and LayerNorm bound is widened by 2 % for the second-order terms dropped above.
+
+State-only GRU (``gru_table``: GruGlobalStateUpdate, the TABLE instance of csrc/gru_ws.cu).  The input side gi = g W_ih^T + b_ih
+is an fp32 table from ``ptgnn_b200_linear_f32`` (``dense`` in ``fp32_dense_mode``, with its own bound), also when the states are
+bf16, so the bf16 form mixes an fp32 gi with bf16 W_hh and h; the kernel's bias vector holds b_hr, b_hz, b_hn only (b_ih is in
+the table).  Its order of adds: r = sigma((h W_hr + b_hr) + gi_r), z likewise, n = tanh(gi_n + r (h W_hn + b_hn)); each of
+those adds rounds once (u of its result), and gi's bound passes through the gates like the GEMM bound.
 """
 import math
 from typing import Dict, List, Optional, Sequence, Tuple
@@ -82,8 +100,19 @@ def bf16_constant(*Ks: int) -> float:
     return (4 * sum(math.ceil(K / 16) for K in Ks) + 4) * U
 
 
+def f16x3_constant(*Ks: int) -> float:
+    return (14 + 2 * sum(math.ceil(K / 16) for K in Ks)) * U
+
+
 def gemm_constant(mode: str, *Ks: int) -> float:
-    return {"tc": tf32_constant, "ffma": ffma_constant, "bf16": bf16_constant}[mode](*Ks)
+    return {"tc": tf32_constant, "ffma": ffma_constant, "bf16": bf16_constant, "3xfp16": f16x3_constant}[mode](*Ks)
+
+
+def _abs_term(mode: str, xa: torch.Tensor, W: torch.Tensor) -> torch.Tensor:
+    """The absolute part of a GEMM bound, [rows or 1, out]: 3xFP16 2^-36 (sum_k |x_k| + sum_k |w_k|) (xa = |x|), else 2^-100 K."""
+    if mode == "3xfp16":
+        return FR.ABS_F16 * (xa.sum(1, keepdim=True) + W.abs().sum(1)[None, :])
+    return torch.full((1, W.shape[0]), ABS_TF32 * W.shape[1], dtype=torch.float64, device=W.device)
 
 
 def fp32_message_mode(H: int, D: int) -> str:
@@ -212,9 +241,31 @@ def _sigmoid_err_mufu(a: torch.Tensor) -> torch.Tensor:
     return 0.5 * _tanh_err_mufu(0.5 * a) + U
 
 
+def _gate_errors(mode: str):
+    return (_sigmoid_err_mufu, _tanh_err_mufu) if mode == "bf16" else (_sigmoid_err_fast, _tanh_err_fast)
+
+
+def _sigmoid_gate(a: torch.Tensor, e: torch.Tensor, mode: str):
+    return torch.sigmoid(a), 0.25 * e + _gate_errors(mode)[0](a.abs() + e)
+
+
+def _gru_blend(z, dz, c, dc, h, mode: str):
+    """n = tanh(c), h' = (1 - z) n + z h from the gates and their bounds -> (ref, bound); bf16: fmaf(z, h - n, n), rounded."""
+    n = torch.tanh(c)
+    dn = dc + _gate_errors(mode)[1](c.abs() + dc)
+    out = (1 - z) * n + z * h
+    e = (1 - z) * dn + dz * ((n - h).abs() + dn) + 3 * U * (((1 - z) * n).abs() + (z * h).abs()) + U * out.abs()
+    if mode == "bf16":
+        e = e + U * z * (h - n).abs()
+    e = 1.02 * e
+    if mode == "bf16":
+        return round_bf16(out, e)
+    return out, e
+
+
 def gru(x: torch.Tensor, ex: Optional[torch.Tensor], h: torch.Tensor, w_ih, w_hh, b_ih, b_hh, mode: str):
     """nn.GRUCell(x, h) in float64 -> (ref, bound), on x's device.  x's kernel version lies within ex (None: exact input); h
-    is exact.  mode 'tc' / 'ffma' (fp32) or 'bf16' (bf16 x, h, weights and output)."""
+    is exact.  mode 'tc' / 'ffma' / '3xfp16' (fp32) or 'bf16' (bf16 x, h, weights and output)."""
     dev = x.device
     H, D = h.shape[1], x.shape[1]
     cast = _bf16 if mode == "bf16" else (lambda t: t.double())
@@ -224,30 +275,49 @@ def gru(x: torch.Tensor, ex: Optional[torch.Tensor], h: torch.Tensor, w_ih, w_hh
     gi, gh = x @ Wi.T, h @ Wh.T
     mi, mh = x.abs() @ Wi.abs().T, h.abs() @ Wh.abs().T
     pe = torch.zeros_like(gi) if ex is None else (ex @ Wi.abs().T) * (1 + 2.0 ** -10)
+    ai = _abs_term(mode, x.abs() if ex is None else x.abs() + ex, Wi)
+    ah = _abs_term(mode, h.abs(), Wh)
     c_rz, c_i, c_h = gemm_constant(mode, D, H), gemm_constant(mode, D), gemm_constant(mode, H)
-    sig_err, tanh_err = (_sigmoid_err_mufu, _tanh_err_mufu) if mode == "bf16" else (_sigmoid_err_fast, _tanh_err_fast)
     g = lambda t, k: t[:, k * H:(k + 1) * H]
     gate = []
     for k in (0, 1):                                            # r, z
         bsum = bi[k * H:(k + 1) * H] + bh[k * H:(k + 1) * H]
         a = g(gi, k) + g(gh, k) + bsum
-        e = c_rz * (g(mi, k) + g(mh, k)) + g(pe, k) + U * (bsum.abs() + a.abs()) + ABS_TF32 * (D + H)
-        gate.append((torch.sigmoid(a), 0.25 * e + sig_err(a.abs() + e)))
+        e = c_rz * (g(mi, k) + g(mh, k)) + g(pe, k) + U * (bsum.abs() + a.abs()) + g(ai, k) + g(ah, k)
+        gate.append(_sigmoid_gate(a, e, mode))
     (r, dr), (z, dz) = gate
     gn = g(gi, 2) + bi[2 * H:]
-    en = c_i * g(mi, 2) + g(pe, 2) + U * gn.abs() + ABS_TF32 * D
+    en = c_i * g(mi, 2) + g(pe, 2) + U * gn.abs() + g(ai, 2)
     gh_n = g(gh, 2) + bh[2 * H:]
-    ehn = c_h * g(mh, 2) + U * gh_n.abs() + ABS_TF32 * H
+    ehn = c_h * g(mh, 2) + U * gh_n.abs() + g(ah, 2)
     c = gn + r * gh_n
     dc = en + r * ehn + dr * (gh_n.abs() + ehn) + U * ((r * gh_n).abs() + c.abs())
-    n = torch.tanh(c)
-    dn = dc + tanh_err(c.abs() + dc)
-    out = (1 - z) * n + z * h
-    e = (1 - z) * dn + dz * ((n - h).abs() + dn) + 3 * U * (((1 - z) * n).abs() + (z * h).abs()) + U * out.abs()
-    e = 1.02 * e
-    if mode == "bf16":
-        return round_bf16(out, e)
-    return out, e
+    return _gru_blend(z, dz, c, dc, h, mode)
+
+
+def gru_table(gi: torch.Tensor, e_gi: torch.Tensor, h: torch.Tensor, w_hh, b_hh, mode: str):
+    """The state-only GRU: GRUCell with the input-side pre-activations given per row -> (ref, bound), on gi's device.  gi [N, 3H]
+    (gates r, z, n; b_ih included) is the float64 table row of each node's graph and its fp32 version lies within e_gi; h is
+    exact.  mode '3xfp16' (fp32 states) or 'bf16' (bf16 h, W_hh and output; gi stays fp32)."""
+    dev = gi.device
+    H = h.shape[1]
+    Wh = (_bf16(w_hh) if mode == "bf16" else w_hh.double()).to(dev)
+    bh = b_hh.double().to(dev)
+    h = h.double().to(dev)
+    gh, mh = h @ Wh.T, h.abs() @ Wh.abs().T
+    ah = _abs_term(mode, h.abs(), Wh)
+    c_h = gemm_constant(mode, H)
+    g = lambda t, k: t[:, k * H:(k + 1) * H]
+    hb = [g(gh, k) + bh[k * H:(k + 1) * H] for k in range(3)]         # h W_h + b_h, one rounding each
+    eh = [c_h * g(mh, k) + g(ah, k) + U * hb[k].abs() for k in range(3)]
+    gate = []
+    for k in (0, 1):                                            # r, z: (h W_h + b_h) + gi
+        a = hb[k] + g(gi, k)
+        gate.append(_sigmoid_gate(a, eh[k] + g(e_gi, k) + U * a.abs(), mode))
+    (r, dr), (z, dz) = gate
+    c = g(gi, 2) + r * hb[2]
+    dc = g(e_gi, 2) + r * eh[2] + dr * (hb[2].abs() + eh[2]) + U * ((r * hb[2]).abs() + c.abs())
+    return _gru_blend(z, dz, c, dc, h, mode)
 
 
 # ---- structured graphs ------------------------------------------------------------------------------------------------
