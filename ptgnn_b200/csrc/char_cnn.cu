@@ -80,11 +80,6 @@ template <bool BF16> static Prepared layout(const Shape &s) {
     return p;
 }
 
-__device__ __forceinline__ uint32_t sw128(int row, int k) {
-    return (uint32_t)(row * 128 + ((((k >> 3) ^ (row & 7)) << 4) | ((k & 7) << 1)));
-}
-__device__ __forceinline__ float round_bf16(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
-
 // ---- preparation: T1, biases, staged weights ------------------------------------------------------------------------------
 template <bool BF16>
 __global__ void prepare_t1_kernel(const float *__restrict__ w1, const float *__restrict__ b1, const float *__restrict__ b2, int C, int F1,
@@ -96,13 +91,13 @@ __global__ void prepare_t1_kernel(const float *__restrict__ w1, const float *__r
             const long long ct = i / F1;
             const int tap = (int)(ct % W1), c = (int)(ct / W1);
             const float x = w1[((long long)f * C + c) * W1 + tap];
-            t1[i] = BF16 ? round_bf16(x) : x;
+            t1[i] = BF16 ? tc::round_bf16(x) : x;
         } else if (i < n + F1) {
             const float x = b1[i - n];
-            b1o[i - n] = BF16 ? round_bf16(x) : x;
+            b1o[i - n] = BF16 ? tc::round_bf16(x) : x;
         } else {
             const float x = b2[i - n - F1];
-            b2o[i - n - F1] = BF16 ? round_bf16(x) : x;
+            b2o[i - n - F1] = BF16 ? tc::round_bf16(x) : x;
         }
     }
 }
@@ -122,15 +117,16 @@ __global__ void prepare_stage_kernel(const float *__restrict__ w, int N, int K, 
         const float x = ng < N ? w[((long long)ng * K + kg) * W + tap] : 0.0f;
         uint8_t *blk = dst + s * sb;
         if (BF16) {
-            *reinterpret_cast<__nv_bfloat16 *>(blk + sw128(n, k)) = __float2bfloat16_rn(x);
+            *reinterpret_cast<__nv_bfloat16 *>(blk + tc::sw128(n, k)) = __float2bfloat16_rn(x);
         } else {
-            const __half hi = __float2half_rn(x), lo = __float2half_rn((x - __half2float(hi)) * 2048.0f);
-            *reinterpret_cast<__half *>(blk + sw128(n, k)) = hi;
-            *reinterpret_cast<__half *>(blk + (size_t)nw * 128 + sw128(n, k)) = lo;
-            bad |= !(fabsf(x) < 65504.0f);
+            __half hi, lo;
+            tc::split_f16(x, hi, lo);
+            *reinterpret_cast<__half *>(blk + tc::sw128(n, k)) = hi;
+            *reinterpret_cast<__half *>(blk + (size_t)nw * 128 + tc::sw128(n, k)) = lo;
+            bad |= !tc::f16_in_range(x);
         }
     }
-    if (bad && status) atomicOr(status + 1, 1);
+    if (bad && status) tc::set_status(status + 1);
 }
 
 // ---- forward ----------------------------------------------------------------------------------------------------------------
@@ -249,14 +245,11 @@ template <bool BF16>
 __device__ __forceinline__ bool put2(uint8_t *base, uint32_t copy_off, int pitch, int row, int col, float x0, float x1) {
     uint8_t *p = base + (size_t)row * pitch + col * 2;
     if (BF16) {
-        *reinterpret_cast<__nv_bfloat162 *>(p) = __floats2bfloat162_rn(x0, x1);
+        *reinterpret_cast<uint32_t *>(p) = __float_as_uint(pack_bf16x2(x0, x1));
         return true;
     }
-    const __half h0 = __float2half_rn(x0), h1 = __float2half_rn(x1);
-    const __half l0 = __float2half_rn((x0 - __half2float(h0)) * 2048.0f), l1 = __float2half_rn((x1 - __half2float(h1)) * 2048.0f);
-    *reinterpret_cast<__half2 *>(p) = __halves2half2(h0, h1);
-    *reinterpret_cast<__half2 *>(p + copy_off) = __halves2half2(l0, l1);
-    return fabsf(x0) < 65504.0f && fabsf(x1) < 65504.0f;
+    tc::split_f16x2(x0, x1, *reinterpret_cast<uint32_t *>(p), *reinterpret_cast<uint32_t *>(p + copy_off));
+    return tc::f16_in_range(x0) && tc::f16_in_range(x1);
 }
 
 template <bool BF16, int NWG>
@@ -305,7 +298,7 @@ __global__ void __launch_bounds__(128 * NWG, 1) char_cnn_kernel(const Args a) {
                         const float4 w = __ldg(reinterpret_cast<const float4 *>(a.t1 + ((long long)ids[t * L + p + tap] * s.w1 + tap) * s.F1 + f));
                         v.x = __fadd_rn(v.x, w.x), v.y = __fadd_rn(v.y, w.y), v.z = __fadd_rn(v.z, w.z), v.w = __fadd_rn(v.w, w.w);
                     }
-                    if (BF16) v.x = round_bf16(v.x), v.y = round_bf16(v.y), v.z = round_bf16(v.z), v.w = round_bf16(v.w);
+                    if (BF16) v.x = tc::round_bf16(v.x), v.y = tc::round_bf16(v.y), v.z = tc::round_bf16(v.z), v.w = tc::round_bf16(v.w);
                     v.x = fmaxf(v.x, 0.f), v.y = fmaxf(v.y, 0.f), v.z = fmaxf(v.z, 0.f), v.w = fmaxf(v.w, 0.f);
                     if (materialise)
                         *reinterpret_cast<float4 *>(a.a1_out + ((tok0 + t) * L1 + p) * s.F1 + f) = v;
@@ -336,9 +329,9 @@ __global__ void __launch_bounds__(128 * NWG, 1) char_cnn_kernel(const Args a) {
 #pragma unroll
                         for (int e = 0; e < 2; ++e) {
                             const int i = 4 * j + 2 * e2 + e;
-                            float v = BF16 ? acc[h][i] : __fadd_rn(acc[h][i], cor[h][i] * (1.0f / 2048.0f));
+                            float v = BF16 ? acc[h][i] : tc::corrected(acc[h][i], cor[h][i]);
                             v = __fadd_rn(v, __ldg(a.b2 + n + e));
-                            if (BF16) v = round_bf16(v);
+                            if (BF16) v = tc::round_bf16(v);
                             x[e] = fmaxf(v, 0.0f);
                         }
                         const bool ok = put2<BF16>(act2, off2, P2, r, n, x[0], x[1]);
@@ -372,8 +365,8 @@ __global__ void __launch_bounds__(128 * NWG, 1) char_cnn_kernel(const Args a) {
 #pragma unroll
                         for (int e = 0; e < 2; ++e) {
                             const int i = 4 * j + 2 * e2 + e, col = h * 64 + 8 * j + 2 * tq + e;
-                            float v = BF16 ? acc[h][i] : __fadd_rn(acc[h][i], cor[h][i] * (1.0f / 2048.0f));
-                            if (BF16) v = round_bf16(v);
+                            float v = BF16 ? acc[h][i] : tc::corrected(acc[h][i], cor[h][i]);
+                            if (BF16) v = tc::round_bf16(v);
                             atomicMax(keys + t * STAGE_ROWS + col, max_key(v, pos));
                         }
                     }
@@ -394,7 +387,7 @@ __global__ void __launch_bounds__(128 * NWG, 1) char_cnn_kernel(const Args a) {
     }
     if (a.status) {
         if (bad_ids) atomicAdd(a.status, bad_ids);
-        if (overflow) atomicOr(a.status + 1, 1);
+        if (overflow) tc::set_status(a.status + 1);
     }
 }
 

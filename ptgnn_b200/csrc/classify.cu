@@ -59,13 +59,11 @@ struct Args {
     int32_t *status;                     // [0] bad ids, [1] an fp32 value outside the fp16 range
 };
 
-__device__ __forceinline__ float round_bf16(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
-
 // torch's sigmoid (1 / (1 + exp(-x)) in fp32, rounded to bf16 for a bf16 tensor) >= 0.5
 template <bool BF16>
 __device__ __forceinline__ bool predict(float v) {
     float p = __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-v)));
-    if (BF16) p = round_bf16(p);
+    if (BF16) p = tc::round_bf16(p);
     return p >= 0.5f;
 }
 
@@ -152,16 +150,12 @@ __global__ void __launch_bounds__(THREADS, 1) classify_kernel(const Args a) {
                     const __nv_bfloat16 *p1 = p0 + 8 * PITCH_B;
                     // through fp32 and back (exact), as the fp32 rows: registers the MMAs read straight from shared-memory loads make
                     // ptxas serialise every wgmma
-                    split2<true>(__bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(p0)), ah[kk][0], al[kk][0], bad);
-                    split2<true>(__bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(p1)), ah[kk][1], al[kk][1], bad);
-                    split2<true>(__bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(p0 + 8)), ah[kk][2], al[kk][2], bad);
-                    split2<true>(__bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(p1 + 8)), ah[kk][3], al[kk][3], bad);
+                    auto ld = [](const __nv_bfloat16 *q) { return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(q)); };
+                    split_frag<true>({ld(p0), ld(p1), ld(p0 + 8), ld(p1 + 8)}, ah[kk], al[kk], bad);
                 } else {
                     const float *p0 = reinterpret_cast<const float *>(st) + (wrow + gq) * PITCH + kk * 16 + 2 * tq, *p1 = p0 + 8 * PITCH;
-                    split2<BF16>(*reinterpret_cast<const float2 *>(p0), ah[kk][0], al[kk][0], bad);
-                    split2<BF16>(*reinterpret_cast<const float2 *>(p1), ah[kk][1], al[kk][1], bad);
-                    split2<BF16>(*reinterpret_cast<const float2 *>(p0 + 8), ah[kk][2], al[kk][2], bad);
-                    split2<BF16>(*reinterpret_cast<const float2 *>(p1 + 8), ah[kk][3], al[kk][3], bad);
+                    auto ld = [](const float *q) { return *reinterpret_cast<const float2 *>(q); };
+                    split_frag<BF16>({ld(p0), ld(p1), ld(p0 + 8), ld(p1 + 8)}, ah[kk], al[kk], bad);
                 }
             }
         }
@@ -214,11 +208,11 @@ __global__ void __launch_bounds__(THREADS, 1) classify_kernel(const Args a) {
                     for (int e1 = 0; e1 < 2; ++e1) {
                         const int i = 4 * j + 2 * e2 + e1;
                         const int col = blk * g.Dc + h * 64 + 8 * j + 2 * tq + e1;
-                        float v = BF16 ? acc[h][i] : __fadd_rn(acc[h][i], cor[h][i] * (1.0f / 2048.0f));
+                        float v = BF16 ? acc[h][i] : tc::corrected(acc[h][i], cor[h][i]);
                         acc[h][i] = cor[h][i] = 0.0f;
                         if (!live || col >= a.C || h * 64 + 8 * j >= ncols) continue;
-                        v = __fadd_rn(v, BF16 ? round_bf16(a.bias[col]) : a.bias[col]);
-                        if (BF16) v = round_bf16(v);      // autocast: the Linear's bf16 output
+                        v = __fadd_rn(v, BF16 ? tc::round_bf16(a.bias[col]) : a.bias[col]);
+                        if (BF16) v = tc::round_bf16(v);      // autocast: the Linear's bf16 output
                         if (GRAD) {
                             float d = 0.0f;         // a row with a bad id: none
                             if (!bad_id && MODE == CE) {
@@ -285,7 +279,7 @@ __global__ void __launch_bounds__(THREADS, 1) classify_kernel(const Args a) {
         }
     }
     cp_async_wait<0>();
-    if (bad && a.status) *reinterpret_cast<volatile int32_t *>(a.status + 1) = 1;
+    if (bad && a.status) tc::set_status(a.status + 1);
 }
 
 // One CTA of 256 threads per ROWS_PER_CTA rows: merge each row's column blocks in order, then the CTA's sums in a fixed tree.

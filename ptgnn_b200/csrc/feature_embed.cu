@@ -38,15 +38,16 @@ __global__ void prepare_kernel(const float *__restrict__ w, int F, int D, int Dc
         const float x = (d < D && f < F) ? w[(long long)d * F + f] : 0.0f;
         uint8_t *base = dst + (size_t)blk * (BF16 ? 1 : 2) * KB * Dc * 128 + (size_t)kb * Dc * 128;
         if (BF16) {
-            *reinterpret_cast<__nv_bfloat16 *>(base + sw128(r, k)) = __float2bfloat16_rn(x);
+            *reinterpret_cast<__nv_bfloat16 *>(base + tc::sw128(r, k)) = __float2bfloat16_rn(x);
         } else {
-            const __half hi = __float2half_rn(x), lo = __float2half_rn((x - __half2float(hi)) * 2048.0f);
-            *reinterpret_cast<__half *>(base + sw128(r, k)) = hi;
-            *reinterpret_cast<__half *>(base + (size_t)KB * Dc * 128 + sw128(r, k)) = lo;
-            bad |= !(fabsf(x) < 65504.0f);
+            __half hi, lo;
+            tc::split_f16(x, hi, lo);
+            *reinterpret_cast<__half *>(base + tc::sw128(r, k)) = hi;
+            *reinterpret_cast<__half *>(base + (size_t)KB * Dc * 128 + tc::sw128(r, k)) = lo;
+            bad |= !tc::f16_in_range(x);
         }
     }
-    if (bad && status) *reinterpret_cast<volatile int32_t *>(status) = 1;
+    if (bad && status) tc::set_status(status);
 }
 
 // ---- forward ------------------------------------------------------------------------------------------------------------------
@@ -128,10 +129,8 @@ __global__ void __launch_bounds__(THREADS, 1) feature_embed_kernel(const Args a)
         for (int kk = 0; kk < 4; ++kk) {
             if (kk < ksteps) {
                 const float *p0 = st + (wrow + gq) * PITCH + kk * 16 + 2 * tq, *p1 = p0 + 8 * PITCH;
-                split2<BF16>(*reinterpret_cast<const float2 *>(p0), ah[kk][0], al[kk][0], bad);
-                split2<BF16>(*reinterpret_cast<const float2 *>(p1), ah[kk][1], al[kk][1], bad);
-                split2<BF16>(*reinterpret_cast<const float2 *>(p0 + 8), ah[kk][2], al[kk][2], bad);
-                split2<BF16>(*reinterpret_cast<const float2 *>(p1 + 8), ah[kk][3], al[kk][3], bad);
+                split_frag<BF16>({*reinterpret_cast<const float2 *>(p0), *reinterpret_cast<const float2 *>(p1),
+                                  *reinterpret_cast<const float2 *>(p0 + 8), *reinterpret_cast<const float2 *>(p1 + 8)}, ah[kk], al[kk], bad);
             }
         }
         tc::fence_acc(acc[0]);
@@ -172,14 +171,14 @@ __global__ void __launch_bounds__(THREADS, 1) feature_embed_kernel(const Args a)
                     const long long row = tile * BM + wrow + gq + 8 * e2;
                     const int col = blk * g.Dc + h * 64 + 8 * j + 2 * tq;
                     const int i = 4 * j + 2 * e2;
-                    float v0 = BF16 ? acc[h][i] : __fadd_rn(acc[h][i], cor[h][i] * (1.0f / 2048.0f));
-                    float v1 = BF16 ? acc[h][i + 1] : __fadd_rn(acc[h][i + 1], cor[h][i + 1] * (1.0f / 2048.0f));
+                    float v0 = BF16 ? acc[h][i] : tc::corrected(acc[h][i], cor[h][i]);
+                    float v1 = BF16 ? acc[h][i + 1] : tc::corrected(acc[h][i + 1], cor[h][i + 1]);
                     acc[h][i] = acc[h][i + 1] = cor[h][i] = cor[h][i + 1] = 0.0f;
                     if (row >= a.N || col >= a.D || h * 64 + 8 * j >= ncols) continue;     // the last column is another block's
                     const long long o = row * a.D + col;
                     if (BF16) {      // autocast: the Linear's bf16 output, then the activation of that bf16 tensor, rounded again
-                        v0 = __bfloat162float(__float2bfloat16_rn(v0));
-                        v1 = __bfloat162float(__float2bfloat16_rn(v1));
+                        v0 = tc::round_bf16(v0);
+                        v1 = tc::round_bf16(v1);
                     }
                     if (a.pre) *reinterpret_cast<float2 *>(a.pre + o) = make_float2(v0, v1);
                     const float y0 = apply_act(v0, a.act), y1 = apply_act(v1, a.act);
@@ -189,7 +188,8 @@ __global__ void __launch_bounds__(THREADS, 1) feature_embed_kernel(const Args a)
                         *reinterpret_cast<float2 *>(static_cast<float *>(a.out) + o) = make_float2(y0, y1);
                         if (a.packed) {        // pack_states' split of the stored value: row = hi[D] | lo'[D]
                             uint32_t hi, lo;
-                            split2<false>(make_float2(y0, y1), hi, lo, bad);
+                            tc::split_f16x2(y0, y1, hi, lo);
+                            bad |= !tc::f16_in_range(y0) | !tc::f16_in_range(y1);
                             uint8_t *prow = a.packed + row * (long long)a.D * 4;
                             *reinterpret_cast<uint32_t *>(prow + col * 2) = hi;
                             *reinterpret_cast<uint32_t *>(prow + (long long)a.D * 2 + col * 2) = lo;
@@ -200,7 +200,7 @@ __global__ void __launch_bounds__(THREADS, 1) feature_embed_kernel(const Args a)
         }
     }
     cp_async_wait<0>();
-    if (bad && a.status) *reinterpret_cast<volatile int32_t *>(a.status) = 1;
+    if (bad && a.status) tc::set_status(a.status);
 }
 
 template <bool BF16, int S>

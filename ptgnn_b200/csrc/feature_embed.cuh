@@ -45,10 +45,6 @@ static inline int stages(const Geometry &g) {
     return s >= 4 ? 4 : (int)s;          // >= 2: the weight slice is at most W_BUDGET
 }
 
-__device__ __forceinline__ uint32_t sw128(int row, int k) {
-    return (uint32_t)(row * 128 + ((((k >> 3) ^ (row & 7)) << 4) | ((k & 7) << 1)));
-}
-
 __device__ __forceinline__ void cp_async_ca(uint32_t dst, const void *src, int bytes, int src_bytes) {
     if (bytes == 16) asm volatile("cp.async.ca.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst), "l"(src), "r"(src_bytes));
     else if (bytes == 8) asm volatile("cp.async.ca.shared.global [%0], [%1], 8, %2;\n" ::"r"(dst), "l"(src), "r"(src_bytes));
@@ -58,26 +54,25 @@ __device__ __forceinline__ void cp_async_ca(uint32_t dst, const void *src, int b
 template <bool BF16>
 __device__ __forceinline__ void mma_cols(float (&d)[32], const uint32_t (&a)[4], uint64_t desc, int width) {
     switch (width) {
-        case 64: tc::wgmma_16_rs_n64<BF16>(d, a, desc); break;
-        case 48: tc::wgmma_16_rs_n48<BF16>(d, a, desc); break;
-        case 32: tc::wgmma_16_rs_n32<BF16>(d, a, desc); break;
-        default: tc::wgmma_16_rs_n16<BF16>(d, a, desc); break;
+        case 64: tc::wgmma_16_rs<BF16, 64>(d, a, desc); break;
+        case 48: tc::wgmma_16_rs<BF16, 48>(d, a, desc); break;
+        case 32: tc::wgmma_16_rs<BF16, 32>(d, a, desc); break;
+        default: tc::wgmma_16_rs<BF16, 16>(d, a, desc); break;
     }
 }
 
-// two fp32 -> the 16-bit operand pair(s) of one A register: hi (fp16 or bf16) and, fp32, lo' = rn16((x - hi) 2^11)
+// the four fp32 pairs of one register A fragment (rows g, g + 8, g, g + 8; columns 2 t, 2 t, 2 t + 8, 2 t + 8) -> its 16-bit operands:
+// hi (fp16 or bf16) and, fp32, lo'
 template <bool BF16>
-__device__ __forceinline__ void split2(float2 v, uint32_t &hi, uint32_t &lo, bool &bad) {
-    if (BF16) {
-        __nv_bfloat162 b = __floats2bfloat162_rn(v.x, v.y);
-        hi = *reinterpret_cast<uint32_t *>(&b);
-    } else {
-        const __half h0 = __float2half_rn(v.x), h1 = __float2half_rn(v.y);
-        const __half l0 = __float2half_rn((v.x - __half2float(h0)) * 2048.0f), l1 = __float2half_rn((v.y - __half2float(h1)) * 2048.0f);
-        __half2 hh = __halves2half2(h0, h1), ll = __halves2half2(l0, l1);
-        hi = *reinterpret_cast<uint32_t *>(&hh);
-        lo = *reinterpret_cast<uint32_t *>(&ll);
-        bad |= !(fabsf(v.x) < 65504.0f) | !(fabsf(v.y) < 65504.0f);
+__device__ __forceinline__ void split_frag(const float2 (&v)[4], uint32_t (&hi)[4], uint32_t (&lo)[4], bool &bad) {
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+        if (BF16) {
+            hi[e] = __float_as_uint(pack_bf16x2(v[e].x, v[e].y));
+        } else {
+            tc::split_f16x2(v[e].x, v[e].y, hi[e], lo[e]);
+            bad |= !tc::f16_in_range(v[e].x) | !tc::f16_in_range(v[e].y);
+        }
     }
 }
 

@@ -93,7 +93,6 @@ __device__ __forceinline__ uint4 ldg_nc_u4(const uint4 *p) {
     return r;
 }
 __device__ __forceinline__ void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
-__device__ __forceinline__ uint32_t swz(int row, int q) { return (uint32_t)(row * 128 + ((q ^ (row & 7)) << 4)); }
 
 // Debug timeline (PTGNN_FUSED_TRACE=1): CTA 0, one thread per role, records (clock64, step, tag) at the pipeline hand-offs into its
 // TRACE_CAP-entry region of the trace buffer; read back with ptgnn_b200_debug_fused_trace (tools/fused_trace.py).
@@ -189,16 +188,6 @@ __device__ __forceinline__ float lds_f32(uint32_t addr) {
     return v;
 }
 
-__device__ __forceinline__ uint32_t pack_h2(__half a, __half b) {
-    return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
-}
-// x -> (hi, lo') fp16 pair; returns false when |x| is not representable (>= 65504, inf, NaN)
-__device__ __forceinline__ bool split_f16(float x, __half &hi, __half &lo) {
-    hi = __float2half_rn(x);
-    lo = __float2half_rn((x - __half2float(hi)) * 2048.0f);
-    return fabsf(x) < 65504.0f;
-}
-
 template <int RED> __device__ __forceinline__ float red_identity() {
     return RED == PTGNN_REDUCE_MAX ? -FLT_MAX : (RED == PTGNN_REDUCE_MIN ? FLT_MAX : 0.0f);
 }
@@ -256,20 +245,17 @@ __device__ __forceinline__ void write_out_block(const Params *p, uint32_t agg_sa
             }
         }
         if (MODE == 1) {
-            __nv_bfloat162 lo = __floats2bfloat162_rn(a.x, a.y), hi = __floats2bfloat162_rn(a.z, a.w);
-            uint2 pk;
-            pk.x = *reinterpret_cast<uint32_t *>(&lo); pk.y = *reinterpret_cast<uint32_t *>(&hi);
-            reinterpret_cast<uint2 *>(p->out)[(size_t)v * (kD / 4) + q] = pk;
-        } else if (MODE == 2) {      // fp16 (hi | lo') row: hi halfs at [0, 128), lo' halfs at [128, 256); packed conversions
-            const __half2 h01 = __floats2half2_rn(a.x, a.y), h23 = __floats2half2_rn(a.z, a.w);
-            const float2 f01 = __half22float2(h01), f23 = __half22float2(h23);
-            const __half2 l01 = __floats2half2_rn((a.x - f01.x) * 2048.0f, (a.y - f01.y) * 2048.0f);
-            const __half2 l23 = __floats2half2_rn((a.z - f23.x) * 2048.0f, (a.w - f23.y) * 2048.0f);
+            reinterpret_cast<uint2 *>(p->out)[(size_t)v * (kD / 4) + q] =
+                make_uint2(__float_as_uint(pack_bf16x2(a.x, a.y)), __float_as_uint(pack_bf16x2(a.z, a.w)));
+        } else if (MODE == 2) {      // fp16 (hi | lo') row: hi halfs at [0, 128), lo' halfs at [128, 256)
+            const float x[4] = {a.x, a.y, a.z, a.w};
+            uint32_t h[2], l[2];
+            tc::split_f16_pairs<2>(x, h, l);
             uint2 *row = reinterpret_cast<uint2 *>(p->out) + (size_t)v * (2 * kD / 4);
-            row[q] = make_uint2(*reinterpret_cast<const uint32_t *>(&h01), *reinterpret_cast<const uint32_t *>(&h23));
-            row[kD / 4 + q] = make_uint2(*reinterpret_cast<const uint32_t *>(&l01), *reinterpret_cast<const uint32_t *>(&l23));
+            row[q] = make_uint2(h[0], h[1]);
+            row[kD / 4 + q] = make_uint2(l[0], l[1]);
             const float big = fmaxf(fmaxf(fabsf(a.x), fabsf(a.y)), fmaxf(fabsf(a.z), fabsf(a.w)));
-            if (!(big < 65504.0f) && p->status != nullptr) *reinterpret_cast<volatile int32_t *>(p->status) = 1;
+            if (!(big < tc::F16_LIMIT) && p->status != nullptr) tc::set_status(p->status);
         } else {
             reinterpret_cast<float4 *>(p->out)[(size_t)v * (kD / 4) + q] = a;
         }
@@ -298,8 +284,6 @@ __device__ __forceinline__ void write_out_block(const Params *p, uint32_t agg_sa
     else if (p->out_mode == 1) { if (plain) write_rows(integral_constant<int, 1>{}, integral_constant<bool, true>{}); else write_rows(integral_constant<int, 1>{}, integral_constant<bool, false>{}); }
     else { if (plain) write_rows(integral_constant<int, 0>{}, integral_constant<bool, true>{}); else write_rows(integral_constant<int, 0>{}, integral_constant<bool, false>{}); }
 }
-
-__device__ __forceinline__ float bf16r(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
 
 // EGC write-out of a finished block (EgcEpilogue): the same row walk as write_out_block.  Lane q's float4 holds slab features 4 q ..
 // 4 q + 3, i.e. bases (4 q) % bases .. of output column(s) col0 + 4 q / bases: bases = 4 -> one column per lane, 8 -> a lane pair
@@ -330,10 +314,10 @@ __device__ __forceinline__ void write_out_block_egc(const Params *p, uint32_t ag
         for (int i = 0; i < 4; ++i) {
             if (RED == PTGNN_REDUCE_MEAN) x[i] /= cdiv;
             if ((RED == PTGNN_REDUCE_MAX || RED == PTGNN_REDUCE_MIN) && x[i] == IDENT) x[i] = 0.0f;
-            if (bf) x[i] = bf16r(x[i]);
+            if (bf) x[i] = tc::round_bf16(x[i]);
         }
         const float *crow = e.coef + (size_t)v * e.coef_stride;
-        auto prod = [&](float A, float w) { const float t = __fmul_rn(A, w); return bf ? bf16r(t) : t; };
+        auto prod = [&](float A, float w) { const float t = __fmul_rn(A, w); return bf ? tc::round_bf16(t) : t; };
         const size_t orow = (size_t)v * e.out_stride;
         auto store1 = [&](int o, float s) {
             if (bf) reinterpret_cast<__nv_bfloat16 *>(p->out)[orow + o] = __float2bfloat16_rn(s);
@@ -365,10 +349,8 @@ __device__ __forceinline__ void write_out_block_egc(const Params *p, uint32_t ag
 #pragma unroll
             for (int i = 0; i < 4; ++i) s[i] = prod(x[i], __ldg(crow + (o + i) / e.dh));
             if (bf) {
-                __nv_bfloat162 lo = __floats2bfloat162_rn(s[0], s[1]), hi = __floats2bfloat162_rn(s[2], s[3]);
-                uint2 pk;
-                pk.x = *reinterpret_cast<uint32_t *>(&lo); pk.y = *reinterpret_cast<uint32_t *>(&hi);
-                *reinterpret_cast<uint2 *>(reinterpret_cast<__nv_bfloat16 *>(p->out) + orow + o) = pk;
+                *reinterpret_cast<uint2 *>(reinterpret_cast<__nv_bfloat16 *>(p->out) + orow + o) =
+                    make_uint2(__float_as_uint(pack_bf16x2(s[0], s[1])), __float_as_uint(pack_bf16x2(s[2], s[3])));
             } else {
                 *reinterpret_cast<float4 *>(reinterpret_cast<float *>(p->out) + orow + o) = make_float4(s[0], s[1], s[2], s[3]);
             }
@@ -594,7 +576,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
                 mbar_wait(&x_empty[slot], ((c_issue / NUM_SLOTS) & 1) ^ 1);
                 trace_mark(p, 2, c_issue);
                 const unsigned char *rows = cur.seg == 0 ? p.src_rows : p.tgt_rows;
-                const uint32_t sbase = smem_u32(ring + slot * SLOT_BYTES) + swz(rsub, q);
+                const uint32_t sbase = smem_u32(ring + slot * SLOT_BYTES) + tc::swz(rsub, q);
 #pragma unroll
                 for (int i = 0; i < NMAX / 8; ++i) {
                     if (idx[i] >= 0) {
@@ -672,17 +654,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
                 const int kc = ks >> 2, kk = ks & 3;
                 const uint64_t x_hi = tc::make_smem_desc_sw128(slot_addr + kc * TILE_BYTES) + kk * 2;
                 const uint64_t x_lo = tc::make_smem_desc_sw128(slot_addr + (KCH + kc) * TILE_BYTES) + kk * 2;
-                auto one = [&](float (&dacc)[32], const uint32_t (&a)[4], uint64_t desc) {
-                    if (NB == 1) tc::wgmma_16_rs_n16<BF16>(dacc, a, desc);
-                    else if (NB == 2) tc::wgmma_16_rs_n32<BF16>(dacc, a, desc);
-                    else if (NB == 3) tc::wgmma_16_rs_n48<BF16>(dacc, a, desc);
-                    else tc::wgmma_16_rs_n64<BF16>(dacc, a, desc);
-                };
-                one(acc_m, wf[0][ks], x_hi);
+                tc::wgmma_16_rs<BF16, 16 * NB>(acc_m, wf[0][ks], x_hi);
                 if (NPROD == 3) {
                     // x * w ~= hi*hi (main) + 2^-11 (hi*lo' + lo'*hi) (correction accumulator, scaled by 2^11)
-                    one(acc_c, wf[0][ks], x_lo);
-                    one(acc_c, wf[NPART - 1][ks], x_hi);
+                    tc::wgmma_16_rs<BF16, 16 * NB>(acc_c, wf[0][ks], x_lo);
+                    tc::wgmma_16_rs<BF16, 16 * NB>(acc_c, wf[NPART - 1][ks], x_hi);
                 }
             }
         };
@@ -733,9 +709,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
                         for (int h = 0; h < 2; ++h) {
                             float v0 = acc_m[4 * j + 2 * h], v1 = acc_m[4 * j + 2 * h + 1];
                             if (NPROD == 3) {
-                                v0 = fmaf(acc_c[4 * j + 2 * h], 1.0f / 2048.0f, v0); v1 = fmaf(acc_c[4 * j + 2 * h + 1], 1.0f / 2048.0f, v1);
+                                v0 = tc::corrected(v0, acc_c[4 * j + 2 * h]); v1 = tc::corrected(v1, acc_c[4 * j + 2 * h + 1]);
                             } else {                    // the autocast Linear's bf16 output
-                                v0 = __bfloat162float(__float2bfloat16_rn(v0)); v1 = __bfloat162float(__float2bfloat16_rn(v1));
+                                v0 = tc::round_bf16(v0); v1 = tc::round_bf16(v1);
                             }
                             *reinterpret_cast<float2 *>(acc_s + (f0 + 8 * h) * ACC_PITCH + 8 * j + 2 * tq) = make_float2(v0, v1);
                         }
@@ -769,17 +745,15 @@ __global__ void __launch_bounds__(256) pack_states_kernel(const float *__restric
         const float4 a = ld_stream_f4(reinterpret_cast<const float4 *>(h + row * K + c8 * 8));
         const float4 b = ld_stream_f4(reinterpret_cast<const float4 *>(h + row * K + c8 * 8 + 4));
         const float x[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-        __half hi[8], lo[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) bad |= !split_f16(x[j], hi[j], lo[j]);
+        for (int j = 0; j < 8; ++j) bad |= !tc::f16_in_range(x[j]);
         uint4 vh, vl;
-        vh.x = pack_h2(hi[0], hi[1]); vh.y = pack_h2(hi[2], hi[3]); vh.z = pack_h2(hi[4], hi[5]); vh.w = pack_h2(hi[6], hi[7]);
-        vl.x = pack_h2(lo[0], lo[1]); vl.y = pack_h2(lo[2], lo[3]); vl.z = pack_h2(lo[4], lo[5]); vl.w = pack_h2(lo[6], lo[7]);
+        tc::split_f16x8(x, vh, vl);
         uint4 *dst = out + row * (K / 4);       // row = 4K bytes = K/4 uint4: hi part first (K/8 uint4), then lo'
         dst[c8] = vh;
         dst[K / 8 + c8] = vl;
     }
-    if (bad && status != nullptr) *reinterpret_cast<volatile int32_t *>(status) = 1;
+    if (bad && status != nullptr) tc::set_status(status);
 }
 
 struct WeightSrc {
@@ -809,25 +783,24 @@ __global__ void __launch_bounds__(256) pack_weights_kernel(const __grid_constant
 #pragma unroll
         for (int j = 0; j < 8; ++j) x[j] = row[j];
         const size_t base = ((size_t)(t * nseg + seg) * NPART) * (K / 8) * 128;
-        if (NPROD == 3) {
+        if (NPROD == 3) {       // scalar conversions: split_f16x8 takes 3 more registers here
             __half hi[8], lo[8];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) bad |= !split_f16(x[j], hi[j], lo[j]);
+            for (int j = 0; j < 8; ++j) {
+                tc::split_f16(x[j], hi[j], lo[j]);
+                bad |= !tc::f16_in_range(x[j]);
+            }
             uint4 vh, vl;
-            vh.x = pack_h2(hi[0], hi[1]); vh.y = pack_h2(hi[2], hi[3]); vh.z = pack_h2(hi[4], hi[5]); vh.w = pack_h2(hi[6], hi[7]);
-            vl.x = pack_h2(lo[0], lo[1]); vl.y = pack_h2(lo[2], lo[3]); vl.z = pack_h2(lo[4], lo[5]); vl.w = pack_h2(lo[6], lo[7]);
+            vh.x = tc::pack_h2(hi[0], hi[1]); vh.y = tc::pack_h2(hi[2], hi[3]); vh.z = tc::pack_h2(hi[4], hi[5]); vh.w = tc::pack_h2(hi[6], hi[7]);
+            vl.x = tc::pack_h2(lo[0], lo[1]); vl.y = tc::pack_h2(lo[2], lo[3]); vl.z = tc::pack_h2(lo[4], lo[5]); vl.w = tc::pack_h2(lo[6], lo[7]);
             out[base + (size_t)c4 * 128 + d] = vh;
             out[base + (size_t)(K / 8 + c4) * 128 + d] = vl;
         } else {
-            uint4 v;
-            __nv_bfloat162 p0 = __floats2bfloat162_rn(x[0], x[1]), p1 = __floats2bfloat162_rn(x[2], x[3]);
-            __nv_bfloat162 p2 = __floats2bfloat162_rn(x[4], x[5]), p3 = __floats2bfloat162_rn(x[6], x[7]);
-            v.x = *reinterpret_cast<uint32_t *>(&p0); v.y = *reinterpret_cast<uint32_t *>(&p1);
-            v.z = *reinterpret_cast<uint32_t *>(&p2); v.w = *reinterpret_cast<uint32_t *>(&p3);
-            out[base + (size_t)c4 * 128 + d] = v;
+            out[base + (size_t)c4 * 128 + d] = make_uint4(__float_as_uint(pack_bf16x2(x[0], x[1])), __float_as_uint(pack_bf16x2(x[2], x[3])),
+                                                          __float_as_uint(pack_bf16x2(x[4], x[5])), __float_as_uint(pack_bf16x2(x[6], x[7])));
         }
     }
-    if (bad && status != nullptr) *reinterpret_cast<volatile int32_t *>(status + 1) = 1;
+    if (bad && status != nullptr) tc::set_status(status + 1);
 }
 
 // =====================================================================================================================

@@ -4,9 +4,7 @@
 //   d_gi = [d_r, d_z, d_n],   d_gh = [d_r, d_z, d_n * r],   d_h_direct = g z
 // with d_n = g (1 - z)(1 - n^2), d_z = g (h - n) z (1 - z), d_r = d_n h_n r (1 - r).  The four GEMM-shaped products around it
 // (gi, gh, d_gi W_ih, d_gh W_hh) run on the dense kernels; as separate torch pointwise ops this was 17 % of a training step.
-#include <cuda_fp16.h>
-
-#include "common.cuh"
+#include "tc_common.cuh"
 
 namespace ptgnn {
 
@@ -65,8 +63,7 @@ extern "C" int ptgnn_b200_gru_gate_grads_f32(const float *gi, const float *gh, c
 }
 
 // Operand preparation for the parameter-gradient GEMMs (dW = A^T B with K = edges or nodes, run as three fp16 tensor-core GEMMs):
-// out row r = split16(x[index ? index[r] : r] * (scale ? *scale : 1)) with split16(v) = (hi = rn16(v), lo = rn16((v - hi) * 2^11)),
-// the forward kernels' 3xFP16 representation.  One pass: gather + scale + split (as separate torch ops -- gather, mul, two casts, sub,
+// out row r = the 3xFP16 split (tc::split_f16x8) of x[index ? index[r] : r] * (scale ? *scale : 1).  One pass: gather + scale + split (as separate torch ops -- gather, mul, two casts, sub,
 // mul -- this was a quarter of a training step).
 namespace ptgnn {
 
@@ -82,17 +79,7 @@ __global__ void __launch_bounds__(256) gather_split_kernel(const float *__restri
         const float4 a = *reinterpret_cast<const float4 *>(x + src_row * cols + c8 * 8);
         const float4 b = *reinterpret_cast<const float4 *>(x + src_row * cols + c8 * 8 + 4);
         const float v[8] = {a.x * s, a.y * s, a.z * s, a.w * s, b.x * s, b.y * s, b.z * s, b.w * s};
-        uint32_t h[4], l[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const __half2 h2 = __floats2half2_rn(v[2 * k], v[2 * k + 1]);
-            const float2 f2 = __half22float2(h2);
-            const __half2 l2 = __floats2half2_rn((v[2 * k] - f2.x) * 2048.0f, (v[2 * k + 1] - f2.y) * 2048.0f);
-            h[k] = *reinterpret_cast<const uint32_t *>(&h2);
-            l[k] = *reinterpret_cast<const uint32_t *>(&l2);
-        }
-        hi[r * c8n + c8] = make_uint4(h[0], h[1], h[2], h[3]);
-        lo[r * c8n + c8] = make_uint4(l[0], l[1], l[2], l[3]);
+        tc::split_f16x8(v, hi[r * c8n + c8], lo[r * c8n + c8]);
     }
 }
 

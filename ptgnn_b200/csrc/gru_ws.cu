@@ -263,7 +263,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gru_ws_kernel(const __grid_con
                         const float mg[4] = {in_m[r], rz_m[r], rz_m[16 + r], hn_m[r]}, cg[4] = {in_c[r], rz_c[r], rz_c[16 + r], hn_c[r]};
                         float a[4];     // i_n, r, z, h_n
 #pragma unroll
-                        for (int gt = 0; gt < 4; ++gt) a[gt] = NPROD == 3 ? fmaf(cg[gt], 1.0f / 2048.0f, mg[gt]) : mg[gt];
+                        for (int gt = 0; gt < 4; ++gt) a[gt] = NPROD == 3 ? tc::corrected(mg[gt], cg[gt]) : mg[gt];
                         const float4 b = bias_s[jb * 32 + u + e];
                         if (TABLE) {
                             const float2 *gp = gv[TABLE ? rh : 0][q];
@@ -293,22 +293,20 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gru_ws_kernel(const __grid_con
                     }
                     if (NPROD == 3) {
                         *reinterpret_cast<float2 *>(static_cast<float *>(p.out) + off + u) = make_float2(o[0], o[1]);
-                        if (p.out_packed != nullptr) {      // same split as pack_states: hi = rn16(x), lo' = rn16((x - hi) * 2^11)
-                            const __half2 h2 = __floats2half2_rn(o[0], o[1]);
-                            const float2 f2 = __half22float2(h2);
-                            const __half2 l2 = __floats2half2_rn((o[0] - f2.x) * 2048.0f, (o[1] - f2.y) * 2048.0f);
+                        if (p.out_packed != nullptr) {      // same split as pack_states
+                            uint32_t h2, l2;
+                            tc::split_f16x2(o[0], o[1], h2, l2);
                             // row r holds 2H halfs: hi at [0, H), lo' at [H, 2H)
                             __half *rowp = p.out_packed + 2 * (long long)row * p.H + jb * 32 + u;
-                            *reinterpret_cast<__half2 *>(rowp) = h2;
-                            *reinterpret_cast<__half2 *>(rowp + p.H) = l2;
+                            *reinterpret_cast<uint32_t *>(rowp) = h2;
+                            *reinterpret_cast<uint32_t *>(rowp + p.H) = l2;
                             big = fmaxf(big, fmaxf(fabsf(o[0]), fabsf(o[1])));
                         }
                     } else {
                         *reinterpret_cast<__nv_bfloat162 *>(static_cast<__nv_bfloat16 *>(p.out) + off + u) = __floats2bfloat162_rn(o[0], o[1]);
                     }
                 }
-                if (NPROD == 3 && p.out_packed != nullptr && !(big < 65504.0f) && p.status != nullptr)
-                    *reinterpret_cast<volatile int32_t *>(p.status) = 1;
+                if (NPROD == 3 && p.out_packed != nullptr && !(big < tc::F16_LIMIT) && p.status != nullptr) tc::set_status(p.status);
             }
         }
     }
@@ -320,11 +318,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gru_ws_kernel(const __grid_con
 // State-only packing (D = 0, w_ih = b_ih = NULL): P2 and the biases of the hidden side only.
 // The parts of one jb are adjacent, so one TMA box of NPART * 96 rows is a chunk's whole B operand.
 // =====================================================================================================================
-__device__ __forceinline__ void split16(float x, uint16_t &hi, uint16_t &lo) {
-    const __half h = __float2half_rn(x);
-    hi = __half_as_ushort(h);
-    lo = __half_as_ushort(__float2half_rn((x - __half2float(h)) * 2048.0f));
-}
 template <int NPROD>
 __global__ void __launch_bounds__(256) pack_gru_ws_kernel(const float *__restrict__ w_ih, const float *__restrict__ w_hh,
                                                           const float *__restrict__ b_ih, const float *__restrict__ b_hh, int H, int D,
@@ -353,10 +346,10 @@ __global__ void __launch_bounds__(256) pack_gru_ws_kernel(const float *__restric
             dst = p2; idx = ((long long)jb * NPART * 96 + n) * H + k; part_stride = 96LL * H;
         }
         if (NPROD == 3) {
-            uint16_t hi, lo;
-            split16(x, hi, lo);
-            dst[idx] = hi;
-            dst[part_stride + idx] = lo;
+            __half hi, lo;
+            tc::split_f16(x, hi, lo);
+            dst[idx] = __half_as_ushort(hi);
+            dst[part_stride + idx] = __half_as_ushort(lo);
         } else {
             const __nv_bfloat16 v = __float2bfloat16_rn(x);
             dst[idx] = *reinterpret_cast<const uint16_t *>(&v);

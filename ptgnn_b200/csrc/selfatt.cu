@@ -66,25 +66,6 @@ struct Fwd {
     static constexpr int SMEM = NP * (A_BYTES + B_BYTES + V_BYTES) + 1024;
 };
 
-// byte offset of 16-bit element (row, k), k < 64, in a K-major SWIZZLE_128B panel (16-byte chunk index XOR row & 7)
-__device__ __forceinline__ uint32_t sw128(int row, int k) {
-    return (uint32_t)(row * 128 + ((((k >> 3) ^ (row & 7)) << 4) | ((k & 7) << 1)));
-}
-
-__device__ __forceinline__ uint32_t pack_h2(__half a, __half b) {
-    return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
-}
-__device__ __forceinline__ uint32_t pack_b2(float a, float b) {
-    __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-    return *reinterpret_cast<uint32_t *>(&v);
-}
-// x -> (hi, lo') fp16 pair; false when |x| is not representable (>= 65504, inf, NaN)
-__device__ __forceinline__ bool split_f16(float x, __half &hi, __half &lo) {
-    hi = __float2half_rn(x);
-    lo = __float2half_rn((x - __half2float(hi)) * 2048.0f);
-    return fabsf(x) < 65504.0f;
-}
-
 // 8 consecutive elements of t at `off` -> one 16-byte word of 16-bit operands (bf16 as stored; fp32: hi and lo' words).
 // Rows past the chunk end read as zeros.  Returns false if an fp32 element is outside the fp16 range.
 template <bool BF16>
@@ -98,38 +79,16 @@ __device__ __forceinline__ bool fetch8(const void *t, long long off, bool valid,
     const float4 x0 = __ldg(reinterpret_cast<const float4 *>(static_cast<const float *>(t) + off));
     const float4 x1 = __ldg(reinterpret_cast<const float4 *>(static_cast<const float *>(t) + off + 4));
     const float x[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
-    uint32_t h[4], l[4];
     bool ok = true;
+    uint32_t h[4], l[4];
 #pragma unroll
-    for (int e = 0; e < 4; ++e) {
-        __half h0, l0, h1, l1;
-        ok &= split_f16(x[2 * e], h0, l0);
-        ok &= split_f16(x[2 * e + 1], h1, l1);
-        h[e] = pack_h2(h0, h1);
-        l[e] = pack_h2(l0, l1);
+    for (int e = 0; e < 4; ++e) {          // pair by pair: split_f16x8's order takes 9 more registers at dv = 64
+        tc::split_f16x2(x[2 * e], x[2 * e + 1], h[e], l[e]);
+        ok &= tc::f16_in_range(x[2 * e]) & tc::f16_in_range(x[2 * e + 1]);
     }
     hi = make_uint4(h[0], h[1], h[2], h[3]);
     lo = make_uint4(l[0], l[1], l[2], l[3]);
     return ok;
-}
-
-template <int N> __device__ __forceinline__ void fence_regs(uint32_t (&a)[N]) {
-#pragma unroll
-    for (int i = 0; i < N; ++i) asm volatile("" : "+r"(a[i])::"memory");
-}
-
-// S[64 x KB] += A[64 x 16] B[KB x 16]^T, both from shared memory
-template <int KB, bool BF16>
-__device__ __forceinline__ void mma_s(float (&d)[KB / 2], uint64_t a, uint64_t b) {
-    if constexpr (KB == 64) tc::wgmma_16_ss_n64<BF16>(d, a, b);
-    else tc::wgmma_16_ss_n32<BF16>(d, a, b);
-}
-// O[64 x min(DV, 64)] += P[64 x 16] (registers) V^T[min(DV, 64) x 16]
-template <int DV, bool BF16>
-__device__ __forceinline__ void mma_o(float (&d)[32], const uint32_t (&a)[4], uint64_t b) {
-    if constexpr (DV == 16) tc::wgmma_16_rs_n16<BF16>(d, a, b);
-    else if constexpr (DV == 32) tc::wgmma_16_rs_n32<BF16>(d, a, b);
-    else tc::wgmma_16_rs_n64<BF16>(d, a, b);
 }
 
 template <int DK, int DV, bool BF16>
@@ -155,7 +114,7 @@ __global__ void __launch_bounds__(128, 1) selfatt_fwd_kernel(const void *__restr
         const int r = it / (DK / 8), c = 8 * (it % (DK / 8));
         uint4 hi, lo;
         ok &= fetch8<BF16>(t, (tl.i0 + r) * ld + col0 + c, tl.i0 + r < tl.end, hi, lo);
-        const uint32_t off = (c / 64) * (TILE * 128) + sw128(r, c % 64);
+        const uint32_t off = (c / 64) * (TILE * 128) + tc::sw128(r, c % 64);
         *reinterpret_cast<uint4 *>(sA + off) = hi;
         if (!BF16) *reinterpret_cast<uint4 *>(sA + F::A_BYTES + off) = lo;
     }
@@ -171,7 +130,7 @@ __global__ void __launch_bounds__(128, 1) selfatt_fwd_kernel(const void *__restr
             const int r = it / (DK / 8), c = 8 * (it % (DK / 8));
             uint4 hi, lo;
             ok &= fetch8<BF16>(t, (j0 + r) * ld + col0 + DK + c, j0 + r < tl.end, hi, lo);
-            const uint32_t off = (c / 64) * (KB * 128) + sw128(r, c % 64);
+            const uint32_t off = (c / 64) * (KB * 128) + tc::sw128(r, c % 64);
             *reinterpret_cast<uint4 *>(sB + off) = hi;
             if (!BF16) *reinterpret_cast<uint4 *>(sB + F::B_BYTES + off) = lo;
         }
@@ -183,7 +142,7 @@ __global__ void __launch_bounds__(128, 1) selfatt_fwd_kernel(const void *__restr
             const uint16_t *l16 = reinterpret_cast<const uint16_t *>(&lo);
 #pragma unroll
             for (int e = 0; e < 8; ++e) {
-                const uint32_t off = sw128(c + e, r);
+                const uint32_t off = tc::sw128(c + e, r);
                 *reinterpret_cast<uint16_t *>(sV + off) = h16[e];
                 if (!BF16) *reinterpret_cast<uint16_t *>(sV + F::V_BYTES + off) = l16[e];
             }
@@ -201,10 +160,10 @@ __global__ void __launch_bounds__(128, 1) selfatt_fwd_kernel(const void *__restr
         for (int kk = 0; kk < DK / 16; ++kk) {
             const uint32_t ka = (kk / 4) * (TILE * 128) + (kk % 4) * 32, kb = (kk / 4) * (KB * 128) + (kk % 4) * 32;
             const uint64_t a_hi = tc::make_smem_desc_sw128(smem_u32(sA + ka)), b_hi = tc::make_smem_desc_sw128(smem_u32(sB + kb));
-            mma_s<KB, BF16>(sm, a_hi, b_hi);
+            tc::wgmma_16_ss<BF16, KB>(sm, a_hi, b_hi);
             if (!BF16) {
-                mma_s<KB, BF16>(sc, a_hi, tc::make_smem_desc_sw128(smem_u32(sB + F::B_BYTES + kb)));
-                mma_s<KB, BF16>(sc, tc::make_smem_desc_sw128(smem_u32(sA + F::A_BYTES + ka)), b_hi);
+                tc::wgmma_16_ss<BF16, KB>(sc, a_hi, tc::make_smem_desc_sw128(smem_u32(sB + F::B_BYTES + kb)));
+                tc::wgmma_16_ss<BF16, KB>(sc, tc::make_smem_desc_sw128(smem_u32(sA + F::A_BYTES + ka)), b_hi);
             }
         }
         tc::wgmma_commit();
@@ -217,7 +176,7 @@ __global__ void __launch_bounds__(128, 1) selfatt_fwd_kernel(const void *__restr
 #pragma unroll
         for (int i = 0; i < SR; ++i) {
             const int col = 8 * (i >> 2) + 2 * tq + (i & 1);
-            float s = BF16 ? sm[i] : fmaf(sc[i], 1.0f / 2048.0f, sm[i]);
+            float s = BF16 ? sm[i] : tc::corrected(sm[i], sc[i]);
             s = col < nvalid ? s / sqrt_dk : -INFINITY;
             sm[i] = s;
             mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s);
@@ -252,19 +211,14 @@ __global__ void __launch_bounds__(128, 1) selfatt_fwd_kernel(const void *__restr
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
                 const float p0 = sm[8 * kk + 2 * e], p1 = sm[8 * kk + 2 * e + 1];
-                if (BF16) {
-                    ah[kk][e] = pack_b2(p0, p1);
-                } else {
-                    const __half h0 = __float2half_rn(p0), h1 = __float2half_rn(p1);
-                    ah[kk][e] = pack_h2(h0, h1);
-                    al[kk][e] = pack_h2(__float2half_rn((p0 - __half2float(h0)) * 2048.0f), __float2half_rn((p1 - __half2float(h1)) * 2048.0f));
-                }
+                if (BF16) ah[kk][e] = __float_as_uint(pack_bf16x2(p0, p1));
+                else tc::split_f16x2(p0, p1, ah[kk][e], al[kk][e]);
             }
         // O += P V (accumulators and A fragments are final before the fence)
 #pragma unroll
         for (int kk = 0; kk < KB / 16; ++kk) {
-            fence_regs(ah[kk]);
-            if (!BF16) fence_regs(al[kk]);
+            tc::fence_acc(ah[kk]);
+            if (!BF16) tc::fence_acc(al[kk]);
         }
 #pragma unroll
         for (int q = 0; q < OG; ++q) {
@@ -278,10 +232,10 @@ __global__ void __launch_bounds__(128, 1) selfatt_fwd_kernel(const void *__restr
             for (int q = 0; q < OG; ++q) {
                 const uint32_t vo = q * (64 * 128) + kk * 32;
                 const uint64_t v_hi = tc::make_smem_desc_sw128(smem_u32(sV + vo));
-                mma_o<DV, BF16>(om[q], ah[kk], v_hi);
+                tc::wgmma_16_rs<BF16, (DV < 64 ? DV : 64)>(om[q], ah[kk], v_hi);
                 if (!BF16) {
-                    mma_o<DV, BF16>(oc[q], ah[kk], tc::make_smem_desc_sw128(smem_u32(sV + F::V_BYTES + vo)));
-                    mma_o<DV, BF16>(oc[q], al[kk], v_hi);
+                    tc::wgmma_16_rs<BF16, (DV < 64 ? DV : 64)>(oc[q], ah[kk], tc::make_smem_desc_sw128(smem_u32(sV + F::V_BYTES + vo)));
+                    tc::wgmma_16_rs<BF16, (DV < 64 ? DV : 64)>(oc[q], al[kk], v_hi);
                 }
             }
         tc::wgmma_commit();
@@ -292,7 +246,7 @@ __global__ void __launch_bounds__(128, 1) selfatt_fwd_kernel(const void *__restr
             if (!BF16) tc::fence_acc(oc[q]);
         }
     }
-    if (!ok && status != nullptr) *reinterpret_cast<volatile int32_t *>(status) = 1;
+    if (!ok && status != nullptr) tc::set_status(status);
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
         l_r[r] += __shfl_xor_sync(0xffffffffu, l_r[r], 1);
@@ -311,12 +265,12 @@ __global__ void __launch_bounds__(128, 1) selfatt_fwd_kernel(const void *__restr
                 const int col = 64 * q + 8 * jj + 2 * tq;
                 float v0 = om[q][i], v1 = om[q][i + 1];
                 if (!BF16) {
-                    v0 = fmaf(oc[q][i], 1.0f / 2048.0f, v0);
-                    v1 = fmaf(oc[q][i + 1], 1.0f / 2048.0f, v1);
+                    v0 = tc::corrected(v0, oc[q][i]);
+                    v1 = tc::corrected(v1, oc[q][i + 1]);
                 }
                 v0 /= l_r[r];
                 v1 /= l_r[r];
-                if (BF16) *reinterpret_cast<uint32_t *>(static_cast<__nv_bfloat16 *>(o) + obase + col) = pack_b2(v0, v1);
+                if (BF16) *reinterpret_cast<uint32_t *>(static_cast<__nv_bfloat16 *>(o) + obase + col) = __float_as_uint(pack_bf16x2(v0, v1));
                 else *reinterpret_cast<float2 *>(static_cast<float *>(o) + obase + col) = make_float2(v0, v1);
             }
         if (tq == 0) lse[(long long)row * heads + h] = m_r[r] + logf(l_r[r]);

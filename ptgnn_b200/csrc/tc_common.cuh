@@ -1,16 +1,23 @@
 // Hopper (sm_90a) tensor-core plumbing for the GEMMs of the hot path: wgmma (tf32 / f16 / bf16, fp32 accumulate in
-// registers), shared-memory matrix descriptors, mbarrier pipelines.  Hand-written inline PTX; no CUTLASS.
+// registers), shared-memory matrix descriptors, mbarrier pipelines, and the two fp32 operand formats.  Hand-written inline
+// PTX; no CUTLASS.
 //
-// fp32 accuracy on TF32 tensor cores ("3xTF32"): every fp32 operand x is split as x = hi + lo with
-// hi = x rounded to TF32 (low 13 mantissa bits zero) and lo = x - hi (exact in fp32, |lo| <= 2^-12 |x|).
-// a*b ~= a_hi*b_hi + a_hi*b_lo + a_lo*b_hi; the dropped a_lo*b_lo term (2^-24) and the TF32 truncation of the lo
-// parts (2^-23) are fp32-rounding level, which is what keeps the layer inside the north_star's 1e-5 tolerance (a single
-// TF32 product would be ~1e-3).
+// fp32 accuracy on 16-bit or TF32 tensor cores takes three products per MMA step, in one of two formats:
+//   * 3xTF32 (the round-1 unfused layers, tc_pipeline.cuh): x = hi + lo with hi = x rounded to TF32 (tf32_hi below) and
+//     lo = x - hi (exact in fp32, |lo| <= 2^-12 |x|).  a*b ~= a_hi*b_hi + a_hi*b_lo + a_lo*b_hi; the dropped a_lo*b_lo term
+//     (2^-24) and the TF32 truncation of the lo parts (2^-23) are fp32-rounding level, which keeps the layer inside 1e-5
+//     (a single TF32 product would be ~1e-3).
+//   * 3xFP16 (every other fp32 tensor-core kernel, DESIGN.md §3.1; the section "3xFP16 operand format" below): hi = rn16(x),
+//     lo' = rn16((x - hi) 2^11); main += hi hi and corr += hi lo' + lo' hi in two accumulators, value = main + 2^-11 corr.
+//     |x| >= 65504 (or inf / NaN) is not representable: the kernel sets a status word and the host raises FloatingPointError.
+// The bf16 variant of each kernel rounds each operand once to bf16 and takes one product.
 //
 // Shared-memory operand layout (K-major, rows of 128 bytes): the canonical SWIZZLE_128B K-major layout -- 8-row groups
 // of 1024 bytes, 16-byte chunk index XOR (row & 7).  One wgmma consumes K = 8 fp32 or 16 16-bit values (32 bytes) per
 // instruction; advancing K inside the 128-byte row is a +32-byte bump of the descriptor's start address.
 #pragma once
+#include <cuda_fp16.h>
+
 #include "common.cuh"
 
 namespace ptgnn {
@@ -83,6 +90,10 @@ template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wg
 template <int N> __device__ __forceinline__ void fence_acc(float (&d)[N]) {
 #pragma unroll
     for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+template <int N> __device__ __forceinline__ void fence_acc(uint32_t (&a)[N]) {       // register A fragments
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+r"(a[i])::"memory");
 }
 
 // D[64 x 32] += A[64 x 8] (tf32, registers) * B[32 x 8]^T (tf32, shared memory descriptor)
@@ -192,6 +203,22 @@ __device__ __forceinline__ void wgmma_16_rs_n48(float (&d)[32], const uint32_t (
             : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
 }
 
+// The MMAs above by width (compile time): N = 16 .. 64 columns from registers, N = 32 or 64 with both operands in shared memory
+template <bool BF16, int N>
+__device__ __forceinline__ void wgmma_16_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b) {
+    static_assert(N == 16 || N == 32 || N == 48 || N == 64, "wgmma_16_rs: N is 16, 32, 48 or 64");
+    if constexpr (N == 16) wgmma_16_rs_n16<BF16>(d, a, desc_b);
+    else if constexpr (N == 32) wgmma_16_rs_n32<BF16>(d, a, desc_b);
+    else if constexpr (N == 48) wgmma_16_rs_n48<BF16>(d, a, desc_b);
+    else wgmma_16_rs_n64<BF16>(d, a, desc_b);
+}
+template <bool BF16, int N>
+__device__ __forceinline__ void wgmma_16_ss(float (&d)[N / 2], uint64_t desc_a, uint64_t desc_b) {
+    static_assert(N == 32 || N == 64, "wgmma_16_ss: N is 32 or 64");
+    if constexpr (N == 32) wgmma_16_ss_n32<BF16>(d, desc_a, desc_b);
+    else wgmma_16_ss_n64<BF16>(d, desc_a, desc_b);
+}
+
 // Tell the compiler a value is the same in every lane (broadcast from lane 0): it may then live in a uniform register.
 __device__ __forceinline__ uint32_t warp_uniform(uint32_t v) { return __shfl_sync(0xffffffffu, v, 0); }
 __device__ __forceinline__ int warp_uniform(int v) { return __shfl_sync(0xffffffffu, v, 0); }
@@ -215,6 +242,67 @@ __device__ __forceinline__ bool elect_one() {
 // carry correctly bumps the exponent -- because two full-rate integer ops beat the conversion pipe in the converters'
 // inner loop.  Rounding overflows to inf only for |x| within 2^-12 of FLT_MAX, where the products overflow anyway.
 __device__ __forceinline__ float tf32_hi(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u); }
+
+
+// ---- 3xFP16 operand format -------------------------------------------------------------------------------------
+// The one definition of the fp32 -> fp16 (hi, lo') split, its range, its correction step and its shared-memory layout.
+// Scalar and packed conversions round identically, so every form below gives the same bits.
+
+// byte offset of 16-bit element k (k < 64) of row `row` in a K-major SWIZZLE_128B panel, and of its 16-byte chunk q (q < 8)
+__device__ __forceinline__ uint32_t sw128(int row, int k) {
+    return (uint32_t)(row * 128 + ((((k >> 3) ^ (row & 7)) << 4) | ((k & 7) << 1)));
+}
+__device__ __forceinline__ uint32_t swz(int row, int q) { return sw128(row, q << 3); }
+
+// |x| < F16_LIMIT is what the split represents; the kernels test it apart from the split (some on a running maximum) and set a
+// status word with set_status when it fails
+constexpr float F16_LIMIT = 65504.0f;
+__device__ __forceinline__ bool f16_in_range(float x) { return fabsf(x) < F16_LIMIT; }
+__device__ __forceinline__ void set_status(int32_t *word) { *reinterpret_cast<volatile int32_t *>(word) = 1; }
+
+// x -> hi = rn16(x), lo' = rn16((x - hi) 2^11)
+__device__ __forceinline__ void split_f16(float x, __half &hi, __half &lo) {
+    hi = __float2half_rn(x);
+    lo = __float2half_rn((x - __half2float(hi)) * 2048.0f);
+}
+__device__ __forceinline__ uint32_t pack_h2(__half a, __half b) {
+    return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
+}
+// pairs (x[2 i], x[2 i + 1]) -> packed hi and lo' words (x[2 i] in the low half), with packed conversions.  Every hi conversion
+// is issued first: pair by pair, the fused write-out's registers are allocated differently and the packing kernels take more.
+template <int N>
+__device__ __forceinline__ void split_f16_pairs(const float (&x)[2 * N], uint32_t (&hi)[N], uint32_t (&lo)[N]) {
+    __half2 h[N];
+    float2 f[N];
+#pragma unroll
+    for (int i = 0; i < N; ++i) h[i] = __floats2half2_rn(x[2 * i], x[2 * i + 1]);
+#pragma unroll
+    for (int i = 0; i < N; ++i) f[i] = __half22float2(h[i]);
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+        const __half2 l = __floats2half2_rn((x[2 * i] - f[i].x) * 2048.0f, (x[2 * i + 1] - f[i].y) * 2048.0f);
+        hi[i] = *reinterpret_cast<const uint32_t *>(&h[i]);
+        lo[i] = *reinterpret_cast<const uint32_t *>(&l);
+    }
+}
+__device__ __forceinline__ void split_f16x2(float a, float b, uint32_t &hi, uint32_t &lo) {
+    const float x[2] = {a, b};
+    uint32_t h[1], l[1];
+    split_f16_pairs<1>(x, h, l);
+    hi = h[0];
+    lo = l[0];
+}
+__device__ __forceinline__ void split_f16x8(const float (&x)[8], uint4 &hi, uint4 &lo) {
+    uint32_t h[4], l[4];
+    split_f16_pairs<4>(x, h, l);
+    hi = make_uint4(h[0], h[1], h[2], h[3]);
+    lo = make_uint4(l[0], l[1], l[2], l[3]);
+}
+// main + 2^-11 corr
+__device__ __forceinline__ float corrected(float main, float corr) { return fmaf(corr, 0x1p-11f, main); }
+
+// the bf16 variant: one rounding (pairs: pack_bf16x2 in common.cuh)
+__device__ __forceinline__ float round_bf16(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
 
 }  // namespace tc
 }  // namespace ptgnn

@@ -89,8 +89,6 @@ struct MmaGroup {       // per K-step: B rows [row_off, row_off + n) -> accumula
     int n, row_off, col_off;   // row_off are multiples of 32 (the accumulators are zeroed at the start of every tile)
 };
 
-__device__ __forceinline__ uint32_t swz(int row, int q) { return (uint32_t)(row * 128 + ((q ^ (row & 7)) << 4)); }
-
 __device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
     asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}" ::"r"(smem_u32(bar)), "r"(bytes)
                  : "memory");

@@ -33,6 +33,7 @@ import torch.nn.functional as F_
 
 import fused_reference as FR
 import unfused_reference as UR
+from helpers import split_f16
 
 U = FR.U
 ABS_F16 = FR.ABS_F16
@@ -56,9 +57,7 @@ def gather_split(x: torch.Tensor, index: Optional[torch.Tensor], scale: Optional
         v = v.index_select(0, index.cpu().long())
     if scale is not None:
         v = v * torch.tensor(scale, dtype=torch.float32)
-    hi = v.half()
-    lo = ((v - hi.float()) * 2048.0).half()
-    return hi, lo
+    return split_f16(v)
 
 
 def split_value(x: torch.Tensor, scale: float = 1.0, index: Optional[torch.Tensor] = None) -> torch.Tensor:

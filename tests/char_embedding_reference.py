@@ -24,6 +24,8 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
+from helpers import split_f16
+
 PRE = "_CharUnitEmbedder__"
 FP32_REL_L2 = 1e-5
 BF16_EMU_REL_L2 = 2e-3
@@ -112,9 +114,7 @@ def emulate_bf16(chars, w1, b1, w2, b2, w3, drop_bias: Optional[int] = None) -> 
 
 
 def _split(x: torch.Tensor):
-    x = x.to(torch.float32)
-    hi = x.half()
-    lo = ((x - hi.float()) * 2048.0).half()
+    hi, lo = split_f16(x)
     return hi.double(), lo.double()
 
 

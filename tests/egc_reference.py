@@ -25,6 +25,7 @@ from typing import Sequence
 import torch
 
 import fused_reference as R
+from helpers import split_f16
 
 U = R.U
 
@@ -95,8 +96,8 @@ def emulate_f32(h, adj, weights, cw, cb, reduce: str, heads: int, bases: int, co
     out_dim = weights[0].shape[0] // bases
 
     def split(x):
-        hi = x.half().float()
-        return hi, ((x - hi) * 2048.0).half().float()
+        hi, lo = split_f16(x)
+        return hi.float(), lo.float()
 
     hh, hl = split(h.float())
     tgts, msgs = [], []

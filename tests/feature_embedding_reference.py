@@ -13,6 +13,8 @@ import math
 
 import torch
 
+from helpers import split_f16
+
 ACTIVATIONS = ("none", "relu", "tanh", "gelu")
 ACT_SLOPE = 1.13          # max |GELU'(x)| (1.129 at x = 2.42); ReLU, Tanh: 1
 
@@ -75,9 +77,7 @@ def bound(x: torch.Tensor, w: torch.Tensor, act: str, bf16: bool = False) -> tor
 
 
 def _split(t: torch.Tensor):
-    t = t.float()
-    hi = t.half()
-    lo = ((t - hi.float()) * 2048.0).half()
+    hi, lo = split_f16(t)
     return hi.double(), lo.double()
 
 

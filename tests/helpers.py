@@ -12,6 +12,14 @@ GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 TOL = 1e-5  # north_star: fp32 node representations within 1e-5 (scaled by max(1, |ref|))
 
 
+def split_f16(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The kernels' 3xFP16 split of x rounded to fp32 (csrc/tc_common.cuh): (hi, lo') fp16 tensors on x's device, with
+    hi = fl16(x) and lo' = fl16(2^11 (x - hi)), bit for bit what the kernels compute."""
+    x = x.float()
+    hi = x.half()
+    return hi, ((x - hi.float()) * 2048.0).half()
+
+
 def load_golden(name: str) -> Dict[str, np.ndarray]:
     with np.load(os.path.join(GOLDEN_DIR, name + ".npz"), allow_pickle=False) as z:
         return {k: z[k] for k in z.files}

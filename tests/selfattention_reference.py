@@ -10,6 +10,8 @@ import math
 import torch
 import torch.nn.functional as F
 
+from helpers import split_f16
+
 PREFIX = "_MultiHeadSelfAttentionMessagePassing__"
 U = 2.0 ** -24          # unit roundoff of fp32
 
@@ -83,8 +85,8 @@ def bound(t: torch.Tensor, n2g: torch.Tensor, heads: int, dk: int, max_num_nodes
 
 
 def _split16(x: torch.Tensor):
-    hi = x.half().float()
-    return hi, ((x - hi) * 2048.0).half().float()
+    hi, lo = split_f16(x)
+    return hi.float(), lo.float()
 
 
 def emulate_kernel(t: torch.Tensor, n2g: torch.Tensor, heads: int, dk: int, max_num_nodes: int, corrections: bool = True) -> torch.Tensor:

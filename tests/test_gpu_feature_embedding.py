@@ -10,6 +10,7 @@ from torch import nn
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import feature_embedding_reference as R  # noqa: E402
+from helpers import split_f16  # noqa: E402
 
 import ptgnn_b200 as P  # noqa: E402
 from ptgnn_b200 import _native as N  # noqa: E402
@@ -125,8 +126,7 @@ def test_packed_output_is_the_split_of_the_fp32_output(act):
         out, packed, _ = EMB.native_feature_embed(x, prepared, 64, N.ACT_NONE if act == "none" else {
             "relu": N.ACT_RELU, "tanh": N.ACT_TANH, "gelu": N.ACT_GELU}[act], want_packed=True)
         assert packed.numel() == N.lib().ptgnn_b200_packed_state_bytes(n, 64)
-        hi = out.half()
-        lo = ((out - hi.float()) * 2048.0).half()
+        hi, lo = split_f16(out)
         rows = packed[:n * 64 * 4].view(torch.float16).view(n, 128)
         assert torch.equal(rows[:, :64].view(torch.int16), hi.view(torch.int16))
         assert torch.equal(rows[:, 64:].view(torch.int16), lo.view(torch.int16))

@@ -19,7 +19,7 @@ import torch
 import fused_reference as FR
 import global_exchange_reference as GX
 import unfused_reference as R
-from helpers import gated_oracle_args, random_adjacency
+from helpers import gated_oracle_args, random_adjacency, split_f16
 
 pytestmark = pytest.mark.gpu
 
@@ -51,9 +51,7 @@ def _twice(fn):
 
 def _packed_split(out: torch.Tensor) -> torch.Tensor:
     """The fp16 (hi | lo') rows of fp32 rows, with round-to-nearest conversions: hi = fl16(x), lo' = fl16(2^11 (x - hi))."""
-    hi = out.to(torch.float16)
-    lo = ((out - hi.float()) * 2048.0).to(torch.float16)
-    return torch.cat([hi, lo], 1)
+    return torch.cat(split_f16(out), 1)
 
 
 # ---- layer instance ------------------------------------------------------------------------------------------------------

@@ -11,13 +11,13 @@ import torch
 
 import fused_reference as FR
 import unfused_reference as R
+from helpers import split_f16
 
 WORST = {}
 
 
 def _split(x: torch.Tensor):
-    hi = x.float().to(torch.float16)
-    lo = ((x.float() - hi.float()) * 2048.0).to(torch.float16)
+    hi, lo = split_f16(x)
     return hi.double(), lo.double()
 
 
