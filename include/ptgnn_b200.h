@@ -210,6 +210,12 @@ size_t ptgnn_b200_block_plan_workspace_bytes(int64_t num_nodes, int64_t num_edge
 int ptgnn_b200_block_plan_build(int64_t num_nodes, int32_t num_types, const int64_t *type_off /*[host]*/,
                                 const int32_t *src32, const int32_t *tgt32, int32_t block_targets, int32_t *group_off,
                                 int32_t *src_f, uint8_t *tl_f, void *workspace, size_t workspace_bytes, void *stream);
+/* The same block plan, and eid_f[E]: the cat(types) position e of the edge at sorted position j (src_f[j] == src32[eid_f[j]]), which
+ * the per-edge dropout mask is defined on. */
+int ptgnn_b200_block_plan_build_with_edge_ids(int64_t num_nodes, int32_t num_types, const int64_t *type_off /*[host]*/,
+                                              const int32_t *src32, const int32_t *tgt32, int32_t block_targets, int32_t *group_off,
+                                              int32_t *src_f, uint8_t *tl_f, int32_t *eid_f, void *workspace, size_t workspace_bytes,
+                                              void *stream);
 
 /* 1 if these dimensions run on the fused layer kernels (message_dim == 128; state_dim in {64, 128} for fp32 states,
  * {64, 128, 256} for bf16 states); otherwise use the unfused entry points above. */
@@ -241,6 +247,45 @@ int ptgnn_b200_gated_forward_fused(int32_t bf16_states, const void *node_states,
                                    void *out_states, void *packed_states_out /* NULL: not written */, void *workspace,
                                    size_t workspace_bytes, void *weight_cache, size_t weight_cache_bytes, int32_t cache_valid,
                                    void *stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Per-edge dropout of GatedMessagePassingLayer in training mode (gatedmessagepassing.py:59: nn.Dropout on the gathered [E_t, H]
+ * source rows), fp32 states, unsharded.  The mask is a pure function of a key, so nothing but the key is kept for the backward.
+ * Element (e, k), e = the edge's cat(types) position, k = the source feature: u = word k % 4 of Philox4x32-10 with
+ * counter (e, k / 4, 0, 0) and key (key[0], key[1]); kept iff u >= round(p 2^32), and a kept element is scaled by 1 / (1 - p).
+ * p = 1 drops every element (messages are exactly 0).  key: two uint32 words in device memory; nothing synchronises.
+ *
+ * edge_dropout_bits: bits [num_edges, K / 32] uint32, bit k % 32 of word k / 32 set for a kept element; row j holds edge eid_f[j]
+ * (eid_f NULL: edge j).  K % 32 == 0.
+ * edge_dropout_apply_f32: out[r, c] = x[index ? index[r] : r, c] / (1 - p) where bit (r, c) of `bits` ([rows, cols / 32]) is set, else 0;
+ * in place (out == x, index NULL) is fine.
+ * gather_split_f16_masked: ptgnn_b200_gather_split_f16 of the masked rows (elements whose bit is clear are 0; no 1 / (1 - p)). */
+int ptgnn_b200_edge_dropout_bits(const uint32_t *key, int64_t num_edges, int32_t K, float p, const int32_t *eid_f, uint32_t *bits,
+                                 void *stream);
+int ptgnn_b200_edge_dropout_apply_f32(const uint32_t *bits, int64_t rows, int32_t cols, float p, const float *x, const int32_t *index,
+                                      float *out, void *stream);
+int ptgnn_b200_gather_split_f16_masked(const float *x, const int32_t *index, int64_t rows_out, int32_t cols, const float *scale,
+                                       const uint32_t *bits, void *hi, void *lo, void *stream);
+/* ptgnn_b200_gated_forward_fused (fp32 states, no gather_states) with the per-edge dropout applied inside the fused aggregation:
+ * eid_f from ptgnn_b200_block_plan_build_with_edge_ids for the same block plan, num_edges = E.  The 1 / (1 - p) scale is folded into
+ * the packed edge weights, so a weight_cache filled here holds scaled weights: keep it apart from the unscaled one (and per p). */
+size_t ptgnn_b200_gated_fused_dropout_workspace_bytes(int64_t num_nodes, int64_t num_edges, int32_t num_types, int32_t state_dim,
+                                                      int32_t message_dim);
+int ptgnn_b200_gated_forward_fused_dropout(const float *node_states, const void *packed_states_in /* NULL: packed here */, int64_t num_nodes,
+                                           int64_t num_edges, int32_t state_dim, int32_t message_dim, int32_t num_types,
+                                           const ptgnn_b200_block_plan *block_plan, const int32_t *eid_f, const int32_t *row_ptr,
+                                           const float *const *edge_weights /*[host] T device pointers, fp32*/, const float *gru_w_ih,
+                                           const float *gru_w_hh, const float *gru_b_ih, const float *gru_b_hh, int32_t reduce,
+                                           const uint32_t *key, float p, void *out_states, void *packed_states_out /* NULL: not written */,
+                                           void *workspace, size_t workspace_bytes, void *weight_cache, size_t weight_cache_bytes,
+                                           int32_t cache_valid, void *stream);
+/* The fp32 aggregate alone, reduce_{e -> v} W_t(e) dropout(h[src(e)]) [num_nodes, 128], with the same mask for the same key (any
+ * reduction; the layer's backward re-computes sum / mean with it). */
+size_t ptgnn_b200_fused_aggregate_dropout_workspace_bytes(int64_t num_nodes, int64_t num_edges, int32_t num_types, int32_t state_dim);
+int ptgnn_b200_fused_aggregate_dropout(const float *node_states, int64_t num_nodes, int64_t num_edges, int32_t state_dim, int32_t num_types,
+                                       const ptgnn_b200_block_plan *block_plan, const int32_t *eid_f, const int32_t *row_ptr,
+                                       const float *const *edge_weights, int32_t reduce, const uint32_t *key, float p, float *out,
+                                       void *workspace, size_t workspace_bytes, void *stream);
 
 /* MlpMessagePassingLayer.forward through the fused kernel (contract of ptgnn_b200_mlp_forward); the message
  * activation and the LayerNorm run in the fused kernel's write-out.  weight_cache (optional, fp32 states; ignored for bf16

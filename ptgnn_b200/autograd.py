@@ -17,10 +17,15 @@ The GRUs (gated layer, GruGlobalStateUpdate) take their gate pre-activations and
 tail (activation, LayerNorm, dense layer: mlpmessagepassing.py:114-117) is differentiated by a local ``torch.autograd.grad`` over
 library ops, and its output Dropout is a torch op applied outside the Function.
 
-The gated layer's training-mode dropout (a per-edge mask on the gathered rows, gatedmessagepassing.py:59) and edge features under
-autograd need the gathered ``[E_t, H]`` rows to exist: they run as the reference writes the layer, with the Linear / scatter / GRUCell
-as differentiable native operators (``gated_forward_composed``).  fp32 states only.  Parity: ``tests/test_gpu_backward.py`` against ``torch.autograd`` through the CPU oracle (1e-4).
+The gated layer's training-mode dropout (a per-edge mask on the gathered rows, gatedmessagepassing.py:59) runs on the fused kernel
+where the eval-mode layer does (fp32 states, unsharded, no edge features): the mask is a pure function of a per-call key
+(csrc/edge_dropout.cuh), the forward applies it inside the fused aggregation, and ``_GatedDropoutFunction`` saves the key instead of
+any ``[E, H]`` tensor and regenerates the mask in its backward (``_aggregation_backward``'s ``drop``).  Other dimensions, and edge
+features under autograd, run as the reference writes the layer, with the Linear / scatter / GRUCell as differentiable native operators
+(``gated_forward_composed``).  fp32 states only.  Parity: ``tests/test_gpu_backward.py`` against ``torch.autograd`` through the CPU
+oracle (1e-4); ``tests/test_gpu_gated_dropout.py`` for the fused dropout.
 """
+import ctypes
 import threading
 from typing import List, Optional, Tuple
 
@@ -66,11 +71,13 @@ def _pow2_scale(x: torch.Tensor):
     return scale, 1.0 / scale
 
 
-def _split16(x: torch.Tensor, index: Optional[torch.Tensor] = None, scale=None):
+def _split16(x: torch.Tensor, index: Optional[torch.Tensor] = None, scale=None, bits: Optional[torch.Tensor] = None):
     """fp32 [rows, cols] -> (hi, lo, inv_scale) with (hi + lo / 2048) * inv_scale ~= x[index] (index: int32 row ids, None = all rows in
     order); hi, lo fp16: the 3xFP16 split of the forward kernels (22 significant bits) of x times ``_pow2_scale(x)``.  The scaling keeps
     gradients (routinely below fp16's normal range) and states beyond fp16's range (PTGNN_B200_FP32_MODE=tf32) at full precision.
-    scale: that pair when the caller already has it.  Gather, scaling and split are one native pass; nothing synchronises."""
+    scale: that pair when the caller already has it.  bits: per-edge dropout keep bits of the output rows (``edge_dropout_bits``):
+    dropped elements are split as 0 (without the 1 / (1 - p) scale).  Gather, scaling, mask and split are one native pass; nothing
+    synchronises."""
     rows = x.shape[0] if index is None else int(index.shape[0])
     cols = x.shape[1]
     hi = torch.empty(rows, cols, dtype=torch.float16, device=x.device)
@@ -79,6 +86,10 @@ def _split16(x: torch.Tensor, index: Optional[torch.Tensor] = None, scale=None):
         return hi, lo, 1.0
     scale, inv = _pow2_scale(x) if scale is None else scale
     x = x.contiguous()
+    if bits is not None:
+        N.call("ptgnn_b200_gather_split_f16_masked", x.device, N.ptr(x), N.ptr(index), rows, cols, N.ptr(scale), N.ptr(bits), N.ptr(hi),
+               N.ptr(lo))
+        return hi, lo, inv
     if cols % 8 != 0:      # rare shapes: torch ops
         v = x if index is None else x.index_select(0, index.long())
         v = v * scale
@@ -175,29 +186,44 @@ class _GatedLayerFunction(torch.autograd.Function):
         return (None, None, None, d_h, d_w_ih, d_w_hh, d_b_ih, d_b_hh, *d_W)
 
 
-def _recompute_aggregate(plan, h, W, reduce_name):
+def _recompute_aggregate(plan, h, W, reduce_name, drop=None):
     """(agg, arg) of agg = reduce_{e -> v} W_t(e) h[src(e)]: arg, for max / min, is which edge won each (target, feature), from the
-    messages and the segmented reduce; sum / mean run the fused kernel where it takes the dimensions, and arg is None."""
+    messages and the segmented reduce; sum / mean run the fused kernel where it takes the dimensions, and arg is None.  drop: the
+    per-edge dropout of the source rows (``EdgeDropout``): sum / mean on the fused kernel with the same key, max / min from the masked,
+    scaled rows."""
+    if drop is not None:
+        if reduce_name in ("max", "min"):
+            x = drop.apply(h, plan.src32)                                    # [E, H] dropout(h[src(e)]), cat(types) order
+            msg = torch.empty(plan.num_edges, W[0].shape[0], dtype=torch.float32, device=h.device)
+            for t, w in enumerate(W):
+                lo, hi = plan.type_off[t], plan.type_off[t + 1]
+                if hi > lo:
+                    msg[lo:hi] = C.linear(x[lo:hi], w)
+            del x
+            return C.segment_reduce(msg, plan, N.REDUCE[reduce_name], return_arg=True)
+        return aggregate_dropout(plan, h, W, N.REDUCE[reduce_name], drop.key, drop.p), None
     if reduce_name in ("max", "min"):
         msg = C.edge_messages(plan, h, None, W, False)                       # [E, D], cat(types) order
         return C.segment_reduce(msg, plan, N.REDUCE[reduce_name], return_arg=True)
     return C.aggregate(plan, h, W, N.REDUCE[reduce_name]), None
 
 
-def _aggregation_backward(plan, adj, h, W, d_agg, reduce_name, arg, d_h, b_all=None, *, W_tgt=None, d_msg=None):
+def _aggregation_backward(plan, adj, h, W, d_agg, reduce_name, arg, d_h, b_all=None, *, W_tgt=None, d_msg=None, drop=None):
     """Backward of agg = reduce_{e -> v} W_t(e) [h[src(e)] ; h[tgt(e)]] (bias-free per-type Linear, then sum / mean / max / min) from
     d_agg [N, D]: returns (d_W per type, d_h + the h part).  W: the columns of W_t that multiply h_src; W_tgt: those that multiply h_tgt
     (None: the messages read h_src only), and d_W[t] is then [d W_src ; d W_tgt] along dim 1.  arg: the winning edge ids of max / min
     ([N, D], E for empty targets).  d_msg: the per-edge message gradients [E, D] when the caller has them (PNA's backward); they replace
     the routing of d_agg through arg.  b_all: the 3xFP16 split of the gathered source states, ``_split16(h, plan.src32)``, when the
-    caller reuses it across calls.
+    caller reuses it across calls.  drop: the per-edge dropout of the source rows (``EdgeDropout``, h_src only): d W_t from the masked,
+    scaled rows, and d h through the per-edge branch below with the mask applied to each edge's row gradient, for every reduction.
     sum / mean: split fp16 GEMMs over edges, and the forward's aggregation with W_t^T on the transposed graph (and, for h_tgt, on the
     graph of each edge's target to itself); otherwise: split fp16 GEMMs over the message gradients, and per type the native linear
     with W_t^T and scatter-add by source (and by target)."""
     num_nodes = h.shape[0]
     E = plan.num_edges
-    dense = d_msg is None and reduce_name in ("sum", "mean")
-    if dense:
+    by_target = d_msg is None and reduce_name in ("sum", "mean")       # every edge's message gradient is its target's d_agg row
+    dense = by_target and drop is None
+    if by_target:
         if reduce_name == "mean":
             d_agg = d_agg / _mean_divisor(plan)[:, None]
         d_agg = d_agg.contiguous()
@@ -207,7 +233,10 @@ def _aggregation_backward(plan, adj, h, W, d_agg, reduce_name, arg, d_h, b_all=N
         if d_msg is None:
             d_msg = _route_to_arg(d_agg, arg, E)
         a_all = _split16(d_msg)
-    if b_all is None:
+    if b_all is None and drop is not None:                               # [E, H] dropout(h[src(e)])
+        b_hi, b_lo, b_inv = _split16(h, plan.src32, bits=drop.bits)
+        b_all = (b_hi, b_lo, b_inv * drop.scale)
+    elif b_all is None:
         b_all = _split16(h, plan.src32)                                  # [E, H] source states
     g_all = None if W_tgt is None else _split16(h, plan.tgt32)           # [E, H] target states
     d_W = []
@@ -220,8 +249,11 @@ def _aggregation_backward(plan, adj, h, W, d_agg, reduce_name, arg, d_h, b_all=N
         d_w = _mm_t_split(a, _slice(b_all, lo, hi))
         d_W.append(d_w if W_tgt is None else torch.cat([d_w, _mm_t_split(a, _slice(g_all, lo, hi))], dim=1))
         if not dense:
-            part = d_msg[lo:hi].contiguous()
-            d_h = d_h + scatter_sum(C.linear(part, w.t().contiguous()), src, dim=0, dim_size=num_nodes)
+            part = d_msg[lo:hi].contiguous() if d_msg is not None else d_agg.index_select(0, plan.tgt32[lo:hi].long())
+            rows = C.linear(part, w.t().contiguous())
+            if drop is not None:
+                drop.apply(rows, None, lo, out=rows)
+            d_h = d_h + scatter_sum(rows, src, dim=0, dim_size=num_nodes)
             if W_tgt is not None:
                 d_h = d_h + scatter_sum(C.linear(part, W_tgt[t].t().contiguous()), tgt, dim=0, dim_size=num_nodes)
     if dense and E > 0:
@@ -236,6 +268,92 @@ def _aggregation_backward(plan, adj, h, W, d_agg, reduce_name, arg, d_h, b_all=N
 
 def gated_forward_with_grad(layer, node_states, adjacency_lists, reduce_name, w_ih, w_hh, b_ih, b_hh, weights):
     return _GatedLayerFunction.apply(layer, adjacency_lists, reduce_name, node_states, w_ih, w_hh, b_ih, b_hh, *weights)
+
+
+# =====================================================================================================================
+# Per-edge dropout of the gated layer on the fused kernel (csrc/edge_dropout.cuh: the mask is a pure function of a per-call key)
+# =====================================================================================================================
+def draw_dropout_key(device) -> torch.Tensor:
+    """The key of one layer call: two 32-bit words (int32 [2], device) from torch's default CUDA generator -- ``torch.manual_seed``
+    reproduces it, every call draws a new one, and nothing synchronises."""
+    return torch.empty(2, dtype=torch.int64, device=device).random_().to(torch.int32)
+
+
+def dropout_scale(p: float) -> float:
+    """1 / (1 - p); 0 for p = 1 (every element is dropped: never a multiplication by inf)."""
+    return 1.0 / (1.0 - p) if p < 1.0 else 0.0
+
+
+def edge_dropout_bits(key: torch.Tensor, num_edges: int, K: int, p: float, eid: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """[E, K / 32] int32 keep bits (bit k % 32 of word k / 32) of the edges eid[j] (None: edge j, cat(types) order)."""
+    bits = torch.empty(num_edges, K // 32, dtype=torch.int32, device=key.device)
+    N.call("ptgnn_b200_edge_dropout_bits", key.device, N.ptr(key), num_edges, K, float(p), N.ptr(eid), N.ptr(bits))
+    return bits
+
+
+class EdgeDropout:
+    """The per-edge dropout of one layer call in the backward: its key, p, and the keep bits in cat(types) order."""
+
+    def __init__(self, key: torch.Tensor, p: float, num_edges: int, K: int):
+        self.key, self.p, self.scale = key, float(p), dropout_scale(p)
+        self.bits = edge_dropout_bits(key, num_edges, K, p)
+
+    def apply(self, x: torch.Tensor, index: Optional[torch.Tensor], row0: int = 0, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Rows r of the result = dropout(x[index[r]]) (index None: x[r]) with the mask of edge row0 + r; ``out=x`` works in place."""
+        rows = x.shape[0] if index is None else int(index.shape[0])
+        if out is None:
+            out = torch.empty(rows, x.shape[1], dtype=torch.float32, device=x.device)
+        N.call("ptgnn_b200_edge_dropout_apply_f32", x.device, N.ptr(self.bits[row0:]) if rows else None, rows, x.shape[1], self.p, N.ptr(x),
+               N.ptr(index), N.ptr(out))
+        return out
+
+
+def aggregate_dropout(plan, h: torch.Tensor, W, reduce_code: int, key: torch.Tensor, p: float) -> torch.Tensor:
+    """``reduce_{e -> v} W_t(e) dropout(h[src(e)])`` [N, 128] fp32 on the fused kernel, with the mask of ``key``."""
+    num_nodes, H = h.shape
+    lib = N.lib()
+    bp = plan.block_plan(edge_ids=True)
+    out = torch.empty(num_nodes, W[0].shape[0], dtype=torch.float32, device=h.device)
+    ws_bytes = lib.ptgnn_b200_fused_aggregate_dropout_workspace_bytes(num_nodes, plan.num_edges, plan.num_types, H)
+    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=h.device)
+    N.call("ptgnn_b200_fused_aggregate_dropout", h.device, N.ptr(h), num_nodes, plan.num_edges, H, plan.num_types, ctypes.byref(bp),
+           N.ptr(plan.block_edge_ids), N.ptr(plan.row_ptr), N.ptr_table(W), reduce_code, N.ptr(key), float(p), N.ptr(out), N.ptr(ws), ws_bytes)
+    return out
+
+
+class _GatedDropoutFunction(torch.autograd.Function):
+    """The gated layer in training mode with per-edge dropout, on the fused kernel.  Saves h, the parameters and the 8-byte key: no
+    ``[E, H]`` tensor (gathered rows or mask) is kept for the backward, which regenerates the mask from the key."""
+
+    @staticmethod
+    def forward(ctx, layer, adjacency_lists, reduce_name, p, h, w_ih, w_hh, b_ih, b_hh, *weights):
+        key = draw_dropout_key(h.device)
+        with torch.no_grad():
+            out = layer._forward_fused_dropout(h.detach(), adjacency_lists, key, p)
+        ctx.save_for_backward(h, key, w_ih, w_hh, b_ih, b_hh, *weights)
+        ctx.adjacency_lists, ctx.reduce_name, ctx.p = adjacency_lists, reduce_name, p
+        return out
+
+    @staticmethod
+    @once_differentiable          # the backward runs native kernels: no double backward
+    def backward(ctx, grad_out):
+        h, key, w_ih, w_hh, b_ih, b_hh, *weights = ctx.saved_tensors
+        adj: List[Tuple[torch.Tensor, torch.Tensor]] = ctx.adjacency_lists
+        g = grad_out.contiguous().float()
+        h = h.detach().contiguous()
+        W = [w.detach().contiguous() for w in weights]
+        w_ih, w_hh = w_ih.detach().contiguous(), w_hh.detach().contiguous()
+        plan = plan_for(adj, h.shape[0])
+        drop = EdgeDropout(key, ctx.p, plan.num_edges, h.shape[1])
+        agg, arg = _recompute_aggregate(plan, h, W, ctx.reduce_name, drop)
+        d_agg, d_h, d_w_ih, d_w_hh, d_b_ih, d_b_hh = _gru_backward(g, agg, h, w_ih, w_hh, b_ih.detach(), b_hh.detach())
+        del agg
+        d_W, d_h = _aggregation_backward(plan, adj, h, W, d_agg, ctx.reduce_name, arg, d_h, drop=drop)
+        return (None, None, None, None, d_h, d_w_ih, d_w_hh, d_b_ih, d_b_hh, *d_W)
+
+
+def gated_dropout_with_grad(layer, node_states, adjacency_lists, reduce_name, p, w_ih, w_hh, b_ih, b_hh, weights):
+    return _GatedDropoutFunction.apply(layer, adjacency_lists, reduce_name, float(p), node_states, w_ih, w_hh, b_ih, b_hh, *weights)
 
 
 # =====================================================================================================================
@@ -465,8 +583,8 @@ class _GRUCellFn(torch.autograd.Function):
 def gated_forward_composed(layer_weights, gru, node_states, adjacency_lists, edge_features, reduce_name, dropout_p: float):
     """GatedMessagePassingLayer.forward exactly as the reference writes it (gatedmessagepassing.py:46-69) -- gather, cat with the edge
     features, Dropout on the per-edge rows, per-type Linear, scatter, GRUCell -- with the Linear / scatter / GRUCell on the native
-    kernels as differentiable operators.  Used where the [E_t, H] gathered rows must exist: per-edge dropout (training mode) and
-    edge features under autograd."""
+    kernels as differentiable operators.  Used where the [E_t, H] gathered rows must exist: per-edge dropout (training mode) at
+    dimensions the fused kernel does not take (``_GatedDropoutFunction`` serves the others) and edge features under autograd."""
     num_nodes = node_states.shape[0]
     plan = plan_for(adjacency_lists, num_nodes)
     msgs = []

@@ -18,10 +18,12 @@ using tc::mbar_init;
 using tc::mbar_wait;
 
 // ---- geometry ------------------------------------------------------------------------------------------------------
-// Roles (16 warps): 0-3 and 4-7 CONSUMERS, two warpgroups | 8-9 ROW GATHERERS | 10 SCHEDULER | 11 idle | 12-15 REDUCER.
+// Roles (16 warps): 0-3 and 4-7 CONSUMERS, two warpgroups | 8-9 ROW GATHERERS | 10 SCHEDULER | 11 MASKER (DROP instances; idle
+// otherwise) | 12-15 REDUCER.
 constexpr int NUM_THREADS = 16 * 32;
 constexpr int GATHER_WARP0 = 8, GATHER_THREADS = 64;
 constexpr int SCHED_WARP = 10;
+constexpr int MASK_WARP = 11;
 constexpr int REDUCER_WARP0 = 12;
 constexpr int SCHED_READER_WARPS = 8 + 2 + 4;          // readers of the scheduler's table: consumers, gatherers, reducer
 constexpr int META_RING = 8;
@@ -64,7 +66,7 @@ struct Geom {
     static constexpr int AGG_OFF = RING_BYTES + ACC_BYTES;
     static constexpr int smem_bytes(int B) { return 1024 + RING_BYTES + ACC_BYTES + agg_bytes(B) + SMEM_TAIL; }
     static_assert(smem_bytes(kMaxBlockTargets) <= 232448, "shared memory budget");
-    static_assert(2 * NUM_SLOTS + 2 * SCHED_RING + 2 <= 256 / 8, "barrier area");
+    static_assert(3 * NUM_SLOTS + 2 * SCHED_RING + 2 <= 256 / 8, "barrier area");      // x_landed: DROP instances only
     // the reducer reads a sub-group's Meta at most NUM_SLOTS + 2 sub-groups behind its writer (see the reducer)
     static_assert(NUM_SLOTS + 2 < META_RING, "Meta ring too short for the slot count");
 };
@@ -81,6 +83,7 @@ struct Params {
     unsigned long long *trace;     // debug (PTGNN_FUSED_TRACE=1): per-role event timeline of CTA 0, else nullptr
     Epilogue epi;
     EgcEpilogue egc;               // read by the EPI_EGC instances only
+    const uint32_t *drop_bits;     // DROP instances: [E, K / 32] keep bits in block-plan order (edge_dropout.cuh)
 };
 // the write-out, fixed at compile time so that each instance carries only its own: the aggregate (+ mean / activation / LayerNorm)
 // or the EGC combination of the bases
@@ -358,7 +361,10 @@ __device__ __forceinline__ void write_out_block_egc(const Params *p, uint32_t ag
     }
 }
 
-template <int NPROD, int K, int NSEG, int RED, int EPI>
+// DROP: per-edge dropout of the gathered rows (fp32 states, one segment, the aggregate write-out).  The masker warp clears the hi
+// and lo' halves of every dropped feature in the landed slot before the consumers see it; the scale 1 / (1 - p) is folded into the
+// packed weights by the host.
+template <int NPROD, int K, int NSEG, int RED, int EPI, bool DROP = false>
 __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const __grid_constant__ Params p) {
     constexpr int NPART = NPROD == 3 ? 2 : 1;                      // hi | lo' parts of a row / of the weights
     constexpr int ROW_BYTES = K * 2 * NPART;                       // one packed state row
@@ -369,6 +375,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
     constexpr int NUM_SLOTS = G::NUM_SLOTS, SLOT_BYTES = G::SLOT_BYTES;
     static_assert(NT == G::NT, "slot size");
     constexpr bool BF16 = NPROD == 1;
+    static_assert(!DROP || (NPROD == 3 && NSEG == 1 && EPI == EPI_AGG), "per-edge dropout: fp32 states, source rows, aggregate write-out");
 
     extern __shared__ unsigned char smem_raw[];
     // 1024-byte aligned ring; the pad is added as an OFFSET so that the pointers keep the shared address space (an integer
@@ -382,14 +389,19 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
     uint64_t *bars = reinterpret_cast<uint64_t *>(tail + META_RING * sizeof(Meta) + SCHED_RING * sizeof(Sched));
     uint64_t *x_full = bars, *x_empty = bars + NUM_SLOTS, *sched_full = bars + 2 * NUM_SLOTS, *sched_empty = sched_full + SCHED_RING;
     uint64_t *acc_full = sched_empty + SCHED_RING, *acc_empty = acc_full + 1;
+    uint64_t *x_landed = acc_empty + 1;        // DROP: the gatherers' copies have landed, the masker may edit the slot
 
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
     const int lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
         // x_full: per gather thread one asynchronous arrival when its copies have landed (cp.async.mbarrier.arrive.noinc) and one
         // ordinary arrival that publishes the step's column metadata
-        for (int s = 0; s < NUM_SLOTS; ++s) { mbar_init(&x_full[s], 2 * GATHER_THREADS); mbar_init(&x_empty[s], 8); }
-        for (int r = 0; r < SCHED_RING; ++r) { mbar_init(&sched_full[r], 1); mbar_init(&sched_empty[r], SCHED_READER_WARPS); }
+        // DROP: the asynchronous arrivals go to x_landed instead, and the masker's one arrival completes x_full
+        for (int s = 0; s < NUM_SLOTS; ++s) { mbar_init(&x_full[s], DROP ? GATHER_THREADS + 1 : 2 * GATHER_THREADS); mbar_init(&x_empty[s], 8); }
+        if constexpr (DROP) {
+            for (int s = 0; s < NUM_SLOTS; ++s) mbar_init(&x_landed[s], GATHER_THREADS);
+        }
+        for (int r = 0; r < SCHED_RING; ++r) { mbar_init(&sched_full[r], 1); mbar_init(&sched_empty[r], SCHED_READER_WARPS + (DROP ? 1 : 0)); }
         mbar_init(acc_full, 8);                // the consumer warps, after staging a sub-group
         mbar_init(acc_empty, 4);               // the reducer warps, after their column walk has read it
         for (int r = 0; r < TRACE_ROLES; ++r) trace_n[r] = 0;
@@ -598,7 +610,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
             while (more) {
                 const uint32_t slot = c_issue % NUM_SLOTS;
                 issue_next();
-                asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(&x_full[slot])) : "memory");
+                asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(DROP ? &x_landed[slot] : &x_full[slot])) : "memory");
                 trace_mark(p, 4, c_done);
                 mbar_arrive(&x_full[slot]);            // release: this thread's metadata stores of the step
                 ++c_done;
@@ -606,6 +618,67 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fused_aggregate_kernel(const _
                 more = has_nxt;
             }
             cp_async_wait<0>();
+        } else if constexpr (DROP) {
+            if (warp == MASK_WARP) {
+                // ============================================ MASKER ============================================
+                // Walks the steps in the same order as the gatherers.  For each, it loads the sub-group's keep bits (K / 32 words per
+                // edge, row j of drop_bits = sorted edge j) one step ahead, waits until the slot's rows have landed, clears the hi and
+                // lo' halves of every dropped feature, and completes x_full.  Lane l takes word l % KW of rows l / KW + RPP i.  The
+                // consumers' fence.proxy.async after their x_full wait orders these generic-proxy stores before their MMAs; the
+                // masker fences as well before it arrives, the writer-side order the PTX memory model documents.
+                constexpr int KW = K / 32, RPP = 32 / KW, PASSES = NMAX / RPP;
+                const int mw = lane % KW, mr = lane / KW;
+                StepGen<NSEG> gen{sched, sched_full, sched_empty, T, NMAX, lane};
+                uint32_t bits_nxt[PASSES];
+                auto fetch_bits = [&](const Step &st) {
+#pragma unroll
+                    for (int i = 0; i < PASSES; ++i) {
+                        const int r = mr + RPP * i;
+                        bits_nxt[i] = r < st.n ? __ldg(p.drop_bits + (size_t)(st.e + r) * KW + mw) : 0xFFFFFFFFu;
+                    }
+                };
+                Step st;
+                int ev;
+                do { ev = gen.next(st); } while (ev == 1);
+                if (ev == 0) fetch_bits(st);
+                for (uint32_t xs = 0; ev == 0; ++xs) {
+                    uint32_t bits[PASSES];
+#pragma unroll
+                    for (int i = 0; i < PASSES; ++i) bits[i] = bits_nxt[i];
+                    const uint32_t slot = xs % NUM_SLOTS;
+                    mbar_wait(&x_landed[slot], (xs / NUM_SLOTS) & 1);
+                    const uint32_t sbase = smem_u32(ring + slot * SLOT_BYTES);
+#pragma unroll
+                    for (int i = 0; i < PASSES; ++i) {
+                        if (bits[i] == 0xFFFFFFFFu) continue;          // every feature kept (or a row >= n)
+                        const int r = mr + RPP * i;
+#pragma unroll
+                        for (int c = 0; c < 4; ++c) {                   // 8-feature chunks k = 32 mw + 8 c ..
+                            const uint32_t m8 = (bits[i] >> (8 * c)) & 0xFFu;
+                            if (m8 == 0xFFu) continue;
+                            const int k = 32 * mw + 8 * c;
+                            uint32_t keep[4];
+#pragma unroll
+                            for (int h = 0; h < 4; ++h) keep[h] = ((m8 >> (2 * h)) & 1u ? 0x0000FFFFu : 0u) | ((m8 >> (2 * h + 1)) & 1u ? 0xFFFF0000u : 0u);
+                            const uint32_t off = sbase + (uint32_t)((k >> 6) * TILE_BYTES) + tc::sw128(r, k & 63);
+#pragma unroll
+                            for (int part = 0; part < 2; ++part) {       // hi, then lo'
+                                const uint32_t a = off + part * KCH * TILE_BYTES;
+                                uint4 v;
+                                asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a));
+                                asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(v.x & keep[0]), "r"(v.y & keep[1]),
+                                             "r"(v.z & keep[2]), "r"(v.w & keep[3]) : "memory");
+                            }
+                        }
+                    }
+                    tc::fence_proxy_async_smem();
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&x_full[slot]);
+                    // the next step's look-up may wait for a scheduler entry: only after this step's arrival (see the gatherers)
+                    do { ev = gen.next(st); } while (ev == 1);
+                    if (ev == 0) fetch_bits(st);
+                }
+            }
         }
     } else {
         // ============================================ CONSUMERS ============================================
@@ -762,7 +835,7 @@ struct WeightSrc {
 // out[(((t * nseg + seg) * npart + part) * (K / 8) + c4) * 128 + d] = 8 elements k = seg K + 8 c4 .. + 7 of row d
 template <int NPROD>
 __global__ void __launch_bounds__(256) pack_weights_kernel(const __grid_constant__ WeightSrc src, int num_types, int K, int nseg,
-                                                           RowMap rows, uint4 *__restrict__ out, int32_t *__restrict__ status) {
+                                                           RowMap rows, uint4 *__restrict__ out, int32_t *__restrict__ status, float scale) {
     constexpr int NPART = NPROD == 3 ? 2 : 1;
     const int per_mat = nseg * (K / 8) * 128;             // (seg, c4, d) triples per type
     const long long total = (long long)num_types * per_mat;
@@ -781,7 +854,7 @@ __global__ void __launch_bounds__(256) pack_weights_kernel(const __grid_constant
         const float *row = src.w[t] + (size_t)srow * (nseg * K) + seg * K + c4 * 8;
         float x[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) x[j] = row[j];
+        for (int j = 0; j < 8; ++j) x[j] = row[j] * scale;
         const size_t base = ((size_t)(t * nseg + seg) * NPART) * (K / 8) * 128;
         if (NPROD == 3) {       // scalar conversions: split_f16x8 takes 3 more registers here
             __half hi[8], lo[8];
@@ -832,12 +905,12 @@ int recommended_block_targets(int64_t num_nodes, int max_block_targets) {
 }
 
 int pack_weights(int nprod, int num_types, int K, int use_target, const float *const *weights, void *packed, int32_t *status,
-                 cudaStream_t st, RowMap rows) {
+                 cudaStream_t st, RowMap rows, float scale) {
     WeightSrc src{};
     for (int t = 0; t < num_types; ++t) src.w[t] = weights[t];
     const int nseg = use_target ? 2 : 1;
     return launch(PTGNN_KERNEL_PACK, st, nprod == 3 ? pack_weights_kernel<3> : pack_weights_kernel<1>, 132, 256, 0, src, num_types, K, nseg, rows,
-                  static_cast<uint4 *>(packed), status);
+                  static_cast<uint4 *>(packed), status, scale);
 }
 
 int pack_states(const float *h, int64_t rows, int K, void *packed, int32_t *status, cudaStream_t st) {
@@ -847,20 +920,20 @@ int pack_states(const float *h, int64_t rows, int K, void *packed, int32_t *stat
     return launch(PTGNN_KERNEL_PACK, st, pack_states_kernel, grid, 256, 0, h, (long long)rows, K, static_cast<uint4 *>(packed), status);
 }
 
-template <int NPROD, int K, int NSEG, int RED, int EPI = EPI_AGG>
+template <int NPROD, int K, int NSEG, int RED, int EPI = EPI_AGG, bool DROP = false>
 static int launch_one(const Params &p, cudaStream_t st) {
     const int sms = sm_count();
     const int grid = p.num_blocks < sms ? p.num_blocks : sms;
-    return launch(PTGNN_KERNEL_MESSAGE, st, fused_aggregate_kernel<NPROD, K, NSEG, RED, EPI>, grid, NUM_THREADS,
+    return launch(PTGNN_KERNEL_MESSAGE, st, fused_aggregate_kernel<NPROD, K, NSEG, RED, EPI, DROP>, grid, NUM_THREADS,
                   Geom<NPROD, K>::smem_bytes(p.B), p);
 }
-template <int NPROD, int K, int NSEG, int EPI = EPI_AGG>
+template <int NPROD, int K, int NSEG, int EPI = EPI_AGG, bool DROP = false>
 static int launch_red(const Params &p, cudaStream_t st) {
     switch (p.reduce) {
-        case PTGNN_REDUCE_SUM: return launch_one<NPROD, K, NSEG, PTGNN_REDUCE_SUM, EPI>(p, st);
-        case PTGNN_REDUCE_MEAN: return launch_one<NPROD, K, NSEG, PTGNN_REDUCE_MEAN, EPI>(p, st);
-        case PTGNN_REDUCE_MAX: return launch_one<NPROD, K, NSEG, PTGNN_REDUCE_MAX, EPI>(p, st);
-        default: return launch_one<NPROD, K, NSEG, PTGNN_REDUCE_MIN, EPI>(p, st);
+        case PTGNN_REDUCE_SUM: return launch_one<NPROD, K, NSEG, PTGNN_REDUCE_SUM, EPI, DROP>(p, st);
+        case PTGNN_REDUCE_MEAN: return launch_one<NPROD, K, NSEG, PTGNN_REDUCE_MEAN, EPI, DROP>(p, st);
+        case PTGNN_REDUCE_MAX: return launch_one<NPROD, K, NSEG, PTGNN_REDUCE_MAX, EPI, DROP>(p, st);
+        default: return launch_one<NPROD, K, NSEG, PTGNN_REDUCE_MIN, EPI, DROP>(p, st);
     }
 }
 template <int NPROD, int K>
@@ -906,6 +979,11 @@ int aggregate(const AggregateArgs &a, cudaStream_t st) {
                             e.col0 + kD / e.bases <= e.out_stride && e.coef_stride % 4 == 0,
                         "fused aggregate: bad EGC write-out (bases %d, dh %d, col0 %d, stride %d)", e.bases, e.dh, e.col0, e.out_stride);
         p.egc = e;
+    }
+    if (a.drop_bits != nullptr) {
+        PTGNN_CHECK_ARG(a.nprod == 3 && !a.use_target && !egc, "fused aggregate: per-edge dropout takes fp32 states, source rows only");
+        p.drop_bits = a.drop_bits;
+        return a.K == 64 ? launch_red<3, 64, 1, EPI_AGG, true>(p, st) : launch_red<3, 128, 1, EPI_AGG, true>(p, st);
     }
 #ifdef PTGNN_FUSED_QUICK   // compile-time experiments (ptxas -v / SASS of the benchmarked instances only); never defined in the build
     return a.nprod == 3 ? launch_one<3, 128, 1, PTGNN_REDUCE_SUM>(p, st) : launch_one<1, 128, 1, PTGNN_REDUCE_SUM>(p, st);

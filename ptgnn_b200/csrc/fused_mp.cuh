@@ -31,6 +31,7 @@
 //   them into the feature-major tile acc_s; they never touch agg_s |
 //   8-9 ROW GATHERERS (16-byte cp.async into a 2- or 3-slot ring, SWIZZLE_128B K-major; Geom in fused_mp.cu) |
 //   10 SCHEDULER (block -> group offsets table ring) |
+//   11 MASKER (per-edge dropout instances only): clears the dropped features of each landed slot before the consumers read it |
 //   12-15 REDUCER: owns agg_s; thread d walks feature d of every staged sub-group, then writes out and resets every finished
 //   block (mean / activation / LayerNorm epilogue).  Consumers and reducer hand acc_s over with two mbarriers (acc_full,
 //   acc_empty), so the walk and the write-out run while the consumers already multiply the next sub-group.
@@ -71,9 +72,10 @@ struct RowMap {
     int bases, dh, col0;
 };
 
-// weights[t]: fp32 [128, nseg*K] row-major (nn.Linear.weight; with a row map: the rows it selects) -> packed
+// weights[t]: fp32 [128, nseg*K] row-major (nn.Linear.weight; with a row map: the rows it selects), times `scale` (the per-edge
+// dropout's 1 / (1 - p)) -> packed
 int pack_weights(int nprod, int num_types, int K, int use_target, const float *const *weights, void *packed, int32_t *status,
-                 cudaStream_t st, RowMap rows = RowMap{0, 0, 0});
+                 cudaStream_t st, RowMap rows = RowMap{0, 0, 0}, float scale = 1.0f);
 // fp32 states [rows, K] -> fp16 (hi | lo') rows of 4K bytes   (NPROD = 3 only; bf16 states are gathered as they are)
 int pack_states(const float *h, int64_t rows, int K, void *packed, int32_t *status, cudaStream_t st);
 
@@ -92,6 +94,8 @@ struct AggregateArgs {
     int out_mode;                   //   (2 = what the weights-stationary GRU kernel takes as its A operand)
     int32_t *status;                // optional: status[0] = 1 if an aggregate is outside the fp16 range (out_mode 2)
     const EgcEpilogue *egc;         // non-null: the EGC write-out (out_mode 0 or 1, one segment) instead of `epi`
+    const uint32_t *drop_bits;      // non-null: per-edge dropout (fp32 states, one segment, no EGC): [E, K / 32] keep bits in block-plan
+                                    //   order (edge_dropout.cuh); the weights must have been packed with the scale 1 / (1 - p)
 };
 int aggregate(const AggregateArgs &a, cudaStream_t st);
 

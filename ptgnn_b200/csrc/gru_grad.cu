@@ -67,8 +67,11 @@ extern "C" int ptgnn_b200_gru_gate_grads_f32(const float *gi, const float *gh, c
 // mul -- this was a quarter of a training step).
 namespace ptgnn {
 
+// MASK: elements whose bit in `bits` ([rows, cols / 32] words, edge_dropout.cuh) is clear are split as 0.
+template <bool MASK>
 __global__ void __launch_bounds__(256) gather_split_kernel(const float *__restrict__ x, const int32_t *__restrict__ index, long long rows, int cols,
-                                                           const float *__restrict__ scale, uint4 *__restrict__ hi, uint4 *__restrict__ lo) {
+                                                           const float *__restrict__ scale, uint4 *__restrict__ hi, uint4 *__restrict__ lo,
+                                                           const uint32_t *__restrict__ bits) {
     const float s = scale != nullptr ? *scale : 1.0f;
     const int c8n = cols / 8;
     const long long total = rows * c8n;
@@ -78,7 +81,12 @@ __global__ void __launch_bounds__(256) gather_split_kernel(const float *__restri
         const long long src_row = index != nullptr ? (long long)index[r] : r;
         const float4 a = *reinterpret_cast<const float4 *>(x + src_row * cols + c8 * 8);
         const float4 b = *reinterpret_cast<const float4 *>(x + src_row * cols + c8 * 8 + 4);
-        const float v[8] = {a.x * s, a.y * s, a.z * s, a.w * s, b.x * s, b.y * s, b.z * s, b.w * s};
+        float v[8] = {a.x * s, a.y * s, a.z * s, a.w * s, b.x * s, b.y * s, b.z * s, b.w * s};
+        if (MASK) {
+            const uint32_t m = bits[r * (cols / 32) + (c8 >> 2)] >> (8 * (c8 & 3));
+#pragma unroll
+            for (int j = 0; j < 8; ++j) v[j] = (m >> j) & 1u ? v[j] : 0.0f;
+        }
         tc::split_f16x8(v, hi[r * c8n + c8], lo[r * c8n + c8]);
     }
 }
@@ -94,6 +102,19 @@ extern "C" int ptgnn_b200_gather_split_f16(const float *x, const int32_t *index,
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const long long total = (long long)rows_out * (cols / 8);
     const long long blocks = (total + 255) / 256;
-    return launch(PTGNN_KERNEL_PACK, st, gather_split_kernel, (unsigned)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, x, index, rows_out, cols,
-                  scale, static_cast<uint4 *>(hi), static_cast<uint4 *>(lo));
+    return launch(PTGNN_KERNEL_PACK, st, gather_split_kernel<false>, (unsigned)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, x, index, rows_out,
+                  cols, scale, static_cast<uint4 *>(hi), static_cast<uint4 *>(lo), nullptr);
+}
+
+extern "C" int ptgnn_b200_gather_split_f16_masked(const float *x, const int32_t *index, int64_t rows_out, int32_t cols, const float *scale,
+                                                  const uint32_t *bits, void *hi, void *lo, void *stream) {
+    using namespace ptgnn;
+    PTGNN_CHECK_ARG(rows_out >= 0 && cols > 0 && cols % 32 == 0, "gather_split_masked: cols=%d must be a positive multiple of 32", cols);
+    if (rows_out == 0) return PTGNN_OK;
+    PTGNN_CHECK_ARG(x && hi && lo && bits, "gather_split_masked: null pointer");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const long long total = (long long)rows_out * (cols / 8);
+    const long long blocks = (total + 255) / 256;
+    return launch(PTGNN_KERNEL_PACK, st, gather_split_kernel<true>, (unsigned)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, x, index, rows_out,
+                  cols, scale, static_cast<uint4 *>(hi), static_cast<uint4 *>(lo), bits);
 }

@@ -7,6 +7,7 @@
 //
 // * skipped when the caller's weight cache is valid.  The packing pass of the states is skipped when the caller hands in their
 // packed form (a stack of gated layers: the previous layer's GRU wrote it).
+#include "edge_dropout.cuh"
 #include "fused_mp.cuh"
 #include "gru_ws.cuh"
 #include "layers.cuh"
@@ -30,18 +31,28 @@ size_t mlp_weight_bytes(int nprod, int T, int H, int D, int Hout, int ut) {
     return fused::packed_weight_bytes(nprod, T, H, ut) + tc::dense_weight_bytes(nprod == 1, Hout, D) + 256;
 }
 
-// workspace: agg | packed states (gathered rows) | packed own rows (sharded run: the GRU's h) | derived weights (no cache)
-struct GatedWs { size_t agg, xpack, xpack_own, weights, total; };
-GatedWs gated_layout(int nprod, int64_t N, int64_t Ns, int T, int H, int D) {
+// workspace: agg | packed states (gathered rows) | packed own rows (sharded run: the GRU's h) | derived weights (no cache) |
+// per-edge dropout keep bits (E_drop edges; 0 without dropout)
+struct GatedWs { size_t agg, xpack, xpack_own, weights, bits, total; };
+GatedWs gated_layout(int nprod, int64_t N, int64_t Ns, int T, int H, int D, int64_t E_drop = 0) {
     Layout l;
     GatedWs w;
     w.agg = l.add_bytes(agg_bytes(nprod, N, D));
     w.xpack = l.add_bytes(fused::packed_state_bytes(nprod, Ns, H));
     w.xpack_own = l.add_bytes(fused::packed_state_bytes(nprod, N, H));
     w.weights = l.add_bytes(gated_weight_bytes(nprod, T, H, D));
+    w.bits = l.add((size_t)E_drop * (H / 32), 4);
     w.total = l.total;
     return w;
 }
+
+// per-edge dropout of the gathered rows: the keep bits in block-plan order, and the scale folded into the packed edge weights
+struct Drop {
+    const int32_t *eid_f;
+    const uint32_t *key;
+    float p;
+    int64_t num_edges;
+};
 
 // workspace: y (pre-dense aggregate) | packed states (gathered rows) | packed target rows (sharded run) | derived weights
 struct MlpWs { size_t y, xpack, xpack_tgt, weights, total; };
@@ -70,7 +81,7 @@ int gated_fused(int nprod, const void *node_states, const void *gather_states, c
                 int D, int T, const ptgnn_b200_block_plan *bp, const int32_t *row_ptr, const float *const *edge_weights,
                 const float *w_ih, const float *w_hh, const float *b_ih, const float *b_hh, int reduce, void *out_states,
                 void *packed_out, void *workspace, size_t workspace_bytes, void *weight_cache, size_t weight_cache_bytes,
-                int cache_valid, cudaStream_t st) {
+                int cache_valid, cudaStream_t st, const Drop *drop = nullptr) {
     PTGNN_CHECK_ARG(bp != nullptr, "gated_forward_fused: null block plan");
     PTGNN_CHECK_ARG(T >= 0 && T <= PTGNN_MAX_EDGE_TYPES, "gated_forward_fused: bad num_types=%d", T);
     if (!gated_ok(nprod, H, D)) {
@@ -84,7 +95,7 @@ int gated_fused(int nprod, const void *node_states, const void *gather_states, c
     PTGNN_CHECK_ARG(node_states && out_states && row_ptr && w_ih && w_hh && b_ih && b_hh, "gated_forward_fused: null pointer");
     PTGNN_CHECK_ARG(bp->group_off && edge_weights && T > 0, "gated_forward_fused: null block plan arrays");
     if (Ns <= 0) Ns = N;
-    const GatedWs L = gated_layout(nprod, N, Ns, T, H, D);
+    const GatedWs L = gated_layout(nprod, N, Ns, T, H, D, drop ? drop->num_edges : 0);
     PTGNN_CHECK_WORKSPACE("gated_forward_fused", workspace, workspace_bytes, L.total);
     char *ws = static_cast<char *>(workspace);
     char *wpack;
@@ -94,7 +105,14 @@ int gated_fused(int nprod, const void *node_states, const void *gather_states, c
     if (rc) return rc;
     char *grupack = wpack + fused::packed_weight_bytes(nprod, T, H, 0);
     if (pack) {
-        rc = fused::pack_weights(nprod, T, H, 0, edge_weights, wpack, bp->status, st);
+        rc = fused::pack_weights(nprod, T, H, 0, edge_weights, wpack, bp->status, st, fused::RowMap{0, 0, 0},
+                                 drop ? edge_dropout_scale(drop->p) : 1.0f);
+        if (rc) return rc;
+    }
+    uint32_t *bits = nullptr;
+    if (drop != nullptr) {
+        bits = reinterpret_cast<uint32_t *>(ws + L.bits);
+        rc = edge_dropout_bits(drop->key, drop->num_edges, H, drop->p, drop->eid_f, bits, st);
         if (rc) return rc;
     }
 
@@ -123,6 +141,7 @@ int gated_fused(int nprod, const void *node_states, const void *gather_states, c
     fused::AggregateArgs a = aggregate_args(nprod, bp, row_ptr, N, H, T, reduce, wpack);
     a.src_rows = src_rows; a.use_target = 0; a.tgt_rows = nullptr;
     a.out = ws + L.agg; a.out_mode = nprod == 3 ? 2 : 1;
+    a.drop_bits = bits;
     rc = fused::aggregate(a, st);
     if (rc) return rc;
     // 3. GRUCell, weights-stationary (the gate weights stay in shared memory, only node rows stream)
@@ -392,6 +411,84 @@ extern "C" int ptgnn_b200_gated_forward_fused(int32_t bf16_states, const void *n
                        message_dim, num_types, block_plan, row_ptr, edge_weights, gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, reduce,
                        out_states, packed_states_out, workspace, workspace_bytes, weight_cache, weight_cache_bytes, cache_valid,
                        static_cast<cudaStream_t>(stream));
+}
+
+// ---- per-edge dropout (GatedMessagePassingLayer in training mode, fp32 states, unsharded) ----------------------------------------
+static int drop_args(const Drop &d, int64_t N, const int32_t *row_ptr) {
+    PTGNN_CHECK_ARG(d.num_edges >= 0 && d.num_edges < INT32_MAX, "per-edge dropout: num_edges out of range");
+    PTGNN_CHECK_ARG(d.p >= 0.0f && d.p <= 1.0f, "per-edge dropout: p=%g outside [0, 1]", (double)d.p);
+    PTGNN_CHECK_ARG(N == 0 || d.num_edges == 0 || (d.eid_f && d.key && row_ptr), "per-edge dropout: null eid_f / key / row_ptr");
+    return PTGNN_OK;
+}
+
+extern "C" size_t ptgnn_b200_gated_fused_dropout_workspace_bytes(int64_t num_nodes, int64_t num_edges, int32_t num_types, int32_t state_dim,
+                                                                 int32_t message_dim) {
+    if (num_nodes < 0 || num_edges < 0 || num_types < 0 || state_dim <= 0 || state_dim % 32 != 0 || message_dim <= 0) return 0;
+    return gated_layout(3, num_nodes, num_nodes, num_types, state_dim, message_dim, num_edges).total;
+}
+extern "C" int ptgnn_b200_gated_forward_fused_dropout(const float *node_states, const void *packed_states_in, int64_t num_nodes,
+                                                      int64_t num_edges, int32_t state_dim, int32_t message_dim, int32_t num_types,
+                                                      const ptgnn_b200_block_plan *block_plan, const int32_t *eid_f, const int32_t *row_ptr,
+                                                      const float *const *edge_weights, const float *gru_w_ih, const float *gru_w_hh,
+                                                      const float *gru_b_ih, const float *gru_b_hh, int32_t reduce, const uint32_t *key, float p,
+                                                      void *out_states, void *packed_states_out, void *workspace, size_t workspace_bytes,
+                                                      void *weight_cache, size_t weight_cache_bytes, int32_t cache_valid, void *stream) {
+    const Drop d{eid_f, key, p, num_edges};
+    const int rc = drop_args(d, num_nodes, row_ptr);
+    if (rc) return rc;
+    return gated_fused(3, node_states, nullptr, packed_states_in, num_nodes, num_nodes, state_dim, message_dim, num_types, block_plan, row_ptr,
+                       edge_weights, gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, reduce, out_states, packed_states_out, workspace, workspace_bytes,
+                       weight_cache, weight_cache_bytes, cache_valid, static_cast<cudaStream_t>(stream), &d);
+}
+
+// workspace: packed states | packed, scaled edge weights | keep bits
+struct AggDropWs { size_t xpack, weights, bits, total; };
+static AggDropWs agg_drop_layout(int64_t N, int64_t E, int T, int H) {
+    Layout l;
+    AggDropWs w;
+    w.xpack = l.add_bytes(fused::packed_state_bytes(3, N, H));
+    w.weights = l.add_bytes(fused::packed_weight_bytes(3, T, H, 0));
+    w.bits = l.add((size_t)E * (H / 32), 4);
+    w.total = l.total;
+    return w;
+}
+extern "C" size_t ptgnn_b200_fused_aggregate_dropout_workspace_bytes(int64_t num_nodes, int64_t num_edges, int32_t num_types, int32_t state_dim) {
+    if (num_nodes < 0 || num_edges < 0 || num_types < 0 || state_dim <= 0 || state_dim % 32 != 0) return 0;
+    return agg_drop_layout(num_nodes, num_edges, num_types, state_dim).total;
+}
+extern "C" int ptgnn_b200_fused_aggregate_dropout(const float *node_states, int64_t num_nodes, int64_t num_edges, int32_t state_dim, int32_t num_types,
+                                                  const ptgnn_b200_block_plan *block_plan, const int32_t *eid_f, const int32_t *row_ptr,
+                                                  const float *const *edge_weights, int32_t reduce, const uint32_t *key, float p, float *out,
+                                                  void *workspace, size_t workspace_bytes, void *stream) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const ptgnn_b200_block_plan *bp = block_plan;
+    const int H = state_dim, T = num_types;
+    PTGNN_CHECK_ARG(bp != nullptr, "fused_aggregate_dropout: null block plan");
+    PTGNN_CHECK_ARG(T > 0 && T <= PTGNN_MAX_EDGE_TYPES, "fused_aggregate_dropout: bad num_types=%d", T);
+    if (!fused::supported(3, H, fused::kD, 0)) {
+        set_error("fused_aggregate_dropout: state_dim=%d is not supported by the fused kernel", H);
+        return PTGNN_E_UNSUPPORTED;
+    }
+    PTGNN_CHECK_ARG(num_nodes >= 0 && num_nodes < INT32_MAX, "fused_aggregate_dropout: sizes out of range");
+    PTGNN_CHECK_ARG(reduce >= PTGNN_REDUCE_SUM && reduce <= PTGNN_REDUCE_MIN, "fused_aggregate_dropout: bad reduce %d", reduce);
+    const Drop d{eid_f, key, p, num_edges};
+    int rc = drop_args(d, num_nodes, row_ptr);
+    if (rc) return rc;
+    if (num_nodes == 0) return PTGNN_OK;
+    PTGNN_CHECK_ARG(node_states && out && edge_weights && bp->group_off, "fused_aggregate_dropout: null pointer");
+    const AggDropWs L = agg_drop_layout(num_nodes, num_edges, T, H);
+    PTGNN_CHECK_WORKSPACE("fused_aggregate_dropout", workspace, workspace_bytes, L.total);
+    char *ws = static_cast<char *>(workspace);
+    if ((rc = fused::pack_weights(3, T, H, 0, edge_weights, ws + L.weights, bp->status, st, fused::RowMap{0, 0, 0}, edge_dropout_scale(p))))
+        return rc;
+    if ((rc = fused::pack_states(node_states, num_nodes, H, ws + L.xpack, bp->status, st))) return rc;
+    uint32_t *bits = reinterpret_cast<uint32_t *>(ws + L.bits);
+    if ((rc = edge_dropout_bits(key, num_edges, H, p, eid_f, bits, st))) return rc;
+    fused::AggregateArgs a = aggregate_args(3, bp, row_ptr, num_nodes, H, T, reduce, ws + L.weights);
+    a.src_rows = ws + L.xpack; a.use_target = 0; a.tgt_rows = nullptr;
+    a.out = out; a.out_mode = 0;
+    a.drop_bits = bits;
+    return fused::aggregate(a, st);
 }
 
 extern "C" size_t ptgnn_b200_mlp_fused_workspace_bytes(int32_t bf16_states, int64_t num_nodes, int64_t num_source_nodes,

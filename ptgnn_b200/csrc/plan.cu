@@ -421,16 +421,19 @@ union OrderSmem {
 };
 
 __device__ __forceinline__ int word_digit(uint64_t w, int d) { return (int)(w >> (d < 4 ? 8 * d : 32)) & (RADIX - 1); }
-__device__ __forceinline__ void write_edge(uint64_t w, int64_t j, const int32_t *src32, int32_t *src_f, uint8_t *tl_f) {
+// EID: also eid_f[j] = the edge's cat(types) position (the word's low half), for the per-edge dropout mask (edge_dropout.cuh)
+template <bool EID>
+__device__ __forceinline__ void write_edge(uint64_t w, int64_t j, const int32_t *src32, int32_t *src_f, uint8_t *tl_f, int32_t *eid_f) {
     src_f[j] = src32[(uint32_t)w];
     tl_f[j] = (uint8_t)(w >> 32);
+    if (EID) eid_f[j] = (int32_t)(uint32_t)w;
 }
 
 // One group of n <= 32 * R words in shared memory, sorted by one warp: the rank of a word is how many words of the group are
 // smaller.  Lane l holds words l, l + 32, ...; each shared word is read once (a broadcast) and compared with all of them.
-template <int R>
+template <int R, bool EID>
 __device__ __forceinline__ void order_small_group(const uint64_t *s, int n, int64_t j0, const int32_t *src32, int32_t *src_f,
-                                                  uint8_t *tl_f) {
+                                                  uint8_t *tl_f, int32_t *eid_f) {
     const int lane = threadIdx.x & 31;
     uint64_t w[R];
     int rank[R];
@@ -447,15 +450,16 @@ __device__ __forceinline__ void order_small_group(const uint64_t *s, int n, int6
     }
 #pragma unroll
     for (int r = 0; r < R; ++r)
-        if (r * 32 + lane < n) write_edge(w[r], j0 + rank[r], src32, src_f, tl_f);
+        if (r * 32 + lane < n) write_edge<EID>(w[r], j0 + rank[r], src32, src_f, tl_f, eid_f);
 }
 
 // One group of n > kWarpGroup words at a[0..n), sorted by the whole CTA: the digit histograms come from one read (they do not
 // depend on the order), digits every word shares are skipped, and each remaining digit is one stable pass, chunk by chunk
 // in input order (within a chunk ranks go by (warp, round, lane), i.e. input position).  Passes alternate between a and b;
 // the last one writes src_f / tl_f at j0 + rank.
+template <bool EID>
 __device__ void order_large_group(uint64_t *a, uint64_t *b, int n, int64_t j0, const int32_t *src32, int32_t *src_f, uint8_t *tl_f,
-                                  OrderSmem &sm) {
+                                  int32_t *eid_f, OrderSmem &sm) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (int i = threadIdx.x; i < ORDER_DIGITS * RADIX; i += ORDER_THREADS) (&sm.cta.hist[0][0])[i] = 0;
     if (threadIdx.x == 0) sm.cta.uniform = 0;
@@ -529,7 +533,7 @@ __device__ void order_large_group(uint64_t *a, uint64_t *b, int n, int64_t j0, c
                 if (valid && lane == __ffs(peers) - 1) sm.cta.warp_hist[warp][digit[r]] += __popc(peers);
                 __syncwarp();
                 if (valid) {
-                    if (d == last) write_edge(w[r], j0 + dst, src32, src_f, tl_f);
+                    if (d == last) write_edge<EID>(w[r], j0 + dst, src32, src_f, tl_f, eid_f);
                     else out[dst] = w[r];
                 }
             }
@@ -539,10 +543,11 @@ __device__ void order_large_group(uint64_t *a, uint64_t *b, int n, int64_t j0, c
     }
 }
 
+template <bool EID>
 __global__ void __launch_bounds__(ORDER_THREADS, 2) block_order_kernel(int64_t num_groups, const int32_t *__restrict__ group_off,
                                                                     uint64_t *__restrict__ words, uint64_t *__restrict__ tmp,
                                                                     const int32_t *__restrict__ src32, int32_t *__restrict__ src_f,
-                                                                    uint8_t *__restrict__ tl_f) {
+                                                                    uint8_t *__restrict__ tl_f, int32_t *__restrict__ eid_f) {
     __shared__ OrderSmem sm;
     __shared__ int off[ORDER_WARPS + 1];
     const int64_t g0 = (int64_t)blockIdx.x * ORDER_WARPS;
@@ -557,14 +562,14 @@ __global__ void __launch_bounds__(ORDER_THREADS, 2) block_order_kernel(int64_t n
             for (int i = lane; i < n; i += 32) s[i] = words[j0 + i];
             __syncwarp();
             switch ((n + 31) / 32) {
-                case 1: order_small_group<1>(s, n, j0, src32, src_f, tl_f); break;
-                case 2: order_small_group<2>(s, n, j0, src32, src_f, tl_f); break;
-                case 3: order_small_group<3>(s, n, j0, src32, src_f, tl_f); break;
-                case 4: order_small_group<4>(s, n, j0, src32, src_f, tl_f); break;
-                case 5: order_small_group<5>(s, n, j0, src32, src_f, tl_f); break;
-                case 6: order_small_group<6>(s, n, j0, src32, src_f, tl_f); break;
-                case 7: order_small_group<7>(s, n, j0, src32, src_f, tl_f); break;
-                case 8: order_small_group<8>(s, n, j0, src32, src_f, tl_f); break;
+                case 1: order_small_group<1, EID>(s, n, j0, src32, src_f, tl_f, eid_f); break;
+                case 2: order_small_group<2, EID>(s, n, j0, src32, src_f, tl_f, eid_f); break;
+                case 3: order_small_group<3, EID>(s, n, j0, src32, src_f, tl_f, eid_f); break;
+                case 4: order_small_group<4, EID>(s, n, j0, src32, src_f, tl_f, eid_f); break;
+                case 5: order_small_group<5, EID>(s, n, j0, src32, src_f, tl_f, eid_f); break;
+                case 6: order_small_group<6, EID>(s, n, j0, src32, src_f, tl_f, eid_f); break;
+                case 7: order_small_group<7, EID>(s, n, j0, src32, src_f, tl_f, eid_f); break;
+                case 8: order_small_group<8, EID>(s, n, j0, src32, src_f, tl_f, eid_f); break;
                 default: break;   // n == 0
             }
         }
@@ -572,7 +577,7 @@ __global__ void __launch_bounds__(ORDER_THREADS, 2) block_order_kernel(int64_t n
     __syncthreads();
     for (int k = 0; k < ng; ++k) {
         const int j0 = off[k], n = off[k + 1] - j0;
-        if (n > kWarpGroup) order_large_group(words + j0, tmp + j0, n, j0, src32, src_f, tl_f, sm);
+        if (n > kWarpGroup) order_large_group<EID>(words + j0, tmp + j0, n, j0, src32, src_f, tl_f, eid_f, sm);
     }
 }
 
@@ -686,10 +691,9 @@ extern "C" size_t ptgnn_b200_block_plan_workspace_bytes(int64_t num_nodes, int64
     return block_plan_ws_layout(num_nodes, num_edges, num_types, block_targets).total;
 }
 
-extern "C" int ptgnn_b200_block_plan_build(int64_t num_nodes, int32_t num_types, const int64_t *type_off,
-                                           const int32_t *src32, const int32_t *tgt32, int32_t block_targets,
-                                           int32_t *group_off, int32_t *src_f, uint8_t *tl_f, void *workspace,
-                                           size_t workspace_bytes, void *stream) {
+static int block_plan_build(int64_t num_nodes, int32_t num_types, const int64_t *type_off, const int32_t *src32, const int32_t *tgt32,
+                            int32_t block_targets, int32_t *group_off, int32_t *src_f, uint8_t *tl_f, int32_t *eid_f, void *workspace,
+                            size_t workspace_bytes, void *stream) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int B = block_targets, T = num_types;
     PTGNN_CHECK_ARG(num_nodes >= 0 && num_nodes < INT32_MAX, "block_plan_build: num_nodes out of range");
@@ -717,6 +721,26 @@ extern "C" int ptgnn_b200_block_plan_build(int64_t num_nodes, int32_t num_types,
                      (int64_t)scan_workspace_elems(groups + 1)));
     PTGNN_TRY(single_pass_scan_i32(group_off, group_off, groups + 1, scan_state, st));
     PTGNN_TRY(launch(PTGNN_KERNEL_PLAN, st, block_scatter_kernel, grid, 256, 0, toff, E, tgt32, B, group_off, slot, words));
-    return launch(PTGNN_KERNEL_PLAN, st, block_order_kernel, (unsigned)ceil_div(groups, ORDER_WARPS), ORDER_THREADS, 0, groups, group_off,
-                  words, tmp, src32, src_f, tl_f);
+    if (eid_f != nullptr)
+        return launch(PTGNN_KERNEL_PLAN, st, block_order_kernel<true>, (unsigned)ceil_div(groups, ORDER_WARPS), ORDER_THREADS, 0, groups,
+                      group_off, words, tmp, src32, src_f, tl_f, eid_f);
+    return launch(PTGNN_KERNEL_PLAN, st, block_order_kernel<false>, (unsigned)ceil_div(groups, ORDER_WARPS), ORDER_THREADS, 0, groups, group_off,
+                  words, tmp, src32, src_f, tl_f, nullptr);
+}
+
+extern "C" int ptgnn_b200_block_plan_build(int64_t num_nodes, int32_t num_types, const int64_t *type_off,
+                                           const int32_t *src32, const int32_t *tgt32, int32_t block_targets,
+                                           int32_t *group_off, int32_t *src_f, uint8_t *tl_f, void *workspace,
+                                           size_t workspace_bytes, void *stream) {
+    return block_plan_build(num_nodes, num_types, type_off, src32, tgt32, block_targets, group_off, src_f, tl_f, nullptr, workspace,
+                            workspace_bytes, stream);
+}
+
+extern "C" int ptgnn_b200_block_plan_build_with_edge_ids(int64_t num_nodes, int32_t num_types, const int64_t *type_off,
+                                                         const int32_t *src32, const int32_t *tgt32, int32_t block_targets,
+                                                         int32_t *group_off, int32_t *src_f, uint8_t *tl_f, int32_t *eid_f,
+                                                         void *workspace, size_t workspace_bytes, void *stream) {
+    PTGNN_CHECK_ARG(eid_f != nullptr, "block_plan_build_with_edge_ids: null eid_f");
+    return block_plan_build(num_nodes, num_types, type_off, src32, tgt32, block_targets, group_off, src_f, tl_f, eid_f, workspace,
+                            workspace_bytes, stream);
 }

@@ -23,7 +23,7 @@ class EdgePlan:
 
     __slots__ = (
         "num_nodes", "num_source_nodes", "num_edges", "num_types", "type_off", "type_off_c", "row_ptr", "src32", "tgt32", "status", "device", "_keepalive", "_validated", "_block", "_sorted", "_counts_c",
-        "_block_targets", "_large_blocks",
+        "_block_targets", "_large_blocks", "_block_eid",
     )
 
     # status words (pinned host memory the kernels write directly, so the host can poll them without synchronising):
@@ -77,6 +77,7 @@ class EdgePlan:
         self._sorted = None
         self.status = torch.zeros(self.STATUS_WORDS, dtype=torch.int32).pin_memory()
         self._block = None
+        self._block_eid = None
         self._counts_c = N.i64_array(counts)
         lib = N.lib()
         ws_bytes = lib.ptgnn_b200_plan_workspace_bytes(num_nodes, E)
@@ -135,8 +136,10 @@ class EdgePlan:
                              "outside [0, K)); the kernels skipped them, results are not valid")
 
     # ---- block plan of the fused kernel (built on first use, shared by all layers of the minibatch) ---------------------
-    def block_plan(self) -> "N.BlockPlanStruct":
-        if self._block is None:
+    def block_plan(self, edge_ids: bool = False) -> "N.BlockPlanStruct":
+        """The fused kernel's block plan.  ``edge_ids``: also build ``block_edge_ids`` (what per-edge dropout needs); a plan built
+        without them is rebuilt with them, so a container whose layers need them asks for them first."""
+        if self._block is None or (edge_ids and self._block_eid is None):
             lib = N.lib()
             B = self._block_targets
             if B is None:
@@ -149,11 +152,24 @@ class EdgePlan:
             tl_f = torch.empty(max(self.num_edges, 1), dtype=torch.uint8, device=dev)
             ws_bytes = lib.ptgnn_b200_block_plan_workspace_bytes(self.num_nodes, self.num_edges, self.num_types, B)
             ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
-            N.call("ptgnn_b200_block_plan_build", dev, self.num_nodes, self.num_types, self.type_off_c, N.ptr(self.src32), N.ptr(self.tgt32),
-                   B, N.ptr(group_off), N.ptr(src_f), N.ptr(tl_f), N.ptr(ws), ws_bytes)
+            eid_f = None
+            if edge_ids:
+                eid_f = torch.empty(max(self.num_edges, 1), dtype=torch.int32, device=dev)
+                N.call("ptgnn_b200_block_plan_build_with_edge_ids", dev, self.num_nodes, self.num_types, self.type_off_c, N.ptr(self.src32),
+                       N.ptr(self.tgt32), B, N.ptr(group_off), N.ptr(src_f), N.ptr(tl_f), N.ptr(eid_f), N.ptr(ws), ws_bytes)
+            else:
+                N.call("ptgnn_b200_block_plan_build", dev, self.num_nodes, self.num_types, self.type_off_c, N.ptr(self.src32),
+                       N.ptr(self.tgt32), B, N.ptr(group_off), N.ptr(src_f), N.ptr(tl_f), N.ptr(ws), ws_bytes)
             struct = N.BlockPlanStruct(B, N.ptr(group_off), N.ptr(src_f), N.ptr(tl_f), self.status.data_ptr() + 4)
             self._block = (struct, group_off, src_f, tl_f, B)
+            self._block_eid = eid_f
         return self._block[0]
+
+    @property
+    def block_edge_ids(self) -> torch.Tensor:
+        """[E] int32: the cat(types) position of the edge at each block-plan position (src_f[j] == src32[block_edge_ids[j]])."""
+        self.block_plan(edge_ids=True)
+        return self._block_eid
 
     @property
     def block_targets(self) -> int:

@@ -141,10 +141,12 @@ class GraphNeuralNetwork(nn.Module):
             adjacency_lists = kept_adj
             edge_feature_embeddings = kept_feats if edge_feature_embeddings is not None else None
             plan = None
+        layers = list(self.__message_passing_layers)
         if node_representations.is_cuda:
             plan = plan_for(adjacency_lists, node_representations.shape[0], plan)
+            if any(getattr(layer, "edge_dropout_active", False) for layer in layers):
+                plan.block_plan(edge_ids=True)       # one build with the ids per-edge dropout needs, not one without and one with
         all_states = [node_representations]
-        layers = list(self.__message_passing_layers)
         outer = current_state_chain()      # forward(): the node embedder may have left the packed form of node_representations there
         # per-thread hand-offs: the layers of this call (and only they) reuse the plan and the graph count, and pass their packed
         # states on

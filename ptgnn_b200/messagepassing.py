@@ -11,8 +11,9 @@ Drop-in for the classes the reference's factories construct
 Constructor signatures, properties, parameter initialisation order and (name-mangled) ``state_dict`` keys are the
 reference's, so reference checkpoints load with ``load_state_dict``.  ``forward`` never touches PyTorch arithmetic:
 it hands raw device pointers to ``libptgnn_b200.so``.  Configurations without a native kernel raise
-``NotImplementedError`` (there is no silent fallback): training-mode dropout, autograd (SURVEY.md §8 f-1), edge
-features (f-4), hidden message-MLP layers and module aggregators such as PNA (f-3).
+``NotImplementedError`` (there is no silent fallback): training-mode dropout outside the gated layer's fp32 paths, autograd
+outside the trainable layers (SURVEY.md §8 f-1), edge features (f-4), hidden message-MLP layers and module aggregators such as
+PNA (f-3).
 """
 from abc import abstractmethod
 from typing import Dict, List, Optional, Tuple, Union
@@ -240,9 +241,19 @@ class GatedMessagePassingLayer(AbstractMessagePassingLayer):
         from . import autograd as _ag
         drop_p = self.__dropout.p if self.training else 0.0
         grad = _ag.needs_grad(self, node_states)
+        if (drop_p > 0 and gather_states is None and node_states.dtype == torch.float32 and self.__edge_feature_dimension == 0
+                and _use_fused(N.lib(), False, self.__state_dimension, self.__message_dimension)):
+            # per-edge dropout (gatedmessagepassing.py:59) inside the fused aggregation: the mask is a function of a per-call key
+            _check_states(node_states, self.__state_dimension, "GatedMessagePassingLayer")
+            h = N.require_cuda(node_states, "node_states", torch.float32)
+            if grad:
+                gru = self.__state_update
+                return _ag.gated_dropout_with_grad(self, h, adjacency_lists, self.__aggregation_fn, drop_p, gru.weight_ih, gru.weight_hh,
+                                                   gru.bias_ih, gru.bias_hh, [lin.weight for lin in linears])
+            return self._forward_fused_dropout(h, adjacency_lists, _ag.draw_dropout_key(h.device), drop_p)
         if drop_p > 0 or (grad and self.__edge_feature_dimension != 0):
-            # per-edge dropout (gatedmessagepassing.py:59) / edge features under autograd: the gathered rows have to exist -- the layer
-            # as the reference writes it, Linear / scatter / GRUCell on the native kernels as differentiable operators
+            # per-edge dropout outside the fused kernel's dimensions / edge features under autograd: the gathered rows have to exist --
+            # the layer as the reference writes it, Linear / scatter / GRUCell on the native kernels as differentiable operators
             if gather_states is not None or node_states.dtype != torch.float32:
                 raise NotImplementedError("training-mode dropout / edge features with gradients: fp32 states, unsharded only")
             _check_states(node_states, self.__state_dimension, "GatedMessagePassingLayer")
@@ -313,6 +324,48 @@ class GatedMessagePassingLayer(AbstractMessagePassingLayer):
                N.ptr(plan.row_ptr), N.ptr(plan.pos), N.ptr(plan.src32), N.ptr_table(weights), N.ptr(w_ih), N.ptr(w_hh), N.ptr(b_ih),
                N.ptr(b_hh), reduce, N.ptr(out), N.ptr(ws), ws_bytes, N.ptr(cache), 0 if cache is None else cache.numel(), int(valid))
         self._weight_cache_filled(kind, h.device)
+        return out
+
+    @property
+    def edge_dropout_active(self) -> bool:
+        """Training mode with per-edge dropout: the layer's fused path then needs the plan's ``block_edge_ids``."""
+        return self.training and self.__dropout.p > 0
+
+    def _forward_fused_dropout(self, h: torch.Tensor, adjacency_lists, key: torch.Tensor, p: float) -> torch.Tensor:
+        """The fused path with per-edge dropout (fp32 states, unsharded, no edge features) for the mask of ``key`` (int32 [2], device):
+        the keep bits are generated up front, the fused kernel clears the dropped features of the gathered rows, and 1 / (1 - p) is
+        folded into the packed edge weights (a weight-cache entry of its own per p)."""
+        num_nodes, H = h.shape
+        D = self.__message_dimension
+        plan = self._plan(adjacency_lists, num_nodes)
+        gru = self.__state_update
+        weights = [N.require_cuda(lin.weight, "edge weight", torch.float32) for lin in self.__edge_message_transformation_layers]
+        w_ih, w_hh = N.require_cuda(gru.weight_ih, "weight_ih", torch.float32), N.require_cuda(gru.weight_hh, "weight_hh", torch.float32)
+        b_ih, b_hh = N.require_cuda(gru.bias_ih, "bias_ih", torch.float32), N.require_cuda(gru.bias_hh, "bias_hh", torch.float32)
+        for i, w in enumerate(weights):
+            _check_shape(w, (D, H), f"edge weight {i}")
+        _check_shape(w_ih, (3 * H, D), "GRUCell.weight_ih"); _check_shape(w_hh, (3 * H, H), "GRUCell.weight_hh")
+        _check_shape(b_ih, (3 * H,), "GRUCell.bias_ih"); _check_shape(b_hh, (3 * H,), "GRUCell.bias_hh")
+        lib = N.lib()
+        kind = ("f32_fused_dropout", float(p))
+        cache, valid = self._weight_cache(kind, lib.ptgnn_b200_gated_fused_weight_cache_bytes(0, plan.num_types, H, D),
+                                          weights + [w_ih, w_hh, b_ih, b_hh], h.device)
+        ws_bytes = lib.ptgnn_b200_gated_fused_dropout_workspace_bytes(num_nodes, plan.num_edges, plan.num_types, H, D)
+        ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=h.device)
+        out = torch.empty_like(h)
+        bp = plan.block_plan(edge_ids=True)
+        chain = current_state_chain()           # the packed states stay unmasked: the mask is applied to the gathered copies
+        packed_in = chain.lookup(h) if chain is not None else None
+        packed_out = None
+        if chain is not None and chain.want_output:
+            packed_out = torch.empty(max(lib.ptgnn_b200_packed_state_bytes(num_nodes, H), 1), dtype=torch.uint8, device=h.device)
+        N.call("ptgnn_b200_gated_forward_fused_dropout", h.device, N.ptr(h), N.ptr(packed_in), num_nodes, plan.num_edges, H, D, plan.num_types,
+               ctypes.byref(bp), N.ptr(plan.block_edge_ids), N.ptr(plan.row_ptr), N.ptr_table(weights), N.ptr(w_ih), N.ptr(w_hh), N.ptr(b_ih),
+               N.ptr(b_hh), _reduce_code(self.__aggregation_fn), N.ptr(key), float(p), N.ptr(out), N.ptr(packed_out), N.ptr(ws), ws_bytes,
+               N.ptr(cache), 0 if cache is None else cache.numel(), int(valid))
+        self._weight_cache_filled(kind, h.device)
+        if chain is not None:
+            chain.store(out, packed_out)
         return out
 
     def _forward_with_edge_features(self, node_states, adjacency_lists, edge_features, gather_states, reduce: int) -> torch.Tensor:
