@@ -286,6 +286,30 @@ int ptgnn_b200_fused_aggregate_dropout(const float *node_states, int64_t num_nod
                                        const ptgnn_b200_block_plan *block_plan, const int32_t *eid_f, const int32_t *row_ptr,
                                        const float *const *edge_weights, int32_t reduce, const uint32_t *key, float p, float *out,
                                        void *workspace, size_t workspace_bytes, void *stream);
+/* The same per-edge dropout on the three-kernel path, for the dimensions the fused kernel does not take: masked messages on the
+ * tensor-core message kernel (the dropped elements of each gathered row are cleared before the 3xTF32 products, and the products are
+ * scaled by 1 / (1 - p)), then the streaming segmented reduce and the GRUCell step of ptgnn_b200_gated_forward.
+ * gated_dropout_supported: 1 if these dimensions run here (state_dim % 32 == 0, message_dim % 16 == 0, message_dim >= 16), else
+ * the entries below return PTGNN_E_UNSUPPORTED.
+ * gated_forward_dropout: the contract of ptgnn_b200_gated_forward with fp32 states and no gather_states; the weight cache is the
+ * one of ptgnn_b200_gated_weight_cache_bytes(0, ...) and holds unscaled weights (shared with the call without dropout).  The
+ * workspace also holds the [E, state_dim / 32] keep bits.
+ * edge_messages_dropout_f32: messages[out_row[e]] = W_t(e) dropout(source_states[src32[e]]), the messages of the same mask for the
+ * same key (the layer's backward re-computes them). */
+int32_t ptgnn_b200_gated_dropout_supported(int32_t state_dim, int32_t message_dim);
+size_t ptgnn_b200_gated_dropout_workspace_bytes(int64_t num_nodes, int64_t num_edges, int32_t num_types, int32_t state_dim,
+                                                int32_t message_dim);
+int ptgnn_b200_gated_forward_dropout(const float *node_states, int64_t num_nodes, int32_t state_dim, int32_t message_dim, int32_t num_types,
+                                     const int64_t *type_off /*[host]*/, const int32_t *row_ptr, const int32_t *pos, const int32_t *src32,
+                                     const float *const *edge_weights /*[host]*/, const float *gru_w_ih, const float *gru_w_hh,
+                                     const float *gru_b_ih, const float *gru_b_hh, int32_t reduce, const uint32_t *key, float p,
+                                     float *out_states, void *workspace, size_t workspace_bytes, void *weight_cache,
+                                     size_t weight_cache_bytes, int32_t cache_valid, void *stream);
+size_t ptgnn_b200_edge_messages_dropout_workspace_bytes(int64_t num_edges, int32_t num_types, int32_t in_dim, int32_t message_dim);
+int ptgnn_b200_edge_messages_dropout_f32(const float *source_states, int32_t in_dim, int32_t message_dim, int32_t num_types,
+                                         const int64_t *type_off /*[host]*/, const int32_t *src32, const int32_t *out_row,
+                                         const float *const *edge_weights /*[host] T device pointers*/, const uint32_t *key, float p,
+                                         float *messages, void *workspace, size_t workspace_bytes, void *stream);
 
 /* MlpMessagePassingLayer.forward through the fused kernel (contract of ptgnn_b200_mlp_forward); the message
  * activation and the LayerNorm run in the fused kernel's write-out.  weight_cache (optional, fp32 states; ignored for bf16

@@ -17,13 +17,14 @@ The GRUs (gated layer, GruGlobalStateUpdate) take their gate pre-activations and
 tail (activation, LayerNorm, dense layer: mlpmessagepassing.py:114-117) is differentiated by a local ``torch.autograd.grad`` over
 library ops, and its output Dropout is a torch op applied outside the Function.
 
-The gated layer's training-mode dropout (a per-edge mask on the gathered rows, gatedmessagepassing.py:59) runs on the fused kernel
-where the eval-mode layer does (fp32 states, unsharded, no edge features): the mask is a pure function of a per-call key
-(csrc/edge_dropout.cuh), the forward applies it inside the fused aggregation, and ``_GatedDropoutFunction`` saves the key instead of
-any ``[E, H]`` tensor and regenerates the mask in its backward (``_aggregation_backward``'s ``drop``).  Other dimensions, and edge
-features under autograd, run as the reference writes the layer, with the Linear / scatter / GRUCell as differentiable native operators
-(``gated_forward_composed``).  fp32 states only.  Parity: ``tests/test_gpu_backward.py`` against ``torch.autograd`` through the CPU
-oracle (1e-4); ``tests/test_gpu_gated_dropout.py`` for the fused dropout.
+The gated layer's training-mode dropout (a per-edge mask on the gathered rows, gatedmessagepassing.py:59) runs on the native kernels
+(fp32 states, unsharded, no edge features): the mask is a pure function of a per-call key (csrc/edge_dropout.cuh), the forward
+applies it inside the fused aggregation or, at the dims the fused kernel does not take, inside the three-kernel path's message
+kernel, and ``_GatedDropoutFunction`` saves the key instead of any ``[E, H]`` tensor and regenerates the mask in its backward
+(``_aggregation_backward``'s ``drop``).  Edge features under autograd, and dims neither path takes, run as the reference writes the
+layer, with the Linear / scatter / GRUCell as differentiable native operators (``gated_forward_composed``).  fp32 states only.
+Parity: ``tests/test_gpu_backward.py`` against ``torch.autograd`` through the CPU oracle (1e-4); ``tests/test_gpu_gated_dropout.py``
+and ``tests/test_gpu_gated_dropout_widths.py`` for the dropout.
 """
 import ctypes
 import threading
@@ -189,8 +190,16 @@ class _GatedLayerFunction(torch.autograd.Function):
 def _recompute_aggregate(plan, h, W, reduce_name, drop=None):
     """(agg, arg) of agg = reduce_{e -> v} W_t(e) h[src(e)]: arg, for max / min, is which edge won each (target, feature), from the
     messages and the segmented reduce; sum / mean run the fused kernel where it takes the dimensions, and arg is None.  drop: the
-    per-edge dropout of the source rows (``EdgeDropout``): sum / mean on the fused kernel with the same key, max / min from the masked,
-    scaled rows."""
+    per-edge dropout of the source rows (``EdgeDropout``): at dims the fused kernel takes, sum / mean on it with the same key and
+    max / min from the masked, scaled rows; at the others, the masked messages of the three-kernel path and the segmented reduce."""
+    from .messagepassing import _use_fused
+
+    if drop is not None and not _use_fused(N.lib(), False, h.shape[1], W[0].shape[0]):
+        # the three-kernel path's masked messages, cat(types) order
+        msg = edge_messages_dropout(plan, h, W, drop.key, drop.p)
+        if reduce_name in ("max", "min"):
+            return C.segment_reduce(msg, plan, N.REDUCE[reduce_name], return_arg=True)
+        return C.segment_reduce(msg, plan, N.REDUCE[reduce_name]), None
     if drop is not None:
         if reduce_name in ("max", "min"):
             x = drop.apply(h, plan.src32)                                    # [E, H] dropout(h[src(e)]), cat(types) order
@@ -321,15 +330,30 @@ def aggregate_dropout(plan, h: torch.Tensor, W, reduce_code: int, key: torch.Ten
     return out
 
 
+def edge_messages_dropout(plan, h: torch.Tensor, W, key: torch.Tensor, p: float) -> torch.Tensor:
+    """``[E, D]`` messages ``W_t(e) dropout(h[src(e)])`` in cat(types) order on the masked message kernel, with the mask of ``key``."""
+    E, H = plan.num_edges, h.shape[1]
+    out = torch.empty(E, W[0].shape[0], dtype=torch.float32, device=h.device)
+    if E == 0:
+        return out
+    lib = N.lib()
+    ident = torch.arange(E, dtype=torch.int32, device=h.device)
+    ws_bytes = lib.ptgnn_b200_edge_messages_dropout_workspace_bytes(E, plan.num_types, H, W[0].shape[0])
+    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=h.device)
+    N.call("ptgnn_b200_edge_messages_dropout_f32", h.device, N.ptr(h), H, W[0].shape[0], plan.num_types, plan.type_off_c, N.ptr(plan.src32),
+           N.ptr(ident), N.ptr_table(W), N.ptr(key), float(p), N.ptr(out), N.ptr(ws), ws_bytes)
+    return out
+
+
 class _GatedDropoutFunction(torch.autograd.Function):
-    """The gated layer in training mode with per-edge dropout, on the fused kernel.  Saves h, the parameters and the 8-byte key: no
+    """The gated layer in training mode with per-edge dropout, on the native kernels.  Saves h, the parameters and the 8-byte key: no
     ``[E, H]`` tensor (gathered rows or mask) is kept for the backward, which regenerates the mask from the key."""
 
     @staticmethod
     def forward(ctx, layer, adjacency_lists, reduce_name, p, h, w_ih, w_hh, b_ih, b_hh, *weights):
         key = draw_dropout_key(h.device)
         with torch.no_grad():
-            out = layer._forward_fused_dropout(h.detach(), adjacency_lists, key, p)
+            out = layer._forward_dropout(h.detach(), adjacency_lists, key, p)
         ctx.save_for_backward(h, key, w_ih, w_hh, b_ih, b_hh, *weights)
         ctx.adjacency_lists, ctx.reduce_name, ctx.p = adjacency_lists, reduce_name, p
         return out
@@ -583,8 +607,8 @@ class _GRUCellFn(torch.autograd.Function):
 def gated_forward_composed(layer_weights, gru, node_states, adjacency_lists, edge_features, reduce_name, dropout_p: float):
     """GatedMessagePassingLayer.forward exactly as the reference writes it (gatedmessagepassing.py:46-69) -- gather, cat with the edge
     features, Dropout on the per-edge rows, per-type Linear, scatter, GRUCell -- with the Linear / scatter / GRUCell on the native
-    kernels as differentiable operators.  Used where the [E_t, H] gathered rows must exist: per-edge dropout (training mode) at
-    dimensions the fused kernel does not take (``_GatedDropoutFunction`` serves the others) and edge features under autograd."""
+    kernels as differentiable operators.  Used where the [E_t, H] gathered rows must exist: edge features under autograd, and per-edge
+    dropout (training mode) at dimensions neither native path takes (``_GatedDropoutFunction`` serves the others)."""
     num_nodes = node_states.shape[0]
     plan = plan_for(adjacency_lists, num_nodes)
     msgs = []

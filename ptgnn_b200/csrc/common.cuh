@@ -146,6 +146,10 @@ __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)_
 __device__ __forceinline__ void cp_async16(uint32_t dst_smem, const void *src, int src_bytes) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst_smem), "l"(src), "r"(src_bytes));
 }
+// 4-byte copy (cp.async takes 4- and 8-byte sizes through L1 only: .ca); src_bytes = 0 zero-fills without reading `src`
+__device__ __forceinline__ void cp_async4(uint32_t dst_smem, const void *src, int src_bytes) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;\n" ::"r"(dst_smem), "l"(src), "r"(src_bytes));
+}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }

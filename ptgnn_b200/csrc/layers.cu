@@ -13,6 +13,7 @@
 //      dense_update_kernel   Linear(+bias) + Tanh of the Mlp layer.
 #include <type_traits>
 
+#include "edge_dropout.cuh"
 #include "gemm_simt.cuh"
 #include "layers.cuh"
 #include "layers_tc.cuh"
@@ -323,9 +324,10 @@ static int check_unfused_dims(const char *who, bool bf16, int64_t N, int64_t E, 
 // [rows, D] messages or aggregates in the state dtype
 static size_t rows_bytes(bool bf16, int64_t rows, int D) { return ws_slice((size_t)rows * D * (bf16 ? 2 : 4) + 16, 1); }
 
-// gated workspace: msg | agg | FFMA GRU packing (fp32) | derived weights = [edge weights | GRU packing] (without a weight cache)
-struct GatedWs { size_t msg, agg, simt, weights, total; };
-static GatedWs gated_layout(bool bf16, int64_t N, int64_t E, int T, int H, int D) {
+// gated workspace: msg | agg | FFMA GRU packing (fp32) | derived weights = [edge weights | GRU packing] (without a weight cache) |
+// per-edge dropout keep bits (E_drop edges; 0 without dropout)
+struct GatedWs { size_t msg, agg, simt, weights, bits, total; };
+static GatedWs gated_layout(bool bf16, int64_t N, int64_t E, int T, int H, int D, int64_t E_drop = 0) {
     Layout l;
     GatedWs w;
     w.msg = l.add_bytes(rows_bytes(bf16, E, D));
@@ -333,8 +335,28 @@ static GatedWs gated_layout(bool bf16, int64_t N, int64_t E, int T, int H, int D
     w.simt = l.add_bytes(bf16 ? 0 : gru_simt_bytes(H, D));
     // fp32 states size the GRU packing for one gate block more than they use
     w.weights = l.add_bytes(tc::edge_weight_bytes(bf16, T, D, H) + tc::gru_pack_bytes(bf16, bf16 ? H : H + 32, D));
+    w.bits = l.add((size_t)E_drop * (H / 32), 4);
     w.total = l.total;
     return w;
+}
+
+// Per-edge dropout of the gathered source rows (edge_dropout.cuh): the key (two device words) and p.  fp32 states only.
+struct EdgeDrop {
+    const uint32_t *key;
+    float p;
+};
+
+// The dims the masked message step takes (PTGNN_E_UNSUPPORTED otherwise): the tensor-core message tiles, and H % 32 == 0 so that
+// one keep-bit word covers one k-chunk of a row.
+static int check_dropout_dims(const char *who, int H, int D) {
+    if (H % 32 == 0 && tc::supported_message(H, D)) return PTGNN_OK;
+    set_error("%s: per-edge dropout needs state dim %% 32 == 0 and message dim %% 16 == 0 (>= 16); got %d, %d", who, H, D);
+    return PTGNN_E_UNSUPPORTED;
+}
+static int check_dropout_args(const char *who, int64_t E, const uint32_t *key, float p) {
+    PTGNN_CHECK_ARG(p >= 0.0f && p <= 1.0f, "%s: p=%g outside [0, 1]", who, (double)p);
+    PTGNN_CHECK_ARG(E == 0 || key, "%s: null key", who);
+    return PTGNN_OK;
 }
 
 // gated weight cache: [edge weights | GRU packing]; 0 when fp32 states run a step on the FFMA kernels (nothing worth caching)
@@ -361,7 +383,7 @@ static int gated_unfused(const void *node_states, const void *gather_states, int
                          const int64_t *type_off, const int32_t *row_ptr, const int32_t *pos, const int32_t *src32,
                          const float *const *edge_weights, const float *w_ih, const float *w_hh, const float *b_ih,
                          const float *b_hh, int reduce, void *out_states, void *workspace, size_t workspace_bytes,
-                         void *weight_cache, size_t weight_cache_bytes, int cache_valid, cudaStream_t st) {
+                         void *weight_cache, size_t weight_cache_bytes, int cache_valid, cudaStream_t st, const EdgeDrop *drop = nullptr) {
     constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
     PTGNN_CHECK_ARG(num_types >= 0 && num_types <= PTGNN_MAX_EDGE_TYPES && type_off, "gated_forward: bad num_types=%d", num_types);
     const int64_t E = type_off[num_types];
@@ -371,7 +393,7 @@ static int gated_unfused(const void *node_states, const void *gather_states, int
     if (N == 0) return PTGNN_OK;
     PTGNN_CHECK_ARG(node_states && out_states && row_ptr && w_ih && w_hh && b_ih && b_hh, "gated_forward: null pointer");
     PTGNN_CHECK_ARG(E == 0 || (pos && src32 && edge_weights), "gated_forward: null edge arrays");
-    const GatedWs L = gated_layout(BF16, N, E, num_types, H, D);
+    const GatedWs L = gated_layout(BF16, N, E, num_types, H, D, drop ? E : 0);
     PTGNN_CHECK_WORKSPACE("gated_forward", workspace, workspace_bytes, L.total);
     char *ws = static_cast<char *>(workspace);
     // a weight cache is not used for dims that have nothing to cache
@@ -386,8 +408,17 @@ static int gated_unfused(const void *node_states, const void *gather_states, int
     const T *hsrc = gather_states ? static_cast<const T *>(gather_states) : h;   // rows that `src32` indexes (sharded runs)
     T *msg = reinterpret_cast<T *>(ws + L.msg), *agg = reinterpret_cast<T *>(ws + L.agg);
 
-    // 1. per-edge messages, written at their target-sorted positions
-    rc = edge_messages(hsrc, h, H, D, 0, num_types, type_off, edge_weights, src32, nullptr, pos, msg, area, pack, st);
+    // 1. per-edge messages, written at their target-sorted positions; with dropout, of the masked source rows
+    if constexpr (!BF16) {
+        if (drop != nullptr) {
+            uint32_t *bits = reinterpret_cast<uint32_t *>(ws + L.bits);
+            rc = edge_dropout_bits(drop->key, E, H, drop->p, nullptr, bits, st);
+            if (!rc)
+                rc = tc::edge_messages_dropout(hsrc, H, D, num_types, type_off, edge_weights, src32, pos,
+                                               tc::MsgDrop{bits, edge_dropout_scale(drop->p)}, msg, area, pack, st);
+        }
+    }
+    if (drop == nullptr) rc = edge_messages(hsrc, h, H, D, 0, num_types, type_off, edge_weights, src32, nullptr, pos, msg, area, pack, st);
     if (rc) return rc;
     // 2. streaming segmented reduce (fp32 accumulation)
     rc = launch_segment_reduce(msg, row_ptr, nullptr, N, E, D, reduce, agg, nullptr, nullptr, st);
@@ -464,7 +495,37 @@ extern "C" int ptgnn_b200_gated_forward(int32_t bf16_states, const void *node_st
     return (bf16_states ? gated_unfused<__nv_bfloat16> : gated_unfused<float>)(
         node_states, gather_states, num_nodes, state_dim, message_dim, num_types, type_off, row_ptr, pos, src32, edge_weights,
         gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, reduce, out_states, workspace, workspace_bytes, weight_cache, weight_cache_bytes,
-        cache_valid, static_cast<cudaStream_t>(stream));
+        cache_valid, static_cast<cudaStream_t>(stream), nullptr);
+}
+
+extern "C" int32_t ptgnn_b200_gated_dropout_supported(int32_t state_dim, int32_t message_dim) {
+    return state_dim > 0 && state_dim <= 1024 && message_dim > 0 && message_dim <= 512 && state_dim % 32 == 0 &&
+           tc::supported_message(state_dim, message_dim);
+}
+
+extern "C" size_t ptgnn_b200_gated_dropout_workspace_bytes(int64_t num_nodes, int64_t num_edges, int32_t num_types, int32_t state_dim,
+                                                           int32_t message_dim) {
+    if (num_nodes < 0 || num_edges < 0 || num_types < 0 || state_dim <= 0 || state_dim % 32 != 0 || message_dim <= 0) return 0;
+    return gated_layout(false, num_nodes, num_edges, num_types, state_dim, message_dim, num_edges).total;
+}
+
+extern "C" int ptgnn_b200_gated_forward_dropout(const float *node_states, int64_t num_nodes, int32_t state_dim, int32_t message_dim,
+                                                int32_t num_types, const int64_t *type_off, const int32_t *row_ptr, const int32_t *pos,
+                                                const int32_t *src32, const float *const *edge_weights, const float *gru_w_ih,
+                                                const float *gru_w_hh, const float *gru_b_ih, const float *gru_b_hh, int32_t reduce,
+                                                const uint32_t *key, float p, float *out_states, void *workspace, size_t workspace_bytes,
+                                                void *weight_cache, size_t weight_cache_bytes, int32_t cache_valid, void *stream) {
+    const char *who = "gated_forward_dropout";
+    PTGNN_CHECK_ARG(num_types >= 0 && num_types <= PTGNN_MAX_EDGE_TYPES && type_off, "%s: bad num_types=%d", who, num_types);
+    const int64_t E = type_off[num_types];
+    int rc = check_layer_dims(who, num_nodes, E, state_dim, message_dim);
+    if (!rc) rc = check_dropout_dims(who, state_dim, message_dim);
+    if (!rc) rc = check_dropout_args(who, E, key, p);
+    if (rc) return rc;
+    const EdgeDrop drop{key, p};
+    return gated_unfused<float>(node_states, nullptr, num_nodes, state_dim, message_dim, num_types, type_off, row_ptr, pos, src32,
+                                edge_weights, gru_w_ih, gru_w_hh, gru_b_ih, gru_b_hh, reduce, out_states, workspace, workspace_bytes,
+                                weight_cache, weight_cache_bytes, cache_valid, static_cast<cudaStream_t>(stream), &drop);
 }
 
 extern "C" size_t ptgnn_b200_mlp_workspace_bytes(int32_t bf16_states, int64_t num_nodes, int64_t num_edges, int32_t num_types,
@@ -531,6 +592,43 @@ extern "C" int ptgnn_b200_edge_messages_f32(const float *source_states, const fl
     }
     return edge_messages(source_states, target_states, in_dim, message_dim, use_target_state ? 1 : 0, num_types, type_off, edge_weights,
                          src32, tgt32, out_row, messages, workspace, true, st);
+}
+
+// workspace: derived edge weights | keep bits [E, H / 32]
+struct MsgDropWs { size_t weights, bits, total; };
+static MsgDropWs msg_drop_layout(int64_t E, int T, int H, int D) {
+    Layout l;
+    MsgDropWs w;
+    w.weights = l.add_bytes(tc::edge_weight_bytes(false, T, D, H));
+    w.bits = l.add((size_t)E * (H / 32), 4);
+    w.total = l.total;
+    return w;
+}
+extern "C" size_t ptgnn_b200_edge_messages_dropout_workspace_bytes(int64_t num_edges, int32_t num_types, int32_t in_dim, int32_t message_dim) {
+    if (num_edges < 0 || num_types < 0 || in_dim <= 0 || in_dim % 32 != 0 || message_dim <= 0) return 0;
+    return msg_drop_layout(num_edges, num_types, in_dim, message_dim).total;
+}
+extern "C" int ptgnn_b200_edge_messages_dropout_f32(const float *source_states, int32_t in_dim, int32_t message_dim, int32_t num_types,
+                                                    const int64_t *type_off, const int32_t *src32, const int32_t *out_row,
+                                                    const float *const *edge_weights, const uint32_t *key, float p, float *messages,
+                                                    void *workspace, size_t workspace_bytes, void *stream) {
+    const char *who = "edge_messages_dropout";
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    PTGNN_CHECK_ARG(num_types >= 0 && num_types <= PTGNN_MAX_EDGE_TYPES && type_off, "%s: bad num_types=%d", who, num_types);
+    const int64_t E = type_off[num_types];
+    int rc = check_layer_dims(who, 0, E, in_dim, message_dim);
+    if (!rc) rc = check_dropout_dims(who, in_dim, message_dim);
+    if (!rc) rc = check_dropout_args(who, E, key, p);
+    if (rc) return rc;
+    if (E == 0) return PTGNN_OK;
+    PTGNN_CHECK_ARG(source_states && src32 && out_row && edge_weights && messages, "%s: null pointer", who);
+    const MsgDropWs L = msg_drop_layout(E, num_types, in_dim, message_dim);
+    PTGNN_CHECK_WORKSPACE(who, workspace, workspace_bytes, L.total);
+    char *ws = static_cast<char *>(workspace);
+    uint32_t *bits = reinterpret_cast<uint32_t *>(ws + L.bits);
+    PTGNN_TRY(edge_dropout_bits(key, E, in_dim, p, nullptr, bits, st));
+    return tc::edge_messages_dropout(source_states, in_dim, message_dim, num_types, type_off, edge_weights, src32, out_row,
+                                     tc::MsgDrop{bits, edge_dropout_scale(p)}, messages, ws + L.weights, true, st);
 }
 
 extern "C" size_t ptgnn_b200_grucell_workspace_bytes(int32_t state_dim, int32_t input_dim) {

@@ -27,7 +27,7 @@ template <> struct Pipe<float> {
     static constexpr CUtensorMapDataType DTYPE = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
     static constexpr int CHUNK_K = tc::CHUNK_K;
     template <class P> static int launch(const typename P::Params &p, int tiles, int category, cudaStream_t st) {
-        return launch_pipeline(tc_pipeline_kernel<P>, p, tc::SMEM_BYTES, tiles, category, st);
+        return launch_pipeline(tc_pipeline_kernel<P>, p, P::DROP ? tc::SMEM_BYTES_DROP : tc::SMEM_BYTES, tiles, category, st);
     }
 };
 template <> struct Pipe<__nv_bfloat16> {
@@ -162,6 +162,7 @@ __device__ __forceinline__ void store_words(int end, int w0, float *stage, const
 template <class T>
 struct MsgPolicy {
     static constexpr bool GATHER = true;
+    static constexpr bool DROP = false;
     struct Params {
         CUtensorMap map_w[B_MAPS<T>];     // [T*D, Kw] (Kw = H, or 2H with target states), box {CHUNK_K, min(128, D)}
         const T *h, *h_tgt;               // rows indexed by src32 / by tgt32 (Mlp layers with use_target_state)
@@ -232,12 +233,29 @@ struct MsgPolicy {
     }
 };
 
+// policy 1b: per-edge messages of GatedMessagePassingLayer with its per-edge dropout (edge_dropout.cuh), fp32 states.  Tile row r
+// is edge e = e0 + r in cat(types) order, the order the mask is defined on, so the keep bits of its k-chunk kc are word kc of row e
+// of the [E, H / 32] bits.  The pipeline clears the dropped elements of the A operand and multiplies the products by 1 / (1 - p)
+// before this store, so the derived weights (and a weight cache holding them) are those of MsgPolicy<float>.
+struct MsgDropPolicy : MsgPolicy<float> {
+    static constexpr bool DROP = true;
+    struct Params : MsgPolicy<float>::Params {
+        const uint32_t *bits;   // [E, H / 32] keep bits, cat(types) order
+        float scale;            // 1 / (1 - p); 0 for p = 1
+    };
+    __device__ static const uint32_t *drop_row(const Params &p, const Tile &ti, int r) {
+        const int e = ti.e0 + r;
+        return e < ti.e_end ? p.bits + (size_t)e * (p.H / 32) : nullptr;
+    }
+};
+
 // =================================================================================================
 // policy 2: nn.GRUCell update, 32 hidden units per tile
 // =================================================================================================
 template <class T>
 struct GruPolicy {
     static constexpr bool GATHER = false;
+    static constexpr bool DROP = false;
     struct Params {
         CUtensorMap map_agg, map_h;                              // [N, D], [N, H], box {CHUNK_K, 128}
         CUtensorMap map_p1[B_MAPS<T>], map_p2[B_MAPS<T>];        // [n_jb*128, D] / [n_jb*128, H], box {CHUNK_K, 128}
@@ -355,6 +373,7 @@ struct GruPolicy {
 template <class T>
 struct DensePolicy {
     static constexpr bool GATHER = false;
+    static constexpr bool DROP = false;
     struct Params {
         CUtensorMap map_y, map_w[B_MAPS<T>];   // [N, D] box {CHUNK_K, 128}; [Hout, D] box {CHUNK_K, min(128, Hout)}
         const float *bias;                     // [Hout] or nullptr
@@ -462,22 +481,45 @@ static int make_b_maps(CUtensorMap (&maps)[B_MAPS<T>], const T *w, const T *w_lo
     return rc;
 }
 
+// Derives the edge weights (unless `scratch` is a weight cache) and fills the message step's parameters; `tiles` = launch tiles.
 template <class T>
-int edge_messages(const T *h_src, const T *h_tgt, int H, int D, int use_target, int num_types, const int64_t *type_off,
-                  const float *const *weights, const int32_t *src32, const int32_t *tgt32, const int32_t *pos, T *msg,
-                  void *scratch, bool pack, cudaStream_t st) {
+static int message_params(typename MsgPolicy<T>::Params &p, int &tiles, const T *h_src, const T *h_tgt, int H, int D, int use_target,
+                          int num_types, const int64_t *type_off, const float *const *weights, const int32_t *src32,
+                          const int32_t *tgt32, const int32_t *pos, T *msg, void *scratch, bool pack, cudaStream_t st) {
     const int Kw = use_target ? 2 * H : H;
     T *w = static_cast<T *>(scratch);
     T *w_lo = reinterpret_cast<T *>(static_cast<char *>(scratch) + ws_slice((size_t)num_types * D * Kw, 4));   // fp32 only
     int rc = pack ? derive_weights(weights, num_types, D * Kw, w, w_lo, st) : PTGNN_OK;   // false: `scratch` is a weight cache
     if (rc) return rc;
-    typename MsgPolicy<T>::Params p{};
     rc = make_b_maps(p.map_w, w, w_lo, (uint64_t)num_types * D, Kw, D < 128 ? D : 128);
     if (rc) return rc;
     p.h = h_src; p.h_tgt = h_tgt; p.src32 = src32; p.tgt32 = tgt32; p.pos = pos; p.msg = msg;
     p.H = H; p.D = D; p.use_target = use_target; p.num_types = num_types; p.n_blocks = (D + 127) / 128;
-    const int tiles = build_type_tiles(type_off, num_types, TILE_M, p.edge_off, p.tile_off);
-    return Pipe<T>::template launch<MsgPolicy<T>>(p, tiles * p.n_blocks, PTGNN_KERNEL_MESSAGE, st);
+    tiles = build_type_tiles(type_off, num_types, TILE_M, p.edge_off, p.tile_off) * p.n_blocks;
+    return PTGNN_OK;
+}
+
+template <class T>
+int edge_messages(const T *h_src, const T *h_tgt, int H, int D, int use_target, int num_types, const int64_t *type_off,
+                  const float *const *weights, const int32_t *src32, const int32_t *tgt32, const int32_t *pos, T *msg,
+                  void *scratch, bool pack, cudaStream_t st) {
+    typename MsgPolicy<T>::Params p{};
+    int tiles = 0;
+    PTGNN_TRY(message_params<T>(p, tiles, h_src, h_tgt, H, D, use_target, num_types, type_off, weights, src32, tgt32, pos, msg, scratch,
+                                pack, st));
+    return Pipe<T>::template launch<MsgPolicy<T>>(p, tiles, PTGNN_KERNEL_MESSAGE, st);
+}
+
+int edge_messages_dropout(const float *h, int H, int D, int num_types, const int64_t *type_off, const float *const *weights,
+                          const int32_t *src32, const int32_t *pos, const MsgDrop &drop, float *msg, void *scratch, bool pack,
+                          cudaStream_t st) {
+    MsgDropPolicy::Params p{};
+    int tiles = 0;
+    PTGNN_TRY(message_params<float>(p, tiles, h, nullptr, H, D, 0, num_types, type_off, weights, src32, nullptr, pos, msg, scratch, pack,
+                                    st));
+    p.bits = drop.bits;
+    p.scale = drop.scale;
+    return Pipe<float>::launch<MsgDropPolicy>(p, tiles, PTGNN_KERNEL_MESSAGE, st);
 }
 
 template <class T>

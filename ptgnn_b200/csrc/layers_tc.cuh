@@ -23,6 +23,16 @@ template <class T>
 int edge_messages(const T *h_src, const T *h_tgt, int H, int D, int use_target, int num_types, const int64_t *type_off,
                   const float *const *weights, const int32_t *src32, const int32_t *tgt32, const int32_t *pos, T *msg,
                   void *scratch, bool pack, cudaStream_t st);
+// The per-edge dropout of GatedMessagePassingLayer (edge_dropout.cuh) on the gathered source rows: keep bits [E, H / 32] in
+// cat(types) order (edge_dropout_bits with eid NULL) and the scale of a kept element (edge_dropout_scale).
+struct MsgDrop {
+    const uint32_t *bits;
+    float scale;
+};
+// messages[pos[e]] = W_t(e) dropout(h[src(e)]), fp32 states, H % 32 == 0 (scratch, pack: as edge_messages with Kw = H)
+int edge_messages_dropout(const float *h, int H, int D, int num_types, const int64_t *type_off, const float *const *weights,
+                          const int32_t *src32, const int32_t *pos, const MsgDrop &drop, float *msg, void *scratch, bool pack,
+                          cudaStream_t st);
 // out = GRUCell(agg, h)                                     (scratch >= gru_pack_bytes)
 template <class T>
 int gru_update(const T *agg, const T *h, int64_t num_nodes, int H, int D, const float *w_ih, const float *w_hh,

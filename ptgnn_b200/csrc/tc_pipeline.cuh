@@ -17,7 +17,9 @@
 //
 // One CTA per SM (grid = #SMs), static round-robin over tiles.
 //   shared memory: 3 slots x 48 KB (raw A | B_hi | B_lo, 128-byte SWIZZLE_128B rows) + 1 KB row indices + the 128 x 132 fp32
-//   accumulator tile (whose rows also serve as the epilogue's transpose buffers once drained)
+//   accumulator tile (whose rows also serve as the epilogue's transpose buffers once drained); DROP policies: + 3 x 512 B of
+//   keep-bit words, one per row and slot, staged by the gatherers with a 4-byte cp.async next to the row and completed on the
+//   same landed[slot] barrier
 // Every mbarrier wait is bounded (tc_common.cuh): a protocol bug traps instead of hanging the GPU.
 //
 // A Policy supplies:
@@ -36,6 +38,10 @@
 //   __device__ static void smem_init(const Params&, float *tables);   bf16 pipeline only: fills its policy tables
 //   __device__ static void store(const Params&, const Tile&, float (&acc)[64], const Pre&, int half, int lane, float* stage,
 //                                float* tables);   (tables: nullptr here, the smem_init area in the bf16 pipeline)
+//   static constexpr bool DROP;   this pipeline only: a keep-bit word per (gathered row, k-chunk) clears dropped A elements, and
+//                          the accumulators are multiplied by Params::scale before the epilogue.  Only when DROP:
+//   __device__ static const uint32_t *drop_row(const Params&, const Tile&, int r);   the words of tile row r, one per k-chunk,
+//                          or nullptr for a row past the tile's end
 // The policies (layers_tc.cu) serve both pipelines; the bf16 one (tc_pipeline_bf16.cuh) takes Segment<__nv_bfloat16>.
 #pragma once
 #include <cuda.h>
@@ -71,6 +77,11 @@ constexpr int BARRIER_BYTES = 256;
 constexpr int ACC_BYTES = TILE_M * ACC_PITCH * 4;
 constexpr int SMEM_BYTES = RING_BYTES + 1024 /*alignment slack*/ + BARRIER_BYTES + INDEX_BYTES + ACC_BYTES;
 static_assert(SMEM_BYTES <= 232448, "shared memory budget");
+// DROP policies: one keep-bit word per row and slot after the accumulator tile (CHUNK_K = 32 features = one word per row)
+constexpr int DROP_BITS_BYTES = NUM_SLOTS * TILE_M * 4;
+constexpr int SMEM_BYTES_DROP = SMEM_BYTES + DROP_BITS_BYTES;
+static_assert(SMEM_BYTES_DROP <= 232448, "shared memory budget (DROP)");
+static_assert(CHUNK_K == 32, "one keep-bit word per row and k-chunk");
 static_assert(4 * STAGE_FLOATS_PER_WARP <= 64 * ACC_PITCH, "a warpgroup's transpose buffers fit in its accumulator rows");
 
 template <class T>       // T = float (this pipeline) or __nv_bfloat16 (tc_pipeline_bf16.cuh); element counts are in T
@@ -259,6 +270,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
                 for (int i = 0; i < 16; ++i) rows[i] = rows_s[rsub + 8 * i];
                 const float *a_q = sg.a + q * 4;
                 const uint32_t soff = swz(rsub, q);     // rows rsub + 8 i share (row & 7): the swizzle term is per-thread constant
+                // DROP: this thread also stages the keep-bit words of tile rows g and g + 64 (zero-filled past the tile's end)
+                const uint32_t *keep_row0 = nullptr, *keep_row1 = nullptr;
+                if constexpr (Policy::DROP) {
+                    keep_row0 = Policy::drop_row(p, t, g);
+                    keep_row1 = Policy::drop_row(p, t, g + 64);
+                }
                 for (int kc = 0; kc < nkc; ++kc, ++c) {
                     const uint32_t slot = c % NUM_SLOTS, use = c / NUM_SLOTS;
                     mbar_wait(&a_free[slot], (use & 1) ^ 1);
@@ -270,6 +287,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
                         const bool ok = k_ok && rows[i] >= 0;
                         const float *src = ok ? a_q + (size_t)rows[i] * sg.lda + kchunk : sg.a;
                         cp_async16(sbase + i * 1024, src, ok ? 16 : 0);
+                    }
+                    if constexpr (Policy::DROP) {
+                        const uint32_t kbase = smem_u32(ring + RING_BYTES + BARRIER_BYTES + INDEX_BYTES + ACC_BYTES) + slot * (TILE_M * 4);
+                        cp_async4(kbase + g * 4, keep_row0 ? keep_row0 + kc : static_cast<const void *>(sg.a), keep_row0 ? 4 : 0);
+                        cp_async4(kbase + (g + 64) * 4, keep_row1 ? keep_row1 + kc : static_cast<const void *>(sg.a), keep_row1 ? 4 : 0);
                     }
                     cp_async_mbar_arrive_noinc(&landed[slot]);
                 }
@@ -335,6 +357,19 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
                             a_lo[ks][i] = __float_as_uint(x - h);
                         }
                     }
+                    if constexpr (Policy::DROP) {
+                        // clear the dropped elements: 0 in both TF32 halves, so the kept elements' products are unchanged.  The keep
+                        // words of rows r0 / r1 are read after the fragment, when its addresses are dead (fewer live registers)
+                        const uint32_t *kw = reinterpret_cast<const uint32_t *>(ring + RING_BYTES + BARRIER_BYTES + INDEX_BYTES + ACC_BYTES) +
+                                             slot * TILE_M;
+                        // this thread's 16 bits in one word: bit 4 j + (i & 1) = row (r0, r1)[i & 1], column tq + 4 j
+                        const uint32_t keep = ((kw[r0] >> tq) & 0x11111111u) | (((kw[r1] >> tq) & 0x11111111u) << 1);
+#pragma unroll
+                        for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+                            for (int i = 0; i < 4; ++i)
+                                if (!((keep >> (8 * ks + 4 * (i >> 1) + (i & 1))) & 1u)) { a_hi[ks][i] = 0u; a_lo[ks][i] = 0u; }
+                    }
                     if (Policy::GATHER) {
                         __syncwarp();
                         if (lane == 0) mbar_arrive(&a_free[slot]);       // raw tile consumed (values are in registers)
@@ -376,6 +411,15 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
             }
             // ---- accumulator tile -> shared memory (main + correction), then the policy epilogue, one row per thread
             named_bar_sync(bar_id, 128);          // the warpgroup's previous epilogue no longer reads these rows
+            if constexpr (Policy::DROP) {
+                // 1 / (1 - p) of the kept elements, applied to the product here rather than in the policy store: a multiply there
+                // kept more registers live through the epilogue (more spills)
+                const float s = p.scale;
+#pragma unroll
+                for (int j = 0; j < 4; ++j)
+#pragma unroll
+                    for (int i = 0; i < 16; ++i) { acc_m[j][i] *= s; acc_c[j][i] *= s; }
+            }
 #pragma unroll
             for (int j = 0; j < 4; ++j)
 #pragma unroll

@@ -63,6 +63,12 @@ def _use_fused(lib, bf16: bool, H: int, D: int) -> bool:
     return fused_allowed(bf16) and bool(lib.ptgnn_b200_fused_supported(int(bf16), H, D))
 
 
+def _native_dropout(lib, H: int, D: int) -> bool:
+    """GatedMessagePassingLayer's per-edge dropout (fp32 states) runs natively at these dims: inside the fused aggregation where it
+    takes them, else on the three-kernel path's masked message kernel."""
+    return _use_fused(lib, False, H, D) or bool(lib.ptgnn_b200_gated_dropout_supported(H, D))
+
+
 def _check_states(node_states: torch.Tensor, expected_dim: int, what: str) -> None:
     if node_states.dim() != 2 or node_states.shape[1] != expected_dim:
         raise ValueError(f"{what}: node_states must be [num_nodes, {expected_dim}], got {tuple(node_states.shape)}")
@@ -242,17 +248,17 @@ class GatedMessagePassingLayer(AbstractMessagePassingLayer):
         drop_p = self.__dropout.p if self.training else 0.0
         grad = _ag.needs_grad(self, node_states)
         if (drop_p > 0 and gather_states is None and node_states.dtype == torch.float32 and self.__edge_feature_dimension == 0
-                and _use_fused(N.lib(), False, self.__state_dimension, self.__message_dimension)):
-            # per-edge dropout (gatedmessagepassing.py:59) inside the fused aggregation: the mask is a function of a per-call key
+                and _native_dropout(N.lib(), self.__state_dimension, self.__message_dimension)):
+            # per-edge dropout (gatedmessagepassing.py:59) inside the native kernels: the mask is a function of a per-call key
             _check_states(node_states, self.__state_dimension, "GatedMessagePassingLayer")
             h = N.require_cuda(node_states, "node_states", torch.float32)
             if grad:
                 gru = self.__state_update
                 return _ag.gated_dropout_with_grad(self, h, adjacency_lists, self.__aggregation_fn, drop_p, gru.weight_ih, gru.weight_hh,
                                                    gru.bias_ih, gru.bias_hh, [lin.weight for lin in linears])
-            return self._forward_fused_dropout(h, adjacency_lists, _ag.draw_dropout_key(h.device), drop_p)
+            return self._forward_dropout(h, adjacency_lists, _ag.draw_dropout_key(h.device), drop_p)
         if drop_p > 0 or (grad and self.__edge_feature_dimension != 0):
-            # per-edge dropout outside the fused kernel's dimensions / edge features under autograd: the gathered rows have to exist --
+            # per-edge dropout outside the native kernels' dimensions / edge features under autograd: the gathered rows have to exist --
             # the layer as the reference writes it, Linear / scatter / GRUCell on the native kernels as differentiable operators
             if gather_states is not None or node_states.dtype != torch.float32:
                 raise NotImplementedError("training-mode dropout / edge features with gradients: fp32 states, unsharded only")
@@ -328,16 +334,12 @@ class GatedMessagePassingLayer(AbstractMessagePassingLayer):
 
     @property
     def edge_dropout_active(self) -> bool:
-        """Training mode with per-edge dropout: the layer's fused path then needs the plan's ``block_edge_ids``."""
-        return self.training and self.__dropout.p > 0
+        """Training mode with per-edge dropout at dims the fused kernel takes: the layer's fused path then needs the plan's
+        ``block_edge_ids`` (the three-kernel path reads the mask in cat(types) order and needs none)."""
+        return self.training and self.__dropout.p > 0 and _use_fused(N.lib(), False, self.__state_dimension, self.__message_dimension)
 
-    def _forward_fused_dropout(self, h: torch.Tensor, adjacency_lists, key: torch.Tensor, p: float) -> torch.Tensor:
-        """The fused path with per-edge dropout (fp32 states, unsharded, no edge features) for the mask of ``key`` (int32 [2], device):
-        the keep bits are generated up front, the fused kernel clears the dropped features of the gathered rows, and 1 / (1 - p) is
-        folded into the packed edge weights (a weight-cache entry of its own per p)."""
-        num_nodes, H = h.shape
-        D = self.__message_dimension
-        plan = self._plan(adjacency_lists, num_nodes)
+    def _dropout_params(self, H: int, D: int):
+        """(edge weights, w_ih, w_hh, b_ih, b_hh) of the dropout paths, checked for the shapes the kernels assume."""
         gru = self.__state_update
         weights = [N.require_cuda(lin.weight, "edge weight", torch.float32) for lin in self.__edge_message_transformation_layers]
         w_ih, w_hh = N.require_cuda(gru.weight_ih, "weight_ih", torch.float32), N.require_cuda(gru.weight_hh, "weight_hh", torch.float32)
@@ -346,6 +348,44 @@ class GatedMessagePassingLayer(AbstractMessagePassingLayer):
             _check_shape(w, (D, H), f"edge weight {i}")
         _check_shape(w_ih, (3 * H, D), "GRUCell.weight_ih"); _check_shape(w_hh, (3 * H, H), "GRUCell.weight_hh")
         _check_shape(b_ih, (3 * H,), "GRUCell.bias_ih"); _check_shape(b_hh, (3 * H,), "GRUCell.bias_hh")
+        return weights, w_ih, w_hh, b_ih, b_hh
+
+    def _forward_dropout(self, h: torch.Tensor, adjacency_lists, key: torch.Tensor, p: float) -> torch.Tensor:
+        """Per-edge dropout (fp32 states, unsharded, no edge features) for the mask of ``key`` (int32 [2], device): on the fused kernel
+        where it takes the dims, else on the three-kernel path."""
+        if _use_fused(N.lib(), False, self.__state_dimension, self.__message_dimension):
+            return self._forward_fused_dropout(h, adjacency_lists, key, p)
+        return self._forward_unfused_dropout(h, adjacency_lists, key, p)
+
+    def _forward_unfused_dropout(self, h: torch.Tensor, adjacency_lists, key: torch.Tensor, p: float) -> torch.Tensor:
+        """The three-kernel path with per-edge dropout: the keep bits in cat(types) order, the masked tensor-core message kernel (the
+        dropped elements of each gathered row are cleared before the products, which are scaled by 1 / (1 - p)), the segmented reduce
+        and the GRUCell step.  The derived weights are those of the path without dropout, so the two share a weight-cache entry."""
+        num_nodes, H = h.shape
+        D = self.__message_dimension
+        plan = self._plan(adjacency_lists, num_nodes)
+        weights, w_ih, w_hh, b_ih, b_hh = self._dropout_params(H, D)
+        lib = N.lib()
+        cache, valid = self._weight_cache("f32", lib.ptgnn_b200_gated_weight_cache_bytes(0, plan.num_types, H, D),
+                                          weights + [w_ih, w_hh, b_ih, b_hh], h.device)
+        ws_bytes = lib.ptgnn_b200_gated_dropout_workspace_bytes(num_nodes, plan.num_edges, plan.num_types, H, D)
+        ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=h.device)
+        out = torch.empty_like(h)
+        N.call("ptgnn_b200_gated_forward_dropout", h.device, N.ptr(h), num_nodes, H, D, plan.num_types, plan.type_off_c, N.ptr(plan.row_ptr),
+               N.ptr(plan.pos), N.ptr(plan.src32), N.ptr_table(weights), N.ptr(w_ih), N.ptr(w_hh), N.ptr(b_ih), N.ptr(b_hh),
+               _reduce_code(self.__aggregation_fn), N.ptr(key), float(p), N.ptr(out), N.ptr(ws), ws_bytes, N.ptr(cache),
+               0 if cache is None else cache.numel(), int(valid))
+        self._weight_cache_filled("f32", h.device)
+        return out
+
+    def _forward_fused_dropout(self, h: torch.Tensor, adjacency_lists, key: torch.Tensor, p: float) -> torch.Tensor:
+        """The fused path with per-edge dropout (fp32 states, unsharded, no edge features) for the mask of ``key`` (int32 [2], device):
+        the keep bits are generated up front, the fused kernel clears the dropped features of the gathered rows, and 1 / (1 - p) is
+        folded into the packed edge weights (a weight-cache entry of its own per p)."""
+        num_nodes, H = h.shape
+        D = self.__message_dimension
+        plan = self._plan(adjacency_lists, num_nodes)
+        weights, w_ih, w_hh, b_ih, b_hh = self._dropout_params(H, D)
         lib = N.lib()
         kind = ("f32_fused_dropout", float(p))
         cache, valid = self._weight_cache(kind, lib.ptgnn_b200_gated_fused_weight_cache_bytes(0, plan.num_types, H, D),
