@@ -363,6 +363,38 @@ int ptgnn_b200_gather_split_f16(const float *x, const int32_t *index, int64_t ro
 int ptgnn_b200_gru_gate_grads_f32(const float *gi, const float *gh, const float *h, const float *grad_out, int64_t num_nodes,
                                   int32_t state_dim, float *d_gi, float *d_gh, float *d_h_direct, void *stream);
 
+/* Backward of MlpMessagePassingLayer with bf16 node states (host side: ptgnn_b200/autograd.py).
+ * edge_weight_grad_bf16: out[t] [message_dim, C] fp32 = sum over the edges e of type t (cat(types) order, type_off [host]) of
+ *   grad_rows[grad_index ? grad_index[e] : e] (x) [node_states[src32[e]] ; node_states[tgt32[e]]], C = in_dim (source half only,
+ *   use_target_state == 0) or 2 in_dim; bf16 operands (grad_rows [*, message_dim], node_states [*, in_dim]), fp32 accumulation.
+ *   The gathered operands are never written to memory.  Split-K over fixed edge chunks with the partials added in chunk order: the
+ *   result depends only on the inputs (no float atomics).  A type without edges gets zeros.  Supported: in_dim, message_dim
+ *   multiples of 8, <= 1024 (PTGNN_E_UNSUPPORTED otherwise). */
+int32_t ptgnn_b200_edge_weight_grad_bf16_supported(int32_t in_dim, int32_t message_dim);
+size_t ptgnn_b200_edge_weight_grad_bf16_workspace_bytes(int64_t num_edges, int32_t num_types, int32_t in_dim, int32_t message_dim,
+                                                        int32_t use_target_state);
+int ptgnn_b200_edge_weight_grad_bf16(const void *grad_rows, const int32_t *grad_index /* NULL: row e */, const void *node_states,
+                                     int32_t in_dim, int32_t message_dim, int32_t num_types, const int64_t *type_off /*[host]*/,
+                                     const int32_t *src32, const int32_t *tgt32, int32_t use_target_state, float *out, void *workspace,
+                                     size_t workspace_bytes, void *stream);
+/* The bf16 aggregate as fp32, reduce_{e -> v} W_t(e) [h_src ; h_tgt] [num_nodes, 128], computed as ptgnn_b200_mlp_forward_fused
+ * computes it for bf16 states (bf16 products, messages rounded to bf16, fp32 reduction) and written before any rounding: the point
+ * the layer's backward differentiates its node-sized tail at.  Dims of ptgnn_b200_fused_supported(1, in_dim, 128). */
+size_t ptgnn_b200_fused_aggregate_bf16_workspace_bytes(int32_t num_types, int32_t in_dim, int32_t use_target_state);
+int ptgnn_b200_fused_aggregate_bf16(const void *node_states, int64_t num_nodes, int32_t in_dim, int32_t num_types,
+                                    const ptgnn_b200_block_plan *block_plan, const int32_t *row_ptr,
+                                    const float *const *edge_weights /*[host] T device pointers, fp32*/, int32_t use_target_state,
+                                    int32_t reduce, float *out, void *workspace, size_t workspace_bytes, void *stream);
+/* The bf16 messages of the three-kernel path: messages[out_row[e]] = bf16(W_t(e) [source_states[src32[e]] ; target_states[tgt32[e]]])
+ * for bf16 states, the contract of ptgnn_b200_edge_messages_f32 otherwise.  Supported (edge_messages_bf16_supported): the bf16
+ * dims of ptgnn_b200_mlp_forward (in_dim % 32 == 0, >= 64; message_dim % 16 == 0 in [64, 256]). */
+int32_t ptgnn_b200_edge_messages_bf16_supported(int32_t in_dim, int32_t message_dim);
+size_t ptgnn_b200_edge_messages_bf16_workspace_bytes(int32_t num_types, int32_t in_dim, int32_t message_dim, int32_t use_target_state);
+int ptgnn_b200_edge_messages_bf16(const void *source_states, const void *target_states /* NULL if unused */, int32_t in_dim,
+                                  int32_t message_dim, int32_t num_types, const int64_t *type_off /*[host]*/, const int32_t *src32,
+                                  const int32_t *tgt32, const int32_t *out_row, const float *const *edge_weights /*[host]*/,
+                                  int32_t use_target_state, void *messages, void *workspace, size_t workspace_bytes, void *stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Device-side minibatch finalisation -- the graph-structure half of GraphNeuralNetworkModel.extend_minibatch_with /
  * finalize_minibatch (ptgnn/neuralmodels/gnn/graphneuralnetwork.py:386-493).  The host concatenates the graphs' LOCAL int32

@@ -12,6 +12,10 @@ their aggregation agg = reduce_{e -> v} W_t(e) [h_src(e) ; h_tgt(e)], ``_aggrega
   edges or nodes) -- library GEMMs on the tensor cores in the forward's 3xFP16 split (``_mm_t_split``: three cuBLAS fp16 GEMMs with
   fp32 accumulation per product, operands scaled by a power of two first); bias gradients are column sums.
 
+The Mlp layer with bf16 states (default message MLP, string aggregation) takes the same steps on the bf16 kernels: the aggregate and
+the transposed aggregations as the bf16 forward computes them, and ``dW_t`` on the gathered bf16 weight-gradient kernel
+(``_weight_grad_bf16``, csrc/wgrad.cu).  Parity: ``tests/test_gpu_mlp_bf16_backward.py``.
+
 The GRUs (gated layer, GruGlobalStateUpdate) take their gate pre-activations and input-gradient products on the native dense kernel
 (``composed.linear``) and the gate derivatives from one native pointwise kernel (``_gru_gate_grads``).  The Mlp layer's node-sized
 tail (activation, LayerNorm, dense layer: mlpmessagepassing.py:114-117) is differentiated by a local ``torch.autograd.grad`` over
@@ -100,12 +104,14 @@ def _split16(x: torch.Tensor, index: Optional[torch.Tensor] = None, scale=None, 
     return hi, lo, inv
 
 
-def _add_aggregate(d_h: torch.Tensor, plan, x: torch.Tensor, weights, scale) -> torch.Tensor:
+def _add_aggregate(d_h: torch.Tensor, plan, x: torch.Tensor, weights, scale, bf16: bool = False) -> torch.Tensor:
     """d_h + sum_{e -> v} W_t(e) x[src(e)] for a gradient x: ``C.aggregate`` on x times its ``_pow2_scale`` pair ``scale``, scaled back in
     the add.  The fused kernel splits its operand into fp16 pairs without scaling, which represents x only to 2^-36 absolute (no
-    precision left for a gradient of 1e-8) and overflows at 65504; the power of two makes both exact in fp32's normal range."""
+    precision left for a gradient of 1e-8) and overflows at 65504; the power of two makes both exact in fp32's normal range.  bf16: x
+    times the scale is rounded to bf16 and aggregated as the bf16 layer forward aggregates its states."""
     s, inv = scale
-    return torch.addcmul(d_h, C.aggregate(plan, x * s, weights, N.REDUCE["sum"]), inv)
+    xs = x * s
+    return torch.addcmul(d_h, C.aggregate(plan, xs.to(torch.bfloat16) if bf16 else xs, weights, N.REDUCE["sum"]), inv)
 
 
 def _mm_t_split(a, b):
@@ -124,6 +130,20 @@ def _mm_t_split(a, b):
     finally:
         matmul.allow_fp16_reduced_precision_reduction = previous
     return main.add_(corr, alpha=1.0 / 2048.0).mul_(a_inv * b_inv)
+
+
+def _weight_grad_bf16(plan, g: torch.Tensor, index: Optional[torch.Tensor], inv, h: torch.Tensor, use_target: bool) -> torch.Tensor:
+    """[T, D, C] fp32: per edge type t, inv * sum_{e in t} g[index[e]] (x) [h[src(e)] ; h[tgt(e)]] (C = 2H with use_target, else the
+    source half, C = H) on the gathered bf16 weight-gradient kernel (csrc/wgrad.cu).  g: bf16 [*, D] rows (index None: row e for edge
+    e, cat(types) order); inv: the fp32 device scalar that undoes g's scaling."""
+    T, D, H = plan.num_types, g.shape[1], h.shape[1]
+    out = torch.empty(T, D, (2 if use_target else 1) * H, dtype=torch.float32, device=h.device)
+    lib = N.lib()
+    ws_bytes = lib.ptgnn_b200_edge_weight_grad_bf16_workspace_bytes(plan.num_edges, T, H, D, int(use_target))
+    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=h.device)
+    N.call("ptgnn_b200_edge_weight_grad_bf16", h.device, N.ptr(g), N.ptr(index), N.ptr(h), H, D, T, plan.type_off_c, N.ptr(plan.src32),
+           N.ptr(plan.tgt32), int(use_target), N.ptr(out), N.ptr(ws), ws_bytes)
+    return out.mul_(inv)
 
 
 def _slice(split, lo_, hi_):
@@ -223,13 +243,16 @@ def _aggregation_backward(plan, adj, h, W, d_agg, reduce_name, arg, d_h, b_all=N
     (None: the messages read h_src only), and d_W[t] is then [d W_src ; d W_tgt] along dim 1.  arg: the winning edge ids of max / min
     ([N, D], E for empty targets).  d_msg: the per-edge message gradients [E, D] when the caller has them (PNA's backward); they replace
     the routing of d_agg through arg.  b_all: the 3xFP16 split of the gathered source states, ``_split16(h, plan.src32)``, when the
-    caller reuses it across calls.  drop: the per-edge dropout of the source rows (``EdgeDropout``, h_src only): d W_t from the masked,
+    caller reuses it across calls.  bf16 h (Mlp layer): the same steps on bf16 operands -- d W_t on the gathered bf16 weight-gradient
+    kernel from d_agg (or d_msg) scaled by a power of two and rounded to bf16, and the transposed aggregations on the bf16 kernels;
+    d_h accumulates in fp32.  drop: the per-edge dropout of the source rows (``EdgeDropout``, h_src only): d W_t from the masked,
     scaled rows, and d h through the per-edge branch below with the mask applied to each edge's row gradient, for every reduction.
     sum / mean: split fp16 GEMMs over edges, and the forward's aggregation with W_t^T on the transposed graph (and, for h_tgt, on the
     graph of each edge's target to itself); otherwise: split fp16 GEMMs over the message gradients, and per type the native linear
     with W_t^T and scatter-add by source (and by target)."""
     num_nodes = h.shape[0]
     E = plan.num_edges
+    bf16 = h.dtype == torch.bfloat16
     by_target = d_msg is None and reduce_name in ("sum", "mean")       # every edge's message gradient is its target's d_agg row
     dense = by_target and drop is None
     if by_target:
@@ -237,26 +260,37 @@ def _aggregation_backward(plan, adj, h, W, d_agg, reduce_name, arg, d_h, b_all=N
             d_agg = d_agg / _mean_divisor(plan)[:, None]
         d_agg = d_agg.contiguous()
         scale = _pow2_scale(d_agg)                                       # one scale for a_all and the transposed aggregations
-        a_all = _split16(d_agg, plan.tgt32, scale)                       # [E, D] rows of d_agg, cat(types) order
+        if bf16:                                                         # d W: the kernel gathers the rows of d_agg itself
+            d_W_all = _weight_grad_bf16(plan, (d_agg * scale[0]).to(torch.bfloat16), plan.tgt32, scale[1], h, W_tgt is not None)
+        else:
+            a_all = _split16(d_agg, plan.tgt32, scale)                   # [E, D] rows of d_agg, cat(types) order
     else:
         if d_msg is None:
             d_msg = _route_to_arg(d_agg, arg, E)
-        a_all = _split16(d_msg)
+        if bf16:
+            s, inv = _pow2_scale(d_msg)
+            d_W_all = _weight_grad_bf16(plan, (d_msg * s).to(torch.bfloat16), None, inv, h, W_tgt is not None)
+        else:
+            a_all = _split16(d_msg)
     if b_all is None and drop is not None:                               # [E, H] dropout(h[src(e)])
         b_hi, b_lo, b_inv = _split16(h, plan.src32, bits=drop.bits)
         b_all = (b_hi, b_lo, b_inv * drop.scale)
-    elif b_all is None:
+    elif b_all is None and not bf16:
         b_all = _split16(h, plan.src32)                                  # [E, H] source states
-    g_all = None if W_tgt is None else _split16(h, plan.tgt32)           # [E, H] target states
+    g_all = None if W_tgt is None or bf16 else _split16(h, plan.tgt32)   # [E, H] target states
     d_W = []
     for t, ((src, tgt), w) in enumerate(zip(adj, W)):
         lo, hi = plan.type_off[t], plan.type_off[t + 1]
-        if hi == lo:
+        if bf16:
+            d_W.append(d_W_all[t])
+        elif hi == lo:
             d_W.append(w.new_zeros(w.shape[0], w.shape[1] + (0 if W_tgt is None else W_tgt[t].shape[1])))
+        else:
+            a = _slice(a_all, lo, hi)
+            d_w = _mm_t_split(a, _slice(b_all, lo, hi))
+            d_W.append(d_w if W_tgt is None else torch.cat([d_w, _mm_t_split(a, _slice(g_all, lo, hi))], dim=1))
+        if hi == lo:
             continue
-        a = _slice(a_all, lo, hi)
-        d_w = _mm_t_split(a, _slice(b_all, lo, hi))
-        d_W.append(d_w if W_tgt is None else torch.cat([d_w, _mm_t_split(a, _slice(g_all, lo, hi))], dim=1))
         if not dense:
             part = d_msg[lo:hi].contiguous() if d_msg is not None else d_agg.index_select(0, plan.tgt32[lo:hi].long())
             rows = C.linear(part, w.t().contiguous())
@@ -268,10 +302,10 @@ def _aggregation_backward(plan, adj, h, W, d_agg, reduce_name, arg, d_h, b_all=N
     if dense and E > 0:
         # d h_src[u] = sum over edges (u -> v, type t) of W_t^T d_agg[v]: the forward's aggregation on the transposed graph
         rplan = plan_for([(tgt, src) for src, tgt in adj], num_nodes)
-        d_h = _add_aggregate(d_h, rplan, d_agg, [w.t().contiguous() for w in W], scale)
+        d_h = _add_aggregate(d_h, rplan, d_agg, [w.t().contiguous() for w in W], scale, bf16)
         if W_tgt is not None:      # d h_tgt: every edge sends W_tgt^T d_agg[v] to its own target v
             tplan = plan_for([(tgt, tgt) for _src, tgt in adj], num_nodes)
-            d_h = _add_aggregate(d_h, tplan, d_agg, [w.t().contiguous() for w in W_tgt], scale)
+            d_h = _add_aggregate(d_h, tplan, d_agg, [w.t().contiguous() for w in W_tgt], scale, bf16)
     return d_W, d_h
 
 
@@ -491,16 +525,20 @@ class _MlpLayerFunction(torch.autograd.Function):
         W = [w.detach().contiguous() for w in weights]
         plan = plan_for(adj, num_nodes)
 
-        # ---- 1. re-compute the aggregate on the native kernels (PNA: with its arg ids; the messages are kept for its backward)
-        msg = C.edge_messages(plan, h, h if use_target else None, W, use_target)
-        arg = None
+        # ---- 1. re-compute the aggregate on the native kernels (PNA: with its arg ids; the messages are kept for its backward).  bf16
+        # states: sum / mean on the kernel the forward ran (``C.aggregate``), max / min from the bf16 messages, both in fp32
+        arg, msg = None, None
+        if h.dtype == torch.bfloat16 and reduce_name in ("sum", "mean"):
+            agg = C.aggregate(plan, h, W, N.REDUCE[reduce_name], use_target)
+        else:
+            msg = C.edge_messages(plan, h, h if use_target else None, W, use_target)
         if pna is not None:
             from .aggregation import native_pna
 
             agg, arg_max, arg_min = native_pna(msg, plan, pna.delta, want_arg=True)
         elif reduce_name in ("max", "min"):
             agg, arg = C.segment_reduce(msg, plan, N.REDUCE[reduce_name], return_arg=True)
-        else:
+        elif msg is not None:
             agg = C.segment_reduce(msg, plan, N.REDUCE[reduce_name])
         if pna is None:
             del msg
@@ -524,8 +562,9 @@ class _MlpLayerFunction(torch.autograd.Function):
             del msg
         Ws = [w[:, :H].contiguous() for w in W]                              # columns multiplying h_src
         Wg = [w[:, H:].contiguous() for w in W] if use_target else None      # columns multiplying h_tgt
-        d_W, d_h = _aggregation_backward(plan, adj, h, Ws, d_agg, reduce_name, arg, torch.zeros_like(h), W_tgt=Wg, d_msg=d_msg)
-        return (None, None, None, None, None, None, d_h, *d_tail, *d_W)
+        d_h = torch.zeros(h.shape, dtype=torch.float32, device=h.device)
+        d_W, d_h = _aggregation_backward(plan, adj, h, Ws, d_agg, reduce_name, arg, d_h, W_tgt=Wg, d_msg=d_msg)
+        return (None, None, None, None, None, None, d_h.to(h.dtype), *d_tail, *d_W)
 
 
 def mlp_forward_with_grad(layer, node_states, adjacency_lists, reduce_name, use_target, message_activation, ln, dense, dense_activation,

@@ -11,7 +11,7 @@ pieces of the C ABI (``ptgnn_b200_edge_messages_f32``, ``ptgnn_b200_linear_f32``
   concatenated targets, exactly what ``mlpmessagepassing.py:100-112`` passes; its own ``torch_scatter`` calls resolve to the native
   segmented reduce through ``ptgnn_b200.torch_scatter_shim``.
 
-fp32 only; the ``[E, D]`` message tensor IS materialised here (these are the slow, general configurations -- none of the reference's
+fp32 only (``edge_messages`` and ``aggregate`` also take bf16 rows, for the bf16 Mlp backward); the ``[E, D]`` message tensor IS materialised here (these are the slow, general configurations -- none of the reference's
 implementations uses them by default); the tail of an Mlp layer (activation, LayerNorm, dense, of whatever width the aggregator
 produced) runs as the module's own device-side torch ops.
 """
@@ -59,16 +59,25 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] =
 
 def edge_messages(plan: EdgePlan, source_rows: torch.Tensor, target_rows: Optional[torch.Tensor], weights: Sequence[torch.Tensor],
                   use_target: bool) -> torch.Tensor:
-    """``[E, D]`` messages in the reference's row order (cat over edge types): row e = W_t(e) [source_rows[src(e)] ; target_rows[tgt(e)]]."""
+    """``[E, D]`` fp32 messages in the reference's row order (cat over edge types): row e = W_t(e) [source_rows[src(e)] ; target_rows[tgt(e)]].
+    bf16 rows: the bf16 messages of the three-kernel path (bf16 products, fp32 accumulation, rounded to bf16), up-cast."""
     D = weights[0].shape[0]
     E = plan.num_edges
-    out = torch.empty(E, D, dtype=torch.float32, device=source_rows.device)
+    bf16 = source_rows.dtype == torch.bfloat16
+    out = torch.empty(E, D, dtype=torch.bfloat16 if bf16 else torch.float32, device=source_rows.device)
     if E == 0:
-        return out
+        return out.float()
     ident = torch.arange(E, dtype=torch.int32, device=source_rows.device)
     ws_list = [N.require_cuda(w, "edge weight", torch.float32) for w in weights]
     lib = N.lib()
     H = source_rows.shape[1]
+    if bf16:
+        ws_bytes = lib.ptgnn_b200_edge_messages_bf16_workspace_bytes(plan.num_types, H, D, int(use_target))
+        ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=source_rows.device)
+        N.call("ptgnn_b200_edge_messages_bf16", source_rows.device, N.ptr(source_rows), N.ptr(target_rows), H, D, plan.num_types,
+               plan.type_off_c, N.ptr(plan.src32), N.ptr(plan.tgt32), N.ptr(ident), N.ptr_table(ws_list), int(use_target), N.ptr(out),
+               N.ptr(ws), ws_bytes)
+        return out.float()
     ws_bytes = lib.ptgnn_b200_edge_messages_workspace_bytes(plan.num_types, H, D, int(use_target))
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=source_rows.device)
     N.call("ptgnn_b200_edge_messages_f32", source_rows.device, N.ptr(source_rows), N.ptr(target_rows), H, D, plan.num_types, plan.type_off_c,
@@ -87,16 +96,30 @@ def segment_reduce(messages: torch.Tensor, plan: EdgePlan, reduce_code: int, ret
     return (out, arg) if return_arg else out
 
 
-def aggregate(plan: EdgePlan, source_rows: torch.Tensor, weights: Sequence[torch.Tensor], reduce_code: int) -> torch.Tensor:
+def aggregate(plan: EdgePlan, source_rows: torch.Tensor, weights: Sequence[torch.Tensor], reduce_code: int, use_target: bool = False) -> torch.Tensor:
     """``reduce_{e -> v} W_type(e) source_rows[src(e)]`` as [num_nodes, D] fp32: the fused gather -> Linear -> segmented-reduce kernel
     where it takes the dimensions (D == 128, K in {64, 128}: no [E, D] message tensor), else ``edge_messages`` + ``segment_reduce``.
-    Used by the backward passes (aggregate re-computation; d h_src on the transposed graph)."""
+    Used by the backward passes (aggregate re-computation; d h_src on the transposed graph).  bf16 rows: the aggregate the bf16 layer
+    forward computes (messages rounded to bf16, fp32 reduction) on the same kernels as that forward, before any rounding of its own;
+    use_target (bf16 only): the messages read [source_rows[src(e)] ; source_rows[tgt(e)]]."""
     import ctypes
 
     from .messagepassing import _use_fused
 
-    D, K = weights[0].shape
+    D = weights[0].shape[0]
+    K = source_rows.shape[1]
     lib = N.lib()
+    if source_rows.dtype == torch.bfloat16:
+        if plan.num_edges == 0 or not _use_fused(lib, True, K, D):
+            return segment_reduce(edge_messages(plan, source_rows, source_rows if use_target else None, weights, use_target), plan, reduce_code)
+        ws_list = [N.require_cuda(w, "edge weight", torch.float32) for w in weights]
+        ws_bytes = lib.ptgnn_b200_fused_aggregate_bf16_workspace_bytes(plan.num_types, K, int(use_target))
+        ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=source_rows.device)
+        out = torch.empty(plan.num_nodes, D, dtype=torch.float32, device=source_rows.device)
+        N.call("ptgnn_b200_fused_aggregate_bf16", source_rows.device, N.ptr(source_rows), plan.num_nodes, K, plan.num_types,
+               ctypes.byref(plan.block_plan()), N.ptr(plan.row_ptr), N.ptr_table(ws_list), int(use_target), reduce_code, N.ptr(out),
+               N.ptr(ws), ws_bytes)
+        return out
     if plan.num_edges == 0 or not _use_fused(lib, False, K, D):
         return segment_reduce(edge_messages(plan, source_rows, None, weights, False), plan, reduce_code)
     rows = N.require_cuda(source_rows, "source_rows", torch.float32)

@@ -594,6 +594,33 @@ extern "C" int ptgnn_b200_edge_messages_f32(const float *source_states, const fl
                          src32, tgt32, out_row, messages, workspace, true, st);
 }
 
+extern "C" int32_t ptgnn_b200_edge_messages_bf16_supported(int32_t in_dim, int32_t message_dim) {
+    return in_dim % 32 == 0 && in_dim >= 64 && in_dim <= 1024 && message_dim % 16 == 0 && message_dim >= 64 && message_dim <= 256;
+}
+extern "C" size_t ptgnn_b200_edge_messages_bf16_workspace_bytes(int32_t num_types, int32_t in_dim, int32_t message_dim, int32_t use_target_state) {
+    if (num_types < 0 || !ptgnn_b200_edge_messages_bf16_supported(in_dim, message_dim)) return 0;
+    return tc::edge_weight_bytes(true, num_types, message_dim, use_target_state ? 2 * in_dim : in_dim) + 256;
+}
+extern "C" int ptgnn_b200_edge_messages_bf16(const void *source_states, const void *target_states, int32_t in_dim, int32_t message_dim,
+                                             int32_t num_types, const int64_t *type_off, const int32_t *src32, const int32_t *tgt32,
+                                             const int32_t *out_row, const float *const *edge_weights, int32_t use_target_state,
+                                             void *messages, void *workspace, size_t workspace_bytes, void *stream) {
+    const char *who = "edge_messages_bf16";
+    PTGNN_CHECK_ARG(num_types >= 0 && num_types <= PTGNN_MAX_EDGE_TYPES && type_off, "%s: bad num_types=%d", who, num_types);
+    const int64_t E = type_off[num_types];
+    int rc = check_unfused_dims(who, true, 0, E, in_dim, message_dim, 0, false);
+    if (rc) return rc;
+    if (E == 0) return PTGNN_OK;
+    PTGNN_CHECK_ARG(source_states && src32 && out_row && edge_weights && messages && (!use_target_state || (target_states && tgt32)),
+                    "%s: null pointer", who);
+    PTGNN_CHECK_WORKSPACE(who, workspace, workspace_bytes,
+                          ptgnn_b200_edge_messages_bf16_workspace_bytes(num_types, in_dim, message_dim, use_target_state));
+    using bf = __nv_bfloat16;
+    return edge_messages(static_cast<const bf *>(source_states), static_cast<const bf *>(target_states), in_dim, message_dim,
+                         use_target_state ? 1 : 0, num_types, type_off, edge_weights, src32, tgt32, out_row, static_cast<bf *>(messages),
+                         workspace, true, static_cast<cudaStream_t>(stream));
+}
+
 // workspace: derived edge weights | keep bits [E, H / 32]
 struct MsgDropWs { size_t weights, bits, total; };
 static MsgDropWs msg_drop_layout(int64_t E, int T, int H, int D) {

@@ -519,3 +519,43 @@ extern "C" int ptgnn_b200_mlp_forward_fused(int32_t bf16_states, const void *nod
                      ln_bias, ln_eps, dense_weight, dense_bias, dense_activation, out_states, workspace, workspace_bytes, weight_cache,
                      weight_cache_bytes, cache_valid, static_cast<cudaStream_t>(stream));
 }
+
+// workspace of the bf16 aggregate alone: the packed (bf16) edge weights
+struct AggBf16Ws { size_t weights, total; };
+static AggBf16Ws agg_bf16_layout(int T, int H, int ut) {
+    Layout l;
+    AggBf16Ws w;
+    w.weights = l.add_bytes(ws_slice(fused::packed_weight_bytes(1, T, H, ut), 1));
+    w.total = l.total;
+    return w;
+}
+extern "C" size_t ptgnn_b200_fused_aggregate_bf16_workspace_bytes(int32_t num_types, int32_t in_dim, int32_t use_target_state) {
+    const int ut = use_target_state ? 1 : 0;
+    if (num_types <= 0 || num_types > PTGNN_MAX_EDGE_TYPES || !fused::supported(1, in_dim, fused::kD, ut)) return 0;
+    return agg_bf16_layout(num_types, in_dim, ut).total;
+}
+extern "C" int ptgnn_b200_fused_aggregate_bf16(const void *node_states, int64_t num_nodes, int32_t in_dim, int32_t num_types,
+                                               const ptgnn_b200_block_plan *block_plan, const int32_t *row_ptr,
+                                               const float *const *edge_weights, int32_t use_target_state, int32_t reduce, float *out,
+                                               void *workspace, size_t workspace_bytes, void *stream) {
+    const char *who = "fused_aggregate_bf16";
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int ut = use_target_state ? 1 : 0;
+    PTGNN_CHECK_ARG(block_plan != nullptr, "%s: null block plan", who);
+    PTGNN_CHECK_ARG(num_types > 0 && num_types <= PTGNN_MAX_EDGE_TYPES, "%s: bad num_types=%d", who, num_types);
+    if (!fused::supported(1, in_dim, fused::kD, ut)) {
+        set_error("%s: in_dim=%d is not supported by the fused kernel (bf16 states)", who, in_dim);
+        return PTGNN_E_UNSUPPORTED;
+    }
+    PTGNN_CHECK_ARG(num_nodes >= 0 && num_nodes < INT32_MAX, "%s: sizes out of range", who);
+    if (num_nodes == 0) return PTGNN_OK;
+    PTGNN_CHECK_ARG(node_states && out && row_ptr && edge_weights, "%s: null pointer", who);
+    const AggBf16Ws L = agg_bf16_layout(num_types, in_dim, ut);
+    PTGNN_CHECK_WORKSPACE(who, workspace, workspace_bytes, L.total);
+    char *wpack = static_cast<char *>(workspace) + L.weights;
+    PTGNN_TRY(fused::pack_weights(1, num_types, in_dim, ut, edge_weights, wpack, block_plan->status, st));
+    fused::AggregateArgs a = aggregate_args(1, block_plan, row_ptr, num_nodes, in_dim, num_types, reduce, wpack);
+    a.src_rows = node_states; a.use_target = ut; a.tgt_rows = node_states;
+    a.out = out; a.out_mode = 0;
+    return fused::aggregate(a, st);
+}

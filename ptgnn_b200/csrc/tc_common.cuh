@@ -154,6 +154,18 @@ __device__ __forceinline__ void wgmma_16_rs_n64(float (&d)[32], const uint32_t (
             : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
 }
 
+// D[64 x 64] += A[64 x 16] * B[16 x 64], bf16 operands from shared memory, both MN-major (imm-trans-a = imm-trans-b = 1): each
+// 128-byte row holds 64 consecutive M (or N) elements of one k, rows of consecutive k follow each other, SWIZZLE_128B (16-byte
+// chunk index XOR (k & 7)), 8-row groups 1024 bytes apart (the stride byte offset of make_smem_desc_sw128).  Advancing k by 16 is
+// a +2048-byte bump of the start address.
+__device__ __forceinline__ void wgmma_bf16_ss_n64_mn(float (&d)[32], uint64_t desc_a, uint64_t desc_b) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\twgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(desc_a), "l"(desc_b), "r"(1));
+}
+
 // Narrower register-A MMAs for a sub-group of at most N <= 64 columns: D[64 x N] += A[64 x 16] * B[N x 16]^T.  Their accumulator
 // fragment is the first N / 2 registers of the m64n64 layout above (columns 8 j .. 8 j + 7 are d[4 j .. 4 j + 3]), so they take
 // the same 32-register array and leave d[N / 2 ..] untouched.

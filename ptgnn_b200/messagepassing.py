@@ -47,7 +47,8 @@ def _refuse_autograd(module: nn.Module, node_states: torch.Tensor) -> None:
     if torch.is_grad_enabled() and (node_states.requires_grad or any(p.requires_grad for p in module.parameters())):
         raise NotImplementedError(
             "this configuration is forward-only (backward, SURVEY.md §8 row f-1, exists for GatedMessagePassingLayer with fp32 "
-            "states and no edge features): call it under torch.no_grad() / torch.inference_mode(), or set requires_grad_(False) "
+            "states and no edge features, and for MlpMessagePassingLayer with its default message MLP: fp32 states, or bf16 states "
+            "with a string aggregation): call it under torch.no_grad() / torch.inference_mode(), or set requires_grad_(False) "
             "on the parameters"
         )
 
@@ -67,6 +68,15 @@ def _native_dropout(lib, H: int, D: int) -> bool:
     """GatedMessagePassingLayer's per-edge dropout (fp32 states) runs natively at these dims: inside the fused aggregation where it
     takes them, else on the three-kernel path's masked message kernel."""
     return _use_fused(lib, False, H, D) or bool(lib.ptgnn_b200_gated_dropout_supported(H, D))
+
+
+def _mlp_bf16_grad_supported(lib, H: int, D: int, use_target: bool) -> bool:
+    """MlpMessagePassingLayer (default message MLP, string aggregation) trains with bf16 states at these dims: the bf16 forward runs
+    (fused or three-kernel), the gathered weight-gradient kernel takes them, and the bf16 aggregation runs on the transposed graph
+    (K = D, D' = H) for d h."""
+    forward = _use_fused(lib, True, H, D) or bool(lib.ptgnn_b200_edge_messages_bf16_supported(H, D))
+    transposed = _use_fused(lib, True, D, H) or bool(lib.ptgnn_b200_edge_messages_bf16_supported(D, H))
+    return forward and transposed and bool(lib.ptgnn_b200_edge_weight_grad_bf16_supported(H, D))
 
 
 def _check_states(node_states: torch.Tensor, expected_dim: int, what: str) -> None:
@@ -573,7 +583,9 @@ class MlpMessagePassingLayer(AbstractMessagePassingLayer):
         # (composed path without gradients, _MlpLayerFunction's PNA mode with them)
         pna_config = plain_mlp and isinstance(self.__aggregation_fn, PnaMessageAggregation)
         grad = _ag.needs_grad(self, node_states)
-        if grad and (not (default_config or pna_config) or gather_states is not None or node_states.dtype != torch.float32):
+        bf16_grad = default_config and node_states.dtype == torch.bfloat16 and _mlp_bf16_grad_supported(
+            N.lib(), self.__input_state_dim, self.__message_dim, self.__use_target_state_as_message_input)
+        if grad and (not (default_config or pna_config) or gather_states is not None or (node_states.dtype != torch.float32 and not bf16_grad)):
             _refuse_autograd(self, node_states)
         if not (default_config or pna_config):
             return self._forward_composed(node_states, adjacency_lists, edge_features, gather_states)
